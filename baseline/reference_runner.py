@@ -2,7 +2,7 @@
 `Tacotron()` + `TacotronLoss` from modules/tacotron2.py, configured by its own params/*.json -- no code of this repository on that path.
 
 Used by `bench.py --impl reference` (CPU, all host threads it can use) and by bench.py's extra baselines (the mandated cfg-1 CPU
-timing, eager PyTorch on the B200).  Test / measurement infrastructure only: the product never imports this module.
+timing, eager PyTorch on the GPU).  Test / measurement infrastructure only: the product never imports this module.
 """
 import os
 import statistics
@@ -130,8 +130,7 @@ def time_cpu(config, regularization, B, L, T, steps, warmup, threads=None):
     ncpu = os.cpu_count() or 1
     scan = None
     if threads is None:
-        # measured on the 128-core B200 host: 8 -> 2.8 s, 16 -> 2.0 s, 32 -> 2.9 s, 64 -> 6.3 s, 128 -> 403 s per step (torch's intra-op
-        # pool collapses on ~10^5 tiny ops); the scan therefore stops at 32 threads
+        # torch's intra-op pool collapses on ~10^5 tiny ops with many threads; the scan therefore stops at 32 threads
         cands = sorted({n for n in (8, 16, 32) if n <= ncpu} or {ncpu})
         threads, scan = pick_threads(r, cands)          # the scan steps double as warm-up
         for _ in range(max(0, warmup - len(cands))):

@@ -40,12 +40,40 @@ def parse():
     ap.add_argument('--ref-frames', type=int, default=100,
                     help='frames per utterance of the CPU reference sample (reference arm / cpu_baseline): the first N of --frames')
     ap.add_argument('--no-extra-baselines', action='store_true',
-                    help='skip the cfg-1 CPU timing and the eager-PyTorch-on-B200 timing of the unmodified reference (N=1 only)')
+                    help='skip the cfg-1 CPU timing and the eager-PyTorch-on-GPU timing of the unmodified reference (N=1 only)')
     ap.add_argument('--no-graph', action='store_true', help='issue every step from Python instead of replaying the captured CUDA graph')
     ap.add_argument('--breakdown', default='', help='write a per-kernel device-time table of one extra (untimed) step to this file')
     ap.add_argument('--precision', default='bf16', choices=['bf16', 'fp32'],
                     help="bf16: tensor-core operands, fp32 master/state (BASELINE configs[1]); fp32: exact parity mode")
+    ap.add_argument('--dump-outputs', default='', metavar='DIR',
+                    help='after the timed steps, write what the last timed step computed as DIR/<name>.npy (float32): the loss, its terms '
+                         'and every parameter gradient (all of it up to 65536 elements, else a fixed seeded sample of 65536 of them)')
     return ap.parse_args()
+
+
+DUMP_SAMPLE = 1 << 16
+
+
+def dump_outputs(out_dir, loss, parts, named_params):
+    """The results of one training step as float32 .npy files (12 MB for the default workload).  Large gradients are sampled at
+    indices drawn from a generator seeded by the tensor size, so two builds of the project write comparable files."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {'loss': loss}
+    arrays.update({f'loss.{k}': v for k, v in parts.items() if torch.is_tensor(v)})
+    for name, p in named_params:
+        g = p.grad.detach().reshape(-1)
+        if g.numel() > DUMP_SAMPLE:
+            idx = torch.randint(0, g.numel(), (DUMP_SAMPLE,), generator=torch.Generator().manual_seed(g.numel()))
+            g = g[idx.to(g.device)]
+        arrays[f'grad.{name}'] = g
+    total = 0
+    for name, t in arrays.items():
+        a = t.detach().float().reshape(-1).cpu().numpy().astype(np.float32)
+        total += a.nbytes
+        np.save(os.path.join(out_dir, f'{name}.npy'), a)
+    assert total <= 64 << 20, f'dumped {total} bytes'
 
 
 def workload(a):
@@ -109,7 +137,7 @@ KERNEL_SHARE = {'lstm_loop_tc_kernel<att>': ('att', 1), 'lstm_loop_tc_kernel<gen
                 'att_bwd_loop_kernel': ('att', 2), 'lstm_bwd_loop_tc_kernel': ('gen', 2), 'lstm_bwd_loop_kernel': ('gen', 2)}
 
 
-def roofline_entry(name, ms, T, dims, peak, precision, traffic=None, fwd_equiv=1, part=None, note=None):
+def roofline_entry(name, ms, T, dims, peak, precision, fwd_equiv=1, part=None, note=None):
     """Fractions of the measured HBM peak for `ms` of device time against T x (share of BYTES_fwd_step) x fwd_equiv, at three element
     widths: the run's own (`frac`: bf16 runs are judged against the bf16 column of SURVEY 8d, w = a = 2), bf16 weights + fp32
     activations (`frac_mixed`), and the fp32-naive figure (`frac_fp32_naive`)."""
@@ -120,7 +148,7 @@ def roofline_entry(name, ms, T, dims, peak, precision, traffic=None, fwd_equiv=1
     e = {'kernel': name, 'bound': 'hbm', 'unit': 'GB/s', 'peak': peak, 'avg_launch_ms': ms,
          'algorithmic_bytes_per_launch': alg(*own), 'achieved': alg(*own) / sec / 1e9, 'frac': alg(*own) / sec / 1e9 / peak,
          'frac_mixed': alg(2, 4) / sec / 1e9 / peak if precision == 'bf16' else None,
-         'frac_fp32_naive': alg(4, 4) / sec / 1e9 / peak, 'traffic': traffic,
+         'frac_fp32_naive': alg(4, 4) / sec / 1e9 / peak,
          'element_width': 'w=a=2 B (bf16 column of SURVEY 8d)' if precision == 'bf16' else 'w=a=4 B (fp32)',
          'algorithmic_bytes_formula': f'{fwd_equiv} x T x BYTES_fwd_step' + (f'[{part} loop share]' if part else '') + ' (SURVEY 8d)'}
     if note:
@@ -128,24 +156,12 @@ def roofline_entry(name, ms, T, dims, peak, precision, traffic=None, fwd_equiv=1
     return e
 
 
-def ncu_traffic(B, L, T):
-    """DRAM bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum) of the loop kernels from the committed ncu capture of the
-    CURRENT kernels at this shape (profiles/r2/ncu_traffic.json, written by tools/ncu_traffic.py from the raw capture); {} if none."""
-    path = os.path.join(ROOT, 'profiles', 'r2', 'ncu_traffic.json')
-    if not os.path.exists(path):
-        return {}
-    d = json.load(open(path))
-    if (d.get('B'), d.get('L'), d.get('T')) != (B, L, T):
-        return {}
-    return {k: v['dram_read'] + v['dram_write'] for k, v in d.get('kernels', {}).items()}
-
-
 def measured_peaks():
     path = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(path):
         d = json.load(open(path))
         return float(d['hbm_gbs']), 'measured (MEASURED_PEAKS.json)'
-    return 6650.0, 'fallback (B200_PROFILING.md)'
+    return 3350.0, 'fallback (H100 SXM data sheet: 3.35 TB/s HBM3)'
 
 
 class ClockSampler:
@@ -191,8 +207,8 @@ def cpu_oracle_frames_per_s(a, steps, warmup, sample_frames=24):
     from oracle import tacotron_oracle as O
     hp, B, L, _ = workload(a)
     T = sample_frames
-    # torch's intra-op pool on a many-core host is dominated by fork/join overhead for this op mix (measured on the
-    # 128-core B200 host: 12.6 frames/s with 128 threads); 16 threads is the best setting we found, and is what is reported.
+    # torch's intra-op pool on a many-core host is dominated by fork/join overhead for this op mix; 16 threads is the best setting we
+    # found, and is what is reported.
     cores = min(os.cpu_count() or 1, 16)
     torch.set_num_threads(cores)
     torch.manual_seed(0)
@@ -232,7 +248,7 @@ def config_dict(a, world, B, L, T):
     return {'workload': f'{a.config} train fwd+bwd, B={B}/GPU L={L} T={T} ({a.regularization} cells), tf=1.0',
             'global_batch': world * B, 'parallelism': f'dp{world}',
             'precision': 'bf16 tensor-core operands, fp32 accumulate / master weights / states' if a.precision == 'bf16' else 'fp32',
-            'l2': 'per-step working set (~5 GB of activations) >> 126 MB L2, no flush needed',
+            'l2': 'per-step working set (~5 GB of activations) >> 50 MB L2, no flush needed',
             'note': 'batch 64 is invalid for the 10-language grouped encoder (B % G == 0); shipped batch 60 used'}
 
 
@@ -288,7 +304,7 @@ def run_reference(a):
 
 def extra_baselines(a, threads):
     """BASELINE.md section 3: the mandated cfg-1 CPU timing (default Params = LJ Speech, B = 16, L = 180, T = 900, full length) and the
-    unmodified reference in eager PyTorch on the B200 (the competitor on the same box) at this run's own workload."""
+    unmodified reference in eager PyTorch on the GPU (the competitor on the same box) at this run's own workload."""
     sys.path.insert(0, os.path.join(ROOT, 'baseline'))
     import reference_runner as R
     if not R.available():
@@ -303,11 +319,11 @@ def extra_baselines(a, threads):
         out['cpu_cfg1_ljspeech_B16'] = {'error': repr(exc)[:200]}
     try:
         r = R.time_gpu_eager(a.config, a.regularization, B, L, T, steps=1, warmup=1)
-        out['eager_pytorch_b200'] = {'value': r['frames_per_s'], 'unit': UNIT, 's_per_step': r['s_per_step'],
+        out['eager_pytorch_gpu'] = {'value': r['frames_per_s'], 'unit': UNIT, 's_per_step': r['s_per_step'],
                                      'sample': f'unmodified reference, eager PyTorch fp32 (ATen / cuDNN / cuBLAS) on cuda:0, {a.config} B={B} L={L} T={T} (full), '
                                                'fwd+loss+bwd, 1 warm-up + 1 timed step'}
     except Exception as exc:      # noqa: BLE001
-        out['eager_pytorch_b200'] = {'error': repr(exc)[:200]}
+        out['eager_pytorch_gpu'] = {'error': repr(exc)[:200]}
     return out
 
 
@@ -346,12 +362,14 @@ def run_b200(a):
     h2d_bytes = sum(v.numel() * v.element_size() for v in host.values())
     F.PROFILE.clear()
 
+    last = {}           # loss terms of the latest eager step (the graphed step keeps its own)
+
     def eager_step(batch):
         bucket.zero()
         post, pre, stop, align, spk, enc = model(batch['text'], batch['text_length'], batch['target'], batch['target_length'],
                                                  batch.get('speakers'), batch.get('languages'), hp.teacher_forcing)
-        loss, _ = crit(batch['text_length'], batch['target_length'], pre, batch['target'], post, batch['target'], stop,
-                       batch['stop_target'], align, batch.get('speakers'), spk, enc, None)
+        loss, last['parts'] = crit(batch['text_length'], batch['target_length'], pre, batch['target'], post, batch['target'], stop,
+                                   batch['stop_target'], align, batch.get('speakers'), spk, enc, None)
         loss.backward()
         bucket.allreduce()
         return loss
@@ -384,7 +402,7 @@ def run_b200(a):
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        loss_val = None
+        loss_val, loss = None, None
         for _ in range(n):
             if from_host and graphed is not None:
                 batch = host                       # GraphedTrainStep copies the pinned host tensors into its static device buffers
@@ -399,7 +417,7 @@ def run_b200(a):
         if world > 1:
             dist.barrier()
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
-        return float(ms), loss_val
+        return float(ms), loss_val, loss
 
     # the clock sampler (an nvidia-smi child process) starts BEFORE the warm-up: its NVML initialisation briefly contends with
     # the CUDA driver, which must not land inside the timed region
@@ -416,9 +434,12 @@ def run_b200(a):
         _lib.kernel_timing(True)          # CUDA events on the launching stream around the dominant kernels, inside the timed steps
     if ncu_range:
         torch.cuda.profiler.start()
-    ms, _ = timed(a.steps, from_host=False)
+    ms, _, last_loss = timed(a.steps, from_host=False)
     if ncu_range:
         torch.cuda.profiler.stop()
+    if a.dump_outputs and rank == 0:      # before the steps below overwrite the gradients
+        dump_outputs(a.dump_outputs, last_loss, graphed.parts if graphed is not None else last['parts'],
+                     [(n, p) for n, p in model.named_parameters() if p.requires_grad])
     launches = (_lib.launch_count() - n0) if graphed is None else launches_per_step * a.steps
     if graphed is not None:
         # events cannot be timed inside a replayed graph: the per-kernel durations come from the SAME kernels issued eagerly, a.steps
@@ -433,7 +454,7 @@ def run_b200(a):
     _lib.kernel_timing(False)
     dec_ms = [s.elapsed_time(e) for s, e in F.PROFILE.get('decoder_fwd', [])]
     decb_ms = [s.elapsed_time(e) for s, e in F.PROFILE.get('decoder_bwd', [])]
-    ms_e2e, loss_val = timed(a.steps, from_host=True)
+    ms_e2e, loss_val, _ = timed(a.steps, from_host=True)
     clocks = sampler.stop() if rank == 0 else None
     if a.breakdown and rank == 0:       # CUPTI kernel times of ONE extra step (not part of any reported number)
         from torch.profiler import profile, ProfilerActivity
@@ -466,20 +487,19 @@ def run_b200(a):
         peak, peak_src = measured_peaks()
         dims = (B, L, M, hp.decoder_dimension, hp.prenet_dimension, hp.attention_dimension, hp.attention_location_dimension,
                 hp.attention_kernel_size, hp.num_mels)
-        traffic = ncu_traffic(B, L, T)
         roofs = []
         for kname, (tot, cnt) in ktimes.items():
             if kname in KERNEL_SHARE and cnt:
                 part, eq = KERNEL_SHARE[kname]
-                roofs.append(roofline_entry(kname, tot / cnt, T, dims, peak, a.precision, traffic.get(kname), eq, part))
+                roofs.append(roofline_entry(kname, tot / cnt, T, dims, peak, a.precision, eq, part))
         if dec_ms:
             roofs.append(roofline_entry('decoder forward op (both forward loops + the time-batched GEMMs around them)', statistics.mean(dec_ms),
-                                        T, dims, peak, a.precision, None, 1, None))
+                                        T, dims, peak, a.precision, 1, None))
         if decb_ms:
             roofs.append(roofline_entry('decoder backward op (both reverse loops, post pass, dW / dX GEMMs)', statistics.mean(decb_ms),
-                                        T, dims, peak, a.precision, None, 2, None))
+                                        T, dims, peak, a.precision, 2, None))
         roofs.append(roofline_entry('whole training step (encoder, decoder, postnet, loss, backward)', ms / a.steps, T, dims, peak, a.precision,
-                                    None, 3, None, note='3 x T x BYTES_fwd_step: decoder bytes only, the encoder / postnet / loss time counts against them'))
+                                    3, None, note='3 x T x BYTES_fwd_step: decoder bytes only, the encoder / postnet / loss time counts against them'))
         loops = [r for r in roofs if r['kernel'] in KERNEL_SHARE]
         roof = dict(max(loops, key=lambda r: r['avg_launch_ms'])) if loops else (dict(roofs[0]) if roofs else None)
         if roof:

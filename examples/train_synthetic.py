@@ -6,7 +6,7 @@
 
 Pieces (all from this repository): `Tacotron` / `TacotronLoss` with the reference's surface, `BucketedPerfectBatchSampler` + `shard`
 for language-balanced, length-bucketed batches, `GradBucket` (flat gradient, one NCCL all-reduce per step), `FlatParams` + `FusedAdam`
-(global-norm clip + Adam + StepLR in one library call).  Needs a B200: there is no CPU path.
+(global-norm clip + Adam + StepLR in one library call).  Needs an H100: there is no CPU path.
 """
 import argparse
 import os

@@ -1,5 +1,5 @@
 /*
- * b200tts -- C ABI of the B200-native Tacotron-2 training hot path (sm_100a only).
+ * b200tts -- C ABI of the Hopper-native Tacotron-2 training hot path (sm_90a only; the b200tts prefix is historical).
  *
  * The reference (Tomiinek/Multilingual_Text_to_Speech) has no FFI / plugin layer: its boundary for this
  * path is the Python nn.Module surface (SURVEY.md section 8b).  This header is the boundary a native
@@ -14,8 +14,8 @@
  *     *_workspace_bytes() queries (256-byte aligned base pointers expected).
  *   - every call enqueues work on `stream` (a cudaStream_t passed as void*) and returns
  *     immediately; 0 = ok, negative = error, message via b200tts_last_error().
- *   - there is NO CPU fallback: every entry point fails with B200TTS_ERR_CUDA when no sm_100 device
- *     is present.
+ *   - there is NO CPU fallback: every entry point that needs the device fails with B200TTS_ERR_CUDA when
+ *     no CUDA device is present and with B200TTS_ERR_UNSUPPORTED when it is not an sm_90 (H100) device.
  */
 #ifndef B200TTS_H_
 #define B200TTS_H_
@@ -43,7 +43,7 @@ int b200tts_version(void);
 unsigned long long b200tts_launch_count(void);
 
 /* Live kernel timing for bench.py's per-kernel roofline: while enabled, the library brackets its dominant kernels (the four persistent
- * decoder loops, the attention post pass, the tcgen05 GEMM) with CUDA events on the launching stream.  enable != 0 starts a fresh
+ * decoder loops, the attention post pass, the wgmma GEMM) with CUDA events on the launching stream.  enable != 0 starts a fresh
  * collection, 0 stops and clears.  After a device synchronize, kernel_timing_read(index, ...) returns the index-th distinct kernel
  * name with the summed duration and the number of launches; it returns 1 past the end of the list.                           */
 int b200tts_kernel_timing(int enable);
@@ -56,10 +56,10 @@ int b200tts_kernel_timing_read(int index, char* name, int name_capacity, float* 
 #define B200TTS_PRECISION_BF16 1
 int b200tts_set_precision(int mode);
 int b200tts_get_precision(void);
-/* Caller-owned device scratch (1024-byte aligned) for the bf16 operand packing of the tcgen05 GEMM path; without it (or when a
+/* Caller-owned device scratch (1024-byte aligned) for the bf16 operand packing of the wgmma GEMM path; without it (or when a
  * problem does not fit) the bf16 mode uses the mma.sync kernel.  ~1.5 GB covers the BASELINE shapes.  NULL releases it. */
 int b200tts_set_scratch(void* ptr, size_t bytes);
-/* Debug / A-B switch: 0 forces the mma.sync bf16 GEMM even when the tcgen05 path is applicable. */
+/* Debug / A-B switch: 0 forces the mma.sync bf16 GEMM even when the wgmma path is applicable. */
 int b200tts_set_tensor_core_gemm(int enabled);
 
 /* ---- generic dense contraction (the time-batched GEMMs of the path) ----------------------- */
@@ -134,14 +134,14 @@ typedef struct {
 size_t b200tts_decoder_workspace_bytes(const b200tts_decoder_shape* shape);
 size_t b200tts_decoder_bwd_workspace_bytes(const b200tts_decoder_shape* shape);
 /* Which kernels a bf16-mode training step of this shape runs on (pure host arithmetic, no device needed): bit 0 = persistent
- * forward loops, bit 1 = their TMA + tcgen05 + TMEM variant, bit 2 = persistent generator reverse loop, bit 3 = its tcgen05
- * variant, bit 4 = persistent attention reverse loop, bit 5 = its tcgen05 product.  0 = the per-step kernel chains.
+ * forward loops, bit 1 = their TMA + wgmma variant, bit 2 = persistent generator reverse loop, bit 3 = its wgmma
+ * variant, bit 4 = persistent attention reverse loop, bit 5 = its wgmma product.  0 = the per-step kernel chains.
  * (The reference has no such limit anywhere: modules/attention.py:67-74 takes any length.) */
 int b200tts_decoder_path(const b200tts_decoder_shape* shape);
 /* Debug: byte offset, inside the decoder forward workspace, of the per-CTA phase cycle counters the persistent
- * kernels leave behind ([2][148][8] int64: attention loop, generator loop). */
+ * kernels leave behind ([2][132][8] int64, one row per SM: attention loop, generator loop). */
 size_t b200tts_debug_persist_profile_offset(const b200tts_decoder_shape* shape);
-/* Same for the backward workspace: which = 0 generator loop, 1 attention loop ([148][8] int64 each). */
+/* Same for the backward workspace: which = 0 generator loop, 1 attention loop ([132][8] int64 each). */
 size_t b200tts_debug_persist_bwd_profile_offset(const b200tts_decoder_shape* shape, int which);
 
 int b200tts_decoder_forward(const b200tts_decoder_shape* shape, const b200tts_decoder_params* params,

@@ -168,7 +168,7 @@ _scratch = None
 
 
 def ensure_scratch(nbytes=3 << 29):
-    """Device scratch for the tcgen05 GEMM's packed bf16 operands (owned here, handed to the library)."""
+    """Device scratch for the wgmma GEMM's packed bf16 operands (owned here, handed to the library)."""
     global _scratch
     import torch
     if _scratch is None or _scratch.numel() < nbytes:

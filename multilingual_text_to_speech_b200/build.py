@@ -1,4 +1,4 @@
-"""In-tree build of libb200tts.so (hand-written sm_100a CUDA + C ABI).  No torch headers are needed:
+"""In-tree build of libb200tts.so (hand-written sm_90a CUDA + C ABI).  No torch headers are needed:
 the library's boundary is plain C (include/b200tts.h) and the Python host binds it with ctypes.
 
     python -m multilingual_text_to_speech_b200.build [--force]
@@ -13,7 +13,7 @@ ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, 'csrc')
 OBJ = os.path.join(PKG, 'csrc', 'build')
 LIB = os.path.join(PKG, 'libb200tts.so')
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr']
 
 
@@ -42,7 +42,7 @@ def is_stale():
 
 
 def build(force=False, verbose=False):
-    """Compile every .cu under csrc/ for sm_100a and link libb200tts.so next to the package.
+    """Compile every .cu under csrc/ for sm_90a and link libb200tts.so next to the package.
 
     Safe under concurrent callers (torchrun starts one process per GPU, each of which calls build()): an exclusive file lock
     serialises the builders and staleness is re-checked under the lock, so at most one of them compiles."""

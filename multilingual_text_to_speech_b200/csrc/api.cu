@@ -67,8 +67,8 @@ static int require_device() {
         cudaGetLastError();
         return B200TTS_ERR_CUDA;
     }
-    if (prop.major != 10) {
-        set_last_error("device %s is sm_%d%d; b200tts is built for sm_100a only", prop.name, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        set_last_error("device %s is sm_%d%d; b200tts is built for sm_90a only", prop.name, prop.major, prop.minor);
         return B200TTS_ERR_UNSUPPORTED;
     }
     cached = 1;
@@ -441,7 +441,7 @@ int b200tts_fill_keep_mask(uint8_t* mask, size_t n, float drop_rate, uint64_t se
     const unsigned threshold = (unsigned)(drop_rate * 65536.0f + 0.5f);
     const unsigned long long key = mix64(seed ^ 0xD6E8FEB86659FD93ull) ^ (stream_id * 0xA24BAED4963EE407ull);
     size_t quads = (n + 15) / 16;
-    int blocks = (int)((quads + 255) / 256 > 148 * 16 ? 148 * 16 : (quads + 255) / 256);
+    int blocks = (int)((quads + 255) / 256 > NUM_SMS * 16 ? NUM_SMS * 16 : (quads + 255) / 256);
     if (blocks < 1) blocks = 1;
     fill_keep_mask_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(mask, n, threshold, key, g_mask_epoch);
     B200_LAUNCH_CHECK();

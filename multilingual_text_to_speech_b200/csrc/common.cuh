@@ -1,4 +1,4 @@
-// Shared device/host helpers for the b200tts hot-path library (sm_100a only).
+// Shared device/host helpers for the b200tts hot-path library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -43,6 +43,9 @@ struct KernelTimer {
     KernelTimer(const char* n, cudaStream_t s) : name(n), st(s) { ktimer_start(n, s); }
     ~KernelTimer() { ktimer_stop(name, st); }
 };
+
+// SMs of the H100 SXM the library is built for: grid sizes of the grid-stride kernels and the co-residency limit of the persistent loops
+constexpr int NUM_SMS = 132;
 
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 static inline size_t align_up_sz(size_t x, size_t a) { return (x + a - 1) / a * a; }
@@ -114,22 +117,22 @@ struct GemmDesc {
     int splitk = 1;
     float* partial = nullptr;     // required when splitk > 1
     int keep_partials = 0;        // 1: leave the reduction to the consumer kernel (C untouched)
-    // optional: op(A) already available as bf16, K contiguous, row stride lda16 elements (16-byte aligned rows): the tcgen05 path
+    // optional: op(A) already available as bf16, K contiguous, row stride lda16 elements (16-byte aligned rows): the wgmma path
     // reads it through TMA directly (no packing pass); A / lda are then ignored by that path
     const void* A16 = nullptr;
     int lda16 = 0;
-    // optional (tcgen05 path, !transB, batch == 1): op(B) = B [K, N] already available as bf16 rows, row stride ldb16 elements (multiple of
+    // optional (wgmma path, !transB, batch == 1): op(B) = B [K, N] already available as bf16 rows, row stride ldb16 elements (multiple of
     // 64, 16-byte aligned base); the columns up to the next multiple of 64 beyond N must be readable (their products are never stored).
     // Read in place through TMA as an MN-major operand: no packing pass
     const void* B16 = nullptr;
     int ldb16 = 0;
-    // optional two-level K (tcgen05 path only; needs !transA && transB): K = kouter * kin, element (row, q * kin + l) of op(A) lives at
+    // optional two-level K (wgmma path only; needs !transA && transB): K = kouter * kin, element (row, q * kin + l) of op(A) lives at
     // A[q * kosA + row * lda + l] (op(B) likewise with kosB): sums a product over `kouter` separately stored slabs in ONE GEMM
     int kin = 0;
     long long kosA = 0, kosB = 0;
 };
 
-// pack cache of the tcgen05 GEMM (gemm_tc.cu): operands packed inside a begin / end scope are reused by later products of the scope
+// pack cache of the wgmma GEMM (gemm_tc.cu): operands packed inside a begin / end scope are reused by later products of the scope
 void tc_pack_cache_begin();
 void tc_pack_cache_end();
 

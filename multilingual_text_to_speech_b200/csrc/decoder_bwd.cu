@@ -11,7 +11,7 @@ namespace {
 
 inline int grid_for(size_t n) {
     size_t g = (n + 255) / 256;
-    return (int)(g > 148 * 16 ? 148 * 16 : (g < 1 ? 1 : g));
+    return (int)(g > NUM_SMS * 16 ? NUM_SMS * 16 : (g < 1 ? 1 : g));
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -527,7 +527,7 @@ int launch_attn_bwd(AttnBwdArgs a, cudaStream_t st) {
 // ---------------------------------------------------------------------------------------------
 struct BwdLayout {
     size_t dfs, dhgd, dctxs, dgg, dhas, dga, dq, dctxt, dcum, dc, dhz, dmemT, dWloc_acc, dWc_acc, dv_acc, dp1, dp0, dwfs,
-        part, gpart, pextra, pextra2, dggb, dgab, total;      // dggb / dgab: bf16 [T, B, 4D] histories of the gate gradients (tcgen05 loops)
+        part, gpart, pextra, pextra2, dggb, dgab, total;      // dggb / dgab: bf16 [T, B, 4D] histories of the gate gradients (wgmma loops)
     int split_gen, split_att;
     size_t gpart_elems;
 };
@@ -585,7 +585,7 @@ int wgemm(cudaStream_t st, const BwdLayout& l, float* ws, int transA, int transB
     return gemm_run_auto(d, ws + l.gpart, l.gpart_elems, st);
 }
 // weight gradient dW (+)= A^T . B with A [K, M] fp32 and B [K, N] fp32; B16 (optional) = the same B as bf16 rows (row stride ldb16) that
-// the persistent forward loops left behind: read in place by the tcgen05 path (MN-major TMA operand), no conversion pass
+// the persistent forward loops left behind: read in place by the wgmma path (MN-major TMA operand), no conversion pass
 int wgemm16(cudaStream_t st, const BwdLayout& l, float* ws, int M, int N, int K, const float* A, int lda, const float* B, int ldb,
             const void* B16, int ldb16, float* C, int ldc, float beta, const void* A16 = nullptr, int lda16 = 0) {
     GemmDesc d;
@@ -608,7 +608,7 @@ size_t decoder_bwd_workspace_floats(const b200tts_decoder_shape& s) { return bwd
 // byte offset of the phase counters of the persistent backward kernels inside the backward workspace (0: generator, 1: attention)
 size_t decoder_bwd_profile_offset(const b200tts_decoder_shape& s, int which) {
     const BwdLayout l = bwd_layout(s);
-    if (which == 0) return l.pextra * sizeof(float) + persist_bwd_gen_extra_bytes(s) - 148 * 8 * 8;
+    if (which == 0) return l.pextra * sizeof(float) + persist_bwd_gen_extra_bytes(s) - NUM_SMS * 8 * 8;
     return l.pextra2 * sizeof(float) + att_bwd_extra(s).barrier + 256;
 }
 
@@ -668,7 +668,7 @@ int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_
     auto W = [&](size_t off) { return bws + off; };
     const float* ai = F(fl.ai);                // [T+1, B, M+D]
     const float* ai1 = ai + (size_t)B * MD;    // rows 1..T
-    // bf16 operand rows the tcgen05 forward loops left in the persistent workspace: aib [T+1, B, Kp_att] = [h_att | ctx | 0], hgb [T+1, B, Kp_gen]
+    // bf16 operand rows the wgmma forward loops left in the persistent workspace: aib [T+1, B, Kp_att] = [h_att | ctx | 0], hgb [T+1, B, Kp_gen]
     // = h_gen (row i+1 = state after step i, row 0 = 0).  The weight-gradient products read them in place (MN-major TMA operands).
     const bool tc_rows = precision_mode() == B200TTS_PRECISION_BF16 && s.training && tc_persist_supported(s) && persist_att_bwd_supported(s);
     const PersistLayout prl = persist_layout(s);
@@ -698,14 +698,14 @@ int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_
 
     // ---- 2. generator LSTM reverse loop ----
     const bool zone = s.cell_kind == B200TTS_CELL_ZONEOUT;
-    // the tcgen05 reverse loops keep their bf16 gate gradients as [T, B, 4D] histories: the time-batched products below read them in place
+    // the wgmma reverse loops keep their bf16 gate gradients as [T, B, 4D] histories: the time-batched products below read them in place
     // (K-major for dX, MN-major for dW) instead of converting the fp32 copies
     const bool hist_gen = precision_mode() == B200TTS_PRECISION_BF16 && persist_bwd_supported(s) && tc_persist_gen_bwd_supported(s) &&
                           !getenv("B200TTS_NO_DGB_HISTORY");
     void* dggb = hist_gen ? static_cast<void*>(W(l.dggb)) : nullptr;
     if (precision_mode() == B200TTS_PRECISION_BF16 && persist_bwd_supported(s)) {
         // bf16 perf mode: one cooperative weight-stationary kernel for the whole reverse recurrence
-        if (tc_persist_gen_bwd_supported(s))      // TMA + tcgen05 + TMEM variant (decoder_persist_bwd_tc.cu)
+        if (tc_persist_gen_bwd_supported(s))      // TMA + wgmma variant (decoder_persist_bwd_tc.cu)
             B200_TRY(tc_persist_gen_bwd_loop(s, w, in, fl, fws, W(l.dhgd), W(l.dgg), reinterpret_cast<unsigned char*>(W(l.pextra)), st, dggb));
         else
             B200_TRY(persist_gen_bwd_loop(s, w, in, fl, fws, W(l.dhgd), W(l.dgg), reinterpret_cast<unsigned char*>(W(l.pextra)), st));
@@ -734,7 +734,7 @@ int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_
     }
     {
         // time-batched generator gradients.  The gate gradients are final now: their packed (transposed / K-contiguous) bf16 copies are
-        // made once and shared by the three weight-gradient and the two input-gradient products (pack cache of the tcgen05 GEMM).
+        // made once and shared by the three weight-gradient and the two input-gradient products (pack cache of the wgmma GEMM).
         PackScope pack_scope;
         B200_TRY(wgemm16(st, l, bws, 4 * D, D, (int)TB, W(l.dgg), 4 * D, F(fl.hg), D, hgb, ldhb, dw.gen_w_hh, D, 1.f, dggb, 4 * D));
         B200_TRY(wgemm16(st, l, bws, 4 * D, D, (int)TB, W(l.dgg), 4 * D, ai1 + M, MD, aib1, ldab, dw.gen_w_ih, D + M, 1.f, dggb, 4 * D));

@@ -336,7 +336,7 @@ int launch_attn_fwd(const AttnFwdArgs& a, cudaStream_t st) {
 
 inline int grid_for(size_t n) {
     size_t g = (n + 255) / 256;
-    return (int)(g > 148 * 16 ? 148 * 16 : (g < 1 ? 1 : g));
+    return (int)(g > NUM_SMS * 16 ? NUM_SMS * 16 : (g < 1 ? 1 : g));
 }
 
 }  // namespace
@@ -543,7 +543,7 @@ int decoder_forward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_p
     if (persistent) {
         // bf16 perf mode: one cooperative, weight-stationary kernel per recurrence (decoder_persist.cu)
         unsigned char* pws = reinterpret_cast<unsigned char*>(c.at(l.persist));
-        const bool tc = tc_persist_supported(s);         // TMA + tcgen05 + TMEM loops (decoder_persist_tc.cu) when D % 64 == 0
+        const bool tc = tc_persist_supported(s);         // TMA + wgmma loops (decoder_persist_tc.cu) when D % 64 == 0
         B200_TRY(persist_att_prep(s, w, in, l, ws, pws, st));
         B200_TRY(tc ? tc_persist_att_loop(s, w, in, l, ws, pws, out.alignments, st) : persist_att_loop(s, w, in, l, ws, pws, out.alignments, st));
         if (tc) {
@@ -552,7 +552,7 @@ int decoder_forward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_p
             const TcPersistGeom g = tc_persist_geom(s);
             const PersistLayout pl = persist_layout(s);
             GemmDesc d;
-            d.A = c.at(l.ai); d.lda = MD;           // (unused by the tcgen05 path)
+            d.A = c.at(l.ai); d.lda = MD;           // (unused by the wgmma path)
             d.A16 = pws + pl.aib + (size_t)B * g.Kp_att * 2; d.lda16 = g.Kp_att;      // operand row 1 (bf16)
             d.B = w.gen_w_ih; d.ldb = D + M; d.transB = 1; d.C = c.at(l.gg); d.ldc = 4 * D; d.bias = c.at(l.bsum_gen);
             d.M = T * B; d.N = 4 * D; d.K = MD; d.beta = 0.f;

@@ -12,7 +12,7 @@ static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; 
 
 static inline int pick_splitk(int M, int N, int K) {
     const int tiles = cdiv(M, 64) * cdiv(N, 64);
-    int s = (148 + tiles / 2) / (tiles > 0 ? tiles : 1);
+    int s = (NUM_SMS + tiles / 2) / (tiles > 0 ? tiles : 1);
     if (s < 1) s = 1;
     if (s > 8) s = 8;
     const int kmax = cdiv(K, 16);
@@ -101,7 +101,7 @@ static inline DecoderLayout decoder_layout(const b200tts_decoder_shape& s) {
 }
 
 int validate_decoder_shape(const b200tts_decoder_shape& s);
-// tcgen05 / TMA persistent forward loops (decoder_persist_tc.cu): operand rows are [h | ctx | 0] in 64-column k-blocks
+// wgmma / TMA persistent forward loops (decoder_persist_tc.cu): operand rows are [h | ctx | 0] in 64-column k-blocks
 struct TcPersistGeom { int Kp_att, Kp_gen, nkb_att, nkb_gen, nkb_h, ch_c_att, n_c_att, alias_att, ch_h_att, slot_att, ch_h_gen, slot_gen; };
 TcPersistGeom tc_persist_geom(const b200tts_decoder_shape& s);
 bool tc_persist_supported(const b200tts_decoder_shape& s);
@@ -117,7 +117,7 @@ int persist_att_loop(const b200tts_decoder_shape& s, const b200tts_decoder_param
 struct AttBwdExtra { int MT; size_t dgb, part, wcb, wcb2, memTf, de, dwpart, dvpart, barrier, total; };
 AttBwdExtra att_bwd_extra(const b200tts_decoder_shape& s);
 bool persist_att_bwd_supported(const b200tts_decoder_shape& s);
-bool persist_att_bwd_tc(const b200tts_decoder_shape& s);      // true: the tcgen05 product variant is the one picked
+bool persist_att_bwd_tc(const b200tts_decoder_shape& s);      // true: the wgmma product variant is the one picked
 int persist_att_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
                          const DecoderLayout& fl, const float* fws, const PersistLayout& pl, const unsigned char* pws,
                          const float* align, const float* dalign, const float* dh_static, const float* dctx_static, float* dgates,

@@ -615,7 +615,7 @@ __global__ void wcomb_kernel(float* __restrict__ WcombT, const float* __restrict
 
 inline int grid_for(size_t n) {
     size_t g = (n + 255) / 256;
-    return (int)(g > 148 * 16 ? 148 * 16 : (g < 1 ? 1 : g));
+    return (int)(g > NUM_SMS * 16 ? NUM_SMS * 16 : (g < 1 ? 1 : g));
 }
 
 }  // namespace
@@ -631,7 +631,7 @@ PersistLayout persist_layout(const b200tts_decoder_shape& s) {
     l.Kp_att = (s.M + s.D + 15) / 16 * 16;
     l.Kp_gen = (s.D + 15) / 16 * 16;
     l.ldm = (s.M + 7) / 8 * 8;
-    // sized for the 64-column k-block padding of the tcgen05 loops (decoder_persist_tc.cu) as well
+    // sized for the 64-column k-block padding of the wgmma loops (decoder_persist_tc.cu) as well
     l.aib = take((T + 1) * B * (size_t)((s.M + s.D + 63) / 64 * 64) * 2);
     l.hgb = take((T + 1) * B * (size_t)((s.D + 63) / 64 * 64) * 2);
     l.memTb = take(B * (size_t)s.L * s.A * 2);
@@ -643,7 +643,7 @@ PersistLayout persist_layout(const b200tts_decoder_shape& s) {
     l.M16 = (s.M + 15) / 16;
     l.memFf = take((size_t)s.B * l.M16 * l.MT * 32 * 16);
     l.memFb = take((size_t)s.B * l.M16 * l.MT * 32 * 16);
-    l.barrier = take(256 + 148 * 8 * 8 * 4);   // barrier + abort flag, then 4 x [148][8] profile counters (att, gen, att roles, gen roles)
+    l.barrier = take(256 + NUM_SMS * 8 * 8 * 4);   // barrier + abort flag, then 4 x [NUM_SMS][8] profile counters (att, gen, att roles, gen roles)
     l.total = off;
     return l;
 }
@@ -651,7 +651,7 @@ PersistLayout persist_layout(const b200tts_decoder_shape& s) {
 bool persist_supported(const b200tts_decoder_shape& s) {
     if (s.D % UNITS != 0) return false;
     const int RB = s.D / UNITS, NBH = (s.B + BT - 1) / BT;
-    if (RB * NBH > 148 || s.B > RB * NBH) return false;
+    if (RB * NBH > NUM_SMS || s.B > RB * NBH) return false;
     const PersistLayout l = persist_layout(s);
     if (s.K > 32) return false;
     const size_t a = loop_smem_bytes(l.Kp_att, s.A, true, s.L, s.M, ATT_STAGES), g = loop_smem_bytes(l.Kp_gen, s.A, false, 0, 0, GEN_STAGES);
@@ -688,9 +688,9 @@ int persist_att_prep(const b200tts_decoder_shape& s, const b200tts_decoder_param
     B200_LAUNCH_CHECK();
     __nv_bfloat16* wcb = reinterpret_cast<__nv_bfloat16*>(pws + l.wcb);
     __nv_bfloat16* memTf = reinterpret_cast<__nv_bfloat16*>(pws + l.memTf);
-    att_prep_kernel<<<148 * 4, 256, 0, st>>>(wcb, memTf, wcombT, ws + fl.memT, B, s.L, s.A, s.K, l.MT);
+    att_prep_kernel<<<NUM_SMS * 4, 256, 0, st>>>(wcb, memTf, wcombT, ws + fl.memT, B, s.L, s.A, s.K, l.MT);
     B200_LAUNCH_CHECK();
-    mem_frag_kernel<<<148 * 4, 256, 0, st>>>(reinterpret_cast<uint4*>(pws + l.memFf), reinterpret_cast<uint4*>(pws + l.memFb), in.memory, B,
+    mem_frag_kernel<<<NUM_SMS * 4, 256, 0, st>>>(reinterpret_cast<uint4*>(pws + l.memFf), reinterpret_cast<uint4*>(pws + l.memFb), in.memory, B,
                                              s.L, M, l.M16, l.MT);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
@@ -743,7 +743,7 @@ int persist_gen_loop(const b200tts_decoder_shape& s, const b200tts_decoder_param
     a.gates = ws + fl.gg; a.cstate = ws + fl.cg;
     a.mask_h = in.mask_gen_h; a.mask_c = in.mask_gen_c; a.kind = s.cell_kind; a.training = s.training; a.rate_h = s.rate_h; a.rate_c = s.rate_c;
     a.barrier = barrier; a.abort_flag = reinterpret_cast<int*>(barrier + 32);
-    a.prof = reinterpret_cast<long long*>(pws + l.barrier + 256) + 148 * 8;
+    a.prof = reinterpret_cast<long long*>(pws + l.barrier + 256) + NUM_SMS * 8;
     return launch_loop(false, a, loop_smem_bytes(l.Kp_gen, s.A, false, 0, 0, GEN_STAGES), st);
 }
 

@@ -272,12 +272,11 @@ __global__ void __launch_bounds__(PT, 1) lstm_bwd_loop_kernel(const BwdLoopArgs 
 constexpr int KBA = 8;            // K-blocks of the attention-loop product (over hidden units)
 constexpr int NBA = 9;            // N-blocks over the M + D output columns  -> 8 x 9 x 2 = 144 CTAs
 constexpr int GLD = 33;           // row stride of the G tile buffer (floats)
-// tcgen05 variant of the product: CTA (kb, nb) of 8 x 18 keeps W^T[n-block of 80 outputs, K-slice kb] as K-major SWIZZLE_128B tiles (UMMA B
+// wgmma variant of the product: CTA (kb, nb) of 8 x 16 keeps W^T[n-block of 80 outputs, K-slice kb] as K-major SWIZZLE_128B tiles (wgmma B
 // operand, N = 80); the whole batch (<= 64 utterances, TMA zero-fills the rest) is the A operand (M = 64), ONE 5-D TMA box per step
-constexpr int NBT = 18;           // n-blocks of the tcgen05 variant  -> 8 x 18 = 144 CTAs (72 pairs)
-constexpr int TUN = 80;           // outputs per n-block (UMMA N); TUN_WIDE when M + D > NBT * TUN (memory dim 512)
+constexpr int NBT = 16;           // n-blocks of the wgmma variant  -> 8 x 16 = 128 CTAs (64 pairs): one per SM of the 132
+constexpr int TUN = 80;           // outputs per n-block (wgmma N); TUN_WIDE when M + D > NBT * TUN (memory dim 512)
 constexpr int TUN_WIDE = 96;
-constexpr int TMEM_COLS_ATT = 128;
 
 struct AttBwdArgs {
     int B, T, D, M, L, A, KC, NOUT, UK, UN, NBH, MT;      // NOUT = M + D, MT = ceil(L / 16)
@@ -334,13 +333,12 @@ __device__ __forceinline__ void build_pairs(uint32_t* Ph, uint32_t* Pl, const fl
     }
 }
 
-// UNC: outputs per n-block of the tcgen05 product (UMMA N), compile-time (80, or 96 for memory dim 512); 0 for the mma.sync variant
+// UNC: outputs per n-block of the wgmma product (wgmma N), compile-time (80, or 96 for memory dim 512); 0 for the mma.sync variant
 template <bool TC, int UNC>
 __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_constant__ CUtensorMap tmG, const AttBwdArgs p) {
     extern __shared__ __align__(1024) unsigned char smem_raw0[];
     unsigned char* smem_raw = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw0) + 1023) & ~(uintptr_t)1023);
-    __shared__ uint64_t full_bar, accum_bar, xb1, xb2;      // xb1 / xb2: arrival of the peer's softmax dot / query-gradient partial + G halo tile
-    __shared__ uint32_t tmem_base_s;
+    __shared__ uint64_t full_bar, xb1, xb2;      // xb1 / xb2: arrival of the peer's softmax dot / query-gradient partial + G halo tile
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int cta = blockIdx.x;
     const int kb = cta % KBA, nb = TC ? cta / KBA : (cta / KBA) % NBA, bh = TC ? 0 : cta / (KBA * NBA);
@@ -348,7 +346,7 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
     const int WLD = UN + 8, ALD = KROWS + 8;
     const int b0 = bh * BT, n0 = nb * UN;
     const int NKT = KROWS / 64;                                                      // TC: k-block tiles of the K-slice
-    // mma.sync: Ws [KROWS][WLD] bf16, As [BT][ALD] bf16.  tcgen05: sW [NKT][UN rows][128 B] swizzled, slot [NKT][64 rows][128 B] (one TMA box).
+    // mma.sync: Ws [KROWS][WLD] bf16, As [BT][ALD] bf16.  wgmma: sW [NKT][UN rows][128 B] swizzled, slot [NKT][64 rows][128 B] (one TMA box).
     // The activation stage `As` doubles as the attention scratch / query-gradient staging in both variants.
     __nv_bfloat16* Ws = reinterpret_cast<__nv_bfloat16*>(smem_raw);
     unsigned char* sW = smem_raw;
@@ -382,18 +380,14 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
     const int uo0 = cta * UOWN;
     if (owner)
         for (int idx = tid; idx < A * UOWN; idx += PT) wq8[(idx / UOWN) * (UOWN + 1) + idx % UOWN] = p.Wq[(size_t)(idx / UOWN) * D + uo0 + idx % UOWN];
-    uint32_t tmem_base = 0, prod_it = 0;
+    uint32_t prod_it = 0;
     if (tid == 0) { tcx::mbar_init(&xb1, 1); tcx::mbar_init(&xb2, 1); tcx::mbar_init_fence(); }
     if (TC) {
-        if (tid == 0) { tcx::mbar_init(&full_bar, 1); tcx::mbar_init(&accum_bar, 1); tcx::mbar_init_fence(); }
-        if (warp == 1) tcx::tmem_alloc<TMEM_COLS_ATT>(&tmem_base_s);
-        tcx::proxy_fence_shared();           // the weight tiles were written through the generic proxy; tcgen05.mma reads them through the async proxy
-        tcx::tc_fence_before();
+        if (tid == 0) { tcx::mbar_init(&full_bar, 1); tcx::mbar_init_fence(); }
+        tcx::proxy_fence_shared();           // the weight tiles were written through the generic proxy; wgmma reads them through the async proxy
     }
     __syncthreads();
     cluster_arrive(); cluster_wait();      // one-time: the peer's exchange mbarriers are initialised before the first remote st.async targets them
-    if (TC) { tcx::tc_fence_after(); tmem_base = tmem_base_s; }
-    const uint32_t idesc = tcx::make_idesc_bf16(64, UNC);
 
     const float inv_h = 1.f / (1.f - p.rate_h), inv_c = 1.f / (1.f - p.rate_c);
     constexpr int MAXE = 3;               // (b, u) pairs per thread: B * 8 / 256 <= 3 for B <= 64... (B <= 96)
@@ -859,7 +853,7 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
         // =========================== P2: [d ctx | d h](i-1) partial = dgates_i[:, kb] . W[kb, nb] ===========================
         if (TC) {
             // TMA: the bf16 gate gradients of the K-slice, all utterances (rows >= B zero-filled), as NKT swizzled [64 x 64] tiles in ONE box;
-            // tcgen05: D[b, n] (TMEM, 64 lanes x 80 columns) = sum over the tiles; warp 0 issues (elected lane), everybody drains TMEM
+            // wgmma: D[b, n] (registers of warpgroup 0: 64 utterances x UN outputs) = sum over the tiles, stored straight to the partials
             if (warp == 0) {
                 if (tcx::elect_one()) {
                     tcx::proxy_fence_shared();       // the slot was last touched through the generic proxy (attention scratch, dq staging)
@@ -868,43 +862,34 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
                     tcx::tma_load_5d(As, &tmG, &full_bar, 0, i * p.dgb_rows, 0, kb, 0);
                 }
                 __syncwarp();
+            }
+            if (warp < 4) {
+                constexpr int NR = UNC > 0 ? UNC / 2 : 1;
+                float acc[NR];
                 tcx::mbar_wait(&full_bar, prod_it & 1);
-                tcx::tc_fence_after();
-                if (tcx::elect_one()) {
-                    for (int c = 0; c < NKT; ++c) {
-                        const uint64_t adesc = tcx::make_sw128_desc(tcx::smem_u32(reinterpret_cast<unsigned char*>(As) + (size_t)c * 8192));
-                        const uint64_t bdesc = tcx::make_sw128_desc(tcx::smem_u32(sW + (size_t)c * UN * 128));
+                tcx::wgmma_fence();
+                for (int c = 0; c < NKT; ++c) {
+                    const uint64_t adesc = tcx::make_sw128_desc(tcx::smem_u32(reinterpret_cast<unsigned char*>(As) + (size_t)c * 8192));
+                    const uint64_t bdesc = tcx::make_sw128_desc(tcx::smem_u32(sW + (size_t)c * UN * 128));
 #pragma unroll
-                        for (int k = 0; k < 4; ++k) tcx::umma_bf16(tmem_base, adesc + 2 * k, bdesc + 2 * k, idesc, (c == 0 && k == 0) ? 0u : 1u);
+                    for (int k = 0; k < 4; ++k) {
+                        if constexpr (UNC == TUN_WIDE) tcx::wgmma_m64n96<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (c | k) != 0);
+                        else if constexpr (UNC == TUN) tcx::wgmma_m64n80<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (c | k) != 0);
                     }
-                    tcx::umma_commit(&accum_bar);
                 }
-                __syncwarp();
+                tcx::wgmma_commit();
+                tcx::wgmma_wait<0>();
+                tcx::wgmma_fence_acc(acc);
+                // fragment: utterance b = 16 warp + lane / 4 + 8 ((r / 2) % 2), output n0 + 8 (r / 4) + 2 (lane % 4) + r % 2 (NOUT % 4 == 0: a pair
+                // is either wholly inside or wholly outside)
+                const int brow = 16 * warp + (lane >> 2), ncol = n0 + 2 * (lane & 3);
+#pragma unroll
+                for (int r = 0; r < NR; r += 2) {
+                    const int b = brow + 8 * ((r >> 1) & 1), n = ncol + 8 * (r >> 2);
+                    if (b < B && n < p.NOUT) *reinterpret_cast<float2*>(p.part + ((size_t)kb * B + b) * p.NOUT + n) = make_float2(acc[r], acc[r + 1]);
+                }
             }
-            tcx::mbar_wait(&accum_bar, prod_it & 1);
-            tcx::tc_fence_after();
             ++prod_it;
-            {   // M = 64 accumulator layout: utterance b sits in TMEM lane (b / 16) * 32 + b % 16; warp = (quadrant, half of the UN = 80 / 96 columns)
-                constexpr int hc = UNC / 2, NJ = hc / 8;
-                const int q = warp & 3, ch = warp >> 2;
-                uint32_t r[NJ > 0 ? NJ : 1][8];
-#pragma unroll
-                for (int j = 0; j < NJ; ++j) tcx::tmem_ld8(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(ch * hc + j * 8), r[j]);
-                tcx::tmem_ld_wait();
-                const int b = q * 16 + lane;
-                if (lane < 16 && b < B) {
-                    float* dst = p.part + ((size_t)kb * B + b) * p.NOUT + n0 + ch * hc;
-#pragma unroll
-                    for (int j = 0; j < NJ; ++j)
-#pragma unroll
-                        for (int h4 = 0; h4 < 2; ++h4)
-                            if (n0 + ch * hc + j * 8 + h4 * 4 < p.NOUT)         // NOUT % 4 == 0 (checked on the host)
-                                *reinterpret_cast<float4*>(dst + j * 8 + h4 * 4) =
-                                    make_float4(__uint_as_float(r[j][h4 * 4]), __uint_as_float(r[j][h4 * 4 + 1]), __uint_as_float(r[j][h4 * 4 + 2]),
-                                                __uint_as_float(r[j][h4 * 4 + 3]));
-                }
-                tcx::tc_fence_before();
-            }
         } else {
             const int segs = UK / 8;
             for (int idx = tid; idx < BT * 4 * segs; idx += PT) {
@@ -955,11 +940,6 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
         BPROF_MARK(6);
     }
     BPROF_FLUSH;
-    if (TC) {
-        tcx::tc_fence_before();
-        __syncthreads();
-        if (warp == 1) tcx::tmem_dealloc<TMEM_COLS_ATT>(tmem_base);
-    }
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -1224,7 +1204,7 @@ AttBwdExtra att_bwd_extra(const b200tts_decoder_shape& s) {
     x.de = take((size_t)s.T * s.B * s.L * 4);
     x.dwpart = take((size_t)s.B * x.MT * s.A * 32 * 4);
     x.dvpart = take((size_t)s.B * x.MT * s.A * 4);
-    x.barrier = take(256 + 148 * 8 * 8);
+    x.barrier = take(256 + NUM_SMS * 8 * 8);
     x.total = off;
     return x;
 }
@@ -1256,7 +1236,7 @@ static bool att_bwd_variant_ok(const b200tts_decoder_shape& s, const AttBwdGeom&
     if (s.A != 128 || s.K > 32 || s.B * 8 > 3 * PT || s.D % KBA != 0) return false;
     if (s.M > 2 * PT || (s.L + 15) / 16 * 16 + 48 > 2 * PT || s.B * (s.A / 4) > 8 * PT) return false;      // register-slot staging of the attention backward
     if (s.D / 8 > g.grid) return false;                       // cell-backward ownership: 8 hidden units per CTA
-    if (g.grid / 2 < s.B || g.grid > 148) return false;       // one CTA pair per utterance, all CTAs co-resident
+    if (g.grid / 2 < s.B || g.grid > NUM_SMS) return false;       // one CTA pair per utterance, all CTAs co-resident
     if (g.tc) {
         if (g.UK % 64 != 0 || s.B > 64 || s.M + s.D > NBT * g.UN || (s.M + s.D) % 4 != 0) return false;
     } else {
@@ -1322,7 +1302,7 @@ int persist_att_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_p
     a.prof = reinterpret_cast<long long*>(extra + x.barrier + 256);
     const float* wcombT = reinterpret_cast<const float*>(pws + pl.wcombT);
     B200_CUDA(cudaMemsetAsync(a.barrier, 0, 256, st));
-    att_bwd_prep_kernel<<<148 * 4, 256, 0, st>>>(wcb, wcb2, memTf, wcombT, fws + fl.memT, B, L, A, s.K, x.MT);
+    att_bwd_prep_kernel<<<NUM_SMS * 4, 256, 0, st>>>(wcb, wcb2, memTf, wcombT, fws + fl.memT, B, L, A, s.K, x.MT);
     B200_LAUNCH_CHECK();
     const size_t smem = geo.smem;
     void* fn = geo.tc ? (geo.UN == TUN ? (void*)att_bwd_loop_kernel<true, TUN> : (void*)att_bwd_loop_kernel<true, TUN_WIDE>)
@@ -1350,7 +1330,7 @@ int persist_att_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_p
     cudaLaunchAttribute attrs[2];
     attrs[0].id = cudaLaunchAttributeCooperative;
     // profiling aid: ncu cannot capture a launch that is BOTH cooperative and clustered; the kernel carries its own grid barrier, so on an
-    // otherwise idle GPU (all CTAs resident: <= 148, one per SM) the cooperative attribute can be dropped for a capture
+    // otherwise idle GPU (all CTAs resident: <= NUM_SMS, one per SM) the cooperative attribute can be dropped for a capture
     attrs[0].val.cooperative = getenv("B200TTS_PROFILE_NO_COOP") ? 0 : 1;
     attrs[1].id = cudaLaunchAttributeClusterDimension;          // the attention backward of an utterance runs on a CTA pair
     attrs[1].val.clusterDim.x = 2; attrs[1].val.clusterDim.y = 1; attrs[1].val.clusterDim.z = 1;
@@ -1390,7 +1370,7 @@ int persist_att_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_p
 
 size_t persist_bwd_gen_extra_bytes(const b200tts_decoder_shape& s) {
     // dgb [B, 4D] bf16 + part [KB, B, D] fp32 + barrier
-    return ((size_t)s.B * 4 * s.D * 2 + 255) / 256 * 256 + ((size_t)KB * s.B * s.D * 4 + 255) / 256 * 256 + 256 + 148 * 8 * 8;
+    return ((size_t)s.B * 4 * s.D * 2 + 255) / 256 * 256 + ((size_t)KB * s.B * s.D * 4 + 255) / 256 * 256 + 256 + NUM_SMS * 8 * 8;
 }
 
 // dgates for all T steps of the generator LSTM.  `extra` = persist_bwd_gen_extra_bytes scratch.

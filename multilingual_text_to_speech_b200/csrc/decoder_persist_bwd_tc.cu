@@ -1,19 +1,20 @@
-// Persistent generator-LSTM BACKWARD loop of the bf16 perf mode on TMA + tcgen05 + TMEM (sm_100a).
+// Persistent generator-LSTM BACKWARD loop of the bf16 perf mode on TMA + wgmma (sm_90a).
 //
 // Reverse step i needs  d h_{i-1}[b, n] = sum_r dgates_i[b, r] . W_hh[r, n]  (r over the 4D gate rows): the transpose of the forward
 // product.  CTA (gate g, n-block nb, batch half bh) keeps W_hh^T[n-block (64 outputs), gate g (D rows of K)] in shared memory as
 // K-major SWIZZLE_128B tiles (A operand, M = 64); per step ONE TMA box brings the bf16 gate gradients [32 utterances x D] of its
-// gate (B operand, N = 32); D / 16 tcgen05 MMAs accumulate in TMEM; the epilogue stores the fp32 partial [gate][b][n] that the next
-// step's cell backward sums over the 4 gates (fixed order, no atomics).  Per step:
+// gate (B operand, N = 32); D / 16 wgmma instructions accumulate in registers; the fp32 partial [gate][b][n] that the next
+// step's cell backward sums over the 4 gates (fixed order, no atomics) is stored straight from them.  Per step:
 //   P1  cell backward of this CTA's 16 hidden units x 32 utterances (operands prefetched during the previous product)
 //   --  grid barrier (gate gradients of all units visible)
-//   P2  TMA + tcgen05 product, TMEM -> partial store
+//   P2  TMA + wgmma product, registers -> partial store
 //   --  grid barrier.
-// Warp roles as in decoder_persist_tc.cu: warps 0-7 compute, warp 8 = TMA producer, warp 9 = MMA issuer (one elected lane each).
+// Warp roles as in decoder_persist_tc.cu: warps 0-7 compute, warps 8-11 = the MMA warpgroup (an elected lane of warp 8 issues the TMA).
 // Reference semantics: autograd replay of modules/layers.py:18-47 (train.py:83).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include "decoder_internal.cuh"
+#include "tc_ptx.cuh"
 
 namespace b200tts {
 
@@ -23,14 +24,13 @@ namespace {
 
 constexpr int NCW = 8;
 constexpr int CT = 32 * NCW;
-constexpr int PT = CT + 64;
+constexpr int PT = CT + 128;            // + the MMA warpgroup
 constexpr int UNITS = 16;               // hidden units of the cell backward per CTA
 constexpr int ROWS = 64;                // outputs (n) per CTA = MMA M
 constexpr int BT = 32;                  // utterances per CTA = MMA N
 constexpr int KB = 64;
 constexpr int WTILE = ROWS * KB * 2;
 constexpr int ATILE = BT * KB * 2;
-constexpr int TMEM_COLS = 32;
 constexpr int NG = 4;                   // gates = K blocks of the product
 
 struct TcBwdArgs {
@@ -79,28 +79,6 @@ __device__ __forceinline__ void tma_load_3d(void* smem, const CUtensorMap* map, 
         ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
         : "memory");
 }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void proxy_fence_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 __device__ __forceinline__ void proxy_fence_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ bool elect_one() {
@@ -121,19 +99,6 @@ __device__ __forceinline__ void st_peer_f32(const float* local_smem, uint32_t pe
 }
 // named barrier among the compute warps only
 __device__ __forceinline__ void csync() { asm volatile("bar.sync 1, %0;" ::"n"(CT) : "memory"); }
-
-// K-major SWIZZLE_128B operand tile (rows of 64 bf16 = 128 B, 8-row groups 1024 B apart): UMMA shared-memory descriptor
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-
-
 
 __device__ __forceinline__ bool grid_barrier(unsigned* counter, unsigned& target, unsigned nblocks, int* abort_flag, int* s_ok) {
     __syncthreads();
@@ -162,8 +127,7 @@ __device__ __forceinline__ bool grid_barrier(unsigned* counter, unsigned& target
 __global__ void __launch_bounds__(PT, 1) lstm_bwd_loop_tc_kernel(const __grid_constant__ CUtensorMap tmG, const TcBwdArgs p) {
     extern __shared__ __align__(1024) unsigned char smem_raw0[];
     unsigned char* smem_raw = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw0) + 1023) & ~(uintptr_t)1023);
-    __shared__ uint64_t full_bar, accum_bar;
-    __shared__ uint32_t tmem_base_s;
+    __shared__ uint64_t full_bar;
     __shared__ int s_ok;
 
     const int tid = threadIdx.x, lane = tid & 31;
@@ -174,11 +138,11 @@ __global__ void __launch_bounds__(PT, 1) lstm_bwd_loop_tc_kernel(const __grid_co
     const int b0 = bh * BT, n0 = nb * ROWS;
     const int u0 = (gsel * NNB + nb) * UNITS;                 // hidden units whose cell backward this CTA owns
     // batch halves are independent (cell backward and product of a CTA serve the same 32 utterances): one barrier counter per half
-    // (per-batch-half barrier counters were measured SLOWER than one grid-wide counter: +0.9 ms on the attention loop; the cost of a
-    // barrier is its latency chain -- store acks, atomic round trip, poll -- not the number of arrivals: tools/microbench/barrier_latency.cu)
+    // (the cost of a barrier is its latency chain -- store acks, atomic round trip, poll -- not the number of arrivals, so one grid-wide
+    // counter is used)
     const unsigned nblocks = gridDim.x;
     unsigned* const bar_counter = p.barrier;
-    const bool compute = warp < NCW, is_producer = warp == NCW, is_mma = warp == NCW + 1;
+    const bool compute = warp < NCW, is_mma = warp >= NCW;
 
     unsigned char* sW = smem_raw;                              // [NNB][64 rows (n)][128 B] swizzled: W^T[n0 + r, gate gsel, k]
     unsigned char* ring = smem_raw + (size_t)NNB * WTILE;      // [NNB][32 rows (b)][128 B] swizzled (one TMA box)
@@ -191,19 +155,11 @@ __global__ void __launch_bounds__(PT, 1) lstm_bwd_loop_tc_kernel(const __grid_co
         *reinterpret_cast<__nv_bfloat16*>(sW + (size_t)kb * WTILE + r * 128 + ((chunk ^ (r & 7)) << 4) + e * 2) = __float2bfloat16_rn(w);
     }
     if (tid == 0) {
-        mbar_init(&full_bar, 1); mbar_init(&accum_bar, 1);
+        mbar_init(&full_bar, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == NCW + 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "n"(TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    proxy_fence_shared();
-    tc_fence_before();
+    proxy_fence_shared();              // the weight tiles were written through the generic proxy; wgmma reads them through the async proxy
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = tmem_base_s;
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BT >> 3) << 17) | ((uint32_t)(ROWS >> 4) << 24);
 
     const float inv_h = 1.f / (1.f - p.rate_h), inv_c = 1.f / (1.f - p.rate_c);
     // cell-backward operands of this thread's two (b, u) pairs, fetched one step ahead (during the previous product)
@@ -303,45 +259,40 @@ __global__ void __launch_bounds__(PT, 1) lstm_bwd_loop_tc_kernel(const __grid_co
         PROF_MARK(1);
         if (i == 0) break;
 
-        // ---------------- P2: partial[gate] = dgates[:, gate block] . W[gate block, n-block]  (TMA + tcgen05) ----------------
-        if (is_producer) {
-            proxy_fence_global();
-            if (elect_one()) {
-                mbar_expect_tx(&full_bar, (uint32_t)NNB * ATILE);
-                tma_load_3d(ring, &tmG, &full_bar, 0, i * p.dgb_rows + b0, gsel * NNB);
-            }
-            __syncwarp();
-        }
+        // ---------------- P2: partial[gate] = dgates[:, gate block] . W[gate block, n-block]  (TMA + wgmma) ----------------
         if (is_mma) {
-            mbar_wait(&full_bar, it & 1);
-            tc_fence_after();
-            if (elect_one()) {
-                for (int c = 0; c < NNB; ++c) {
-                    const uint64_t adesc = make_sw128_desc(smem_u32(sW + (size_t)c * WTILE));
-                    const uint64_t bdesc = make_sw128_desc(smem_u32(ring + (size_t)c * ATILE));
-#pragma unroll
-                    for (int k = 0; k < KB / 16; ++k) umma_bf16(tmem_base, adesc + 2 * k, bdesc + 2 * k, idesc, (c == 0 && k == 0) ? 0u : 1u);
+            if (warp == NCW) {
+                proxy_fence_global();
+                if (elect_one()) {
+                    mbar_expect_tx(&full_bar, (uint32_t)NNB * ATILE);
+                    tma_load_3d(ring, &tmG, &full_bar, 0, i * p.dgb_rows + b0, gsel * NNB);
                 }
-                umma_commit(&accum_bar);
+                __syncwarp();
             }
-            __syncwarp();
+            mbar_wait(&full_bar, it & 1);
+            float acc[16];                   // the first instruction overwrites (scale-d = 0)
+            tcx::wgmma_fence();
+            for (int c = 0; c < NNB; ++c) {
+                const uint64_t adesc = tcx::make_sw128_desc(smem_u32(sW + (size_t)c * WTILE));
+                const uint64_t bdesc = tcx::make_sw128_desc(smem_u32(ring + (size_t)c * ATILE));
+#pragma unroll
+                for (int k = 0; k < KB / 16; ++k) tcx::wgmma_m64n32<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (c | k) != 0);
+            }
+            tcx::wgmma_commit();
+            tcx::wgmma_wait<0>();
+            tcx::wgmma_fence_acc(acc);
+            // accumulator row = output n0 + row, column = utterance b0 + column (fragment layout: tc_ptx.cuh)
+            const int row = 16 * (warp - NCW) + (lane >> 2), n = n0 + row;
+#pragma unroll
+            for (int r = 0; r < 16; ++r) {
+                const int b = b0 + 8 * (r >> 2) + 2 * (lane & 3) + (r & 1), nn = n + 8 * ((r >> 1) & 1);
+                if (b < B && nn < D) p.part[((size_t)gsel * B + b) * D + nn] = acc[r];
+            }
         }
         if (compute) {
             prefetch(i - 1);                 // operands of the next cell backward: their latency hides behind the product
             prefetch_l2(i - 2);
-            mbar_wait(&accum_bar, it & 1);
-            tc_fence_after();
             PROF_MARK(2);
-            const int q = warp & 3, c0 = (warp >> 2) * 16;
-            uint32_t r[16];
-            tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, r);
-            if (lane < 16) {
-                const int n = n0 + q * 16 + lane;
-#pragma unroll
-                for (int j = 0; j < 16; ++j)
-                    if (b0 + c0 + j < B && n < D) p.part[((size_t)gsel * B + b0 + c0 + j) * D + n] = __uint_as_float(r[j]);
-            }
-            tc_fence_before();
         }
         ++it;
         PROF_MARK(3);
@@ -351,11 +302,6 @@ __global__ void __launch_bounds__(PT, 1) lstm_bwd_loop_tc_kernel(const __grid_co
     if (p.prof && tid == 0)
         for (int k = 0; k < 8; ++k) p.prof[(size_t)cta * 8 + k] = prof_acc[k];
 #undef PROF_MARK
-    tc_fence_before();
-    __syncthreads();
-    if (warp == NCW + 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS));
-    }
 }
 
 size_t bwd_tc_smem_bytes(int D) { return 1024 + (size_t)(D / KB) * (WTILE + ATILE); }
@@ -365,11 +311,11 @@ size_t bwd_tc_smem_bytes(int D) { return 1024 + (size_t)(D / KB) * (WTILE + ATIL
 bool tc_persist_gen_bwd_supported(const b200tts_decoder_shape& s) {
     if (s.D % KB != 0 || s.D % (NG * (s.D / KB) * UNITS) != 0) return false;       // 4 x D/64 CTAs per batch half x 16 units = D
     const int NBH = (s.B + BT - 1) / BT;
-    if (NG * (s.D / KB) * NBH > 148) return false;
+    if (NG * (s.D / KB) * NBH > NUM_SMS) return false;
     return bwd_tc_smem_bytes(s.D) <= 227 * 1024 - 1088;
 }
 
-// dgates for all T steps of the generator LSTM (tcgen05 variant); `extra` = persist_bwd_gen_extra_bytes scratch (same layout as the
+// dgates for all T steps of the generator LSTM (wgmma variant); `extra` = persist_bwd_gen_extra_bytes scratch (same layout as the
 // mma.sync variant: dgb [B, 4D] bf16, then the partial buffer (4 of its 8 slabs are used), then barrier + profile counters).
 int tc_persist_gen_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
                             const DecoderLayout& fl, const float* fws, const float* dh_static, float* dgates, unsigned char* extra,
@@ -400,7 +346,7 @@ int tc_persist_gen_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decode
     B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, PT, smem));
     B200_CUDA(cudaGetDevice(&dev));
     B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    B200_REQUIRE(per_sm * sms >= grid, "tcgen05 persistent backward: %d CTAs cannot be co-resident", grid);
+    B200_REQUIRE(per_sm * sms >= grid, "wgmma persistent backward: %d CTAs cannot be co-resident", grid);
     void* params[] = {&tm, &a};
     KernelTimer kt("lstm_bwd_loop_tc_kernel", st);
     B200_CUDA(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(PT), params, smem, st));

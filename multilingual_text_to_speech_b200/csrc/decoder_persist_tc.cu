@@ -1,14 +1,14 @@
-// Persistent recurrent kernels of the bf16 perf mode (forward), Blackwell-native: TMA + tcgen05 + TMEM.
+// Persistent recurrent kernels of the bf16 perf mode (forward), Hopper-native: TMA + wgmma + thread-block clusters.
 //
 // ONE cooperative launch runs all T steps of an LSTM recurrence (attention-LSTM + location-sensitive attention, or the
 // generator LSTM).  CTA (rb, bh) owns 16 hidden units x {i,f,g,o} = 64 gate rows and a batch half of 32 utterances:
 //   * weight-stationary: the bf16 slice W[64 rows, K] lives in shared memory for the whole sequence, laid out as
-//     K-major SWIZZLE_128B tiles of 64 x 64 (8 KB) -- the A operand of tcgen05.mma (M = 64);
+//     K-major SWIZZLE_128B tiles of 64 x 64 (8 KB) -- the A operand of wgmma (M = 64);
 //   * per step the bf16 activation operand [32 utterances x K] is fetched by TMA (cp.async.bulk.tensor, 64-column boxes,
-//     SWIZZLE_128B) into a small ring -- the B operand (N = 32); one elected thread issues tcgen05.mma.kind::f16
-//     (K = 16 per instruction), the fp32 accumulator [64 x 32] lives in TMEM; tcgen05.commit recycles ring slots;
-//   * warp roles: warps 0-7 compute (epilogue: tcgen05.ld -> LSTM cell / regulariser -> state stores, attention),
-//     warp 8 lane 0 = TMA producer, warp 9 lane 0 = MMA issuer;
+//     SWIZZLE_128B) into a small ring -- the B operand (N = 32); the MMA warpgroup issues wgmma.mma_async m64n32k16,
+//     the fp32 accumulator [64 x 32] lives in its registers and is staged to shared memory for the epilogue;
+//   * warp roles: warps 0-7 compute (epilogue: LSTM cell / regulariser -> state stores, attention), warps 8-11 = the MMA
+//     warpgroup (an elected lane of warp 8 issues the TMA loads);
 //   * the K range is ordered [h | ctx]: the h part (available after the cell barrier) is loaded and multiplied WHILE
 //     the attention of the same step runs; only the short ctx part (5 boxes) follows the attention barrier;
 //   * grid barriers are monotonic counters in global memory; every wait carries a clock64 watchdog.
@@ -19,6 +19,7 @@
 #include <stdlib.h>
 #include <cuda_bf16.h>
 #include "decoder_internal.cuh"
+#include "tc_ptx.cuh"
 
 namespace b200tts {
 
@@ -29,14 +30,13 @@ namespace {
 
 constexpr int NCW = 8;                  // compute warps
 constexpr int CT = 32 * NCW;            // compute threads
-constexpr int PT = CT + 64;             // + TMA producer warp + MMA issuer warp
+constexpr int PT = CT + 128;            // + the MMA warpgroup (warps 8-11)
 constexpr int UNITS = 16;               // hidden units per CTA
 constexpr int ROWS = 4 * UNITS;         // gate rows per CTA (MMA M)
 constexpr int BT = 32;                  // utterances per CTA (MMA N)
 constexpr int KB = 64;                  // K columns per tile / TMA box (128-byte rows)
 constexpr int WTILE = ROWS * KB * 2;    // 8 KB
 constexpr int ATILE = BT * KB * 2;      // 4 KB
-constexpr int TMEM_COLS = 32;
 
 struct TcLoopArgs {
     int B, T, D, K, Kp, RB, NBH;
@@ -62,7 +62,7 @@ struct TcLoopArgs {
     float* cum; float* align; long long align_bstride;
     unsigned* barrier; int* abort_flag;
     long long* prof;                          // [grid][8] phase cycles seen by compute thread 0
-    long long* prof2;                         // [grid][8] MMA issuer (0-3) / TMA producer (4-7) waits
+    long long* prof2;                         // [grid][8] MMA warpgroup: operand waits / products of the ctx (0, 1) and h (2, 3) parts
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -97,28 +97,6 @@ __device__ __forceinline__ void tma_load_3d(void* smem, const CUtensorMap* map, 
         ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
         : "memory");
 }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void proxy_fence_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 __device__ __forceinline__ void proxy_fence_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ bool elect_one() {
@@ -145,17 +123,6 @@ __device__ __forceinline__ void st_async_peer_f32(const float* local_smem, const
 }
 // named barrier among the compute warps only
 __device__ __forceinline__ void csync() { asm volatile("bar.sync 1, %0;" ::"n"(CT) : "memory"); }
-
-// K-major SWIZZLE_128B operand tile (rows of 64 bf16 = 128 B, 8-row groups 1024 B apart): UMMA shared-memory descriptor
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
 
 __device__ __forceinline__ void ldmatrix_x4(uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3, const void* p) {
     const uint32_t addr = (uint32_t)__cvta_generic_to_shared(p);
@@ -250,8 +217,7 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
                                                              const TcLoopArgs p) {
     extern __shared__ __align__(1024) unsigned char smem_raw0[];
     unsigned char* smem_raw = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw0) + 1023) & ~(uintptr_t)1023);
-    __shared__ uint64_t full_bar, full2_bar, empty_bar, accum_bar, xchg_bar;
-    __shared__ uint32_t tmem_base_s;
+    __shared__ uint64_t full_bar, full2_bar, accum_bar, xchg_bar;
     __shared__ int s_ok;
 
     const int tid = threadIdx.x, lane = tid & 31;
@@ -262,13 +228,12 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
     const int Kp = p.Kp, D = p.D, B = p.B;
     // the two batch halves never exchange data (a CTA's LSTM rows and the attention pairs it hosts serve the same 32 utterances):
     // each half synchronises on its own barrier counter, 64 arrivals instead of 128
-    // (per-batch-half barrier counters were measured SLOWER than one grid-wide counter: +0.9 ms on the attention loop; the cost of a
-    // barrier is its latency chain -- store acks, atomic round trip, poll -- not the number of arrivals: tools/microbench/barrier_latency.cu)
+    // (the cost of a barrier is its latency chain -- store acks, atomic round trip, poll -- not the number of arrivals, so one grid-wide
+    // counter is used)
     const unsigned nblocks = gridDim.x;
     unsigned* const bar_counter = p.barrier;
     const bool compute = warp < NCW;
-    const bool is_producer = (warp == NCW);        // whole warps run the role loops; one elected lane issues the TMA / MMA instructions
-    const bool is_mma = (warp == NCW + 1);
+    const bool is_mma = warp >= NCW;               // the MMA warpgroup; one elected lane of its first warp issues the TMA loads
 
     // ---- shared memory carve-up (1024-byte aligned base: SWIZZLE_128B atoms) ----
     size_t off = 0;
@@ -279,7 +244,7 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
         off += ALIAS ? (ring_b > sum_b ? ring_b : sum_b) : ring_b;
     }
     // accumulator staging [32 utterances][64 gate rows + 1]: its own buffer, or (large memory dims, where the resident weight slice leaves no
-    // room) the TMA slot itself -- between the commit of a step's last MMA and the next TMA issue nobody else touches the slot
+    // room) the TMA slot itself -- between the completion of a step's last MMA and the next TMA issue nobody else touches the slot
     float* s_sum = ALIAS ? reinterpret_cast<float*>(ring) : reinterpret_cast<float*>(smem_raw + off);
     off += ALIAS ? 0 : (size_t)BT * (ROWS + 1) * 4;
     float* s_hs = reinterpret_cast<float*>(smem_raw + off); off += ATT ? (size_t)UNITS * (BT + 4) * 4 : 0;
@@ -299,105 +264,91 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
         for (int idx = tid; idx < (p.A / 2) * 40; idx += PT) sWcB[idx] = p.WcB[(size_t)(cta & 1) * (p.A / 2) * 40 + idx];
     }
     if (tid == 0) {
-        mbar_init(&full_bar, 1); mbar_init(&full2_bar, 1); mbar_init(&empty_bar, 1); mbar_init(&xchg_bar, 1);
-        mbar_init(&accum_bar, 1);
+        mbar_init(&full_bar, 1); mbar_init(&full2_bar, 1); mbar_init(&xchg_bar, 1);
+        mbar_init(&accum_bar, 128);    // every thread of the MMA warpgroup arrives once its accumulator fragment is staged
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == NCW + 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "n"(TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    proxy_fence_shared();              // the weight tiles were written through the generic proxy; tcgen05.mma reads via the async proxy
-    tc_fence_before();
+    proxy_fence_shared();              // the weight tiles were written through the generic proxy; wgmma reads via the async proxy
     __syncthreads();
     if (ATT) { cluster_arrive(); cluster_wait(); }      // one-time: the peer's exchange mbarrier is initialised before any remote st.async targets it
-    tc_fence_after();
-    const uint32_t tmem_base = tmem_base_s;
-    // instruction descriptor: D = F32, A = B = BF16, both K-major, N >> 3 at bit 17, M >> 4 at bit 24
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BT >> 3) << 17) | ((uint32_t)(ROWS >> 4) << 24);
 
     // A TMA instruction costs ~500 cycles of issue time whatever its size (measured), so the operand is fetched with FEW LARGE
     // boxes: the tensor maps are 3-D {64 columns, rows, k-block} (k-block stride 128 B), one instruction brings ch k-blocks
     // of [32 rows x 128 B] = ch swizzled 4 KB tiles into the single ring slot.
-    uint32_t prod_it = 0, cons_it = 0;            // running chunk counters of the producer / MMA thread
-    long long rp[4] = {0, 0, 0, 0};               // role-thread cycle counters (see prof2)
-    // TMA producer: operand row block of `step`; part 0 = ctx k-blocks (one instruction), part 1 = h k-blocks (n_h instructions)
-    auto produce = [&](int step, int part) {
+    uint32_t mma_it = 0;                          // completed phases of full_bar (and of full2_bar: the generator loop uses both once per step)
+    long long rp[4] = {0, 0, 0, 0};               // MMA warpgroup cycle counters (see prof2)
+    float acc[16];                                // accumulator fragment of this MMA-warpgroup thread (fragment layout: tc_ptx.cuh)
+    // MMA warpgroup: acc (+)= W[:, kb] . act[:, kb]^T over the k-blocks of `part` of the operand row block of `step` (part 0 = ctx k-blocks,
+    // part 1 = h k-blocks, which start a new accumulation); signal_accum: stage the finished accumulator in s_sum for the epilogue
+    auto mma_part = [&](int step, int part, bool signal_accum) {
         const long long t0 = clock64();
-        proxy_fence_global();          // generic-proxy writes of other CTAs (ordered by the grid barrier) -> async-proxy reads
-        const long long t1 = clock64();
+        long long t1 = t0;
         const int n = part ? p.n_h : (ALIAS ? p.n_c : 1), ch = part ? p.ch_h : p.ch_c;
         if (!ATT) {
             // generator loop: the whole operand fits in the ring, so its (<= 2) chunks go to their own offsets with their own barriers and
             // are requested back to back -- the MMAs of the first half run while the second half is still in flight.  (All slots are free
             // here: the previous step's MMAs completed before its cell phase, and the grid barrier lies in between.)
-            if (elect_one()) {
-                for (int j = 0; j < n; ++j) {
-                    uint64_t* fb = j ? &full2_bar : &full_bar;
-                    mbar_expect_tx(fb, (uint32_t)ch * ATILE);
-                    tma_load_3d(ring + (size_t)j * ch * ATILE, &tmH, fb, 0, step * B + b0, j * ch);
-                }
-            }
-            __syncwarp();
-            ++prod_it;
-            rp[2 * part] += t1 - t0; rp[2 * part + 1] += clock64() - t1;
-            return;
-        }
-        for (int j = 0; j < n; ++j) {
-            mbar_wait(&empty_bar, (prod_it & 1) ^ 1);
-            if (elect_one()) {
-                if (ALIAS) proxy_fence_shared();           // the slot doubled as the accumulator staging (generic proxy) since its last MMA
-                mbar_expect_tx(&full_bar, (uint32_t)ch * ATILE);
-                tma_load_3d(ring, part ? &tmH : &tmC, &full_bar, 0, step * B + b0, part ? j * ch : p.nkb_h + j * ch);
-            }
-            __syncwarp();
-            ++prod_it;
-        }
-        rp[2 * part] += t1 - t0; rp[2 * part + 1] += clock64() - t1;
-    };
-    // MMA issuer: acc (+)= W[:, kb] . act[:, kb]^T over the k-blocks of the part
-    auto consume = [&](int part, bool signal_accum) {
-        const long long t0 = clock64();
-        long long t1 = t0;
-        const int n = part ? p.n_h : (ALIAS ? p.n_c : 1), ch = part ? p.ch_h : p.ch_c;
-        if (!ATT) {
-            for (int j = 0; j < n; ++j) {
-                mbar_wait(j ? &full2_bar : &full_bar, cons_it & 1);
-                if (j == 0) t1 = clock64();
-                tc_fence_after();
+            if (warp == NCW) {
+                proxy_fence_global();  // generic-proxy writes of other CTAs (ordered by the grid barrier) -> async-proxy reads
                 if (elect_one()) {
-                    for (int c = 0; c < ch; ++c) {
-                        const uint64_t adesc = make_sw128_desc(smem_u32(sW + (size_t)(j * ch + c) * WTILE));
-                        const uint64_t bdesc = make_sw128_desc(smem_u32(ring + (size_t)(j * ch + c) * ATILE));
-#pragma unroll
-                        for (int k = 0; k < KB / 16; ++k) umma_bf16(tmem_base, adesc + 2 * k, bdesc + 2 * k, idesc, (j == 0 && c == 0 && k == 0) ? 0u : 1u);
+                    for (int j = 0; j < n; ++j) {
+                        uint64_t* fb = j ? &full2_bar : &full_bar;
+                        mbar_expect_tx(fb, (uint32_t)ch * ATILE);
+                        tma_load_3d(ring + (size_t)j * ch * ATILE, &tmH, fb, 0, step * B + b0, j * ch);
                     }
-                    if (j == n - 1) umma_commit(&accum_bar);
                 }
                 __syncwarp();
             }
-            ++cons_it;
-            rp[2 * part] += t1 - t0; rp[2 * part + 1] += clock64() - t1;
-            return;
-        }
-        for (int j = 0; j < n; ++j) {
-            mbar_wait(&full_bar, cons_it & 1);
-            if (j == 0) t1 = clock64();
-            tc_fence_after();
-            const int kb0 = part ? j * ch : p.nkb_h + j * ch;
-            if (elect_one()) {
+            for (int j = 0; j < n; ++j) {
+                mbar_wait(j ? &full2_bar : &full_bar, mma_it & 1);
+                if (j == 0) t1 = clock64();
+                tcx::wgmma_fence();
                 for (int c = 0; c < ch; ++c) {
-                    const uint64_t adesc = make_sw128_desc(smem_u32(sW + (size_t)(kb0 + c) * WTILE));
-                    const uint64_t bdesc = make_sw128_desc(smem_u32(ring + (size_t)c * ATILE));
+                    const uint64_t adesc = tcx::make_sw128_desc(smem_u32(sW + (size_t)(j * ch + c) * WTILE));
+                    const uint64_t bdesc = tcx::make_sw128_desc(smem_u32(ring + (size_t)(j * ch + c) * ATILE));
+#pragma unroll
+                    for (int k = 0; k < KB / 16; ++k) tcx::wgmma_m64n32<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (j | c | k) != 0);
+                }
+                tcx::wgmma_commit();
+            }
+            ++mma_it;
+            tcx::wgmma_wait<0>();
+            tcx::wgmma_fence_acc(acc);
+        } else {
+            for (int j = 0; j < n; ++j) {
+                if (warp == NCW) {
+                    if (j == 0) proxy_fence_global();
+                    if (elect_one()) {
+                        if (ALIAS) proxy_fence_shared();   // the slot doubled as the accumulator staging (generic proxy) since its last MMA
+                        mbar_expect_tx(&full_bar, (uint32_t)ch * ATILE);
+                        tma_load_3d(ring, part ? &tmH : &tmC, &full_bar, 0, step * B + b0, part ? j * ch : p.nkb_h + j * ch);
+                    }
+                    __syncwarp();
+                }
+                mbar_wait(&full_bar, mma_it & 1);
+                ++mma_it;
+                if (j == 0) t1 = clock64();
+                const int kb0 = part ? j * ch : p.nkb_h + j * ch;
+                tcx::wgmma_fence();
+                for (int c = 0; c < ch; ++c) {
+                    const uint64_t adesc = tcx::make_sw128_desc(smem_u32(sW + (size_t)(kb0 + c) * WTILE));
+                    const uint64_t bdesc = tcx::make_sw128_desc(smem_u32(ring + (size_t)c * ATILE));
 #pragma unroll
                     for (int k = 0; k < KB / 16; ++k)
-                        umma_bf16(tmem_base, adesc + 2 * k, bdesc + 2 * k, idesc, (part == 1 && j == 0 && c == 0 && k == 0) ? 0u : 1u);
+                        tcx::wgmma_m64n32<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (part == 1 && j == 0 && c == 0 && k == 0) ? 0u : 1u);
                 }
-                umma_commit(&empty_bar);
-                if (signal_accum && j == n - 1) umma_commit(&accum_bar);
+                tcx::wgmma_commit();
+                tcx::wgmma_wait<0>();
+                tcx::wgmma_fence_acc(acc);
+                tcx::wg_sync(NCW / 4);     // the whole warpgroup is done with the slot before the next TMA (or the staging) overwrites it
             }
-            __syncwarp();
-            ++cons_it;
+        }
+        if (signal_accum) {
+            // s_sum[utterance][gate row]: row = 16 (warp - NCW) + lane / 4 + 8 ((r / 2) % 2), utterance = 8 (r / 4) + 2 (lane % 4) + r % 2
+            const int row = 16 * (warp - NCW) + (lane >> 2), col = 2 * (lane & 3);
+#pragma unroll
+            for (int r = 0; r < 16; ++r) s_sum[(8 * (r >> 2) + col + (r & 1)) * (ROWS + 1) + row + 8 * ((r >> 1) & 1)] = acc[r];
+            tcx::mbar_arrive(&accum_bar);
         }
         rp[2 * part] += t1 - t0; rp[2 * part + 1] += clock64() - t1;
     };
@@ -429,9 +380,7 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
     } while (0)
 
     // prologue: the h part of step 0 (operand row 0 is all zeros)
-    if (is_producer) produce(0, 1);
-    if (is_mma) consume(1, !ATT || p.nkb_h == p.nkb);
-    __syncwarp();
+    if (is_mma) mma_part(0, 1, !ATT || p.nkb_h == p.nkb);
 
     // Epilogue operands of this thread's two (b, u) pairs.  The input-projection gates and the keep masks of step i+1 are fetched
     // (from DRAM) right after the cell barrier of step i, i.e. a whole attention phase ahead; c and the regularised h are carried
@@ -482,26 +431,10 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
     bool alive = true;
     for (int i = 0; i < p.T && alive; ++i) {
         // =================== ctx part of the gate product (the context of step i-1 is visible now) ===================
-        if (ATT && p.nkb_h < p.nkb) {
-            if (is_producer) produce(i, 0);
-            if (is_mma) consume(0, true);
-            __syncwarp();
-        }
+        if (ATT && p.nkb_h < p.nkb && is_mma) mma_part(i, 0, true);
         if (compute) {
-            // accumulator [64 gate rows x 32 utterances]: TMEM lane 32 * gate + unit, column = utterance
+            // accumulator [64 gate rows x 32 utterances] staged by the MMA warpgroup: s_sum[utterance][gate * 16 + unit]
             mbar_wait(&accum_bar, i & 1);
-            tc_fence_after();
-            {
-                const int q = warp & 3, c0 = (warp >> 2) * 16;
-                uint32_t r[16];
-                tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, r);
-                if (lane < UNITS) {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) s_sum[(c0 + j) * (ROWS + 1) + q * UNITS + lane] = __uint_as_float(r[j]);
-                }
-            }
-            tc_fence_before();
-            csync();
             PROF_MARK(0);
             // =================== LSTM cell + regulariser (2 (b, u) pairs per thread) ===================
 #pragma unroll
@@ -583,11 +516,9 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
         if (!grid_barrier(bar_counter, target, nblocks, p.abort_flag, &s_ok)) { alive = false; break; }
         PROF_MARK(2);
 
-        // =================== h part of step i+1: TMA + tcgen05 run while the attention of step i is computed ===================
+        // =================== h part of step i+1: TMA + wgmma run while the attention of step i is computed ===================
         if (i + 1 < p.T) {
-            if (is_producer) produce(i + 1, 1);
-            if (is_mma) { tc_fence_after(); consume(1, !ATT || p.nkb_h == p.nkb); }
-            __syncwarp();
+            if (is_mma) mma_part(i + 1, 1, !ATT || p.nkb_h == p.nkb);
             if (compute) { prefetch_l2(i + 2); if (!ATT) prefetch(i + 1, false); }
         }
 
@@ -859,13 +790,8 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
     if (p.prof && tid == 0)
         for (int k = 0; k < 8; ++k) p.prof[(size_t)cta * 8 + k] = prof_acc[k];
 #undef PROF_MARK
-    if (p.prof2 && (is_mma || is_producer) && lane == 0)
-        for (int k = 0; k < 4; ++k) p.prof2[(size_t)cta * 8 + (is_producer ? 4 : 0) + k] = rp[k];
-    tc_fence_before();
-    __syncthreads();
-    if (warp == NCW + 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS));
-    }
+    if (p.prof2 && warp == NCW && lane == 0)
+        for (int k = 0; k < 4; ++k) p.prof2[(size_t)cta * 8 + k] = rp[k];
 }
 
 // shared memory of one loop CTA with a ring slot of slot_kb k-blocks; alias: the accumulator staging shares the slot
@@ -895,7 +821,7 @@ int largest_divisor_le(int n, int cap) {
 
 }  // namespace
 
-// column geometry of the bf16 operand rows of the tcgen05 loops: [h (D) | ctx (M) | zero pad], 64-column k-blocks
+// column geometry of the bf16 operand rows of the wgmma loops: [h (D) | ctx (M) | zero pad], 64-column k-blocks
 TcPersistGeom tc_persist_geom(const b200tts_decoder_shape& s) {
     TcPersistGeom g{};
     g.nkb_att = (s.D + s.M + KB - 1) / KB;
@@ -923,7 +849,7 @@ TcPersistGeom tc_persist_geom(const b200tts_decoder_shape& s) {
 bool tc_persist_supported(const b200tts_decoder_shape& s) {
     if (s.D % KB != 0 || s.D % UNITS != 0) return false;
     const int RB = s.D / UNITS, NBH = (s.B + BT - 1) / BT;
-    if (RB * NBH > 148 || s.B > RB * NBH) return false;
+    if (RB * NBH > NUM_SMS || s.B > RB * NBH) return false;
     if (s.K > 32 || s.A != 128) return false;
     const TcPersistGeom g = tc_persist_geom(s);
     return g.ch_c_att >= 1 && g.ch_c_att <= 256 && g.slot_att >= g.ch_c_att && g.ch_h_att >= 1 && g.ch_h_gen >= 1 && g.slot_att >= 2 &&
@@ -942,23 +868,23 @@ static int launch_tc_loop(bool att, const TcLoopArgs& a, const CUtensorMap& tmH,
     cudaLaunchAttribute attrs[2];
     attrs[0].id = cudaLaunchAttributeCooperative;
     // profiling aid: ncu cannot capture a launch that is BOTH cooperative and clustered; the kernel carries its own grid barrier, so on an
-    // otherwise idle GPU (all CTAs resident: <= 148, one per SM) the cooperative attribute can be dropped for a capture
+    // otherwise idle GPU (all CTAs resident: <= NUM_SMS, one per SM) the cooperative attribute can be dropped for a capture
     attrs[0].val.cooperative = getenv("B200TTS_PROFILE_NO_COOP") ? 0 : 1;
     cfg.attrs = attrs; cfg.numAttrs = 1;
     if (att) {      // the attention runs on CTA pairs: clusters of 2 (distributed shared memory + cluster barrier)
-        B200_REQUIRE(grid % 2 == 0 && grid / 2 >= a.B, "tcgen05 attention loop: %d CTAs cannot form %d pairs", grid, a.B);
+        B200_REQUIRE(grid % 2 == 0 && grid / 2 >= a.B, "wgmma attention loop: %d CTAs cannot form %d pairs", grid, a.B);
         attrs[1].id = cudaLaunchAttributeClusterDimension;
         attrs[1].val.clusterDim.x = 2; attrs[1].val.clusterDim.y = 1; attrs[1].val.clusterDim.z = 1;
         cfg.numAttrs = 2;
         int nclusters = 0;
         B200_CUDA(cudaOccupancyMaxActiveClusters(&nclusters, fn, &cfg));
-        B200_REQUIRE(nclusters * 2 >= grid, "tcgen05 attention loop: only %d CTA pairs can be co-resident, %d needed", nclusters, grid / 2);
+        B200_REQUIRE(nclusters * 2 >= grid, "wgmma attention loop: only %d CTA pairs can be co-resident, %d needed", nclusters, grid / 2);
     } else {
         int per_sm = 0, dev = 0, sms = 0;
         B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, PT, smem));
         B200_CUDA(cudaGetDevice(&dev));
         B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-        B200_REQUIRE(per_sm * sms >= grid, "tcgen05 persistent loop: %d CTAs cannot be co-resident (%d per SM x %d SMs)", grid, per_sm, sms);
+        B200_REQUIRE(per_sm * sms >= grid, "wgmma persistent loop: %d CTAs cannot be co-resident (%d per SM x %d SMs)", grid, per_sm, sms);
     }
     KernelTimer kt(att ? "lstm_loop_tc_kernel<att>" : "lstm_loop_tc_kernel<gen>", st);
     B200_CUDA(cudaLaunchKernelExC(&cfg, fn, params));
@@ -1000,7 +926,7 @@ int tc_persist_att_loop(const b200tts_decoder_shape& s, const b200tts_decoder_pa
     a.align = align; a.align_bstride = (long long)T * s.L;
     a.barrier = barrier; a.abort_flag = reinterpret_cast<int*>(barrier + 32);
     a.prof = reinterpret_cast<long long*>(pws + l.barrier + 256);
-    a.prof2 = a.prof + 2 * 148 * 8;
+    a.prof2 = a.prof + 2 * NUM_SMS * 8;
     size_t smem = tc_loop_smem_bytes(g.nkb_att, a.slot_kb, s.A, true, s.L, g.alias_att != 0);
     const size_t tab = (size_t)l.MT * 32 * 8;          // shared B-fragment table of the context product, when it fits behind the scratch
     a.use_btab = (smem + tab <= SMEM_LIMIT && !getenv("B200TTS_NO_BTAB")) ? 1 : 0;
@@ -1028,8 +954,8 @@ int tc_persist_gen_loop(const b200tts_decoder_shape& s, const b200tts_decoder_pa
     a.gates = ws + fl.gg; a.cstate = ws + fl.cg;
     a.mask_h = in.mask_gen_h; a.mask_c = in.mask_gen_c; a.kind = s.cell_kind; a.training = s.training; a.rate_h = s.rate_h; a.rate_c = s.rate_c;
     a.barrier = barrier; a.abort_flag = reinterpret_cast<int*>(barrier + 32);
-    a.prof = reinterpret_cast<long long*>(pws + l.barrier + 256) + 148 * 8;
-    a.prof2 = a.prof + 2 * 148 * 8;
+    a.prof = reinterpret_cast<long long*>(pws + l.barrier + 256) + NUM_SMS * 8;
+    a.prof2 = a.prof + 2 * NUM_SMS * 8;
     return launch_tc_loop(false, a, tmH, tmH, tc_loop_smem_bytes(g.nkb_gen, a.slot_kb, s.A, false, 0), st);
 }
 

@@ -18,7 +18,7 @@ namespace {
 
 inline int grid_for(size_t n) {
     size_t g = (n + 255) / 256;
-    return (int)(g > 148 * 16 ? 148 * 16 : (g < 1 ? 1 : g));
+    return (int)(g > NUM_SMS * 16 ? NUM_SMS * 16 : (g < 1 ? 1 : g));
 }
 
 // col[nb, i*k + t, l] = x[nb, i, l + t*dil - pad]  (zero outside)      nb runs over (row, group) pairs
@@ -655,7 +655,7 @@ int convblock_forward_impl(const b200tts_convblock_shape& s, const float* x, con
     float* invstd = mean + align_up_sz(d.Ct, 64);
     bool implicit = s.stage == 2;                 // batch norm only: there is no product, x plays the role of the convolution output
     if (s.stage == 2) conv = const_cast<float*>(x);
-    if (!implicit && precision_mode() != 0 && s.k > 1)       // bf16 perf mode: implicit convolution on the tcgen05 GEMM (TMA row shifts per tap, no im2col)
+    if (!implicit && precision_mode() != 0 && s.k > 1)       // bf16 perf mode: implicit convolution on the wgmma GEMM (TMA row shifts per tap, no im2col)
         B200_TRY(gemm_tc_conv(weight, x, conv, s.NB, s.G, s.Cout, s.Cin, s.L, s.k, s.dilation, d.pad, 0, 0.f, st, &implicit));
     if (!implicit) {
         const float* col = x;
@@ -748,7 +748,7 @@ int convblock_backward_impl(const b200tts_convblock_shape& s, const float* x, co
         if (precision_mode() != 0 && s.k > 1)   // bf16 perf mode: K over (sample row, position), the shifted-input operand packed straight from x
             B200_TRY(gemm_tc_conv_dw(dz, x, dweight, s.NB, s.G, s.Cout, s.Cin, s.L, s.k, s.dilation, d.pad, st, &fused));
         if (!fused && precision_mode() != 0 && s.NB > 1) {
-            // ONE batched tcgen05 GEMM whose K runs over (sample row, position): K = NB * L (two-level K of the packer)
+            // ONE batched wgmma GEMM whose K runs over (sample row, position): K = NB * L (two-level K of the packer)
             B200_TRY(ensure_col());
             GemmDesc g;
             g.A = dz; g.lda = s.L; g.transA = 0; g.strideA = (long long)s.Cout * s.L; g.kosA = (long long)d.Ct * s.L;
@@ -879,7 +879,7 @@ int generator_backward_impl(int G, int gd, int bn, long long R, const float* e, 
     if (bn == 8 && G <= GEN_FG && (reinterpret_cast<uintptr_t>(Wk) & 15) == 0 && (reinterpret_cast<uintptr_t>(dWk) & 15) == 0 &&
         !getenv("B200TTS_GENERATOR_UNFUSED")) {
         // ONE coalesced pass over dout and Wk (fused dWk / dbk / per-block deb partials), then the fixed-order reduction of the partials
-        const int fblk = (int)(((size_t)R + 255) / 256 < 148 * 2 ? ((size_t)R + 255) / 256 : 148 * 2);
+        const int fblk = (int)(((size_t)R + 255) / 256 < NUM_SMS * 2 ? ((size_t)R + 255) / 256 : NUM_SMS * 2);
         generator_bwd_fused_kernel<<<fblk, 256, 0, st>>>(dWk, dbk, scratch, dout, Wk, eb, G, (size_t)R);
         B200_LAUNCH_CHECK();
         generator_tail_bwd_kernel<<<1, 256, 0, st>>>(deb, scratch, fblk, e, Wb, de, dWb, dbb, G, gd, bn);     // finish + dWb + dbb + de

@@ -214,7 +214,7 @@ int gemm_tc_try(const GemmDesc& d, cudaStream_t st, bool* handled);
 
 int gemm_bf16(const GemmDesc& d, cudaStream_t stream) {
     if (d.M <= 0 || d.N <= 0 || d.batch <= 0) return B200TTS_OK;
-    {   // tcgen05 / TMEM / TMA path for the large contractions (gemm_tc.cu); falls through when not applicable
+    {   // wgmma / TMA path for the large contractions (gemm_tc.cu); falls through when not applicable
         bool handled = false;
         B200_TRY(gemm_tc_try(d, stream, &handled));
         if (handled) return B200TTS_OK;
@@ -241,7 +241,7 @@ int gemm_bf16(const GemmDesc& d, cudaStream_t stream) {
     if (d.splitk > 1 && !d.keep_partials) {
         const size_t total = (size_t)d.batch * d.M * d.N;
         int blocks = (int)((total + 255) / 256);
-        if (blocks > 148 * 8) blocks = 148 * 8;
+        if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
         splitk_reduce_kernel<<<blocks, 256, 0, stream>>>(d.partial, d.C, d.bias, d.M, d.N, d.ldc, d.batch, d.splitk, d.strideC,
                                                           d.alpha, d.beta);
         B200_LAUNCH_CHECK();

@@ -247,7 +247,7 @@ int gemm_f32(const GemmDesc& d, cudaStream_t stream) {
     if (d.splitk > 1 && !d.keep_partials) {
         const size_t total = (size_t)d.batch * d.M * d.N;
         int blocks = (int)((total + 255) / 256);
-        if (blocks > 148 * 8) blocks = 148 * 8;
+        if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
         splitk_reduce_kernel<<<blocks, 256, 0, stream>>>(d.partial, d.C, d.bias, d.M, d.N, d.ldc, d.batch, d.splitk,
                                                           d.strideC, d.alpha, d.beta);
         B200_LAUNCH_CHECK();
@@ -269,12 +269,12 @@ int gemm_run_auto(GemmDesc d, float* scratch, size_t scratch_elems, cudaStream_t
     return gemm_auto_impl(d, scratch, scratch_elems, stream, g_precision != 0);
 }
 
-// Picks a split-K factor so that small-output / long-K products still fill the 148 SMs, bounded by the
+// Picks a split-K factor so that small-output / long-K products still fill the NUM_SMS SMs, bounded by the
 // scratch the caller provides for the partial sums.
 int gemm_tc_try(const GemmDesc& d, cudaStream_t st, bool* handled);
 
 static int gemm_auto_impl(GemmDesc d, float* scratch, size_t scratch_elems, cudaStream_t stream, bool bf16) {
-    if (bf16) {     // long-K products run un-split on the tcgen05 kernel (no partial round trip); it declines what it cannot take
+    if (bf16) {     // long-K products run un-split on the wgmma kernel (no partial round trip); it declines what it cannot take
         d.splitk = 1; d.partial = nullptr; d.keep_partials = 0;
         bool handled = false;
         B200_TRY(gemm_tc_try(d, stream, &handled));
@@ -283,8 +283,8 @@ static int gemm_auto_impl(GemmDesc d, float* scratch, size_t scratch_elems, cuda
     const bool big = bf16 || (d.M > 64 && d.N > 64);
     const long long tiles = (long long)(big ? cdiv(d.M, 128) * cdiv(d.N, 128) : cdiv(d.M, 64) * cdiv(d.N, 64)) * d.batch;
     int s = 1;
-    if (tiles < 148 && scratch) {
-        s = (int)((296 + tiles - 1) / tiles);
+    if (tiles < NUM_SMS && scratch) {
+        s = (int)((2 * NUM_SMS + tiles - 1) / tiles);
         const int kmax = cdiv(d.K, 128);
         if (s > kmax) s = kmax;
         if (s > 160) s = 160;

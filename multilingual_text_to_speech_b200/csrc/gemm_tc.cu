@@ -1,114 +1,37 @@
-// tcgen05 / TMEM / TMA bf16 GEMM for the time-batched contractions of the perf mode (sm_100a only).
+// wgmma / TMA bf16 GEMM for the time-batched contractions of the perf mode (sm_90a).
 //
 //   C[M, N] (fp32) = alpha * A[M, K] . B[N, K]^T + beta * C + bias[n]
 //
 // Operands are first packed to bf16, K-major (pack kernels below: fp32 -> bf16, transposing when the source is
 // M/N-contiguous), then one warp-specialised kernel per 128 x 128 output tile:
-//   warp 4 (one lane)  : TMA producer  -- cp.async.bulk.tensor (128B swizzle) into a 4-stage shared-memory ring,
+//   warp 8 (one lane)  : TMA producer  -- cp.async.bulk.tensor (128B swizzle) into a 3-stage shared-memory ring,
 //                        mbarrier expect_tx / complete_tx
-//   warp 5 (one lane)  : MMA issuer    -- tcgen05.mma.cta_group::1.kind::f16, M = 128, N = 128, K = 16 per instruction,
-//                        accumulator in TMEM (128 lanes x 128 columns fp32); tcgen05.commit frees ring slots
-//   warps 0-3          : epilogue      -- tcgen05.ld (32 lanes x 32 columns per instruction) -> staged through the (now idle)
-//                        operand ring so that every global store is a full 512-byte row segment -> alpha/beta/bias -> global
-// Two CTAs are co-resident per SM (3 x 32 KB ring each, 128 TMEM columns each): one tile's epilogue overlaps the other's main loop.
+//   warps 0-7          : two consumer warpgroups, one per 64-row half of the tile -- wgmma.mma_async m64n128k16 from the swizzled
+//                        ring, fp32 accumulator in registers; one wgmma group stays in flight while the previous stage is released;
+//                        epilogue: accumulators staged through the (then idle) ring so that every global store is a full 512-byte row
+//                        segment -> alpha/beta/bias -> global
+// Two CTAs are co-resident per SM (3 x 32 KB ring each): one tile's epilogue overlaps the other's main loop.
 // Every mbarrier wait carries a clock64 watchdog that traps instead of hanging the device.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include "common.cuh"
+#include "tc_ptx.cuh"
 
 namespace b200tts {
 
 namespace {
 
+using namespace tcx;
+
 constexpr int TBM = 128, TBN = 128, TBK = 64;
 constexpr int STAGES = 3;
 constexpr int STAGE_BYTES = (TBM + TBN) * TBK * 2;          // 32 KB
-constexpr int TC_THREADS = 192;
-constexpr int TMEM_COLS = 128;
-constexpr int STG_LD = TBN + 4;                             // fp32 row stride of the epilogue staging tile (16-byte aligned, conflict-free)
-static_assert(4 * 32 * STG_LD * 4 <= STAGES * STAGE_BYTES, "epilogue staging must fit in the operand ring");
+constexpr int TC_THREADS = 288;                             // 2 consumer warpgroups + 1 producer warp
+constexpr int STG_LD = TBN + 8;                             // fp32 row stride of the epilogue staging tile (conflict-free float2 writes)
+static_assert(TBM * STG_LD * 4 <= STAGES * STAGE_BYTES, "epilogue staging must fit in the operand ring");
 
-// ------------------------------------------------------------------------------------------------
-// PTX wrappers
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    const uint32_t addr = smem_u32(bar);
-    const long long t0 = clock64();
-    for (;;) {
-        uint32_t done;
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done)
-            : "r"(addr), "r"(parity)
-            : "memory");
-        if (done) return;
-        if (clock64() - t0 > 4000000000ll) __trap();       // ~2 s: a protocol bug must not hang the GPU
-    }
-}
-__device__ __forceinline__ void tma_load_3d(void* smem, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// K-major, 128-byte swizzled operand tile (rows of 64 bf16 = 128 B, 8-row groups 1024 B apart): UMMA shared-memory descriptor
-// (cute::UMMA::SmemDescriptor: start >> 4 | LBO << 16 | SBO << 32 | version 1 << 46 | SWIZZLE_128B (2) << 61)
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;                 // leading byte offset (unused for swizzled K-major; canonical value 1)
-    d |= (uint64_t)(1024 >> 4) << 32;       // stride byte offset: next 8-row group
-    d |= (uint64_t)1 << 46;                 // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                 // SWIZZLE_128B
-    return d;
-}
-
-// MN-major, 128-byte swizzled operand tile: 64-element (128 B) lines along MN, one line per k row, 8-row groups 1024 B apart (stride
-// byte offset), the next 64-element MN chunk 8 KB further (leading byte offset); a K = 16 instruction step advances 16 rows = 2048 B
-// (canonical layout Swizzle<3,4,3> o ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units, cute::UMMA::make_umma_desc<Major::MN>)
-__device__ __forceinline__ uint64_t make_sw128_mn_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)(8192 >> 4) << 16;       // leading byte offset: next 64-wide MN chunk
-    d |= (uint64_t)(1024 >> 4) << 32;       // stride byte offset: next group of 8 k rows
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
+// named barrier among the 256 consumer threads
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 struct TcArgs {
     float* C; const float* bias;
@@ -130,13 +53,13 @@ struct TcArgs {
     int a_mn, b_mn;
 };
 
+template <int AMN, int BMN>
 __global__ void __launch_bounds__(TC_THREADS, 2)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcArgs p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // 1024-byte aligned ring (128B swizzle atoms are 1024 B)
     uint8_t* ring = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES], tmem_full_bar;
-    __shared__ uint32_t tmem_base_smem;
+    __shared__ uint64_t full_bar[STAGES], empty_bar[STAGES];
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.y * TBM, n0 = blockIdx.x * TBN;
@@ -147,20 +70,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int nk = p.ksplit > 1 ? min(p.kper, nk_all - kb_lo) : nk_all;       // k-blocks of this CTA: [kb_lo, kb_lo + nk)
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(&tmem_full_bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }   // empty: one arrival per consumer warp
+        mbar_init_fence();
     }
-    if (warp == 5) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_smem)), "r"(TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = tmem_base_smem;
 
-    if (warp == 4) {
+    if (warp == 8) {
         if (lane == 0) {
             for (int kb = 0; kb < nk; ++kb) {
                 const int s = kb % STAGES;
@@ -168,9 +83,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 mbar_wait(&empty_bar[s], ph ^ 1);
                 mbar_expect_tx(&full_bar[s], STAGE_BYTES);
                 uint8_t* sa = ring + (size_t)s * STAGE_BYTES;
-                if (p.a_mn) tma_load_3d(sa, &tmA, &full_bar[s], 0, (kb_lo + kb) * TBK, m0 >> 6);
+                if (AMN) tma_load_3d(sa, &tmA, &full_bar[s], 0, (kb_lo + kb) * TBK, m0 >> 6);
                 else tma_load_3d(sa, &tmA, &full_bar[s], (kb_lo + kb) * TBK, m0, az);
-                if (p.b_mn) {
+                if (BMN) {
                     tma_load_3d(sa + TBM * TBK * 2, &tmB, &full_bar[s], 0, (kb_lo + kb) * TBK, n0 >> 6);
                 } else if (p.conv_cb > 0) {
                     const int t = (kb_lo + kb) / p.conv_cb, cb = (kb_lo + kb) % p.conv_cb;
@@ -181,86 +96,85 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 }
             }
         }
-    } else if (warp == 5) {
-        if (lane == 0) {
-            // instruction descriptor (cute::UMMA::InstrDescriptor): D = F32, A = B = BF16, both K-major, N >> 3, M >> 4
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TBN >> 3) << 17) | ((uint32_t)(TBM >> 4) << 24) |
-                                   (p.a_mn ? (1u << 15) : 0u) | (p.b_mn ? (1u << 16) : 0u);      // bits 15 / 16: A / B MN-major
-            const uint64_t a_step = p.a_mn ? (2048 >> 4) : 2, b_step = p.b_mn ? (2048 >> 4) : 2;   // address-field advance per K = 16
-            for (int kb = 0; kb < nk; ++kb) {
-                const int s = kb % STAGES;
-                const uint32_t ph = (kb / STAGES) & 1;
-                mbar_wait(&full_bar[s], ph);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t a_addr = smem_u32(ring + (size_t)s * STAGE_BYTES);
-                const uint64_t adesc = p.a_mn ? make_sw128_mn_desc(a_addr) : make_sw128_desc(a_addr);
-                const uint64_t bdesc = p.b_mn ? make_sw128_mn_desc(a_addr + TBM * TBK * 2) : make_sw128_desc(a_addr + TBM * TBK * 2);
+        return;
+    }
+
+    // consumer warpgroup wg multiplies rows [64 wg, 64 wg + 64) of the tile: its A rows are the second 8 KB half of the stage's A tile
+    // (K-major: 64 rows x 128 B; MN-major: the second 64-column chunk)
+    const int wg = warp >> 2;
+    float acc[64];
 #pragma unroll
-                for (int k = 0; k < TBK / 16; ++k)        // K-major: advance 16 bf16 = 32 B inside the swizzle atom (+2); MN-major: 16 rows
-                    umma_bf16(tmem_base, adesc + a_step * k, bdesc + b_step * k, idesc, (kb | k) != 0);
-                umma_commit(&empty_bar[s]);               // implicit tcgen05.fence::before_thread_sync
-            }
-            umma_commit(&tmem_full_bar);
-        }
-    } else {
-        // epilogue: warp w owns TMEM lanes [32w, 32w + 32) = rows m0 + 32w + lane.  tmem_full implies every MMA (and therefore
-        // every TMA load) of this tile has completed, so the operand ring is free to stage the fp32 tile.
-        mbar_wait(&tmem_full_bar, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        float* stg = reinterpret_cast<float*>(ring) + (size_t)warp * 32 * STG_LD;
-#pragma unroll 1
-        for (int c = 0; c < TBN / 32; ++c) {
-            uint32_t r[32];
-            tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(c * 32), r);
-            float4* dst = reinterpret_cast<float4*>(stg + (size_t)lane * STG_LD + c * 32);
+    for (int r = 0; r < 64; ++r) acc[r] = 0.f;
+    const uint64_t a_step = AMN ? (2048 >> 4) : 2, b_step = BMN ? (2048 >> 4) : 2;   // address-field advance per K = 16
+    for (int kb = 0; kb < nk; ++kb) {
+        const int s = kb % STAGES;
+        mbar_wait(&full_bar[s], (kb / STAGES) & 1);
+        const uint32_t a_addr = smem_u32(ring + (size_t)s * STAGE_BYTES) + wg * 8192;
+        const uint32_t b_addr = smem_u32(ring + (size_t)s * STAGE_BYTES + TBM * TBK * 2);
+        const uint64_t adesc = AMN ? make_sw128_mn_desc(a_addr) : make_sw128_desc(a_addr);
+        const uint64_t bdesc = BMN ? make_sw128_mn_desc(b_addr) : make_sw128_desc(b_addr);
+        wgmma_fence();
 #pragma unroll
-            for (int j = 0; j < 8; ++j)
-                dst[j] = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]), __uint_as_float(r[4 * j + 2]),
-                                     __uint_as_float(r[4 * j + 3]));
-        }
-        __syncwarp();
-        const bool part = p.ksplit > 1;
-        float* cbase = part ? p.partial + (size_t)blockIdx.z * p.M * p.N : p.C + (size_t)bz * p.strideC;
-        const int ldc = part ? p.N : p.ldc;
-        const float alpha = part ? 1.f : p.alpha, beta = part ? 0.f : p.beta;
-        const float* bias = part ? nullptr : p.bias;
-        const int rows = min(32, p.M - (m0 + warp * 32));
-        const int n = n0 + 4 * lane;
-        const bool vec = ((ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(cbase) & 15) == 0) && (n0 + TBN <= p.N);   // warp-uniform
-        if (vec) {
-            float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (bias) bv = make_float4(bias[n], bias[n + 1], bias[n + 2], bias[n + 3]);
-#pragma unroll 4
-            for (int rr = 0; rr < rows; ++rr) {
-                const float4 a = *reinterpret_cast<const float4*>(stg + (size_t)rr * STG_LD + 4 * lane);
-                float4* cp = reinterpret_cast<float4*>(cbase + (size_t)(m0 + warp * 32 + rr) * ldc + n);
-                float4 v = make_float4(fmaf(alpha, a.x, bv.x), fmaf(alpha, a.y, bv.y), fmaf(alpha, a.z, bv.z), fmaf(alpha, a.w, bv.w));
-                if (beta != 0.f) {
-                    const float4 o = *cp;
-                    v.x = fmaf(beta, o.x, v.x); v.y = fmaf(beta, o.y, v.y); v.z = fmaf(beta, o.z, v.z); v.w = fmaf(beta, o.w, v.w);
-                }
-                *cp = v;
-            }
-        } else {
-            for (int rr = 0; rr < rows; ++rr) {
-                float* crow = cbase + (size_t)(m0 + warp * 32 + rr) * ldc;
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const int nn = n0 + j * 32 + lane;
-                    if (nn < p.N) {
-                        float v = alpha * stg[(size_t)rr * STG_LD + j * 32 + lane];
-                        if (bias) v += bias[nn];
-                        if (beta != 0.f) v += beta * crow[nn];
-                        crow[nn] = v;
-                    }
-                }
-            }
+        for (int k = 0; k < TBK / 16; ++k) wgmma_m64n128<AMN, BMN>(acc, adesc + a_step * k, bdesc + b_step * k, 1u);
+        wgmma_commit();
+        if (kb > 0) {                       // the group of stage kb - 1 has completed: release its slot
+            wgmma_wait<1>();
+            wgmma_fence_acc(acc);
+            if (lane == 0) mbar_arrive(&empty_bar[(kb - 1) % STAGES]);
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 5) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    // every wgmma of both warpgroups (and therefore every TMA load) of this tile has completed before the ring is reused as staging
+    consumer_sync();
+    float* stg = reinterpret_cast<float*>(ring);
+    {
+        const int w4 = warp & 3, row0 = wg * 64 + w4 * 16 + (lane >> 2), col0 = 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+                *reinterpret_cast<float2*>(stg + (size_t)(row0 + 8 * h) * STG_LD + 8 * j + col0) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+    }
+    consumer_sync();
+    // warp w stores rows [16 w, 16 w + 16) of the tile, lane = 4 consecutive columns
+    const bool part = p.ksplit > 1;
+    float* cbase = part ? p.partial + (size_t)blockIdx.z * p.M * p.N : p.C + (size_t)bz * p.strideC;
+    const int ldc = part ? p.N : p.ldc;
+    const float alpha = part ? 1.f : p.alpha, beta = part ? 0.f : p.beta;
+    const float* bias = part ? nullptr : p.bias;
+    const int rows = min(16, p.M - (m0 + warp * 16));
+    const float* wstg = stg + (size_t)warp * 16 * STG_LD;
+    const int n = n0 + 4 * lane;
+    const bool vec = ((ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(cbase) & 15) == 0) && (n0 + TBN <= p.N);   // warp-uniform
+    if (vec) {
+        float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (bias) bv = make_float4(bias[n], bias[n + 1], bias[n + 2], bias[n + 3]);
+#pragma unroll 4
+        for (int rr = 0; rr < rows; ++rr) {
+            const float4 a = *reinterpret_cast<const float4*>(wstg + (size_t)rr * STG_LD + 4 * lane);
+            float4* cp = reinterpret_cast<float4*>(cbase + (size_t)(m0 + warp * 16 + rr) * ldc + n);
+            float4 v = make_float4(fmaf(alpha, a.x, bv.x), fmaf(alpha, a.y, bv.y), fmaf(alpha, a.z, bv.z), fmaf(alpha, a.w, bv.w));
+            if (beta != 0.f) {
+                const float4 o = *cp;
+                v.x = fmaf(beta, o.x, v.x); v.y = fmaf(beta, o.y, v.y); v.z = fmaf(beta, o.z, v.z); v.w = fmaf(beta, o.w, v.w);
+            }
+            *cp = v;
+        }
+    } else {
+        for (int rr = 0; rr < rows; ++rr) {
+            float* crow = cbase + (size_t)(m0 + warp * 16 + rr) * ldc;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int nn = n0 + j * 32 + lane;
+                if (nn < p.N) {
+                    float v = alpha * wstg[(size_t)rr * STG_LD + j * 32 + lane];
+                    if (bias) v += bias[nn];
+                    if (beta != 0.f) v += beta * crow[nn];
+                    crow[nn] = v;
+                }
+            }
+        }
     }
 }
 
@@ -474,20 +388,38 @@ int tc_make_mapN_bf16(void* map, const void* base, int rank, const unsigned long
     return B200TTS_OK;
 }
 
+// one instantiation per operand-major combination (the wgmma transpose flags are immediates)
+static int launch_gemm_tc(dim3 grid, const CUtensorMap& tmA, const CUtensorMap& tmB, const TcArgs& a, cudaStream_t st) {
+    typedef void (*TcKernel)(const CUtensorMap, const CUtensorMap, const TcArgs);
+    const TcKernel fn = a.a_mn ? (a.b_mn ? gemm_tc_kernel<1, 1> : gemm_tc_kernel<1, 0>) : (a.b_mn ? gemm_tc_kernel<0, 1> : gemm_tc_kernel<0, 0>);
+    const size_t smem = (size_t)STAGES * STAGE_BYTES + 1024;
+    static bool configured[2][2] = {{false, false}, {false, false}};     // the shared-memory limit is set once per instantiation
+    if (!configured[a.a_mn][a.b_mn]) {
+        B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        configured[a.a_mn][a.b_mn] = true;
+    }
+    {
+        KernelTimer kt("gemm_tc_kernel", st);
+        fn<<<grid, TC_THREADS, smem, st>>>(tmA, tmB, a);
+    }
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
 void set_tc_scratch(void* ptr, size_t bytes) { g_scratch.ptr = static_cast<unsigned char*>(ptr); g_scratch.bytes = bytes; g_ncache = 0; g_cache_off = 0; }
 void tc_pack_cache_begin() { g_cache_on = true; g_ncache = 0; g_cache_off = 0; }
 void tc_pack_cache_end() { g_cache_on = false; g_ncache = 0; g_cache_off = 0; }
 void set_tc_enabled(int on) { g_tc_enabled = on; }
 int tc_enabled() { return g_tc_enabled; }
 
-// Returns B200TTS_OK and sets *handled = true when the tcgen05 path ran; *handled = false -> caller uses the mma.sync path.
+// Returns B200TTS_OK and sets *handled = true when the wgmma path ran; *handled = false -> caller uses the mma.sync path.
 // Split-K decision shared by the dense and the convolution weight-gradient products: with fewer output tiles than CTA slots (2 per SM)
 // and a long K, K is cut into `splits` ranges of `kper` k-blocks; the partial tiles live at the END of the scratch, clear of the
 // packed (and cached) operands that occupy its first `used` bytes.  Leaves a.ksplit = 1 when it does not pay or does not fit.
 static void pick_ksplit(TcArgs& a, int M, int N, int K, size_t used) {
     const int tiles = cdiv(N, TBN) * cdiv(M, TBM), nk = cdiv(K, TBK);
-    if (tiles > 148 || nk < 64) return;
-    int want = 296 / tiles;
+    if (tiles > NUM_SMS || nk < 64) return;
+    int want = 2 * NUM_SMS / tiles;
     if (want > nk / 16) want = nk / 16;
     if (want > 32) want = 32;
     if (want < 2) return;
@@ -584,22 +516,11 @@ int gemm_tc_try(const GemmDesc& d, cudaStream_t st, bool* handled) {
     // few output tiles and a long K (weight gradients over all (step, utterance) rows): split K over the idle SMs
     if (d.batch == 1)
         pick_ksplit(a, d.M, d.N, d.K, (g_cache_on ? g_cache_off : 0) + (pack_a ? a_bytes : 0) + (pack_b ? b_bytes : 0));
-    const size_t smem = (size_t)STAGES * STAGE_BYTES + 1024;
-    static bool configured = false;
-    if (!configured) {
-        B200_CUDA(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured = true;
-    }
-    dim3 grid(cdiv(d.N, TBN), cdiv(d.M, TBM), a.ksplit > 1 ? a.ksplit : d.batch);
-    {
-        KernelTimer kt("gemm_tc_kernel", st);
-        gemm_tc_kernel<<<grid, TC_THREADS, smem, st>>>(tmA, tmB, a);
-    }
-    B200_LAUNCH_CHECK();
+    B200_TRY(launch_gemm_tc(dim3(cdiv(d.N, TBN), cdiv(d.M, TBM), a.ksplit > 1 ? a.ksplit : d.batch), tmA, tmB, a, st));
     if (a.ksplit > 1) {
         const size_t total = (size_t)d.M * d.N;
         int blocks = (int)((total + 255) / 256);
-        if (blocks > 148 * 8) blocks = 148 * 8;
+        if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
         tc_splitk_reduce_kernel<<<blocks, 256, 0, st>>>(a.partial, d.C, d.bias, d.M, d.N, d.ldc, a.ksplit, d.alpha, d.beta);
         B200_LAUNCH_CHECK();
     }
@@ -608,7 +529,7 @@ int gemm_tc_try(const GemmDesc& d, cudaStream_t st, bool* handled) {
 }
 
 
-// Implicit 1-D convolution on the tcgen05 GEMM (no im2col):  out[row, g][m, l] (+)= sum_{t, c} Wp[g][m][t * Cred + c] . in[row][g * Cred + c][l + t * dil - pad]
+// Implicit 1-D convolution on the wgmma GEMM (no im2col):  out[row, g][m, l] (+)= sum_{t, c} Wp[g][m][t * Cred + c] . in[row][g * Cred + c][l + t * dil - pad]
 //   forward        : Wp = weights packed (co, t, ci), in = x,        Cred = Cin,  rows m = Cout, dil/pad as given
 //   input gradient : Wp = weights packed (ci, t, co), in = d conv,   Cred = Cout, rows m = Cin,  dil -> -dil, pad -> -pad
 // `in` is [NB, G * Cred, L] fp32; its position-major bf16 copy [NB][L][G * Cred] is made here (one transposing pass, 1x the activation).
@@ -646,20 +567,13 @@ int gemm_tc_conv(const float* weight, const float* in, float* out, int NB, int G
     a.batch = NB * G; a.a_batch_mod = G; a.strideC = (long long)Mrows * L;
     a.conv_cb = CredP / TBK; a.conv_dil = bwd ? -dil : dil; a.conv_pad = bwd ? -pad : pad; a.conv_G = G; a.conv_cin = CredP;
     a.ksplit = 1; a.kper = 0; a.partial = nullptr; a.a_mn = 0; a.b_mn = 0;
-    const size_t smem = (size_t)STAGES * STAGE_BYTES + 1024;
-    B200_CUDA(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    dim3 grid(cdiv(L, TBN), cdiv(Mrows, TBM), NB * G);
-    {
-        KernelTimer kt("gemm_tc_kernel", st);
-        gemm_tc_kernel<<<grid, TC_THREADS, smem, st>>>(tmA, tmB, a);
-    }
-    B200_LAUNCH_CHECK();
+    B200_TRY(launch_gemm_tc(dim3(cdiv(L, TBN), cdiv(Mrows, TBM), NB * G), tmA, tmB, a, st));
     *handled = true;
     return B200TTS_OK;
 }
 
 
-// Weight gradient of a 1-D convolution in ONE batched tcgen05 GEMM:  dW[g][co][ci * k + t] += sum_{q, l} dz[q][g, co][l] . x[q][g, ci][l + t dil - pad].
+// Weight gradient of a 1-D convolution in ONE batched wgmma GEMM:  dW[g][co][ci * k + t] += sum_{q, l} dz[q][g, co][l] . x[q][g, ci][l + t dil - pad].
 // A = dz packed with a two-level K (sample row, position); B = the shifted input packed straight from x (pack_im2col_kcontig_kernel).
 int gemm_tc_conv_dw(const float* dz, const float* x, float* dweight, int NB, int G, int Cout, int Cin, int L, int k, int dil, int pad,
                     cudaStream_t st, bool* handled) {
@@ -689,18 +603,11 @@ int gemm_tc_conv_dw(const float* dz, const float* x, float* dweight, int NB, int
     a.conv_cb = 0; a.conv_dil = 0; a.conv_pad = 0; a.conv_G = 1; a.conv_cin = 0;
     a.ksplit = 1; a.kper = 0; a.partial = nullptr; a.a_mn = 0; a.b_mn = 0;
     if (G == 1) pick_ksplit(a, Cout, R, K, a_bytes + b_bytes);      // postnet convolutions: 16 .. 80 tiles over K = NB * L
-    const size_t smem = (size_t)STAGES * STAGE_BYTES + 1024;
-    B200_CUDA(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    dim3 grid(cdiv(R, TBN), cdiv(Cout, TBM), a.ksplit > 1 ? a.ksplit : G);
-    {
-        KernelTimer kt("gemm_tc_kernel", st);
-        gemm_tc_kernel<<<grid, TC_THREADS, smem, st>>>(tmA, tmB, a);
-    }
-    B200_LAUNCH_CHECK();
+    B200_TRY(launch_gemm_tc(dim3(cdiv(R, TBN), cdiv(Cout, TBM), a.ksplit > 1 ? a.ksplit : G), tmA, tmB, a, st));
     if (a.ksplit > 1) {
         const size_t total = (size_t)Cout * R;
         int blocks = (int)((total + 255) / 256);
-        if (blocks > 148 * 8) blocks = 148 * 8;
+        if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
         tc_splitk_reduce_kernel<<<blocks, 256, 0, st>>>(a.partial, dweight, nullptr, Cout, R, R, a.ksplit, 1.f, 1.f);
         B200_LAUNCH_CHECK();
     }

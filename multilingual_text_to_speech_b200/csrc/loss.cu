@@ -9,7 +9,7 @@ namespace b200tts {
 namespace {
 
 constexpr int LT = 256;
-constexpr int LOSS_BLOCKS = 148 * 4;
+constexpr int LOSS_BLOCKS = NUM_SMS * 4;
 
 struct LossArgs {
     int B, N, T, L;
@@ -151,7 +151,7 @@ int loss_backward_impl(const b200tts_loss_shape& s, const float* pre, const floa
                        float* d_pre, float* d_post, float* d_stop, float* d_align, cudaStream_t st) {
     const LossArgs a = make_args(s, pre, pre_t, post, post_t, stop, stop_t, nullptr, text_len, target_len);
     const double nmel = (double)s.B * s.N * s.T, nstop = (double)s.B * s.T;
-    loss_backward_kernel<<<148 * 8, LT, 0, st>>>(a, grad_losses, d_pre, d_post, d_stop, d_align, (float)(4.0 / nmel), (float)(2.0 / nmel),
+    loss_backward_kernel<<<NUM_SMS * 8, LT, 0, st>>>(a, grad_losses, d_pre, d_post, d_stop, d_align, (float)(4.0 / nmel), (float)(2.0 / nmel),
                                                  (float)(1.0 / (nstop * (s.N + 2))), (float)(1.0 / s.B));
     B200_LAUNCH_CHECK();
     return B200TTS_OK;

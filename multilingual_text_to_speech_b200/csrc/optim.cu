@@ -7,7 +7,7 @@ namespace b200tts {
 
 namespace {
 
-constexpr int NORM_BLOCKS = 1184;      // 148 SMs x 8
+constexpr int NORM_BLOCKS = NUM_SMS * 8;
 
 __global__ void __launch_bounds__(256) sqnorm_partial_kernel(const float* __restrict__ g, size_t n, float* __restrict__ partial) {
     __shared__ float red[64];
@@ -77,7 +77,7 @@ int adam_clip_step_impl(float* p, float* g, float* m, float* v, size_t n, float 
     B200_LAUNCH_CHECK();
     const double bc1 = 1.0 - pow((double)beta1, (double)step), bc2 = 1.0 - pow((double)beta2, (double)step);
     size_t ub = (n + 255) / 256;
-    const int ublk = (int)(ub > 148 * 16 ? 148 * 16 : ub);
+    const int ublk = (int)(ub > NUM_SMS * 16 ? NUM_SMS * 16 : ub);
     adam_clip_kernel<<<ublk, 256, 0, st>>>(p, g, m, v, n, lr, beta1, beta2, eps, weight_decay, (float)bc1, (float)sqrt(bc2), norm);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;

@@ -11,7 +11,7 @@ namespace {
 
 inline int grid_for(size_t n) {
     size_t g = (n + 255) / 256;
-    return (int)(g > 148 * 16 ? 148 * 16 : (g < 1 ? 1 : g));
+    return (int)(g > NUM_SMS * 16 ? NUM_SMS * 16 : (g < 1 ? 1 : g));
 }
 
 // xp[dir][j, b, :] = x[b, t(dir, j), :]   with t(0, j) = j, t(1, j) = L-1-j

@@ -1,7 +1,7 @@
 """A whole training step (forward + TacotronLoss + backward into the flat gradient bucket) as ONE CUDA graph.
 
-The step of the bf16 mode is ~1200 kernel launches issued from Python; between them the GPU idles for 2 - 15 ms per step depending on the
-host (profiles/SUMMARY_r2.md).  Every library call only enqueues work on the current stream (no allocation, no synchronisation, host
+The step of the bf16 mode is ~1200 kernel launches issued from Python; between them the GPU idles for milliseconds per step depending on the
+host.  Every library call only enqueues work on the current stream (no allocation, no synchronisation, host
 arguments read at enqueue time), so the step can be captured once and replayed: the launch overhead disappears and the step time becomes
 the sum of its kernels.  Static shapes are the contract (one graph per batch shape -- bucketed batches, utils/samplers.py, keep the number
 of shapes small); dropout masks stay fresh because the graph increments a device-side epoch that the mask generator mixes into its keys

@@ -29,7 +29,7 @@ def build_model(checkpoint, force_cpu=False):
     """Load hyper-parameters and weights from a reference-format checkpoint and build the model."""
     from ..modules.tacotron2 import Tacotron
     if force_cpu or not torch.cuda.is_available():
-        raise RuntimeError('the B200-native Tacotron has no CPU path; a CUDA device is required')
+        raise RuntimeError('this Tacotron has no CPU path; a CUDA device (H100) is required')
     state = torch.load(checkpoint, map_location='cuda')
     hp.load_state_dict(state['parameters'])
     model = Tacotron()

@@ -1,4 +1,4 @@
-"""Whole-model parity: the B200 Tacotron (host modules + library) against golden vectors of the unmodified reference."""
+"""Whole-model parity: this package's Tacotron (host modules + library) against golden vectors of the unmodified reference."""
 import torch
 
 from helpers import Golden, assert_close

@@ -156,7 +156,7 @@ def tape_for(hp, frames=T):
 
 
 def run_gpu(mode, fx=None, with_grads=True, verbose=True):
-    """The B200 path (host modules + libb200tts.so) on the fixture's inputs in precision `mode`; returns a report of errors
+    """This package's path (host modules + libb200tts.so) on the fixture's inputs in precision `mode`; returns a report of errors
     against the UNMODIFIED reference's recorded results.  Asserts nothing: the callers hold the gates."""
     from multilingual_text_to_speech_b200 import _lib
     from multilingual_text_to_speech_b200.modules.tacotron2 import TacotronLoss

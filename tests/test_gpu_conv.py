@@ -1,4 +1,4 @@
-"""bf16 perf-mode convolution paths of the conv block (implicit tcgen05 convolution forward / input gradient, fused weight
+"""bf16 perf-mode convolution paths of the conv block (implicit wgmma convolution forward / input gradient, fused weight
 gradient) against the library's own fp32 parity path (itself pinned to the reference by the golden model tests)."""
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): GEMM, attention step and the fused decoder fwd/bwd through the C ABI
+"""GPU parity tests (run on an H100): GEMM, attention step and the fused decoder fwd/bwd through the C ABI
 against the CPU oracle / golden vectors of the unmodified reference.  Tolerance: rtol 1e-3, atol 1e-4 (north_star),
 alignment argmax bit-exact."""
 import pytest
@@ -143,7 +143,7 @@ def test_gemm_bf16_mode(M, N, K, ta, tb, splitk):
     dict(B=80, L=50, T=10, kind='dropout', seed=8),             # B > 64 (configs[3..4] run 65 / 80 per GPU): decoded as two slices
     dict(B=65, L=44, T=9, M=292, kind='zoneout', seed=9),
     # memory dim 512 (monolingual default, BASELINE configs[0]): accumulator staging aliased onto the TMA slot, ctx part in several TMA
-    # instructions (forward), UMMA N = 96 n-blocks (attention reverse product)
+    # instructions (forward), wgmma N = 96 n-blocks (attention reverse product)
     dict(B=16, L=60, T=14, M=512, kind='zoneout', seed=10),
     dict(B=52, L=300, T=8, M=512, kind='dropout', seed=11),
     dict(B=9, L=37, T=11, M=384, kind='dropout', seed=12),
@@ -159,7 +159,7 @@ def test_decoder_bf16_perf_mode(kw):
     (128, 1024, 20000, True, False), (81, 1312, 9000, True, False),        # few tiles, long K: split-K over the idle SMs (+ reduction launch)
 ])
 def test_gemm_tcgen05_path(M, N, K, ta, tb):
-    """tcgen05 / TMEM / TMA GEMM (gemm_tc.cu) against fp64 on bf16-rounded operands, and against the mma.sync kernel."""
+    """wgmma / TMA GEMM (gemm_tc.cu) against fp64 on bf16-rounded operands, and against the mma.sync kernel."""
     from multilingual_text_to_speech_b200 import functional as F, _lib
     g = torch.Generator().manual_seed(M + 3 * N + 7 * K)
     a = torch.randn((K, M) if ta else (M, K), generator=g)
@@ -180,6 +180,6 @@ def test_gemm_tcgen05_path(M, N, K, ta, tb):
     finally:
         _lib.set_tensor_core_gemm(True)
         _lib.set_precision('fp32')
-    assert used in (3, 4), f'expected pack + pack + tcgen05 kernel (+ split-K reduction), saw {used} launches'
-    assert_close(out, ref, 1e-4, 2e-4 * (K ** 0.5), f'tcgen05 gemm {M}x{N}x{K}')
-    assert_close(out, out2, 1e-4, 2e-4 * (K ** 0.5), 'tcgen05 vs mma.sync')
+    assert used in (3, 4), f'expected pack + pack + wgmma kernel (+ split-K reduction), saw {used} launches'
+    assert_close(out, ref, 1e-4, 2e-4 * (K ** 0.5), f'wgmma gemm {M}x{N}x{K}')
+    assert_close(out, out2, 1e-4, 2e-4 * (K ** 0.5), 'wgmma vs mma.sync')

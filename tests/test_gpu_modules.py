@@ -1,18 +1,16 @@
-"""Module-level forwards of the boundary (SURVEY 8b) against the UNMODIFIED reference classes imported from baseline/_ref (CPU, fp32):
-ZoneoutLSTMCell / DropoutLSTMCell (modules/layers.py:18-47), Conv1dGenerated / BatchNorm1dGenerated (modules/generated.py:7-96),
-forward values and gradients through the library ops."""
+"""Module-level forwards of the boundary (SURVEY 8b) against golden vectors of the UNMODIFIED reference classes (CPU, fp32;
+tests/golden/make_golden_modules.py -> tests/golden/modules.npz): ZoneoutLSTMCell / DropoutLSTMCell (modules/layers.py:18-47),
+Conv1dGenerated / BatchNorm1dGenerated (modules/generated.py:7-96), LocationSensitiveAttention (modules/attention.py:6-86),
+forward values and gradients through the library ops.  The cases themselves are in tests/module_cases.py."""
 import os
-import sys
+import numpy as np
 import pytest
 import torch
 
-from helpers import assert_close, ROOT
+import module_cases as C
+from helpers import assert_close, GOLDEN_DIR
 
 pytestmark = pytest.mark.gpu
-sys.path.insert(0, os.path.join(ROOT, 'baseline'))
-import reference_runner as R      # noqa: E402
-
-needs_ref = pytest.mark.skipif(not R.available(), reason='baseline/_ref (the unmodified reference) is not installed')
 
 
 @pytest.fixture(scope='module', autouse=True)
@@ -22,35 +20,17 @@ def _built():
     assert torch.cuda.is_available()
 
 
-def _copy_params(dst, src):
-    dst.load_state_dict(src.state_dict(), strict=True)
+@pytest.fixture(scope='module')
+def golden():
+    return np.load(os.path.join(GOLDEN_DIR, 'modules.npz'))
 
 
-@needs_ref
-@pytest.mark.parametrize('kind', ['zoneout', 'dropout'])
-def test_lstm_cells_match_reference_eval_mode(kind):
-    R.load()
-    from modules.layers import ZoneoutLSTMCell as RZ, DropoutLSTMCell as RD
-    from multilingual_text_to_speech_b200.modules.layers import ZoneoutLSTMCell, DropoutLSTMCell
-    torch.manual_seed(3)
-    I, H, B = 544, 1024, 7
-    ref = (RZ(I, H, 0.1, 0.1) if kind == 'zoneout' else RD(I, H, 0.1)).eval()
-    own = (ZoneoutLSTMCell(I, H, 0.1, 0.1) if kind == 'zoneout' else DropoutLSTMCell(I, H, 0.1)).eval()
-    _copy_params(own, ref)
-    own = own.cuda()
-    x, h, c = torch.randn(B, I), torch.randn(B, H), torch.randn(B, H)
-    xr, hr, cr = (t.clone().requires_grad_(True) for t in (x, h, c))
-    xo, ho, co = (t.cuda().requires_grad_(True) for t in (x, h, c))
-    h1, c1 = ref(xr, hr, cr)
-    h2, c2 = own(xo, ho, co)
-    assert_close(h2, h1, 1e-3, 1e-5, 'h'); assert_close(c2, c1, 1e-3, 1e-5, 'c')
-    gh, gc = torch.randn(B, H), torch.randn(B, H)
-    ((h1 * gh).sum() + (c1 * gc).sum()).backward()
-    ((h2 * gh.cuda()).sum() + (c2 * gc.cuda()).sum()).backward()
-    for name, a, b in (('dx', xo, xr), ('dh', ho, hr), ('dc', co, cr)):
-        assert_close(a.grad, b.grad, 2e-3, 1e-5, name)
-    for (n, p), (_, q) in zip(own.named_parameters(), ref.named_parameters()):
-        assert_close(p.grad, q.grad, 2e-3, 1e-4 * float(q.grad.abs().max()), 'd' + n)
+def _check(golden, prefix, result, tol):
+    """tol(key) -> (rtol, atol relative to the reference tensor's largest magnitude, absolute atol floor)."""
+    for key, t in result.items():
+        got, ref, amax = C.unpack_like(golden, prefix, key, t)
+        rtol, atol_rel, atol_abs = tol(key)
+        assert_close(got, ref, rtol, atol_rel * amax + atol_abs, f'{prefix}.{key}')
 
 
 def test_zoneout_cell_train_mode_with_masks():
@@ -85,81 +65,56 @@ def test_zoneout_cell_train_mode_with_masks():
         assert_close(a.grad, b.grad, 2e-3, 1e-5, name)
 
 
-@needs_ref
+@pytest.mark.parametrize('kind', ['zoneout', 'dropout'])
+def test_lstm_cells_match_reference_eval_mode(kind, golden):
+    from multilingual_text_to_speech_b200.modules.layers import ZoneoutLSTMCell, DropoutLSTMCell
+    I, H = 544, 1024
+    own = ZoneoutLSTMCell(I, H, 0.1, 0.1) if kind == 'zoneout' else DropoutLSTMCell(I, H, 0.1)
+    res = C.lstm_case(kind, own, 'cuda')
+    _check(golden, f'lstm_{kind}', res,
+           lambda k: (1e-3, 0.0, 1e-5) if k in ('h', 'c') else (2e-3, 0.0, 1e-5) if k in ('dx', 'dh', 'dc') else (2e-3, 1e-4, 0.0))
+
+
 @pytest.mark.parametrize('train', [True, False])
-def test_generated_conv_and_batchnorm_match_reference(train):
-    R.load()
-    from modules.generated import Conv1dGenerated as RC, BatchNorm1dGenerated as RB
+def test_generated_conv_and_batchnorm_match_reference(train, golden):
     from multilingual_text_to_speech_b200.modules.generated import Conv1dGenerated, BatchNorm1dGenerated
-    torch.manual_seed(5)
-    G, gd, bn, Cin, Cout, k, dil, NB, L = 3, 6, 4, 8, 12, 3, 2, 4, 21
-    e = torch.randn(G, gd)
-    x = torch.randn(NB, G * Cin, L + (k - 1) * dil)          # the caller pads (ConvBlockGenerated pads before the convolution)
-    rc = RC(gd, bn, G * Cin, G * Cout, k, padding=0, dilation=dil, groups=G, bias=False).train(train)
-    oc = Conv1dGenerated(gd, bn, G * Cin, G * Cout, k, padding=0, dilation=dil, groups=G, bias=False).train(train)
-    _copy_params(oc, rc)
-    rb = RB(gd, bn, G * Cout, groups=G).train(train)
-    ob = BatchNorm1dGenerated(gd, bn, G * Cout, groups=G).train(train)
-    _copy_params(ob, rb)
-    oc, ob = oc.cuda(), ob.cuda()
-    er, xr = e.clone().requires_grad_(True), x.clone().requires_grad_(True)
-    eo, xo = e.cuda().requires_grad_(True), x.cuda().requires_grad_(True)
-    y1 = rc(er, xr)                                          # un-padded ("valid") convolution, as in the reference
-    y2 = oc(eo, xo)
-    assert y1.shape == y2.shape and y1.shape[2] == L
-    assert_close(y2, y1, 1e-3, 1e-5, 'generated convolution')
-    z1, z2 = rb(er, y1), ob(eo, y2)
-    assert_close(z2, z1, 1e-3, 1e-4, 'generated batch norm')
-    gz = torch.randn_like(z1)
-    (z1 * gz).sum().backward()
-    (z2 * gz.cuda()).sum().backward()
-    assert_close(eo.grad, er.grad, 3e-3, 1e-4 * float(er.grad.abs().max()), 'd generator embedding')
-    assert_close(xo.grad, xr.grad, 3e-3, 1e-4 * float(xr.grad.abs().max()), 'dx')
-    for (n, p), (_, q) in zip(list(oc.named_parameters()) + list(ob.named_parameters()), list(rc.named_parameters()) + list(rb.named_parameters())):
-        assert_close(p.grad, q.grad, 3e-3, 2e-4 * float(q.grad.abs().max()) + 1e-9, 'd' + n)
-    if train:
-        assert_close(ob.running_mean, rb.running_mean, 1e-3, 1e-6, 'running_mean')
-        assert_close(ob.running_var, rb.running_var, 1e-3, 1e-6, 'running_var')
-        assert int(ob.num_batches_tracked) == int(rb.num_batches_tracked) == 1
+    G, gd, bn, Cin, Cout, k, dil = 3, 6, 4, 8, 12, 3, 2
+    oc = Conv1dGenerated(gd, bn, G * Cin, G * Cout, k, padding=0, dilation=dil, groups=G, bias=False)
+    ob = BatchNorm1dGenerated(gd, bn, G * Cout, groups=G)
+    res = C.conv_case(train, oc, ob, 'cuda')
+    assert res['y'].shape[2] == 21                           # un-padded ("valid") convolution, as in the reference
+    if not train:
+        for key in ('running_mean', 'running_var', 'num_batches_tracked'):
+            res.pop(key)
+    else:
+        assert int(res['num_batches_tracked']) == 1
+
+    def tol(key):
+        if key == 'y':
+            return 1e-3, 0.0, 1e-5
+        if key == 'z':
+            return 1e-3, 0.0, 1e-4
+        if key in ('running_mean', 'running_var', 'num_batches_tracked'):
+            return 1e-3, 0.0, 1e-6
+        if key in ('de', 'dx'):
+            return 3e-3, 1e-4, 0.0
+        return 3e-3, 2e-4, 1e-9
+    _check(golden, f'conv_train{int(train)}', res, tol)
 
 
-@needs_ref
-def test_attention_module_forward_and_autograd_match_reference():
+def test_attention_module_forward_and_autograd_match_reference(golden):
     """LocationSensitiveAttention.reset + three forward steps (attention.py:23-28, 39-45, 67-86) with gradients through the carried
     cumulative weights, against the reference module."""
-    R.load()
-    from modules.attention import LocationSensitiveAttention as RA
     from multilingual_text_to_speech_b200.modules.attention import LocationSensitiveAttention
-    torch.manual_seed(7)
-    B, L, M, D, A, C, K = 5, 37, 288, 1024, 128, 32, 31
-    ref = RA(K, C, False, A, D, M)
-    own = LocationSensitiveAttention(K, C, False, A, D, M)
-    with torch.no_grad():
-        for prm in ref.parameters():
-            prm.mul_(3.0)
-    _copy_params(own, ref)
-    own = own.cuda()
-    lens = torch.tensor([37, 30, 37, 12, 25])
-    mask = torch.arange(L)[None, :] < lens[:, None]
-    memory = torch.randn(B, L, M)
-    queries = [torch.randn(B, D) for _ in range(3)]
-    mr = memory.clone().requires_grad_(True); qr = [q.clone().requires_grad_(True) for q in queries]
-    mo = memory.cuda().requires_grad_(True); qo = [q.cuda().requires_grad_(True) for q in queries]
-    ref.reset(mr, B, L, memory.device)
-    own.reset(mo, B, L, mo.device)
-    gen = torch.Generator().manual_seed(1)
-    loss_r, loss_o = 0.0, 0.0
-    for step in range(3):
-        c1, w1 = ref(qr[step], mr, mask, None)
-        c2, w2 = own(qo[step], mo, mask.cuda(), None)
-        assert_close(w2, w1, 1e-3, 1e-6, f'weights step {step}')
-        assert_close(c2, c1, 1e-3, 1e-5, f'context step {step}')
-        gc, gw = torch.randn(B, M, generator=gen), torch.randn(B, L, generator=gen)
-        loss_r = loss_r + (c1 * gc).sum() + (w1 * gw).sum()
-        loss_o = loss_o + (c2 * gc.cuda()).sum() + (w2 * gw.cuda()).sum()
-    loss_r.backward(); loss_o.backward()
-    assert_close(mo.grad, mr.grad, 3e-3, 1e-4 * float(mr.grad.abs().max()), 'd memory')
-    for step in range(3):
-        assert_close(qo[step].grad, qr[step].grad, 3e-3, 1e-4 * float(qr[step].grad.abs().max()), f'd query {step}')
-    for (n, p), (_, q) in zip(own.named_parameters(), ref.named_parameters()):
-        assert_close(p.grad, q.grad, 3e-3, 2e-4 * float(q.grad.abs().max()), 'd' + n)
+    d = C.ATT_DIMS
+    res = C.attention_case(LocationSensitiveAttention(d['K'], d['C'], False, d['A'], d['D'], d['M']), 'cuda')
+
+    def tol(key):
+        if key.startswith('weights'):
+            return 1e-3, 0.0, 1e-6
+        if key.startswith('context'):
+            return 1e-3, 0.0, 1e-5
+        if key == 'dmemory' or key.startswith('dquery'):
+            return 3e-3, 1e-4, 0.0
+        return 3e-3, 2e-4, 0.0
+    _check(golden, 'attention', res, tol)

@@ -67,7 +67,7 @@ def test_fused_adam_needs_gpu():
 
 
 def test_decoder_path_covers_baseline_configs(lib):
-    """BASELINE configs[1..4] run on the persistent tcgen05 kernels in every pass (host-side path query, no GPU needed): memory
+    """BASELINE configs[1..4] run on the persistent wgmma kernels in every pass (host-side path query, no GPU needed): memory
     dims 288 (generated_training / generated_switching) and 292 (shared_switching), per-GPU batches up to 64, texts up to 300.
     The monolingual default (memory dim 512, configs[0]) fits too (accumulator staging aliased onto the TMA slot, wider n-blocks)."""
     def path(B, L, T, M, kind=1, training=1):
@@ -78,7 +78,7 @@ def test_decoder_path_covers_baseline_configs(lib):
             for L, T in ((180, 900), (300, 1200)):
                 for kind in (0, 1):
                     assert path(B, L, T, M, kind) == 0b111111, (B, L, T, M, kind, bin(path(B, L, T, M, kind)))
-    assert path(64, 180, 900, 288, training=0) & 0b11 == 0b11          # inference / evaluation: forward loops on tcgen05
+    assert path(64, 180, 900, 288, training=0) & 0b11 == 0b11          # inference / evaluation: forward loops on wgmma
     for B, L in ((16, 180), (52, 180), (64, 300)):
         assert path(B, L, 900, 512) == 0b111111, (B, L, bin(path(B, L, 900, 512)))
 
