@@ -136,6 +136,8 @@ size_t b200tts_decoder_bwd_workspace_bytes(const b200tts_decoder_shape* shape);
 /* Which kernels a bf16-mode training step of this shape runs on (pure host arithmetic, no device needed): bit 0 = persistent
  * forward loops, bit 1 = their TMA + wgmma variant, bit 2 = persistent generator reverse loop, bit 3 = its wgmma
  * variant, bit 4 = persistent attention reverse loop, bit 5 = its wgmma product.  0 = the per-step kernel chains.
+ * Every persistent loop is a TMA + wgmma kernel, so each variant bit (1, 3, 5) is set exactly when its loop bit (0, 2, 4)
+ * is; a pass whose loop bit is clear runs the per-step kernel chains.
  * (The reference has no such limit anywhere: modules/attention.py:67-74 takes any length.) */
 int b200tts_decoder_path(const b200tts_decoder_shape* shape);
 /* Debug: byte offset, inside the decoder forward workspace, of the per-CTA phase cycle counters the persistent

@@ -244,23 +244,8 @@ size_t b200tts_decoder_workspace_bytes(const b200tts_decoder_shape* shape) {
 
 int b200tts_decoder_path(const b200tts_decoder_shape* shape) {
     if (!shape || validate_decoder_shape(*shape) != B200TTS_OK) return 0;
-    const b200tts_decoder_shape& s = *shape;
-    int bits = 0;
-    const bool att_bwd = persist_att_bwd_supported(s);
-    const bool fwd_loops = tc_persist_supported(s) || persist_supported(s);
-    if (fwd_loops && (!s.training || att_bwd)) {
-        bits |= 1;
-        if (tc_persist_supported(s)) bits |= 2;
-    }
-    if (persist_bwd_supported(s)) {
-        bits |= 4;
-        if (tc_persist_gen_bwd_supported(s)) bits |= 8;
-    }
-    if (s.training && fwd_loops && att_bwd) {
-        bits |= 16;
-        if (persist_att_bwd_tc(s)) bits |= 32;
-    }
-    return bits;
+    const PersistPlan p = persist_plan(*shape);
+    return (p.fwd ? 1 | 2 : 0) | (p.gen_bwd ? 4 | 8 : 0) | (p.att_bwd ? 16 | 32 : 0);
 }
 
 size_t b200tts_decoder_bwd_workspace_bytes(const b200tts_decoder_shape* shape) {

@@ -668,14 +668,15 @@ int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_
     auto W = [&](size_t off) { return bws + off; };
     const float* ai = F(fl.ai);                // [T+1, B, M+D]
     const float* ai1 = ai + (size_t)B * MD;    // rows 1..T
+    const PersistPlan plan = precision_mode() == B200TTS_PRECISION_BF16 ? persist_plan(s) : PersistPlan{};
     // bf16 operand rows the wgmma forward loops left in the persistent workspace: aib [T+1, B, Kp_att] = [h_att | ctx | 0], hgb [T+1, B, Kp_gen]
     // = h_gen (row i+1 = state after step i, row 0 = 0).  The weight-gradient products read them in place (MN-major TMA operands).
-    const bool tc_rows = precision_mode() == B200TTS_PRECISION_BF16 && s.training && tc_persist_supported(s) && persist_att_bwd_supported(s);
+    // A training forward ran those loops exactly when the attention reverse loop runs.
     const PersistLayout prl = persist_layout(s);
     const TcPersistGeom tcg = tc_persist_geom(s);
-    const unsigned char* pws_rows = reinterpret_cast<const unsigned char*>(F(fl.persist));
-    const __nv_bfloat16* aib = tc_rows ? reinterpret_cast<const __nv_bfloat16*>(pws_rows + prl.aib) : nullptr;
-    const __nv_bfloat16* hgb = tc_rows ? reinterpret_cast<const __nv_bfloat16*>(pws_rows + prl.hgb) : nullptr;
+    const unsigned char* pws = reinterpret_cast<const unsigned char*>(F(fl.persist));
+    const __nv_bfloat16* aib = plan.att_bwd ? reinterpret_cast<const __nv_bfloat16*>(pws + prl.aib) : nullptr;
+    const __nv_bfloat16* hgb = plan.att_bwd ? reinterpret_cast<const __nv_bfloat16*>(pws + prl.hgb) : nullptr;
     const int ldab = tcg.Kp_att, ldhb = tcg.Kp_gen;
     const __nv_bfloat16* aib1 = aib ? aib + (size_t)B * ldab : nullptr;      // rows 1..T
     const __nv_bfloat16* hgb1 = hgb ? hgb + (size_t)B * ldhb : nullptr;
@@ -698,17 +699,12 @@ int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_
 
     // ---- 2. generator LSTM reverse loop ----
     const bool zone = s.cell_kind == B200TTS_CELL_ZONEOUT;
-    // the wgmma reverse loops keep their bf16 gate gradients as [T, B, 4D] histories: the time-batched products below read them in place
-    // (K-major for dX, MN-major for dW) instead of converting the fp32 copies
-    const bool hist_gen = precision_mode() == B200TTS_PRECISION_BF16 && persist_bwd_supported(s) && tc_persist_gen_bwd_supported(s) &&
-                          !getenv("B200TTS_NO_DGB_HISTORY");
-    void* dggb = hist_gen ? static_cast<void*>(W(l.dggb)) : nullptr;
-    if (precision_mode() == B200TTS_PRECISION_BF16 && persist_bwd_supported(s)) {
-        // bf16 perf mode: one cooperative weight-stationary kernel for the whole reverse recurrence
-        if (tc_persist_gen_bwd_supported(s))      // TMA + wgmma variant (decoder_persist_bwd_tc.cu)
-            B200_TRY(tc_persist_gen_bwd_loop(s, w, in, fl, fws, W(l.dhgd), W(l.dgg), reinterpret_cast<unsigned char*>(W(l.pextra)), st, dggb));
-        else
-            B200_TRY(persist_gen_bwd_loop(s, w, in, fl, fws, W(l.dhgd), W(l.dgg), reinterpret_cast<unsigned char*>(W(l.pextra)), st));
+    // the persistent reverse loops keep their bf16 gate gradients as [T, B, 4D] histories: the time-batched products below read them in
+    // place (K-major for dX, MN-major for dW) instead of converting the fp32 copies
+    void* dggb = plan.gen_bwd ? static_cast<void*>(W(l.dggb)) : nullptr;
+    if (plan.gen_bwd) {
+        // bf16 perf mode: one cooperative weight-stationary TMA + wgmma kernel for the whole reverse recurrence (decoder_persist_bwd_tc.cu)
+        B200_TRY(tc_persist_gen_bwd_loop(s, w, in, fl, fws, W(l.dhgd), W(l.dgg), reinterpret_cast<unsigned char*>(W(l.pextra)), st, dggb));
     } else {
     for (int i = T - 1; i >= 0; --i) {
             CellBwdArgs ca{};
@@ -746,13 +742,10 @@ int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_
     }
 
     // ---- 3. attention LSTM + attention reverse loop ----
-    const bool persist_att = precision_mode() == B200TTS_PRECISION_BF16 && s.training && (tc_persist_supported(s) || persist_supported(s)) &&
-                             persist_att_bwd_supported(s);
-    void* dgab = (persist_att && persist_att_bwd_tc(s) && !getenv("B200TTS_NO_DGB_HISTORY")) ? static_cast<void*>(W(l.dgab)) : nullptr;
-    if (persist_att) {
+    void* dgab = plan.att_bwd ? static_cast<void*>(W(l.dgab)) : nullptr;
+    if (plan.att_bwd) {
         // bf16 perf mode: cooperative weight-stationary kernel (tensor-core attention backward inside), then a parallel post pass
-        const PersistLayout pl = persist_layout(s);
-        B200_TRY(persist_att_bwd_loop(s, w, in, fl, fws, pl, reinterpret_cast<const unsigned char*>(F(fl.persist)), fwd_out.alignments,
+        B200_TRY(persist_att_bwd_loop(s, w, in, fl, fws, prl, pws, fwd_out.alignments,
                                       dout.d_alignments, W(l.dhas), W(l.dctxs), W(l.dga), W(l.dq), W(l.dctxt), W(l.dmemT),
                                       reinterpret_cast<unsigned char*>(W(l.pextra2)), dw, st, dgab));
     } else {
@@ -810,7 +803,7 @@ int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_
     }
     // d Wq = dQ^T . h_att
     B200_TRY(wgemm16(st, l, bws, A, D, (int)TB, W(l.dq), A, ai1 + M, MD, aib1, ldab, dw.attn_query, D, 1.f));
-    if (!persist_att) {
+    if (!plan.att_bwd) {
         batchsum_add_kernel<<<grid_for((size_t)A * C), 256, 0, st>>>(dw.attn_location, W(l.dWloc_acc), B, (size_t)A * C);
         B200_LAUNCH_CHECK();
         batchsum_add_kernel<<<grid_for((size_t)C * K), 256, 0, st>>>(dw.attn_loc_features, W(l.dWc_acc), B, (size_t)C * K);

@@ -537,20 +537,17 @@ int decoder_forward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_p
     B200_TRY(launch_fill(c.at(l.cum), 0.f, (size_t)B * s.L, st));
     }
 
-    // the persistent forward rounds memory / memT to bf16; only the persistent backward recomputes with the same operands
-    const bool persistent = !sequential && state == nullptr && precision_mode() == B200TTS_PRECISION_BF16 &&
-                            (tc_persist_supported(s) || persist_supported(s)) && (!s.training || persist_att_bwd_supported(s));
+    const bool persistent = !sequential && state == nullptr && precision_mode() == B200TTS_PRECISION_BF16 && persist_plan(s).fwd;
     if (persistent) {
-        // bf16 perf mode: one cooperative, weight-stationary kernel per recurrence (decoder_persist.cu)
+        // bf16 perf mode: one cooperative, weight-stationary TMA + wgmma kernel per recurrence (decoder_persist_tc.cu)
         unsigned char* pws = reinterpret_cast<unsigned char*>(c.at(l.persist));
-        const bool tc = tc_persist_supported(s);         // TMA + wgmma loops (decoder_persist_tc.cu) when D % 64 == 0
+        const TcPersistGeom g = tc_persist_geom(s);
+        const PersistLayout pl = persist_layout(s);
         B200_TRY(persist_att_prep(s, w, in, l, ws, pws, st));
-        B200_TRY(tc ? tc_persist_att_loop(s, w, in, l, ws, pws, out.alignments, st) : persist_att_loop(s, w, in, l, ws, pws, out.alignments, st));
-        if (tc) {
+        B200_TRY(tc_persist_att_loop(s, w, in, l, ws, pws, out.alignments, st));
+        {
             // the attention loop left [h_att | ctx] of every step as bf16 operand rows in exactly the column order of W_ih of the
             // generator LSTM: ONE product, its A operand read by TMA straight from those rows (no packing, no second accumulate pass)
-            const TcPersistGeom g = tc_persist_geom(s);
-            const PersistLayout pl = persist_layout(s);
             GemmDesc d;
             d.A = c.at(l.ai); d.lda = MD;           // (unused by the wgmma path)
             d.A16 = pws + pl.aib + (size_t)B * g.Kp_att * 2; d.lda16 = g.Kp_att;      // operand row 1 (bf16)
@@ -559,14 +556,9 @@ int decoder_forward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_p
             bool handled = false;
             B200_TRY(gemm_tc_try(d, st, &handled));
             if (!handled) B200_TRY(gen_input_proj(c, 0, T));
-        } else {
-            B200_TRY(gen_input_proj(c, 0, T));
         }
-        B200_TRY(tc ? tc_persist_gen_loop(s, w, in, l, ws, pws, st) : persist_gen_loop(s, w, in, l, ws, pws, st));
-        bool fp_done = false;
-        if (tc) {       // frame / stop projection straight from the bf16 operand rows of the two loops (h_gen, then ctx accumulated on top)
-            const TcPersistGeom g = tc_persist_geom(s);
-            const PersistLayout pl = persist_layout(s);
+        B200_TRY(tc_persist_gen_loop(s, w, in, l, ws, pws, st));
+        {       // frame / stop projection straight from the bf16 operand rows of the two loops (h_gen, then ctx accumulated on top)
             const int N1 = N + 1;
             GemmDesc d;
             d.A = c.at(l.hg) + BD; d.lda = D;
@@ -585,10 +577,10 @@ int decoder_forward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_p
                 if (!h2) {      // second half on the generic path
                     B200_TRY(run_gemm(c.st, T * B, N1, M, c.at(l.ai) + (size_t)B * MD, MD, c.at(l.wfs) + D, D + M, true, c.at(l.fs), N1, nullptr, 1.f));
                 }
-                fp_done = true;
+            } else {
+                B200_TRY(frame_proj(c, 0, T));
             }
         }
-        if (!fp_done) B200_TRY(frame_proj(c, 0, T));
     } else if (!sequential) {
         for (int i = 0; i < T; ++i) B200_TRY(att_step(c, i, out.alignments));
         B200_TRY(gen_input_proj(c, 0, T));

@@ -22,11 +22,8 @@ static inline int pick_splitk(int M, int N, int K) {
 
 // Extras of the persistent bf16 kernels (decoder_persist.cu); offsets in BYTES from the region base.
 struct PersistLayout {
-    int Kp_att, Kp_gen, ldm;
-    size_t aib;      // bf16 [T+1, B, Kp_att]  [ctx | h_att] operands
-    size_t hgb;      // bf16 [T+1, B, Kp_gen]  h_gen operands
-    size_t memTb;    // bf16 [B, L, A]
-    size_t memb;     // bf16 [B, L, ldm]
+    size_t aib;      // bf16 [T+1, B, Kp_att]  [h_att | ctx | 0] operands (Kp_att, Kp_gen: TcPersistGeom)
+    size_t hgb;      // bf16 [T+1, B, Kp_gen]  [h_gen | 0] operands
     size_t wcombT;   // f32  [K, A]
     size_t wcb;      // bf16 [A, 40]   Wcomb[a][k]
     size_t memTf;    // bf16 [B, MT, 32, 64] fragment-major memory projection
@@ -38,7 +35,14 @@ struct PersistLayout {
     size_t total;
 };
 PersistLayout persist_layout(const b200tts_decoder_shape& s);
-bool persist_supported(const b200tts_decoder_shape& s);
+
+// Which decoder recurrences run as one persistent TMA + wgmma launch in the bf16 perf mode (decoder_persist.cu); every other shape
+// runs the per-step kernel chains.
+//   fwd:     attention-LSTM + attention loop and generator-LSTM loop (decoder_persist_tc.cu)
+//   gen_bwd: generator-LSTM reverse loop (decoder_persist_bwd_tc.cu)
+//   att_bwd: attention-LSTM + attention reverse loop (decoder_persist_bwd.cu); training only, and only after the persistent forward
+struct PersistPlan { bool fwd = false, gen_bwd = false, att_bwd = false; };
+PersistPlan persist_plan(const b200tts_decoder_shape& s);
 
 // All offsets are in floats from the workspace base.
 struct DecoderLayout {
@@ -109,31 +113,23 @@ int tc_persist_att_loop(const b200tts_decoder_shape& s, const b200tts_decoder_pa
                         const DecoderLayout& fl, float* ws, unsigned char* pws, float* align, cudaStream_t st);
 int tc_persist_gen_loop(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
                         const DecoderLayout& fl, float* ws, unsigned char* pws, cudaStream_t st);
-// attention operands of the persistent loops (bf16 memory, Wcomb, fragment-major projections) -> persistent workspace
+// attention operands of the persistent loops (Wcomb, fragment-major projections) -> persistent workspace
 int persist_att_prep(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
                      const DecoderLayout& fl, float* ws, unsigned char* pws, cudaStream_t st);
-int persist_att_loop(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
-                     const DecoderLayout& fl, float* ws, unsigned char* pws, float* align, cudaStream_t st);
-struct AttBwdExtra { int MT; size_t dgb, part, wcb, wcb2, memTf, de, dwpart, dvpart, barrier, total; };
+struct AttBwdExtra { int MT; size_t part, wcb, wcb2, memTf, de, dwpart, dvpart, barrier, total; };
 AttBwdExtra att_bwd_extra(const b200tts_decoder_shape& s);
 bool persist_att_bwd_supported(const b200tts_decoder_shape& s);
-bool persist_att_bwd_tc(const b200tts_decoder_shape& s);      // true: the wgmma product variant is the one picked
+// dgb_hist: [T, B, 4D] bf16 history of the gate gradients (out), read in place by the time-batched weight-gradient products
 int persist_att_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
                          const DecoderLayout& fl, const float* fws, const PersistLayout& pl, const unsigned char* pws,
                          const float* align, const float* dalign, const float* dh_static, const float* dctx_static, float* dgates,
                          float* dq, float* dctx_tot, float* dmemT, unsigned char* extra, const b200tts_decoder_params& dw,
-                         cudaStream_t st, void* dgb_hist = nullptr);      // dgb_hist: optional [T, B, 4D] bf16 history of the gate gradients
-bool persist_bwd_supported(const b200tts_decoder_shape& s);
+                         cudaStream_t st, void* dgb_hist);
 size_t persist_bwd_gen_extra_bytes(const b200tts_decoder_shape& s);
-int persist_gen_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
-                         const DecoderLayout& fl, const float* fws, const float* dh_static, float* dgates, unsigned char* extra,
-                         cudaStream_t st);
 bool tc_persist_gen_bwd_supported(const b200tts_decoder_shape& s);
 int tc_persist_gen_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
                             const DecoderLayout& fl, const float* fws, const float* dh_static, float* dgates, unsigned char* extra,
-                            cudaStream_t st, void* dgb_hist = nullptr);
-int persist_gen_loop(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
-                     const DecoderLayout& fl, float* ws, unsigned char* pws, cudaStream_t st);
+                            cudaStream_t st, void* dgb_hist);
 
 // ---- LSTM cell kernels (decoder_fwd.cu / decoder_bwd.cu), shared with the encoder bi-LSTM ----
 struct CellFwdArgs {

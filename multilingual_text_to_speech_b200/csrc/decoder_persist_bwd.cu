@@ -1,16 +1,20 @@
-// Persistent recurrent kernels of the bf16 perf mode (backward): reverse-time LSTM loops.
+// Persistent attention-LSTM + attention reverse loop of the bf16 perf mode (TMA + wgmma + CTA pairs), and its parallel post pass.
 //
-// Per reverse step the recurrence needs  d x_{i-1} = dgates_i . W   (K = 4D gate rows -> N output columns), the
-// transpose of the forward product.  2-D weight-stationary partition: CTA (kb, nb, bh) keeps the bf16 block
-// W[K-block kb (4 x UK gate rows), N-block nb] in shared memory for the whole sequence, owns a batch half, and
-//   P1  runs the LSTM-cell backward for a 1/NB share of its K-block's hidden units (dgates -> fp32 for the dW GEMMs,
-//       bf16 for the tensor cores),
+// Reverse step i needs  [d ctx | d h_att]_{i-1} = dgates_i . [W_ih[:, P:] | W_hh]  (K = 4D gate rows -> M + D output columns), the
+// transpose of the forward product.  CTA (kb, nb) of 8 x 16 keeps W^T[n-block of 80 outputs (96 for memory dim 512), K-slice kb of
+// 4 x D/8 gate rows] in shared memory as K-major SWIZZLE_128B tiles (wgmma B operand) for the whole sequence.  Per step:
+//   PA  attention backward of one utterance per CTA pair (cluster of 2): d weights, softmax backward, energies backward and d cum on
+//       the tensor cores (mma.sync), the two ranks exchanging partials through distributed shared memory;
 //   --  grid barrier
-//   P2  streams the bf16 dgates of its K-block (32 x 4UK) and multiplies (warps split N; ldmatrix.trans B fragments)
-//       writing an fp32 partial [32 x UN] that the next step's P1 sums over the KB K-blocks (deterministic order),
+//   PB  LSTM-cell backward of 8 hidden units x every utterance (CTAs < D/8): gate gradients -> fp32 for the weight-gradient products
+//       and a bf16 [T, B, 4D] history;
+//   --  grid barrier (gate gradients of all units visible)
+//   P2  ONE 5-D TMA box brings the bf16 gate gradients of the K-slice for the whole batch (<= 64 utterances, rows beyond B zero-filled),
+//       the A operand (M = 64); warpgroup 0 runs wgmma m64n80k16 / m64n96k16 and stores the fp32 partial [B x n-block] that the next
+//       step sums over the 8 K-slices (fixed order, no atomics);
 //   --  grid barrier.
-// Reference semantics: autograd replay of modules/layers.py:18-47 (train.py:83).
-#include <stdlib.h>
+// The post pass then accumulates, in parallel over all steps, what the recurrence does not need: d memT, d Wcomb, d v.
+// Reference semantics: autograd replay of modules/layers.py:18-47 and modules/attention.py:39-86 (train.py:83).
 #include <cuda_bf16.h>
 #include "decoder_internal.cuh"
 #include "tc_ptx.cuh"
@@ -20,48 +24,15 @@ namespace b200tts {
 namespace {
 
 constexpr int PT = 256;
-constexpr int BT = 32;
-constexpr int KB = 8;            // K-blocks (over hidden units)
-constexpr int NBK = 8;           // N-blocks (over output columns)
 
-struct BwdLoopArgs {
-    int B, T, D, NOUT, UK, UN, NBH;        // NOUT output columns (D for the generator loop), UN = ceil(NOUT / NBK / 8) * 8
-    const float* W; int ldw;               // fp32 [4D, ldw]: dgates . W
-    const float* gates;                    // [T, B, 4D] activated gates (forward)
-    const float* cstate;                   // [T+1, B, D]
-    const float* dh_static;                // [T, B, D]
-    const uint8_t* mask_h; const uint8_t* mask_c;
-    int kind, training; float rate_h, rate_c;
-    float* dgates;                         // [T, B, 4D] out (fp32)
-    __nv_bfloat16* dgb;                    // [B, 4D] staging (bf16)
-    float* part;                           // [KB, B, NOUT] partial products of the previous reverse step
-    int hcol;                              // column of d h inside the NOUT outputs (0 for the generator loop)
-    unsigned* barrier; int* abort_flag;
-    long long* prof;
-};
-
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
-    const uint32_t s = (uint32_t)__cvta_generic_to_shared(smem);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gmem));
-}
-__device__ __forceinline__ void cp_async_commit_wait() { asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;\n" ::); }
 __device__ __forceinline__ void ldmatrix_x4(uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3, const void* p) {
     const uint32_t addr = (uint32_t)__cvta_generic_to_shared(p);
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3, const void* p) {
-    const uint32_t addr = (uint32_t)__cvta_generic_to_shared(p);
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];\n" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
 }
 __device__ __forceinline__ void mma_bf16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
     asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
                  : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ unsigned ld_acquire(const unsigned* p) {
-    unsigned v;
-    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];\n" : "=r"(v) : "l"(p) : "memory");
-    return v;
 }
 struct NoOverlap { __device__ __forceinline__ void operator()() const {} };
 // `overlap` runs on every thread BETWEEN the CTA's arrival and its wait: work that does not depend on other CTAs (next step's operand
@@ -98,14 +69,9 @@ __device__ __forceinline__ bool grid_barrier(unsigned* counter, unsigned& target
     return s_ok != 0;
 }
 
-// thread-block cluster (CTA pair) primitives: split arrive / wait barrier and a distributed-shared-memory store
+// thread-block cluster (CTA pair) split arrive / wait barrier
 __device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
 __device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
-__device__ __forceinline__ void st_peer_f32(const float* local_smem, uint32_t peer_rank, float v) {
-    uint32_t ra;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"((uint32_t)__cvta_generic_to_shared(local_smem)), "r"(peer_rank));
-    asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(ra), "f"(v) : "memory");
-}
 __device__ __forceinline__ void l2_prefetch(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 // remote store that completes its 4 bytes on the PEER's mbarrier (data + signal in one instruction): the pair exchanges need no cluster
 // barrier and none of the memory fence its release semantics imply
@@ -129,166 +95,27 @@ __device__ __forceinline__ float tanh_exp(float x) { return 2.f * __fdividef(1.f
             for (int k9 = 0; k9 < 8; ++k9) p.prof[(size_t)blockIdx.x * 8 + k9] = prof_acc[k9];                   \
     } while (0)
 
-// Generator-LSTM reverse loop (no attention): NOUT = D.
-__global__ void __launch_bounds__(PT, 1) lstm_bwd_loop_kernel(const BwdLoopArgs p) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int cta = blockIdx.x;
-    const int kb = cta % KB, nb = (cta / KB) % NBK, bh = cta / (KB * NBK);
-    const int B = p.B, D = p.D, UK = p.UK, UN = p.UN, KROWS = 4 * UK;
-    const int WLD = UN + 8, ALD = KROWS + 8;
-    const int b0 = bh * BT, n0 = nb * UN;
-    __nv_bfloat16* Ws = reinterpret_cast<__nv_bfloat16*>(smem_raw);                 // [KROWS][WLD]  (k rows, n contiguous)
-    __nv_bfloat16* As = Ws + (size_t)KROWS * WLD;                                    // [BT][ALD]
-    const unsigned nblocks = gridDim.x;
-
-    // resident weight block: row r = g*UK + uk  <->  gate row g*D + kb*UK + uk ; column n <-> output n0 + n
-    for (int idx = tid; idx < KROWS * UN; idx += PT) {
-        const int r = idx / UN, n = idx % UN;
-        const int g = r / UK, uk = r % UK;
-        float w = 0.f;
-        if (n0 + n < p.NOUT) w = p.W[(size_t)(g * D + kb * UK + uk) * p.ldw + n0 + n];
-        Ws[r * WLD + n] = __float2bfloat16_rn(w);
-    }
-    __syncthreads();
-
-    // P1 ownership: hidden units [kb*UK + nb*UP, +UP) with UP = UK / NBK, for the 32 utterances of this batch half
-    const int UP = UK / NBK;
-    const float inv_h = 1.f / (1.f - p.rate_h), inv_c = 1.f / (1.f - p.rate_c);
-    constexpr int MAXE = 4;                       // (b, u) pairs per thread: BT * UP / PT  (UP <= 32)
-    float dc_reg[MAXE], dhz_reg[MAXE];
-#pragma unroll
-    for (int e = 0; e < MAXE; ++e) { dc_reg[e] = 0.f; dhz_reg[e] = 0.f; }
-    unsigned target = 0;
-    BPROF_DECL
-
-    for (int i = p.T - 1; i >= 0; --i) {
-        const bool last = (i == p.T - 1);
-        // ---------------- P1: LSTM cell backward ----------------
-#pragma unroll
-        for (int e = 0; e < MAXE; ++e) {
-            const int idx = tid + e * PT;
-            if (idx < BT * UP) {
-                const int bl = idx / UP, up = idx % UP, b = b0 + bl, u = kb * UK + nb * UP + up;
-                if (b < B) {
-                    const size_t bu = (size_t)b * D + u, g0 = ((size_t)i * B + b) * 4 * D + u;
-                    float dh = p.dh_static[(size_t)i * B * D + bu];
-                    float dc_in = 0.f;
-                    if (!last) {
-                        float rec = 0.f;
-                        for (int k2 = 0; k2 < KB; ++k2) rec += __ldcg(p.part + ((size_t)k2 * B + b) * p.NOUT + p.hcol + u);
-                        dh += rec + dhz_reg[e];
-                        dc_in = dc_reg[e];
-                    }
-                    const float gi = p.gates[g0], gf = p.gates[g0 + D], gg = p.gates[g0 + 2 * D], go = p.gates[g0 + 3 * D];
-                    const float cp = p.cstate[(size_t)i * B * D + bu];
-                    const float tc = tanhf(gf * cp + gi * gg);
-                    const size_t mi = (size_t)i * B * D + bu;
-                    float dhn, dcn, dc_prev_direct = 0.f, dh_prev_direct = 0.f;
-                    if (p.kind == B200TTS_CELL_ZONEOUT) {
-                        float kh, kc;
-                        if (p.training) {
-                            kh = (1.f - p.rate_h) * (p.mask_h ? (float)p.mask_h[mi] * inv_h : 1.f);
-                            kc = (1.f - p.rate_c) * (p.mask_c ? (float)p.mask_c[mi] * inv_c : 1.f);
-                        } else { kh = 1.f - p.rate_h; kc = 1.f - p.rate_c; }
-                        dhn = dh * kh; dh_prev_direct = dh - dhn;
-                        dcn = dc_in * kc + dhn * go * (1.f - tc * tc);
-                        dc_prev_direct = dc_in - dc_in * kc;
-                    } else {
-                        dhn = (p.training && p.mask_h) ? dh * (float)p.mask_h[mi] * inv_h : dh;
-                        dcn = dc_in + dhn * go * (1.f - tc * tc);
-                    }
-                    const float di = dcn * gg * gi * (1.f - gi), df = dcn * cp * gf * (1.f - gf);
-                    const float dg = dcn * gi * (1.f - gg * gg), dO = dhn * tc * go * (1.f - go);
-                    p.dgates[g0] = di; p.dgates[g0 + D] = df; p.dgates[g0 + 2 * D] = dg; p.dgates[g0 + 3 * D] = dO;
-                    __nv_bfloat16* db = p.dgb + (size_t)b * 4 * D + u;
-                    db[0] = __float2bfloat16_rn(di); db[D] = __float2bfloat16_rn(df);
-                    db[2 * D] = __float2bfloat16_rn(dg); db[3 * D] = __float2bfloat16_rn(dO);
-                    dc_reg[e] = dcn * gf + dc_prev_direct;
-                    dhz_reg[e] = dh_prev_direct;
-                }
-            }
-        }
-        BPROF_MARK(0);
-        if (!grid_barrier(p.barrier, target, nblocks, p.abort_flag)) return;
-        BPROF_MARK(1);
-        if (i == 0) break;
-
-        // ---------------- P2: partial[kb] = dgates[:, K-block kb] . W[K-block kb, N-block nb] ----------------
-        {
-            const int segs = UK / 8;                       // 16-byte segments per gate block per row
-            for (int idx = tid; idx < BT * 4 * segs; idx += PT) {
-                const int r = idx / (4 * segs), rem = idx % (4 * segs), g = rem / segs, sg = rem % segs;
-                __nv_bfloat16* d = As + r * ALD + g * UK + sg * 8;
-                if (b0 + r < B) cp_async16(d, p.dgb + (size_t)(b0 + r) * 4 * D + g * D + kb * UK + sg * 8);
-                else *reinterpret_cast<uint4*>(d) = make_uint4(0u, 0u, 0u, 0u);
-            }
-            cp_async_commit_wait();
-            __syncthreads();
-            // warps split N: warp w owns n-tile pairs {w, w+8, ...} (16 columns each)
-            const int npairs = UN / 16;
-            for (int np = warp; np < npairs; np += 8) {
-                float acc[2][2][4];
-#pragma unroll
-                for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-                    for (int nt = 0; nt < 2; ++nt)
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) acc[mt][nt][e] = 0.f;
-                for (int kk = 0; kk < KROWS; kk += 16) {
-                    uint32_t af[2][4], bf[4];
-#pragma unroll
-                    for (int mt = 0; mt < 2; ++mt)
-                        ldmatrix_x4(af[mt][0], af[mt][1], af[mt][2], af[mt][3], As + (mt * 16 + (lane & 15)) * ALD + kk + (lane >> 4) * 8);
-                    ldmatrix_x4_trans(bf[0], bf[1], bf[2], bf[3],
-                                      Ws + (size_t)(kk + (lane & 7) + ((lane >> 3) & 1) * 8) * WLD + np * 16 + (lane >> 4) * 8);
-#pragma unroll
-                    for (int mt = 0; mt < 2; ++mt) {
-                        mma_bf16(acc[mt][0], af[mt], bf[0], bf[1]);
-                        mma_bf16(acc[mt][1], af[mt], bf[2], bf[3]);
-                    }
-                }
-                const int g = lane >> 2, tq = lane & 3;
-#pragma unroll
-                for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-                    for (int nt = 0; nt < 2; ++nt)
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            const int b = b0 + mt * 16 + g + 8 * (e >> 1);
-                            const int n = n0 + np * 16 + nt * 8 + 2 * tq + (e & 1);
-                            if (b < B && n < p.NOUT) p.part[((size_t)kb * B + b) * p.NOUT + n] = acc[mt][nt][e];
-                        }
-            }
-        }
-        if (!grid_barrier(p.barrier, target, nblocks, p.abort_flag)) return;
-    }
-}
-
-
 // =================================================================================================
 // Attention-LSTM + attention reverse loop
 // =================================================================================================
-constexpr int KBA = 8;            // K-blocks of the attention-loop product (over hidden units)
-constexpr int NBA = 9;            // N-blocks over the M + D output columns  -> 8 x 9 x 2 = 144 CTAs
+constexpr int KBA = 8;            // K-slices of the product (over hidden units)
 constexpr int GLD = 33;           // row stride of the G tile buffer (floats)
-// wgmma variant of the product: CTA (kb, nb) of 8 x 16 keeps W^T[n-block of 80 outputs, K-slice kb] as K-major SWIZZLE_128B tiles (wgmma B
-// operand, N = 80); the whole batch (<= 64 utterances, TMA zero-fills the rest) is the A operand (M = 64), ONE 5-D TMA box per step
-constexpr int NBT = 16;           // n-blocks of the wgmma variant  -> 8 x 16 = 128 CTAs (64 pairs): one per SM of the 132
+constexpr int NBT = 16;           // n-blocks of the product  -> 8 x 16 = 128 CTAs (64 pairs): one per SM of the 132
 constexpr int TUN = 80;           // outputs per n-block (wgmma N); TUN_WIDE when M + D > NBT * TUN (memory dim 512)
 constexpr int TUN_WIDE = 96;
 
 struct AttBwdArgs {
-    int B, T, D, M, L, A, KC, NOUT, UK, UN, NBH, MT;      // NOUT = M + D, MT = ceil(L / 16)
+    int B, T, D, M, L, A, KC, NOUT, UK, UN, MT;           // NOUT = M + D, UK = D / KBA, MT = ceil(L / 16)
     const float* W; int ldw;                              // wcat_att fp32 [4D, M + D]
     const float* gates; const float* cstate;              // forward saves
     const float* dh_static;                               // [T, B, D]   (from the generator input projection)
     const float* dctx_static;                             // [T, B, M]
     const uint8_t* mask_h; const uint8_t* mask_c;
     int kind, training; float rate_h, rate_c;
-    float* dgates; __nv_bfloat16* dgb; float* part;       // as in BwdLoopArgs; part [KBA, B, NOUT]
-    long long dgb_step;                                   // bf16 gate gradients: 0 = [B, 4D] staging reused every step, B * 4D = [T, B, 4D] history
-    int dgb_rows;                                         // rows of one step inside the TMA source (0 for the staging, B for the history)
+    float* dgates;                                        // [T, B, 4D] out (fp32)
+    __nv_bfloat16* dgb;                                   // [T, B, 4D] out: bf16 history of the gate gradients, TMA source of the product
+    long long dgb_step; int dgb_rows;                     // elements (B * 4D) and TMA rows (B) of one step of the history
+    float* part;                                          // [KBA, B, NOUT] partial products of the previous reverse step
     // attention
     const float* q; const float* cum; const float* align; long long align_bstride;
     const float* dalign; long long dalign_bstride;        // may be null
@@ -296,10 +123,8 @@ struct AttBwdArgs {
     const __nv_bfloat16* WcB;                             // [A][40]   Wcomb[a][k], k contiguous (k >= KC zero)
     const __nv_bfloat16* WcB2;                            // [32][A+8] Wcomb^T[k][a], a contiguous
     const __nv_bfloat16* memTf;                           // [B][MT][32 lanes][64] fragment-major memory projection
-    const __nv_bfloat16* memb; int ldm;                   // [B, L, ldm]
     const uint4* memFb; int M16;                          // [B][MT][M16][32] A fragments (rows = positions, k = memory dims), bf16
     const int* lengths;
-    int dqp_after_g;                                      // 1: dq partials live after the G tile buffer, 0: alias the scratch head
     float* dctx_tot;                                      // [T, B, M] out
     float* dq;                                            // [T, B, A] out
     float* de;                                            // [T, B, L] out (softmax-backward energies, consumed by the post pass)
@@ -317,41 +142,23 @@ __device__ __forceinline__ float tanh_fast(float x) {
     return y;
 }
 
-// Build the Toeplitz pair arrays of the zero-padded cumulative weights: Ph[x] = (hi[x], hi[x+1]), Pl likewise, where
-// cumpad[j] = cum[j - half] and cum = hi + lo with hi, lo in bf16 (16 mantissa bits in total).
-__device__ __forceinline__ void build_pairs(uint32_t* Ph, uint32_t* Pl, const float* cum, int L, int half, int n, int tid, int nthreads) {
-    for (int x = tid; x < n; x += nthreads) {
-        float c0 = 0.f, c1 = 0.f;
-        const int l0 = x - half, l1 = x + 1 - half;
-        if (l0 >= 0 && l0 < L) c0 = __ldcg(cum + l0);
-        if (l1 >= 0 && l1 < L) c1 = __ldcg(cum + l1);
-        const __nv_bfloat16 h0 = __float2bfloat16_rn(c0), h1 = __float2bfloat16_rn(c1);
-        const float r0 = c0 - __bfloat162float(h0), r1 = c1 - __bfloat162float(h1);
-        __nv_bfloat162 hp; hp.x = h0; hp.y = h1;
-        Ph[x] = *reinterpret_cast<uint32_t*>(&hp);
-        Pl[x] = pack2(r0, r1);
-    }
-}
-
-// UNC: outputs per n-block of the wgmma product (wgmma N), compile-time (80, or 96 for memory dim 512); 0 for the mma.sync variant
-template <bool TC, int UNC>
+// UNC: outputs per n-block of the product (wgmma N), compile-time: 80, or 96 for memory dim 512
+template <int UNC>
 __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_constant__ CUtensorMap tmG, const AttBwdArgs p) {
     extern __shared__ __align__(1024) unsigned char smem_raw0[];
     unsigned char* smem_raw = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw0) + 1023) & ~(uintptr_t)1023);
     __shared__ uint64_t full_bar, xb1, xb2;      // xb1 / xb2: arrival of the peer's softmax dot / query-gradient partial + G halo tile
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int cta = blockIdx.x;
-    const int kb = cta % KBA, nb = TC ? cta / KBA : (cta / KBA) % NBA, bh = TC ? 0 : cta / (KBA * NBA);
+    const int kb = cta % KBA, nb = cta / KBA;
     const int B = p.B, D = p.D, UK = p.UK, UN = p.UN, KROWS = 4 * UK, M = p.M, L = p.L, A = p.A;
-    const int WLD = UN + 8, ALD = KROWS + 8;
-    const int b0 = bh * BT, n0 = nb * UN;
-    const int NKT = KROWS / 64;                                                      // TC: k-block tiles of the K-slice
-    // mma.sync: Ws [KROWS][WLD] bf16, As [BT][ALD] bf16.  wgmma: sW [NKT][UN rows][128 B] swizzled, slot [NKT][64 rows][128 B] (one TMA box).
-    // The activation stage `As` doubles as the attention scratch / query-gradient staging in both variants.
-    __nv_bfloat16* Ws = reinterpret_cast<__nv_bfloat16*>(smem_raw);
+    const int n0 = nb * UN;
+    const int NKT = KROWS / 64;                                                      // k-block tiles of the K-slice
+    // sW [NKT][UN rows][128 B] swizzled, slot As [NKT][64 rows][128 B] (one TMA box).  The slot doubles as the attention scratch and
+    // the query-gradient staging.
     unsigned char* sW = smem_raw;
-    __nv_bfloat16* As = TC ? reinterpret_cast<__nv_bfloat16*>(smem_raw + (size_t)NKT * UN * 128) : Ws + (size_t)KROWS * WLD;
-    unsigned char* extra = TC ? reinterpret_cast<unsigned char*>(As) + (size_t)NKT * 8192 : reinterpret_cast<unsigned char*>(As + (size_t)BT * ALD);
+    __nv_bfloat16* As = reinterpret_cast<__nv_bfloat16*>(smem_raw + (size_t)NKT * UN * 128);
+    unsigned char* extra = reinterpret_cast<unsigned char*>(As) + (size_t)NKT * 8192;
     __nv_bfloat16* sWcB = reinterpret_cast<__nv_bfloat16*>(extra);                   // [A][40]
     __nv_bfloat16* sWcB2 = sWcB + (size_t)A * 40;                                    // [32][A+8]
     float* dcum = reinterpret_cast<float*>(sWcB2 + (size_t)32 * (A + 8));            // [L16 + 32] persistent d cum
@@ -364,12 +171,9 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
         const int g = r / UK, uk = r % UK;
         float w = 0.f;
         if (n0 + n < p.NOUT) w = p.W[(size_t)(g * D + kb * UK + uk) * p.ldw + n0 + n];
-        if (TC) {       // W^T[n][k] of k-block tile c = r / 64 (same order as the TMA box: gate-major, then 64-row halves), SWIZZLE_128B
-            const int c = r >> 6, kc = r & 63;
-            *reinterpret_cast<__nv_bfloat16*>(sW + (size_t)c * UN * 128 + n * 128 + ((((kc >> 3) ^ (n & 7))) << 4) + (kc & 7) * 2) = __float2bfloat16_rn(w);
-        } else {
-            Ws[r * WLD + n] = __float2bfloat16_rn(w);
-        }
+        // W^T[n][k] of k-block tile c = r / 64 (same order as the TMA box: gate-major, then 64-row halves), SWIZZLE_128B
+        const int c = r >> 6, kc = r & 63;
+        *reinterpret_cast<__nv_bfloat16*>(sW + (size_t)c * UN * 128 + n * 128 + ((((kc >> 3) ^ (n & 7))) << 4) + (kc & 7) * 2) = __float2bfloat16_rn(w);
     }
     for (int idx = tid; idx < A * 40; idx += PT) sWcB[idx] = p.WcB[idx];
     for (int idx = tid; idx < 32 * (A + 8); idx += PT) sWcB2[idx] = p.WcB2[idx];
@@ -382,10 +186,8 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
         for (int idx = tid; idx < A * UOWN; idx += PT) wq8[(idx / UOWN) * (UOWN + 1) + idx % UOWN] = p.Wq[(size_t)(idx / UOWN) * D + uo0 + idx % UOWN];
     uint32_t prod_it = 0;
     if (tid == 0) { tcx::mbar_init(&xb1, 1); tcx::mbar_init(&xb2, 1); tcx::mbar_init_fence(); }
-    if (TC) {
-        if (tid == 0) { tcx::mbar_init(&full_bar, 1); tcx::mbar_init_fence(); }
-        tcx::proxy_fence_shared();           // the weight tiles were written through the generic proxy; wgmma reads them through the async proxy
-    }
+    if (tid == 0) { tcx::mbar_init(&full_bar, 1); tcx::mbar_init_fence(); }
+    tcx::proxy_fence_shared();           // the weight tiles were written through the generic proxy; wgmma reads them through the async proxy
     __syncthreads();
     cluster_arrive(); cluster_wait();      // one-time: the peer's exchange mbarriers are initialised before the first remote st.async targets them
 
@@ -846,95 +648,49 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
         BPROF_MARK(3);
         // the operands of the next cell backward are fetched between this CTA's arrival and its wait (the compiler parks them in local
         // memory, i.e. the thread waits for the loads right there: under the barrier that wait is free)
-        if (!grid_barrier(p.barrier, target, nblocks, p.abort_flag, TC, [&]() { pb_prefetch(i - 1); })) break;
+        if (!grid_barrier(p.barrier, target, nblocks, p.abort_flag, true, [&]() { pb_prefetch(i - 1); })) break;
         BPROF_MARK(4);
         if (i == 0) break;
 
         // =========================== P2: [d ctx | d h](i-1) partial = dgates_i[:, kb] . W[kb, nb] ===========================
-        if (TC) {
-            // TMA: the bf16 gate gradients of the K-slice, all utterances (rows >= B zero-filled), as NKT swizzled [64 x 64] tiles in ONE box;
-            // wgmma: D[b, n] (registers of warpgroup 0: 64 utterances x UN outputs) = sum over the tiles, stored straight to the partials
-            if (warp == 0) {
-                if (tcx::elect_one()) {
-                    tcx::proxy_fence_shared();       // the slot was last touched through the generic proxy (attention scratch, dq staging)
-                    tcx::proxy_fence_global();
-                    tcx::mbar_expect_tx(&full_bar, (uint32_t)NKT * 8192);
-                    tcx::tma_load_5d(As, &tmG, &full_bar, 0, i * p.dgb_rows, 0, kb, 0);
-                }
-                __syncwarp();
+        // TMA: the bf16 gate gradients of the K-slice, all utterances (rows >= B zero-filled), as NKT swizzled [64 x 64] tiles in ONE box;
+        // wgmma: D[b, n] (registers of warpgroup 0: 64 utterances x UN outputs) = sum over the tiles, stored straight to the partials
+        if (warp == 0) {
+            if (tcx::elect_one()) {
+                tcx::proxy_fence_shared();       // the slot was last touched through the generic proxy (attention scratch, dq staging)
+                tcx::proxy_fence_global();
+                tcx::mbar_expect_tx(&full_bar, (uint32_t)NKT * 8192);
+                tcx::tma_load_5d(As, &tmG, &full_bar, 0, i * p.dgb_rows, 0, kb, 0);
             }
-            if (warp < 4) {
-                constexpr int NR = UNC > 0 ? UNC / 2 : 1;
-                float acc[NR];
-                tcx::mbar_wait(&full_bar, prod_it & 1);
-                tcx::wgmma_fence();
-                for (int c = 0; c < NKT; ++c) {
-                    const uint64_t adesc = tcx::make_sw128_desc(tcx::smem_u32(reinterpret_cast<unsigned char*>(As) + (size_t)c * 8192));
-                    const uint64_t bdesc = tcx::make_sw128_desc(tcx::smem_u32(sW + (size_t)c * UN * 128));
+            __syncwarp();
+        }
+        if (warp < 4) {
+            constexpr int NR = UNC / 2;
+            float acc[NR];
+            tcx::mbar_wait(&full_bar, prod_it & 1);
+            tcx::wgmma_fence();
+            for (int c = 0; c < NKT; ++c) {
+                const uint64_t adesc = tcx::make_sw128_desc(tcx::smem_u32(reinterpret_cast<unsigned char*>(As) + (size_t)c * 8192));
+                const uint64_t bdesc = tcx::make_sw128_desc(tcx::smem_u32(sW + (size_t)c * UN * 128));
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        if constexpr (UNC == TUN_WIDE) tcx::wgmma_m64n96<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (c | k) != 0);
-                        else if constexpr (UNC == TUN) tcx::wgmma_m64n80<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (c | k) != 0);
-                    }
-                }
-                tcx::wgmma_commit();
-                tcx::wgmma_wait<0>();
-                tcx::wgmma_fence_acc(acc);
-                // fragment: utterance b = 16 warp + lane / 4 + 8 ((r / 2) % 2), output n0 + 8 (r / 4) + 2 (lane % 4) + r % 2 (NOUT % 4 == 0: a pair
-                // is either wholly inside or wholly outside)
-                const int brow = 16 * warp + (lane >> 2), ncol = n0 + 2 * (lane & 3);
-#pragma unroll
-                for (int r = 0; r < NR; r += 2) {
-                    const int b = brow + 8 * ((r >> 1) & 1), n = ncol + 8 * (r >> 2);
-                    if (b < B && n < p.NOUT) *reinterpret_cast<float2*>(p.part + ((size_t)kb * B + b) * p.NOUT + n) = make_float2(acc[r], acc[r + 1]);
+                for (int k = 0; k < 4; ++k) {
+                    if constexpr (UNC == TUN_WIDE) tcx::wgmma_m64n96<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (c | k) != 0);
+                    else if constexpr (UNC == TUN) tcx::wgmma_m64n80<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (c | k) != 0);
                 }
             }
-            ++prod_it;
-        } else {
-            const int segs = UK / 8;
-            for (int idx = tid; idx < BT * 4 * segs; idx += PT) {
-                const int r = idx / (4 * segs), rem = idx % (4 * segs), g = rem / segs, sg = rem % segs;
-                __nv_bfloat16* d = As + r * ALD + g * UK + sg * 8;
-                if (b0 + r < B) cp_async16(d, p.dgb + (size_t)i * p.dgb_step + (size_t)(b0 + r) * 4 * D + g * D + kb * UK + sg * 8);
-                else *reinterpret_cast<uint4*>(d) = make_uint4(0u, 0u, 0u, 0u);
-            }
-            cp_async_commit_wait();
-            __syncthreads();
-            const int npairs = UN / 16;
-            for (int np = warp; np < npairs; np += 8) {
-                float acc[2][2][4];
+            tcx::wgmma_commit();
+            tcx::wgmma_wait<0>();
+            tcx::wgmma_fence_acc(acc);
+            // fragment: utterance b = 16 warp + lane / 4 + 8 ((r / 2) % 2), output n0 + 8 (r / 4) + 2 (lane % 4) + r % 2 (NOUT % 4 == 0: a pair
+            // is either wholly inside or wholly outside)
+            const int brow = 16 * warp + (lane >> 2), ncol = n0 + 2 * (lane & 3);
 #pragma unroll
-                for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-                    for (int nt = 0; nt < 2; ++nt)
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) acc[mt][nt][e] = 0.f;
-                for (int kk = 0; kk < KROWS; kk += 16) {
-                    uint32_t af[2][4], bf[4];
-#pragma unroll
-                    for (int mt = 0; mt < 2; ++mt)
-                        ldmatrix_x4(af[mt][0], af[mt][1], af[mt][2], af[mt][3], As + (mt * 16 + (lane & 15)) * ALD + kk + (lane >> 4) * 8);
-                    ldmatrix_x4_trans(bf[0], bf[1], bf[2], bf[3],
-                                      Ws + (size_t)(kk + (lane & 7) + ((lane >> 3) & 1) * 8) * WLD + np * 16 + (lane >> 4) * 8);
-#pragma unroll
-                    for (int mt = 0; mt < 2; ++mt) {
-                        mma_bf16(acc[mt][0], af[mt], bf[0], bf[1]);
-                        mma_bf16(acc[mt][1], af[mt], bf[2], bf[3]);
-                    }
-                }
-                const int g = lane >> 2, tq = lane & 3;
-#pragma unroll
-                for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-                    for (int nt = 0; nt < 2; ++nt)
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            const int b = b0 + mt * 16 + g + 8 * (e >> 1);
-                            const int n = n0 + np * 16 + nt * 8 + 2 * tq + (e & 1);
-                            if (b < B && n < p.NOUT) p.part[((size_t)kb * B + b) * p.NOUT + n] = acc[mt][nt][e];
-                        }
+            for (int r = 0; r < NR; r += 2) {
+                const int b = brow + 8 * ((r >> 1) & 1), n = ncol + 8 * (r >> 2);
+                if (b < B && n < p.NOUT) *reinterpret_cast<float2*>(p.part + ((size_t)kb * B + b) * p.NOUT + n) = make_float2(acc[r], acc[r + 1]);
             }
         }
+        ++prod_it;
         BPROF_MARK(5);
         if (!grid_barrier(p.barrier, target, nblocks, p.abort_flag)) break;
         BPROF_MARK(6);
@@ -1181,13 +937,6 @@ __global__ void att_bwd_finish_kernel(float* __restrict__ dWloc, float* __restri
 
 }  // namespace
 
-bool persist_bwd_supported(const b200tts_decoder_shape& s) {
-    if (s.D % (KB * 16) != 0 || s.B > 2 * BT) return false;
-    const int UK = s.D / KB;
-    if (UK / NBK > 32 || (UK % NBK) != 0) return false;
-    return true;
-}
-
 // -------------------------------------------------------------------------------------------------
 // attention loop, host side
 // -------------------------------------------------------------------------------------------------
@@ -1196,7 +945,6 @@ AttBwdExtra att_bwd_extra(const b200tts_decoder_shape& s) {
     size_t off = 0;
     auto take = [&](size_t n) { size_t o = off; off = (off + n + 255) / 256 * 256; return o; };
     x.MT = (s.L + 15) / 16;
-    x.dgb = take((size_t)s.B * 4 * s.D * 2);
     x.part = take((size_t)KBA * s.B * (s.M + s.D) * 4);
     x.wcb = take((size_t)s.A * 40 * 2);
     x.wcb2 = take((size_t)32 * (s.A + 8) * 2);
@@ -1209,60 +957,38 @@ AttBwdExtra att_bwd_extra(const b200tts_decoder_shape& s) {
     return x;
 }
 
-// Geometry of the two product variants of the attention reverse loop.
+// Geometry of the attention reverse loop.
 struct AttBwdGeom {
-    bool tc; int UK, UN, NBH, grid; size_t region, smem;      // region = bytes of the activation stage (= attention scratch capacity)
+    int UK, UN, grid; size_t region, smem;      // region = bytes of the TMA slot (= attention scratch capacity)
 };
-static AttBwdGeom att_bwd_geom(const b200tts_decoder_shape& s, bool tc) {
+static AttBwdGeom att_bwd_geom(const b200tts_decoder_shape& s) {
     AttBwdGeom g{};
-    g.tc = tc;
     g.UK = s.D / KBA;
     const int L16 = (s.L + 15) / 16 * 16;
     const size_t extras = (size_t)s.A * 40 * 2 + (size_t)32 * (s.A + 8) * 2 + (size_t)(L16 + 32) * 4 + (size_t)s.A * 9 * 4;
-    if (tc) {
-        g.UN = (s.M + s.D <= NBT * TUN) ? TUN : TUN_WIDE; g.NBH = 1; g.grid = KBA * NBT;
-        const int NKT = 4 * g.UK / 64;
-        g.region = (size_t)NKT * 8192;
-        g.smem = 1024 + (size_t)NKT * g.UN * 128 + g.region + extras;
-    } else {
-        g.UN = (cdiv(s.M + s.D, NBA) + 15) / 16 * 16; g.NBH = (s.B + BT - 1) / BT; g.grid = KBA * NBA * g.NBH;
-        g.region = (size_t)BT * (4 * g.UK + 8) * 2;
-        g.smem = 1024 + (size_t)4 * g.UK * (g.UN + 8) * 2 + g.region + extras;
-    }
+    g.UN = (s.M + s.D <= NBT * TUN) ? TUN : TUN_WIDE; g.grid = KBA * NBT;
+    const int NKT = 4 * g.UK / 64;
+    g.region = (size_t)NKT * 8192;
+    g.smem = 1024 + (size_t)NKT * g.UN * 128 + g.region + extras;
     return g;
 }
 
-static bool att_bwd_variant_ok(const b200tts_decoder_shape& s, const AttBwdGeom& g) {
+bool persist_att_bwd_supported(const b200tts_decoder_shape& s) {
+    const AttBwdGeom g = att_bwd_geom(s);
     if (s.A != 128 || s.K > 32 || s.B * 8 > 3 * PT || s.D % KBA != 0) return false;
     if (s.M > 2 * PT || (s.L + 15) / 16 * 16 + 48 > 2 * PT || s.B * (s.A / 4) > 8 * PT) return false;      // register-slot staging of the attention backward
     if (s.D / 8 > g.grid) return false;                       // cell-backward ownership: 8 hidden units per CTA
     if (g.grid / 2 < s.B || g.grid > NUM_SMS) return false;       // one CTA pair per utterance, all CTAs co-resident
-    if (g.tc) {
-        if (g.UK % 64 != 0 || s.B > 64 || s.M + s.D > NBT * g.UN || (s.M + s.D) % 4 != 0) return false;
-    } else {
-        if (!persist_bwd_supported(s) || s.B > 2 * BT) return false;
-    }
+    if (g.UK % 64 != 0 || s.B > 64 || s.M + s.D > NBT * g.UN || (s.M + s.D) % 4 != 0) return false;
     const int MT = (s.L + 15) / 16, L16 = MT * 16, HT0 = (MT + 1) / 2;
-    // attention-backward scratch of one CTA of the pair (aliases the activation stage)
+    // attention-backward scratch of one CTA of the pair (aliases the TMA slot)
     const size_t fl = (size_t)((s.M + 3) & ~3) + 3 * (size_t)L16 + 2 * s.A + 2 * (size_t)(L16 + 48) + 64 + (size_t)(HT0 + 1) * 16 * GLD +
                       8 * (size_t)s.A + s.A + 4 + (size_t)((s.M + 15) / 16) * 32 * 2;
     if (fl * 4 > g.region) return false;
-    // the cell-backward phase stages the query gradients [B][A] fp32 + [64][8] products in the (then idle) activation stage
+    // the cell-backward phase stages the query gradients [B][A] fp32 + [64][8] products in the (then idle) TMA slot
     if ((size_t)s.B * s.A * 4 + 64 * 8 * 4 > g.region) return false;
     return g.smem <= 227 * 1024;
 }
-
-static bool att_bwd_pick(const b200tts_decoder_shape& s, AttBwdGeom* out) {
-    for (int tc = 1; tc >= 0; --tc) {
-        if (tc && getenv("B200TTS_ATT_BWD_MMA_SYNC")) continue;      // A/B switch: force the mma.sync product
-        const AttBwdGeom g = att_bwd_geom(s, tc != 0);
-        if (att_bwd_variant_ok(s, g)) { if (out) *out = g; return true; }
-    }
-    return false;
-}
-
-bool persist_att_bwd_supported(const b200tts_decoder_shape& s) { return att_bwd_pick(s, nullptr); }
-bool persist_att_bwd_tc(const b200tts_decoder_shape& s) { AttBwdGeom g{}; return att_bwd_pick(s, &g) && g.tc; }
 
 int tc_make_mapN_bf16(void* map, const void* base, int rank, const unsigned long long* dims, const unsigned long long* strides, const unsigned* box);
 
@@ -1273,19 +999,16 @@ int persist_att_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_p
                          cudaStream_t st, void* dgb_hist) {
     const AttBwdExtra x = att_bwd_extra(s);
     const int B = s.B, D = s.D, M = s.M, T = s.T, L = s.L, A = s.A;
+    B200_REQUIRE(persist_att_bwd_supported(s), "persistent attention backward: shape not supported");
+    const AttBwdGeom geo = att_bwd_geom(s);
     AttBwdArgs a{};
-    AttBwdGeom geo{};
-    B200_REQUIRE(att_bwd_pick(s, &geo), "persistent attention backward: shape not supported");
     a.B = B; a.T = T; a.D = D; a.M = M; a.L = L; a.A = A; a.KC = s.K; a.NOUT = M + D; a.UK = geo.UK;
-    a.UN = geo.UN; a.NBH = geo.NBH; a.MT = x.MT;
+    a.UN = geo.UN; a.MT = x.MT;
     a.W = fws + fl.wcat_att; a.ldw = M + D;
     a.gates = fws + fl.ga; a.cstate = fws + fl.ca; a.dh_static = dh_static; a.dctx_static = dctx_static;
     a.mask_h = in.mask_att_h; a.mask_c = in.mask_att_c; a.kind = s.cell_kind; a.training = s.training; a.rate_h = s.rate_h; a.rate_c = s.rate_c;
     a.dgates = dgates;
-    // bf16 gate gradients: a [T, B, 4D] history when the caller wants to feed the time-batched products from it (no conversion pass),
-    // else a [B, 4D] staging reused every step
-    a.dgb = dgb_hist ? static_cast<__nv_bfloat16*>(dgb_hist) : reinterpret_cast<__nv_bfloat16*>(extra + x.dgb);
-    a.dgb_step = dgb_hist ? (long long)B * 4 * D : 0; a.dgb_rows = dgb_hist ? B : 0;
+    a.dgb = static_cast<__nv_bfloat16*>(dgb_hist); a.dgb_step = (long long)B * 4 * D; a.dgb_rows = B;
     a.part = reinterpret_cast<float*>(extra + x.part);
     a.q = fws + fl.q; a.cum = fws + fl.cum; a.align = align; a.align_bstride = (long long)T * L;
     a.dalign = dalign; a.dalign_bstride = (long long)T * L;
@@ -1294,9 +1017,7 @@ int persist_att_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_p
     __nv_bfloat16* wcb2 = reinterpret_cast<__nv_bfloat16*>(extra + x.wcb2);
     __nv_bfloat16* memTf = reinterpret_cast<__nv_bfloat16*>(extra + x.memTf);
     a.WcB = wcb; a.WcB2 = wcb2; a.memTf = memTf;
-    a.memb = reinterpret_cast<const __nv_bfloat16*>(pws + pl.memb); a.ldm = pl.ldm;
     a.memFb = reinterpret_cast<const uint4*>(pws + pl.memFb); a.M16 = pl.M16;
-    a.dqp_after_g = 1;
     a.lengths = in.text_lengths; a.dctx_tot = dctx_tot; a.dq = dq; a.de = reinterpret_cast<float*>(extra + x.de);
     a.barrier = reinterpret_cast<unsigned*>(extra + x.barrier); a.abort_flag = reinterpret_cast<int*>(a.barrier + 32);
     a.prof = reinterpret_cast<long long*>(extra + x.barrier + 256);
@@ -1305,8 +1026,7 @@ int persist_att_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_p
     att_bwd_prep_kernel<<<NUM_SMS * 4, 256, 0, st>>>(wcb, wcb2, memTf, wcombT, fws + fl.memT, B, L, A, s.K, x.MT);
     B200_LAUNCH_CHECK();
     const size_t smem = geo.smem;
-    void* fn = geo.tc ? (geo.UN == TUN ? (void*)att_bwd_loop_kernel<true, TUN> : (void*)att_bwd_loop_kernel<true, TUN_WIDE>)
-                      : (void*)att_bwd_loop_kernel<false, 0>;
+    void* fn = geo.UN == TUN ? (void*)att_bwd_loop_kernel<TUN> : (void*)att_bwd_loop_kernel<TUN_WIDE>;
     B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int grid = geo.grid;
     int per_sm = 0, dev = 0, sms = 0;
@@ -1314,24 +1034,19 @@ int persist_att_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_p
     B200_CUDA(cudaGetDevice(&dev));
     B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     B200_REQUIRE(per_sm * sms >= grid && grid % 2 == 0 && grid / 2 >= B, "persistent attention backward: %d CTAs cannot be co-resident / paired", grid);
+    // bf16 gate-gradient history dgb [T, B, 4D] as {64 k, T * B rows, UK/64 halves, KBA k-slices, 4 gates}: element (row, g, kb, h, c) at
+    // row * 4D + g * D + kb * UK + h * 64 + c; one box = {64, 64 rows, UK/64, 1, 4} = the whole K-slice of a CTA for one step
     CUtensorMap tm;
-    memset(&tm, 0, sizeof(tm));
-    if (geo.tc) {
-        // bf16 gate gradients dgb [B, 4D] as {64 k, B rows, UK/64 halves, KBA k-slices, 4 gates}: element (b, g, kb, h, c) at
-        // b * 4D + g * D + kb * UK + h * 64 + c; one box = {64, 64 rows, UK/64, 1, 4} = the whole K-slice of a CTA
-        const unsigned long long dims[5] = {64ull, (unsigned long long)(dgb_hist ? (size_t)T * B : (size_t)B), (unsigned long long)(geo.UK / 64), (unsigned long long)KBA, 4ull};
-        const unsigned long long strides[4] = {(unsigned long long)4 * D * 2, 128ull, (unsigned long long)geo.UK * 2, (unsigned long long)D * 2};
-        const unsigned box[5] = {64u, 64u, (unsigned)(geo.UK / 64), 1u, 4u};
-        B200_TRY(tc_make_mapN_bf16(&tm, a.dgb, 5, dims, strides, box));
-    }
+    const unsigned long long dims[5] = {64ull, (unsigned long long)T * B, (unsigned long long)(geo.UK / 64), (unsigned long long)KBA, 4ull};
+    const unsigned long long strides[4] = {(unsigned long long)4 * D * 2, 128ull, (unsigned long long)geo.UK * 2, (unsigned long long)D * 2};
+    const unsigned box[5] = {64u, 64u, (unsigned)(geo.UK / 64), 1u, 4u};
+    B200_TRY(tc_make_mapN_bf16(&tm, a.dgb, 5, dims, strides, box));
     void* params[] = {&tm, &a};
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(grid); cfg.blockDim = dim3(PT); cfg.dynamicSmemBytes = smem; cfg.stream = st;
     cudaLaunchAttribute attrs[2];
     attrs[0].id = cudaLaunchAttributeCooperative;
-    // profiling aid: ncu cannot capture a launch that is BOTH cooperative and clustered; the kernel carries its own grid barrier, so on an
-    // otherwise idle GPU (all CTAs resident: <= NUM_SMS, one per SM) the cooperative attribute can be dropped for a capture
-    attrs[0].val.cooperative = getenv("B200TTS_PROFILE_NO_COOP") ? 0 : 1;
+    attrs[0].val.cooperative = 1;
     attrs[1].id = cudaLaunchAttributeClusterDimension;          // the attention backward of an utterance runs on a CTA pair
     attrs[1].val.clusterDim.x = 2; attrs[1].val.clusterDim.y = 1; attrs[1].val.clusterDim.z = 1;
     cfg.attrs = attrs; cfg.numAttrs = 2;
@@ -1364,49 +1079,6 @@ int persist_att_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_p
     B200_LAUNCH_CHECK();
     att_bwd_finish_kernel<<<1, 512, (size_t)A * 32 * 4, st>>>(dw.attn_location, dw.attn_loc_features, dw.attn_energy, dWsum, dvsum,
                                                              w.attn_location, w.attn_loc_features, A, s.C, s.K);
-    B200_LAUNCH_CHECK();
-    return B200TTS_OK;
-}
-
-size_t persist_bwd_gen_extra_bytes(const b200tts_decoder_shape& s) {
-    // dgb [B, 4D] bf16 + part [KB, B, D] fp32 + barrier
-    return ((size_t)s.B * 4 * s.D * 2 + 255) / 256 * 256 + ((size_t)KB * s.B * s.D * 4 + 255) / 256 * 256 + 256 + NUM_SMS * 8 * 8;
-}
-
-// dgates for all T steps of the generator LSTM.  `extra` = persist_bwd_gen_extra_bytes scratch.
-int persist_gen_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
-                         const DecoderLayout& fl, const float* fws, const float* dh_static, float* dgates, unsigned char* extra,
-                         cudaStream_t st) {
-    const int B = s.B, D = s.D;
-    BwdLoopArgs a{};
-    a.B = B; a.T = s.T; a.D = D; a.NOUT = D; a.UK = D / KB; a.UN = (cdiv(D, NBK) + 15) / 16 * 16; a.NBH = (B + BT - 1) / BT;
-    a.W = w.gen_w_hh; a.ldw = D;
-    a.gates = fws + fl.gg; a.cstate = fws + fl.cg; a.dh_static = dh_static;
-    a.mask_h = in.mask_gen_h; a.mask_c = in.mask_gen_c; a.kind = s.cell_kind; a.training = s.training; a.rate_h = s.rate_h; a.rate_c = s.rate_c;
-    a.dgates = dgates;
-    size_t off = 0;
-    a.dgb = reinterpret_cast<__nv_bfloat16*>(extra + off); off += ((size_t)B * 4 * D * 2 + 255) / 256 * 256;
-    a.part = reinterpret_cast<float*>(extra + off); off += ((size_t)KB * B * D * 4 + 255) / 256 * 256;
-    a.barrier = reinterpret_cast<unsigned*>(extra + off);
-    a.abort_flag = reinterpret_cast<int*>(a.barrier + 32);
-    a.prof = reinterpret_cast<long long*>(extra + off + 256);
-    a.hcol = 0;
-    B200_CUDA(cudaMemsetAsync(a.barrier, 0, 256, st));
-    const size_t smem = ((size_t)4 * a.UK * (a.UN + 8) + (size_t)BT * (4 * a.UK + 8)) * 2;
-    B200_REQUIRE(smem <= 227 * 1024, "persistent backward: %zu B of shared memory needed", smem);
-    void* fn = (void*)lstm_bwd_loop_kernel;
-    B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const int grid = KB * NBK * a.NBH;
-    int per_sm = 0, dev = 0, sms = 0;
-    B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, PT, smem));
-    B200_CUDA(cudaGetDevice(&dev));
-    B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    B200_REQUIRE(per_sm * sms >= grid, "persistent backward: %d CTAs cannot be co-resident", grid);
-    void* params[] = {&a};
-    {
-        KernelTimer kt("lstm_bwd_loop_kernel", st);
-        B200_CUDA(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(PT), params, smem, st));
-    }
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }

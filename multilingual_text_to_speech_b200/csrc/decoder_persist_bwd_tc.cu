@@ -40,8 +40,8 @@ struct TcBwdArgs {
     const uint8_t* mask_h; const uint8_t* mask_c;
     int kind, training; float rate_h, rate_c;
     float* dgates;                            // [T, B, 4D] out (fp32)
-    __nv_bfloat16* dgb;                       // [B, 4D] staging (bf16), TMA source -- or a [T, B, 4D] history (dgb_step = B * 4D, dgb_rows = B)
-    long long dgb_step; int dgb_rows;
+    __nv_bfloat16* dgb;                       // [T, B, 4D] out: bf16 history of the gate gradients, TMA source of the product
+    long long dgb_step; int dgb_rows;         // elements (B * 4D) and TMA rows (B) of one step of the history
     float* part;                              // [NG, B, D] partial products of the previous reverse step
     unsigned* barrier; int* abort_flag;
     long long* prof;
@@ -305,18 +305,22 @@ __global__ void __launch_bounds__(PT, 1) lstm_bwd_loop_tc_kernel(const __grid_co
 }
 
 size_t bwd_tc_smem_bytes(int D) { return 1024 + (size_t)(D / KB) * (WTILE + ATILE); }
+size_t part_bytes(const b200tts_decoder_shape& s) { return ((size_t)NG * s.B * s.D * 4 + 255) / 256 * 256; }
 
 }  // namespace
 
 bool tc_persist_gen_bwd_supported(const b200tts_decoder_shape& s) {
+    if (s.D % 128 != 0 || s.D > 2048 || s.B > 64) return false;                      // the shapes this loop is validated on
     if (s.D % KB != 0 || s.D % (NG * (s.D / KB) * UNITS) != 0) return false;       // 4 x D/64 CTAs per batch half x 16 units = D
     const int NBH = (s.B + BT - 1) / BT;
     if (NG * (s.D / KB) * NBH > NUM_SMS) return false;
     return bwd_tc_smem_bytes(s.D) <= 227 * 1024 - 1088;
 }
 
-// dgates for all T steps of the generator LSTM (wgmma variant); `extra` = persist_bwd_gen_extra_bytes scratch (same layout as the
-// mma.sync variant: dgb [B, 4D] bf16, then the partial buffer (4 of its 8 slabs are used), then barrier + profile counters).
+size_t persist_bwd_gen_extra_bytes(const b200tts_decoder_shape& s) { return part_bytes(s) + 256 + NUM_SMS * 8 * 8; }
+
+// dgates for all T steps of the generator LSTM, and their bf16 [T, B, 4D] history `dgb_hist`; `extra` = persist_bwd_gen_extra_bytes
+// scratch: the partial buffer [NG, B, D], then barrier + profile counters.
 int tc_persist_gen_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
                             const DecoderLayout& fl, const float* fws, const float* dh_static, float* dgates, unsigned char* extra,
                             cudaStream_t st, void* dgb_hist) {
@@ -327,17 +331,14 @@ int tc_persist_gen_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decode
     a.gates = fws + fl.gg; a.cstate = fws + fl.cg; a.dh_static = dh_static;
     a.mask_h = in.mask_gen_h; a.mask_c = in.mask_gen_c; a.kind = s.cell_kind; a.training = s.training; a.rate_h = s.rate_h; a.rate_c = s.rate_c;
     a.dgates = dgates;
-    size_t off = 0;
-    a.dgb = dgb_hist ? static_cast<__nv_bfloat16*>(dgb_hist) : reinterpret_cast<__nv_bfloat16*>(extra + off);
-    a.dgb_step = dgb_hist ? (long long)B * 4 * D : 0; a.dgb_rows = dgb_hist ? B : 0;
-    off += ((size_t)B * 4 * D * 2 + 255) / 256 * 256;
-    a.part = reinterpret_cast<float*>(extra + off); off += ((size_t)8 * B * D * 4 + 255) / 256 * 256;
-    a.barrier = reinterpret_cast<unsigned*>(extra + off);
+    a.dgb = static_cast<__nv_bfloat16*>(dgb_hist); a.dgb_step = (long long)B * 4 * D; a.dgb_rows = B;
+    a.part = reinterpret_cast<float*>(extra);
+    a.barrier = reinterpret_cast<unsigned*>(extra + part_bytes(s));
     a.abort_flag = reinterpret_cast<int*>(a.barrier + 32);
-    a.prof = reinterpret_cast<long long*>(extra + off + 256);
+    a.prof = reinterpret_cast<long long*>(extra + part_bytes(s) + 256);
     B200_CUDA(cudaMemsetAsync(a.barrier, 0, 256, st));
-    CUtensorMap tm;        // {64 columns, B rows, 4D/64 k-blocks}: k-block stride 128 B, row stride 4D * 2 B
-    B200_TRY(tc_make_map3_bf16(&tm, a.dgb, KB, dgb_hist ? s.T * B : B, 4 * D / KB, (size_t)4 * D * 2, 128, KB, BT, a.NNB));
+    CUtensorMap tm;        // {64 columns, T * B rows, 4D/64 k-blocks}: k-block stride 128 B, row stride 4D * 2 B
+    B200_TRY(tc_make_map3_bf16(&tm, a.dgb, KB, s.T * B, 4 * D / KB, (size_t)4 * D * 2, 128, KB, BT, a.NNB));
     const size_t smem = bwd_tc_smem_bytes(D);
     void* fn = (void*)lstm_bwd_loop_tc_kernel;
     B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -16,7 +16,6 @@
 // writes it, so the backward pass is unaffected.
 // Reference semantics: modules/tacotron2.py:180-198, modules/layers.py:18-47, modules/attention.py:39-86.
 #include <cuda.h>
-#include <stdlib.h>
 #include <cuda_bf16.h>
 #include "decoder_internal.cuh"
 #include "tc_ptx.cuh"
@@ -867,9 +866,7 @@ static int launch_tc_loop(bool att, const TcLoopArgs& a, const CUtensorMap& tmH,
     cfg.gridDim = dim3(grid); cfg.blockDim = dim3(PT); cfg.dynamicSmemBytes = smem; cfg.stream = st;
     cudaLaunchAttribute attrs[2];
     attrs[0].id = cudaLaunchAttributeCooperative;
-    // profiling aid: ncu cannot capture a launch that is BOTH cooperative and clustered; the kernel carries its own grid barrier, so on an
-    // otherwise idle GPU (all CTAs resident: <= NUM_SMS, one per SM) the cooperative attribute can be dropped for a capture
-    attrs[0].val.cooperative = getenv("B200TTS_PROFILE_NO_COOP") ? 0 : 1;
+    attrs[0].val.cooperative = 1;
     cfg.attrs = attrs; cfg.numAttrs = 1;
     if (att) {      // the attention runs on CTA pairs: clusters of 2 (distributed shared memory + cluster barrier)
         B200_REQUIRE(grid % 2 == 0 && grid / 2 >= a.B, "wgmma attention loop: %d CTAs cannot form %d pairs", grid, a.B);
@@ -929,7 +926,7 @@ int tc_persist_att_loop(const b200tts_decoder_shape& s, const b200tts_decoder_pa
     a.prof2 = a.prof + 2 * NUM_SMS * 8;
     size_t smem = tc_loop_smem_bytes(g.nkb_att, a.slot_kb, s.A, true, s.L, g.alias_att != 0);
     const size_t tab = (size_t)l.MT * 32 * 8;          // shared B-fragment table of the context product, when it fits behind the scratch
-    a.use_btab = (smem + tab <= SMEM_LIMIT && !getenv("B200TTS_NO_BTAB")) ? 1 : 0;
+    a.use_btab = smem + tab <= SMEM_LIMIT ? 1 : 0;
     if (a.use_btab) smem += tab;
     return launch_tc_loop(true, a, tmH, tmC, smem, st);
 }

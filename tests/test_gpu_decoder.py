@@ -147,9 +147,11 @@ def test_gemm_bf16_mode(M, N, K, ta, tb, splitk):
     dict(B=16, L=60, T=14, M=512, kind='zoneout', seed=10),
     dict(B=52, L=300, T=8, M=512, kind='dropout', seed=11),
     dict(B=9, L=37, T=11, M=384, kind='dropout', seed=12),
+    dict(B=4, L=40, T=12, D=1280, kind='zoneout', seed=13),      # D = 1280: off the persistent loops, per-step chains in bf16
 ])
 def test_decoder_bf16_perf_mode(kw):
-    """Persistent weight-stationary bf16 kernels (decoder_persist.cu) + bf16 tensor-core GEMMs."""
+    """bf16 perf mode: persistent weight-stationary TMA + wgmma loops (decoder_persist_tc.cu, decoder_persist_bwd_tc.cu,
+    decoder_persist_bwd.cu) + bf16 tensor-core GEMMs; shapes off those loops run the per-step chains in bf16."""
     dc.run_case_bf16(dc.full_dim_case(**kw), check_grads=True, verbose=True)
 
 

@@ -83,6 +83,28 @@ def test_decoder_path_covers_baseline_configs(lib):
         assert path(B, L, 900, 512) == 0b111111, (B, L, bin(path(B, L, 900, 512)))
 
 
+def _decoder_path(lib, B, L, M, D, training):
+    s = _lib.DecoderShape(B, L, 900, M, D, 256, 128, 32, 31, 80, 1, training, 0.1, 0.1, 0.5)
+    return lib.b200tts_decoder_path(ctypes.byref(s))
+
+
+def test_decoder_path_variant_bits_pair_with_loop_bits(lib):
+    """Every persistent loop is a TMA + wgmma kernel: each variant bit (1, 3, 5) is set exactly when its loop bit (0, 2, 4) is."""
+    for D in (512, 960, 1024, 1040, 1152, 1280, 2048):
+        for M in (128, 288, 512):
+            for B in (1, 8, 33, 64):
+                for training in (0, 1):
+                    bits = _decoder_path(lib, B, 180, M, D, training)
+                    for loop in (0, 2, 4):
+                        assert (bits >> loop) & 1 == (bits >> (loop + 1)) & 1, (D, M, B, training, bin(bits))
+
+
+def test_decoder_path_off_the_wgmma_loops_is_the_per_step_chains(lib):
+    """Shapes no wgmma loop accepts run every such pass on the per-step chains (no mma.sync persistent loops)."""
+    assert _decoder_path(lib, 8, 180, 288, 1280, 1) == 0          # D = 1280 training: the generator reverse loop included
+    assert _decoder_path(lib, 8, 180, 288, 1040, 0) & 0b11 == 0   # no-grad forward with D % 64 != 0
+
+
 def test_grad_targets_accumulate_in_place_only_into_bound_leaf_gradients():
     """functional._grad_targets: a leaf parameter whose .grad is a dense fp32 tensor of its own shape (the GradBucket views) is the
     accumulation target itself and autograd gets None; anything else gets a fresh zero tensor that autograd accumulates as usual."""
