@@ -9,9 +9,10 @@
 //   PB  LSTM-cell backward of 8 hidden units x every utterance (CTAs < D/8): gate gradients -> fp32 for the weight-gradient products
 //       and a bf16 [T, B, 4D] history;
 //   --  grid barrier (gate gradients of all units visible)
-//   P2  ONE 5-D TMA box brings the bf16 gate gradients of the K-slice for the whole batch (<= 64 utterances, rows beyond B zero-filled),
-//       the A operand (M = 64); warpgroup 0 runs wgmma m64n80k16 / m64n96k16 and stores the fp32 partial [B x n-block] that the next
-//       step sums over the 8 K-slices (fixed order, no atomics);
+//   P2  the bf16 gate gradients of the K-slice for the whole batch (<= 64 utterances, rows beyond B zero-filled), the A operand
+//       (M = 64), arrive as two 5-D TMA boxes of two gates each: the CTAs of a pair share the K-slice (and differ in the n-block), and
+//       each issues one box with multicast into both; warpgroup 0 runs wgmma m64n80k16 / m64n96k16 and stores the fp32 partial
+//       [B x n-block] that the next step sums over the 8 K-slices (fixed order, no atomics);
 //   --  grid barrier.
 // The post pass then accumulates, in parallel over all steps, what the recurrence does not need: d memT, d Wcomb, d v.
 // Reference semantics: autograd replay of modules/layers.py:18-47 and modules/attention.py:39-86 (train.py:83).
@@ -69,9 +70,6 @@ __device__ __forceinline__ bool grid_barrier(unsigned* counter, unsigned& target
     return s_ok != 0;
 }
 
-// thread-block cluster (CTA pair) split arrive / wait barrier
-__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
-__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
 __device__ __forceinline__ void l2_prefetch(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 // remote store that completes its 4 bytes on the PEER's mbarrier (data + signal in one instruction): the pair exchanges need no cluster
 // barrier and none of the memory fence its release semantics imply
@@ -147,10 +145,12 @@ template <int UNC>
 __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_constant__ CUtensorMap tmG, const AttBwdArgs p) {
     extern __shared__ __align__(1024) unsigned char smem_raw0[];
     unsigned char* smem_raw = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw0) + 1023) & ~(uintptr_t)1023);
-    __shared__ uint64_t full_bar, xb1, xb2;      // xb1 / xb2: arrival of the peer's softmax dot / query-gradient partial + G halo tile
+    __shared__ uint64_t full_bar[2], xb1, xb2;   // full_bar[r]: rank r's half of the P2 operand; xb1 / xb2: arrival of the peer's softmax dot /
+                                                 // query-gradient partial + G halo tile
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int cta = blockIdx.x;
-    const int kb = cta % KBA, nb = cta / KBA;
+    // the CTA pair (2k, 2k+1) = one cluster shares the K-slice kb and takes two n-blocks: both need the same operand in P2
+    const int kb = (cta >> 1) % KBA, nb = 2 * (cta >> 4) + (cta & 1);
     const int B = p.B, D = p.D, UK = p.UK, UN = p.UN, KROWS = 4 * UK, M = p.M, L = p.L, A = p.A;
     const int n0 = nb * UN;
     const int NKT = KROWS / 64;                                                      // k-block tiles of the K-slice
@@ -186,10 +186,11 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
         for (int idx = tid; idx < A * UOWN; idx += PT) wq8[(idx / UOWN) * (UOWN + 1) + idx % UOWN] = p.Wq[(size_t)(idx / UOWN) * D + uo0 + idx % UOWN];
     uint32_t prod_it = 0;
     if (tid == 0) { tcx::mbar_init(&xb1, 1); tcx::mbar_init(&xb2, 1); tcx::mbar_init_fence(); }
-    if (tid == 0) { tcx::mbar_init(&full_bar, 1); tcx::mbar_init_fence(); }
+    if (tid == 0) { tcx::mbar_init(&full_bar[0], 1); tcx::mbar_init(&full_bar[1], 1); tcx::mbar_init_fence(); }
     tcx::proxy_fence_shared();           // the weight tiles were written through the generic proxy; wgmma reads them through the async proxy
     __syncthreads();
-    cluster_arrive(); cluster_wait();      // one-time: the peer's exchange mbarriers are initialised before the first remote st.async targets them
+    // one-time: the peer's mbarriers are initialised before the first remote st.async or multicast TMA of this CTA targets them
+    tcx::cluster_arrive(); tcx::cluster_wait();
 
     const float inv_h = 1.f / (1.f - p.rate_h), inv_c = 1.f / (1.f - p.rate_c);
     constexpr int MAXE = 3;               // (b, u) pairs per thread: B * 8 / 256 <= 3 for B <= 64... (B <= 96)
@@ -653,23 +654,30 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
         if (i == 0) break;
 
         // =========================== P2: [d ctx | d h](i-1) partial = dgates_i[:, kb] . W[kb, nb] ===========================
-        // TMA: the bf16 gate gradients of the K-slice, all utterances (rows >= B zero-filled), as NKT swizzled [64 x 64] tiles in ONE box;
+        // TMA: the bf16 gate gradients of the K-slice, all utterances (rows >= B zero-filled), as NKT swizzled [64 x 64] tiles; the pair
+        // shares kb, so rank r issues ONE box of gates {2r, 2r+1} with multicast into both slots, completing on full_bar[r] of both CTAs; each
+        // CTA arms both barriers with NKT/2 tiles, and the MMAs of the first half run while the second half may still be in flight.  Both CTAs
+        // last touched their slot (attention scratch, dq staging) before the grid barrier above, so the peer's slot is free.
         // wgmma: D[b, n] (registers of warpgroup 0: 64 utterances x UN outputs) = sum over the tiles, stored straight to the partials
         if (warp == 0) {
             if (tcx::elect_one()) {
+                const int r = cta & 1;
                 tcx::proxy_fence_shared();       // the slot was last touched through the generic proxy (attention scratch, dq staging)
                 tcx::proxy_fence_global();
-                tcx::mbar_expect_tx(&full_bar, (uint32_t)NKT * 8192);
-                tcx::tma_load_5d(As, &tmG, &full_bar, 0, i * p.dgb_rows, 0, kb, 0);
+                tcx::mbar_expect_tx(&full_bar[0], (uint32_t)(NKT / 2) * 8192);
+                tcx::mbar_expect_tx(&full_bar[1], (uint32_t)(NKT / 2) * 8192);
+                tcx::tma_load_5d_mc(reinterpret_cast<unsigned char*>(As) + (size_t)r * (NKT / 2) * 8192, &tmG, &full_bar[r], 0x3, 0, i * p.dgb_rows, 0,
+                                    kb, 2 * r);
             }
             __syncwarp();
         }
         if (warp < 4) {
             constexpr int NR = UNC / 2;
             float acc[NR];
-            tcx::mbar_wait(&full_bar, prod_it & 1);
+            tcx::mbar_wait(&full_bar[0], prod_it & 1);
             tcx::wgmma_fence();
             for (int c = 0; c < NKT; ++c) {
+                if (c == NKT / 2) tcx::mbar_wait(&full_bar[1], prod_it & 1);
                 const uint64_t adesc = tcx::make_sw128_desc(tcx::smem_u32(reinterpret_cast<unsigned char*>(As) + (size_t)c * 8192));
                 const uint64_t bdesc = tcx::make_sw128_desc(tcx::smem_u32(sW + (size_t)c * UN * 128));
 #pragma unroll
@@ -696,6 +704,11 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
         BPROF_MARK(6);
     }
     BPROF_FLUSH;
+    // no CTA exits while a multicast it issued may still be landing in its peer.  A watchdog abort leaves the loop through the shared abort
+    // flag, which every CTA checks at each grid barrier, so both ranks of a pair stop at the same barrier -- unless the flag is raised just
+    // as that barrier completes: the rank that went on then waits for the peer's half of the next operand and ends in the trap of
+    // mbar_wait (~2 s), not in a hang
+    tcx::cluster_arrive(); tcx::cluster_wait();
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -1035,11 +1048,12 @@ int persist_att_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_p
     B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     B200_REQUIRE(per_sm * sms >= grid && grid % 2 == 0 && grid / 2 >= B, "persistent attention backward: %d CTAs cannot be co-resident / paired", grid);
     // bf16 gate-gradient history dgb [T, B, 4D] as {64 k, T * B rows, UK/64 halves, KBA k-slices, 4 gates}: element (row, g, kb, h, c) at
-    // row * 4D + g * D + kb * UK + h * 64 + c; one box = {64, 64 rows, UK/64, 1, 4} = the whole K-slice of a CTA for one step
+    // row * 4D + g * D + kb * UK + h * 64 + c; one box = {64, 64 rows, UK/64, 1, 2} = two gates of a CTA's K-slice for one step (each rank
+    // of a pair fetches two of the four)
     CUtensorMap tm;
     const unsigned long long dims[5] = {64ull, (unsigned long long)T * B, (unsigned long long)(geo.UK / 64), (unsigned long long)KBA, 4ull};
     const unsigned long long strides[4] = {(unsigned long long)4 * D * 2, 128ull, (unsigned long long)geo.UK * 2, (unsigned long long)D * 2};
-    const unsigned box[5] = {64u, 64u, (unsigned)(geo.UK / 64), 1u, 4u};
+    const unsigned box[5] = {64u, 64u, (unsigned)(geo.UK / 64), 1u, 2u};
     B200_TRY(tc_make_mapN_bf16(&tm, a.dgb, 5, dims, strides, box));
     void* params[] = {&tm, &a};
     cudaLaunchConfig_t cfg{};

@@ -2,12 +2,14 @@
 //
 // Reverse step i needs  d h_{i-1}[b, n] = sum_r dgates_i[b, r] . W_hh[r, n]  (r over the 4D gate rows): the transpose of the forward
 // product.  CTA (gate g, n-block nb, batch half bh) keeps W_hh^T[n-block (64 outputs), gate g (D rows of K)] in shared memory as
-// K-major SWIZZLE_128B tiles (A operand, M = 64); per step ONE TMA box brings the bf16 gate gradients [32 utterances x D] of its
-// gate (B operand, N = 32); D / 16 wgmma instructions accumulate in registers; the fp32 partial [gate][b][n] that the next
-// step's cell backward sums over the 4 gates (fixed order, no atomics) is stored straight from them.  Per step:
+// K-major SWIZZLE_128B tiles (A operand, M = 64); per step the bf16 gate gradients [32 utterances x D] of its gate arrive by TMA
+// (B operand, N = 32); D / 16 wgmma instructions accumulate in registers; the fp32 partial [gate][b][n] that the next
+// step's cell backward sums over the 4 gates (fixed order, no atomics) is stored straight from them.  The launch is cooperative
+// with clusters of 2: the CTAs of a pair share (gate, batch half), differ in the n-block, and each issues ONE multicast TMA box of
+// half the operand's k-blocks into both CTAs, so every operand byte leaves L2 once per pair.  Per step:
 //   P1  cell backward of this CTA's 16 hidden units x 32 utterances (operands prefetched during the previous product)
 //   --  grid barrier (gate gradients of all units visible)
-//   P2  TMA + wgmma product, registers -> partial store
+//   P2  multicast TMA + wgmma product, registers -> partial store
 //   --  grid barrier.
 // Warp roles as in decoder_persist_tc.cu: warps 0-7 compute, warps 8-11 = the MMA warpgroup (an elected lane of warp 8 issues the TMA).
 // Reference semantics: autograd replay of modules/layers.py:18-47 (train.py:83).
@@ -48,55 +50,11 @@ struct TcBwdArgs {
 };
 
 // ------------------------------------------------------------------------------------------------
-// PTX wrappers
+// PTX wrappers (mbarrier, TMA, fences and the cluster barrier: tc_ptx.cuh)
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    const uint32_t addr = smem_u32(bar);
-    const long long t0 = clock64();
-    for (;;) {
-        uint32_t done;
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done)
-            : "r"(addr), "r"(parity)
-            : "memory");
-        if (done) return;
-        if (clock64() - t0 > 4000000000ll) __trap();       // ~2 s: a protocol bug must not hang the GPU
-    }
-}
-__device__ __forceinline__ void tma_load_3d(void* smem, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-__device__ __forceinline__ void proxy_fence_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
-__device__ __forceinline__ void proxy_fence_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
 __device__ __forceinline__ void l2_prefetch(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 // tanh of the recomputed cell state in the reverse loops: the same ex2-based form the forward loops of the bf16 mode use (~1e-6 relative)
 __device__ __forceinline__ float tanh_exp(float x) { return 2.f * __fdividef(1.f, 1.f + __expf(-2.f * x)) - 1.f; }
-// thread-block cluster (CTA pair) primitives: split arrive / wait barrier and a distributed-shared-memory store
-__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
-__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
-__device__ __forceinline__ void st_peer_f32(const float* local_smem, uint32_t peer_rank, float v) {
-    uint32_t ra;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(local_smem)), "r"(peer_rank));
-    asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(ra), "f"(v) : "memory");
-}
 // named barrier among the compute warps only
 __device__ __forceinline__ void csync() { asm volatile("bar.sync 1, %0;" ::"n"(CT) : "memory"); }
 
@@ -104,7 +62,7 @@ __device__ __forceinline__ bool grid_barrier(unsigned* counter, unsigned& target
     __syncthreads();
     if (threadIdx.x == 0) {
         target += nblocks;
-        proxy_fence_global();          // the bf16 gate gradients written above are read by other CTAs through TMA (async proxy)
+        tcx::proxy_fence_global();          // the bf16 gate gradients written above are read by other CTAs through TMA (async proxy)
         asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
         int ok = 1;
         const long long t0 = clock64();
@@ -133,7 +91,8 @@ __global__ void __launch_bounds__(PT, 1) lstm_bwd_loop_tc_kernel(const __grid_co
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
     const int cta = blockIdx.x;
-    const int gsel = cta % NG, nb = (cta / NG) % p.NNB, bh = cta / (NG * p.NNB);
+    // the CTA pair (2k, 2k+1) = one cluster shares (gate, batch half) and takes two n-blocks: both need the same operand every step
+    const int gsel = (cta >> 1) % NG, nb = 2 * ((cta >> 3) % (p.NNB / 2)) + (cta & 1), bh = cta / (NG * p.NNB);
     const int B = p.B, D = p.D, NNB = p.NNB;
     const int b0 = bh * BT, n0 = nb * ROWS;
     const int u0 = (gsel * NNB + nb) * UNITS;                 // hidden units whose cell backward this CTA owns
@@ -155,11 +114,12 @@ __global__ void __launch_bounds__(PT, 1) lstm_bwd_loop_tc_kernel(const __grid_co
         *reinterpret_cast<__nv_bfloat16*>(sW + (size_t)kb * WTILE + r * 128 + ((chunk ^ (r & 7)) << 4) + e * 2) = __float2bfloat16_rn(w);
     }
     if (tid == 0) {
-        mbar_init(&full_bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        tcx::mbar_init(&full_bar, 1);
+        tcx::mbar_init_fence();
     }
-    proxy_fence_shared();              // the weight tiles were written through the generic proxy; wgmma reads them through the async proxy
+    tcx::proxy_fence_shared();              // the weight tiles were written through the generic proxy; wgmma reads them through the async proxy
     __syncthreads();
+    tcx::cluster_arrive(); tcx::cluster_wait();     // one-time: the peer's mbarrier is initialised before this CTA's first multicast targets it
 
     const float inv_h = 1.f / (1.f - p.rate_h), inv_c = 1.f / (1.f - p.rate_c);
     // cell-backward operands of this thread's two (b, u) pairs, fetched one step ahead (during the previous product)
@@ -260,21 +220,25 @@ __global__ void __launch_bounds__(PT, 1) lstm_bwd_loop_tc_kernel(const __grid_co
         if (i == 0) break;
 
         // ---------------- P2: partial[gate] = dgates[:, gate block] . W[gate block, n-block]  (TMA + wgmma) ----------------
+        // the operand is fetched once per CTA pair: rank r issues k-blocks [r NNB/2, (r+1) NNB/2) of the gate's D columns with multicast
+        // into both rings, and each CTA arms its barrier with the whole NNB tiles.  The peer may write into this ring now: both CTAs'
+        // previous products completed before they arrived at the grid barriers in between.
         if (is_mma) {
             if (warp == NCW) {
-                proxy_fence_global();
-                if (elect_one()) {
-                    mbar_expect_tx(&full_bar, (uint32_t)NNB * ATILE);
-                    tma_load_3d(ring, &tmG, &full_bar, 0, i * p.dgb_rows + b0, gsel * NNB);
+                tcx::proxy_fence_global();
+                if (tcx::elect_one()) {
+                    const int r = cta & 1;
+                    tcx::mbar_expect_tx(&full_bar, (uint32_t)NNB * ATILE);
+                    tcx::tma_load_3d_mc(ring + (size_t)r * (NNB / 2) * ATILE, &tmG, &full_bar, 0x3, 0, i * p.dgb_rows + b0, gsel * NNB + r * (NNB / 2));
                 }
                 __syncwarp();
             }
-            mbar_wait(&full_bar, it & 1);
+            tcx::mbar_wait(&full_bar, it & 1);
             float acc[16];                   // the first instruction overwrites (scale-d = 0)
             tcx::wgmma_fence();
             for (int c = 0; c < NNB; ++c) {
-                const uint64_t adesc = tcx::make_sw128_desc(smem_u32(sW + (size_t)c * WTILE));
-                const uint64_t bdesc = tcx::make_sw128_desc(smem_u32(ring + (size_t)c * ATILE));
+                const uint64_t adesc = tcx::make_sw128_desc(tcx::smem_u32(sW + (size_t)c * WTILE));
+                const uint64_t bdesc = tcx::make_sw128_desc(tcx::smem_u32(ring + (size_t)c * ATILE));
 #pragma unroll
                 for (int k = 0; k < KB / 16; ++k) tcx::wgmma_m64n32<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (c | k) != 0);
             }
@@ -302,6 +266,11 @@ __global__ void __launch_bounds__(PT, 1) lstm_bwd_loop_tc_kernel(const __grid_co
     if (p.prof && tid == 0)
         for (int k = 0; k < 8; ++k) p.prof[(size_t)cta * 8 + k] = prof_acc[k];
 #undef PROF_MARK
+    // no CTA exits while a multicast it issued may still be landing in its peer.  A watchdog abort leaves the loop through the shared abort
+    // flag, which every CTA checks at each grid barrier, so both ranks of a pair stop at the same barrier -- unless the flag is raised just
+    // as that barrier completes: the rank that went on then waits for the peer's half of the next operand and ends in the trap of
+    // mbar_wait (~2 s), not in a hang
+    tcx::cluster_arrive(); tcx::cluster_wait();
 }
 
 size_t bwd_tc_smem_bytes(int D) { return 1024 + (size_t)(D / KB) * (WTILE + ATILE); }
@@ -312,6 +281,7 @@ size_t part_bytes(const b200tts_decoder_shape& s) { return ((size_t)NG * s.B * s
 bool tc_persist_gen_bwd_supported(const b200tts_decoder_shape& s) {
     if (s.D % 128 != 0 || s.D > 2048 || s.B > 64) return false;                      // the shapes this loop is validated on
     if (s.D % KB != 0 || s.D % (NG * (s.D / KB) * UNITS) != 0) return false;       // 4 x D/64 CTAs per batch half x 16 units = D
+    if ((s.D / KB) % 2 != 0) return false;                                          // the n-blocks pair up (one operand half per rank)
     const int NBH = (s.B + BT - 1) / BT;
     if (NG * (s.D / KB) * NBH > NUM_SMS) return false;
     return bwd_tc_smem_bytes(s.D) <= 227 * 1024 - 1088;
@@ -337,20 +307,27 @@ int tc_persist_gen_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decode
     a.abort_flag = reinterpret_cast<int*>(a.barrier + 32);
     a.prof = reinterpret_cast<long long*>(extra + part_bytes(s) + 256);
     B200_CUDA(cudaMemsetAsync(a.barrier, 0, 256, st));
-    CUtensorMap tm;        // {64 columns, T * B rows, 4D/64 k-blocks}: k-block stride 128 B, row stride 4D * 2 B
-    B200_TRY(tc_make_map3_bf16(&tm, a.dgb, KB, s.T * B, 4 * D / KB, (size_t)4 * D * 2, 128, KB, BT, a.NNB));
+    // {64 columns, T * B rows, 4D/64 k-blocks}: k-block stride 128 B, row stride 4D * 2 B; a box is half of one gate (NNB/2 k-blocks)
+    CUtensorMap tm;
+    B200_TRY(tc_make_map3_bf16(&tm, a.dgb, KB, s.T * B, 4 * D / KB, (size_t)4 * D * 2, 128, KB, BT, a.NNB / 2));
     const size_t smem = bwd_tc_smem_bytes(D);
     void* fn = (void*)lstm_bwd_loop_tc_kernel;
     B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int grid = NG * a.NNB * a.NBH;
-    int per_sm = 0, dev = 0, sms = 0;
-    B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, PT, smem));
-    B200_CUDA(cudaGetDevice(&dev));
-    B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    B200_REQUIRE(per_sm * sms >= grid, "wgmma persistent backward: %d CTAs cannot be co-resident", grid);
     void* params[] = {&tm, &a};
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(PT); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cudaLaunchAttribute attrs[2];
+    attrs[0].id = cudaLaunchAttributeCooperative;
+    attrs[0].val.cooperative = 1;
+    attrs[1].id = cudaLaunchAttributeClusterDimension;          // CTA pairs share the per-step operand (multicast TMA)
+    attrs[1].val.clusterDim.x = 2; attrs[1].val.clusterDim.y = 1; attrs[1].val.clusterDim.z = 1;
+    cfg.attrs = attrs; cfg.numAttrs = 2;
+    int nclusters = 0;
+    B200_CUDA(cudaOccupancyMaxActiveClusters(&nclusters, fn, &cfg));
+    B200_REQUIRE(nclusters * 2 >= grid, "wgmma persistent backward: only %d CTA pairs can be co-resident, %d needed", nclusters, grid / 2);
     KernelTimer kt("lstm_bwd_loop_tc_kernel", st);
-    B200_CUDA(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(PT), params, smem, st));
+    B200_CUDA(cudaLaunchKernelExC(&cfg, fn, params));
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }

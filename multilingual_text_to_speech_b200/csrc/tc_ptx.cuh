@@ -47,6 +47,24 @@ __device__ __forceinline__ void tma_load_5d(void* smem, const CUtensorMap* map, 
         ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
         : "memory");
 }
+// multicast variants: ONE issue writes the box to the same shared-memory offset in every CTA of the cluster named in cta_mask and completes
+// its bytes on the mbarrier at the same offset in each of them (every receiving CTA arms its own barrier)
+__device__ __forceinline__ void tma_load_3d_mc(void* smem, const CUtensorMap* map, uint64_t* bar, uint16_t cta_mask, int c0, int c1, int c2) {
+    asm volatile(
+        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5, %6}], [%2], %3;"
+        ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "h"(cta_mask), "r"(c0), "r"(c1), "r"(c2)
+        : "memory");
+}
+__device__ __forceinline__ void tma_load_5d_mc(void* smem, const CUtensorMap* map, uint64_t* bar, uint16_t cta_mask, int c0, int c1, int c2, int c3,
+                                               int c4) {
+    asm volatile(
+        "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5, %6, %7, %8}], [%2], %3;"
+        ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "h"(cta_mask), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+        : "memory");
+}
+// thread-block cluster barrier, split into arrive and wait (every thread of every CTA of the cluster)
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
 __device__ __forceinline__ void proxy_fence_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 __device__ __forceinline__ void proxy_fence_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ bool elect_one() {
