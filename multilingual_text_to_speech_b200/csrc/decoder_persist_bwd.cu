@@ -162,7 +162,8 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
     __nv_bfloat16* sWcB = reinterpret_cast<__nv_bfloat16*>(extra);                   // [A][40]
     __nv_bfloat16* sWcB2 = sWcB + (size_t)A * 40;                                    // [32][A+8]
     float* dcum = reinterpret_cast<float*>(sWcB2 + (size_t)32 * (A + 8));            // [L16 + 32] persistent d cum
-    float* wq8 = dcum + (p.MT * 16 + 32);                                            // [A][8 + 1] query weights of this CTA's 8 units
+    uint4* wqf = reinterpret_cast<uint4*>(dcum + (p.MT * 16 + 32));                  // [A / 16][32 lanes] Wq B fragments of this CTA's 8 units
+    float* s_dhq = reinterpret_cast<float*>(wqf + (size_t)(A / 16) * 32);            // [2 halves of A][64][8] query part of d h
     const unsigned nblocks = gridDim.x;
     const int L16 = p.MT * 16;
 
@@ -182,8 +183,23 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
     const int UOWN = 8;
     const bool owner = cta * UOWN < D;
     const int uo0 = cta * UOWN;
+    // B fragments (bf16 hi / lo split) of Wq[:, 8 owned units] for the query term of the cell backward: constant over the loop, built once.
+    // Entry (k-step kk, lane): {hi, hi, lo, lo} of rows a = 16 kk + 2 (lane % 4) (+1) (+8), column lane / 4
     if (owner)
-        for (int idx = tid; idx < A * UOWN; idx += PT) wq8[(idx / UOWN) * (UOWN + 1) + idx % UOWN] = p.Wq[(size_t)(idx / UOWN) * D + uo0 + idx % UOWN];
+        for (int idx = tid; idx < (A / 16) * 32; idx += PT) {
+            const int kk = idx >> 5, g = (idx >> 2) & 7, tq = idx & 3;
+            uint32_t f[4];
+#pragma unroll
+            for (int r2 = 0; r2 < 2; ++r2) {
+                const int a = kk * 16 + 2 * tq + 8 * r2;
+                const float x0 = p.Wq[(size_t)a * D + uo0 + g], x1 = p.Wq[(size_t)(a + 1) * D + uo0 + g];
+                const __nv_bfloat16 h0 = __float2bfloat16_rn(x0), h1 = __float2bfloat16_rn(x1);
+                __nv_bfloat162 hp; hp.x = h0; hp.y = h1;
+                f[r2] = *reinterpret_cast<uint32_t*>(&hp);
+                f[2 + r2] = pack2(x0 - __bfloat162float(h0), x1 - __bfloat162float(h1));
+            }
+            wqf[idx] = make_uint4(f[0], f[1], f[2], f[3]);
+        }
     uint32_t prod_it = 0;
     if (tid == 0) { tcx::mbar_init(&xb1, 1); tcx::mbar_init(&xb2, 1); tcx::mbar_init_fence(); }
     if (tid == 0) { tcx::mbar_init(&full_bar[0], 1); tcx::mbar_init(&full_bar[1], 1); tcx::mbar_init_fence(); }
@@ -262,7 +278,9 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
             }
             const int len = pa_len;                        // loaded once, before the loop
             const int mtiles = (len + 15) / 16;
-            constexpr int KT = 6;                          // k-tiles (16 memory dims) per register batch of the dw product
+            // k-tiles (16 memory dims) per register batch of the dw product.  A batch of all 18 k-tiles at M = 288 (one L2 round trip instead
+            // of three), issued before the staging, was measured slower: the kernel sits at its 255-register cap and spilled in every phase
+            constexpr int KT = 6;
             {   // Staging of the step's operands.  EVERY global load of the phase is issued before the first dependent instruction: ONE L2
                 // round trip instead of five serial ones (partial d ctx sums, alignment row, query, cumulative weights, d alignment);
                 // two register slots per thread cover M <= 2 PT and L16 + 48 <= 2 PT (checked on the host)
@@ -418,7 +436,8 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
                         mma_bf16(sacc[2 * np + 1], al, bf[2], bf[3]);
                     }
                 }
-                // ds = de[l] * v[a] * (1 - tanh^2(S + q + bias + memT)); fragment-major memory projection: 64 bf16 per lane
+                // ds = de[l] * v[a] * (1 - tanh^2(S + q + bias + memT)); fragment-major memory projection: 64 bf16 per lane.  Requesting
+                // these fragments before the Toeplitz MMAs was measured slower (register spills at the 255-register cap)
                 const uint4* mf = reinterpret_cast<const uint4*>(p.memTf + (((size_t)b * p.MT + mt) * 32 + lane) * 64);
                 const float de0 = s_de[l0 + g], de1 = s_de[l0 + g + 8];
                 uint32_t dsA[16][2];
@@ -462,8 +481,18 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
 #pragma unroll
                     for (int e = 0; e < 4; ++e) s_G[(l0 - g_lo + g + 8 * (e >> 1)) * GLD + nt * 8 + 2 * tq + (e & 1)] = gacc[nt][e];
             }
+            // the G tiles were written through the generic proxy; the bulk copy below reads the boundary tile through the async proxy
+            tcx::proxy_fence_shared();
+            __syncthreads();                               // every warp is done with s_de / s_qb / s_vv / Ph / Pl, and G is complete
+            {   // the boundary tile of G goes to the peer's halo rows (rank 0 sends its last tile, rank 1 its first) as ONE bulk copy of
+                // 16 x GLD floats (2112 B: rows of 132 B, tile and s_G 16-byte aligned) that completes on the peer's xb2
+                const int ht = hf ? HT0 : HT0 - 1;             // tile sent
+                const int peer_g_lo = hf ? 0 : (HT0 - 1) * 16;
+                if (tid == 0 && ht >= t_lo && ht < t_hi)
+                    tcx::bulk_copy_to_peer(s_G + (size_t)(ht * 16 - peer_g_lo) * GLD, s_G + (size_t)(ht * 16 - g_lo) * GLD, 16 * GLD * 4, &xb2,
+                                           (uint32_t)(hf ^ 1));
+            }
             // dq[a] = sum_l ds[l, a]: reduce over the 8 row lanes, then over warps
-            __syncthreads();                               // every warp is done with s_de / s_qb / s_vv / Ph / Pl
 #pragma unroll
             for (int nt = 0; nt < 16; ++nt)
 #pragma unroll
@@ -481,15 +510,7 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
                 for (int w8 = 0; w8 < 8; ++w8) pdq += s_dqp[w8 * A + tid];
                 st_async_peer_f32(s_dqx + tid, &xb2, (uint32_t)(hf ^ 1), pdq);
             }
-            {   // the boundary tile of G goes to the peer's halo rows (rank 0 sends its last tile, rank 1 its first)
-                const int ht = hf ? HT0 : HT0 - 1;             // tile sent
-                const int peer_g_lo = hf ? 0 : (HT0 - 1) * 16;
-                if (ht >= t_lo && ht < t_hi)
-                    for (int idx = tid; idx < 16 * GLD; idx += PT) {
-                        const int l = ht * 16 + idx / GLD, k = idx % GLD;
-                        st_async_peer_f32(s_G + (size_t)(l - peer_g_lo) * GLD + k, &xb2, (uint32_t)(hf ^ 1), s_G[(size_t)(l - g_lo) * GLD + k]);
-                    }
-                // what the PEER sends here: its A query-gradient partials, and its boundary tile if it has one (rank 0 always does; rank 1 only
+            {   // what the PEER sends here: its A query-gradient partials, and its boundary tile if it has one (rank 0 always does; rank 1 only
                 // when it owns tiles at all)
                 const bool peer_sends_tile = hf ? true : (HT0 < p.MT);
                 if (tid == 0) tcx::mbar_expect_tx(&xb2, (uint32_t)(A * 4 + (peer_sends_tile ? 16 * GLD * 4 : 0)));
@@ -532,10 +553,9 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
                 }
             }
             // d h (query part) = dq[b, :] . Wq[:, u] on the tensor cores: A = dq rows staged in shared memory (bf16 hi + lo),
-            // B = this CTA's 8 columns of Wq (bf16 hi + lo, register resident); hi.hi + lo.hi + hi.lo = fp32-equivalent
-            // (As is idle between PA and P2: [B][A] query gradients, row b rotated by 8 (b & 7) floats against bank conflicts, then [64][8] products)
+            // B = this CTA's 8 columns of Wq (bf16 hi + lo, prebuilt in wqf); hi.hi + lo.hi + hi.lo = fp32-equivalent
+            // (As is idle between PA and P2: [B][A] query gradients, row b rotated by 8 (b & 7) floats against bank conflicts)
             float* s_dq = reinterpret_cast<float*>(As);
-            float* s_dhq = s_dq + (size_t)B * A;
             {
                 constexpr int NQ = 8;                     // float4 per thread: B * A / 4 <= NQ * PT  (A = 128, B <= 64: checked on the host)
                 const float4* dq4 = reinterpret_cast<const float4*>(p.dq + (size_t)i * B * A);      // [B][A] block of this step, contiguous
@@ -577,26 +597,15 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
                         ah[r4] = *reinterpret_cast<uint32_t*>(&hp);
                         al[r4] = pack2(x.x - __bfloat162float(h0), x.y - __bfloat162float(h1));
                     }
-                    uint32_t bh[2], bl[2];
-#pragma unroll
-                    for (int r2 = 0; r2 < 2; ++r2) {
-                        const int a = a0 + 2 * tq + 8 * r2;
-                        const float x0 = wq8[a * (UOWN + 1) + g], x1 = wq8[(a + 1) * (UOWN + 1) + g];
-                        const __nv_bfloat16 h0 = __float2bfloat16_rn(x0), h1 = __float2bfloat16_rn(x1);
-                        __nv_bfloat162 hp; hp.x = h0; hp.y = h1;
-                        bh[r2] = *reinterpret_cast<uint32_t*>(&hp);
-                        bl[r2] = pack2(x0 - __bfloat162float(h0), x1 - __bfloat162float(h1));
-                    }
-                    mma_bf16(acc, ah, bh[0], bh[1]);
-                    mma_bf16(acc, al, bh[0], bh[1]);
-                    mma_bf16(acc, ah, bl[0], bl[1]);
+                    const uint4 wf = wqf[(a0 >> 4) * 32 + lane];
+                    mma_bf16(acc, ah, wf.x, wf.y);
+                    mma_bf16(acc, al, wf.x, wf.y);
+                    mma_bf16(acc, ah, wf.z, wf.w);
                 }
-                __syncthreads();                                       // every warp is done reading s_dq (s_dhq may overlap its unused tail rows)
-                float* d0 = s_dhq + (mt * 16 + g) * UOWN + 2 * tq;
-                float* d1 = s_dhq + (mt * 16 + g + 8) * UOWN + 2 * tq;
-                if (kh == 0) { d0[0] = acc[0]; d0[1] = acc[1]; d1[0] = acc[2]; d1[1] = acc[3]; }
-                __syncthreads();
-                if (kh == 1) { d0[0] += acc[0]; d0[1] += acc[1]; d1[0] += acc[2]; d1[1] += acc[3]; }
+                // each half of the A range to its own slab (outside the dq staging): one barrier, the sum is taken where it is read
+                float* d0 = s_dhq + ((kh * 64) + mt * 16 + g) * UOWN + 2 * tq;
+                float* d1 = d0 + 8 * UOWN;
+                d0[0] = acc[0]; d0[1] = acc[1]; d1[0] = acc[2]; d1[1] = acc[3];
                 __syncthreads();
             }
 #pragma unroll
@@ -605,7 +614,7 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
                 if (idx < B * UOWN) {
                     const int b = idx / UOWN, uu = idx % UOWN, u = uo0 + uu;
                     const size_t bu = (size_t)b * D + u, g0 = ((size_t)i * B + b) * 4 * D + u;
-                    float dh = dhs_[e] + s_dhq[b * UOWN + uu];
+                    float dh = dhs_[e] + (s_dhq[b * UOWN + uu] + s_dhq[(64 + b) * UOWN + uu]);
                     float dc_in = 0.f;
                     if (!last) {
                         dh += rec_[e] + dhz_reg[e];
@@ -978,7 +987,8 @@ static AttBwdGeom att_bwd_geom(const b200tts_decoder_shape& s) {
     AttBwdGeom g{};
     g.UK = s.D / KBA;
     const int L16 = (s.L + 15) / 16 * 16;
-    const size_t extras = (size_t)s.A * 40 * 2 + (size_t)32 * (s.A + 8) * 2 + (size_t)(L16 + 32) * 4 + (size_t)s.A * 9 * 4;
+    // Wcomb in two layouts, d cum, Wq fragments (A / 16 x 32 x 16 B), two [64][8] slabs of the query part of d h
+    const size_t extras = (size_t)s.A * 40 * 2 + (size_t)32 * (s.A + 8) * 2 + (size_t)(L16 + 32) * 4 + (size_t)s.A * 32 + 2 * 64 * 8 * 4;
     g.UN = (s.M + s.D <= NBT * TUN) ? TUN : TUN_WIDE; g.grid = KBA * NBT;
     const int NKT = 4 * g.UK / 64;
     g.region = (size_t)NKT * 8192;
@@ -998,7 +1008,8 @@ bool persist_att_bwd_supported(const b200tts_decoder_shape& s) {
     const size_t fl = (size_t)((s.M + 3) & ~3) + 3 * (size_t)L16 + 2 * s.A + 2 * (size_t)(L16 + 48) + 64 + (size_t)(HT0 + 1) * 16 * GLD +
                       8 * (size_t)s.A + s.A + 4 + (size_t)((s.M + 15) / 16) * 32 * 2;
     if (fl * 4 > g.region) return false;
-    // the cell-backward phase stages the query gradients [B][A] fp32 + [64][8] products in the (then idle) TMA slot
+    // the cell-backward phase stages the query gradients [B][A] fp32 in the (then idle) TMA slot.  The bound keeps 2 KB to spare (a [64][8]
+    // slab), which holds B <= 60 at D = 512: the shapes this loop accepts are the ones its tests cover
     if ((size_t)s.B * s.A * 4 + 64 * 8 * 4 > g.region) return false;
     return g.smem <= 227 * 1024;
 }

@@ -62,6 +62,17 @@ __device__ __forceinline__ void tma_load_5d_mc(void* smem, const CUtensorMap* ma
         ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "h"(cta_mask), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
         : "memory");
 }
+// bulk copy of `bytes` (a multiple of 16; both addresses 16-byte aligned) from this CTA's shared memory to the peer CTA `peer_rank` of the
+// cluster: dst and bar are given as this CTA's addresses of the same-offset buffer / mbarrier in the peer, whose barrier the copy completes
+// its bytes on.  The source must have been made visible to the async proxy (proxy_fence_shared after the generic writes).
+__device__ __forceinline__ void bulk_copy_to_peer(const void* dst, const void* src, uint32_t bytes, const uint64_t* bar, uint32_t peer_rank) {
+    uint32_t rd, rb;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rd) : "r"(smem_u32(dst)), "r"(peer_rank));
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rb) : "r"(smem_u32(bar)), "r"(peer_rank));
+    asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(rd), "r"(smem_u32(src)), "r"(bytes), "r"(rb)
+                 : "memory");
+}
 // thread-block cluster barrier, split into arrive and wait (every thread of every CTA of the cluster)
 __device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
 __device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
