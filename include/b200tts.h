@@ -36,6 +36,9 @@ extern "C" {
 #define B200TTS_CELL_DROPOUT 0 /* DropoutLSTMCell  modules/layers.py:37-47 */
 #define B200TTS_CELL_ZONEOUT 1 /* ZoneoutLSTMCell  modules/layers.py:18-34 */
 
+#define B200TTS_ATT_LOCATION 0 /* LocationSensitiveAttention  modules/attention.py:48-86 (hp.attention_type "location_sensitive") */
+#define B200TTS_ATT_FORWARD 1  /* ForwardAttention            modules/attention.py:89-124 (hp.attention_type "forward") */
+
 /* ---- library ---------------------------------------------------------------------------- */
 const char* b200tts_last_error(void);
 int b200tts_version(void);
@@ -80,6 +83,10 @@ typedef struct {
     int training;           /* nn.Module.training of the cells (prenet dropout is always on) */
     float rate_h, rate_c;   /* dropout_hidden | (zoneout_hidden, zoneout_cell) */
     float prenet_rate;      /* hp.dropout used by the prenet */
+    int att_kind;           /* B200TTS_ATT_*; 0 (location-sensitive) in a zero-initialised shape.  B200TTS_ATT_FORWARD: C and K
+                               are ignored, params.attn_location / attn_loc_features must be NULL, the cumulative-weight rows of
+                               the workspace (and b200tts_decoder_state.cum_weights) hold the forward variable alpha, and every
+                               recurrence runs on the per-step kernel chains in both precision modes (b200tts_decoder_path = 0) */
 } b200tts_decoder_shape;
 
 /* Parameter block in the reference's own layouts ([out, in] Linear weights; names = state_dict keys). */
@@ -137,7 +144,7 @@ size_t b200tts_decoder_bwd_workspace_bytes(const b200tts_decoder_shape* shape);
  * forward loops, bit 1 = their TMA + wgmma variant, bit 2 = persistent generator reverse loop, bit 3 = its wgmma
  * variant, bit 4 = persistent attention reverse loop, bit 5 = its wgmma product.  0 = the per-step kernel chains.
  * Every persistent loop is a TMA + wgmma kernel, so each variant bit (1, 3, 5) is set exactly when its loop bit (0, 2, 4)
- * is; a pass whose loop bit is clear runs the per-step kernel chains.
+ * is; a pass whose loop bit is clear runs the per-step kernel chains.  Forward attention (att_kind = B200TTS_ATT_FORWARD) always gives 0.
  * (The reference has no such limit anywhere: modules/attention.py:67-74 takes any length.) */
 int b200tts_decoder_path(const b200tts_decoder_shape* shape);
 /* Debug: byte offset, inside the decoder forward workspace, of the per-CTA phase cycle counters the persistent
@@ -156,7 +163,7 @@ typedef struct {
     float* att_h; float* att_c; /* [B, D] attention-LSTM state */
     float* gen_h; float* gen_c; /* [B, D] generator-LSTM state */
     float* context;             /* [B, M] last attention context */
-    float* cum_weights;         /* [B, L] cumulative attention weights */
+    float* cum_weights;         /* [B, L] cumulative attention weights (forward attention: the last alignment = alpha) */
     float* frame;               /* [B, N] last predicted frame (input of the next free-running step) */
 } b200tts_decoder_state;
 
@@ -207,6 +214,27 @@ int b200tts_attention_step_backward(int B, int L, int M, int A, int C, int K, co
                                     const float* weights, const float* d_context, const float* d_weights, float* d_cum, float* d_q,
                                     float* d_memory_transform, float* d_w_location, float* d_w_loc_features, float* d_w_energy,
                                     float* workspace, void* stream);
+
+/* ---- single forward-attention step: ForwardAttention.forward, modules/attention.py:23-45,89-124 ----
+ * e = v . tanh(query . Wq^T + memory_transform + bias) over ALL L positions; s = softmax(e) (padding included);
+ * a[l] = (alpha[l] + alpha[l-1]) * s[l]; a[l] = 0 for l >= text_lengths; w = clamp(a, 1e-6) / sum; context = w . memory.
+ * alpha [B, L] is read and replaced by w in place (ForwardAttention.reset sets alpha[:, 0] = 1); context [B, M], weights [B, L]
+ * written.  workspace floats: b200tts_forward_attention_step_workspace_elems(B, L, A); its head holds q = query . Wq^T [B, A]. */
+size_t b200tts_forward_attention_step_workspace_elems(int B, int L, int A);
+int b200tts_forward_attention_step(int B, int L, int M, int D, int A, const float* query, const float* memory,
+                                   const float* memory_transform, const int32_t* text_lengths, const float* w_query,
+                                   const float* bias, const float* w_energy, float* alpha, float* context, float* weights,
+                                   float* workspace, void* stream);
+/* Backward of one forward-attention step.  q [B, A] as the forward left it; alpha_prev [B, L] the alpha the step CONSUMED; weights
+ * [B, L] its output.  d_alpha [B, L]: in = gradient of the new alpha (= weights), out = gradient of alpha_prev.  d_q [B, A] out (the
+ * caller forms d query, d Wq and d bias = sum_b d_q); d_memory_transform [B, L, A] and d_w_energy [A] are ACCUMULATED (+=), the latter
+ * from per-utterance partials reduced over the batch in a fixed order.
+ * workspace floats: b200tts_forward_attention_step_backward_workspace_elems(B, M, A).                                             */
+size_t b200tts_forward_attention_step_backward_workspace_elems(int B, int M, int A);
+int b200tts_forward_attention_step_backward(int B, int L, int M, int A, const float* q, const float* memory, const float* memory_transform,
+                                            const int32_t* text_lengths, const float* bias, const float* w_energy, const float* alpha_prev,
+                                            const float* weights, const float* d_context, const float* d_weights, float* d_alpha,
+                                            float* d_q, float* d_memory_transform, float* d_w_energy, float* workspace, void* stream);
 
 /* ---- convolution block: ConvBlock / HighwayConvBlock / ConvBlockGenerated / HighwayConvBlockGenerated ----
  * modules/layers.py:50-178.  x [NB, G*Cin, L] -> pad((k-1)*dil/2) -> grouped Conv1d(no bias) -> BatchNorm1d

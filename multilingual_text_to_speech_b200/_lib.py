@@ -11,6 +11,7 @@ _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG, 'libb200tts.so')
 
 CELL_DROPOUT, CELL_ZONEOUT = 0, 1
+ATT_LOCATION, ATT_FORWARD = 0, 1
 
 
 class B200TTSError(RuntimeError):
@@ -19,7 +20,7 @@ class B200TTSError(RuntimeError):
 
 class DecoderShape(Structure):
     _fields_ = [(n, c_int) for n in ('B', 'L', 'T', 'M', 'D', 'P', 'A', 'C', 'K', 'N', 'cell_kind', 'training')] + \
-               [('rate_h', c_float), ('rate_c', c_float), ('prenet_rate', c_float)]
+               [('rate_h', c_float), ('rate_c', c_float), ('prenet_rate', c_float), ('att_kind', c_int)]
 
 
 DECODER_PARAM_FIELDS = ('prenet_w0', 'prenet_b0', 'prenet_w1', 'prenet_b1', 'att_w_ih', 'att_w_hh', 'att_b_ih', 'att_b_hh',
@@ -99,6 +100,10 @@ SIGNATURES = {
     'b200tts_attention_step': (c_int, [c_int] * 7 + [c_void_p] * 13),
     'b200tts_attention_step_backward_workspace_elems': (c_size_t, [c_int] * 5),
     'b200tts_attention_step_backward': (c_int, [c_int] * 6 + [c_void_p] * 20),
+    'b200tts_forward_attention_step_workspace_elems': (c_size_t, [c_int, c_int, c_int]),
+    'b200tts_forward_attention_step': (c_int, [c_int] * 5 + [c_void_p] * 12),
+    'b200tts_forward_attention_step_backward_workspace_elems': (c_size_t, [c_int] * 3),
+    'b200tts_forward_attention_step_backward': (c_int, [c_int] * 4 + [c_void_p] * 16),
     'b200tts_convblock_saved_bytes': (c_size_t, [POINTER(ConvBlockShape)]),
     'b200tts_convblock_workspace_bytes': (c_size_t, [POINTER(ConvBlockShape)]),
     'b200tts_convblock_forward': (c_int, [POINTER(ConvBlockShape), c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p,

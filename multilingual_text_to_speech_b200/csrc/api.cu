@@ -91,6 +91,14 @@ int attention_step_impl(int B, int L, int M, int D, int A, int C, int K, const f
                         const float* memT, const int* lengths, const float* Wq, const float* Wloc, const float* Wc,
                         const float* bias, const float* v, float* cum, float* ctx, float* weights, float* workspace,
                         cudaStream_t st);
+int forward_attention_step_impl(int B, int L, int M, int D, int A, const float* query, const float* memory, const float* memT,
+                                const int* lengths, const float* Wq, const float* bias, const float* v, float* alpha, float* ctx,
+                                float* weights, float* workspace, cudaStream_t st);
+size_t forward_attention_step_backward_workspace_elems(int B, int M, int A);
+int forward_attention_step_backward_impl(int B, int L, int M, int A, const float* q, const float* memory, const float* memT,
+                                         const int* lengths, const float* bias, const float* v, const float* alpha_prev,
+                                         const float* weights, const float* d_ctx, const float* d_weights, float* d_alpha, float* d_q,
+                                         float* d_memT, float* d_v, float* ws, cudaStream_t st);
 
 
 size_t convblock_saved_floats(const b200tts_convblock_shape& s);
@@ -312,6 +320,34 @@ int b200tts_attention_step_backward(int B, int L, int M, int A, int C, int K, co
     return attention_step_backward_impl(B, L, M, A, C, K, q, memory, memory_transform, text_lengths, w_location, w_loc_features, bias,
                                         w_energy, cum_prev, weights, d_context, d_weights, d_cum, d_q, d_memory_transform, d_w_location,
                                         d_w_loc_features, d_w_energy, workspace, (cudaStream_t)stream);
+}
+
+size_t b200tts_forward_attention_step_workspace_elems(int B, int L, int A) { return (size_t)B * A + (size_t)B * L; }
+
+int b200tts_forward_attention_step(int B, int L, int M, int D, int A, const float* query, const float* memory,
+                                   const float* memory_transform, const int32_t* text_lengths, const float* w_query,
+                                   const float* bias, const float* w_energy, float* alpha, float* context, float* weights,
+                                   float* workspace, void* stream) {
+    B200_TRY(require_device());
+    B200_REQUIRE(query && memory && memory_transform && text_lengths && w_query && bias && w_energy && alpha && context && weights &&
+                 workspace, "forward_attention_step: null argument");
+    return forward_attention_step_impl(B, L, M, D, A, query, memory, memory_transform, text_lengths, w_query, bias, w_energy, alpha,
+                                       context, weights, workspace, (cudaStream_t)stream);
+}
+
+size_t b200tts_forward_attention_step_backward_workspace_elems(int B, int M, int A) {
+    return forward_attention_step_backward_workspace_elems(B, M, A);
+}
+int b200tts_forward_attention_step_backward(int B, int L, int M, int A, const float* q, const float* memory, const float* memory_transform,
+                                            const int32_t* text_lengths, const float* bias, const float* w_energy, const float* alpha_prev,
+                                            const float* weights, const float* d_context, const float* d_weights, float* d_alpha,
+                                            float* d_q, float* d_memory_transform, float* d_w_energy, float* workspace, void* stream) {
+    B200_TRY(require_device());
+    B200_REQUIRE(q && memory && memory_transform && text_lengths && bias && w_energy && alpha_prev && weights && d_context && d_alpha &&
+                 d_q && d_memory_transform && d_w_energy && workspace, "forward_attention_step_backward: null argument");
+    return forward_attention_step_backward_impl(B, L, M, A, q, memory, memory_transform, text_lengths, bias, w_energy, alpha_prev,
+                                                weights, d_context, d_weights, d_alpha, d_q, d_memory_transform, d_w_energy, workspace,
+                                                (cudaStream_t)stream);
 }
 
 size_t b200tts_convblock_saved_bytes(const b200tts_convblock_shape* s) { return s ? convblock_saved_floats(*s) * sizeof(float) : 0; }

@@ -486,6 +486,147 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_kernel(const AttnBwdArgs
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Forward-attention step backward (modules/attention.py:89-124), one CTA per utterance.  Recomputes the transition
+// probabilities from the saved query and alpha (no energy storage) with the forward's own code (fwd_att_transition), so
+// the clamp decisions match the forward bit for bit.  Chain: w = c / S  ->  c = clamp(a, 1e-6) (gradient where a >= 1e-6)
+// -> a = 0 beyond the length (in-place mask: no gradient) -> a = (alpha + alpha shifted) * s -> softmax -> tanh energies.
+// ---------------------------------------------------------------------------------------------
+struct FwdAttnBwdArgs {
+    const float* q;            // [B, A] saved query of this step
+    const float* memT;         // [B, L, A]
+    const float* memory;       // [B, L, M]
+    const int* lengths;
+    const float* bias; const float* v;
+    const float* alpha_prev;   // [B, L] alpha the step consumed
+    const float* w;  long long w_bstride;            // &align[0, i, 0] (= the alpha the step produced)
+    const float* dalign; long long dalign_bstride;   // &d_align[0, i, 0] or null
+    const float* dctx_static;  // [B, M]
+    const float* part; int nsplit; size_t part_stride; int ld_part;   // recurrent d ctx partials (cols [0, M)); null on last step
+    float* dalpha;             // [B, L] in: d alpha_{i+1}, out: d alpha_i
+    float* dctx_tot;           // [B, M] out
+    float* dq;                 // [B, A] out
+    float* dmemT;              // [B, L, A] +=
+    float* dv_acc;             // [B, A] +=  (per-utterance partials, reduced over the batch in a fixed order afterwards)
+    int B, L, M, A, last;
+};
+
+static inline size_t fwd_attn_bwd_smem_floats(int L, int M, int A) {
+    const size_t Lp = (L + 3) & ~3;
+    return (size_t)2 * A + 3 * Lp + 64 + ((M + 3) & ~3) + (size_t)(ATT_THREADS / 32) * A;
+}
+
+__global__ void __launch_bounds__(ATT_THREADS) fwd_attn_bwd_kernel(const FwdAttnBwdArgs p) {
+    extern __shared__ __align__(16) float sm[];
+    const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    constexpr int NW = ATT_THREADS / 32;
+    const int L = p.L, A = p.A, M = p.M, Lp = (L + 3) & ~3;
+    float* qb = sm; float* vv = qb + A;
+    float* s = vv + A; float* g = s + Lp; float* da = g + Lp;
+    float* red = da + Lp; float* dctx = red + 64; float* cred = dctx + ((M + 3) & ~3);
+    int len = p.lengths[b];
+    len = len < 0 ? 0 : (len > L ? L : len);
+    const float* alpha = p.alpha_prev + (size_t)b * L;
+    const float* w = p.w + (size_t)b * p.w_bstride;
+
+    // ---- phase 1: stage q + bias, v, d context ----
+    for (int a = tid; a < A; a += ATT_THREADS) { qb[a] = p.q[(size_t)b * A + a] + p.bias[a]; vv[a] = p.v[a]; }
+    for (int m = tid; m < M; m += ATT_THREADS) {
+        float gm = p.dctx_static[(size_t)b * M + m];
+        if (!p.last)
+            for (int k = 0; k < p.nsplit; ++k) gm += p.part[k * p.part_stride + (size_t)b * p.ld_part + m];
+        dctx[m] = gm;
+        p.dctx_tot[(size_t)b * M + m] = gm;
+    }
+    __syncthreads();
+
+    // ---- phase 2: transition probabilities s (recomputed); d w[l] = d align + d alpha_{i+1} + <d ctx, memory[l]> over all L ----
+    fwd_att_transition(qb, vv, p.memT + (size_t)b * L * A, L, A, s, red);
+    for (int l = warp; l < L; l += NW) {
+        const float* row = p.memory + ((size_t)b * L + l) * M;
+        float acc = 0.f;
+        for (int m = lane; m < M; m += 32) acc = fmaf(dctx[m], row[m], acc);
+        acc = warp_sum(acc);
+        if (lane == 0) {
+            float gl = acc + (p.last ? 0.f : p.dalpha[(size_t)b * L + l]);
+            if (p.dalign) gl += p.dalign[(size_t)b * p.dalign_bstride + l];
+            g[l] = gl;
+        }
+    }
+    __syncthreads();
+
+    // ---- phase 3: L1 normalisation and clamp: d c = (d w - <d w, w>) / S;  d a = d c where l < len and a >= 1e-6 ----
+    float dot = 0.f, csum = 0.f;
+    for (int l = tid; l < L; l += ATT_THREADS) {
+        dot = fmaf(g[l], w[l], dot);
+        csum += fmaxf(fwd_att_product(alpha, s, l, len), FWD_ATT_FLOOR);
+    }
+    dot = block_sum(dot, red);
+    const float denom = fmaxf(block_sum(csum, red), FWD_ATT_NORM_EPS);
+    for (int l = tid; l < L; l += ATT_THREADS) {
+        const float a = fwd_att_product(alpha, s, l, len);
+        da[l] = (l < len && a >= FWD_ATT_FLOOR) ? (g[l] - dot) / denom : 0.f;
+    }
+    __syncthreads();
+
+    // ---- phase 4: the product: d alpha[l] = d a[l] s[l] + d a[l+1] s[l+1];  d s[l] = d a[l] (alpha[l] + alpha[l-1]) ----
+    float sds = 0.f;
+    for (int l = tid; l < L; l += ATT_THREADS) {
+        const float dnext = l + 1 < L ? da[l + 1] * s[l + 1] : 0.f;
+        p.dalpha[(size_t)b * L + l] = fmaf(da[l], s[l], dnext);
+        const float ds = da[l] * (alpha[l] + (l > 0 ? alpha[l - 1] : 0.f));
+        g[l] = ds;
+        sds = fmaf(s[l], ds, sds);
+    }
+    // softmax backward: d e[l] = s[l] (d s[l] - <s, d s>)
+    sds = block_sum(sds, red);
+    for (int l = tid; l < L; l += ATT_THREADS) g[l] = s[l] * (g[l] - sds);
+    __syncthreads();
+
+    // ---- phase 5: energy backward over every position: d pre = d e v (1 - tanh^2) -> d q, d memT; d v += d e tanh ----
+    float dq_reg[4] = {0.f, 0.f, 0.f, 0.f}, dv_reg[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int l = warp; l < L; l += NW) {
+        const float del = g[l];
+        const size_t row = ((size_t)b * L + l) * A;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int a = lane + 32 * j;
+            if (a < A) {
+                const float th = tanhf(qb[a] + p.memT[row + a]);
+                const float dpre = del * vv[a] * (1.f - th * th);
+                dv_reg[j] = fmaf(del, th, dv_reg[j]);
+                dq_reg[j] += dpre;
+                p.dmemT[row + a] += dpre;
+            }
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const int a = lane + 32 * j;
+        if (a < A) cred[warp * A + a] = dq_reg[j];
+    }
+    __syncthreads();
+    for (int a = tid; a < A; a += ATT_THREADS) {
+        float acc = 0.f;
+#pragma unroll
+        for (int w8 = 0; w8 < NW; ++w8) acc += cred[w8 * A + a];
+        p.dq[(size_t)b * A + a] = acc;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const int a = lane + 32 * j;
+        if (a < A) cred[warp * A + a] = dv_reg[j];
+    }
+    __syncthreads();
+    for (int a = tid; a < A; a += ATT_THREADS) {
+        float acc = 0.f;
+#pragma unroll
+        for (int w8 = 0; w8 < NW; ++w8) acc += cred[w8 * A + a];
+        p.dv_acc[(size_t)b * A + a] += acc;
+    }
+}
+
 }  // namespace
 int launch_cell_bwd(const CellBwdArgs& a, cudaStream_t st) {
     const int Bp = (a.B + 7) & ~7;
@@ -522,6 +663,19 @@ int launch_attn_bwd(AttnBwdArgs a, cudaStream_t st) {
     return B200TTS_OK;
 }
 
+int launch_fwd_attn_bwd(const FwdAttnBwdArgs& a, cudaStream_t st) {
+    const size_t smem = fwd_attn_bwd_smem_floats(a.L, a.M, a.A) * sizeof(float);
+    B200_REQUIRE(smem <= 227 * 1024, "forward attention backward: shared memory %zu B exceeds 227 KB (L=%d)", smem, a.L);
+    static size_t configured = 48 * 1024;
+    if (smem > configured) {
+        B200_CUDA(cudaFuncSetAttribute(fwd_attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        configured = smem;
+    }
+    fwd_attn_bwd_kernel<<<a.B, ATT_THREADS, smem, st>>>(a);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
 // ---------------------------------------------------------------------------------------------
 // backward workspace
 // ---------------------------------------------------------------------------------------------
@@ -536,7 +690,8 @@ BwdLayout bwd_layout(const b200tts_decoder_shape& s) {
     BwdLayout l;
     size_t off = 0;
     auto take = [&](size_t n) { size_t o = off; off = align_up(off + n, 64); return o; };
-    const size_t T = s.T, B = s.B, D = s.D, M = s.M, P = s.P, A = s.A, N = s.N, L = s.L, C = s.C, K = s.K;
+    const size_t T = s.T, B = s.B, D = s.D, M = s.M, P = s.P, A = s.A, N = s.N, L = s.L;
+    const size_t C = forward_attention(s) ? 0 : s.C, K = forward_attention(s) ? 0 : s.K;     // ignored for forward attention
     l.dfs = take(T * B * (N + 1));
     l.dhgd = take(T * B * D);
     l.dctxs = take(T * B * M);
@@ -645,13 +800,39 @@ int attention_step_backward_impl(int B, int L, int M, int A, int C, int K, const
     return B200TTS_OK;
 }
 
+// standalone backward of one forward-attention step: per-utterance d v partials in the workspace, reduced over the batch here
+size_t forward_attention_step_backward_workspace_elems(int B, int M, int A) { return (size_t)B * ((size_t)A + M); }
+int forward_attention_step_backward_impl(int B, int L, int M, int A, const float* q, const float* memory, const float* memT,
+                                         const int* lengths, const float* bias, const float* v, const float* alpha_prev,
+                                         const float* weights, const float* d_ctx, const float* d_weights, float* d_alpha, float* d_q,
+                                         float* d_memT, float* d_v, float* ws, cudaStream_t st) {
+    B200_REQUIRE(B > 0 && L > 0 && A > 0 && A <= 128 && M > 0 && M <= 512,
+                 "forward_attention_step_backward: unsupported dims B=%d L=%d A=%d M=%d", B, L, A, M);
+    float* dv_acc = ws;
+    float* dctx_tot = dv_acc + (size_t)B * A;
+    B200_TRY(launch_fill(dv_acc, 0.f, (size_t)B * A, st));
+    FwdAttnBwdArgs fa{};
+    fa.q = q; fa.memT = memT; fa.memory = memory; fa.lengths = lengths; fa.bias = bias; fa.v = v;
+    fa.alpha_prev = alpha_prev; fa.w = weights; fa.w_bstride = L; fa.dalign = d_weights; fa.dalign_bstride = L;
+    fa.dctx_static = d_ctx; fa.part = nullptr; fa.nsplit = 0; fa.part_stride = 0; fa.ld_part = 0;
+    fa.dalpha = d_alpha; fa.dctx_tot = dctx_tot; fa.dq = d_q; fa.dmemT = d_memT; fa.dv_acc = dv_acc;
+    fa.B = B; fa.L = L; fa.M = M; fa.A = A; fa.last = 0;
+    B200_TRY(launch_fwd_attn_bwd(fa, st));
+    batchsum_add_kernel<<<1, 256, 0, st>>>(d_v, dv_acc, B, (size_t)A);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
 int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
                           const b200tts_decoder_outputs& fwd_out, const b200tts_decoder_output_grads& dout, const float* fws,
                           float* bws, size_t bws_bytes, const b200tts_decoder_params& dw, float* d_memory, cudaStream_t st) {
     B200_TRY(validate_decoder_shape(s));
     B200_REQUIRE(fwd_out.alignments, "decoder_backward: the forward alignments tensor is required");
-    B200_REQUIRE(s.A % 4 == 0 && s.C % 4 == 0 && (s.A / 4) * (s.C / 4) <= ATT_THREADS,
+    const bool fwd_att = forward_attention(s);
+    B200_REQUIRE(fwd_att || (s.A % 4 == 0 && s.C % 4 == 0 && (s.A / 4) * (s.C / 4) <= ATT_THREADS),
                  "decoder_backward: attention dims A=%d C=%d unsupported (need A%%4==0, C%%4==0, A*C<=4096)", s.A, s.C);
+    B200_REQUIRE(!fwd_att || (!w.attn_location && !w.attn_loc_features && !dw.attn_location && !dw.attn_loc_features),
+                 "decoder_backward: forward attention has no location weights (pass NULL)");
     if (in.teacher)
         for (int i = 0; i < s.T; ++i)
             if (!in.teacher[i]) {
@@ -750,11 +931,27 @@ int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_
                                       reinterpret_cast<unsigned char*>(W(l.pextra2)), dw, st, dgab));
     } else {
     B200_TRY(launch_fill(W(l.dmemT), 0.f, (size_t)B * L * A, st));
-        B200_TRY(launch_fill(W(l.dWloc_acc), 0.f, (size_t)B * A * C, st));
-        B200_TRY(launch_fill(W(l.dWc_acc), 0.f, (size_t)B * C * K, st));
+        if (!fwd_att) {
+            B200_TRY(launch_fill(W(l.dWloc_acc), 0.f, (size_t)B * A * C, st));
+            B200_TRY(launch_fill(W(l.dWc_acc), 0.f, (size_t)B * C * K, st));
+        }
         B200_TRY(launch_fill(W(l.dv_acc), 0.f, (size_t)B * A, st));
         for (int i = T - 1; i >= 0; --i) {
             const int last = (i == T - 1);
+            if (fwd_att) {
+                FwdAttnBwdArgs fa{};
+                fa.q = F(fl.q) + (size_t)i * B * A; fa.memT = F(fl.memT); fa.memory = in.memory; fa.lengths = in.text_lengths;
+                fa.bias = w.attn_bias; fa.v = w.attn_energy;
+                fa.alpha_prev = F(fl.cum) + (size_t)i * B * L;
+                fa.w = fwd_out.alignments + (size_t)i * L; fa.w_bstride = (long long)T * L;
+                fa.dalign = dout.d_alignments ? dout.d_alignments + (size_t)i * L : nullptr; fa.dalign_bstride = (long long)T * L;
+                fa.dctx_static = W(l.dctxs) + (size_t)i * B * M;
+                fa.part = W(l.part); fa.nsplit = l.split_att; fa.part_stride = (size_t)B * MD; fa.ld_part = MD;
+                fa.dalpha = W(l.dcum); fa.dctx_tot = W(l.dctxt) + (size_t)i * B * M; fa.dq = W(l.dq) + (size_t)i * B * A;
+                fa.dmemT = W(l.dmemT); fa.dv_acc = W(l.dv_acc);
+                fa.B = B; fa.L = L; fa.M = M; fa.A = A; fa.last = last;
+                B200_TRY(launch_fwd_attn_bwd(fa, st));
+            } else {
             AttnBwdArgs aa{};
             aa.q = F(fl.q) + (size_t)i * B * A; aa.memT = F(fl.memT); aa.memory = in.memory; aa.lengths = in.text_lengths;
             aa.Wc = w.attn_loc_features; aa.Wloc = w.attn_location; aa.bias = w.attn_bias; aa.v = w.attn_energy;
@@ -767,13 +964,14 @@ int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_
             aa.dmemT = W(l.dmemT); aa.dWloc_acc = W(l.dWloc_acc); aa.dWc_acc = W(l.dWc_acc); aa.dv_acc = W(l.dv_acc);
             aa.B = B; aa.L = L; aa.M = M; aa.A = A; aa.C = C; aa.K = K; aa.last = last;
             B200_TRY(launch_attn_bwd(aa, st));
+            }
 
             CellBwdArgs ca{};
             ca.gates = F(fl.ga) + (size_t)i * B4D;
             ca.c_prev = F(fl.ca) + (size_t)i * BD;
             ca.dh_static = W(l.dhas) + (size_t)i * BD; ca.ld_dhs = D;
             ca.part = W(l.part); ca.nsplit = l.split_att; ca.part_stride = (size_t)B * MD; ca.ld_part = MD; ca.part_col0 = M;
-            ca.dq = aa.dq; ca.Wq = w.attn_query; ca.A = A;
+            ca.dq = W(l.dq) + (size_t)i * B * A; ca.Wq = w.attn_query; ca.A = A;
             ca.dc_state = W(l.dc); ca.dhz_state = zone ? W(l.dhz) : nullptr;
             ca.mask_h = in.mask_att_h ? in.mask_att_h + (size_t)i * BD : nullptr;
             ca.mask_c = in.mask_att_c ? in.mask_att_c + (size_t)i * BD : nullptr;
@@ -804,10 +1002,12 @@ int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_
     // d Wq = dQ^T . h_att
     B200_TRY(wgemm16(st, l, bws, A, D, (int)TB, W(l.dq), A, ai1 + M, MD, aib1, ldab, dw.attn_query, D, 1.f));
     if (!plan.att_bwd) {
-        batchsum_add_kernel<<<grid_for((size_t)A * C), 256, 0, st>>>(dw.attn_location, W(l.dWloc_acc), B, (size_t)A * C);
-        B200_LAUNCH_CHECK();
-        batchsum_add_kernel<<<grid_for((size_t)C * K), 256, 0, st>>>(dw.attn_loc_features, W(l.dWc_acc), B, (size_t)C * K);
-        B200_LAUNCH_CHECK();
+        if (!fwd_att) {
+            batchsum_add_kernel<<<grid_for((size_t)A * C), 256, 0, st>>>(dw.attn_location, W(l.dWloc_acc), B, (size_t)A * C);
+            B200_LAUNCH_CHECK();
+            batchsum_add_kernel<<<grid_for((size_t)C * K), 256, 0, st>>>(dw.attn_loc_features, W(l.dWc_acc), B, (size_t)C * K);
+            B200_LAUNCH_CHECK();
+        }
         batchsum_add_kernel<<<1, 256, 0, st>>>(dw.attn_energy, W(l.dv_acc), B, (size_t)A);
         B200_LAUNCH_CHECK();
     }

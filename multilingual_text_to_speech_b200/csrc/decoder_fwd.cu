@@ -309,6 +309,100 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnFwdArgs
     }
 }
 
+// =============================================================================================
+// Forward-attention step (modules/attention.py:23-45, 89-124), one CTA per utterance:
+//   s = softmax(v . tanh(q + memT + bias)) over all L;  a = (alpha + alpha shifted by one) * s, zero at l >= length;
+//   w = clamp(a, 1e-6) / max(sum, 1e-12);  context = w . memory over all L;  w is the alignment row and the next alpha.
+// =============================================================================================
+struct FwdAttnArgs {
+    const float* qpart; int nq;        // [nq, B, A] partial queries (summed here)
+    float* q_save;                     // [B, A] or null
+    const float* memT;                 // [B, L, A]
+    const float* memory;               // [B, L, M]
+    const int* lengths;                // [B]
+    const float* bias; const float* v; // [A]
+    const float* alpha_prev; float* alpha_next;   // [B, L] (distinct buffers)
+    float* align; long long align_bstride;        // &align[0, i, 0]; stride between utterances
+    float* ctx_out; int ld_ctx;        // [B, ld]
+    int B, L, M, A;
+};
+
+static inline size_t fwd_attn_smem_floats(int L, int M, int A) {
+    return (size_t)2 * A + ((L + 3) & ~3) + 64 + (size_t)(ATT_THREADS / 32) * M;
+}
+
+__global__ void __launch_bounds__(ATT_THREADS) fwd_attn_fwd_kernel(const FwdAttnArgs p) {
+    extern __shared__ __align__(16) float sm[];
+    const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    constexpr int NW = ATT_THREADS / 32;
+    const int L = p.L, A = p.A, M = p.M;
+    float* qb = sm;
+    float* vv = qb + A;
+    float* s = vv + A;
+    float* red = s + ((L + 3) & ~3);
+    float* cred = red + 64;
+    int len = p.lengths[b];
+    len = len < 0 ? 0 : (len > L ? L : len);
+    const float* alpha = p.alpha_prev + (size_t)b * L;
+
+    for (int a = tid; a < A; a += ATT_THREADS) {
+        float q = 0.f;
+        for (int k = 0; k < p.nq; ++k) q += p.qpart[((size_t)k * p.B + b) * A + a];
+        if (p.q_save) p.q_save[(size_t)b * A + a] = q;
+        qb[a] = q + p.bias[a];
+        vv[a] = p.v[a];
+    }
+    __syncthreads();
+    fwd_att_transition(qb, vv, p.memT + (size_t)b * L * A, L, A, s, red);
+
+    float csum = 0.f;
+    for (int l = tid; l < L; l += ATT_THREADS) {
+        const float c = fmaxf(fwd_att_product(alpha, s, l, len), FWD_ATT_FLOOR);
+        s[l] = c;           // each thread rewrites only the positions it read
+        csum += c;
+    }
+    const float denom = fmaxf(block_sum(csum, red), FWD_ATT_NORM_EPS);
+    for (int l = tid; l < L; l += ATT_THREADS) {
+        const float w = s[l] / denom;
+        s[l] = w;
+        p.align[(size_t)b * p.align_bstride + l] = w;
+        p.alpha_next[(size_t)b * L + l] = w;
+    }
+    __syncthreads();
+
+    // context[m] = sum over every l < L of w[l] * memory[b, l, m]
+    float acc[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) acc[j] = 0.f;
+    for (int l = warp; l < L; l += NW) {
+        const float w = s[l];
+        const float* row = p.memory + ((size_t)b * L + l) * M;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            const int m = lane + 32 * j;
+            if (m < M) acc[j] = fmaf(w, row[m], acc[j]);
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+        const int m = lane + 32 * j;
+        if (m < M) cred[warp * M + m] = acc[j];
+    }
+    __syncthreads();
+    for (int m = tid; m < M; m += ATT_THREADS) {
+        float acc_m = 0.f;
+#pragma unroll
+        for (int w = 0; w < NW; ++w) acc_m += cred[w * M + m];
+        p.ctx_out[(size_t)b * p.ld_ctx + m] = acc_m;
+    }
+}
+
+// alpha_0 = one-hot at position 0 (ForwardAttention.reset, attention.py:103-106): dst[r * ld] = 1 for every row r
+__global__ void set_first_column_kernel(float* __restrict__ dst, int ld, int rows) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r < rows) dst[(size_t)r * ld] = 1.f;
+}
+
 }  // namespace
 int launch_cell_fwd(const CellFwdArgs& a, cudaStream_t st) {
     const int Bp = (a.B + 7) & ~7;
@@ -330,6 +424,19 @@ int launch_attn_fwd(const AttnFwdArgs& a, cudaStream_t st) {
         configured = smem;
     }
     attn_fwd_kernel<<<a.B, ATT_THREADS, smem, st>>>(a);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+int launch_fwd_attn(const FwdAttnArgs& a, cudaStream_t st) {
+    const size_t smem = fwd_attn_smem_floats(a.L, a.M, a.A) * sizeof(float);
+    B200_REQUIRE(smem <= 227 * 1024, "forward attention step: shared memory %zu B exceeds 227 KB (L=%d M=%d)", smem, a.L, a.M);
+    static size_t configured = 48 * 1024;
+    if (smem > configured) {
+        B200_CUDA(cudaFuncSetAttribute(fwd_attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        configured = smem;
+    }
+    fwd_attn_fwd_kernel<<<a.B, ATT_THREADS, smem, st>>>(a);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }
@@ -361,10 +468,14 @@ int launch_fill(float* dst, float value, size_t n, cudaStream_t st) {
 
 int validate_decoder_shape(const b200tts_decoder_shape& s) {
     B200_REQUIRE(s.B > 0 && s.L > 0 && s.T > 0, "decoder: empty batch/sequence (B=%d L=%d T=%d)", s.B, s.L, s.T);
-    B200_REQUIRE(s.M > 0 && s.D > 0 && s.P > 0 && s.A > 0 && s.C > 0 && s.K > 0 && s.N > 0, "decoder: non-positive dimension");
-    B200_REQUIRE(s.K % 2 == 1, "decoder: attention kernel size must be odd (got %d)", s.K);
+    B200_REQUIRE(s.att_kind == B200TTS_ATT_LOCATION || s.att_kind == B200TTS_ATT_FORWARD, "decoder: bad attention kind %d", s.att_kind);
+    B200_REQUIRE(s.M > 0 && s.D > 0 && s.P > 0 && s.A > 0 && s.N > 0, "decoder: non-positive dimension");
     B200_REQUIRE(s.A <= 128 && s.A % 4 == 0, "decoder: attention dimension %d unsupported (need <= 128, multiple of 4)", s.A);
-    B200_REQUIRE(s.C <= 32 && s.C % 4 == 0, "decoder: location channels %d unsupported (need <= 32, multiple of 4)", s.C);
+    if (!forward_attention(s)) {        // forward attention has no location features: C and K are ignored
+        B200_REQUIRE(s.C > 0 && s.K > 0, "decoder: non-positive location dimension");
+        B200_REQUIRE(s.K % 2 == 1, "decoder: attention kernel size must be odd (got %d)", s.K);
+        B200_REQUIRE(s.C <= 32 && s.C % 4 == 0, "decoder: location channels %d unsupported (need <= 32, multiple of 4)", s.C);
+    }
     B200_REQUIRE(s.M <= 512, "decoder: memory dimension %d > 512 unsupported", s.M);
     B200_REQUIRE(s.cell_kind == B200TTS_CELL_DROPOUT || s.cell_kind == B200TTS_CELL_ZONEOUT, "decoder: bad cell kind %d", s.cell_kind);
     B200_REQUIRE(s.rate_h >= 0.f && s.rate_h < 1.f && s.rate_c >= 0.f && s.rate_c < 1.f && s.prenet_rate >= 0.f && s.prenet_rate < 1.f,
@@ -431,6 +542,18 @@ int att_step(const FwdCtx& c, int i, float* align_out) {
     ca.Wq = c.w.attn_query; ca.A = s.A; ca.qpart = c.at(l.qpart);
     ca.B = s.B; ca.D = s.D;
     B200_TRY(launch_cell_fwd(ca, c.st));
+    if (forward_attention(s)) {
+        FwdAttnArgs fa{};
+        fa.qpart = c.at(l.qpart); fa.nq = l.ncell_blocks;
+        fa.q_save = c.at(l.q) + (size_t)i * s.B * s.A;
+        fa.memT = c.at(l.memT); fa.memory = c.in.memory; fa.lengths = c.in.text_lengths;
+        fa.bias = c.w.attn_bias; fa.v = c.w.attn_energy;
+        fa.alpha_prev = c.at(l.cum) + (size_t)i * s.B * s.L; fa.alpha_next = c.at(l.cum) + (size_t)(i + 1) * s.B * s.L;
+        fa.align = align_out + (size_t)i * s.L; fa.align_bstride = (long long)s.T * s.L;
+        fa.ctx_out = ai_n; fa.ld_ctx = (int)MD;
+        fa.B = s.B; fa.L = s.L; fa.M = s.M; fa.A = s.A;
+        return launch_fwd_attn(fa, c.st);
+    }
     AttnFwdArgs aa{};
     aa.qpart = c.at(l.qpart); aa.nq = l.ncell_blocks;
     aa.q_save = c.at(l.q) + (size_t)i * s.B * s.A;
@@ -497,6 +620,10 @@ int decoder_forward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_p
                  ws_bytes, l.total * sizeof(float));
     B200_REQUIRE(in.memory && in.text_lengths && in.target, "decoder_forward: memory / text_lengths / target must be given");
     B200_REQUIRE(out.spectrogram && out.stop && out.alignments, "decoder_forward: null output");
+    if (forward_attention(s))
+        B200_REQUIRE(!w.attn_location && !w.attn_loc_features, "decoder_forward: forward attention has no location weights (pass NULL)");
+    else
+        B200_REQUIRE(w.attn_location && w.attn_loc_features, "decoder_forward: location-sensitive attention needs its location weights");
     const int B = s.B, T = s.T, D = s.D, M = s.M, P = s.P, N = s.N, MD = M + D;
     const size_t BD = (size_t)B * D;
     bool sequential = false;
@@ -535,6 +662,10 @@ int decoder_forward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_p
     B200_TRY(launch_fill(c.at(l.hg), 0.f, BD, st));
     B200_TRY(launch_fill(c.at(l.cg), 0.f, BD, st));
     B200_TRY(launch_fill(c.at(l.cum), 0.f, (size_t)B * s.L, st));
+    if (forward_attention(s)) {
+        set_first_column_kernel<<<cdiv(B, 128), 128, 0, st>>>(c.at(l.cum), s.L, B);
+        B200_LAUNCH_CHECK();
+    }
     }
 
     const bool persistent = !sequential && state == nullptr && precision_mode() == B200TTS_PRECISION_BF16 && persist_plan(s).fwd;
@@ -638,6 +769,26 @@ int attention_step_impl(int B, int L, int M, int D, int A, int C, int K, const f
     aa.B = B; aa.L = L; aa.M = M; aa.A = A; aa.C = C; aa.K = K;
     B200_TRY(launch_attn_fwd(aa, st));
     B200_TRY(launch_copy2d(cum, L, cum_next, L, B, L, st));
+    return B200TTS_OK;
+}
+
+// ---- standalone forward-attention step (module-level parity of ForwardAttention.forward) ----
+int forward_attention_step_impl(int B, int L, int M, int D, int A, const float* query, const float* memory, const float* memT,
+                                const int* lengths, const float* Wq, const float* bias, const float* v, float* alpha, float* ctx,
+                                float* weights, float* workspace, cudaStream_t st) {
+    B200_REQUIRE(B > 0 && L > 0 && D > 0 && A > 0 && A <= 128 && M > 0 && M <= 512,
+                 "forward_attention_step: unsupported dims B=%d L=%d D=%d A=%d M=%d", B, L, D, A, M);
+    // q = query . Wq^T into workspace[0 : B*A]; the new alpha into workspace[B*A : B*A + B*L], then copied back
+    float* q = workspace;
+    float* alpha_next = workspace + (size_t)B * A;
+    B200_TRY(run_gemm(st, B, A, D, query, D, Wq, D, true, q, A, nullptr, 0.f));
+    FwdAttnArgs fa{};
+    fa.qpart = q; fa.nq = 1; fa.q_save = nullptr; fa.memT = memT; fa.memory = memory; fa.lengths = lengths;
+    fa.bias = bias; fa.v = v; fa.alpha_prev = alpha; fa.alpha_next = alpha_next;
+    fa.align = weights; fa.align_bstride = L; fa.ctx_out = ctx; fa.ld_ctx = M;
+    fa.B = B; fa.L = L; fa.M = M; fa.A = A;
+    B200_TRY(launch_fwd_attn(fa, st));
+    B200_TRY(launch_copy2d(alpha, L, alpha_next, L, B, L, st));
     return B200TTS_OK;
 }
 

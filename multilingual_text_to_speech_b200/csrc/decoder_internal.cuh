@@ -54,7 +54,7 @@ struct DecoderLayout {
     size_t ca;       // [T+1, B, D]    attention LSTM cell state (row 0 = 0)
     size_t hg, cg;   // [T+1, B, D]    generator LSTM states
     size_t q;        // [T, B, A]      attention queries
-    size_t cum;      // [T+1, B, L]    cumulative attention weights BEFORE step i
+    size_t cum;      // [T+1, B, L]    cumulative attention weights BEFORE step i (forward attention: alpha BEFORE step i)
     size_t memT;     // [B, L, A]      memory . Wm^T
     size_t fs;       // [T, B, N+1]    frame | stop logits, time-major
     // derived parameters
@@ -105,6 +105,43 @@ static inline DecoderLayout decoder_layout(const b200tts_decoder_shape& s) {
 }
 
 int validate_decoder_shape(const b200tts_decoder_shape& s);
+static inline bool forward_attention(const b200tts_decoder_shape& s) { return s.att_kind == B200TTS_ATT_FORWARD; }
+
+// ---- forward attention (modules/attention.py:89-124): the part of the step its forward and backward kernels share, so that the
+// backward recomputes bit-identical transition probabilities and takes the same clamp decisions as the forward did ----
+// s[l] = softmax over ALL l < L of v . tanh(qb + memT[l])  (qb = q + bias; the reference does not mask before this softmax).
+// One CTA, blockDim.x a multiple of 32; s >= L floats, red >= 33 floats; ends with a __syncthreads.
+__device__ __forceinline__ void fwd_att_transition(const float* qb, const float* vv, const float* __restrict__ memT, int L, int A,
+                                                   float* s, float* red) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    for (int l = warp; l < L; l += nw) {
+        const float* mt = memT + (size_t)l * A;
+        float e = 0.f;
+        for (int a = lane; a < A; a += 32) e = fmaf(vv[a], tanhf(qb[a] + mt[a]), e);
+        e = warp_sum(e);
+        if (lane == 0) s[l] = e;
+    }
+    __syncthreads();
+    float mx = -INFINITY;
+    for (int l = threadIdx.x; l < L; l += blockDim.x) mx = fmaxf(mx, s[l]);
+    mx = block_max(mx, red);
+    float sum = 0.f;
+    for (int l = threadIdx.x; l < L; l += blockDim.x) {
+        const float ex = expf(s[l] - mx);
+        s[l] = ex;
+        sum += ex;
+    }
+    sum = block_sum(sum, red);
+    for (int l = threadIdx.x; l < L; l += blockDim.x) s[l] = s[l] / sum;
+    __syncthreads();
+}
+// a[l] = (alpha[l] + alpha[l-1]) * s[l] for l < len, 0 beyond (the reference's in-place mask); the weights before the clamp
+__device__ __forceinline__ float fwd_att_product(const float* __restrict__ alpha, const float* s, int l, int len) {
+    return l < len ? (alpha[l] + (l > 0 ? alpha[l - 1] : 0.f)) * s[l] : 0.f;
+}
+constexpr float FWD_ATT_FLOOR = 1e-6f;      // torch.clamp(energies, 1e-6) (attention.py:119)
+constexpr float FWD_ATT_NORM_EPS = 1e-12f;  // F.normalize(p=1) eps
+
 // wgmma / TMA persistent forward loops (decoder_persist_tc.cu): operand rows are [h | ctx | 0] in 64-column k-blocks
 struct TcPersistGeom { int Kp_att, Kp_gen, nkb_att, nkb_gen, nkb_h, ch_c_att, n_c_att, alias_att, ch_h_att, slot_att, ch_h_gen, slot_gen; };
 TcPersistGeom tc_persist_geom(const b200tts_decoder_shape& s);

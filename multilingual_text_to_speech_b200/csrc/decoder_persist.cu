@@ -85,6 +85,8 @@ __global__ void wcomb_kernel(float* __restrict__ WcombT, const float* __restrict
 // ---------------------------------------------------------------------------------------------
 PersistPlan persist_plan(const b200tts_decoder_shape& s) {
     PersistPlan p;
+    // the persistent attention loops are built around the location term; forward attention runs the per-step chains
+    if (forward_attention(s)) return p;
     // a training forward runs persistent only together with the persistent attention reverse loop: the forward loops round
     // memory / memT to bf16, and only that reverse loop recomputes the attention with the same operands
     const bool att_bwd = persist_att_bwd_supported(s);
@@ -102,7 +104,7 @@ PersistLayout persist_layout(const b200tts_decoder_shape& s) {
     const TcPersistGeom g = tc_persist_geom(s);
     l.aib = take((T + 1) * B * (size_t)g.Kp_att * 2);
     l.hgb = take((T + 1) * B * (size_t)g.Kp_gen * 2);
-    l.wcombT = take((size_t)s.K * s.A * 4);
+    l.wcombT = take(forward_attention(s) ? 0 : (size_t)s.K * s.A * 4);     // K is ignored for forward attention
     l.wcb = take((size_t)s.A * 40 * 2);
     l.MT = (s.L + 15) / 16;
     l.memTf = take((size_t)s.B * l.MT * 32 * 64 * 2);

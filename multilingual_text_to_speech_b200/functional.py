@@ -157,6 +157,54 @@ class AttentionStepFunction(torch.autograd.Function):
         return d_query, d_memory, d_memT, d_cum, None, d_wq, d_wloc, d_wc, d_bias, d_v
 
 
+class ForwardAttentionStepFunction(torch.autograd.Function):
+    """One ForwardAttention step WITH autograd (reference modules/attention.py:23-45, 89-124): returns (context, weights); the weights
+    are also the next alpha.  Forward and backward are the library's single-step forward-attention ops."""
+
+    @staticmethod
+    def forward(ctx, query, memory, memT, alpha_prev, text_lengths, w_query, bias, w_energy):
+        _require_cuda(query, memory, memT, alpha_prev)
+        query, memory, memT, alpha_prev = _f32c(query), _f32c(memory), _f32c(memT), _f32c(alpha_prev)
+        w_query, bias, w_energy = _f32c(w_query), _f32c(bias), _f32c(w_energy)
+        lengths = text_lengths.to(torch.int32).contiguous()
+        B, L, M = memory.shape
+        D, A = query.shape[1], w_query.shape[0]
+        lib = _lib.load()
+        ws = torch.empty(lib.b200tts_forward_attention_step_workspace_elems(B, L, A), device=query.device, dtype=torch.float32)
+        context = torch.empty(B, M, device=query.device, dtype=torch.float32)
+        weights = torch.empty(B, L, device=query.device, dtype=torch.float32)
+        alpha = alpha_prev.clone()
+        check(lib.b200tts_forward_attention_step(B, L, M, D, A, ptr(query), ptr(memory), ptr(memT), ptr(lengths), ptr(w_query), ptr(bias),
+                                                 ptr(w_energy), ptr(alpha), ptr(context), ptr(weights), ptr(ws), _stream()),
+              'b200tts_forward_attention_step')
+        q = ws[:B * A].view(B, A).clone()              # the forward left q = query . Wq^T at the head of its workspace
+        ctx.dims = (B, L, M, D, A)
+        ctx.save_for_backward(query, memory, memT, alpha_prev, lengths, q, weights, w_query, bias, w_energy)
+        return context, weights
+
+    @staticmethod
+    def backward(ctx, d_context, d_weights):
+        query, memory, memT, alpha_prev, lengths, q, weights, w_query, bias, w_energy = ctx.saved_tensors
+        B, L, M, D, A = ctx.dims
+        dev = query.device
+        z = lambda *shape: torch.zeros(*shape, device=dev, dtype=torch.float32)   # noqa: E731
+        d_context = _f32c(d_context) if d_context is not None else z(B, M)
+        d_weights = _f32c(d_weights) if d_weights is not None else None
+        d_alpha = z(B, L)           # in: no gradient beyond the weights themselves; out: gradient of alpha_prev
+        d_q, d_memT, d_v = z(B, A), z(B, L, A), torch.zeros_like(w_energy)
+        lib = _lib.load()
+        ws = torch.empty(lib.b200tts_forward_attention_step_backward_workspace_elems(B, M, A), device=dev, dtype=torch.float32)
+        check(lib.b200tts_forward_attention_step_backward(B, L, M, A, ptr(q), ptr(memory), ptr(memT), ptr(lengths), ptr(bias), ptr(w_energy),
+                                                          ptr(alpha_prev), ptr(weights), ptr(d_context), ptr(d_weights), ptr(d_alpha),
+                                                          ptr(d_q), ptr(d_memT), ptr(d_v), ptr(ws), _stream()),
+              'b200tts_forward_attention_step_backward')
+        d_query = gemm(d_q, w_query, False, False)                       # [B, A] . [A, D]
+        d_wq = gemm(d_q, query, True, False)                             # [A, B] . [B, D]
+        d_bias = d_q.sum(0, keepdim=True).view_as(bias)
+        d_memory = weights.unsqueeze(2) * d_context.unsqueeze(1)         # context = weights . memory
+        return d_query, d_memory, d_memT, d_alpha, None, d_wq, d_bias, d_v
+
+
 # ------------------------------------------------------------------------------------------------
 # fused decoder
 # ------------------------------------------------------------------------------------------------
@@ -173,10 +221,18 @@ class DecoderConfig:
         self.teacher = teacher               # None (all teacher forced) or host bool/uint8 array [T]
 
 
+def _attention_dims(byname):
+    """(att_kind, C, K): forward attention is the parameter set without location weights (both None)."""
+    if byname['attn_location'] is None and byname['attn_loc_features'] is None:
+        return _lib.ATT_FORWARD, 0, 0
+    return _lib.ATT_LOCATION, byname['attn_loc_features'].shape[0], byname['attn_loc_features'].shape[-1]
+
+
 def _decoder_structs(cfg, shape_dims, params, memory, text_lengths, target):
     B, L, T, M, D, P, A, C, K, N = shape_dims
+    att_kind = _attention_dims(dict(zip(DECODER_PARAM_FIELDS, params)))[0]
     shape = DecoderShape(B, L, T, M, D, P, A, C, K, N, cfg.cell_kind, int(cfg.training), cfg.rate_h, cfg.rate_c,
-                         cfg.prenet_rate)
+                         cfg.prenet_rate, att_kind)
     pstruct = DecoderParams(*[ptr(p) for p in params])
     teacher_np = None
     if cfg.teacher is not None:
@@ -206,7 +262,7 @@ class DecoderFunction(torch.autograd.Function):
         assert len(params) == len(DECODER_PARAM_FIELDS)
         _require_cuda(memory, target, text_lengths, *params)
         memory, target = _f32c(memory), _f32c(target)
-        params = [_f32c(p) for p in params]
+        params = [None if p is None else _f32c(p) for p in params]
         text_lengths = text_lengths.to(torch.int32).contiguous()
         byname = dict(zip(DECODER_PARAM_FIELDS, params))
         B, L, M = memory.shape
@@ -214,7 +270,7 @@ class DecoderFunction(torch.autograd.Function):
         D = byname['att_w_hh'].shape[1]
         P = byname['prenet_w1'].shape[0]
         A = byname['attn_query'].shape[0]
-        C, K = byname['attn_loc_features'].shape[0], byname['attn_loc_features'].shape[-1]
+        _, C, K = _attention_dims(byname)
         assert byname['att_w_ih'].shape == (4 * D, P + M) and byname['gen_w_ih'].shape == (4 * D, D + M)
         dims = (B, L, T, M, D, P, A, C, K, N)
         shape, pstruct, inputs, teacher_np = _decoder_structs(cfg, dims, params, memory, text_lengths, target)
@@ -278,12 +334,12 @@ def decoder_forward_chunk(cfg, memory, text_lengths, params, state, frames):
     _require_cuda(memory, text_lengths, *params)
     with torch.no_grad():
         memory = _f32c(memory)
-        params = [_f32c(p) for p in params]
+        params = [None if p is None else _f32c(p) for p in params]
         text_lengths = text_lengths.to(torch.int32).contiguous()
         byname = dict(zip(DECODER_PARAM_FIELDS, params))
         B, L, M = memory.shape
         D, P, A = byname['att_w_hh'].shape[1], byname['prenet_w1'].shape[0], byname['attn_query'].shape[0]
-        C, K = byname['attn_loc_features'].shape[0], byname['attn_loc_features'].shape[-1]
+        _, C, K = _attention_dims(byname)
         N = byname['frame_w'].shape[0]
         T = int(frames)
         target = torch.zeros(B, N, T, device=memory.device, dtype=torch.float32)
@@ -309,7 +365,8 @@ MAX_PERSIST_BATCH = 64
 
 
 def decoder_forward(cfg, memory, target, text_lengths, params):
-    """params: list of the 22 decoder parameter tensors in DECODER_PARAM_FIELDS order.
+    """params: list of the 22 decoder parameter tensors in DECODER_PARAM_FIELDS order; forward attention (ForwardAttention) passes None
+    for the two location weights (attn_location, attn_loc_features), which selects B200TTS_ATT_FORWARD.
 
     Utterances are independent inside the decoder (only the weights are shared), so a batch larger than the persistent kernels' tile
     (B > 64: BASELINE configs[3..4] run 65 / 80 per GPU) is decoded as ceil(B / 64) equal slices through the same fused op instead of

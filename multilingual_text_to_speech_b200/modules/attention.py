@@ -1,8 +1,9 @@
-"""Attention modules (surface of reference modules/attention.py:6-86).
+"""Attention modules (surface of reference modules/attention.py:6-124).
 
-Only LocationSensitiveAttention is on the hot path (the forward-attention variants of the reference are
-documented as undebugged and cannot run, SURVEY.md section 2).  Inside training the attention runs fused in the
-decoder op; the module-level `reset` / `forward` API is kept and calls the library's single-step op.
+LocationSensitiveAttention (the default, hp.attention_type "location_sensitive") and ForwardAttention ("forward") are provided.
+Inside training both run fused in the decoder op; the module-level `reset` / `forward` API is kept and calls the library's
+single-step ops.  ForwardAttentionWithTransition ("forward_transition_agent") is not: the reference cannot run it (its `reset`
+takes three arguments, the decoder passes four), so there is no behaviour to match.
 """
 import torch
 from torch.nn import Linear, Parameter, Conv1d
@@ -45,5 +46,30 @@ class LocationSensitiveAttention(AttentionBase):
         ctx, w, cum = F.AttentionStepFunction.apply(query, memory, self._memory_transform, self._prev_weights, lengths, self._query.weight,
                                                     self._location.weight, self._loc_features.weight, self._bias, self._energy.weight)
         self._prev_weights = cum
+        self._prev_context = ctx
+        return ctx, w
+
+
+class ForwardAttention(AttentionBase):
+    """Forward attention without the transition agent (attention.py:89-124, https://arxiv.org/abs/1807.06736).
+
+    Per step: s = softmax(v . tanh(W_q h + memT + b)) over every position (padding included, as in the reference);
+    a = (alpha + alpha shifted right by one) * s; a = 0 beyond the text length; w = clamp(a, 1e-6) normalised to sum 1.
+    w is the alignment and the next alpha; the context is w . memory over every position.  So unlike the location-sensitive
+    attention, the alignments are not exactly zero beyond the text length (they are about 1e-6 / sum there)."""
+
+    def reset(self, encoded_input, batch_size, max_len, device):
+        """AttentionBase.reset, then alpha[:, 0] = 1 (attention.py:103-106)."""
+        super().reset(encoded_input, batch_size, max_len, device)
+        self._prev_weights[:, 0] = 1
+        return self._prev_context
+
+    def forward(self, query, memory, mask, prev_decoder_output):
+        """(context, weights) for one decoder step; `prev_decoder_output` is unused, as in the reference.  The new alpha (= weights)
+        replaces `_prev_weights` with autograd history through the library's single-step backward."""
+        lengths = mask.sum(dim=1).to(torch.int32)
+        ctx, w = F.ForwardAttentionStepFunction.apply(query, memory, self._memory_transform, self._prev_weights, lengths,
+                                                      self._query.weight, self._bias, self._energy.weight)
+        self._prev_weights = w
         self._prev_context = ctx
         return ctx, w

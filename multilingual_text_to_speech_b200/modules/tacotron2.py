@@ -16,7 +16,7 @@ from ..rng import MaskSource
 from ..params.params import Params as hp
 from ..utils import lengths_to_mask
 from .layers import ZoneoutLSTMCell, DropoutLSTMCell, ConvBlock
-from .attention import LocationSensitiveAttention
+from .attention import LocationSensitiveAttention, ForwardAttention
 from .encoder import Encoder, MultiEncoder, ConditionalEncoder, ConvolutionalEncoder, GeneratedConvolutionalEncoder
 from .classifier import ReversalClassifier
 
@@ -61,7 +61,7 @@ class Postnet(torch.nn.Module):
 
 
 class Decoder(torch.nn.Module):
-    """Attention LSTM -> location-sensitive attention -> generator LSTM -> frame / stop projections
+    """Attention LSTM -> location-sensitive or forward attention -> generator LSTM -> frame / stop projections
     (tacotron2.py:79-219), executed by b200tts_decoder_forward / _backward."""
 
     def __init__(self, output_dim, decoder_dim, attention, generator_rnn, attention_rnn, context_dim, prenet, prenet_dim, max_frames):
@@ -93,10 +93,13 @@ class Decoder(torch.nn.Module):
         pre, att = self._prenet._layers, self._attention
         assert len(pre) == 2, 'the fused decoder implements the 2-layer prenet used by every configuration'
         a, g = self._attention_lstm, self._generator_lstm
+        # forward attention has no location weights: None selects it in the fused op
+        loc, loc_features = getattr(att, '_location', None), getattr(att, '_loc_features', None)
         return [pre[0].weight, pre[0].bias, pre[1].weight, pre[1].bias,
                 a.weight_ih, a.weight_hh, a.bias_ih, a.bias_hh, g.weight_ih, g.weight_hh, g.bias_ih, g.bias_hh,
-                att._query.weight, att._memory.weight, att._location.weight, att._loc_features.weight, att._bias,
-                att._energy.weight, self._frame_prediction.weight, self._frame_prediction.bias,
+                att._query.weight, att._memory.weight, loc.weight if loc is not None else None,
+                loc_features.weight if loc_features is not None else None,
+                att._bias, att._energy.weight, self._frame_prediction.weight, self._frame_prediction.bias,
                 self._stop_prediction.weight, self._stop_prediction.bias]
 
     def _cell_config(self):
@@ -310,7 +313,13 @@ class Tacotron(torch.nn.Module):
         if name == 'location_sensitive':
             return LocationSensitiveAttention(hp.attention_kernel_size, hp.attention_location_dimension, False,
                                               hp.attention_dimension, hp.decoder_dimension, memory_dimension)
-        raise NotImplementedError(f'attention type {name} is out of scope (undebugged in the reference)')
+        if name == 'forward':
+            return ForwardAttention(hp.attention_dimension, hp.decoder_dimension, memory_dimension)
+        if name == 'forward_transition_agent':
+            raise NotImplementedError('attention type forward_transition_agent is not provided: the reference cannot run it '
+                                      '(ForwardAttentionWithTransition.reset takes 3 arguments but the decoder passes 4), '
+                                      'so there is no reference behaviour to match')
+        raise NotImplementedError(f'attention type {name} is out of scope')
 
     def _get_postnet(self, name):
         if name == 'conv':
