@@ -2,6 +2,7 @@
 """Minimal training loop on synthetic data: what `train.py:49-95, 255-272` of the reference looks like on this framework.
 
     python examples/train_synthetic.py --steps 20                                   # one GPU
+    python examples/train_synthetic.py --steps 20 --tf-start 5 --tf-steps 20        # teacher forcing decays from 1.0 after step 5
     torchrun --nproc-per-node 8 --master-addr 127.0.0.1 examples/train_synthetic.py  # data parallel, one rank per GPU
 
 Pieces (all from this repository): `Tacotron` / `TacotronLoss` with the reference's surface, `BucketedPerfectBatchSampler` + `shard`
@@ -9,6 +10,7 @@ for language-balanced, length-bucketed batches, `GradBucket` (flat gradient, one
 (global-norm clip + Adam + StepLR in one library call).  Needs an H100: there is no CPU path.
 """
 import argparse
+import math
 import os
 import random
 import sys
@@ -17,6 +19,19 @@ import torch
 import torch.distributed as dist
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+
+def cos_decay(global_step, decay_steps):
+    """The reference's teacher-forcing schedule (train.py:18-26): 1.0 at step 0, cosine down to 0.0 at `decay_steps`."""
+    global_step = min(global_step, decay_steps)
+    return 0.5 * (1 + math.cos(math.pi * global_step / decay_steps))
+
+
+def teacher_forcing_ratio(hp, global_step):
+    """train.py:58-60: the constant hp.teacher_forcing, or the cosine decay that starts at hp.teacher_forcing_start_steps."""
+    if hp.constant_teacher_forcing:
+        return hp.teacher_forcing
+    return cos_decay(max(global_step - hp.teacher_forcing_start_steps, 0), hp.teacher_forcing_steps)
 
 
 class SyntheticCorpus:
@@ -50,6 +65,9 @@ def main():
     ap.add_argument('--config', default='generated_training')
     ap.add_argument('--steps', type=int, default=20)
     ap.add_argument('--batch', type=int, default=60, help='per-GPU batch (a multiple of the number of languages)')
+    ap.add_argument('--tf-start', type=int, default=None,
+                    help='decay teacher forcing from this step on (hp.teacher_forcing_start_steps; default: the config\'s schedule)')
+    ap.add_argument('--tf-steps', type=int, default=None, help='length of the decay (hp.teacher_forcing_steps)')
     a = ap.parse_args()
     from multilingual_text_to_speech_b200 import configs, _lib
     from multilingual_text_to_speech_b200.modules.tacotron2 import Tacotron, TacotronLoss
@@ -64,7 +82,14 @@ def main():
     if world > 1:
         os.environ.setdefault('MASTER_ADDR', '127.0.0.1')
         dist.init_process_group('nccl', device_id=dev)
-    hp = configs.apply(a.config, decoder_regularization='zoneout')
+    schedule = {}
+    if a.tf_start is not None or a.tf_steps is not None:
+        schedule['constant_teacher_forcing'] = False
+        if a.tf_start is not None:
+            schedule['teacher_forcing_start_steps'] = a.tf_start
+        if a.tf_steps is not None:
+            schedule['teacher_forcing_steps'] = a.tf_steps
+    hp = configs.apply(a.config, decoder_regularization='zoneout', **schedule)
     _lib.set_precision('bf16')
     torch.manual_seed(0)
     model = Tacotron().to(dev).train()
@@ -85,8 +110,9 @@ def main():
                 continue
             b = corpus.collate(shard(global_batch, rank, world, G), dev)
             bucket.zero()
+            tf = teacher_forcing_ratio(hp, step)
             post, pre, stop, align, spk, enc = model(b['text'], b['text_length'], b['target'], b['target_length'], None, b['languages'],
-                                                     hp.teacher_forcing)
+                                                     tf)
             loss, parts = crit(b['text_length'], b['target_length'], pre, b['target'], post, b['target'], stop, b['stop_target'], align,
                                None, spk, enc, None)
             loss.backward()
@@ -95,7 +121,7 @@ def main():
             crit.update_states()
             step += 1
             if rank == 0 and step % 5 == 0:
-                print(f'step {step}: loss {float(loss):.4f}  grad norm {float(info[0]):.3f}  clip x{float(info[1]):.3f}  lr {opt.current_lr():.2e}',
+                print(f'step {step}: tf {tf:.3f}  loss {float(loss):.4f}  grad norm {float(info[0]):.3f}  clip x{float(info[1]):.3f}  lr {opt.current_lr():.2e}',
                       flush=True)
             if step >= a.steps:
                 if world > 1:

@@ -119,7 +119,9 @@ typedef struct {
     const float* memory;          /* [B, L, M] encoder output ++ speaker/language embeddings */
     const int32_t* text_lengths;  /* [B] */
     const float* target;          /* [B, N, T] ground-truth mel frames */
-    const uint8_t* teacher;       /* [host] [T] 1 = ground truth fed at step i (tacotron2.py:171,181); NULL = all 1 */
+    const uint8_t* teacher;       /* [host] [T] 1 = ground truth fed at step i (tacotron2.py:171,181); NULL = all 1.  0 = free-running:
+                                     step i is fed the frame predicted at step i-1 (zeros at step 0), and the backward
+                                     differentiates through that frame (no detach, as in the reference) */
     /* keep masks, NULL = no dropout at that site.  Time-major: row i belongs to decoder step i. */
     const uint8_t* mask_prenet0;  /* [T, B, P] */
     const uint8_t* mask_prenet1;  /* [T, B, P] */
@@ -140,7 +142,8 @@ typedef struct {
 /* Bytes of the forward workspace; it also carries everything the backward pass re-reads. */
 size_t b200tts_decoder_workspace_bytes(const b200tts_decoder_shape* shape);
 size_t b200tts_decoder_bwd_workspace_bytes(const b200tts_decoder_shape* shape);
-/* Which kernels a bf16-mode training step of this shape runs on (pure host arithmetic, no device needed): bit 0 = persistent
+/* Which kernels a bf16-mode training step with every decoder step teacher-forced runs on for this shape (pure host arithmetic, no
+ * device needed; a decode with a free-running step runs the per-step kernel chains, forward and backward): bit 0 = persistent
  * forward loops, bit 1 = their TMA + wgmma variant, bit 2 = persistent generator reverse loop, bit 3 = its wgmma
  * variant, bit 4 = persistent attention reverse loop, bit 5 = its wgmma product.  0 = the per-step kernel chains.
  * Every persistent loop is a TMA + wgmma kernel, so each variant bit (1, 3, 5) is set exactly when its loop bit (0, 2, 4)
@@ -179,7 +182,8 @@ typedef struct {
     const float* d_alignments;  /* [B, T, L] or NULL */
 } b200tts_decoder_output_grads;
 
-/* Backward of the teacher-forced decode (autograd replay of tacotron2.py:148-209, train.py:83).
+/* Backward of the decode (autograd replay of tacotron2.py:148-209, train.py:83), free-running steps included: their gradient
+ * flows back through the fed-back frame into the previous step's frame projection, generator LSTM and attention.
  * `fwd_workspace` is the buffer the matching forward call filled and `fwd_out` its outputs (the
  * alignments are re-read).  Parameter gradients are ACCUMULATED into `d_params` (+=, like autograd
  * .grad); `d_memory` [B, L, M] is overwritten (may be NULL). */

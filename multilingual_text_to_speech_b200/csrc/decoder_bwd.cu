@@ -1,7 +1,9 @@
-// Decoder backward (BPTT) for the teacher-forced decode: the reverse of decoder_fwd.cu.
+// Decoder backward (BPTT): the reverse of decoder_fwd.cu.
 // Restates what torch autograd replays for Decoder._decode (reference modules/tacotron2.py:148-209,
 // train.py:83): frame/stop projection grads -> generator LSTM reverse loop -> attention LSTM +
 // location-sensitive attention reverse loop (energies recomputed, never stored) -> time-batched dW GEMMs.
+// A decode with free-running steps (teacher forcing < 1) runs the two reverse loops as a segmented sweep
+// instead, because each such step sends gradient back through the frame it was fed.
 #include <cuda_bf16.h>
 #include "decoder_internal.cuh"
 
@@ -98,6 +100,64 @@ __global__ void relu_dropout_bwd_kernel(float* __restrict__ dz, const float* __r
                                         float scale, size_t n) {
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
         dz[i] = y[i] > 0.f ? dy[i] * scale : 0.f;
+}
+
+// Feedback of a free-running step f >= 1 into the frame it was fed, x_f = FS[f-1, :, 0:N] (tacotron2.py:171,181; not detached),
+// one CTA per utterance.  dp1 = d p1_f (the product dga_f . W_ih_att[:, :P], taken by the GEMM before this kernel):
+//   dz1 = dp1 * scale1 * (p1 > 0);  dp0 = dz1 . W1;  dz0 = dp0 * scale0 * (p0 > 0);  dx = dz0 . W0
+//   dFS[f-1, b, 0:N] += dx;  [d h_gen | d ctx]_{f-1} += dx . Wfs[0:N, :]   (direct / static parts, consumed by the reverse steps f-1)
+// Every sum runs in a fixed order (no atomics).
+struct FeedbackArgs {
+    const float* dp1;                  // [B, P]
+    const float* p0; const float* p1;  // [B, P] step f's prenet activations (after relu + dropout)
+    const float* W0; const float* W1;  // prenet_w0 [P, N], prenet_w1 [P, P]
+    const float* wfs;                  // [N+1, D+M]
+    float* dfs;                        // [B, N+1] row f-1
+    float* dhgd;                       // [B, D]   row f-1
+    float* dctxs;                      // [B, M]   row f-1
+    float scale0, scale1;
+    int B, P, N, D, M;
+};
+constexpr int FEEDBACK_THREADS = 256;
+__host__ __device__ inline int feedback_slices(int N) { const int s = FEEDBACK_THREADS / N; return s < 1 ? 1 : s; }
+inline size_t feedback_smem_floats(int P, int N) { return (size_t)2 * P + (size_t)(feedback_slices(N) + 1) * N; }
+
+__global__ void __launch_bounds__(FEEDBACK_THREADS) frame_feedback_bwd_kernel(const FeedbackArgs p) {
+    extern __shared__ __align__(16) float sm[];
+    const int b = blockIdx.x, tid = threadIdx.x, P = p.P, N = p.N, DM = p.D + p.M;
+    const int ns = feedback_slices(N), per = (P + ns - 1) / ns;
+    float* dz1 = sm; float* dz0 = dz1 + P; float* xpart = dz0 + P; float* dx = xpart + (size_t)ns * N;
+    const size_t row = (size_t)b * P;
+    for (int j = tid; j < P; j += FEEDBACK_THREADS) dz1[j] = p.p1[row + j] > 0.f ? p.dp1[row + j] * p.scale1 : 0.f;
+    __syncthreads();
+    // dp0[j] = sum_k dz1[k] W1[k, j]  (W1 rows are the layer's outputs)
+    for (int j = tid; j < P; j += FEEDBACK_THREADS) {
+        float acc = 0.f;
+        for (int k = 0; k < P; ++k) acc = fmaf(dz1[k], p.W1[(size_t)k * P + j], acc);
+        dz0[j] = p.p0[row + j] > 0.f ? acc * p.scale0 : 0.f;
+    }
+    __syncthreads();
+    // dx[n] = sum_j dz0[j] W0[j, n]: `ns` slices of j per column, then the slices in order
+    for (int t = tid; t < ns * N; t += FEEDBACK_THREADS) {
+        const int n = t % N, sl = t / N, j1 = min(P, (sl + 1) * per);
+        float acc = 0.f;
+        for (int j = sl * per; j < j1; ++j) acc = fmaf(dz0[j], p.W0[(size_t)j * N + n], acc);
+        xpart[(size_t)sl * N + n] = acc;
+    }
+    __syncthreads();
+    for (int n = tid; n < N; n += FEEDBACK_THREADS) {
+        float acc = 0.f;
+        for (int sl = 0; sl < ns; ++sl) acc += xpart[(size_t)sl * N + n];
+        dx[n] = acc;
+        p.dfs[(size_t)b * (N + 1) + n] += acc;
+    }
+    __syncthreads();
+    for (int c = tid; c < DM; c += FEEDBACK_THREADS) {
+        float acc = 0.f;
+        for (int n = 0; n < N; ++n) acc = fmaf(dx[n], p.wfs[(size_t)n * DM + c], acc);
+        if (c < p.D) p.dhgd[(size_t)b * p.D + c] += acc;
+        else p.dctxs[(size_t)b * p.M + c - p.D] += acc;
+    }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -681,7 +741,9 @@ int launch_fwd_attn_bwd(const FwdAttnBwdArgs& a, cudaStream_t st) {
 // ---------------------------------------------------------------------------------------------
 struct BwdLayout {
     size_t dfs, dhgd, dctxs, dgg, dhas, dga, dq, dctxt, dcum, dc, dhz, dmemT, dWloc_acc, dWc_acc, dv_acc, dp1, dp0, dwfs,
-        part, gpart, pextra, pextra2, dggb, dgab, total;      // dggb / dgab: bf16 [T, B, 4D] histories of the gate gradients (wgmma loops)
+        part, gpart, pextra, pextra2, dggb, dgab,     // dggb / dgab: bf16 [T, B, 4D] histories of the gate gradients (wgmma loops)
+        part_gen, dc_gen, dhz_gen,      // generator-recurrence state of the segmented sweep (inside the dgab region)
+        total;
     int split_gen, split_att;
     size_t gpart_elems;
 };
@@ -720,7 +782,15 @@ BwdLayout bwd_layout(const b200tts_decoder_shape& s) {
     l.pextra = take(persist_bwd_gen_extra_bytes(s) / sizeof(float) + 64);
     l.pextra2 = take(att_bwd_extra(s).total / sizeof(float) + 64);
     l.dggb = take(T * B * 4 * D / 2 + 64);
-    l.dgab = take(T * B * 4 * D / 2 + 64);
+    // The segmented sweep (decodes with free-running steps) runs both recurrences in turn with state carried across segments: the
+    // attention recurrence keeps part / dc / dhz, the generator gets its own.  That sweep never runs the persistent attention reverse
+    // loop, the only writer of dgab, so its generator state lives in the dgab region (grown only where T < 5 leaves it too small).
+    const size_t seg_gen = align_up(pg, 64) + 2 * align_up(B * D, 64);
+    const size_t ngab = T * B * 4 * D / 2 + 64;
+    l.dgab = take(ngab > seg_gen ? ngab : seg_gen);
+    l.part_gen = l.dgab;
+    l.dc_gen = l.part_gen + align_up(pg, 64);
+    l.dhz_gen = l.dc_gen + align_up(B * D, 64);
     l.total = off;
     return l;
 }
@@ -755,6 +825,214 @@ int xgemm16(cudaStream_t st, const BwdLayout& l, float* ws, int M, int N, int K,
     d.A = A; d.B = B; d.C = C; d.M = M; d.N = N; d.K = K; d.lda = lda; d.ldb = ldb; d.ldc = ldc; d.transA = 0; d.transB = 0; d.beta = beta;
     d.A16 = A16; d.lda16 = lda16;
     return gemm_run_auto(d, ws + l.gpart, l.gpart_elems, st);
+}
+
+// ---------------------------------------------------------------------------------------------
+// pieces of one decoder backward call, shared by the teacher-forced path and the segmented sweep
+// ---------------------------------------------------------------------------------------------
+struct BwdCtx {
+    const b200tts_decoder_shape& s;
+    const b200tts_decoder_params& w;
+    const b200tts_decoder_inputs& in;
+    const b200tts_decoder_outputs& fwd_out;
+    const b200tts_decoder_output_grads& dout;
+    const DecoderLayout& fl;
+    const BwdLayout& l;
+    const float* fws;
+    float* bws;
+    cudaStream_t st;
+    const float* F(size_t off) const { return fws + off; }
+    float* W(size_t off) const { return bws + off; }
+    bool free_running(int i) const { return in.teacher && !in.teacher[i]; }
+};
+
+// d [frame_w ; stop_w] = dFS^T . [h_gen | ctx];  d frame_b, d stop_b = column sums of dFS
+int frame_weight_grads(const BwdCtx& c, const b200tts_decoder_params& dw, const __nv_bfloat16* hgb1, int ldhb,
+                       const __nv_bfloat16* aib1, int ldab) {
+    const auto& s = c.s; const auto& l = c.l;
+    const int D = s.D, M = s.M, N = s.N, N1 = N + 1, MD = M + D;
+    const size_t TB = (size_t)s.T * s.B;
+    const float* ai1 = c.F(c.fl.ai) + (size_t)s.B * MD;
+    B200_TRY(wgemm16(c.st, l, c.bws, N1, D, (int)TB, c.W(l.dfs), N1, c.F(c.fl.hg) + (size_t)s.B * D, D, hgb1, ldhb, c.W(l.dwfs), D + M, 0.f));
+    B200_TRY(wgemm16(c.st, l, c.bws, N1, M, (int)TB, c.W(l.dfs), N1, ai1, MD, aib1 ? aib1 + D : nullptr, ldab, c.W(l.dwfs) + D, D + M, 0.f));
+    add2d_kernel<<<grid_for((size_t)N * (D + M)), 256, 0, c.st>>>(dw.frame_w, D + M, c.W(l.dwfs), D + M, N, D + M);
+    B200_LAUNCH_CHECK();
+    add2d_kernel<<<grid_for((size_t)(D + M)), 256, 0, c.st>>>(dw.stop_w, D + M, c.W(l.dwfs) + (size_t)N * (D + M), D + M, 1, D + M);
+    B200_LAUNCH_CHECK();
+    B200_TRY(colsum_add(dw.frame_b, nullptr, c.W(l.dfs), TB, N, N1, c.W(l.gpart), c.st));
+    B200_TRY(colsum_add(dw.stop_b, nullptr, c.W(l.dfs) + N, TB, 1, N1, c.W(l.gpart), c.st));
+    return B200TTS_OK;
+}
+
+// generator-LSTM reverse step i on the per-step chain: cell backward (carried d c / zoneout d h in dc / dhz), then the recurrent
+// d h_gen_{i-1} = dgates_i . W_hh as split-K partials into `part`, which step i-1 consumes
+int gen_bwd_step(const BwdCtx& c, int i, float* part, float* dc, float* dhz) {
+    const auto& s = c.s; const auto& l = c.l;
+    const int B = s.B, D = s.D;
+    const size_t BD = (size_t)B * D, B4D = 4 * BD;
+    CellBwdArgs ca{};
+    ca.gates = c.F(c.fl.gg) + (size_t)i * B4D;
+    ca.c_prev = c.F(c.fl.cg) + (size_t)i * BD;
+    ca.dh_static = c.W(l.dhgd) + (size_t)i * BD; ca.ld_dhs = D;
+    ca.part = part; ca.nsplit = l.split_gen; ca.part_stride = BD; ca.ld_part = D; ca.part_col0 = 0;
+    ca.dq = nullptr; ca.Wq = nullptr; ca.A = 0;
+    ca.dc_state = dc; ca.dhz_state = s.cell_kind == B200TTS_CELL_ZONEOUT ? dhz : nullptr;
+    ca.mask_h = c.in.mask_gen_h ? c.in.mask_gen_h + (size_t)i * BD : nullptr;
+    ca.mask_c = c.in.mask_gen_c ? c.in.mask_gen_c + (size_t)i * BD : nullptr;
+    ca.kind = s.cell_kind; ca.training = s.training; ca.rate_h = s.rate_h; ca.rate_c = s.rate_c;
+    ca.dgates = c.W(l.dgg) + (size_t)i * B4D; ca.B = B; ca.D = D; ca.last = (i == s.T - 1);
+    B200_TRY(launch_cell_bwd(ca, c.st));
+    if (i > 0) {
+        GemmDesc d;      // d h_gen_{i-1} (recurrent) = dgates_i . W_hh
+        d.A = ca.dgates; d.lda = 4 * D; d.B = c.w.gen_w_hh; d.ldb = D; d.transB = 0; d.M = B; d.N = D; d.K = 4 * D;
+        d.splitk = l.split_gen; d.partial = part; d.keep_partials = 1;
+        if (d.splitk == 1) { d.C = part; d.ldc = D; d.keep_partials = 0; d.partial = nullptr; }
+        B200_TRY(gemm_run(d, c.st));
+    }
+    return B200TTS_OK;
+}
+
+// time-batched generator-LSTM weight gradients from the final gate gradients (dggb: their bf16 history, or null)
+int gen_weight_grads(const BwdCtx& c, const b200tts_decoder_params& dw, const __nv_bfloat16* hgb, int ldhb, const __nv_bfloat16* aib1,
+                     int ldab, const void* dggb) {
+    const auto& s = c.s; const auto& l = c.l;
+    const int D = s.D, M = s.M, MD = M + D;
+    const size_t TB = (size_t)s.T * s.B;
+    const float* ai1 = c.F(c.fl.ai) + (size_t)s.B * MD;
+    B200_TRY(wgemm16(c.st, l, c.bws, 4 * D, D, (int)TB, c.W(l.dgg), 4 * D, c.F(c.fl.hg), D, hgb, ldhb, dw.gen_w_hh, D, 1.f, dggb, 4 * D));
+    B200_TRY(wgemm16(c.st, l, c.bws, 4 * D, D, (int)TB, c.W(l.dgg), 4 * D, ai1 + M, MD, aib1, ldab, dw.gen_w_ih, D + M, 1.f, dggb, 4 * D));
+    B200_TRY(wgemm16(c.st, l, c.bws, 4 * D, M, (int)TB, c.W(l.dgg), 4 * D, ai1, MD, aib1 ? aib1 + D : nullptr, ldab, dw.gen_w_ih + D, D + M, 1.f,
+                     dggb, 4 * D));
+    B200_TRY(colsum_add(dw.gen_b_ih, dw.gen_b_hh, c.W(l.dgg), TB, 4 * D, 4 * D, c.W(l.gpart), c.st));
+    return B200TTS_OK;
+}
+
+// d h_att (static part) and d ctx (generator-input part, accumulated onto what is there) of steps [i0, i1)
+int gen_input_grads(const BwdCtx& c, int i0, int i1, const void* dggb) {
+    const auto& s = c.s; const auto& l = c.l;
+    const int B = s.B, D = s.D, M = s.M;
+    const int rows = (i1 - i0) * B;
+    const float* dgg = c.W(l.dgg) + (size_t)i0 * B * 4 * D;
+    const void* dgg16 = dggb ? static_cast<const void*>(static_cast<const __nv_bfloat16*>(dggb) + (size_t)i0 * B * 4 * D) : nullptr;
+    B200_TRY(xgemm16(c.st, l, c.bws, rows, D, 4 * D, dgg, 4 * D, dgg16, 4 * D, c.w.gen_w_ih, D + M, c.W(l.dhas) + (size_t)i0 * B * D, D, 0.f));
+    B200_TRY(xgemm16(c.st, l, c.bws, rows, M, 4 * D, dgg, 4 * D, dgg16, 4 * D, c.w.gen_w_ih + D, D + M, c.W(l.dctxs) + (size_t)i0 * B * M, M, 1.f));
+    return B200TTS_OK;
+}
+
+// zero the accumulators of the attention reverse steps on the per-step chains
+int att_chain_init(const BwdCtx& c) {
+    const auto& s = c.s; const auto& l = c.l;
+    B200_TRY(launch_fill(c.W(l.dmemT), 0.f, (size_t)s.B * s.L * s.A, c.st));
+    if (!forward_attention(s)) {
+        B200_TRY(launch_fill(c.W(l.dWloc_acc), 0.f, (size_t)s.B * s.A * s.C, c.st));
+        B200_TRY(launch_fill(c.W(l.dWc_acc), 0.f, (size_t)s.B * s.C * s.K, c.st));
+    }
+    B200_TRY(launch_fill(c.W(l.dv_acc), 0.f, (size_t)s.B * s.A, c.st));
+    return B200TTS_OK;
+}
+
+// attention reverse step i on the per-step chain: attention backward (d cum / d alpha carried in dcum), attention-LSTM cell backward
+// (carried state in dc / dhz), then the recurrent [d ctx_{i-1} | d h_att_{i-1}] = dgates_i . [W_ih[:, P:] | W_hh] as split-K partials
+// into `part`, which step i-1 consumes
+int att_bwd_step(const BwdCtx& c, int i, float* part, float* dc, float* dhz) {
+    const auto& s = c.s; const auto& l = c.l; const auto& fl = c.fl; const auto& w = c.w;
+    const int B = s.B, T = s.T, D = s.D, M = s.M, A = s.A, L = s.L, MD = M + D;
+    const size_t BD = (size_t)B * D, B4D = 4 * BD;
+    const int last = (i == T - 1);
+    if (forward_attention(s)) {
+        FwdAttnBwdArgs fa{};
+        fa.q = c.F(fl.q) + (size_t)i * B * A; fa.memT = c.F(fl.memT); fa.memory = c.in.memory; fa.lengths = c.in.text_lengths;
+        fa.bias = w.attn_bias; fa.v = w.attn_energy;
+        fa.alpha_prev = c.F(fl.cum) + (size_t)i * B * L;
+        fa.w = c.fwd_out.alignments + (size_t)i * L; fa.w_bstride = (long long)T * L;
+        fa.dalign = c.dout.d_alignments ? c.dout.d_alignments + (size_t)i * L : nullptr; fa.dalign_bstride = (long long)T * L;
+        fa.dctx_static = c.W(l.dctxs) + (size_t)i * B * M;
+        fa.part = part; fa.nsplit = l.split_att; fa.part_stride = (size_t)B * MD; fa.ld_part = MD;
+        fa.dalpha = c.W(l.dcum); fa.dctx_tot = c.W(l.dctxt) + (size_t)i * B * M; fa.dq = c.W(l.dq) + (size_t)i * B * A;
+        fa.dmemT = c.W(l.dmemT); fa.dv_acc = c.W(l.dv_acc);
+        fa.B = B; fa.L = L; fa.M = M; fa.A = A; fa.last = last;
+        B200_TRY(launch_fwd_attn_bwd(fa, c.st));
+    } else {
+        AttnBwdArgs aa{};
+        aa.q = c.F(fl.q) + (size_t)i * B * A; aa.memT = c.F(fl.memT); aa.memory = c.in.memory; aa.lengths = c.in.text_lengths;
+        aa.Wc = w.attn_loc_features; aa.Wloc = w.attn_location; aa.bias = w.attn_bias; aa.v = w.attn_energy;
+        aa.cum_prev = c.F(fl.cum) + (size_t)i * B * L;
+        aa.w = c.fwd_out.alignments + (size_t)i * L; aa.w_bstride = (long long)T * L;
+        aa.dalign = c.dout.d_alignments ? c.dout.d_alignments + (size_t)i * L : nullptr; aa.dalign_bstride = (long long)T * L;
+        aa.dctx_static = c.W(l.dctxs) + (size_t)i * B * M;
+        aa.part = part; aa.nsplit = l.split_att; aa.part_stride = (size_t)B * MD; aa.ld_part = MD;
+        aa.dcum = c.W(l.dcum); aa.dctx_tot = c.W(l.dctxt) + (size_t)i * B * M; aa.dq = c.W(l.dq) + (size_t)i * B * A;
+        aa.dmemT = c.W(l.dmemT); aa.dWloc_acc = c.W(l.dWloc_acc); aa.dWc_acc = c.W(l.dWc_acc); aa.dv_acc = c.W(l.dv_acc);
+        aa.B = B; aa.L = L; aa.M = M; aa.A = A; aa.C = s.C; aa.K = s.K; aa.last = last;
+        B200_TRY(launch_attn_bwd(aa, c.st));
+    }
+
+    CellBwdArgs ca{};
+    ca.gates = c.F(fl.ga) + (size_t)i * B4D;
+    ca.c_prev = c.F(fl.ca) + (size_t)i * BD;
+    ca.dh_static = c.W(l.dhas) + (size_t)i * BD; ca.ld_dhs = D;
+    ca.part = part; ca.nsplit = l.split_att; ca.part_stride = (size_t)B * MD; ca.ld_part = MD; ca.part_col0 = M;
+    ca.dq = c.W(l.dq) + (size_t)i * B * A; ca.Wq = w.attn_query; ca.A = A;
+    ca.dc_state = dc; ca.dhz_state = s.cell_kind == B200TTS_CELL_ZONEOUT ? dhz : nullptr;
+    ca.mask_h = c.in.mask_att_h ? c.in.mask_att_h + (size_t)i * BD : nullptr;
+    ca.mask_c = c.in.mask_att_c ? c.in.mask_att_c + (size_t)i * BD : nullptr;
+    ca.kind = s.cell_kind; ca.training = s.training; ca.rate_h = s.rate_h; ca.rate_c = s.rate_c;
+    ca.dgates = c.W(l.dga) + (size_t)i * B4D; ca.B = B; ca.D = D; ca.last = last;
+    B200_TRY(launch_cell_bwd(ca, c.st));
+    if (i > 0) {
+        GemmDesc d;      // [d ctx_{i-1} | d h_att_{i-1}] (recurrent) = dgates_i . [W_ih[:, P:] | W_hh]
+        d.A = ca.dgates; d.lda = 4 * D; d.B = c.F(fl.wcat_att); d.ldb = MD; d.transB = 0; d.M = B; d.N = MD; d.K = 4 * D;
+        d.splitk = l.split_att; d.partial = part; d.keep_partials = 1;
+        if (d.splitk == 1) { d.C = part; d.ldc = MD; d.keep_partials = 0; d.partial = nullptr; }
+        B200_TRY(gemm_run(d, c.st));
+    }
+    return B200TTS_OK;
+}
+
+// dropout scale of the prenet layer whose keep masks are `mask` (NULL: no dropout there)
+inline float prenet_scale(const b200tts_decoder_shape& s, const uint8_t* mask) { return mask ? 1.f / (1.f - s.prenet_rate) : 1.f; }
+
+// relu + dropout backward of one prenet layer over all T steps, in place on dz [T, B, P].  Teacher-forced steps were dropped with the
+// time-batched masks (mask_tf), free-running steps with the per-step masks (mask_fr); a caller may pass either set without the other,
+// so each maximal run of steps with one scale gets one launch (a teacher-forced decode: a single launch over every row).
+int prenet_relu_bwd(const BwdCtx& c, float* dz, const float* y, const uint8_t* mask_tf, const uint8_t* mask_fr) {
+    const auto& s = c.s;
+    const size_t BP = (size_t)s.B * s.P;
+    const float scale_tf = prenet_scale(s, mask_tf), scale_fr = prenet_scale(s, mask_fr);
+    auto scale_of = [&](int i) { return c.free_running(i) ? scale_fr : scale_tf; };
+    for (int i0 = 0; i0 < s.T;) {
+        const float scale = scale_of(i0);
+        int i1 = i0 + 1;
+        while (i1 < s.T && scale_of(i1) == scale) ++i1;
+        const size_t n = (size_t)(i1 - i0) * BP;
+        relu_dropout_bwd_kernel<<<grid_for(n), 256, 0, c.st>>>(dz + (size_t)i0 * BP, dz + (size_t)i0 * BP, y + (size_t)i0 * BP, scale, n);
+        B200_LAUNCH_CHECK();
+        i0 = i1;
+    }
+    return B200TTS_OK;
+}
+
+// feedback of free-running step f >= 1 into row f-1: d p1_f = dga_f . W_ih_att[:, :P] (long K = 4D: the GEMM, into row f of dp1, which
+// the time-batched prenet pass rewrites later), then the rest of the chain in frame_feedback_bwd_kernel
+int frame_feedback(const BwdCtx& c, int f) {
+    const auto& s = c.s; const auto& l = c.l;
+    const int B = s.B, D = s.D, M = s.M, P = s.P, N = s.N;
+    float* dp1 = c.W(l.dp1) + (size_t)f * B * P;
+    B200_TRY(xgemm16(c.st, l, c.bws, B, P, 4 * D, c.W(l.dga) + (size_t)f * B * 4 * D, 4 * D, nullptr, 0, c.w.att_w_ih, P + M, dp1, P, 0.f));
+    FeedbackArgs a{};
+    a.dp1 = dp1;
+    a.p0 = c.F(c.fl.p0) + (size_t)f * B * P; a.p1 = c.F(c.fl.p1) + (size_t)f * B * P;
+    a.W0 = c.w.prenet_w0; a.W1 = c.w.prenet_w1; a.wfs = c.F(c.fl.wfs);
+    a.dfs = c.W(l.dfs) + (size_t)(f - 1) * B * (N + 1);
+    a.dhgd = c.W(l.dhgd) + (size_t)(f - 1) * B * D;
+    a.dctxs = c.W(l.dctxs) + (size_t)(f - 1) * B * M;
+    a.scale0 = prenet_scale(s, c.in.mask_step_prenet0); a.scale1 = prenet_scale(s, c.in.mask_step_prenet1);
+    a.B = B; a.P = P; a.N = N; a.D = D; a.M = M;
+    const size_t smem = feedback_smem_floats(P, N) * sizeof(float);
+    B200_REQUIRE(smem <= 48 * 1024, "decoder_backward: frame feedback needs %zu B of shared memory (P=%d N=%d)", smem, P, N);
+    frame_feedback_bwd_kernel<<<B, FEEDBACK_THREADS, smem, c.st>>>(a);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
 }
 
 }  // namespace
@@ -833,23 +1111,24 @@ int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_
                  "decoder_backward: attention dims A=%d C=%d unsupported (need A%%4==0, C%%4==0, A*C<=4096)", s.A, s.C);
     B200_REQUIRE(!fwd_att || (!w.attn_location && !w.attn_loc_features && !dw.attn_location && !dw.attn_loc_features),
                  "decoder_backward: forward attention has no location weights (pass NULL)");
+    // a decode with a free-running step ran its forward on the per-step chains (decoder_fwd.cu) and takes the segmented sweep below
+    bool free_running = false;
     if (in.teacher)
-        for (int i = 0; i < s.T; ++i)
-            if (!in.teacher[i]) {
-                set_last_error("decoder_backward: step %d is free-running; backward through free-running steps is not implemented", i);
-                return B200TTS_ERR_UNSUPPORTED;
-            }
+        for (int i = 0; i < s.T; ++i) free_running |= (in.teacher[i] == 0);
     const DecoderLayout fl = decoder_layout(s);
     const BwdLayout l = bwd_layout(s);
     B200_REQUIRE(bws_bytes >= l.total * sizeof(float), "decoder_backward: workspace too small (%zu < %zu bytes)", bws_bytes,
                  l.total * sizeof(float));
     const int B = s.B, T = s.T, D = s.D, M = s.M, P = s.P, N = s.N, A = s.A, L = s.L, C = s.C, K = s.K, MD = M + D, N1 = N + 1;
-    const size_t BD = (size_t)B * D, B4D = 4 * BD, TB = (size_t)T * B;
+    const size_t TB = (size_t)T * B;
     auto F = [&](size_t off) { return fws + off; };
     auto W = [&](size_t off) { return bws + off; };
+    const BwdCtx c{s, w, in, fwd_out, dout, fl, l, fws, bws, st};
     const float* ai = F(fl.ai);                // [T+1, B, M+D]
     const float* ai1 = ai + (size_t)B * MD;    // rows 1..T
-    const PersistPlan plan = precision_mode() == B200TTS_PRECISION_BF16 ? persist_plan(s) : PersistPlan{};
+    // the segmented sweep runs on the per-step chains only: it reads neither the persistent workspace nor the bf16 operand rows, which a
+    // sequential forward never wrote
+    const PersistPlan plan = precision_mode() == B200TTS_PRECISION_BF16 && !free_running ? persist_plan(s) : PersistPlan{};
     // bf16 operand rows the wgmma forward loops left in the persistent workspace: aib [T+1, B, Kp_att] = [h_att | ctx | 0], hgb [T+1, B, Kp_gen]
     // = h_gen (row i+1 = state after step i, row 0 = 0).  The weight-gradient products read them in place (MN-major TMA operands).
     // A training forward ran those loops exactly when the attention reverse loop runs.
@@ -868,123 +1147,61 @@ int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_
     // d h_gen (direct) and d ctx (projection part)
     B200_TRY(wgemm(st, l, bws, 0, 0, (int)TB, D, N1, W(l.dfs), N1, F(fl.wfs), D + M, W(l.dhgd), D, 0.f));
     B200_TRY(wgemm(st, l, bws, 0, 0, (int)TB, M, N1, W(l.dfs), N1, F(fl.wfs) + D, D + M, W(l.dctxs), M, 0.f));
-    // d [frame_w ; stop_w] = dFS^T . [h_gen | ctx]
-    B200_TRY(wgemm16(st, l, bws, N1, D, (int)TB, W(l.dfs), N1, F(fl.hg) + BD, D, hgb1, ldhb, W(l.dwfs), D + M, 0.f));
-    B200_TRY(wgemm16(st, l, bws, N1, M, (int)TB, W(l.dfs), N1, ai1, MD, aib1 ? aib1 + D : nullptr, ldab, W(l.dwfs) + D, D + M, 0.f));
-    add2d_kernel<<<grid_for((size_t)N * (D + M)), 256, 0, st>>>(dw.frame_w, D + M, W(l.dwfs), D + M, N, D + M);
-    B200_LAUNCH_CHECK();
-    add2d_kernel<<<grid_for((size_t)(D + M)), 256, 0, st>>>(dw.stop_w, D + M, W(l.dwfs) + (size_t)N * (D + M), D + M, 1, D + M);
-    B200_LAUNCH_CHECK();
-    B200_TRY(colsum_add(dw.frame_b, nullptr, W(l.dfs), TB, N, N1, W(l.gpart), st));
-    B200_TRY(colsum_add(dw.stop_b, nullptr, W(l.dfs) + N, TB, 1, N1, W(l.gpart), st));
 
-    // ---- 2. generator LSTM reverse loop ----
-    const bool zone = s.cell_kind == B200TTS_CELL_ZONEOUT;
-    // the persistent reverse loops keep their bf16 gate gradients as [T, B, 4D] histories: the time-batched products below read them in
-    // place (K-major for dX, MN-major for dW) instead of converting the fp32 copies
-    void* dggb = plan.gen_bwd ? static_cast<void*>(W(l.dggb)) : nullptr;
-    if (plan.gen_bwd) {
-        // bf16 perf mode: one cooperative weight-stationary TMA + wgmma kernel for the whole reverse recurrence (decoder_persist_bwd_tc.cu)
-        B200_TRY(tc_persist_gen_bwd_loop(s, w, in, fl, fws, W(l.dhgd), W(l.dgg), reinterpret_cast<unsigned char*>(W(l.pextra)), st, dggb));
-    } else {
-    for (int i = T - 1; i >= 0; --i) {
-            CellBwdArgs ca{};
-            ca.gates = F(fl.gg) + (size_t)i * B4D;
-            ca.c_prev = F(fl.cg) + (size_t)i * BD;
-            ca.dh_static = W(l.dhgd) + (size_t)i * BD; ca.ld_dhs = D;
-            ca.part = W(l.part); ca.nsplit = l.split_gen; ca.part_stride = BD; ca.ld_part = D; ca.part_col0 = 0;
-            ca.dq = nullptr; ca.Wq = nullptr; ca.A = 0;
-            ca.dc_state = W(l.dc); ca.dhz_state = zone ? W(l.dhz) : nullptr;
-            ca.mask_h = in.mask_gen_h ? in.mask_gen_h + (size_t)i * BD : nullptr;
-            ca.mask_c = in.mask_gen_c ? in.mask_gen_c + (size_t)i * BD : nullptr;
-            ca.kind = s.cell_kind; ca.training = s.training; ca.rate_h = s.rate_h; ca.rate_c = s.rate_c;
-            ca.dgates = W(l.dgg) + (size_t)i * B4D; ca.B = B; ca.D = D; ca.last = (i == T - 1);
-            B200_TRY(launch_cell_bwd(ca, st));
-            if (i > 0) {
-                GemmDesc d;      // d h_gen_{i-1} (recurrent) = dgates_i . W_hh
-                d.A = ca.dgates; d.lda = 4 * D; d.B = w.gen_w_hh; d.ldb = D; d.transB = 0; d.M = B; d.N = D; d.K = 4 * D;
-                d.splitk = l.split_gen; d.partial = W(l.part); d.keep_partials = 1;
-                if (d.splitk == 1) { d.C = W(l.part); d.ldc = D; d.keep_partials = 0; d.partial = nullptr; }
-                B200_TRY(gemm_run(d, st));
-            }
-        }
-    }
-    {
-        // time-batched generator gradients.  The gate gradients are final now: their packed (transposed / K-contiguous) bf16 copies are
-        // made once and shared by the three weight-gradient and the two input-gradient products (pack cache of the wgmma GEMM).
-        PackScope pack_scope;
-        B200_TRY(wgemm16(st, l, bws, 4 * D, D, (int)TB, W(l.dgg), 4 * D, F(fl.hg), D, hgb, ldhb, dw.gen_w_hh, D, 1.f, dggb, 4 * D));
-        B200_TRY(wgemm16(st, l, bws, 4 * D, D, (int)TB, W(l.dgg), 4 * D, ai1 + M, MD, aib1, ldab, dw.gen_w_ih, D + M, 1.f, dggb, 4 * D));
-        B200_TRY(wgemm16(st, l, bws, 4 * D, M, (int)TB, W(l.dgg), 4 * D, ai1, MD, aib1 ? aib1 + D : nullptr, ldab, dw.gen_w_ih + D, D + M, 1.f, dggb, 4 * D));
-        B200_TRY(colsum_add(dw.gen_b_ih, dw.gen_b_hh, W(l.dgg), TB, 4 * D, 4 * D, W(l.gpart), st));
-        // d h_att (static part) and d ctx (generator-input part, accumulated onto the projection part)
-        B200_TRY(xgemm16(st, l, bws, (int)TB, D, 4 * D, W(l.dgg), 4 * D, dggb, 4 * D, w.gen_w_ih, D + M, W(l.dhas), D, 0.f));
-        B200_TRY(xgemm16(st, l, bws, (int)TB, M, 4 * D, W(l.dgg), 4 * D, dggb, 4 * D, w.gen_w_ih + D, D + M, W(l.dctxs), M, 1.f));
-    }
-
-    // ---- 3. attention LSTM + attention reverse loop ----
     void* dgab = plan.att_bwd ? static_cast<void*>(W(l.dgab)) : nullptr;
-    if (plan.att_bwd) {
-        // bf16 perf mode: cooperative weight-stationary kernel (tensor-core attention backward inside), then a parallel post pass
-        B200_TRY(persist_att_bwd_loop(s, w, in, fl, fws, prl, pws, fwd_out.alignments,
-                                      dout.d_alignments, W(l.dhas), W(l.dctxs), W(l.dga), W(l.dq), W(l.dctxt), W(l.dmemT),
-                                      reinterpret_cast<unsigned char*>(W(l.pextra2)), dw, st, dgab));
-    } else {
-    B200_TRY(launch_fill(W(l.dmemT), 0.f, (size_t)B * L * A, st));
-        if (!fwd_att) {
-            B200_TRY(launch_fill(W(l.dWloc_acc), 0.f, (size_t)B * A * C, st));
-            B200_TRY(launch_fill(W(l.dWc_acc), 0.f, (size_t)B * C * K, st));
-        }
-        B200_TRY(launch_fill(W(l.dv_acc), 0.f, (size_t)B * A, st));
-        for (int i = T - 1; i >= 0; --i) {
-            const int last = (i == T - 1);
-            if (fwd_att) {
-                FwdAttnBwdArgs fa{};
-                fa.q = F(fl.q) + (size_t)i * B * A; fa.memT = F(fl.memT); fa.memory = in.memory; fa.lengths = in.text_lengths;
-                fa.bias = w.attn_bias; fa.v = w.attn_energy;
-                fa.alpha_prev = F(fl.cum) + (size_t)i * B * L;
-                fa.w = fwd_out.alignments + (size_t)i * L; fa.w_bstride = (long long)T * L;
-                fa.dalign = dout.d_alignments ? dout.d_alignments + (size_t)i * L : nullptr; fa.dalign_bstride = (long long)T * L;
-                fa.dctx_static = W(l.dctxs) + (size_t)i * B * M;
-                fa.part = W(l.part); fa.nsplit = l.split_att; fa.part_stride = (size_t)B * MD; fa.ld_part = MD;
-                fa.dalpha = W(l.dcum); fa.dctx_tot = W(l.dctxt) + (size_t)i * B * M; fa.dq = W(l.dq) + (size_t)i * B * A;
-                fa.dmemT = W(l.dmemT); fa.dv_acc = W(l.dv_acc);
-                fa.B = B; fa.L = L; fa.M = M; fa.A = A; fa.last = last;
-                B200_TRY(launch_fwd_attn_bwd(fa, st));
-            } else {
-            AttnBwdArgs aa{};
-            aa.q = F(fl.q) + (size_t)i * B * A; aa.memT = F(fl.memT); aa.memory = in.memory; aa.lengths = in.text_lengths;
-            aa.Wc = w.attn_loc_features; aa.Wloc = w.attn_location; aa.bias = w.attn_bias; aa.v = w.attn_energy;
-            aa.cum_prev = F(fl.cum) + (size_t)i * B * L;
-            aa.w = fwd_out.alignments + (size_t)i * L; aa.w_bstride = (long long)T * L;
-            aa.dalign = dout.d_alignments ? dout.d_alignments + (size_t)i * L : nullptr; aa.dalign_bstride = (long long)T * L;
-            aa.dctx_static = W(l.dctxs) + (size_t)i * B * M;
-            aa.part = W(l.part); aa.nsplit = l.split_att; aa.part_stride = (size_t)B * MD; aa.ld_part = MD;
-            aa.dcum = W(l.dcum); aa.dctx_tot = W(l.dctxt) + (size_t)i * B * M; aa.dq = W(l.dq) + (size_t)i * B * A;
-            aa.dmemT = W(l.dmemT); aa.dWloc_acc = W(l.dWloc_acc); aa.dWc_acc = W(l.dWc_acc); aa.dv_acc = W(l.dv_acc);
-            aa.B = B; aa.L = L; aa.M = M; aa.A = A; aa.C = C; aa.K = K; aa.last = last;
-            B200_TRY(launch_attn_bwd(aa, st));
-            }
+    if (!free_running) {
+        B200_TRY(frame_weight_grads(c, dw, hgb1, ldhb, aib1, ldab));
 
-            CellBwdArgs ca{};
-            ca.gates = F(fl.ga) + (size_t)i * B4D;
-            ca.c_prev = F(fl.ca) + (size_t)i * BD;
-            ca.dh_static = W(l.dhas) + (size_t)i * BD; ca.ld_dhs = D;
-            ca.part = W(l.part); ca.nsplit = l.split_att; ca.part_stride = (size_t)B * MD; ca.ld_part = MD; ca.part_col0 = M;
-            ca.dq = W(l.dq) + (size_t)i * B * A; ca.Wq = w.attn_query; ca.A = A;
-            ca.dc_state = W(l.dc); ca.dhz_state = zone ? W(l.dhz) : nullptr;
-            ca.mask_h = in.mask_att_h ? in.mask_att_h + (size_t)i * BD : nullptr;
-            ca.mask_c = in.mask_att_c ? in.mask_att_c + (size_t)i * BD : nullptr;
-            ca.kind = s.cell_kind; ca.training = s.training; ca.rate_h = s.rate_h; ca.rate_c = s.rate_c;
-            ca.dgates = W(l.dga) + (size_t)i * B4D; ca.B = B; ca.D = D; ca.last = last;
-            B200_TRY(launch_cell_bwd(ca, st));
-            if (i > 0) {
-                GemmDesc d;      // [d ctx_{i-1} | d h_att_{i-1}] (recurrent) = dgates_i . [W_ih[:, P:] | W_hh]
-                d.A = ca.dgates; d.lda = 4 * D; d.B = F(fl.wcat_att); d.ldb = MD; d.transB = 0; d.M = B; d.N = MD; d.K = 4 * D;
-                d.splitk = l.split_att; d.partial = W(l.part); d.keep_partials = 1;
-                if (d.splitk == 1) { d.C = W(l.part); d.ldc = MD; d.keep_partials = 0; d.partial = nullptr; }
-                B200_TRY(gemm_run(d, st));
-            }
+        // ---- 2. generator LSTM reverse loop ----
+        // the persistent reverse loops keep their bf16 gate gradients as [T, B, 4D] histories: the time-batched products below read them
+        // in place (K-major for dX, MN-major for dW) instead of converting the fp32 copies
+        void* dggb = plan.gen_bwd ? static_cast<void*>(W(l.dggb)) : nullptr;
+        if (plan.gen_bwd) {
+            // bf16 perf mode: one cooperative weight-stationary TMA + wgmma kernel for the whole reverse recurrence (decoder_persist_bwd_tc.cu)
+            B200_TRY(tc_persist_gen_bwd_loop(s, w, in, fl, fws, W(l.dhgd), W(l.dgg), reinterpret_cast<unsigned char*>(W(l.pextra)), st, dggb));
+        } else {
+            for (int i = T - 1; i >= 0; --i) B200_TRY(gen_bwd_step(c, i, W(l.part), W(l.dc), W(l.dhz)));
+        }
+        {
+            // time-batched generator gradients.  The gate gradients are final now: their packed (transposed / K-contiguous) bf16 copies are
+            // made once and shared by the three weight-gradient and the two input-gradient products (pack cache of the wgmma GEMM).
+            PackScope pack_scope;
+            B200_TRY(gen_weight_grads(c, dw, hgb, ldhb, aib1, ldab, dggb));
+            B200_TRY(gen_input_grads(c, 0, T, dggb));
+        }
+
+        // ---- 3. attention LSTM + attention reverse loop ----
+        if (plan.att_bwd) {
+            // bf16 perf mode: cooperative weight-stationary kernel (tensor-core attention backward inside), then a parallel post pass
+            B200_TRY(persist_att_bwd_loop(s, w, in, fl, fws, prl, pws, fwd_out.alignments,
+                                          dout.d_alignments, W(l.dhas), W(l.dctxs), W(l.dga), W(l.dq), W(l.dctxt), W(l.dmemT),
+                                          reinterpret_cast<unsigned char*>(W(l.pextra2)), dw, st, dgab));
+        } else {
+            B200_TRY(att_chain_init(c));
+            for (int i = T - 1; i >= 0; --i) B200_TRY(att_bwd_step(c, i, W(l.part), W(l.dc), W(l.dhz)));
+        }
+    } else {
+        // ---- 2-3. at least one free-running step: segmented reverse sweep on the per-step chains ----
+        // A free-running step f >= 1 feeds prenet(frame_{f-1}) and autograd follows it (tacotron2.py:171,181: no detach), so the attention
+        // reverse step f has to finish before the generator reverse step f-1 can start.  [0, T) is cut at every such f.  Each segment
+        // [f, e), from the end: generator reverse steps e-1 .. f, the generator-input gradients of its rows, attention reverse steps
+        // e-1 .. f, then the feedback of step f into row f-1 (dFS, d h_gen, d ctx).  Both recurrences carry state across segments at the
+        // same time: the generator's lives in part_gen / dc_gen / dhz_gen, the attention's in part / dc / dhz / dcum.
+        B200_TRY(att_chain_init(c));
+        int e = T;
+        for (int f = T - 1; f >= 0; --f) {
+            if (f > 0 && !c.free_running(f)) continue;
+            for (int i = e - 1; i >= f; --i) B200_TRY(gen_bwd_step(c, i, W(l.part_gen), W(l.dc_gen), W(l.dhz_gen)));
+            B200_TRY(gen_input_grads(c, f, e, nullptr));
+            for (int i = e - 1; i >= f; --i) B200_TRY(att_bwd_step(c, i, W(l.part), W(l.dc), W(l.dhz)));
+            if (f > 0) B200_TRY(frame_feedback(c, f));       // step 0 was fed the zero frame: nothing to send
+            e = f;
+        }
+        // dFS is final only now: the fed-back rows changed it after the products of section 1
+        B200_TRY(frame_weight_grads(c, dw, nullptr, 0, nullptr, 0));
+        {
+            PackScope pack_scope;
+            B200_TRY(gen_weight_grads(c, dw, nullptr, 0, nullptr, 0, nullptr));
         }
     }
 
@@ -1018,18 +1235,14 @@ int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_
                        (long long)T * L, (long long)M, (long long)L * M));
         B200_TRY(wgemm(st, l, bws, 0, 0, B * L, M, A, W(l.dmemT), A, w.attn_memory, M, d_memory, M, 1.f));
     }
-    // prenet: d P1 = dGA . W_ih[:, :P]; through dropout+relu; layer 1; layer 0
+    // prenet: d P1 = dGA . W_ih[:, :P]; through dropout+relu; layer 1; layer 0.  Row i = step i's prenet, free-running ones included.
     {
-        const float scale1 = in.mask_prenet1 ? 1.f / (1.f - s.prenet_rate) : 1.f;
-        const float scale0 = in.mask_prenet0 ? 1.f / (1.f - s.prenet_rate) : 1.f;
         B200_TRY(xgemm16(st, l, bws, (int)TB, P, 4 * D, W(l.dga), 4 * D, dgab, 4 * D, w.att_w_ih, P + M, W(l.dp1), P, 0.f));
-        relu_dropout_bwd_kernel<<<grid_for(TB * P), 256, 0, st>>>(W(l.dp1), W(l.dp1), F(fl.p1), scale1, TB * P);
-        B200_LAUNCH_CHECK();
+        B200_TRY(prenet_relu_bwd(c, W(l.dp1), F(fl.p1), in.mask_prenet1, in.mask_step_prenet1));
         B200_TRY(wgemm(st, l, bws, 1, 0, P, P, (int)TB, W(l.dp1), P, F(fl.p0), P, dw.prenet_w1, P, 1.f));
         B200_TRY(colsum_add(dw.prenet_b1, nullptr, W(l.dp1), TB, P, P, W(l.gpart), st));
         B200_TRY(wgemm(st, l, bws, 0, 0, (int)TB, P, P, W(l.dp1), P, w.prenet_w1, P, W(l.dp0), P, 0.f));
-        relu_dropout_bwd_kernel<<<grid_for(TB * P), 256, 0, st>>>(W(l.dp0), W(l.dp0), F(fl.p0), scale0, TB * P);
-        B200_LAUNCH_CHECK();
+        B200_TRY(prenet_relu_bwd(c, W(l.dp0), F(fl.p0), in.mask_prenet0, in.mask_step_prenet0));
         B200_TRY(wgemm(st, l, bws, 1, 0, P, N, (int)TB, W(l.dp0), P, F(fl.xtm), N, dw.prenet_w0, N, 1.f));
         B200_TRY(colsum_add(dw.prenet_b0, nullptr, W(l.dp0), TB, P, P, W(l.gpart), st));
     }

@@ -39,6 +39,11 @@ class GraphedTrainStep:
     FIELDS = ('text', 'text_length', 'target', 'target_length', 'stop_target', 'speakers', 'languages')
 
     def __init__(self, model, criterion, bucket, example_batch, teacher_forcing=1.0, warmup=3):
+        if float(teacher_forcing) < 1.0:
+            # the per-step teacher-forcing coins are drawn on the host and decide which kernels a decode launches: one captured graph
+            # would replay one frozen coin pattern at every step.  Run such steps eagerly (the backward supports them).
+            raise ValueError(f'GraphedTrainStep needs teacher_forcing = 1.0 (got {teacher_forcing}): a CUDA graph would replay one fixed '
+                             'pattern of free-running steps; run steps with teacher forcing below 1.0 eagerly')
         self.model, self.criterion, self.bucket, self.tf = model, criterion, bucket, float(teacher_forcing)
         dev = next(model.parameters()).device
         self.static = {k: (example_batch[k].to(dev).clone() if example_batch.get(k) is not None else None) for k in self.FIELDS}
