@@ -87,6 +87,11 @@ typedef struct {
                                are ignored, params.attn_location / attn_loc_features must be NULL, the cumulative-weight rows of
                                the workspace (and b200tts_decoder_state.cum_weights) hold the forward variable alpha, and every
                                recurrence runs on the per-step kernel chains in both precision modes (b200tts_decoder_path = 0) */
+    int att_extent;         /* forward attention only (location-sensitive attention ignores it).  0 in a zero-initialised shape: the
+                               transition softmax, the 1e-6 floor, the normalisation and the context run over all L positions, padding
+                               included (the reference's training semantics).  1: over each utterance's own text length; weights at
+                               l >= length are 0, so a padded batch decodes every utterance as it decodes alone.  Forward and chunk
+                               entry points only: b200tts_decoder_backward rejects 1. */
 } b200tts_decoder_shape;
 
 /* Parameter block in the reference's own layouts ([out, in] Linear weights; names = state_dict keys). */
@@ -267,6 +272,14 @@ int b200tts_convblock_forward(const b200tts_convblock_shape* shape, const float*
                               const float* gamma, const float* beta, int affine_gstride, float* running_mean,
                               float* running_var, const uint8_t* keep, float* out, void* saved, void* workspace,
                               void* stream);
+/* The same for a padded batch of utterances in eval mode, whole block (stage 0) only: lengths [NB] int32 (device); every output at a
+ * position l >= lengths[n] of sample n is written as 0 by the fused epilogue.  Fed a zero-padded input, each sample's output then
+ * equals running the block on that sample alone (conv1d pads with zeros); with every length == L it is bit-identical to
+ * b200tts_convblock_forward.  Training or stage 1 / 2 is rejected.                                                                */
+int b200tts_convblock_forward_masked(const b200tts_convblock_shape* shape, const int32_t* lengths, const float* x, const float* weight,
+                                     const float* gamma, const float* beta, int affine_gstride, float* running_mean,
+                                     float* running_var, const uint8_t* keep, float* out, void* saved, void* workspace,
+                                     void* stream);
 /* dx overwritten; dweight / dgamma / dbeta accumulated (+=).                                         */
 int b200tts_convblock_backward(const b200tts_convblock_shape* shape, const float* x, const float* weight,
                                const float* gamma, const float* beta, int affine_gstride, const uint8_t* keep,

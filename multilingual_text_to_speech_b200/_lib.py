@@ -20,7 +20,7 @@ class B200TTSError(RuntimeError):
 
 class DecoderShape(Structure):
     _fields_ = [(n, c_int) for n in ('B', 'L', 'T', 'M', 'D', 'P', 'A', 'C', 'K', 'N', 'cell_kind', 'training')] + \
-               [('rate_h', c_float), ('rate_c', c_float), ('prenet_rate', c_float), ('att_kind', c_int)]
+               [('rate_h', c_float), ('rate_c', c_float), ('prenet_rate', c_float), ('att_kind', c_int), ('att_extent', c_int)]
 
 
 DECODER_PARAM_FIELDS = ('prenet_w0', 'prenet_b0', 'prenet_w1', 'prenet_b1', 'att_w_ih', 'att_w_hh', 'att_b_ih', 'att_b_hh',
@@ -108,6 +108,8 @@ SIGNATURES = {
     'b200tts_convblock_workspace_bytes': (c_size_t, [POINTER(ConvBlockShape)]),
     'b200tts_convblock_forward': (c_int, [POINTER(ConvBlockShape), c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
                                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'b200tts_convblock_forward_masked': (c_int, [POINTER(ConvBlockShape), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                                 c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'b200tts_convblock_backward': (c_int, [POINTER(ConvBlockShape), c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'b200tts_lstm_cell_forward': (c_int, [c_int, c_int, c_int, c_int, c_float, c_float] + [c_void_p] * 8),

@@ -105,7 +105,7 @@ size_t convblock_saved_floats(const b200tts_convblock_shape& s);
 size_t convblock_workspace_floats(const b200tts_convblock_shape& s);
 int convblock_forward_impl(const b200tts_convblock_shape& s, const float* x, const float* weight, const float* gamma,
                            const float* beta, int affine_gstride, float* running_mean, float* running_var, const uint8_t* keep,
-                           float* out, float* saved, float* ws, cudaStream_t st);
+                           float* out, float* saved, float* ws, cudaStream_t st, const int32_t* lengths = nullptr);
 int convblock_backward_impl(const b200tts_convblock_shape& s, const float* x, const float* weight, const float* gamma,
                             const float* beta, int affine_gstride, const uint8_t* keep, const float* saved, const float* dout,
                             float* dx, float* dweight, float* dgamma, float* dbeta, float* ws, cudaStream_t st);
@@ -361,6 +361,17 @@ int b200tts_convblock_forward(const b200tts_convblock_shape* shape, const float*
     B200_TRY(require_device());
     return convblock_forward_impl(*shape, x, weight, gamma, beta, affine_gstride, running_mean, running_var, keep, out, (float*)saved,
                                   (float*)workspace, (cudaStream_t)stream);
+}
+
+int b200tts_convblock_forward_masked(const b200tts_convblock_shape* shape, const int32_t* lengths, const float* x, const float* weight,
+                                     const float* gamma, const float* beta, int affine_gstride, float* running_mean, float* running_var,
+                                     const uint8_t* keep, float* out, void* saved, void* workspace, void* stream) {
+    B200_REQUIRE(shape && lengths && x && out && saved && workspace, "convblock_forward_masked: null argument");
+    B200_REQUIRE(shape->stage == 0 && !shape->training, "convblock_forward_masked: eval mode and the whole block (stage 0) only");
+    B200_REQUIRE(weight && gamma && beta, "convblock_forward_masked: null parameter");
+    B200_TRY(require_device());
+    return convblock_forward_impl(*shape, x, weight, gamma, beta, affine_gstride, running_mean, running_var, keep, out, (float*)saved,
+                                  (float*)workspace, (cudaStream_t)stream, lengths);
 }
 
 int b200tts_convblock_backward(const b200tts_convblock_shape* shape, const float* x, const float* weight, const float* gamma,

@@ -1106,6 +1106,8 @@ int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_
                           float* bws, size_t bws_bytes, const b200tts_decoder_params& dw, float* d_memory, cudaStream_t st) {
     B200_TRY(validate_decoder_shape(s));
     B200_REQUIRE(fwd_out.alignments, "decoder_backward: the forward alignments tensor is required");
+    B200_REQUIRE(s.att_extent == 0, "decoder_backward: att_extent = 1 (attention over each utterance's own length) is for inference only; "
+                 "training keeps the reference's softmax over the padded extent");
     const bool fwd_att = forward_attention(s);
     B200_REQUIRE(fwd_att || (s.A % 4 == 0 && s.C % 4 == 0 && (s.A / 4) * (s.C / 4) <= ATT_THREADS),
                  "decoder_backward: attention dims A=%d C=%d unsupported (need A%%4==0, C%%4==0, A*C<=4096)", s.A, s.C);

@@ -325,6 +325,7 @@ struct FwdAttnArgs {
     float* align; long long align_bstride;        // &align[0, i, 0]; stride between utterances
     float* ctx_out; int ld_ctx;        // [B, ld]
     int B, L, M, A;
+    int own_extent;                    // 1: every sum runs over l < lengths[b] instead of l < L (b200tts_decoder_shape.att_extent)
 };
 
 static inline size_t fwd_attn_smem_floats(int L, int M, int A) {
@@ -344,6 +345,9 @@ __global__ void __launch_bounds__(ATT_THREADS) fwd_attn_fwd_kernel(const FwdAttn
     int len = p.lengths[b];
     len = len < 0 ? 0 : (len > L ? L : len);
     const float* alpha = p.alpha_prev + (size_t)b * L;
+    // the extent of the softmax, the floor, the normalisation and the context: the padded L (the reference's training semantics) or
+    // the utterance's own length, which gives a padded batch the loop bounds, and so the partial sums, of decoding it alone
+    const int Le = p.own_extent ? len : L;
 
     for (int a = tid; a < A; a += ATT_THREADS) {
         float q = 0.f;
@@ -353,28 +357,28 @@ __global__ void __launch_bounds__(ATT_THREADS) fwd_attn_fwd_kernel(const FwdAttn
         vv[a] = p.v[a];
     }
     __syncthreads();
-    fwd_att_transition(qb, vv, p.memT + (size_t)b * L * A, L, A, s, red);
+    fwd_att_transition(qb, vv, p.memT + (size_t)b * L * A, Le, A, s, red);
 
     float csum = 0.f;
-    for (int l = tid; l < L; l += ATT_THREADS) {
+    for (int l = tid; l < Le; l += ATT_THREADS) {
         const float c = fmaxf(fwd_att_product(alpha, s, l, len), FWD_ATT_FLOOR);
         s[l] = c;           // each thread rewrites only the positions it read
         csum += c;
     }
     const float denom = fmaxf(block_sum(csum, red), FWD_ATT_NORM_EPS);
     for (int l = tid; l < L; l += ATT_THREADS) {
-        const float w = s[l] / denom;
+        const float w = l < Le ? s[l] / denom : 0.f;
         s[l] = w;
         p.align[(size_t)b * p.align_bstride + l] = w;
         p.alpha_next[(size_t)b * L + l] = w;
     }
     __syncthreads();
 
-    // context[m] = sum over every l < L of w[l] * memory[b, l, m]
+    // context[m] = sum over every l < Le of w[l] * memory[b, l, m]
     float acc[16];
 #pragma unroll
     for (int j = 0; j < 16; ++j) acc[j] = 0.f;
-    for (int l = warp; l < L; l += NW) {
+    for (int l = warp; l < Le; l += NW) {
         const float w = s[l];
         const float* row = p.memory + ((size_t)b * L + l) * M;
 #pragma unroll
@@ -469,6 +473,7 @@ int launch_fill(float* dst, float value, size_t n, cudaStream_t st) {
 int validate_decoder_shape(const b200tts_decoder_shape& s) {
     B200_REQUIRE(s.B > 0 && s.L > 0 && s.T > 0, "decoder: empty batch/sequence (B=%d L=%d T=%d)", s.B, s.L, s.T);
     B200_REQUIRE(s.att_kind == B200TTS_ATT_LOCATION || s.att_kind == B200TTS_ATT_FORWARD, "decoder: bad attention kind %d", s.att_kind);
+    B200_REQUIRE(s.att_extent == 0 || s.att_extent == 1, "decoder: bad attention extent %d", s.att_extent);
     B200_REQUIRE(s.M > 0 && s.D > 0 && s.P > 0 && s.A > 0 && s.N > 0, "decoder: non-positive dimension");
     B200_REQUIRE(s.A <= 128 && s.A % 4 == 0, "decoder: attention dimension %d unsupported (need <= 128, multiple of 4)", s.A);
     if (!forward_attention(s)) {        // forward attention has no location features: C and K are ignored
@@ -551,7 +556,7 @@ int att_step(const FwdCtx& c, int i, float* align_out) {
         fa.alpha_prev = c.at(l.cum) + (size_t)i * s.B * s.L; fa.alpha_next = c.at(l.cum) + (size_t)(i + 1) * s.B * s.L;
         fa.align = align_out + (size_t)i * s.L; fa.align_bstride = (long long)s.T * s.L;
         fa.ctx_out = ai_n; fa.ld_ctx = (int)MD;
-        fa.B = s.B; fa.L = s.L; fa.M = s.M; fa.A = s.A;
+        fa.B = s.B; fa.L = s.L; fa.M = s.M; fa.A = s.A; fa.own_extent = s.att_extent;
         return launch_fwd_attn(fa, c.st);
     }
     AttnFwdArgs aa{};

@@ -123,6 +123,7 @@ struct BlockArgs {
     const uint8_t* keep; float keep_scale;    // [NB, G*Cout, L] or null
     const float* xin;       // [NB, G*Cin, L] block input (highway only)
     int NB, G, Cout, L, act, highway;
+    const int* lengths;     // [NB] or null (forward only): outputs at positions l >= lengths[nb] are written as 0
 };
 
 // idx -> (nb, g, c, l) of a [NB, G, Cf, L] tensor; 32-bit arithmetic whenever the tensor has fewer than 2^32 elements
@@ -142,6 +143,7 @@ __global__ void block_fwd_kernel(const BlockArgs p, float* __restrict__ out) {
     for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
         int l, c, g; size_t nb;
         split_index(idx, total <= 0xffffffffull, p.L, Cf, p.G, l, c, g, nb);
+        if (p.lengths && l >= p.lengths[nb]) { out[idx] = 0.f; continue; }
         auto value = [&](int o) {
             const int ch = g * p.Cout + o;
             const size_t ci = (nb * p.G * p.Cout + ch) * p.L + l;
@@ -191,14 +193,24 @@ __global__ void __launch_bounds__(256) block_fwd_vec4_kernel(const BlockArgs p, 
             return a;
         };
         const size_t oi = (size_t)row * p.L + 4 * l4;
+        // a float4 group may straddle the utterance's length: the lanes at or past it are zeroed one by one
+        const int valid = p.lengths ? p.lengths[nb] - 4 * (int)l4 : 4;
+        if (valid <= 0) { st4(out + oi, make_float4(0.f, 0.f, 0.f, 0.f)); continue; }
+        float4 r;
         if (p.highway) {
             const float4 h1 = value(c), h2 = value(Cf + c), xi = ld4(p.xin + oi);
             const float s0 = sigmoidf_acc(h1.x), s1 = sigmoidf_acc(h1.y), s2 = sigmoidf_acc(h1.z), s3 = sigmoidf_acc(h1.w);
-            st4(out + oi, make_float4(h2.x * s0 + xi.x * (1.f - s0), h2.y * s1 + xi.y * (1.f - s1), h2.z * s2 + xi.z * (1.f - s2),
-                                      h2.w * s3 + xi.w * (1.f - s3)));
+            r = make_float4(h2.x * s0 + xi.x * (1.f - s0), h2.y * s1 + xi.y * (1.f - s1), h2.z * s2 + xi.z * (1.f - s2),
+                            h2.w * s3 + xi.w * (1.f - s3));
         } else {
-            st4(out + oi, value(c));
+            r = value(c);
         }
+        if (valid < 4) {
+            r.w = 0.f;
+            if (valid < 3) r.z = 0.f;
+            if (valid < 2) r.y = 0.f;
+        }
+        st4(out + oi, r);
     }
 }
 
@@ -647,8 +659,10 @@ size_t convblock_workspace_floats(const b200tts_convblock_shape& s) {
 
 int convblock_forward_impl(const b200tts_convblock_shape& s, const float* x, const float* weight, const float* gamma,
                            const float* beta, int affine_gstride, float* running_mean, float* running_var, const uint8_t* keep,
-                           float* out, float* saved, float* ws, cudaStream_t st) {
+                           float* out, float* saved, float* ws, cudaStream_t st, const int32_t* lengths) {
     B200_TRY(validate_block(s));
+    // padded batches: only the fused epilogue of an eval-mode whole block knows the lengths (training statistics would need them too)
+    B200_REQUIRE(!lengths || (s.stage == 0 && !s.training), "convblock_forward_masked: lengths need an eval-mode whole block (stage 0)");
     const BlockDims d = block_dims(s);
     float* conv = s.stage == 1 ? out : saved;     // convolution only: the product IS the output
     float* mean = saved + align_up_sz(d.conv_elems, 64);
@@ -680,7 +694,7 @@ int convblock_forward_impl(const b200tts_convblock_shape& s, const float* x, con
     }
     B200_LAUNCH_CHECK();
     BlockArgs a{conv, mean, invstd, gamma, beta, affine_gstride, (s.training && s.dropout > 0.f) ? keep : nullptr,
-                1.f / (1.f - s.dropout), x, s.NB, s.G, s.Cout, s.L, s.activation, s.highway};
+                1.f / (1.f - s.dropout), x, s.NB, s.G, s.Cout, s.L, s.activation, s.highway, lengths};
     if (vec4_ok(s, d, conv, out, x, a.keep))
         block_fwd_vec4_kernel<<<grid_for((size_t)s.NB * s.G * d.Cf * (s.L / 4)), 256, 0, st>>>(a, out);
     else

@@ -213,7 +213,8 @@ class DecoderConfig:
 
     MASK_NAMES = ('prenet0', 'prenet1', 'att_h', 'att_c', 'gen_h', 'gen_c', 'step_prenet0', 'step_prenet1')
 
-    def __init__(self, cell_kind, training, rate_h, rate_c, prenet_rate, masks=None, teacher=None):
+    def __init__(self, cell_kind, training, rate_h, rate_c, prenet_rate, masks=None, teacher=None, att_extent=0):
+        self.att_extent = int(att_extent)    # 1: forward attention over each utterance's own length (inference of padded batches)
         self.cell_kind = int(cell_kind)
         self.training = bool(training)
         self.rate_h, self.rate_c, self.prenet_rate = float(rate_h), float(rate_c), float(prenet_rate)
@@ -232,7 +233,7 @@ def _decoder_structs(cfg, shape_dims, params, memory, text_lengths, target):
     B, L, T, M, D, P, A, C, K, N = shape_dims
     att_kind = _attention_dims(dict(zip(DECODER_PARAM_FIELDS, params)))[0]
     shape = DecoderShape(B, L, T, M, D, P, A, C, K, N, cfg.cell_kind, int(cfg.training), cfg.rate_h, cfg.rate_c,
-                         cfg.prenet_rate, att_kind)
+                         cfg.prenet_rate, att_kind, cfg.att_extent)
     pstruct = DecoderParams(*[ptr(p) for p in params])
     teacher_np = None
     if cfg.teacher is not None:
@@ -324,6 +325,11 @@ class DecoderState:
         self.att_h, self.att_c, self.gen_h, self.gen_c = z(B, D), z(B, D), z(B, D), z(B, D)
         self.context, self.cum_weights, self.frame = z(B, M), z(B, L), z(B, N)
         self.first = True
+
+    def select(self, rows):
+        """Keep only the utterances `rows` (a device index tensor), in that order: a finished utterance leaves the decode."""
+        for name in ('att_h', 'att_c', 'gen_h', 'gen_c', 'context', 'cum_weights', 'frame'):
+            setattr(self, name, getattr(self, name).index_select(0, rows).contiguous())
 
     def struct(self):
         return _lib.DecoderState(*[ptr(t) for t in (self.att_h, self.att_c, self.gen_h, self.gen_c, self.context, self.cum_weights, self.frame)])
@@ -460,6 +466,31 @@ class ConvBlockFunction(torch.autograd.Function):
             full = dgb.view(G, gs)
             g_gamma, g_beta = full[:, :Cout], full[:, Cout:]
         return dx, r_weight, g_gamma, g_beta, None, None, None, None
+
+
+def conv_block_masked(x, lengths, weight, gamma, beta, running_mean, running_var, groups, kernel, dilation, activation, highway, eps,
+                      gstride):
+    """Eval-mode whole block over a zero-padded batch (no autograd): sample n keeps its first lengths[n] positions and every output
+    past them is 0, so each sample's output equals running the block on it alone."""
+    _require_cuda(x, weight, gamma, beta, lengths)
+    with torch.no_grad():
+        x, weight = _f32c(x), _f32c(weight)
+        NB, GC, L = x.shape
+        G = groups
+        Cin, Cout = GC // G, weight.shape[0] // G
+        assert weight.shape[1] == Cin and weight.shape[2] == kernel, (weight.shape, Cin, kernel)
+        assert gamma.stride(-1) == 1 and beta.stride(-1) == 1
+        lengths = lengths.to(device=x.device, dtype=torch.int32).contiguous()
+        assert tuple(lengths.shape) == (NB,), (tuple(lengths.shape), NB)
+        shape = _lib.ConvBlockShape(NB, G, Cin, Cout, L, kernel, dilation, ACTIVATIONS[activation], int(highway), 0, eps, 0.0, 0.0, 0)
+        lib = _lib.load()
+        saved = _bytes(lib.b200tts_convblock_saved_bytes(ctypes.byref(shape)), x.device)
+        ws = _bytes(lib.b200tts_convblock_workspace_bytes(ctypes.byref(shape)), x.device)
+        out = torch.empty(NB, G * (Cout // 2 if highway else Cout), L, device=x.device, dtype=torch.float32)
+        check(lib.b200tts_convblock_forward_masked(ctypes.byref(shape), ptr(lengths), ptr(x), ptr(weight), ptr(gamma), ptr(beta), gstride,
+                                                   ptr(running_mean), ptr(running_var), None, ptr(out), ptr(saved), ptr(ws), _stream()),
+              'b200tts_convblock_forward_masked')
+    return out
 
 
 def conv_block(x, weight, gamma, beta, running_mean, running_var, keep, groups, kernel, dilation, activation, highway,

@@ -11,6 +11,12 @@ def get_activation(name):
     return {'relu': ReLU(), 'sigmoid': Sigmoid(), 'tanh': Tanh(), 'identity': Identity()}[name]
 
 
+def _require_eval(block):
+    """The length-masked block normalises with the running statistics and applies no dropout: it exists for eval mode only."""
+    if block.training:
+        raise RuntimeError('conv block: per-sample lengths (a zero-padded batch) are supported in eval mode only; call .eval() first')
+
+
 class ZoneoutLSTMCell(torch.nn.LSTMCell):
     """LSTM cell with zoneout (layers.py:18-34).  Inside `Decoder` the recurrence runs in the fused decoder op, which reads the
     parameters and `zoneout_h` / `zoneout_c` from here; the standalone `forward` is one library cell step (with autograd)."""
@@ -80,7 +86,14 @@ class ConvBlock(torch.nn.Module):
             bn.num_batches_tracked += 1
         return out
 
-    def forward(self, x):
+    def forward(self, x, lengths=None):
+        """lengths (eval only): per-sample lengths of a zero-padded batch; outputs past each length are 0."""
+        if lengths is not None:
+            _require_eval(self)
+            conv, bn = self._block[1], self._block[2]
+            return F.conv_block_masked(x, lengths, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, self._groups,
+                                       self._kernel, self._dilation, self._activation_name, self._highway, bn.eps,
+                                       conv.weight.shape[0] // self._groups)
         return self._run(x)
 
 
@@ -113,13 +126,19 @@ class ConvBlockGenerated(torch.nn.Module):
         self._mask_key = None
         self._highway = False
 
-    def forward(self, x):
+    def forward(self, x, lengths=None):
+        """lengths (eval only): per-sample lengths of a zero-padded batch; outputs past each length are 0."""
+        if lengths is not None:
+            _require_eval(self)
         e, x = x
         bn = self._regularizer
         G = self._groups
         kernel = self._convolution.generate(e)                 # [G*Cout, Cin, k]
         affine = bn.generate(e)                                # [G, 2*Cout]
         cout = kernel.shape[0] // G
+        if lengths is not None:
+            return e, F.conv_block_masked(x, lengths, kernel, affine[:, :cout], affine[:, cout:], bn.running_mean, bn.running_var, G,
+                                          self._kernel, self._dilation, self._activation_name, self._highway, bn._eps, 2 * cout)
         keep = None
         if self.training and self._dropout_rate > 0.0:
             keep = MaskSource.keep_mask(self._mask_key, (x.shape[0], kernel.shape[0], x.shape[2]), self._dropout_rate, x.device)

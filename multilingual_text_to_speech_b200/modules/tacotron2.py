@@ -56,7 +56,14 @@ class Postnet(torch.nn.Module):
             block._mask_key = f'post{j}'
         self._convs = Sequential(*blocks)
 
-    def forward(self, x, x_lengths):
+    def forward(self, x, x_lengths, padded=False):
+        """padded (eval only): every frame of x at or after x_lengths[b] is 0, and so is every block output there."""
+        if padded:
+            lengths = x_lengths.to(device=x.device, dtype=torch.int32)
+            y = x.contiguous()
+            for block in self._convs:
+                y = block(y, lengths)
+            return y + x
         return self._convs(x.contiguous()) + x
 
 
@@ -177,10 +184,30 @@ class Decoder(torch.nn.Module):
             encoded_input = self._add_conditional_embedding(encoded_input, self._language_embedding, language)
         return encoded_input
 
-    def _decode_inference(self, encoded_input, mask, speaker, language):
+    @staticmethod
+    def _tape_part(tape, done, frames, columns):
+        """Rows [done, done + frames) of a recorded step-prenet tape [T, B_tape, P], restricted to the utterances' tape columns.  A tape
+        ends where the reference's loop stopped; frames decoded past it get all-ones rows and are discarded by the stop rule."""
+        part = tape[done:done + frames]
+        if list(columns) != list(range(tape.shape[1])):
+            part = part[:, list(columns)]
+        if part.shape[0] < frames:
+            part = torch.cat([part, torch.ones(frames - part.shape[0], len(columns), tape.shape[2], dtype=part.dtype, device=part.device)])
+        return part
+
+    @staticmethod
+    def _retire(rows, rules):
+        """Positions (into `rows`, the original indices of the utterances still decoding) of the utterances whose stop cut is unknown."""
+        return [j for j, r in enumerate(rows) if rules[r].cut is None]
+
+    def _decode_inference(self, encoded_input, mask, speaker, language, att_extent=0, tape_columns=None):
         """Free-running decode in chunks with carried state and early exit (tacotron2.py:148-209 with target=None): every chunk is one
         library call; between chunks the stop rule reads the chunk's stop logits.  B == 1 reproduces the reference; B > 1 (which the
-        reference cannot run: it uses the stop token as a Python bool) stops once every utterance has finished."""
+        reference cannot run: it uses the stop token as a Python bool) keeps one stop rule per utterance, and an utterance whose cut is
+        known leaves the decode: the state, memory, lengths and rules are compacted to the utterances still running, and the next
+        chunk runs at the smaller batch.  `att_extent` = 1 runs forward attention over each utterance's own length; `tape_columns`
+        gives each utterance's column of a recorded mask tape (default: column b for utterance b).
+        -> (spectrogram [B, T', N], stop [B, T'], alignment [B, T', L], cuts): T' = max(cuts); utterance b is zero past cuts[b]."""
         memory = self._memory(encoded_input, speaker, language)
         B, L, M = memory.shape
         device = memory.device
@@ -189,7 +216,9 @@ class Decoder(torch.nn.Module):
         lengths = mask.sum(dim=1).to(torch.int32)
         state = F.DecoderState(B, D, M, L, N, device)
         rules = [self._StopRule(hp.stop_frames) for _ in range(B)]
-        specs, stops, aligns = [], [], []
+        rows = list(range(B))                  # original index of every utterance still decoding
+        columns = list(range(B)) if tape_columns is None else list(tape_columns)
+        outs = [[] for _ in range(B)]
         done = 0
         params = self._param_list()
         while done < self._max_frames:
@@ -199,36 +228,48 @@ class Decoder(torch.nn.Module):
                 tape = MaskSource.raw(name)
                 if MaskSource.tape is not None:
                     if tape is not None:
-                        # a recorded tape ends where the reference's loop stopped; frames decoded past it are discarded by the stop rule
-                        part = tape[done:done + Tc].to(device=device, dtype=torch.uint8)
-                        if part.shape[0] < Tc:
-                            part = torch.cat([part, torch.ones(Tc - part.shape[0], B, P, dtype=torch.uint8, device=device)])
-                        masks[name] = part.contiguous()
+                        masks[name] = self._tape_part(tape, done, Tc, [columns[r] for r in rows]).to(device=device, dtype=torch.uint8).contiguous()
                 else:
-                    m = MaskSource.keep_mask(name, (Tc, B, P), self._prenet._dropout_rate, device)
+                    m = MaskSource.keep_mask(name, (Tc, len(rows), P), self._prenet._dropout_rate, device)
                     if m is not None:
                         masks[name] = m
             if self.training:
                 for name in ('att_h', 'gen_h') + (('att_c', 'gen_c') if kind == _lib.CELL_ZONEOUT else ()):
-                    m = MaskSource.keep_mask(name, (Tc, B, D), rate_c if name.endswith('_c') else rate_h, device)
+                    m = MaskSource.keep_mask(name, (Tc, len(rows), D), rate_c if name.endswith('_c') else rate_h, device)
                     if m is not None:
                         masks[name] = m
-            cfg = F.DecoderConfig(kind, self.training, rate_h, rate_c, self._prenet._dropout_rate, masks, np.zeros(Tc, dtype=np.uint8))
+            cfg = F.DecoderConfig(kind, self.training, rate_h, rate_c, self._prenet._dropout_rate, masks, np.zeros(Tc, dtype=np.uint8),
+                                  att_extent)
             spec, stop, align = F.decoder_forward_chunk(cfg, memory, lengths, params, state, Tc)
-            specs.append(spec); stops.append(stop); aligns.append(align)
             done += Tc
             host_stop = stop.float().cpu()
-            cuts = [rule.feed(host_stop[b]) for b, rule in enumerate(rules)]
-            if all(c is not None for c in cuts):
+            for j, r in enumerate(rows):
+                rules[r].feed(host_stop[j])
+                outs[r].append((spec[j], stop[j], align[j]))
+            keep = self._retire(rows, rules)
+            if not keep:
                 break
-        spectrogram, stop, alignment = torch.cat(specs, 1), torch.cat(stops, 1), torch.cat(aligns, 1)
+            if len(keep) < len(rows):
+                idx = torch.tensor(keep, device=device)
+                state.select(idx)
+                memory, lengths = memory.index_select(0, idx), lengths.index_select(0, idx)
+                rows = [rows[j] for j in keep]
         cuts = [r.cut if r.cut is not None else done for r in rules]
-        cut = max(cuts)
-        return spectrogram[:, :cut], stop[:, :cut], alignment[:, :cut]
+        if B == 1:
+            spectrogram, stop, alignment = (torch.cat([o[k] for o in outs[0]], 0)[:cuts[0]].unsqueeze(0) for k in range(3))
+            return spectrogram, stop, alignment, cuts
+        T = max(cuts)
+        spectrogram = torch.zeros(B, T, N, device=device)
+        stop = torch.zeros(B, T, device=device)
+        alignment = torch.zeros(B, T, L, device=device)
+        for b in range(B):
+            for k, dst in enumerate((spectrogram, stop, alignment)):
+                dst[b, :cuts[b]] = torch.cat([o[k] for o in outs[b]], 0)[:cuts[b]]
+        return spectrogram, stop, alignment, cuts
 
     def _decode(self, encoded_input, mask, target, teacher_forcing_ratio, speaker, language):
         if target is None:
-            return self._decode_inference(encoded_input, mask, speaker, language)
+            return self._decode_inference(encoded_input, mask, speaker, language)[:3]
         encoded_input = self._memory(encoded_input, speaker, language)
         B, T = encoded_input.shape[0], target.shape[2]
         device = encoded_input.device
@@ -349,20 +390,102 @@ class Tacotron(torch.nn.Module):
 
     def inference(self, text, speaker=None, language=None):
         """synthesize.py entry point (tacotron2.py:387-408): text int64 [L], speaker int64 [1] | None, language int64 [1] |
-        float [1, L, G] (per-character language mixing) | None -> post-net spectrogram [num_mels, T']."""
-        text = text.unsqueeze(0)                     # pretend having a batch of size 1
-        if speaker is not None and speaker.dim() == 1:
-            speaker = speaker.unsqueeze(1).expand((-1, text.size(1)))
-        if language is not None and language.dim() == 1:
-            language = language.unsqueeze(1).expand((-1, text.size(1)))
+        float [1, L, G] (per-character language mixing) | None -> post-net spectrogram [num_mels, T'].  The one-utterance case of
+        `inference_batch`."""
+        return self.inference_batch([text], None if speaker is None else [speaker], None if language is None else [language])[0]
+
+    def inference_batch(self, texts, speakers=None, languages=None, max_batch=64):
+        """Synthesise many utterances at once: texts is a list of int64 [L_i]; speakers / languages are None or lists with one entry per
+        text in the forms `inference` takes (speaker int64 [1]; language int64 [1] or float [1, L_i, G]).  -> one post-net spectrogram
+        [num_mels, T_i] per text, in input order.  Texts are sorted by length and decoded in padded groups of at most max_batch (eval
+        mode, no grad); each utterance's output equals `inference` of it alone given the same prenet dropout masks (a recorded tape,
+        [T, len(texts), P] with one column per text).  Without a tape a batched run draws other masks than single runs do."""
+        speakers, languages = _check_batch_inputs(texts, speakers, languages)
+        was_training = self.training
+        self.eval()
+        outputs = [None] * len(texts)
+        try:
+            with torch.no_grad():
+                for group in _batch_plan([int(t.shape[0]) for t in texts], max_batch):
+                    posts = self._inference_group([texts[i] for i in group], None if speakers is None else [speakers[i] for i in group],
+                                                  None if languages is None else [languages[i] for i in group], group)
+                    for i, post in zip(group, posts):
+                        outputs[i] = post
+        finally:
+            self.train(was_training)
+        return outputs
+
+    def _inference_group(self, texts, speakers, languages, tape_columns):
+        device = self._embedding.weight.device
+        B, Lmax = len(texts), max(int(t.shape[0]) for t in texts)
+        lengths = torch.tensor([int(t.shape[0]) for t in texts], device=device)
+        text = torch.zeros(B, Lmax, dtype=torch.long, device=device)
+        for b, t in enumerate(texts):
+            text[b, :t.shape[0]] = t.to(device)
+        speaker = language = None
+        if speakers is not None:
+            speaker = torch.cat([s.reshape(1).to(device) for s in speakers]).unsqueeze(1).expand(-1, Lmax)
+        if languages is not None:
+            if languages[0].dim() == 1:
+                language = torch.cat([g.reshape(1).to(device) for g in languages]).unsqueeze(1).expand(-1, Lmax)
+            else:
+                language = torch.zeros(B, Lmax, languages[0].shape[2], device=device)
+                for b, g in enumerate(languages):
+                    language[b, :g.shape[1]] = g[0].to(device=device, dtype=torch.float32)
+        # padded characters embed to 0 (the padding row of the table is not zero: xavier_uniform_ ran after padding_idx was set)
         embedded = F.embedding(self._embedding.weight, text, padding_idx=0)
-        encoded = self._encoder(embedded, torch.LongTensor([text.size(1)]).to(text.device), language)
+        embedded = embedded.masked_fill(~lengths_to_mask(lengths, Lmax).unsqueeze(2), 0.0)
+        encoded = self._encoder(embedded, lengths, language, padded=True)
         if language is not None and language.dim() == 3:
             language = torch.argmax(language, dim=2)  # one-hot into indices for the decoder's language embedding
-        prediction = self._decoder.inference(encoded, speaker, language)
-        prediction = prediction.transpose(1, 2)
-        post_prediction = self._postnet(prediction, torch.LongTensor([prediction.size(2)]))
-        return post_prediction.squeeze(0)
+        mask = lengths_to_mask(lengths, Lmax)
+        prediction, _, _, cuts = self._decoder._decode_inference(encoded, mask, speaker, language, att_extent=1, tape_columns=tape_columns)
+        post = self._postnet(prediction.transpose(1, 2), torch.tensor(cuts, device=device), padded=True)
+        return [post[b, :, :cuts[b]] for b in range(B)]
+
+
+def _check_batch_inputs(texts, speakers, languages):
+    """Validate the per-utterance arguments of Tacotron.inference_batch -> (speakers, languages) as lists or None."""
+    texts = list(texts)
+    if not texts:
+        raise ValueError('inference_batch: no texts given')
+    for t in texts:
+        if not torch.is_tensor(t) or t.dim() != 1 or t.shape[0] < 1 or t.dtype != torch.int64:
+            raise ValueError('inference_batch: every text must be a non-empty int64 tensor [L]')
+    out = []
+    for name, items in (('speakers', speakers), ('languages', languages)):
+        if items is not None:
+            items = list(items)
+            if len(items) != len(texts):
+                raise ValueError(f'inference_batch: {len(items)} {name} for {len(texts)} texts')
+            if any(x is None for x in items):
+                raise ValueError(f'inference_batch: {name} must be given for every text or for none')
+        out.append(items)
+    speakers, languages = out
+    if speakers is not None and any(s.numel() != 1 or s.dtype != torch.int64 for s in speakers):
+        raise ValueError('inference_batch: a speaker is an int64 tensor [1]')
+    if speakers is None and hp.multi_speaker and hp.speaker_embedding_dimension > 0:
+        raise ValueError('inference_batch: a multi-speaker model needs one speaker per text')
+    if languages is not None:
+        forms = {'index' if g.dim() == 1 else 'mix' for g in languages}
+        if len(forms) > 1:
+            raise ValueError('inference_batch: languages mix int64 [1] ids and float [1, L, G] weights; use one form for all texts')
+        for t, g in zip(texts, languages):
+            if g.dim() == 1:
+                if g.numel() != 1 or g.dtype != torch.int64:
+                    raise ValueError('inference_batch: a language id is an int64 tensor [1]')
+            elif g.dim() != 3 or g.shape[0] != 1 or g.shape[1] != t.shape[0] or not g.is_floating_point() \
+                    or g.shape[2] != languages[0].shape[2]:
+                raise ValueError('inference_batch: per-character language weights are float [1, L, G] with L the text length')
+    return speakers, languages
+
+
+def _batch_plan(lengths, max_batch):
+    """Utterance indices sorted by text length (stable), cut into consecutive groups of at most max_batch."""
+    if int(max_batch) < 1:
+        raise ValueError(f'inference_batch: max_batch must be >= 1 (got {max_batch})')
+    order = sorted(range(len(lengths)), key=lambda i: lengths[i])
+    return [order[k:k + max_batch] for k in range(0, len(order), max_batch)]
 
 
 class TacotronLoss(torch.nn.Module):
