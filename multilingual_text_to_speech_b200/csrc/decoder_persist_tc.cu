@@ -30,6 +30,10 @@ namespace {
 constexpr int NCW = 8;                  // compute warps
 constexpr int CT = 32 * NCW;            // compute threads
 constexpr int PT = CT + 128;            // + the MMA warpgroup (warps 8-11)
+// per-thread registers after the role split (setmaxnreg): 128 R_MMA + CT R_CMP <= 64512 (= PT x 168, what the launch allocates)
+constexpr int R_MMA = 56;
+constexpr int R_CMP = 224;
+static_assert(128 * R_MMA + CT * R_CMP <= PT * 168 && R_MMA % 8 == 0 && R_CMP % 8 == 0, "register split exceeds the CTA's allocation");
 constexpr int UNITS = 16;               // hidden units per CTA
 constexpr int ROWS = 4 * UNITS;         // gate rows per CTA (MMA M)
 constexpr int BT = 32;                  // utterances per CTA (MMA N)
@@ -74,6 +78,9 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
+// Out of line on purpose: an inlined trap makes ptxas drop the setmaxnreg.inc limit of the code around it back to the launch's 168
+// registers (measured with -Xptxas -v: the compute warps then spill), a call to this function does not.
+__device__ __noinline__ __attribute__((noreturn)) void watchdog_trap() { __trap(); }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     const uint32_t addr = smem_u32(bar);
     const long long t0 = clock64();
@@ -87,7 +94,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
             : "r"(addr), "r"(parity)
             : "memory");
         if (done) return;
-        if (clock64() - t0 > 4000000000ll) __trap();       // ~2 s: a protocol bug must not hang the GPU
+        if (clock64() - t0 > 4000000000ll) watchdog_trap();       // ~2 s: a protocol bug must not hang the GPU
     }
 }
 __device__ __forceinline__ void tma_load_3d(void* smem, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
@@ -122,6 +129,12 @@ __device__ __forceinline__ void st_async_peer_f32(const float* local_smem, const
 }
 // named barrier among the compute warps only
 __device__ __forceinline__ void csync() { asm volatile("bar.sync 1, %0;" ::"n"(CT) : "memory"); }
+// per-thread register limit of the executing warpgroup (all its warps execute it): dec returns registers to the CTA's pool, inc waits until
+// the pool holds enough
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 __device__ __forceinline__ void ldmatrix_x4(uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3, const void* p) {
     const uint32_t addr = (uint32_t)__cvta_generic_to_shared(p);
@@ -208,6 +221,15 @@ __device__ __forceinline__ bool grid_barrier(unsigned* counter, unsigned& target
     __syncthreads();
     return *s_ok != 0;
 }
+// The MMA warpgroup's side of grid_barrier: it arrives at the same two CTA-wide barriers from its own loop, in the same order, and leaves
+// the arrival and the polling to thread 0.  Staying in the CTA barrier (instead of waiting on an mbarrier that thread 0 signals) keeps the
+// ordering the single loop had: the TMA issued after the barrier reads other CTAs' rows only after thread 0's acquire fence, and the
+// watchdog verdict s_ok reaches both roles through the same barrier.
+__device__ __forceinline__ bool grid_barrier_mma(const int* s_ok) {
+    __syncthreads();
+    __syncthreads();
+    return *s_ok != 0;
+}
 
 // ALIAS (large memory dims only): the accumulator staging lives in the TMA slot and the ctx part arrives in p.n_c TMA instructions; the
 // common instantiation keeps both compile-time constant (this kernel sits at its register cap: every live value counts)
@@ -231,7 +253,6 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
     // counter is used)
     const unsigned nblocks = gridDim.x;
     unsigned* const bar_counter = p.barrier;
-    const bool compute = warp < NCW;
     const bool is_mma = warp >= NCW;               // the MMA warpgroup; one elected lane of its first warp issues the TMA loads
 
     // ---- shared memory carve-up (1024-byte aligned base: SWIZZLE_128B atoms) ----
@@ -354,10 +375,33 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
         rp[2 * part] += t1 - t0; rp[2 * part + 1] += clock64() - t1;
     };
 
+    // ---- role split: from here on the MMA warpgroup and the compute warps run separate step loops ----
+    // __launch_bounds__(PT, 1) caps every thread at 65536 / PT = 168 registers.  The MMA warpgroup needs far fewer (accumulator fragment,
+    // descriptors, loop state; ptxas ignores a limit of 40); the compute warps run the cell, the query projection, the energies, the
+    // softmax and the context product, whose prefetched fragments spill at 168.  setmaxnreg hands the MMA warpgroup's unused registers to
+    // them.  ptxas allocates up to a raised limit only in code that just one role reaches, so each role has its own step loop; both follow
+    // the same per-step protocol in the same order.
+    if (is_mma) {
+        setmaxnreg_dec<R_MMA>();
+        // prologue: the h part of step 0 (operand row 0 is all zeros)
+        mma_part(0, 1, !ATT || p.nkb_h == p.nkb);
+        for (int i = 0; i < p.T; ++i) {
+            if (ATT && p.nkb_h < p.nkb) mma_part(i, 0, true);     // ctx part: the context of step i-1 is visible now
+            if (ALIAS) proxy_fence_shared();
+            if (!grid_barrier_mma(&s_ok)) break;
+            if (i + 1 < p.T) mma_part(i + 1, 1, !ATT || p.nkb_h == p.nkb);   // h part of step i+1, under the attention of step i
+            if (ATT && !grid_barrier_mma(&s_ok)) break;
+        }
+        if (p.prof2 && warp == NCW && lane == 0)
+            for (int k = 0; k < 4; ++k) p.prof2[(size_t)cta * 8 + k] = rp[k];
+        return;
+    }
+    setmaxnreg_inc<R_CMP>();
+
     // B fragments (k = this CTA's 16 hidden units, n = attention dims of the n-tiles {2 warp, 2 warp + 1}) of the query projection,
     // split into bf16 hi + lo, resident in registers for the whole sequence
     uint32_t wqh[2][2] = {{0u, 0u}, {0u, 0u}}, wql[2][2] = {{0u, 0u}, {0u, 0u}};
-    if (ATT && compute) {
+    if (ATT) {
         const int g = lane >> 2, tq = lane & 3;
 #pragma unroll
         for (int j = 0; j < 2; ++j)
@@ -373,15 +417,21 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
     }
     const float inv_h = 1.f / (1.f - p.rate_h), inv_c = 1.f / (1.f - p.rate_c);
     unsigned target = 0;
-    long long prof_acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    long long prof_t = clock64();
+    // phase cycle sums [0, 8) and the last mark [8] of thread 0.  The attention loop keeps them in shared memory: in registers they would
+    // hold 18 registers of every compute thread for the whole loop.  The generator loop has registers to spare, and thread 0 (which also
+    // arrives at the grid barrier) keeps them in registers there: with the shared-memory round trips that loop measured slower.
+    __shared__ long long prof_sm[9];
+    long long prof_rg[9];
+    long long* const prof_acc = ATT ? prof_sm : prof_rg;
+    if (tid == 0) {
+        for (int k = 0; k < 8; ++k) prof_acc[k] = 0;
+        prof_acc[8] = clock64();
+    }
 #define PROF_MARK(slot)                                                      \
     do {                                                                     \
-        if (p.prof && tid == 0) { const long long now = clock64(); prof_acc[slot] += now - prof_t; prof_t = now; } \
+        if (p.prof && tid == 0) { const long long now = clock64(); prof_acc[slot] += now - prof_acc[8]; prof_acc[8] = now; } \
     } while (0)
 
-    // prologue: the h part of step 0 (operand row 0 is all zeros)
-    if (is_mma) mma_part(0, 1, !ATT || p.nkb_h == p.nkb);
 
     // Epilogue operands of this thread's two (b, u) pairs.  The input-projection gates and the keep masks of step i+1 are fetched
     // (from DRAM) right after the cell barrier of step i, i.e. a whole attention phase ahead; c and the regularised h are carried
@@ -425,91 +475,88 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
             }
         }
     };
-    if (compute) { prefetch_l2(0); prefetch(0, true); prefetch_l2(1); }
+    prefetch_l2(0); prefetch(0, true); prefetch_l2(1);
 
     int att_len = 0;               // ATT: clamped text length of the utterance this CTA pair serves
     if (ATT && (cta >> 1) < B) { const int l0 = p.lengths[cta >> 1]; att_len = l0 < 0 ? 0 : (l0 > p.L ? p.L : l0); }
     bool alive = true;
     for (int i = 0; i < p.T && alive; ++i) {
-        // =================== ctx part of the gate product (the context of step i-1 is visible now) ===================
-        if (ATT && p.nkb_h < p.nkb && is_mma) mma_part(i, 0, true);
-        if (compute) {
-            // accumulator [64 gate rows x 32 utterances] staged by the MMA warpgroup: s_sum[utterance][gate * 16 + unit]
-            mbar_wait(&accum_bar, i & 1);
-            PROF_MARK(0);
-            // =================== LSTM cell + regulariser (2 (b, u) pairs per thread) ===================
+        // =================== the ctx part of the gate product (MMA warpgroup) is staged once the context of step i-1 is visible ===================
+        // accumulator [64 gate rows x 32 utterances] staged by the MMA warpgroup: s_sum[utterance][gate * 16 + unit]
+        mbar_wait(&accum_bar, i & 1);
+        PROF_MARK(0);
+        // =================== LSTM cell + regulariser (2 (b, u) pairs per thread) ===================
 #pragma unroll
-            for (int e2 = 0; e2 < 2; ++e2) {
-                const int idx = tid + e2 * CT;
-                const int bl = idx / UNITS, uu = idx % UNITS, b = b0 + bl, u = u0 + uu;
-                float hs = 0.f;
-                if (b < B && u < D) {
-                    const size_t g0 = ((size_t)i * B + b) * 4 * D + u;
-                    const float zi = pre[e2][0] + s_sum[bl * (ROWS + 1) + uu];
-                    const float zf = pre[e2][1] + s_sum[bl * (ROWS + 1) + UNITS + uu];
-                    const float zg = pre[e2][2] + s_sum[bl * (ROWS + 1) + 2 * UNITS + uu];
-                    const float zo = pre[e2][3] + s_sum[bl * (ROWS + 1) + 3 * UNITS + uu];
-                    const float gi = sigmoid_fast(zi), gf = sigmoid_fast(zf), gg = tanh_exp(zg), go = sigmoid_fast(zo);
-                    const size_t bu = (size_t)b * D + u;
-                    const float cp = pre[e2][4];
-                    float cn = gf * cp + gi * gg;
-                    float hn = go * tanh_exp(cn);
-                    p.gates[g0] = gi; p.gates[g0 + D] = gf; p.gates[g0 + 2 * D] = gg; p.gates[g0 + 3 * D] = go;
-                    if (p.kind == B200TTS_CELL_ZONEOUT) {
-                        const float hp = pre[e2][5];
-                        if (p.training) {
-                            float dh = hn - hp, dc = cn - cp;
-                            if (p.mask_h) dh = dh * (float)pm[e2][0] * inv_h;
-                            if (p.mask_c) dc = dc * (float)pm[e2][1] * inv_c;
-                            hn = (1.f - p.rate_h) * dh + hp;
-                            cn = (1.f - p.rate_c) * dc + cp;
-                        } else {
-                            hn = p.rate_h * hp + (1.f - p.rate_h) * hn;
-                            cn = p.rate_c * cp + (1.f - p.rate_c) * cn;
-                        }
-                    } else if (p.training && p.mask_h) {
-                        hn = hn * (float)pm[e2][0] * inv_h;
+        for (int e2 = 0; e2 < 2; ++e2) {
+            const int idx = tid + e2 * CT;
+            const int bl = idx / UNITS, uu = idx % UNITS, b = b0 + bl, u = u0 + uu;
+            float hs = 0.f;
+            if (b < B && u < D) {
+                const size_t g0 = ((size_t)i * B + b) * 4 * D + u;
+                const float zi = pre[e2][0] + s_sum[bl * (ROWS + 1) + uu];
+                const float zf = pre[e2][1] + s_sum[bl * (ROWS + 1) + UNITS + uu];
+                const float zg = pre[e2][2] + s_sum[bl * (ROWS + 1) + 2 * UNITS + uu];
+                const float zo = pre[e2][3] + s_sum[bl * (ROWS + 1) + 3 * UNITS + uu];
+                const float gi = sigmoid_fast(zi), gf = sigmoid_fast(zf), gg = tanh_exp(zg), go = sigmoid_fast(zo);
+                const size_t bu = (size_t)b * D + u;
+                const float cp = pre[e2][4];
+                float cn = gf * cp + gi * gg;
+                float hn = go * tanh_exp(cn);
+                p.gates[g0] = gi; p.gates[g0 + D] = gf; p.gates[g0 + 2 * D] = gg; p.gates[g0 + 3 * D] = go;
+                if (p.kind == B200TTS_CELL_ZONEOUT) {
+                    const float hp = pre[e2][5];
+                    if (p.training) {
+                        float dh = hn - hp, dc = cn - cp;
+                        if (p.mask_h) dh = dh * (float)pm[e2][0] * inv_h;
+                        if (p.mask_c) dc = dc * (float)pm[e2][1] * inv_c;
+                        hn = (1.f - p.rate_h) * dh + hp;
+                        cn = (1.f - p.rate_c) * dc + cp;
+                    } else {
+                        hn = p.rate_h * hp + (1.f - p.rate_h) * hn;
+                        cn = p.rate_c * cp + (1.f - p.rate_c) * cn;
                     }
-                    p.cstate[(size_t)(i + 1) * B * D + bu] = cn;
-                    p.actf[((size_t)(i + 1) * B + b) * p.ldf + p.hcol + u] = hn;
-                    p.actb[((size_t)(i + 1) * B + b) * Kp + u] = __float2bfloat16_rn(hn);
-                    hs = hn;
-                    pre[e2][4] = cn; pre[e2][5] = hn;           // state of the next step
+                } else if (p.training && p.mask_h) {
+                    hn = hn * (float)pm[e2][0] * inv_h;
                 }
-                if (ATT) s_hs[uu * (BT + 4) + bl] = hs;
+                p.cstate[(size_t)(i + 1) * B * D + bu] = cn;
+                p.actf[((size_t)(i + 1) * B + b) * p.ldf + p.hcol + u] = hn;
+                p.actb[((size_t)(i + 1) * B + b) * Kp + u] = __float2bfloat16_rn(hn);
+                hs = hn;
+                pre[e2][4] = cn; pre[e2][5] = hn;           // state of the next step
             }
-            if (ATT) {
-                csync();
-                // partial query projection of this CTA's 16 hidden units on the tensor cores: qpart[rb, b, a] = sum_u h[b, u] Wq[a, u].
-                // h and Wq are split into bf16 hi + lo and three products are summed (hi.hi + lo.hi + hi.lo), i.e. fp32-equivalent.
-                {
-                    const int g = lane >> 2, tq = lane & 3;
-                    uint32_t ah[2][4], al[2][4];
+            if (ATT) s_hs[uu * (BT + 4) + bl] = hs;
+        }
+        if (ATT) {
+            csync();
+            // partial query projection of this CTA's 16 hidden units on the tensor cores: qpart[rb, b, a] = sum_u h[b, u] Wq[a, u].
+            // h and Wq are split into bf16 hi + lo and three products are summed (hi.hi + lo.hi + hi.lo), i.e. fp32-equivalent.
+            {
+                const int g = lane >> 2, tq = lane & 3;
+                uint32_t ah[2][4], al[2][4];
 #pragma unroll
-                    for (int mt = 0; mt < 2; ++mt)
+                for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-                        for (int r4 = 0; r4 < 4; ++r4) {
-                            const int bl = mt * 16 + g + 8 * (r4 & 1), k = 2 * tq + 8 * (r4 >> 1);
-                            const float x0 = s_hs[k * (BT + 4) + bl], x1 = s_hs[(k + 1) * (BT + 4) + bl];
-                            const __nv_bfloat16 h0 = __float2bfloat16_rn(x0), h1 = __float2bfloat16_rn(x1);
-                            __nv_bfloat162 hp2; hp2.x = h0; hp2.y = h1;
-                            ah[mt][r4] = *reinterpret_cast<uint32_t*>(&hp2);
-                            al[mt][r4] = pack2(x0 - __bfloat162float(h0), x1 - __bfloat162float(h1));
-                        }
+                    for (int r4 = 0; r4 < 4; ++r4) {
+                        const int bl = mt * 16 + g + 8 * (r4 & 1), k = 2 * tq + 8 * (r4 >> 1);
+                        const float x0 = s_hs[k * (BT + 4) + bl], x1 = s_hs[(k + 1) * (BT + 4) + bl];
+                        const __nv_bfloat16 h0 = __float2bfloat16_rn(x0), h1 = __float2bfloat16_rn(x1);
+                        __nv_bfloat162 hp2; hp2.x = h0; hp2.y = h1;
+                        ah[mt][r4] = *reinterpret_cast<uint32_t*>(&hp2);
+                        al[mt][r4] = pack2(x0 - __bfloat162float(h0), x1 - __bfloat162float(h1));
+                    }
 #pragma unroll
-                    for (int mt = 0; mt < 2; ++mt)
+                for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-                        for (int j = 0; j < 2; ++j) {
-                            float acc[4] = {0.f, 0.f, 0.f, 0.f};
-                            mma_bf16(acc, ah[mt], wqh[j][0], wqh[j][1]);
-                            mma_bf16(acc, al[mt], wqh[j][0], wqh[j][1]);
-                            mma_bf16(acc, ah[mt], wql[j][0], wql[j][1]);
-                            const int a = (2 * warp + j) * 8 + 2 * tq;
-                            const int bA = b0 + mt * 16 + g, bB = bA + 8;
-                            if (bA < B) *reinterpret_cast<float2*>(p.qpart + ((size_t)rb * B + bA) * p.A + a) = make_float2(acc[0], acc[1]);
-                            if (bB < B) *reinterpret_cast<float2*>(p.qpart + ((size_t)rb * B + bB) * p.A + a) = make_float2(acc[2], acc[3]);
-                        }
-                }
+                    for (int j = 0; j < 2; ++j) {
+                        float acc[4] = {0.f, 0.f, 0.f, 0.f};
+                        mma_bf16(acc, ah[mt], wqh[j][0], wqh[j][1]);
+                        mma_bf16(acc, al[mt], wqh[j][0], wqh[j][1]);
+                        mma_bf16(acc, ah[mt], wql[j][0], wql[j][1]);
+                        const int a = (2 * warp + j) * 8 + 2 * tq;
+                        const int bA = b0 + mt * 16 + g, bB = bA + 8;
+                        if (bA < B) *reinterpret_cast<float2*>(p.qpart + ((size_t)rb * B + bA) * p.A + a) = make_float2(acc[0], acc[1]);
+                        if (bB < B) *reinterpret_cast<float2*>(p.qpart + ((size_t)rb * B + bB) * p.A + a) = make_float2(acc[2], acc[3]);
+                    }
             }
         }
         PROF_MARK(1);
@@ -517,18 +564,15 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
         if (!grid_barrier(bar_counter, target, nblocks, p.abort_flag, &s_ok)) { alive = false; break; }
         PROF_MARK(2);
 
-        // =================== h part of step i+1: TMA + wgmma run while the attention of step i is computed ===================
-        if (i + 1 < p.T) {
-            if (is_mma) mma_part(i + 1, 1, !ATT || p.nkb_h == p.nkb);
-            if (compute) { prefetch_l2(i + 2); if (!ATT) prefetch(i + 1, false); }
-        }
+        // =================== h part of step i+1 (MMA warpgroup): TMA + wgmma run while the attention of step i is computed ===================
+        if (i + 1 < p.T) { prefetch_l2(i + 2); if (!ATT) prefetch(i + 1, false); }
 
         if (ATT) {
             // =================== attention: one CTA PAIR (cluster of 2) per utterance ===================
             // pair pc = cta >> 1 serves utterance pc; rank hf = cta & 1 owns the attention dims [64 hf, 64 hf + 64) of the energies
             // (partial sums exchanged through distributed shared memory, one cluster barrier) and one half of the context tiles.
             const int pc = cta >> 1, hf = cta & 1;
-            if (compute && pc < B) {
+            if (pc < B) {
                 const int b = pc, L = p.L, A = p.A, AH = p.A / 2, M = p.M, half = (p.KC - 1) / 2, L16 = p.MT * 16;
                 float* qb = scratch;                       // [AH]  query + bias of this rank's attention dims
                 float* vv = qb + AH;                       // [AH]  persistent: energy vector
@@ -782,7 +826,7 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
             }
             PROF_MARK(6);
             // next step's epilogue operands (L2 hits: prefetched a step ago) are requested between the arrival and the wait
-            if (!grid_barrier(bar_counter, target, nblocks, p.abort_flag, &s_ok, [&]() { if (compute && i + 1 < p.T) prefetch(i + 1, false); })) {
+            if (!grid_barrier(bar_counter, target, nblocks, p.abort_flag, &s_ok, [&]() { if (i + 1 < p.T) prefetch(i + 1, false); })) {
                 alive = false; break;
             }
             PROF_MARK(7);
@@ -791,8 +835,6 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
     if (p.prof && tid == 0)
         for (int k = 0; k < 8; ++k) p.prof[(size_t)cta * 8 + k] = prof_acc[k];
 #undef PROF_MARK
-    if (p.prof2 && warp == NCW && lane == 0)
-        for (int k = 0; k < 4; ++k) p.prof2[(size_t)cta * 8 + k] = rp[k];
 }
 
 // shared memory of one loop CTA with a ring slot of slot_kb k-blocks; alias: the accumulator staging shares the slot
