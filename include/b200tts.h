@@ -130,8 +130,8 @@ typedef struct {
     /* keep masks, NULL = no dropout at that site.  Time-major: row i belongs to decoder step i. */
     const uint8_t* mask_prenet0;  /* [T, B, P] */
     const uint8_t* mask_prenet1;  /* [T, B, P] */
-    const uint8_t* mask_att_h;    /* [T, B, D] */
-    const uint8_t* mask_att_c;    /* [T, B, D] zoneout only */
+    const uint8_t* mask_att_h;    /* [T, B, D]; 8-byte aligned on the persistent attention reverse loop */
+    const uint8_t* mask_att_c;    /* [T, B, D] zoneout only; 8-byte aligned there too */
     const uint8_t* mask_gen_h;    /* [T, B, D] */
     const uint8_t* mask_gen_c;    /* [T, B, D] zoneout only */
     const uint8_t* mask_step_prenet0; /* [T, B, P] prenet masks of free-running steps */

@@ -71,6 +71,15 @@ __device__ __forceinline__ bool grid_barrier(unsigned* counter, unsigned& target
 }
 
 __device__ __forceinline__ void l2_prefetch(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
+// asynchronous global -> shared copies: 16 bytes bypassing L1 (.cg; also right for data other CTAs wrote during the launch), and 8 bytes.
+// The thread that issued them waits with cp_async_wait_all; a CTA barrier after that wait makes them visible to the other threads
+__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem) : "memory");
+}
+__device__ __forceinline__ void cp_async8(void* smem, const void* gmem) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 // remote store that completes its 4 bytes on the PEER's mbarrier (data + signal in one instruction): the pair exchanges need no cluster
 // barrier and none of the memory fence its release semantics imply
 __device__ __forceinline__ void st_async_peer_f32(const float* local_smem, const uint64_t* local_bar, uint32_t peer_rank, float v) {
@@ -164,6 +173,11 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
     float* dcum = reinterpret_cast<float*>(sWcB2 + (size_t)32 * (A + 8));            // [L16 + 32] persistent d cum
     uint4* wqf = reinterpret_cast<uint4*>(dcum + (p.MT * 16 + 32));                  // [A / 16][32 lanes] Wq B fragments of this CTA's 8 units
     float* s_dhq = reinterpret_cast<float*>(wqf + (size_t)(A / 16) * 32);            // [2 halves of A][64][8] query part of d h
+    // cell-backward staging (owner CTAs), [..][B][8 units] each, outside the TMA slot: the operands of the next step are in flight while
+    // P2's TMA refills the slot
+    float* s_pbo = s_dhq + 2 * 64 * 8;                                               // [6][B][8] gates i, f, g, o, c, d h static
+    uint8_t* s_pbm = reinterpret_cast<uint8_t*>(s_pbo + (size_t)6 * B * 8);          // [2][B][8] zoneout / dropout keep bytes h, c
+    float* s_rp = reinterpret_cast<float*>(s_pbm + (size_t)2 * B * 8);               // [KBA][B][8] recurrent partial sums
     const unsigned nblocks = gridDim.x;
     const int L16 = p.MT * 16;
 
@@ -238,27 +252,26 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
     BPROF_DECL
 
     const int pc = cta >> 1;
-    // cell-backward operands of this thread's (b, u) pairs (owner CTAs): fetched a whole reverse step ahead, at the end of the previous
-    // cell phase, so that their DRAM latency never sits on the critical path
-    float gi_[MAXE], gf_[MAXE], gg_[MAXE], go_[MAXE], cp_[MAXE], dhs_[MAXE];
-    uint8_t mh_[MAXE], mc_[MAXE];
-    auto pb_prefetch = [&](int step) {
-#pragma unroll
-        for (int e = 0; e < MAXE; ++e) {
-            const int idx = tid + e * PT;
-            gi_[e] = gf_[e] = gg_[e] = go_[e] = cp_[e] = dhs_[e] = 0.f; mh_[e] = 1; mc_[e] = 1;
-            if (owner && idx < B * UOWN && step >= 0) {
-                const int b = idx / UOWN, u = uo0 + idx % UOWN;
-                const size_t bu = (size_t)b * D + u, g0 = ((size_t)step * B + b) * 4 * D + u, mi = (size_t)step * B * D + bu;
-                gi_[e] = p.gates[g0]; gf_[e] = p.gates[g0 + D]; gg_[e] = p.gates[g0 + 2 * D]; go_[e] = p.gates[g0 + 3 * D];
-                cp_[e] = p.cstate[mi];
-                dhs_[e] = p.dh_static[mi];
-                if (p.training && p.mask_h) mh_[e] = p.mask_h[mi];
-                if (p.training && p.mask_c) mc_[e] = p.mask_c[mi];
-            }
+    // cell-backward operands of the owned units x every utterance: copied into s_pbo / s_pbm a whole reverse step ahead, under the grid
+    // barrier that ends the previous cell phase, so that neither their DRAM latency nor registers to hold them sit on the loop.  Each
+    // (utterance, operand) is one 32-byte run of 8 floats (uo0 = 8 cta) and 8 mask bytes; the keep masks are read only when training with
+    // masks, so only then copied
+    auto pb_stage = [&](int step) {
+        if (!owner || step < 0) return;
+        const size_t row = (size_t)step * B;
+        for (int c = tid; c < 12 * B; c += PT) {
+            const int k = c / (2 * B), r = c - k * 2 * B, b = r >> 1, h4 = (r & 1) * 4;
+            const float* src = k < 4 ? p.gates + (row + b) * 4 * D + (size_t)k * D : (k == 4 ? p.cstate : p.dh_static) + (row + b) * D;
+            cp_async16(s_pbo + (k * B + b) * UOWN + h4, src + uo0 + h4);
         }
+        if (p.training)
+            for (int c = tid; c < 2 * B; c += PT) {
+                const int k = c / B, b = c - k * B;
+                const uint8_t* m = k ? p.mask_c : p.mask_h;
+                if (m) cp_async8(s_pbm + (k * B + b) * UOWN, m + (row + b) * D + uo0);
+            }
     };
-    pb_prefetch(p.T - 1);
+    pb_stage(p.T - 1);
     int pa_len = 0;
     if (pc < B) { const int l0 = p.lengths[pc]; pa_len = l0 < 0 ? 0 : (l0 > L ? L : l0); }
     for (int i = p.T - 1; i >= 0; --i) {
@@ -279,7 +292,8 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
             const int len = pa_len;                        // loaded once, before the loop
             const int mtiles = (len + 15) / 16;
             // k-tiles (16 memory dims) per register batch of the dw product.  A batch of all 18 k-tiles at M = 288 (one L2 round trip instead
-            // of three), issued before the staging, was measured slower: the kernel sits at its 255-register cap and spilled in every phase
+            // of three) was measured slower, also with the cell operands staged in shared memory: the kernel sits at its 255-register cap and
+            // spilled in every phase (9 k-tiles as well)
             constexpr int KT = 6;
             {   // Staging of the step's operands.  EVERY global load of the phase is issued before the first dependent instruction: ONE L2
                 // round trip instead of five serial ones (partial d ctx sums, alignment row, query, cumulative weights, d alignment);
@@ -437,7 +451,7 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
                     }
                 }
                 // ds = de[l] * v[a] * (1 - tanh^2(S + q + bias + memT)); fragment-major memory projection: 64 bf16 per lane.  Requesting
-                // these fragments before the Toeplitz MMAs was measured slower (register spills at the 255-register cap)
+                // the first job's fragments before the softmax exchange was measured slower (register spills at the 255-register cap)
                 const uint4* mf = reinterpret_cast<const uint4*>(p.memTf + (((size_t)b * p.MT + mt) * 32 + lane) * 64);
                 const float de0 = s_de[l0 + g], de1 = s_de[l0 + g + 8];
                 uint32_t dsA[16][2];
@@ -536,51 +550,38 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
 
         // =========================== PB: attention-LSTM cell backward ===========================
         if (owner) {
-            // recurrent partial sums of this thread's (b, u) pairs (written by the product of the previous reverse step)
-            // ... requested together with the query gradients of ALL utterances (staged below): one L2 round trip for both.  (The loop
-            // this replaces issued load -> dependent shared-memory store per iteration: eight serial round trips per step.)
+            // the recurrent partial sums of the owned units (written by the product of the previous reverse step) and the query gradients
+            // of ALL utterances go straight to shared memory: one L2 round trip for both, waited for together with this step's operands.
+            // (As is idle between PA and P2: [B][A] query gradients, row b rotated by 8 (b & 7) floats against bank conflicts)
+            float* s_dq = reinterpret_cast<float*>(As);
+            if (!last)
+                for (int c = tid; c < KBA * B * 2; c += PT) {
+                    const int kb2 = c >> 1, h4 = (c & 1) * 4;          // kb2 = k2 * B + b
+                    cp_async16(s_rp + kb2 * UOWN + h4, p.part + (size_t)kb2 * p.NOUT + M + uo0 + h4);
+                }
+            {
+                const float4* dq4 = reinterpret_cast<const float4*>(p.dq + (size_t)i * B * A);      // [B][A] block of this step, contiguous
+                for (int idx = tid; idx < B * 32; idx += PT) {                                       // A == 128 (host check): 32 float4 per utterance
+                    const int b = idx >> 5, c4 = idx & 31;
+                    cp_async16(s_dq + b * A + ((c4 * 4 + 8 * (b & 7)) & (A - 1)), dq4 + idx);
+                }
+            }
+            cp_async_wait_all();
+            __syncthreads();
             float rec_[MAXE];
-            float r8[MAXE][KBA];
 #pragma unroll
             for (int e = 0; e < MAXE; ++e) {
                 const int idx = tid + e * PT;
-#pragma unroll
-                for (int k2 = 0; k2 < KBA; ++k2) r8[e][k2] = 0.f;
+                float rs = 0.f;
                 if (idx < B * UOWN && !last) {
-                    const int b = idx / UOWN, u = uo0 + idx % UOWN;
 #pragma unroll
-                    for (int k2 = 0; k2 < KBA; ++k2) r8[e][k2] = __ldcg(p.part + ((size_t)k2 * B + b) * p.NOUT + M + u);
+                    for (int k2 = 0; k2 < KBA; ++k2) rs += s_rp[k2 * B * UOWN + idx];
                 }
+                rec_[e] = rs;
             }
             // d h (query part) = dq[b, :] . Wq[:, u] on the tensor cores: A = dq rows staged in shared memory (bf16 hi + lo),
             // B = this CTA's 8 columns of Wq (bf16 hi + lo, prebuilt in wqf); hi.hi + lo.hi + hi.lo = fp32-equivalent
-            // (As is idle between PA and P2: [B][A] query gradients, row b rotated by 8 (b & 7) floats against bank conflicts)
-            float* s_dq = reinterpret_cast<float*>(As);
             {
-                constexpr int NQ = 8;                     // float4 per thread: B * A / 4 <= NQ * PT  (A = 128, B <= 64: checked on the host)
-                const float4* dq4 = reinterpret_cast<const float4*>(p.dq + (size_t)i * B * A);      // [B][A] block of this step, contiguous
-                float4 qv[NQ];
-#pragma unroll
-                for (int j = 0; j < NQ; ++j) {
-                    const int idx = tid + j * PT;
-                    if (idx < B * 32) qv[j] = __ldcg(dq4 + idx);         // A == 128 (host check): 32 float4 per utterance
-                }
-#pragma unroll
-                for (int e = 0; e < MAXE; ++e) {
-                    float rs = 0.f;
-#pragma unroll
-                    for (int k2 = 0; k2 < KBA; ++k2) rs += r8[e][k2];
-                    rec_[e] = rs;
-                }
-#pragma unroll
-                for (int j = 0; j < NQ; ++j) {
-                    const int idx = tid + j * PT;
-                    if (idx < B * 32) {
-                        const int b = idx >> 5, c4 = idx & 31;
-                        *reinterpret_cast<float4*>(s_dq + b * A + ((c4 * 4 + 8 * (b & 7)) & (A - 1))) = qv[j];
-                    }
-                }
-                __syncthreads();
                 const int g = lane >> 2, tq = lane & 3, mt = warp & 3, kh = warp >> 2;      // warp = (16-utterance tile, half of the A range)
                 float acc[4] = {0.f, 0.f, 0.f, 0.f};
                 const int ksteps = A / 32;                                // k-steps of 16 per half
@@ -614,27 +615,28 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
                 if (idx < B * UOWN) {
                     const int b = idx / UOWN, uu = idx % UOWN, u = uo0 + uu;
                     const size_t bu = (size_t)b * D + u, g0 = ((size_t)i * B + b) * 4 * D + u;
-                    float dh = dhs_[e] + (s_dhq[b * UOWN + uu] + s_dhq[(64 + b) * UOWN + uu]);
+                    const int BU = B * UOWN;                   // idx = b * UOWN + uu: this pair's slot in each [B][8] staging array
+                    float dh = s_pbo[5 * BU + idx] + (s_dhq[b * UOWN + uu] + s_dhq[(64 + b) * UOWN + uu]);
                     float dc_in = 0.f;
                     if (!last) {
                         dh += rec_[e] + dhz_reg[e];
                         dc_in = dc_reg[e];
                     }
-                    const float gi = gi_[e], gf = gf_[e], gg = gg_[e], go = go_[e];
-                    const float cp = cp_[e];
+                    const float gi = s_pbo[idx], gf = s_pbo[BU + idx], gg = s_pbo[2 * BU + idx], go = s_pbo[3 * BU + idx];
+                    const float cp = s_pbo[4 * BU + idx];
                     const float tc = tanh_exp(gf * cp + gi * gg);
                     float dhn, dcn, dc_prev_direct = 0.f, dh_prev_direct = 0.f;
                     if (p.kind == B200TTS_CELL_ZONEOUT) {
                         float kh, kc;
                         if (p.training) {
-                            kh = (1.f - p.rate_h) * (p.mask_h ? (float)mh_[e] * inv_h : 1.f);
-                            kc = (1.f - p.rate_c) * (p.mask_c ? (float)mc_[e] * inv_c : 1.f);
+                            kh = (1.f - p.rate_h) * (p.mask_h ? (float)s_pbm[idx] * inv_h : 1.f);
+                            kc = (1.f - p.rate_c) * (p.mask_c ? (float)s_pbm[BU + idx] * inv_c : 1.f);
                         } else { kh = 1.f - p.rate_h; kc = 1.f - p.rate_c; }
                         dhn = dh * kh; dh_prev_direct = dh - dhn;
                         dcn = dc_in * kc + dhn * go * (1.f - tc * tc);
                         dc_prev_direct = dc_in - dc_in * kc;
                     } else {
-                        dhn = (p.training && p.mask_h) ? dh * (float)mh_[e] * inv_h : dh;
+                        dhn = (p.training && p.mask_h) ? dh * (float)s_pbm[idx] * inv_h : dh;
                         dcn = dc_in + dhn * go * (1.f - tc * tc);
                     }
                     const float di = dcn * gg * gi * (1.f - gi), df = dcn * cp * gf * (1.f - gf);
@@ -645,7 +647,7 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
                     db[2 * D] = __float2bfloat16_rn(dg); db[3 * D] = __float2bfloat16_rn(dO);
                     dc_reg[e] = dcn * gf + dc_prev_direct;
                     dhz_reg[e] = dh_prev_direct;
-                    if (i > 1 && (uu & 7) == 0) {      // DRAM -> L2 two steps ahead (the register prefetch below runs one step ahead)
+                    if (i > 1 && (uu & 7) == 0) {      // DRAM -> L2 two steps ahead (the shared-memory staging below runs one step ahead)
                         const size_t g1 = g0 - (size_t)2 * B * 4 * D, m1 = (size_t)(i - 2) * B * D + bu;
                         l2_prefetch(p.gates + g1); l2_prefetch(p.gates + g1 + D); l2_prefetch(p.gates + g1 + 2 * D); l2_prefetch(p.gates + g1 + 3 * D);
                         l2_prefetch(p.cstate + m1); l2_prefetch(p.dh_static + m1);
@@ -656,9 +658,9 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
             }
         }
         BPROF_MARK(3);
-        // the operands of the next cell backward are fetched between this CTA's arrival and its wait (the compiler parks them in local
-        // memory, i.e. the thread waits for the loads right there: under the barrier that wait is free)
-        if (!grid_barrier(p.barrier, target, nblocks, p.abort_flag, true, [&]() { pb_prefetch(i - 1); })) break;
+        // the copies of the next cell backward's operands are issued between this CTA's arrival and its wait: the barrier's leading
+        // __syncthreads means every thread is done reading the staging buffer, and they complete while PA runs
+        if (!grid_barrier(p.barrier, target, nblocks, p.abort_flag, true, [&]() { pb_stage(i - 1); })) break;
         BPROF_MARK(4);
         if (i == 0) break;
 
@@ -987,8 +989,10 @@ static AttBwdGeom att_bwd_geom(const b200tts_decoder_shape& s) {
     AttBwdGeom g{};
     g.UK = s.D / KBA;
     const int L16 = (s.L + 15) / 16 * 16;
-    // Wcomb in two layouts, d cum, Wq fragments (A / 16 x 32 x 16 B), two [64][8] slabs of the query part of d h
-    const size_t extras = (size_t)s.A * 40 * 2 + (size_t)32 * (s.A + 8) * 2 + (size_t)(L16 + 32) * 4 + (size_t)s.A * 32 + 2 * 64 * 8 * 4;
+    // Wcomb in two layouts, d cum, Wq fragments (A / 16 x 32 x 16 B), two [64][8] slabs of the query part of d h, and the cell-backward
+    // staging of 8 units x B utterances: 6 fp32 operands, 2 mask bytes, KBA recurrent partials
+    const size_t extras = (size_t)s.A * 40 * 2 + (size_t)32 * (s.A + 8) * 2 + (size_t)(L16 + 32) * 4 + (size_t)s.A * 32 + 2 * 64 * 8 * 4 +
+                          (size_t)s.B * 8 * (6 * 4 + 2 + KBA * 4);
     g.UN = (s.M + s.D <= NBT * TUN) ? TUN : TUN_WIDE; g.grid = KBA * NBT;
     const int NKT = 4 * g.UK / 64;
     g.region = (size_t)NKT * 8192;
@@ -999,7 +1003,7 @@ static AttBwdGeom att_bwd_geom(const b200tts_decoder_shape& s) {
 bool persist_att_bwd_supported(const b200tts_decoder_shape& s) {
     const AttBwdGeom g = att_bwd_geom(s);
     if (s.A != 128 || s.K > 32 || s.B * 8 > 3 * PT || s.D % KBA != 0) return false;
-    if (s.M > 2 * PT || (s.L + 15) / 16 * 16 + 48 > 2 * PT || s.B * (s.A / 4) > 8 * PT) return false;      // register-slot staging of the attention backward
+    if (s.M > 2 * PT || (s.L + 15) / 16 * 16 + 48 > 2 * PT) return false;      // register-slot staging of the attention backward
     if (s.D / 8 > g.grid) return false;                       // cell-backward ownership: 8 hidden units per CTA
     if (g.grid / 2 < s.B || g.grid > NUM_SMS) return false;       // one CTA pair per utterance, all CTAs co-resident
     if (g.UK % 64 != 0 || s.B > 64 || s.M + s.D > NBT * g.UN || (s.M + s.D) % 4 != 0) return false;
@@ -1025,6 +1029,9 @@ int persist_att_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_p
     const int B = s.B, D = s.D, M = s.M, T = s.T, L = s.L, A = s.A;
     B200_REQUIRE(persist_att_bwd_supported(s), "persistent attention backward: shape not supported");
     const AttBwdGeom geo = att_bwd_geom(s);
+    // the cell backward copies each utterance's 8 keep bytes of a CTA's units as one 8-byte asynchronous copy
+    B200_REQUIRE(!s.training || ((uintptr_t)in.mask_att_h | (uintptr_t)in.mask_att_c) % 8 == 0,
+                 "persistent attention backward: the attention-LSTM keep masks must be 8-byte aligned");
     AttBwdArgs a{};
     a.B = B; a.T = T; a.D = D; a.M = M; a.L = L; a.A = A; a.KC = s.K; a.NOUT = M + D; a.UK = geo.UK;
     a.UN = geo.UN; a.MT = x.MT;
