@@ -160,6 +160,13 @@ int b200tts_decoder_path(const b200tts_decoder_shape* shape);
 size_t b200tts_debug_persist_profile_offset(const b200tts_decoder_shape* shape);
 /* Same for the backward workspace: which = 0 generator loop, 1 attention loop ([132][8] int64 each). */
 size_t b200tts_debug_persist_bwd_profile_offset(const b200tts_decoder_shape* shape, int which);
+/* Debug: where a decoder call keeps its per-step state, so that tests can check every step of a decode.  Fills out[0 .. n) with
+ * byte offsets, in this order:
+ *   forward workspace:  ai, ca, hg, cg, ga, gg, q, cum, memT, fs, p1, aib, hgb
+ *   backward workspace: dfs, dhgd, dctxs, dgg, dhas, dga, dq, dctxt, dmemT, dggb, dgab
+ *   row strides (in elements) of aib and hgb: Kp_att, Kp_gen
+ * Returns the number of values written (26 when n >= 26), 0 for a rejected shape. */
+int b200tts_debug_decoder_views(const b200tts_decoder_shape* shape, size_t* out, int n);
 
 int b200tts_decoder_forward(const b200tts_decoder_shape* shape, const b200tts_decoder_params* params,
                             const b200tts_decoder_inputs* in, const b200tts_decoder_outputs* out, void* workspace,

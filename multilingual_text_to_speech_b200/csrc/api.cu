@@ -170,6 +170,7 @@ int loss_backward_impl(const b200tts_loss_shape& s, const float* pre, const floa
                        const float* stop, const float* stop_t, const int* text_len, const int* target_len, const float* grad_losses,
                        float* d_pre, float* d_post, float* d_stop, float* d_align, cudaStream_t st);
 size_t decoder_bwd_profile_offset(const b200tts_decoder_shape& s, int which);
+void decoder_bwd_view_offsets(const b200tts_decoder_shape& s, size_t* out);
 void set_tc_scratch(void* ptr, size_t bytes);
 size_t adam_clip_scratch_floats();
 int adam_clip_step_impl(float* p, float* g, float* m, float* v, size_t n, float lr, float beta1, float beta2, float eps, float weight_decay,
@@ -232,6 +233,24 @@ size_t b200tts_debug_persist_bwd_profile_offset(const b200tts_decoder_shape* sha
 size_t b200tts_debug_persist_profile_offset(const b200tts_decoder_shape* shape) {
     if (!shape || validate_decoder_shape(*shape) != B200TTS_OK) return 0;
     return decoder_layout(*shape).persist * sizeof(float) + persist_layout(*shape).barrier + 256;
+}
+int b200tts_debug_decoder_views(const b200tts_decoder_shape* shape, size_t* out, int n) {
+    if (!shape || !out || validate_decoder_shape(*shape) != B200TTS_OK) return 0;
+    const DecoderLayout l = decoder_layout(*shape);
+    const PersistLayout pl = persist_layout(*shape);
+    const TcPersistGeom g = tc_persist_geom(*shape);
+    const size_t pbase = l.persist * sizeof(float);
+    size_t v[26];
+    const size_t fwd[11] = {l.ai, l.ca, l.hg, l.cg, l.ga, l.gg, l.q, l.cum, l.memT, l.fs, l.p1};
+    for (int k = 0; k < 11; ++k) v[k] = fwd[k] * sizeof(float);
+    v[11] = pbase + pl.aib;
+    v[12] = pbase + pl.hgb;
+    decoder_bwd_view_offsets(*shape, v + 13);
+    v[24] = (size_t)g.Kp_att;
+    v[25] = (size_t)g.Kp_gen;
+    const int m = n < 26 ? n : 26;
+    for (int k = 0; k < m; ++k) out[k] = v[k];
+    return m;
 }
 
 int b200tts_gemm_f32(int transA, int transB, int M, int N, int K, float alpha, const float* A, int lda, const float* B,

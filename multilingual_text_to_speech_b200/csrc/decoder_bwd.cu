@@ -1044,6 +1044,12 @@ size_t decoder_bwd_profile_offset(const b200tts_decoder_shape& s, int which) {
     if (which == 0) return l.pextra * sizeof(float) + persist_bwd_gen_extra_bytes(s) - NUM_SMS * 8 * 8;
     return l.pextra2 * sizeof(float) + att_bwd_extra(s).barrier + 256;
 }
+// byte offsets of the per-step histories of the backward workspace: dfs, dhgd, dctxs, dgg, dhas, dga, dq, dctxt, dmemT, dggb, dgab
+void decoder_bwd_view_offsets(const b200tts_decoder_shape& s, size_t* out) {
+    const BwdLayout l = bwd_layout(s);
+    const size_t offs[11] = {l.dfs, l.dhgd, l.dctxs, l.dgg, l.dhas, l.dga, l.dq, l.dctxt, l.dmemT, l.dggb, l.dgab};
+    for (int k = 0; k < 11; ++k) out[k] = offs[k] * sizeof(float);
+}
 
 // standalone backward of one attention step (module-level API): per-utterance accumulators in the workspace, reduced over the batch here
 size_t attention_step_backward_workspace_elems(int B, int M, int A, int C, int K) {
