@@ -68,6 +68,7 @@ def main():
     ap.add_argument('--tf-start', type=int, default=None,
                     help='decay teacher forcing from this step on (hp.teacher_forcing_start_steps; default: the config\'s schedule)')
     ap.add_argument('--tf-steps', type=int, default=None, help='length of the decay (hp.teacher_forcing_steps)')
+    ap.add_argument('--outputs-per-step', type=int, default=1, help='mel frames predicted per decoder step (hp.outputs_per_step)')
     a = ap.parse_args()
     from multilingual_text_to_speech_b200 import configs, _lib
     from multilingual_text_to_speech_b200.modules.tacotron2 import Tacotron, TacotronLoss
@@ -89,7 +90,7 @@ def main():
             schedule['teacher_forcing_start_steps'] = a.tf_start
         if a.tf_steps is not None:
             schedule['teacher_forcing_steps'] = a.tf_steps
-    hp = configs.apply(a.config, decoder_regularization='zoneout', **schedule)
+    hp = configs.apply(a.config, decoder_regularization='zoneout', outputs_per_step=a.outputs_per_step, **schedule)
     _lib.set_precision('bf16')
     torch.manual_seed(0)
     model = Tacotron().to(dev).train()

@@ -92,6 +92,13 @@ typedef struct {
                                included (the reference's training semantics).  1: over each utterance's own text length; weights at
                                l >= length are 0, so a padded batch decodes every utterance as it decodes alone.  Forward and chunk
                                entry points only: b200tts_decoder_backward rejects 1. */
+    int R;                  /* frames per decoder step (reduction factor, hp.outputs_per_step); 0 in a zero-initialised shape means 1.
+                               T keeps counting target frames; the decode runs S = ceil(T / R) steps, and step i is fed frame i*R - 1
+                               (zeros at step 0).  Arrays with S rows (one per step): the keep masks, `teacher`, `alignments` /
+                               `d_alignments` and every per-step row of both workspaces.  Arrays with T frames: target, spectrogram,
+                               stop and their gradients; frames of the last step past T are dropped (zero gradient).  The parameters
+                               predict R frames per step: frame_w [R*N, D+M], frame_b [R*N], stop_w [R, D+M], stop_b [R], row block j
+                               (rows j*N .. j*N+N-1 of frame_w, row j of stop_w) = frame j of the step.  Negative R is rejected. */
 } b200tts_decoder_shape;
 
 /* Parameter block in the reference's own layouts ([out, in] Linear weights; names = state_dict keys). */
@@ -124,24 +131,24 @@ typedef struct {
     const float* memory;          /* [B, L, M] encoder output ++ speaker/language embeddings */
     const int32_t* text_lengths;  /* [B] */
     const float* target;          /* [B, N, T] ground-truth mel frames */
-    const uint8_t* teacher;       /* [host] [T] 1 = ground truth fed at step i (tacotron2.py:171,181); NULL = all 1.  0 = free-running:
-                                     step i is fed the frame predicted at step i-1 (zeros at step 0), and the backward
+    const uint8_t* teacher;       /* [host] [S] 1 = ground truth fed at step i (tacotron2.py:171,181); NULL = all 1.  0 = free-running:
+                                     step i is fed the last frame predicted at step i-1 (zeros at step 0), and the backward
                                      differentiates through that frame (no detach, as in the reference) */
-    /* keep masks, NULL = no dropout at that site.  Time-major: row i belongs to decoder step i. */
-    const uint8_t* mask_prenet0;  /* [T, B, P] */
-    const uint8_t* mask_prenet1;  /* [T, B, P] */
-    const uint8_t* mask_att_h;    /* [T, B, D]; 8-byte aligned on the persistent attention reverse loop */
-    const uint8_t* mask_att_c;    /* [T, B, D] zoneout only; 8-byte aligned there too */
-    const uint8_t* mask_gen_h;    /* [T, B, D] */
-    const uint8_t* mask_gen_c;    /* [T, B, D] zoneout only */
-    const uint8_t* mask_step_prenet0; /* [T, B, P] prenet masks of free-running steps */
-    const uint8_t* mask_step_prenet1; /* [T, B, P] */
+    /* keep masks, NULL = no dropout at that site.  Time-major: row i belongs to decoder step i (S = ceil(T / R) rows). */
+    const uint8_t* mask_prenet0;  /* [S, B, P] */
+    const uint8_t* mask_prenet1;  /* [S, B, P] */
+    const uint8_t* mask_att_h;    /* [S, B, D]; 8-byte aligned on the persistent attention reverse loop */
+    const uint8_t* mask_att_c;    /* [S, B, D] zoneout only; 8-byte aligned there too */
+    const uint8_t* mask_gen_h;    /* [S, B, D] */
+    const uint8_t* mask_gen_c;    /* [S, B, D] zoneout only */
+    const uint8_t* mask_step_prenet0; /* [S, B, P] prenet masks of free-running steps */
+    const uint8_t* mask_step_prenet1; /* [S, B, P] */
 } b200tts_decoder_inputs;
 
 typedef struct {
     float* spectrogram; /* [B, T, N] */
     float* stop;        /* [B, T]   logits */
-    float* alignments;  /* [B, T, L] */
+    float* alignments;  /* [B, S, L]  one row per decoder step */
 } b200tts_decoder_outputs;
 
 /* Bytes of the forward workspace; it also carries everything the backward pass re-reads. */
@@ -179,11 +186,12 @@ typedef struct {
     float* gen_h; float* gen_c; /* [B, D] generator-LSTM state */
     float* context;             /* [B, M] last attention context */
     float* cum_weights;         /* [B, L] cumulative attention weights (forward attention: the last alignment = alpha) */
-    float* frame;               /* [B, N] last predicted frame (input of the next free-running step) */
+    float* frame;               /* [B, N] last predicted frame, the last of the last step's R (input of the next free-running step) */
 } b200tts_decoder_state;
 
 /* b200tts_decoder_forward on a chunk of T frames: `first` != 0 starts from the zero state (tacotron2.py:164-168), otherwise from
- * `state`; on return `state` holds the state after the chunk's last step.  Uses the per-step kernels (any precision mode). */
+ * `state`; on return `state` holds the state after the chunk's last step.  Uses the per-step kernels (any precision mode).  A chunk
+ * holds whole steps: T % R != 0 is rejected. */
 int b200tts_decoder_forward_chunk(const b200tts_decoder_shape* shape, const b200tts_decoder_params* params,
                                   const b200tts_decoder_inputs* in, const b200tts_decoder_outputs* out, b200tts_decoder_state* state,
                                   int first, void* workspace, size_t workspace_bytes, void* stream);
@@ -191,7 +199,7 @@ int b200tts_decoder_forward_chunk(const b200tts_decoder_shape* shape, const b200
 typedef struct {
     const float* d_spectrogram; /* [B, T, N] or NULL */
     const float* d_stop;        /* [B, T]    or NULL */
-    const float* d_alignments;  /* [B, T, L] or NULL */
+    const float* d_alignments;  /* [B, S, L] or NULL */
 } b200tts_decoder_output_grads;
 
 /* Backward of the decode (autograd replay of tacotron2.py:148-209, train.py:83), free-running steps included: their gradient
@@ -338,12 +346,15 @@ int b200tts_bilstm_backward(const b200tts_bilstm_shape* shape, const b200tts_bil
 
 /* ---- loss: TacotronLoss.forward, modules/tacotron2.py:439-485 (guided attention :439-457 in closed form) ----
  * pre / post / targets [B, N, T]; stop (logits, padded positions already filled as in tacotron2.py:380) / stop_target [B, T]; alignment
- * [B, T, L]; lengths int32 [B].  losses[4] (device) = { 2*MSE(pre), MSE(post), BCEWithLogits(pos_weight)/(N+2), guided attention }.   */
+ * [B, S, L] with S = ceil(T / R); lengths int32 [B].  losses[4] (device) = { 2*MSE(pre), MSE(post), BCEWithLogits(pos_weight)/(N+2),
+ * guided attention }.  The guided term runs on the step grid: utterance b has ceil(target_lengths[b] / R) steps, which take the place of
+ * its frame count in the weight and the division (R = 1: the reference's formula).                                                     */
 typedef struct {
     int B, N, T, L;
     int guided;            /* hp.guided_attention_loss and guided_att_steps > 0 */
     float guided_g;        /* current variance (TacotronLoss._g) */
     float stop_pos_weight; /* 100 in the reference (tacotron2.py:465) */
+    int R;                 /* frames per decoder step of the alignment rows; 0 in a zero-initialised shape means 1 */
 } b200tts_loss_shape;
 size_t b200tts_loss_workspace_bytes(void);
 int b200tts_tacotron_loss_forward(const b200tts_loss_shape* shape, const float* pre, const float* pre_target, const float* post,

@@ -20,7 +20,7 @@ class B200TTSError(RuntimeError):
 
 class DecoderShape(Structure):
     _fields_ = [(n, c_int) for n in ('B', 'L', 'T', 'M', 'D', 'P', 'A', 'C', 'K', 'N', 'cell_kind', 'training')] + \
-               [('rate_h', c_float), ('rate_c', c_float), ('prenet_rate', c_float), ('att_kind', c_int), ('att_extent', c_int)]
+               [('rate_h', c_float), ('rate_c', c_float), ('prenet_rate', c_float), ('att_kind', c_int), ('att_extent', c_int), ('R', c_int)]
 
 
 DECODER_PARAM_FIELDS = ('prenet_w0', 'prenet_b0', 'prenet_w1', 'prenet_b1', 'att_w_ih', 'att_w_hh', 'att_b_ih', 'att_b_hh',
@@ -56,7 +56,7 @@ class ConvBlockShape(Structure):
 
 
 class LossShape(Structure):
-    _fields_ = [(n, c_int) for n in ('B', 'N', 'T', 'L', 'guided')] + [('guided_g', c_float), ('stop_pos_weight', c_float)]
+    _fields_ = [(n, c_int) for n in ('B', 'N', 'T', 'L', 'guided')] + [('guided_g', c_float), ('stop_pos_weight', c_float), ('R', c_int)]
 
 
 class BiLSTMShape(Structure):

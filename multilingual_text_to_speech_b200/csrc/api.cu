@@ -226,26 +226,29 @@ int b200tts_set_scratch(void* ptr, size_t bytes) {
     return B200TTS_OK;
 }
 int b200tts_set_tensor_core_gemm(int enabled) { set_tc_enabled(enabled ? 1 : 0); return B200TTS_OK; }
+// Every query below answers for the step shape (T -> ceil(T / R) steps) that the forward and backward calls run on.
 size_t b200tts_debug_persist_bwd_profile_offset(const b200tts_decoder_shape* shape, int which) {
     if (!shape || validate_decoder_shape(*shape) != B200TTS_OK) return 0;
-    return decoder_bwd_profile_offset(*shape, which);
+    return decoder_bwd_profile_offset(step_shape(*shape), which);
 }
 size_t b200tts_debug_persist_profile_offset(const b200tts_decoder_shape* shape) {
     if (!shape || validate_decoder_shape(*shape) != B200TTS_OK) return 0;
-    return decoder_layout(*shape).persist * sizeof(float) + persist_layout(*shape).barrier + 256;
+    const b200tts_decoder_shape s = step_shape(*shape);
+    return decoder_layout(s).persist * sizeof(float) + persist_layout(s).barrier + 256;
 }
 int b200tts_debug_decoder_views(const b200tts_decoder_shape* shape, size_t* out, int n) {
     if (!shape || !out || validate_decoder_shape(*shape) != B200TTS_OK) return 0;
-    const DecoderLayout l = decoder_layout(*shape);
-    const PersistLayout pl = persist_layout(*shape);
-    const TcPersistGeom g = tc_persist_geom(*shape);
+    const b200tts_decoder_shape s = step_shape(*shape);
+    const DecoderLayout l = decoder_layout(s);
+    const PersistLayout pl = persist_layout(s);
+    const TcPersistGeom g = tc_persist_geom(s);
     const size_t pbase = l.persist * sizeof(float);
     size_t v[26];
     const size_t fwd[11] = {l.ai, l.ca, l.hg, l.cg, l.ga, l.gg, l.q, l.cum, l.memT, l.fs, l.p1};
     for (int k = 0; k < 11; ++k) v[k] = fwd[k] * sizeof(float);
     v[11] = pbase + pl.aib;
     v[12] = pbase + pl.hgb;
-    decoder_bwd_view_offsets(*shape, v + 13);
+    decoder_bwd_view_offsets(s, v + 13);
     v[24] = (size_t)g.Kp_att;
     v[25] = (size_t)g.Kp_gen;
     const int m = n < 26 ? n : 26;
@@ -266,18 +269,18 @@ int b200tts_gemm_f32(int transA, int transB, int M, int N, int K, float alpha, c
 
 size_t b200tts_decoder_workspace_bytes(const b200tts_decoder_shape* shape) {
     if (!shape || validate_decoder_shape(*shape) != B200TTS_OK) return 0;
-    return decoder_layout(*shape).total * sizeof(float);
+    return decoder_layout(step_shape(*shape)).total * sizeof(float);
 }
 
 int b200tts_decoder_path(const b200tts_decoder_shape* shape) {
     if (!shape || validate_decoder_shape(*shape) != B200TTS_OK) return 0;
-    const PersistPlan p = persist_plan(*shape);
+    const PersistPlan p = persist_plan(step_shape(*shape));
     return (p.fwd ? 1 | 2 : 0) | (p.gen_bwd ? 4 | 8 : 0) | (p.att_bwd ? 16 | 32 : 0);
 }
 
 size_t b200tts_decoder_bwd_workspace_bytes(const b200tts_decoder_shape* shape) {
     if (!shape || validate_decoder_shape(*shape) != B200TTS_OK) return 0;
-    return decoder_bwd_workspace_floats(*shape) * sizeof(float);
+    return decoder_bwd_workspace_floats(step_shape(*shape)) * sizeof(float);
 }
 
 int b200tts_decoder_forward(const b200tts_decoder_shape* shape, const b200tts_decoder_params* params,
@@ -294,6 +297,8 @@ int b200tts_decoder_forward_chunk(const b200tts_decoder_shape* shape, const b200
     B200_REQUIRE(shape && params && in && out && state, "decoder_forward_chunk: null argument");
     B200_REQUIRE(state->att_h && state->att_c && state->gen_h && state->gen_c && state->context && state->cum_weights && state->frame,
                  "decoder_forward_chunk: every state buffer is required");
+    B200_REQUIRE(shape->R < 0 || shape->T % frames_per_step(*shape) == 0,
+                 "decoder_forward_chunk: a chunk holds whole decoder steps (T=%d is not a multiple of R=%d)", shape->T, shape->R);
     B200_TRY(require_device());
     return decoder_forward_impl(*shape, *params, *in, *out, (float*)workspace, workspace_bytes, (cudaStream_t)stream, state, first);
 }

@@ -19,17 +19,22 @@ inline int grid_for(size_t n) {
 // ---------------------------------------------------------------------------------------------
 // utility kernels
 // ---------------------------------------------------------------------------------------------
-// dFS[i, b, n] = d_spec[b, i, n] (n < N), dFS[i, b, N] = d_stop[b, i]
+// The inverse of split_frames_kernel: dFS [S, B, R*(N+1)] from the per-frame gradients, frame k = i*R + j of step i, slot j:
+// dFS[i, b, j*N + n] = d_spec[b, k, n], dFS[i, b, R*N + j] = d_stop[b, k]; 0 for the frames of the last step past T.
 __global__ void gather_frame_grads_kernel(float* __restrict__ dfs, const float* __restrict__ dspec,
-                                          const float* __restrict__ dstop, int B, int T, int N) {
-    const size_t total = (size_t)B * T * (N + 1);
+                                          const float* __restrict__ dstop, int B, int S, int T, int N, int R) {
+    const int W = R * (N + 1), RN = R * N;
+    const size_t total = (size_t)B * S * W;
     for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
-        const int n = idx % (N + 1);
-        const int b = (idx / (N + 1)) % B;
-        const int i = idx / ((size_t)(N + 1) * B);
+        const int c = idx % W;
+        const int b = (idx / W) % B;
+        const int i = idx / ((size_t)W * B);
+        const int j = c < RN ? c / N : c - RN, k = i * R + j;
         float v = 0.f;
-        if (n < N) { if (dspec) v = dspec[((size_t)b * T + i) * N + n]; }
-        else if (dstop) v = dstop[(size_t)b * T + i];
+        if (k < T) {
+            if (c < RN) { if (dspec) v = dspec[((size_t)b * T + k) * N + c - j * N]; }
+            else if (dstop) v = dstop[(size_t)b * T + k];
+        }
         dfs[idx] = v;
     }
 }
@@ -105,14 +110,16 @@ __global__ void relu_dropout_bwd_kernel(float* __restrict__ dz, const float* __r
 // Feedback of a free-running step f >= 1 into the frame it was fed, x_f = FS[f-1, :, 0:N] (tacotron2.py:171,181; not detached),
 // one CTA per utterance.  dp1 = d p1_f (the product dga_f . W_ih_att[:, :P], taken by the GEMM before this kernel):
 //   dz1 = dp1 * scale1 * (p1 > 0);  dp0 = dz1 . W1;  dz0 = dp0 * scale0 * (p0 > 0);  dx = dz0 . W0
-//   dFS[f-1, b, 0:N] += dx;  [d h_gen | d ctx]_{f-1} += dx . Wfs[0:N, :]   (direct / static parts, consumed by the reverse steps f-1)
+//   dFS[f-1, b, (R-1)N : RN] += dx;  [d h_gen | d ctx]_{f-1} += dx . Wfs[(R-1)N : RN, :]   (the fed-back frame is the last of step f-1's R;
+//   direct / static parts, consumed by the reverse steps f-1)
 // Every sum runs in a fixed order (no atomics).
 struct FeedbackArgs {
     const float* dp1;                  // [B, P]
     const float* p0; const float* p1;  // [B, P] step f's prenet activations (after relu + dropout)
     const float* W0; const float* W1;  // prenet_w0 [P, N], prenet_w1 [P, P]
-    const float* wfs;                  // [N+1, D+M]
-    float* dfs;                        // [B, N+1] row f-1
+    const float* wfs;                  // [N, D+M]   rows of the fed-back frame in [frame_w ; stop_w]
+    float* dfs;                        // [B, ld_fs] the fed-back frame's columns of dFS row f-1
+    int ld_fs;
     float* dhgd;                       // [B, D]   row f-1
     float* dctxs;                      // [B, M]   row f-1
     float scale0, scale1;
@@ -149,7 +156,7 @@ __global__ void __launch_bounds__(FEEDBACK_THREADS) frame_feedback_bwd_kernel(co
         float acc = 0.f;
         for (int sl = 0; sl < ns; ++sl) acc += xpart[(size_t)sl * N + n];
         dx[n] = acc;
-        p.dfs[(size_t)b * (N + 1) + n] += acc;
+        p.dfs[(size_t)b * p.ld_fs + n] += acc;
     }
     __syncthreads();
     for (int c = tid; c < DM; c += FEEDBACK_THREADS) {
@@ -752,9 +759,9 @@ BwdLayout bwd_layout(const b200tts_decoder_shape& s) {
     BwdLayout l;
     size_t off = 0;
     auto take = [&](size_t n) { size_t o = off; off = align_up(off + n, 64); return o; };
-    const size_t T = s.T, B = s.B, D = s.D, M = s.M, P = s.P, A = s.A, N = s.N, L = s.L;
+    const size_t T = s.T, B = s.B, D = s.D, M = s.M, P = s.P, A = s.A, L = s.L, W = fs_width(s);
     const size_t C = forward_attention(s) ? 0 : s.C, K = forward_attention(s) ? 0 : s.K;     // ignored for forward attention
-    l.dfs = take(T * B * (N + 1));
+    l.dfs = take(T * B * W);
     l.dhgd = take(T * B * D);
     l.dctxs = take(T * B * M);
     l.dgg = take(T * B * 4 * D);
@@ -771,7 +778,7 @@ BwdLayout bwd_layout(const b200tts_decoder_shape& s) {
     l.dv_acc = take(B * A);
     l.dp1 = take(T * B * P);
     l.dp0 = take(T * B * P);
-    l.dwfs = take((N + 1) * (D + M));
+    l.dwfs = take(W * (D + M));
     l.split_gen = pick_splitk(s.B, s.D, 4 * s.D);
     l.split_att = pick_splitk(s.B, s.M + s.D, 4 * s.D);
     const size_t pg = (size_t)l.split_gen * B * D, pa = (size_t)l.split_att * B * (M + D);
@@ -850,17 +857,17 @@ struct BwdCtx {
 int frame_weight_grads(const BwdCtx& c, const b200tts_decoder_params& dw, const __nv_bfloat16* hgb1, int ldhb,
                        const __nv_bfloat16* aib1, int ldab) {
     const auto& s = c.s; const auto& l = c.l;
-    const int D = s.D, M = s.M, N = s.N, N1 = N + 1, MD = M + D;
+    const int D = s.D, M = s.M, RN = s.R * s.N, N1 = fs_width(s), MD = M + D;
     const size_t TB = (size_t)s.T * s.B;
     const float* ai1 = c.F(c.fl.ai) + (size_t)s.B * MD;
     B200_TRY(wgemm16(c.st, l, c.bws, N1, D, (int)TB, c.W(l.dfs), N1, c.F(c.fl.hg) + (size_t)s.B * D, D, hgb1, ldhb, c.W(l.dwfs), D + M, 0.f));
     B200_TRY(wgemm16(c.st, l, c.bws, N1, M, (int)TB, c.W(l.dfs), N1, ai1, MD, aib1 ? aib1 + D : nullptr, ldab, c.W(l.dwfs) + D, D + M, 0.f));
-    add2d_kernel<<<grid_for((size_t)N * (D + M)), 256, 0, c.st>>>(dw.frame_w, D + M, c.W(l.dwfs), D + M, N, D + M);
+    add2d_kernel<<<grid_for((size_t)RN * (D + M)), 256, 0, c.st>>>(dw.frame_w, D + M, c.W(l.dwfs), D + M, RN, D + M);
     B200_LAUNCH_CHECK();
-    add2d_kernel<<<grid_for((size_t)(D + M)), 256, 0, c.st>>>(dw.stop_w, D + M, c.W(l.dwfs) + (size_t)N * (D + M), D + M, 1, D + M);
+    add2d_kernel<<<grid_for((size_t)s.R * (D + M)), 256, 0, c.st>>>(dw.stop_w, D + M, c.W(l.dwfs) + (size_t)RN * (D + M), D + M, s.R, D + M);
     B200_LAUNCH_CHECK();
-    B200_TRY(colsum_add(dw.frame_b, nullptr, c.W(l.dfs), TB, N, N1, c.W(l.gpart), c.st));
-    B200_TRY(colsum_add(dw.stop_b, nullptr, c.W(l.dfs) + N, TB, 1, N1, c.W(l.gpart), c.st));
+    B200_TRY(colsum_add(dw.frame_b, nullptr, c.W(l.dfs), TB, RN, N1, c.W(l.gpart), c.st));
+    B200_TRY(colsum_add(dw.stop_b, nullptr, c.W(l.dfs) + RN, TB, s.R, N1, c.W(l.gpart), c.st));
     return B200TTS_OK;
 }
 
@@ -1016,14 +1023,14 @@ int prenet_relu_bwd(const BwdCtx& c, float* dz, const float* y, const uint8_t* m
 // the time-batched prenet pass rewrites later), then the rest of the chain in frame_feedback_bwd_kernel
 int frame_feedback(const BwdCtx& c, int f) {
     const auto& s = c.s; const auto& l = c.l;
-    const int B = s.B, D = s.D, M = s.M, P = s.P, N = s.N;
+    const int B = s.B, D = s.D, M = s.M, P = s.P, N = s.N, W = fs_width(s), last = (s.R - 1) * N;
     float* dp1 = c.W(l.dp1) + (size_t)f * B * P;
     B200_TRY(xgemm16(c.st, l, c.bws, B, P, 4 * D, c.W(l.dga) + (size_t)f * B * 4 * D, 4 * D, nullptr, 0, c.w.att_w_ih, P + M, dp1, P, 0.f));
     FeedbackArgs a{};
     a.dp1 = dp1;
     a.p0 = c.F(c.fl.p0) + (size_t)f * B * P; a.p1 = c.F(c.fl.p1) + (size_t)f * B * P;
-    a.W0 = c.w.prenet_w0; a.W1 = c.w.prenet_w1; a.wfs = c.F(c.fl.wfs);
-    a.dfs = c.W(l.dfs) + (size_t)(f - 1) * B * (N + 1);
+    a.W0 = c.w.prenet_w0; a.W1 = c.w.prenet_w1; a.wfs = c.F(c.fl.wfs) + (size_t)last * (D + M);
+    a.dfs = c.W(l.dfs) + (size_t)(f - 1) * B * W + last; a.ld_fs = W;
     a.dhgd = c.W(l.dhgd) + (size_t)(f - 1) * B * D;
     a.dctxs = c.W(l.dctxs) + (size_t)(f - 1) * B * M;
     a.scale0 = prenet_scale(s, c.in.mask_step_prenet0); a.scale1 = prenet_scale(s, c.in.mask_step_prenet1);
@@ -1107,10 +1114,11 @@ int forward_attention_step_backward_impl(int B, int L, int M, int A, const float
     return B200TTS_OK;
 }
 
-int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
+int decoder_backward_impl(const b200tts_decoder_shape& frames, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
                           const b200tts_decoder_outputs& fwd_out, const b200tts_decoder_output_grads& dout, const float* fws,
                           float* bws, size_t bws_bytes, const b200tts_decoder_params& dw, float* d_memory, cudaStream_t st) {
-    B200_TRY(validate_decoder_shape(s));
+    B200_TRY(validate_decoder_shape(frames));
+    const b200tts_decoder_shape s = step_shape(frames);     // T = decoder steps from here on; frames.T = target frames
     B200_REQUIRE(fwd_out.alignments, "decoder_backward: the forward alignments tensor is required");
     B200_REQUIRE(s.att_extent == 0, "decoder_backward: att_extent = 1 (attention over each utterance's own length) is for inference only; "
                  "training keeps the reference's softmax over the padded extent");
@@ -1127,7 +1135,7 @@ int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_
     const BwdLayout l = bwd_layout(s);
     B200_REQUIRE(bws_bytes >= l.total * sizeof(float), "decoder_backward: workspace too small (%zu < %zu bytes)", bws_bytes,
                  l.total * sizeof(float));
-    const int B = s.B, T = s.T, D = s.D, M = s.M, P = s.P, N = s.N, A = s.A, L = s.L, C = s.C, K = s.K, MD = M + D, N1 = N + 1;
+    const int B = s.B, T = s.T, D = s.D, M = s.M, P = s.P, N = s.N, A = s.A, L = s.L, C = s.C, K = s.K, MD = M + D, N1 = fs_width(s);
     const size_t TB = (size_t)T * B;
     auto F = [&](size_t off) { return fws + off; };
     auto W = [&](size_t off) { return bws + off; };
@@ -1150,7 +1158,7 @@ int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_
     const __nv_bfloat16* hgb1 = hgb ? hgb + (size_t)B * ldhb : nullptr;
 
     // ---- 1. frame / stop projection backward (time-batched) ----
-    gather_frame_grads_kernel<<<grid_for(TB * N1), 256, 0, st>>>(W(l.dfs), dout.d_spectrogram, dout.d_stop, B, T, N);
+    gather_frame_grads_kernel<<<grid_for(TB * N1), 256, 0, st>>>(W(l.dfs), dout.d_spectrogram, dout.d_stop, B, T, frames.T, N, s.R);
     B200_LAUNCH_CHECK();
     // d h_gen (direct) and d ctx (projection part)
     B200_TRY(wgemm(st, l, bws, 0, 0, (int)TB, D, N1, W(l.dfs), N1, F(fl.wfs), D + M, W(l.dhgd), D, 0.f));

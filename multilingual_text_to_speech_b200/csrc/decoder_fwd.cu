@@ -28,8 +28,9 @@ __global__ void fill_kernel(float* __restrict__ dst, float v, size_t n) {
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) dst[i] = v;
 }
 
-// Xtm[i, b, n] = (i == 0) ? 0 : target[b, n, i-1]      (tacotron2.py:126-134 without the prenet)
-__global__ void prep_target_kernel(float* __restrict__ xtm, const float* __restrict__ target, int B, int N, int T) {
+// Xtm[i, b, n] = (i == 0) ? 0 : target[b, n, i*R - 1]   (tacotron2.py:126-134 without the prenet; step i is fed the last frame of
+// step i-1's group).  T = steps, Tf = frames of target.
+__global__ void prep_target_kernel(float* __restrict__ xtm, const float* __restrict__ target, int B, int N, int T, int R, int Tf) {
     // tile transpose over (n, i) for one b: 32 x 32 tiles through shared memory
     __shared__ float tile[32][33];
     const int b = blockIdx.z;
@@ -37,7 +38,7 @@ __global__ void prep_target_kernel(float* __restrict__ xtm, const float* __restr
     for (int r = threadIdx.y; r < 32; r += blockDim.y) {
         const int n = n0 + r, i = i0 + threadIdx.x;       // read along i (contiguous in target)
         float v = 0.f;
-        if (n < N && i < T && i > 0) v = target[((size_t)b * N + n) * T + i - 1];
+        if (n < N && i < T && i > 0) v = target[((size_t)b * N + n) * Tf + (size_t)i * R - 1];
         tile[r][threadIdx.x] = v;
     }
     __syncthreads();
@@ -56,17 +57,20 @@ __global__ void relu_dropout_kernel(float* __restrict__ x, const uint8_t* __rest
     }
 }
 
-// spec[b, i, n] = FS[i, b, n]; stop[b, i] = FS[i, b, N]
+// Frame k = i*R + j of utterance b (step i, slot j) from the step rows FS [S, B, R*(N+1)] = [R frames | R stop logits]:
+// spec[b, k, n] = FS[i, b, j*N + n]; stop[b, k] = FS[i, b, R*N + j].  Only the T frames are written: the tail of the last step is dropped.
 __global__ void split_frames_kernel(float* __restrict__ spec, float* __restrict__ stop, const float* __restrict__ fs,
-                                    int B, int T, int N) {
+                                    int B, int T, int N, int R) {
     const size_t total = (size_t)B * T * (N + 1);
+    const int W = R * (N + 1);
     for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
         const int n = idx % (N + 1);
-        const int i = (idx / (N + 1)) % T;
+        const int k = (idx / (N + 1)) % T;
         const int b = idx / ((size_t)(N + 1) * T);
-        const float v = fs[((size_t)i * B + b) * (N + 1) + n];
-        if (n < N) spec[((size_t)b * T + i) * N + n] = v;
-        else stop[(size_t)b * T + i] = v;
+        const int i = k / R, j = k - i * R;
+        const float* row = fs + ((size_t)i * B + b) * W;
+        if (n < N) spec[((size_t)b * T + k) * N + n] = row[j * N + n];
+        else stop[(size_t)b * T + k] = row[R * N + j];
     }
 }
 
@@ -472,6 +476,7 @@ int launch_fill(float* dst, float value, size_t n, cudaStream_t st) {
 
 int validate_decoder_shape(const b200tts_decoder_shape& s) {
     B200_REQUIRE(s.B > 0 && s.L > 0 && s.T > 0, "decoder: empty batch/sequence (B=%d L=%d T=%d)", s.B, s.L, s.T);
+    B200_REQUIRE(s.R >= 0, "decoder: frames per step R=%d must be >= 1 (0 means 1)", s.R);
     B200_REQUIRE(s.att_kind == B200TTS_ATT_LOCATION || s.att_kind == B200TTS_ATT_FORWARD, "decoder: bad attention kind %d", s.att_kind);
     B200_REQUIRE(s.att_extent == 0 || s.att_extent == 1, "decoder: bad attention extent %d", s.att_extent);
     B200_REQUIRE(s.M > 0 && s.D > 0 && s.P > 0 && s.A > 0 && s.N > 0, "decoder: non-positive dimension");
@@ -603,7 +608,7 @@ int gen_input_proj(const FwdCtx& c, int step0, int nsteps) {
 }
 int frame_proj(const FwdCtx& c, int step0, int nsteps) {
     const auto& s = c.s; const auto& l = c.lay;
-    const int MD = s.M + s.D, rows = nsteps * s.B, N1 = s.N + 1;
+    const int MD = s.M + s.D, rows = nsteps * s.B, N1 = fs_width(s);
     const float* hg = c.at(l.hg) + (size_t)(step0 + 1) * s.B * s.D;
     const float* ai = c.at(l.ai) + (size_t)(step0 + 1) * s.B * MD;
     float* fs = c.at(l.fs) + (size_t)step0 * s.B * N1;
@@ -614,10 +619,11 @@ int frame_proj(const FwdCtx& c, int step0, int nsteps) {
 
 }  // namespace
 
-int decoder_forward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
+int decoder_forward_impl(const b200tts_decoder_shape& frames, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
                          const b200tts_decoder_outputs& out, float* ws, size_t ws_bytes, cudaStream_t st,
                          const b200tts_decoder_state* state, int first) {
-    B200_TRY(validate_decoder_shape(s));
+    B200_TRY(validate_decoder_shape(frames));
+    const b200tts_decoder_shape s = step_shape(frames);     // T = decoder steps from here on; Tf = target frames
     const bool resume = state != nullptr && !first;       // chunked decode: start from the carried state
     FwdCtx c{s, w, in, decoder_layout(s), ws, st};
     const auto& l = c.lay;
@@ -630,6 +636,7 @@ int decoder_forward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_p
     else
         B200_REQUIRE(w.attn_location && w.attn_loc_features, "decoder_forward: location-sensitive attention needs its location weights");
     const int B = s.B, T = s.T, D = s.D, M = s.M, P = s.P, N = s.N, MD = M + D;
+    const int R = s.R, Tf = frames.T, RN = R * N, W = fs_width(s);
     const size_t BD = (size_t)B * D;
     bool sequential = false;
     if (in.teacher)
@@ -640,15 +647,15 @@ int decoder_forward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_p
     B200_TRY(launch_copy2d(c.at(l.wcat_att) + M, MD, w.att_w_hh, D, 4 * D, D, st));
     B200_TRY(launch_add_vec(c.at(l.bsum_att), w.att_b_ih, w.att_b_hh, 4 * D, st));
     B200_TRY(launch_add_vec(c.at(l.bsum_gen), w.gen_b_ih, w.gen_b_hh, 4 * D, st));
-    B200_TRY(launch_copy2d(c.at(l.wfs), D + M, w.frame_w, D + M, N, D + M, st));
-    B200_TRY(launch_copy2d(c.at(l.wfs) + (size_t)N * (D + M), D + M, w.stop_w, D + M, 1, D + M, st));
-    B200_TRY(launch_copy2d(c.at(l.bfs), N, w.frame_b, N, 1, N, st));
-    B200_TRY(launch_copy2d(c.at(l.bfs) + N, 1, w.stop_b, 1, 1, 1, st));
+    B200_TRY(launch_copy2d(c.at(l.wfs), D + M, w.frame_w, D + M, RN, D + M, st));
+    B200_TRY(launch_copy2d(c.at(l.wfs) + (size_t)RN * (D + M), D + M, w.stop_w, D + M, R, D + M, st));
+    B200_TRY(launch_copy2d(c.at(l.bfs), RN, w.frame_b, RN, 1, RN, st));
+    B200_TRY(launch_copy2d(c.at(l.bfs) + RN, R, w.stop_b, R, 1, R, st));
 
     // ---- time-batched prologue: prenet over all frames, attention-LSTM input projection, memory projection ----
     {
         dim3 grid(cdiv(T, 32), cdiv(N, 32), B), block(32, 8);
-        prep_target_kernel<<<grid, block, 0, st>>>(c.at(l.xtm), in.target, B, N, T);
+        prep_target_kernel<<<grid, block, 0, st>>>(c.at(l.xtm), in.target, B, N, T, R, Tf);
         B200_LAUNCH_CHECK();
     }
     B200_TRY(prenet_rows(c, T * B, c.at(l.xtm), c.at(l.p0), c.at(l.p1), in.mask_prenet0, in.mask_prenet1));
@@ -695,7 +702,7 @@ int decoder_forward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_p
         }
         B200_TRY(tc_persist_gen_loop(s, w, in, l, ws, pws, st));
         {       // frame / stop projection straight from the bf16 operand rows of the two loops (h_gen, then ctx accumulated on top)
-            const int N1 = N + 1;
+            const int N1 = W;
             GemmDesc d;
             d.A = c.at(l.hg) + BD; d.lda = D;
             d.A16 = pws + pl.hgb + (size_t)B * g.Kp_gen * 2; d.lda16 = g.Kp_gen;
@@ -729,7 +736,7 @@ int decoder_forward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_p
                 float* x = c.at(l.xtm) + (size_t)i * B * N;
                 if (i == 0 && resume) B200_TRY(launch_copy2d(x, N, state->frame, N, B, N, st));
                 else if (i == 0) B200_TRY(launch_fill(x, 0.f, (size_t)B * N, st));
-                else B200_TRY(launch_copy2d(x, N, c.at(l.fs) + (size_t)(i - 1) * B * (N + 1), N + 1, B, N, st));
+                else B200_TRY(launch_copy2d(x, N, c.at(l.fs) + (size_t)(i - 1) * B * W + RN - N, W, B, N, st));
                 const uint8_t* m0 = in.mask_step_prenet0 ? in.mask_step_prenet0 + (size_t)i * B * P : nullptr;
                 const uint8_t* m1 = in.mask_step_prenet1 ? in.mask_step_prenet1 + (size_t)i * B * P : nullptr;
                 B200_TRY(prenet_rows(c, B, x, c.at(l.p0) + (size_t)i * B * P, c.at(l.p1) + (size_t)i * B * P, m0, m1));
@@ -742,7 +749,7 @@ int decoder_forward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_p
             B200_TRY(frame_proj(c, i, 1));
         }
     }
-    split_frames_kernel<<<grid_for((size_t)B * T * (N + 1)), 256, 0, st>>>(out.spectrogram, out.stop, c.at(l.fs), B, T, N);
+    split_frames_kernel<<<grid_for((size_t)B * Tf * (N + 1)), 256, 0, st>>>(out.spectrogram, out.stop, c.at(l.fs), B, Tf, N, R);
     B200_LAUNCH_CHECK();
     if (state) {        // state after the last step of the chunk
         const float* ai_T = c.at(l.ai) + (size_t)T * B * MD;
@@ -752,7 +759,7 @@ int decoder_forward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_p
         B200_TRY(launch_copy2d(state->gen_h, D, c.at(l.hg) + (size_t)T * BD, D, B, D, st));
         B200_TRY(launch_copy2d(state->gen_c, D, c.at(l.cg) + (size_t)T * BD, D, B, D, st));
         B200_TRY(launch_copy2d(state->cum_weights, s.L, c.at(l.cum) + (size_t)T * B * s.L, s.L, B, s.L, st));
-        B200_TRY(launch_copy2d(state->frame, N, c.at(l.fs) + (size_t)(T - 1) * B * (N + 1), N + 1, B, N, st));
+        B200_TRY(launch_copy2d(state->frame, N, c.at(l.fs) + (size_t)(T - 1) * B * W + RN - N, W, B, N, st));
     }
     return B200TTS_OK;
 }

@@ -56,12 +56,12 @@ struct DecoderLayout {
     size_t q;        // [T, B, A]      attention queries
     size_t cum;      // [T+1, B, L]    cumulative attention weights BEFORE step i (forward attention: alpha BEFORE step i)
     size_t memT;     // [B, L, A]      memory . Wm^T
-    size_t fs;       // [T, B, N+1]    frame | stop logits, time-major
+    size_t fs;       // [T, B, R*(N+1)] R frames | R stop logits of each step, time-major
     // derived parameters
     size_t wcat_att; // [4D, M+D] = [W_ih_att[:, P:] | W_hh_att]
     size_t bsum_att, bsum_gen;  // [4D]
-    size_t wfs;      // [N+1, D+M] = [frame_w ; stop_w]
-    size_t bfs;      // [N+1]
+    size_t wfs;      // [R*(N+1), D+M] = [frame_w ; stop_w]
+    size_t bfs;      // [R*(N+1)]
     // scratch
     size_t qpart;    // [max(ncell_blocks, D/16), B, A]
     size_t part;     // split-K partials
@@ -69,6 +69,21 @@ struct DecoderLayout {
     size_t total;
     int split_att, split_gen, ncell_blocks;
 };
+
+// Frames per decoder step (b200tts_decoder_shape.R, 0 = 1).
+static inline int frames_per_step(const b200tts_decoder_shape& s) { return s.R > 0 ? s.R : 1; }
+// The frames <-> steps mapping: the entry points turn the caller's shape (T = target frames) into this step shape (T = S = ceil(T / R)
+// decoder steps, R normalised), and everything behind them -- layouts, persist_plan, the recurrences -- sees only steps.  The frame-level
+// edges (prep_target_kernel, the [frame ; stop] projection of width R*(N+1), split_frames / gather_frame_grads and the fed-back frame)
+// read R from it and take the frame count as a separate argument.
+static inline b200tts_decoder_shape step_shape(const b200tts_decoder_shape& frames) {
+    b200tts_decoder_shape s = frames;
+    s.R = frames_per_step(frames);
+    s.T = frames.T > 0 ? (frames.T + s.R - 1) / s.R : frames.T;
+    return s;
+}
+// width of one [frame ; stop] row of a step: R*N frame values, then R stop logits
+static inline int fs_width(const b200tts_decoder_shape& s) { return frames_per_step(s) * (s.N + 1); }
 
 static inline DecoderLayout decoder_layout(const b200tts_decoder_shape& s) {
     DecoderLayout l;
@@ -87,12 +102,13 @@ static inline DecoderLayout decoder_layout(const b200tts_decoder_shape& s) {
     l.q = take(T * B * A);
     l.cum = take((T + 1) * B * L);
     l.memT = take(B * L * A);
-    l.fs = take(T * B * (N + 1));
+    const size_t W = fs_width(s);
+    l.fs = take(T * B * W);
     l.wcat_att = take(4 * D * (M + D));
     l.bsum_att = take(4 * D);
     l.bsum_gen = take(4 * D);
-    l.wfs = take((N + 1) * (D + M));
-    l.bfs = take(N + 1);
+    l.wfs = take(W * (D + M));
+    l.bfs = take(W);
     l.ncell_blocks = cdiv(s.D, CELL_UNITS);
     l.qpart = take((size_t)cdiv(s.D, 16) * B * A);
     l.split_att = pick_splitk(s.B, 4 * s.D, s.M + s.D);

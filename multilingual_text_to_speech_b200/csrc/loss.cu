@@ -13,6 +13,7 @@ constexpr int LOSS_BLOCKS = NUM_SMS * 4;
 
 struct LossArgs {
     int B, N, T, L;
+    int R, S;               // frames per decoder step; alignment rows S = ceil(T / R) (the guided term's step grid)
     float inv2g2, pos_weight;
     int guided;
     const float* pre; const float* pre_t; const float* post; const float* post_t;
@@ -51,12 +52,12 @@ __global__ void __launch_bounds__(LT) loss_partial_kernel(const LossArgs a, floa
     const size_t nstop = (size_t)a.B * a.T;
     for (size_t i = gid; i < nstop; i += gstride) s_stop += stop_bce(a.stop[i], a.stop_t[i], a.pos_weight);
     if (a.guided) {
-        // one (b, t) row per warp iteration: lanes stride over the text positions
+        // one (b, step t) row per warp iteration: lanes stride over the text positions.  Utterance b has Tb = ceil(target_len / R) steps.
         const int lane = threadIdx.x & 31;
-        const size_t wid = gid >> 5, wstride = gstride >> 5;
-        for (size_t row = wid; row < nstop; row += wstride) {
-            const int b = (int)(row / a.T), t = (int)(row % a.T);
-            const int Tb = a.target_len[b], Lb = min(a.text_len[b], a.L);
+        const size_t wid = gid >> 5, wstride = gstride >> 5, nrows = (size_t)a.B * a.S;
+        for (size_t row = wid; row < nrows; row += wstride) {
+            const int b = (int)(row / a.S), t = (int)(row % a.S);
+            const int Tb = (a.target_len[b] + a.R - 1) / a.R, Lb = min(a.text_len[b], a.L);
             if (t >= Tb) continue;
             const float* al = a.align + row * a.L;
             float acc = 0.f;
@@ -107,11 +108,11 @@ __global__ void __launch_bounds__(LT) loss_backward_kernel(const LossArgs a, con
             d_stop[i] = g_stop * ((1.f - y) - (1.f + (a.pos_weight - 1.f) * y) * sneg);
         }
     if (d_align) {
-        const size_t nal = nstop * a.L;
+        const size_t nal = (size_t)a.B * a.S * a.L;
         for (size_t i = gid; i < nal; i += gstride) {
             const size_t row = i / a.L;
-            const int l = (int)(i % a.L), b = (int)(row / a.T), t = (int)(row % a.T);
-            const int Tb = a.target_len[b], Lb = min(a.text_len[b], a.L);
+            const int l = (int)(i % a.L), b = (int)(row / a.S), t = (int)(row % a.S);
+            const int Tb = (a.target_len[b] + a.R - 1) / a.R, Lb = min(a.text_len[b], a.L);
             d_align[i] = (a.guided && t < Tb && l < Lb) ? g_att * guided_weight(t, l, Tb, Lb, a.inv2g2) / (float)Tb : 0.f;
         }
     }
@@ -125,6 +126,7 @@ static LossArgs make_args(const b200tts_loss_shape& s, const float* pre, const f
                           const float* stop, const float* stop_t, const float* align, const int* text_len, const int* target_len) {
     LossArgs a{};
     a.B = s.B; a.N = s.N; a.T = s.T; a.L = s.L;
+    a.R = s.R > 0 ? s.R : 1; a.S = (s.T + a.R - 1) / a.R;
     a.inv2g2 = 1.f / (2.f * s.guided_g * s.guided_g); a.pos_weight = s.stop_pos_weight; a.guided = s.guided;
     a.pre = pre; a.pre_t = pre_t; a.post = post; a.post_t = post_t; a.stop = stop; a.stop_t = stop_t; a.align = align;
     a.text_len = text_len; a.target_len = target_len;
@@ -134,7 +136,7 @@ static LossArgs make_args(const b200tts_loss_shape& s, const float* pre, const f
 int loss_forward_impl(const b200tts_loss_shape& s, const float* pre, const float* pre_t, const float* post, const float* post_t,
                       const float* stop, const float* stop_t, const float* align, const int* text_len, const int* target_len, float* losses,
                       float* ws, cudaStream_t st) {
-    B200_REQUIRE(s.B > 0 && s.N > 0 && s.T > 0 && s.L > 0, "loss_forward: bad shape");
+    B200_REQUIRE(s.B > 0 && s.N > 0 && s.T > 0 && s.L > 0 && s.R >= 0, "loss_forward: bad shape");
     B200_REQUIRE(!s.guided || s.guided_g > 0.f, "loss_forward: guided attention needs a positive variance");
     const LossArgs a = make_args(s, pre, pre_t, post, post_t, stop, stop_t, align, text_len, target_len);
     loss_partial_kernel<<<LOSS_BLOCKS, LT, 0, st>>>(a, ws);
@@ -149,6 +151,7 @@ int loss_forward_impl(const b200tts_loss_shape& s, const float* pre, const float
 int loss_backward_impl(const b200tts_loss_shape& s, const float* pre, const float* pre_t, const float* post, const float* post_t,
                        const float* stop, const float* stop_t, const int* text_len, const int* target_len, const float* grad_losses,
                        float* d_pre, float* d_post, float* d_stop, float* d_align, cudaStream_t st) {
+    B200_REQUIRE(s.R >= 0, "loss_backward: bad shape");
     const LossArgs a = make_args(s, pre, pre_t, post, post_t, stop, stop_t, nullptr, text_len, target_len);
     const double nmel = (double)s.B * s.N * s.T, nstop = (double)s.B * s.T;
     loss_backward_kernel<<<NUM_SMS * 8, LT, 0, st>>>(a, grad_losses, d_pre, d_post, d_stop, d_align, (float)(4.0 / nmel), (float)(2.0 / nmel),

@@ -209,17 +209,23 @@ class ForwardAttentionStepFunction(torch.autograd.Function):
 # fused decoder
 # ------------------------------------------------------------------------------------------------
 class DecoderConfig:
-    """Non-tensor arguments of one decode: shapes, regulariser settings, dropout masks, teacher-forcing coins."""
+    """Non-tensor arguments of one decode: shapes, regulariser settings, dropout masks, teacher-forcing coins.  With r frames per
+    step (outputs_per_step) a decode of T frames runs S = ceil(T / r) steps: masks and coins have one row per step."""
 
     MASK_NAMES = ('prenet0', 'prenet1', 'att_h', 'att_c', 'gen_h', 'gen_c', 'step_prenet0', 'step_prenet1')
 
-    def __init__(self, cell_kind, training, rate_h, rate_c, prenet_rate, masks=None, teacher=None, att_extent=0):
+    def __init__(self, cell_kind, training, rate_h, rate_c, prenet_rate, masks=None, teacher=None, att_extent=0, outputs_per_step=1):
         self.att_extent = int(att_extent)    # 1: forward attention over each utterance's own length (inference of padded batches)
         self.cell_kind = int(cell_kind)
         self.training = bool(training)
         self.rate_h, self.rate_c, self.prenet_rate = float(rate_h), float(rate_c), float(prenet_rate)
-        self.masks = dict(masks or {})       # name -> uint8 CUDA tensor, time-major ([T, B, P] / [T, B, D])
-        self.teacher = teacher               # None (all teacher forced) or host bool/uint8 array [T]
+        self.masks = dict(masks or {})       # name -> uint8 CUDA tensor, time-major ([S, B, P] / [S, B, D])
+        self.teacher = teacher               # None (all teacher forced) or host bool/uint8 array [S]
+        self.outputs_per_step = int(outputs_per_step)
+
+    def steps(self, frames):
+        """Decoder steps of a decode of `frames` frames."""
+        return -(-int(frames) // self.outputs_per_step)
 
 
 def _attention_dims(byname):
@@ -231,16 +237,17 @@ def _attention_dims(byname):
 
 def _decoder_structs(cfg, shape_dims, params, memory, text_lengths, target):
     B, L, T, M, D, P, A, C, K, N = shape_dims
+    S = cfg.steps(T)
     att_kind = _attention_dims(dict(zip(DECODER_PARAM_FIELDS, params)))[0]
     shape = DecoderShape(B, L, T, M, D, P, A, C, K, N, cfg.cell_kind, int(cfg.training), cfg.rate_h, cfg.rate_c,
-                         cfg.prenet_rate, att_kind, cfg.att_extent)
+                         cfg.prenet_rate, att_kind, cfg.att_extent, cfg.outputs_per_step)
     pstruct = DecoderParams(*[ptr(p) for p in params])
     teacher_np = None
     if cfg.teacher is not None:
         teacher_np = np.ascontiguousarray(np.asarray(cfg.teacher).astype(np.uint8))
-        assert teacher_np.shape == (T,)
-    expect = {'prenet0': (T, B, P), 'prenet1': (T, B, P), 'step_prenet0': (T, B, P), 'step_prenet1': (T, B, P),
-              'att_h': (T, B, D), 'att_c': (T, B, D), 'gen_h': (T, B, D), 'gen_c': (T, B, D)}
+        assert teacher_np.shape == (S,)
+    expect = {'prenet0': (S, B, P), 'prenet1': (S, B, P), 'step_prenet0': (S, B, P), 'step_prenet1': (S, B, P),
+              'att_h': (S, B, D), 'att_c': (S, B, D), 'gen_h': (S, B, D), 'gen_c': (S, B, D)}
     mp = {}
     for name in DecoderConfig.MASK_NAMES:
         m = cfg.masks.get(name)
@@ -256,7 +263,8 @@ def _decoder_structs(cfg, shape_dims, params, memory, text_lengths, target):
 
 
 class DecoderFunction(torch.autograd.Function):
-    """Decoder._decode (reference modules/tacotron2.py:148-209) as one fused op with a hand-written backward."""
+    """Decoder._decode (reference modules/tacotron2.py:148-209) as one fused op with a hand-written backward.  Returns spectrogram
+    [B, T, N] and stop logits [B, T] per frame, and the alignment [B, S, L] per decoder step."""
 
     @staticmethod
     def forward(ctx, cfg, memory, target, text_lengths, *params):
@@ -282,7 +290,7 @@ class DecoderFunction(torch.autograd.Function):
         ws = torch.empty(nbytes, dtype=torch.uint8, device=memory.device)
         spec = torch.empty(B, T, N, device=memory.device, dtype=torch.float32)
         stop = torch.empty(B, T, device=memory.device, dtype=torch.float32)
-        align = torch.empty(B, T, L, device=memory.device, dtype=torch.float32)
+        align = torch.empty(B, cfg.steps(T), L, device=memory.device, dtype=torch.float32)
         outs = DecoderOutputs(ptr(spec), ptr(stop), ptr(align))
         with _Timed('decoder_fwd'):
             check(lib.b200tts_decoder_forward(ctypes.byref(shape), ctypes.byref(pstruct), ctypes.byref(inputs),
@@ -336,7 +344,8 @@ class DecoderState:
 
 
 def decoder_forward_chunk(cfg, memory, text_lengths, params, state, frames):
-    """`frames` free-running decoder steps continuing from `state` (updated in place); no autograd (inference)."""
+    """`frames` free-running frames (frames / r decoder steps; a multiple of r) continuing from `state` (updated in place); no autograd
+    (inference).  -> spectrogram [B, frames, N], stop [B, frames], alignment [B, frames / r, L]."""
     _require_cuda(memory, text_lengths, *params)
     with torch.no_grad():
         memory = _f32c(memory)
@@ -346,7 +355,7 @@ def decoder_forward_chunk(cfg, memory, text_lengths, params, state, frames):
         B, L, M = memory.shape
         D, P, A = byname['att_w_hh'].shape[1], byname['prenet_w1'].shape[0], byname['attn_query'].shape[0]
         _, C, K = _attention_dims(byname)
-        N = byname['frame_w'].shape[0]
+        N = byname['frame_w'].shape[0] // cfg.outputs_per_step
         T = int(frames)
         target = torch.zeros(B, N, T, device=memory.device, dtype=torch.float32)
         shape, pstruct, inputs, teacher_np = _decoder_structs(cfg, (B, L, T, M, D, P, A, C, K, N), params, memory, text_lengths, target)
@@ -357,7 +366,7 @@ def decoder_forward_chunk(cfg, memory, text_lengths, params, state, frames):
         ws = torch.empty(nbytes, dtype=torch.uint8, device=memory.device)
         spec = torch.empty(B, T, N, device=memory.device, dtype=torch.float32)
         stop = torch.empty(B, T, device=memory.device, dtype=torch.float32)
-        align = torch.empty(B, T, L, device=memory.device, dtype=torch.float32)
+        align = torch.empty(B, cfg.steps(T), L, device=memory.device, dtype=torch.float32)
         outs = DecoderOutputs(ptr(spec), ptr(stop), ptr(align))
         st = state.struct()
         check(lib.b200tts_decoder_forward_chunk(ctypes.byref(shape), ctypes.byref(pstruct), ctypes.byref(inputs), ctypes.byref(outs),
@@ -385,7 +394,8 @@ def decoder_forward(cfg, memory, target, text_lengths, params):
     outs = []
     for lo, hi in zip(bounds[:-1], bounds[1:]):
         masks = {k: v[:, lo:hi].contiguous() for k, v in cfg.masks.items()}
-        sub = DecoderConfig(cfg.cell_kind, cfg.training, cfg.rate_h, cfg.rate_c, cfg.prenet_rate, masks, cfg.teacher)
+        sub = DecoderConfig(cfg.cell_kind, cfg.training, cfg.rate_h, cfg.rate_c, cfg.prenet_rate, masks, cfg.teacher,
+                            outputs_per_step=cfg.outputs_per_step)
         outs.append(DecoderFunction.apply(sub, memory[lo:hi], target[lo:hi], text_lengths[lo:hi], *params))
     return tuple(torch.cat([o[j] for o in outs], dim=0) for j in range(3))
 
@@ -702,7 +712,7 @@ class TacotronLossFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, pre, post, stop, align, pre_target, post_target, stop_target, text_lengths, target_lengths, meta):
-        guided, g, pos_weight = meta
+        guided, g, pos_weight, r = meta
         _require_cuda(pre, post, stop, pre_target, post_target, stop_target)
         pre, post, stop, pre_target, post_target, stop_target = [_f32c(t) for t in (pre, post, stop, pre_target, post_target, stop_target)]
         align = _f32c(align) if align is not None else None
@@ -711,7 +721,7 @@ class TacotronLossFunction(torch.autograd.Function):
         dev = pre.device
         tl = text_lengths.to(device=dev, dtype=torch.int32).contiguous()
         ml = target_lengths.to(device=dev, dtype=torch.int32).contiguous()
-        shape = _lib.LossShape(B, N, T, L, int(bool(guided) and align is not None), float(g), float(pos_weight))
+        shape = _lib.LossShape(B, N, T, L, int(bool(guided) and align is not None), float(g), float(pos_weight), int(r))
         lib = _lib.load()
         ws = _bytes(lib.b200tts_loss_workspace_bytes(), dev)
         losses = torch.empty(4, device=dev, dtype=torch.float32)
@@ -739,7 +749,9 @@ class TacotronLossFunction(torch.autograd.Function):
         return d_pre, d_post, d_stop, d_align, None, None, None, None, None, None
 
 
-def tacotron_loss(pre, post, stop, align, pre_target, post_target, stop_target, text_lengths, target_lengths, guided, g, pos_weight=100.0):
-    """-> tensor [4]: mel_pre, mel_pos, stop_token, guided_att (0 when `guided` is false)."""
+def tacotron_loss(pre, post, stop, align, pre_target, post_target, stop_target, text_lengths, target_lengths, guided, g, pos_weight=100.0,
+                  outputs_per_step=1):
+    """-> tensor [4]: mel_pre, mel_pos, stop_token, guided_att (0 when `guided` is false).  align [B, ceil(T / r), L] has one row per decoder
+    step; the guided term uses each utterance's step count ceil(target_length / r) in place of its frame count."""
     return TacotronLossFunction.apply(pre, post, stop, align, pre_target, post_target, stop_target, text_lengths, target_lengths,
-                                      (guided, g, pos_weight))
+                                      (guided, g, pos_weight, outputs_per_step))

@@ -69,10 +69,18 @@ class Postnet(torch.nn.Module):
 
 class Decoder(torch.nn.Module):
     """Attention LSTM -> location-sensitive or forward attention -> generator LSTM -> frame / stop projections
-    (tacotron2.py:79-219), executed by b200tts_decoder_forward / _backward."""
+    (tacotron2.py:79-219), executed by b200tts_decoder_forward / _backward.
 
-    def __init__(self, output_dim, decoder_dim, attention, generator_rnn, attention_rnn, context_dim, prenet, prenet_dim, max_frames):
+    With `outputs_per_step` = r > 1 each decoder step predicts r frames (row block j of the projections = frame j of the step, one stop
+    logit per frame) and is fed the last frame of the previous step: T frames take ceil(T / r) sequential steps.  The alignment then has
+    one row per step."""
+
+    def __init__(self, output_dim, decoder_dim, attention, generator_rnn, attention_rnn, context_dim, prenet, prenet_dim, max_frames,
+                 outputs_per_step=1):
         super().__init__()
+        self._outputs_per_step = r = int(outputs_per_step)
+        if r < 1:
+            raise ValueError(f'outputs_per_step must be >= 1 (got {r})')
         self._prenet = prenet
         self._attention = attention
         self._output_dim = output_dim
@@ -80,8 +88,8 @@ class Decoder(torch.nn.Module):
         self._max_frames = max_frames
         self._attention_lstm = attention_rnn
         self._generator_lstm = generator_rnn
-        self._frame_prediction = Linear(context_dim + decoder_dim, output_dim)
-        self._stop_prediction = Linear(context_dim + decoder_dim, 1)
+        self._frame_prediction = Linear(context_dim + decoder_dim, r * output_dim)
+        self._stop_prediction = Linear(context_dim + decoder_dim, r)
         self._speaker_embedding, self._language_embedding = None, None
         if hp.multi_speaker and hp.speaker_embedding_dimension > 0:
             self._speaker_embedding = self._get_embedding(hp.speaker_embedding_dimension, hp.speaker_number)
@@ -115,8 +123,11 @@ class Decoder(torch.nn.Module):
             return _lib.CELL_ZONEOUT, cell.zoneout_h, cell.zoneout_c
         return _lib.CELL_DROPOUT, cell._dropout.p, 0.0
 
+    def _steps(self, frames):
+        return -(-int(frames) // self._outputs_per_step)
+
     def _masks(self, B, T, device, teacher):
-        """Keep masks for one decode, time-major.  With a mask tape active the reference's own draws are replayed."""
+        """Keep masks for one decode of T steps, time-major.  With a mask tape active the reference's own draws are replayed."""
         P, D = self._prenet._layers[0].weight.shape[0], self._decoder_dim
         kind, rate_h, rate_c = self._cell_config()
         masks = {}
@@ -154,7 +165,8 @@ class Decoder(torch.nn.Module):
                 return i + 1
         return len(stop_logits)
 
-    # frames decoded per library call in inference: the stop rule (one device -> host read of the chunk's stop logits) runs between chunks
+    # frames decoded per library call in inference (rounded down to whole steps): the stop rule (one device -> host read of the chunk's stop
+    # logits) runs between chunks
     inference_chunk = 128
 
     class _StopRule:
@@ -186,8 +198,9 @@ class Decoder(torch.nn.Module):
 
     @staticmethod
     def _tape_part(tape, done, frames, columns):
-        """Rows [done, done + frames) of a recorded step-prenet tape [T, B_tape, P], restricted to the utterances' tape columns.  A tape
-        ends where the reference's loop stopped; frames decoded past it get all-ones rows and are discarded by the stop rule."""
+        """Rows [done, done + frames) of a recorded step-prenet tape [steps, B_tape, P] (here `done` and `frames` count decoder steps),
+        restricted to the utterances' tape columns.  A tape ends where the reference's loop stopped; steps decoded past it get all-ones rows
+        and are discarded by the stop rule."""
         part = tape[done:done + frames]
         if list(columns) != list(range(tape.shape[1])):
             part = part[:, list(columns)]
@@ -207,7 +220,9 @@ class Decoder(torch.nn.Module):
         known leaves the decode: the state, memory, lengths and rules are compacted to the utterances still running, and the next
         chunk runs at the smaller batch.  `att_extent` = 1 runs forward attention over each utterance's own length; `tape_columns`
         gives each utterance's column of a recorded mask tape (default: column b for utterance b).
-        -> (spectrogram [B, T', N], stop [B, T'], alignment [B, T', L], cuts): T' = max(cuts); utterance b is zero past cuts[b]."""
+        -> (spectrogram [B, T', N], stop [B, T'], alignment [B, ceil(T' / r), L], cuts): T' = max(cuts) frames; utterance b is zero past
+        cuts[b] (its alignment past ceil(cuts[b] / r) steps).  The stop rule reads the r stop logits of each step in frame order, and
+        hp.max_output_length counts frames."""
         memory = self._memory(encoded_input, speaker, language)
         B, L, M = memory.shape
         device = memory.device
@@ -219,33 +234,36 @@ class Decoder(torch.nn.Module):
         rows = list(range(B))                  # original index of every utterance still decoding
         columns = list(range(B)) if tape_columns is None else list(tape_columns)
         outs = [[] for _ in range(B)]
-        done = 0
+        done = 0                               # frames decoded (a whole number of steps)
         params = self._param_list()
+        r = self._outputs_per_step
+        chunk_steps = max(1, self.inference_chunk // r)
         while done < self._max_frames:
-            Tc = min(self.inference_chunk, self._max_frames - done)
+            Sc = min(chunk_steps, self._steps(self._max_frames - done))
+            Tc = Sc * r
             masks = {}
             for name in ('step_prenet0', 'step_prenet1'):
                 tape = MaskSource.raw(name)
                 if MaskSource.tape is not None:
                     if tape is not None:
-                        masks[name] = self._tape_part(tape, done, Tc, [columns[r] for r in rows]).to(device=device, dtype=torch.uint8).contiguous()
+                        masks[name] = self._tape_part(tape, done // r, Sc, [columns[j] for j in rows]).to(device=device, dtype=torch.uint8).contiguous()
                 else:
-                    m = MaskSource.keep_mask(name, (Tc, len(rows), P), self._prenet._dropout_rate, device)
+                    m = MaskSource.keep_mask(name, (Sc, len(rows), P), self._prenet._dropout_rate, device)
                     if m is not None:
                         masks[name] = m
             if self.training:
                 for name in ('att_h', 'gen_h') + (('att_c', 'gen_c') if kind == _lib.CELL_ZONEOUT else ()):
-                    m = MaskSource.keep_mask(name, (Tc, len(rows), D), rate_c if name.endswith('_c') else rate_h, device)
+                    m = MaskSource.keep_mask(name, (Sc, len(rows), D), rate_c if name.endswith('_c') else rate_h, device)
                     if m is not None:
                         masks[name] = m
-            cfg = F.DecoderConfig(kind, self.training, rate_h, rate_c, self._prenet._dropout_rate, masks, np.zeros(Tc, dtype=np.uint8),
-                                  att_extent)
+            cfg = F.DecoderConfig(kind, self.training, rate_h, rate_c, self._prenet._dropout_rate, masks, np.zeros(Sc, dtype=np.uint8),
+                                  att_extent, outputs_per_step=r)
             spec, stop, align = F.decoder_forward_chunk(cfg, memory, lengths, params, state, Tc)
             done += Tc
             host_stop = stop.float().cpu()
-            for j, r in enumerate(rows):
-                rules[r].feed(host_stop[j])
-                outs[r].append((spec[j], stop[j], align[j]))
+            for j, u in enumerate(rows):
+                rules[u].feed(host_stop[j])
+                outs[u].append((spec[j], stop[j], align[j]))
             keep = self._retire(rows, rules)
             if not keep:
                 break
@@ -254,26 +272,28 @@ class Decoder(torch.nn.Module):
                 state.select(idx)
                 memory, lengths = memory.index_select(0, idx), lengths.index_select(0, idx)
                 rows = [rows[j] for j in keep]
-        cuts = [r.cut if r.cut is not None else done for r in rules]
+        cuts = [min(rule.cut if rule.cut is not None else done, self._max_frames) for rule in rules]
+        ends = lambda cut: (cut, cut, self._steps(cut))       # noqa: E731 -- rows kept of spectrogram, stop (frames), alignment (steps)
         if B == 1:
-            spectrogram, stop, alignment = (torch.cat([o[k] for o in outs[0]], 0)[:cuts[0]].unsqueeze(0) for k in range(3))
+            spectrogram, stop, alignment = (torch.cat([o[k] for o in outs[0]], 0)[:ends(cuts[0])[k]].unsqueeze(0) for k in range(3))
             return spectrogram, stop, alignment, cuts
         T = max(cuts)
         spectrogram = torch.zeros(B, T, N, device=device)
         stop = torch.zeros(B, T, device=device)
-        alignment = torch.zeros(B, T, L, device=device)
+        alignment = torch.zeros(B, self._steps(T), L, device=device)
         for b in range(B):
             for k, dst in enumerate((spectrogram, stop, alignment)):
-                dst[b, :cuts[b]] = torch.cat([o[k] for o in outs[b]], 0)[:cuts[b]]
+                e = ends(cuts[b])[k]
+                dst[b, :e] = torch.cat([o[k] for o in outs[b]], 0)[:e]
         return spectrogram, stop, alignment, cuts
 
     def _decode(self, encoded_input, mask, target, teacher_forcing_ratio, speaker, language):
         if target is None:
             return self._decode_inference(encoded_input, mask, speaker, language)[:3]
         encoded_input = self._memory(encoded_input, speaker, language)
-        B, T = encoded_input.shape[0], target.shape[2]
+        B, T = encoded_input.shape[0], self._steps(target.shape[2])
         device = encoded_input.device
-        # one coin per step, shared by the batch (tacotron2.py:171); drawn on the host: it steers the launch sequence
+        # one coin per decoder step, shared by the batch (tacotron2.py:171); drawn on the host: it steers the launch sequence
         tape_teacher = MaskSource.raw('teacher')
         if tape_teacher is not None:
             teacher = np.asarray(tape_teacher.cpu()).astype(np.uint8)
@@ -282,7 +302,8 @@ class Decoder(torch.nn.Module):
             MaskSource.counter += 1
         teacher = None if teacher.all() else teacher
         kind, rate_h, rate_c = self._cell_config()
-        cfg = F.DecoderConfig(kind, self.training, rate_h, rate_c, self._prenet._dropout_rate, self._masks(B, T, device, teacher), teacher)
+        cfg = F.DecoderConfig(kind, self.training, rate_h, rate_c, self._prenet._dropout_rate, self._masks(B, T, device, teacher), teacher,
+                              outputs_per_step=self._outputs_per_step)
         lengths = mask.sum(dim=1).to(torch.int32)
         return F.decoder_forward(cfg, encoded_input, target, lengths, self._param_list())
 
@@ -325,7 +346,7 @@ class Tacotron(torch.nn.Module):
             generator_rnn = DropoutLSTMCell(gen_cell_dimension, hp.decoder_dimension, hp.dropout_hidden)
             attention_rnn = DropoutLSTMCell(att_cell_dimension, hp.decoder_dimension, hp.dropout_hidden)
         self._decoder = Decoder(hp.num_mels, hp.decoder_dimension, self._attention, generator_rnn, attention_rnn,
-                                decoder_input_dimension, self._prenet, hp.prenet_dimension, hp.max_output_length)
+                                decoder_input_dimension, self._prenet, hp.prenet_dimension, hp.max_output_length, hp.outputs_per_step)
         self._postnet = self._get_postnet('cbhg' if hp.predict_linear else 'conv')
 
     def _get_encoder(self, name):
@@ -515,7 +536,7 @@ class TacotronLoss(torch.nn.Module):
                 alignment, speaker, speaker_prediction, encoder_outputs, classifier):
         guided = bool(hp.guided_attention_loss) and self._g_steps > 0
         terms = F.tacotron_loss(pre_prediction, post_prediction, stop, alignment if guided else None, pre_target, post_target,
-                                target_stop, source_length, target_length, guided, self._g, 100.0)
+                                target_stop, source_length, target_length, guided, self._g, 100.0, hp.outputs_per_step)
         losses = {'mel_pre': terms[0], 'mel_pos': terms[1], 'stop_token': terms[2]}
         if hp.reversal_classifier:
             losses['lang_class'] = ReversalClassifier.loss(source_length.to(stop.device), speaker, speaker_prediction)

@@ -8,6 +8,8 @@ installed on the class at import time).
 
 Extra (new) attributes, all with defaults that reproduce the reference behaviour:
   * ``b200_precision``  -- "fp32" (parity mode) or "bf16" (tensor-core perf mode) for the CUDA hot path.
+  * ``outputs_per_step`` -- reduction factor r: mel frames predicted per decoder step (1 = the reference's decoder).  A decode of T
+    frames runs ceil(T / r) sequential steps; the alignment has one row per step.
 """
 import json
 
@@ -117,6 +119,7 @@ _AUDIO = dict(
 
 _B200 = dict(
     b200_precision="fp32",
+    outputs_per_step=1,
 )
 
 _DEFAULTS = {}
