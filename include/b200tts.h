@@ -282,7 +282,10 @@ typedef struct {
 size_t b200tts_convblock_saved_bytes(const b200tts_convblock_shape* shape);
 size_t b200tts_convblock_workspace_bytes(const b200tts_convblock_shape* shape);
 /* running_mean / running_var [G*Cout] are updated in place when training (may be NULL then). keep: uint8
- * [NB, G*Cout, L] or NULL.  out [NB, G*Cf, L] with Cf = highway ? Cout/2 : Cout.                     */
+ * [NB, G*Cout, L] or NULL.  out [NB, G*Cf, L] with Cf = highway ? Cout/2 : Cout.
+ * saved (fp32, n = NB*G*Cout*L, Ct = G*Cout, a64(m) = m rounded up to a multiple of 64): floats [0, n) hold the convolution
+ * product before batch norm (stage 0; unused by stages 1 and 2), then mean [Ct] at a64(n) and invstd [Ct] at a64(n) + a64(Ct):
+ * the batch statistics when training, running_mean and 1/sqrt(running_var + eps) in eval.                                       */
 int b200tts_convblock_forward(const b200tts_convblock_shape* shape, const float* x, const float* weight,
                               const float* gamma, const float* beta, int affine_gstride, float* running_mean,
                               float* running_var, const uint8_t* keep, float* out, void* saved, void* workspace,

@@ -714,13 +714,14 @@ int convblock_backward_impl(const b200tts_convblock_shape& s, const float* x, co
     float* col = ws;
     float* dcol = col + align_up_sz(d.col_elems, 64);
     float* dz = dcol + align_up_sz(d.col_elems, 64);
+    // the per-channel sums live in the workspace whatever the stage: placed after a stage 2 dz they would land past the caller's dx
+    float* s1 = dz + align_up_sz(d.conv_elems, 64);
+    float* s2 = s1 + align_up_sz(d.Ct, 64);
+    float* scratch = s2 + align_up_sz(d.Ct, 64);
     if (s.stage == 2) {      // batch norm only: the gradient w.r.t. the normalised input IS dx
         B200_REQUIRE(dx, "convblock_backward: stage 2 needs dx");
         dz = dx;
     }
-    float* s1 = dz + align_up_sz(d.conv_elems, 64);
-    float* s2 = s1 + align_up_sz(d.Ct, 64);
-    float* scratch = s2 + align_up_sz(d.Ct, 64);
 
     BlockArgs a{conv, mean, invstd, gamma, beta, affine_gstride, (s.training && s.dropout > 0.f) ? keep : nullptr,
                 1.f / (1.f - s.dropout), x, s.NB, s.G, s.Cout, s.L, s.activation, s.highway};
