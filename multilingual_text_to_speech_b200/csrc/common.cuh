@@ -49,6 +49,11 @@ constexpr int NUM_SMS = 132;
 
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 static inline size_t align_up_sz(size_t x, size_t a) { return (x + a - 1) / a * a; }
+// grid of a 256-thread grid-stride kernel over n elements: one thread per element, at most 16 CTAs per SM
+static inline int grid_for(size_t n) {
+    size_t g = (n + 255) / 256;
+    return (int)(g > NUM_SMS * 16 ? NUM_SMS * 16 : (g < 1 ? 1 : g));
+}
 
 // ---------------------------------------------------------------------------------------------
 // device helpers
@@ -138,6 +143,13 @@ void tc_pack_cache_end();
 
 int gemm_f32(const GemmDesc& d, cudaStream_t stream);
 int gemm_bf16(const GemmDesc& d, cudaStream_t stream);
+// wgmma path (gemm_tc.cu): returns B200TTS_OK and sets *handled = true when it ran; *handled = false: the shape is not one it takes, the
+// caller runs its own path
+int gemm_tc_try(const GemmDesc& d, cudaStream_t st, bool* handled);
+// bf16 tensor maps with SWIZZLE_128B (gemm_tc.cu).  map3: dims {d0, d1, d2} (d0 contiguous), byte strides of d1 / d2, box {b0, b1, b2}.
+// mapN: rank <= 5; dims / box: `rank` entries (innermost first), strides: rank - 1 byte strides
+int tc_make_map3_bf16(void* map, const void* base, int d0, int d1, int d2, size_t stride1, size_t stride2, int b0, int b1, int b2);
+int tc_make_mapN_bf16(void* map, const void* base, int rank, const unsigned long long* dims, const unsigned long long* strides, const unsigned* box);
 // Precision mode of the library (b200tts_set_precision): 0 = fp32-exact (parity mode), 1 = bf16 tensor-core operands.
 int precision_mode();
 void set_precision_mode(int mode);

@@ -11,11 +11,6 @@ namespace b200tts {
 
 namespace {
 
-inline int grid_for(size_t n) {
-    size_t g = (n + 255) / 256;
-    return (int)(g > NUM_SMS * 16 ? NUM_SMS * 16 : (g < 1 ? 1 : g));
-}
-
 // ---------------------------------------------------------------------------------------------
 // utility kernels
 // ---------------------------------------------------------------------------------------------

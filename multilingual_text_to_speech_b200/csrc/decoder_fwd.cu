@@ -6,8 +6,6 @@
 
 namespace b200tts {
 
-int gemm_tc_try(const GemmDesc& d, cudaStream_t st, bool* handled);      // gemm_tc.cu
-
 // =============================================================================================
 // small utility kernels
 // =============================================================================================
@@ -447,11 +445,6 @@ int launch_fwd_attn(const FwdAttnArgs& a, cudaStream_t st) {
     fwd_attn_fwd_kernel<<<a.B, ATT_THREADS, smem, st>>>(a);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
-}
-
-inline int grid_for(size_t n) {
-    size_t g = (n + 255) / 256;
-    return (int)(g > NUM_SMS * 16 ? NUM_SMS * 16 : (g < 1 ? 1 : g));
 }
 
 }  // namespace

@@ -43,6 +43,12 @@ PersistLayout persist_layout(const b200tts_decoder_shape& s);
 //   att_bwd: attention-LSTM + attention reverse loop (decoder_persist_bwd.cu); training only, and only after the persistent forward
 struct PersistPlan { bool fwd = false, gen_bwd = false, att_bwd = false; };
 PersistPlan persist_plan(const b200tts_decoder_shape& s);
+// dynamic shared memory one CTA of a persistent loop may take: the 227 KB an SM offers a block, less room for the loops' static shared memory
+// (mbarriers, barrier verdict, phase counters: 1 KB as ptxas lays it out)
+constexpr size_t PERSIST_SMEM_LIMIT = 227 * 1024 - 1088;
+// Cooperative launch of a persistent loop (decoder_persist.cu): sets the kernel's dynamic shared-memory limit, checks that all `grid` CTAs
+// (and, with `pairs`, all grid / 2 clusters of 2) can be co-resident, and launches under the kernel timer `name`.
+int launch_persistent(const char* name, const void* fn, int grid, int threads, size_t smem, bool pairs, void** params, cudaStream_t st);
 
 // All offsets are in floats from the workspace base.
 struct DecoderLayout {

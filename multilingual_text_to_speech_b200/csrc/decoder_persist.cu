@@ -5,21 +5,20 @@
 //     per-step kernel chains;
 //   * persist_layout: the byte layout of the persistent workspace region (bf16 operand rows of the forward loops,
 //     attention operands, grid barrier and profile counters);
+//   * launch_persistent: the cooperative launch all three loops share;
 //   * persist_att_prep: the attention operands both the forward (decoder_persist_tc.cu) and the reverse
 //     (decoder_persist_bwd.cu) attention loops read: Wcomb = Wloc . Wc, its bf16 copy, and fragment-major bf16 copies of
 //     the memory projection and of the encoder memory.
 // Reference semantics: modules/attention.py:39-86.
 #include <cuda_bf16.h>
 #include "decoder_internal.cuh"
+#include "tc_ptx.cuh"
 
 namespace b200tts {
 
 namespace {
 
-__device__ __forceinline__ uint32_t pack2(float lo, float hi) {
-    __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-    return *reinterpret_cast<uint32_t*>(&v);
-}
+using namespace tcx;
 
 // WcB[a][40] = bf16 Wcomb[a][k] (zero for k >= KC);  memTf = fragment-major bf16 memory projection:
 // memTf[b][mt][lane][nt*4 + e] = memT[b][mt*16 + (lane>>2) + 8*(e>>1)][nt*8 + 2*(lane&3) + (e&1)]
@@ -114,6 +113,32 @@ PersistLayout persist_layout(const b200tts_decoder_shape& s) {
     l.barrier = take(256 + NUM_SMS * 8 * 8 * 4);   // barrier + abort flag, then 4 x [NUM_SMS][8] profile counters (att, gen, att roles, gen roles)
     l.total = off;
     return l;
+}
+
+int launch_persistent(const char* name, const void* fn, int grid, int threads, size_t smem, bool pairs, void** params, cudaStream_t st) {
+    B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int per_sm = 0, dev = 0, sms = 0;
+    B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, threads, smem));
+    B200_CUDA(cudaGetDevice(&dev));
+    B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    B200_REQUIRE(per_sm * sms >= grid, "%s: %d CTAs cannot be co-resident (%d per SM x %d SMs)", name, grid, per_sm, sms);
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cudaLaunchAttribute attrs[2];
+    attrs[0].id = cudaLaunchAttributeCooperative;
+    attrs[0].val.cooperative = 1;
+    attrs[1].id = cudaLaunchAttributeClusterDimension;
+    attrs[1].val.clusterDim.x = 2; attrs[1].val.clusterDim.y = 1; attrs[1].val.clusterDim.z = 1;
+    cfg.attrs = attrs; cfg.numAttrs = pairs ? 2 : 1;
+    if (pairs) {
+        int nclusters = 0;
+        B200_CUDA(cudaOccupancyMaxActiveClusters(&nclusters, fn, &cfg));
+        B200_REQUIRE(nclusters * 2 >= grid, "%s: only %d CTA pairs can be co-resident, %d needed", name, nclusters, grid / 2);
+    }
+    KernelTimer kt(name, st);
+    B200_CUDA(cudaLaunchKernelExC(&cfg, fn, params));
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
 }
 
 // Wcomb and the fragment-major projections shared by the forward and backward persistent kernels

@@ -24,53 +24,10 @@ namespace b200tts {
 
 namespace {
 
+using namespace tcx;
+
 constexpr int PT = 256;
 
-__device__ __forceinline__ void ldmatrix_x4(uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3, const void* p) {
-    const uint32_t addr = (uint32_t)__cvta_generic_to_shared(p);
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void mma_bf16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-struct NoOverlap { __device__ __forceinline__ void operator()() const {} };
-// `overlap` runs on every thread BETWEEN the CTA's arrival and its wait: work that does not depend on other CTAs (next step's operand
-// prefetch) hides under the barrier latency instead of delaying the arrival
-template <typename Overlap = NoOverlap>
-__device__ __forceinline__ bool grid_barrier(unsigned* counter, unsigned& target, unsigned nblocks, int* abort_flag, bool async_fence = false,
-                                             Overlap overlap = Overlap()) {
-    __shared__ int s_ok;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        target += nblocks;
-        if (async_fence) tcx::proxy_fence_global();     // global data written above is read by other CTAs through TMA (async proxy)
-        // arrival = ONE release-reduction (cumulative over the CTA's writes, which the __syncthreads above made visible to thread 0);
-        // the wait polls with relaxed loads and issues a single acquire fence after the last one
-        asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
-    }
-    overlap();
-    if (threadIdx.x == 0) {
-        int ok = 1;
-        const long long t0 = clock64();
-        unsigned polls = 0;
-        for (;;) {
-            unsigned v;
-            asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(counter) : "memory");
-            if (v >= target) break;
-            if ((++polls & 255u) == 0 && (clock64() - t0 > 4000000000ll || *reinterpret_cast<volatile int*>(abort_flag))) {
-                ok = 0; *abort_flag = 1; break;
-            }
-        }
-        asm volatile("fence.acquire.gpu;" ::: "memory");
-        s_ok = ok;
-    }
-    __syncthreads();
-    return s_ok != 0;
-}
-
-__device__ __forceinline__ void l2_prefetch(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 // asynchronous global -> shared copies: 16 bytes bypassing L1 (.cg; also right for data other CTAs wrote during the launch), and 8 bytes.
 // The thread that issued them waits with cp_async_wait_all; a CTA barrier after that wait makes them visible to the other threads
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
@@ -80,16 +37,6 @@ __device__ __forceinline__ void cp_async8(void* smem, const void* gmem) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem) : "memory");
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
-// remote store that completes its 4 bytes on the PEER's mbarrier (data + signal in one instruction): the pair exchanges need no cluster
-// barrier and none of the memory fence its release semantics imply
-__device__ __forceinline__ void st_async_peer_f32(const float* local_smem, const uint64_t* local_bar, uint32_t peer_rank, float v) {
-    uint32_t ra, rb;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"((uint32_t)__cvta_generic_to_shared(local_smem)), "r"(peer_rank));
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rb) : "r"((uint32_t)__cvta_generic_to_shared(local_bar)), "r"(peer_rank));
-    asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(ra), "r"(__float_as_uint(v)), "r"(rb) : "memory");
-}
-// tanh of the recomputed cell state in the reverse loops: the same ex2-based form the forward loops of the bf16 mode use (~1e-6 relative)
-__device__ __forceinline__ float tanh_exp(float x) { return 2.f * __fdividef(1.f, 1.f + __expf(-2.f * x)) - 1.f; }
 
 #define BPROF_DECL long long prof_acc[8] = {0, 0, 0, 0, 0, 0, 0, 0}; long long prof_t = clock64();
 #define BPROF_MARK(slot)                                                                                         \
@@ -139,16 +86,6 @@ struct AttBwdArgs {
     long long* prof;
 };
 
-__device__ __forceinline__ uint32_t pack2(float lo, float hi) {
-    __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-    return *reinterpret_cast<uint32_t*>(&v);
-}
-__device__ __forceinline__ float tanh_fast(float x) {
-    float y;
-    asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
-    return y;
-}
-
 // UNC: outputs per n-block of the product (wgmma N), compile-time: 80, or 96 for memory dim 512
 template <int UNC>
 __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_constant__ CUtensorMap tmG, const AttBwdArgs p) {
@@ -156,6 +93,7 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
     unsigned char* smem_raw = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw0) + 1023) & ~(uintptr_t)1023);
     __shared__ uint64_t full_bar[2], xb1, xb2;   // full_bar[r]: rank r's half of the P2 operand; xb1 / xb2: arrival of the peer's softmax dot /
                                                  // query-gradient partial + G halo tile
+    __shared__ int s_ok;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int cta = blockIdx.x;
     // the CTA pair (2k, 2k+1) = one cluster shares the K-slice kb and takes two n-blocks: both need the same operand in P2
@@ -215,12 +153,12 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
             wqf[idx] = make_uint4(f[0], f[1], f[2], f[3]);
         }
     uint32_t prod_it = 0;
-    if (tid == 0) { tcx::mbar_init(&xb1, 1); tcx::mbar_init(&xb2, 1); tcx::mbar_init_fence(); }
-    if (tid == 0) { tcx::mbar_init(&full_bar[0], 1); tcx::mbar_init(&full_bar[1], 1); tcx::mbar_init_fence(); }
-    tcx::proxy_fence_shared();           // the weight tiles were written through the generic proxy; wgmma reads them through the async proxy
+    if (tid == 0) { mbar_init(&xb1, 1); mbar_init(&xb2, 1); mbar_init_fence(); }
+    if (tid == 0) { mbar_init(&full_bar[0], 1); mbar_init(&full_bar[1], 1); mbar_init_fence(); }
+    proxy_fence_shared();           // the weight tiles were written through the generic proxy; wgmma reads them through the async proxy
     __syncthreads();
     // one-time: the peer's mbarriers are initialised before the first remote st.async or multicast TMA of this CTA targets them
-    tcx::cluster_arrive(); tcx::cluster_wait();
+    cluster_arrive(); cluster_wait();
 
     const float inv_h = 1.f / (1.f - p.rate_h), inv_c = 1.f / (1.f - p.rate_c);
     constexpr int MAXE = 3;               // (b, u) pairs per thread: B * 8 / 256 <= 3 for B <= 64... (B <= 96)
@@ -412,8 +350,8 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
             float pdot = 0.f;
             for (int l = t_lo * 16 + tid; l < t_hi * 16 && l < len; l += PT) pdot = fmaf(s_w[l], s_de[l], pdot);
             pdot = block_sum(pdot, s_red);
-            if (tid == 0) { tcx::mbar_expect_tx(&xb1, 4); st_async_peer_f32(s_dotx, &xb1, (uint32_t)(hf ^ 1), pdot); }
-            tcx::mbar_wait(&xb1, (uint32_t)(p.T - 1 - i) & 1);
+            if (tid == 0) { mbar_expect_tx(&xb1, 4); st_async_peer_f32(s_dotx, &xb1, (uint32_t)(hf ^ 1), pdot); }
+            mbar_wait(&xb1, (uint32_t)(p.T - 1 - i) & 1);
             const float dot = pdot + s_dotx[0];           // a + b == b + a: both ranks get the same value
             for (int l = t_lo * 16 + tid; l < t_hi * 16; l += PT) {
                 const float d = l < len ? s_w[l] * (s_de[l] - dot) : 0.f;
@@ -496,14 +434,14 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
                     for (int e = 0; e < 4; ++e) s_G[(l0 - g_lo + g + 8 * (e >> 1)) * GLD + nt * 8 + 2 * tq + (e & 1)] = gacc[nt][e];
             }
             // the G tiles were written through the generic proxy; the bulk copy below reads the boundary tile through the async proxy
-            tcx::proxy_fence_shared();
+            proxy_fence_shared();
             __syncthreads();                               // every warp is done with s_de / s_qb / s_vv / Ph / Pl, and G is complete
             {   // the boundary tile of G goes to the peer's halo rows (rank 0 sends its last tile, rank 1 its first) as ONE bulk copy of
                 // 16 x GLD floats (2112 B: rows of 132 B, tile and s_G 16-byte aligned) that completes on the peer's xb2
                 const int ht = hf ? HT0 : HT0 - 1;             // tile sent
                 const int peer_g_lo = hf ? 0 : (HT0 - 1) * 16;
                 if (tid == 0 && ht >= t_lo && ht < t_hi)
-                    tcx::bulk_copy_to_peer(s_G + (size_t)(ht * 16 - peer_g_lo) * GLD, s_G + (size_t)(ht * 16 - g_lo) * GLD, 16 * GLD * 4, &xb2,
+                    bulk_copy_to_peer(s_G + (size_t)(ht * 16 - peer_g_lo) * GLD, s_G + (size_t)(ht * 16 - g_lo) * GLD, 16 * GLD * 4, &xb2,
                                            (uint32_t)(hf ^ 1));
             }
             // dq[a] = sum_l ds[l, a]: reduce over the 8 row lanes, then over warps
@@ -527,9 +465,9 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
             {   // what the PEER sends here: its A query-gradient partials, and its boundary tile if it has one (rank 0 always does; rank 1 only
                 // when it owns tiles at all)
                 const bool peer_sends_tile = hf ? true : (HT0 < p.MT);
-                if (tid == 0) tcx::mbar_expect_tx(&xb2, (uint32_t)(A * 4 + (peer_sends_tile ? 16 * GLD * 4 : 0)));
+                if (tid == 0) mbar_expect_tx(&xb2, (uint32_t)(A * 4 + (peer_sends_tile ? 16 * GLD * 4 : 0)));
             }
-            tcx::mbar_wait(&xb2, (uint32_t)(p.T - 1 - i) & 1);
+            mbar_wait(&xb2, (uint32_t)(p.T - 1 - i) & 1);
             if (hf == 0 && tid < A) p.dq[((size_t)i * B + b) * A + tid] = pdq + s_dqx[tid];
             // d cum_{i-1}[j] = d cum_i[j] + sum_k G[j + half - k, k] for the own positions (their G rows: own tiles + the halo tile)
             for (int j = t_lo * 16 + tid; j < t_hi * 16 && j < L; j += PT) {
@@ -545,7 +483,7 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
             for (int j = t_lo * 16 + tid; j < t_hi * 16 && j < L; j += PT) dcum[j] = s_stage[j];
         }
         BPROF_MARK(1);
-        if (!grid_barrier(p.barrier, target, nblocks, p.abort_flag)) break;
+        if (!grid_barrier(p.barrier, target, nblocks, p.abort_flag, &s_ok, false)) break;
         BPROF_MARK(2);
 
         // =========================== PB: attention-LSTM cell backward ===========================
@@ -660,7 +598,7 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
         BPROF_MARK(3);
         // the copies of the next cell backward's operands are issued between this CTA's arrival and its wait: the barrier's leading
         // __syncthreads means every thread is done reading the staging buffer, and they complete while PA runs
-        if (!grid_barrier(p.barrier, target, nblocks, p.abort_flag, true, [&]() { pb_stage(i - 1); })) break;
+        if (!grid_barrier(p.barrier, target, nblocks, p.abort_flag, &s_ok, true, [&]() { pb_stage(i - 1); })) break;
         BPROF_MARK(4);
         if (i == 0) break;
 
@@ -671,13 +609,13 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
         // last touched their slot (attention scratch, dq staging) before the grid barrier above, so the peer's slot is free.
         // wgmma: D[b, n] (registers of warpgroup 0: 64 utterances x UN outputs) = sum over the tiles, stored straight to the partials
         if (warp == 0) {
-            if (tcx::elect_one()) {
+            if (elect_one()) {
                 const int r = cta & 1;
-                tcx::proxy_fence_shared();       // the slot was last touched through the generic proxy (attention scratch, dq staging)
-                tcx::proxy_fence_global();
-                tcx::mbar_expect_tx(&full_bar[0], (uint32_t)(NKT / 2) * 8192);
-                tcx::mbar_expect_tx(&full_bar[1], (uint32_t)(NKT / 2) * 8192);
-                tcx::tma_load_5d_mc(reinterpret_cast<unsigned char*>(As) + (size_t)r * (NKT / 2) * 8192, &tmG, &full_bar[r], 0x3, 0, i * p.dgb_rows, 0,
+                proxy_fence_shared();       // the slot was last touched through the generic proxy (attention scratch, dq staging)
+                proxy_fence_global();
+                mbar_expect_tx(&full_bar[0], (uint32_t)(NKT / 2) * 8192);
+                mbar_expect_tx(&full_bar[1], (uint32_t)(NKT / 2) * 8192);
+                tma_load_5d_mc(reinterpret_cast<unsigned char*>(As) + (size_t)r * (NKT / 2) * 8192, &tmG, &full_bar[r], 0x3, 0, i * p.dgb_rows, 0,
                                     kb, 2 * r);
             }
             __syncwarp();
@@ -685,21 +623,21 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
         if (warp < 4) {
             constexpr int NR = UNC / 2;
             float acc[NR];
-            tcx::mbar_wait(&full_bar[0], prod_it & 1);
-            tcx::wgmma_fence();
+            mbar_wait(&full_bar[0], prod_it & 1);
+            wgmma_fence();
             for (int c = 0; c < NKT; ++c) {
-                if (c == NKT / 2) tcx::mbar_wait(&full_bar[1], prod_it & 1);
-                const uint64_t adesc = tcx::make_sw128_desc(tcx::smem_u32(reinterpret_cast<unsigned char*>(As) + (size_t)c * 8192));
-                const uint64_t bdesc = tcx::make_sw128_desc(tcx::smem_u32(sW + (size_t)c * UN * 128));
+                if (c == NKT / 2) mbar_wait(&full_bar[1], prod_it & 1);
+                const uint64_t adesc = make_sw128_desc(smem_u32(reinterpret_cast<unsigned char*>(As) + (size_t)c * 8192));
+                const uint64_t bdesc = make_sw128_desc(smem_u32(sW + (size_t)c * UN * 128));
 #pragma unroll
                 for (int k = 0; k < 4; ++k) {
-                    if constexpr (UNC == TUN_WIDE) tcx::wgmma_m64n96<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (c | k) != 0);
-                    else if constexpr (UNC == TUN) tcx::wgmma_m64n80<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (c | k) != 0);
+                    if constexpr (UNC == TUN_WIDE) wgmma_m64n96<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (c | k) != 0);
+                    else if constexpr (UNC == TUN) wgmma_m64n80<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (c | k) != 0);
                 }
             }
-            tcx::wgmma_commit();
-            tcx::wgmma_wait<0>();
-            tcx::wgmma_fence_acc(acc);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_acc(acc);
             // fragment: utterance b = 16 warp + lane / 4 + 8 ((r / 2) % 2), output n0 + 8 (r / 4) + 2 (lane % 4) + r % 2 (NOUT % 4 == 0: a pair
             // is either wholly inside or wholly outside)
             const int brow = 16 * warp + (lane >> 2), ncol = n0 + 2 * (lane & 3);
@@ -711,7 +649,7 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
         }
         ++prod_it;
         BPROF_MARK(5);
-        if (!grid_barrier(p.barrier, target, nblocks, p.abort_flag)) break;
+        if (!grid_barrier(p.barrier, target, nblocks, p.abort_flag, &s_ok, false)) break;
         BPROF_MARK(6);
     }
     BPROF_FLUSH;
@@ -719,7 +657,7 @@ __global__ void __launch_bounds__(PT, 1) att_bwd_loop_kernel(const __grid_consta
     // flag, which every CTA checks at each grid barrier, so both ranks of a pair stop at the same barrier -- unless the flag is raised just
     // as that barrier completes: the rank that went on then waits for the peer's half of the next operand and ends in the trap of
     // mbar_wait (~2 s), not in a hang
-    tcx::cluster_arrive(); tcx::cluster_wait();
+    cluster_arrive(); cluster_wait();
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -1015,10 +953,8 @@ bool persist_att_bwd_supported(const b200tts_decoder_shape& s) {
     // the cell-backward phase stages the query gradients [B][A] fp32 in the (then idle) TMA slot.  The bound keeps 2 KB to spare (a [64][8]
     // slab), which holds B <= 60 at D = 512: the shapes this loop accepts are the ones its tests cover
     if ((size_t)s.B * s.A * 4 + 64 * 8 * 4 > g.region) return false;
-    return g.smem <= 227 * 1024;
+    return g.smem <= PERSIST_SMEM_LIMIT;
 }
-
-int tc_make_mapN_bf16(void* map, const void* base, int rank, const unsigned long long* dims, const unsigned long long* strides, const unsigned* box);
 
 int persist_att_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
                          const DecoderLayout& fl, const float* fws, const PersistLayout& pl, const unsigned char* pws,
@@ -1056,15 +992,8 @@ int persist_att_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_p
     B200_CUDA(cudaMemsetAsync(a.barrier, 0, 256, st));
     att_bwd_prep_kernel<<<NUM_SMS * 4, 256, 0, st>>>(wcb, wcb2, memTf, wcombT, fws + fl.memT, B, L, A, s.K, x.MT);
     B200_LAUNCH_CHECK();
-    const size_t smem = geo.smem;
-    void* fn = geo.UN == TUN ? (void*)att_bwd_loop_kernel<TUN> : (void*)att_bwd_loop_kernel<TUN_WIDE>;
-    B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int grid = geo.grid;
-    int per_sm = 0, dev = 0, sms = 0;
-    B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, PT, smem));
-    B200_CUDA(cudaGetDevice(&dev));
-    B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    B200_REQUIRE(per_sm * sms >= grid && grid % 2 == 0 && grid / 2 >= B, "persistent attention backward: %d CTAs cannot be co-resident / paired", grid);
+    B200_REQUIRE(grid % 2 == 0 && grid / 2 >= B, "persistent attention backward: %d CTAs cannot form %d pairs", grid, B);
     // bf16 gate-gradient history dgb [T, B, 4D] as {64 k, T * B rows, UK/64 halves, KBA k-slices, 4 gates}: element (row, g, kb, h, c) at
     // row * 4D + g * D + kb * UK + h * 64 + c; one box = {64, 64 rows, UK/64, 1, 2} = two gates of a CTA's K-slice for one step (each rank
     // of a pair fetches two of the four)
@@ -1074,22 +1003,9 @@ int persist_att_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_p
     const unsigned box[5] = {64u, 64u, (unsigned)(geo.UK / 64), 1u, 2u};
     B200_TRY(tc_make_mapN_bf16(&tm, a.dgb, 5, dims, strides, box));
     void* params[] = {&tm, &a};
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(PT); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attrs[2];
-    attrs[0].id = cudaLaunchAttributeCooperative;
-    attrs[0].val.cooperative = 1;
-    attrs[1].id = cudaLaunchAttributeClusterDimension;          // the attention backward of an utterance runs on a CTA pair
-    attrs[1].val.clusterDim.x = 2; attrs[1].val.clusterDim.y = 1; attrs[1].val.clusterDim.z = 1;
-    cfg.attrs = attrs; cfg.numAttrs = 2;
-    int nclusters = 0;
-    B200_CUDA(cudaOccupancyMaxActiveClusters(&nclusters, fn, &cfg));
-    B200_REQUIRE(nclusters * 2 >= grid, "persistent attention backward: only %d CTA pairs can be co-resident, %d needed", nclusters, grid / 2);
-    {
-        KernelTimer kt("att_bwd_loop_kernel", st);
-        B200_CUDA(cudaLaunchKernelExC(&cfg, fn, params));
-    }
-    B200_LAUNCH_CHECK();
+    // the attention backward of an utterance runs on a CTA pair
+    const void* fn = geo.UN == TUN ? (void*)att_bwd_loop_kernel<TUN> : (void*)att_bwd_loop_kernel<TUN_WIDE>;
+    B200_TRY(launch_persistent("att_bwd_loop_kernel", fn, grid, PT, geo.smem, true, params, st));
     // parallel post pass
     AttPostArgs pp{};
     pp.B = B; pp.T = T; pp.L = L; pp.A = A; pp.KC = s.K; pp.MT = x.MT;

@@ -20,9 +20,9 @@
 
 namespace b200tts {
 
-int tc_make_map3_bf16(void* map, const void* base, int d0, int d1, int d2, size_t stride1, size_t stride2, int b0, int b1, int b2);
-
 namespace {
+
+using namespace tcx;
 
 constexpr int NCW = 8;
 constexpr int CT = 32 * NCW;
@@ -48,39 +48,6 @@ struct TcBwdArgs {
     unsigned* barrier; int* abort_flag;
     long long* prof;
 };
-
-// ------------------------------------------------------------------------------------------------
-// PTX wrappers (mbarrier, TMA, fences and the cluster barrier: tc_ptx.cuh)
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void l2_prefetch(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
-// tanh of the recomputed cell state in the reverse loops: the same ex2-based form the forward loops of the bf16 mode use (~1e-6 relative)
-__device__ __forceinline__ float tanh_exp(float x) { return 2.f * __fdividef(1.f, 1.f + __expf(-2.f * x)) - 1.f; }
-// named barrier among the compute warps only
-__device__ __forceinline__ void csync() { asm volatile("bar.sync 1, %0;" ::"n"(CT) : "memory"); }
-
-__device__ __forceinline__ bool grid_barrier(unsigned* counter, unsigned& target, unsigned nblocks, int* abort_flag, int* s_ok) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        target += nblocks;
-        tcx::proxy_fence_global();          // the bf16 gate gradients written above are read by other CTAs through TMA (async proxy)
-        asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
-        int ok = 1;
-        const long long t0 = clock64();
-        unsigned polls = 0;
-        for (;;) {
-            unsigned v;
-            asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(counter) : "memory");
-            if (v >= target) break;
-            if ((++polls & 255u) == 0 && (clock64() - t0 > 4000000000ll || *reinterpret_cast<volatile int*>(abort_flag))) {
-                ok = 0; *abort_flag = 1; break;
-            }
-        }
-        asm volatile("fence.acquire.gpu;" ::: "memory");
-        *s_ok = ok;
-    }
-    __syncthreads();
-    return *s_ok != 0;
-}
 
 __global__ void __launch_bounds__(PT, 1) lstm_bwd_loop_tc_kernel(const __grid_constant__ CUtensorMap tmG, const TcBwdArgs p) {
     extern __shared__ __align__(1024) unsigned char smem_raw0[];
@@ -114,12 +81,12 @@ __global__ void __launch_bounds__(PT, 1) lstm_bwd_loop_tc_kernel(const __grid_co
         *reinterpret_cast<__nv_bfloat16*>(sW + (size_t)kb * WTILE + r * 128 + ((chunk ^ (r & 7)) << 4) + e * 2) = __float2bfloat16_rn(w);
     }
     if (tid == 0) {
-        tcx::mbar_init(&full_bar, 1);
-        tcx::mbar_init_fence();
+        mbar_init(&full_bar, 1);
+        mbar_init_fence();
     }
-    tcx::proxy_fence_shared();              // the weight tiles were written through the generic proxy; wgmma reads them through the async proxy
+    proxy_fence_shared();              // the weight tiles were written through the generic proxy; wgmma reads them through the async proxy
     __syncthreads();
-    tcx::cluster_arrive(); tcx::cluster_wait();     // one-time: the peer's mbarrier is initialised before this CTA's first multicast targets it
+    cluster_arrive(); cluster_wait();     // one-time: the peer's mbarrier is initialised before this CTA's first multicast targets it
 
     const float inv_h = 1.f / (1.f - p.rate_h), inv_c = 1.f / (1.f - p.rate_c);
     // cell-backward operands of this thread's two (b, u) pairs, fetched one step ahead (during the previous product)
@@ -215,7 +182,7 @@ __global__ void __launch_bounds__(PT, 1) lstm_bwd_loop_tc_kernel(const __grid_co
             }
         }
         PROF_MARK(0);
-        if (!grid_barrier(bar_counter, target, nblocks, p.abort_flag, &s_ok)) break;
+        if (!grid_barrier(bar_counter, target, nblocks, p.abort_flag, &s_ok, true)) break;
         PROF_MARK(1);
         if (i == 0) break;
 
@@ -225,26 +192,26 @@ __global__ void __launch_bounds__(PT, 1) lstm_bwd_loop_tc_kernel(const __grid_co
         // previous products completed before they arrived at the grid barriers in between.
         if (is_mma) {
             if (warp == NCW) {
-                tcx::proxy_fence_global();
-                if (tcx::elect_one()) {
+                proxy_fence_global();
+                if (elect_one()) {
                     const int r = cta & 1;
-                    tcx::mbar_expect_tx(&full_bar, (uint32_t)NNB * ATILE);
-                    tcx::tma_load_3d_mc(ring + (size_t)r * (NNB / 2) * ATILE, &tmG, &full_bar, 0x3, 0, i * p.dgb_rows + b0, gsel * NNB + r * (NNB / 2));
+                    mbar_expect_tx(&full_bar, (uint32_t)NNB * ATILE);
+                    tma_load_3d_mc(ring + (size_t)r * (NNB / 2) * ATILE, &tmG, &full_bar, 0x3, 0, i * p.dgb_rows + b0, gsel * NNB + r * (NNB / 2));
                 }
                 __syncwarp();
             }
-            tcx::mbar_wait(&full_bar, it & 1);
+            mbar_wait(&full_bar, it & 1);
             float acc[16];                   // the first instruction overwrites (scale-d = 0)
-            tcx::wgmma_fence();
+            wgmma_fence();
             for (int c = 0; c < NNB; ++c) {
-                const uint64_t adesc = tcx::make_sw128_desc(tcx::smem_u32(sW + (size_t)c * WTILE));
-                const uint64_t bdesc = tcx::make_sw128_desc(tcx::smem_u32(ring + (size_t)c * ATILE));
+                const uint64_t adesc = make_sw128_desc(smem_u32(sW + (size_t)c * WTILE));
+                const uint64_t bdesc = make_sw128_desc(smem_u32(ring + (size_t)c * ATILE));
 #pragma unroll
-                for (int k = 0; k < KB / 16; ++k) tcx::wgmma_m64n32<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (c | k) != 0);
+                for (int k = 0; k < KB / 16; ++k) wgmma_m64n32<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (c | k) != 0);
             }
-            tcx::wgmma_commit();
-            tcx::wgmma_wait<0>();
-            tcx::wgmma_fence_acc(acc);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_acc(acc);
             // accumulator row = output n0 + row, column = utterance b0 + column (fragment layout: tc_ptx.cuh)
             const int row = 16 * (warp - NCW) + (lane >> 2), n = n0 + row;
 #pragma unroll
@@ -260,7 +227,7 @@ __global__ void __launch_bounds__(PT, 1) lstm_bwd_loop_tc_kernel(const __grid_co
         }
         ++it;
         PROF_MARK(3);
-        if (!grid_barrier(bar_counter, target, nblocks, p.abort_flag, &s_ok)) break;
+        if (!grid_barrier(bar_counter, target, nblocks, p.abort_flag, &s_ok, true)) break;
         PROF_MARK(4);
     }
     if (p.prof && tid == 0)
@@ -270,7 +237,7 @@ __global__ void __launch_bounds__(PT, 1) lstm_bwd_loop_tc_kernel(const __grid_co
     // flag, which every CTA checks at each grid barrier, so both ranks of a pair stop at the same barrier -- unless the flag is raised just
     // as that barrier completes: the rank that went on then waits for the peer's half of the next operand and ends in the trap of
     // mbar_wait (~2 s), not in a hang
-    tcx::cluster_arrive(); tcx::cluster_wait();
+    cluster_arrive(); cluster_wait();
 }
 
 size_t bwd_tc_smem_bytes(int D) { return 1024 + (size_t)(D / KB) * (WTILE + ATILE); }
@@ -284,7 +251,7 @@ bool tc_persist_gen_bwd_supported(const b200tts_decoder_shape& s) {
     if ((s.D / KB) % 2 != 0) return false;                                          // the n-blocks pair up (one operand half per rank)
     const int NBH = (s.B + BT - 1) / BT;
     if (NG * (s.D / KB) * NBH > NUM_SMS) return false;
-    return bwd_tc_smem_bytes(s.D) <= 227 * 1024 - 1088;
+    return bwd_tc_smem_bytes(s.D) <= PERSIST_SMEM_LIMIT;
 }
 
 size_t persist_bwd_gen_extra_bytes(const b200tts_decoder_shape& s) { return part_bytes(s) + 256 + NUM_SMS * 8 * 8; }
@@ -310,26 +277,10 @@ int tc_persist_gen_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decode
     // {64 columns, T * B rows, 4D/64 k-blocks}: k-block stride 128 B, row stride 4D * 2 B; a box is half of one gate (NNB/2 k-blocks)
     CUtensorMap tm;
     B200_TRY(tc_make_map3_bf16(&tm, a.dgb, KB, s.T * B, 4 * D / KB, (size_t)4 * D * 2, 128, KB, BT, a.NNB / 2));
-    const size_t smem = bwd_tc_smem_bytes(D);
-    void* fn = (void*)lstm_bwd_loop_tc_kernel;
-    B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const int grid = NG * a.NNB * a.NBH;
     void* params[] = {&tm, &a};
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(PT); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attrs[2];
-    attrs[0].id = cudaLaunchAttributeCooperative;
-    attrs[0].val.cooperative = 1;
-    attrs[1].id = cudaLaunchAttributeClusterDimension;          // CTA pairs share the per-step operand (multicast TMA)
-    attrs[1].val.clusterDim.x = 2; attrs[1].val.clusterDim.y = 1; attrs[1].val.clusterDim.z = 1;
-    cfg.attrs = attrs; cfg.numAttrs = 2;
-    int nclusters = 0;
-    B200_CUDA(cudaOccupancyMaxActiveClusters(&nclusters, fn, &cfg));
-    B200_REQUIRE(nclusters * 2 >= grid, "wgmma persistent backward: only %d CTA pairs can be co-resident, %d needed", nclusters, grid / 2);
-    KernelTimer kt("lstm_bwd_loop_tc_kernel", st);
-    B200_CUDA(cudaLaunchKernelExC(&cfg, fn, params));
-    B200_LAUNCH_CHECK();
-    return B200TTS_OK;
+    // CTA pairs share the per-step operand (multicast TMA)
+    return launch_persistent("lstm_bwd_loop_tc_kernel", (const void*)lstm_bwd_loop_tc_kernel, NG * a.NNB * a.NBH, PT, bwd_tc_smem_bytes(D), true,
+                             params, st);
 }
 
 }  // namespace b200tts

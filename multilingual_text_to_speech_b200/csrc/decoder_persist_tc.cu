@@ -22,10 +22,9 @@
 
 namespace b200tts {
 
-// gemm_tc.cu: 3-D bf16 tensor map, dims {d0, d1, d2} (d0 contiguous), byte strides of d1 / d2, box {b0, b1, b2}, SWIZZLE_128B
-int tc_make_map3_bf16(void* map, const void* base, int d0, int d1, int d2, size_t stride1, size_t stride2, int b0, int b1, int b2);
-
 namespace {
+
+using namespace tcx;
 
 constexpr int NCW = 8;                  // compute warps
 constexpr int CT = 32 * NCW;            // compute threads
@@ -68,67 +67,6 @@ struct TcLoopArgs {
     long long* prof2;                         // [grid][8] MMA warpgroup: operand waits / products of the ctx (0, 1) and h (2, 3) parts
 };
 
-// ------------------------------------------------------------------------------------------------
-// PTX wrappers
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-// Out of line on purpose: an inlined trap makes ptxas drop the setmaxnreg.inc limit of the code around it back to the launch's 168
-// registers (measured with -Xptxas -v: the compute warps then spill), a call to this function does not.
-__device__ __noinline__ __attribute__((noreturn)) void watchdog_trap() { __trap(); }
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    const uint32_t addr = smem_u32(bar);
-    const long long t0 = clock64();
-    for (;;) {
-        uint32_t done;
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done)
-            : "r"(addr), "r"(parity)
-            : "memory");
-        if (done) return;
-        if (clock64() - t0 > 4000000000ll) watchdog_trap();       // ~2 s: a protocol bug must not hang the GPU
-    }
-}
-__device__ __forceinline__ void tma_load_3d(void* smem, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-__device__ __forceinline__ void proxy_fence_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
-__device__ __forceinline__ void proxy_fence_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void l2_prefetch(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
-// thread-block cluster (CTA pair) primitives: split arrive / wait barrier and a distributed-shared-memory store
-__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
-__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
-__device__ __forceinline__ void st_peer_f32(const float* local_smem, uint32_t peer_rank, float v) {
-    uint32_t ra;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(local_smem)), "r"(peer_rank));
-    asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(ra), "f"(v) : "memory");
-}
-// remote store that completes bytes on the PEER's mbarrier: data + signal in one instruction, no cluster barrier (and none of the memory
-// fence its release semantics imply) on the exchange path
-__device__ __forceinline__ void st_async_peer_f32(const float* local_smem, const uint64_t* local_bar, uint32_t peer_rank, float v) {
-    uint32_t ra, rb;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(local_smem)), "r"(peer_rank));
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rb) : "r"(smem_u32(local_bar)), "r"(peer_rank));
-    asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(ra), "r"(__float_as_uint(v)), "r"(rb) : "memory");
-}
-// named barrier among the compute warps only
-__device__ __forceinline__ void csync() { asm volatile("bar.sync 1, %0;" ::"n"(CT) : "memory"); }
 // per-thread register limit of the executing warpgroup (all its warps execute it): dec returns registers to the CTA's pool, inc waits until
 // the pool holds enough
 template <int N>
@@ -136,41 +74,16 @@ __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.
 template <int N>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
-__device__ __forceinline__ void ldmatrix_x4(uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3, const void* p) {
-    const uint32_t addr = (uint32_t)__cvta_generic_to_shared(p);
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void mma_bf16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ unsigned ld_acquire(const unsigned* p) {
-    unsigned v;
-    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];\n" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ uint32_t pack2(float lo, float hi) {
-    __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-    return *reinterpret_cast<uint32_t*>(&v);
-}
-__device__ __forceinline__ float tanh_fast(float x) {
-    float y;
-    asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
-    return y;
-}
-
-// gate nonlinearities of the bf16 perf mode: ex2-based, ~1e-6 relative error (the operands of the products are bf16 anyway)
+// gate nonlinearity of the bf16 perf mode: ex2-based, ~1e-6 relative error (the operands of the products are bf16 anyway); tanh: tanh_exp
 __device__ __forceinline__ float sigmoid_fast(float x) { return __fdividef(1.f, 1.f + __expf(-x)); }
-__device__ __forceinline__ float tanh_exp(float x) { return 2.f * __fdividef(1.f, 1.f + __expf(-2.f * x)) - 1.f; }
 
 // Block-wide max / sum among the CT compute threads (named barrier 1); `scratch` holds >= 33 floats.
 __device__ __forceinline__ float cblock_max(float v, float* scratch) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     v = warp_max(v);
-    csync();
+    csync<CT>();
     if (lane == 0) scratch[warp] = v;
-    csync();
+    csync<CT>();
     float t = scratch[lane & (NCW - 1)];
 #pragma unroll
     for (int o = NCW / 2; o > 0; o >>= 1) t = fmaxf(t, __shfl_xor_sync(0xffffffffu, t, o));
@@ -179,56 +92,13 @@ __device__ __forceinline__ float cblock_max(float v, float* scratch) {
 __device__ __forceinline__ float cblock_sum(float v, float* scratch) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     v = warp_sum(v);
-    csync();
+    csync<CT>();
     if (lane == 0) scratch[warp] = v;
-    csync();
+    csync<CT>();
     float t = scratch[lane & (NCW - 1)];
 #pragma unroll
     for (int o = NCW / 2; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
     return t;
-}
-
-// Monotonic-counter grid barrier over ALL threads of every CTA.  Returns false if the watchdog fired.
-// Arrival is ONE release-reduction (cumulative: it orders the whole CTA's writes, which the preceding __syncthreads made
-// visible to thread 0); the wait polls with relaxed loads and issues a single acquire fence after the last one.
-struct NoOverlap { __device__ __forceinline__ void operator()() const {} };
-// `overlap` runs on every thread BETWEEN the CTA's arrival and its wait: work that does not depend on other CTAs (next step's operand
-// prefetch) hides under the barrier latency instead of delaying the arrival
-template <typename Overlap = NoOverlap>
-__device__ __forceinline__ bool grid_barrier(unsigned* counter, unsigned& target, unsigned nblocks, int* abort_flag, int* s_ok, Overlap overlap = Overlap()) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        target += nblocks;
-        proxy_fence_global();          // the bf16 operand rows written above are read by other CTAs through TMA (async proxy)
-        asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
-    }
-    overlap();
-    if (threadIdx.x == 0) {
-        int ok = 1;
-        const long long t0 = clock64();
-        unsigned polls = 0;
-        for (;;) {                      // nothing but the counter load in the polling loop: its round trip is the barrier latency
-            unsigned v;
-            asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(counter) : "memory");
-            if (v >= target) break;
-            if ((++polls & 255u) == 0 && (clock64() - t0 > 4000000000ll || *reinterpret_cast<volatile int*>(abort_flag))) {
-                ok = 0; *abort_flag = 1; break;
-            }
-        }
-        asm volatile("fence.acquire.gpu;" ::: "memory");
-        *s_ok = ok;
-    }
-    __syncthreads();
-    return *s_ok != 0;
-}
-// The MMA warpgroup's side of grid_barrier: it arrives at the same two CTA-wide barriers from its own loop, in the same order, and leaves
-// the arrival and the polling to thread 0.  Staying in the CTA barrier (instead of waiting on an mbarrier that thread 0 signals) keeps the
-// ordering the single loop had: the TMA issued after the barrier reads other CTAs' rows only after thread 0's acquire fence, and the
-// watchdog verdict s_ok reaches both roles through the same barrier.
-__device__ __forceinline__ bool grid_barrier_mma(const int* s_ok) {
-    __syncthreads();
-    __syncthreads();
-    return *s_ok != 0;
 }
 
 // ALIAS (large memory dims only): the accumulator staging lives in the TMA slot and the ctx part arrives in p.n_c TMA instructions; the
@@ -324,18 +194,18 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
             for (int j = 0; j < n; ++j) {
                 mbar_wait(j ? &full2_bar : &full_bar, mma_it & 1);
                 if (j == 0) t1 = clock64();
-                tcx::wgmma_fence();
+                wgmma_fence();
                 for (int c = 0; c < ch; ++c) {
-                    const uint64_t adesc = tcx::make_sw128_desc(smem_u32(sW + (size_t)(j * ch + c) * WTILE));
-                    const uint64_t bdesc = tcx::make_sw128_desc(smem_u32(ring + (size_t)(j * ch + c) * ATILE));
+                    const uint64_t adesc = make_sw128_desc(smem_u32(sW + (size_t)(j * ch + c) * WTILE));
+                    const uint64_t bdesc = make_sw128_desc(smem_u32(ring + (size_t)(j * ch + c) * ATILE));
 #pragma unroll
-                    for (int k = 0; k < KB / 16; ++k) tcx::wgmma_m64n32<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (j | c | k) != 0);
+                    for (int k = 0; k < KB / 16; ++k) wgmma_m64n32<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (j | c | k) != 0);
                 }
-                tcx::wgmma_commit();
+                wgmma_commit();
             }
             ++mma_it;
-            tcx::wgmma_wait<0>();
-            tcx::wgmma_fence_acc(acc);
+            wgmma_wait<0>();
+            wgmma_fence_acc(acc);
         } else {
             for (int j = 0; j < n; ++j) {
                 if (warp == NCW) {
@@ -351,18 +221,18 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
                 ++mma_it;
                 if (j == 0) t1 = clock64();
                 const int kb0 = part ? j * ch : p.nkb_h + j * ch;
-                tcx::wgmma_fence();
+                wgmma_fence();
                 for (int c = 0; c < ch; ++c) {
-                    const uint64_t adesc = tcx::make_sw128_desc(smem_u32(sW + (size_t)(kb0 + c) * WTILE));
-                    const uint64_t bdesc = tcx::make_sw128_desc(smem_u32(ring + (size_t)c * ATILE));
+                    const uint64_t adesc = make_sw128_desc(smem_u32(sW + (size_t)(kb0 + c) * WTILE));
+                    const uint64_t bdesc = make_sw128_desc(smem_u32(ring + (size_t)c * ATILE));
 #pragma unroll
                     for (int k = 0; k < KB / 16; ++k)
-                        tcx::wgmma_m64n32<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (part == 1 && j == 0 && c == 0 && k == 0) ? 0u : 1u);
+                        wgmma_m64n32<0, 0>(acc, adesc + 2 * k, bdesc + 2 * k, (part == 1 && j == 0 && c == 0 && k == 0) ? 0u : 1u);
                 }
-                tcx::wgmma_commit();
-                tcx::wgmma_wait<0>();
-                tcx::wgmma_fence_acc(acc);
-                tcx::wg_sync(NCW / 4);     // the whole warpgroup is done with the slot before the next TMA (or the staging) overwrites it
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_acc(acc);
+                wg_sync(NCW / 4);     // the whole warpgroup is done with the slot before the next TMA (or the staging) overwrites it
             }
         }
         if (signal_accum) {
@@ -370,7 +240,7 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
             const int row = 16 * (warp - NCW) + (lane >> 2), col = 2 * (lane & 3);
 #pragma unroll
             for (int r = 0; r < 16; ++r) s_sum[(8 * (r >> 2) + col + (r & 1)) * (ROWS + 1) + row + 8 * ((r >> 1) & 1)] = acc[r];
-            tcx::mbar_arrive(&accum_bar);
+            mbar_arrive(&accum_bar);
         }
         rp[2 * part] += t1 - t0; rp[2 * part + 1] += clock64() - t1;
     };
@@ -527,7 +397,7 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
             if (ATT) s_hs[uu * (BT + 4) + bl] = hs;
         }
         if (ATT) {
-            csync();
+            csync<CT>();
             // partial query projection of this CTA's 16 hidden units on the tensor cores: qpart[rb, b, a] = sum_u h[b, u] Wq[a, u].
             // h and Wq are split into bf16 hi + lo and three products are summed (hi.hi + lo.hi + hi.lo), i.e. fp32-equivalent.
             {
@@ -561,7 +431,7 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
         }
         PROF_MARK(1);
         if (ALIAS) proxy_fence_shared();             // generic-proxy accesses of the staging precede the TMA writes that follow the barrier
-        if (!grid_barrier(bar_counter, target, nblocks, p.abort_flag, &s_ok)) { alive = false; break; }
+        if (!grid_barrier(bar_counter, target, nblocks, p.abort_flag, &s_ok, true)) { alive = false; break; }
         PROF_MARK(2);
 
         // =================== h part of step i+1 (MMA warpgroup): TMA + wgmma run while the attention of step i is computed ===================
@@ -591,7 +461,7 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
                 if (i == 0) {                              // one-time: constants and the initial cumulative weights into shared memory
                     for (int a2 = tid; a2 < AH; a2 += CT) { vv[a2] = p.v[hf * AH + a2]; bias_s[a2] = p.bias[hf * AH + a2]; }
                     for (int l = tid; l < L16; l += CT) cum_s[l] = l < L ? p.cum[(size_t)b * L + l] : 0.f;
-                    csync();
+                    csync<CT>();
                 }
                 // memory-projection fragments of this warp's first energy job and memory fragments of its first context tile:
                 // neither depends on this step's state, so they are requested first and land behind the query reduction
@@ -643,7 +513,7 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
                             }
                     }
                     *reinterpret_cast<float4*>(cred + sl * AH + a4 * 4) = qs;
-                    csync();
+                    csync<CT>();
                     for (int a2 = tid; a2 < AH; a2 += CT) {
                         float q = 0.f;
 #pragma unroll
@@ -652,7 +522,7 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
                         qb[a2] = q + bias_s[a2];
                     }
                 }
-                csync();
+                csync<CT>();
                 PROF_MARK(3);
                 // energies on the tensor cores: S[l, a] = sum_k cumpad[l + k] * Wcomb[a, k].  job = (16-position tile, quarter of the
                 // attention dims: 4 n-tiles of 8 within this rank's half) -> 2 mtiles jobs, 3 per warp for L = 180
@@ -707,7 +577,7 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
                         if (tq == 0) { eq[qh * L16 + l0 + g] = e0; eq[qh * L16 + l0 + g + 8] = e1; }
                     }
                 }
-                csync();
+                csync<CT>();
                 // this rank's partial energies: own copy + the peer's copy through distributed shared memory.  Every remote store completes its
                 // 4 bytes on the PEER's exchange mbarrier (st.async), which that CTA armed with the L16 * 4 bytes it expects: no cluster barrier
                 if (tid == 0) mbar_expect_tx(&xchg_bar, (uint32_t)L16 * 4);
@@ -716,7 +586,7 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
                     epart[hf * L16 + l] = v;
                     st_async_peer_f32(epart + hf * L16 + l, &xchg_bar, (uint32_t)(hf ^ 1), v);
                 }
-                csync();                                   // own copies visible to the whole CTA
+                csync<CT>();                                   // own copies visible to the whole CTA
                 mbar_wait(&xchg_bar, i & 1);               // the peer's L16 values have landed (acquire)
                 PROF_MARK(4);
                 float mx = -INFINITY;
@@ -737,7 +607,7 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
                         else cum_next[l] = cn;
                     }
                 }
-                csync();
+                csync<CT>();
                 if (p.use_btab) {
                     // B fragments (hi(w) in column 0, lo(w) in column 1) of every 16-position k-tile, built ONCE per CTA: they depend on the k-tile
                     // only, and every warp used to rebuild all of them (~40 instructions per fragment and warp)
@@ -753,7 +623,7 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
                         }
                         btab[idx] = f;
                     }
-                    csync();
+                    csync<CT>();
                 }
                 PROF_MARK(5);
                 // context on the tensor cores: ctx[m] = sum_l memory[l, m] * w[l] for this rank's half of the 16-row tiles.  A = memory^T
@@ -826,7 +696,7 @@ __global__ void __launch_bounds__(PT, 1) lstm_loop_tc_kernel(const __grid_consta
             }
             PROF_MARK(6);
             // next step's epilogue operands (L2 hits: prefetched a step ago) are requested between the arrival and the wait
-            if (!grid_barrier(bar_counter, target, nblocks, p.abort_flag, &s_ok, [&]() { if (i + 1 < p.T) prefetch(i + 1, false); })) {
+            if (!grid_barrier(bar_counter, target, nblocks, p.abort_flag, &s_ok, true, [&]() { if (i + 1 < p.T) prefetch(i + 1, false); })) {
                 alive = false; break;
             }
             PROF_MARK(7);
@@ -848,12 +718,10 @@ size_t tc_loop_smem_bytes(int nkb, int slot_kb, int A, bool att, int L, bool ali
     }
     return b;
 }
-constexpr size_t SMEM_LIMIT = 227 * 1024 - 1088;    // leave room for the static barriers (1 KB of static shared memory)
-
 // largest ring slot (in k-blocks, <= want) that fits
 int pick_slot(int nkb, int A, bool att, int L, int want, bool alias = false) {
     int kb = want;
-    while (kb >= 1 && tc_loop_smem_bytes(nkb, kb, A, att, L, alias) > SMEM_LIMIT) --kb;
+    while (kb >= 1 && tc_loop_smem_bytes(nkb, kb, A, att, L, alias) > PERSIST_SMEM_LIMIT) --kb;
     return kb;
 }
 int largest_divisor_le(int n, int cap) {
@@ -900,37 +768,15 @@ bool tc_persist_supported(const b200tts_decoder_shape& s) {
 }
 
 static int launch_tc_loop(bool att, const TcLoopArgs& a, const CUtensorMap& tmH, const CUtensorMap& tmC, size_t smem, cudaStream_t st) {
-    void* fn = att ? (a.alias_sum ? (void*)lstm_loop_tc_kernel<true, true> : (void*)lstm_loop_tc_kernel<true, false>) : (void*)lstm_loop_tc_kernel<false, false>;
-    B200_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const void* fn = att ? (a.alias_sum ? (void*)lstm_loop_tc_kernel<true, true> : (void*)lstm_loop_tc_kernel<true, false>)
+                         : (void*)lstm_loop_tc_kernel<false, false>;
     const int grid = a.RB * a.NBH;
+    // the attention runs on CTA pairs: clusters of 2 (distributed shared memory + cluster barrier)
+    B200_REQUIRE(!att || (grid % 2 == 0 && grid / 2 >= a.B), "wgmma attention loop: %d CTAs cannot form %d pairs", grid, a.B);
     TcLoopArgs args = a;
     CUtensorMap mapH = tmH, mapC = tmC;
     void* params[] = {&mapH, &mapC, &args};
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(PT); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attrs[2];
-    attrs[0].id = cudaLaunchAttributeCooperative;
-    attrs[0].val.cooperative = 1;
-    cfg.attrs = attrs; cfg.numAttrs = 1;
-    if (att) {      // the attention runs on CTA pairs: clusters of 2 (distributed shared memory + cluster barrier)
-        B200_REQUIRE(grid % 2 == 0 && grid / 2 >= a.B, "wgmma attention loop: %d CTAs cannot form %d pairs", grid, a.B);
-        attrs[1].id = cudaLaunchAttributeClusterDimension;
-        attrs[1].val.clusterDim.x = 2; attrs[1].val.clusterDim.y = 1; attrs[1].val.clusterDim.z = 1;
-        cfg.numAttrs = 2;
-        int nclusters = 0;
-        B200_CUDA(cudaOccupancyMaxActiveClusters(&nclusters, fn, &cfg));
-        B200_REQUIRE(nclusters * 2 >= grid, "wgmma attention loop: only %d CTA pairs can be co-resident, %d needed", nclusters, grid / 2);
-    } else {
-        int per_sm = 0, dev = 0, sms = 0;
-        B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, PT, smem));
-        B200_CUDA(cudaGetDevice(&dev));
-        B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-        B200_REQUIRE(per_sm * sms >= grid, "wgmma persistent loop: %d CTAs cannot be co-resident (%d per SM x %d SMs)", grid, per_sm, sms);
-    }
-    KernelTimer kt(att ? "lstm_loop_tc_kernel<att>" : "lstm_loop_tc_kernel<gen>", st);
-    B200_CUDA(cudaLaunchKernelExC(&cfg, fn, params));
-    B200_LAUNCH_CHECK();
-    return B200TTS_OK;
+    return launch_persistent(att ? "lstm_loop_tc_kernel<att>" : "lstm_loop_tc_kernel<gen>", fn, grid, PT, smem, att, params, st);
 }
 
 // Attention-LSTM + attention loop (all T steps).  Expects: ga = input projection, ai row 0 = 0, ca row 0 = 0, cum row 0 = 0,
@@ -970,7 +816,7 @@ int tc_persist_att_loop(const b200tts_decoder_shape& s, const b200tts_decoder_pa
     a.prof2 = a.prof + 2 * NUM_SMS * 8;
     size_t smem = tc_loop_smem_bytes(g.nkb_att, a.slot_kb, s.A, true, s.L, g.alias_att != 0);
     const size_t tab = (size_t)l.MT * 32 * 8;          // shared B-fragment table of the context product, when it fits behind the scratch
-    a.use_btab = smem + tab <= SMEM_LIMIT ? 1 : 0;
+    a.use_btab = smem + tab <= PERSIST_SMEM_LIMIT ? 1 : 0;
     if (a.use_btab) smem += tab;
     return launch_tc_loop(true, a, tmH, tmC, smem, st);
 }

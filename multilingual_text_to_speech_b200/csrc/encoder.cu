@@ -8,18 +8,12 @@
 
 namespace b200tts {
 
-int gemm_tc_try(const GemmDesc& d, cudaStream_t st, bool* handled);      // gemm_tc.cu
 int gemm_tc_conv(const float* weight, const float* in, float* out, int NB, int G, int Cout, int Cin, int L, int k, int dil, int pad, int bwd,
                  float beta, cudaStream_t st, bool* handled);
 int gemm_tc_conv_dw(const float* dz, const float* x, float* dweight, int NB, int G, int Cout, int Cin, int L, int k, int dil, int pad,
                     cudaStream_t st, bool* handled);
 
 namespace {
-
-inline int grid_for(size_t n) {
-    size_t g = (n + 255) / 256;
-    return (int)(g > NUM_SMS * 16 ? NUM_SMS * 16 : (g < 1 ? 1 : g));
-}
 
 // col[nb, i*k + t, l] = x[nb, i, l + t*dil - pad]  (zero outside)      nb runs over (row, group) pairs
 __global__ void im2col1d_kernel(float* __restrict__ col, const float* __restrict__ x, size_t NBG, int Cin, int L, int k, int dil, int pad) {

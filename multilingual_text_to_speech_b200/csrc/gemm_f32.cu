@@ -271,8 +271,6 @@ int gemm_run_auto(GemmDesc d, float* scratch, size_t scratch_elems, cudaStream_t
 
 // Picks a split-K factor so that small-output / long-K products still fill the NUM_SMS SMs, bounded by the
 // scratch the caller provides for the partial sums.
-int gemm_tc_try(const GemmDesc& d, cudaStream_t st, bool* handled);
-
 static int gemm_auto_impl(GemmDesc d, float* scratch, size_t scratch_elems, cudaStream_t stream, bool bf16) {
     if (bf16) {     // long-K products run un-split on the wgmma kernel (no partial round trip); it declines what it cannot take
         d.splitk = 1; d.partial = nullptr; d.keep_partials = 0;

@@ -182,10 +182,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 // operand packing: fp32 (either orientation) -> bf16 [batch][rows][Kp], K contiguous, Kp % 8 == 0
 // ------------------------------------------------------------------------------------------------
 // Thread = 8 consecutive k of one row -> ONE 16-byte store (Kp % 8 == 0); rows ride on blockIdx.y: no per-element 64-bit division.
-__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
-    __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-    return *reinterpret_cast<uint32_t*>(&v);
-}
 __global__ void pack_kcontig_kernel(__nv_bfloat16* __restrict__ dst, const float* __restrict__ src, int ld, long long bstride, int rows,
                                     int K, int Kp, int kin, long long kos) {
     const float* s = src + (size_t)blockIdx.z * bstride;
@@ -210,7 +206,7 @@ __global__ void pack_kcontig_kernel(__nv_bfloat16* __restrict__ dst, const float
                     }
                 }
             }
-            *reinterpret_cast<uint4*>(drow + k) = make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
+            *reinterpret_cast<uint4*>(drow + k) = make_uint4(pack2(v[0], v[1]), pack2(v[2], v[3]), pack2(v[4], v[5]), pack2(v[6], v[7]));
         }
     }
 }
@@ -230,7 +226,7 @@ __global__ void pack_transpose_kernel(__nv_bfloat16* __restrict__ dst, const flo
     for (int j = threadIdx.y; j < 32; j += blockDim.y) {
         const int r = r0 + j, k = k0 + 2 * threadIdx.x;
         if (r < rows && k < Kp)        // Kp is even: the pair (k, k + 1) is inside the padded row
-            *reinterpret_cast<uint32_t*>(d + (size_t)r * Kp + k) = pack_bf16x2(tile[2 * threadIdx.x][j], tile[2 * threadIdx.x + 1][j]);
+            *reinterpret_cast<uint32_t*>(d + (size_t)r * Kp + k) = pack2(tile[2 * threadIdx.x][j], tile[2 * threadIdx.x + 1][j]);
     }
 }
 
@@ -288,7 +284,7 @@ __global__ void pack_im2col_kcontig_kernel(__nv_bfloat16* __restrict__ dst, cons
                 v[j] = (kk0 + j < NB * L && ls >= 0 && ls < L) ? xrow[(size_t)q * G * Cin * L + ls] : 0.f;
                 if (++l == L) { l = 0; ++q; }
             }
-            *reinterpret_cast<uint4*>(drow + kk0) = make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
+            *reinterpret_cast<uint4*>(drow + kk0) = make_uint4(pack2(v[0], v[1]), pack2(v[2], v[3]), pack2(v[4], v[5]), pack2(v[6], v[7]));
         }
     }
 }
@@ -412,7 +408,6 @@ void tc_pack_cache_end() { g_cache_on = false; g_ncache = 0; g_cache_off = 0; }
 void set_tc_enabled(int on) { g_tc_enabled = on; }
 int tc_enabled() { return g_tc_enabled; }
 
-// Returns B200TTS_OK and sets *handled = true when the wgmma path ran; *handled = false -> caller uses the mma.sync path.
 // Split-K decision shared by the dense and the convolution weight-gradient products: with fewer output tiles than CTA slots (2 per SM)
 // and a long K, K is cut into `splits` ranges of `kper` k-blocks; the partial tiles live at the END of the scratch, clear of the
 // packed (and cached) operands that occupy its first `used` bytes.  Leaves a.ksplit = 1 when it does not pay or does not fit.

@@ -9,11 +9,6 @@ namespace b200tts {
 
 namespace {
 
-inline int grid_for(size_t n) {
-    size_t g = (n + 255) / 256;
-    return (int)(g > NUM_SMS * 16 ? NUM_SMS * 16 : (g < 1 ? 1 : g));
-}
-
 // xp[dir][j, b, :] = x[b, t(dir, j), :]   with t(0, j) = j, t(1, j) = L-1-j
 __global__ void to_processing_order_kernel(float* __restrict__ xp, const float* __restrict__ x, int B, int L, int E) {
     const size_t per = (size_t)L * B * E;

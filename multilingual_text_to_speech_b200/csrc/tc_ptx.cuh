@@ -1,7 +1,9 @@
 // PTX wrappers for the Hopper data path (sm_90a): mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA with the accumulator in
-// registers, operands in shared memory), proxy fences.  Shared by every kernel that issues wgmma.
+// registers, operands in shared memory), proxy fences, mma.sync, distributed shared memory, and the grid barrier of the persistent loops.
+// The one home of these primitives: every kernel file that needs one includes this header and says `using namespace tcx;`.
 #pragma once
 #include <cuda.h>
+#include <cuda_bf16.h>
 #include <stdint.h>
 
 namespace b200tts {
@@ -18,6 +20,9 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// Out of line on purpose: an inlined trap makes ptxas drop the setmaxnreg.inc limit of the code around it back to the launch's uniform
+// register cap (measured with -Xptxas -v: the compute warps of the forward loops then spill), a call to this function does not.
+static __device__ __noinline__ __attribute__((noreturn)) void watchdog_trap() { __trap(); }
 // spin on the phase parity; a protocol bug must not hang the GPU: trap after ~2 s
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     const uint32_t addr = smem_u32(bar);
@@ -32,7 +37,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
             : "r"(addr), "r"(parity)
             : "memory");
         if (done) return;
-        if (clock64() - t0 > 4000000000ll) __trap();
+        if (clock64() - t0 > 4000000000ll) watchdog_trap();
     }
 }
 __device__ __forceinline__ void tma_load_3d(void* smem, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
@@ -62,13 +67,24 @@ __device__ __forceinline__ void tma_load_5d_mc(void* smem, const CUtensorMap* ma
         ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "h"(cta_mask), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
         : "memory");
 }
+// distributed shared memory: the shared::cluster address of the same-offset location in the cluster's CTA `rank`
+__device__ __forceinline__ uint32_t peer_addr(const void* local_smem, uint32_t rank) {
+    uint32_t ra;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(local_smem)), "r"(rank));
+    return ra;
+}
+__device__ __forceinline__ void st_cluster_f32(uint32_t addr, float v) { asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory"); }
+// remote store that completes its 4 bytes on the PEER's mbarrier (data + signal in one instruction): a pair exchange needs no cluster barrier
+// and none of the memory fence its release semantics imply
+__device__ __forceinline__ void st_async_peer_f32(const float* local_smem, const uint64_t* local_bar, uint32_t peer_rank, float v) {
+    const uint32_t ra = peer_addr(local_smem, peer_rank), rb = peer_addr(local_bar, peer_rank);
+    asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(ra), "r"(__float_as_uint(v)), "r"(rb) : "memory");
+}
 // bulk copy of `bytes` (a multiple of 16; both addresses 16-byte aligned) from this CTA's shared memory to the peer CTA `peer_rank` of the
 // cluster: dst and bar are given as this CTA's addresses of the same-offset buffer / mbarrier in the peer, whose barrier the copy completes
 // its bytes on.  The source must have been made visible to the async proxy (proxy_fence_shared after the generic writes).
 __device__ __forceinline__ void bulk_copy_to_peer(const void* dst, const void* src, uint32_t bytes, const uint64_t* bar, uint32_t peer_rank) {
-    uint32_t rd, rb;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rd) : "r"(smem_u32(dst)), "r"(peer_rank));
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rb) : "r"(smem_u32(bar)), "r"(peer_rank));
+    const uint32_t rd = peer_addr(dst, peer_rank), rb = peer_addr(bar, peer_rank);
     asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(rd), "r"(smem_u32(src)), "r"(bytes), "r"(rb)
                  : "memory");
@@ -82,6 +98,80 @@ __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
     return pred != 0;
+}
+__device__ __forceinline__ void l2_prefetch(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
+// named barrier 1 among the first N threads of the CTA (the compute warps of a warp-specialised kernel)
+template <int N>
+__device__ __forceinline__ void csync() { asm volatile("bar.sync 1, %0;" ::"n"(N) : "memory"); }
+
+// ---- mma.sync (one warp) ----
+__device__ __forceinline__ void ldmatrix_x4(uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3, const void* p) {
+    const uint32_t addr = (uint32_t)__cvta_generic_to_shared(p);
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
+}
+__device__ __forceinline__ void mma_bf16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+// two floats -> one bf16x2 register (round to nearest), lo in the low half
+__device__ __forceinline__ uint32_t pack2(float lo, float hi) {
+    __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
+    return *reinterpret_cast<uint32_t*>(&v);
+}
+__device__ __forceinline__ float tanh_fast(float x) {
+    float y;
+    asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
+    return y;
+}
+// tanh of the bf16 perf mode's cell (forward loops, and the recomputed cell state of the reverse loops): ex2-based, ~1e-6 relative error
+__device__ __forceinline__ float tanh_exp(float x) { return 2.f * __fdividef(1.f, 1.f + __expf(-2.f * x)) - 1.f; }
+
+// ---- grid barrier of the cooperative persistent loops ----
+// Monotonic-counter barrier over ALL threads of every CTA; returns false if the watchdog fired (~2 s) or another CTA raised the abort
+// flag.  Arrival is ONE release-reduction (cumulative: it orders the whole CTA's writes, which the preceding __syncthreads made visible to
+// thread 0); the wait polls with relaxed loads and issues a single acquire fence after the last one.
+//   s_ok:        the caller's __shared__ int, through which thread 0 hands the verdict to the CTA
+//   async_fence: the data written before the barrier is read by other CTAs through TMA (async proxy); pass a literal, so it folds away
+//   overlap:     runs on every thread BETWEEN the CTA's arrival and its wait: work that does not depend on other CTAs (the next step's
+//                operand prefetch) hides under the barrier latency instead of delaying the arrival
+struct NoOverlap { __device__ __forceinline__ void operator()() const {} };
+template <typename Overlap = NoOverlap>
+__device__ __forceinline__ bool grid_barrier(unsigned* counter, unsigned& target, unsigned nblocks, int* abort_flag, int* s_ok, bool async_fence,
+                                             Overlap overlap = Overlap()) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        target += nblocks;
+        if (async_fence) proxy_fence_global();
+        asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
+    }
+    overlap();
+    if (threadIdx.x == 0) {
+        int ok = 1;
+        const long long t0 = clock64();
+        unsigned polls = 0;
+        for (;;) {                      // nothing but the counter load in the polling loop: its round trip is the barrier latency
+            unsigned v;
+            asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(counter) : "memory");
+            if (v >= target) break;
+            if ((++polls & 255u) == 0 && (clock64() - t0 > 4000000000ll || *reinterpret_cast<volatile int*>(abort_flag))) {
+                ok = 0; *abort_flag = 1; break;
+            }
+        }
+        asm volatile("fence.acquire.gpu;" ::: "memory");
+        *s_ok = ok;
+    }
+    __syncthreads();
+    return *s_ok != 0;
+}
+// The side of grid_barrier of a warpgroup that runs its own step loop (the MMA warpgroup of the forward loops): it arrives at the same two
+// CTA-wide barriers, in the same order, and leaves the arrival and the polling to thread 0.  Staying in the CTA barrier (instead of waiting on
+// an mbarrier that thread 0 signals) keeps the ordering of a single loop: a TMA issued after the barrier reads other CTAs' rows only after
+// thread 0's acquire fence, and the watchdog verdict s_ok reaches both roles through the same barrier.
+__device__ __forceinline__ bool grid_barrier_mma(const int* s_ok) {
+    __syncthreads();
+    __syncthreads();
+    return *s_ok != 0;
 }
 
 // ---- wgmma (all 128 threads of a warpgroup = 4 consecutive warps starting at a multiple of 4 execute these) ----
