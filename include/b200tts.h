@@ -417,6 +417,46 @@ int b200tts_griffinlim(const b200tts_vocoder_shape* shape, const float* S, const
  * largest sample, not the largest magnitude, as the reference's Python max() is. */
 int b200tts_deemphasis_normalize(const b200tts_vocoder_shape* shape, float* wave, const int32_t* off, void* stream);
 
+/* ---- audio analysis: audio.spectrogram and mel_cepstral_distorision, reference utils/audio.py:66-78, 117-161 (librosa 0.7.0) ----
+ * Packed ragged layout: utterance b owns samples [soff[b], soff[b+1]) of an fp32 waveform (L_b >= 1) and frames [off[b], off[b+1]) with
+ * F_b = 1 + L_b / hop (soff, off: int32 [B+1], device, both starting at 0; the caller keeps them consistent).  Spectra are frame-major
+ * [total_frames, bins] fp32 with bins = K = N/2 + 1 (linear) or n_mels.  No utterance reads another's data and nothing uses atomics: every
+ * result is bit-reproducible and independent of the batch it is computed in.  Supported: even N <= 2048 whose N/2 has no prime factor
+ * above 31, 1 <= win <= N (periodic Hann centre-padded to N), hop >= 1. */
+typedef struct {
+    int B, total_samples, total_frames;
+    int N, hop, win;
+    int n_mels;          /* 0: linear magnitudes [total_frames, K]; > 0: mel magnitudes [total_frames, n_mels] */
+    double preemphasis;  /* pre-emphasis coefficient a: y[n] - a y[n-1] before the padding; 0 = off */
+} b200tts_analysis_shape;
+/* Host only: the stft_magnitude workspace (fp64 twiddles and window, mel filter ranges); 0 for an invalid shape (message set). */
+size_t b200tts_analysis_workspace_bytes(const b200tts_analysis_shape* shape);
+/* |stft(preemphasis(y), center=True, pad_mode='reflect', window='hann')| per utterance: the transform in fp64, rounded to complex64, the
+ * magnitude in fp32; np.pad's repeated reflection when L_b < N/2.  mel_basis [n_mels, K] (NULL when n_mels = 0): out = mel_basis . |X|,
+ * each filter summing its nonzero bins in ascending order in fp32.  workspace: 256-byte aligned, b200tts_analysis_workspace_bytes. */
+int b200tts_stft_magnitude(const b200tts_analysis_shape* shape, const float* wave, const int32_t* soff, const int32_t* off,
+                           const float* mel_basis, float* out, void* workspace, size_t workspace_bytes, void* stream);
+/* librosa amplitude_to_db(S, ref=np.max, amin=1e-5, top_db=None) per utterance, fp32: 10 log10(max(1e-10, S^2)) minus the same of the
+ * utterance's largest |S|.  S and out [total_frames, bins] (bins from shape->n_mels); out may be S. */
+int b200tts_amplitude_to_db(const b200tts_analysis_shape* shape, const float* S, const int32_t* off, float* out, void* stream);
+/* librosa mfcc(S = mel_db / 10, n_mfcc): scipy.fftpack.dct(type=2, norm='ortho') over the n_mels axis, the first n_mfcc coefficients
+ * (c0 included).  mel_db [total_frames, n_mels] -> out [total_frames, n_mfcc], fp32 (the DCT matrix from fp64, rounded to fp32). */
+int b200tts_mel_cepstrum(int total_frames, int n_mels, int n_mfcc, const float* mel_db, float* out, void* stream);
+#define B200TTS_MCD_CUT 0
+#define B200TTS_MCD_STRETCH 1
+#define B200TTS_MCD_DTW 2
+/* DTW keeps three anti-diagonals of (fp64, int32) in shared memory: the shorter sequence of a pair may have at most this many frames. */
+#define B200TTS_DTW_MAX_FRAMES 6455
+/* Mel cepstral distortion of B pairs (reference mel_cepstral_distorision): pair b is cep_a frames [off_a[b], off_a[b+1]) against cep_b
+ * frames [off_b[b], off_b[b+1]) (each [frames, n_mfcc] fp32; off_a, off_b int32 [B+1], device; every sequence non-empty).  The frame
+ * distance is the Euclidean distance over coefficients 1..n_mfcc-1, summed in index order in fp32; means and costs accumulate in fp64.
+ * CUT: mean over the first min(F_a, F_b) frame pairs.  STRETCH: the shorter sequence indexed at i * n // m over the longer length m (the
+ * first when the lengths are equal).  DTW: the exact dynamic-time-warping optimum (fastdtw's recurrence without its radius-1
+ * approximation): path cost / path length.  mcd_out: double [B]; path_len_out: int32 [B] (pairs averaged over) or NULL.  A DTW pair whose
+ * shorter side exceeds B200TTS_DTW_MAX_FRAMES gets NaN and path length -1. */
+int b200tts_mel_cepstral_distortion(int B, int n_mfcc, int mode, const float* cep_a, const int32_t* off_a, const float* cep_b,
+                                    const int32_t* off_b, double* mcd_out, int32_t* path_len_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

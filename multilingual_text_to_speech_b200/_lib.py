@@ -5,7 +5,7 @@ eager-PyTorch or CPU fallback (north_star: "no CPU fallback").
 """
 import ctypes
 import os
-from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_longlong, c_size_t, c_uint8, c_uint64, c_ulonglong, c_void_p
+from ctypes import POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int32, c_longlong, c_size_t, c_uint8, c_uint64, c_ulonglong, c_void_p
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG, 'libb200tts.so')
@@ -73,6 +73,15 @@ class BiLSTMParams(Structure):
 class VocoderShape(Structure):
     _fields_ = [(n, c_int) for n in ('B', 'total_frames', 'N', 'hop', 'win', 'n_mels')] + \
                [(n, c_float) for n in ('power', 'momentum', 'preemphasis')] + [('nnls_iters', c_int)]
+
+
+class AnalysisShape(Structure):
+    _fields_ = [(n, c_int) for n in ('B', 'total_samples', 'total_frames', 'N', 'hop', 'win', 'n_mels')] + [('preemphasis', c_double)]
+
+
+# include/b200tts.h: B200TTS_MCD_CUT / _STRETCH / _DTW and B200TTS_DTW_MAX_FRAMES
+MCD_MODES = {'cut': 0, 'stretch': 1, 'dtw': 2}
+DTW_MAX_FRAMES = 6455
 
 
 # name -> (restype, argtypes); the "-m not gpu" suite checks every symbol of the header resolves
@@ -145,6 +154,11 @@ SIGNATURES = {
     'b200tts_griffinlim': (c_int, [POINTER(VocoderShape), c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t,
                                    c_void_p]),
     'b200tts_deemphasis_normalize': (c_int, [POINTER(VocoderShape), c_void_p, c_void_p, c_void_p]),
+    'b200tts_analysis_workspace_bytes': (c_size_t, [POINTER(AnalysisShape)]),
+    'b200tts_stft_magnitude': (c_int, [POINTER(AnalysisShape), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    'b200tts_amplitude_to_db': (c_int, [POINTER(AnalysisShape), c_void_p, c_void_p, c_void_p, c_void_p]),
+    'b200tts_mel_cepstrum': (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    'b200tts_mel_cepstral_distortion': (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -184,6 +184,15 @@ int spectrogram_magnitude_impl(const b200tts_vocoder_shape& s, const float* log_
 int griffinlim_impl(const b200tts_vocoder_shape& s, const float* S, const int* off, float* angles, float* rebuilt, int first, int iters,
                     float* wave, void* ws, size_t ws_bytes, cudaStream_t st);
 int deemphasis_normalize_impl(const b200tts_vocoder_shape& s, float* wave, const int* off, cudaStream_t st);
+size_t analysis_workspace_bytes(const b200tts_analysis_shape& s);
+int stft_magnitude_impl(const b200tts_analysis_shape& s, const float* wave, const int* soff, const int* off, const float* mel_basis, float* out,
+                        void* ws, size_t ws_bytes, cudaStream_t st);
+int amplitude_to_db_impl(const b200tts_analysis_shape& s, const float* S, const int* off, float* out, cudaStream_t st);
+int mel_cepstrum_validate(int total_frames, int n_mels, int n_mfcc);
+int mcd_validate(int B, int n_mfcc, int mode);
+int mel_cepstrum_impl(int total_frames, int n_mels, int n_mfcc, const float* mel_db, float* out, cudaStream_t st);
+int mel_cepstral_distortion_impl(int B, int n_mfcc, int mode, const float* cep_a, const int* off_a, const float* cep_b, const int* off_b,
+                                 double* mcd, int* path_len, cudaStream_t st);
 }
 using namespace b200tts;
 
@@ -564,6 +573,35 @@ int b200tts_deemphasis_normalize(const b200tts_vocoder_shape* shape, float* wave
     B200_REQUIRE(shape && wave && off, "deemphasis_normalize: null argument");
     B200_TRY(require_device());
     return deemphasis_normalize_impl(*shape, wave, off, (cudaStream_t)stream);
+}
+
+size_t b200tts_analysis_workspace_bytes(const b200tts_analysis_shape* shape) {
+    if (!shape) { set_last_error("analysis_workspace_bytes: null shape"); return 0; }
+    return analysis_workspace_bytes(*shape);
+}
+int b200tts_stft_magnitude(const b200tts_analysis_shape* shape, const float* wave, const int32_t* soff, const int32_t* off,
+                           const float* mel_basis, float* out, void* workspace, size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(shape && wave && soff && off && out, "stft_magnitude: null argument");
+    B200_TRY(require_device());
+    return stft_magnitude_impl(*shape, wave, soff, off, mel_basis, out, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_amplitude_to_db(const b200tts_analysis_shape* shape, const float* S, const int32_t* off, float* out, void* stream) {
+    B200_REQUIRE(shape && S && off && out, "amplitude_to_db: null argument");
+    B200_TRY(require_device());
+    return amplitude_to_db_impl(*shape, S, off, out, (cudaStream_t)stream);
+}
+int b200tts_mel_cepstrum(int total_frames, int n_mels, int n_mfcc, const float* mel_db, float* out, void* stream) {
+    B200_REQUIRE(mel_db && out, "mel_cepstrum: null argument");
+    B200_TRY(mel_cepstrum_validate(total_frames, n_mels, n_mfcc));
+    B200_TRY(require_device());
+    return mel_cepstrum_impl(total_frames, n_mels, n_mfcc, mel_db, out, (cudaStream_t)stream);
+}
+int b200tts_mel_cepstral_distortion(int B, int n_mfcc, int mode, const float* cep_a, const int32_t* off_a, const float* cep_b,
+                                    const int32_t* off_b, double* mcd_out, int32_t* path_len_out, void* stream) {
+    B200_REQUIRE(cep_a && off_a && cep_b && off_b && mcd_out, "mel_cepstral_distortion: null argument");
+    B200_TRY(mcd_validate(B, n_mfcc, mode));
+    B200_TRY(require_device());
+    return mel_cepstral_distortion_impl(B, n_mfcc, mode, cep_a, off_a, cep_b, off_b, mcd_out, path_len_out, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -9,84 +9,19 @@
 // on inputs spanning 80 dB, so no reduced-precision tensor-core DFT.
 #include <float.h>
 #include <algorithm>
-#include "common.cuh"
+#include "fft.cuh"
 
 namespace b200tts {
 
 namespace {
 
-constexpr int FFT_MAX_STAGES = 12;
 constexpr int FRAMES_PER_CTA = 4;
 constexpr int FFT_THREADS = 256;
 constexpr int NNLS_WARPS = 8;
 constexpr int DEEMPH_THREADS = 1024;
 
-struct FftPlan {
-    int M, N, nst;
-    int radix[FFT_MAX_STAGES];
-};
-
-// radix-4 stages first, then one radix 2, then the odd primes in ascending order: the cost of a stage is M * radix multiply-adds
-int make_plan(int N, FftPlan* p) {
-    if (N < 2 || N > 2048 || (N & 1)) return 0;
-    p->N = N;
-    p->M = N / 2;
-    p->nst = 0;
-    int m = p->M;
-    while (m % 4 == 0) { p->radix[p->nst++] = 4; m /= 4; }
-    if (m % 2 == 0) { p->radix[p->nst++] = 2; m /= 2; }
-    for (int q = 3; q <= 31; q += 2)
-        while (m % q == 0) { p->radix[p->nst++] = q; m /= q; }
-    return m == 1;
-}
-
 __device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
 __device__ __forceinline__ float2 cmulc(float2 a, float2 b) { return make_float2(a.x * b.x + a.y * b.y, a.y * b.x - a.x * b.y); }   // a * conj(b)
-
-// Complex FFT of length M over `nfr` frames stored at a[f * ld ...], ping-ponging with b; returns the buffer holding the result.
-// Stage s (radix R, Ns = product of the earlier radices): output o = blk * Ns * R + j * Ns + k reads inputs jj + r * M / R with
-// jj = blk * Ns + k, weighted by W_M^(r * (k + j * Ns) * M / (Ns * R)) -- the stage twiddle and the radix-R DFT in one root (conjugated for
-// the inverse).  Each output is computed by one thread in ascending r.
-__device__ float2* block_cfft(float2* a, float2* b, int ld, int nfr, const FftPlan& p, const float2* __restrict__ tw, bool inverse) {
-    const int M = p.M;
-    int Ns = 1;
-    for (int s = 0; s < p.nst; ++s) {
-        const int R = p.radix[s], NsR = Ns * R, sc = M / NsR, st = M / R;
-        for (int idx = threadIdx.x; idx < nfr * M; idx += blockDim.x) {
-            const int f = idx / M, o = idx - f * M;
-            const int k = o % Ns, j = (o / Ns) % R, blk = o / NsR;
-            const float2* in = a + f * ld + blk * Ns + k;
-            const int e = (k + j * Ns) * sc;
-            int ti = 0;
-            float2 acc = make_float2(0.f, 0.f);
-            for (int r = 0; r < R; ++r) {
-                const float2 v = in[r * st];
-                const float2 w = tw[ti];
-                acc.x = fmaf(v.x, w.x, acc.x);
-                acc.y = fmaf(v.y, w.x, acc.y);
-                if (inverse) { acc.x = fmaf(-v.y, -w.y, acc.x); acc.y = fmaf(v.x, -w.y, acc.y); }
-                else         { acc.x = fmaf(-v.y, w.y, acc.x);  acc.y = fmaf(v.x, w.y, acc.y); }
-                ti += e;
-                if (ti >= M) ti -= M;
-            }
-            b[f * ld + o] = acc;
-        }
-        __syncthreads();
-        float2* t = a; a = b; b = t;
-        Ns = NsR;
-    }
-    return a;
-}
-
-// utterance of frame f: the b with off[b] <= f < off[b + 1]
-__device__ __forceinline__ int utterance_of(const int* __restrict__ off, int B, int f) {
-    int lo = 0, hi = B - 1;
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (off[mid] <= f) lo = mid; else hi = mid - 1;
-    }
-    return lo;
-}
 
 // Sample q of the untrimmed overlap-add of utterance frames [0, F) (q in [0, N + hop * (F - 1))), divided by the window sum-square where
 // that exceeds tiny(float32) (librosa istft).  The contributing frames are added in ascending order, as librosa's overlap-add does.
@@ -106,47 +41,7 @@ __device__ __forceinline__ float ola_sample(const float* __restrict__ frames, co
 
 // Twiddles W_M^j, W_N^k (k <= M) and the periodic Hann window of length win centre-padded to N, all from fp64 and rounded to fp32.
 __global__ void vocoder_tables_kernel(int N, int win, float2* __restrict__ twM, float2* __restrict__ twN, float* __restrict__ window) {
-    const int M = N / 2, lpad = (N - win) / 2;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < N + 2 * M + 1; i += gridDim.x * blockDim.x) {
-        double s, c;
-        if (i < M) {
-            sincospi(-2.0 * i / M, &s, &c);
-            twM[i] = make_float2((float)c, (float)s);
-        } else if (i < 2 * M + 1) {
-            const int k = i - M;
-            sincospi(-2.0 * k / N, &s, &c);
-            twN[k] = make_float2((float)c, (float)s);
-        } else {
-            const int n = i - 2 * M - 1;
-            const int m = n - lpad;
-            window[n] = (m >= 0 && m < win) ? (float)(0.5 - 0.5 * cospi(2.0 * m / win)) : 0.f;
-        }
-    }
-}
-
-struct FftSmem {
-    float2 *twM, *twN;
-    float* window;
-    float2* buf;      // 2 * FRAMES_PER_CTA buffers of M + 1 entries
-};
-
-__device__ __forceinline__ FftSmem load_tables(const FftPlan& p, const float2* twM, const float2* twN, const float* window) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    FftSmem s;
-    const int M = p.M;
-    s.twM = reinterpret_cast<float2*>(smem_raw);
-    s.twN = s.twM + M;
-    s.buf = s.twN + (M + 1);
-    s.window = reinterpret_cast<float*>(s.buf + 2 * FRAMES_PER_CTA * (M + 1));
-    for (int i = threadIdx.x; i < M; i += blockDim.x) s.twM[i] = twM[i];
-    for (int i = threadIdx.x; i <= M; i += blockDim.x) s.twN[i] = twN[i];
-    for (int i = threadIdx.x; i < p.N; i += blockDim.x) s.window[i] = window[i];
-    __syncthreads();
-    return s;
-}
-
-size_t fft_smem_bytes(const FftPlan& p) {
-    return (size_t)(p.M + (p.M + 1) + 2 * FRAMES_PER_CTA * (p.M + 1)) * sizeof(float2) + (size_t)p.N * sizeof(float);
+    fill_fft_tables(N, win, twM, twN, window);
 }
 
 // (a) per frame: X = S * angles -> inverse real FFT (numpy irfft: 1/N, imaginary parts of the DC and Nyquist bins ignored) -> times the
@@ -155,7 +50,7 @@ __global__ void __launch_bounds__(FFT_THREADS) vocoder_istft_frames_kernel(FftPl
                                                                            const float2* __restrict__ angles, const float2* __restrict__ twM,
                                                                            const float2* __restrict__ twN, const float* __restrict__ window,
                                                                            float* __restrict__ frames) {
-    const FftSmem sm = load_tables(p, twM, twN, window);
+    const FftSmem<float2> sm = load_tables<float2, FRAMES_PER_CTA>(p, twM, twN, window);
     const int M = p.M, K = M + 1, ld = M + 1, f0 = blockIdx.x * FRAMES_PER_CTA;
     const int nfr = min(FRAMES_PER_CTA, total - f0);
     float2* X = sm.buf;
@@ -195,7 +90,7 @@ __global__ void __launch_bounds__(FFT_THREADS) vocoder_stft_update_kernel(FftPla
                                                                           const float2* __restrict__ twN, const float* __restrict__ window,
                                                                           float2* __restrict__ rebuilt, float2* __restrict__ angles,
                                                                           float mom, int first) {
-    const FftSmem sm = load_tables(p, twM, twN, window);
+    const FftSmem<float2> sm = load_tables<float2, FRAMES_PER_CTA>(p, twM, twN, window);
     const int M = p.M, N = p.N, K = M + 1, ld = M + 1, f0 = blockIdx.x * FRAMES_PER_CTA;
     const int nfr = min(FRAMES_PER_CTA, total - f0);
     float2* Z = sm.buf;
@@ -204,15 +99,7 @@ __global__ void __launch_bounds__(FFT_THREADS) vocoder_stft_update_kernel(FftPla
         const int f = i / N, n = i - f * N;
         const int gf = f0 + f, b = utterance_of(off, B, gf);
         const int ob = off[b], F = off[b + 1] - ob, L = hop * (F - 1);
-        int s = (gf - ob) * hop + n - N / 2;                          // sample of the trimmed signal before the padding is resolved
-        if (L == 1) {
-            s = 0;
-        } else {
-            const int period = 2 * (L - 1);
-            s %= period;
-            if (s < 0) s += period;
-            if (s >= L) s = period - s;
-        }
+        const int s = reflect_index((gf - ob) * hop + n - N / 2, L);  // sample of the trimmed signal
         const float y = ola_sample(frames + (size_t)ob * N, sm.window, N, hop, F, s + N / 2);
         reinterpret_cast<float*>(Z + f * ld)[n] = y * sm.window[n];
     }
@@ -462,7 +349,7 @@ int griffinlim_impl(const b200tts_vocoder_shape& s, const float* S, const int* o
 
     vocoder_tables_kernel<<<cdiv(s.N + s.N + 1, 256), 256, 0, st>>>(s.N, s.win, twM, twN, window);
     B200_LAUNCH_CHECK();
-    const size_t smem = fft_smem_bytes(p);
+    const size_t smem = fft_smem_bytes<float2, FRAMES_PER_CTA>(p);
     B200_CUDA(cudaFuncSetAttribute(vocoder_istft_frames_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     B200_CUDA(cudaFuncSetAttribute(vocoder_stft_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int grid = cdiv(s.total_frames, FRAMES_PER_CTA);

@@ -798,3 +798,61 @@ def deemphasis_normalize(shape, wave, off):
     _require_cuda(wave, off)
     check(_lib.load().b200tts_deemphasis_normalize(ctypes.byref(shape), ptr(wave), ptr(off), _stream()), 'b200tts_deemphasis_normalize')
     return wave
+
+
+# ------------------------------------------------------------------------------------------------
+# audio analysis (packed ragged layout: utterance b owns samples soff[b]:soff[b+1] and frames off[b]:off[b+1])
+# ------------------------------------------------------------------------------------------------
+def analysis_workspace(shape, device):
+    """Workspace of b200tts_stft_magnitude for `shape` (a _lib.AnalysisShape); raises on an invalid shape."""
+    n = _lib.load().b200tts_analysis_workspace_bytes(ctypes.byref(shape))
+    if n == 0:
+        raise _lib.B200TTSError(f'b200tts_analysis_workspace_bytes: {_lib.load().b200tts_last_error().decode()}')
+    return _bytes(n, device)
+
+
+def stft_magnitude(shape, wave, soff, off, mel_basis=None, workspace=None):
+    """wave fp32 [total_samples] -> |STFT| [total_frames, K], or mel_basis . |STFT| [total_frames, n_mels] when shape.n_mels > 0."""
+    _require_cuda(wave, soff, off, mel_basis)
+    if mel_basis is not None and not (mel_basis.dtype == torch.float32 and mel_basis.is_contiguous()):
+        raise ValueError('the mel basis must be a contiguous fp32 [n_mels, K] tensor')
+    assert soff.dtype == torch.int32 and off.dtype == torch.int32 and wave.dtype == torch.float32 and wave.is_contiguous()
+    ws = analysis_workspace(shape, wave.device) if workspace is None else workspace
+    out = torch.empty(shape.total_frames, shape.n_mels or shape.N // 2 + 1, device=wave.device, dtype=torch.float32)
+    check(_lib.load().b200tts_stft_magnitude(ctypes.byref(shape), ptr(wave), ptr(soff), ptr(off), ptr(mel_basis), ptr(out), ptr(ws),
+                                             ws.numel(), _stream()), 'b200tts_stft_magnitude')
+    return out
+
+
+def amplitude_to_db(shape, S, off, out=None):
+    """Per utterance amplitude_to_db(ref=max): S [total_frames, bins] -> dB, into `out` (may be S; new tensor when None)."""
+    _require_cuda(S, off, out)
+    assert S.dtype == torch.float32 and S.is_contiguous() and off.dtype == torch.int32
+    out = torch.empty_like(S) if out is None else out
+    check(_lib.load().b200tts_amplitude_to_db(ctypes.byref(shape), ptr(S), ptr(off), ptr(out), _stream()), 'b200tts_amplitude_to_db')
+    return out
+
+
+def mel_cepstrum(mel_db, n_mfcc):
+    """mel_db [total_frames, n_mels] -> DCT-II (ortho) of mel_db / 10, first n_mfcc coefficients [total_frames, n_mfcc]."""
+    _require_cuda(mel_db)
+    mel_db = _f32c(mel_db)
+    out = torch.empty(mel_db.shape[0], n_mfcc, device=mel_db.device, dtype=torch.float32)
+    check(_lib.load().b200tts_mel_cepstrum(mel_db.shape[0], mel_db.shape[1], int(n_mfcc), ptr(mel_db), ptr(out), _stream()),
+          'b200tts_mel_cepstrum')
+    return out
+
+
+def mel_cepstral_distortion(cep_a, off_a, cep_b, off_b, mode):
+    """Packed cepstra [frames, n_mfcc] of B pairs -> (mcd float64 [B], path length int32 [B]); mode 'cut', 'stretch' or 'dtw'."""
+    _require_cuda(cep_a, off_a, cep_b, off_b)
+    if mode not in _lib.MCD_MODES:
+        raise ValueError(f'unknown mode {mode!r}; expected one of {sorted(_lib.MCD_MODES)}')
+    assert off_a.dtype == torch.int32 and off_b.dtype == torch.int32 and cep_a.shape[1] == cep_b.shape[1]
+    cep_a, cep_b = _f32c(cep_a), _f32c(cep_b)
+    B = off_a.numel() - 1
+    mcd = torch.empty(B, device=cep_a.device, dtype=torch.float64)
+    plen = torch.empty(B, device=cep_a.device, dtype=torch.int32)
+    check(_lib.load().b200tts_mel_cepstral_distortion(B, cep_a.shape[1], _lib.MCD_MODES[mode], ptr(cep_a), ptr(off_a), ptr(cep_b), ptr(off_b),
+                                                      ptr(mcd), ptr(plen), _stream()), 'b200tts_mel_cepstral_distortion')
+    return mcd, plen

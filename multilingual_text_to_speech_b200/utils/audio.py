@@ -1,8 +1,9 @@
-"""Spectrogram -> waveform with the reference's names (reference utils/audio.py:49-51, 88-114; librosa 0.7.0 mel_to_stft + griffinlim).
+"""Audio with the reference's names (reference utils/audio.py:49-161; librosa 0.7.0): spectrogram -> waveform (mel_to_stft + griffinlim),
+waveform -> log (mel) spectrogram (stft, melspectrogram, amplitude_to_db), MFCCs and the mel cepstral distortion.
 
-Every stage runs in the library's vocoder kernels on the GPU, in fp32 whatever the precision mode is.  Spectrograms go in as [bins, F]
-(numpy or torch); a batch is packed frame-major, and each waveform equals what its spectrogram gives on its own.  The dataset side (loading,
-trimming, the forward mel front end, MCD) and writing .wav files are not provided."""
+Every stage runs in the library's kernels on the GPU whatever the precision mode is.  Spectrograms go in and out as [bins, F] (numpy or
+torch); a batch is packed frame-major, and each result equals what its input gives on its own.  The rest of the dataset side (loading,
+trimming, duration) and writing .wav files are not provided."""
 import numpy as np
 import torch
 
@@ -29,6 +30,12 @@ def db_to_amplitude(x):
     if isinstance(x, torch.Tensor):
         return torch.pow(torch.pow(10.0, 0.1 * x), 0.5)
     return np.power(np.power(10.0, 0.1 * np.asarray(x)), 0.5)
+
+
+def normalize_spectrogram(S, is_mel):
+    """Normalize log-magnitude spectrogram (the constants are the ones train.py sets from the training set)."""
+    if is_mel: return (S - hp.mel_normalize_mean) / hp.mel_normalize_variance
+    else:      return (S - hp.lin_normalize_mean) / hp.lin_normalize_variance
 
 
 def denormalize_spectrogram(S, is_mel):
@@ -173,3 +180,147 @@ def inverse_spectrogram(s, mel=False, phases=None):
 def inverse_mel_spectrogram(s, phases=None):
     """Convert log-mel-spectrogram to waveform."""
     return inverse_spectrogram(s, True, phases)
+
+
+def analysis_shape(B, total_samples, total_frames, mel):
+    """The library shape of an analysis batch under the current hp."""
+    return _lib.AnalysisShape(int(B), int(total_samples), int(total_frames), int(hp.num_fft), ms_to_frames(hp.stft_shift_ms),
+                              ms_to_frames(hp.stft_window_ms), int(hp.num_mels) if mel else 0,
+                              float(hp.preemphasis) if hp.use_preemphasis else 0.0)
+
+
+def _work_device(tensors):
+    """The device of the first CUDA tensor, else the current CUDA device."""
+    device = next((t.device for t in tensors if t.is_cuda), None)
+    if device is None:
+        device = torch.device('cuda', torch.cuda.current_device()) if torch.cuda.is_available() else torch.device('cuda')
+    return device
+
+
+def _as_float_tensor(x, what, dims):
+    """numpy or torch -> (tensor, came as numpy); ValueError unless it is a non-empty floating array of `dims` dimensions."""
+    is_np = not isinstance(x, torch.Tensor)
+    if is_np:
+        x = np.asarray(x)
+        if not np.issubdtype(x.dtype, np.floating):
+            raise ValueError(f'{what} has dtype {x.dtype}; expected floating point')
+        x = torch.from_numpy(np.ascontiguousarray(x))
+    elif not torch.is_floating_point(x):
+        raise ValueError(f'{what} has dtype {x.dtype}; expected floating point')
+    if x.dim() != dims or x.numel() == 0:
+        raise ValueError(f'{what} has shape {tuple(x.shape)}; expected a non-empty {dims}-D array')
+    return x, is_np
+
+
+def _return_like(t, is_np, src):
+    if is_np:
+        return t.cpu().numpy()
+    return t if src.is_cuda else t.cpu()
+
+
+def spectrogram_batch(waveforms, mel=False):
+    """Waveforms [L_i] -> log-magnitude (mel) spectrograms [bins, F_i], F_i = 1 + L_i // hop, in input order (reference
+    utils/audio.py:66-78): pre-emphasis (hp.use_preemphasis), |stft| with centre reflect padding, the mel projection when `mel`, then
+    amplitude_to_db relative to each utterance's own maximum.  Waveforms are computed in fp32: a float64 input is rounded to fp32 first (16-bit
+    PCM scaled by 2^-15 is exact); the transform itself runs in fp64.  The work runs on the device of the first CUDA input, or on the current
+    CUDA device when no input is on one.  numpy in -> numpy out; torch in -> torch out, on that device for CUDA inputs and on the CPU for CPU
+    inputs."""
+    if not isinstance(waveforms, (list, tuple)) or len(waveforms) == 0:
+        raise ValueError('spectrogram_batch expects a non-empty list of 1-D waveforms')
+    ins = [_as_float_tensor(w, f'waveform {i}', 1) for i, w in enumerate(waveforms)]
+    waves = [t for t, _ in ins]
+    hop = ms_to_frames(hp.stft_shift_ms)
+    lengths = [int(w.numel()) for w in waves]
+    frames = [1 + n // hop for n in lengths]
+    soff_host = np.concatenate([[0], np.cumsum(lengths)]).astype(np.int64)
+    off_host = np.concatenate([[0], np.cumsum(frames)]).astype(np.int64)
+    if soff_host[-1] >= 2 ** 31:
+        raise ValueError(f'{soff_host[-1]} samples in one batch; at most 2^31 - 1')
+    device = _work_device(waves)
+    with torch.cuda.device(device):
+        shape = analysis_shape(len(waves), soff_host[-1], off_host[-1], mel)
+        wave = torch.cat([w.to(device=device, dtype=torch.float32) for w in waves]).contiguous()
+        soff = torch.from_numpy(soff_host.astype(np.int32)).to(device)
+        off = torch.from_numpy(off_host.astype(np.int32)).to(device)
+        basis = mel_tables(hp.sample_rate, hp.num_fft, hp.num_mels, device)[0] if mel else None
+        S = F.stft_magnitude(shape, wave, soff, off, basis)
+        F.amplitude_to_db(shape, S, off, out=S)
+    return [_return_like(S[off_host[i]:off_host[i + 1]].t().contiguous(), ins[i][1], waves[i]) for i in range(len(waves))]
+
+
+def spectrogram(y, mel=False):
+    """Convert waveform to log-magnitude spectrogram [bins, 1 + len(y) // hop] (reference utils/audio.py:66-73)."""
+    return spectrogram_batch([y], mel)[0]
+
+
+def mel_spectrogram(y):
+    """Convert waveform to log-mel-spectrogram."""
+    return spectrogram(y, True)
+
+
+def _cepstra(specs, device):
+    """[n_mels, F_i] tensors -> packed cepstra [sum F, n_mfcc] on `device` and host frame offsets."""
+    off_host = np.concatenate([[0], np.cumsum([s.shape[1] for s in specs])]).astype(np.int64)
+    mel_db = torch.cat([s.to(device=device, dtype=torch.float32).t() for s in specs]).contiguous()
+    return F.mel_cepstrum(mel_db, hp.num_mfcc), off_host
+
+
+def _check_mfcc_input(S, what):
+    t, is_np = _as_float_tensor(S, what, 2)
+    if t.shape[0] < hp.num_mfcc:
+        raise ValueError(f'{what} has {t.shape[0]} mel bands; hp.num_mfcc = {hp.num_mfcc} needs at least as many')
+    return t, is_np
+
+
+def get_spectrogram_mfcc(S):
+    """Compute MFCCs [hp.num_mfcc, F] of a log-mel spectrogram [n_mels, F]: librosa 0.7.0 mfcc(S=S/10), the orthonormal DCT-II over the
+    mel axis, c0 included (reference utils/audio.py:117-119)."""
+    t, is_np = _check_mfcc_input(S, 'spectrogram')
+    device = _work_device([t])
+    with torch.cuda.device(device):
+        cep, _ = _cepstra([t], device)
+    return _return_like(cep.t().contiguous(), is_np, t)
+
+
+def mel_cepstral_distortion_batch(S1s, S2s, mode='dtw'):
+    """Mel cepstral distortion of each pair (S1s[i], S2s[i]) of log-mel spectrograms [n_mels, F] (reference mel_cepstral_distorision, utils/
+    audio.py:127-161): MFCCs without c0, then the mean Euclidean frame distance over the frames paired by `mode`: 'cut' (the first min(F1, F2)
+    frames), 'stretch' (the shorter sequence indexed at i * n // m) or 'dtw'.  'dtw' is the exact dynamic-time-warping optimum, cost / path
+    length; the reference calls fastdtw with radius 1, which approximates that optimum, so the two agree when fastdtw finds the optimal path
+    and may differ otherwise.  Returns float64, one value per pair: a numpy array unless the first
+    input is a torch tensor (then a torch tensor on its device).  The work runs on the device of the first CUDA input, else on the current
+    device."""
+    if not isinstance(S1s, (list, tuple)) or not isinstance(S2s, (list, tuple)) or len(S1s) == 0:
+        raise ValueError('mel_cepstral_distortion_batch expects two non-empty lists of [n_mels, frames] spectrograms')
+    if len(S1s) != len(S2s):
+        raise ValueError(f'{len(S1s)} spectrograms against {len(S2s)}')
+    if mode not in _lib.MCD_MODES:
+        raise ValueError(f'unknown mode {mode!r}; expected one of {sorted(_lib.MCD_MODES)}')
+    a = [_check_mfcc_input(s, f'S1s[{i}]') for i, s in enumerate(S1s)]
+    b = [_check_mfcc_input(s, f'S2s[{i}]') for i, s in enumerate(S2s)]
+    for i, ((x, _), (y, _)) in enumerate(zip(a, b)):
+        if x.shape[0] != y.shape[0]:
+            raise ValueError(f'pair {i} has {x.shape[0]} and {y.shape[0]} mel bands')
+        if mode == 'dtw' and min(x.shape[1], y.shape[1]) > _lib.DTW_MAX_FRAMES:
+            raise ValueError(f'pair {i} ({x.shape[1]} x {y.shape[1]} frames): dtw keeps three anti-diagonals in shared memory, so the shorter '
+                             f'sequence may have at most {_lib.DTW_MAX_FRAMES} frames')
+    xs, ys = [t for t, _ in a], [t for t, _ in b]
+    device = _work_device(xs + ys)
+    with torch.cuda.device(device):
+        cep_a, off_a = _cepstra(xs, device)
+        cep_b, off_b = _cepstra(ys, device)
+        mcd, _ = F.mel_cepstral_distortion(cep_a, torch.from_numpy(off_a.astype(np.int32)).to(device), cep_b,
+                                           torch.from_numpy(off_b.astype(np.int32)).to(device), mode)
+    return _return_like(mcd, a[0][1], xs[0])
+
+
+def mel_cepstral_distorision(S1, S2, mode):
+    """Compute Mel Cepstral Distorsion between two mel spectrograms (reference spelling; see mel_cepstral_distortion_batch).
+
+    Arguments:
+        S1 and S2 -- mel spectrograms
+        mode -- 'cut' to cut off frames of longer seq.
+                'stretch' to stretch linearly the shorter seq.
+                'dtw' to compute DTW with minimal possible MCD (exact DTW, not fastdtw's approximation)
+    """
+    return float(mel_cepstral_distortion_batch([S1], [S2], mode)[0])
