@@ -74,6 +74,39 @@ int b200tts_gemm_f32(int transA, int transB, int M, int N, int K, float alpha, c
                      long long strideA, long long strideB, long long strideC, int splitk, float* workspace,
                      void* stream);
 
+/* Debug: the library's whole GEMM descriptor (GemmDesc in csrc/common.cuh: the same fields in the same order, the same meaning),
+ * so that tests can drive every feature of the dense contraction directly: batch strides, a_batch_mod, explicit split-K with
+ * keep_partials, bf16 operands read in place (A16 / B16) and the two-level K (kin, kosA, kosB). */
+typedef struct {
+    const float* A;
+    const float* B;
+    float* C;
+    const float* bias;
+    int M, N, K;
+    int lda, ldb, ldc;
+    int transA, transB;
+    float alpha, beta;
+    int batch;
+    long long strideA, strideB, strideC;
+    int a_batch_mod;
+    int splitk;
+    float* partial;
+    int keep_partials;
+    const void* A16;
+    int lda16;
+    const void* B16;
+    int ldb16;
+    int kin;
+    long long kosA, kosB;
+} b200tts_gemm_desc;
+/* route 0: the precision-mode dispatch (fp32 SIMT kernel, or the bf16 kernels: wgmma when it takes the shape, else mma.sync); the
+ * descriptor's splitk / partial / keep_partials are used as given.  route 1: the auto-split dispatch, which picks the split-K factor
+ * itself within `partial` (partial_elems floats; NULL = no split).  Returns a B200TTS_* status. */
+int b200tts_debug_gemm(const b200tts_gemm_desc* desc, int route, float* partial, size_t partial_elems, void* stream);
+/* Debug: open (1) or close (0) a pack-cache scope of the wgmma GEMM: inside it, bf16 operand packs are kept in the scratch and
+ * reused by later products that read the same source view (the source buffers must not change while it is open). */
+int b200tts_debug_gemm_pack_cache(int open);
+
 /* ---- decoder: Decoder._decode, modules/tacotron2.py:148-209 -------------------------------- */
 typedef struct {
     int B, L, T;            /* batch, padded text length, mel frames */

@@ -79,6 +79,17 @@ class AnalysisShape(Structure):
     _fields_ = [(n, c_int) for n in ('B', 'total_samples', 'total_frames', 'N', 'hop', 'win', 'n_mels')] + [('preemphasis', c_double)]
 
 
+class GemmDesc(Structure):
+    """b200tts_gemm_desc: the library's whole GEMM descriptor (csrc/common.cuh GemmDesc), for b200tts_debug_gemm."""
+    _fields_ = [('A', c_void_p), ('B', c_void_p), ('C', c_void_p), ('bias', c_void_p)] + \
+               [(n, c_int) for n in ('M', 'N', 'K', 'lda', 'ldb', 'ldc', 'transA', 'transB')] + \
+               [('alpha', c_float), ('beta', c_float), ('batch', c_int)] + \
+               [(n, c_longlong) for n in ('strideA', 'strideB', 'strideC')] + \
+               [('a_batch_mod', c_int), ('splitk', c_int), ('partial', c_void_p), ('keep_partials', c_int),
+                ('A16', c_void_p), ('lda16', c_int), ('B16', c_void_p), ('ldb16', c_int), ('kin', c_int),
+                ('kosA', c_longlong), ('kosB', c_longlong)]
+
+
 # include/b200tts.h: B200TTS_MCD_CUT / _STRETCH / _DTW and B200TTS_DTW_MAX_FRAMES
 MCD_MODES = {'cut': 0, 'stretch': 1, 'dtw': 2}
 DTW_MAX_FRAMES = 6455
@@ -101,6 +112,8 @@ SIGNATURES = {
     'b200tts_gemm_f32': (c_int, [c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_int, c_void_p, c_int, c_float,
                                  c_void_p, c_int, c_void_p, c_int, c_longlong, c_longlong, c_longlong, c_int, c_void_p,
                                  c_void_p]),
+    'b200tts_debug_gemm': (c_int, [POINTER(GemmDesc), c_int, c_void_p, c_size_t, c_void_p]),
+    'b200tts_debug_gemm_pack_cache': (c_int, [c_int]),
     'b200tts_decoder_workspace_bytes': (c_size_t, [POINTER(DecoderShape)]),
     'b200tts_decoder_bwd_workspace_bytes': (c_size_t, [POINTER(DecoderShape)]),
     'b200tts_decoder_path': (c_int, [POINTER(DecoderShape)]),

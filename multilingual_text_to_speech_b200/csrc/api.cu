@@ -283,6 +283,30 @@ int b200tts_gemm_f32(int transA, int transB, int M, int N, int K, float alpha, c
     return gemm_run(d, (cudaStream_t)stream);
 }
 
+static_assert(sizeof(b200tts_gemm_desc) == sizeof(GemmDesc), "b200tts_gemm_desc must list the fields of GemmDesc");
+int b200tts_debug_gemm(const b200tts_gemm_desc* desc, int route, float* partial, size_t partial_elems, void* stream) {
+    B200_REQUIRE(desc, "debug_gemm: null descriptor");
+    B200_REQUIRE(route == 0 || route == 1, "debug_gemm: unknown route %d", route);
+    B200_TRY(require_device());
+    const b200tts_gemm_desc& s = *desc;
+    GemmDesc d;
+    d.A = s.A; d.B = s.B; d.C = s.C; d.bias = s.bias;
+    d.M = s.M; d.N = s.N; d.K = s.K; d.lda = s.lda; d.ldb = s.ldb; d.ldc = s.ldc;
+    d.transA = s.transA; d.transB = s.transB; d.alpha = s.alpha; d.beta = s.beta;
+    d.batch = s.batch; d.strideA = s.strideA; d.strideB = s.strideB; d.strideC = s.strideC; d.a_batch_mod = s.a_batch_mod;
+    d.splitk = s.splitk; d.partial = s.partial; d.keep_partials = s.keep_partials;
+    d.A16 = s.A16; d.lda16 = s.lda16; d.B16 = s.B16; d.ldb16 = s.ldb16;
+    d.kin = s.kin; d.kosA = s.kosA; d.kosB = s.kosB;
+    if (route == 0) return gemm_run(d, (cudaStream_t)stream);
+    return gemm_run_auto(d, partial, partial ? partial_elems : 0, (cudaStream_t)stream);
+}
+
+int b200tts_debug_gemm_pack_cache(int open) {
+    if (open) tc_pack_cache_begin();
+    else tc_pack_cache_end();
+    return B200TTS_OK;
+}
+
 size_t b200tts_decoder_workspace_bytes(const b200tts_decoder_shape* shape) {
     if (!shape || validate_decoder_shape(*shape) != B200TTS_OK) return 0;
     return decoder_layout(step_shape(*shape)).total * sizeof(float);

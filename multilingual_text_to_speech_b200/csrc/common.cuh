@@ -122,8 +122,10 @@ struct GemmDesc {
     int splitk = 1;
     float* partial = nullptr;     // required when splitk > 1
     int keep_partials = 0;        // 1: leave the reduction to the consumer kernel (C untouched)
-    // optional: op(A) already available as bf16, K contiguous, row stride lda16 elements (16-byte aligned rows): the wgmma path
-    // reads it through TMA directly (no packing pass); A / lda are then ignored by that path
+    // optional (wgmma path, batch == 1): op(A) already available as bf16, read through TMA directly (no packing pass); A / lda are then
+    // ignored by that path, the other paths still multiply A.  !transA: [M, K] rows, K contiguous, row stride lda16 (multiple of 8,
+    // 16-byte aligned base).  transA (and kin == 0): [K, M] rows, M contiguous, row stride lda16 (multiple of 64, 16-byte aligned base),
+    // an MN-major operand like B16: the columns up to the next multiple of 64 beyond M must be readable (their products are never stored)
     const void* A16 = nullptr;
     int lda16 = 0;
     // optional (wgmma path, !transB, batch == 1): op(B) = B [K, N] already available as bf16 rows, row stride ldb16 elements (multiple of
@@ -132,7 +134,8 @@ struct GemmDesc {
     const void* B16 = nullptr;
     int ldb16 = 0;
     // optional two-level K (wgmma path only; needs !transA && transB): K = kouter * kin, element (row, q * kin + l) of op(A) lives at
-    // A[q * kosA + row * lda + l] (op(B) likewise with kosB): sums a product over `kouter` separately stored slabs in ONE GEMM
+    // A[q * kosA + row * lda + l] (op(B) likewise with kosB): sums a product over `kouter` separately stored slabs in ONE GEMM.
+    // gemm_f32 / gemm_bf16 reject kin > 0 (B200TTS_ERR_INVALID) when the wgmma path does not take the product
     int kin = 0;
     long long kosA = 0, kosB = 0;
 };

@@ -205,6 +205,7 @@ int gemm_bf16(const GemmDesc& d, cudaStream_t stream) {
         B200_TRY(gemm_tc_try(d, stream, &handled));
         if (handled) return B200TTS_OK;
     }
+    B200_REQUIRE(d.kin == 0, "gemm_bf16: two-level K (kin = %d) is taken by the wgmma path only, which declined this product", d.kin);
     B200_REQUIRE(d.A && d.B && (d.C || (d.splitk > 1 && d.keep_partials)), "gemm_bf16: null operand");
     B200_REQUIRE(d.splitk >= 1 && (d.splitk == 1 || d.partial), "gemm_bf16: split-K needs a partial workspace");
     KernelArgs p;

@@ -217,6 +217,7 @@ int gemm_f32(const GemmDesc& d, cudaStream_t stream) {
     if (d.M <= 0 || d.N <= 0 || d.batch <= 0) return B200TTS_OK;
     B200_REQUIRE(d.A && d.B && (d.C || (d.splitk > 1 && d.keep_partials)), "gemm_f32: null operand");
     B200_REQUIRE(d.splitk >= 1 && (d.splitk == 1 || d.partial), "gemm_f32: split-K needs a partial workspace");
+    B200_REQUIRE(d.kin == 0, "gemm_f32: two-level K (kin = %d) is taken by the wgmma path only", d.kin);
     KernelArgs p;
     p.A = d.A; p.B = d.B; p.C = d.C; p.bias = d.bias; p.partial = d.partial;
     p.M = d.M; p.N = d.N; p.K = d.K; p.lda = d.lda; p.ldb = d.ldb; p.ldc = d.ldc;
