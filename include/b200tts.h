@@ -271,6 +271,10 @@ int b200tts_attention_step_backward(int B, int L, int M, int A, int C, int K, co
                                     const float* weights, const float* d_context, const float* d_weights, float* d_cum, float* d_q,
                                     float* d_memory_transform, float* d_w_location, float* d_w_loc_features, float* d_w_energy,
                                     float* workspace, void* stream);
+/* The per-chunk position count LC the attention backward kernel runs (L, M, A, C, K) with: it processes each utterance's positions in
+ * chunks of LC, the largest multiple of 4 (at most L rounded up to 4) whose shared memory fits in 220 KB.  0 for dims the backward
+ * rejects, including an L for which not even 4-row chunks fit in the 227 KB limit.  Host only. */
+int b200tts_debug_attention_backward_chunk(int L, int M, int A, int C, int K);
 
 /* ---- single forward-attention step: ForwardAttention.forward, modules/attention.py:23-45,89-124 ----
  * e = v . tanh(query . Wq^T + memory_transform + bias) over ALL L positions; s = softmax(e) (padding included);

@@ -83,6 +83,8 @@ int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_
                           float* bws, size_t bws_bytes, const b200tts_decoder_params& dw, float* d_memory, cudaStream_t st);
 size_t decoder_bwd_workspace_floats(const b200tts_decoder_shape& s);
 size_t attention_step_backward_workspace_elems(int B, int M, int A, int C, int K);
+int attention_step_backward_validate(int B, int L, int M, int A, int C, int K);
+int attention_backward_chunk(int L, int M, int A, int C, int K);
 int attention_step_backward_impl(int B, int L, int M, int A, int C, int K, const float* q, const float* memory, const float* memT,
                                  const int* lengths, const float* Wloc, const float* Wc, const float* bias, const float* v,
                                  const float* cum_prev, const float* weights, const float* d_ctx, const float* d_weights, float* d_cum,
@@ -361,9 +363,12 @@ int b200tts_attention_step(int B, int L, int M, int D, int A, int C, int K, cons
                            const float* memory_transform, const int32_t* text_lengths, const float* w_query,
                            const float* w_location, const float* w_loc_features, const float* bias, const float* w_energy,
                            float* cum_weights, float* context, float* weights, float* workspace, void* stream) {
+    B200_REQUIRE(query && memory && memory_transform && text_lengths && w_query && w_location && w_loc_features && bias && w_energy &&
+                 cum_weights && context && weights && workspace, "attention_step: null argument");
+    B200_REQUIRE(B > 0 && L > 0 && M > 0 && D > 0 && A > 0 && C > 0 && K > 0,
+                 "attention_step: non-positive dimension (B=%d L=%d M=%d D=%d A=%d C=%d K=%d)", B, L, M, D, A, C, K);
+    B200_REQUIRE(A % 4 == 0, "attention_step: attention dimension %d must be a multiple of 4", A);
     B200_TRY(require_device());
-    B200_REQUIRE(query && memory && memory_transform && text_lengths && cum_weights && context && weights && workspace,
-                 "attention_step: null argument");
     return attention_step_impl(B, L, M, D, A, C, K, query, memory, memory_transform, text_lengths, w_query, w_location,
                                w_loc_features, bias, w_energy, cum_weights, context, weights, workspace, (cudaStream_t)stream);
 }
@@ -377,14 +382,17 @@ int b200tts_attention_step_backward(int B, int L, int M, int A, int C, int K, co
                                     const float* weights, const float* d_context, const float* d_weights, float* d_cum, float* d_q,
                                     float* d_memory_transform, float* d_w_location, float* d_w_loc_features, float* d_w_energy,
                                     float* workspace, void* stream) {
-    B200_TRY(require_device());
     B200_REQUIRE(q && memory && memory_transform && text_lengths && w_location && w_loc_features && bias && w_energy && cum_prev && weights &&
                  d_context && d_cum && d_q && d_memory_transform && d_w_location && d_w_loc_features && d_w_energy && workspace,
                  "attention_step_backward: null argument");
+    B200_TRY(attention_step_backward_validate(B, L, M, A, C, K));
+    B200_TRY(require_device());
     return attention_step_backward_impl(B, L, M, A, C, K, q, memory, memory_transform, text_lengths, w_location, w_loc_features, bias,
                                         w_energy, cum_prev, weights, d_context, d_weights, d_cum, d_q, d_memory_transform, d_w_location,
                                         d_w_loc_features, d_w_energy, workspace, (cudaStream_t)stream);
 }
+
+int b200tts_debug_attention_backward_chunk(int L, int M, int A, int C, int K) { return attention_backward_chunk(L, M, A, C, K); }
 
 size_t b200tts_forward_attention_step_workspace_elems(int B, int L, int A) { return (size_t)B * A + (size_t)B * L; }
 
@@ -466,6 +474,8 @@ int b200tts_lstm_cell_backward(int B, int D, int cell_kind, int training, float 
                                const uint8_t* mask_h, const uint8_t* mask_c, const float* d_h, float* d_c, float* d_h_prev, float* d_gates,
                                void* stream) {
     B200_REQUIRE(B > 0 && D > 0 && gates && c_prev && d_h && d_c && d_h_prev && d_gates, "lstm_cell_backward: bad argument");
+    B200_REQUIRE(cell_kind == B200TTS_CELL_DROPOUT || cell_kind == B200TTS_CELL_ZONEOUT, "lstm_cell_backward: bad cell kind %d", cell_kind);
+    B200_REQUIRE(rate_h >= 0.f && rate_h < 1.f && rate_c >= 0.f && rate_c < 1.f, "lstm_cell_backward: rates must be in [0, 1)");
     B200_TRY(require_device());
     B200_CUDA(cudaMemsetAsync(d_h_prev, 0, (size_t)B * D * sizeof(float), (cudaStream_t)stream));
     CellBwdArgs a{};

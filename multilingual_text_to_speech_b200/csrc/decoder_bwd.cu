@@ -1057,12 +1057,28 @@ void decoder_bwd_view_offsets(const b200tts_decoder_shape& s, size_t* out) {
 size_t attention_step_backward_workspace_elems(int B, int M, int A, int C, int K) {
     return (size_t)B * ((size_t)A * C + (size_t)C * K + A + M);
 }
+int attention_step_backward_validate(int B, int L, int M, int A, int C, int K) {
+    B200_REQUIRE(B > 0 && L > 0 && M > 0 && A > 0 && C > 0 && K > 0, "attention_step_backward: non-positive dimension (B=%d L=%d M=%d A=%d C=%d K=%d)",
+                 B, L, M, A, C, K);
+    B200_REQUIRE(A <= 128 && A % 4 == 0 && C % 4 == 0 && (A / 4) * (C / 4) <= ATT_THREADS && M <= 512 && (K % 2) == 1,
+                 "attention_step_backward: unsupported dims A=%d C=%d M=%d K=%d", A, C, M, K);
+    return B200TTS_OK;
+}
+// the per-chunk position count LC launch_attn_bwd runs these dims with, or 0 when not even 4-row chunks fit in shared memory
+int attention_backward_chunk(int L, int M, int A, int C, int K) {
+    if (attention_step_backward_validate(1, L, M, A, C, K) != B200TTS_OK) return 0;
+    const int LC = pick_attn_bwd_chunk(L, M, A, C, K);
+    if ((size_t)attn_bwd_smem(L, M, A, C, K, LC).total * sizeof(float) > 227 * 1024) {
+        set_last_error("attention backward: L=%d does not fit in shared memory (M=%d A=%d C=%d K=%d)", L, M, A, C, K);
+        return 0;
+    }
+    return LC;
+}
 int attention_step_backward_impl(int B, int L, int M, int A, int C, int K, const float* q, const float* memory, const float* memT,
                                  const int* lengths, const float* Wloc, const float* Wc, const float* bias, const float* v,
                                  const float* cum_prev, const float* weights, const float* d_ctx, const float* d_weights, float* d_cum,
                                  float* d_q, float* d_memT, float* d_Wloc, float* d_Wc, float* d_v, float* ws, cudaStream_t st) {
-    B200_REQUIRE(A <= 128 && A % 4 == 0 && C % 4 == 0 && (A / 4) * (C / 4) <= ATT_THREADS && M <= 512 && (K % 2) == 1,
-                 "attention_step_backward: unsupported dims A=%d C=%d M=%d K=%d", A, C, M, K);
+    B200_TRY(attention_step_backward_validate(B, L, M, A, C, K));
     float* dWloc_acc = ws;
     float* dWc_acc = dWloc_acc + (size_t)B * A * C;
     float* dv_acc = dWc_acc + (size_t)B * C * K;

@@ -110,11 +110,11 @@ def sigmoid_err(z, mode):
     """Maximum error of the gate sigmoid.  persist: sigmoid_fast = __fdividef(1, 1 + __expf(-x)) (decoder_persist_tc.cu:164):
     __expf is within 2 + floor(|1.173 x|) ulp and __fdividef within 2 ulp (CUDA C++ Programming Guide, intrinsic functions);
     an error e of exp(-x) moves 1 / (1 + exp(-x)) by s (1 - s) e.  Otherwise sigmoidf_acc = 1 / (1 + expf(-x)) (common.cuh:97):
-    expf within 2 ulp, IEEE division."""
+    expf within 2 ulp, then two roundings (the sum 1 + expf(-x) and the IEEE division), 2^-24 of s each."""
     s = torch.sigmoid(z)
     if mode == 'persist':
         return s * (1 - s) * ((2 + 1.173 * z.abs()) * ULP1 + U) + 2 * ULP1 * s
-    return s * (1 - s) * (2 * ULP1 + U) + U * s
+    return s * (1 - s) * (2 * ULP1 + U) + 2 * U * s
 
 
 def tanh_gate_err(x, mode):
@@ -266,12 +266,20 @@ def attention_weights(q, cum, memTr, lengths, prm, mode, wcomb=None):
     b_e = b_t @ v.abs() + (A + 2) * U * (t.abs() @ v.abs())
     lens = lengths.to(cum.device).long().clamp(0, L)
     valid = torch.arange(L, device=cum.device)[None, :] < lens[:, None]           # [B, L]
-    em = e.masked_fill(~valid[None], -math.inf)
-    w = torch.softmax(em, -1).masked_fill(~valid[None], 0.0)
-    spread = (e - em.max(-1, keepdim=True).values).abs().masked_fill(~valid[None], 0.0)
-    b_ew = b_e.masked_fill(~valid[None], 0.0)
-    b_w = w * (b_ew + (w * b_ew).sum(-1, keepdim=True)) + w * (U * spread + (lens[None, :, None].double() + 8) * U)
+    w, b_w = softmax(e, b_e, valid[None], lens[None, :, None])
     return w, b_w, valid
+
+
+def softmax(e, b_e, valid, n):
+    """fp32 softmax over the last dim where `valid` (0 elsewhere): exp(e - max) / sum of the n valid terms, from energies e with bound
+    b_e.  A weight below the fp32 range comes out as 0 or a subnormal: 4 subnormal ulps (2^-147) absolute cover the expf underflow
+    and the division by a sum >= 1.  -> (weights, bound)"""
+    em = e.masked_fill(~valid, -math.inf)
+    w = torch.softmax(em, -1).masked_fill(~valid, 0.0)
+    spread = (e - em.max(-1, keepdim=True).values).abs().masked_fill(~valid, 0.0)
+    b_ew = b_e.masked_fill(~valid, 0.0)
+    b_w = w * (b_ew + (w * b_ew).sum(-1, keepdim=True)) + w * (U * spread + (torch.as_tensor(n).double() + 8) * U)
+    return w, b_w + valid * 2.0 ** -147
 
 
 def _dims(v):
@@ -449,6 +457,45 @@ def _reverse(v, cfg, mode, rep, name, hist, hist_b, gates, cstate, static, extra
     return rep
 
 
+def attention_backward(dw, b_dw, w, lens, t, b_t, v_e, wcb, wcb_abs, K, mode):
+    """One step of the location-sensitive attention backward from the total d weights dw [B, L] (zero at l >= len, bound b_dw), the
+    kernel's weights w [B, L] and t = tanh(energy argument) [B, L, A] recomputed by energy_tanh (bound b_t).  Wcomb = Wloc . Wc
+    [A, K] as the location term reads it (wcb, and |Wloc| . |Wc| or |Wcomb| as wcb_abs).  The persistent reverse loop
+    (decoder_persist_bwd.cu:411-422, :453-492) and the per-step kernel (decoder_bwd.cu attn_bwd_kernel, phases 3-5) share this math:
+        softmax backward   de = w (dw - <w, dw>)
+        energies backward  ds = de v (1 - t^2)                   (ds rounded to bf16 before the location term in persist mode)
+        location term      dloc[j] = sum_k G[j + half - k, k],  G = ds . Wcomb
+    -> {de, b_de, ds, b_ds, dloc, b_loc, a_loc (sum of |G| terms)}"""
+    B, L = dw.shape
+    half = (K - 1) // 2
+    dot = (w * dw).sum(-1, keepdim=True)
+    b_dot = (w * b_dw).sum(-1, keepdim=True) + (lens[:, None].double() + 2) * U * (w * dw).abs().sum(-1, keepdim=True)
+    de = w * (dw - dot)
+    b_de = w * (b_dw + b_dot) + 2 * U * (w * (dw.abs() + dot.abs()))
+    s = 1 - t * t
+    b_s = 2 * t.abs() * b_t + b_t * b_t + 2 * U * (s.abs() + t * t)
+    ds = de[..., None] * v_e * s
+    b_ds = v_e.abs() * (s.abs() * b_de[..., None] + de.abs()[..., None] * b_s) + 3 * U * ds.abs()
+    if mode == 'persist':
+        dsr = rn(ds)
+        b_dsr = b_ds + 2.0 ** -8 * ds.abs()          # RN of the kernel's ds vs RN of the reference: at most one bf16 ulp apart + b_ds
+    else:
+        dsr, b_dsr = ds, b_ds
+    A = v_e.numel()
+    G = dsr @ wcb                                                              # [B, L, K]
+    aG = dsr.abs() @ wcb_abs
+    b_G = b_dsr @ wcb_abs + (A + 2) * U * aG
+    dloc, b_loc, a_loc = torch.zeros_like(dw), torch.zeros_like(dw), torch.zeros_like(dw)
+    for k in range(K):
+        lo, hi = max(0, k - half), min(L, L + k - half)                       # j with 0 <= l = j + half - k < L
+        if lo >= hi:
+            continue
+        dloc[:, lo:hi] += G[:, lo + half - k:hi + half - k, k]
+        b_loc[:, lo:hi] += b_G[:, lo + half - k:hi + half - k, k]
+        a_loc[:, lo:hi] += G[:, lo + half - k:hi + half - k, k].abs()
+    return {'de': de, 'b_de': b_de, 'ds': ds, 'b_ds': b_ds, 'dloc': dloc, 'b_loc': b_loc, 'a_loc': a_loc}
+
+
 class AttentionReverse:
     """The attention backward of the attention reverse loop, step by step (decoder_persist_bwd.cu:298-545; the per-step chains:
     att_bwd_step, decoder_bwd.cu:937-968), from the kernel's own total d context, alignments, queries and cumulative weights.  The d cum
@@ -493,7 +540,7 @@ class AttentionReverse:
 
     def step(self, i):
         v, mode, rep = self.v, self.mode, self.rep
-        T, M, L, A, K, half = self.T, self.M, self.L, self.A, self.K, self.half
+        T, M, L, K = self.T, self.M, self.L, self.K
         last = i == T - 1
         valid = self.valid
         if i == self.lose_carry_at:
@@ -521,20 +568,11 @@ class AttentionReverse:
             b_dw = b_dw + self.b_dcum
         b_dw = (b_dw + 2 * U * dw.abs()).masked_fill(~valid, 0.0)
         dw = dw.masked_fill(~valid, 0.0)
-        # ---- softmax backward with the kernel's weights (:411-422)
+        # ---- softmax, energies and location-term backward with the kernel's weights and t recomputed from its q and cum
         w = self.al[:, i].double().masked_fill(~valid, 0.0)
-        dot = (w * dw).sum(-1, keepdim=True)
-        b_dot = (w * b_dw).sum(-1, keepdim=True) + (self.lens[:, None].double() + 2) * U * (w * dw).abs().sum(-1, keepdim=True)
-        de = w * (dw - dot)
-        b_de = w * (b_dw + b_dot) + 2 * U * (w * (dw.abs() + dot.abs()))
-        # ---- energies backward: ds = de v (1 - t^2) with t recomputed from the kernel's q and cum (:453-473)
         t, b_t = energy_tanh(v['q'][i:i + 1], v['cum'][i:i + 1], self.memTr, self.prm, mode, self.wcomb)
-        t, b_t = t[0], b_t[0]                                                  # [B, L, A]
-        s = 1 - t * t
-        b_s = 2 * t.abs() * b_t + b_t * b_t + 2 * U * (s.abs() + t * t)
-        ve = self.v_e
-        ds = de[..., None] * ve * s
-        b_ds = ve.abs() * (s.abs() * b_de[..., None] + de.abs()[..., None] * b_s) + 3 * U * ds.abs()
+        ab = attention_backward(dw, b_dw, w, self.lens, t[0], b_t[0], self.v_e, self.wcb, self.wcb_abs, K, mode)
+        ds, b_ds = ab['ds'], ab['b_ds']
         dq = ds.sum(1)
         b_dq = b_ds.sum(1) + (L + 4) * U * ds.abs().sum(1)
         if self.fill:
@@ -542,25 +580,9 @@ class AttentionReverse:
         rep.add('dq', i, (v['dq'][i].double() - dq).abs()[None], b_dq[None])
         self.dmemT = self.dmemT + ds
         self.b_dmemT = self.b_dmemT + b_ds + U * self.dmemT.abs()
-        # ---- d cum of step i-1: carry + sum_k G[j + half - k, k], G = ds . Wcomb, ds rounded to bf16 in persist mode (:473, :476-492)
-        if mode == 'persist':
-            dsr = rn(ds)
-            b_dsr = b_ds + 2.0 ** -8 * ds.abs()          # RN of the kernel's ds vs RN of the reference: at most one bf16 ulp apart + b_ds
-        else:
-            dsr, b_dsr = ds, b_ds
-        G = dsr @ self.wcb                                                     # [B, L, K]
-        aG = dsr.abs() @ self.wcb_abs
-        b_G = b_dsr @ self.wcb_abs + (A + 2) * U * aG
-        dloc, b_loc, a_loc = torch.zeros_like(self.dcum), torch.zeros_like(self.dcum), torch.zeros_like(self.dcum)
-        for k in range(K):
-            lo, hi = max(0, k - half), min(L, L + k - half)                   # j with 0 <= l = j + half - k < L
-            if lo >= hi:
-                continue
-            dloc[:, lo:hi] += G[:, lo + half - k:hi + half - k, k]
-            b_loc[:, lo:hi] += b_G[:, lo + half - k:hi + half - k, k]
-            a_loc[:, lo:hi] += G[:, lo + half - k:hi + half - k, k].abs()
-        self.dcum = self.dcum + dloc
-        self.b_dcum = self.b_dcum + b_loc + (K + 2) * U * (a_loc + self.dcum.abs())
+        # ---- d cum of step i-1: carry + the location term's transposed convolution
+        self.dcum = self.dcum + ab['dloc']
+        self.b_dcum = self.b_dcum + ab['b_loc'] + (K + 2) * U * (ab['a_loc'] + self.dcum.abs())
 
     def finish(self):
         if self.fill:

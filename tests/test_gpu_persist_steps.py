@@ -112,6 +112,14 @@ def test_step_checker_on_the_fp32_per_step_chains():
     _step_check(8, 40, 12, 288, 1024, 'zoneout', precision='fp32', expect_mode='fp32')
 
 
+def test_step_checker_on_the_fp32_per_step_chains_two_attention_chunks():
+    """L = 300: the decoder's per-step attention backward runs each utterance's positions in two chunks (LC = 172)"""
+    from multilingual_text_to_speech_b200 import _lib
+    LC = _lib.load().b200tts_debug_attention_backward_chunk(300, 288, 128, 32, 31)
+    assert -(-300 // LC) == 2, LC
+    _step_check(8, 300, 6, 288, 1024, 'zoneout', precision='fp32', expect_mode='fp32')
+
+
 def test_step_checker_on_the_bf16_per_step_chains_d1280():
     _step_check(8, 60, 10, 288, 1280, 'zoneout', expect_mode='chain_bf16')
 
