@@ -494,6 +494,86 @@ int b200tts_mel_cepstrum(int total_frames, int n_mels, int n_mfcc, const float* 
 int b200tts_mel_cepstral_distortion(int B, int n_mfcc, int mode, const float* cep_a, const int32_t* off_a, const float* cep_b,
                                     const int32_t* off_b, double* mcd_out, int32_t* path_len_out, void* stream);
 
+/* ---- WaveRNN vocoder (fatchord architecture): mel -> waveform, one GRU step per sample over fold rows ----
+ * The MelResNet and the time-batched conditioning products run on the convolution-block and GEMM entry points; these entry points add
+ * the mel upsampling layers, the folding, the persistent sample loop and the unfolding.  Fold rows: utterance b's F_b hop sample
+ * positions are cut into folds of fold_len = target + 2 overlap samples starting every target + overlap (fold_with_overlap, the tail
+ * zero-padded); the rows of all utterances are numbered consecutively.  These entry points are fp32 whatever b200tts_set_precision
+ * says, except the loop's recurrent products (bf16 operands, fp32 accumulation and state); the convolution-block and GEMM stages follow
+ * the precision mode, which WaveRNN.generate_batch sets to fp32 for the duration of a call. */
+#define B200TTS_WAVERNN_RAW 0
+#define B200TTS_WAVERNN_MOL 1
+/* out[c, i] = sum_{k=-s..s} fir[k + s] in[c, (i + k) / s] over 0 <= i + k < len s: nearest stretch x s, then the FIR of 2s+1 taps with zero
+ * padding s (an upsampling layer pair).  in [C, len], out [C, len s], fp32. */
+int b200tts_wavernn_upsample_layer(int C, int len, int scale, const float* fir, const float* in, float* out, void* stream);
+typedef struct {
+    int B, rows;          /* utterances; fold rows of all of them */
+    int n_mels, aux_dims; /* feature columns: the mel path, then the MelResNet output (all four quarters) */
+    int hop, pad, scale;  /* hop = the product of the upsampling factors; pad frames on each side; scale = the last factor */
+    int target, overlap;
+    int max_frames;       /* aux is [B, max_frames, aux_dims] */
+} b200tts_wavernn_fold_shape;
+/* feat [nsteps, rows, n_mels + aux_dims] for the loop steps [t0, t0 + nsteps): row r (utterance row_utt[r], fold row_fold[r]) at step t is
+ * sample position q = fold (target + overlap) + t; zero for q >= F_b hop.  Mel columns: the last upsampling layer (taps fir [2 scale + 1])
+ * at the uncut position q + pad hop, from mel_up + mel_off[b], the penultimate layer [n_mels, (F_b + 2 pad) hop / scale] of the padded
+ * mel; aux columns: aux[b, q / hop, :].  frames, row_utt, row_fold: int32; mel_off: int64 element offsets; all on the device. */
+int b200tts_wavernn_fold(const b200tts_wavernn_fold_shape* shape, const float* mel_up, const int64_t* mel_off, const int32_t* frames,
+                         const int32_t* row_utt, const int32_t* row_fold, const float* fir, const float* aux, int t0, int nsteps, float* feat,
+                         void* stream);
+typedef struct {
+    int rows;             /* fold rows of one loop */
+    int rnn_dims;         /* R: a multiple of 128, at most 640 */
+    int fc_dims;          /* a multiple of 128, at most 2048 */
+    int n_out;            /* fc3 outputs: RAW 2^bits (2..2048 classes), MOL 3 x mixtures (mixtures <= 32) */
+    int mode;             /* B200TTS_WAVERNN_RAW / _MOL */
+    int fold_len;         /* steps of a fold row: the row length of the uniform tape and of the output */
+} b200tts_wavernn_shape;
+/* fp32, row-major, on the device.  The loop multiplies bf16 copies of w_hh1, w_ih2x, w_hh2, w_fc1x, w_fc2x and w_fc3. */
+typedef struct {
+    const float* w_hh1;   /* rnn1.weight_hh_l0 [3R, R] */
+    const float* b_hh1;   /* [3R] */
+    const float* u1;      /* rnn1.weight_ih_l0 . I.weight[:, 0] [3R]: the previous sample's share of GRU1's input gates */
+    const float* w_prev;  /* I.weight[:, 0] [R] */
+    const float* w_ih2x;  /* rnn2.weight_ih_l0[:, :R] [3R, R] */
+    const float* w_hh2;   /* [3R, R] */
+    const float* b_hh2;   /* [3R] */
+    const float* w_fc1x;  /* fc1.weight[:, :R] [fc, R] */
+    const float* w_fc2x;  /* fc2.weight[:, :fc] [fc, fc] */
+    const float* w_fc3;   /* [n_out, fc] */
+    const float* b_fc3;   /* [n_out] */
+} b200tts_wavernn_params;
+/* The products of one chunk of steps that do not depend on the previous sample, [nsteps, rows, width] fp32:
+ *   c = I.weight[:, 1:] . [mel, a1] + I.bias (R);  g1 = rnn1.weight_ih_l0 . c + b_ih1 (3R);  c2 = rnn2.weight_ih_l0[:, R:] . a2 + b_ih2 (3R);
+ *   p1 = fc1.weight[:, R:] . a3 + fc1.bias (fc);  p2 = fc2.weight[:, fc:] . a4 + fc2.bias (fc). */
+typedef struct { const float *c, *g1, *c2, *p1, *p2; } b200tts_wavernn_cond;
+/* Host only: the loop workspace (packed bf16 weights, state, activation rows, grid barrier); 0 for an invalid shape (message set). */
+size_t b200tts_wavernn_workspace_bytes(const b200tts_wavernn_shape* shape);
+/* Packs the weights into the workspace (256-byte aligned) and zeroes the state (h1 = h2 = 0, previous sample 0) and the abort flag. */
+int b200tts_wavernn_prepare(const b200tts_wavernn_shape* shape, const b200tts_wavernn_params* params, void* workspace, size_t workspace_bytes,
+                            void* stream);
+/* Steps [t0, t0 + nsteps) of every row, one cooperative launch of 128 CTAs (B200TTS_ERR_INVALID when they cannot be co-resident), carrying
+ * the state in the workspace from the previous call.  Per step: x = c + w_prev prev; h1 = GRU(x, h1); x += h1; h2 = GRU([x, a2], h2); x += h2;
+ * x = relu(fc1 [x, a3]); x = relu(fc2 [x, a4]); logits = fc3 x (torch GRU gate order r, z, n).  Sampling from the uniform tape
+ * uniforms [rows, fold_len, U]: RAW (U = 1): k = the smallest class whose softmax CDF exceeds u, sample 2k / (n_out - 1) - 1; MOL
+ * (U = mixtures + 1): each u mapped to 1e-5 + (1 - 2e-5) u, the component argmax(logit - log(-log u_j)), sample mean + exp(max(log_scale,
+ * log 1e-14)) (log u - log(1 - u)) clamped to [-1, 1].  The sample is the next step's prev and goes to out[row, t] ([rows, fold_len]).
+ * dbg (NULL: off) [nsteps, rows, 4R + 2 fc + n_out] receives each step's h1, bf16(x after GRU1), h2, bf16(x after GRU2), bf16(y1),
+ * bf16(y2) and the logits.  A grid-barrier timeout (about 2 s) raises the abort flag and ends the launch: see b200tts_wavernn_aborted. */
+int b200tts_wavernn_run(const b200tts_wavernn_shape* shape, const b200tts_wavernn_params* params, const b200tts_wavernn_cond* cond, int t0,
+                        int nsteps, const float* uniforms, float* out, float* dbg, void* workspace, size_t workspace_bytes, void* stream);
+/* Synchronises the stream and sets *aborted to the loop's abort flag (nonzero: a launch since the last prepare timed out). */
+int b200tts_wavernn_aborted(const b200tts_wavernn_shape* shape, const void* workspace, size_t workspace_bytes, int* aborted, void* stream);
+/* Optional de-emphasis of the loop's folded samples, in place, before b200tts_wavernn_unfold: each of `rows` rows of `len` samples is
+ * mu-law decoded when mu > 0 (fp64, then fp32; pass mu = 0 to unfold afterwards), then filtered by lfilter([1], [1, -a]) on the Griffin-Lim
+ * de-emphasis scan (fp32, without its normalisation).  a in (-1, 1); a = 0 only decodes. */
+int b200tts_wavernn_deemphasis(int rows, int len, int mu, float a, float* y, void* stream);
+/* Utterance b's (F_b - 1) hop samples at wave + wave_off[b] from its folds y[row_off[b] .. row_off[b + 1]) ([rows, target + 2 overlap]):
+ * mu-law decoded when mu > 0 (sign(y) / mu ((1 + mu)^|y| - 1)), the first and last `overlap` samples of each fold multiplied by
+ * [overlap / 2 zeros, sqrt(0.5 (1 + t))] and [sqrt(0.5 (1 - t)), zeros] (t = linspace(-1, 1, overlap - overlap / 2)), overlap-added in fold
+ * order, and the last 20 hop samples multiplied by linspace(1, 0, 20 hop).  fp64 arithmetic, fp32 output; total = sum (F_b - 1) hop. */
+int b200tts_wavernn_unfold(int B, int hop, int target, int overlap, int mu, const int32_t* frames, const int32_t* row_off, const int64_t* wave_off,
+                           long long total, const float* y, float* wave, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

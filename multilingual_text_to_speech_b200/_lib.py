@@ -90,6 +90,28 @@ class GemmDesc(Structure):
                 ('kosA', c_longlong), ('kosB', c_longlong)]
 
 
+class WaveRNNFoldShape(Structure):
+    _fields_ = [(n, c_int) for n in ('B', 'rows', 'n_mels', 'aux_dims', 'hop', 'pad', 'scale', 'target', 'overlap', 'max_frames')]
+
+
+class WaveRNNShape(Structure):
+    _fields_ = [(n, c_int) for n in ('rows', 'rnn_dims', 'fc_dims', 'n_out', 'mode', 'fold_len')]
+
+
+WAVERNN_PARAM_FIELDS = ('w_hh1', 'b_hh1', 'u1', 'w_prev', 'w_ih2x', 'w_hh2', 'b_hh2', 'w_fc1x', 'w_fc2x', 'w_fc3', 'b_fc3')
+
+
+class WaveRNNParams(Structure):
+    _fields_ = [(n, c_void_p) for n in WAVERNN_PARAM_FIELDS]
+
+
+class WaveRNNCond(Structure):
+    _fields_ = [(n, c_void_p) for n in ('c', 'g1', 'c2', 'p1', 'p2')]
+
+
+# include/b200tts.h: B200TTS_WAVERNN_RAW / _MOL
+WAVERNN_MODES = {'RAW': 0, 'MOL': 1}
+
 # include/b200tts.h: B200TTS_MCD_CUT / _STRETCH / _DTW and B200TTS_DTW_MAX_FRAMES
 MCD_MODES = {'cut': 0, 'stretch': 1, 'dtw': 2}
 DTW_MAX_FRAMES = 6455
@@ -173,6 +195,15 @@ SIGNATURES = {
     'b200tts_amplitude_to_db': (c_int, [POINTER(AnalysisShape), c_void_p, c_void_p, c_void_p, c_void_p]),
     'b200tts_mel_cepstrum': (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     'b200tts_mel_cepstral_distortion': (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'b200tts_wavernn_upsample_layer': (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'b200tts_wavernn_fold': (c_int, [POINTER(WaveRNNFoldShape)] + [c_void_p] * 7 + [c_int, c_int, c_void_p, c_void_p]),
+    'b200tts_wavernn_workspace_bytes': (c_size_t, [POINTER(WaveRNNShape)]),
+    'b200tts_wavernn_prepare': (c_int, [POINTER(WaveRNNShape), POINTER(WaveRNNParams), c_void_p, c_size_t, c_void_p]),
+    'b200tts_wavernn_run': (c_int, [POINTER(WaveRNNShape), POINTER(WaveRNNParams), POINTER(WaveRNNCond), c_int, c_int, c_void_p, c_void_p,
+                                    c_void_p, c_void_p, c_size_t, c_void_p]),
+    'b200tts_wavernn_aborted': (c_int, [POINTER(WaveRNNShape), c_void_p, c_size_t, POINTER(c_int), c_void_p]),
+    'b200tts_wavernn_deemphasis': (c_int, [c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
+    'b200tts_wavernn_unfold': (c_int, [c_int] * 5 + [c_void_p] * 3 + [c_longlong, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -195,6 +195,22 @@ int mcd_validate(int B, int n_mfcc, int mode);
 int mel_cepstrum_impl(int total_frames, int n_mels, int n_mfcc, const float* mel_db, float* out, cudaStream_t st);
 int mel_cepstral_distortion_impl(int B, int n_mfcc, int mode, const float* cep_a, const int* off_a, const float* cep_b, const int* off_b,
                                  double* mcd, int* path_len, cudaStream_t st);
+int wavernn_upsample_layer_check(int C, int len, int scale);
+int wavernn_upsample_layer_impl(int C, int len, int scale, const float* fir, const float* in, float* out, cudaStream_t st);
+int wavernn_fold_check(const b200tts_wavernn_fold_shape& s, int t0, int nsteps);
+int wavernn_fold_impl(const b200tts_wavernn_fold_shape& s, const float* mel_up, const long long* mel_off, const int* frames, const int* row_utt,
+                      const int* row_fold, const float* fir, const float* aux, int t0, int nsteps, float* feat, cudaStream_t st);
+size_t wavernn_workspace_bytes(const b200tts_wavernn_shape& s);
+int wavernn_check(const b200tts_wavernn_shape& s, void* ws, size_t ws_bytes);
+int wavernn_prepare_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, void* ws, size_t ws_bytes, cudaStream_t st);
+int wavernn_run_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, const b200tts_wavernn_cond& cond, int t0, int nsteps,
+                     const float* uniforms, float* out, float* dbg, void* ws, size_t ws_bytes, cudaStream_t st);
+int wavernn_aborted_impl(const b200tts_wavernn_shape& s, const void* ws, size_t ws_bytes, int* aborted, cudaStream_t st);
+int wavernn_deemphasis_check(int rows, int len, int mu, float a);
+int wavernn_deemphasis_impl(int rows, int len, int mu, float a, float* y, cudaStream_t st);
+int wavernn_unfold_check(int B, int hop, int target, int overlap, int mu);
+int wavernn_unfold_impl(int B, int hop, int target, int overlap, int mu, const int* frames, const int* row_off, const long long* wave_off,
+                        long long total, const float* y, float* wave, cudaStream_t st);
 }
 using namespace b200tts;
 
@@ -636,6 +652,60 @@ int b200tts_mel_cepstral_distortion(int B, int n_mfcc, int mode, const float* ce
     B200_TRY(mcd_validate(B, n_mfcc, mode));
     B200_TRY(require_device());
     return mel_cepstral_distortion_impl(B, n_mfcc, mode, cep_a, off_a, cep_b, off_b, mcd_out, path_len_out, (cudaStream_t)stream);
+}
+
+int b200tts_wavernn_upsample_layer(int C, int len, int scale, const float* fir, const float* in, float* out, void* stream) {
+    B200_REQUIRE(fir && in && out, "wavernn_upsample_layer: null argument");
+    B200_TRY(wavernn_upsample_layer_check(C, len, scale));
+    B200_TRY(require_device());
+    return wavernn_upsample_layer_impl(C, len, scale, fir, in, out, (cudaStream_t)stream);
+}
+int b200tts_wavernn_fold(const b200tts_wavernn_fold_shape* shape, const float* mel_up, const int64_t* mel_off, const int32_t* frames,
+                         const int32_t* row_utt, const int32_t* row_fold, const float* fir, const float* aux, int t0, int nsteps, float* feat,
+                         void* stream) {
+    B200_REQUIRE(shape && mel_up && mel_off && frames && row_utt && row_fold && fir && feat, "wavernn_fold: null argument");
+    B200_REQUIRE(aux || shape->aux_dims == 0, "wavernn_fold: null aux");
+    B200_TRY(wavernn_fold_check(*shape, t0, nsteps));
+    B200_TRY(require_device());
+    return wavernn_fold_impl(*shape, mel_up, reinterpret_cast<const long long*>(mel_off), frames, row_utt, row_fold, fir, aux, t0, nsteps, feat,
+                             (cudaStream_t)stream);
+}
+size_t b200tts_wavernn_workspace_bytes(const b200tts_wavernn_shape* shape) {
+    if (!shape) { set_last_error("wavernn_workspace_bytes: null shape"); return 0; }
+    return wavernn_workspace_bytes(*shape);
+}
+int b200tts_wavernn_prepare(const b200tts_wavernn_shape* shape, const b200tts_wavernn_params* params, void* workspace, size_t workspace_bytes,
+                            void* stream) {
+    B200_REQUIRE(shape && params, "wavernn_prepare: null argument");
+    B200_TRY(wavernn_check(*shape, workspace, workspace_bytes));
+    B200_TRY(require_device());
+    return wavernn_prepare_impl(*shape, *params, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_wavernn_run(const b200tts_wavernn_shape* shape, const b200tts_wavernn_params* params, const b200tts_wavernn_cond* cond, int t0,
+                        int nsteps, const float* uniforms, float* out, float* dbg, void* workspace, size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(shape && params && cond, "wavernn_run: null argument");
+    B200_TRY(wavernn_check(*shape, workspace, workspace_bytes));
+    B200_TRY(require_device());
+    return wavernn_run_impl(*shape, *params, *cond, t0, nsteps, uniforms, out, dbg, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_wavernn_aborted(const b200tts_wavernn_shape* shape, const void* workspace, size_t workspace_bytes, int* aborted, void* stream) {
+    B200_REQUIRE(shape && aborted, "wavernn_aborted: null argument");
+    B200_TRY(require_device());
+    return wavernn_aborted_impl(*shape, workspace, workspace_bytes, aborted, (cudaStream_t)stream);
+}
+int b200tts_wavernn_deemphasis(int rows, int len, int mu, float a, float* y, void* stream) {
+    B200_REQUIRE(y, "wavernn_deemphasis: null argument");
+    B200_TRY(wavernn_deemphasis_check(rows, len, mu, a));
+    B200_TRY(require_device());
+    return wavernn_deemphasis_impl(rows, len, mu, a, y, (cudaStream_t)stream);
+}
+int b200tts_wavernn_unfold(int B, int hop, int target, int overlap, int mu, const int32_t* frames, const int32_t* row_off, const int64_t* wave_off,
+                           long long total, const float* y, float* wave, void* stream) {
+    B200_REQUIRE(frames && row_off && wave_off && y && wave, "wavernn_unfold: null argument");
+    B200_TRY(wavernn_unfold_check(B, hop, target, overlap, mu));
+    B200_TRY(require_device());
+    return wavernn_unfold_impl(B, hop, target, overlap, mu, frames, row_off, reinterpret_cast<const long long*>(wave_off), total, y, wave,
+                               (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -220,14 +220,23 @@ __global__ void __launch_bounds__(NNLS_WARPS * 32) vocoder_mel_nnls_kernel(int t
 // De-emphasis y[n] = x[n] + a y[n - 1] (scipy lfilter([1], [1, -a])) and y /= max(y), one CTA per utterance.  Two-level scan of the
 // first-order recurrence: each thread runs its contiguous chunk from 0 and keeps (a^len, last value); the block scans those affine maps
 // (warp shuffles, then across warps); each thread re-runs its chunk from its carry.  The division is by the largest sample, not the largest
-// magnitude, as the reference's Python max(y) is.
+// magnitude, as the reference's Python max(y) is.  Rows (the WaveRNN folds): CTA b filters the row wave[b hop, (b + 1) hop) and does not
+// normalise; off is not read.
+template <bool Rows>
 __global__ void __launch_bounds__(DEEMPH_THREADS) vocoder_deemphasis_kernel(int hop, const int* __restrict__ off, float a,
                                                                            float* __restrict__ wave) {
     __shared__ float wa[32], wv[32], red[64];
     const int b = blockIdx.x;
-    const int ob = off[b];
-    const int L = hop * (off[b + 1] - ob - 1);
-    float* y = wave + (size_t)hop * (ob - b);
+    int L;
+    float* y;
+    if constexpr (Rows) {
+        L = hop;
+        y = wave + (size_t)hop * b;
+    } else {
+        const int ob = off[b];
+        L = hop * (off[b + 1] - ob - 1);
+        y = wave + (size_t)hop * (ob - b);
+    }
     const int chunk = (L + blockDim.x - 1) / blockDim.x;
     const int s0 = min(L, (int)threadIdx.x * chunk), s1 = min(L, s0 + chunk);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -260,6 +269,7 @@ __global__ void __launch_bounds__(DEEMPH_THREADS) vocoder_deemphasis_kernel(int 
     } else {
         for (int i = s0; i < s1; ++i) mx = fmaxf(mx, y[i]);
     }
+    if constexpr (Rows) return;
     mx = block_max(mx, red);
     for (int i = s0; i < s1; ++i) y[i] = y[i] / mx;
 }
@@ -381,7 +391,15 @@ int deemphasis_normalize_impl(const b200tts_vocoder_shape& s, float* wave, const
     FftPlan p;
     B200_TRY(vocoder_validate(s, &p));
     KernelTimer kt("vocoder_deemphasis", st);
-    vocoder_deemphasis_kernel<<<s.B, DEEMPH_THREADS, 0, st>>>(s.hop, off, s.preemphasis, wave);
+    vocoder_deemphasis_kernel<false><<<s.B, DEEMPH_THREADS, 0, st>>>(s.hop, off, s.preemphasis, wave);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+// y[r, :] = lfilter([1], [1, -a], y[r, :]) for each of `rows` rows of `len` samples, no normalisation (the WaveRNN folds)
+int deemphasis_rows_impl(int rows, int len, float a, float* y, cudaStream_t st) {
+    if (a == 0.f) return B200TTS_OK;
+    vocoder_deemphasis_kernel<true><<<rows, DEEMPH_THREADS, 0, st>>>(len, nullptr, a, y);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }

@@ -1,0 +1,611 @@
+// WaveRNN vocoder (fatchord architecture): mel -> waveform, one GRU step per audio sample.
+//
+//   * wavernn_upsample_layer_kernel: nearest stretch x s then the 1-channel FIR of 2s+1 taps with zero padding s (one up_layers pair of
+//     the upsampling network), every layer but the last, per utterance;
+//   * wavernn_fold_kernel: the last layer of the mel path evaluated at the positions a chunk of the sample loop needs, the `indent` cut, the
+//     nearest stretch of the MelResNet output (aux) and fold_with_overlap, as the [steps, rows, n_mels + aux_dims] rows of the conditioning
+//     GEMMs (the products that do not depend on the previous sample run in the library GEMM before the loop);
+//   * wavernn_loop_kernel: the persistent sample loop, one cooperative launch per chunk of steps (below);
+//   * wavernn_unfold_kernel: mu-law decode, the square-root cross-fades, overlap-add, the cut to (F - 1) hop samples and the linear fade-out.
+//
+// The sample loop.  128 CTAs of 256 threads; CTA c owns hidden units [c U, (c + 1) U) of both GRUs (U = rnn_dims / 128; the r, z and n rows
+// of its units form one 16-row weight tile per GRU matrix), fc1 / fc2 outputs [c V, (c + 1) V) (V = fc_dims / 128) and fc3 outputs
+// [c O, (c + 1) O) (O = ceil(n_out / 128)).  Its six bf16 tiles (W_hh1, the x part of W_ih2, W_hh2, the x parts of fc1 and fc2, fc3; 96 KB at
+// rnn = fc = 512) stay in shared memory for the whole launch, fragment-major so that each lane fetches its mma.sync A fragment with one
+// 16-byte load.  Activations travel between CTAs as bf16 rows in global memory (L2): every CTA multiplies its tiles by all fold rows, 8 rows
+// per m16n8k16 N tile, N tiles spread over the 8 warps, fp32 accumulation.  The K dimension is permuted identically in both operands
+// (lane t takes 8 consecutive elements per 32-element block), so a B fragment is one 16-byte load too.  One step of all rows:
+//   1. h1 = GRU1(G1 + u1 prev, W_hh1 h1 + b_hh1);  x1 = c + w prev + h1
+//   2. h2 = GRU2(W_ih2x x1 + C2, W_hh2 h2 + b_hh2);  x2 = x1 + h2
+//   3. y1 = relu(fc1x x2 + P1)     4. y2 = relu(fc2x y1 + P2)     5. logits = fc3 y2 + b3
+//   6. one warp per row samples from its logits (fixed-order reductions) and writes the row's next input
+// with a grid barrier after each stage: six per sample.  h1 and h2 are double-buffered by step parity (stage 1 / 2 of step t reads the
+// previous step's rows while owners write this step's).  fp32 state (h1, h2, x1, prev) is only read by its owner.
+#include <cuda_bf16.h>
+#include <math.h>
+#include "decoder_internal.cuh"
+#include "tc_ptx.cuh"
+
+namespace b200tts {
+
+namespace {
+
+using namespace tcx;
+
+constexpr int WR_CTAS = 128;
+constexpr int WR_THREADS = 256;
+constexpr int WR_WARPS = WR_THREADS / 32;
+constexpr int WR_MATS = 6;
+
+__device__ __forceinline__ __nv_bfloat16 bf(float v) { return __float2bfloat16_rn(v); }
+
+// ---- upsampling ----
+// out[c, i] = sum_{k=-s..s} w[k + s] in[c, (i + k) / s] over 0 <= i + k < len s (zero padding), i in [0, len s)
+__global__ void wavernn_upsample_layer_kernel(int C, int len, int s, const float* __restrict__ w, const float* __restrict__ in,
+                                              float* __restrict__ out) {
+    const long long n = (long long)C * len * s;
+    const int lo = len * s;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < n; idx += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(idx / lo), i = (int)(idx - (long long)c * lo);
+        const float* x = in + (size_t)c * len;
+        float acc = 0.f;
+        for (int k = -s; k <= s; ++k) {
+            const int j = i + k;
+            if (j >= 0 && j < lo) acc = fmaf(w[k + s], x[j / s], acc);
+        }
+        out[idx] = acc;
+    }
+}
+
+// feat[i, r, :] for loop steps t0 + i of fold row r: the row's utterance b and fold f give the sample position q = f (target + overlap) +
+// t0 + i of the utterance's F hop positions (zero beyond them: the tail padding of fold_with_overlap).  Columns [0, n_mels): the last mel
+// layer at the uncut position q + pad hop; columns [n_mels, n_mels + aux_dims): aux[b, q / hop, :].
+__global__ void wavernn_fold_kernel(b200tts_wavernn_fold_shape s, const float* __restrict__ mel_up, const long long* __restrict__ mel_off,
+                                    const int* __restrict__ frames, const int* __restrict__ row_utt, const int* __restrict__ row_fold,
+                                    const float* __restrict__ fir, const float* __restrict__ aux, int t0, int nsteps, float* __restrict__ feat) {
+    const int D = s.n_mels + s.aux_dims;
+    const long long n = (long long)nsteps * s.rows * D;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < n; idx += (long long)gridDim.x * blockDim.x) {
+        const int col = (int)(idx % D);
+        const long long ir = idx / D;
+        const int r = (int)(ir % s.rows), i = (int)(ir / s.rows);
+        const int b = row_utt[r], F = frames[b];
+        const long long q = (long long)row_fold[r] * (s.target + s.overlap) + t0 + i;
+        float v = 0.f;
+        if (q < (long long)F * s.hop) {
+            if (col < s.n_mels) {
+                const int len = (F + 2 * s.pad) * s.hop / s.scale;       // samples of the penultimate layer
+                const int lo = len * s.scale;
+                const float* x = mel_up + mel_off[b] + (size_t)col * len;
+                const int p = (int)q + s.pad * s.hop;
+                float acc = 0.f;
+                for (int k = -s.scale; k <= s.scale; ++k) {
+                    const int j = p + k;
+                    if (j >= 0 && j < lo) acc = fmaf(fir[k + s.scale], x[j / s.scale], acc);
+                }
+                v = acc;
+            } else {
+                v = aux[((size_t)b * s.max_frames + q / s.hop) * s.aux_dims + (col - s.n_mels)];
+            }
+        }
+        feat[idx] = v;
+    }
+}
+
+// ---- the sample loop ----
+struct WrDims {
+    int R, Fc, n_out, U, V, O;
+    int K[WR_MATS];       // inner dimension of each tile
+    int off[WR_MATS];     // uint4 offset of each tile inside one CTA's packed block
+    int per_cta;          // uint4 per CTA
+};
+__host__ __device__ inline WrDims wr_dims(int R, int Fc, int n_out) {
+    WrDims d;
+    d.R = R; d.Fc = Fc; d.n_out = n_out;
+    d.U = R / WR_CTAS; d.V = Fc / WR_CTAS; d.O = (n_out + WR_CTAS - 1) / WR_CTAS;
+    const int K[WR_MATS] = {R, R, R, R, Fc, Fc};
+    int o = 0;
+    for (int m = 0; m < WR_MATS; ++m) { d.K[m] = K[m]; d.off[m] = o; o += 2 * K[m]; }    // 16 rows x K bf16 = 2 K uint4
+    d.per_cta = o;
+    return d;
+}
+
+// weight row of tile row i of matrix m in CTA c (-1: zero row)
+__host__ __device__ inline int wr_tile_row(const WrDims& d, int m, int c, int i) {
+    if (m <= 2) return i < 3 * d.U ? (i / d.U) * d.R + c * d.U + i % d.U : -1;
+    if (m <= 4) return i < d.V ? c * d.V + i : -1;
+    const int o = c * d.O + i;
+    return (i < d.O && o < d.n_out) ? o : -1;
+}
+
+struct WrWeights { const float* w[WR_MATS]; };
+
+// packed[c][tile m][kb][s][lane] = {W[g][kk..kk+1], W[g+8][kk..kk+1], W[g][kk+2..kk+3], W[g+8][kk+2..kk+3]}, kk = 32 kb + 8 t + 4 s
+__global__ void wavernn_pack_kernel(WrDims d, WrWeights W, uint4* __restrict__ packed) {
+    const long long n = (long long)WR_CTAS * d.per_cta;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < n; idx += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(idx / d.per_cta), j = (int)(idx % d.per_cta);
+        int m = WR_MATS - 1;
+        while (d.off[m] > j) --m;
+        const int e = j - d.off[m];
+        const int lane = e & 31, s = (e >> 5) & 1, kb = e >> 6;
+        const int g = lane >> 2, t = lane & 3, kk = kb * 32 + 8 * t + 4 * s, K = d.K[m];
+        const int r0 = wr_tile_row(d, m, c, g), r1 = wr_tile_row(d, m, c, g + 8);
+        auto at = [&](int r, int k) { return r < 0 ? 0.f : W.w[m][(size_t)r * K + k]; };
+        uint4 v;
+        v.x = pack2(at(r0, kk), at(r0, kk + 1));
+        v.y = pack2(at(r1, kk), at(r1, kk + 1));
+        v.z = pack2(at(r0, kk + 2), at(r0, kk + 3));
+        v.w = pack2(at(r1, kk + 2), at(r1, kk + 3));
+        packed[idx] = v;
+    }
+}
+
+struct WrLoopArgs {
+    WrDims d;
+    int rows, mode, L, t0, nsteps;
+    const uint4* packed;
+    const float *b_hh1, *u1, *w_prev, *b_hh2, *b_fc3;
+    const float *cc, *g1, *c2, *p1, *p2;
+    const float* uni;
+    float* out;
+    float* dbg;
+    float *h1, *h2, *x1, *prev, *logits;
+    __nv_bfloat16 *h1b, *h2b, *x1b, *x2b, *y1b, *y2b;     // h1b / h2b: two slots of [rows, R]
+    unsigned* bar;
+    int* abort_flag;
+};
+
+// acc (16 x 8 tile: weight rows x fold rows row0..row0+7) = tile . act[row0 + n, 0:K]^T
+__device__ __forceinline__ void wr_mma(float (&acc)[4], const uint4* __restrict__ tile, const __nv_bfloat16* act, int K, int row0, int rows,
+                                       int lane) {
+    acc[0] = acc[1] = acc[2] = acc[3] = 0.f;
+    const int r = row0 + (lane >> 2), t = lane & 3;
+    const bool ok = r < rows;
+    const uint4* ap = reinterpret_cast<const uint4*>(act + (size_t)(ok ? r : 0) * K) + t;
+    const int nkb = K / 32;
+#pragma unroll 4
+    for (int kb = 0; kb < nkb; ++kb) {
+        uint4 v = make_uint4(0, 0, 0, 0);
+        if (ok) v = __ldcg(ap + kb * 4);
+        const uint4 a0 = tile[(kb * 2) * 32 + lane], a1 = tile[(kb * 2 + 1) * 32 + lane];
+        const uint32_t f0[4] = {a0.x, a0.y, a0.z, a0.w}, f1[4] = {a1.x, a1.y, a1.z, a1.w};
+        mma_bf16(acc, f0, v.x, v.y);
+        mma_bf16(acc, f1, v.z, v.w);
+    }
+}
+// the 16 x 8 accumulator tile into the warp's shared scratch [16][8]
+__device__ __forceinline__ void wr_spill(float* ep, const float (&acc)[4], int lane) {
+    const int g = lane >> 2, t = lane & 3;
+    ep[g * 8 + 2 * t] = acc[0];
+    ep[g * 8 + 2 * t + 1] = acc[1];
+    ep[(g + 8) * 8 + 2 * t] = acc[2];
+    ep[(g + 8) * 8 + 2 * t + 1] = acc[3];
+    __syncwarp();
+}
+
+__device__ __forceinline__ float gru_cell(float gir, float giz, float gin, float ghr, float ghz, float ghn, float h) {
+    const float r = sigmoidf_acc(gir + ghr), z = sigmoidf_acc(giz + ghz);
+    const float nn = tanhf(fmaf(r, ghn, gin));
+    return fmaf(z, h - nn, nn);       // (1 - z) n + z h
+}
+
+__global__ void __launch_bounds__(WR_THREADS, 1) wavernn_loop_kernel(WrLoopArgs a) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    __shared__ float s_ep[WR_WARPS][2][16 * 8];
+    __shared__ int s_ok;
+    const WrDims& d = a.d;
+    uint4* wt = reinterpret_cast<uint4*>(smem_raw);
+    const int c = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    {
+        const uint4* src = a.packed + (size_t)c * d.per_cta;
+        for (int i = threadIdx.x; i < d.per_cta; i += WR_THREADS) wt[i] = src[i];
+    }
+    __syncthreads();
+    const int R = d.R, Fc = d.Fc, rows = a.rows, ntiles = (rows + 7) / 8;
+    const int Ddbg = 4 * R + 2 * Fc + d.n_out;
+    const int U = d.U, V = d.V, O = d.O;
+    float* ep0 = s_ep[warp][0];
+    float* ep1 = s_ep[warp][1];
+    unsigned target = 0;
+
+    for (int i = 0; i < a.nsteps; ++i) {
+        const int tg = a.t0 + i;
+        const int cur = tg & 1, prv = cur ^ 1;
+        float* dbg = a.dbg ? a.dbg + (size_t)i * rows * Ddbg : nullptr;
+        // 1. GRU1
+        for (int nt = warp; nt < ntiles; nt += WR_WARPS) {
+            float acc[4];
+            wr_mma(acc, wt + d.off[0], a.h1b + (size_t)prv * rows * R, R, nt * 8, rows, lane);
+            wr_spill(ep0, acc, lane);
+            for (int e = lane; e < U * 8; e += 32) {
+                const int j = e >> 3, n = e & 7, row = nt * 8 + n, u = c * U + j;
+                if (row < rows) {
+                    const float p = __ldcg(a.prev + row);
+                    const float* g1 = a.g1 + ((size_t)i * rows + row) * 3 * R;
+                    const float gir = fmaf(a.u1[u], p, g1[u]), giz = fmaf(a.u1[R + u], p, g1[R + u]), gin = fmaf(a.u1[2 * R + u], p, g1[2 * R + u]);
+                    const float ghr = ep0[j * 8 + n] + a.b_hh1[u], ghz = ep0[(U + j) * 8 + n] + a.b_hh1[R + u],
+                                ghn = ep0[(2 * U + j) * 8 + n] + a.b_hh1[2 * R + u];
+                    const size_t o = (size_t)row * R + u;
+                    const float h = gru_cell(gir, giz, gin, ghr, ghz, ghn, a.h1[o]);
+                    const float x = fmaf(a.w_prev[u], p, a.cc[((size_t)i * rows + row) * R + u]) + h;
+                    const __nv_bfloat16 xb = bf(x);
+                    a.h1[o] = h;
+                    a.h1b[(size_t)cur * rows * R + o] = bf(h);
+                    a.x1[o] = x;
+                    a.x1b[o] = xb;
+                    if (dbg) { float* q = dbg + (size_t)row * Ddbg; q[u] = h; q[R + u] = __bfloat162float(xb); }
+                }
+            }
+            __syncwarp();
+        }
+        if (!grid_barrier(a.bar, target, gridDim.x, a.abort_flag, &s_ok, false)) return;
+        // 2. GRU2
+        for (int nt = warp; nt < ntiles; nt += WR_WARPS) {
+            float acc[4];
+            wr_mma(acc, wt + d.off[1], a.x1b, R, nt * 8, rows, lane);
+            wr_spill(ep0, acc, lane);
+            wr_mma(acc, wt + d.off[2], a.h2b + (size_t)prv * rows * R, R, nt * 8, rows, lane);
+            wr_spill(ep1, acc, lane);
+            for (int e = lane; e < U * 8; e += 32) {
+                const int j = e >> 3, n = e & 7, row = nt * 8 + n, u = c * U + j;
+                if (row < rows) {
+                    const float* c2 = a.c2 + ((size_t)i * rows + row) * 3 * R;
+                    const float gir = ep0[j * 8 + n] + c2[u], giz = ep0[(U + j) * 8 + n] + c2[R + u], gin = ep0[(2 * U + j) * 8 + n] + c2[2 * R + u];
+                    const float ghr = ep1[j * 8 + n] + a.b_hh2[u], ghz = ep1[(U + j) * 8 + n] + a.b_hh2[R + u],
+                                ghn = ep1[(2 * U + j) * 8 + n] + a.b_hh2[2 * R + u];
+                    const size_t o = (size_t)row * R + u;
+                    const float h = gru_cell(gir, giz, gin, ghr, ghz, ghn, a.h2[o]);
+                    const __nv_bfloat16 xb = bf(a.x1[o] + h);
+                    a.h2[o] = h;
+                    a.h2b[(size_t)cur * rows * R + o] = bf(h);
+                    a.x2b[o] = xb;
+                    if (dbg) { float* q = dbg + (size_t)row * Ddbg; q[2 * R + u] = h; q[3 * R + u] = __bfloat162float(xb); }
+                }
+            }
+            __syncwarp();
+        }
+        if (!grid_barrier(a.bar, target, gridDim.x, a.abort_flag, &s_ok, false)) return;
+        // 3. / 4. fc1, fc2
+        for (int st = 0; st < 2; ++st) {
+            const __nv_bfloat16* in = st == 0 ? a.x2b : a.y1b;
+            __nv_bfloat16* outb = st == 0 ? a.y1b : a.y2b;
+            const float* P = st == 0 ? a.p1 : a.p2;
+            const int K = st == 0 ? R : Fc;
+            for (int nt = warp; nt < ntiles; nt += WR_WARPS) {
+                float acc[4];
+                wr_mma(acc, wt + d.off[3 + st], in, K, nt * 8, rows, lane);
+                wr_spill(ep0, acc, lane);
+                for (int e = lane; e < V * 8; e += 32) {
+                    const int j = e >> 3, n = e & 7, row = nt * 8 + n, o = c * V + j;
+                    if (row < rows) {
+                        const __nv_bfloat16 yb = bf(fmaxf(ep0[j * 8 + n] + P[((size_t)i * rows + row) * Fc + o], 0.f));
+                        outb[(size_t)row * Fc + o] = yb;
+                        if (dbg) dbg[(size_t)row * Ddbg + 4 * R + st * Fc + o] = __bfloat162float(yb);
+                    }
+                }
+                __syncwarp();
+            }
+            if (!grid_barrier(a.bar, target, gridDim.x, a.abort_flag, &s_ok, false)) return;
+        }
+        // 5. fc3
+        if (c * O < d.n_out) {
+            for (int nt = warp; nt < ntiles; nt += WR_WARPS) {
+                float acc[4];
+                wr_mma(acc, wt + d.off[5], a.y2b, Fc, nt * 8, rows, lane);
+                wr_spill(ep0, acc, lane);
+                for (int e = lane; e < O * 8; e += 32) {
+                    const int j = e >> 3, n = e & 7, row = nt * 8 + n, o = c * O + j;
+                    if (row < rows && o < d.n_out) {
+                        const float l = ep0[j * 8 + n] + a.b_fc3[o];
+                        a.logits[(size_t)row * d.n_out + o] = l;
+                        if (dbg) dbg[(size_t)row * Ddbg + 4 * R + 2 * Fc + o] = l;
+                    }
+                }
+                __syncwarp();
+            }
+        }
+        if (!grid_barrier(a.bar, target, gridDim.x, a.abort_flag, &s_ok, false)) return;
+        // 6. sample, one warp per row
+        for (int row = c * WR_WARPS + warp; row < rows; row += WR_CTAS * WR_WARPS) {
+            const float* lg = a.logits + (size_t)row * d.n_out;
+            float sample;
+            if (a.mode == B200TTS_WAVERNN_RAW) {
+                const int n = d.n_out, per = (n + 31) / 32, k0 = lane * per, k1 = min(n, k0 + per);
+                const float u = a.uni[(size_t)row * a.L + tg];
+                float mx = -INFINITY;
+                for (int k = k0; k < k1; ++k) mx = fmaxf(mx, __ldcg(lg + k));
+                mx = warp_max(mx);
+                float part = 0.f;
+                for (int k = k0; k < k1; ++k) part += expf(__ldcg(lg + k) - mx);
+                float incl = part;                                // inclusive scan over lanes, fixed order
+                for (int o = 1; o < 32; o <<= 1) {
+                    const float v = __shfl_up_sync(0xffffffffu, incl, o);
+                    if (lane >= o) incl += v;
+                }
+                const float total = __shfl_sync(0xffffffffu, incl, 31);
+                const float thr = u * total;
+                const unsigned hit = __ballot_sync(0xffffffffu, incl > thr && k1 > k0);
+                int k = n - 1;                                    // rounding put u S at or beyond the last partial sum: the last class
+                if (hit) {
+                    const int src = __ffs(hit) - 1;
+                    int kk = k1 - 1;
+                    if (lane == src) {
+                        float cum = incl - part;
+                        for (int q = k0; q < k1; ++q) {
+                            cum += expf(__ldcg(lg + q) - mx);
+                            if (cum > thr) { kk = q; break; }
+                        }
+                    }
+                    k = __shfl_sync(0xffffffffu, kk, src);
+                }
+                sample = 2.f * (float)k / (float)(n - 1) - 1.f;
+            } else {
+                const int nr = d.n_out / 3, U1 = nr + 1;
+                const float* uu = a.uni + ((size_t)row * a.L + tg) * U1;
+                // bi starts as a valid component on every lane and only ever takes another lane's bi: it stays in [0, nr) even when
+                // NaN scores make every comparison false, so the loads below stay inside the row's logits
+                float best = -INFINITY;
+                int bi = 0;
+                if (lane < nr) {
+                    const float u = fmaf(1.f - 2e-5f, uu[lane], 1e-5f);
+                    best = __ldcg(lg + lane) - logf(-logf(u));
+                    bi = lane;
+                }
+                for (int o = 16; o > 0; o >>= 1) {             // argmax, the lowest index among equal values
+                    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+                    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+                    if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+                }
+                const float mean = __ldcg(lg + nr + bi);
+                const float ls = fmaxf(__ldcg(lg + 2 * nr + bi), -32.23619130191664f);   // log(1e-14)
+                const float u = fmaf(1.f - 2e-5f, uu[nr], 1e-5f);
+                sample = fminf(fmaxf(mean + expf(ls) * (logf(u) - logf(1.f - u)), -1.f), 1.f);
+            }
+            if (lane == 0) {
+                a.prev[row] = sample;
+                a.out[(size_t)row * a.L + tg] = sample;
+            }
+        }
+        if (!grid_barrier(a.bar, target, gridDim.x, a.abort_flag, &s_ok, false)) return;
+    }
+}
+
+// element k of numpy.linspace(-1, 1, n): k * step + start, the last one exactly 1
+__device__ __forceinline__ double linspace_pm1(long long k, int n) {
+    if (n == 1) return -1.0;
+    return k == n - 1 ? 1.0 : (double)k * (2.0 / (n - 1)) + -1.0;
+}
+
+// wave of utterance b (packed at wave_off[b], (F_b - 1) hop samples): sample i sums, over the folds f of the utterance in ascending order,
+// fade(j) y[f, j] with j = i - f (target + overlap) in [0, L); mu-law decoded first (RAW); times the final linear fade-out.  fp64, then fp32.
+__global__ void wavernn_unfold_kernel(int B, int hop, int target, int overlap, int mu, const int* __restrict__ frames,
+                                      const int* __restrict__ row_off, const long long* __restrict__ wave_off, const float* __restrict__ y,
+                                      float* __restrict__ wave, long long total) {
+    const int L = target + 2 * overlap, sil = overlap / 2, fl = overlap - sil, fo = 20 * hop;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
+        int lo = 0, hi = B - 1;
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (wave_off[mid] <= idx) lo = mid; else hi = mid - 1;
+        }
+        const int b = lo;
+        const long long i = idx - wave_off[b];
+        const long long len = (long long)(frames[b] - 1) * hop;
+        const int r0 = row_off[b], nf = row_off[b + 1] - r0;
+        double acc = 0.0;
+        for (int f = 0; f < nf; ++f) {
+            const long long j = i - (long long)f * (target + overlap);
+            if (j < 0 || j >= L) continue;
+            double v = y[(size_t)(r0 + f) * L + j];
+            if (mu > 0) v = (v > 0 ? 1.0 : (v < 0 ? -1.0 : 0.0)) / mu * (pow(1.0 + mu, fabs(v)) - 1.0);
+            double w = 1.0;
+            if (j < overlap) w = j < sil ? 0.0 : sqrt(0.5 * (1.0 + linspace_pm1(j - sil, fl)));
+            else if (j >= L - overlap) {
+                const long long k = j - (L - overlap);
+                w = k >= fl ? 0.0 : sqrt(0.5 * (1.0 - linspace_pm1(k, fl)));
+            }
+            acc += v * w;
+        }
+        const long long k = i - (len - fo);
+        if (k >= 0) acc *= (k == fo - 1) ? 0.0 : 1.0 + k * (-1.0 / (fo - 1));
+        wave[idx] = (float)acc;
+    }
+}
+
+// in place: y = mu-law decode of y (fp64, then fp32), ahead of the de-emphasis scan
+__global__ void wavernn_mulaw_kernel(long long n, int mu, float* __restrict__ y) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const double v = y[i];
+        y[i] = (float)((v > 0 ? 1.0 : (v < 0 ? -1.0 : 0.0)) / mu * (pow(1.0 + mu, fabs(v)) - 1.0));
+    }
+}
+
+}  // namespace
+
+int deemphasis_rows_impl(int rows, int len, float a, float* y, cudaStream_t st);    // vocoder.cu
+
+int wavernn_deemphasis_check(int rows, int len, int mu, float a) {
+    B200_REQUIRE(rows >= 1 && len >= 1 && mu >= 0 && (long long)rows * len < (1ll << 40), "wavernn_deemphasis: bad arguments (rows = %d, "
+                 "len = %d, mu = %d)", rows, len, mu);
+    B200_REQUIRE(a == a && a > -1.f && a < 1.f, "wavernn_deemphasis: the coefficient must lie in (-1, 1)");
+    return B200TTS_OK;
+}
+
+int wavernn_deemphasis_impl(int rows, int len, int mu, float a, float* y, cudaStream_t st) {
+    B200_TRY(wavernn_deemphasis_check(rows, len, mu, a));
+    KernelTimer kt("wavernn_deemphasis", st);
+    if (mu > 0) {
+        wavernn_mulaw_kernel<<<grid_for((size_t)rows * len), 256, 0, st>>>((long long)rows * len, mu, y);
+        B200_LAUNCH_CHECK();
+    }
+    return deemphasis_rows_impl(rows, len, a, y, st);
+}
+
+// ---------------------------------------------------------------------------------------------
+// host side
+// ---------------------------------------------------------------------------------------------
+static int wavernn_validate(const b200tts_wavernn_shape& s) {
+    B200_REQUIRE(s.rows >= 1, "wavernn: need at least one fold row (rows = %d)", s.rows);
+    B200_REQUIRE(s.rnn_dims >= WR_CTAS && s.rnn_dims % WR_CTAS == 0 && s.rnn_dims <= 5 * WR_CTAS,
+                 "wavernn: rnn_dims %d must be a multiple of %d, at most %d", s.rnn_dims, WR_CTAS, 5 * WR_CTAS);
+    B200_REQUIRE(s.fc_dims >= WR_CTAS && s.fc_dims % WR_CTAS == 0 && s.fc_dims <= 16 * WR_CTAS,
+                 "wavernn: fc_dims %d must be a multiple of %d, at most %d", s.fc_dims, WR_CTAS, 16 * WR_CTAS);
+    if (s.mode == B200TTS_WAVERNN_RAW) {
+        B200_REQUIRE(s.n_out >= 2 && s.n_out <= 16 * WR_CTAS, "wavernn: RAW needs 2 to %d classes (n_out = %d)", 16 * WR_CTAS, s.n_out);
+    } else {
+        B200_REQUIRE(s.mode == B200TTS_WAVERNN_MOL, "wavernn: unknown mode %d", s.mode);
+        B200_REQUIRE(s.n_out % 3 == 0 && s.n_out >= 3 && s.n_out <= 96, "wavernn: MOL needs 3 x (1..32) outputs (n_out = %d)", s.n_out);
+    }
+    B200_REQUIRE(s.fold_len >= 1, "wavernn: fold length %d must be positive", s.fold_len);
+    B200_REQUIRE((long long)s.rows * s.fold_len * (s.n_out / 3 + 1) < (1ll << 40), "wavernn: batch too large");
+    return B200TTS_OK;
+}
+
+// workspace: packed weights, fp32 state and scratch, bf16 activation rows, barrier; each region 256-byte aligned
+struct WrLayout { size_t packed, h1, h2, x1, prev, logits, h1b, h2b, x1b, x2b, y1b, y2b, bar, bytes; };
+static WrLayout wr_layout(const b200tts_wavernn_shape& s) {
+    const WrDims d = wr_dims(s.rnn_dims, s.fc_dims, s.n_out);
+    const size_t rows = s.rows, R = s.rnn_dims, Fc = s.fc_dims;
+    WrLayout l;
+    size_t off = 0;
+    auto take = [&](size_t n) { const size_t o = off; off = align_up_sz(off + n, 256); return o; };
+    l.packed = take((size_t)WR_CTAS * d.per_cta * 16);
+    l.h1 = take(rows * R * 4);
+    l.h2 = take(rows * R * 4);
+    l.x1 = take(rows * R * 4);
+    l.prev = take(rows * 4);
+    l.logits = take(rows * s.n_out * 4);
+    l.h1b = take(2 * rows * R * 2);
+    l.h2b = take(2 * rows * R * 2);
+    l.x1b = take(rows * R * 2);
+    l.x2b = take(rows * R * 2);
+    l.y1b = take(rows * Fc * 2);
+    l.y2b = take(rows * Fc * 2);
+    l.bar = take(256);            // counter, then the abort flag at +128
+    l.bytes = off;
+    return l;
+}
+
+size_t wavernn_workspace_bytes(const b200tts_wavernn_shape& s) {
+    if (wavernn_validate(s) != B200TTS_OK) return 0;
+    return wr_layout(s).bytes;
+}
+
+int wavernn_check(const b200tts_wavernn_shape& s, void* ws, size_t ws_bytes) {
+    B200_TRY(wavernn_validate(s));
+    const WrLayout l = wr_layout(s);
+    B200_REQUIRE(ws && ws_bytes >= l.bytes, "wavernn: workspace of %zu bytes is smaller than the %zu required", ws_bytes, l.bytes);
+    B200_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "wavernn: workspace must be 256-byte aligned");
+    return B200TTS_OK;
+}
+
+int wavernn_prepare_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, void* ws, size_t ws_bytes, cudaStream_t st) {
+    B200_TRY(wavernn_check(s, ws, ws_bytes));
+    B200_REQUIRE(p.w_hh1 && p.w_ih2x && p.w_hh2 && p.w_fc1x && p.w_fc2x && p.w_fc3, "wavernn_prepare: null weight");
+    const WrLayout l = wr_layout(s);
+    const WrDims d = wr_dims(s.rnn_dims, s.fc_dims, s.n_out);
+    unsigned char* base = static_cast<unsigned char*>(ws);
+    B200_CUDA(cudaMemsetAsync(base + l.h1, 0, l.bytes - l.h1, st));    // zero state, zero previous sample, barrier and abort flag
+    WrWeights W{{p.w_hh1, p.w_ih2x, p.w_hh2, p.w_fc1x, p.w_fc2x, p.w_fc3}};
+    wavernn_pack_kernel<<<grid_for((size_t)WR_CTAS * d.per_cta), 256, 0, st>>>(d, W, reinterpret_cast<uint4*>(base + l.packed));
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+int wavernn_run_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, const b200tts_wavernn_cond& cond, int t0, int nsteps,
+                     const float* uniforms, float* out, float* dbg, void* ws, size_t ws_bytes, cudaStream_t st) {
+    B200_TRY(wavernn_check(s, ws, ws_bytes));
+    B200_REQUIRE(p.b_hh1 && p.u1 && p.w_prev && p.b_hh2 && p.b_fc3, "wavernn_run: null parameter");
+    B200_REQUIRE(cond.c && cond.g1 && cond.c2 && cond.p1 && cond.p2, "wavernn_run: null conditioning");
+    B200_REQUIRE(uniforms && out, "wavernn_run: null uniforms or output");
+    B200_REQUIRE(t0 >= 0 && nsteps >= 1 && t0 + nsteps <= s.fold_len, "wavernn_run: steps [%d, %d) outside the fold length %d", t0, t0 + nsteps,
+                 s.fold_len);
+    const WrLayout l = wr_layout(s);
+    unsigned char* base = static_cast<unsigned char*>(ws);
+    WrLoopArgs a;
+    a.d = wr_dims(s.rnn_dims, s.fc_dims, s.n_out);
+    a.rows = s.rows; a.mode = s.mode; a.L = s.fold_len; a.t0 = t0; a.nsteps = nsteps;
+    a.packed = reinterpret_cast<const uint4*>(base + l.packed);
+    a.b_hh1 = p.b_hh1; a.u1 = p.u1; a.w_prev = p.w_prev; a.b_hh2 = p.b_hh2; a.b_fc3 = p.b_fc3;
+    a.cc = cond.c; a.g1 = cond.g1; a.c2 = cond.c2; a.p1 = cond.p1; a.p2 = cond.p2;
+    a.uni = uniforms; a.out = out; a.dbg = dbg;
+    a.h1 = reinterpret_cast<float*>(base + l.h1);
+    a.h2 = reinterpret_cast<float*>(base + l.h2);
+    a.x1 = reinterpret_cast<float*>(base + l.x1);
+    a.prev = reinterpret_cast<float*>(base + l.prev);
+    a.logits = reinterpret_cast<float*>(base + l.logits);
+    a.h1b = reinterpret_cast<__nv_bfloat16*>(base + l.h1b);
+    a.h2b = reinterpret_cast<__nv_bfloat16*>(base + l.h2b);
+    a.x1b = reinterpret_cast<__nv_bfloat16*>(base + l.x1b);
+    a.x2b = reinterpret_cast<__nv_bfloat16*>(base + l.x2b);
+    a.y1b = reinterpret_cast<__nv_bfloat16*>(base + l.y1b);
+    a.y2b = reinterpret_cast<__nv_bfloat16*>(base + l.y2b);
+    a.bar = reinterpret_cast<unsigned*>(base + l.bar);
+    a.abort_flag = reinterpret_cast<int*>(base + l.bar + 128);
+    B200_CUDA(cudaMemsetAsync(a.bar, 0, sizeof(unsigned), st));       // the abort flag persists until the next prepare
+    void* params[] = {&a};
+    return launch_persistent("wavernn_loop", (const void*)wavernn_loop_kernel, WR_CTAS, WR_THREADS, (size_t)a.d.per_cta * 16, false, params, st);
+}
+
+int wavernn_aborted_impl(const b200tts_wavernn_shape& s, const void* ws, size_t ws_bytes, int* aborted, cudaStream_t st) {
+    B200_TRY(wavernn_check(s, const_cast<void*>(ws), ws_bytes));
+    const WrLayout l = wr_layout(s);
+    B200_CUDA(cudaMemcpyAsync(aborted, static_cast<const unsigned char*>(ws) + l.bar + 128, sizeof(int), cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    return B200TTS_OK;
+}
+
+int wavernn_upsample_layer_check(int C, int len, int scale) {
+    B200_REQUIRE(C >= 1 && len >= 1 && scale >= 1 && (long long)C * len * scale < (1ll << 40) && (long long)len * scale < (1ll << 31),
+                 "wavernn_upsample_layer: bad dimensions (C = %d, len = %d, scale = %d)", C, len, scale);
+    return B200TTS_OK;
+}
+
+int wavernn_upsample_layer_impl(int C, int len, int scale, const float* fir, const float* in, float* out, cudaStream_t st) {
+    B200_TRY(wavernn_upsample_layer_check(C, len, scale));
+    KernelTimer kt("wavernn_upsample", st);
+    wavernn_upsample_layer_kernel<<<grid_for((size_t)C * len * scale), 256, 0, st>>>(C, len, scale, fir, in, out);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+int wavernn_fold_check(const b200tts_wavernn_fold_shape& s, int t0, int nsteps) {
+    B200_REQUIRE(s.B >= 1 && s.rows >= s.B && s.n_mels >= 1 && s.aux_dims >= 0 && s.max_frames >= 1,
+                 "wavernn_fold: bad dimensions (B = %d, rows = %d, n_mels = %d, aux_dims = %d, max_frames = %d)", s.B, s.rows, s.n_mels,
+                 s.aux_dims, s.max_frames);
+    B200_REQUIRE(s.hop >= 1 && s.scale >= 1 && s.hop % s.scale == 0 && s.pad >= 0,
+                 "wavernn_fold: the hop %d must be a multiple of the last upsampling factor %d (pad %d)", s.hop, s.scale, s.pad);
+    B200_REQUIRE(s.target >= 1 && s.overlap >= 0, "wavernn_fold: bad target %d / overlap %d", s.target, s.overlap);
+    B200_REQUIRE(t0 >= 0 && nsteps >= 1 && t0 + nsteps <= s.target + 2 * s.overlap, "wavernn_fold: steps [%d, %d) outside the fold length %d",
+                 t0, t0 + nsteps, s.target + 2 * s.overlap);
+    return B200TTS_OK;
+}
+
+int wavernn_fold_impl(const b200tts_wavernn_fold_shape& s, const float* mel_up, const long long* mel_off, const int* frames, const int* row_utt,
+                      const int* row_fold, const float* fir, const float* aux, int t0, int nsteps, float* feat, cudaStream_t st) {
+    B200_TRY(wavernn_fold_check(s, t0, nsteps));
+    KernelTimer kt("wavernn_fold", st);
+    wavernn_fold_kernel<<<grid_for((size_t)nsteps * s.rows * (s.n_mels + s.aux_dims)), 256, 0, st>>>(s, mel_up, mel_off, frames, row_utt, row_fold,
+                                                                                                    fir, aux, t0, nsteps, feat);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+int wavernn_unfold_check(int B, int hop, int target, int overlap, int mu) {
+    B200_REQUIRE(B >= 1 && hop >= 1 && target >= 1 && overlap >= 0 && mu >= 0, "wavernn_unfold: bad arguments (B = %d, hop = %d, target = %d, "
+                 "overlap = %d, mu = %d)", B, hop, target, overlap, mu);
+    return B200TTS_OK;
+}
+
+int wavernn_unfold_impl(int B, int hop, int target, int overlap, int mu, const int* frames, const int* row_off, const long long* wave_off,
+                        long long total, const float* y, float* wave, cudaStream_t st) {
+    B200_TRY(wavernn_unfold_check(B, hop, target, overlap, mu));
+    if (total <= 0) return B200TTS_OK;
+    KernelTimer kt("wavernn_unfold", st);
+    wavernn_unfold_kernel<<<grid_for((size_t)total), 256, 0, st>>>(B, hop, target, overlap, mu, frames, row_off, wave_off, y, wave, total);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+}  // namespace b200tts

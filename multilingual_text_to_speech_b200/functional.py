@@ -856,3 +856,76 @@ def mel_cepstral_distortion(cep_a, off_a, cep_b, off_b, mode):
     check(_lib.load().b200tts_mel_cepstral_distortion(B, cep_a.shape[1], _lib.MCD_MODES[mode], ptr(cep_a), ptr(off_a), ptr(cep_b), ptr(off_b),
                                                       ptr(mcd), ptr(plen), _stream()), 'b200tts_mel_cepstral_distortion')
     return mcd, plen
+
+
+# ------------------------------------------------------------------------------------------------
+# WaveRNN vocoder (fold rows: see include/b200tts.h)
+# ------------------------------------------------------------------------------------------------
+def wavernn_upsample_layer(x, fir, scale):
+    """x [C, len] -> [C, len * scale]: nearest stretch x scale, then the FIR fir [2 scale + 1] with zero padding scale."""
+    _require_cuda(x, fir)
+    x, fir = _f32c(x), _f32c(fir)
+    out = torch.empty(x.shape[0], x.shape[1] * scale, device=x.device, dtype=torch.float32)
+    check(_lib.load().b200tts_wavernn_upsample_layer(x.shape[0], x.shape[1], int(scale), ptr(fir), ptr(x), ptr(out), _stream()),
+          'b200tts_wavernn_upsample_layer')
+    return out
+
+
+def wavernn_fold(shape, mel_up, mel_off, frames, row_utt, row_fold, fir, aux, t0, nsteps, out=None):
+    """feat [nsteps, rows, n_mels + aux_dims] of the loop steps [t0, t0 + nsteps) (shape: a _lib.WaveRNNFoldShape)."""
+    _require_cuda(mel_up, mel_off, frames, row_utt, row_fold, fir, aux)
+    if out is None:
+        out = torch.empty(nsteps, shape.rows, shape.n_mels + shape.aux_dims, device=mel_up.device, dtype=torch.float32)
+    check(_lib.load().b200tts_wavernn_fold(ctypes.byref(shape), ptr(mel_up), ptr(mel_off), ptr(frames), ptr(row_utt), ptr(row_fold), ptr(fir),
+                                           ptr(aux), int(t0), int(nsteps), ptr(out), _stream()), 'b200tts_wavernn_fold')
+    return out
+
+
+def wavernn_workspace(shape, device):
+    """Workspace of the sample loop for `shape` (a _lib.WaveRNNShape); raises on an invalid shape."""
+    n = _lib.load().b200tts_wavernn_workspace_bytes(ctypes.byref(shape))
+    if n == 0:
+        raise _lib.B200TTSError(f'b200tts_wavernn_workspace_bytes: {_lib.load().b200tts_last_error().decode()}')
+    buf = torch.empty(n + 256, dtype=torch.uint8, device=device)
+    off = (-buf.data_ptr()) % 256
+    return buf[off:off + n]
+
+
+def wavernn_params(weights):
+    """_lib.WaveRNNParams from a dict of fp32 contiguous CUDA tensors named as its fields (the caller keeps them alive)."""
+    return _lib.WaveRNNParams(*[ptr(weights[n]) for n in _lib.WAVERNN_PARAM_FIELDS])
+
+
+def wavernn_prepare(shape, params, ws):
+    check(_lib.load().b200tts_wavernn_prepare(ctypes.byref(shape), ctypes.byref(params), ptr(ws), ws.numel(), _stream()),
+          'b200tts_wavernn_prepare')
+
+
+def wavernn_run(shape, params, cond, t0, nsteps, uniforms, out, ws, dbg=None):
+    """Loop steps [t0, t0 + nsteps); cond: (c, g1, c2, p1, p2) [nsteps, rows, width] fp32 CUDA tensors."""
+    cs = _lib.WaveRNNCond(*[ptr(t) for t in cond])
+    check(_lib.load().b200tts_wavernn_run(ctypes.byref(shape), ctypes.byref(params), ctypes.byref(cs), int(t0), int(nsteps), ptr(uniforms),
+                                          ptr(out), ptr(dbg), ptr(ws), ws.numel(), _stream()), 'b200tts_wavernn_run')
+
+
+def wavernn_aborted(shape, ws):
+    flag = ctypes.c_int(0)
+    check(_lib.load().b200tts_wavernn_aborted(ctypes.byref(shape), ptr(ws), ws.numel(), ctypes.byref(flag), _stream()), 'b200tts_wavernn_aborted')
+    return flag.value != 0
+
+
+def wavernn_deemphasis(y, mu, a):
+    """In place on the folded samples y [rows, len]: mu-law decode (mu > 0), then lfilter([1], [1, -a]) along each row."""
+    _require_cuda(y)
+    assert y.dtype == torch.float32 and y.is_contiguous() and y.dim() == 2
+    check(_lib.load().b200tts_wavernn_deemphasis(y.shape[0], y.shape[1], int(mu), float(a), ptr(y), _stream()), 'b200tts_wavernn_deemphasis')
+    return y
+
+
+def wavernn_unfold(y, frames, row_off, wave_off, total, hop, target, overlap, mu):
+    """Folded samples y [rows, target + 2 overlap] -> the packed waveform [total] (mu-law decoded when mu > 0)."""
+    _require_cuda(y, frames, row_off, wave_off)
+    wave = torch.empty(max(int(total), 1), device=y.device, dtype=torch.float32)
+    check(_lib.load().b200tts_wavernn_unfold(frames.numel(), int(hop), int(target), int(overlap), int(mu), ptr(frames), ptr(row_off),
+                                             ptr(wave_off), int(total), ptr(_f32c(y)), ptr(wave), _stream()), 'b200tts_wavernn_unfold')
+    return wave[:int(total)]

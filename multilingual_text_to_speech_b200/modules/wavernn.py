@@ -1,0 +1,316 @@
+"""WaveRNN vocoder, the fatchord architecture (github.com/fatchord/WaveRNN, models/fatchord_version.py) as the reference's published samples
+use it: log-mel spectrogram -> waveform on the GPU.
+
+Submodule and parameter names follow fatchord, so its state_dict (or one of a fork with the same architecture) loads with load_state_dict.
+Only batched (folded) generation is provided, without training.  Mels go in as given: any normalisation a generation script applies
+before the vocoder is the caller's business.
+
+Stages of generate_batch (all on the library's kernels):
+  * upsampling network: MelResNet on the convolution-block op (eval-mode batch norm) and the GEMM, the mel path's stretch + FIR layers on
+    b200tts_wavernn_upsample_layer (the last one evaluated inside the fold kernel, with the `indent` cut);
+  * per chunk of loop steps: the folded features (b200tts_wavernn_fold), the products that do not depend on the previous sample on the GEMM,
+    then the persistent sample loop (b200tts_wavernn_run);
+  * b200tts_wavernn_unfold: mu-law decode (RAW), cross-fade, overlap-add, cut to (F - 1) hop samples and the 20-hop fade-out."""
+import numpy as np
+import torch
+from torch import nn
+
+from .. import _lib
+from .. import functional as F
+
+# fp32 bytes of the conditioning products and folded features held at once: bounds the chunk of loop steps
+COND_BYTES = 512 << 20
+LOG_SCALE_MIN = float(np.log(1e-14))
+
+
+class ResBlock(nn.Module):
+    def __init__(self, dims):
+        super().__init__()
+        self.conv1 = nn.Conv1d(dims, dims, kernel_size=1, bias=False)
+        self.conv2 = nn.Conv1d(dims, dims, kernel_size=1, bias=False)
+        self.batch_norm1 = nn.BatchNorm1d(dims)
+        self.batch_norm2 = nn.BatchNorm1d(dims)
+
+
+class MelResNet(nn.Module):
+    def __init__(self, res_blocks, in_dims, compute_dims, res_out_dims, pad):
+        super().__init__()
+        self.conv_in = nn.Conv1d(in_dims, compute_dims, kernel_size=2 * pad + 1, bias=False)
+        self.batch_norm = nn.BatchNorm1d(compute_dims)
+        self.layers = nn.ModuleList([ResBlock(compute_dims) for _ in range(res_blocks)])
+        self.conv_out = nn.Conv1d(compute_dims, res_out_dims, kernel_size=1)
+
+
+class Stretch2d(nn.Module):
+    def __init__(self, x_scale, y_scale):
+        super().__init__()
+        self.x_scale, self.y_scale = x_scale, y_scale
+
+
+class UpsampleNetwork(nn.Module):
+    def __init__(self, feat_dims, upsample_scales, compute_dims, res_blocks, res_out_dims, pad):
+        super().__init__()
+        total_scale = int(np.prod(upsample_scales))
+        self.indent = pad * total_scale
+        self.resnet = MelResNet(res_blocks, feat_dims, compute_dims, res_out_dims, pad)
+        self.resnet_stretch = Stretch2d(total_scale, 1)
+        self.up_layers = nn.ModuleList()
+        for scale in upsample_scales:
+            k = scale * 2 + 1
+            conv = nn.Conv2d(1, 1, kernel_size=(1, k), padding=(0, scale), bias=False)
+            conv.weight.data.fill_(1.0 / k)
+            self.up_layers.append(Stretch2d(scale, 1))
+            self.up_layers.append(conv)
+
+
+def fold_count(total_len, target, overlap):
+    """Folds of fold_with_overlap for a sequence of total_len samples."""
+    n = (total_len - overlap) // (target + overlap)
+    if total_len - (n * (overlap + target) + overlap) != 0:
+        n += 1
+    return n
+
+
+class WaveRNN(nn.Module):
+    def __init__(self, rnn_dims, fc_dims, bits, pad, upsample_factors, feat_dims, compute_dims, res_out_dims, res_blocks, hop_length,
+                 sample_rate, mode='RAW'):
+        super().__init__()
+        if mode not in _lib.WAVERNN_MODES:
+            raise ValueError(f'unknown mode {mode!r}; expected RAW or MOL')
+        if int(np.prod(upsample_factors)) != hop_length:
+            raise ValueError(f'hop_length {hop_length} must equal the product of upsample_factors {tuple(upsample_factors)}')
+        if res_out_dims % 4:
+            raise ValueError(f'res_out_dims {res_out_dims} must be divisible by 4')
+        self.mode = mode
+        self.pad = pad
+        self.n_classes = 2 ** bits if mode == 'RAW' else 30
+        self.rnn_dims, self.fc_dims, self.feat_dims = rnn_dims, fc_dims, feat_dims
+        self.aux_dims = res_out_dims // 4
+        self.hop_length, self.sample_rate = hop_length, sample_rate
+        self.upsample_factors = tuple(int(s) for s in upsample_factors)
+        self.upsample = UpsampleNetwork(feat_dims, upsample_factors, compute_dims, res_blocks, res_out_dims, pad)
+        self.I = nn.Linear(feat_dims + self.aux_dims + 1, rnn_dims)
+        self.rnn1 = nn.GRU(rnn_dims, rnn_dims, batch_first=True)
+        self.rnn2 = nn.GRU(rnn_dims + self.aux_dims, rnn_dims, batch_first=True)
+        self.fc1 = nn.Linear(rnn_dims + self.aux_dims, fc_dims)
+        self.fc2 = nn.Linear(fc_dims + self.aux_dims, fc_dims)
+        self.fc3 = nn.Linear(fc_dims, self.n_classes)
+        self.register_buffer('step', torch.zeros(1, dtype=torch.long))
+        # the loop's shape limits, checked here rather than at the first call
+        shape = _lib.WaveRNNShape(1, rnn_dims, fc_dims, self.n_classes, _lib.WAVERNN_MODES[mode], 1)
+        if _lib.load().b200tts_wavernn_workspace_bytes(shape) == 0:
+            raise ValueError(_lib.load().b200tts_last_error().decode())
+
+    # ---- shapes ----
+    def uniforms_per_step(self):
+        return 1 if self.mode == 'RAW' else self.n_classes // 3 + 1
+
+    def tape_shape(self, frames, target=11000, overlap=550):
+        """Shape of one mel's uniform tape: (folds, target + 2 overlap, uniforms per step)."""
+        return fold_count(frames * self.hop_length, target, overlap), target + 2 * overlap, self.uniforms_per_step()
+
+    # ---- public API ----
+    def generate(self, mel, target=11000, overlap=550, uniforms=None, generator=None, preemphasis=0.0):
+        """One mel [feat_dims, F]: generate_batch([mel])[0]."""
+        return self.generate_batch([mel], target, overlap, None if uniforms is None else [uniforms], generator, preemphasis)[0]
+
+    def generate_batch(self, mels, target=11000, overlap=550, uniforms=None, generator=None, preemphasis=0.0):
+        """Mels [feat_dims, F_i] (F_i >= 21, as given: no normalisation is applied) -> one waveform of (F_i - 1) hop samples per mel, in input
+        order.  `uniforms`: one tape per mel of tape_shape(F_i, target, overlap), values in [0, 1); by default drawn with torch.rand on the
+        device (`generator` optional).  preemphasis (default 0 = off): each fold is de-emphasised, lfilter([1], [1, -preemphasis]), after
+        the mu-law decode and before the cross-fade; nothing is normalised.  Every stage runs in fp32 (the library's precision mode is set to
+        fp32 for the call and restored after it), except the loop's recurrent products (bf16 operands, fp32 accumulation).  The work runs on the device of the first CUDA input, or on the current CUDA device.  numpy in -> numpy
+        out; torch in -> torch out, on that device for CUDA inputs and on the CPU for CPU inputs."""
+        specs, as_numpy = self._check_mels(mels)
+        frames = [int(s.shape[1]) for s in specs]
+        tapes = self._check_uniforms(uniforms, frames, target, overlap)
+        if not -1.0 < float(preemphasis) < 1.0:
+            raise ValueError(f'preemphasis {preemphasis} must lie in (-1, 1)')
+        device = next((s.device for s in specs if s.is_cuda), None)
+        if device is None:
+            device = torch.device('cuda', torch.cuda.current_device()) if torch.cuda.is_available() else torch.device('cuda')
+        precision = _lib.get_precision()
+        try:
+            _lib.set_precision('fp32')
+            with torch.cuda.device(device), torch.no_grad():
+                wave, wave_off = self._generate(specs, frames, tapes, target, overlap, generator, device, preemphasis=float(preemphasis))
+        finally:
+            _lib.set_precision(precision)
+        out = []
+        for i, f in enumerate(frames):
+            w = wave[int(wave_off[i]): int(wave_off[i]) + (f - 1) * self.hop_length]
+            if as_numpy[i]:
+                out.append(w.cpu().numpy())
+            else:
+                out.append(w if mels[i].is_cuda else w.cpu())
+        return out
+
+    # ---- checks ----
+    def _check_mels(self, mels):
+        if not isinstance(mels, (list, tuple)) or len(mels) == 0:
+            raise ValueError('generate_batch expects a non-empty list of [feat_dims, frames] mels')
+        as_numpy = [not isinstance(m, torch.Tensor) for m in mels]
+        specs = []
+        for i, m in enumerate(mels):
+            t = torch.as_tensor(np.asarray(m) if as_numpy[i] else m)
+            if t.dim() != 2 or t.shape[0] != self.feat_dims:
+                raise ValueError(f'mel {i} has shape {tuple(t.shape)}; expected [{self.feat_dims}, frames]')
+            if t.shape[1] < 21:
+                raise ValueError(f'mel {i} has {t.shape[1]} frames; the 20-hop fade-out needs at least 21')
+            if not torch.is_floating_point(t):
+                raise ValueError(f'mel {i} is not floating point')
+            if not bool(torch.isfinite(t).all()):
+                raise ValueError(f'mel {i} has non-finite values')
+            specs.append(t)
+        return specs, as_numpy
+
+    def _check_uniforms(self, uniforms, frames, target, overlap):
+        if target < 1 or overlap < 0:
+            raise ValueError(f'target {target} must be positive and overlap {overlap} non-negative')
+        if uniforms is None:
+            return None
+        if len(uniforms) != len(frames):
+            raise ValueError(f'{len(uniforms)} uniform tapes for {len(frames)} mels')
+        tapes = []
+        for i, u in enumerate(uniforms):
+            u = torch.as_tensor(np.asarray(u) if not isinstance(u, torch.Tensor) else u)
+            want = self.tape_shape(frames[i], target, overlap)
+            if tuple(u.shape) != want:
+                raise ValueError(f'uniform tape {i} has shape {tuple(u.shape)}; expected {want}')
+            if not torch.is_floating_point(u):
+                raise ValueError(f'uniform tape {i} is not floating point')
+            if u.numel() and (bool((u < 0).any()) or bool((u >= 1).any()) or bool(torch.isnan(u).any())):
+                raise ValueError(f'uniform tape {i} has values outside [0, 1)')
+            tapes.append(u)
+        return tapes
+
+    # ---- stages ----
+    def fold_plan(self, frames, target, overlap):
+        """(row_utt, row_fold, row_off) host int32 arrays of the fold rows of utterances with these frame counts."""
+        n = [fold_count(f * self.hop_length, target, overlap) for f in frames]
+        row_utt = np.repeat(np.arange(len(frames)), n).astype(np.int32)
+        row_fold = np.concatenate([np.arange(k) for k in n]).astype(np.int32)
+        row_off = np.concatenate([[0], np.cumsum(n)]).astype(np.int32)
+        return row_utt, row_fold, row_off
+
+    def upsample_batch(self, specs, device):
+        """(mel_up, mel_off, aux): the mel path up to its penultimate layer, packed per utterance as [feat_dims, (F + 2 pad) hop / s_last]
+        at element offset mel_off[b], and the MelResNet output aux [B, max F, res_out_dims]."""
+        frames = [int(s.shape[1]) for s in specs]
+        B, Fm, p = len(specs), max(frames), self.pad
+        rn = self.upsample.resnet
+        d = lambda t: t.detach().to(device=device, dtype=torch.float32).contiguous()
+        x = torch.zeros(B, self.feat_dims, Fm, device=device, dtype=torch.float32)
+        for i, s in enumerate(specs):
+            x[i, :, :frames[i]] = s.to(device=device, dtype=torch.float32)
+        lengths = torch.tensor(frames, device=device, dtype=torch.int32)
+
+        def block(inp, conv, bn, activation):
+            return F.conv_block_masked(inp, lengths, d(conv.weight), d(bn.weight), d(bn.bias), d(bn.running_mean), d(bn.running_var), 1,
+                                       conv.kernel_size[0], 1, activation, False, bn.eps, bn.weight.shape[0])
+        # conv_in has no padding but reads the mel padded by `pad` zero frames: the same as a zero-padded convolution of the mel itself
+        h = block(x, rn.conv_in, rn.batch_norm, 'relu')
+        for layer in rn.layers:
+            y = block(h, layer.conv1, layer.batch_norm1, 'relu')
+            h = h + block(y, layer.conv2, layer.batch_norm2, 'identity')
+        w_out, b_out = d(rn.conv_out.weight.reshape(rn.conv_out.out_channels, -1)), d(rn.conv_out.bias)
+        aux = torch.empty(B, Fm, rn.conv_out.out_channels, device=device, dtype=torch.float32)
+        for i in range(B):
+            F.gemm(h[i], w_out, trans_a=True, trans_b=True, bias=b_out, out=aux[i])
+        ups = []
+        for i, s in enumerate(specs):
+            m = torch.zeros(self.feat_dims, frames[i] + 2 * p, device=device, dtype=torch.float32)
+            m[:, p:p + frames[i]] = s.to(device=device, dtype=torch.float32)
+            for j, scale in enumerate(self.upsample_factors[:-1]):
+                m = F.wavernn_upsample_layer(m, d(self.upsample.up_layers[2 * j + 1].weight.reshape(-1)), scale)
+            ups.append(m.reshape(-1))
+        mel_off = np.concatenate([[0], np.cumsum([u.numel() for u in ups])[:-1]]).astype(np.int64)
+        return torch.cat(ups), mel_off, aux
+
+    def loop_weights(self, device):
+        """fp32 contiguous tensors on `device` of the loop parameters (_lib.WAVERNN_PARAM_FIELDS) and of the conditioning products."""
+        R, Fc, A = self.rnn_dims, self.fc_dims, self.aux_dims
+        f = lambda t: t.detach().to(device=device, dtype=torch.float32).contiguous()
+        w = {
+            'w_hh1': f(self.rnn1.weight_hh_l0), 'b_hh1': f(self.rnn1.bias_hh_l0),
+            'w_prev': f(self.I.weight[:, 0]),
+            'w_ih2x': f(self.rnn2.weight_ih_l0[:, :R]), 'w_hh2': f(self.rnn2.weight_hh_l0), 'b_hh2': f(self.rnn2.bias_hh_l0),
+            'w_fc1x': f(self.fc1.weight[:, :R]), 'w_fc2x': f(self.fc2.weight[:, :Fc]), 'w_fc3': f(self.fc3.weight), 'b_fc3': f(self.fc3.bias),
+            # conditioning
+            'w_I': f(self.I.weight[:, 1:]), 'b_I': f(self.I.bias), 'w_ih1': f(self.rnn1.weight_ih_l0), 'b_ih1': f(self.rnn1.bias_ih_l0),
+            'w_ih2a': f(self.rnn2.weight_ih_l0[:, R:]), 'b_ih2': f(self.rnn2.bias_ih_l0),
+            'w_fc1a': f(self.fc1.weight[:, R:]), 'b_fc1': f(self.fc1.bias), 'w_fc2a': f(self.fc2.weight[:, Fc:]), 'b_fc2': f(self.fc2.bias),
+        }
+        assert w['w_fc1x'].shape[1] == R and w['w_fc2a'].shape[1] == A
+        w['u1'] = F.gemm(w['w_ih1'], w['w_prev'].reshape(-1, 1)).reshape(-1).contiguous()
+        return w
+
+    def conditioning(self, w, feat):
+        """The loop's inputs that do not depend on the previous sample, from feat [S, rows, n_mels + aux_dims]: (c, g1, c2, p1, p2)."""
+        S, rows, D = feat.shape
+        nm, A = self.feat_dims, self.aux_dims
+        X = feat.reshape(S * rows, D)
+        c = F.gemm(X[:, :nm + A], w['w_I'], trans_b=True, bias=w['b_I'])
+        g1 = F.gemm(c, w['w_ih1'], trans_b=True, bias=w['b_ih1'])
+        c2 = F.gemm(X[:, nm + A:nm + 2 * A], w['w_ih2a'], trans_b=True, bias=w['b_ih2'])
+        p1 = F.gemm(X[:, nm + 2 * A:nm + 3 * A], w['w_fc1a'], trans_b=True, bias=w['b_fc1'])
+        p2 = F.gemm(X[:, nm + 3 * A:nm + 4 * A], w['w_fc2a'], trans_b=True, bias=w['b_fc2'])
+        return tuple(t.reshape(S, rows, -1) for t in (c, g1, c2, p1, p2))
+
+    def chunk_steps(self, rows, fold_len):
+        # floats per step and row: the features, c, g1, c2, p1 and p2
+        per_step = rows * 4 * (self.feat_dims + 4 * self.aux_dims + 7 * self.rnn_dims + 2 * self.fc_dims)
+        return int(max(1, min(fold_len, COND_BYTES // per_step)))
+
+    def _generate(self, specs, frames, tapes, target, overlap, generator, device, trace=None, preemphasis=0.0):
+        """(packed waveform, host offsets).  trace (a dict, tests): receives the stage inputs and outputs; trace['dbg'], if given, is the
+        loop's debug buffer [fold_len, rows, 4 R + 2 fc + n_out]."""
+        row_utt, row_fold, row_off = self.fold_plan(frames, target, overlap)
+        rows, L, hop = int(row_off[-1]), target + 2 * overlap, self.hop_length
+        mel_up, mel_off, aux = self.upsample_batch(specs, device)
+        dev = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(device)
+        frames_d, row_utt_d, row_fold_d, row_off_d, mel_off_d = dev(np.asarray(frames, np.int32)), dev(row_utt), dev(row_fold), dev(row_off), \
+            dev(mel_off)
+        fshape = _lib.WaveRNNFoldShape(len(frames), rows, self.feat_dims, 4 * self.aux_dims, hop, self.pad, self.upsample_factors[-1], target,
+                                       overlap, max(frames))
+        fir = self.upsample.up_layers[-1].weight.detach().reshape(-1).float().contiguous().to(device)
+        U = self.uniforms_per_step()
+        if tapes is None:
+            uni = torch.rand(rows, L, U, device=device, dtype=torch.float32, generator=generator)
+        else:
+            uni = torch.cat([t.to(device=device, dtype=torch.float32) for t in tapes]).contiguous()
+        w = self.loop_weights(device)
+        shape = _lib.WaveRNNShape(rows, self.rnn_dims, self.fc_dims, self.n_classes, _lib.WAVERNN_MODES[self.mode], L)
+        ws = F.wavernn_workspace(shape, device)
+        params = F.wavernn_params(w)
+        F.wavernn_prepare(shape, params, ws)
+        y = torch.empty(rows, L, device=device, dtype=torch.float32)
+        S = self.chunk_steps(rows, L)
+        for t0 in range(0, L, S):
+            n = min(S, L - t0)
+            feat = F.wavernn_fold(fshape, mel_up, mel_off_d, frames_d, row_utt_d, row_fold_d, fir, aux, t0, n)
+            cond = self.conditioning(w, feat)
+            dbg = None if trace is None or trace.get('dbg') is None else trace['dbg'][t0:t0 + n]
+            F.wavernn_run(shape, params, cond, t0, n, uni, y, ws, dbg)
+            if trace is not None and t0 == 0:
+                trace.update(feat=feat, cond=cond, chunk=n)
+        if F.wavernn_aborted(shape, ws):
+            raise _lib.B200TTSError('wavernn: the sample loop timed out at a grid barrier')
+        wave, wave_off = self.postprocess(y, frames, target, overlap, preemphasis)
+        if trace is not None:
+            trace.update(folded=y, uniforms=uni, weights=w, row_off=row_off, wave_off=wave_off, mel_up=mel_up, mel_off=mel_off, aux=aux)
+        return wave, wave_off
+
+    def postprocess(self, y, frames, target, overlap, preemphasis=0.0):
+        """The loop's folded samples y [rows, target + 2 overlap] (CUDA) -> (packed waveform, host offsets): mu-law decode (RAW), optional
+        de-emphasis of each fold, cross-fade and overlap-add, cut to (F - 1) hop samples, 20-hop fade-out.  y is not modified."""
+        hop, device = self.hop_length, y.device
+        _, _, row_off = self.fold_plan(frames, target, overlap)
+        dev = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(device)
+        wave_off = np.concatenate([[0], np.cumsum([(f - 1) * hop for f in frames])]).astype(np.int64)
+        mu = self.n_classes - 1 if self.mode == 'RAW' else 0
+        if preemphasis:
+            y = F.wavernn_deemphasis(y.clone(), mu, preemphasis)          # decodes the mu-law first
+            mu = 0
+        wave = F.wavernn_unfold(y, dev(np.asarray(frames, np.int32)), dev(row_off), dev(wave_off), int(wave_off[-1]), hop, target, overlap, mu)
+        return wave, wave_off
