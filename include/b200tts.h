@@ -574,6 +574,53 @@ int b200tts_wavernn_deemphasis(int rows, int len, int mu, float a, float* y, voi
 int b200tts_wavernn_unfold(int B, int hop, int target, int overlap, int mu, const int32_t* frames, const int32_t* row_off, const int64_t* wave_off,
                            long long total, const float* y, float* wave, void* stream);
 
+/* ---- WaveRNN training: the teacher-forced forward, the loss and the backward ----
+ * The MelResNet, the input products of the GRUs, the fully connected layers and every weight gradient run on the convolution-block and
+ * GEMM entry points (they follow the precision mode); these entry points add the GRU sequence loops (fp32 in both precision modes), the
+ * adjoints of the upsampling layers and of the aux stretch, and the losses.  All fp32, row-major, on the device, stream-ordered. */
+typedef struct {
+    int B;                /* utterances: 1 to 64 */
+    int T;                /* steps: 1 to 4400 (16 hops of 275 samples) */
+    int R;                /* hidden size: a multiple of 128, at most 640 */
+} b200tts_gru_seq_shape;
+/* Host only: bytes of the forward's saved state ([B, T, 4R]: r, z, n, W_hn h + b_hn of every step) and of the loops' workspace (grid
+ * barrier, abort flag, the reverse loop's carry); 0 for an invalid shape (message set).  The workspace must be 256-byte aligned and zeroed by
+ * the caller before its first loop; after that, loops of one shape (both GRUs of a model, forward and reverse) may share it in stream
+ * order, and its abort flag collects a timeout of any of them. */
+size_t b200tts_gru_seq_saved_bytes(const b200tts_gru_seq_shape* shape);
+size_t b200tts_gru_seq_workspace_bytes(const b200tts_gru_seq_shape* shape);
+/* torch.nn.GRU (batch_first, one layer, gate order r, z, n, h0 = 0) given its input products gi = x W_ih^T + b_ih [B, T, 3R]:
+ * r = s(gi_r + W_hr h + b_hr), z = s(gi_z + W_hz h + b_hz), n = tanh(gi_n + r (W_hn h + b_hn)), h' = (1 - z) n + z h.  h [B, T, R]: every
+ * step's output.  One cooperative launch of 128 CTAs (B200TTS_ERR_INVALID when they cannot be co-resident); a grid-barrier timeout
+ * (about 2 s) raises the abort flag and ends the launch: see b200tts_gru_seq_aborted.  The flag is never cleared by the loops. */
+int b200tts_gru_seq_forward(const b200tts_gru_seq_shape* shape, const float* gi, const float* w_hh, const float* b_hh, float* h, void* saved,
+                            void* workspace, size_t workspace_bytes, void* stream);
+/* The reverse of b200tts_gru_seq_forward (same w_hh, h and saved state) for the external gradient dh_ext [B, T, R] of every step's output:
+ * dgi [B, T, 3R] = the gradient of gi = [dr^, dz^, dn^] and dgh [B, T, 3R] = the gradient of W_hh h + b_hh = [dr^, dz^, r dn^] (both
+ * overwritten), from which the caller forms d W_ih, d b_ih, d x, d W_hh = sum_t dgh_t^T h_{t-1} and d b_hh.  dh_dbg (NULL: off) [B, T, R]
+ * receives every step's total dh = dh_ext + z dh_next + W_hh^T dgh_next.  One cooperative launch of 128 CTAs. */
+int b200tts_gru_seq_backward(const b200tts_gru_seq_shape* shape, const float* w_hh, const float* h, const void* saved, const float* dh_ext,
+                             float* dgi, float* dgh, float* dh_dbg, void* workspace, size_t workspace_bytes, void* stream);
+/* Synchronises the stream and sets *aborted to the loops' abort flag (nonzero: a loop on this workspace timed out since it was zeroed). */
+int b200tts_gru_seq_aborted(const b200tts_gru_seq_shape* shape, const void* workspace, size_t workspace_bytes, int* aborted, void* stream);
+/* The adjoint of b200tts_wavernn_upsample_layer (C, len, scale, fir, in as there) for dout [C, len scale]: din [C, len] (overwritten; NULL:
+ * not formed) and dfir [2 scale + 1] += the FIR gradient (NULL: not formed; needs `in` and the workspace, summed in a fixed order). */
+size_t b200tts_wavernn_upsample_layer_backward_workspace_bytes(int C, int len, int scale);
+int b200tts_wavernn_upsample_layer_backward(int C, int len, int scale, const float* fir, const float* in, const float* dout, float* din,
+                                            float* dfir, void* workspace, size_t workspace_bytes, void* stream);
+/* The adjoint of the aux stretch aux_up[b, t, c] = aux[b, t / hop, c]: daux[b, f, c] = sum_{q < hop} dup[b, f hop + q, c] (overwritten).
+ * dup [B, F hop, C], daux [B, F, C]. */
+int b200tts_wavernn_stretch_backward(int B, int F, int C, int hop, const float* dup, float* daux, void* stream);
+/* Mean loss over N rows of logits [N, n_out] into loss[0], and dlogits [N, n_out] = its gradient (both overwritten), summed in a fixed order.
+ * RAW: cross entropy against int32 labels [N] (a label outside [0, n_out) gives NaN).  MOL: fatchord's discretized_mix_logistic_loss
+ * (65536 classes, log scales clamped below at log 1e-14) against fp32 targets [N] in [-1, 1]; n_out = 3 x mixtures. */
+size_t b200tts_wavernn_loss_workspace_bytes(long long N);
+/* out[c] += sum over the rows of x [rows, cols] (fp32, summed in a fixed order of 64 row chunks): the bias gradients of the GRUs. */
+size_t b200tts_column_sum_workspace_bytes(int cols);
+int b200tts_column_sum(long long rows, int cols, const float* x, float* out, void* workspace, size_t workspace_bytes, void* stream);
+int b200tts_wavernn_loss(int mode, long long N, int n_out, const float* logits, const void* target, float* loss, float* dlogits, void* workspace,
+                         size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -109,6 +109,10 @@ class WaveRNNCond(Structure):
     _fields_ = [(n, c_void_p) for n in ('c', 'g1', 'c2', 'p1', 'p2')]
 
 
+class GRUSeqShape(Structure):
+    _fields_ = [(n, c_int) for n in ('B', 'T', 'R')]
+
+
 # include/b200tts.h: B200TTS_WAVERNN_RAW / _MOL
 WAVERNN_MODES = {'RAW': 0, 'MOL': 1}
 
@@ -204,6 +208,18 @@ SIGNATURES = {
     'b200tts_wavernn_aborted': (c_int, [POINTER(WaveRNNShape), c_void_p, c_size_t, POINTER(c_int), c_void_p]),
     'b200tts_wavernn_deemphasis': (c_int, [c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
     'b200tts_wavernn_unfold': (c_int, [c_int] * 5 + [c_void_p] * 3 + [c_longlong, c_void_p, c_void_p, c_void_p]),
+    'b200tts_gru_seq_saved_bytes': (c_size_t, [POINTER(GRUSeqShape)]),
+    'b200tts_gru_seq_workspace_bytes': (c_size_t, [POINTER(GRUSeqShape)]),
+    'b200tts_gru_seq_forward': (c_int, [POINTER(GRUSeqShape)] + [c_void_p] * 6 + [c_size_t, c_void_p]),
+    'b200tts_gru_seq_backward': (c_int, [POINTER(GRUSeqShape)] + [c_void_p] * 8 + [c_size_t, c_void_p]),
+    'b200tts_gru_seq_aborted': (c_int, [POINTER(GRUSeqShape), c_void_p, c_size_t, POINTER(c_int), c_void_p]),
+    'b200tts_wavernn_upsample_layer_backward_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
+    'b200tts_wavernn_upsample_layer_backward': (c_int, [c_int] * 3 + [c_void_p] * 6 + [c_size_t, c_void_p]),
+    'b200tts_wavernn_stretch_backward': (c_int, [c_int] * 4 + [c_void_p] * 3),
+    'b200tts_wavernn_loss_workspace_bytes': (c_size_t, [c_longlong]),
+    'b200tts_column_sum_workspace_bytes': (c_size_t, [c_int]),
+    'b200tts_column_sum': (c_int, [c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    'b200tts_wavernn_loss': (c_int, [c_int, c_longlong, c_int] + [c_void_p] * 5 + [c_size_t, c_void_p]),
 }
 
 _lib = None

@@ -211,6 +211,26 @@ int wavernn_deemphasis_impl(int rows, int len, int mu, float a, float* y, cudaSt
 int wavernn_unfold_check(int B, int hop, int target, int overlap, int mu);
 int wavernn_unfold_impl(int B, int hop, int target, int overlap, int mu, const int* frames, const int* row_off, const long long* wave_off,
                         long long total, const float* y, float* wave, cudaStream_t st);
+size_t gru_seq_saved_bytes(const b200tts_gru_seq_shape& s);
+size_t gru_seq_workspace_bytes(const b200tts_gru_seq_shape& s);
+int gru_seq_check(const b200tts_gru_seq_shape& s, void* ws, size_t ws_bytes);
+int gru_seq_forward_impl(const b200tts_gru_seq_shape& s, const float* gi, const float* w_hh, const float* b_hh, float* h, void* saved, void* ws,
+                         size_t ws_bytes, cudaStream_t st);
+int gru_seq_backward_impl(const b200tts_gru_seq_shape& s, const float* w_hh, const float* h, const void* saved, const float* dh_ext, float* dgi,
+                          float* dgh, float* dh_dbg, void* ws, size_t ws_bytes, cudaStream_t st);
+int gru_seq_aborted_impl(const b200tts_gru_seq_shape& s, const void* ws, size_t ws_bytes, int* aborted, cudaStream_t st);
+size_t wavernn_upsample_layer_backward_workspace_bytes(int C, int len, int scale);
+int wavernn_upsample_layer_backward_impl(int C, int len, int scale, const float* fir, const float* in, const float* dout, float* din, float* dfir,
+                                         void* ws, size_t ws_bytes, cudaStream_t st);
+int wavernn_stretch_backward_check(int B, int F, int C, int hop);
+int wavernn_stretch_backward_impl(int B, int F, int C, int hop, const float* dup, float* daux, cudaStream_t st);
+int wavernn_loss_check(int mode, long long N, int n_out);
+size_t wavernn_loss_workspace_bytes(long long N);
+size_t column_sum_workspace_bytes(int cols);
+int column_sum_check(long long rows, int cols);
+int column_sum_impl(long long rows, int cols, const float* x, float* out, void* ws, size_t ws_bytes, cudaStream_t st);
+int wavernn_loss_impl(int mode, long long N, int n_out, const float* logits, const void* target, float* loss, float* dlogits, void* ws,
+                      size_t ws_bytes, cudaStream_t st);
 }
 using namespace b200tts;
 
@@ -706,6 +726,65 @@ int b200tts_wavernn_unfold(int B, int hop, int target, int overlap, int mu, cons
     B200_TRY(require_device());
     return wavernn_unfold_impl(B, hop, target, overlap, mu, frames, row_off, reinterpret_cast<const long long*>(wave_off), total, y, wave,
                                (cudaStream_t)stream);
+}
+
+size_t b200tts_gru_seq_saved_bytes(const b200tts_gru_seq_shape* shape) {
+    if (!shape) { set_last_error("gru_seq_saved_bytes: null shape"); return 0; }
+    return gru_seq_saved_bytes(*shape);
+}
+size_t b200tts_gru_seq_workspace_bytes(const b200tts_gru_seq_shape* shape) {
+    if (!shape) { set_last_error("gru_seq_workspace_bytes: null shape"); return 0; }
+    return gru_seq_workspace_bytes(*shape);
+}
+int b200tts_gru_seq_forward(const b200tts_gru_seq_shape* shape, const float* gi, const float* w_hh, const float* b_hh, float* h, void* saved,
+                            void* workspace, size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(shape && gi && w_hh && b_hh && h && saved, "gru_seq_forward: null argument");
+    B200_TRY(gru_seq_check(*shape, workspace, workspace_bytes));
+    B200_TRY(require_device());
+    return gru_seq_forward_impl(*shape, gi, w_hh, b_hh, h, saved, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_gru_seq_backward(const b200tts_gru_seq_shape* shape, const float* w_hh, const float* h, const void* saved, const float* dh_ext,
+                             float* dgi, float* dgh, float* dh_dbg, void* workspace, size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(shape && w_hh && h && saved && dh_ext && dgi && dgh, "gru_seq_backward: null argument");
+    B200_TRY(gru_seq_check(*shape, workspace, workspace_bytes));
+    B200_TRY(require_device());
+    return gru_seq_backward_impl(*shape, w_hh, h, saved, dh_ext, dgi, dgh, dh_dbg, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_gru_seq_aborted(const b200tts_gru_seq_shape* shape, const void* workspace, size_t workspace_bytes, int* aborted, void* stream) {
+    B200_REQUIRE(shape && aborted, "gru_seq_aborted: null argument");
+    B200_TRY(require_device());
+    return gru_seq_aborted_impl(*shape, workspace, workspace_bytes, aborted, (cudaStream_t)stream);
+}
+size_t b200tts_wavernn_upsample_layer_backward_workspace_bytes(int C, int len, int scale) {
+    return wavernn_upsample_layer_backward_workspace_bytes(C, len, scale);
+}
+int b200tts_wavernn_upsample_layer_backward(int C, int len, int scale, const float* fir, const float* in, const float* dout, float* din,
+                                            float* dfir, void* workspace, size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(fir && dout && (din || dfir), "wavernn_upsample_layer_backward: null argument");
+    B200_TRY(wavernn_upsample_layer_check(C, len, scale));
+    B200_TRY(require_device());
+    return wavernn_upsample_layer_backward_impl(C, len, scale, fir, in, dout, din, dfir, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_wavernn_stretch_backward(int B, int F, int C, int hop, const float* dup, float* daux, void* stream) {
+    B200_REQUIRE(dup && daux, "wavernn_stretch_backward: null argument");
+    B200_TRY(wavernn_stretch_backward_check(B, F, C, hop));
+    B200_TRY(require_device());
+    return wavernn_stretch_backward_impl(B, F, C, hop, dup, daux, (cudaStream_t)stream);
+}
+size_t b200tts_wavernn_loss_workspace_bytes(long long N) { return wavernn_loss_workspace_bytes(N); }
+size_t b200tts_column_sum_workspace_bytes(int cols) { return column_sum_workspace_bytes(cols); }
+int b200tts_column_sum(long long rows, int cols, const float* x, float* out, void* workspace, size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(x && out, "column_sum: null argument");
+    B200_TRY(column_sum_check(rows, cols));
+    B200_TRY(require_device());
+    return column_sum_impl(rows, cols, x, out, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_wavernn_loss(int mode, long long N, int n_out, const float* logits, const void* target, float* loss, float* dlogits, void* workspace,
+                         size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(logits && target && loss && dlogits, "wavernn_loss: null argument");
+    B200_TRY(wavernn_loss_check(mode, N, n_out));
+    B200_TRY(require_device());
+    return wavernn_loss_impl(mode, N, n_out, logits, target, loss, dlogits, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -929,3 +929,213 @@ def wavernn_unfold(y, frames, row_off, wave_off, total, hop, target, overlap, mu
     check(_lib.load().b200tts_wavernn_unfold(frames.numel(), int(hop), int(target), int(overlap), int(mu), ptr(frames), ptr(row_off),
                                              ptr(wave_off), int(total), ptr(_f32c(y)), ptr(wave), _stream()), 'b200tts_wavernn_unfold')
     return wave[:int(total)]
+
+
+# ------------------------------------------------------------------------------------------------
+# WaveRNN training
+# ------------------------------------------------------------------------------------------------
+def _aligned_bytes(n, device, align=256):
+    buf = torch.empty(int(n) + align, dtype=torch.uint8, device=device)
+    off = (-buf.data_ptr()) % align
+    return buf[off:off + int(n)]
+
+
+def gru_seq_shape(B, T, R):
+    """_lib.GRUSeqShape; raises on a shape the loops do not take."""
+    shape = _lib.GRUSeqShape(int(B), int(T), int(R))
+    if _lib.load().b200tts_gru_seq_workspace_bytes(ctypes.byref(shape)) == 0:
+        raise _lib.B200TTSError(f'b200tts_gru_seq: {_lib.load().b200tts_last_error().decode()}')
+    return shape
+
+
+def gru_seq_aborted(shape, ws):
+    flag = ctypes.c_int(0)
+    check(_lib.load().b200tts_gru_seq_aborted(ctypes.byref(shape), ptr(ws), ws.numel(), ctypes.byref(flag), _stream()), 'b200tts_gru_seq_aborted')
+    return flag.value != 0
+
+
+class GRUSeqGuard:
+    """One zeroed loop workspace for GRU loops of one shape (both GRUs of a training step, forward and reverse, in stream order) and its
+    abort flag, which collects a grid-barrier timeout of any of them.  check() synchronises, reads the flag once and raises if it is set."""
+
+    def __init__(self, shape, device):
+        self.shape = shape
+        self.ws = _aligned_bytes(_lib.load().b200tts_gru_seq_workspace_bytes(ctypes.byref(shape)), device)
+        self.ws.zero_()
+        self.checked = False
+
+    def check(self):
+        self.checked = True
+        if gru_seq_aborted(self.shape, self.ws):
+            raise _lib.B200TTSError('gru_seq: a GRU loop timed out at a grid barrier')
+
+
+def column_sum(x, out):
+    """out += x.sum(0) for x [rows, cols] (fp32, fixed order)."""
+    rows, cols = x.shape
+    ws = _bytes(_lib.load().b200tts_column_sum_workspace_bytes(cols), x.device)
+    check(_lib.load().b200tts_column_sum(rows, cols, ptr(x), ptr(out), ptr(ws), ws.numel(), _stream()), 'b200tts_column_sum')
+    return out
+
+
+class GRUSeqFunction(torch.autograd.Function):
+    """torch.nn.GRU (batch_first, one layer, h0 = 0) on the persistent fp32 sequence loops: x [B, T, in] -> every step's output [B, T, R].
+    gi = x W_ih^T + b_ih runs on the library GEMM before the loop; the backward's weight and input gradients are GEMMs over the loop's
+    dgi / dgh histories, the bias gradients fixed-order column sums.  The loops run on `guard`'s workspace; check_fwd / check_bwd read its
+    abort flag after the forward / reverse loop.  `trace` (a dict or None, tests): receives the input, gi, the outputs, the saved state and,
+    after the backward, dgi, dgh and every step's total dh."""
+
+    @staticmethod
+    def forward(ctx, x, w_ih, w_hh, b_ih, b_hh, trace, guard, check_fwd, check_bwd):
+        _require_cuda(x, w_ih, w_hh, b_ih, b_hh)
+        B, T, In = x.shape
+        R = w_hh.shape[1]
+        shape = guard.shape
+        assert (shape.B, shape.T, shape.R) == (B, T, R), ((shape.B, shape.T, shape.R), (B, T, R))
+        w_ih, w_hh, b_ih, b_hh = _f32c(w_ih), _f32c(w_hh), _f32c(b_ih), _f32c(b_hh)
+        x2 = _f32c(x).reshape(B * T, In)
+        gi = gemm(x2, w_ih, trans_b=True, bias=b_ih)
+        lib = _lib.load()
+        h = torch.empty(B, T, R, device=x.device, dtype=torch.float32)
+        saved = torch.empty(B, T, 4 * R, device=x.device, dtype=torch.float32)
+        with _Timed('gru_seq_fwd'):
+            check(lib.b200tts_gru_seq_forward(ctypes.byref(shape), ptr(gi), ptr(w_hh), ptr(b_hh), ptr(h), ptr(saved), ptr(guard.ws),
+                                              guard.ws.numel(), _stream()), 'b200tts_gru_seq_forward')
+        if check_fwd:
+            guard.check()
+        if trace is not None:
+            trace.update(x=x2, gi=gi.view(B, T, 3 * R), h=h, saved=saved)
+        ctx.guard, ctx.check_bwd, ctx.trace = guard, check_bwd, trace
+        ctx.save_for_backward(x2, w_ih, w_hh, b_ih, b_hh, h, saved)
+        return h
+
+    @staticmethod
+    def backward(ctx, dh):
+        x2, w_ih, w_hh, b_ih, b_hh, h, saved = ctx.saved_tensors
+        guard, trace = ctx.guard, ctx.trace
+        shape = guard.shape
+        B, T, R = shape.B, shape.T, shape.R
+        dh = _f32c(dh)
+        dgi = torch.empty(B, T, 3 * R, device=dh.device, dtype=torch.float32)
+        dgh = torch.empty_like(dgi)
+        dh_dbg = torch.empty(B, T, R, device=dh.device, dtype=torch.float32) if trace is not None else None
+        lib = _lib.load()
+        with _Timed('gru_seq_bwd'):
+            check(lib.b200tts_gru_seq_backward(ctypes.byref(shape), ptr(w_hh), ptr(h), ptr(saved), ptr(dh), ptr(dgi), ptr(dgh), ptr(dh_dbg),
+                                               ptr(guard.ws), guard.ws.numel(), _stream()), 'b200tts_gru_seq_backward')
+        if ctx.check_bwd:
+            guard.check()
+        if trace is not None:
+            trace.update(dgi=dgi, dgh=dgh, dh=dh_dbg, dh_ext=dh)
+        dgi2, dgh2, h2 = dgi.view(B * T, 3 * R), dgh.view(B * T, 3 * R), h.view(B * T, R)
+        (dw_ih, dw_hh, db_ih, db_hh), returned = _grad_targets(ctx.saved_tensors[1:5])
+        sk = 8 if B * T > 4096 else 1
+        gemm(dgi2, x2, True, False, out=dw_ih, beta=1.0, splitk=sk)
+        # d W_hh = sum over b and t >= 1 of dgh[b, t]^T h[b, t - 1]: the flat rows shifted by one pair every dgh row but the first with the
+        # h row before it, which for t = 0 of utterance b >= 1 is h[b - 1, T - 1]; those B - 1 products are taken back out
+        gemm(dgh2[1:], h2[:-1], True, False, out=dw_hh, beta=1.0, splitk=sk)
+        if B > 1:
+            gemm(dgh[1:, 0], h[:-1, T - 1], True, False, out=dw_hh, beta=1.0, alpha=-1.0)
+        column_sum(dgi2, db_ih)
+        column_sum(dgh2, db_hh)
+        dx = gemm(dgi2, w_ih).view(B, T, -1) if ctx.needs_input_grad[0] else None
+        return (dx, *returned, None, None, None, None)
+
+
+def gru_seq(x, w_ih, w_hh, b_ih, b_hh, trace=None, guard=None, check_fwd=None, check_bwd=None):
+    """One GRU on the sequence loops.  Without a guard the call owns a fresh one and reads its abort flag once: after the reverse loop when
+    a backward will run, else after the forward loop."""
+    if guard is None:
+        guard = GRUSeqGuard(gru_seq_shape(x.shape[0], x.shape[1], w_hh.shape[1]), x.device)
+        grads = torch.is_grad_enabled() and any(t.requires_grad for t in (x, w_ih, w_hh, b_ih, b_hh))
+        check_fwd, check_bwd = not grads, grads
+    return GRUSeqFunction.apply(x, w_ih, w_hh, b_ih, b_hh, trace, guard, bool(check_fwd), bool(check_bwd))
+
+
+class WaveRNNUpsampleLayerFunction(torch.autograd.Function):
+    """One upsampling layer pair (nearest stretch x scale, FIR of 2 scale + 1 taps, zero padding scale) of every row of x [C, len] ->
+    [C, len scale]; the backward is the library's adjoint (d fir accumulated into its .grad view when there is one)."""
+
+    @staticmethod
+    def forward(ctx, x, fir, scale):
+        _require_cuda(x, fir)
+        x, f = _f32c(x), _f32c(fir).reshape(-1)
+        out = torch.empty(x.shape[0], x.shape[1] * scale, device=x.device, dtype=torch.float32)
+        check(_lib.load().b200tts_wavernn_upsample_layer(x.shape[0], x.shape[1], int(scale), ptr(f), ptr(x), ptr(out), _stream()),
+              'b200tts_wavernn_upsample_layer')
+        ctx.scale = int(scale)
+        ctx.save_for_backward(x, fir)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        x, fir = ctx.saved_tensors
+        C, L = x.shape
+        lib = _lib.load()
+        dout = _f32c(dout)
+        din = torch.empty_like(x) if ctx.needs_input_grad[0] else None
+        (dfir,), (ret,) = _grad_targets((fir,))
+        ws = _bytes(lib.b200tts_wavernn_upsample_layer_backward_workspace_bytes(C, L, ctx.scale), x.device)
+        check(lib.b200tts_wavernn_upsample_layer_backward(C, L, ctx.scale, ptr(_f32c(fir).reshape(-1)), ptr(x), ptr(dout), ptr(din), ptr(dfir),
+                                                          ptr(ws), ws.numel(), _stream()), 'b200tts_wavernn_upsample_layer_backward')
+        return din, ret, None
+
+
+def wavernn_upsample_layer_train(x, fir, scale):
+    return WaveRNNUpsampleLayerFunction.apply(x, fir, scale)
+
+
+class WaveRNNStretchFunction(torch.autograd.Function):
+    """aux [B, F, C] -> [B, F hop, C], each frame repeated hop times; the backward sums each frame's hop positions on the library."""
+
+    @staticmethod
+    def forward(ctx, aux, hop):
+        _require_cuda(aux)
+        ctx.hop, ctx.dims = int(hop), tuple(aux.shape)
+        return _f32c(aux).repeat_interleave(int(hop), dim=1)
+
+    @staticmethod
+    def backward(ctx, dup):
+        B, Fr, C = ctx.dims
+        dup = _f32c(dup)
+        daux = torch.empty(B, Fr, C, device=dup.device, dtype=torch.float32)
+        check(_lib.load().b200tts_wavernn_stretch_backward(B, Fr, C, ctx.hop, ptr(dup), ptr(daux), _stream()), 'b200tts_wavernn_stretch_backward')
+        return daux, None
+
+
+def wavernn_stretch(aux, hop):
+    return WaveRNNStretchFunction.apply(aux, hop)
+
+
+class WaveRNNLossFunction(torch.autograd.Function):
+    """Mean RAW cross entropy / MOL discretized-logistic loss of logits [N, n_out] (one fused kernel writes the loss and d logits)."""
+
+    @staticmethod
+    def forward(ctx, logits, target, mode):
+        _require_cuda(logits, target)
+        logits = _f32c(logits)
+        N, n = logits.shape
+        lib = _lib.load()
+        if mode == 'RAW':
+            target = target.to(torch.int32).contiguous()
+        else:
+            target = _f32c(target)
+        if target.numel() != N:
+            raise ValueError(f'{target.numel()} targets for {N} rows of logits')
+        loss = torch.empty((), device=logits.device, dtype=torch.float32)
+        dlogits = torch.empty_like(logits)
+        ws = _bytes(lib.b200tts_wavernn_loss_workspace_bytes(N), logits.device)
+        with _Timed('wavernn_loss'):
+            check(lib.b200tts_wavernn_loss(_lib.WAVERNN_MODES[mode], N, n, ptr(logits), ptr(target), ptr(loss), ptr(dlogits), ptr(ws), ws.numel(),
+                                           _stream()), 'b200tts_wavernn_loss')
+        ctx.save_for_backward(dlogits)
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        (dlogits,) = ctx.saved_tensors
+        return dlogits * g, None, None
+
+
+def wavernn_loss_rows(logits, target, mode):
+    return WaveRNNLossFunction.apply(logits, target, mode)

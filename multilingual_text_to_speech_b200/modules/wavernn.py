@@ -2,15 +2,22 @@
 use it: log-mel spectrogram -> waveform on the GPU.
 
 Submodule and parameter names follow fatchord, so its state_dict (or one of a fork with the same architecture) loads with load_state_dict.
-Only batched (folded) generation is provided, without training.  Mels go in as given: any normalisation a generation script applies
-before the vocoder is the caller's business.
+Batched (folded) generation (generate_batch) and teacher-forced training (forward, wavernn_loss, vocoder_batch) are provided.  Mels go
+in as given: any normalisation a generation script applies before the vocoder is the caller's business.
 
 Stages of generate_batch (all on the library's kernels):
   * upsampling network: MelResNet on the convolution-block op (eval-mode batch norm) and the GEMM, the mel path's stretch + FIR layers on
     b200tts_wavernn_upsample_layer (the last one evaluated inside the fold kernel, with the `indent` cut);
   * per chunk of loop steps: the folded features (b200tts_wavernn_fold), the products that do not depend on the previous sample on the GEMM,
     then the persistent sample loop (b200tts_wavernn_run);
-  * b200tts_wavernn_unfold: mu-law decode (RAW), cross-fade, overlap-add, cut to (F - 1) hop samples and the 20-hop fade-out."""
+  * b200tts_wavernn_unfold: mu-law decode (RAW), cross-fade, overlap-add, cut to (F - 1) hop samples and the 20-hop fade-out.
+
+Stages of forward (training, with autograd):
+  * MelResNet on the convolution-block op (train-mode batch norm updates the running statistics like nn.BatchNorm1d): conv_in as its
+    convolution-only stage over the mel window (the 'same'-padded op's middle outputs are the unpadded convolution), then its batch-norm
+    stage; conv_out and every linear layer on the library GEMM; the aux stretch and the mel path's layers with their library adjoints;
+  * both GRUs on the persistent fp32 sequence loops (b200tts_gru_seq_forward / _backward);
+  * wavernn_loss: one fused kernel per mode writes the loss and d logits."""
 import numpy as np
 import torch
 from torch import nn
@@ -21,6 +28,88 @@ from .. import functional as F
 # fp32 bytes of the conditioning products and folded features held at once: bounds the chunk of loop steps
 COND_BYTES = 512 << 20
 LOG_SCALE_MIN = float(np.log(1e-14))
+# training windows the sequence loops take: at most this many hops of samples, at most 64 of them
+MAX_TRAIN_HOPS = 16
+MAX_TRAIN_BATCH = 64
+
+
+# ---- labels and training windows (fatchord's utils/distribution.py, utils/dsp.py and collate_vocoder) ----
+def label_2_float(x, bits):
+    """2 x / (2^bits - 1) - 1, in fp32 like fatchord's torch expression."""
+    return 2 * torch.as_tensor(x).float() / (2 ** bits - 1.) - 1.
+
+
+def float_2_label(x, bits):
+    """trunc(clip((x + 1) (2^bits - 1) / 2, 0, 2^bits - 1)) as int64: fatchord's MOL labels of a waveform in [-1, 1]."""
+    x = np.asarray(x, dtype=np.float64)
+    if x.size and np.abs(x).max() > 1.0:
+        raise ValueError('float_2_label expects samples in [-1, 1]')
+    return np.clip((x + 1.) * (2 ** bits - 1) / 2, 0, 2 ** bits - 1).astype(np.int64)
+
+
+def encode_mu_law(x, mu):
+    """fatchord's encode_mu_law(x, mu = 2^bits): floor((sign(x) log(1 + m|x|) / log(1 + m) + 1) / 2 m + 0.5) with m = mu - 1, int64."""
+    m = mu - 1
+    x = np.asarray(x, dtype=np.float64)
+    fx = np.sign(x) * np.log(1 + m * np.abs(x)) / np.log(1 + m)
+    return np.floor((fx + 1) / 2 * m + 0.5).astype(np.int64)
+
+
+def mel_window(seq_len, hop, pad):
+    """Frames of one training window's mel: seq_len / hop + 2 pad."""
+    if seq_len < hop or seq_len % hop:
+        raise ValueError(f'seq_len {seq_len} must be a positive multiple of the hop {hop}')
+    return seq_len // hop + 2 * pad
+
+
+def draw_offsets(frames, seq_len, hop, pad, rng=None):
+    """One mel offset per utterance of `frames` frames, uniform in [0, F - 2 - (mel_win + 2 pad)) as fatchord's collate_vocoder draws them."""
+    rng = np.random.default_rng() if rng is None else rng
+    win = mel_window(seq_len, hop, pad)
+    hi = [int(f) - 2 - (win + 2 * pad) for f in frames]
+    if min(hi) < 1:
+        raise ValueError(f'an utterance of {min(frames)} frames is too short for a window of {win} frames')
+    return [int(rng.integers(0, h)) for h in hi]
+
+
+def vocoder_batch(mels, labels, offsets, mode, bits, seq_len, pad, hop):
+    """fatchord's collate_vocoder with explicit offsets: host mels [feat, F_i], integer labels [samples_i] and mel offsets o_i ->
+    (x [B, seq_len] fp32, y [B, seq_len] (RAW int64 labels, MOL fp32 in [-1, 1]), m [B, feat, mel_win] fp32) on the CPU.  m = mel[:, o:o +
+    mel_win]; the labels window starts at (o + pad) hop and holds seq_len + 1 labels; x = label_2_float(labels[:seq_len], 16 for MOL, else
+    bits), y = labels[1:] (MOL: label_2_float(y, 16))."""
+    if mode not in _lib.WAVERNN_MODES:
+        raise ValueError(f'unknown mode {mode!r}; expected RAW or MOL')
+    if not (len(mels) == len(labels) == len(offsets)) or len(mels) == 0:
+        raise ValueError(f'{len(mels)} mels, {len(labels)} label sequences and {len(offsets)} offsets: need as many of each, at least one')
+    win = mel_window(seq_len, hop, pad)
+    ms, ls = [], []
+    for i, (mel, lab, o) in enumerate(zip(mels, labels, offsets)):
+        mel, lab, o = np.asarray(mel), np.asarray(lab), int(o)
+        s0 = (o + pad) * hop
+        if o < 0 or o + win > mel.shape[-1] or s0 + seq_len + 1 > lab.shape[0]:
+            raise ValueError(f'offset {o} of item {i} leaves its window outside the mel ({mel.shape[-1]} frames) or the labels '
+                             f'({lab.shape[0]})')
+        ms.append(mel[:, o:o + win])
+        ls.append(lab[s0:s0 + seq_len + 1])
+    m = torch.tensor(np.stack(ms).astype(np.float32))
+    lab = torch.tensor(np.stack(ls).astype(np.int64))
+    b = 16 if mode == 'MOL' else bits
+    x = label_2_float(lab[:, :seq_len], b)
+    y = lab[:, 1:]
+    if mode == 'MOL':
+        y = label_2_float(y, b)
+    return x, y, m
+
+
+def wavernn_loss(logits, y, mode):
+    """fatchord's training loss of forward's logits [B, T, n_classes] against y [B, T]: RAW F.cross_entropy against the labels, MOL
+    discretized_mix_logistic_loss (65536 classes, log scales clamped at log 1e-14); the mean over B T, with autograd."""
+    if mode not in _lib.WAVERNN_MODES:
+        raise ValueError(f'unknown mode {mode!r}; expected RAW or MOL')
+    n = logits.shape[-1]
+    if tuple(y.shape) != tuple(logits.shape[:-1]):
+        raise ValueError(f'targets of shape {tuple(y.shape)} for logits of shape {tuple(logits.shape)}')
+    return F.wavernn_loss_rows(logits.reshape(-1, n), y.reshape(-1).to(logits.device), mode)
 
 
 class ResBlock(nn.Module):
@@ -108,6 +197,79 @@ class WaveRNN(nn.Module):
     def tape_shape(self, frames, target=11000, overlap=550):
         """Shape of one mel's uniform tape: (folds, target + 2 overlap, uniforms per step)."""
         return fold_count(frames * self.hop_length, target, overlap), target + 2 * overlap, self.uniforms_per_step()
+
+    # ---- training ----
+    def forward(self, x, mels, trace=None):
+        """fatchord's teacher-forced WaveRNN.forward: x [B, T] (the previous samples as floats), mels [B, feat_dims, T / hop + 2 pad] ->
+        logits [B, T, n_classes], with autograd; increments the `step` buffer.  T a multiple of the hop, at most 16 hops; B at most 64.
+        Batch norm uses batch statistics (and updates the running ones) in training mode, the running statistics in eval mode.  The GRUs run
+        in fp32; the rest follows the library's precision mode.  A grid-barrier timeout of a GRU loop raises B200TTSError after the backward's
+        last loop, after the forward when no backward can follow, or at the next call when a backward could follow but did not run.
+        trace (a dict or None, tests): receives 'rnn1' / 'rnn2' loop traces and the last hidden layer 'y2'."""
+        dev = self.I.weight.device
+        x, mels = x.to(dev, torch.float32), mels.to(dev, torch.float32)
+        B, T = x.shape
+        hop, p = self.hop_length, self.pad
+        if T < hop or T % hop or T // hop > MAX_TRAIN_HOPS or not 1 <= B <= MAX_TRAIN_BATCH:
+            raise ValueError(f'x of shape {tuple(x.shape)}: need 1 to {MAX_TRAIN_BATCH} windows of a multiple of the hop {hop}, at most '
+                             f'{MAX_TRAIN_HOPS} hops')
+        if tuple(mels.shape) != (B, self.feat_dims, T // hop + 2 * p):
+            raise ValueError(f'mels of shape {tuple(mels.shape)}; expected {(B, self.feat_dims, T // hop + 2 * p)}')
+        pending = getattr(self, '_pending_guard', None)
+        if pending is not None and not pending.checked:
+            pending.check()          # the previous call's loops were never followed by a backward: read their abort flag now
+        self._pending_guard = None
+        self.step += 1
+        mel_up, aux = self.upsample_train(mels)
+        A = self.aux_dims
+        a1, a2, a3, a4 = (aux[:, :, A * i:A * (i + 1)] for i in range(4))
+        tr = (lambda k: trace.setdefault(k, {})) if trace is not None else (lambda k: None)
+        x1 = F.linear(torch.cat([x.unsqueeze(-1), mel_up, a1], dim=2), self.I.weight, self.I.bias)
+        r1, r2 = self.rnn1, self.rnn2
+        # both GRUs share one loop workspace, whose abort flag is read once per call: after GRU1's reverse loop (the last loop of the
+        # backward), or after GRU2's forward loop when no backward follows
+        guard = F.GRUSeqGuard(F.gru_seq_shape(B, T, self.rnn_dims), dev)
+        grads = torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())
+        x2 = x1 + F.gru_seq(x1, r1.weight_ih_l0, r1.weight_hh_l0, r1.bias_ih_l0, r1.bias_hh_l0, tr('rnn1'), guard, False, grads)
+        x3 = x2 + F.gru_seq(torch.cat([x2, a2], dim=2), r2.weight_ih_l0, r2.weight_hh_l0, r2.bias_ih_l0, r2.bias_hh_l0, tr('rnn2'), guard,
+                            not grads, False)
+        if grads:
+            self._pending_guard = guard
+        y1 = torch.relu(F.linear(torch.cat([x3, a3], dim=2), self.fc1.weight, self.fc1.bias))
+        y2 = torch.relu(F.linear(torch.cat([y1, a4], dim=2), self.fc2.weight, self.fc2.bias))
+        if trace is not None:
+            trace['y2'] = y2
+        return F.linear(y2, self.fc3.weight, self.fc3.bias)
+
+    def upsample_train(self, mels):
+        """UpsampleNetwork.forward with autograd: mels [B, feat, W] -> (mel path [B, (W - 2 pad) hop, feat], aux [B, (W - 2 pad) hop, res_out])."""
+        B, _, W = mels.shape
+        p, hop, tr = self.pad, self.hop_length, self.training
+        rn = self.upsample.resnet
+        k = rn.conv_in.kernel_size[0]
+
+        def bn_stage(h, bn, activation, conv=None):
+            if tr:
+                bn.num_batches_tracked += 1
+            if conv is None:
+                return F.conv_block(h, None, bn.weight, bn.bias, bn.running_mean, bn.running_var, None, 1, 1, 1, activation, False, tr, bn.eps,
+                                    bn.momentum, 0.0, bn.weight.shape[0], stage=2)
+            return F.conv_block(h, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, None, 1, conv.kernel_size[0], 1, activation,
+                                False, tr, bn.eps, bn.momentum, 0.0, bn.weight.shape[0])
+        # conv_in is unpadded: the middle W - 2 pad outputs of the 'same'-padded convolution
+        h = F.conv_block(mels, rn.conv_in.weight, None, None, None, None, None, 1, k, 1, 'identity', False, tr, 0.0, 0.0, 0.0, 0, stage=1)
+        h = bn_stage(h[:, :, p:W - p].contiguous(), rn.batch_norm, 'relu')
+        for layer in rn.layers:
+            y = bn_stage(h, layer.batch_norm1, 'relu', layer.conv1)
+            h = h + bn_stage(y, layer.batch_norm2, 'identity', layer.conv2)
+        co = rn.conv_out
+        aux = F.linear(h.transpose(1, 2), co.weight.view(co.out_channels, co.in_channels), co.bias)
+        aux = F.wavernn_stretch(aux, hop)
+        m = mels.reshape(B * self.feat_dims, W)
+        for j, scale in enumerate(self.upsample_factors):
+            m = F.wavernn_upsample_layer_train(m, self.upsample.up_layers[2 * j + 1].weight, scale)
+        m = m[:, p * hop:(W - p) * hop].reshape(B, self.feat_dims, -1).transpose(1, 2)
+        return m, aux
 
     # ---- public API ----
     def generate(self, mel, target=11000, overlap=550, uniforms=None, generator=None, preemphasis=0.0):
