@@ -340,6 +340,23 @@ int b200tts_convblock_backward(const b200tts_convblock_shape* shape, const float
                                const float* gamma, const float* beta, int affine_gstride, const uint8_t* keep,
                                const void* saved, const float* dout, float* dx, float* dweight, float* dgamma,
                                float* dbeta, void* workspace, void* stream);
+/* The same pair for a batch whose channel blocks hold different numbers of utterances (every stage, training and eval):
+ * counts [G] int32 (device).  Rows nb < counts[g] of channel block g are occupied, rows nb >= counts[g] are vacant.
+ * - Batch-norm statistics of block g run over its occupied rows only (n = counts[g] * L); the running statistics of a block
+ *   with counts[g] == 0 are left unchanged, and its gamma / beta (and, through the zero dz, its weights) get exactly 0.
+ * - Vacant rows of out (every stage), of the batch-norm input gradient and of dx are written as exact 0.  Vacant rows of x
+ *   must be finite: the weight-gradient products add 0 * x for them.
+ * - G and NB restate what the counts were derived for and must equal shape->G / shape->NB.  A device-side count outside
+ *   [0, NB] is clamped into it (no row outside the tensor is ever addressed).
+ * With every count == NB the results are bit-identical to b200tts_convblock_forward / b200tts_convblock_backward.      */
+int b200tts_convblock_forward_counts(const b200tts_convblock_shape* shape, const int32_t* counts, int G, int NB, const float* x,
+                                     const float* weight, const float* gamma, const float* beta, int affine_gstride,
+                                     float* running_mean, float* running_var, const uint8_t* keep, float* out, void* saved,
+                                     void* workspace, void* stream);
+int b200tts_convblock_backward_counts(const b200tts_convblock_shape* shape, const int32_t* counts, int G, int NB, const float* x,
+                                      const float* weight, const float* gamma, const float* beta, int affine_gstride,
+                                      const uint8_t* keep, const void* saved, const float* dout, float* dx, float* dweight,
+                                      float* dgamma, float* dbeta, void* workspace, void* stream);
 
 /* ---- one LSTM cell step: ZoneoutLSTMCell.forward / DropoutLSTMCell.forward, modules/layers.py:26-34,44-47 ----
  * gates [B, 4D]: in = x . W_ih^T + b_ih + h . W_hh^T + b_hh (order i, f, g, o), out = the activated gates (saved for the backward);

@@ -167,6 +167,11 @@ SIGNATURES = {
                                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'b200tts_convblock_backward': (c_int, [POINTER(ConvBlockShape), c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'b200tts_convblock_forward_counts': (c_int, [POINTER(ConvBlockShape), c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                 c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'b200tts_convblock_backward_counts': (c_int, [POINTER(ConvBlockShape), c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                  c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                  c_void_p]),
     'b200tts_lstm_cell_forward': (c_int, [c_int, c_int, c_int, c_int, c_float, c_float] + [c_void_p] * 8),
     'b200tts_lstm_cell_backward': (c_int, [c_int, c_int, c_int, c_int, c_float, c_float] + [c_void_p] * 9),
     'b200tts_generator_workspace_bytes': (c_size_t, [c_int, c_int]),

@@ -107,10 +107,12 @@ size_t convblock_saved_floats(const b200tts_convblock_shape& s);
 size_t convblock_workspace_floats(const b200tts_convblock_shape& s);
 int convblock_forward_impl(const b200tts_convblock_shape& s, const float* x, const float* weight, const float* gamma,
                            const float* beta, int affine_gstride, float* running_mean, float* running_var, const uint8_t* keep,
-                           float* out, float* saved, float* ws, cudaStream_t st, const int32_t* lengths = nullptr);
+                           float* out, float* saved, float* ws, cudaStream_t st, const int32_t* lengths = nullptr,
+                           const int32_t* counts = nullptr);
 int convblock_backward_impl(const b200tts_convblock_shape& s, const float* x, const float* weight, const float* gamma,
                             const float* beta, int affine_gstride, const uint8_t* keep, const float* saved, const float* dout,
-                            float* dx, float* dweight, float* dgamma, float* dbeta, float* ws, cudaStream_t st);
+                            float* dx, float* dweight, float* dgamma, float* dbeta, float* ws, cudaStream_t st,
+                            const int32_t* counts = nullptr);
 size_t generator_workspace_floats(int G, int bn);
 int generator_forward_impl(int G, int gd, int bn, long long R, const float* e, const float* Wb, const float* bb, const float* Wk,
                            const float* bk, float* eb, float* out, cudaStream_t st);
@@ -491,6 +493,32 @@ int b200tts_convblock_backward(const b200tts_convblock_shape* shape, const float
     B200_TRY(require_device());
     return convblock_backward_impl(*shape, x, weight, gamma, beta, affine_gstride, keep, (const float*)saved, dout, dx, dweight, dgamma,
                                    dbeta, (float*)workspace, (cudaStream_t)stream);
+}
+
+int b200tts_convblock_forward_counts(const b200tts_convblock_shape* shape, const int32_t* counts, int G, int NB, const float* x,
+                                     const float* weight, const float* gamma, const float* beta, int affine_gstride, float* running_mean,
+                                     float* running_var, const uint8_t* keep, float* out, void* saved, void* workspace, void* stream) {
+    B200_REQUIRE(shape && counts && x && out && saved && workspace, "convblock_forward_counts: null argument");
+    B200_REQUIRE(G == shape->G && NB == shape->NB, "convblock_forward_counts: counts are for G=%d, NB=%d but the shape has G=%d, NB=%d", G, NB,
+                 shape->G, shape->NB);
+    B200_REQUIRE((weight || shape->stage == 2) && ((gamma && beta) || shape->stage == 1), "convblock_forward_counts: null parameter");
+    B200_TRY(require_device());
+    return convblock_forward_impl(*shape, x, weight, gamma, beta, affine_gstride, running_mean, running_var, keep, out, (float*)saved,
+                                  (float*)workspace, (cudaStream_t)stream, nullptr, counts);
+}
+
+int b200tts_convblock_backward_counts(const b200tts_convblock_shape* shape, const int32_t* counts, int G, int NB, const float* x,
+                                      const float* weight, const float* gamma, const float* beta, int affine_gstride, const uint8_t* keep,
+                                      const void* saved, const float* dout, float* dx, float* dweight, float* dgamma, float* dbeta,
+                                      void* workspace, void* stream) {
+    B200_REQUIRE(shape && counts && x && saved && dout && workspace, "convblock_backward_counts: null argument");
+    B200_REQUIRE(G == shape->G && NB == shape->NB, "convblock_backward_counts: counts are for G=%d, NB=%d but the shape has G=%d, NB=%d", G, NB,
+                 shape->G, shape->NB);
+    B200_REQUIRE((weight || shape->stage == 2) && ((gamma && beta) || shape->stage == 1), "convblock_backward_counts: null parameter");
+    B200_REQUIRE(dx || !shape->highway, "convblock_backward_counts: highway blocks need dx");
+    B200_TRY(require_device());
+    return convblock_backward_impl(*shape, x, weight, gamma, beta, affine_gstride, keep, (const float*)saved, dout, dx, dweight, dgamma,
+                                   dbeta, (float*)workspace, (cudaStream_t)stream, counts);
 }
 
 int b200tts_lstm_cell_forward(int B, int D, int cell_kind, int training, float rate_h, float rate_c, float* gates, const float* h_prev,

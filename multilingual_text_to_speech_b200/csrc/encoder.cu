@@ -79,16 +79,31 @@ __device__ __forceinline__ float channel_sum(const float* __restrict__ x, int c,
     return (a0 + a1) + (a2 + a3);
 }
 
+// Rows of channel block g that hold utterances: counts[g] clamped to [0, NB], so that a count out of range never addresses a row
+// outside the tensor (a count above NB reads as NB, a negative one as 0).  Without counts every row is occupied.
+__device__ __forceinline__ int block_rows(const int* __restrict__ counts, int g, int NB) {
+    if (!counts) return NB;
+    const int n = counts[g];
+    return n < 0 ? 0 : (n > NB ? NB : n);
+}
+
 // per-channel batch statistics over (NB, L); x [NB, Ct, L].  One CTA per channel, two passes (mean, then variance).
+// counts (or null): channel block g = c / Cout takes its statistics over its occupied rows q < counts[g] only, summed in the same
+// order as the whole slab; a block with no occupied row writes mean 0 / invstd 0 and leaves its running statistics as they are.
 __global__ void __launch_bounds__(256) bn_stats_kernel(const float* __restrict__ x, float* __restrict__ mean, float* __restrict__ invstd,
                                                        float* __restrict__ running_mean, float* __restrict__ running_var, int NB,
-                                                       int Ct, int L, float eps, float momentum) {
+                                                       int Ct, int L, float eps, float momentum, const int* __restrict__ counts, int Cout) {
     __shared__ float red[64];
     const int c = blockIdx.x;
-    const int n = NB * L;
-    const float s = channel_sum(x, c, NB, Ct, L, [](float v, int, int) { return v; });
+    const int rows = block_rows(counts, c / Cout, NB);
+    if (rows == 0) {
+        if (threadIdx.x == 0) { mean[c] = 0.f; invstd[c] = 0.f; }
+        return;
+    }
+    const int n = rows * L;
+    const float s = channel_sum(x, c, rows, Ct, L, [](float v, int, int) { return v; });
     const float mu = block_sum(s, red) / (float)n;
-    const float v = channel_sum(x, c, NB, Ct, L, [mu](float xv, int, int) { const float d = xv - mu; return d * d; });
+    const float v = channel_sum(x, c, rows, Ct, L, [mu](float xv, int, int) { const float d = xv - mu; return d * d; });
     const float var = block_sum(v, red) / (float)n;
     if (threadIdx.x == 0) {
         mean[c] = mu;
@@ -118,6 +133,7 @@ struct BlockArgs {
     const float* xin;       // [NB, G*Cin, L] block input (highway only)
     int NB, G, Cout, L, act, highway;
     const int* lengths;     // [NB] or null (forward only): outputs at positions l >= lengths[nb] are written as 0
+    const int* counts;      // [G] or null: rows nb >= counts[g] of channel block g are vacant; their outputs and gradients are written as 0
 };
 
 // idx -> (nb, g, c, l) of a [NB, G, Cf, L] tensor; 32-bit arithmetic whenever the tensor has fewer than 2^32 elements
@@ -138,6 +154,7 @@ __global__ void block_fwd_kernel(const BlockArgs p, float* __restrict__ out) {
         int l, c, g; size_t nb;
         split_index(idx, total <= 0xffffffffull, p.L, Cf, p.G, l, c, g, nb);
         if (p.lengths && l >= p.lengths[nb]) { out[idx] = 0.f; continue; }
+        if (p.counts && (int)nb >= block_rows(p.counts, g, p.NB)) { out[idx] = 0.f; continue; }
         auto value = [&](int o) {
             const int ch = g * p.Cout + o;
             const size_t ci = (nb * p.G * p.Cout + ch) * p.L + l;
@@ -188,7 +205,8 @@ __global__ void __launch_bounds__(256) block_fwd_vec4_kernel(const BlockArgs p, 
         };
         const size_t oi = (size_t)row * p.L + 4 * l4;
         // a float4 group may straddle the utterance's length: the lanes at or past it are zeroed one by one
-        const int valid = p.lengths ? p.lengths[nb] - 4 * (int)l4 : 4;
+        int valid = p.lengths ? p.lengths[nb] - 4 * (int)l4 : 4;
+        if (p.counts && (int)nb >= block_rows(p.counts, (int)g, p.NB)) valid = 0;      // vacant row
         if (valid <= 0) { st4(out + oi, make_float4(0.f, 0.f, 0.f, 0.f)); continue; }
         float4 r;
         if (p.highway) {
@@ -216,6 +234,13 @@ __global__ void __launch_bounds__(256) block_bwd_prep_vec4_kernel(const BlockArg
         const unsigned row = idx / (unsigned)L4, l4 = idx - row * (unsigned)L4;
         const unsigned r2 = row / (unsigned)Cf, c = row - r2 * (unsigned)Cf, nb = r2 / (unsigned)p.G, g = r2 - nb * (unsigned)p.G;
         const size_t oi = (size_t)row * p.L + 4 * l4;
+        if (p.counts && (int)nb >= block_rows(p.counts, (int)g, p.NB)) {       // vacant row: no gradient anywhere
+            const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+            const size_t ci = ((size_t)(nb * p.G * p.Cout + g * p.Cout + c)) * p.L + 4 * l4;
+            st4(dz + ci, z);
+            if (p.highway) { st4(dz + ci + (size_t)Cf * p.L, z); st4(dx_skip + oi, z); }
+            continue;
+        }
         const float4 go4 = ld4(dout + oi);
         const float go[4] = {go4.x, go4.y, go4.z, go4.w};
         float zs[2][4], as[2][4], ks[2][4];
@@ -265,15 +290,22 @@ __global__ void __launch_bounds__(256) block_bwd_prep_vec4_kernel(const BlockArg
 __global__ void __launch_bounds__(256) bn_bwd_apply_vec4_kernel(float* __restrict__ dz, const float* __restrict__ conv,
                                                                 const float* __restrict__ mean, const float* __restrict__ invstd,
                                                                 const float* __restrict__ gamma, int affine_gstride, const float* __restrict__ s1,
-                                                                const float* __restrict__ s2, int NB, int G, int Cout, int L, int training) {
+                                                                const float* __restrict__ s2, int NB, int G, int Cout, int L, int training,
+                                                                const int* __restrict__ counts) {
     const int Ct = G * Cout, L4 = L >> 2;
     const unsigned total = (unsigned)NB * Ct * L4;
-    const float inv_n = 1.f / (float)(NB * L);
+    const float inv_n_all = 1.f / (float)(NB * L);
     for (unsigned idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += gridDim.x * blockDim.x) {
         const unsigned row = idx / (unsigned)L4, l4 = idx - row * (unsigned)L4;
         const int ch = (int)(row % (unsigned)Ct);
-        const float is = invstd[ch], gm = gamma[(ch / Cout) * affine_gstride + ch % Cout] * is;
         const size_t i = (size_t)row * L + 4 * l4;
+        float inv_n = inv_n_all;
+        if (counts) {
+            const int rows = block_rows(counts, ch / Cout, NB);
+            if ((int)(row / (unsigned)Ct) >= rows) { st4(dz + i, make_float4(0.f, 0.f, 0.f, 0.f)); continue; }
+            inv_n = 1.f / (float)(rows * L);
+        }
+        const float is = invstd[ch], gm = gamma[(ch / Cout) * affine_gstride + ch % Cout] * is;
         float4 d = ld4(dz + i);
         if (training) {
             const float a = s1[ch] * inv_n, b = is * s2[ch] * inv_n, mu = mean[ch];
@@ -292,6 +324,12 @@ __global__ void block_bwd_prep_kernel(const BlockArgs p, const float* __restrict
     for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
         int l, c, g; size_t nb;
         split_index(idx, total <= 0xffffffffull, p.L, Cf, p.G, l, c, g, nb);
+        if (p.counts && (int)nb >= block_rows(p.counts, g, p.NB)) {      // vacant row: no gradient anywhere
+            const size_t ci = (nb * p.G * p.Cout + g * p.Cout + c) * p.L + l;
+            dz[ci] = 0.f;
+            if (p.highway) { dz[ci + (size_t)Cf * p.L] = 0.f; dx_skip[idx] = 0.f; }
+            continue;
+        }
         float zs[2], as[2], ks[2];
         size_t cis[2];
         const int nch = p.highway ? 2 : 1;
@@ -320,9 +358,11 @@ __global__ void block_bwd_prep_kernel(const BlockArgs p, const float* __restrict
 __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const float* __restrict__ dz, const float* __restrict__ conv,
                                                             const float* __restrict__ mean, const float* __restrict__ invstd,
                                                             float* __restrict__ s1o, float* __restrict__ s2o, float* __restrict__ dgamma,
-                                                            float* __restrict__ dbeta, int affine_gstride, int NB, int G, int Cout, int L) {
+                                                            float* __restrict__ dbeta, int affine_gstride, int NB, int G, int Cout, int L,
+                                                            const int* __restrict__ counts) {
     __shared__ float red[64];
     const int ch = blockIdx.x, Ct = G * Cout;
+    NB = block_rows(counts, ch / Cout, NB);      // the occupied rows of this channel's block (all of them without counts)
     const float mu = mean[ch], is = invstd[ch];
     float s1, s2;
     const bool vec = (L & 3) == 0 && (reinterpret_cast<uintptr_t>(dz) & 15) == 0 && (reinterpret_cast<uintptr_t>(conv) & 15) == 0;
@@ -368,16 +408,33 @@ __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const float* __restr
 // dconv = gamma * invstd * (dz - s1/n - xhat * s2/n)   (training);  gamma * invstd * dz (eval).  In place on dz.
 __global__ void bn_bwd_apply_kernel(float* __restrict__ dz, const float* __restrict__ conv, const float* __restrict__ mean,
                                     const float* __restrict__ invstd, const float* __restrict__ gamma, int affine_gstride,
-                                    const float* __restrict__ s1, const float* __restrict__ s2, int NB, int G, int Cout, int L, int training) {
+                                    const float* __restrict__ s1, const float* __restrict__ s2, int NB, int G, int Cout, int L, int training,
+                                    const int* __restrict__ counts) {
     const int Ct = G * Cout;
     const size_t total = (size_t)NB * Ct * L;
-    const float inv_n = 1.f / (float)(NB * L);
+    const float inv_n_all = 1.f / (float)(NB * L);
     for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
         const int ch = total <= 0xffffffffull ? (int)(((unsigned)idx / (unsigned)L) % (unsigned)Ct) : (int)((idx / L) % Ct);
+        float inv_n = inv_n_all;
+        if (counts) {
+            const int rows = block_rows(counts, ch / Cout, NB);
+            if ((long long)(idx / ((size_t)L * Ct)) >= rows) { dz[idx] = 0.f; continue; }
+            inv_n = 1.f / (float)(rows * L);
+        }
         const float gm = gamma[(ch / Cout) * affine_gstride + ch % Cout] * invstd[ch];
         float d = dz[idx];
         if (training) d = d - s1[ch] * inv_n - (conv[idx] - mean[ch]) * invstd[ch] * s2[ch] * inv_n;
         dz[idx] = gm * d;
+    }
+}
+
+// x [NB, G*C, L]: every vacant row (nb >= counts[g]) of channel block g set to 0.  The convolution-only stage's output and gradient.
+__global__ void zero_vacant_kernel(float* __restrict__ x, const int* __restrict__ counts, int NB, int G, int C, int L) {
+    const size_t total = (size_t)NB * G * C * L;
+    for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
+        const size_t row = idx / L;
+        const int g = (int)((row % ((size_t)G * C)) / C);
+        if ((long long)(row / ((size_t)G * C)) >= block_rows(counts, g, NB)) x[idx] = 0.f;
     }
 }
 
@@ -653,7 +710,7 @@ size_t convblock_workspace_floats(const b200tts_convblock_shape& s) {
 
 int convblock_forward_impl(const b200tts_convblock_shape& s, const float* x, const float* weight, const float* gamma,
                            const float* beta, int affine_gstride, float* running_mean, float* running_var, const uint8_t* keep,
-                           float* out, float* saved, float* ws, cudaStream_t st, const int32_t* lengths) {
+                           float* out, float* saved, float* ws, cudaStream_t st, const int32_t* lengths, const int32_t* counts) {
     B200_TRY(validate_block(s));
     // padded batches: only the fused epilogue of an eval-mode whole block knows the lengths (training statistics would need them too)
     B200_REQUIRE(!lengths || (s.stage == 0 && !s.training), "convblock_forward_masked: lengths need an eval-mode whole block (stage 0)");
@@ -679,16 +736,23 @@ int convblock_forward_impl(const b200tts_convblock_shape& s, const float* x, con
         g.M = s.Cout; g.N = s.L; g.K = s.Cin * s.k; g.batch = s.NB * s.G;
         B200_TRY(gemm_run(g, st));
     }
-    if (s.stage == 1) return B200TTS_OK;
+    if (s.stage == 1) {
+        if (counts) {
+            zero_vacant_kernel<<<grid_for(d.conv_elems), 256, 0, st>>>(out, counts, s.NB, s.G, s.Cout, s.L);
+            B200_LAUNCH_CHECK();
+        }
+        return B200TTS_OK;
+    }
     if (s.training) {
-        bn_stats_kernel<<<(int)d.Ct, 256, 0, st>>>(conv, mean, invstd, running_mean, running_var, s.NB, (int)d.Ct, s.L, s.eps, s.momentum);
+        bn_stats_kernel<<<(int)d.Ct, 256, 0, st>>>(conv, mean, invstd, running_mean, running_var, s.NB, (int)d.Ct, s.L, s.eps, s.momentum,
+                                                   counts, s.Cout);
     } else {
         B200_REQUIRE(running_mean && running_var, "convblock: eval mode needs running statistics");
         bn_eval_stats_kernel<<<cdiv(d.Ct, 256), 256, 0, st>>>(mean, invstd, running_mean, running_var, (int)d.Ct, s.eps);
     }
     B200_LAUNCH_CHECK();
     BlockArgs a{conv, mean, invstd, gamma, beta, affine_gstride, (s.training && s.dropout > 0.f) ? keep : nullptr,
-                1.f / (1.f - s.dropout), x, s.NB, s.G, s.Cout, s.L, s.activation, s.highway, lengths};
+                1.f / (1.f - s.dropout), x, s.NB, s.G, s.Cout, s.L, s.activation, s.highway, lengths, counts};
     if (vec4_ok(s, d, conv, out, x, a.keep))
         block_fwd_vec4_kernel<<<grid_for((size_t)s.NB * s.G * d.Cf * (s.L / 4)), 256, 0, st>>>(a, out);
     else
@@ -699,7 +763,7 @@ int convblock_forward_impl(const b200tts_convblock_shape& s, const float* x, con
 
 int convblock_backward_impl(const b200tts_convblock_shape& s, const float* x, const float* weight, const float* gamma,
                             const float* beta, int affine_gstride, const uint8_t* keep, const float* saved, const float* dout,
-                            float* dx, float* dweight, float* dgamma, float* dbeta, float* ws, cudaStream_t st) {
+                            float* dx, float* dweight, float* dgamma, float* dbeta, float* ws, cudaStream_t st, const int32_t* counts) {
     B200_TRY(validate_block(s));
     const BlockDims d = block_dims(s);
     const float* conv = s.stage == 2 ? x : saved;
@@ -718,9 +782,13 @@ int convblock_backward_impl(const b200tts_convblock_shape& s, const float* x, co
     }
 
     BlockArgs a{conv, mean, invstd, gamma, beta, affine_gstride, (s.training && s.dropout > 0.f) ? keep : nullptr,
-                1.f / (1.f - s.dropout), x, s.NB, s.G, s.Cout, s.L, s.activation, s.highway};
+                1.f / (1.f - s.dropout), x, s.NB, s.G, s.Cout, s.L, s.activation, s.highway, nullptr, counts};
     if (s.stage == 1) {      // convolution only: dout is the gradient of the product
         B200_CUDA(cudaMemcpyAsync(dz, dout, d.conv_elems * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        if (counts) {
+            zero_vacant_kernel<<<grid_for(d.conv_elems), 256, 0, st>>>(dz, counts, s.NB, s.G, s.Cout, s.L);
+            B200_LAUNCH_CHECK();
+        }
     } else {
     const bool v4 = vec4_ok(s, d, conv, dz, x, a.keep) && (reinterpret_cast<uintptr_t>(dout) & 15) == 0 && (!s.highway || (reinterpret_cast<uintptr_t>(dx) & 15) == 0);
     if (v4)
@@ -728,14 +796,15 @@ int convblock_backward_impl(const b200tts_convblock_shape& s, const float* x, co
     else
         block_bwd_prep_kernel<<<grid_for((size_t)s.NB * s.G * d.Cf * s.L), 256, 0, st>>>(a, dout, dz, dx);
     B200_LAUNCH_CHECK();
-    bn_bwd_reduce_kernel<<<(int)d.Ct, 256, 0, st>>>(dz, conv, mean, invstd, s1, s2, dgamma, dbeta, affine_gstride, s.NB, s.G, s.Cout, s.L);
+    bn_bwd_reduce_kernel<<<(int)d.Ct, 256, 0, st>>>(dz, conv, mean, invstd, s1, s2, dgamma, dbeta, affine_gstride, s.NB, s.G, s.Cout, s.L,
+                                               counts);
     B200_LAUNCH_CHECK();
     if (v4)
         bn_bwd_apply_vec4_kernel<<<grid_for(d.conv_elems / 4), 256, 0, st>>>(dz, conv, mean, invstd, gamma, affine_gstride, s1, s2, s.NB, s.G,
-                                                                           s.Cout, s.L, s.training);
+                                                                           s.Cout, s.L, s.training, counts);
     else
         bn_bwd_apply_kernel<<<grid_for(d.conv_elems), 256, 0, st>>>(dz, conv, mean, invstd, gamma, affine_gstride, s1, s2, s.NB, s.G, s.Cout,
-                                                                    s.L, s.training);
+                                                                    s.L, s.training, counts);
     B200_LAUNCH_CHECK();
     }
     if (s.stage == 2) return B200TTS_OK;

@@ -415,10 +415,12 @@ class ConvBlockFunction(torch.autograd.Function):
 
     x [NB, G*Cin, L]; weight [G*Cout, Cin, k]; gamma/beta: flat tensors addressed (g, o) -> [g*gstride + o]
     (a [G, 2*Cout] generated affine passes gamma = aff, beta = aff[:, Cout:] views with gstride = 2*Cout).
+    counts (or None): int32 [G] on the device, the occupied rows of each channel block (b200tts_convblock_forward_counts); rows
+    nb >= counts[g] of block g are vacant and their outputs and gradients are 0.
     """
 
     @staticmethod
-    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, keep, meta):
+    def forward(ctx, x, weight, gamma, beta, running_mean, running_var, keep, counts, meta):
         (G, k, dilation, activation, highway, training, eps, momentum, dropout, gstride, stage) = meta
         _require_cuda(x, weight, gamma, beta)
         x = _f32c(x)
@@ -441,10 +443,16 @@ class ConvBlockFunction(torch.autograd.Function):
         out = torch.empty(NB, G * Cf, L, device=x.device, dtype=torch.float32)
         if keep is not None:
             assert keep.dtype == torch.uint8 and keep.is_contiguous() and tuple(keep.shape) == (NB, G * Cout, L)
-        check(lib.b200tts_convblock_forward(ctypes.byref(shape), ptr(x), ptr(weight), ptr(gamma), ptr(beta), gstride,
-                                            ptr(running_mean), ptr(running_var), ptr(keep), ptr(out), ptr(saved), ptr(ws), _stream()),
-              'b200tts_convblock_forward')
-        ctx.shape, ctx.gstride, ctx.saved_buf, ctx.keep = shape, gstride, saved, keep
+        if counts is None:
+            check(lib.b200tts_convblock_forward(ctypes.byref(shape), ptr(x), ptr(weight), ptr(gamma), ptr(beta), gstride,
+                                                ptr(running_mean), ptr(running_var), ptr(keep), ptr(out), ptr(saved), ptr(ws), _stream()),
+                  'b200tts_convblock_forward')
+        else:
+            assert counts.dtype == torch.int32 and counts.is_cuda and tuple(counts.shape) == (G,), (counts.dtype, tuple(counts.shape), G)
+            check(lib.b200tts_convblock_forward_counts(ctypes.byref(shape), ptr(counts), G, NB, ptr(x), ptr(weight), ptr(gamma), ptr(beta),
+                                                       gstride, ptr(running_mean), ptr(running_var), ptr(keep), ptr(out), ptr(saved), ptr(ws),
+                                                       _stream()), 'b200tts_convblock_forward_counts')
+        ctx.shape, ctx.gstride, ctx.saved_buf, ctx.keep, ctx.counts = shape, gstride, saved, keep, counts
         ctx.save_for_backward(x, weight, gamma, beta)
         return out
 
@@ -459,23 +467,31 @@ class ConvBlockFunction(torch.autograd.Function):
         (dweight,), (r_weight,) = _grad_targets((weight,))           # leaf convolution weights accumulate straight into .grad
         # gamma / beta may be strided views of one generated-affine tensor: produce gradients in the same geometry
         G, Cout, gs = shape.G, shape.Cout, ctx.gstride
+
+        def run(weight, gamma, beta, keep, dgamma, dbeta):
+            if ctx.counts is None:
+                check(lib.b200tts_convblock_backward(ctypes.byref(shape), ptr(x), ptr(weight), ptr(gamma), ptr(beta), gs, ptr(keep),
+                                                     ptr(ctx.saved_buf), ptr(dout), ptr(dx), ptr(dweight), ptr(dgamma), ptr(dbeta),
+                                                     ptr(ws), _stream()), 'b200tts_convblock_backward')
+            else:
+                check(lib.b200tts_convblock_backward_counts(ctypes.byref(shape), ptr(ctx.counts), G, shape.NB, ptr(x), ptr(weight), ptr(gamma),
+                                                            ptr(beta), gs, ptr(keep), ptr(ctx.saved_buf), ptr(dout), ptr(dx), ptr(dweight),
+                                                            ptr(dgamma), ptr(dbeta), ptr(ws), _stream()), 'b200tts_convblock_backward_counts')
+
         if shape.stage == 1:    # convolution only: no affine parameters
-            check(lib.b200tts_convblock_backward(ctypes.byref(shape), ptr(x), ptr(weight), None, None, gs, None, ptr(ctx.saved_buf), ptr(dout),
-                                                 ptr(dx), ptr(dweight), None, None, ptr(ws), _stream()), 'b200tts_convblock_backward')
-            return dx, r_weight, None, None, None, None, None, None
+            run(weight, None, None, None, None, None)
+            return dx, r_weight, None, None, None, None, None, None, None
         if gs == Cout:      # plain batch norm: separate dense gamma / beta (leaf parameters accumulate straight into .grad)
             (dgamma, dbeta), (g_gamma, g_beta) = _grad_targets((gamma, beta))
             dgb = None
         else:               # generated affine [G, 2*Cout]: gamma = [:, :Cout], beta = [:, Cout:]
             dgb = torch.zeros(2 * G * Cout, device=x.device, dtype=torch.float32)
             dgamma, dbeta = dgb, dgb[Cout:]
-        check(lib.b200tts_convblock_backward(ctypes.byref(shape), ptr(x), ptr(weight), ptr(gamma), ptr(beta), gs, ptr(ctx.keep),
-                                             ptr(ctx.saved_buf), ptr(dout), ptr(dx), ptr(dweight), ptr(dgamma), ptr(dbeta),
-                                             ptr(ws), _stream()), 'b200tts_convblock_backward')
+        run(weight, gamma, beta, ctx.keep, dgamma, dbeta)
         if dgb is not None:
             full = dgb.view(G, gs)
             g_gamma, g_beta = full[:, :Cout], full[:, Cout:]
-        return dx, r_weight, g_gamma, g_beta, None, None, None, None
+        return dx, r_weight, g_gamma, g_beta, None, None, None, None, None
 
 
 def conv_block_masked(x, lengths, weight, gamma, beta, running_mean, running_var, groups, kernel, dilation, activation, highway, eps,
@@ -504,10 +520,11 @@ def conv_block_masked(x, lengths, weight, gamma, beta, running_mean, running_var
 
 
 def conv_block(x, weight, gamma, beta, running_mean, running_var, keep, groups, kernel, dilation, activation, highway,
-               training, eps, momentum, dropout, gstride, stage=0):
-    """stage 0: the whole block; 1: grouped convolution only (gamma / beta None); 2: batch norm (+ activation / dropout) only (weight None)."""
+               training, eps, momentum, dropout, gstride, stage=0, counts=None):
+    """stage 0: the whole block; 1: grouped convolution only (gamma / beta None); 2: batch norm (+ activation / dropout) only (weight None).
+    counts: None (every row of every channel block is an utterance) or int32 [groups] on the device, the occupied rows per block."""
     meta = (groups, kernel, dilation, activation, highway, training, eps, momentum, dropout, gstride, stage)
-    return ConvBlockFunction.apply(x, weight, gamma, beta, running_mean, running_var, keep, meta)
+    return ConvBlockFunction.apply(x, weight, gamma, beta, running_mean, running_var, keep, counts, meta)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -10,6 +10,8 @@ of shapes small); dropout masks stay fresh because the graph increments a device
     step = GraphedTrainStep(model, criterion, bucket, example_batch)     # warm-up + capture (drop every reference to an autograd graph
                                                                          # built before: its AccumulateGrad nodes are bound to ITS stream)
     loss = step(batch)            # copies the batch into the static input buffers, replays, returns the (static) loss tensor
+                                  # (batches of the captured shape and layout: a grouped encoder's batch in the reference layout,
+                                  # utterance b of language b % G, which the constructor checks on the example batch)
     bucket.allreduce(); optimizer.step()
 """
 import ctypes
@@ -17,6 +19,7 @@ import ctypes
 import torch
 
 from . import _lib
+from .modules.encoder import ConvolutionalEncoder, GeneratedConvolutionalEncoder, encoder_layout, language_ids, reference_layout
 
 
 _CAPTURE_STREAMS = {}
@@ -35,6 +38,18 @@ def capture_stream(device):
     return _CAPTURE_STREAMS[key]
 
 
+def _require_reference_layout(model, batch):
+    """A grouped encoder routes a batch by reading its language labels, a device-to-host copy that a capture cannot contain.  The layout
+    is decided here, from the example batch, before capture: the captured step runs the reference layout (utterance b under language
+    b % G) without reading labels, and any other example batch is refused."""
+    langs = batch.get('languages')
+    for m in model.modules():
+        if isinstance(m, (ConvolutionalEncoder, GeneratedConvolutionalEncoder)) and encoder_layout(langs, batch['text'].shape[0], m._groups):
+            raise ValueError('GraphedTrainStep captures grouped-encoder batches in the reference layout only (B divisible by the '
+                             f'{m._groups} languages and utterance b of language b % {m._groups}); the example batch has languages '
+                             f'{language_ids(langs)}.  Run such batches eagerly: the encoder routes them by their labels')
+
+
 class GraphedTrainStep:
     FIELDS = ('text', 'text_length', 'target', 'target_length', 'stop_target', 'speakers', 'languages')
 
@@ -44,6 +59,7 @@ class GraphedTrainStep:
             # would replay one frozen coin pattern at every step.  Run such steps eagerly (the backward supports them).
             raise ValueError(f'GraphedTrainStep needs teacher_forcing = 1.0 (got {teacher_forcing}): a CUDA graph would replay one fixed '
                              'pattern of free-running steps; run steps with teacher forcing below 1.0 eagerly')
+        _require_reference_layout(model, example_batch)
         self.model, self.criterion, self.bucket, self.tf = model, criterion, bucket, float(teacher_forcing)
         dev = next(model.parameters()).device
         self.static = {k: (example_batch[k].to(dev).clone() if example_batch.get(k) is not None else None) for k in self.FIELDS}
@@ -52,7 +68,7 @@ class GraphedTrainStep:
         self.loss, self.parts = None, None
         side = capture_stream(dev)
         side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):                       # warm-up on a side stream (workspaces, lazy attribute settings, pack caches)
+        with torch.cuda.stream(side), reference_layout():   # warm-up on a side stream (workspaces, lazy attribute settings, pack caches)
             for _ in range(warmup):
                 self._body()
         torch.cuda.current_stream(dev).wait_stream(side)
@@ -61,7 +77,7 @@ class GraphedTrainStep:
         # used on, and the engine joins every such "leaf stream" at the end of backward -- a leaf stream that is not the capture stream would
         # be a dependency on uncaptured work as soon as a step sends it no gradient (the library accumulates most gradients in place)
         self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph, stream=side):
+        with torch.cuda.graph(self.graph, stream=side), reference_layout():
             self._body()
         torch.cuda.synchronize(dev)
 

@@ -1,4 +1,6 @@
 """Encoders (surface of reference modules/encoder.py:9-221) on the b200tts library ops."""
+import contextlib
+
 import torch
 from torch.nn import Sequential, ModuleList, LSTM, Embedding
 
@@ -86,8 +88,18 @@ def _language_share(x_langs):
     return torch.where(total != 0, x_langs / torch.where(total != 0, total, torch.ones_like(total)), torch.zeros_like(x_langs))
 
 
-def _run_blocks(blocks, x, lengths):
-    """A Sequential of conv blocks; with `lengths` (a zero-padded eval batch) every block zeroes the positions past them."""
+def _run_blocks(blocks, x, lengths, counts=None):
+    """A Sequential of conv blocks; with `lengths` (a zero-padded eval batch) every block zeroes the positions past them; with `counts`
+    (a routed batch, GroupLayout) every block takes per-language batch statistics over the occupied rows and zeroes the vacant ones."""
+    if counts is not None:
+        if isinstance(x, tuple):
+            e, x = x
+            for block in blocks:
+                _, x = block((e, x), counts=counts)
+            return e, x
+        for block in blocks:
+            x = block(x, counts=counts)
+        return x
     if lengths is None:
         return blocks(x)
     if isinstance(x, tuple):                 # generated blocks pass (generator embedding, x)
@@ -115,6 +127,91 @@ def _mix_languages(per_language, x_langs):
     return mixed
 
 
+class GroupLayout:
+    """Where the utterances of a batch sit in a grouped encoder's channel-blocked layout [n_max, G*F, L].
+
+    Utterance b has language l_b; language g's utterances, in batch order, fill rows 0 .. n_g - 1 of channel block g (utterance b at
+    row ranks[b]), n_max = max_g n_g, and rows q >= n_g of block g are vacant (zero in, zero out).  `reference` is True when this is
+    the reference's own reshape: B divisible by G and l_b = b % G, so that ranks[b] = b // G and nothing is vacant."""
+
+    def __init__(self, ids, groups):
+        self.groups = groups
+        self.ids = [int(g) for g in ids]
+        if any(g < 0 or g >= groups for g in self.ids):
+            raise ValueError(f'language ids must lie in [0, {groups}) for a grouped encoder of {groups} languages (got {sorted(set(self.ids))})')
+        self.counts = [0] * groups
+        self.ranks = []
+        for g in self.ids:
+            self.ranks.append(self.counts[g])
+            self.counts[g] += 1
+        self.n_max = max(self.counts) if self.ids else 0
+        B = len(self.ids)
+        self.reference = B % groups == 0 and all(g == b % groups for b, g in enumerate(self.ids))
+
+    def rows(self):
+        """Flat row of each utterance in the [n_max * G, F, L] view of the layout: rank * G + language."""
+        return [r * self.groups + g for r, g in zip(self.ranks, self.ids)]
+
+    def device_tensors(self, device):
+        """(counts int32 [G], rows int64 [B]) on `device`, in one host-to-device copy from pinned memory."""
+        host = torch.tensor(self.counts + self.rows(), dtype=torch.int32)
+        if torch.device(device).type == 'cuda':
+            host = host.pin_memory()
+        dev = host.to(device, non_blocking=True)
+        return dev[:self.groups], dev[self.groups:].long()
+
+
+def language_ids(x_langs):
+    """Per-utterance language l_b = x_langs[b, 0] of int [B] / [B, L] ids, or the argmax of float [B, L, G] weights, as a host list.
+    A CPU tensor is read where it is (no device synchronisation); a CUDA one costs one device-to-host copy of B ints, which waits for
+    the work queued before it on the stream."""
+    ids = x_langs
+    if ids.dim() == 3:
+        ids = ids[:, 0].argmax(dim=-1)
+    elif ids.dim() == 2:
+        ids = ids[:, 0]
+    if ids.is_cuda:
+        ids = ids.cpu()
+    return ids.tolist()
+
+
+_REFERENCE_SCOPE = [0]
+
+
+@contextlib.contextmanager
+def reference_layout():
+    """Inside this scope the grouped encoders take every batch to be in the reference layout (utterance b under language b % G) without
+    reading its labels.  A CUDA graph capture needs it: reading CUDA labels is a device-to-host copy, which a capture does not allow.
+    The caller vouches for the layout (graph.GraphedTrainStep checks its example batch with `encoder_layout` before capturing)."""
+    _REFERENCE_SCOPE[0] += 1
+    try:
+        yield
+    finally:
+        _REFERENCE_SCOPE[0] -= 1
+
+
+def encoder_layout(x_langs, batch, groups, padded=False):
+    """The layout decision shared by both grouped encoders for a batch of `batch` utterances: None when the batch runs as the
+    reference's reshape (reference layout, no labels, one language, the inference mixing branch, or inside `reference_layout()`), else
+    the GroupLayout to route it through.  Labels for another number of utterances than `batch` are rejected."""
+    if groups == 1 or x_langs is None or _REFERENCE_SCOPE[0] or padded or x_langs.shape[0] == 1:
+        return None
+    if x_langs.shape[0] != batch:
+        raise ValueError(f'language labels for {x_langs.shape[0]} utterances given for a batch of {batch}')
+    layout = GroupLayout(language_ids(x_langs), groups)
+    return None if layout.reference else layout
+
+
+def _routed(x, layout, output_dim, run):
+    """x [B, L, F] -> scattered into the zero layout [n_max, G*F, L], run(x, counts), the rows of the utterances gathered back -> [B, L, E]."""
+    B, L, Fdim = x.shape
+    G = layout.groups
+    counts, rows = layout.device_tensors(x.device)
+    padded = x.new_zeros(layout.n_max * G, Fdim, L).index_copy(0, rows, x.transpose(1, 2))
+    y = run(padded.view(layout.n_max, G * Fdim, L), counts)
+    return y.reshape(layout.n_max * G, output_dim, L).index_select(0, rows).transpose(1, 2)
+
+
 def _expand_groups(x, x_langs, padded, groups):
     """Inference input of a grouped encoder: one utterance (the reference's batch-1 branch) or a padded batch is repeated for every
     language, row b*G + g = utterance b under language g, so that sample row b of the grouped layout is utterance b."""
@@ -127,7 +224,8 @@ def _expand_groups(x, x_langs, padded, groups):
 class ConvolutionalEncoder(torch.nn.Module):
     """Fully convolutional grouped encoder with plain weights (encoder.py:100-156).
 
-    Input [B, L, F] with B divisible by the number of languages and sample b belonging to language b % groups."""
+    Input [B, L, F]; utterance b is encoded with the weights, batch-norm statistics and dropout of its own language x_langs[b, 0]
+    (GroupLayout).  Without labels, utterance b belongs to language b % groups and B must be divisible by the number of languages."""
 
     def __init__(self, input_dim, output_dim, dropout, groups=1):
         super().__init__()
@@ -145,6 +243,9 @@ class ConvolutionalEncoder(torch.nn.Module):
         self._layers = Sequential(*layers)
 
     def forward(self, x, x_lenghts=None, x_langs=None, padded=False):
+        layout = encoder_layout(x_langs, x.shape[0], self._groups, padded)
+        if layout is not None:
+            return _routed(x, layout, self._output_dim, lambda h, counts: _run_blocks(self._layers, h, None, counts))
         x, mixing = _expand_groups(x, x_langs, padded, self._groups)
         bs = x.shape[0]
         if bs % self._groups != 0:
@@ -180,8 +281,12 @@ class GeneratedConvolutionalEncoder(torch.nn.Module):
         self._embedding = Embedding(groups, embedding_dim)
 
     def forward(self, x, x_lenghts=None, x_langs=None, padded=False):
-        x, mixing = _expand_groups(x, x_langs, padded, self._groups)
+        """Utterance b is encoded with the generated weights, batch-norm statistics and dropout of its language x_langs[b, 0] (GroupLayout)."""
         e = self._embedding.weight                       # Embedding(arange(groups)) == the table itself
+        layout = encoder_layout(x_langs, x.shape[0], self._groups, padded)
+        if layout is not None:
+            return _routed(x, layout, self._output_dim, lambda h, counts: _run_blocks(self._layers, (e, h), None, counts)[1])
+        x, mixing = _expand_groups(x, x_langs, padded, self._groups)
         bs = x.shape[0]
         if bs % self._groups != 0:
             raise _lib.B200TTSError(f'batch size {bs} must be divisible by the number of languages {self._groups}')

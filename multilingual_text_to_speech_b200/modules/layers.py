@@ -72,7 +72,7 @@ class ConvBlock(torch.nn.Module):
         self._mask_key = None
         self._highway = False
 
-    def _run(self, x):
+    def _run(self, x, counts=None):
         conv, bn = self._block[1], self._block[2]
         G = self._groups
         cout = conv.weight.shape[0] // G
@@ -81,20 +81,21 @@ class ConvBlock(torch.nn.Module):
             keep = MaskSource.keep_mask(self._mask_key, (x.shape[0], conv.weight.shape[0], x.shape[2]), self._dropout_rate, x.device)
         out = F.conv_block(x, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, keep, G, self._kernel,
                            self._dilation, self._activation_name, self._highway, self.training, bn.eps, bn.momentum,
-                           self._dropout_rate if keep is not None else 0.0, cout)
+                           self._dropout_rate if keep is not None else 0.0, cout, counts=counts)
         if self.training:
             bn.num_batches_tracked += 1
         return out
 
-    def forward(self, x, lengths=None):
-        """lengths (eval only): per-sample lengths of a zero-padded batch; outputs past each length are 0."""
+    def forward(self, x, lengths=None, counts=None):
+        """lengths (eval only): per-sample lengths of a zero-padded batch; outputs past each length are 0.
+        counts: int32 [groups] on the device, the utterances in each channel block (rows past them are vacant, see F.conv_block)."""
         if lengths is not None:
             _require_eval(self)
             conv, bn = self._block[1], self._block[2]
             return F.conv_block_masked(x, lengths, conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var, self._groups,
                                        self._kernel, self._dilation, self._activation_name, self._highway, bn.eps,
                                        conv.weight.shape[0] // self._groups)
-        return self._run(x)
+        return self._run(x, counts)
 
 
 class HighwayConvBlock(ConvBlock):
@@ -126,8 +127,9 @@ class ConvBlockGenerated(torch.nn.Module):
         self._mask_key = None
         self._highway = False
 
-    def forward(self, x, lengths=None):
-        """lengths (eval only): per-sample lengths of a zero-padded batch; outputs past each length are 0."""
+    def forward(self, x, lengths=None, counts=None):
+        """lengths (eval only): per-sample lengths of a zero-padded batch; outputs past each length are 0.
+        counts: int32 [groups] on the device, the utterances in each channel block (rows past them are vacant, see F.conv_block)."""
         if lengths is not None:
             _require_eval(self)
         e, x = x
@@ -144,7 +146,7 @@ class ConvBlockGenerated(torch.nn.Module):
             keep = MaskSource.keep_mask(self._mask_key, (x.shape[0], kernel.shape[0], x.shape[2]), self._dropout_rate, x.device)
         out = F.conv_block(x, kernel, affine[:, :cout], affine[:, cout:], bn.running_mean, bn.running_var, keep, G,
                            self._kernel, self._dilation, self._activation_name, self._highway, self.training, bn._eps,
-                           bn._momentum, self._dropout_rate if keep is not None else 0.0, 2 * cout)
+                           bn._momentum, self._dropout_rate if keep is not None else 0.0, 2 * cout, counts=counts)
         if self.training:
             bn.num_batches_tracked += 1
         return e, out
