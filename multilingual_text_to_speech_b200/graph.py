@@ -10,16 +10,21 @@ of shapes small); dropout masks stay fresh because the graph increments a device
     step = GraphedTrainStep(model, criterion, bucket, example_batch)     # warm-up + capture (drop every reference to an autograd graph
                                                                          # built before: its AccumulateGrad nodes are bound to ITS stream)
     loss = step(batch)            # copies the batch into the static input buffers, replays, returns the (static) loss tensor
-                                  # (batches of the captured shape and layout: a grouped encoder's batch in the reference layout,
-                                  # utterance b of language b % G, which the constructor checks on the example batch)
     bucket.allreduce(); optimizer.step()
+
+A grouped encoder (ConvolutionalEncoder / GeneratedConvolutionalEncoder) routes each utterance to its own language's channel block
+(modules/encoder.py GroupLayout).  An example batch in the reference layout (utterance b of language b % G) is captured as that reshape,
+and its replays read no labels.  With `max_per_language` the step is captured in the routed layout at that fixed capacity of rows
+per language; each call then builds the batch's GroupLayout on the host and copies its counts and rows into static device buffers
+before the replay, so one graph serves every language pattern within the capacity (StaticRouting).  An example batch outside the
+reference layout needs that capacity: without `max_per_language` it is refused.
 """
 import ctypes
 
 import torch
 
 from . import _lib
-from .modules.encoder import ConvolutionalEncoder, GeneratedConvolutionalEncoder, encoder_layout, language_ids, reference_layout
+from .modules.encoder import ConvolutionalEncoder, GeneratedConvolutionalEncoder, GroupLayout, encoder_layout, given_layout, language_ids
 
 
 _CAPTURE_STREAMS = {}
@@ -38,37 +43,88 @@ def capture_stream(device):
     return _CAPTURE_STREAMS[key]
 
 
-def _require_reference_layout(model, batch):
-    """A grouped encoder routes a batch by reading its language labels, a device-to-host copy that a capture cannot contain.  The layout
-    is decided here, from the example batch, before capture: the captured step runs the reference layout (utterance b under language
-    b % G) without reading labels, and any other example batch is refused."""
+class StaticRouting:
+    """The routing of a graph captured in the routed layout [capacity, G*F, L]: counts int32 [G] and rows int64 [B] (GroupLayout.counts
+    and rows()) in one static int32 buffer on the device, refilled from each batch's labels before its replay.
+
+    `layout(x_langs)` reads the labels and checks them without touching the buffer: CPU labels are read in place with no device
+    synchronisation; CUDA labels cost one device-to-host copy of B ints, which waits for the work queued before it on the stream (the
+    same read an eager routed step makes).  `load(layout)` fills the buffer with one host-to-device copy from pinned memory."""
+
+    def __init__(self, groups, batch, capacity, device):
+        pad = groups + groups % 2             # rows start 8-byte aligned
+        self.groups, self.batch, self.capacity = groups, batch, capacity
+        self.buffer = torch.zeros(pad + 2 * batch, dtype=torch.int32, device=device)
+        self.counts, self.rows = self.buffer[:groups], self.buffer[pad:].view(torch.int64)
+
+    def layout(self, x_langs):
+        ids = language_ids(x_langs)
+        if len(ids) != self.batch:
+            raise ValueError(f'language labels for {len(ids)} utterances given for a graph captured at a batch of {self.batch}')
+        return GroupLayout(ids, self.groups, self.capacity)
+
+    def load(self, layout):
+        pad = self.buffer.numel() - 2 * self.batch
+        host = torch.cat((torch.tensor(layout.counts + [0] * (pad - self.groups), dtype=torch.int32),
+                          torch.tensor(layout.rows(), dtype=torch.int64).view(torch.int32)))
+        if self.buffer.is_cuda:
+            host = host.pin_memory()
+        self.buffer.copy_(host, non_blocking=True)
+
+    def given(self):
+        """The (counts, rows, capacity) routing of modules.encoder.given_layout."""
+        return self.counts, self.rows, self.capacity
+
+
+def _static_routing(model, batch, max_per_language, device):
+    """None when the step is captured as the reference reshape (no grouped encoder, no labels, or no `max_per_language` and an example
+    batch that the encoders run unrouted), else the StaticRouting at capacity `max_per_language`.  The capacity fixes the encoder's
+    work and the batches a graph accepts, so it is never guessed from one example batch: a routed example without it is refused."""
+    groups = [m._groups for m in model.modules() if isinstance(m, (ConvolutionalEncoder, GeneratedConvolutionalEncoder)) and m._groups > 1]
     langs = batch.get('languages')
-    for m in model.modules():
-        if isinstance(m, (ConvolutionalEncoder, GeneratedConvolutionalEncoder)) and encoder_layout(langs, batch['text'].shape[0], m._groups):
-            raise ValueError('GraphedTrainStep captures grouped-encoder batches in the reference layout only (B divisible by the '
-                             f'{m._groups} languages and utterance b of language b % {m._groups}); the example batch has languages '
-                             f'{language_ids(langs)}.  Run such batches eagerly: the encoder routes them by their labels')
+    if not groups or langs is None:
+        return None
+    G, B = groups[0], batch['text'].shape[0]
+    if max_per_language is None:
+        if encoder_layout(langs, B, G) is None:
+            return None
+        n_max = GroupLayout(language_ids(langs), G).n_max
+        raise ValueError('GraphedTrainStep captures grouped-encoder batches outside the reference layout (B divisible by the '
+                         f'{G} languages and utterance b of language b % {G}) only at a fixed capacity of utterances per language: '
+                         f'pass max_per_language, the most utterances of one language any batch of this shape will have (the example '
+                         f'batch has {n_max}).  The encoder then runs {G} x max_per_language rows per step')
+    if int(max_per_language) < 1:
+        raise ValueError(f'max_per_language must be at least 1 (got {max_per_language})')
+    return StaticRouting(G, B, int(max_per_language), device)
 
 
 class GraphedTrainStep:
     FIELDS = ('text', 'text_length', 'target', 'target_length', 'stop_target', 'speakers', 'languages')
 
-    def __init__(self, model, criterion, bucket, example_batch, teacher_forcing=1.0, warmup=3):
+    def __init__(self, model, criterion, bucket, example_batch, teacher_forcing=1.0, warmup=3, max_per_language=None):
+        """max_per_language: the capacity, in utterances per language, of the routed layout a grouped encoder is captured in (see the
+        module docstring); a batch with more utterances of one language raises ValueError, the example batch included.  Balanced
+        samplers (PerfectBatchSampler, BucketedPerfectBatchSampler, shard) give ceil(B / G); imbalanced ones (RandomImbalancedSampler)
+        need a bound.  None: the example batch must be in the reference layout, and is captured as the reference's reshape.  Ignored
+        without a grouped encoder."""
         if float(teacher_forcing) < 1.0:
             # the per-step teacher-forcing coins are drawn on the host and decide which kernels a decode launches: one captured graph
             # would replay one frozen coin pattern at every step.  Run such steps eagerly (the backward supports them).
             raise ValueError(f'GraphedTrainStep needs teacher_forcing = 1.0 (got {teacher_forcing}): a CUDA graph would replay one fixed '
                              'pattern of free-running steps; run steps with teacher forcing below 1.0 eagerly')
-        _require_reference_layout(model, example_batch)
-        self.model, self.criterion, self.bucket, self.tf = model, criterion, bucket, float(teacher_forcing)
         dev = next(model.parameters()).device
+        self.routing = _static_routing(model, example_batch, max_per_language, dev)
+        if self.routing is not None:
+            self.routing.load(self.routing.layout(example_batch['languages']))
+        given = None if self.routing is None else self.routing.given()
+        self.model, self.criterion, self.bucket, self.tf = model, criterion, bucket, float(teacher_forcing)
         self.static = {k: (example_batch[k].to(dev).clone() if example_batch.get(k) is not None else None) for k in self.FIELDS}
         self.epoch = torch.zeros(1, dtype=torch.int64, device=dev)
         _lib.check(_lib.load().b200tts_set_mask_epoch(ctypes.c_void_p(self.epoch.data_ptr())), 'b200tts_set_mask_epoch')
         self.loss, self.parts = None, None
         side = capture_stream(dev)
         side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side), reference_layout():   # warm-up on a side stream (workspaces, lazy attribute settings, pack caches)
+        with torch.cuda.stream(side), given_layout(given):   # warm-up on a side stream (workspaces, lazy attribute settings, pack caches)
             for _ in range(warmup):
                 self._body()
         torch.cuda.current_stream(dev).wait_stream(side)
@@ -77,7 +133,7 @@ class GraphedTrainStep:
         # used on, and the engine joins every such "leaf stream" at the end of backward -- a leaf stream that is not the capture stream would
         # be a dependency on uncaptured work as soon as a step sends it no gradient (the library accumulates most gradients in place)
         self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph, stream=side), reference_layout():
+        with torch.cuda.graph(self.graph, stream=side), given_layout(given):
             self._body()
         torch.cuda.synchronize(dev)
 
@@ -92,6 +148,10 @@ class GraphedTrainStep:
         self.loss.backward()
 
     def __call__(self, batch):
+        """Copies the batch into the static buffers and replays.  A routed graph first reads the batch's labels (StaticRouting.layout:
+        a batch over the capacity raises ValueError before any static buffer is written) and copies its counts and rows in."""
+        if self.routing is not None:
+            self.routing.load(self.routing.layout(batch['languages']))
         for k in self.FIELDS:
             dst = self.static[k]
             if dst is not None:

@@ -128,13 +128,15 @@ def _mix_languages(per_language, x_langs):
 
 
 class GroupLayout:
-    """Where the utterances of a batch sit in a grouped encoder's channel-blocked layout [n_max, G*F, L].
+    """Where the utterances of a batch sit in a grouped encoder's channel-blocked layout [nb, G*F, L].
 
     Utterance b has language l_b; language g's utterances, in batch order, fill rows 0 .. n_g - 1 of channel block g (utterance b at
-    row ranks[b]), n_max = max_g n_g, and rows q >= n_g of block g are vacant (zero in, zero out).  `reference` is True when this is
-    the reference's own reshape: B divisible by G and l_b = b % G, so that ranks[b] = b // G and nothing is vacant."""
+    row ranks[b]), n_max = max_g n_g, and rows q >= n_g of block g are vacant (zero in, zero out).  The layout has nb = n_max rows per
+    block, or nb = `capacity` when one is given: a fixed size that many batches share (a CUDA graph, graph.GraphedTrainStep), and a
+    language with more than `capacity` utterances raises ValueError.  `reference` is True when this is the reference's own reshape:
+    B divisible by G and l_b = b % G, so that ranks[b] = b // G and nothing is vacant."""
 
-    def __init__(self, ids, groups):
+    def __init__(self, ids, groups, capacity=None):
         self.groups = groups
         self.ids = [int(g) for g in ids]
         if any(g < 0 or g >= groups for g in self.ids):
@@ -145,11 +147,18 @@ class GroupLayout:
             self.ranks.append(self.counts[g])
             self.counts[g] += 1
         self.n_max = max(self.counts) if self.ids else 0
+        if capacity is not None:
+            over = [(g, n) for g, n in enumerate(self.counts) if n > capacity]
+            if over:
+                g, n = over[0]
+                raise ValueError(f'language {g} has {n} utterances in this batch, more than the layout capacity of {capacity} per language')
+        self.capacity = capacity
+        self.nb = self.n_max if capacity is None else capacity
         B = len(self.ids)
         self.reference = B % groups == 0 and all(g == b % groups for b, g in enumerate(self.ids))
 
     def rows(self):
-        """Flat row of each utterance in the [n_max * G, F, L] view of the layout: rank * G + language."""
+        """Flat row of each utterance in the [nb * G, F, L] view of the layout: rank * G + language."""
         return [r * self.groups + g for r, g in zip(self.ranks, self.ids)]
 
     def device_tensors(self, device):
@@ -175,27 +184,40 @@ def language_ids(x_langs):
     return ids.tolist()
 
 
-_REFERENCE_SCOPE = [0]
+_GIVEN_LAYOUT = []
 
 
 @contextlib.contextmanager
-def reference_layout():
-    """Inside this scope the grouped encoders take every batch to be in the reference layout (utterance b under language b % G) without
-    reading its labels.  A CUDA graph capture needs it: reading CUDA labels is a device-to-host copy, which a capture does not allow.
-    The caller vouches for the layout (graph.GraphedTrainStep checks its example batch with `encoder_layout` before capturing)."""
-    _REFERENCE_SCOPE[0] += 1
+def given_layout(routing=None):
+    """Inside this scope the grouped encoders take the layout of every batch as given instead of reading its labels.  A CUDA graph
+    capture needs it: reading CUDA labels is a device-to-host copy, which a capture does not allow.
+
+    routing None: the reference layout (utterance b under language b % G).  routing (counts, rows, capacity): the routed layout
+    [capacity, G*F, L] whose occupied rows per language (int32 [G]) and utterance rows (int64 [B], GroupLayout.rows()) the device
+    tensors `counts` and `rows` hold.  The encoders read them on the device only, so one captured graph serves whatever they hold at
+    each replay.  The caller vouches for the layout (graph.GraphedTrainStep checks its example batch, and builds the GroupLayout of
+    every batch on the host and copies it in before each replay)."""
+    _GIVEN_LAYOUT.append(routing)
     try:
         yield
     finally:
-        _REFERENCE_SCOPE[0] -= 1
+        _GIVEN_LAYOUT.pop()
+
+
+def reference_layout():
+    """given_layout() of the reference layout: every batch is taken to have utterance b under language b % G."""
+    return given_layout()
 
 
 def encoder_layout(x_langs, batch, groups, padded=False):
     """The layout decision shared by both grouped encoders for a batch of `batch` utterances: None when the batch runs as the
-    reference's reshape (reference layout, no labels, one language, the inference mixing branch, or inside `reference_layout()`), else
-    the GroupLayout to route it through.  Labels for another number of utterances than `batch` are rejected."""
-    if groups == 1 or x_langs is None or _REFERENCE_SCOPE[0] or padded or x_langs.shape[0] == 1:
+    reference's reshape (reference layout, no labels, one language, the inference mixing branch, or inside `reference_layout()`), the
+    routing of `given_layout(routing)` inside that scope, else the GroupLayout to route it through.  Labels for another number of
+    utterances than `batch` are rejected."""
+    if groups == 1 or x_langs is None or padded or x_langs.shape[0] == 1:
         return None
+    if _GIVEN_LAYOUT:
+        return _GIVEN_LAYOUT[-1]
     if x_langs.shape[0] != batch:
         raise ValueError(f'language labels for {x_langs.shape[0]} utterances given for a batch of {batch}')
     layout = GroupLayout(language_ids(x_langs), groups)
@@ -203,13 +225,20 @@ def encoder_layout(x_langs, batch, groups, padded=False):
 
 
 def _routed(x, layout, output_dim, run):
-    """x [B, L, F] -> scattered into the zero layout [n_max, G*F, L], run(x, counts), the rows of the utterances gathered back -> [B, L, E]."""
+    """x [B, L, F] -> scattered into the zero layout [nb, G*F, L], run(x, counts), the rows of the utterances gathered back -> [B, L, E].
+    layout: a GroupLayout, whose counts and rows are copied to the device here, or a given (counts, rows, capacity) routing."""
     B, L, Fdim = x.shape
-    G = layout.groups
-    counts, rows = layout.device_tensors(x.device)
-    padded = x.new_zeros(layout.n_max * G, Fdim, L).index_copy(0, rows, x.transpose(1, 2))
-    y = run(padded.view(layout.n_max, G * Fdim, L), counts)
-    return y.reshape(layout.n_max * G, output_dim, L).index_select(0, rows).transpose(1, 2)
+    if isinstance(layout, GroupLayout):
+        counts, rows = layout.device_tensors(x.device)
+        nb = layout.nb
+    else:
+        counts, rows, nb = layout
+        if rows.shape[0] != B:
+            raise ValueError(f'the given layout routes {rows.shape[0]} utterances, the batch has {B}')
+    G = counts.shape[0]
+    padded = x.new_zeros(nb * G, Fdim, L).index_copy(0, rows, x.transpose(1, 2))
+    y = run(padded.view(nb, G * Fdim, L), counts)
+    return y.reshape(nb * G, output_dim, L).index_select(0, rows).transpose(1, 2)
 
 
 def _expand_groups(x, x_langs, padded, groups):
