@@ -102,7 +102,7 @@ __device__ __forceinline__ float block_max(float v, float* scratch) {
 __device__ __forceinline__ float sigmoidf_acc(float x) { return 1.f / (1.f + expf(-x)); }
 
 // ---------------------------------------------------------------------------------------------
-// GEMM (gemm_f32.cu):  C = alpha * op(A) . op(B) + beta * C + bias[n]
+// GEMM (gemm.cu):  C = alpha * op(A) . op(B) + beta * C + bias[n]
 //   op(A)(m,k) = transA ? A[k*lda+m] : A[m*lda+k];  op(B)(k,n) = transB ? B[n*ldb+k] : B[k*ldb+n]
 //   batch > 1: pointers advance by stride{A,B,C}.  splitk > 1: raw partial sums are written to
 //   `partial` as [splitk][batch][M][N] (dense) and, unless `keep_partials`, reduced into C.
@@ -135,7 +135,7 @@ struct GemmDesc {
     int ldb16 = 0;
     // optional two-level K (wgmma path only; needs !transA && transB): K = kouter * kin, element (row, q * kin + l) of op(A) lives at
     // A[q * kosA + row * lda + l] (op(B) likewise with kosB): sums a product over `kouter` separately stored slabs in ONE GEMM.
-    // gemm_f32 / gemm_bf16 reject kin > 0 (B200TTS_ERR_INVALID) when the wgmma path does not take the product
+    // the SIMT and mma.sync kernels reject kin > 0 (B200TTS_ERR_INVALID) when the wgmma path does not take the product
     int kin = 0;
     long long kosA = 0, kosB = 0;
 };
@@ -144,8 +144,22 @@ struct GemmDesc {
 void tc_pack_cache_begin();
 void tc_pack_cache_end();
 
-int gemm_f32(const GemmDesc& d, cudaStream_t stream);
-int gemm_bf16(const GemmDesc& d, cudaStream_t stream);
+// Arguments of the SIMT (gemm.cu) and mma.sync (gemm_bf16.cu) kernels, filled from a GemmDesc by gemm.cu.  kcontig: the operand is
+// contiguous along k; vec: 16-byte vector loads are legal; kchunk: k range of one split, a multiple of the kernel's k-block.
+struct GemmKernelArgs {
+    const float* A; const float* B; float* C; const float* bias; float* partial;
+    int M, N, K, lda, ldb, ldc;
+    int a_kcontig, b_kcontig, a_vec, b_vec;
+    float alpha, beta;
+    int batch, splitk, kchunk, a_batch_mod;
+    long long strideA, strideB, strideC;
+};
+constexpr int GEMM_MMA_BK = 32;     // k-block of the mma.sync kernel
+int launch_gemm_mma(const GemmKernelArgs& p, cudaStream_t stream);
+// Split-K reduction shared by every GEMM path: C[b] = alpha * sum_{z = 0 .. splitk - 1} partial[z][b] + bias[n] + beta * C[b], summed in
+// that fixed order (deterministic); partial is [splitk][batch][M][N] (dense), C[b] starts at C + b * strideC with row stride ldc
+int splitk_reduce(const float* partial, float* C, const float* bias, int M, int N, int ldc, int batch, int splitk, long long strideC,
+                  float alpha, float beta, cudaStream_t stream);
 // wgmma path (gemm_tc.cu): returns B200TTS_OK and sets *handled = true when it ran; *handled = false: the shape is not one it takes, the
 // caller runs its own path
 int gemm_tc_try(const GemmDesc& d, cudaStream_t st, bool* handled);
@@ -156,10 +170,11 @@ int tc_make_mapN_bf16(void* map, const void* base, int rank, const unsigned long
 // Precision mode of the library (b200tts_set_precision): 0 = fp32-exact (parity mode), 1 = bf16 tensor-core operands.
 int precision_mode();
 void set_precision_mode(int mode);
-// Dispatch on the precision mode.
+// Dispatch on the precision mode: bf16 mode tries the wgmma path, then runs mma.sync; fp32 mode runs the SIMT kernel.
 int gemm_run(const GemmDesc& d, cudaStream_t stream);
 int gemm_run_auto(GemmDesc d, float* scratch, size_t scratch_elems, cudaStream_t stream);
-size_t gemm_partial_elems(const GemmDesc& d);
+// The SIMT kernel whatever the precision mode.
+int gemm_f32(const GemmDesc& d, cudaStream_t stream);
 int gemm_f32_auto(GemmDesc d, float* scratch, size_t scratch_elems, cudaStream_t stream);
 
 }  // namespace b200tts

@@ -1,6 +1,6 @@
 // bf16 tensor-core GEMM (fp32 in / fp32 out, operands rounded to bf16 on the way into shared memory,
 // fp32 accumulation) for the perf mode ("bf16 fwd / fp32 master", BASELINE.json configs[1]).
-// Same GemmDesc contract as gemm_f32 (transposes, batch strides, a_batch_mod, deterministic split-K).
+// Same GemmDesc contract as the SIMT kernel (transposes, batch strides, a_batch_mod, split-K); host setup in gemm.cu.
 // 128x128x32 CTA tile, 8 warps (2 x 4), each warp 64x32 through mma.sync.m16n8k16 fed by ldmatrix.
 #include <cuda_bf16.h>
 #include "common.cuh"
@@ -12,17 +12,8 @@ namespace {
 
 using namespace tcx;
 
-constexpr int BM = 128, BN = 128, BK = 32, LDS = BK + 8;   // smem row stride in bf16 (80 B: conflict-free ldmatrix)
+constexpr int BM = 128, BN = 128, BK = GEMM_MMA_BK, LDS = BK + 8;   // smem row stride in bf16 (80 B: conflict-free ldmatrix)
 constexpr int NT = 256;
-
-struct KernelArgs {
-    const float* A; const float* B; float* C; const float* bias; float* partial;
-    int M, N, K, lda, ldb, ldc;
-    int a_kcontig, b_kcontig, a_vec, b_vec;
-    float alpha, beta;
-    int batch, splitk, kchunk, a_batch_mod;
-    long long strideA, strideB, strideC;
-};
 
 // Stage a 128 x 32 operand tile: global fp32 -> registers (16 floats / thread).
 //   kcontig: element (r, k) at base[r*ld + k]; else at base[k*ld + r].
@@ -91,7 +82,7 @@ __device__ __forceinline__ void tile_store(__nv_bfloat16* sm, bool kcontig, bool
     }
 }
 
-__global__ void __launch_bounds__(NT) gemm_bf16_kernel(const KernelArgs p) {
+__global__ void __launch_bounds__(NT) gemm_bf16_kernel(const GemmKernelArgs p) {
     __shared__ __align__(16) __nv_bfloat16 As[2][BM * LDS];
     __shared__ __align__(16) __nv_bfloat16 Bs[2][BN * LDS];
     const int z = blockIdx.z;
@@ -177,62 +168,12 @@ __global__ void __launch_bounds__(NT) gemm_bf16_kernel(const KernelArgs p) {
             }
 }
 
-__global__ void splitk_reduce_kernel(const float* __restrict__ partial, float* __restrict__ C, const float* __restrict__ bias, int M,
-                                     int N, int ldc, int batch, int splitk, long long strideC, float alpha, float beta) {
-    const size_t total = (size_t)batch * M * N;
-    for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
-        const int n = idx % N;
-        const int m = (idx / N) % M;
-        const int b = idx / ((size_t)M * N);
-        float s = 0.f;
-        for (int k = 0; k < splitk; ++k) s += partial[(size_t)k * total + idx];
-        s *= alpha;
-        if (bias) s += bias[n];
-        float* c = C + (size_t)b * strideC + (size_t)m * ldc + n;
-        if (beta != 0.f) s += beta * *c;
-        *c = s;
-    }
-}
-
-inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
 }  // namespace
 
-int gemm_bf16(const GemmDesc& d, cudaStream_t stream) {
-    if (d.M <= 0 || d.N <= 0 || d.batch <= 0) return B200TTS_OK;
-    {   // wgmma / TMA path for the large contractions (gemm_tc.cu); falls through when not applicable
-        bool handled = false;
-        B200_TRY(gemm_tc_try(d, stream, &handled));
-        if (handled) return B200TTS_OK;
-    }
-    B200_REQUIRE(d.kin == 0, "gemm_bf16: two-level K (kin = %d) is taken by the wgmma path only, which declined this product", d.kin);
-    B200_REQUIRE(d.A && d.B && (d.C || (d.splitk > 1 && d.keep_partials)), "gemm_bf16: null operand");
-    B200_REQUIRE(d.splitk >= 1 && (d.splitk == 1 || d.partial), "gemm_bf16: split-K needs a partial workspace");
-    KernelArgs p;
-    p.A = d.A; p.B = d.B; p.C = d.C; p.bias = d.bias; p.partial = d.partial;
-    p.M = d.M; p.N = d.N; p.K = d.K; p.lda = d.lda; p.ldb = d.ldb; p.ldc = d.ldc;
-    p.a_kcontig = !d.transA; p.b_kcontig = d.transB;
-    p.alpha = d.alpha; p.beta = d.beta; p.batch = d.batch; p.splitk = d.splitk;
-    p.strideA = d.strideA; p.strideB = d.strideB; p.strideC = d.strideC; p.a_batch_mod = d.a_batch_mod;
-    int kchunk = cdiv(d.K > 0 ? d.K : 1, d.splitk);
-    p.kchunk = cdiv(kchunk, BK) * BK;
-    auto vec_ok = [&](const float* ptr, int ld, long long stride, bool kcontig, int rows) {
-        if (!aligned16(ptr) || (ld & 3) || (stride & 3)) return false;
-        return kcontig ? ((d.K & 3) == 0) : ((rows & 3) == 0);
-    };
-    p.a_vec = vec_ok(d.A, d.lda, d.strideA, p.a_kcontig, d.M);
-    p.b_vec = vec_ok(d.B, d.ldb, d.strideB, p.b_kcontig, d.N);
-    dim3 grid(cdiv(d.N, BN), cdiv(d.M, BM), d.batch * d.splitk);
+int launch_gemm_mma(const GemmKernelArgs& p, cudaStream_t stream) {
+    dim3 grid(cdiv(p.N, BN), cdiv(p.M, BM), p.batch * p.splitk);
     gemm_bf16_kernel<<<grid, NT, 0, stream>>>(p);
     B200_LAUNCH_CHECK();
-    if (d.splitk > 1 && !d.keep_partials) {
-        const size_t total = (size_t)d.batch * d.M * d.N;
-        int blocks = (int)((total + 255) / 256);
-        if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
-        splitk_reduce_kernel<<<blocks, 256, 0, stream>>>(d.partial, d.C, d.bias, d.M, d.N, d.ldc, d.batch, d.splitk, d.strideC,
-                                                          d.alpha, d.beta);
-        B200_LAUNCH_CHECK();
-    }
     return B200TTS_OK;
 }
 

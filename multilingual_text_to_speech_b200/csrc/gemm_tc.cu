@@ -230,23 +230,6 @@ __global__ void pack_transpose_kernel(__nv_bfloat16* __restrict__ dst, const flo
     }
 }
 
-// C = alpha * sum_z partial[z] + beta * C + bias   (fixed order over the splits: deterministic)
-__global__ void tc_splitk_reduce_kernel(const float* __restrict__ partial, float* __restrict__ C, const float* __restrict__ bias, int M, int N,
-                                        int ldc, int ksplit, float alpha, float beta) {
-    const size_t total = (size_t)M * N;
-    for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
-        const int n = idx % N;
-        const size_t m = idx / N;
-        float s = 0.f;
-        for (int z = 0; z < ksplit; ++z) s += partial[(size_t)z * total + idx];
-        s *= alpha;
-        if (bias) s += bias[n];
-        float* c = C + m * ldc + n;
-        if (beta != 0.f) s += beta * *c;
-        *c = s;
-    }
-}
-
 // Convolution weights W[g][co][ci][t] (fp32) -> bf16 A operands with K ordered (tap, channel):
 //   forward : dst[g][co][t * Cin + ci]            (rows = output channels)
 //   backward: dst[g][ci][t * Cout + co]           (rows = input channels: the input-gradient convolution)
@@ -437,13 +420,13 @@ int gemm_tc_try(const GemmDesc& d, cudaStream_t st, bool* handled) {
     const int abatch = d.a_batch_mod > 0 ? d.a_batch_mod : d.batch;
     const bool a16ok = d.A16 != nullptr && d.batch == 1 && (d.lda16 % 8) == 0 && (reinterpret_cast<uintptr_t>(d.A16) & 15) == 0;
     // A16 with transA: the bf16 matrix is [K, M] row-major (e.g. the gate-gradient history of the reverse loops) = an MN-major operand in place
-    const bool a_mn_ready = a16ok && d.transA && d.kin == 0 && (d.lda16 % 64) == 0 && !getenv("B200TTS_NO_MN_MAJOR");
+    const bool a_mn_ready = a16ok && d.transA && d.kin == 0 && (d.lda16 % 64) == 0;
     const bool a_ready = (a16ok && !d.transA) || a_mn_ready;
     // MN-major operands (op(A) = A^T with A [K, M], op(B) = B [K, N]: weight gradients): the bf16 copy keeps the source's row-major
     // [K][MN] layout (a plain row conversion, no transpose; MN padded to 64) and is keyed exactly like the K-contiguous copy another product
     // makes of the same matrix, so e.g. the gate gradients are converted ONCE for their dX (K-major use) and dW (MN-major use) products
-    const bool a_mn = d.transA && !a_ready && d.batch == 1 && d.kin == 0 && !getenv("B200TTS_NO_MN_MAJOR");
-    const bool b_mn = !d.transB && d.batch == 1 && d.kin == 0 && !getenv("B200TTS_NO_MN_MAJOR");
+    const bool a_mn = d.transA && !a_ready && d.batch == 1 && d.kin == 0;
+    const bool b_mn = !d.transB && d.batch == 1 && d.kin == 0;
     const bool b_ready = b_mn && d.B16 != nullptr && (d.ldb16 % 64) == 0 && (reinterpret_cast<uintptr_t>(d.B16) & 15) == 0;
     const int Mp64 = (d.M + 63) / 64 * 64, Np64 = (d.N + 63) / 64 * 64;
     const size_t a_bytes = a_ready ? 0 : a_mn ? ((size_t)d.K * Mp64 * 2 + 1023) / 1024 * 1024 : ((size_t)abatch * d.M * Kp * 2 + 1023) / 1024 * 1024;
@@ -512,13 +495,7 @@ int gemm_tc_try(const GemmDesc& d, cudaStream_t st, bool* handled) {
     if (d.batch == 1)
         pick_ksplit(a, d.M, d.N, d.K, (g_cache_on ? g_cache_off : 0) + (pack_a ? a_bytes : 0) + (pack_b ? b_bytes : 0));
     B200_TRY(launch_gemm_tc(dim3(cdiv(d.N, TBN), cdiv(d.M, TBM), a.ksplit > 1 ? a.ksplit : d.batch), tmA, tmB, a, st));
-    if (a.ksplit > 1) {
-        const size_t total = (size_t)d.M * d.N;
-        int blocks = (int)((total + 255) / 256);
-        if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
-        tc_splitk_reduce_kernel<<<blocks, 256, 0, st>>>(a.partial, d.C, d.bias, d.M, d.N, d.ldc, a.ksplit, d.alpha, d.beta);
-        B200_LAUNCH_CHECK();
-    }
+    if (a.ksplit > 1) B200_TRY(splitk_reduce(a.partial, d.C, d.bias, d.M, d.N, d.ldc, 1, a.ksplit, 0, d.alpha, d.beta, st));
     *handled = true;
     return B200TTS_OK;
 }
@@ -599,13 +576,7 @@ int gemm_tc_conv_dw(const float* dz, const float* x, float* dweight, int NB, int
     a.ksplit = 1; a.kper = 0; a.partial = nullptr; a.a_mn = 0; a.b_mn = 0;
     if (G == 1) pick_ksplit(a, Cout, R, K, a_bytes + b_bytes);      // postnet convolutions: 16 .. 80 tiles over K = NB * L
     B200_TRY(launch_gemm_tc(dim3(cdiv(R, TBN), cdiv(Cout, TBM), a.ksplit > 1 ? a.ksplit : G), tmA, tmB, a, st));
-    if (a.ksplit > 1) {
-        const size_t total = (size_t)Cout * R;
-        int blocks = (int)((total + 255) / 256);
-        if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
-        tc_splitk_reduce_kernel<<<blocks, 256, 0, st>>>(a.partial, dweight, nullptr, Cout, R, R, a.ksplit, 1.f, 1.f);
-        B200_LAUNCH_CHECK();
-    }
+    if (a.ksplit > 1) B200_TRY(splitk_reduce(a.partial, dweight, nullptr, Cout, R, R, 1, a.ksplit, 0, 1.f, 1.f, st));
     *handled = true;
     return B200TTS_OK;
 }

@@ -14,7 +14,7 @@ returns NaN; so is all of C when beta == 0, and the bf16 columns the wgmma path 
 
 Routes (one kernel path each):
     f32       fp32 mode, gemm_run                    -> gemm_f32 (SIMT, k-block 16)
-    mma       bf16 mode, tensor-core GEMM off        -> gemm_bf16 (mma.sync, k-block 32)
+    mma       bf16 mode, tensor-core GEMM off        -> gemm_bf16_kernel (mma.sync, k-block 32)
     wgmma     bf16 mode, tensor-core GEMM on         -> gemm_tc_try (TMA + wgmma, k-block 64), mma.sync when it declines
     auto_f32  fp32 mode, gemm_run_auto               -> gemm_f32 with its own split-K factor
     auto_bf16 bf16 mode, gemm_run_auto               -> wgmma un-split, else mma.sync with its own split-K factor
@@ -292,7 +292,7 @@ def within(actual, expected, rtol, atol):
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
-# which kernels a route launches (host decisions of gemm_tc.cu / gemm_f32.cu, mirrored)
+# which kernels a route launches (host decisions of gemm_tc.cu / gemm.cu, mirrored)
 # ---------------------------------------------------------------------------------------------------------------------------
 def tc_plan(c, scratch_bytes, used0=0):
     """What gemm_tc_try does with c and a scratch of `scratch_bytes` whose first `used0` bytes hold cached packs (nothing cached for

@@ -91,12 +91,12 @@ def rn(x):
 
 def rw(w, mode):
     """A weight as the products read it: bf16 RN in both bf16 modes (decoder_persist_tc.cu:281, decoder_persist_bwd_tc.cu:114,
-    decoder_persist_bwd.cu:191 pack the resident slices that way; gemm_bf16.cu:83-91 packs every GEMM operand the same way)."""
+    decoder_persist_bwd.cu:191 pack the resident slices that way; gemm_bf16.cu:74-82 packs every GEMM operand the same way)."""
     return w.double() if mode == 'fp32' else rn(w)
 
 
 def ra(x, mode):
-    """An fp32 activation operand of a bf16-mode GEMM (gemm_bf16.cu:83-91); unrounded in fp32 mode."""
+    """An fp32 activation operand of a bf16-mode GEMM (gemm_bf16.cu:74-82); unrounded in fp32 mode."""
     return x.double() if mode == 'fp32' else rn(x)
 
 
