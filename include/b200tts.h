@@ -538,6 +538,20 @@ int b200tts_wavernn_fold(const b200tts_wavernn_fold_shape* shape, const float* m
                          const int32_t* row_utt, const int32_t* row_fold, const float* fir, const float* aux, int t0, int nsteps, float* feat,
                          void* stream);
 typedef struct {
+    int n_mels, aux_dims; /* feature columns, as in b200tts_wavernn_fold_shape */
+    int hop, pad, scale;
+    int frames;           /* the mel's frame count F once it is known (positions from F hop on are 0), 0 while the mel is still arriving */
+    long long m0;         /* the mel window holds samples [m0, m0 + mel_len) of the penultimate layer of the padded mel */
+    int mel_len;
+    int a0, aux_len;      /* the aux window holds frames [a0, a0 + aux_len) */
+} b200tts_wavernn_window_shape;
+/* feat [nsteps, n_mels + aux_dims] for the sample positions [s0, s0 + nsteps) of one unfolded row (one utterance, no folds): the columns
+ * b200tts_wavernn_fold writes for these positions, with the same arithmetic, read from windows: mel_win [n_mels, mel_len] holds the
+ * penultimate layer's samples [m0, m0 + mel_len) (equal to the whole padded mel's wherever they are read), aux_win [aux_len, aux_dims] the
+ * MelResNet output's frames [a0, a0 + aux_len).  B200TTS_ERR_INVALID when a read would fall outside a window. */
+int b200tts_wavernn_window(const b200tts_wavernn_window_shape* shape, const float* mel_win, const float* fir, const float* aux_win, long long s0,
+                           int nsteps, float* feat, void* stream);
+typedef struct {
     int rows;             /* fold rows of one loop */
     int rnn_dims;         /* R: a multiple of 128, at most 640 */
     int fc_dims;          /* a multiple of 128, at most 2048 */
@@ -578,6 +592,11 @@ int b200tts_wavernn_prepare(const b200tts_wavernn_shape* shape, const b200tts_wa
  * bf16(y2) and the logits.  A grid-barrier timeout (about 2 s) raises the abort flag and ends the launch: see b200tts_wavernn_aborted. */
 int b200tts_wavernn_run(const b200tts_wavernn_shape* shape, const b200tts_wavernn_params* params, const b200tts_wavernn_cond* cond, int t0,
                         int nsteps, const float* uniforms, float* out, float* dbg, void* workspace, size_t workspace_bytes, void* stream);
+/* A stream of unknown length: nsteps (at most shape->fold_len) more steps of every row after the t steps run since the last prepare, from the
+ * state left in the workspace, exactly as b200tts_wavernn_run would run steps [t, t + nsteps).  uniforms [rows, nsteps, U] and out
+ * [rows, nsteps] hold this call's steps only; cond as for b200tts_wavernn_run. */
+int b200tts_wavernn_run_stream(const b200tts_wavernn_shape* shape, const b200tts_wavernn_params* params, const b200tts_wavernn_cond* cond,
+                               long long t, int nsteps, const float* uniforms, float* out, void* workspace, size_t workspace_bytes, void* stream);
 /* Synchronises the stream and sets *aborted to the loop's abort flag (nonzero: a launch since the last prepare timed out). */
 int b200tts_wavernn_aborted(const b200tts_wavernn_shape* shape, const void* workspace, size_t workspace_bytes, int* aborted, void* stream);
 /* Optional de-emphasis of the loop's folded samples, in place, before b200tts_wavernn_unfold: each of `rows` rows of `len` samples is
@@ -618,6 +637,11 @@ int b200tts_gru_seq_forward(const b200tts_gru_seq_shape* shape, const float* gi,
  * receives every step's total dh = dh_ext + z dh_next + W_hh^T dgh_next.  One cooperative launch of 128 CTAs. */
 int b200tts_gru_seq_backward(const b200tts_gru_seq_shape* shape, const float* w_hh, const float* h, const void* saved, const float* dh_ext,
                              float* dgi, float* dgh, float* dh_dbg, void* workspace, size_t workspace_bytes, void* stream);
+/* A stream of unknown length: nsteps (at most shape->fold_len) more steps of every row after the t steps run since the last prepare, from the
+ * state left in the workspace, exactly as b200tts_wavernn_run would run steps [t, t + nsteps).  uniforms [rows, nsteps, U] and out
+ * [rows, nsteps] hold this call's steps only; cond as for b200tts_wavernn_run. */
+int b200tts_wavernn_run_stream(const b200tts_wavernn_shape* shape, const b200tts_wavernn_params* params, const b200tts_wavernn_cond* cond,
+                               long long t, int nsteps, const float* uniforms, float* out, void* workspace, size_t workspace_bytes, void* stream);
 /* Synchronises the stream and sets *aborted to the loops' abort flag (nonzero: a loop on this workspace timed out since it was zeroed). */
 int b200tts_gru_seq_aborted(const b200tts_gru_seq_shape* shape, const void* workspace, size_t workspace_bytes, int* aborted, void* stream);
 /* The adjoint of b200tts_wavernn_upsample_layer (C, len, scale, fir, in as there) for dout [C, len scale]: din [C, len] (overwritten; NULL:

@@ -94,6 +94,11 @@ class WaveRNNFoldShape(Structure):
     _fields_ = [(n, c_int) for n in ('B', 'rows', 'n_mels', 'aux_dims', 'hop', 'pad', 'scale', 'target', 'overlap', 'max_frames')]
 
 
+class WaveRNNWindowShape(Structure):
+    _fields_ = [(n, c_int) for n in ('n_mels', 'aux_dims', 'hop', 'pad', 'scale', 'frames')] + [('m0', c_longlong)] + \
+               [(n, c_int) for n in ('mel_len', 'a0', 'aux_len')]
+
+
 class WaveRNNShape(Structure):
     _fields_ = [(n, c_int) for n in ('rows', 'rnn_dims', 'fc_dims', 'n_out', 'mode', 'fold_len')]
 
@@ -206,10 +211,13 @@ SIGNATURES = {
     'b200tts_mel_cepstral_distortion': (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'b200tts_wavernn_upsample_layer': (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     'b200tts_wavernn_fold': (c_int, [POINTER(WaveRNNFoldShape)] + [c_void_p] * 7 + [c_int, c_int, c_void_p, c_void_p]),
+    'b200tts_wavernn_window': (c_int, [POINTER(WaveRNNWindowShape), c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_void_p, c_void_p]),
     'b200tts_wavernn_workspace_bytes': (c_size_t, [POINTER(WaveRNNShape)]),
     'b200tts_wavernn_prepare': (c_int, [POINTER(WaveRNNShape), POINTER(WaveRNNParams), c_void_p, c_size_t, c_void_p]),
     'b200tts_wavernn_run': (c_int, [POINTER(WaveRNNShape), POINTER(WaveRNNParams), POINTER(WaveRNNCond), c_int, c_int, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_size_t, c_void_p]),
+    'b200tts_wavernn_run_stream': (c_int, [POINTER(WaveRNNShape), POINTER(WaveRNNParams), POINTER(WaveRNNCond), c_longlong, c_int, c_void_p,
+                                           c_void_p, c_void_p, c_size_t, c_void_p]),
     'b200tts_wavernn_aborted': (c_int, [POINTER(WaveRNNShape), c_void_p, c_size_t, POINTER(c_int), c_void_p]),
     'b200tts_wavernn_deemphasis': (c_int, [c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
     'b200tts_wavernn_unfold': (c_int, [c_int] * 5 + [c_void_p] * 3 + [c_longlong, c_void_p, c_void_p, c_void_p]),

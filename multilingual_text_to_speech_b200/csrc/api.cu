@@ -202,6 +202,11 @@ int wavernn_upsample_layer_impl(int C, int len, int scale, const float* fir, con
 int wavernn_fold_check(const b200tts_wavernn_fold_shape& s, int t0, int nsteps);
 int wavernn_fold_impl(const b200tts_wavernn_fold_shape& s, const float* mel_up, const long long* mel_off, const int* frames, const int* row_utt,
                       const int* row_fold, const float* fir, const float* aux, int t0, int nsteps, float* feat, cudaStream_t st);
+int wavernn_window_check(const b200tts_wavernn_window_shape& s, long long s0, int nsteps);
+int wavernn_window_impl(const b200tts_wavernn_window_shape& s, const float* mel_up, const float* fir, const float* aux, long long s0, int nsteps,
+                        float* feat, cudaStream_t st);
+int wavernn_run_stream_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, const b200tts_wavernn_cond& cond, long long t,
+                            int nsteps, const float* uniforms, float* out, void* ws, size_t ws_bytes, cudaStream_t st);
 size_t wavernn_workspace_bytes(const b200tts_wavernn_shape& s);
 int wavernn_check(const b200tts_wavernn_shape& s, void* ws, size_t ws_bytes);
 int wavernn_prepare_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, void* ws, size_t ws_bytes, cudaStream_t st);
@@ -718,6 +723,14 @@ int b200tts_wavernn_fold(const b200tts_wavernn_fold_shape* shape, const float* m
     return wavernn_fold_impl(*shape, mel_up, reinterpret_cast<const long long*>(mel_off), frames, row_utt, row_fold, fir, aux, t0, nsteps, feat,
                              (cudaStream_t)stream);
 }
+int b200tts_wavernn_window(const b200tts_wavernn_window_shape* shape, const float* mel_win, const float* fir, const float* aux_win, long long s0,
+                           int nsteps, float* feat, void* stream) {
+    B200_REQUIRE(shape && mel_win && fir && feat, "wavernn_window: null argument");
+    B200_REQUIRE(aux_win || shape->aux_dims == 0, "wavernn_window: null aux");
+    B200_TRY(wavernn_window_check(*shape, s0, nsteps));
+    B200_TRY(require_device());
+    return wavernn_window_impl(*shape, mel_win, fir, aux_win, s0, nsteps, feat, (cudaStream_t)stream);
+}
 size_t b200tts_wavernn_workspace_bytes(const b200tts_wavernn_shape* shape) {
     if (!shape) { set_last_error("wavernn_workspace_bytes: null shape"); return 0; }
     return wavernn_workspace_bytes(*shape);
@@ -735,6 +748,13 @@ int b200tts_wavernn_run(const b200tts_wavernn_shape* shape, const b200tts_wavern
     B200_TRY(wavernn_check(*shape, workspace, workspace_bytes));
     B200_TRY(require_device());
     return wavernn_run_impl(*shape, *params, *cond, t0, nsteps, uniforms, out, dbg, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_wavernn_run_stream(const b200tts_wavernn_shape* shape, const b200tts_wavernn_params* params, const b200tts_wavernn_cond* cond,
+                               long long t, int nsteps, const float* uniforms, float* out, void* workspace, size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(shape && params && cond, "wavernn_run_stream: null argument");
+    B200_TRY(wavernn_check(*shape, workspace, workspace_bytes));
+    B200_TRY(require_device());
+    return wavernn_run_stream_impl(*shape, *params, *cond, t, nsteps, uniforms, out, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 int b200tts_wavernn_aborted(const b200tts_wavernn_shape* shape, const void* workspace, size_t workspace_bytes, int* aborted, void* stream) {
     B200_REQUIRE(shape && aborted, "wavernn_aborted: null argument");

@@ -5,6 +5,8 @@
 //   * wavernn_fold_kernel: the last layer of the mel path evaluated at the positions a chunk of the sample loop needs, the `indent` cut, the
 //     nearest stretch of the MelResNet output (aux) and fold_with_overlap, as the [steps, rows, n_mels + aux_dims] rows of the conditioning
 //     GEMMs (the products that do not depend on the previous sample run in the library GEMM before the loop);
+//   * wavernn_window_kernel: the same rows for consecutive sample positions of one unfolded row, read from windows of the penultimate mel
+//     layer and of aux (streaming generation, where the mel arrives in chunks);
 //   * wavernn_loop_kernel: the persistent sample loop, one cooperative launch per chunk of steps (below);
 //   * wavernn_unfold_kernel: mu-law decode, the square-root cross-fades, overlap-add, the cut to (F - 1) hop samples and the linear fade-out.
 //
@@ -22,6 +24,7 @@
 // with a grid barrier after each stage: six per sample.  h1 and h2 are double-buffered by step parity (stage 1 / 2 of step t reads the
 // previous step's rows while owners write this step's).  fp32 state (h1, h2, x1, prev) is only read by its owner.
 #include <cuda_bf16.h>
+#include <climits>
 #include <math.h>
 #include "decoder_internal.cuh"
 #include "tc_ptx.cuh"
@@ -92,6 +95,36 @@ __global__ void wavernn_fold_kernel(b200tts_wavernn_fold_shape s, const float* _
     }
 }
 
+// feat[i, :] for the sample positions q = s0 + i of one unfolded row (zero for q >= F hop once F is known): wavernn_fold_kernel's arithmetic,
+// with the penultimate layer read from a window x [n_mels, mel_len] that holds its samples [m0, m0 + mel_len), and aux from a window
+// [aux_len, aux_dims] that holds frames [a0, a0 + aux_len).  lo bounds the whole last layer ((F + 2 pad) hop, or past every read while F
+// is unknown); the host checks that every read falls inside the windows.
+__global__ void wavernn_window_kernel(b200tts_wavernn_window_shape s, long long lo, const float* __restrict__ x, const float* __restrict__ fir,
+                                      const float* __restrict__ aux, long long s0, int nsteps, float* __restrict__ feat) {
+    const int D = s.n_mels + s.aux_dims;
+    const long long n = (long long)nsteps * D;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < n; idx += (long long)gridDim.x * blockDim.x) {
+        const int col = (int)(idx % D);
+        const long long q = s0 + idx / D;
+        float v = 0.f;
+        if (s.frames == 0 || q < (long long)s.frames * s.hop) {
+            if (col < s.n_mels) {
+                const float* xc = x + (size_t)col * s.mel_len;
+                const long long p = q + (long long)s.pad * s.hop;
+                float acc = 0.f;
+                for (int k = -s.scale; k <= s.scale; ++k) {
+                    const long long j = p + k;
+                    if (j >= 0 && j < lo) acc = fmaf(fir[k + s.scale], xc[j / s.scale - s.m0], acc);
+                }
+                v = acc;
+            } else {
+                v = aux[(size_t)(q / s.hop - s.a0) * s.aux_dims + (col - s.n_mels)];
+            }
+        }
+        feat[idx] = v;
+    }
+}
+
 // ---- the sample loop ----
 struct WrDims {
     int R, Fc, n_out, U, V, O;
@@ -144,6 +177,7 @@ __global__ void wavernn_pack_kernel(WrDims d, WrWeights W, uint4* __restrict__ p
 struct WrLoopArgs {
     WrDims d;
     int rows, mode, L, t0, nsteps;
+    int io0;              // step of uniforms / out column 0: 0 for a fold, t0 for a stream call (whose columns are its own steps)
     const uint4* packed;
     const float *b_hh1, *u1, *w_prev, *b_hh2, *b_fc3;
     const float *cc, *g1, *c2, *p1, *p2;
@@ -210,7 +244,7 @@ __global__ void __launch_bounds__(WR_THREADS, 1) wavernn_loop_kernel(WrLoopArgs 
     unsigned target = 0;
 
     for (int i = 0; i < a.nsteps; ++i) {
-        const int tg = a.t0 + i;
+        const int tg = a.t0 + i, ti = tg - a.io0;
         const int cur = tg & 1, prv = cur ^ 1;
         float* dbg = a.dbg ? a.dbg + (size_t)i * rows * Ddbg : nullptr;
         // 1. GRU1
@@ -312,7 +346,7 @@ __global__ void __launch_bounds__(WR_THREADS, 1) wavernn_loop_kernel(WrLoopArgs 
             float sample;
             if (a.mode == B200TTS_WAVERNN_RAW) {
                 const int n = d.n_out, per = (n + 31) / 32, k0 = lane * per, k1 = min(n, k0 + per);
-                const float u = a.uni[(size_t)row * a.L + tg];
+                const float u = a.uni[(size_t)row * a.L + ti];
                 float mx = -INFINITY;
                 for (int k = k0; k < k1; ++k) mx = fmaxf(mx, __ldcg(lg + k));
                 mx = warp_max(mx);
@@ -342,7 +376,7 @@ __global__ void __launch_bounds__(WR_THREADS, 1) wavernn_loop_kernel(WrLoopArgs 
                 sample = 2.f * (float)k / (float)(n - 1) - 1.f;
             } else {
                 const int nr = d.n_out / 3, U1 = nr + 1;
-                const float* uu = a.uni + ((size_t)row * a.L + tg) * U1;
+                const float* uu = a.uni + ((size_t)row * a.L + ti) * U1;
                 // bi starts as a valid component on every lane and only ever takes another lane's bi: it stays in [0, nr) even when
                 // NaN scores make every comparison false, so the loads below stay inside the row's logits
                 float best = -INFINITY;
@@ -364,7 +398,7 @@ __global__ void __launch_bounds__(WR_THREADS, 1) wavernn_loop_kernel(WrLoopArgs 
             }
             if (lane == 0) {
                 a.prev[row] = sample;
-                a.out[(size_t)row * a.L + tg] = sample;
+                a.out[(size_t)row * a.L + ti] = sample;
             }
         }
         if (!grid_barrier(a.bar, target, gridDim.x, a.abort_flag, &s_ok, false)) return;
@@ -513,19 +547,17 @@ int wavernn_prepare_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_p
     return B200TTS_OK;
 }
 
-int wavernn_run_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, const b200tts_wavernn_cond& cond, int t0, int nsteps,
-                     const float* uniforms, float* out, float* dbg, void* ws, size_t ws_bytes, cudaStream_t st) {
-    B200_TRY(wavernn_check(s, ws, ws_bytes));
+// steps [t0, t0 + nsteps) from the state in the workspace; uniforms / out rows of L columns, column 0 at step io0
+static int wavernn_launch(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, const b200tts_wavernn_cond& cond, int t0, int io0,
+                          int L, int nsteps, const float* uniforms, float* out, float* dbg, void* ws, cudaStream_t st) {
     B200_REQUIRE(p.b_hh1 && p.u1 && p.w_prev && p.b_hh2 && p.b_fc3, "wavernn_run: null parameter");
     B200_REQUIRE(cond.c && cond.g1 && cond.c2 && cond.p1 && cond.p2, "wavernn_run: null conditioning");
     B200_REQUIRE(uniforms && out, "wavernn_run: null uniforms or output");
-    B200_REQUIRE(t0 >= 0 && nsteps >= 1 && t0 + nsteps <= s.fold_len, "wavernn_run: steps [%d, %d) outside the fold length %d", t0, t0 + nsteps,
-                 s.fold_len);
     const WrLayout l = wr_layout(s);
     unsigned char* base = static_cast<unsigned char*>(ws);
     WrLoopArgs a;
     a.d = wr_dims(s.rnn_dims, s.fc_dims, s.n_out);
-    a.rows = s.rows; a.mode = s.mode; a.L = s.fold_len; a.t0 = t0; a.nsteps = nsteps;
+    a.rows = s.rows; a.mode = s.mode; a.L = L; a.t0 = t0; a.io0 = io0; a.nsteps = nsteps;
     a.packed = reinterpret_cast<const uint4*>(base + l.packed);
     a.b_hh1 = p.b_hh1; a.u1 = p.u1; a.w_prev = p.w_prev; a.b_hh2 = p.b_hh2; a.b_fc3 = p.b_fc3;
     a.cc = cond.c; a.g1 = cond.g1; a.c2 = cond.c2; a.p1 = cond.p1; a.p2 = cond.p2;
@@ -546,6 +578,24 @@ int wavernn_run_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_param
     B200_CUDA(cudaMemsetAsync(a.bar, 0, sizeof(unsigned), st));       // the abort flag persists until the next prepare
     void* params[] = {&a};
     return launch_persistent("wavernn_loop", (const void*)wavernn_loop_kernel, WR_CTAS, WR_THREADS, (size_t)a.d.per_cta * 16, false, params, st);
+}
+
+int wavernn_run_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, const b200tts_wavernn_cond& cond, int t0, int nsteps,
+                     const float* uniforms, float* out, float* dbg, void* ws, size_t ws_bytes, cudaStream_t st) {
+    B200_TRY(wavernn_check(s, ws, ws_bytes));
+    B200_REQUIRE(t0 >= 0 && nsteps >= 1 && t0 + nsteps <= s.fold_len, "wavernn_run: steps [%d, %d) outside the fold length %d", t0, t0 + nsteps,
+                 s.fold_len);
+    return wavernn_launch(s, p, cond, t0, 0, s.fold_len, nsteps, uniforms, out, dbg, ws, st);
+}
+
+int wavernn_run_stream_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, const b200tts_wavernn_cond& cond, long long t,
+                            int nsteps, const float* uniforms, float* out, void* ws, size_t ws_bytes, cudaStream_t st) {
+    B200_TRY(wavernn_check(s, ws, ws_bytes));
+    B200_REQUIRE(t >= 0 && nsteps >= 1 && nsteps <= s.fold_len, "wavernn_run_stream: %d steps after %lld (at most fold_len = %d per call)",
+                 nsteps, t, s.fold_len);
+    // the loop only needs the step's parity (which slot of the double-buffered h1 / h2 rows is the previous step's)
+    const int t0 = (int)(t & 1);
+    return wavernn_launch(s, p, cond, t0, t0, nsteps, nsteps, uniforms, out, nullptr, ws, st);
 }
 
 int wavernn_aborted_impl(const b200tts_wavernn_shape& s, const void* ws, size_t ws_bytes, int* aborted, cudaStream_t st) {
@@ -588,6 +638,40 @@ int wavernn_fold_impl(const b200tts_wavernn_fold_shape& s, const float* mel_up, 
     KernelTimer kt("wavernn_fold", st);
     wavernn_fold_kernel<<<grid_for((size_t)nsteps * s.rows * (s.n_mels + s.aux_dims)), 256, 0, st>>>(s, mel_up, mel_off, frames, row_utt, row_fold,
                                                                                                     fir, aux, t0, nsteps, feat);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+// every read of the positions [s0, s0 + nsteps) must fall inside the windows
+int wavernn_window_check(const b200tts_wavernn_window_shape& s, long long s0, int nsteps) {
+    B200_REQUIRE(s.n_mels >= 1 && s.aux_dims >= 0 && s.frames >= 0 && s.mel_len >= 1 && s.aux_len >= 0 && s.m0 >= 0 && s.a0 >= 0,
+                 "wavernn_window: bad dimensions (n_mels = %d, aux_dims = %d, frames = %d, mel_len = %d, aux_len = %d, m0 = %lld, a0 = %d)",
+                 s.n_mels, s.aux_dims, s.frames, s.mel_len, s.aux_len, s.m0, s.a0);
+    B200_REQUIRE(s.hop >= 1 && s.scale >= 1 && s.hop % s.scale == 0 && s.pad >= 0,
+                 "wavernn_window: the hop %d must be a multiple of the last upsampling factor %d (pad %d)", s.hop, s.scale, s.pad);
+    B200_REQUIRE(s0 >= 0 && nsteps >= 1, "wavernn_window: positions [%lld, %lld)", s0, s0 + nsteps);
+    long long q1 = s0 + nsteps;                          // positions [s0, q1) read the windows
+    if (s.frames > 0 && q1 > (long long)s.frames * s.hop) q1 = (long long)s.frames * s.hop;
+    if (q1 <= s0) return B200TTS_OK;
+    const long long lo = s.frames > 0 ? (long long)(s.frames + 2 * s.pad) * s.hop : LLONG_MAX;
+    long long j0 = s0 + (long long)s.pad * s.hop - s.scale, j1 = q1 - 1 + (long long)s.pad * s.hop + s.scale;
+    if (j0 < 0) j0 = 0;
+    if (j1 > lo - 1) j1 = lo - 1;
+    B200_REQUIRE(j0 / s.scale >= s.m0 && j1 / s.scale < s.m0 + s.mel_len,
+                 "wavernn_window: positions [%lld, %lld) read penultimate samples [%lld, %lld], outside the window [%lld, %lld)", s0, q1,
+                 j0 / s.scale, j1 / s.scale, s.m0, s.m0 + s.mel_len);
+    B200_REQUIRE(s.aux_dims == 0 || (s0 / s.hop >= s.a0 && (q1 - 1) / s.hop < (long long)s.a0 + s.aux_len),
+                 "wavernn_window: positions [%lld, %lld) read aux frames [%lld, %lld], outside the window [%d, %d)", s0, q1, s0 / s.hop,
+                 (q1 - 1) / s.hop, s.a0, s.a0 + s.aux_len);
+    return B200TTS_OK;
+}
+
+int wavernn_window_impl(const b200tts_wavernn_window_shape& s, const float* mel_up, const float* fir, const float* aux, long long s0, int nsteps,
+                        float* feat, cudaStream_t st) {
+    B200_TRY(wavernn_window_check(s, s0, nsteps));
+    KernelTimer kt("wavernn_window", st);
+    const long long lo = s.frames > 0 ? (long long)(s.frames + 2 * s.pad) * s.hop : LLONG_MAX;
+    wavernn_window_kernel<<<grid_for((size_t)nsteps * (s.n_mels + s.aux_dims)), 256, 0, st>>>(s, lo, mel_up, fir, aux, s0, nsteps, feat);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }

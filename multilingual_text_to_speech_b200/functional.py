@@ -898,6 +898,17 @@ def wavernn_fold(shape, mel_up, mel_off, frames, row_utt, row_fold, fir, aux, t0
     return out
 
 
+def wavernn_window(shape, mel_win, fir, aux_win, s0, nsteps):
+    """feat [nsteps, n_mels + aux_dims] of the sample positions [s0, s0 + nsteps) of one unfolded row, from the windows (shape: a
+    _lib.WaveRNNWindowShape)."""
+    _require_cuda(mel_win, fir, aux_win)
+    mel_win, aux_win = _f32c(mel_win), _f32c(aux_win)
+    out = torch.empty(int(nsteps), shape.n_mels + shape.aux_dims, device=mel_win.device, dtype=torch.float32)
+    check(_lib.load().b200tts_wavernn_window(ctypes.byref(shape), ptr(mel_win), ptr(_f32c(fir)), ptr(aux_win), int(s0), int(nsteps), ptr(out),
+                                             _stream()), 'b200tts_wavernn_window')
+    return out
+
+
 def wavernn_workspace(shape, device):
     """Workspace of the sample loop for `shape` (a _lib.WaveRNNShape); raises on an invalid shape."""
     n = _lib.load().b200tts_wavernn_workspace_bytes(ctypes.byref(shape))
@@ -923,6 +934,14 @@ def wavernn_run(shape, params, cond, t0, nsteps, uniforms, out, ws, dbg=None):
     cs = _lib.WaveRNNCond(*[ptr(t) for t in cond])
     check(_lib.load().b200tts_wavernn_run(ctypes.byref(shape), ctypes.byref(params), ctypes.byref(cs), int(t0), int(nsteps), ptr(uniforms),
                                           ptr(out), ptr(dbg), ptr(ws), ws.numel(), _stream()), 'b200tts_wavernn_run')
+
+
+def wavernn_run_stream(shape, params, cond, t, nsteps, uniforms, out, ws):
+    """nsteps more loop steps after the t run since the last prepare; uniforms [rows, nsteps, U] and out [rows, nsteps] hold this call's
+    steps only."""
+    cs = _lib.WaveRNNCond(*[ptr(t_) for t_ in cond])
+    check(_lib.load().b200tts_wavernn_run_stream(ctypes.byref(shape), ctypes.byref(params), ctypes.byref(cs), int(t), int(nsteps), ptr(uniforms),
+                                                 ptr(out), ptr(ws), ws.numel(), _stream()), 'b200tts_wavernn_run_stream')
 
 
 def wavernn_aborted(shape, ws):

@@ -56,6 +56,10 @@ class Postnet(torch.nn.Module):
             block._mask_key = f'post{j}'
         self._convs = Sequential(*blocks)
 
+    def halo(self):
+        """Frames on each side of an output frame that it depends on: the blocks' reaches added up."""
+        return sum((block._kernel - 1) * block._dilation // 2 for block in self._convs)
+
     def forward(self, x, x_lengths, padded=False):
         """padded (eval only): every frame of x at or after x_lengths[b] is 0, and so is every block output there."""
         if padded:
@@ -213,16 +217,14 @@ class Decoder(torch.nn.Module):
         """Positions (into `rows`, the original indices of the utterances still decoding) of the utterances whose stop cut is unknown."""
         return [j for j, r in enumerate(rows) if rules[r].cut is None]
 
-    def _decode_inference(self, encoded_input, mask, speaker, language, att_extent=0, tape_columns=None):
-        """Free-running decode in chunks with carried state and early exit (tacotron2.py:148-209 with target=None): every chunk is one
-        library call; between chunks the stop rule reads the chunk's stop logits.  B == 1 reproduces the reference; B > 1 (which the
-        reference cannot run: it uses the stop token as a Python bool) keeps one stop rule per utterance, and an utterance whose cut is
-        known leaves the decode: the state, memory, lengths and rules are compacted to the utterances still running, and the next
-        chunk runs at the smaller batch.  `att_extent` = 1 runs forward attention over each utterance's own length; `tape_columns`
-        gives each utterance's column of a recorded mask tape (default: column b for utterance b).
-        -> (spectrogram [B, T', N], stop [B, T'], alignment [B, ceil(T' / r), L], cuts): T' = max(cuts) frames; utterance b is zero past
-        cuts[b] (its alignment past ceil(cuts[b] / r) steps).  The stop rule reads the r stop logits of each step in frame order, and
-        hp.max_output_length counts frames."""
+    def _inference_chunks(self, encoded_input, mask, speaker, language, att_extent=0, tape_columns=None, chunk_frames=None):
+        """The chunk loop of free-running inference (tacotron2.py:148-209 with target=None): every chunk is one library call of
+        chunk_frames (default inference_chunk) frames rounded down to whole steps; after each it feeds the chunk's stop logits to the
+        utterances' stop rules and yields (rows, spec [b, Tc, N], stop [b, Tc], alignment [b, Tc / r, L], rules, done): rows are the
+        original indices of the b utterances the chunk decoded, rules the stop rule of every utterance, done the frames decoded so far.
+        Then an utterance whose cut is known leaves the decode: the state, memory, lengths and rules are compacted to the utterances still
+        running, and the next chunk runs at the smaller batch.  The loop ends when every cut is known or hp.max_output_length frames are
+        decoded.  The rule reads the r stop logits of each step in frame order."""
         memory = self._memory(encoded_input, speaker, language)
         B, L, M = memory.shape
         device = memory.device
@@ -233,11 +235,10 @@ class Decoder(torch.nn.Module):
         rules = [self._StopRule(hp.stop_frames) for _ in range(B)]
         rows = list(range(B))                  # original index of every utterance still decoding
         columns = list(range(B)) if tape_columns is None else list(tape_columns)
-        outs = [[] for _ in range(B)]
         done = 0                               # frames decoded (a whole number of steps)
         params = self._param_list()
         r = self._outputs_per_step
-        chunk_steps = max(1, self.inference_chunk // r)
+        chunk_steps = max(1, (self.inference_chunk if chunk_frames is None else int(chunk_frames)) // r)
         while done < self._max_frames:
             Sc = min(chunk_steps, self._steps(self._max_frames - done))
             Tc = Sc * r
@@ -263,7 +264,7 @@ class Decoder(torch.nn.Module):
             host_stop = stop.float().cpu()
             for j, u in enumerate(rows):
                 rules[u].feed(host_stop[j])
-                outs[u].append((spec[j], stop[j], align[j]))
+            yield rows, spec, stop, align, rules, done
             keep = self._retire(rows, rules)
             if not keep:
                 break
@@ -272,6 +273,22 @@ class Decoder(torch.nn.Module):
                 state.select(idx)
                 memory, lengths = memory.index_select(0, idx), lengths.index_select(0, idx)
                 rows = [rows[j] for j in keep]
+
+    def _decode_inference(self, encoded_input, mask, speaker, language, att_extent=0, tape_columns=None):
+        """Free-running decode in chunks with carried state and early exit (_inference_chunks).  B == 1 reproduces the reference; B > 1
+        (which the reference cannot run: it uses the stop token as a Python bool) keeps one stop rule per utterance.  `att_extent` = 1 runs
+        forward attention over each utterance's own length; `tape_columns` gives each utterance's column of a recorded mask tape (default:
+        column b for utterance b).
+        -> (spectrogram [B, T', N], stop [B, T'], alignment [B, ceil(T' / r), L], cuts): T' = max(cuts) frames; utterance b is zero past
+        cuts[b] (its alignment past ceil(cuts[b] / r) steps).  hp.max_output_length counts frames."""
+        B, L = encoded_input.shape[0], encoded_input.shape[1]
+        device = encoded_input.device
+        N = self._output_dim
+        outs = [[] for _ in range(B)]
+        done = 0
+        for rows, spec, stop, align, rules, done in self._inference_chunks(encoded_input, mask, speaker, language, att_extent, tape_columns):
+            for j, u in enumerate(rows):
+                outs[u].append((spec[j], stop[j], align[j]))
         cuts = [min(rule.cut if rule.cut is not None else done, self._max_frames) for rule in rules]
         ends = lambda cut: (cut, cut, self._steps(cut))       # noqa: E731 -- rows kept of spectrogram, stop (frames), alignment (steps)
         if B == 1:
@@ -436,7 +453,52 @@ class Tacotron(torch.nn.Module):
             self.train(was_training)
         return outputs
 
-    def _inference_group(self, texts, speakers, languages, tape_columns):
+    def inference_stream(self, text, speaker=None, language=None, chunk_frames=None):
+        """Streaming `inference`: a generator of post-net spectrogram chunks [num_mels, n_k] whose concatenation is inference(text,
+        speaker, language), the same stop cut and, given the same prenet dropout masks, the same decoded frames.  Takes the inputs
+        `inference` takes.  The decoder runs in chunks of chunk_frames frames (default Decoder.inference_chunk, rounded down to whole
+        decoder steps); after every chunk one item is yielded: the post-net over the frames that became final (stream_release), computed
+        over a window with the post-net's halo of decoded frames on the left and, once the cut is known, the zeros past it on the right.
+        An item may hold no frames (a chunk shorter than the halo).  The model is in eval mode, without autograd, until the generator
+        ends or is closed; prenet dropout stays on, as in `inference`, and a MaskSource tape is replayed the same way."""
+        speakers, languages = _check_batch_inputs([text], None if speaker is None else [speaker], None if language is None else [language])
+        if chunk_frames is not None and int(chunk_frames) < 1:
+            raise ValueError(f'inference_stream: chunk_frames must be >= 1 (got {chunk_frames})')
+        was_training = self.training
+        self.eval()
+        try:
+            with torch.no_grad():
+                encoded, mask, speaker, language = self._encode_group([text], speakers, languages)
+            dec, halo = self._decoder, self._postnet.halo()
+            pre, released = [], 0
+            chunks = dec._inference_chunks(encoded, mask, speaker, language, att_extent=1, tape_columns=[0], chunk_frames=chunk_frames)
+            while True:
+                with torch.no_grad():
+                    item = next(chunks, None)
+                    if item is None:
+                        return
+                    _, spec, _, _, rules, done = item
+                    pre.append(spec[0])
+                    end = stream_release(done, rules[0].cut, dec._max_frames, halo)
+                    final = rules[0].cut is not None or done >= dec._max_frames
+                    post = self._postnet_window(torch.cat(pre, 0), released, end, halo, end if final else done)
+                released = end
+                yield post
+        finally:
+            self.train(was_training)
+
+    def _postnet_window(self, pre, t0, t1, halo, avail):
+        """Post-net output frames [t0, t1) [num_mels, t1 - t0] from the decoded frames pre [>= avail, N], of which the first `avail` count
+        (the rest lie past the stop cut): run over frames [t0 - halo, t1 + halo) within [0, avail), zero-padded at the window's ends."""
+        w0, w1 = postnet_window(t0, t1, halo, avail)
+        if t1 <= t0:
+            return pre.new_zeros(pre.shape[1], 0)
+        x = pre[w0:w1].t().unsqueeze(0).contiguous()
+        post = self._postnet(x, torch.tensor([w1 - w0], device=x.device), padded=True)
+        return post[0, :, t0 - w0:t1 - w0]
+
+    def _encode_group(self, texts, speakers, languages):
+        """Padded batch of texts -> (encoder output, mask, speaker, language) in the decoder's forms."""
         device = self._embedding.weight.device
         B, Lmax = len(texts), max(int(t.shape[0]) for t in texts)
         lengths = torch.tensor([int(t.shape[0]) for t in texts], device=device)
@@ -459,10 +521,31 @@ class Tacotron(torch.nn.Module):
         encoded = self._encoder(embedded, lengths, language, padded=True)
         if language is not None and language.dim() == 3:
             language = torch.argmax(language, dim=2)  # one-hot into indices for the decoder's language embedding
-        mask = lengths_to_mask(lengths, Lmax)
+        return encoded, lengths_to_mask(lengths, Lmax), speaker, language
+
+    def _inference_group(self, texts, speakers, languages, tape_columns):
+        device = self._embedding.weight.device
+        encoded, mask, speaker, language = self._encode_group(texts, speakers, languages)
+        B = len(texts)
         prediction, _, _, cuts = self._decoder._decode_inference(encoded, mask, speaker, language, att_extent=1, tape_columns=tape_columns)
         post = self._postnet(prediction.transpose(1, 2), torch.tensor(cuts, device=device), padded=True)
         return [post[b, :, :cuts[b]] for b in range(B)]
+
+
+def stream_release(done, cut, max_frames, halo):
+    """Frames of a streamed utterance whose post-net output is final after `done` decoded frames: every frame up to the stop cut once it is
+    known (or up to max_frames once the decode has reached it), else every frame with `halo` decoded frames to its right."""
+    if cut is not None:
+        return min(cut, max_frames)
+    if done >= max_frames:
+        return max_frames
+    return max(done - halo, 0)
+
+
+def postnet_window(t0, t1, halo, avail):
+    """The decoded frames [w0, w1) the post-net runs over to produce its final frames [t0, t1), of `avail` decoded frames (the whole
+    utterance once the cut is known): `halo` frames on each side, clipped to the decoded ones."""
+    return max(t0 - halo, 0), min(t1 + halo, avail)
 
 
 def _check_batch_inputs(texts, speakers, languages):

@@ -18,6 +18,8 @@ Stages of forward (training, with autograd):
     stage; conv_out and every linear layer on the library GEMM; the aux stretch and the mel path's layers with their library adjoints;
   * both GRUs on the persistent fp32 sequence loops (b200tts_gru_seq_forward / _backward);
   * wavernn_loss: one fused kernel per mode writes the loss and d logits."""
+import contextlib
+
 import numpy as np
 import torch
 from torch import nn
@@ -307,6 +309,104 @@ class WaveRNN(nn.Module):
                 out.append(w if mels[i].is_cuda else w.cpu())
         return out
 
+    # ---- streaming ----
+    def generate_stream(self, mel_chunks, uniforms=None, generator=None, preemphasis=0.0):
+        """Streaming form of generate(mel, target=F hop, overlap=0), fatchord's unbatched generation: mel_chunks is an iterable of
+        [feat_dims, n_k] mels (n_k >= 0, as given: no normalisation), whose concatenation is the mel of F >= 21 frames; yields waveform
+        chunks whose concatenation is that call's (F - 1) hop samples, bit for bit given the same uniform tape.  A sample's loop features are
+        final once lookahead() frames follow its frame, so the loop runs up to there after each input chunk; the last 20 hops it has run are
+        held back until the input ends, because the fade-out lands on them.  uniforms: the tape [1, T, U] of generate (step t reads
+        uniforms[0, t]; T >= (F - 1) hop), by default drawn with torch.rand per call of the loop (`generator` optional).  preemphasis as in
+        generate_batch, de-emphasised sequentially across chunks: within fp32 roundings of the one-shot call, not bit for bit.  Runs on the
+        device of the first CUDA chunk, or the current CUDA device, in fp32 (the precision mode is set for each stretch of work and restored
+        before every yield).  Chunks come out as the first chunk went in: numpy, CUDA tensors, or CPU tensors."""
+        if not -1.0 < float(preemphasis) < 1.0:
+            raise ValueError(f'preemphasis {preemphasis} must lie in (-1, 1)')
+        tape = self._check_stream_tape(uniforms)
+        st = None
+        for i, chunk in enumerate(mel_chunks):
+            spec, as_numpy = self._check_chunk(chunk, i)
+            if st is None:
+                st = _Stream(self, spec.device if spec.is_cuda else None, as_numpy, not as_numpy and spec.is_cuda, tape, generator, preemphasis)
+            if spec.shape[1]:
+                out = st.feed(spec)
+                if out is not None:
+                    yield out
+        if st is None or st.frames < 21:
+            raise ValueError(f'the mel stream ended after {0 if st is None else st.frames} frames; the 20-hop fade-out needs at least 21')
+        yield st.finish()
+
+    def lookahead(self):
+        """Frames past a sample's own frame that its loop features read: `pad` for conv_in (the rest of the MelResNet is pointwise) or the
+        reach of the mel path's stretch + FIR layers, whichever is larger."""
+        return max(self.pad, self._mel_path_reads(0, self.hop_length)[-1][1] - self.pad)
+
+    def _mel_path_reads(self, s0, s1):
+        """Inclusive index ranges that the features of sample positions [s0, s1) read, layer by layer from the last mel-path layer's input
+        down to the padded mel's frames: a stretch + FIR layer of scale s reads its input at (i + k) // s for |k| <= s."""
+        lo, hi = s0 + self.pad * self.hop_length, s1 - 1 + self.pad * self.hop_length
+        out = []
+        for scale in reversed(self.upsample_factors):
+            lo, hi = lo // scale - 1, hi // scale + 1
+            out.append((lo, hi))
+        return out
+
+    def window_plan(self, s0, s1, known, final):
+        """The windows the features of sample positions [s0, s1) are computed from, with `known` mel frames arrived (`final`: the whole
+        mel): the padded-mel frames [P0, P1) the mel path runs over, the mel frames [r0, r1) the MelResNet runs over, and the aux frames
+        [a0, a1) the features read.  Outside the mel's ends both run on the zero padding the whole-mel computation sees; elsewhere each
+        window reaches as far as the reads do, so the values read equal the whole mel's."""
+        p, hop = self.pad, self.hop_length
+        P0, P1 = self._mel_path_reads(s0, s1)[-1]
+        P0, P1 = max(P0, 0), P1 + 1
+        a0, a1 = s0 // hop, (s1 - 1) // hop + 1
+        r0, r1 = max(a0 - p, 0), a1 + p
+        if final:
+            P1, r1 = min(P1, known + 2 * p), min(r1, known)
+        elif P1 - p > known or r1 > known:
+            raise ValueError(f'positions [{s0}, {s1}) read mel frames past the {known} that have arrived')
+        return (P0, P1), (r0, r1), (a0, a1)
+
+    def window_features(self, mel, s0, s1, final):
+        """Loop features [s1 - s0, feat_dims + res_out_dims] of sample positions [s0, s1) from the mel frames that have arrived, mel
+        [feat_dims, known] on the device (final: the whole mel): equal, bit for bit, to b200tts_wavernn_fold's at these positions."""
+        known, p, hop, s_last = int(mel.shape[1]), self.pad, self.hop_length, self.upsample_factors[-1]
+        (P0, P1), (r0, r1), _ = self.window_plan(s0, s1, known, final)
+        device = mel.device
+        win = torch.zeros(self.feat_dims, P1 - P0, device=device, dtype=torch.float32)
+        lo, hi = max(P0, p), min(P1, known + p)
+        win[:, lo - P0:hi - P0] = mel[:, lo - p:hi - p]
+        mel_up = self._mel_path(win, device)
+        aux = self._resnet(mel[:, r0:r1].unsqueeze(0).contiguous(), [r1 - r0], device)[0]
+        shape = _lib.WaveRNNWindowShape(self.feat_dims, aux.shape[1], hop, p, s_last, known if final else 0, P0 * (hop // s_last),
+                                        mel_up.shape[1], r0, r1 - r0)
+        fir = self.upsample.up_layers[-1].weight.detach().reshape(-1).to(device=device, dtype=torch.float32).contiguous()
+        return F.wavernn_window(shape, mel_up, fir, aux, s0, s1 - s0)
+
+    def _check_chunk(self, chunk, i):
+        as_numpy = not isinstance(chunk, torch.Tensor)
+        t = torch.as_tensor(np.asarray(chunk) if as_numpy else chunk)
+        if t.dim() != 2 or t.shape[0] != self.feat_dims:
+            raise ValueError(f'mel chunk {i} has shape {tuple(t.shape)}; expected [{self.feat_dims}, frames]')
+        if not torch.is_floating_point(t):
+            raise ValueError(f'mel chunk {i} is not floating point')
+        if not bool(torch.isfinite(t).all()):
+            raise ValueError(f'mel chunk {i} has non-finite values')
+        return t, as_numpy
+
+    def _check_stream_tape(self, uniforms):
+        if uniforms is None:
+            return None
+        u = torch.as_tensor(np.asarray(uniforms) if not isinstance(uniforms, torch.Tensor) else uniforms)
+        U = self.uniforms_per_step()
+        if u.dim() != 3 or u.shape[0] != 1 or u.shape[2] != U:
+            raise ValueError(f'uniform tape of shape {tuple(u.shape)}; expected [1, steps, {U}]')
+        if not torch.is_floating_point(u):
+            raise ValueError('uniform tape is not floating point')
+        if u.numel() and (bool((u < 0).any()) or bool((u >= 1).any()) or bool(torch.isnan(u).any())):
+            raise ValueError('uniform tape has values outside [0, 1)')
+        return u
+
     # ---- checks ----
     def _check_mels(self, mels):
         if not isinstance(mels, (list, tuple)) or len(mels) == 0:
@@ -360,11 +460,22 @@ class WaveRNN(nn.Module):
         at element offset mel_off[b], and the MelResNet output aux [B, max F, res_out_dims]."""
         frames = [int(s.shape[1]) for s in specs]
         B, Fm, p = len(specs), max(frames), self.pad
-        rn = self.upsample.resnet
-        d = lambda t: t.detach().to(device=device, dtype=torch.float32).contiguous()
         x = torch.zeros(B, self.feat_dims, Fm, device=device, dtype=torch.float32)
         for i, s in enumerate(specs):
             x[i, :, :frames[i]] = s.to(device=device, dtype=torch.float32)
+        aux = self._resnet(x, frames, device)
+        ups = []
+        for i, s in enumerate(specs):
+            m = torch.zeros(self.feat_dims, frames[i] + 2 * p, device=device, dtype=torch.float32)
+            m[:, p:p + frames[i]] = s.to(device=device, dtype=torch.float32)
+            ups.append(self._mel_path(m, device).reshape(-1))
+        mel_off = np.concatenate([[0], np.cumsum([u.numel() for u in ups])[:-1]]).astype(np.int64)
+        return torch.cat(ups), mel_off, aux
+
+    def _resnet(self, x, frames, device):
+        """The MelResNet of a zero-padded batch x [B, feat_dims, W] whose mel b has frames[b] frames -> aux [B, W, res_out_dims]."""
+        rn = self.upsample.resnet
+        d = lambda t: t.detach().to(device=device, dtype=torch.float32).contiguous()
         lengths = torch.tensor(frames, device=device, dtype=torch.int32)
 
         def block(inp, conv, bn, activation):
@@ -376,18 +487,17 @@ class WaveRNN(nn.Module):
             y = block(h, layer.conv1, layer.batch_norm1, 'relu')
             h = h + block(y, layer.conv2, layer.batch_norm2, 'identity')
         w_out, b_out = d(rn.conv_out.weight.reshape(rn.conv_out.out_channels, -1)), d(rn.conv_out.bias)
-        aux = torch.empty(B, Fm, rn.conv_out.out_channels, device=device, dtype=torch.float32)
-        for i in range(B):
+        aux = torch.empty(x.shape[0], x.shape[2], rn.conv_out.out_channels, device=device, dtype=torch.float32)
+        for i in range(x.shape[0]):
             F.gemm(h[i], w_out, trans_a=True, trans_b=True, bias=b_out, out=aux[i])
-        ups = []
-        for i, s in enumerate(specs):
-            m = torch.zeros(self.feat_dims, frames[i] + 2 * p, device=device, dtype=torch.float32)
-            m[:, p:p + frames[i]] = s.to(device=device, dtype=torch.float32)
-            for j, scale in enumerate(self.upsample_factors[:-1]):
-                m = F.wavernn_upsample_layer(m, d(self.upsample.up_layers[2 * j + 1].weight.reshape(-1)), scale)
-            ups.append(m.reshape(-1))
-        mel_off = np.concatenate([[0], np.cumsum([u.numel() for u in ups])[:-1]]).astype(np.int64)
-        return torch.cat(ups), mel_off, aux
+        return aux
+
+    def _mel_path(self, m, device):
+        """Every mel-path layer but the last over frames of the padded mel m [feat_dims, W] (zero beyond them) -> [feat_dims, W hop / s_last]."""
+        for j, scale in enumerate(self.upsample_factors[:-1]):
+            fir = self.upsample.up_layers[2 * j + 1].weight.detach().reshape(-1).to(device=device, dtype=torch.float32).contiguous()
+            m = F.wavernn_upsample_layer(m, fir, scale)
+        return m
 
     def loop_weights(self, device):
         """fp32 contiguous tensors on `device` of the loop parameters (_lib.WAVERNN_PARAM_FIELDS) and of the conditioning products."""
@@ -476,3 +586,99 @@ class WaveRNN(nn.Module):
             mu = 0
         wave = F.wavernn_unfold(y, dev(np.asarray(frames, np.int32)), dev(row_off), dev(wave_off), int(wave_off[-1]), hop, target, overlap, mu)
         return wave, wave_off
+
+
+class _Stream:
+    """The state of one generate_stream: the mel frames that have arrived, the loop workspace carried across calls, and the samples the
+    loop has run but not yet released (raw loop outputs, or de-emphasised ones with preemphasis)."""
+
+    def __init__(self, model, device, as_numpy, on_cuda, tape, generator, preemphasis):
+        if device is None:
+            device = torch.device('cuda', torch.cuda.current_device()) if torch.cuda.is_available() else torch.device('cuda')
+        self.m, self.device, self.as_numpy, self.on_cuda = model, device, as_numpy, on_cuda
+        self.tape, self.generator, self.a = tape, generator, float(preemphasis)
+        self.hop, self.lookahead = model.hop_length, model.lookahead()
+        self.mu = model.n_classes - 1 if model.mode == 'RAW' else 0
+        self.mel = torch.zeros(model.feat_dims, 0, device=device, dtype=torch.float32)
+        self.steps = 0                 # loop steps run
+        self.released = 0              # samples yielded
+        self.pending = torch.zeros(0, device=device, dtype=torch.float32)       # samples [released, steps)
+        self.last = torch.zeros(1, device=device, dtype=torch.float32)          # the last de-emphasised sample
+        with self._fp32():
+            self.w = model.loop_weights(device)
+            self.S = model.chunk_steps(1, 1 << 30)
+            self.shape = _lib.WaveRNNShape(1, model.rnn_dims, model.fc_dims, model.n_classes, _lib.WAVERNN_MODES[model.mode], self.S)
+            self.ws = F.wavernn_workspace(self.shape, device)
+            self.params = F.wavernn_params(self.w)
+            F.wavernn_prepare(self.shape, self.params, self.ws)
+
+    @property
+    def frames(self):
+        return int(self.mel.shape[1])
+
+    @contextlib.contextmanager
+    def _fp32(self):
+        precision = _lib.get_precision()
+        try:
+            _lib.set_precision('fp32')
+            with torch.cuda.device(self.device), torch.no_grad():
+                yield
+        finally:
+            _lib.set_precision(precision)
+
+    def feed(self, spec):
+        """Takes one non-empty chunk; returns the samples it releases, or None."""
+        with self._fp32():
+            self.mel = torch.cat([self.mel, spec.to(device=self.device, dtype=torch.float32)], dim=1)
+            ready = min(self.frames - self.lookahead, self.frames - 1) * self.hop      # samples whose features are final
+            self._run(ready, False)
+            n = (self.steps - 20 * self.hop) - self.released                          # the last 20 hops wait for the fade-out
+            if n <= 0:
+                return None
+            # an unfold that ends 20 hops past the samples it writes applies no fade
+            wave = self._unfold(n, n // self.hop + 21)
+        return self._out(wave)
+
+    def finish(self):
+        with self._fp32():
+            F_ = self.frames
+            self._run((F_ - 1) * self.hop, True)
+            wave = self._unfold((F_ - 1) * self.hop - self.released, F_ - self.released // self.hop)
+        return self._out(wave)
+
+    def _run(self, end, final):
+        m, U = self.m, self.m.uniforms_per_step()
+        while self.steps < end:
+            t, n = self.steps, min(self.S, end - self.steps)
+            if self.tape is not None:
+                if self.tape.shape[1] < t + n:
+                    raise ValueError(f'the uniform tape holds {self.tape.shape[1]} steps; the stream needs at least {t + n}')
+                uni = self.tape[:, t:t + n].to(device=self.device, dtype=torch.float32).contiguous()
+            else:
+                uni = torch.rand(1, n, U, device=self.device, dtype=torch.float32, generator=self.generator)
+            feat = m.window_features(self.mel, t, t + n, final)
+            cond = m.conditioning(self.w, feat.unsqueeze(1))
+            y = torch.empty(1, n, device=self.device, dtype=torch.float32)
+            F.wavernn_run_stream(self.shape, self.params, cond, t, n, uni, y, self.ws)
+            if self.a:
+                if self.mu:
+                    y = F.wavernn_deemphasis(y, self.mu, 0.0)                    # a = 0: the mu-law decode only
+                y = F.wavernn_deemphasis(torch.cat([self.last, y[0]]).reshape(1, -1), 0, self.a)[:, 1:]
+                self.last = y[0, -1:].clone()
+            self.pending = torch.cat([self.pending, y[0]])
+            self.steps += n
+
+    def _unfold(self, n, frames):
+        """The next n pending samples through b200tts_wavernn_unfold as one fold of an utterance of `frames` frames: decoded (RAW,
+        without preemphasis) and faded out over the last 20 hops of (frames - 1) hop samples."""
+        y, self.pending = self.pending[:n].reshape(1, n).contiguous(), self.pending[n:]
+        self.released += n
+        d = lambda a: torch.tensor(a, device=self.device)
+        return F.wavernn_unfold(y, d([frames]).int(), d([0, 1]).int(), d([0, n]).long(), n, self.hop, n, 0, 0 if self.a else self.mu)
+
+    def _out(self, wave):
+        if F.wavernn_aborted(self.shape, self.ws):
+            raise _lib.B200TTSError('wavernn: the sample loop timed out at a grid barrier')
+        if self.as_numpy:
+            return wave.cpu().numpy()
+        return wave if self.on_cuda else wave.cpu()
