@@ -551,6 +551,23 @@ typedef struct {
  * MelResNet output's frames [a0, a0 + aux_len).  B200TTS_ERR_INVALID when a read would fall outside a window. */
 int b200tts_wavernn_window(const b200tts_wavernn_window_shape* shape, const float* mel_win, const float* fir, const float* aux_win, long long s0,
                            int nsteps, float* feat, void* stream);
+/* Rows of one call of b200tts_wavernn_window_rows and segments of b200tts_wavernn_upsample_segments: at most this many. */
+#define B200TTS_WAVERNN_MAX_STREAMS 64
+typedef struct {
+    b200tts_wavernn_window_shape w;   /* the row's window, as for b200tts_wavernn_window; n_mels, aux_dims, hop, pad, scale equal in every row */
+    long long s0;                     /* the row's first position (its steps run so far) */
+    long long mel_off, aux_off;       /* element offsets of the row's mel and aux windows in the packed buffers */
+    int n;                            /* positions [s0, s0 + n), 0 to nsteps */
+} b200tts_wavernn_window_row;
+/* b200tts_wavernn_window for active_rows rows in one launch: feat [nsteps, active_rows, n_mels + aux_dims], row r's step i the features of
+ * position rows[r].s0 + i for i < rows[r].n, zero past it.  rows: host descriptors, each checked as b200tts_wavernn_window checks its shape. */
+int b200tts_wavernn_window_rows(const b200tts_wavernn_window_row* rows, int active_rows, int nsteps, const float* mel, const float* fir,
+                                const float* aux, float* feat, void* stream);
+/* b200tts_wavernn_upsample_layer over nseg packed segments (1 to B200TTS_WAVERNN_MAX_STREAMS): segment g is in [C, lens[g]] right after
+ * segment g - 1 and goes to out [C, lens[g] scale] at scale times its input offset; each equal to its own b200tts_wavernn_upsample_layer.
+ * lens: host int32. */
+int b200tts_wavernn_upsample_segments(int C, int nseg, const int32_t* lens, int scale, const float* fir, const float* in, float* out,
+                                      void* stream);
 typedef struct {
     int rows;             /* fold rows of one loop */
     int rnn_dims;         /* R: a multiple of 128, at most 640 */
@@ -597,6 +614,19 @@ int b200tts_wavernn_run(const b200tts_wavernn_shape* shape, const b200tts_wavern
  * [rows, nsteps] hold this call's steps only; cond as for b200tts_wavernn_run. */
 int b200tts_wavernn_run_stream(const b200tts_wavernn_shape* shape, const b200tts_wavernn_params* params, const b200tts_wavernn_cond* cond,
                                long long t, int nsteps, const float* uniforms, float* out, void* workspace, size_t workspace_bytes, void* stream);
+/* Concurrent streams, one per row of one loop: row r has run row_t[r] steps since it was last reset (or prepared) and runs row_n[r] (0 to
+ * nsteps) more in this call, exactly as b200tts_wavernn_run_stream would run them on that row alone: its step i reads cond[i, r],
+ * uniforms[r, i] and writes out[r, i], with the h1 / h2 slot parity of step row_t[r] + i.  Past its budget a row writes nothing (state,
+ * previous sample, activation rows and out columns keep their values).  Only the first active_rows rows (at most shape->rows) are computed;
+ * cond is [nsteps, active_rows, width], uniforms [active_rows, nsteps, U], out [active_rows, nsteps]; nsteps at most shape->fold_len.
+ * row_t int64, row_n int32, both [active_rows] on the device. */
+int b200tts_wavernn_run_rows(const b200tts_wavernn_shape* shape, const b200tts_wavernn_params* params, const b200tts_wavernn_cond* cond,
+                             const int64_t* row_t, const int32_t* row_n, int active_rows, int nsteps, const float* uniforms, float* out,
+                             void* workspace, size_t workspace_bytes, void* stream);
+/* Zeroes h1, h2, both h1 / h2 activation slots and the previous sample of the `count` listed rows (host int32, each in [0, shape->rows)),
+ * as b200tts_wavernn_prepare leaves them, so that a row can start a new stream without a prepare. */
+int b200tts_wavernn_reset_rows(const b200tts_wavernn_shape* shape, void* workspace, size_t workspace_bytes, const int32_t* rows, int count,
+                               void* stream);
 /* Synchronises the stream and sets *aborted to the loop's abort flag (nonzero: a launch since the last prepare timed out). */
 int b200tts_wavernn_aborted(const b200tts_wavernn_shape* shape, const void* workspace, size_t workspace_bytes, int* aborted, void* stream);
 /* Optional de-emphasis of the loop's folded samples, in place, before b200tts_wavernn_unfold: each of `rows` rows of `len` samples is
@@ -637,11 +667,6 @@ int b200tts_gru_seq_forward(const b200tts_gru_seq_shape* shape, const float* gi,
  * receives every step's total dh = dh_ext + z dh_next + W_hh^T dgh_next.  One cooperative launch of 128 CTAs. */
 int b200tts_gru_seq_backward(const b200tts_gru_seq_shape* shape, const float* w_hh, const float* h, const void* saved, const float* dh_ext,
                              float* dgi, float* dgh, float* dh_dbg, void* workspace, size_t workspace_bytes, void* stream);
-/* A stream of unknown length: nsteps (at most shape->fold_len) more steps of every row after the t steps run since the last prepare, from the
- * state left in the workspace, exactly as b200tts_wavernn_run would run steps [t, t + nsteps).  uniforms [rows, nsteps, U] and out
- * [rows, nsteps] hold this call's steps only; cond as for b200tts_wavernn_run. */
-int b200tts_wavernn_run_stream(const b200tts_wavernn_shape* shape, const b200tts_wavernn_params* params, const b200tts_wavernn_cond* cond,
-                               long long t, int nsteps, const float* uniforms, float* out, void* workspace, size_t workspace_bytes, void* stream);
 /* Synchronises the stream and sets *aborted to the loops' abort flag (nonzero: a loop on this workspace timed out since it was zeroed). */
 int b200tts_gru_seq_aborted(const b200tts_gru_seq_shape* shape, const void* workspace, size_t workspace_bytes, int* aborted, void* stream);
 /* The adjoint of b200tts_wavernn_upsample_layer (C, len, scale, fir, in as there) for dout [C, len scale]: din [C, len] (overwritten; NULL:

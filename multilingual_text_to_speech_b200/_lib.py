@@ -99,6 +99,13 @@ class WaveRNNWindowShape(Structure):
                [(n, c_int) for n in ('mel_len', 'a0', 'aux_len')]
 
 
+class WaveRNNWindowRow(Structure):
+    _fields_ = [('w', WaveRNNWindowShape), ('s0', c_longlong), ('mel_off', c_longlong), ('aux_off', c_longlong), ('n', c_int)]
+
+
+WAVERNN_MAX_STREAMS = 64
+
+
 class WaveRNNShape(Structure):
     _fields_ = [(n, c_int) for n in ('rows', 'rnn_dims', 'fc_dims', 'n_out', 'mode', 'fold_len')]
 
@@ -218,6 +225,11 @@ SIGNATURES = {
                                     c_void_p, c_void_p, c_size_t, c_void_p]),
     'b200tts_wavernn_run_stream': (c_int, [POINTER(WaveRNNShape), POINTER(WaveRNNParams), POINTER(WaveRNNCond), c_longlong, c_int, c_void_p,
                                            c_void_p, c_void_p, c_size_t, c_void_p]),
+    'b200tts_wavernn_run_rows': (c_int, [POINTER(WaveRNNShape), POINTER(WaveRNNParams), POINTER(WaveRNNCond), c_void_p, c_void_p, c_int, c_int,
+                                         c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    'b200tts_wavernn_reset_rows': (c_int, [POINTER(WaveRNNShape), c_void_p, c_size_t, POINTER(c_int), c_int, c_void_p]),
+    'b200tts_wavernn_window_rows': (c_int, [POINTER(WaveRNNWindowRow), c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'b200tts_wavernn_upsample_segments': (c_int, [c_int, c_int, POINTER(c_int), c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     'b200tts_wavernn_aborted': (c_int, [POINTER(WaveRNNShape), c_void_p, c_size_t, POINTER(c_int), c_void_p]),
     'b200tts_wavernn_deemphasis': (c_int, [c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
     'b200tts_wavernn_unfold': (c_int, [c_int] * 5 + [c_void_p] * 3 + [c_longlong, c_void_p, c_void_p, c_void_p]),

@@ -212,6 +212,17 @@ int wavernn_check(const b200tts_wavernn_shape& s, void* ws, size_t ws_bytes);
 int wavernn_prepare_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, void* ws, size_t ws_bytes, cudaStream_t st);
 int wavernn_run_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, const b200tts_wavernn_cond& cond, int t0, int nsteps,
                      const float* uniforms, float* out, float* dbg, void* ws, size_t ws_bytes, cudaStream_t st);
+int wavernn_run_rows_check(const b200tts_wavernn_shape& s, int active_rows, int nsteps);
+int wavernn_run_rows_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, const b200tts_wavernn_cond& cond, const long long* row_t,
+                          const int* row_n, int active_rows, int nsteps, const float* uniforms, float* out, void* ws, size_t ws_bytes,
+                          cudaStream_t st);
+int wavernn_reset_rows_check(const b200tts_wavernn_shape& s, const int* rows, int count);
+int wavernn_reset_rows_impl(const b200tts_wavernn_shape& s, void* ws, size_t ws_bytes, const int* rows, int count, cudaStream_t st);
+int wavernn_window_rows_check(const b200tts_wavernn_window_row* rows, int active_rows, int nsteps);
+int wavernn_window_rows_impl(const b200tts_wavernn_window_row* rows, int active_rows, int nsteps, const float* mel, const float* fir,
+                             const float* aux, float* feat, cudaStream_t st);
+int wavernn_upsample_segments_check(int C, int nseg, const int* lens, int scale);
+int wavernn_upsample_segments_impl(int C, int nseg, const int* lens, int scale, const float* fir, const float* in, float* out, cudaStream_t st);
 int wavernn_aborted_impl(const b200tts_wavernn_shape& s, const void* ws, size_t ws_bytes, int* aborted, cudaStream_t st);
 int wavernn_deemphasis_check(int rows, int len, int mu, float a);
 int wavernn_deemphasis_impl(int rows, int len, int mu, float a, float* y, cudaStream_t st);
@@ -755,6 +766,40 @@ int b200tts_wavernn_run_stream(const b200tts_wavernn_shape* shape, const b200tts
     B200_TRY(wavernn_check(*shape, workspace, workspace_bytes));
     B200_TRY(require_device());
     return wavernn_run_stream_impl(*shape, *params, *cond, t, nsteps, uniforms, out, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_wavernn_run_rows(const b200tts_wavernn_shape* shape, const b200tts_wavernn_params* params, const b200tts_wavernn_cond* cond,
+                             const int64_t* row_t, const int32_t* row_n, int active_rows, int nsteps, const float* uniforms, float* out,
+                             void* workspace, size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(shape && params && cond, "wavernn_run_rows: null argument");
+    B200_REQUIRE(row_t && row_n && uniforms && out, "wavernn_run_rows: null row_t, row_n, uniforms or output");
+    B200_TRY(wavernn_check(*shape, workspace, workspace_bytes));
+    B200_TRY(wavernn_run_rows_check(*shape, active_rows, nsteps));
+    B200_TRY(require_device());
+    return wavernn_run_rows_impl(*shape, *params, *cond, reinterpret_cast<const long long*>(row_t), row_n, active_rows, nsteps, uniforms, out,
+                                 workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_wavernn_reset_rows(const b200tts_wavernn_shape* shape, void* workspace, size_t workspace_bytes, const int32_t* rows, int count,
+                               void* stream) {
+    B200_REQUIRE(shape, "wavernn_reset_rows: null argument");
+    B200_TRY(wavernn_check(*shape, workspace, workspace_bytes));
+    B200_TRY(wavernn_reset_rows_check(*shape, rows, count));
+    B200_TRY(require_device());
+    return wavernn_reset_rows_impl(*shape, workspace, workspace_bytes, rows, count, (cudaStream_t)stream);
+}
+int b200tts_wavernn_window_rows(const b200tts_wavernn_window_row* rows, int active_rows, int nsteps, const float* mel, const float* fir,
+                                const float* aux, float* feat, void* stream) {
+    B200_REQUIRE(mel && fir && feat, "wavernn_window_rows: null argument");
+    B200_TRY(wavernn_window_rows_check(rows, active_rows, nsteps));
+    B200_REQUIRE(aux || rows[0].w.aux_dims == 0, "wavernn_window_rows: null aux");
+    B200_TRY(require_device());
+    return wavernn_window_rows_impl(rows, active_rows, nsteps, mel, fir, aux, feat, (cudaStream_t)stream);
+}
+int b200tts_wavernn_upsample_segments(int C, int nseg, const int32_t* lens, int scale, const float* fir, const float* in, float* out,
+                                      void* stream) {
+    B200_REQUIRE(fir && in && out, "wavernn_upsample_segments: null argument");
+    B200_TRY(wavernn_upsample_segments_check(C, nseg, lens, scale));
+    B200_TRY(require_device());
+    return wavernn_upsample_segments_impl(C, nseg, lens, scale, fir, in, out, (cudaStream_t)stream);
 }
 int b200tts_wavernn_aborted(const b200tts_wavernn_shape* shape, const void* workspace, size_t workspace_bytes, int* aborted, void* stream) {
     B200_REQUIRE(shape && aborted, "wavernn_aborted: null argument");

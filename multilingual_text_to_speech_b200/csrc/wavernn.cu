@@ -60,6 +60,30 @@ __global__ void wavernn_upsample_layer_kernel(int C, int len, int s, const float
     }
 }
 
+// wavernn_upsample_layer_kernel over packed segments: segment g is [C, len_g] at in + in_off[g] and [C, len_g s] at out + s in_off[g]
+struct WrSegments { int n, C; long long in_off[B200TTS_WAVERNN_MAX_STREAMS + 1]; int len[B200TTS_WAVERNN_MAX_STREAMS]; };
+__global__ void wavernn_upsample_segments_kernel(const __grid_constant__ WrSegments g, int s, const float* __restrict__ w,
+                                                 const float* __restrict__ in, float* __restrict__ out) {
+    const long long n = g.in_off[g.n] * s;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < n; idx += (long long)gridDim.x * blockDim.x) {
+        int lo_g = 0, hi_g = g.n - 1;
+        while (lo_g < hi_g) {
+            const int mid = (lo_g + hi_g + 1) >> 1;
+            if (g.in_off[mid] * s <= idx) lo_g = mid; else hi_g = mid - 1;
+        }
+        const int len = g.len[lo_g], lo = len * s;
+        const long long e = idx - g.in_off[lo_g] * s;
+        const int c = (int)(e / lo), i = (int)(e - (long long)c * lo);
+        const float* x = in + g.in_off[lo_g] + (size_t)c * len;
+        float acc = 0.f;
+        for (int k = -s; k <= s; ++k) {
+            const int j = i + k;
+            if (j >= 0 && j < lo) acc = fmaf(w[k + s], x[j / s], acc);
+        }
+        out[idx] = acc;
+    }
+}
+
 // feat[i, r, :] for loop steps t0 + i of fold row r: the row's utterance b and fold f give the sample position q = f (target + overlap) +
 // t0 + i of the utterance's F hop positions (zero beyond them: the tail padding of fold_with_overlap).  Columns [0, n_mels): the last mel
 // layer at the uncut position q + pad hop; columns [n_mels, n_mels + aux_dims): aux[b, q / hop, :].
@@ -119,6 +143,40 @@ __global__ void wavernn_window_kernel(b200tts_wavernn_window_shape s, long long 
                 v = acc;
             } else {
                 v = aux[(size_t)(q / s.hop - s.a0) * s.aux_dims + (col - s.n_mels)];
+            }
+        }
+        feat[idx] = v;
+    }
+}
+
+// wavernn_window_kernel for many rows: row r's positions are [s0, s0 + n) (zero for steps i >= n), its windows at mel + mel_off and
+// aux + aux_off.  feat [nsteps, rows, n_mels + aux_dims].
+struct WrWinRow { long long s0, m0, lo, mel_off, aux_off; int n, frames, mel_len, a0; };
+struct WrWinRows { WrWinRow r[B200TTS_WAVERNN_MAX_STREAMS]; };
+__global__ void wavernn_window_rows_kernel(int n_mels, int aux_dims, int hop, int pad, int scale, int rows, const __grid_constant__ WrWinRows w,
+                                           const float* __restrict__ mel, const float* __restrict__ fir, const float* __restrict__ aux,
+                                           int nsteps, float* __restrict__ feat) {
+    const int D = n_mels + aux_dims;
+    const long long n = (long long)nsteps * rows * D;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < n; idx += (long long)gridDim.x * blockDim.x) {
+        const int col = (int)(idx % D);
+        const long long ir = idx / D;
+        const int r = (int)(ir % rows), i = (int)(ir / rows);
+        const WrWinRow& s = w.r[r];
+        const long long q = s.s0 + i;
+        float v = 0.f;
+        if (i < s.n && (s.frames == 0 || q < (long long)s.frames * hop)) {
+            if (col < n_mels) {
+                const float* xc = mel + s.mel_off + (size_t)col * s.mel_len;
+                const long long p = q + (long long)pad * hop;
+                float acc = 0.f;
+                for (int k = -scale; k <= scale; ++k) {
+                    const long long j = p + k;
+                    if (j >= 0 && j < s.lo) acc = fmaf(fir[k + scale], xc[j / scale - s.m0], acc);
+                }
+                v = acc;
+            } else {
+                v = aux[s.aux_off + (size_t)(q / hop - s.a0) * aux_dims + (col - n_mels)];
             }
         }
         feat[idx] = v;
@@ -188,6 +246,11 @@ struct WrLoopArgs {
     __nv_bfloat16 *h1b, *h2b, *x1b, *x2b, *y1b, *y2b;     // h1b / h2b: two slots of [rows, R]
     unsigned* bar;
     int* abort_flag;
+    // ragged instantiation only: row r runs its steps i < row_n[r] with h1 / h2 slot parity (row_t[r] + i) & 1; rows = the active rows,
+    // slot = the elements of one h1b / h2b slot (the workspace's rows x R)
+    const long long* row_t;
+    const int* row_n;
+    size_t slot;
 };
 
 // acc (16 x 8 tile: weight rows x fold rows row0..row0+7) = tile . act[row0 + n, 0:K]^T
@@ -224,6 +287,9 @@ __device__ __forceinline__ float gru_cell(float gir, float giz, float gin, float
     return fmaf(z, h - nn, nn);       // (1 - z) n + z h
 }
 
+// RAGGED = false: every row runs steps [t0, t0 + nsteps) (wavernn_run / _run_stream).  RAGGED = true: each row runs its own budget of this
+// call's nsteps from its own step count (wavernn_run_rows); a row past its budget writes nothing.
+template <bool RAGGED>
 __global__ void __launch_bounds__(WR_THREADS, 1) wavernn_loop_kernel(WrLoopArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     __shared__ float s_ep[WR_WARPS][2][16 * 8];
@@ -244,17 +310,23 @@ __global__ void __launch_bounds__(WR_THREADS, 1) wavernn_loop_kernel(WrLoopArgs 
     unsigned target = 0;
 
     for (int i = 0; i < a.nsteps; ++i) {
-        const int tg = a.t0 + i, ti = tg - a.io0;
+        const int tg = a.t0 + i, ti = RAGGED ? i : tg - a.io0;
         const int cur = tg & 1, prv = cur ^ 1;
+        // ragged: the previous step's h1b / h2b slot of this lane's operand row (wr_mma reads row nt * 8 + lane / 4), by the row's own parity
+        auto prv_slot = [&](const __nv_bfloat16* base, int nt) {
+            const int r = nt * 8 + (lane >> 2);
+            return r < rows ? base + (size_t)(((a.row_t[r] + i) & 1) ^ 1) * a.slot : base;
+        };
         float* dbg = a.dbg ? a.dbg + (size_t)i * rows * Ddbg : nullptr;
         // 1. GRU1
         for (int nt = warp; nt < ntiles; nt += WR_WARPS) {
             float acc[4];
-            wr_mma(acc, wt + d.off[0], a.h1b + (size_t)prv * rows * R, R, nt * 8, rows, lane);
+            if constexpr (RAGGED) wr_mma(acc, wt + d.off[0], prv_slot(a.h1b, nt), R, nt * 8, rows, lane);
+            else wr_mma(acc, wt + d.off[0], a.h1b + (size_t)prv * rows * R, R, nt * 8, rows, lane);
             wr_spill(ep0, acc, lane);
             for (int e = lane; e < U * 8; e += 32) {
                 const int j = e >> 3, n = e & 7, row = nt * 8 + n, u = c * U + j;
-                if (row < rows) {
+                if (row < rows && (!RAGGED || i < a.row_n[row])) {
                     const float p = __ldcg(a.prev + row);
                     const float* g1 = a.g1 + ((size_t)i * rows + row) * 3 * R;
                     const float gir = fmaf(a.u1[u], p, g1[u]), giz = fmaf(a.u1[R + u], p, g1[R + u]), gin = fmaf(a.u1[2 * R + u], p, g1[2 * R + u]);
@@ -265,7 +337,8 @@ __global__ void __launch_bounds__(WR_THREADS, 1) wavernn_loop_kernel(WrLoopArgs 
                     const float x = fmaf(a.w_prev[u], p, a.cc[((size_t)i * rows + row) * R + u]) + h;
                     const __nv_bfloat16 xb = bf(x);
                     a.h1[o] = h;
-                    a.h1b[(size_t)cur * rows * R + o] = bf(h);
+                    if constexpr (RAGGED) a.h1b[(size_t)((a.row_t[row] + i) & 1) * a.slot + o] = bf(h);
+                    else a.h1b[(size_t)cur * rows * R + o] = bf(h);
                     a.x1[o] = x;
                     a.x1b[o] = xb;
                     if (dbg) { float* q = dbg + (size_t)row * Ddbg; q[u] = h; q[R + u] = __bfloat162float(xb); }
@@ -279,11 +352,12 @@ __global__ void __launch_bounds__(WR_THREADS, 1) wavernn_loop_kernel(WrLoopArgs 
             float acc[4];
             wr_mma(acc, wt + d.off[1], a.x1b, R, nt * 8, rows, lane);
             wr_spill(ep0, acc, lane);
-            wr_mma(acc, wt + d.off[2], a.h2b + (size_t)prv * rows * R, R, nt * 8, rows, lane);
+            if constexpr (RAGGED) wr_mma(acc, wt + d.off[2], prv_slot(a.h2b, nt), R, nt * 8, rows, lane);
+            else wr_mma(acc, wt + d.off[2], a.h2b + (size_t)prv * rows * R, R, nt * 8, rows, lane);
             wr_spill(ep1, acc, lane);
             for (int e = lane; e < U * 8; e += 32) {
                 const int j = e >> 3, n = e & 7, row = nt * 8 + n, u = c * U + j;
-                if (row < rows) {
+                if (row < rows && (!RAGGED || i < a.row_n[row])) {
                     const float* c2 = a.c2 + ((size_t)i * rows + row) * 3 * R;
                     const float gir = ep0[j * 8 + n] + c2[u], giz = ep0[(U + j) * 8 + n] + c2[R + u], gin = ep0[(2 * U + j) * 8 + n] + c2[2 * R + u];
                     const float ghr = ep1[j * 8 + n] + a.b_hh2[u], ghz = ep1[(U + j) * 8 + n] + a.b_hh2[R + u],
@@ -292,7 +366,8 @@ __global__ void __launch_bounds__(WR_THREADS, 1) wavernn_loop_kernel(WrLoopArgs 
                     const float h = gru_cell(gir, giz, gin, ghr, ghz, ghn, a.h2[o]);
                     const __nv_bfloat16 xb = bf(a.x1[o] + h);
                     a.h2[o] = h;
-                    a.h2b[(size_t)cur * rows * R + o] = bf(h);
+                    if constexpr (RAGGED) a.h2b[(size_t)((a.row_t[row] + i) & 1) * a.slot + o] = bf(h);
+                    else a.h2b[(size_t)cur * rows * R + o] = bf(h);
                     a.x2b[o] = xb;
                     if (dbg) { float* q = dbg + (size_t)row * Ddbg; q[2 * R + u] = h; q[3 * R + u] = __bfloat162float(xb); }
                 }
@@ -312,7 +387,7 @@ __global__ void __launch_bounds__(WR_THREADS, 1) wavernn_loop_kernel(WrLoopArgs 
                 wr_spill(ep0, acc, lane);
                 for (int e = lane; e < V * 8; e += 32) {
                     const int j = e >> 3, n = e & 7, row = nt * 8 + n, o = c * V + j;
-                    if (row < rows) {
+                    if (row < rows && (!RAGGED || i < a.row_n[row])) {
                         const __nv_bfloat16 yb = bf(fmaxf(ep0[j * 8 + n] + P[((size_t)i * rows + row) * Fc + o], 0.f));
                         outb[(size_t)row * Fc + o] = yb;
                         if (dbg) dbg[(size_t)row * Ddbg + 4 * R + st * Fc + o] = __bfloat162float(yb);
@@ -330,7 +405,7 @@ __global__ void __launch_bounds__(WR_THREADS, 1) wavernn_loop_kernel(WrLoopArgs 
                 wr_spill(ep0, acc, lane);
                 for (int e = lane; e < O * 8; e += 32) {
                     const int j = e >> 3, n = e & 7, row = nt * 8 + n, o = c * O + j;
-                    if (row < rows && o < d.n_out) {
+                    if (row < rows && o < d.n_out && (!RAGGED || i < a.row_n[row])) {
                         const float l = ep0[j * 8 + n] + a.b_fc3[o];
                         a.logits[(size_t)row * d.n_out + o] = l;
                         if (dbg) dbg[(size_t)row * Ddbg + 4 * R + 2 * Fc + o] = l;
@@ -342,6 +417,7 @@ __global__ void __launch_bounds__(WR_THREADS, 1) wavernn_loop_kernel(WrLoopArgs 
         if (!grid_barrier(a.bar, target, gridDim.x, a.abort_flag, &s_ok, false)) return;
         // 6. sample, one warp per row
         for (int row = c * WR_WARPS + warp; row < rows; row += WR_CTAS * WR_WARPS) {
+            if (RAGGED && i >= a.row_n[row]) continue;
             const float* lg = a.logits + (size_t)row * d.n_out;
             float sample;
             if (a.mode == B200TTS_WAVERNN_RAW) {
@@ -402,6 +478,21 @@ __global__ void __launch_bounds__(WR_THREADS, 1) wavernn_loop_kernel(WrLoopArgs 
             }
         }
         if (!grid_barrier(a.bar, target, gridDim.x, a.abort_flag, &s_ok, false)) return;
+    }
+}
+
+// zero the recurrent state of the listed rows: h1, h2, both slots of h1b / h2b, the previous sample
+struct WrRowList { int n; int row[B200TTS_WAVERNN_MAX_STREAMS]; };
+__global__ void wavernn_reset_rows_kernel(const __grid_constant__ WrRowList l, int rows, int R, float* __restrict__ h1, float* __restrict__ h2,
+                                          float* __restrict__ prev, __nv_bfloat16* __restrict__ h1b, __nv_bfloat16* __restrict__ h2b) {
+    const long long n = (long long)l.n * R;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < n; idx += (long long)gridDim.x * blockDim.x) {
+        const int k = (int)(idx / R), u = (int)(idx % R);
+        const size_t o = (size_t)l.row[k] * R + u, slot = (size_t)rows * R;
+        h1[o] = 0.f;
+        h2[o] = 0.f;
+        h1b[o] = h1b[slot + o] = h2b[o] = h2b[slot + o] = __float2bfloat16_rn(0.f);
+        if (u == 0) prev[l.row[k]] = 0.f;
     }
 }
 
@@ -548,8 +639,10 @@ int wavernn_prepare_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_p
 }
 
 // steps [t0, t0 + nsteps) from the state in the workspace; uniforms / out rows of L columns, column 0 at step io0
+// ragged (row_t / row_n non-null): `rows` active rows, each from its own step count
 static int wavernn_launch(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, const b200tts_wavernn_cond& cond, int t0, int io0,
-                          int L, int nsteps, const float* uniforms, float* out, float* dbg, void* ws, cudaStream_t st) {
+                          int L, int nsteps, const float* uniforms, float* out, float* dbg, void* ws, cudaStream_t st,
+                          const long long* row_t = nullptr, const int* row_n = nullptr, int rows = 0) {
     B200_REQUIRE(p.b_hh1 && p.u1 && p.w_prev && p.b_hh2 && p.b_fc3, "wavernn_run: null parameter");
     B200_REQUIRE(cond.c && cond.g1 && cond.c2 && cond.p1 && cond.p2, "wavernn_run: null conditioning");
     B200_REQUIRE(uniforms && out, "wavernn_run: null uniforms or output");
@@ -557,7 +650,8 @@ static int wavernn_launch(const b200tts_wavernn_shape& s, const b200tts_wavernn_
     unsigned char* base = static_cast<unsigned char*>(ws);
     WrLoopArgs a;
     a.d = wr_dims(s.rnn_dims, s.fc_dims, s.n_out);
-    a.rows = s.rows; a.mode = s.mode; a.L = L; a.t0 = t0; a.io0 = io0; a.nsteps = nsteps;
+    a.rows = row_t ? rows : s.rows; a.mode = s.mode; a.L = L; a.t0 = t0; a.io0 = io0; a.nsteps = nsteps;
+    a.row_t = row_t; a.row_n = row_n; a.slot = (size_t)s.rows * s.rnn_dims;
     a.packed = reinterpret_cast<const uint4*>(base + l.packed);
     a.b_hh1 = p.b_hh1; a.u1 = p.u1; a.w_prev = p.w_prev; a.b_hh2 = p.b_hh2; a.b_fc3 = p.b_fc3;
     a.cc = cond.c; a.g1 = cond.g1; a.c2 = cond.c2; a.p1 = cond.p1; a.p2 = cond.p2;
@@ -577,7 +671,8 @@ static int wavernn_launch(const b200tts_wavernn_shape& s, const b200tts_wavernn_
     a.abort_flag = reinterpret_cast<int*>(base + l.bar + 128);
     B200_CUDA(cudaMemsetAsync(a.bar, 0, sizeof(unsigned), st));       // the abort flag persists until the next prepare
     void* params[] = {&a};
-    return launch_persistent("wavernn_loop", (const void*)wavernn_loop_kernel, WR_CTAS, WR_THREADS, (size_t)a.d.per_cta * 16, false, params, st);
+    const void* fn = row_t ? (const void*)wavernn_loop_kernel<true> : (const void*)wavernn_loop_kernel<false>;
+    return launch_persistent("wavernn_loop", fn, WR_CTAS, WR_THREADS, (size_t)a.d.per_cta * 16, false, params, st);
 }
 
 int wavernn_run_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, const b200tts_wavernn_cond& cond, int t0, int nsteps,
@@ -598,6 +693,45 @@ int wavernn_run_stream_impl(const b200tts_wavernn_shape& s, const b200tts_wavern
     return wavernn_launch(s, p, cond, t0, t0, nsteps, nsteps, uniforms, out, nullptr, ws, st);
 }
 
+int wavernn_run_rows_check(const b200tts_wavernn_shape& s, int active_rows, int nsteps) {
+    B200_REQUIRE(active_rows >= 1 && active_rows <= s.rows && nsteps >= 1 && nsteps <= s.fold_len,
+                 "wavernn_run_rows: %d active rows of %d, %d steps (at most fold_len = %d per call)", active_rows, s.rows, nsteps, s.fold_len);
+    return B200TTS_OK;
+}
+
+int wavernn_run_rows_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, const b200tts_wavernn_cond& cond, const long long* row_t,
+                          const int* row_n, int active_rows, int nsteps, const float* uniforms, float* out, void* ws, size_t ws_bytes,
+                          cudaStream_t st) {
+    B200_TRY(wavernn_check(s, ws, ws_bytes));
+    B200_TRY(wavernn_run_rows_check(s, active_rows, nsteps));
+    B200_REQUIRE(row_t && row_n, "wavernn_run_rows: null row_t or row_n");
+    return wavernn_launch(s, p, cond, 0, 0, nsteps, nsteps, uniforms, out, nullptr, ws, st, row_t, row_n, active_rows);
+}
+
+int wavernn_reset_rows_check(const b200tts_wavernn_shape& s, const int* rows, int count) {
+    B200_REQUIRE(rows && count >= 1 && count <= s.rows, "wavernn_reset_rows: %d rows of a loop of %d", count, s.rows);
+    for (int k = 0; k < count; ++k)
+        B200_REQUIRE(rows[k] >= 0 && rows[k] < s.rows, "wavernn_reset_rows: row %d outside [0, %d)", rows[k], s.rows);
+    return B200TTS_OK;
+}
+
+int wavernn_reset_rows_impl(const b200tts_wavernn_shape& s, void* ws, size_t ws_bytes, const int* rows, int count, cudaStream_t st) {
+    B200_TRY(wavernn_check(s, ws, ws_bytes));
+    B200_TRY(wavernn_reset_rows_check(s, rows, count));
+    const WrLayout l = wr_layout(s);
+    unsigned char* base = static_cast<unsigned char*>(ws);
+    for (int k0 = 0; k0 < count; k0 += B200TTS_WAVERNN_MAX_STREAMS) {
+        WrRowList list;
+        list.n = count - k0 < B200TTS_WAVERNN_MAX_STREAMS ? count - k0 : B200TTS_WAVERNN_MAX_STREAMS;
+        for (int k = 0; k < list.n; ++k) list.row[k] = rows[k0 + k];
+        wavernn_reset_rows_kernel<<<grid_for((size_t)list.n * s.rnn_dims), 256, 0, st>>>(
+            list, s.rows, s.rnn_dims, reinterpret_cast<float*>(base + l.h1), reinterpret_cast<float*>(base + l.h2),
+            reinterpret_cast<float*>(base + l.prev), reinterpret_cast<__nv_bfloat16*>(base + l.h1b), reinterpret_cast<__nv_bfloat16*>(base + l.h2b));
+        B200_LAUNCH_CHECK();
+    }
+    return B200TTS_OK;
+}
+
 int wavernn_aborted_impl(const b200tts_wavernn_shape& s, const void* ws, size_t ws_bytes, int* aborted, cudaStream_t st) {
     B200_TRY(wavernn_check(s, const_cast<void*>(ws), ws_bytes));
     const WrLayout l = wr_layout(s);
@@ -616,6 +750,29 @@ int wavernn_upsample_layer_impl(int C, int len, int scale, const float* fir, con
     B200_TRY(wavernn_upsample_layer_check(C, len, scale));
     KernelTimer kt("wavernn_upsample", st);
     wavernn_upsample_layer_kernel<<<grid_for((size_t)C * len * scale), 256, 0, st>>>(C, len, scale, fir, in, out);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+int wavernn_upsample_segments_check(int C, int nseg, const int* lens, int scale) {
+    B200_REQUIRE(lens && nseg >= 1 && nseg <= B200TTS_WAVERNN_MAX_STREAMS, "wavernn_upsample_segments: %d segments (1 to %d)", nseg,
+                 B200TTS_WAVERNN_MAX_STREAMS);
+    long long total = 0;
+    for (int g = 0; g < nseg; ++g) {
+        B200_TRY(wavernn_upsample_layer_check(C, lens[g], scale));
+        total += lens[g];
+    }
+    B200_REQUIRE((long long)C * total * scale < (1ll << 40), "wavernn_upsample_segments: %lld samples in all", total);
+    return B200TTS_OK;
+}
+
+int wavernn_upsample_segments_impl(int C, int nseg, const int* lens, int scale, const float* fir, const float* in, float* out, cudaStream_t st) {
+    B200_TRY(wavernn_upsample_segments_check(C, nseg, lens, scale));
+    WrSegments g;
+    g.n = nseg; g.C = C; g.in_off[0] = 0;
+    for (int k = 0; k < nseg; ++k) { g.len[k] = lens[k]; g.in_off[k + 1] = g.in_off[k] + (long long)C * lens[k]; }
+    KernelTimer kt("wavernn_upsample", st);
+    wavernn_upsample_segments_kernel<<<grid_for((size_t)g.in_off[nseg] * scale), 256, 0, st>>>(g, scale, fir, in, out);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }
@@ -672,6 +829,39 @@ int wavernn_window_impl(const b200tts_wavernn_window_shape& s, const float* mel_
     KernelTimer kt("wavernn_window", st);
     const long long lo = s.frames > 0 ? (long long)(s.frames + 2 * s.pad) * s.hop : LLONG_MAX;
     wavernn_window_kernel<<<grid_for((size_t)nsteps * (s.n_mels + s.aux_dims)), 256, 0, st>>>(s, lo, mel_up, fir, aux, s0, nsteps, feat);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+// every row: wavernn_window_check of its own window, and the shared columns and factors of row 0
+int wavernn_window_rows_check(const b200tts_wavernn_window_row* rows, int active_rows, int nsteps) {
+    B200_REQUIRE(rows && active_rows >= 1 && active_rows <= B200TTS_WAVERNN_MAX_STREAMS && nsteps >= 1,
+                 "wavernn_window_rows: %d rows (1 to %d), %d steps", active_rows, B200TTS_WAVERNN_MAX_STREAMS, nsteps);
+    const b200tts_wavernn_window_shape& w0 = rows[0].w;
+    for (int r = 0; r < active_rows; ++r) {
+        const b200tts_wavernn_window_row& d = rows[r];
+        B200_REQUIRE(d.w.n_mels == w0.n_mels && d.w.aux_dims == w0.aux_dims && d.w.hop == w0.hop && d.w.pad == w0.pad && d.w.scale == w0.scale,
+                     "wavernn_window_rows: row %d's columns or factors differ from row 0's", r);
+        B200_REQUIRE(d.n >= 0 && d.n <= nsteps && d.mel_off >= 0 && d.aux_off >= 0, "wavernn_window_rows: row %d runs %d of %d steps "
+                     "(offsets %lld, %lld)", r, d.n, nsteps, d.mel_off, d.aux_off);
+        if (d.n > 0) B200_TRY(wavernn_window_check(d.w, d.s0, d.n));
+    }
+    return B200TTS_OK;
+}
+
+int wavernn_window_rows_impl(const b200tts_wavernn_window_row* rows, int active_rows, int nsteps, const float* mel, const float* fir,
+                             const float* aux, float* feat, cudaStream_t st) {
+    B200_TRY(wavernn_window_rows_check(rows, active_rows, nsteps));
+    const b200tts_wavernn_window_shape& w0 = rows[0].w;
+    WrWinRows w;
+    for (int r = 0; r < active_rows; ++r) {
+        const b200tts_wavernn_window_row& d = rows[r];
+        w.r[r] = WrWinRow{d.s0, d.w.m0, d.w.frames > 0 ? (long long)(d.w.frames + 2 * d.w.pad) * d.w.hop : LLONG_MAX, d.mel_off, d.aux_off, d.n,
+                          d.w.frames, d.w.mel_len, d.w.a0};
+    }
+    KernelTimer kt("wavernn_window", st);
+    wavernn_window_rows_kernel<<<grid_for((size_t)nsteps * active_rows * (w0.n_mels + w0.aux_dims)), 256, 0, st>>>(
+        w0.n_mels, w0.aux_dims, w0.hop, w0.pad, w0.scale, active_rows, w, mel, fir, aux, nsteps, feat);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }

@@ -72,6 +72,19 @@ def gemm(a, b, trans_a=False, trans_b=False, bias=None, out=None, beta=0.0, alph
     return out
 
 
+def gemm_tn_batched(a, b, bias=None):
+    """out[i] = a[i]^T b^T + bias for a [B, K, M], b [N, K] -> [B, M, N] in one launch, each out[i] equal to gemm(a[i], b, trans_a=True,
+    trans_b=True, bias=bias)."""
+    _require_cuda(a, b)
+    a, b = a.contiguous(), b.contiguous()
+    B, K, M = a.shape
+    N = b.shape[0]
+    out = torch.empty(B, M, N, device=a.device, dtype=torch.float32)
+    check(_lib.load().b200tts_gemm_f32(1, 1, M, N, K, 1.0, ptr(a), M, ptr(b), K, 0.0, ptr(out), N, ptr(bias), B, K * M, 0, M * N, 1, None,
+                                       _stream()), 'b200tts_gemm_f32')
+    return out
+
+
 # ------------------------------------------------------------------------------------------------
 # dropout keep-masks
 # ------------------------------------------------------------------------------------------------
@@ -909,6 +922,31 @@ def wavernn_window(shape, mel_win, fir, aux_win, s0, nsteps):
     return out
 
 
+def wavernn_upsample_segments(x, lens, fir, scale):
+    """wavernn_upsample_layer over packed segments: x holds [C, lens[g]] for each g one after another (flat) -> the same packing of
+    [C, lens[g] scale], each segment equal to its own wavernn_upsample_layer."""
+    _require_cuda(x, fir)
+    x, fir = _f32c(x), _f32c(fir)
+    n = len(lens)
+    C = x.numel() // max(sum(lens), 1)
+    out = torch.empty(x.numel() * scale, device=x.device, dtype=torch.float32)
+    check(_lib.load().b200tts_wavernn_upsample_segments(C, n, (ctypes.c_int * n)(*lens), int(scale), ptr(fir), ptr(x), ptr(out), _stream()),
+          'b200tts_wavernn_upsample_segments')
+    return out
+
+
+def wavernn_window_rows(rows, nsteps, mel, fir, aux):
+    """feat [nsteps, len(rows), n_mels + aux_dims] of many rows' positions (rows: _lib.WaveRNNWindowRow descriptors) from the packed mel and
+    aux windows."""
+    _require_cuda(mel, fir, aux)
+    n = len(rows)
+    w0 = rows[0].w
+    out = torch.empty(int(nsteps), n, w0.n_mels + w0.aux_dims, device=mel.device, dtype=torch.float32)
+    check(_lib.load().b200tts_wavernn_window_rows((_lib.WaveRNNWindowRow * n)(*rows), n, int(nsteps), ptr(_f32c(mel)), ptr(_f32c(fir)),
+                                                  ptr(_f32c(aux)), ptr(out), _stream()), 'b200tts_wavernn_window_rows')
+    return out
+
+
 def wavernn_workspace(shape, device):
     """Workspace of the sample loop for `shape` (a _lib.WaveRNNShape); raises on an invalid shape."""
     n = _lib.load().b200tts_wavernn_workspace_bytes(ctypes.byref(shape))
@@ -942,6 +980,22 @@ def wavernn_run_stream(shape, params, cond, t, nsteps, uniforms, out, ws):
     cs = _lib.WaveRNNCond(*[ptr(t_) for t_ in cond])
     check(_lib.load().b200tts_wavernn_run_stream(ctypes.byref(shape), ctypes.byref(params), ctypes.byref(cs), int(t), int(nsteps), ptr(uniforms),
                                                  ptr(out), ptr(ws), ws.numel(), _stream()), 'b200tts_wavernn_run_stream')
+
+
+def wavernn_run_rows(shape, params, cond, row_t, row_n, nsteps, uniforms, out, ws):
+    """Up to nsteps more steps of each of the first len(row_t) rows: row r has run row_t[r] steps (int64, device) and runs row_n[r] (int32,
+    device); cond [nsteps, rows, width], uniforms [rows, nsteps, U], out [rows, nsteps]."""
+    cs = _lib.WaveRNNCond(*[ptr(t_) for t_ in cond])
+    check(_lib.load().b200tts_wavernn_run_rows(ctypes.byref(shape), ctypes.byref(params), ctypes.byref(cs), ptr(row_t), ptr(row_n),
+                                               int(row_t.numel()), int(nsteps), ptr(uniforms), ptr(out), ptr(ws), ws.numel(), _stream()),
+          'b200tts_wavernn_run_rows')
+
+
+def wavernn_reset_rows(shape, ws, rows):
+    """Zero the recurrent state of the listed rows (host ints)."""
+    n = len(rows)
+    check(_lib.load().b200tts_wavernn_reset_rows(ctypes.byref(shape), ptr(ws), ws.numel(), (ctypes.c_int * n)(*rows), n, _stream()),
+          'b200tts_wavernn_reset_rows')
 
 
 def wavernn_aborted(shape, ws):

@@ -460,42 +460,76 @@ class Tacotron(torch.nn.Module):
         decoder steps); after every chunk one item is yielded: the post-net over the frames that became final (stream_release), computed
         over a window with the post-net's halo of decoded frames on the left and, once the cut is known, the zeros past it on the right.
         An item may hold no frames (a chunk shorter than the halo).  The model is in eval mode, without autograd, until the generator
-        ends or is closed; prenet dropout stays on, as in `inference`, and a MaskSource tape is replayed the same way."""
-        speakers, languages = _check_batch_inputs([text], None if speaker is None else [speaker], None if language is None else [language])
+        ends or is closed; prenet dropout stays on, as in `inference`, and a MaskSource tape is replayed the same way.  The one-text case
+        of `inference_streams`."""
+        for item in self._streams([text], None if speaker is None else [speaker], None if language is None else [language], chunk_frames,
+                                  'inference_stream'):
+            yield item[0]
+
+    def inference_streams(self, texts, speakers=None, languages=None, chunk_frames=None):
+        """`inference_stream` for up to 64 texts decoded as one group: takes `inference_batch`'s inputs (text i reads column i of a
+        recorded mask tape) and yields, after every decoder call, {i: post-net chunk [num_mels, n]} for each text the call decoded (a chunk
+        may hold no frames).  The frames released by one call go through the post-net as one padded batch.  Concatenated per text, the
+        chunks are inference_batch's output for that text; in fp32 mode they equal inference_stream of that text alone with its tape
+        column, bit for bit."""
+        yield from self._streams(texts, speakers, languages, chunk_frames, 'inference_streams')
+
+    def _streams(self, texts, speakers, languages, chunk_frames, name):
+        speakers, languages = _check_batch_inputs(texts, speakers, languages)
+        texts = list(texts)
+        if len(texts) > MAX_STREAM_TEXTS:
+            raise ValueError(f'{name}: at most {MAX_STREAM_TEXTS} texts decode as one group (got {len(texts)})')
         if chunk_frames is not None and int(chunk_frames) < 1:
-            raise ValueError(f'inference_stream: chunk_frames must be >= 1 (got {chunk_frames})')
+            raise ValueError(f'{name}: chunk_frames must be >= 1 (got {chunk_frames})')
         was_training = self.training
         self.eval()
         try:
             with torch.no_grad():
-                encoded, mask, speaker, language = self._encode_group([text], speakers, languages)
+                encoded, mask, speaker, language = self._encode_group(texts, speakers, languages)
             dec, halo = self._decoder, self._postnet.halo()
-            pre, released = [], 0
-            chunks = dec._inference_chunks(encoded, mask, speaker, language, att_extent=1, tape_columns=[0], chunk_frames=chunk_frames)
+            B = len(texts)
+            pre, released = [[] for _ in range(B)], [0] * B
+            chunks = dec._inference_chunks(encoded, mask, speaker, language, att_extent=1, tape_columns=list(range(B)), chunk_frames=chunk_frames)
             while True:
                 with torch.no_grad():
                     item = next(chunks, None)
                     if item is None:
                         return
-                    _, spec, _, _, rules, done = item
-                    pre.append(spec[0])
-                    end = stream_release(done, rules[0].cut, dec._max_frames, halo)
-                    final = rules[0].cut is not None or done >= dec._max_frames
-                    post = self._postnet_window(torch.cat(pre, 0), released, end, halo, end if final else done)
-                released = end
-                yield post
+                    rows, spec, _, _, rules, done = item
+                    spans = {}
+                    for j, u in enumerate(rows):
+                        pre[u].append(spec[j])
+                        end = stream_release(done, rules[u].cut, dec._max_frames, halo)
+                        final = rules[u].cut is not None or done >= dec._max_frames
+                        spans[u] = (released[u], end, end if final else done)
+                        released[u] = end
+                    posts = self._postnet_windows(pre, spans, halo)
+                yield posts
         finally:
             self.train(was_training)
 
-    def _postnet_window(self, pre, t0, t1, halo, avail):
-        """Post-net output frames [t0, t1) [num_mels, t1 - t0] from the decoded frames pre [>= avail, N], of which the first `avail` count
-        (the rest lie past the stop cut): run over frames [t0 - halo, t1 + halo) within [0, avail), zero-padded at the window's ends."""
-        w0, w1 = postnet_window(t0, t1, halo, avail)
-        if t1 <= t0:
-            return pre.new_zeros(pre.shape[1], 0)
-        x = pre[w0:w1].t().unsqueeze(0).contiguous()
-        post = self._postnet(x, torch.tensor([w1 - w0], device=x.device), padded=True)
-        return post[0, :, t0 - w0:t1 - w0]
+    def _postnet_windows(self, pre, spans, halo):
+        """{u: post-net output frames [t0, t1) [num_mels, t1 - t0]} for spans {u: (t0, t1, avail)} of the decoded frames pre[u] (chunks of
+        [n, N], of which the first `avail` count; the rest lie past the stop cut): each run over frames [t0 - halo, t1 + halo) within
+        [0, avail), zero-padded at the window's ends, all windows in one padded post-net batch."""
+        N = pre[next(iter(spans))][0].shape[1]
+        out, wins = {}, []
+        for u, (t0, t1, avail) in spans.items():
+            if t1 <= t0:
+                out[u] = pre[u][0].new_zeros(N, 0)
+            else:
+                w0, w1 = postnet_window(t0, t1, halo, avail)
+                wins.append((u, t0, t1, w0, w1))
+        if wins:
+            W = max(w1 - w0 for *_, w0, w1 in wins)
+            x = pre[wins[0][0]][0].new_zeros(len(wins), N, W)
+            for b, (u, t0, t1, w0, w1) in enumerate(wins):
+                x[b, :, :w1 - w0] = torch.cat(pre[u], 0)[w0:w1].t()
+            lengths = torch.tensor([w1 - w0 for *_, w0, w1 in wins], device=x.device)
+            post = self._postnet(x, lengths, padded=True)
+            for b, (u, t0, t1, w0, w1) in enumerate(wins):
+                out[u] = post[b, :, t0 - w0:t1 - w0]
+        return out
 
     def _encode_group(self, texts, speakers, languages):
         """Padded batch of texts -> (encoder output, mask, speaker, language) in the decoder's forms."""
@@ -530,6 +564,10 @@ class Tacotron(torch.nn.Module):
         prediction, _, _, cuts = self._decoder._decode_inference(encoded, mask, speaker, language, att_extent=1, tape_columns=tape_columns)
         post = self._postnet(prediction.transpose(1, 2), torch.tensor(cuts, device=device), padded=True)
         return [post[b, :, :cuts[b]] for b in range(B)]
+
+
+# texts of one inference_streams group at most: the batch inference_batch decodes at once by default
+MAX_STREAM_TEXTS = 64
 
 
 def stream_release(done, cut, max_frames, halo):

@@ -29,6 +29,9 @@ from .. import functional as F
 
 # fp32 bytes of the conditioning products and folded features held at once: bounds the chunk of loop steps
 COND_BYTES = 512 << 20
+# loop steps per StreamPool.run at most, in hops (then bounded by COND_BYTES): 16 hops are 0.2 s of audio at 22050 Hz, so a stream's chunks
+# come at least that often while it is behind, and the host work around each loop call is spread over 4400 steps
+POOL_CALL_HOPS = 16
 LOG_SCALE_MIN = float(np.log(1e-14))
 # training windows the sequence loops take: at most this many hops of samples, at most 64 of them
 MAX_TRAIN_HOPS = 16
@@ -336,6 +339,10 @@ class WaveRNN(nn.Module):
             raise ValueError(f'the mel stream ended after {0 if st is None else st.frames} frames; the 20-hop fade-out needs at least 21')
         yield st.finish()
 
+    def stream_pool(self, max_streams, preemphasis=0.0, generator=None):
+        """A StreamPool of up to max_streams (1 to 64) concurrent generate_stream-like streams sharing one sample loop."""
+        return StreamPool(self, max_streams, preemphasis, generator)
+
     def lookahead(self):
         """Frames past a sample's own frame that its loop features read: `pad` for conv_in (the rest of the MelResNet is pointwise) or the
         reach of the mel path's stretch + FIR layers, whichever is larger."""
@@ -487,10 +494,7 @@ class WaveRNN(nn.Module):
             y = block(h, layer.conv1, layer.batch_norm1, 'relu')
             h = h + block(y, layer.conv2, layer.batch_norm2, 'identity')
         w_out, b_out = d(rn.conv_out.weight.reshape(rn.conv_out.out_channels, -1)), d(rn.conv_out.bias)
-        aux = torch.empty(x.shape[0], x.shape[2], rn.conv_out.out_channels, device=device, dtype=torch.float32)
-        for i in range(x.shape[0]):
-            F.gemm(h[i], w_out, trans_a=True, trans_b=True, bias=b_out, out=aux[i])
-        return aux
+        return F.gemm_tn_batched(h, w_out, b_out)
 
     def _mel_path(self, m, device):
         """Every mel-path layer but the last over frames of the padded mel m [feat_dims, W] (zero beyond them) -> [feat_dims, W hop / s_last]."""
@@ -682,3 +686,293 @@ class _Stream:
         if self.as_numpy:
             return wave.cpu().numpy()
         return wave if self.on_cuda else wave.cpu()
+
+
+class _PoolStream:
+    """One stream of a StreamPool: its loop row, the mel frames that have arrived, its uniform tape (fp32 on the device, or None), the steps
+    run and the samples released.  Its run but unreleased samples [released, steps) sit in the pool's per-row ring buffer."""
+
+    def __init__(self, slot, device, feat_dims, tape):
+        self.slot, self.tape = slot, tape
+        self.mel = torch.zeros(feat_dims, 0, device=device, dtype=torch.float32)
+        self.chunks = 0
+        self.steps = 0
+        self.released = 0
+        self.ended = False
+
+    @property
+    def frames(self):
+        return int(self.mel.shape[1])
+
+
+class StreamPool:
+    """Concurrent streaming generation: up to max_streams streams, each a generate_stream, advance together in one sample loop whose rows
+    run independently (b200tts_wavernn_run_rows).  open() takes the lowest free row and resets it; feed() and end() add a stream's mel
+    frames and mark its end; run() makes one loop call over every stream with samples ready, under generate_stream's rule (lookahead()
+    frames after a sample's frame, the last 20 hops held back until end()), at most POOL_CALL_HOPS hops per call, and returns {sid: waveform
+    chunk} (CUDA tensors) for the streams that released samples.  A stream's row is freed when its final chunk is returned.
+
+    For each stream the concatenated chunks equal generate_stream of the same mel with the same uniform tape, bit for bit, whenever it
+    joined, whatever else shares the loop and however its mel was chunked.  With preemphasis the stream is de-emphasised across calls and
+    stays within generate_batch's bound.  Without a tape the uniforms are drawn with torch.rand (`generator` optional) once per call for all
+    rows, so they differ from a solo run's draws.  Every call runs in fp32 (the precision mode is set for the call and restored after it)
+    on the CUDA device that was current when the pool was made; each run() reads the loop's abort flag once.  The device work of a run()
+    is a fixed number of launches whatever the number of streams: the per-stream windows, tapes and samples are gathered and scattered
+    with indices built on the host."""
+
+    def __init__(self, model, max_streams, preemphasis=0.0, generator=None):
+        if not 1 <= int(max_streams) <= _lib.WAVERNN_MAX_STREAMS:
+            raise ValueError(f'a stream pool holds 1 to {_lib.WAVERNN_MAX_STREAMS} streams (got {max_streams})')
+        if not -1.0 < float(preemphasis) < 1.0:
+            raise ValueError(f'preemphasis {preemphasis} must lie in (-1, 1)')
+        self.m, self.a, self.generator = model, float(preemphasis), generator
+        self.device = torch.device('cuda', torch.cuda.current_device()) if torch.cuda.is_available() else torch.device('cuda')
+        self.rows = int(max_streams)
+        self.hop, self.lookahead = model.hop_length, model.lookahead()
+        self.mu = model.n_classes - 1 if model.mode == 'RAW' else 0
+        self.slots = [None] * self.rows          # sid of the stream on each row
+        self.streams = {}
+        self.next_sid = 0
+        with self._fp32():
+            self.w = model.loop_weights(self.device)
+            self.S = min(POOL_CALL_HOPS * self.hop, model.chunk_steps(self.rows, 1 << 30))
+            self.shape = _lib.WaveRNNShape(self.rows, model.rnn_dims, model.fc_dims, model.n_classes, _lib.WAVERNN_MODES[model.mode], self.S)
+            self.ws = F.wavernn_workspace(self.shape, self.device)
+            self.params = F.wavernn_params(self.w)
+            F.wavernn_prepare(self.shape, self.params, self.ws)
+            fir = lambda j: model.upsample.up_layers[2 * j + 1].weight.detach().reshape(-1).to(self.device, torch.float32).contiguous()  # noqa
+            self.firs = [fir(j) for j in range(len(model.upsample_factors))]
+            self.last = torch.zeros(self.rows, device=self.device, dtype=torch.float32)     # each row's last de-emphasised sample
+            # per-row ring of the samples run but not released: at most 20 held-back hops, the partial hop and one call's steps
+            self.P = self.S + 22 * self.hop
+            self.ring = torch.zeros(self.rows * self.P + 2, device=self.device, dtype=torch.float32)   # + a write sink and a zero
+
+    @contextlib.contextmanager
+    def _fp32(self):
+        precision = _lib.get_precision()
+        try:
+            _lib.set_precision('fp32')
+            with torch.cuda.device(self.device), torch.no_grad():
+                yield
+        finally:
+            _lib.set_precision(precision)
+
+    def open(self, uniforms=None):
+        """A new stream on the lowest free row -> its id.  uniforms: its tape [1, T, U] as for generate_stream, or None."""
+        tape = self.m._check_stream_tape(uniforms)
+        free = [r for r in range(self.rows) if self.slots[r] is None]
+        if not free:
+            raise ValueError(f'the stream pool is full: {self.rows} streams are open')
+        slot, sid = free[0], self.next_sid
+        with self._fp32():
+            F.wavernn_reset_rows(self.shape, self.ws, [slot])
+            self.last[slot] = 0.0
+            if tape is not None:
+                tape = tape[0].to(device=self.device, dtype=torch.float32).contiguous()
+            self.streams[sid] = _PoolStream(slot, self.device, self.m.feat_dims, tape)
+        self.slots[slot] = sid
+        self.next_sid += 1
+        return sid
+
+    def _stream(self, sid):
+        st = self.streams.get(sid)
+        if st is None:
+            raise ValueError(f'unknown or finished stream {sid}')
+        if st.ended:
+            raise ValueError(f'stream {sid} has ended')
+        return st
+
+    def feed(self, sid, mel_chunk):
+        """Appends mel frames [feat_dims, n] (n >= 0, as given) to stream sid."""
+        st = self._stream(sid)
+        spec, _ = self.m._check_chunk(mel_chunk, st.chunks)
+        st.chunks += 1
+        if spec.shape[1]:
+            st.mel = torch.cat([st.mel, spec.to(device=self.device, dtype=torch.float32)], dim=1)
+
+    def end(self, sid):
+        """Marks the end of stream sid's mel (at least 21 frames)."""
+        st = self._stream(sid)
+        if st.frames < 21:
+            raise ValueError(f'the mel stream ended after {st.frames} frames; the 20-hop fade-out needs at least 21')
+        st.ended = True
+
+    def plan(self):
+        """{sid: (steps run, steps of the next call)} for every stream with ready samples."""
+        out = {}
+        for sid, st in self.streams.items():
+            F_ = st.frames
+            end = (F_ - 1) * self.hop if st.ended else max(min(F_ - self.lookahead, F_ - 1), 0) * self.hop
+            n = min(self.S, end - st.steps)
+            if n > 0:
+                out[sid] = (st.steps, n)
+        return out
+
+    def release_plan(self):
+        """[(sid, samples, frames)] of every stream with samples to release: the final chunk once the stream has ended and run all its
+        (F - 1) hop steps (frames: the utterance length left, so that the unfold places the fade-out), else the whole hops run more than 20
+        hops ago (frames: 21 hops more than it writes, so that no fade lands on them)."""
+        hop, rel = self.hop, []
+        for sid, st in self.streams.items():
+            F_ = st.frames
+            if st.ended and st.steps == (F_ - 1) * hop:
+                n, frames = (F_ - 1) * hop - st.released, F_ - st.released // hop
+            else:
+                n = (st.steps - 20 * hop) // hop * hop - st.released
+                frames = n // hop + 21
+            if n > 0:
+                rel.append((sid, n, frames))
+        return rel
+
+    def run(self):
+        """One loop call over every stream with ready samples -> {sid: the waveform chunk it releases}."""
+        plan = self.plan()
+        for sid, (t, n) in plan.items():
+            tape = self.streams[sid].tape
+            if tape is not None and tape.shape[0] < t + n:
+                raise ValueError(f'the uniform tape holds {tape.shape[0]} steps; the stream needs at least {t + n}')
+        with self._fp32():
+            if plan:
+                self._loop(plan)
+            released = self._release()
+            if F.wavernn_aborted(self.shape, self.ws):
+                raise _lib.B200TTSError('wavernn: the sample loop timed out at a grid barrier')
+        for sid in released:
+            st = self.streams[sid]
+            if st.ended and st.released == (st.frames - 1) * self.hop:
+                self.slots[st.slot] = None
+                del self.streams[sid]
+        return released
+
+    def _upload(self, a):
+        return torch.from_numpy(np.ascontiguousarray(a)).to(self.device)
+
+    def _loop(self, plan):
+        m, dev, U = self.m, self.device, self.m.uniforms_per_step()
+        live = sorted(plan, key=lambda sid: self.streams[sid].slot)
+        active = self.streams[live[-1]].slot + 1
+        nmax = max(n for _, n in plan.values())
+        feat = self._features(live, plan, active, nmax)
+        cond = m.conditioning(self.w, feat)
+        slot = np.array([self.streams[sid].slot for sid in live], np.int64)
+        t = np.array([plan[sid][0] for sid in live], np.int64)
+        n = np.array([plan[sid][1] for sid in live], np.int64)
+        row_t, row_n = np.zeros(active, np.int64), np.zeros(active, np.int32)
+        row_t[slot], row_n[slot] = t, n
+        # uniforms: the taped rows' steps gathered from their tapes (source 0 is a zero), the rest drawn
+        taped = [sid for sid in live if self.streams[sid].tape is not None]
+        if taped:
+            src = torch.cat([torch.zeros(1, device=dev)] + [self.streams[sid].tape[plan[sid][0]:plan[sid][0] + plan[sid][1]].reshape(-1)
+                                                            for sid in taped])
+            idx = np.zeros((active, nmax, U), np.int64)
+            off = 1
+            i = np.arange(nmax)[:, None] * U + np.arange(U)[None, :]
+            for sid in taped:
+                st, k = self.streams[sid], plan[sid][1]
+                idx[st.slot, :k] = off + i[:k]
+                off += k * U
+            uni = src[self._upload(idx)]
+        if len(taped) < len(live):
+            drawn = torch.rand(active, nmax, U, device=dev, dtype=torch.float32, generator=self.generator)
+            if taped:
+                has = np.zeros((active, 1, 1), bool)
+                has[[self.streams[sid].slot for sid in taped]] = True
+                uni = torch.where(self._upload(has), uni, drawn)
+            else:
+                uni = drawn
+        y = torch.zeros(active, nmax, device=dev, dtype=torch.float32)
+        F.wavernn_run_rows(self.shape, self.params, cond, self._upload(row_t), self._upload(row_n), nmax, uni, y, self.ws)
+        if self.a:
+            if self.mu:
+                y = F.wavernn_deemphasis(y, self.mu, 0.0)                    # a = 0: the mu-law decode only
+            y = F.wavernn_deemphasis(torch.cat([self.last[:active, None], y], 1).contiguous(), 0, self.a)[:, 1:]
+            sl = self._upload(slot)
+            self.last[sl] = y[sl, self._upload(n - 1)]
+        # into the ring: row r's step i at slot r P + (row_t + i) mod P; steps past a row's budget go to the sink
+        i = np.arange(nmax)[None, :]
+        dst = np.where(i < row_n[:, None], np.arange(active)[:, None] * self.P + (row_t[:, None] + i) % self.P, self.rows * self.P)
+        self.ring.index_put_((self._upload(dst.reshape(-1)),), y.reshape(-1))
+        for sid in live:
+            self.streams[sid].steps += plan[sid][1]
+
+    def window_layout(self, live, plan):
+        """The host side of _features: (sources [(sid, frame0, frame1)] packed side by side, then a zero column; the gather index of the
+        packed mel-path windows followed by the padded MelResNet batch; window lengths; MelResNet widths and batch width; window-row
+        descriptors without the aux width, as (slot, frames or 0, m0, mel_len, a0, aux_len, s0, mel_off, aux_off / aux width, n))."""
+        m = self.m
+        p, hop, s_last, C = m.pad, self.hop, m.upsample_factors[-1], m.feat_dims
+        srcs, wins, res = [], [], []
+        for sid in live:
+            st, (t, n) = self.streams[sid], plan[sid]
+            (P0, P1), (r0, r1), _ = m.window_plan(t, t + n, st.frames, st.ended)
+            lo, hi = max(P0, p), min(P1, st.frames + p)
+            wins.append((P0, P1, lo, hi))
+            res.append((r0, r1))
+            srcs.append((sid, lo - p, max(hi, lo) - p))
+        srcs += [(sid, r0, r1) for sid, (r0, r1) in zip(live, res)]
+        off = np.concatenate([[0], np.cumsum([b - a for _, a, b in srcs])])
+        Wt = int(off[-1]) + 1                       # the last column is zero
+        c = np.arange(C)[:, None] * Wt
+        parts, lens, desc, mel_off = [], [], [], 0
+        for b, (sid, (P0, P1, lo, hi)) in enumerate(zip(live, wins)):
+            P = np.arange(P0, P1)
+            col = np.where((P >= lo) & (P < hi), off[b] + P - lo, Wt - 1)
+            parts.append((c + col[None, :]).reshape(-1))
+            lens.append(P1 - P0)
+        widths = [r1 - r0 for r0, r1 in res]
+        W = max(widths)
+        w = np.arange(W)[None, :]
+        col = np.where(w < np.array(widths)[:, None], off[len(live):-1, None] + w, Wt - 1)
+        parts.append((c[None, :, :] + col[:, None, :]).reshape(-1))
+        scale = int(np.prod(m.upsample_factors[:-1]))
+        for b, sid in enumerate(live):
+            st, (t, n) = self.streams[sid], plan[sid]
+            P0, r0 = wins[b][0], res[b][0]
+            desc.append((st.slot, st.frames if st.ended else 0, P0 * (hop // s_last), lens[b] * scale, r0, widths[b], t, mel_off, b * W, n))
+            mel_off += C * lens[b] * scale
+        return srcs, np.concatenate(parts), lens, widths, W, desc
+
+    def _features(self, live, plan, active, nmax):
+        """Loop features [nmax, active, feat_dims + res_out_dims] of every live stream's next steps, in a fixed number of launches: one
+        gather of every window, the mel-path layers on the packed windows, the MelResNet over the padded batch of windows, one
+        window-rows launch."""
+        m, dev = self.m, self.device
+        p, hop, s_last, C = m.pad, self.hop, m.upsample_factors[-1], m.feat_dims
+        srcs, idx, lens, widths, W, desc = self.window_layout(live, plan)
+        packed = torch.cat([self.streams[sid].mel[:, a:b] for sid, a, b in srcs] + [torch.zeros(C, 1, device=dev)], dim=1)
+        g = packed.reshape(-1)[self._upload(idx)]
+        nw = C * sum(lens)
+        x, batch = g[:nw], g[nw:].view(len(live), C, W)
+        for j, scale in enumerate(m.upsample_factors[:-1]):
+            x = F.wavernn_upsample_segments(x, lens, self.firs[j], scale)
+            lens = [ln * scale for ln in lens]
+        aux = m._resnet(batch, widths, dev)
+        A = aux.shape[2]
+        blank = _lib.WaveRNNWindowShape(C, A, hop, p, s_last, 0, 0, 1, 0, 0)
+        rows = [_lib.WaveRNNWindowRow(blank, 0, 0, 0, 0) for _ in range(active)]
+        for slot, frames, m0, mel_len, a0, aux_len, s0, mel_off, aux_row, n in desc:
+            shape = _lib.WaveRNNWindowShape(C, A, hop, p, s_last, frames, m0, mel_len, a0, aux_len)
+            rows[slot] = _lib.WaveRNNWindowRow(shape, s0, mel_off, aux_row * A, n)
+        return F.wavernn_window_rows(rows, nmax, x, self.firs[-1], aux)
+
+    def _release(self):
+        """Every stream's releasable samples, gathered from the ring, through one b200tts_wavernn_unfold, each stream one fold of one
+        utterance -> {sid: chunk}."""
+        rel = self.release_plan()
+        if not rel:
+            return {}
+        L = max(n for _, n, _ in rel)
+        i = np.arange(L)[None, :]
+        slot = np.array([self.streams[sid].slot for sid, _, _ in rel])[:, None]
+        start = np.array([self.streams[sid].released for sid, _, _ in rel])[:, None]
+        n = np.array([n for _, n, _ in rel])[:, None]
+        src = np.where(i < n, slot * self.P + (start + i) % self.P, self.rows * self.P + 1)
+        y = self.ring[self._upload(src)]
+        for sid, k, _ in rel:
+            self.streams[sid].released += k
+        wave_off = np.concatenate([[0], np.cumsum(n[:, 0])])
+        meta = self._upload(np.concatenate([[f for *_, f in rel], np.arange(len(rel) + 1), wave_off]).astype(np.int64))
+        B = len(rel)
+        wave = F.wavernn_unfold(y, meta[:B].int(), meta[B:2 * B + 1].int(), meta[2 * B + 1:], int(wave_off[-1]), self.hop, L, 0,
+                                0 if self.a else self.mu)
+        return {sid: wave[int(wave_off[b]):int(wave_off[b + 1])] for b, (sid, *_) in enumerate(rel)}
