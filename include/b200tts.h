@@ -229,6 +229,15 @@ int b200tts_decoder_forward_chunk(const b200tts_decoder_shape* shape, const b200
                                   const b200tts_decoder_inputs* in, const b200tts_decoder_outputs* out, b200tts_decoder_state* state,
                                   int first, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Rows of a b200tts_decoder_state listed per launch of b200tts_decoder_state_reset_rows (more are split over several launches). */
+#define B200TTS_DECODER_RESET_MAX_ROWS 64
+/* Writes the initial state of a decode into the `count` listed rows (host int32, each in [0, shape->B)) of `state`, whose buffers hold
+ * shape->B rows of width L, M, D and N: zeros, and for forward attention (shape->att_kind) the one-hot alpha_0 in cum_weights.  A chunk
+ * with `first` = 0 then continues such a row exactly as a chunk with `first` != 0 starts a fresh decode: both write the state through the
+ * same kernel.  The other rows are untouched, so texts can join a running decode.  Only B, L, M, D, N and att_kind of `shape` are read. */
+int b200tts_decoder_state_reset_rows(const b200tts_decoder_shape* shape, b200tts_decoder_state* state, const int32_t* rows, int count,
+                                     void* stream);
+
 typedef struct {
     const float* d_spectrogram; /* [B, T, N] or NULL */
     const float* d_stop;        /* [B, T]    or NULL */
@@ -428,6 +437,26 @@ int b200tts_fill_keep_mask(uint8_t* mask, size_t n, float drop_rate, uint64_t se
 /* Optional DEVICE-side epoch mixed into every mask key (NULL = off): a training step captured in a CUDA graph bakes the host seeds into
  * its kernel nodes, so the graph increments *epoch (a device uint64 the caller owns) once per replay and every replay draws new masks. */
 int b200tts_set_mask_epoch(const uint64_t* device_epoch);
+/* Per-row keep masks, time-major [steps, rows, width] (1 = keep), in one launch: element (i, r, p) is decision (step0[r] + i) * width + p
+ * of the stream b200tts_fill_keep_mask draws for (seeds[r], stream_id).  So a row's masks over steps [0, S), however they are cut into
+ * calls, are the rows of one b200tts_fill_keep_mask(n = S * width, seeds[r], stream_id) call.  seeds (uint64) and step0 (int64, >= 0)
+ * are DEVICE arrays of `rows` entries.  The device epoch of b200tts_set_mask_epoch is NOT mixed in: the draws depend on the seed alone
+ * (the equality above holds while no epoch is set). */
+int b200tts_fill_keep_mask_rows(uint8_t* mask, int steps, int rows, int width, float drop_rate, const uint64_t* seeds, const int64_t* step0,
+                                uint64_t stream_id, void* stream);
+/* Per-row uniforms in [0, 1), [rows, nsteps, width] (the layout b200tts_wavernn_run_rows reads with width = uniforms per step), in one
+ * launch: element (r, i, u) is draw (t0[r] + i) * width + u of the counter-based stream keyed by (seeds[r], stream_id): the top 24 bits
+ * of splitmix64 over the key and the draw index, times 2^-24.  A row's draws do not depend on how its steps are split into calls.  seeds
+ * (uint64) and t0 (int64, >= 0) are DEVICE arrays of `rows` entries.
+ *
+ * Stream ids under one request seed: B200TTS_SEED_STREAM_PRENET0 and _PRENET1 for the decoder's
+ * two per-step prenet dropout sites (b200tts_fill_keep_mask_rows, width P, one step per decoder step), B200TTS_SEED_STREAM_VOCODER for
+ * the WaveRNN sample loop's uniforms (b200tts_fill_uniform_rows, one step per sample). */
+int b200tts_fill_uniform_rows(float* out, int rows, int nsteps, int width, const uint64_t* seeds, const int64_t* t0, uint64_t stream_id,
+                              void* stream);
+#define B200TTS_SEED_STREAM_PRENET0 0x5EED000000000001ull
+#define B200TTS_SEED_STREAM_PRENET1 0x5EED000000000002ull
+#define B200TTS_SEED_STREAM_VOCODER 0x5EED000000000003ull
 
 /* ---- optimizer step on flat buffers: clip_grad_norm_ + torch.optim.Adam with coupled L2 decay (train.py:84-85, 260-271) ----
  * p, g, m, v: n fp32 elements each (the flat parameter buffer, the flat all-reduced gradient, Adam moments); g is overwritten with

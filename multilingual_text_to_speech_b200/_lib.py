@@ -105,6 +105,9 @@ class WaveRNNWindowRow(Structure):
 
 WAVERNN_MAX_STREAMS = 64
 
+# include/b200tts.h: the stream ids of the draws under one request seed (b200tts_fill_keep_mask_rows, b200tts_fill_uniform_rows)
+SEED_STREAMS = {'step_prenet0': 0x5EED000000000001, 'step_prenet1': 0x5EED000000000002, 'vocoder': 0x5EED000000000003}
+
 
 class WaveRNNShape(Structure):
     _fields_ = [(n, c_int) for n in ('rows', 'rnn_dims', 'fc_dims', 'n_out', 'mode', 'fold_len')]
@@ -159,6 +162,7 @@ SIGNATURES = {
                                         POINTER(DecoderOutputs), c_void_p, c_size_t, c_void_p]),
     'b200tts_decoder_forward_chunk': (c_int, [POINTER(DecoderShape), POINTER(DecoderParams), POINTER(DecoderInputs),
                                               POINTER(DecoderOutputs), POINTER(DecoderState), c_int, c_void_p, c_size_t, c_void_p]),
+    'b200tts_decoder_state_reset_rows': (c_int, [POINTER(DecoderShape), POINTER(DecoderState), POINTER(c_int), c_int, c_void_p]),
     'b200tts_decoder_backward': (c_int, [POINTER(DecoderShape), POINTER(DecoderParams), POINTER(DecoderInputs),
                                          POINTER(DecoderOutputs), POINTER(DecoderOutputGrads), c_void_p, c_void_p,
                                          c_size_t, POINTER(DecoderParams), c_void_p, c_void_p]),
@@ -205,6 +209,8 @@ SIGNATURES = {
     'b200tts_tacotron_loss_backward': (c_int, [POINTER(LossShape)] + [c_void_p] * 14),
     'b200tts_set_mask_epoch': (c_int, [c_void_p]),
     'b200tts_fill_keep_mask': (c_int, [c_void_p, c_size_t, c_float, c_uint64, c_uint64, c_void_p]),
+    'b200tts_fill_keep_mask_rows': (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_uint64, c_void_p]),
+    'b200tts_fill_uniform_rows': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_uint64, c_void_p]),
     'b200tts_vocoder_workspace_bytes': (c_size_t, [POINTER(VocoderShape)]),
     'b200tts_vocoder_fft_plan': (c_int, [c_int, POINTER(c_int), c_int]),
     'b200tts_spectrogram_magnitude': (c_int, [POINTER(VocoderShape), c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p]),

@@ -78,6 +78,9 @@ static int require_device() {
 int decoder_forward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
                          const b200tts_decoder_outputs& out, float* ws, size_t ws_bytes, cudaStream_t st,
                          const b200tts_decoder_state* state = nullptr, int first = 1);
+int decoder_state_reset_rows_check(const b200tts_decoder_shape& s, const b200tts_decoder_state& state, const int* rows, int count);
+int decoder_state_reset_rows_impl(const b200tts_decoder_shape& s, const b200tts_decoder_state& state, const int* rows, int count,
+                                  cudaStream_t st);
 int decoder_backward_impl(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
                           const b200tts_decoder_outputs& fwd_out, const b200tts_decoder_output_grads& dout, const float* fws,
                           float* bws, size_t bws_bytes, const b200tts_decoder_params& dw, float* d_memory, cudaStream_t st);
@@ -135,6 +138,13 @@ __host__ __device__ __forceinline__ unsigned long long mix64(unsigned long long 
     z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
     return z ^ (z >> 31);
 }
+// the key of stream (seed, stream_id), and the 64-bit draw of group g of it (4 keep decisions or one uniform)
+__host__ __device__ __forceinline__ unsigned long long stream_key(unsigned long long seed, unsigned long long stream_id) {
+    return mix64(seed ^ 0xD6E8FEB86659FD93ull) ^ (stream_id * 0xA24BAED4963EE407ull);
+}
+__device__ __forceinline__ unsigned long long stream_draw(unsigned long long key, unsigned long long g) {
+    return mix64(key + g * 0x9E3779B97F4A7C15ull);
+}
 __global__ void fill_keep_mask_kernel(uint8_t* __restrict__ mask, size_t n, unsigned threshold, unsigned long long key,
                                       const unsigned long long* __restrict__ epoch) {
     if (epoch) key ^= mix64(*epoch * 0xC2B2AE3D27D4EB4Full + 0x165667B19E3779F9ull);
@@ -146,7 +156,7 @@ __global__ void fill_keep_mask_kernel(uint8_t* __restrict__ mask, size_t n, unsi
         uint32_t w[4];
 #pragma unroll
         for (int gg = 0; gg < 4; ++gg) {
-            const unsigned long long r = mix64(key + (q * 4 + gg) * 0x9E3779B97F4A7C15ull);
+            const unsigned long long r = stream_draw(key, q * 4 + gg);
             uint32_t v = 0;
 #pragma unroll
             for (int j = 0; j < 4; ++j) v |= ((((unsigned)(r >> (16 * j)) & 0xFFFFu) >= threshold) ? 1u : 0u) << (8 * j);
@@ -159,6 +169,34 @@ __global__ void fill_keep_mask_kernel(uint8_t* __restrict__ mask, size_t n, unsi
             for (int e = 0; e < 16; ++e)
                 if (i0 + e < n) mask[i0 + e] = (uint8_t)((w[e >> 2] >> (8 * (e & 3))) & 0xFFu);
         }
+    }
+}
+// element (i, r, p) of [steps, rows, width]: decision d = (step0[r] + i) * width + p of row r's stream, i.e. 16-bit field d % 4 of
+// draw d / 4, as fill_keep_mask_kernel makes it
+__global__ void fill_keep_mask_rows_kernel(uint8_t* __restrict__ mask, int steps, int rows, int width, unsigned threshold,
+                                           const unsigned long long* __restrict__ seeds, const long long* __restrict__ step0,
+                                           unsigned long long stream_id) {
+    const long long n = (long long)steps * rows * width;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < n; idx += (long long)gridDim.x * blockDim.x) {
+        const int p = (int)(idx % width);
+        const long long ir = idx / width;
+        const int r = (int)(ir % rows);
+        const long long i = ir / rows;
+        const unsigned long long d = (unsigned long long)(step0[r] + i) * width + p;
+        const unsigned long long v = stream_draw(stream_key(seeds[r], stream_id), d >> 2);
+        mask[idx] = (((unsigned)(v >> (16 * (d & 3))) & 0xFFFFu) >= threshold) ? 1 : 0;
+    }
+}
+
+// element (r, i, u) of [rows, nsteps, width]: the top 24 bits of draw (t0[r] + i) * width + u of row r's stream, times 2^-24
+__global__ void fill_uniform_rows_kernel(float* __restrict__ out, int rows, int nsteps, int width, const unsigned long long* __restrict__ seeds,
+                                         const long long* __restrict__ t0, unsigned long long stream_id) {
+    const long long n = (long long)rows * nsteps * width;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < n; idx += (long long)gridDim.x * blockDim.x) {
+        const long long per_row = (long long)nsteps * width;
+        const int r = (int)(idx / per_row);
+        const unsigned long long d = (unsigned long long)(t0[r] * width + idx % per_row);
+        out[idx] = (float)(stream_draw(stream_key(seeds[r], stream_id), d) >> 40) * 0x1p-24f;
     }
 }
 }  // namespace
@@ -399,6 +437,14 @@ int b200tts_decoder_forward_chunk(const b200tts_decoder_shape* shape, const b200
     return decoder_forward_impl(*shape, *params, *in, *out, (float*)workspace, workspace_bytes, (cudaStream_t)stream, state, first);
 }
 
+int b200tts_decoder_state_reset_rows(const b200tts_decoder_shape* shape, b200tts_decoder_state* state, const int32_t* rows, int count,
+                                     void* stream) {
+    B200_REQUIRE(shape && state, "decoder_state_reset_rows: null argument");
+    B200_TRY(decoder_state_reset_rows_check(*shape, *state, rows, count));
+    B200_TRY(require_device());
+    return decoder_state_reset_rows_impl(*shape, *state, rows, count, (cudaStream_t)stream);
+}
+
 int b200tts_decoder_backward(const b200tts_decoder_shape* shape, const b200tts_decoder_params* params,
                              const b200tts_decoder_inputs* in, const b200tts_decoder_outputs* fwd_out,
                              const b200tts_decoder_output_grads* dout, const void* fwd_workspace, void* bwd_workspace,
@@ -625,11 +671,38 @@ int b200tts_fill_keep_mask(uint8_t* mask, size_t n, float drop_rate, uint64_t se
     B200_REQUIRE(drop_rate >= 0.f && drop_rate < 1.f, "fill_keep_mask: rate must be in [0,1)");
     if (n == 0) return B200TTS_OK;
     const unsigned threshold = (unsigned)(drop_rate * 65536.0f + 0.5f);
-    const unsigned long long key = mix64(seed ^ 0xD6E8FEB86659FD93ull) ^ (stream_id * 0xA24BAED4963EE407ull);
+    const unsigned long long key = stream_key(seed, stream_id);
     size_t quads = (n + 15) / 16;
     int blocks = (int)((quads + 255) / 256 > NUM_SMS * 16 ? NUM_SMS * 16 : (quads + 255) / 256);
     if (blocks < 1) blocks = 1;
     fill_keep_mask_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(mask, n, threshold, key, g_mask_epoch);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+int b200tts_fill_keep_mask_rows(uint8_t* mask, int steps, int rows, int width, float drop_rate, const uint64_t* seeds, const int64_t* step0,
+                                uint64_t stream_id, void* stream) {
+    B200_REQUIRE(steps >= 0 && rows >= 1 && width >= 1, "fill_keep_mask_rows: %d steps, %d rows, width %d", steps, rows, width);
+    B200_REQUIRE((mask || steps == 0) && seeds && step0, "fill_keep_mask_rows: null mask, seeds or step0");
+    B200_REQUIRE(drop_rate >= 0.f && drop_rate < 1.f, "fill_keep_mask_rows: rate must be in [0,1)");
+    B200_TRY(require_device());
+    if (steps == 0) return B200TTS_OK;
+    const unsigned threshold = (unsigned)(drop_rate * 65536.0f + 0.5f);
+    fill_keep_mask_rows_kernel<<<grid_for((size_t)steps * rows * width), 256, 0, (cudaStream_t)stream>>>(
+        mask, steps, rows, width, threshold, reinterpret_cast<const unsigned long long*>(seeds), reinterpret_cast<const long long*>(step0),
+        stream_id);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+int b200tts_fill_uniform_rows(float* out, int rows, int nsteps, int width, const uint64_t* seeds, const int64_t* t0, uint64_t stream_id,
+                              void* stream) {
+    B200_REQUIRE(rows >= 1 && nsteps >= 0 && width >= 1, "fill_uniform_rows: %d rows, %d steps, width %d", rows, nsteps, width);
+    B200_REQUIRE((out || nsteps == 0) && seeds && t0, "fill_uniform_rows: null output, seeds or t0");
+    B200_TRY(require_device());
+    if (nsteps == 0) return B200TTS_OK;
+    fill_uniform_rows_kernel<<<grid_for((size_t)rows * nsteps * width), 256, 0, (cudaStream_t)stream>>>(
+        out, rows, nsteps, width, reinterpret_cast<const unsigned long long*>(seeds), reinterpret_cast<const long long*>(t0), stream_id);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }

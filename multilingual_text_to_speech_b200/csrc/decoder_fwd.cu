@@ -403,10 +403,46 @@ __global__ void __launch_bounds__(ATT_THREADS) fwd_attn_fwd_kernel(const FwdAttn
     }
 }
 
-// alpha_0 = one-hot at position 0 (ForwardAttention.reset, attention.py:103-106): dst[r * ld] = 1 for every row r
-__global__ void set_first_column_kernel(float* __restrict__ dst, int ld, int rows) {
-    const int r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r < rows) dst[(size_t)r * ld] = 1.f;
+// The initial state of a decode (tacotron2.py:164-168): every buffer zero, and for forward attention alpha_0 = one-hot at position 0
+// (ForwardAttention.reset, attention.py:103-106).  Its one definition: the first chunk of a decode writes it into the step-0 rows of its
+// workspace, b200tts_decoder_state_reset_rows into the listed rows of a carried state.
+struct DecInitRows {
+    float* ctx; int ld_ctx;             // [rows, M] at row stride ld_ctx
+    float* att_h; int ld_att_h;         // [rows, D] at row stride ld_att_h
+    float* att_c; float* gen_h; float* gen_c;   // [rows, D]
+    float* cum;                         // [rows, L]
+    float* frame;                       // [rows, N]; N = 0 when absent
+    int M, D, L, N, one_hot;
+    int n;                              // listed rows; 0: rows 0 .. count - 1
+    int row[B200TTS_DECODER_RESET_MAX_ROWS];
+};
+__global__ void decoder_init_rows_kernel(const __grid_constant__ DecInitRows a, int count) {
+    const int W = a.M + 4 * a.D + a.L + a.N;
+    const long long n = (long long)count * W;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < n; idx += (long long)gridDim.x * blockDim.x) {
+        const int k = (int)(idx / W);
+        int c = (int)(idx % W);
+        const size_t r = a.n ? (size_t)a.row[k] : (size_t)k;
+        if (c < a.M) { a.ctx[r * a.ld_ctx + c] = 0.f; continue; }
+        c -= a.M;
+        if (c < a.D) { a.att_h[r * a.ld_att_h + c] = 0.f; continue; }
+        c -= a.D;
+        if (c < a.D) { a.att_c[r * a.D + c] = 0.f; continue; }
+        c -= a.D;
+        if (c < a.D) { a.gen_h[r * a.D + c] = 0.f; continue; }
+        c -= a.D;
+        if (c < a.D) { a.gen_c[r * a.D + c] = 0.f; continue; }
+        c -= a.D;
+        if (c < a.L) { a.cum[r * a.L + c] = (a.one_hot && c == 0) ? 1.f : 0.f; continue; }
+        a.frame[r * a.N + c - a.L] = 0.f;
+    }
+}
+
+int launch_init_rows(const DecInitRows& a, int count, cudaStream_t st) {
+    if (count <= 0) return B200TTS_OK;
+    decoder_init_rows_kernel<<<grid_for((size_t)count * (a.M + 4 * a.D + a.L + a.N)), 256, 0, st>>>(a, count);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
 }
 
 }  // namespace
@@ -661,16 +697,12 @@ int decoder_forward_impl(const b200tts_decoder_shape& frames, const b200tts_deco
         B200_TRY(launch_copy2d(c.at(l.hg), D, state->gen_h, D, B, D, st));
         B200_TRY(launch_copy2d(c.at(l.cg), D, state->gen_c, D, B, D, st));
         B200_TRY(launch_copy2d(c.at(l.cum), s.L, state->cum_weights, s.L, B, s.L, st));
-    } else {
-    B200_TRY(launch_fill(c.at(l.ai), 0.f, (size_t)B * MD, st));
-    B200_TRY(launch_fill(c.at(l.ca), 0.f, BD, st));
-    B200_TRY(launch_fill(c.at(l.hg), 0.f, BD, st));
-    B200_TRY(launch_fill(c.at(l.cg), 0.f, BD, st));
-    B200_TRY(launch_fill(c.at(l.cum), 0.f, (size_t)B * s.L, st));
-    if (forward_attention(s)) {
-        set_first_column_kernel<<<cdiv(B, 128), 128, 0, st>>>(c.at(l.cum), s.L, B);
-        B200_LAUNCH_CHECK();
-    }
+    } else {        // the step-0 rows of the workspace; the step-0 frame is zero-filled by the free-running step below
+        DecInitRows a{};
+        a.ctx = c.at(l.ai); a.ld_ctx = MD; a.att_h = c.at(l.ai) + M; a.ld_att_h = MD;
+        a.att_c = c.at(l.ca); a.gen_h = c.at(l.hg); a.gen_c = c.at(l.cg); a.cum = c.at(l.cum);
+        a.M = M; a.D = D; a.L = s.L; a.one_hot = forward_attention(s);
+        B200_TRY(launch_init_rows(a, B, st));
     }
 
     const bool persistent = !sequential && state == nullptr && precision_mode() == B200TTS_PRECISION_BF16 && persist_plan(s).fwd;
@@ -794,6 +826,35 @@ int forward_attention_step_impl(int B, int L, int M, int D, int A, const float* 
     fa.B = B; fa.L = L; fa.M = M; fa.A = A;
     B200_TRY(launch_fwd_attn(fa, st));
     B200_TRY(launch_copy2d(alpha, L, alpha_next, L, B, L, st));
+    return B200TTS_OK;
+}
+
+// ---- initial state of listed rows of a carried state (b200tts_decoder_state_reset_rows) ----
+int decoder_state_reset_rows_check(const b200tts_decoder_shape& s, const b200tts_decoder_state& state, const int* rows, int count) {
+    B200_REQUIRE(s.B > 0 && s.L > 0 && s.M > 0 && s.D > 0 && s.N > 0, "decoder_state_reset_rows: non-positive dimension (B=%d L=%d M=%d D=%d N=%d)",
+                 s.B, s.L, s.M, s.D, s.N);
+    B200_REQUIRE(s.att_kind == B200TTS_ATT_LOCATION || s.att_kind == B200TTS_ATT_FORWARD, "decoder_state_reset_rows: bad attention kind %d",
+                 s.att_kind);
+    B200_REQUIRE(state.att_h && state.att_c && state.gen_h && state.gen_c && state.context && state.cum_weights && state.frame,
+                 "decoder_state_reset_rows: every state buffer is required");
+    B200_REQUIRE(rows && count >= 1 && count <= s.B, "decoder_state_reset_rows: %d rows of a state of %d", count, s.B);
+    for (int k = 0; k < count; ++k)
+        B200_REQUIRE(rows[k] >= 0 && rows[k] < s.B, "decoder_state_reset_rows: row %d outside [0, %d)", rows[k], s.B);
+    return B200TTS_OK;
+}
+
+int decoder_state_reset_rows_impl(const b200tts_decoder_shape& s, const b200tts_decoder_state& state, const int* rows, int count,
+                                  cudaStream_t st) {
+    B200_TRY(decoder_state_reset_rows_check(s, state, rows, count));
+    DecInitRows a{};
+    a.ctx = state.context; a.ld_ctx = s.M; a.att_h = state.att_h; a.ld_att_h = s.D;
+    a.att_c = state.att_c; a.gen_h = state.gen_h; a.gen_c = state.gen_c; a.cum = state.cum_weights; a.frame = state.frame;
+    a.M = s.M; a.D = s.D; a.L = s.L; a.N = s.N; a.one_hot = forward_attention(s);
+    for (int k0 = 0; k0 < count; k0 += B200TTS_DECODER_RESET_MAX_ROWS) {
+        a.n = count - k0 < B200TTS_DECODER_RESET_MAX_ROWS ? count - k0 : B200TTS_DECODER_RESET_MAX_ROWS;
+        for (int k = 0; k < a.n; ++k) a.row[k] = rows[k0 + k];
+        B200_TRY(launch_init_rows(a, a.n, st));
+    }
     return B200TTS_OK;
 }
 

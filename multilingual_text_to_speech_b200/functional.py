@@ -96,6 +96,31 @@ def fill_keep_mask(shape, rate, seed, stream_id, device):
     return mask
 
 
+def _seed_tensor(seeds, device):
+    """Request seeds (ints in [0, 2^64)) as a device int64 tensor holding their uint64 bits."""
+    return torch.tensor([int(s) - (1 << 64) if int(s) >= 1 << 63 else int(s) for s in seeds], dtype=torch.int64, device=device)
+
+
+def fill_keep_mask_rows(steps, width, rate, seeds, step0, stream_id, device):
+    """Seeded keep masks [steps, len(seeds), width] (b200tts_fill_keep_mask_rows): row r continues, from step step0[r], the stream of
+    fill_keep_mask((S, width), rate, seeds[r], stream_id)."""
+    mask = torch.empty(int(steps), len(seeds), int(width), dtype=torch.uint8, device=device)
+    s, t = _seed_tensor(seeds, device), torch.tensor([int(v) for v in step0], dtype=torch.int64, device=device)
+    check(_lib.load().b200tts_fill_keep_mask_rows(ptr(mask), int(steps), len(seeds), int(width), float(rate), ptr(s), ptr(t), int(stream_id),
+                                                 _stream()), 'b200tts_fill_keep_mask_rows')
+    return mask
+
+
+def fill_uniform_rows(nsteps, width, seeds, t0, stream_id, device):
+    """Seeded uniforms in [0, 1), [len(seeds), nsteps, width] (b200tts_fill_uniform_rows): row r holds draws [t0[r] width, (t0[r] +
+    nsteps) width) of the stream keyed by (seeds[r], stream_id)."""
+    out = torch.empty(len(seeds), int(nsteps), int(width), dtype=torch.float32, device=device)
+    s, t = _seed_tensor(seeds, device), torch.tensor([int(v) for v in t0], dtype=torch.int64, device=device)
+    check(_lib.load().b200tts_fill_uniform_rows(ptr(out), len(seeds), int(nsteps), int(width), ptr(s), ptr(t), int(stream_id), _stream()),
+          'b200tts_fill_uniform_rows')
+    return out
+
+
 # ------------------------------------------------------------------------------------------------
 # single attention step (module-level API of LocationSensitiveAttention)
 # ------------------------------------------------------------------------------------------------
@@ -351,6 +376,28 @@ class DecoderState:
         """Keep only the utterances `rows` (a device index tensor), in that order: a finished utterance leaves the decode."""
         for name in ('att_h', 'att_c', 'gen_h', 'gen_c', 'context', 'cum_weights', 'frame'):
             setattr(self, name, getattr(self, name).index_select(0, rows).contiguous())
+
+    def grow(self, b, L):
+        """Appends b rows (their values unset until reset_rows) and re-pads cum_weights to L positions: zeros past a row's old width
+        (attention weights past a text's length are zero), or the first L positions when L is smaller."""
+        for name in ('att_h', 'att_c', 'gen_h', 'gen_c', 'context', 'frame'):
+            t = getattr(self, name)
+            setattr(self, name, torch.cat([t, t.new_empty(b, t.shape[1])]) if b else t)
+        cum = self.cum_weights
+        out = cum.new_zeros(cum.shape[0] + b, L)
+        w = min(L, cum.shape[1])
+        out[:cum.shape[0], :w] = cum[:, :w]
+        self.cum_weights = out
+
+    def reset_rows(self, rows, forward_attention):
+        """The initial state of a decode in `rows` (host ints; b200tts_decoder_state_reset_rows); other rows are untouched."""
+        B, L = self.cum_weights.shape
+        shape = DecoderShape(B=B, L=L, M=self.context.shape[1], D=self.att_h.shape[1], N=self.frame.shape[1],
+                             att_kind=_lib.ATT_FORWARD if forward_attention else _lib.ATT_LOCATION)
+        rows = [int(r) for r in rows]
+        st = self.struct()
+        check(_lib.load().b200tts_decoder_state_reset_rows(ctypes.byref(shape), ctypes.byref(st), (ctypes.c_int * len(rows))(*rows), len(rows),
+                                                           _stream()), 'b200tts_decoder_state_reset_rows')
 
     def struct(self):
         return _lib.DecoderState(*[ptr(t) for t in (self.att_h, self.att_c, self.gen_h, self.gen_c, self.context, self.cum_weights, self.frame)])

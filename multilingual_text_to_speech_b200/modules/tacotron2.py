@@ -218,61 +218,24 @@ class Decoder(torch.nn.Module):
         return [j for j, r in enumerate(rows) if rules[r].cut is None]
 
     def _inference_chunks(self, encoded_input, mask, speaker, language, att_extent=0, tape_columns=None, chunk_frames=None):
-        """The chunk loop of free-running inference (tacotron2.py:148-209 with target=None): every chunk is one library call of
-        chunk_frames (default inference_chunk) frames rounded down to whole steps; after each it feeds the chunk's stop logits to the
-        utterances' stop rules and yields (rows, spec [b, Tc, N], stop [b, Tc], alignment [b, Tc / r, L], rules, done): rows are the
-        original indices of the b utterances the chunk decoded, rules the stop rule of every utterance, done the frames decoded so far.
-        Then an utterance whose cut is known leaves the decode: the state, memory, lengths and rules are compacted to the utterances still
-        running, and the next chunk runs at the smaller batch.  The loop ends when every cut is known or hp.max_output_length frames are
-        decoded.  The rule reads the r stop logits of each step in frame order."""
+        """The chunk loop of free-running inference (tacotron2.py:148-209 with target=None) over a batch whose texts all open at the
+        first call: every chunk is one library call of chunk_frames (default inference_chunk) frames rounded down to whole steps; after
+        each it feeds the chunk's stop logits to the utterances' stop rules and yields (rows, spec [b, Tc, N], stop [b, Tc], alignment
+        [b, Tc / r, L], rules, done): rows are the original indices of the b utterances the chunk decoded, rules the stop rule of every
+        utterance, done the frames decoded so far.  Then an utterance whose cut is known leaves the decode (_DecodeRows.retire) and the next
+        chunk runs at the smaller batch.  The loop ends when every cut is known or hp.max_output_length frames are decoded.  The rule reads
+        the r stop logits of each step in frame order.  Utterance b reads column tape_columns[b] (default b) of an active mask tape."""
         memory = self._memory(encoded_input, speaker, language)
-        B, L, M = memory.shape
-        device = memory.device
-        P, D, N = self._prenet._layers[0].weight.shape[0], self._decoder_dim, self._output_dim
-        kind, rate_h, rate_c = self._cell_config()
-        lengths = mask.sum(dim=1).to(torch.int32)
-        state = F.DecoderState(B, D, M, L, N, device)
-        rules = [self._StopRule(hp.stop_frames) for _ in range(B)]
-        rows = list(range(B))                  # original index of every utterance still decoding
+        B = memory.shape[0]
         columns = list(range(B)) if tape_columns is None else list(tape_columns)
-        done = 0                               # frames decoded (a whole number of steps)
-        params = self._param_list()
-        r = self._outputs_per_step
-        chunk_steps = max(1, (self.inference_chunk if chunk_frames is None else int(chunk_frames)) // r)
-        while done < self._max_frames:
-            Sc = min(chunk_steps, self._steps(self._max_frames - done))
-            Tc = Sc * r
-            masks = {}
-            for name in ('step_prenet0', 'step_prenet1'):
-                tape = MaskSource.raw(name)
-                if MaskSource.tape is not None:
-                    if tape is not None:
-                        masks[name] = self._tape_part(tape, done // r, Sc, [columns[j] for j in rows]).to(device=device, dtype=torch.uint8).contiguous()
-                else:
-                    m = MaskSource.keep_mask(name, (Sc, len(rows), P), self._prenet._dropout_rate, device)
-                    if m is not None:
-                        masks[name] = m
-            if self.training:
-                for name in ('att_h', 'gen_h') + (('att_c', 'gen_c') if kind == _lib.CELL_ZONEOUT else ()):
-                    m = MaskSource.keep_mask(name, (Sc, len(rows), D), rate_c if name.endswith('_c') else rate_h, device)
-                    if m is not None:
-                        masks[name] = m
-            cfg = F.DecoderConfig(kind, self.training, rate_h, rate_c, self._prenet._dropout_rate, masks, np.zeros(Sc, dtype=np.uint8),
-                                  att_extent, outputs_per_step=r)
-            spec, stop, align = F.decoder_forward_chunk(cfg, memory, lengths, params, state, Tc)
-            done += Tc
-            host_stop = stop.float().cpu()
-            for j, u in enumerate(rows):
-                rules[u].feed(host_stop[j])
-            yield rows, spec, stop, align, rules, done
-            keep = self._retire(rows, rules)
-            if not keep:
-                break
-            if len(keep) < len(rows):
-                idx = torch.tensor(keep, device=device)
-                state.select(idx)
-                memory, lengths = memory.index_select(0, idx), lengths.index_select(0, idx)
-                rows = [rows[j] for j in keep]
+        rows = _DecodeRows(self, att_extent)
+        rows.add(memory, [int(n) for n in mask.sum(dim=1).tolist()], list(range(B)), [('shared', c) for c in columns])
+        rules = list(rows.rules)
+        chunk_steps = max(1, (self.inference_chunk if chunk_frames is None else int(chunk_frames)) // self._outputs_per_step)
+        while len(rows):
+            spec, stop, align = rows.step(chunk_steps)
+            yield list(rows.keys), spec, stop, align, rules, rows.done[0]
+            rows.retire()
 
     def _decode_inference(self, encoded_input, mask, speaker, language, att_extent=0, tape_columns=None):
         """Free-running decode in chunks with carried state and early exit (_inference_chunks).  B == 1 reproduces the reference; B > 1
@@ -287,6 +250,8 @@ class Decoder(torch.nn.Module):
         outs = [[] for _ in range(B)]
         done = 0
         for rows, spec, stop, align, rules, done in self._inference_chunks(encoded_input, mask, speaker, language, att_extent, tape_columns):
+            if align.shape[2] < L:          # the chunk ran after the longest text left: its weights past the shorter ones are zero
+                align = TF.pad(align, (0, L - align.shape[2]))
             for j, u in enumerate(rows):
                 outs[u].append((spec[j], stop[j], align[j]))
         cuts = [min(rule.cut if rule.cut is not None else done, self._max_frames) for rule in rules]
@@ -481,32 +446,15 @@ class Tacotron(torch.nn.Module):
             raise ValueError(f'{name}: at most {MAX_STREAM_TEXTS} texts decode as one group (got {len(texts)})')
         if chunk_frames is not None and int(chunk_frames) < 1:
             raise ValueError(f'{name}: chunk_frames must be >= 1 (got {chunk_frames})')
-        was_training = self.training
-        self.eval()
-        try:
-            with torch.no_grad():
-                encoded, mask, speaker, language = self._encode_group(texts, speakers, languages)
-            dec, halo = self._decoder, self._postnet.halo()
-            B = len(texts)
-            pre, released = [[] for _ in range(B)], [0] * B
-            chunks = dec._inference_chunks(encoded, mask, speaker, language, att_extent=1, tape_columns=list(range(B)), chunk_frames=chunk_frames)
-            while True:
-                with torch.no_grad():
-                    item = next(chunks, None)
-                    if item is None:
-                        return
-                    rows, spec, _, _, rules, done = item
-                    spans = {}
-                    for j, u in enumerate(rows):
-                        pre[u].append(spec[j])
-                        end = stream_release(done, rules[u].cut, dec._max_frames, halo)
-                        final = rules[u].cut is not None or done >= dec._max_frames
-                        spans[u] = (released[u], end, end if final else done)
-                        released[u] = end
-                    posts = self._postnet_windows(pre, spans, halo)
-                yield posts
-        finally:
-            self.train(was_training)
+        pool = self.decoder_pool(len(texts), chunk_frames)
+        for i, text in enumerate(texts):        # ids 0 .. B - 1: text i reads column i of a recorded mask tape
+            pool.open(text, None if speakers is None else speakers[i], None if languages is None else languages[i])
+        while pool.ids:
+            yield pool.run()
+
+    def decoder_pool(self, max_texts=64, chunk_frames=None):
+        """A DecoderPool of up to max_texts texts decoded in chunks of chunk_frames frames (default Decoder.inference_chunk)."""
+        return DecoderPool(self, max_texts, chunk_frames)
 
     def _postnet_windows(self, pre, spans, halo):
         """{u: post-net output frames [t0, t1) [num_mels, t1 - t0]} for spans {u: (t0, t1, avail)} of the decoded frames pre[u] (chunks of
@@ -568,6 +516,264 @@ class Tacotron(torch.nn.Module):
 
 # texts of one inference_streams group at most: the batch inference_batch decodes at once by default
 MAX_STREAM_TEXTS = 64
+
+PRENET_SITES = ('step_prenet0', 'step_prenet1')
+
+
+class _DecodeRows:
+    """The rows of a running free-running decode, one per text, and its one chunk loop (Decoder._inference_chunks, DecoderPool).  It
+    holds the memory [B, L, M] and lengths of the open texts, re-padded to the longest of them (L grows when a longer text joins and
+    shrinks when the longest leaves; attention weights past a text's length are exact zeros, so a row's frames do not depend on L), the
+    carried DecoderState, and per row its key, stop rule, frames decoded and prenet mask source:
+      * ('tape', {site: [S, P]}): the row's own recorded masks, step i of the row reading row i (all-ones past the tape's end);
+      * ('seed', seed): b200tts_fill_keep_mask_rows at the row's own step count, stream _lib.SEED_STREAMS[site];
+      * ('shared', column): with a MaskSource tape active, that column of it; otherwise one MaskSource draw over every shared row per
+        call, as the batched decode has always drawn."""
+
+    def __init__(self, dec, att_extent):
+        self.dec, self.att_extent = dec, att_extent
+        self.memory = self.lengths = self.state = None
+        self.keys, self.rules, self.done, self.sources, self.text_len = [], [], [], [], []
+
+    def __len__(self):
+        return len(self.keys)
+
+    def add(self, memory, lengths, keys, sources):
+        """Appends texts: memory [b, Lb, M] (speaker / language columns included), lengths (host ints), one key and one mask source each.
+        The memory, lengths and cum_weights are re-padded to the longest open text and the new state rows are set to a decode's initial
+        state (b200tts_decoder_state_reset_rows)."""
+        dec, n, b = self.dec, len(self.keys), memory.shape[0]
+        L = max(list(lengths) + self.text_len)
+        M, device = memory.shape[2], memory.device
+        if n == 0:
+            self.memory = memory[:, :L]
+            self.lengths = torch.tensor(lengths, dtype=torch.int32, device=device)
+            self.state = F.DecoderState(0, dec._decoder_dim, M, L, dec._output_dim, device)
+        else:
+            grown = memory.new_zeros(n + b, L, M)
+            grown[:n, :self.memory.shape[1]] = self.memory
+            grown[n:, :min(L, memory.shape[1])] = memory[:, :L]
+            self.memory = grown
+            self.lengths = torch.cat([self.lengths, torch.tensor(lengths, dtype=torch.int32, device=device)])
+        self.state.grow(b, L)
+        self.state.reset_rows(range(n, n + b), getattr(dec._attention, '_location', None) is None)
+        self.state.first = False
+        self.keys += list(keys)
+        self.rules += [dec._StopRule(hp.stop_frames) for _ in range(b)]
+        self.done += [0] * b
+        self.sources += list(sources)
+        self.text_len += list(lengths)
+
+    def keep(self, js):
+        """Keeps rows js (positions, in order); the memory and cum_weights shrink to the longest text left."""
+        if len(js) == len(self.keys):
+            return
+        if not js:
+            self.__init__(self.dec, self.att_extent)
+            return
+        idx = torch.tensor(js, device=self.memory.device)
+        self.state.select(idx)
+        self.memory, self.lengths = self.memory.index_select(0, idx), self.lengths.index_select(0, idx)
+        for name in ('keys', 'rules', 'done', 'sources', 'text_len'):
+            setattr(self, name, [getattr(self, name)[j] for j in js])
+        L = max(self.text_len)
+        if L < self.memory.shape[1]:
+            self.memory = self.memory[:, :L].contiguous()
+            self.state.cum_weights = self.state.cum_weights[:, :L].contiguous()
+
+    def retire(self):
+        """Rows whose stop cut is known or that reached hp.max_output_length frames leave -> their keys."""
+        alive = set(self.dec._retire(range(len(self.keys)), self.rules))
+        js = [j for j in range(len(self.keys)) if j in alive and self.done[j] < self.dec._max_frames]
+        gone = [k for j, k in enumerate(self.keys) if j not in js]
+        self.keep(js)
+        return gone
+
+    def close(self, key):
+        self.keep([j for j, k in enumerate(self.keys) if k != key])
+
+    def _prenet_masks(self, Sc):
+        """{site: keep masks [Sc, B, P]} for the next call (a site without masks runs without dropout)."""
+        dec = self.dec
+        P, rate, r = dec._prenet._layers[0].weight.shape[0], dec._prenet._dropout_rate, dec._outputs_per_step
+        device, B = self.memory.device, len(self.keys)
+        kinds = [src[0] for src in self.sources]
+        shared = [j for j, k in enumerate(kinds) if k == 'shared']
+        masks = {}
+        for name in PRENET_SITES:
+            part = None
+            if shared:
+                if MaskSource.tape is not None:
+                    tape = MaskSource.raw(name)
+                    if tape is not None:
+                        by_done = {}
+                        for j in shared:
+                            by_done.setdefault(self.done[j], []).append(j)
+                        if len(by_done) == 1:
+                            part = dec._tape_part(tape, self.done[shared[0]] // r, Sc, [self.sources[j][1] for j in shared])
+                        else:
+                            part = torch.cat([dec._tape_part(tape, self.done[j] // r, Sc, [self.sources[j][1]]) for j in shared], 1)
+                        part = part.to(device=device, dtype=torch.uint8).contiguous()
+                else:
+                    part = MaskSource.keep_mask(name, (Sc, len(shared), P), rate, device)
+            if len(shared) == B:
+                if part is not None:
+                    masks[name] = part
+                continue
+            full = torch.ones(Sc, B, P, dtype=torch.uint8, device=device)
+            if part is not None:
+                full[:, shared] = part
+            seeded = [j for j, k in enumerate(kinds) if k == 'seed']
+            if seeded:
+                full[:, seeded] = F.fill_keep_mask_rows(Sc, P, rate, [self.sources[j][1] for j in seeded], [self.done[j] // r for j in seeded],
+                                                        _lib.SEED_STREAMS[name], device)
+            for j, k in enumerate(kinds):
+                if k == 'tape':
+                    full[:, j] = dec._tape_part(self.sources[j][1][name].unsqueeze(1), self.done[j] // r, Sc, [0])[:, 0].to(device)
+            masks[name] = full
+        return masks
+
+    def step(self, chunk_steps):
+        """One library call over every row: min(chunk_steps, the steps the furthest-from-done row has left) steps; feeds each row's stop
+        rule and step count -> (spec [B, Tc, N], stop [B, Tc], alignment [B, Tc / r, L]).  A row decoded past hp.max_output_length
+        discards those frames."""
+        dec = self.dec
+        r = dec._outputs_per_step
+        Sc = min(chunk_steps, max(dec._steps(dec._max_frames - d) for d in self.done))
+        D, device = dec._decoder_dim, self.memory.device
+        kind, rate_h, rate_c = dec._cell_config()
+        masks = self._prenet_masks(Sc)
+        if dec.training:
+            for name in ('att_h', 'gen_h') + (('att_c', 'gen_c') if kind == _lib.CELL_ZONEOUT else ()):
+                m = MaskSource.keep_mask(name, (Sc, len(self.keys), D), rate_c if name.endswith('_c') else rate_h, device)
+                if m is not None:
+                    masks[name] = m
+        cfg = F.DecoderConfig(kind, dec.training, rate_h, rate_c, dec._prenet._dropout_rate, masks, np.zeros(Sc, dtype=np.uint8),
+                              self.att_extent, outputs_per_step=r)
+        spec, stop, align = F.decoder_forward_chunk(cfg, self.memory, self.lengths, dec._param_list(), self.state, Sc * r)
+        host_stop = stop.float().cpu()
+        for j in range(len(self.keys)):
+            self.rules[j].feed(host_stop[j])
+            self.done[j] += Sc * r
+        return spec, stop, align
+
+
+class DecoderPool:
+    """Continuous-batching decode: texts join the running decoder group at any call and leave at their stop cut.  open() queues a text;
+    run() encodes the texts opened since the last call as one padded group (one per form of speaker / language inputs), appends their rows
+    to the running ones (_DecodeRows.add), makes one decoder call over every open text and returns {id: post-net chunk [num_mels, n]} as
+    Tacotron.inference_streams does (the released frames of every text through the post-net as one padded batch).  A text's chunks,
+    concatenated, are inference_stream of it alone, bit for bit in fp32 mode given the same masks, whenever it joined and whatever shares
+    its calls; every text keeps its own step count, stop rule and hp.max_output_length.
+
+    Prenet dropout masks per text: `masks` (a tape {'step_prenet0': [S, P], 'step_prenet1': [S, P]}) if given, else `seed` (draws that
+    depend on the seed and the text's own steps only: its masks are one b200tts_fill_keep_mask((S, P), seed, _lib.SEED_STREAMS[site])
+    call per site), else one shared MaskSource draw per call over such texts (with a MaskSource tape active: column `id` of it).  The
+    model runs each call in eval mode without autograd and is restored after it."""
+
+    def __init__(self, tacotron, max_texts=64, chunk_frames=None):
+        if not 1 <= int(max_texts) <= MAX_STREAM_TEXTS:
+            raise ValueError(f'a decoder pool holds 1 to {MAX_STREAM_TEXTS} texts (got {max_texts})')
+        if chunk_frames is not None and int(chunk_frames) < 1:
+            raise ValueError(f'decoder_pool: chunk_frames must be >= 1 (got {chunk_frames})')
+        self.t, self.max_texts = tacotron, int(max_texts)
+        dec = tacotron._decoder
+        self.chunk_steps = max(1, (dec.inference_chunk if chunk_frames is None else int(chunk_frames)) // dec._outputs_per_step)
+        self.rows = _DecodeRows(dec, att_extent=1)
+        self.queue = []                        # (id, text, speaker, language, source) opened since the last call
+        self.pre, self.released = {}, {}       # per open text: its decoded chunks [n, N], the frames its post-net chunks cover
+        self.next_id = 0
+
+    @property
+    def ids(self):
+        """Every open text: queued, then decoding."""
+        return [q[0] for q in self.queue] + list(self.rows.keys)
+
+    def check(self, text, speaker=None, language=None, seed=None, masks=None):
+        """Validates one text's inputs (ValueError) -> its mask source ('tape', {site: uint8 [S, P]}), ('seed', seed) or ('shared', None)."""
+        _check_batch_inputs([text], None if speaker is None else [speaker], None if language is None else [language])
+        if masks is not None:
+            P = self.t._decoder._prenet._layers[0].weight.shape[0]
+            if not isinstance(masks, dict) or set(masks) != set(PRENET_SITES):
+                raise ValueError(f'a mask tape is a dict with exactly the keys {PRENET_SITES}')
+            for k, v in masks.items():
+                if not torch.is_tensor(v) or v.dim() != 2 or v.shape[0] < 1 or v.shape[1] != P:
+                    raise ValueError(f'mask tape {k!r} must be a tensor [S >= 1, {P}]')
+                if not bool(((v == 0) | (v == 1)).all()):
+                    raise ValueError(f'mask tape {k!r} holds values other than 0 and 1')
+            device = self.t._embedding.weight.device
+            return 'tape', {k: v.to(device=device, dtype=torch.uint8).contiguous() for k, v in masks.items()}
+        if seed is not None:
+            if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= int(seed) < 1 << 64:
+                raise ValueError(f'a seed is an int in [0, 2^64) (got {seed!r})')
+            return 'seed', int(seed)
+        return 'shared', None
+
+    def open(self, text, speaker=None, language=None, seed=None, masks=None):
+        """Queues a text for the next run() -> its id.  Takes `inference`'s text, speaker and language, and a seed or a mask tape."""
+        source = self.check(text, speaker, language, seed, masks)
+        if len(self.ids) >= self.max_texts:
+            raise ValueError(f'the decoder pool is full: {self.max_texts} texts are open')
+        tid = self.next_id
+        self.next_id += 1
+        if source[0] == 'shared':
+            source = ('shared', tid)
+        self.queue.append((tid, text, speaker, language, source))
+        return tid
+
+    def close(self, tid):
+        """Drops an open text before its stop cut."""
+        if tid in self.rows.keys:
+            self.rows.close(tid)
+            del self.pre[tid], self.released[tid]
+        elif any(q[0] == tid for q in self.queue):
+            self.queue = [q for q in self.queue if q[0] != tid]
+        else:
+            raise ValueError(f'unknown or finished text {tid}')
+
+    def _admit(self):
+        t, groups = self.t, {}
+        for q in self.queue:
+            _, _, speaker, language, _ = q
+            form = (speaker is None, None if language is None else (language.dim(), language.shape[-1] if language.dim() == 3 else 0))
+            groups.setdefault(form, []).append(q)
+        self.queue = []
+        for group in groups.values():
+            ids, texts, speakers, languages, sources = zip(*group)
+            encoded, mask, speaker, language = t._encode_group(list(texts), None if speakers[0] is None else list(speakers),
+                                                                None if languages[0] is None else list(languages))
+            memory = t._decoder._memory(encoded, speaker, language)
+            self.rows.add(memory, [int(x.shape[0]) for x in texts], ids, sources)
+            for i in ids:
+                self.pre[i], self.released[i] = [], 0
+
+    def run(self):
+        """One decoder call over every open text -> {id: post-net chunk [num_mels, n]} (a chunk may hold no frames).  A text leaves after
+        the call that finds its stop cut or reaches hp.max_output_length frames."""
+        t = self.t
+        if not self.queue and not len(self.rows):
+            return {}
+        was_training = t.training
+        t.eval()
+        try:
+            with torch.no_grad():
+                if self.queue:
+                    self._admit()
+                spec, _, _ = self.rows.step(self.chunk_steps)
+                dec, halo, rows, spans = t._decoder, t._postnet.halo(), self.rows, {}
+                for j, u in enumerate(rows.keys):
+                    self.pre[u].append(spec[j])
+                    done, cut = rows.done[j], rows.rules[j].cut
+                    end = stream_release(done, cut, dec._max_frames, halo)
+                    final = cut is not None or done >= dec._max_frames
+                    spans[u] = (self.released[u], end, end if final else done)
+                    self.released[u] = end
+                posts = t._postnet_windows(self.pre, spans, halo)
+                for u in rows.retire():
+                    del self.pre[u], self.released[u]
+                return posts
+        finally:
+            t.train(was_training)
 
 
 def stream_release(done, cut, max_frames, halo):

@@ -692,8 +692,8 @@ class _PoolStream:
     """One stream of a StreamPool: its loop row, the mel frames that have arrived, its uniform tape (fp32 on the device, or None), the steps
     run and the samples released.  Its run but unreleased samples [released, steps) sit in the pool's per-row ring buffer."""
 
-    def __init__(self, slot, device, feat_dims, tape):
-        self.slot, self.tape = slot, tape
+    def __init__(self, slot, device, feat_dims, tape, seed=None):
+        self.slot, self.tape, self.seed = slot, tape, seed
         self.mel = torch.zeros(feat_dims, 0, device=device, dtype=torch.float32)
         self.chunks = 0
         self.steps = 0
@@ -710,12 +710,14 @@ class StreamPool:
     run independently (b200tts_wavernn_run_rows).  open() takes the lowest free row and resets it; feed() and end() add a stream's mel
     frames and mark its end; run() makes one loop call over every stream with samples ready, under generate_stream's rule (lookahead()
     frames after a sample's frame, the last 20 hops held back until end()), at most POOL_CALL_HOPS hops per call, and returns {sid: waveform
-    chunk} (CUDA tensors) for the streams that released samples.  A stream's row is freed when its final chunk is returned.
+    chunk} (CUDA tensors) for the streams that released samples.  A stream's row is freed when its final chunk is returned, or at once by
+    close().
 
     For each stream the concatenated chunks equal generate_stream of the same mel with the same uniform tape, bit for bit, whenever it
     joined, whatever else shares the loop and however its mel was chunked.  With preemphasis the stream is de-emphasised across calls and
     stays within generate_batch's bound.  Without a tape the uniforms are drawn with torch.rand (`generator` optional) once per call for all
-    rows, so they differ from a solo run's draws.  Every call runs in fp32 (the precision mode is set for the call and restored after it)
+    rows, so they differ from a solo run's draws; a stream opened with a seed draws its own (b200tts_fill_uniform_rows at its own step count,
+    stream _lib.SEED_STREAMS['vocoder']), which depend on the seed alone: its tape is one fill_uniform_rows row over [0, T).  Every call runs in fp32 (the precision mode is set for the call and restored after it)
     on the CUDA device that was current when the pool was made; each run() reads the loop's abort flag once.  The device work of a run()
     is a fixed number of launches whatever the number of streams: the per-stream windows, tapes and samples are gathered and scattered
     with indices built on the host."""
@@ -757,9 +759,12 @@ class StreamPool:
         finally:
             _lib.set_precision(precision)
 
-    def open(self, uniforms=None):
-        """A new stream on the lowest free row -> its id.  uniforms: its tape [1, T, U] as for generate_stream, or None."""
+    def open(self, uniforms=None, seed=None):
+        """A new stream on the lowest free row -> its id.  uniforms: its tape [1, T, U] as for generate_stream, or None; seed (an int in
+        [0, 2^64), used without a tape): the stream draws its uniforms from it."""
         tape = self.m._check_stream_tape(uniforms)
+        if seed is not None and (isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= int(seed) < 1 << 64):
+            raise ValueError(f'a seed is an int in [0, 2^64) (got {seed!r})')
         free = [r for r in range(self.rows) if self.slots[r] is None]
         if not free:
             raise ValueError(f'the stream pool is full: {self.rows} streams are open')
@@ -769,10 +774,17 @@ class StreamPool:
             self.last[slot] = 0.0
             if tape is not None:
                 tape = tape[0].to(device=self.device, dtype=torch.float32).contiguous()
-            self.streams[sid] = _PoolStream(slot, self.device, self.m.feat_dims, tape)
+            self.streams[sid] = _PoolStream(slot, self.device, self.m.feat_dims, tape, None if seed is None else int(seed))
         self.slots[slot] = sid
         self.next_sid += 1
         return sid
+
+    def close(self, sid):
+        """Drops stream sid and frees its row at once, whatever it has run or released."""
+        st = self.streams.pop(sid, None)
+        if st is None:
+            raise ValueError(f'unknown or finished stream {sid}')
+        self.slots[st.slot] = None
 
     def _stream(self, sid):
         st = self.streams.get(sid)
@@ -859,11 +871,16 @@ class StreamPool:
         n = np.array([plan[sid][1] for sid in live], np.int64)
         row_t, row_n = np.zeros(active, np.int64), np.zeros(active, np.int32)
         row_t[slot], row_n[slot] = t, n
-        # uniforms: the taped rows' steps gathered from their tapes (source 0 is a zero), the rest drawn
+        # uniforms: the taped rows' steps gathered from their tapes (source 0 is a zero) and the seeded rows' from one seeded draw, in one
+        # gather; the other rows' drawn for the call
         taped = [sid for sid in live if self.streams[sid].tape is not None]
-        if taped:
-            src = torch.cat([torch.zeros(1, device=dev)] + [self.streams[sid].tape[plan[sid][0]:plan[sid][0] + plan[sid][1]].reshape(-1)
-                                                            for sid in taped])
+        seeded = [sid for sid in live if self.streams[sid].tape is None and self.streams[sid].seed is not None]
+        if taped or seeded:
+            parts = [torch.zeros(1, device=dev)] + [self.streams[sid].tape[plan[sid][0]:plan[sid][0] + plan[sid][1]].reshape(-1) for sid in taped]
+            if seeded:
+                parts.append(F.fill_uniform_rows(nmax, U, [self.streams[sid].seed for sid in seeded], [plan[sid][0] for sid in seeded],
+                                                 _lib.SEED_STREAMS['vocoder'], dev).reshape(-1))
+            src = torch.cat(parts)
             idx = np.zeros((active, nmax, U), np.int64)
             off = 1
             i = np.arange(nmax)[:, None] * U + np.arange(U)[None, :]
@@ -871,12 +888,16 @@ class StreamPool:
                 st, k = self.streams[sid], plan[sid][1]
                 idx[st.slot, :k] = off + i[:k]
                 off += k * U
+            for sid in seeded:
+                st, k = self.streams[sid], plan[sid][1]
+                idx[st.slot, :k] = off + i[:k]
+                off += nmax * U
             uni = src[self._upload(idx)]
-        if len(taped) < len(live):
+        if len(taped) + len(seeded) < len(live):
             drawn = torch.rand(active, nmax, U, device=dev, dtype=torch.float32, generator=self.generator)
-            if taped:
+            if taped or seeded:
                 has = np.zeros((active, 1, 1), bool)
-                has[[self.streams[sid].slot for sid in taped]] = True
+                has[[self.streams[sid].slot for sid in taped + seeded]] = True
                 uni = torch.where(self._upload(has), uni, drawn)
             else:
                 uni = drawn
