@@ -409,6 +409,15 @@ int b200tts_bilstm_forward(const b200tts_bilstm_shape* shape, const b200tts_bils
 int b200tts_bilstm_backward(const b200tts_bilstm_shape* shape, const b200tts_bilstm_params* params,
                             const int32_t* lengths, const void* saved, const float* dout, float* dx,
                             const b200tts_bilstm_params* d_params, void* workspace, void* stream);
+/* Debug: where the bi-LSTM keeps its per-step state, so that tests can check every step of both directions (pure host arithmetic,
+ * no device needed).  Fills out[0 .. n) in this order:
+ *   saved (byte offsets):     xp [2][L][B][E], gates [2][L][B][4H], hs [2][L + 1][B][H], cs [2][L + 1][B][H], bsum [2][4H]
+ *   workspace (byte offsets): dg [2][L][B][4H], dxp [2][L][B][E]
+ *   split-K factors of the per-step chain's recurrent products (forward, backward), 1 if the persistent kernel runs the recurrence
+ * Direction-major, in processing order (step j is position j forward, L-1-j reverse).  The persistent kernel reads
+ * B200TTS_BILSTM_CHAIN as the forward and backward calls do.  Returns the number of values written (10 when n >= 10), 0 for a
+ * rejected shape. */
+int b200tts_debug_bilstm_layout(const b200tts_bilstm_shape* shape, size_t* out, int n);
 
 /* ---- loss: TacotronLoss.forward, modules/tacotron2.py:439-485 (guided attention :439-457 in closed form) ----
  * pre / post / targets [B, N, T]; stop (logits, padded positions already filled as in tacotron2.py:380) / stop_target [B, T]; alignment

@@ -204,6 +204,7 @@ SIGNATURES = {
                                        c_void_p, c_void_p]),
     'b200tts_bilstm_backward': (c_int, [POINTER(BiLSTMShape), POINTER(BiLSTMParams), c_void_p, c_void_p, c_void_p, c_void_p,
                                         POINTER(BiLSTMParams), c_void_p, c_void_p]),
+    'b200tts_debug_bilstm_layout': (c_int, [POINTER(BiLSTMShape), POINTER(c_size_t), c_int]),
     'b200tts_loss_workspace_bytes': (c_size_t, []),
     'b200tts_tacotron_loss_forward': (c_int, [POINTER(LossShape)] + [c_void_p] * 12),
     'b200tts_tacotron_loss_backward': (c_int, [POINTER(LossShape)] + [c_void_p] * 14),

@@ -126,6 +126,7 @@ int embedding_backward_impl(float* dtable, int V, const float* dout, int ldo, co
                             cudaStream_t st);
 size_t bilstm_saved_floats(const b200tts_bilstm_shape& s);
 size_t bilstm_workspace_floats(const b200tts_bilstm_shape& s);
+void bilstm_view_offsets(const b200tts_bilstm_shape& s, size_t* v);
 int bilstm_forward_impl(const b200tts_bilstm_shape& s, const b200tts_bilstm_params& w, const float* x, const int* lengths, float* out,
                         float* saved, float* ws, cudaStream_t st);
 int bilstm_backward_impl(const b200tts_bilstm_shape& s, const b200tts_bilstm_params& w, const int* lengths, const float* saved,
@@ -362,6 +363,14 @@ int b200tts_debug_decoder_views(const b200tts_decoder_shape* shape, size_t* out,
     v[24] = (size_t)g.Kp_att;
     v[25] = (size_t)g.Kp_gen;
     const int m = n < 26 ? n : 26;
+    for (int k = 0; k < m; ++k) out[k] = v[k];
+    return m;
+}
+int b200tts_debug_bilstm_layout(const b200tts_bilstm_shape* shape, size_t* out, int n) {
+    if (!shape || !out || shape->B <= 0 || shape->L <= 0 || shape->E <= 0 || shape->H <= 0) return 0;
+    size_t v[10];
+    bilstm_view_offsets(*shape, v);
+    const int m = n < 10 ? n : 10;
     for (int k = 0; k < m; ++k) out[k] = v[k];
     return m;
 }

@@ -77,6 +77,16 @@ RnnLayout rnn_layout(const b200tts_bilstm_shape& s) {
 
 size_t bilstm_saved_floats(const b200tts_bilstm_shape& s) { return rnn_layout(s).total; }
 size_t bilstm_workspace_floats(const b200tts_bilstm_shape& s) { return rnn_layout(s).wtotal; }
+// b200tts_debug_bilstm_layout: byte offsets of xp, gates, hs, cs, bsum (saved) and dg, dxp (workspace), the split-K factors of the
+// chain's recurrent products (forward, backward) and whether the persistent kernel runs
+void bilstm_view_offsets(const b200tts_bilstm_shape& s, size_t* v) {
+    const RnnLayout l = rnn_layout(s);
+    const size_t f[7] = {l.xp, l.gates, l.hs, l.cs, l.bsum, l.dg, l.dxp};
+    for (int k = 0; k < 7; ++k) v[k] = f[k] * sizeof(float);
+    v[7] = (size_t)l.split;
+    v[8] = (size_t)l.split_b;
+    v[9] = bilstm_persist_supported(s) ? 1 : 0;
+}
 
 int bilstm_forward_impl(const b200tts_bilstm_shape& s, const b200tts_bilstm_params& w, const float* x, const int* lengths, float* out,
                         float* saved, float* ws, cudaStream_t st) {
