@@ -677,6 +677,24 @@ int b200tts_wavernn_deemphasis(int rows, int len, int mu, float a, float* y, voi
  * order, and the last 20 hop samples multiplied by linspace(1, 0, 20 hop).  fp64 arithmetic, fp32 output; total = sum (F_b - 1) hop. */
 int b200tts_wavernn_unfold(int B, int hop, int target, int overlap, int mu, const int32_t* frames, const int32_t* row_off, const int64_t* wave_off,
                            long long total, const float* y, float* wave, void* stream);
+/* One stream of b200tts_wavernn_unfold_streams: the output positions [q0, q1) of its utterance, written at wave + wave_off (each stream right
+ * after the previous one, the first at 0).  Fold f of the utterance (f in [fold0, fold0 + nfolds), every fold that covers a position of the
+ * range) reads its samples through source entry src + f - fold0. */
+typedef struct {
+    long long q0, q1, wave_off;
+    int frames;           /* F once it is known (the fade-out lands on the 20 hops before (F - 1) hop; q1 <= (F - 1) hop), 0 while unknown */
+    int fold0, nfolds, src;
+} b200tts_wavernn_unfold_stream;
+/* Incremental unfold of up to B200TTS_WAVERNN_MAX_STREAMS folded streams in one launch, with b200tts_wavernn_unfold's fp64 arithmetic (the
+ * same device functions): position q of a stream sums, over the folds f with 0 <= j = q - f (target + overlap) < target + 2 overlap in
+ * ascending order, fold f's sample j, mu-law decoded when mu > 0 and cross-faded; an absent fold (base[e] < 0) adds nothing.  Times the
+ * linear fade-out when frames > 0.  Fold sample j of source entry e is y[base[e] + j mod period[e]] (a slot of pool-owned storage; period
+ * >= 1).  So the positions of an utterance whose folds all exist, cut into ranges of any size, equal b200tts_wavernn_unfold of the whole
+ * utterance bit for bit.  streams: host descriptors, checked without a device; base (int64) and period (int32): nsrc entries on the
+ * device; total = the sum of q1 - q0. */
+int b200tts_wavernn_unfold_streams(int nstreams, int hop, int target, int overlap, int mu, const b200tts_wavernn_unfold_stream* streams,
+                                   const int64_t* base, const int32_t* period, int nsrc, long long total, const float* y, float* wave,
+                                   void* stream);
 
 /* ---- WaveRNN training: the teacher-forced forward, the loss and the backward ----
  * The MelResNet, the input products of the GRUs, the fully connected layers and every weight gradient run on the convolution-block and

@@ -103,6 +103,10 @@ class WaveRNNWindowRow(Structure):
     _fields_ = [('w', WaveRNNWindowShape), ('s0', c_longlong), ('mel_off', c_longlong), ('aux_off', c_longlong), ('n', c_int)]
 
 
+class WaveRNNUnfoldStream(Structure):
+    _fields_ = [(n, c_longlong) for n in ('q0', 'q1', 'wave_off')] + [(n, c_int) for n in ('frames', 'fold0', 'nfolds', 'src')]
+
+
 WAVERNN_MAX_STREAMS = 64
 
 # include/b200tts.h: the stream ids of the draws under one request seed (b200tts_fill_keep_mask_rows, b200tts_fill_uniform_rows)
@@ -240,6 +244,8 @@ SIGNATURES = {
     'b200tts_wavernn_aborted': (c_int, [POINTER(WaveRNNShape), c_void_p, c_size_t, POINTER(c_int), c_void_p]),
     'b200tts_wavernn_deemphasis': (c_int, [c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
     'b200tts_wavernn_unfold': (c_int, [c_int] * 5 + [c_void_p] * 3 + [c_longlong, c_void_p, c_void_p, c_void_p]),
+    'b200tts_wavernn_unfold_streams': (c_int, [c_int] * 5 + [POINTER(WaveRNNUnfoldStream), c_void_p, c_void_p, c_int, c_longlong, c_void_p,
+                                                          c_void_p, c_void_p]),
     'b200tts_gru_seq_saved_bytes': (c_size_t, [POINTER(GRUSeqShape)]),
     'b200tts_gru_seq_workspace_bytes': (c_size_t, [POINTER(GRUSeqShape)]),
     'b200tts_gru_seq_forward': (c_int, [POINTER(GRUSeqShape)] + [c_void_p] * 6 + [c_size_t, c_void_p]),

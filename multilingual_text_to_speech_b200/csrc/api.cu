@@ -268,6 +268,11 @@ int wavernn_deemphasis_impl(int rows, int len, int mu, float a, float* y, cudaSt
 int wavernn_unfold_check(int B, int hop, int target, int overlap, int mu);
 int wavernn_unfold_impl(int B, int hop, int target, int overlap, int mu, const int* frames, const int* row_off, const long long* wave_off,
                         long long total, const float* y, float* wave, cudaStream_t st);
+int wavernn_unfold_streams_check(int nstreams, int hop, int target, int overlap, int mu, const b200tts_wavernn_unfold_stream* streams,
+                                 int nsrc, long long total);
+int wavernn_unfold_streams_impl(int nstreams, int hop, int target, int overlap, int mu, const b200tts_wavernn_unfold_stream* streams,
+                                const long long* base, const int* period, int nsrc, long long total, const float* y, float* wave,
+                                cudaStream_t st);
 size_t gru_seq_saved_bytes(const b200tts_gru_seq_shape& s);
 size_t gru_seq_workspace_bytes(const b200tts_gru_seq_shape& s);
 int gru_seq_check(const b200tts_gru_seq_shape& s, void* ws, size_t ws_bytes);
@@ -901,6 +906,15 @@ int b200tts_wavernn_unfold(int B, int hop, int target, int overlap, int mu, cons
     B200_TRY(require_device());
     return wavernn_unfold_impl(B, hop, target, overlap, mu, frames, row_off, reinterpret_cast<const long long*>(wave_off), total, y, wave,
                                (cudaStream_t)stream);
+}
+int b200tts_wavernn_unfold_streams(int nstreams, int hop, int target, int overlap, int mu, const b200tts_wavernn_unfold_stream* streams,
+                                   const int64_t* base, const int32_t* period, int nsrc, long long total, const float* y, float* wave,
+                                   void* stream) {
+    B200_REQUIRE(base && period && y && wave, "wavernn_unfold_streams: null argument");
+    B200_TRY(wavernn_unfold_streams_check(nstreams, hop, target, overlap, mu, streams, nsrc, total));
+    B200_TRY(require_device());
+    return wavernn_unfold_streams_impl(nstreams, hop, target, overlap, mu, streams, reinterpret_cast<const long long*>(base), period, nsrc,
+                                       total, y, wave, (cudaStream_t)stream);
 }
 
 size_t b200tts_gru_seq_saved_bytes(const b200tts_gru_seq_shape* shape) {

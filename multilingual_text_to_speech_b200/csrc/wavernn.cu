@@ -502,6 +502,26 @@ __device__ __forceinline__ double linspace_pm1(long long k, int n) {
     return k == n - 1 ? 1.0 : (double)k * (2.0 / (n - 1)) + -1.0;
 }
 
+// The per-sample arithmetic of the unfold, shared by wavernn_unfold_kernel and wavernn_unfold_streams_kernel: acc += fold sample v at fold
+// position j in [0, L), mu-law decoded (mu > 0), times the square-root cross-fade (sil = overlap / 2, fl = overlap - sil).  The product and
+// the sum are one expression, as the compiler contracts them.
+__device__ __forceinline__ void unfold_add(double& acc, double v, long long j, int L, int overlap, int sil, int fl, int mu) {
+    if (mu > 0) v = (v > 0 ? 1.0 : (v < 0 ? -1.0 : 0.0)) / mu * (pow(1.0 + mu, fabs(v)) - 1.0);
+    double w = 1.0;
+    if (j < overlap) w = j < sil ? 0.0 : sqrt(0.5 * (1.0 + linspace_pm1(j - sil, fl)));
+    else if (j >= L - overlap) {
+        const long long k = j - (L - overlap);
+        w = k >= fl ? 0.0 : sqrt(0.5 * (1.0 - linspace_pm1(k, fl)));
+    }
+    acc += v * w;
+}
+
+// the linear fade-out over the fo = 20 hop samples before the cut: k = position - (cut - fo)
+__device__ __forceinline__ double unfold_fade_out(double acc, long long k, int fo) {
+    if (k >= 0) acc *= (k == fo - 1) ? 0.0 : 1.0 + k * (-1.0 / (fo - 1));
+    return acc;
+}
+
 // wave of utterance b (packed at wave_off[b], (F_b - 1) hop samples): sample i sums, over the folds f of the utterance in ascending order,
 // fade(j) y[f, j] with j = i - f (target + overlap) in [0, L); mu-law decoded first (RAW); times the final linear fade-out.  fp64, then fp32.
 __global__ void wavernn_unfold_kernel(int B, int hop, int target, int overlap, int mu, const int* __restrict__ frames,
@@ -522,18 +542,43 @@ __global__ void wavernn_unfold_kernel(int B, int hop, int target, int overlap, i
         for (int f = 0; f < nf; ++f) {
             const long long j = i - (long long)f * (target + overlap);
             if (j < 0 || j >= L) continue;
-            double v = y[(size_t)(r0 + f) * L + j];
-            if (mu > 0) v = (v > 0 ? 1.0 : (v < 0 ? -1.0 : 0.0)) / mu * (pow(1.0 + mu, fabs(v)) - 1.0);
-            double w = 1.0;
-            if (j < overlap) w = j < sil ? 0.0 : sqrt(0.5 * (1.0 + linspace_pm1(j - sil, fl)));
-            else if (j >= L - overlap) {
-                const long long k = j - (L - overlap);
-                w = k >= fl ? 0.0 : sqrt(0.5 * (1.0 - linspace_pm1(k, fl)));
-            }
-            acc += v * w;
+            unfold_add(acc, y[(size_t)(r0 + f) * L + j], j, L, overlap, sil, fl, mu);
         }
-        const long long k = i - (len - fo);
-        if (k >= 0) acc *= (k == fo - 1) ? 0.0 : 1.0 + k * (-1.0 / (fo - 1));
+        wave[idx] = (float)unfold_fade_out(acc, i - (len - fo), fo);
+    }
+}
+
+struct WrUnfoldStreams {
+    int n;
+    b200tts_wavernn_unfold_stream s[B200TTS_WAVERNN_MAX_STREAMS];
+};
+
+// wave[s.wave_off + q - s.q0] for q in [s.q0, s.q1) of every stream s: wavernn_unfold_kernel's sum over the folds f covering q, in ascending
+// order, of fold f's sample at j = q - f (target + overlap), read from y[base[e] + j mod period[e]] (e = s.src + f - s.fold0; an absent
+// fold, base < 0, adds nothing); then the fade-out before (F - 1) hop when F = s.frames is known.  One thread per output sample.
+__global__ void wavernn_unfold_streams_kernel(WrUnfoldStreams g, int hop, int target, int overlap, int mu, const long long* __restrict__ base,
+                                              const int* __restrict__ period, const float* __restrict__ y, float* __restrict__ wave,
+                                              long long total) {
+    const int L = target + 2 * overlap, sil = overlap / 2, fl = overlap - sil, fo = 20 * hop, step = target + overlap;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
+        int lo = 0, hi = g.n - 1;
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (g.s[mid].wave_off <= idx) lo = mid; else hi = mid - 1;
+        }
+        const b200tts_wavernn_unfold_stream& s = g.s[lo];
+        const long long q = s.q0 + (idx - s.wave_off);
+        // folds covering q: f step <= q < f step + L
+        const long long f_hi = q / step, f_lo = q >= L ? (q - L) / step + 1 : 0;
+        double acc = 0.0;
+        for (long long f = f_lo; f <= f_hi; ++f) {
+            const int e = s.src + (int)(f - s.fold0);
+            const long long b = base[e];
+            if (b < 0) continue;
+            const long long j = q - f * step;
+            unfold_add(acc, y[b + j % period[e]], j, L, overlap, sil, fl, mu);
+        }
+        if (s.frames > 0) acc = unfold_fade_out(acc, q - ((long long)(s.frames - 1) * hop - fo), fo);
         wave[idx] = (float)acc;
     }
 }
@@ -878,6 +923,44 @@ int wavernn_unfold_impl(int B, int hop, int target, int overlap, int mu, const i
     if (total <= 0) return B200TTS_OK;
     KernelTimer kt("wavernn_unfold", st);
     wavernn_unfold_kernel<<<grid_for((size_t)total), 256, 0, st>>>(B, hop, target, overlap, mu, frames, row_off, wave_off, y, wave, total);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+// every stream: a non-empty range, packed right after the previous one, whose covering folds all have entries inside [0, nsrc)
+int wavernn_unfold_streams_check(int nstreams, int hop, int target, int overlap, int mu, const b200tts_wavernn_unfold_stream* streams,
+                                 int nsrc, long long total) {
+    B200_TRY(wavernn_unfold_check(1, hop, target, overlap, mu));
+    B200_REQUIRE(streams && nstreams >= 1 && nstreams <= B200TTS_WAVERNN_MAX_STREAMS && nsrc >= 1,
+                 "wavernn_unfold_streams: %d streams (1 to %d), %d fold sources", nstreams, B200TTS_WAVERNN_MAX_STREAMS, nsrc);
+    const long long step = (long long)target + overlap, L = step + overlap;
+    long long off = 0;
+    for (int b = 0; b < nstreams; ++b) {
+        const b200tts_wavernn_unfold_stream& s = streams[b];
+        B200_REQUIRE(s.q0 >= 0 && s.q1 > s.q0 && s.wave_off == off && s.frames >= 0,
+                     "wavernn_unfold_streams: stream %d writes positions [%lld, %lld) at %lld (expected %lld; frames %d)", b, s.q0, s.q1,
+                     s.wave_off, off, s.frames);
+        B200_REQUIRE(s.frames == 0 || s.q1 <= (long long)(s.frames - 1) * hop, "wavernn_unfold_streams: stream %d writes up to %lld, past the "
+                     "cut %lld of its %d frames", b, s.q1, (long long)(s.frames - 1) * hop, s.frames);
+        const long long f_lo = s.q0 >= L ? (s.q0 - L) / step + 1 : 0, f_hi = (s.q1 - 1) / step;
+        B200_REQUIRE(s.fold0 >= 0 && s.fold0 <= f_lo && (long long)s.fold0 + s.nfolds > f_hi && s.src >= 0 && (long long)s.src + s.nfolds <= nsrc,
+                     "wavernn_unfold_streams: stream %d's positions [%lld, %lld) read folds %lld to %lld; it lists folds %d to %d at sources "
+                     "[%d, %d) of %d", b, s.q0, s.q1, f_lo, f_hi, s.fold0, s.fold0 + s.nfolds - 1, s.src, s.src + s.nfolds, nsrc);
+        off += s.q1 - s.q0;
+    }
+    B200_REQUIRE(total == off, "wavernn_unfold_streams: total %lld, the streams write %lld", total, off);
+    return B200TTS_OK;
+}
+
+int wavernn_unfold_streams_impl(int nstreams, int hop, int target, int overlap, int mu, const b200tts_wavernn_unfold_stream* streams,
+                                const long long* base, const int* period, int nsrc, long long total, const float* y, float* wave,
+                                cudaStream_t st) {
+    B200_TRY(wavernn_unfold_streams_check(nstreams, hop, target, overlap, mu, streams, nsrc, total));
+    WrUnfoldStreams g;
+    g.n = nstreams;
+    for (int b = 0; b < nstreams; ++b) g.s[b] = streams[b];
+    KernelTimer kt("wavernn_unfold", st);
+    wavernn_unfold_streams_kernel<<<grid_for((size_t)total), 256, 0, st>>>(g, hop, target, overlap, mu, base, period, y, wave, total);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }

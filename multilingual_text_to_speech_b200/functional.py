@@ -1068,6 +1068,19 @@ def wavernn_unfold(y, frames, row_off, wave_off, total, hop, target, overlap, mu
     return wave[:int(total)]
 
 
+def wavernn_unfold_streams(y, streams, base, period, hop, target, overlap, mu):
+    """Positions [q0, q1) of each folded stream (streams: _lib.WaveRNNUnfoldStream descriptors) from fold samples in the storage y, fold
+    source e at y[base[e] + j mod period[e]] (base int64 and period int32 on the device) -> the packed waveform [sum q1 - q0]."""
+    _require_cuda(y, base, period)
+    n = len(streams)
+    total = sum(int(s.q1 - s.q0) for s in streams)
+    wave = torch.empty(max(total, 1), device=y.device, dtype=torch.float32)
+    check(_lib.load().b200tts_wavernn_unfold_streams(n, int(hop), int(target), int(overlap), int(mu), (_lib.WaveRNNUnfoldStream * n)(*streams),
+                                                     ptr(base), ptr(period), base.numel(), total, ptr(_f32c(y)), ptr(wave), _stream()),
+          'b200tts_wavernn_unfold_streams')
+    return wave[:total]
+
+
 # ------------------------------------------------------------------------------------------------
 # WaveRNN training
 # ------------------------------------------------------------------------------------------------

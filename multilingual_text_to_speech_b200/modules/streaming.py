@@ -6,28 +6,29 @@ Each stage lags the one before it by a bounded number of frames, whatever the ut
   * the vocoder runs its sample loop up to `WaveRNN.lookahead()` (2 at pad 2, factors 5 x 5 x 11) frames behind the last mel frame it has;
   * it holds back the last 20 hops of samples it has run until the mel ends, because the fade-out lands on them."""
 from .tacotron2 import MAX_STREAM_TEXTS, Tacotron, _check_batch_inputs
-from .wavernn import WaveRNN
+from .wavernn import FoldedStreamPool, WaveRNN
 
 
 def speech_stream(tacotron: Tacotron, wavernn: WaveRNN, text, speaker=None, language=None, mel_transform=None, chunk_frames=None,
-                  uniforms=None, generator=None, preemphasis=0.0):
+                  uniforms=None, generator=None, preemphasis=0.0, target=None, overlap=None):
     """Yields waveform chunks of `text` as the decoder produces it: tacotron.inference_stream(text, speaker, language, chunk_frames) fed,
     through mel_transform, into wavernn.generate_stream(…, uniforms, generator, preemphasis).  mel_transform (default: none) maps a
     post-net chunk [num_mels, n] to the vocoder's input frames [feat_dims, n] frame by frame, for example
     utils.audio.denormalize_spectrogram; it must not look at neighbouring frames, since each chunk is transformed alone.  The audio equals
-    wavernn.generate(mel, target=F hop, overlap=0) of the concatenated transformed mel, bit for bit given the same uniform tape."""
+    wavernn.generate(mel, target=F hop, overlap=0) of the concatenated transformed mel, bit for bit given the same uniform tape.  With
+    target and overlap (folded streaming, WaveRNN.generate_stream's), it equals wavernn.generate(mel, target, overlap) instead."""
     mels = tacotron.inference_stream(text, speaker, language, chunk_frames)
     if mel_transform is not None:
         mels = (mel_transform(m) for m in mels)
-    yield from wavernn.generate_stream(mels, uniforms, generator, preemphasis)
+    yield from wavernn.generate_stream(mels, uniforms, generator, preemphasis, target, overlap)
 
 
 def speech_streams(tacotron: Tacotron, wavernn: WaveRNN, texts, speakers=None, languages=None, mel_transform=None, chunk_frames=None,
-                   uniforms=None, generator=None, preemphasis=0.0):
+                   uniforms=None, generator=None, preemphasis=0.0, target=None, overlap=None):
     """speech_stream for up to 64 texts at once: yields (i, waveform chunk) for text i.  Every text is submitted to one SpeechServer(…,
     max_streams=len(texts)) at once and the server steps until it is idle: each step runs one decoder call over the texts still decoding
     (text i reads column i of a recorded mask tape), feeds its post-net chunks (through mel_transform) into the vocoder pool and makes one
-    pool.run().  uniforms: None or one tape [1, T_i, U] per text.  Each text's audio equals speech_stream of that text alone, bit for bit
+    pool.run().  uniforms: None or one tape [1, T_i, U] per text ([K_i, target + 2 overlap, U] with target and overlap).  Each text's audio equals speech_stream of that text alone, bit for bit
     given its tape, in fp32 mode (where the decoded frames of a group equal those of single texts).  A text that decodes fewer than 21
     frames raises ValueError when its stream ends, as speech_stream does, and that ends the generator for every text of the group."""
     texts = list(texts)
@@ -36,7 +37,7 @@ def speech_streams(tacotron: Tacotron, wavernn: WaveRNN, texts, speakers=None, l
     if uniforms is not None and len(uniforms) != len(texts):
         raise ValueError(f'{len(uniforms)} uniform tapes for {len(texts)} texts')
     speakers, languages = _check_batch_inputs(texts, speakers, languages)
-    server = SpeechServer(tacotron, wavernn, len(texts), mel_transform, chunk_frames, preemphasis, generator)
+    server = SpeechServer(tacotron, wavernn, len(texts), mel_transform, chunk_frames, preemphasis, generator, target, overlap)
     ids = [server.submit(text, None if speakers is None else speakers[i], None if languages is None else languages[i],
                          uniforms=None if uniforms is None else uniforms[i]) for i, text in enumerate(texts)]
     text_of = {rid: i for i, rid in enumerate(ids)}
@@ -73,12 +74,16 @@ class SpeechServer:
     it) and uniform tape (`uniforms` [1, T, U]), whatever joins or leaves around it.  With a `seed` instead, the masks and uniforms it does
     not get from a tape are drawn from the seed alone (_lib.SEED_STREAMS), so the request gives the same bits alone, in a full server, at
     any join call and at any chunk_frames.  Without either, its masks and uniforms come from draws shared with the other such requests of
-    each call."""
+    each call.
+
+    With target and overlap the vocoder pool is a FoldedStreamPool: each request's audio is speech_stream(…, target, overlap) of it
+    alone, which equals generate(mel, target, overlap) of its mel; tapes are [K, target + 2 overlap, U].  Admission stays at most
+    max_streams requests; their folds share the loop's 64 rows."""
 
     def __init__(self, tacotron: Tacotron, wavernn: WaveRNN, max_streams=64, mel_transform=None, chunk_frames=None, preemphasis=0.0,
-                 generator=None):
+                 generator=None, target=None, overlap=None):
         self.decoder = tacotron.decoder_pool(max_streams, chunk_frames)
-        self.pool = wavernn.stream_pool(max_streams, preemphasis, generator)
+        self.pool = wavernn.stream_pool(max_streams, preemphasis, generator, target, overlap)
         self.wavernn, self.mel_transform = wavernn, mel_transform
         self.requests = {}                     # id -> _Request, queued or admitted
         self.pending, self.failed = [], {}
@@ -91,7 +96,10 @@ class SpeechServer:
     def submit(self, text, speaker=None, language=None, seed=None, masks=None, uniforms=None):
         """Queues a request -> its id.  Its inputs are checked now (ValueError)."""
         self.decoder.check(text, speaker, language, seed, masks)
-        self.wavernn._check_stream_tape(uniforms)
+        if isinstance(self.pool, FoldedStreamPool):
+            self.wavernn._check_stream_tape(uniforms, self.pool.fold_len)
+        else:
+            self.wavernn._check_stream_tape(uniforms)
         rid = self.next_id
         self.next_id += 1
         self.requests[rid] = _Request(text, speaker, language, seed, masks, uniforms)

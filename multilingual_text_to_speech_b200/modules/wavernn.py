@@ -313,7 +313,7 @@ class WaveRNN(nn.Module):
         return out
 
     # ---- streaming ----
-    def generate_stream(self, mel_chunks, uniforms=None, generator=None, preemphasis=0.0):
+    def generate_stream(self, mel_chunks, uniforms=None, generator=None, preemphasis=0.0, target=None, overlap=None):
         """Streaming form of generate(mel, target=F hop, overlap=0), fatchord's unbatched generation: mel_chunks is an iterable of
         [feat_dims, n_k] mels (n_k >= 0, as given: no normalisation), whose concatenation is the mel of F >= 21 frames; yields waveform
         chunks whose concatenation is that call's (F - 1) hop samples, bit for bit given the same uniform tape.  A sample's loop features are
@@ -322,7 +322,15 @@ class WaveRNN(nn.Module):
         uniforms[0, t]; T >= (F - 1) hop), by default drawn with torch.rand per call of the loop (`generator` optional).  preemphasis as in
         generate_batch, de-emphasised sequentially across chunks: within fp32 roundings of the one-shot call, not bit for bit.  Runs on the
         device of the first CUDA chunk, or the current CUDA device, in fp32 (the precision mode is set for each stretch of work and restored
-        before every yield).  Chunks come out as the first chunk went in: numpy, CUDA tensors, or CPU tensors."""
+        before every yield).  Chunks come out as the first chunk went in: numpy, CUDA tensors, or CPU tensors.
+
+        With target and overlap: the streaming form of generate(mel, target, overlap), fatchord's folded generation, through a one-stream
+        FoldedStreamPool (its folds run as rows of one loop): the chunks concatenate to that call's samples bit for bit given the same tape
+        uniforms [folds, target + 2 overlap, U] (fold k step j reads uniforms[k, j]); preemphasis de-emphasises each fold from a zero state,
+        within generate_batch's bound."""
+        if target is not None or overlap is not None:
+            yield from self._generate_stream_folded(mel_chunks, uniforms, generator, preemphasis, target, overlap)
+            return
         if not -1.0 < float(preemphasis) < 1.0:
             raise ValueError(f'preemphasis {preemphasis} must lie in (-1, 1)')
         tape = self._check_stream_tape(uniforms)
@@ -339,9 +347,34 @@ class WaveRNN(nn.Module):
             raise ValueError(f'the mel stream ended after {0 if st is None else st.frames} frames; the 20-hop fade-out needs at least 21')
         yield st.finish()
 
-    def stream_pool(self, max_streams, preemphasis=0.0, generator=None):
-        """A StreamPool of up to max_streams (1 to 64) concurrent generate_stream-like streams sharing one sample loop."""
-        return StreamPool(self, max_streams, preemphasis, generator)
+    def stream_pool(self, max_streams, preemphasis=0.0, generator=None, target=None, overlap=None):
+        """A StreamPool of up to max_streams (1 to 64) concurrent generate_stream-like streams sharing one sample loop; with target and
+        overlap, a FoldedStreamPool of up to max_streams folded streams on the loop's 64 rows."""
+        if target is None and overlap is None:
+            return StreamPool(self, max_streams, preemphasis, generator)
+        return FoldedStreamPool(self, max_streams, target, overlap, preemphasis, generator)
+
+    def _generate_stream_folded(self, mel_chunks, uniforms, generator, preemphasis, target, overlap):
+        pool = sid = fmt = None
+        for i, chunk in enumerate(mel_chunks):
+            spec, as_numpy = self._check_chunk(chunk, i)
+            if pool is None:
+                device = spec.device if spec.is_cuda else (torch.device('cuda', torch.cuda.current_device()) if torch.cuda.is_available()
+                                                           else torch.device('cuda'))
+                fmt = (as_numpy, not as_numpy and spec.is_cuda)
+                with torch.cuda.device(device):
+                    pool = FoldedStreamPool(self, 1, target, overlap, preemphasis, generator)
+                sid = pool.open(uniforms)
+            if spec.shape[1]:
+                pool.feed(sid, spec)
+                for w in pool.drain():
+                    yield _as_input(w[sid], *fmt)
+        if pool is None or pool.streams[sid].frames < 21:
+            raise ValueError(f'the mel stream ended after {0 if pool is None else pool.streams[sid].frames} frames; the 20-hop fade-out needs '
+                             f'at least 21')
+        pool.end(sid)
+        for w in pool.drain():
+            yield _as_input(w[sid], *fmt)
 
     def lookahead(self):
         """Frames past a sample's own frame that its loop features read: `pad` for conv_in (the rest of the MelResNet is pointwise) or the
@@ -401,12 +434,16 @@ class WaveRNN(nn.Module):
             raise ValueError(f'mel chunk {i} has non-finite values')
         return t, as_numpy
 
-    def _check_stream_tape(self, uniforms):
+    def _check_stream_tape(self, uniforms, fold_len=None):
+        """A stream's uniform tape: [1, steps, U], or with fold_len (a folded stream) [folds, fold_len, U]."""
         if uniforms is None:
             return None
         u = torch.as_tensor(np.asarray(uniforms) if not isinstance(uniforms, torch.Tensor) else uniforms)
         U = self.uniforms_per_step()
-        if u.dim() != 3 or u.shape[0] != 1 or u.shape[2] != U:
+        if fold_len is not None:
+            if u.dim() != 3 or u.shape[0] < 1 or u.shape[1] != fold_len or u.shape[2] != U:
+                raise ValueError(f'uniform tape of shape {tuple(u.shape)}; expected [folds, {fold_len}, {U}] (target + 2 overlap = {fold_len})')
+        elif u.dim() != 3 or u.shape[0] != 1 or u.shape[2] != U:
             raise ValueError(f'uniform tape of shape {tuple(u.shape)}; expected [1, steps, {U}]')
         if not torch.is_floating_point(u):
             raise ValueError('uniform tape is not floating point')
@@ -590,6 +627,12 @@ class WaveRNN(nn.Module):
             mu = 0
         wave = F.wavernn_unfold(y, dev(np.asarray(frames, np.int32)), dev(row_off), dev(wave_off), int(wave_off[-1]), hop, target, overlap, mu)
         return wave, wave_off
+
+
+def _as_input(wave, as_numpy, on_cuda):
+    if as_numpy:
+        return wave.cpu().numpy()
+    return wave if on_cuda else wave.cpu()
 
 
 class _Stream:
@@ -860,44 +903,61 @@ class StreamPool:
         return torch.from_numpy(np.ascontiguousarray(a)).to(self.device)
 
     def _loop(self, plan):
-        m, dev, U = self.m, self.device, self.m.uniforms_per_step()
         live = sorted(plan, key=lambda sid: self.streams[sid].slot)
-        active = self.streams[live[-1]].slot + 1
-        nmax = max(n for _, n in plan.values())
-        feat = self._features(live, plan, active, nmax)
-        cond = m.conditioning(self.w, feat)
+        steps = {sid: plan[sid][0] for sid in live}
+        y, active, nmax = self._step_rows(live, self.streams, plan, steps, lambda sid, t, n: self.streams[sid].tape[t:t + n], steps)
         slot = np.array([self.streams[sid].slot for sid in live], np.int64)
-        t = np.array([plan[sid][0] for sid in live], np.int64)
-        n = np.array([plan[sid][1] for sid in live], np.int64)
         row_t, row_n = np.zeros(active, np.int64), np.zeros(active, np.int32)
-        row_t[slot], row_n[slot] = t, n
+        row_t[slot] = [plan[sid][0] for sid in live]
+        row_n[slot] = [plan[sid][1] for sid in live]
+        # into the ring: row r's step i at slot r P + (row_t + i) mod P; steps past a row's budget go to the sink
+        i = np.arange(nmax)[None, :]
+        dst = np.where(i < row_n[:, None], np.arange(active)[:, None] * self.P + (row_t[:, None] + i) % self.P, self.rows * self.P)
+        self.ring.index_put_((self._upload(dst.reshape(-1)),), y.reshape(-1))
+        for sid in live:
+            self.streams[sid].steps += plan[sid][1]
+
+    def _step_rows(self, live, rows, plan, steps, tape_of, draw0):
+        """One loop call over the rows `live` (keys of `rows`, whose entries have slot, mel, frames, ended, tape and seed), sorted by slot:
+        row k runs the features of positions plan[k] = (t, n) from its own steps[k] steps (the loop's slot parity), reading the uniforms
+        tape_of(k, steps[k], n) [n, U] of a taped row, or draws from draw0[k] of a seeded row's stream.  -> (y [active, nmax], de-emphasised
+        with preemphasis, active, nmax); self.last carries each row's last de-emphasised sample."""
+        m, dev, U = self.m, self.device, self.m.uniforms_per_step()
+        active = rows[live[-1]].slot + 1
+        nmax = max(plan[k][1] for k in live)
+        feat = self._features(live, plan, active, nmax, rows)
+        cond = m.conditioning(self.w, feat)
+        slot = np.array([rows[k].slot for k in live], np.int64)
+        n = np.array([plan[k][1] for k in live], np.int64)
+        row_t, row_n = np.zeros(active, np.int64), np.zeros(active, np.int32)
+        row_t[slot], row_n[slot] = [steps[k] for k in live], n
         # uniforms: the taped rows' steps gathered from their tapes (source 0 is a zero) and the seeded rows' from one seeded draw, in one
         # gather; the other rows' drawn for the call
-        taped = [sid for sid in live if self.streams[sid].tape is not None]
-        seeded = [sid for sid in live if self.streams[sid].tape is None and self.streams[sid].seed is not None]
+        taped = [k for k in live if rows[k].tape is not None]
+        seeded = [k for k in live if rows[k].tape is None and rows[k].seed is not None]
         if taped or seeded:
-            parts = [torch.zeros(1, device=dev)] + [self.streams[sid].tape[plan[sid][0]:plan[sid][0] + plan[sid][1]].reshape(-1) for sid in taped]
+            parts = [torch.zeros(1, device=dev)] + [tape_of(k, steps[k], plan[k][1]).reshape(-1) for k in taped]
             if seeded:
-                parts.append(F.fill_uniform_rows(nmax, U, [self.streams[sid].seed for sid in seeded], [plan[sid][0] for sid in seeded],
+                parts.append(F.fill_uniform_rows(nmax, U, [rows[k].seed for k in seeded], [draw0[k] for k in seeded],
                                                  _lib.SEED_STREAMS['vocoder'], dev).reshape(-1))
             src = torch.cat(parts)
             idx = np.zeros((active, nmax, U), np.int64)
             off = 1
             i = np.arange(nmax)[:, None] * U + np.arange(U)[None, :]
-            for sid in taped:
-                st, k = self.streams[sid], plan[sid][1]
-                idx[st.slot, :k] = off + i[:k]
-                off += k * U
-            for sid in seeded:
-                st, k = self.streams[sid], plan[sid][1]
-                idx[st.slot, :k] = off + i[:k]
+            for k in taped:
+                c = plan[k][1]
+                idx[rows[k].slot, :c] = off + i[:c]
+                off += c * U
+            for k in seeded:
+                c = plan[k][1]
+                idx[rows[k].slot, :c] = off + i[:c]
                 off += nmax * U
             uni = src[self._upload(idx)]
         if len(taped) + len(seeded) < len(live):
             drawn = torch.rand(active, nmax, U, device=dev, dtype=torch.float32, generator=self.generator)
             if taped or seeded:
                 has = np.zeros((active, 1, 1), bool)
-                has[[self.streams[sid].slot for sid in taped + seeded]] = True
+                has[[rows[k].slot for k in taped + seeded]] = True
                 uni = torch.where(self._upload(has), uni, drawn)
             else:
                 uni = drawn
@@ -909,22 +969,19 @@ class StreamPool:
             y = F.wavernn_deemphasis(torch.cat([self.last[:active, None], y], 1).contiguous(), 0, self.a)[:, 1:]
             sl = self._upload(slot)
             self.last[sl] = y[sl, self._upload(n - 1)]
-        # into the ring: row r's step i at slot r P + (row_t + i) mod P; steps past a row's budget go to the sink
-        i = np.arange(nmax)[None, :]
-        dst = np.where(i < row_n[:, None], np.arange(active)[:, None] * self.P + (row_t[:, None] + i) % self.P, self.rows * self.P)
-        self.ring.index_put_((self._upload(dst.reshape(-1)),), y.reshape(-1))
-        for sid in live:
-            self.streams[sid].steps += plan[sid][1]
+        return y, active, nmax
 
-    def window_layout(self, live, plan):
+    def window_layout(self, live, plan, rows=None):
         """The host side of _features: (sources [(sid, frame0, frame1)] packed side by side, then a zero column; the gather index of the
         packed mel-path windows followed by the padded MelResNet batch; window lengths; MelResNet widths and batch width; window-row
-        descriptors without the aux width, as (slot, frames or 0, m0, mel_len, a0, aux_len, s0, mel_off, aux_off / aux width, n))."""
+        descriptors without the aux width, as (slot, frames or 0, m0, mel_len, a0, aux_len, s0, mel_off, aux_off / aux width, n)).  rows:
+        the loop rows of the keys in `live` (default: the streams)."""
+        rows = self.streams if rows is None else rows
         m = self.m
         p, hop, s_last, C = m.pad, self.hop, m.upsample_factors[-1], m.feat_dims
         srcs, wins, res = [], [], []
         for sid in live:
-            st, (t, n) = self.streams[sid], plan[sid]
+            st, (t, n) = rows[sid], plan[sid]
             (P0, P1), (r0, r1), _ = m.window_plan(t, t + n, st.frames, st.ended)
             lo, hi = max(P0, p), min(P1, st.frames + p)
             wins.append((P0, P1, lo, hi))
@@ -947,20 +1004,21 @@ class StreamPool:
         parts.append((c[None, :, :] + col[:, None, :]).reshape(-1))
         scale = int(np.prod(m.upsample_factors[:-1]))
         for b, sid in enumerate(live):
-            st, (t, n) = self.streams[sid], plan[sid]
+            st, (t, n) = rows[sid], plan[sid]
             P0, r0 = wins[b][0], res[b][0]
             desc.append((st.slot, st.frames if st.ended else 0, P0 * (hop // s_last), lens[b] * scale, r0, widths[b], t, mel_off, b * W, n))
             mel_off += C * lens[b] * scale
         return srcs, np.concatenate(parts), lens, widths, W, desc
 
-    def _features(self, live, plan, active, nmax):
+    def _features(self, live, plan, active, nmax, rows=None):
         """Loop features [nmax, active, feat_dims + res_out_dims] of every live stream's next steps, in a fixed number of launches: one
         gather of every window, the mel-path layers on the packed windows, the MelResNet over the padded batch of windows, one
         window-rows launch."""
         m, dev = self.m, self.device
         p, hop, s_last, C = m.pad, self.hop, m.upsample_factors[-1], m.feat_dims
-        srcs, idx, lens, widths, W, desc = self.window_layout(live, plan)
-        packed = torch.cat([self.streams[sid].mel[:, a:b] for sid, a, b in srcs] + [torch.zeros(C, 1, device=dev)], dim=1)
+        rows = self.streams if rows is None else rows
+        srcs, idx, lens, widths, W, desc = self.window_layout(live, plan, rows)
+        packed = torch.cat([rows[sid].mel[:, a:b] for sid, a, b in srcs] + [torch.zeros(C, 1, device=dev)], dim=1)
         g = packed.reshape(-1)[self._upload(idx)]
         nw = C * sum(lens)
         x, batch = g[:nw], g[nw:].view(len(live), C, W)
@@ -997,3 +1055,307 @@ class StreamPool:
         wave = F.wavernn_unfold(y, meta[:B].int(), meta[B:2 * B + 1].int(), meta[2 * B + 1:], int(wave_off[-1]), self.hop, L, 0,
                                 0 if self.a else self.mu)
         return {sid: wave[int(wave_off[b]):int(wave_off[b + 1])] for b, (sid, *_) in enumerate(rel)}
+
+
+class _Fold:
+    """Fold k of a folded stream: sample positions [start, start + fold_len) with start = k (target + overlap), its loop row (None before
+    its grant and once it has run every step it needs), its storage slot (None once its samples are all released) and the steps it has
+    run.  It reads the stream's mel, tape and seed, as a StreamPool row reads its stream's."""
+
+    def __init__(self, st, k, start):
+        self.st, self.k, self.start = st, k, start
+        self.slot = self.store = None
+        self.steps = 0
+        self.done = False
+
+    mel = property(lambda self: self.st.mel)
+    frames = property(lambda self: self.st.frames)
+    ended = property(lambda self: self.st.ended)
+    seed = property(lambda self: self.st.seed)
+    tape = property(lambda self: self.st.tape)
+
+
+class _FoldedStream(_PoolStream):
+    """One stream of a FoldedStreamPool: a _PoolStream without a row of its own; `folds` lists the folds opened so far, fold k at index k."""
+
+    def __init__(self, sid, device, feat_dims, tape, seed=None):
+        super().__init__(None, device, feat_dims, tape, seed)
+        self.sid = sid
+        self.folds = []
+
+
+class FoldedStreamPool(StreamPool):
+    """Folded streaming generation: up to max_streams streams, each the streaming form of generate(mel, target, overlap) (fatchord's
+    folded generation, the library's default), whose folds run as rows of one 64-row sample loop (b200tts_wavernn_run_rows).  The
+    interface is StreamPool's: open / feed / end / run / close / streams.
+
+    Fold geometry is fold_count's: with L = target + 2 overlap, fold k covers positions [k (target + overlap), k (target + overlap) + L) and
+    exists iff k (target + overlap) + overlap < F hop.  While the mel arrives, fold k opens only once its existence is certain (it exists
+    for the frames that have arrived).  It runs up to generate_stream's readiness rule (lookahead() frames after a sample's frame), and
+    once F is known up to min(L, (F - 1) hop - k (target + overlap)) steps: samples at or past the cut are never needed.  Fold k step j
+    reads tape[k, j] (tape [K, L, U], K at least the folds the stream ends up running), or, seeded, draw (k L + j) U + u of the vocoder
+    stream (b200tts_fill_uniform_rows at t0 = k L + j): its tape is one seeded row of K L steps reshaped to [K, L, U].  De-emphasis runs
+    per fold from a zero state, as postprocess does per fold row.
+
+    Rows: each run() grants free loop rows to the waiting folds in order of k (target + overlap) minus the samples their stream has
+    released (ties by stream id), so the fold whose audio is needed soonest goes first; a new stream's fold 0 is not starved by old
+    streams' later folds.  A fold's row is freed as soon as it has run every step it needs; its unreleased samples wait in pool-owned
+    storage of L samples per fold.  The storage holds 64 folds plus, per stream, the finished folds that can wait on the release: those
+    within 21 hops + L of its release point, so that a row never waits for storage.  Each run() runs at most POOL_CALL_HOPS hops, bounded
+    by COND_BYTES at the rows it runs.
+
+    Release: position q is final when every existing fold covering it has run step q - k (target + overlap); a fold whose existence is
+    still undecided blocks the positions it would cover.  Before end() the final positions are released in whole hops, 20 hops behind
+    (the fade-out may land there); after it, every final position.  Each run() writes every stream's chunk with one
+    b200tts_wavernn_unfold_streams launch, whose arithmetic is b200tts_wavernn_unfold's: a stream's chunks concatenate to generate(mel,
+    target, overlap, uniforms=tape) bit for bit, whatever joins or leaves the pool and however its mel is chunked.  With preemphasis each
+    fold is de-emphasised across calls, within generate_batch's bound.  close() frees every row and all storage of a stream at once."""
+
+    def __init__(self, model, max_streams, target, overlap, preemphasis=0.0, generator=None):
+        if not 1 <= int(max_streams) <= _lib.WAVERNN_MAX_STREAMS:
+            raise ValueError(f'a stream pool holds 1 to {_lib.WAVERNN_MAX_STREAMS} streams (got {max_streams})')
+        if target is None or overlap is None or int(target) != target or int(overlap) != overlap or target < 1 or overlap < 0:
+            raise ValueError(f'a folded stream pool needs an integer target >= 1 and overlap >= 0 (got {target!r}, {overlap!r})')
+        if not -1.0 < float(preemphasis) < 1.0:
+            raise ValueError(f'preemphasis {preemphasis} must lie in (-1, 1)')
+        self.a, self.generator = float(preemphasis), generator
+        self._layout(model, max_streams, target, overlap, _lib.WAVERNN_MAX_STREAMS)
+        self.device = torch.device('cuda', torch.cuda.current_device()) if torch.cuda.is_available() else torch.device('cuda')
+        nrows, L = len(self.slots), self.fold_len
+        with self._fp32():
+            self.w = model.loop_weights(self.device)
+            self.shape = _lib.WaveRNNShape(nrows, model.rnn_dims, model.fc_dims, model.n_classes, _lib.WAVERNN_MODES[model.mode], self.S)
+            self.ws = F.wavernn_workspace(self.shape, self.device)
+            self.params = F.wavernn_params(self.w)
+            F.wavernn_prepare(self.shape, self.params, self.ws)
+            fir = lambda j: model.upsample.up_layers[2 * j + 1].weight.detach().reshape(-1).to(self.device, torch.float32).contiguous()  # noqa
+            self.firs = [fir(j) for j in range(len(model.upsample_factors))]
+            self.last = torch.zeros(nrows, device=self.device, dtype=torch.float32)      # each row's last de-emphasised sample
+            self.store = torch.zeros(self.nstore * L + 1, device=self.device, dtype=torch.float32)     # + a write sink
+
+    def _layout(self, model, max_streams, target, overlap, nrows):
+        """The host state of a pool with nrows loop rows: geometry, rows, streams and storage slots (ValueError past COND_BYTES)."""
+        self.m = model
+        self.target, self.overlap = int(target), int(overlap)
+        self.step, self.fold_len = self.target + self.overlap, self.target + 2 * self.overlap
+        self.rows = int(max_streams)                         # streams admitted at once
+        self.hop, self.lookahead = model.hop_length, model.lookahead()
+        self.mu = model.n_classes - 1 if model.mode == 'RAW' else 0
+        self.S = POOL_CALL_HOPS * self.hop
+        self.slots = [None] * nrows                          # the fold on each loop row
+        self.streams = {}
+        self.next_sid = 0
+        self.hold = -(-(21 * self.hop + self.fold_len) // self.step) + 1      # finished folds of one stream that can wait on its release
+        self.nstore = nrows + self.rows * self.hold
+        if self.nstore * self.fold_len * 4 > COND_BYTES:
+            raise ValueError(f'target {target} and overlap {overlap}: the fold storage of {self.nstore} folds of {self.fold_len} samples '
+                             f'exceeds {COND_BYTES >> 20} MiB')
+        self.free_store = list(range(self.nstore))
+
+    # ---- streams ----
+    def open(self, uniforms=None, seed=None):
+        """A new stream -> its id.  uniforms: its tape [K, target + 2 overlap, U], or None; seed (an int in [0, 2^64), used without a
+        tape): the stream draws its uniforms from it.  No loop row is taken until its first fold is granted one."""
+        tape = self.m._check_stream_tape(uniforms, self.fold_len)
+        if seed is not None and (isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= int(seed) < 1 << 64):
+            raise ValueError(f'a seed is an int in [0, 2^64) (got {seed!r})')
+        if len(self.streams) >= self.rows:
+            raise ValueError(f'the stream pool is full: {self.rows} streams are open')
+        sid = self.next_sid
+        with self._fp32():
+            if tape is not None:
+                tape = tape.to(device=self.device, dtype=torch.float32).contiguous()
+            self.streams[sid] = _FoldedStream(sid, self.device, self.m.feat_dims, tape, None if seed is None else int(seed))
+        self.next_sid += 1
+        return sid
+
+    def close(self, sid):
+        """Drops stream sid and frees every loop row and all storage of it at once, whatever it has run or released."""
+        st = self.streams.pop(sid, None)
+        if st is None:
+            raise ValueError(f'unknown or finished stream {sid}')
+        for f in st.folds:
+            self._free(f)
+
+    def _free(self, f):
+        if f.slot is not None:
+            self.slots[f.slot] = None
+            f.slot = None
+        if f.store is not None:
+            self.free_store.append(f.store)
+            f.store = None
+
+    # ---- geometry ----
+    def folds_known(self, st):
+        """Folds of stream st whose existence is certain: fold_count of the samples of the frames that have arrived (all of them once it
+        has ended)."""
+        return fold_count(st.frames * self.hop, self.target, self.overlap)
+
+    def ready(self, st):
+        """The positions below which st's samples can run: generate_stream's readiness rule, (F - 1) hop once it has ended."""
+        F_ = st.frames
+        return (F_ - 1) * self.hop if st.ended else max(min(F_ - self.lookahead, F_ - 1), 0) * self.hop
+
+    def needed(self, st, k):
+        """Steps fold k of st can run so far: up to the ready positions, at most the fold length (<= 0: none)."""
+        return min(self.fold_len, self.ready(st) - k * self.step)
+
+    def final(self, st):
+        """The end of st's final positions: every position below it has been run by every existing fold that covers it."""
+        P = (st.frames - 1) * self.hop if st.ended else 1 << 62
+        for f in st.folds:
+            if not f.done:
+                P = min(P, f.start + f.steps)
+        # the first fold without a grant blocks the positions it covers while its existence is undecided, or while it exists and has
+        # steps to run
+        n = len(st.folds)
+        if not st.ended or (n < self.folds_known(st) and self.needed(st, n) > 0):
+            P = min(P, n * self.step)
+        return P
+
+    # ---- one call ----
+    def grants(self):
+        """[(stream, k)] of the folds granted a row in the next run(), in grant order: the folds whose existence is certain and that have
+        steps to run, by k (target + overlap) minus their stream's released samples, then stream id, while a row and storage are free."""
+        wait = []
+        for sid, st in self.streams.items():
+            for k in range(len(st.folds), self.folds_known(st)):
+                if self.needed(st, k) <= 0:
+                    break
+                wait.append((k * self.step - st.released, sid, k))
+        wait.sort()
+        n = min(self.slots.count(None), len(self.free_store), len(wait))
+        return [(self.streams[sid], k) for _, sid, k in wait[:n]]
+
+    def plan(self):
+        """{fold: (position, steps of the next call)} for every fold on a row with steps to run.  The call's budget: POOL_CALL_HOPS hops,
+        bounded by COND_BYTES at the rows it runs."""
+        work = {f: self.needed(f.st, f.k) - f.steps for f in self.slots if f is not None}
+        work = {f: n for f, n in work.items() if n > 0}
+        if not work:
+            return {}
+        S = min(self.S, self.m.chunk_steps(max(f.slot for f in work) + 1, 1 << 30))
+        return {f: (f.start + f.steps, min(S, n)) for f, n in work.items()}
+
+    def release_plan(self):
+        """[(sid, q0, q1, frames)] of every stream with positions to release: [released, final) once it has ended (frames F), else the whole
+        hops of it more than 20 hops behind (frames 0: no fade-out)."""
+        rel = []
+        for sid, st in self.streams.items():
+            P = self.final(st)
+            q1 = P if st.ended else (P - 20 * self.hop) // self.hop * self.hop
+            if q1 > st.released:
+                rel.append((sid, st.released, q1, st.frames if st.ended else 0))
+        return rel
+
+    def drain(self):
+        """Runs until no fold has work left -> the non-empty {sid: chunk} results, in order."""
+        out = []
+        while True:
+            busy = bool(self.grants() or self.plan())
+            r = self.run()
+            if r:
+                out.append(r)
+            if not busy:
+                return out
+
+    def run(self):
+        """Grants rows, makes one loop call over every fold with steps to run and releases the final positions -> {sid: the waveform chunk
+        it releases}.  A fold beyond a stream's tape raises ValueError before any device work."""
+        self._retire()
+        grants = self.grants()
+        for st, k in grants:
+            if st.tape is not None and k >= st.tape.shape[0]:
+                raise ValueError(f'the uniform tape holds {st.tape.shape[0]} folds; stream {st.sid} needs fold {k}')
+        with self._fp32():
+            if grants:
+                self._reset(self._grant(grants))
+            plan = self.plan()
+            if plan:
+                self._loop(plan)
+            rel = self.release_plan()
+            released = self._release(rel) if rel else {}
+            if F.wavernn_aborted(self.shape, self.ws):
+                raise _lib.B200TTSError('wavernn: the sample loop timed out at a grid barrier')
+        for sid in list(self.streams):
+            st = self.streams[sid]
+            if st.ended and st.released == (st.frames - 1) * self.hop:
+                self.close(sid)
+        return released
+
+    # ---- host bookkeeping ----
+    def _grant(self, grants):
+        """Opens the granted folds on the lowest free rows, each with a storage slot -> the rows."""
+        free = [r for r, f in enumerate(self.slots) if f is None]
+        for (st, k), slot in zip(grants, free):
+            f = _Fold(st, k, k * self.step)
+            f.slot, f.store = slot, self.free_store.pop()
+            st.folds.append(f)
+            self.slots[slot] = f
+        return free[:len(grants)]
+
+    def _advance(self, plan):
+        for f, (_, n) in plan.items():
+            f.steps += n
+        self._retire()
+
+    def _retire(self):
+        """Frees the row of every fold that has run every step it needs: its fold length, or up to the cut once the mel has ended."""
+        for f in self.slots:
+            if f is not None and (f.steps == self.fold_len or f.st.ended and f.steps == self.needed(f.st, f.k)):
+                f.done = True
+                self.slots[f.slot] = None
+                f.slot = None
+
+    def _mark_released(self, rel):
+        """Advances each stream's released samples and frees the storage of its finished folds whose samples are all released."""
+        for sid, _, q1, _ in rel:
+            st = self.streams[sid]
+            st.released = q1
+            for f in st.folds:
+                if f.done and f.store is not None and f.start + f.steps <= q1:
+                    self.free_store.append(f.store)
+                    f.store = None
+
+    # ---- device work ----
+    def _reset(self, slots):
+        F.wavernn_reset_rows(self.shape, self.ws, slots)
+        self.last[self._upload(np.array(slots, np.int64))] = 0.0
+
+    def _loop(self, plan):
+        live = sorted(plan, key=lambda f: f.slot)
+        L = self.fold_len
+        steps = {f: f.steps for f in live}
+        y, active, nmax = self._step_rows(live, {f: f for f in live}, plan, steps, lambda f, s, n: f.st.tape[f.k, s:s + n],
+                                          {f: f.k * L + f.steps for f in live})
+        # into the storage: fold f's step s at f.store L + s; steps past a row's budget go to the sink
+        base, row_n = np.full(active, self.nstore * L, np.int64), np.zeros(active, np.int64)
+        for f in live:
+            base[f.slot], row_n[f.slot] = f.store * L + f.steps, plan[f][1]
+        i = np.arange(nmax)[None, :]
+        dst = np.where(i < row_n[:, None], base[:, None] + i, self.nstore * L)
+        self.store.index_put_((self._upload(dst.reshape(-1)),), y.reshape(-1))
+        self._advance(plan)
+
+    def unfold_layout(self, rel):
+        """The host side of _release: (b200tts_wavernn_unfold_streams descriptors, the storage base of each fold source entry or -1 for a
+        fold that does not exist)."""
+        L, descs, base, off = self.fold_len, [], [], 0
+        for sid, q0, q1, frames in rel:
+            st = self.streams[sid]
+            f0 = (q0 - L) // self.step + 1 if q0 >= L else 0
+            f1 = (q1 - 1) // self.step
+            descs.append(_lib.WaveRNNUnfoldStream(q0, q1, off, frames, f0, f1 - f0 + 1, len(base)))
+            # a fold that covers a final position has been opened if it exists
+            base += [st.folds[k].store * L if k < len(st.folds) else -1 for k in range(f0, f1 + 1)]
+            off += q1 - q0
+        return descs, base
+
+    def _release(self, rel):
+        """Every stream's final positions through one b200tts_wavernn_unfold_streams launch -> {sid: chunk}."""
+        descs, base = self.unfold_layout(rel)
+        b = self._upload(np.array(base, np.int64))
+        wave = F.wavernn_unfold_streams(self.store, descs, b, torch.full_like(b, self.fold_len, dtype=torch.int32), self.hop, self.target,
+                                        self.overlap, 0 if self.a else self.mu)
+        self._mark_released(rel)
+        return {sid: wave[d.wave_off:d.wave_off + q1 - q0] for d, (sid, q0, q1, _) in zip(descs, rel)}

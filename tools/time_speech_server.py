@@ -10,6 +10,8 @@ default --frames 200, through the decoder's stop rule; the stop token itself nev
 round by round after one warm-up of each:
   * server: one SpeechServer(max_streams=64); a request is submitted at its arrival time and every step() runs one decoder call and one
     vocoder call over everything admitted;
+  * server-folded: the server arm with target=11000, overlap=550: folded vocoding (the library's default, generate_batch's), each
+    request's folds running as rows of the shared 64-row loop;
   * groups: each time the previous group has ended, one speech_streams group of whatever has arrived (at most 64), run to its end.
 Per request: queueing delay (arrival to admission), time to first audio and RTF from arrival (time to its last chunk / its audio
 duration), and the largest gap between its chunks; p50, p95 and max over the trace.  Overall: audio-seconds per wall second (trace start
@@ -25,6 +27,7 @@ import time
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+ARMS = ('server', 'server-folded', 'groups')
 
 
 def parse_args(argv=None):
@@ -119,8 +122,8 @@ def main(argv=None):
         torch.cuda.synchronize()
         joins.append((n, time.perf_counter() - t0))
 
-    def serve(voc, trace):
-        server = SpeechServer(taco, voc, 64, None, a.chunk)
+    def serve(voc, trace, folded=False):
+        server = SpeechServer(taco, voc, 64, None, a.chunk, target=11000 if folded else None, overlap=550 if folded else None)
         n, ids, stamps, admitted = len(trace), {}, {i: [] for i in range(len(trace))}, {}
         nxt = 0
         t0 = time.perf_counter()
@@ -169,7 +172,7 @@ def main(argv=None):
         joins.clear()
         try:
             torch.cuda.synchronize()
-            stamps, admitted = (serve if arm == 'server' else groups)(voc, trace)
+            stamps, admitted = groups(voc, trace) if arm == 'groups' else serve(voc, trace, arm == 'server-folded')
         finally:
             T.Decoder._StopRule = StopRule
             T.DecoderPool.run, T.DecoderPool._admit = orig_run, orig_admit
@@ -186,20 +189,20 @@ def main(argv=None):
         torch.manual_seed(2)
         voc = WaveRNN(**dict(DIMS, mode=mode)).cuda().eval()
         warm = make_trace(64.0, 8, a.frames, a.seed + 1000)
-        for arm in ('server', 'groups'):
+        for arm in ARMS:
             run(arm, voc, warm)
         for rate in a.rates:
             trace = make_trace(rate, a.requests, a.frames, a.seed)
-            res = {'server': [], 'groups': []}
+            res = {arm: [] for arm in ARMS}
             for _ in range(a.rounds):
-                for arm in ('server', 'groups'):
+                for arm in ARMS:
                     res[arm].append(run(arm, voc, trace))
             for arm, rs in res.items():
                 pool = lambda k: [x for r in rs for x in r[k]]       # noqa: E731 -- every request of every round
                 row = dict(mode=mode, arm=arm, rate=rate, requests=a.requests, queue_s=percentiles(pool('queue')),
                            first_audio_s=percentiles(pool('first')), gap_s=percentiles(pool('gap')), rtf=percentiles(pool('rtf')),
                            audio_s_per_s=float(np.median([r['audio_per_s'] for r in rs])))
-                if arm == 'server':
+                if arm != 'groups':
                     runs = pool('dec_runs')
                     row['decoder_run_ms'] = {f'{lo}-{hi}': round(1e3 * float(np.median([t for n, t in runs if lo <= n <= hi])), 2)
                                              for lo, hi in ((1, 8), (9, 16), (17, 32), (33, 64)) if any(lo <= n <= hi for n, _ in runs)}

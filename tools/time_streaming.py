@@ -7,6 +7,7 @@ The stop projection's bias is set so that the stop token never fires: every utte
 round by round on the same text:
   * stream/<chunk>: speech_stream at that decoder chunk: time to first audio, the wall time between chunks, and the real-time factor
     (wall time / audio duration);
+  * fstream/<chunk>: speech_stream(…, target=11000, overlap=550): folded streaming, whose audio equals the folded arm's;
   * unfolded: Tacotron.inference, then WaveRNN.generate(mel, target=F hop, overlap=0) (one row);
   * folded: Tacotron.inference, then WaveRNN.generate_batch([mel], 11000, 550).
 Every time is a host clock that ends in torch.cuda.synchronize().  The card's name and power limit are read in the same run."""
@@ -55,14 +56,15 @@ def main():
     for mode in a.modes.split(','):
         torch.manual_seed(2)
         voc = WaveRNN(**dict(DIMS, mode=mode)).cuda().eval()
-        arms = [f'stream/{c}' for c in chunks] + ['unfolded', 'folded']
+        arms = [f'stream/{c}' for c in chunks] + [f'fstream/{c}' for c in chunks] + ['unfolded', 'folded']
 
         def run(arm):
             torch.cuda.synchronize()
             t0 = time.perf_counter()
             stamps = []
-            if arm.startswith('stream/'):
-                for w in speech_stream(taco, voc, text, chunk_frames=int(arm.split('/')[1])):
+            if '/' in arm:
+                fold = dict(target=11000, overlap=550) if arm.startswith('fstream/') else {}
+                for w in speech_stream(taco, voc, text, chunk_frames=int(arm.split('/')[1]), **fold):
                     torch.cuda.synchronize()
                     stamps.append((time.perf_counter() - t0, int(w.shape[0])))
             else:
