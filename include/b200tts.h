@@ -132,6 +132,12 @@ typedef struct {
                                stop and their gradients; frames of the last step past T are dropped (zero gradient).  The parameters
                                predict R frames per step: frame_w [R*N, D+M], frame_b [R*N], stop_w [R, D+M], stop_b [R], row block j
                                (rows j*N .. j*N+N-1 of frame_w, row j of stop_w) = frame j of the step.  Negative R is rejected. */
+    int att_window_back, att_window_ahead;  /* windowed synthesis, location-sensitive attention and b200tts_decoder_forward_chunk only;
+                               ahead = 0 (a zero-initialised shape) is off.  Otherwise (back >= 0, ahead >= 1) each step of utterance b
+                               gives energies only to positions [c - back, c + ahead] within [0, length_b), where c is
+                               b200tts_decoder_state.attended[b]; the softmax and the context run over those positions, every other
+                               weight is exactly 0, and after the step c becomes the lowest position of the row's largest weight.
+                               b200tts_decoder_forward and _backward, and forward attention, reject a window. */
 } b200tts_decoder_shape;
 
 /* Parameter block in the reference's own layouts ([out, in] Linear weights; names = state_dict keys). */
@@ -212,7 +218,7 @@ int b200tts_decoder_forward(const b200tts_decoder_shape* shape, const b200tts_de
                             const b200tts_decoder_inputs* in, const b200tts_decoder_outputs* out, void* workspace,
                             size_t workspace_bytes, void* stream);
 
-/* Decoder state carried between chunks of one decode (all device pointers, fp32; every field required): lets a caller decode in
+/* Decoder state carried between chunks of one decode (all device pointers, fp32 but `attended`; every field but `attended` required): lets a caller decode in
  * chunks of T frames and stop early, as the reference's inference loop does (Decoder.inference, tacotron2.py:201-207,216-219). */
 typedef struct {
     float* att_h; float* att_c; /* [B, D] attention-LSTM state */
@@ -220,6 +226,8 @@ typedef struct {
     float* context;             /* [B, M] last attention context */
     float* cum_weights;         /* [B, L] cumulative attention weights (forward attention: the last alignment = alpha) */
     float* frame;               /* [B, N] last predicted frame, the last of the last step's R (input of the next free-running step) */
+    int32_t* attended;          /* [B] window centre: the first argmax of the last alignment row, 0 before step 0.  Read and written only
+                                   with a window (shape->att_window_ahead >= 1); may be NULL without one */
 } b200tts_decoder_state;
 
 /* b200tts_decoder_forward on a chunk of T frames: `first` != 0 starts from the zero state (tacotron2.py:164-168), otherwise from
@@ -234,7 +242,8 @@ int b200tts_decoder_forward_chunk(const b200tts_decoder_shape* shape, const b200
 /* Writes the initial state of a decode into the `count` listed rows (host int32, each in [0, shape->B)) of `state`, whose buffers hold
  * shape->B rows of width L, M, D and N: zeros, and for forward attention (shape->att_kind) the one-hot alpha_0 in cum_weights.  A chunk
  * with `first` = 0 then continues such a row exactly as a chunk with `first` != 0 starts a fresh decode: both write the state through the
- * same kernel.  The other rows are untouched, so texts can join a running decode.  Only B, L, M, D, N and att_kind of `shape` are read. */
+ * same kernel.  The other rows are untouched, so texts can join a running decode.  Only B, L, M, D, N and att_kind of `shape` are read.
+ * A non-NULL state->attended gets 0 in the listed rows. */
 int b200tts_decoder_state_reset_rows(const b200tts_decoder_shape* shape, b200tts_decoder_state* state, const int32_t* rows, int count,
                                      void* stream);
 

@@ -20,7 +20,8 @@ class B200TTSError(RuntimeError):
 
 class DecoderShape(Structure):
     _fields_ = [(n, c_int) for n in ('B', 'L', 'T', 'M', 'D', 'P', 'A', 'C', 'K', 'N', 'cell_kind', 'training')] + \
-               [('rate_h', c_float), ('rate_c', c_float), ('prenet_rate', c_float), ('att_kind', c_int), ('att_extent', c_int), ('R', c_int)]
+               [('rate_h', c_float), ('rate_c', c_float), ('prenet_rate', c_float), ('att_kind', c_int), ('att_extent', c_int), ('R', c_int),
+                                                                     ('att_window_back', c_int), ('att_window_ahead', c_int)]
 
 
 DECODER_PARAM_FIELDS = ('prenet_w0', 'prenet_b0', 'prenet_w1', 'prenet_b1', 'att_w_ih', 'att_w_hh', 'att_b_ih', 'att_b_hh',
@@ -43,7 +44,7 @@ class DecoderOutputs(Structure):
 
 
 class DecoderState(Structure):
-    _fields_ = [(n, c_void_p) for n in ('att_h', 'att_c', 'gen_h', 'gen_c', 'context', 'cum_weights', 'frame')]
+    _fields_ = [(n, c_void_p) for n in ('att_h', 'att_c', 'gen_h', 'gen_c', 'context', 'cum_weights', 'frame', 'attended')]
 
 
 class DecoderOutputGrads(Structure):

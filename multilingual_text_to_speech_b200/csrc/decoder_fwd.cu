@@ -174,6 +174,9 @@ struct AttnFwdArgs {
     float* ctx_out; int ld_ctx;        // [B, ld]
     float* ctx_out2; int ld_ctx2;      // optional second copy
     int B, L, M, A, C, K;
+    // windowed synthesis (attn_fwd_kernel<true>): per utterance the window centre c, read at the start of the step and overwritten
+    // with the step's first argmax; only positions [c - win_back, c + win_ahead] within [0, length) get an energy
+    int* attended; int win_back, win_ahead;
 };
 
 static inline size_t attn_fwd_smem_floats(int L, int M, int A, int C, int K) {
@@ -182,6 +185,9 @@ static inline size_t attn_fwd_smem_floats(int L, int M, int A, int C, int K) {
            (size_t)(ATT_THREADS / 32) * M;
 }
 
+// WINDOW = false is the step every path ran before windowed synthesis existed, compiled to the same instructions.  WINDOW = true runs
+// the same loops over [lo, hi) instead of [0, len); a window that covers [0, len) therefore gives the bits of WINDOW = false.
+template <bool WINDOW>
 __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnFwdArgs p) {
     extern __shared__ __align__(16) float sm[];
     const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -199,6 +205,13 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnFwdArgs
     float* cred = red + 64;
     int len = p.lengths[b];
     len = len < 0 ? 0 : (len > L ? L : len);
+    int lo = 0, hi = len;
+    if constexpr (WINDOW) {
+        const int c = p.attended[b];        // read by every thread before the first barrier; written back after the last one
+        lo = c > p.win_back ? c - p.win_back : 0;
+        hi = p.win_ahead >= len - c ? len : c + p.win_ahead + 1;
+        if (hi < lo) hi = lo;
+    }
 
     for (int a = tid; a < A; a += ATT_THREADS) {
         float q = 0.f;
@@ -222,14 +235,14 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnFwdArgs
     for (int idx = tid; idx < C * Lp; idx += ATT_THREADS) {
         const int c = idx / Lp, l = idx % Lp;
         float acc = 0.f;
-        if (l < L)
+        if (l < L && (!WINDOW || (l >= (lo & ~3) && l < hi)))
             for (int k = 0; k < K; ++k) acc = fmaf(Wcs[c * K + k], cump[l + k], acc);
         f[idx] = acc;
     }
     __syncthreads();
 
     // energies: warp = 4 consecutive positions, lane = attention dims {lane, lane+32, lane+64, lane+96}
-    for (int l0 = warp * 4; l0 < len; l0 += NW * 4) {
+    for (int l0 = (lo & ~3) + warp * 4; l0 < hi; l0 += NW * 4) {
         float s[4][4];
 #pragma unroll
         for (int i = 0; i < 4; ++i)
@@ -249,7 +262,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnFwdArgs
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
             const int l = l0 + i;
-            if (l < len) {                      // warp-uniform
+            if ((!WINDOW || l >= lo) && l < hi) {       // warp-uniform
                 float ep = 0.f;
                 const float* mt = p.memT + ((size_t)b * L + l) * A;
 #pragma unroll
@@ -264,22 +277,37 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnFwdArgs
     }
     __syncthreads();
 
-    // masked softmax over l < len (energies[~mask] = -inf, attention.py:77-83)
+    // masked softmax over l < len (energies[~mask] = -inf, attention.py:77-83), or over the window
     float mx = -INFINITY;
-    for (int l = tid; l < len; l += ATT_THREADS) mx = fmaxf(mx, e[l]);
+    for (int l = lo + tid; l < hi; l += ATT_THREADS) mx = fmaxf(mx, e[l]);
     mx = block_max(mx, red);
     float sum = 0.f;
-    for (int l = tid; l < len; l += ATT_THREADS) {
+    for (int l = lo + tid; l < hi; l += ATT_THREADS) {
         const float ex = expf(e[l] - mx);
         e[l] = ex;
         sum += ex;
     }
     sum = block_sum(sum, red);
+    float best_w = -1.f;        // WINDOW: this thread's first largest weight and its position
+    int best_l = 0;
     for (int l = tid; l < L; l += ATT_THREADS) {
-        const float w = l < len ? e[l] / sum : 0.f;
+        const float w = (!WINDOW || l >= lo) && l < hi ? e[l] / sum : 0.f;
         e[l] = w;
         p.align[(size_t)b * p.align_bstride + l] = w;
         p.cum_next[(size_t)b * L + l] = cump[l + half] + w;
+        if constexpr (WINDOW)
+            if (w > best_w) { best_w = w; best_l = l; }
+    }
+    __shared__ float arg_w[WINDOW ? NW : 1];
+    __shared__ int arg_l[WINDOW ? NW : 1];
+    if constexpr (WINDOW) {     // first argmax of the row: the largest weight, then the lowest position
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float ow = __shfl_xor_sync(0xffffffffu, best_w, o);
+            const int ol = __shfl_xor_sync(0xffffffffu, best_l, o);
+            if (ow > best_w || (ow == best_w && ol < best_l)) { best_w = ow; best_l = ol; }
+        }
+        if (lane == 0) { arg_w[warp] = best_w; arg_l[warp] = best_l; }
     }
     __syncthreads();
 
@@ -287,7 +315,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnFwdArgs
     float acc[16];
 #pragma unroll
     for (int j = 0; j < 16; ++j) acc[j] = 0.f;
-    for (int l = warp; l < len; l += NW) {
+    for (int l = lo + warp; l < hi; l += NW) {
         const float w = e[l];
         const float* row = p.memory + ((size_t)b * L + l) * M;
 #pragma unroll
@@ -308,6 +336,15 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnFwdArgs
         for (int w = 0; w < NW; ++w) s += cred[w * M + m];
         p.ctx_out[(size_t)b * p.ld_ctx + m] = s;
         if (p.ctx_out2) p.ctx_out2[(size_t)b * p.ld_ctx2 + m] = s;
+    }
+    if constexpr (WINDOW) {
+        if (tid == 0) {
+            float bw = arg_w[0];
+            int bl = arg_l[0];
+            for (int w = 1; w < NW; ++w)
+                if (arg_w[w] > bw || (arg_w[w] == bw && arg_l[w] < bl)) { bw = arg_w[w]; bl = arg_l[w]; }
+            p.attended[b] = bl;
+        }
     }
 }
 
@@ -412,6 +449,7 @@ struct DecInitRows {
     float* att_c; float* gen_h; float* gen_c;   // [rows, D]
     float* cum;                         // [rows, L]
     float* frame;                       // [rows, N]; N = 0 when absent
+    int* attended;                      // [rows] window centres, or null
     int M, D, L, N, one_hot;
     int n;                              // listed rows; 0: rows 0 .. count - 1
     int row[B200TTS_DECODER_RESET_MAX_ROWS];
@@ -433,7 +471,11 @@ __global__ void decoder_init_rows_kernel(const __grid_constant__ DecInitRows a, 
         c -= a.D;
         if (c < a.D) { a.gen_c[r * a.D + c] = 0.f; continue; }
         c -= a.D;
-        if (c < a.L) { a.cum[r * a.L + c] = (a.one_hot && c == 0) ? 1.f : 0.f; continue; }
+        if (c < a.L) {
+            a.cum[r * a.L + c] = (a.one_hot && c == 0) ? 1.f : 0.f;
+            if (c == 0 && a.attended) a.attended[r] = 0;
+            continue;
+        }
         a.frame[r * a.N + c - a.L] = 0.f;
     }
 }
@@ -457,17 +499,23 @@ int launch_cell_fwd(const CellFwdArgs& a, cudaStream_t st) {
 }
 namespace {
 
+template <bool WINDOW>
+int launch_attn_fwd_as(const AttnFwdArgs& a, size_t smem, cudaStream_t st) {
+    static size_t configured = 0;
+    if (smem > configured) {
+        B200_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<WINDOW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        configured = smem;
+    }
+    attn_fwd_kernel<WINDOW><<<a.B, ATT_THREADS, smem, st>>>(a);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+// a.attended != NULL selects the windowed step
 int launch_attn_fwd(const AttnFwdArgs& a, cudaStream_t st) {
     const size_t smem = attn_fwd_smem_floats(a.L, a.M, a.A, a.C, a.K) * sizeof(float);
     B200_REQUIRE(smem <= 227 * 1024, "attention step: shared memory %zu B exceeds 227 KB (L=%d M=%d)", smem, a.L, a.M);
-    static size_t configured = 0;
-    if (smem > configured) {
-        B200_CUDA(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured = smem;
-    }
-    attn_fwd_kernel<<<a.B, ATT_THREADS, smem, st>>>(a);
-    B200_LAUNCH_CHECK();
-    return B200TTS_OK;
+    return a.attended ? launch_attn_fwd_as<true>(a, smem, st) : launch_attn_fwd_as<false>(a, smem, st);
 }
 
 int launch_fwd_attn(const FwdAttnArgs& a, cudaStream_t st) {
@@ -516,6 +564,11 @@ int validate_decoder_shape(const b200tts_decoder_shape& s) {
         B200_REQUIRE(s.C <= 32 && s.C % 4 == 0, "decoder: location channels %d unsupported (need <= 32, multiple of 4)", s.C);
     }
     B200_REQUIRE(s.M <= 512, "decoder: memory dimension %d > 512 unsupported", s.M);
+    B200_REQUIRE(s.att_window_back >= 0 && s.att_window_ahead >= 0 && (s.att_window_ahead > 0 || s.att_window_back == 0),
+                 "decoder: bad attention window [%d, %d] (need back >= 0 and ahead >= 1, or both 0 for none)", s.att_window_back,
+                 s.att_window_ahead);
+    B200_REQUIRE(!(attention_window(s) && forward_attention(s)),
+                 "decoder: an attention window needs location-sensitive attention (forward attention moves at most one position a step)");
     B200_REQUIRE(s.cell_kind == B200TTS_CELL_DROPOUT || s.cell_kind == B200TTS_CELL_ZONEOUT, "decoder: bad cell kind %d", s.cell_kind);
     B200_REQUIRE(s.rate_h >= 0.f && s.rate_h < 1.f && s.rate_c >= 0.f && s.rate_c < 1.f && s.prenet_rate >= 0.f && s.prenet_rate < 1.f,
                  "decoder: dropout / zoneout rates must be in [0, 1)");
@@ -534,6 +587,7 @@ struct FwdCtx {
     DecoderLayout lay;
     float* ws;
     cudaStream_t st;
+    int* attended = nullptr;            // the carried window centres, with a window
     float* at(size_t off) const { return ws + off; }
 };
 
@@ -602,6 +656,7 @@ int att_step(const FwdCtx& c, int i, float* align_out) {
     aa.align = align_out + (size_t)i * s.L; aa.align_bstride = (long long)s.T * s.L;
     aa.ctx_out = ai_n; aa.ld_ctx = (int)MD; aa.ctx_out2 = nullptr; aa.ld_ctx2 = 0;
     aa.B = s.B; aa.L = s.L; aa.M = s.M; aa.A = s.A; aa.C = s.C; aa.K = s.K;
+    aa.attended = c.attended; aa.win_back = s.att_window_back; aa.win_ahead = s.att_window_ahead;
     B200_TRY(launch_attn_fwd(aa, c.st));
     return B200TTS_OK;
 }
@@ -655,6 +710,11 @@ int decoder_forward_impl(const b200tts_decoder_shape& frames, const b200tts_deco
     const b200tts_decoder_shape s = step_shape(frames);     // T = decoder steps from here on; Tf = target frames
     const bool resume = state != nullptr && !first;       // chunked decode: start from the carried state
     FwdCtx c{s, w, in, decoder_layout(s), ws, st};
+    if (attention_window(s)) {
+        B200_REQUIRE(state != nullptr && state->attended != nullptr,
+                     "decoder_forward: an attention window needs a carried state with `attended` (b200tts_decoder_forward_chunk)");
+        c.attended = state->attended;   // read and written in place by every step: one CTA per utterance
+    }
     const auto& l = c.lay;
     B200_REQUIRE(ws != nullptr && ws_bytes >= l.total * sizeof(float), "decoder_forward: workspace too small (%zu < %zu bytes)",
                  ws_bytes, l.total * sizeof(float));
@@ -701,7 +761,7 @@ int decoder_forward_impl(const b200tts_decoder_shape& frames, const b200tts_deco
         DecInitRows a{};
         a.ctx = c.at(l.ai); a.ld_ctx = MD; a.att_h = c.at(l.ai) + M; a.ld_att_h = MD;
         a.att_c = c.at(l.ca); a.gen_h = c.at(l.hg); a.gen_c = c.at(l.cg); a.cum = c.at(l.cum);
-        a.M = M; a.D = D; a.L = s.L; a.one_hot = forward_attention(s);
+        a.M = M; a.D = D; a.L = s.L; a.one_hot = forward_attention(s); a.attended = c.attended;
         B200_TRY(launch_init_rows(a, B, st));
     }
 
@@ -849,6 +909,7 @@ int decoder_state_reset_rows_impl(const b200tts_decoder_shape& s, const b200tts_
     DecInitRows a{};
     a.ctx = state.context; a.ld_ctx = s.M; a.att_h = state.att_h; a.ld_att_h = s.D;
     a.att_c = state.att_c; a.gen_h = state.gen_h; a.gen_c = state.gen_c; a.cum = state.cum_weights; a.frame = state.frame;
+    a.attended = state.attended;
     a.M = s.M; a.D = s.D; a.L = s.L; a.N = s.N; a.one_hot = forward_attention(s);
     for (int k0 = 0; k0 < count; k0 += B200TTS_DECODER_RESET_MAX_ROWS) {
         a.n = count - k0 < B200TTS_DECODER_RESET_MAX_ROWS ? count - k0 : B200TTS_DECODER_RESET_MAX_ROWS;

@@ -252,8 +252,11 @@ class DecoderConfig:
 
     MASK_NAMES = ('prenet0', 'prenet1', 'att_h', 'att_c', 'gen_h', 'gen_c', 'step_prenet0', 'step_prenet1')
 
-    def __init__(self, cell_kind, training, rate_h, rate_c, prenet_rate, masks=None, teacher=None, att_extent=0, outputs_per_step=1):
+    def __init__(self, cell_kind, training, rate_h, rate_c, prenet_rate, masks=None, teacher=None, att_extent=0, outputs_per_step=1,
+                 att_window=None):
         self.att_extent = int(att_extent)    # 1: forward attention over each utterance's own length (inference of padded batches)
+        # (back, ahead) or None: windowed location-sensitive attention, decoder_forward_chunk only (b200tts_decoder_shape.att_window_*)
+        self.att_window = None if att_window is None else (int(att_window[0]), int(att_window[1]))
         self.cell_kind = int(cell_kind)
         self.training = bool(training)
         self.rate_h, self.rate_c, self.prenet_rate = float(rate_h), float(rate_c), float(prenet_rate)
@@ -278,7 +281,7 @@ def _decoder_structs(cfg, shape_dims, params, memory, text_lengths, target):
     S = cfg.steps(T)
     att_kind = _attention_dims(dict(zip(DECODER_PARAM_FIELDS, params)))[0]
     shape = DecoderShape(B, L, T, M, D, P, A, C, K, N, cfg.cell_kind, int(cfg.training), cfg.rate_h, cfg.rate_c,
-                         cfg.prenet_rate, att_kind, cfg.att_extent, cfg.outputs_per_step)
+                         cfg.prenet_rate, att_kind, cfg.att_extent, cfg.outputs_per_step, *(cfg.att_window or (0, 0)))
     pstruct = DecoderParams(*[ptr(p) for p in params])
     teacher_np = None
     if cfg.teacher is not None:
@@ -370,11 +373,12 @@ class DecoderState:
         z = lambda *shape: torch.zeros(*shape, device=device, dtype=torch.float32)   # noqa: E731
         self.att_h, self.att_c, self.gen_h, self.gen_c = z(B, D), z(B, D), z(B, D), z(B, D)
         self.context, self.cum_weights, self.frame = z(B, M), z(B, L), z(B, N)
+        self.attended = torch.zeros(B, device=device, dtype=torch.int32)     # window centres (read only with a window)
         self.first = True
 
     def select(self, rows):
         """Keep only the utterances `rows` (a device index tensor), in that order: a finished utterance leaves the decode."""
-        for name in ('att_h', 'att_c', 'gen_h', 'gen_c', 'context', 'cum_weights', 'frame'):
+        for name in ('att_h', 'att_c', 'gen_h', 'gen_c', 'context', 'cum_weights', 'frame', 'attended'):
             setattr(self, name, getattr(self, name).index_select(0, rows).contiguous())
 
     def grow(self, b, L):
@@ -383,6 +387,8 @@ class DecoderState:
         for name in ('att_h', 'att_c', 'gen_h', 'gen_c', 'context', 'frame'):
             t = getattr(self, name)
             setattr(self, name, torch.cat([t, t.new_empty(b, t.shape[1])]) if b else t)
+        if b:
+            self.attended = torch.cat([self.attended, self.attended.new_empty(b)])
         cum = self.cum_weights
         out = cum.new_zeros(cum.shape[0] + b, L)
         w = min(L, cum.shape[1])
@@ -400,12 +406,14 @@ class DecoderState:
                                                            _stream()), 'b200tts_decoder_state_reset_rows')
 
     def struct(self):
-        return _lib.DecoderState(*[ptr(t) for t in (self.att_h, self.att_c, self.gen_h, self.gen_c, self.context, self.cum_weights, self.frame)])
+        return _lib.DecoderState(*[ptr(t) for t in (self.att_h, self.att_c, self.gen_h, self.gen_c, self.context, self.cum_weights, self.frame,
+                                                    self.attended)])
 
 
 def decoder_forward_chunk(cfg, memory, text_lengths, params, state, frames):
     """`frames` free-running frames (frames / r decoder steps; a multiple of r) continuing from `state` (updated in place); no autograd
-    (inference).  -> spectrogram [B, frames, N], stop [B, frames], alignment [B, frames / r, L]."""
+    (inference).  cfg.att_window, if set, confines each step's attention to the window around state.attended, which the call advances.
+    -> spectrogram [B, frames, N], stop [B, frames], alignment [B, frames / r, L]."""
     _require_cuda(memory, text_lengths, *params)
     with torch.no_grad():
         memory = _f32c(memory)

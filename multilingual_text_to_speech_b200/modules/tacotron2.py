@@ -217,18 +217,19 @@ class Decoder(torch.nn.Module):
         """Positions (into `rows`, the original indices of the utterances still decoding) of the utterances whose stop cut is unknown."""
         return [j for j, r in enumerate(rows) if rules[r].cut is None]
 
-    def _inference_chunks(self, encoded_input, mask, speaker, language, att_extent=0, tape_columns=None, chunk_frames=None):
+    def _inference_chunks(self, encoded_input, mask, speaker, language, att_extent=0, tape_columns=None, chunk_frames=None, att_window=None):
         """The chunk loop of free-running inference (tacotron2.py:148-209 with target=None) over a batch whose texts all open at the
         first call: every chunk is one library call of chunk_frames (default inference_chunk) frames rounded down to whole steps; after
         each it feeds the chunk's stop logits to the utterances' stop rules and yields (rows, spec [b, Tc, N], stop [b, Tc], alignment
         [b, Tc / r, L], rules, done): rows are the original indices of the b utterances the chunk decoded, rules the stop rule of every
         utterance, done the frames decoded so far.  Then an utterance whose cut is known leaves the decode (_DecodeRows.retire) and the next
         chunk runs at the smaller batch.  The loop ends when every cut is known or hp.max_output_length frames are decoded.  The rule reads
-        the r stop logits of each step in frame order.  Utterance b reads column tape_columns[b] (default b) of an active mask tape."""
+        the r stop logits of each step in frame order.  Utterance b reads column tape_columns[b] (default b) of an active mask tape.
+        att_window: None or (back, ahead), windowed attention (inference_attention_window)."""
         memory = self._memory(encoded_input, speaker, language)
         B = memory.shape[0]
         columns = list(range(B)) if tape_columns is None else list(tape_columns)
-        rows = _DecodeRows(self, att_extent)
+        rows = _DecodeRows(self, att_extent, att_window)
         rows.add(memory, [int(n) for n in mask.sum(dim=1).tolist()], list(range(B)), [('shared', c) for c in columns])
         rules = list(rows.rules)
         chunk_steps = max(1, (self.inference_chunk if chunk_frames is None else int(chunk_frames)) // self._outputs_per_step)
@@ -237,11 +238,11 @@ class Decoder(torch.nn.Module):
             yield list(rows.keys), spec, stop, align, rules, rows.done[0]
             rows.retire()
 
-    def _decode_inference(self, encoded_input, mask, speaker, language, att_extent=0, tape_columns=None):
+    def _decode_inference(self, encoded_input, mask, speaker, language, att_extent=0, tape_columns=None, att_window=None):
         """Free-running decode in chunks with carried state and early exit (_inference_chunks).  B == 1 reproduces the reference; B > 1
         (which the reference cannot run: it uses the stop token as a Python bool) keeps one stop rule per utterance.  `att_extent` = 1 runs
         forward attention over each utterance's own length; `tape_columns` gives each utterance's column of a recorded mask tape (default:
-        column b for utterance b).
+        column b for utterance b); `att_window` confines each step's attention (inference_attention_window).
         -> (spectrogram [B, T', N], stop [B, T'], alignment [B, ceil(T' / r), L], cuts): T' = max(cuts) frames; utterance b is zero past
         cuts[b] (its alignment past ceil(cuts[b] / r) steps).  hp.max_output_length counts frames."""
         B, L = encoded_input.shape[0], encoded_input.shape[1]
@@ -249,7 +250,8 @@ class Decoder(torch.nn.Module):
         N = self._output_dim
         outs = [[] for _ in range(B)]
         done = 0
-        for rows, spec, stop, align, rules, done in self._inference_chunks(encoded_input, mask, speaker, language, att_extent, tape_columns):
+        for rows, spec, stop, align, rules, done in self._inference_chunks(encoded_input, mask, speaker, language, att_extent, tape_columns,
+                                                                           att_window=att_window):
             if align.shape[2] < L:          # the chunk ran after the longest text left: its weights past the shorter ones are zero
                 align = TF.pad(align, (0, L - align.shape[2]))
             for j, u in enumerate(rows):
@@ -402,8 +404,10 @@ class Tacotron(torch.nn.Module):
         text in the forms `inference` takes (speaker int64 [1]; language int64 [1] or float [1, L_i, G]).  -> one post-net spectrogram
         [num_mels, T_i] per text, in input order.  Texts are sorted by length and decoded in padded groups of at most max_batch (eval
         mode, no grad); each utterance's output equals `inference` of it alone given the same prenet dropout masks (a recorded tape,
-        [T, len(texts), P] with one column per text).  Without a tape a batched run draws other masks than single runs do."""
+        [T, len(texts), P] with one column per text).  Without a tape a batched run draws other masks than single runs do.
+        hp.inference_attention_window is read once per call."""
         speakers, languages = _check_batch_inputs(texts, speakers, languages)
+        window = inference_attention_window()
         was_training = self.training
         self.eval()
         outputs = [None] * len(texts)
@@ -411,7 +415,7 @@ class Tacotron(torch.nn.Module):
             with torch.no_grad():
                 for group in _batch_plan([int(t.shape[0]) for t in texts], max_batch):
                     posts = self._inference_group([texts[i] for i in group], None if speakers is None else [speakers[i] for i in group],
-                                                  None if languages is None else [languages[i] for i in group], group)
+                                                  None if languages is None else [languages[i] for i in group], group, window)
                     for i, post in zip(group, posts):
                         outputs[i] = post
         finally:
@@ -505,17 +509,32 @@ class Tacotron(torch.nn.Module):
             language = torch.argmax(language, dim=2)  # one-hot into indices for the decoder's language embedding
         return encoded, lengths_to_mask(lengths, Lmax), speaker, language
 
-    def _inference_group(self, texts, speakers, languages, tape_columns):
+    def _inference_group(self, texts, speakers, languages, tape_columns, att_window):
         device = self._embedding.weight.device
         encoded, mask, speaker, language = self._encode_group(texts, speakers, languages)
         B = len(texts)
-        prediction, _, _, cuts = self._decoder._decode_inference(encoded, mask, speaker, language, att_extent=1, tape_columns=tape_columns)
+        prediction, _, _, cuts = self._decoder._decode_inference(encoded, mask, speaker, language, att_extent=1, tape_columns=tape_columns,
+                                                                 att_window=att_window)
         post = self._postnet(prediction.transpose(1, 2), torch.tensor(cuts, device=device), padded=True)
         return [post[b, :, :cuts[b]] for b in range(B)]
 
 
 # texts of one inference_streams group at most: the batch inference_batch decodes at once by default
 MAX_STREAM_TEXTS = 64
+
+
+def inference_attention_window():
+    """hp.inference_attention_window checked -> None (off) or (back, ahead) with back >= 0, ahead >= 1.  ValueError for any other value,
+    and for a window with forward attention, which already moves at most one position per step."""
+    w = hp.inference_attention_window
+    if w is None:
+        return None
+    ok = isinstance(w, (list, tuple)) and len(w) == 2 and all(isinstance(x, (int, np.integer)) and not isinstance(x, bool) for x in w)
+    if not ok or int(w[0]) < 0 or int(w[1]) < 1:
+        raise ValueError(f'inference_attention_window must be None or [back >= 0, ahead >= 1] of ints (got {w!r})')
+    if hp.attention_type == 'forward':
+        raise ValueError('inference_attention_window needs location-sensitive attention: forward attention moves at most one position a step')
+    return int(w[0]), int(w[1])
 
 PRENET_SITES = ('step_prenet0', 'step_prenet1')
 
@@ -528,10 +547,11 @@ class _DecodeRows:
       * ('tape', {site: [S, P]}): the row's own recorded masks, step i of the row reading row i (all-ones past the tape's end);
       * ('seed', seed): b200tts_fill_keep_mask_rows at the row's own step count, stream _lib.SEED_STREAMS[site];
       * ('shared', column): with a MaskSource tape active, that column of it; otherwise one MaskSource draw over every shared row per
-        call, as the batched decode has always drawn."""
+        call, as the batched decode has always drawn.
+    att_window (None or (back, ahead)) goes to every call; each row's window centre is carried in the DecoderState."""
 
-    def __init__(self, dec, att_extent):
-        self.dec, self.att_extent = dec, att_extent
+    def __init__(self, dec, att_extent, att_window=None):
+        self.dec, self.att_extent, self.att_window = dec, att_extent, att_window
         self.memory = self.lengths = self.state = None
         self.keys, self.rules, self.done, self.sources, self.text_len = [], [], [], [], []
 
@@ -569,7 +589,7 @@ class _DecodeRows:
         if len(js) == len(self.keys):
             return
         if not js:
-            self.__init__(self.dec, self.att_extent)
+            self.__init__(self.dec, self.att_extent, self.att_window)
             return
         idx = torch.tensor(js, device=self.memory.device)
         self.state.select(idx)
@@ -649,7 +669,7 @@ class _DecodeRows:
                 if m is not None:
                     masks[name] = m
         cfg = F.DecoderConfig(kind, dec.training, rate_h, rate_c, dec._prenet._dropout_rate, masks, np.zeros(Sc, dtype=np.uint8),
-                              self.att_extent, outputs_per_step=r)
+                              self.att_extent, outputs_per_step=r, att_window=self.att_window)
         spec, stop, align = F.decoder_forward_chunk(cfg, self.memory, self.lengths, dec._param_list(), self.state, Sc * r)
         host_stop = stop.float().cpu()
         for j in range(len(self.keys)):
@@ -669,7 +689,8 @@ class DecoderPool:
     Prenet dropout masks per text: `masks` (a tape {'step_prenet0': [S, P], 'step_prenet1': [S, P]}) if given, else `seed` (draws that
     depend on the seed and the text's own steps only: its masks are one b200tts_fill_keep_mask((S, P), seed, _lib.SEED_STREAMS[site])
     call per site), else one shared MaskSource draw per call over such texts (with a MaskSource tape active: column `id` of it).  The
-    model runs each call in eval mode without autograd and is restored after it."""
+    model runs each call in eval mode without autograd and is restored after it.  hp.inference_attention_window is read when the pool is
+    built and kept for its life."""
 
     def __init__(self, tacotron, max_texts=64, chunk_frames=None):
         if not 1 <= int(max_texts) <= MAX_STREAM_TEXTS:
@@ -679,7 +700,7 @@ class DecoderPool:
         self.t, self.max_texts = tacotron, int(max_texts)
         dec = tacotron._decoder
         self.chunk_steps = max(1, (dec.inference_chunk if chunk_frames is None else int(chunk_frames)) // dec._outputs_per_step)
-        self.rows = _DecodeRows(dec, att_extent=1)
+        self.rows = _DecodeRows(dec, att_extent=1, att_window=inference_attention_window())
         self.queue = []                        # (id, text, speaker, language, source) opened since the last call
         self.pre, self.released = {}, {}       # per open text: its decoded chunks [n, N], the frames its post-net chunks cover
         self.next_id = 0

@@ -120,6 +120,9 @@ _AUDIO = dict(
 _B200 = dict(
     b200_precision="fp32",
     outputs_per_step=1,
+    # synthesis only: None, or [back, ahead] -- each free-running decoder step attends only to positions [c - back, c + ahead], c being
+    # the position the previous step attended most (0 before the first step); location-sensitive attention only
+    inference_attention_window=None,
 )
 
 _DEFAULTS = {}
