@@ -432,7 +432,9 @@ int b200tts_debug_bilstm_layout(const b200tts_bilstm_shape* shape, size_t* out, 
  * pre / post / targets [B, N, T]; stop (logits, padded positions already filled as in tacotron2.py:380) / stop_target [B, T]; alignment
  * [B, S, L] with S = ceil(T / R); lengths int32 [B].  losses[4] (device) = { 2*MSE(pre), MSE(post), BCEWithLogits(pos_weight)/(N+2),
  * guided attention }.  The guided term runs on the step grid: utterance b has ceil(target_lengths[b] / R) steps, which take the place of
- * its frame count in the weight and the division (R = 1: the reference's formula).                                                     */
+ * its frame count in the weight and the division (R = 1: the reference's formula).  The four mel buffers need no more than float
+ * alignment: the forward reads them four floats at a time with 16-byte loads when all four are 16-byte aligned and with scalar loads
+ * otherwise, in the same order and with the same arithmetic, so the result does not depend on their alignment.                     */
 typedef struct {
     int B, N, T, L;
     int guided;            /* hp.guided_attention_loss and guided_att_steps > 0 */

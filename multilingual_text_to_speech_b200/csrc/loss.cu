@@ -31,6 +31,14 @@ __device__ __forceinline__ float guided_weight(int t, int l, int Tb, int Lb, flo
     return 1.f - expf(-d * d * inv2g2);
 }
 
+// four consecutive floats: one 16-byte load when the caller's buffers allow it, four scalar loads otherwise (same arithmetic after)
+template <bool VEC>
+__device__ __forceinline__ float4 load4(const float* p) {
+    if constexpr (VEC) return *reinterpret_cast<const float4*>(p);
+    else return make_float4(p[0], p[1], p[2], p[3]);
+}
+
+template <bool VEC>
 __global__ void __launch_bounds__(LT) loss_partial_kernel(const LossArgs a, float* __restrict__ partial) {
     __shared__ float red[4][LT / 32];
     const size_t gid = (size_t)blockIdx.x * LT + threadIdx.x, gstride = (size_t)gridDim.x * LT;
@@ -38,8 +46,8 @@ __global__ void __launch_bounds__(LT) loss_partial_kernel(const LossArgs a, floa
     const size_t nmel = (size_t)a.B * a.N * a.T;
     for (size_t i = gid * 4; i < nmel; i += gstride * 4) {
         if (i + 3 < nmel) {
-            const float4 p = *reinterpret_cast<const float4*>(a.pre + i), pt = *reinterpret_cast<const float4*>(a.pre_t + i);
-            const float4 q = *reinterpret_cast<const float4*>(a.post + i), qt = *reinterpret_cast<const float4*>(a.post_t + i);
+            const float4 p = load4<VEC>(a.pre + i), pt = load4<VEC>(a.pre_t + i);
+            const float4 q = load4<VEC>(a.post + i), qt = load4<VEC>(a.post_t + i);
             s_pre += (p.x - pt.x) * (p.x - pt.x) + (p.y - pt.y) * (p.y - pt.y) + (p.z - pt.z) * (p.z - pt.z) + (p.w - pt.w) * (p.w - pt.w);
             s_post += (q.x - qt.x) * (q.x - qt.x) + (q.y - qt.y) * (q.y - qt.y) + (q.z - qt.z) * (q.z - qt.z) + (q.w - qt.w) * (q.w - qt.w);
         } else {
@@ -139,7 +147,12 @@ int loss_forward_impl(const b200tts_loss_shape& s, const float* pre, const float
     B200_REQUIRE(s.B > 0 && s.N > 0 && s.T > 0 && s.L > 0 && s.R >= 0, "loss_forward: bad shape");
     B200_REQUIRE(!s.guided || s.guided_g > 0.f, "loss_forward: guided attention needs a positive variance");
     const LossArgs a = make_args(s, pre, pre_t, post, post_t, stop, stop_t, align, text_len, target_len);
-    loss_partial_kernel<<<LOSS_BLOCKS, LT, 0, st>>>(a, ws);
+    const uintptr_t addr_bits = reinterpret_cast<uintptr_t>(pre) | reinterpret_cast<uintptr_t>(pre_t) | reinterpret_cast<uintptr_t>(post) |
+                                reinterpret_cast<uintptr_t>(post_t);
+    if ((addr_bits & 15) == 0)
+        loss_partial_kernel<true><<<LOSS_BLOCKS, LT, 0, st>>>(a, ws);
+    else
+        loss_partial_kernel<false><<<LOSS_BLOCKS, LT, 0, st>>>(a, ws);
     B200_LAUNCH_CHECK();
     const double nmel = (double)s.B * s.N * s.T, nstop = (double)s.B * s.T;
     loss_final_kernel<<<1, 32, 0, st>>>(ws, LOSS_BLOCKS, losses, (float)(2.0 / nmel), (float)(1.0 / nmel), (float)(1.0 / (nstop * (s.N + 2))),
