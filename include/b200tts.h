@@ -736,6 +736,22 @@ int b200tts_gru_seq_backward(const b200tts_gru_seq_shape* shape, const float* w_
                              float* dgi, float* dgh, float* dh_dbg, void* workspace, size_t workspace_bytes, void* stream);
 /* Synchronises the stream and sets *aborted to the loops' abort flag (nonzero: a loop on this workspace timed out since it was zeroed). */
 int b200tts_gru_seq_aborted(const b200tts_gru_seq_shape* shape, const void* workspace, size_t workspace_bytes, int* aborted, void* stream);
+/* Enqueues a copy of the loops' abort flag (one int) to dst (pinned host or device memory) on the stream, without synchronising: the caller
+ * reads *dst once the work enqueued before it has completed (an event recorded after the call).  For a training step captured in a CUDA
+ * graph, whose flag is read after the replay instead of inside it. */
+int b200tts_gru_seq_abort_flag_copy(const b200tts_gru_seq_shape* shape, const void* workspace, size_t workspace_bytes, int* dst, void* stream);
+/* Training windows from a corpus in device memory, one launch: fatchord's collate_vocoder with explicit offsets.
+ *   mels: fp32 [feat, total_frames], the utterances' mels side by side (utterance u's frames from frame_start[u]);
+ *   labels: uint16 [sum N_u] (utterance u's samples from sample_start[u]); frame_start, sample_start: int64, one per utterance;
+ *   table: int32 [B, 2] of (utterance u, mel offset o);
+ *   m [B, feat, mel_win] = mel_u[:, o : o + mel_win] with mel_win = seq_len / hop + 2 pad; the label window lab = labels_u[(o + pad) hop :
+ *   (o + pad) hop + seq_len + 1]; x [B, seq_len] fp32 = label_2_float(lab[:seq_len], MOL ? 16 : bits); y [B, seq_len] = lab[1:] as int64
+ *   (RAW) or label_2_float(lab[1:], 16) as fp32 (MOL).  label_2_float(v, b) = 2 v / (2^b - 1) - 1, each fp32 operation IEEE-rounded.
+ * Limits, checked on the host: mode RAW or MOL, bits 1 to 16, B 1 to 64, seq_len a positive multiple of the hop and at most 16 hops, pad 0 to
+ * 64, feat 1 to 1024.  The table is NOT checked: every window must lie inside its utterance's mel and labels (the caller validates it). */
+int b200tts_wavernn_cut_windows(int mode, int bits, int B, int feat, int seq_len, int pad, int hop, const float* mels, long long total_frames,
+                                const int64_t* frame_start, const uint16_t* labels, const int64_t* sample_start, const int32_t* table, float* x,
+                                void* y, float* m, void* stream);
 /* The adjoint of b200tts_wavernn_upsample_layer (C, len, scale, fir, in as there) for dout [C, len scale]: din [C, len] (overwritten; NULL:
  * not formed) and dfir [2 scale + 1] += the FIR gradient (NULL: not formed; needs `in` and the workspace, summed in a fixed order). */
 size_t b200tts_wavernn_upsample_layer_backward_workspace_bytes(int C, int len, int scale);

@@ -252,6 +252,8 @@ SIGNATURES = {
     'b200tts_gru_seq_forward': (c_int, [POINTER(GRUSeqShape)] + [c_void_p] * 6 + [c_size_t, c_void_p]),
     'b200tts_gru_seq_backward': (c_int, [POINTER(GRUSeqShape)] + [c_void_p] * 8 + [c_size_t, c_void_p]),
     'b200tts_gru_seq_aborted': (c_int, [POINTER(GRUSeqShape), c_void_p, c_size_t, POINTER(c_int), c_void_p]),
+    'b200tts_gru_seq_abort_flag_copy': (c_int, [POINTER(GRUSeqShape), c_void_p, c_size_t, c_void_p, c_void_p]),
+    'b200tts_wavernn_cut_windows': (c_int, [c_int] * 7 + [c_void_p, c_longlong] + [c_void_p] * 8),
     'b200tts_wavernn_upsample_layer_backward_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
     'b200tts_wavernn_upsample_layer_backward': (c_int, [c_int] * 3 + [c_void_p] * 6 + [c_size_t, c_void_p]),
     'b200tts_wavernn_stretch_backward': (c_int, [c_int] * 4 + [c_void_p] * 3),

@@ -281,6 +281,11 @@ int gru_seq_forward_impl(const b200tts_gru_seq_shape& s, const float* gi, const 
 int gru_seq_backward_impl(const b200tts_gru_seq_shape& s, const float* w_hh, const float* h, const void* saved, const float* dh_ext, float* dgi,
                           float* dgh, float* dh_dbg, void* ws, size_t ws_bytes, cudaStream_t st);
 int gru_seq_aborted_impl(const b200tts_gru_seq_shape& s, const void* ws, size_t ws_bytes, int* aborted, cudaStream_t st);
+int gru_seq_abort_flag_copy_impl(const b200tts_gru_seq_shape& s, const void* ws, size_t ws_bytes, int* dst, cudaStream_t st);
+int wavernn_cut_windows_check(int mode, int bits, int B, int feat, int seq_len, int pad, int hop, long long total_frames);
+int wavernn_cut_windows_impl(int mode, int bits, int B, int feat, int seq_len, int pad, int hop, const float* mels, long long total_frames,
+                             const long long* frame_start, const unsigned short* labels, const long long* sample_start, const int* table,
+                             float* x, void* y, float* m, cudaStream_t st);
 size_t wavernn_upsample_layer_backward_workspace_bytes(int C, int len, int scale);
 int wavernn_upsample_layer_backward_impl(int C, int len, int scale, const float* fir, const float* in, const float* dout, float* din, float* dfir,
                                          void* ws, size_t ws_bytes, cudaStream_t st);
@@ -948,6 +953,21 @@ int b200tts_gru_seq_aborted(const b200tts_gru_seq_shape* shape, const void* work
     B200_REQUIRE(shape && aborted, "gru_seq_aborted: null argument");
     B200_TRY(require_device());
     return gru_seq_aborted_impl(*shape, workspace, workspace_bytes, aborted, (cudaStream_t)stream);
+}
+int b200tts_gru_seq_abort_flag_copy(const b200tts_gru_seq_shape* shape, const void* workspace, size_t workspace_bytes, int* dst, void* stream) {
+    B200_REQUIRE(shape && dst, "gru_seq_abort_flag_copy: null argument");
+    B200_TRY(gru_seq_check(*shape, const_cast<void*>(workspace), workspace_bytes));
+    B200_TRY(require_device());
+    return gru_seq_abort_flag_copy_impl(*shape, workspace, workspace_bytes, dst, (cudaStream_t)stream);
+}
+int b200tts_wavernn_cut_windows(int mode, int bits, int B, int feat, int seq_len, int pad, int hop, const float* mels, long long total_frames,
+                                const int64_t* frame_start, const uint16_t* labels, const int64_t* sample_start, const int32_t* table, float* x,
+                                void* y, float* m, void* stream) {
+    B200_REQUIRE(mels && frame_start && labels && sample_start && table && x && y && m, "wavernn_cut_windows: null argument");
+    B200_TRY(wavernn_cut_windows_check(mode, bits, B, feat, seq_len, pad, hop, total_frames));
+    B200_TRY(require_device());
+    return wavernn_cut_windows_impl(mode, bits, B, feat, seq_len, pad, hop, mels, total_frames, reinterpret_cast<const long long*>(frame_start),
+                                    labels, reinterpret_cast<const long long*>(sample_start), table, x, y, m, (cudaStream_t)stream);
 }
 size_t b200tts_wavernn_upsample_layer_backward_workspace_bytes(int C, int len, int scale) {
     return wavernn_upsample_layer_backward_workspace_bytes(C, len, scale);

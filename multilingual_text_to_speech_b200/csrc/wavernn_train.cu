@@ -463,6 +463,12 @@ int gru_seq_aborted_impl(const b200tts_gru_seq_shape& s, const void* ws, size_t 
     return B200TTS_OK;
 }
 
+int gru_seq_abort_flag_copy_impl(const b200tts_gru_seq_shape& s, const void* ws, size_t ws_bytes, int* dst, cudaStream_t st) {
+    B200_TRY(gru_seq_check(s, const_cast<void*>(ws), ws_bytes));
+    B200_CUDA(cudaMemcpyAsync(dst, static_cast<const unsigned char*>(ws) + 128, sizeof(int), cudaMemcpyDefault, st));
+    return B200TTS_OK;
+}
+
 int wavernn_upsample_layer_check(int C, int len, int scale);      // wavernn.cu
 
 size_t wavernn_upsample_layer_backward_workspace_bytes(int C, int len, int scale) {

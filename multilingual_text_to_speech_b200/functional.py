@@ -1297,3 +1297,27 @@ class WaveRNNLossFunction(torch.autograd.Function):
 
 def wavernn_loss_rows(logits, target, mode):
     return WaveRNNLossFunction.apply(logits, target, mode)
+
+
+def wavernn_cut_windows(mode, bits, seq_len, pad, hop, mels, frame_start, labels, sample_start, table, out=None):
+    """Training windows of the device corpus (mels fp32 [feat, total frames], labels uint16, int64 frame / sample starts per utterance) for
+    the device table int32 [B, 2] of (utterance, mel offset): (x [B, seq_len] fp32, y [B, seq_len] (RAW int64, MOL fp32), m [B, feat,
+    mel_win] fp32), written into `out` when given.  The table is not checked (modules/wavernn.py VocoderCorpus validates it on the host)."""
+    _require_cuda(mels, frame_start, labels, sample_start, table)
+    B, feat = table.shape[0], mels.shape[0]
+    if out is None:
+        win = seq_len // hop + 2 * pad
+        out = (torch.empty(B, seq_len, device=mels.device, dtype=torch.float32),
+               torch.empty(B, seq_len, device=mels.device, dtype=torch.float32 if mode == 'MOL' else torch.int64),
+               torch.empty(B, feat, win, device=mels.device, dtype=torch.float32))
+    x, y, m = out
+    check(_lib.load().b200tts_wavernn_cut_windows(_lib.WAVERNN_MODES[mode], int(bits), B, feat, int(seq_len), int(pad), int(hop), ptr(mels),
+                                                  mels.shape[1], ptr(frame_start), ptr(labels), ptr(sample_start), ptr(table), ptr(x), ptr(y),
+                                                  ptr(m), _stream()), 'b200tts_wavernn_cut_windows')
+    return x, y, m
+
+
+def gru_seq_abort_flag_copy(guard, dst):
+    """Enqueue a copy of `guard`'s abort flag into dst (one int32, pinned host or device) on the current stream, without synchronising."""
+    check(_lib.load().b200tts_gru_seq_abort_flag_copy(ctypes.byref(guard.shape), ptr(guard.ws), guard.ws.numel(), ptr(dst), _stream()),
+          'b200tts_gru_seq_abort_flag_copy')

@@ -24,6 +24,7 @@ import ctypes
 import torch
 
 from . import _lib
+from . import functional as F
 from .modules.encoder import ConvolutionalEncoder, GeneratedConvolutionalEncoder, GroupLayout, encoder_layout, given_layout, language_ids
 
 
@@ -161,3 +162,138 @@ class GraphedTrainStep:
 
     def close(self):
         _lib.check(_lib.load().b200tts_set_mask_epoch(None), 'b200tts_set_mask_epoch')
+
+
+class DeferredAbortCheck:
+    """The GRU loops' abort flag of a captured vocoder step, read after the replay instead of inside it (a read inside would synchronise).
+
+    After each replay `after_replay(n)` enqueues an asynchronous copy of the flag into a host slot and records an event.  `poll()` (at the
+    next call) reads, oldest first, every copied flag whose event has completed, without waiting; `wait()` (check() and close()) waits for
+    all of them.  A set flag raises B200TTSError naming its replay.  At most `depth` flags are outstanding: the replay after that waits for
+    the oldest copy, which keeps the host at most `depth` replays ahead of the device.
+
+    copy_flag(slot) enqueues the copy into `slot` (int32 [1]); new_event() returns an object with record(), query() and synchronize()
+    (torch.cuda.Event on the device; a stand-in in the host tests)."""
+
+    def __init__(self, copy_flag, new_event, depth=4, pin=True):
+        from collections import deque
+        self._copy, self._new_event, self.depth = copy_flag, new_event, int(depth)
+        self._free = [torch.zeros(1, dtype=torch.int32, pin_memory=pin) for _ in range(self.depth)]
+        self._pending = deque()
+
+    def after_replay(self, replay):
+        while len(self._pending) >= self.depth:
+            self._pending[0][2].synchronize()
+            self._read_oldest()
+        slot = self._free.pop()
+        self._copy(slot)
+        ev = self._new_event()
+        ev.record()
+        self._pending.append((replay, slot, ev))
+
+    def poll(self):
+        while self._pending and self._pending[0][2].query():
+            self._read_oldest()
+
+    def wait(self):
+        while self._pending:
+            self._pending[0][2].synchronize()
+            self._read_oldest()
+
+    def _read_oldest(self):
+        replay, slot, _ = self._pending.popleft()
+        flag = int(slot[0])
+        slot.zero_()
+        self._free.append(slot)
+        if flag:
+            raise _lib.B200TTSError(f'GraphedVocoderStep: a GRU loop of replay {replay} timed out at a grid barrier')
+
+
+class GraphedVocoderStep:
+    """One WaveRNN training step as ONE CUDA graph: the windows cut from a device-resident corpus (modules.wavernn.VocoderCorpus),
+    WaveRNN.forward, wavernn_loss and the backward into the flat gradient bucket.  The optimizer step stays outside the graph
+    (FusedAdam takes the learning rate and the step count by value), as does the all-reduce of a data-parallel run:
+
+        step = GraphedVocoderStep(model, bucket, corpus, batch_size)     # warm-up + capture on capture_stream(device)
+        loss = step(ids, offsets)     # host-validated table -> static device table (one pinned copy), replay; loss: a device tensor
+        bucket.allreduce(); optimizer.step()
+
+    A call does not synchronise.  The GRU loops' abort flag (a grid-barrier timeout) is zeroed inside the graph, copied to pinned host memory
+    after each replay and read by a later call, check() or close() (DeferredAbortCheck), which raise B200TTSError naming the replay.
+    The batch-norm running statistics, num_batches_tracked and the model's `step` buffer are updated inside the graph, as an eager step
+    updates them; the warm-up's updates are rolled back, so constructing the step leaves the model's buffers as they were.  The precision
+    mode is fixed at capture: a call under another mode raises ValueError.  As with GraphedTrainStep, eager steps that precede the capture
+    on the same model should run on capture_stream(device)."""
+
+    def __init__(self, model, bucket, corpus, batch_size, warmup=3, abort_depth=4):
+        from .modules.wavernn import MAX_TRAIN_BATCH
+        B = int(batch_size)
+        if not 1 <= B <= MAX_TRAIN_BATCH:
+            raise ValueError(f'batch_size {batch_size}: need 1 to {MAX_TRAIN_BATCH} windows per step')
+        n_classes = 2 ** corpus.bits if corpus.mode == 'RAW' else model.n_classes
+        if (corpus.mode, corpus.hop, corpus.pad, corpus.feat, n_classes) != (model.mode, model.hop_length, model.pad, model.feat_dims,
+                                                                           model.n_classes):
+            raise ValueError(f'corpus (mode {corpus.mode}, hop {corpus.hop}, pad {corpus.pad}, {corpus.feat} mel channels, bits '
+                             f'{corpus.bits}) does not match the model (mode {model.mode}, hop {model.hop_length}, pad {model.pad}, '
+                             f'{model.feat_dims} mel channels, {model.n_classes} classes)')
+        first = next((u for u in range(len(corpus)) if corpus.labels_ok[u] and corpus.win <= corpus.frames[u]
+                      and corpus.pad * corpus.hop + corpus.seq_len + 1 <= corpus.samples[u]), None)
+        if first is None:
+            raise ValueError('the corpus has no utterance long enough for one window')
+        dev = corpus.device
+        self.model, self.bucket, self.corpus, self.batch_size = model, bucket, corpus, B
+        self.precision = _lib.get_precision()
+        self.table = torch.from_numpy(corpus.table([first] * B, [0] * B)).to(dev)
+        self.loss = None
+        self.replays = 0
+        saved = {k: v.clone() for k, v in model.named_buffers()}
+        side = capture_stream(dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):
+            for _ in range(warmup):
+                self._body()
+        torch.cuda.current_stream(dev).wait_stream(side)
+        torch.cuda.synchronize(dev)
+        with torch.no_grad():
+            for k, v in model.named_buffers():
+                v.copy_(saved[k])
+        torch.cuda.synchronize(dev)
+        model._graph_guard = None
+        self.graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.graph, stream=side):
+            self._body()
+        torch.cuda.synchronize(dev)
+        self.guard, model._graph_guard = model._graph_guard, None
+        if self.guard is None:
+            raise _lib.B200TTSError('GraphedVocoderStep: the captured forward left no GRU loop guard')
+        self.abort = DeferredAbortCheck(lambda slot: F.gru_seq_abort_flag_copy(self.guard, slot), torch.cuda.Event, abort_depth)
+
+    def _body(self):
+        from .modules.wavernn import wavernn_loss
+        self.bucket.zero()
+        x, y, m = self.corpus.cut(self.table)
+        self.loss = wavernn_loss(self.model(x, m), y, self.model.mode)
+        self.loss.backward()
+
+    def __call__(self, ids, offsets):
+        """Validates the (ids, offsets) table on the host (VocoderCorpus.table), reads the flags of earlier replays that have completed,
+        copies the table in and replays.  Returns the loss, a device tensor the next replay overwrites."""
+        table = self.corpus.table(ids, offsets)
+        if len(table) != self.batch_size:
+            raise ValueError(f'{len(table)} windows for a step captured at a batch of {self.batch_size}')
+        mode = _lib.get_precision()
+        if mode != self.precision:
+            raise ValueError(f'GraphedVocoderStep was captured in {self.precision} mode; the precision mode is now {mode}')
+        self.abort.poll()
+        self.table.copy_(torch.from_numpy(table).pin_memory(), non_blocking=True)
+        self.graph.replay()
+        self.replays += 1
+        self.abort.after_replay(self.replays)
+        return self.loss
+
+    def check(self):
+        """Waits for every replay's abort flag and raises B200TTSError if one is set."""
+        self.abort.wait()
+
+    def close(self):
+        self.check()

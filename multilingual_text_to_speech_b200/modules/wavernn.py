@@ -106,6 +106,101 @@ def vocoder_batch(mels, labels, offsets, mode, bits, seq_len, pad, hop):
     return x, y, m
 
 
+class VocoderCorpus:
+    """A WaveRNN training corpus packed into one GPU's memory once, from which each batch's windows are cut on the device in one launch
+    (b200tts_wavernn_cut_windows): `batch(ids, offsets)` returns vocoder_batch's (x, y, m) for the same utterances and offsets, bit for bit,
+    without host slicing or a host-to-device copy of the windows.
+
+    mels: host mels [feat, F_i]; labels: integer labels [N_i] (RAW labels of `bits` bits, or MOL's 16-bit labels), in [0, 2^16).  Device
+    footprint: 2 bytes per sample plus 4 feat bytes per frame; a corpus larger than one GPU's memory is the caller's to shard or subset.
+    The lengths stay on the host, so `batch` validates its table (ids, offsets, the utterances' labels) from host data alone and raises
+    ValueError before any device work; an utterance whose labels lie outside [0, 2^16) is stored as zeros and refused by `batch`."""
+
+    def __init__(self, mels, labels, mode, bits, seq_len, pad, hop, device):
+        if mode not in _lib.WAVERNN_MODES:
+            raise ValueError(f'unknown mode {mode!r}; expected RAW or MOL')
+        if len(mels) != len(labels) or len(mels) == 0:
+            raise ValueError(f'{len(mels)} mels and {len(labels)} label sequences: need as many of each, at least one')
+        if not 1 <= int(bits) <= 16:
+            raise ValueError(f'bits {bits} outside [1, 16]')
+        self.win = mel_window(seq_len, hop, pad)
+        if seq_len // hop > MAX_TRAIN_HOPS:
+            raise ValueError(f'seq_len {seq_len}: at most {MAX_TRAIN_HOPS} hops of {hop}')
+        self.mode, self.bits, self.seq_len, self.pad, self.hop = mode, int(bits), int(seq_len), int(pad), int(hop)
+        self.device = torch.device(device)
+        mels = [np.asarray(m, dtype=np.float32) for m in mels]
+        self.feat = mels[0].shape[0] if mels[0].ndim == 2 else -1
+        for i, m in enumerate(mels):
+            if m.ndim != 2 or m.shape[0] != self.feat or m.shape[1] < 1:
+                raise ValueError(f'mel {i} of shape {m.shape}: expected [{self.feat}, frames >= 1]')
+        packed, self.labels_ok = [], []
+        for i, lab in enumerate(labels):
+            lab = np.asarray(lab)
+            if lab.ndim != 1 or not (np.issubdtype(lab.dtype, np.integer) or lab.size == 0):
+                raise ValueError(f'labels {i} of shape {lab.shape} and dtype {lab.dtype}: expected one integer sequence')
+            ok = lab.size == 0 or (int(lab.min()) >= 0 and int(lab.max()) < 1 << 16)
+            self.labels_ok.append(ok)
+            packed.append(lab.astype(np.uint16) if ok else np.zeros(lab.shape, np.uint16))
+        self.frames = [m.shape[1] for m in mels]
+        self.samples = [p.shape[0] for p in packed]
+        self.frame_start = np.concatenate(([0], np.cumsum(self.frames)[:-1])).astype(np.int64)
+        self.sample_start = np.concatenate(([0], np.cumsum(self.samples)[:-1])).astype(np.int64)
+        dev = self.device
+        self.mels = torch.from_numpy(np.concatenate(mels, axis=1)).to(dev)
+        # uint16 labels held in an int16 tensor (the kernel reads the bits as uint16)
+        self.labels = torch.from_numpy(np.concatenate(packed).view(np.int16)).to(dev)
+        self.frame_start_dev = torch.from_numpy(self.frame_start).to(dev)
+        self.sample_start_dev = torch.from_numpy(self.sample_start).to(dev)
+
+    def __len__(self):
+        return len(self.frames)
+
+    @property
+    def nbytes(self):
+        return 2 * sum(self.samples) + 4 * self.feat * sum(self.frames)
+
+    def _check_ids(self, ids):
+        for i, u in enumerate(ids):
+            if not 0 <= int(u) < len(self.frames):
+                raise ValueError(f'utterance id {u} of item {i} outside [0, {len(self.frames)})')
+
+    def draw_offsets(self, ids, rng=None):
+        """draw_offsets for the utterances `ids`: the same draws from the same numpy generator."""
+        self._check_ids(ids)
+        return draw_offsets([self.frames[int(u)] for u in ids], self.seq_len, self.hop, self.pad, rng)
+
+    def table(self, ids, offsets):
+        """The host table int32 [B, 2] of (utterance, mel offset), validated as vocoder_batch validates its windows: ValueError for B outside
+        1 to 64, an id out of range, a window outside its utterance's mel or labels, or an utterance whose labels lie outside [0, 2^16)."""
+        ids, offsets = list(ids), list(offsets)
+        if len(ids) != len(offsets) or len(ids) == 0:
+            raise ValueError(f'{len(ids)} utterance ids and {len(offsets)} offsets: need as many of each, at least one')
+        if len(ids) > MAX_TRAIN_BATCH:
+            raise ValueError(f'a batch of {len(ids)} windows: need 1 to {MAX_TRAIN_BATCH}')
+        self._check_ids(ids)
+        for i, (u, o) in enumerate(zip(ids, offsets)):
+            u, o = int(u), int(o)
+            if o < 0 or o + self.win > self.frames[u] or (o + self.pad) * self.hop + self.seq_len + 1 > self.samples[u]:
+                raise ValueError(f'offset {o} of item {i} leaves its window outside the mel ({self.frames[u]} frames) or the labels '
+                                 f'({self.samples[u]})')
+            if not self.labels_ok[u]:
+                raise ValueError(f'labels of utterance {u} (item {i}) lie outside [0, 65536)')
+        return np.array([[int(u), int(o)] for u, o in zip(ids, offsets)], dtype=np.int32)
+
+    def cut(self, table, out=None):
+        """(x, y, m) of the device table int32 [B, 2], which is not checked (see `table`); written into `out` when given."""
+        return F.wavernn_cut_windows(self.mode, self.bits, self.seq_len, self.pad, self.hop, self.mels, self.frame_start_dev, self.labels,
+                                     self.sample_start_dev, table, out)
+
+    def batch(self, ids, offsets):
+        """vocoder_batch(mels[ids], labels[ids], offsets, ...) on the device: (x [B, seq_len] fp32, y [B, seq_len] (RAW int64, MOL fp32),
+        m [B, feat, mel_win] fp32).  The table is validated on the host, then copied in with one pinned host-to-device copy."""
+        host = torch.from_numpy(self.table(ids, offsets))
+        if self.device.type == 'cuda':
+            host = host.pin_memory()
+        return self.cut(host.to(self.device, non_blocking=True))
+
+
 def wavernn_loss(logits, y, mode):
     """fatchord's training loss of forward's logits [B, T, n_classes] against y [B, T]: RAW F.cross_entropy against the labels, MOL
     discretized_mix_logistic_loss (65536 classes, log scales clamped at log 1e-14); the mean over B T, with autograd."""
@@ -220,8 +315,11 @@ class WaveRNN(nn.Module):
                              f'{MAX_TRAIN_HOPS} hops')
         if tuple(mels.shape) != (B, self.feat_dims, T // hop + 2 * p):
             raise ValueError(f'mels of shape {tuple(mels.shape)}; expected {(B, self.feat_dims, T // hop + 2 * p)}')
+        # under CUDA-graph capture no flag is read (a read synchronises): the loops' guard goes to `_graph_guard`, whose flag the captured
+        # step (graph.GraphedVocoderStep) reads after each replay
+        capturing = dev.type == 'cuda' and torch.cuda.is_current_stream_capturing()
         pending = getattr(self, '_pending_guard', None)
-        if pending is not None and not pending.checked:
+        if pending is not None and not pending.checked and not capturing:
             pending.check()          # the previous call's loops were never followed by a backward: read their abort flag now
         self._pending_guard = None
         self.step += 1
@@ -235,10 +333,13 @@ class WaveRNN(nn.Module):
         # backward), or after GRU2's forward loop when no backward follows
         guard = F.GRUSeqGuard(F.gru_seq_shape(B, T, self.rnn_dims), dev)
         grads = torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())
-        x2 = x1 + F.gru_seq(x1, r1.weight_ih_l0, r1.weight_hh_l0, r1.bias_ih_l0, r1.bias_hh_l0, tr('rnn1'), guard, False, grads)
+        x2 = x1 + F.gru_seq(x1, r1.weight_ih_l0, r1.weight_hh_l0, r1.bias_ih_l0, r1.bias_hh_l0, tr('rnn1'), guard, False,
+                            grads and not capturing)
         x3 = x2 + F.gru_seq(torch.cat([x2, a2], dim=2), r2.weight_ih_l0, r2.weight_hh_l0, r2.bias_ih_l0, r2.bias_hh_l0, tr('rnn2'), guard,
-                            not grads, False)
-        if grads:
+                            not grads and not capturing, False)
+        if capturing:
+            self._graph_guard = guard
+        elif grads:
             self._pending_guard = guard
         y1 = torch.relu(F.linear(torch.cat([x3, a3], dim=2), self.fc1.weight, self.fc1.bias))
         y2 = torch.relu(F.linear(torch.cat([y1, a4], dim=2), self.fc2.weight, self.fc2.bias))
