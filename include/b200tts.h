@@ -594,22 +594,20 @@ typedef struct {
     int mel_len;
     int a0, aux_len;      /* the aux window holds frames [a0, a0 + aux_len) */
 } b200tts_wavernn_window_shape;
-/* feat [nsteps, n_mels + aux_dims] for the sample positions [s0, s0 + nsteps) of one unfolded row (one utterance, no folds): the columns
- * b200tts_wavernn_fold writes for these positions, with the same arithmetic, read from windows: mel_win [n_mels, mel_len] holds the
- * penultimate layer's samples [m0, m0 + mel_len) (equal to the whole padded mel's wherever they are read), aux_win [aux_len, aux_dims] the
- * MelResNet output's frames [a0, a0 + aux_len).  B200TTS_ERR_INVALID when a read would fall outside a window. */
-int b200tts_wavernn_window(const b200tts_wavernn_window_shape* shape, const float* mel_win, const float* fir, const float* aux_win, long long s0,
-                           int nsteps, float* feat, void* stream);
 /* Rows of one call of b200tts_wavernn_window_rows and segments of b200tts_wavernn_upsample_segments: at most this many. */
 #define B200TTS_WAVERNN_MAX_STREAMS 64
 typedef struct {
-    b200tts_wavernn_window_shape w;   /* the row's window, as for b200tts_wavernn_window; n_mels, aux_dims, hop, pad, scale equal in every row */
+    b200tts_wavernn_window_shape w;   /* the row's windows; n_mels, aux_dims, hop, pad, scale equal in every row */
     long long s0;                     /* the row's first position (its steps run so far) */
     long long mel_off, aux_off;       /* element offsets of the row's mel and aux windows in the packed buffers */
     int n;                            /* positions [s0, s0 + n), 0 to nsteps */
 } b200tts_wavernn_window_row;
-/* b200tts_wavernn_window for active_rows rows in one launch: feat [nsteps, active_rows, n_mels + aux_dims], row r's step i the features of
- * position rows[r].s0 + i for i < rows[r].n, zero past it.  rows: host descriptors, each checked as b200tts_wavernn_window checks its shape. */
+/* feat [nsteps, active_rows, n_mels + aux_dims] of active_rows unfolded rows (one utterance each, no folds) in one launch: row r's step i
+ * holds the features of sample position q = rows[r].s0 + i for i < rows[r].n, zero past it.  They are the columns b200tts_wavernn_fold
+ * writes for q, with the same arithmetic (zero for q >= F hop once F = w.frames is known), read from the row's windows: mel + mel_off
+ * [n_mels, mel_len] holds the penultimate layer's samples [m0, m0 + mel_len) (equal to the whole padded mel's wherever they are read),
+ * aux + aux_off [aux_len, aux_dims] the MelResNet output's frames [a0, a0 + aux_len).  rows: host descriptors.  B200TTS_ERR_INVALID when a
+ * read of a row with n > 0 would fall outside its windows. */
 int b200tts_wavernn_window_rows(const b200tts_wavernn_window_row* rows, int active_rows, int nsteps, const float* mel, const float* fir,
                                 const float* aux, float* feat, void* stream);
 /* b200tts_wavernn_upsample_layer over nseg packed segments (1 to B200TTS_WAVERNN_MAX_STREAMS): segment g is in [C, lens[g]] right after

@@ -230,7 +230,6 @@ SIGNATURES = {
     'b200tts_mel_cepstral_distortion': (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'b200tts_wavernn_upsample_layer': (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     'b200tts_wavernn_fold': (c_int, [POINTER(WaveRNNFoldShape)] + [c_void_p] * 7 + [c_int, c_int, c_void_p, c_void_p]),
-    'b200tts_wavernn_window': (c_int, [POINTER(WaveRNNWindowShape), c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_void_p, c_void_p]),
     'b200tts_wavernn_workspace_bytes': (c_size_t, [POINTER(WaveRNNShape)]),
     'b200tts_wavernn_prepare': (c_int, [POINTER(WaveRNNShape), POINTER(WaveRNNParams), c_void_p, c_size_t, c_void_p]),
     'b200tts_wavernn_run': (c_int, [POINTER(WaveRNNShape), POINTER(WaveRNNParams), POINTER(WaveRNNCond), c_int, c_int, c_void_p, c_void_p,

@@ -242,8 +242,6 @@ int wavernn_fold_check(const b200tts_wavernn_fold_shape& s, int t0, int nsteps);
 int wavernn_fold_impl(const b200tts_wavernn_fold_shape& s, const float* mel_up, const long long* mel_off, const int* frames, const int* row_utt,
                       const int* row_fold, const float* fir, const float* aux, int t0, int nsteps, float* feat, cudaStream_t st);
 int wavernn_window_check(const b200tts_wavernn_window_shape& s, long long s0, int nsteps);
-int wavernn_window_impl(const b200tts_wavernn_window_shape& s, const float* mel_up, const float* fir, const float* aux, long long s0, int nsteps,
-                        float* feat, cudaStream_t st);
 int wavernn_run_stream_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, const b200tts_wavernn_cond& cond, long long t,
                             int nsteps, const float* uniforms, float* out, void* ws, size_t ws_bytes, cudaStream_t st);
 size_t wavernn_workspace_bytes(const b200tts_wavernn_shape& s);
@@ -830,14 +828,6 @@ int b200tts_wavernn_fold(const b200tts_wavernn_fold_shape* shape, const float* m
     B200_TRY(require_device());
     return wavernn_fold_impl(*shape, mel_up, reinterpret_cast<const long long*>(mel_off), frames, row_utt, row_fold, fir, aux, t0, nsteps, feat,
                              (cudaStream_t)stream);
-}
-int b200tts_wavernn_window(const b200tts_wavernn_window_shape* shape, const float* mel_win, const float* fir, const float* aux_win, long long s0,
-                           int nsteps, float* feat, void* stream) {
-    B200_REQUIRE(shape && mel_win && fir && feat, "wavernn_window: null argument");
-    B200_REQUIRE(aux_win || shape->aux_dims == 0, "wavernn_window: null aux");
-    B200_TRY(wavernn_window_check(*shape, s0, nsteps));
-    B200_TRY(require_device());
-    return wavernn_window_impl(*shape, mel_win, fir, aux_win, s0, nsteps, feat, (cudaStream_t)stream);
 }
 size_t b200tts_wavernn_workspace_bytes(const b200tts_wavernn_shape* shape) {
     if (!shape) { set_last_error("wavernn_workspace_bytes: null shape"); return 0; }

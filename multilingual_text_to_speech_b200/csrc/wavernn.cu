@@ -5,8 +5,8 @@
 //   * wavernn_fold_kernel: the last layer of the mel path evaluated at the positions a chunk of the sample loop needs, the `indent` cut, the
 //     nearest stretch of the MelResNet output (aux) and fold_with_overlap, as the [steps, rows, n_mels + aux_dims] rows of the conditioning
 //     GEMMs (the products that do not depend on the previous sample run in the library GEMM before the loop);
-//   * wavernn_window_kernel: the same rows for consecutive sample positions of one unfolded row, read from windows of the penultimate mel
-//     layer and of aux (streaming generation, where the mel arrives in chunks);
+//   * wavernn_window_rows_kernel: the same rows for consecutive sample positions of unfolded rows, each read from its own windows of the
+//     penultimate mel layer and of aux (streaming generation, where the mel arrives in chunks);
 //   * wavernn_loop_kernel: the persistent sample loop, one cooperative launch per chunk of steps (below);
 //   * wavernn_unfold_kernel: mu-law decode, the square-root cross-fades, overlap-add, the cut to (F - 1) hop samples and the linear fade-out.
 //
@@ -119,38 +119,10 @@ __global__ void wavernn_fold_kernel(b200tts_wavernn_fold_shape s, const float* _
     }
 }
 
-// feat[i, :] for the sample positions q = s0 + i of one unfolded row (zero for q >= F hop once F is known): wavernn_fold_kernel's arithmetic,
-// with the penultimate layer read from a window x [n_mels, mel_len] that holds its samples [m0, m0 + mel_len), and aux from a window
-// [aux_len, aux_dims] that holds frames [a0, a0 + aux_len).  lo bounds the whole last layer ((F + 2 pad) hop, or past every read while F
-// is unknown); the host checks that every read falls inside the windows.
-__global__ void wavernn_window_kernel(b200tts_wavernn_window_shape s, long long lo, const float* __restrict__ x, const float* __restrict__ fir,
-                                      const float* __restrict__ aux, long long s0, int nsteps, float* __restrict__ feat) {
-    const int D = s.n_mels + s.aux_dims;
-    const long long n = (long long)nsteps * D;
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < n; idx += (long long)gridDim.x * blockDim.x) {
-        const int col = (int)(idx % D);
-        const long long q = s0 + idx / D;
-        float v = 0.f;
-        if (s.frames == 0 || q < (long long)s.frames * s.hop) {
-            if (col < s.n_mels) {
-                const float* xc = x + (size_t)col * s.mel_len;
-                const long long p = q + (long long)s.pad * s.hop;
-                float acc = 0.f;
-                for (int k = -s.scale; k <= s.scale; ++k) {
-                    const long long j = p + k;
-                    if (j >= 0 && j < lo) acc = fmaf(fir[k + s.scale], xc[j / s.scale - s.m0], acc);
-                }
-                v = acc;
-            } else {
-                v = aux[(size_t)(q / s.hop - s.a0) * s.aux_dims + (col - s.n_mels)];
-            }
-        }
-        feat[idx] = v;
-    }
-}
-
-// wavernn_window_kernel for many rows: row r's positions are [s0, s0 + n) (zero for steps i >= n), its windows at mel + mel_off and
-// aux + aux_off.  feat [nsteps, rows, n_mels + aux_dims].
+// feat[i, r, :] for the sample positions q = s0 + i (i < n, zero past it) of unfolded row r (zero for q >= F hop once F is known):
+// wavernn_fold_kernel's arithmetic, with the penultimate layer read from the row's window mel + mel_off [n_mels, mel_len] that holds its
+// samples [m0, m0 + mel_len), and aux from its window aux + aux_off [aux_len, aux_dims] that holds frames [a0, a0 + aux_len).  lo bounds the
+// whole last layer ((F + 2 pad) hop, or past every read while F is unknown); the host checks that every read falls inside the windows.
 struct WrWinRow { long long s0, m0, lo, mel_off, aux_off; int n, frames, mel_len, a0; };
 struct WrWinRows { WrWinRow r[B200TTS_WAVERNN_MAX_STREAMS]; };
 __global__ void wavernn_window_rows_kernel(int n_mels, int aux_dims, int hop, int pad, int scale, int rows, const __grid_constant__ WrWinRows w,
@@ -847,11 +819,11 @@ int wavernn_fold_impl(const b200tts_wavernn_fold_shape& s, const float* mel_up, 
 // every read of the positions [s0, s0 + nsteps) must fall inside the windows
 int wavernn_window_check(const b200tts_wavernn_window_shape& s, long long s0, int nsteps) {
     B200_REQUIRE(s.n_mels >= 1 && s.aux_dims >= 0 && s.frames >= 0 && s.mel_len >= 1 && s.aux_len >= 0 && s.m0 >= 0 && s.a0 >= 0,
-                 "wavernn_window: bad dimensions (n_mels = %d, aux_dims = %d, frames = %d, mel_len = %d, aux_len = %d, m0 = %lld, a0 = %d)",
+                 "wavernn_window_rows: bad dimensions (n_mels = %d, aux_dims = %d, frames = %d, mel_len = %d, aux_len = %d, m0 = %lld, a0 = %d)",
                  s.n_mels, s.aux_dims, s.frames, s.mel_len, s.aux_len, s.m0, s.a0);
     B200_REQUIRE(s.hop >= 1 && s.scale >= 1 && s.hop % s.scale == 0 && s.pad >= 0,
-                 "wavernn_window: the hop %d must be a multiple of the last upsampling factor %d (pad %d)", s.hop, s.scale, s.pad);
-    B200_REQUIRE(s0 >= 0 && nsteps >= 1, "wavernn_window: positions [%lld, %lld)", s0, s0 + nsteps);
+                 "wavernn_window_rows: the hop %d must be a multiple of the last upsampling factor %d (pad %d)", s.hop, s.scale, s.pad);
+    B200_REQUIRE(s0 >= 0 && nsteps >= 1, "wavernn_window_rows: positions [%lld, %lld)", s0, s0 + nsteps);
     long long q1 = s0 + nsteps;                          // positions [s0, q1) read the windows
     if (s.frames > 0 && q1 > (long long)s.frames * s.hop) q1 = (long long)s.frames * s.hop;
     if (q1 <= s0) return B200TTS_OK;
@@ -860,21 +832,11 @@ int wavernn_window_check(const b200tts_wavernn_window_shape& s, long long s0, in
     if (j0 < 0) j0 = 0;
     if (j1 > lo - 1) j1 = lo - 1;
     B200_REQUIRE(j0 / s.scale >= s.m0 && j1 / s.scale < s.m0 + s.mel_len,
-                 "wavernn_window: positions [%lld, %lld) read penultimate samples [%lld, %lld], outside the window [%lld, %lld)", s0, q1,
+                 "wavernn_window_rows: positions [%lld, %lld) read penultimate samples [%lld, %lld], outside the window [%lld, %lld)", s0, q1,
                  j0 / s.scale, j1 / s.scale, s.m0, s.m0 + s.mel_len);
     B200_REQUIRE(s.aux_dims == 0 || (s0 / s.hop >= s.a0 && (q1 - 1) / s.hop < (long long)s.a0 + s.aux_len),
-                 "wavernn_window: positions [%lld, %lld) read aux frames [%lld, %lld], outside the window [%d, %d)", s0, q1, s0 / s.hop,
+                 "wavernn_window_rows: positions [%lld, %lld) read aux frames [%lld, %lld], outside the window [%d, %d)", s0, q1, s0 / s.hop,
                  (q1 - 1) / s.hop, s.a0, s.a0 + s.aux_len);
-    return B200TTS_OK;
-}
-
-int wavernn_window_impl(const b200tts_wavernn_window_shape& s, const float* mel_up, const float* fir, const float* aux, long long s0, int nsteps,
-                        float* feat, cudaStream_t st) {
-    B200_TRY(wavernn_window_check(s, s0, nsteps));
-    KernelTimer kt("wavernn_window", st);
-    const long long lo = s.frames > 0 ? (long long)(s.frames + 2 * s.pad) * s.hop : LLONG_MAX;
-    wavernn_window_kernel<<<grid_for((size_t)nsteps * (s.n_mels + s.aux_dims)), 256, 0, st>>>(s, lo, mel_up, fir, aux, s0, nsteps, feat);
-    B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }
 
@@ -904,7 +866,7 @@ int wavernn_window_rows_impl(const b200tts_wavernn_window_row* rows, int active_
         w.r[r] = WrWinRow{d.s0, d.w.m0, d.w.frames > 0 ? (long long)(d.w.frames + 2 * d.w.pad) * d.w.hop : LLONG_MAX, d.mel_off, d.aux_off, d.n,
                           d.w.frames, d.w.mel_len, d.w.a0};
     }
-    KernelTimer kt("wavernn_window", st);
+    KernelTimer kt("wavernn_window_rows", st);
     wavernn_window_rows_kernel<<<grid_for((size_t)nsteps * active_rows * (w0.n_mels + w0.aux_dims)), 256, 0, st>>>(
         w0.n_mels, w0.aux_dims, w0.hop, w0.pad, w0.scale, active_rows, w, mel, fir, aux, nsteps, feat);
     B200_LAUNCH_CHECK();

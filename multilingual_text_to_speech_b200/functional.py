@@ -966,17 +966,6 @@ def wavernn_fold(shape, mel_up, mel_off, frames, row_utt, row_fold, fir, aux, t0
     return out
 
 
-def wavernn_window(shape, mel_win, fir, aux_win, s0, nsteps):
-    """feat [nsteps, n_mels + aux_dims] of the sample positions [s0, s0 + nsteps) of one unfolded row, from the windows (shape: a
-    _lib.WaveRNNWindowShape)."""
-    _require_cuda(mel_win, fir, aux_win)
-    mel_win, aux_win = _f32c(mel_win), _f32c(aux_win)
-    out = torch.empty(int(nsteps), shape.n_mels + shape.aux_dims, device=mel_win.device, dtype=torch.float32)
-    check(_lib.load().b200tts_wavernn_window(ctypes.byref(shape), ptr(mel_win), ptr(_f32c(fir)), ptr(aux_win), int(s0), int(nsteps), ptr(out),
-                                             _stream()), 'b200tts_wavernn_window')
-    return out
-
-
 def wavernn_upsample_segments(x, lens, fir, scale):
     """wavernn_upsample_layer over packed segments: x holds [C, lens[g]] for each g one after another (flat) -> the same packing of
     [C, lens[g] scale], each segment equal to its own wavernn_upsample_layer."""

@@ -421,41 +421,19 @@ class WaveRNN(nn.Module):
         final once lookahead() frames follow its frame, so the loop runs up to there after each input chunk; the last 20 hops it has run are
         held back until the input ends, because the fade-out lands on them.  uniforms: the tape [1, T, U] of generate (step t reads
         uniforms[0, t]; T >= (F - 1) hop), by default drawn with torch.rand per call of the loop (`generator` optional).  preemphasis as in
-        generate_batch, de-emphasised sequentially across chunks: within fp32 roundings of the one-shot call, not bit for bit.  Runs on the
-        device of the first CUDA chunk, or the current CUDA device, in fp32 (the precision mode is set for each stretch of work and restored
-        before every yield).  Chunks come out as the first chunk went in: numpy, CUDA tensors, or CPU tensors.
+        generate_batch, de-emphasised sequentially across chunks: within fp32 roundings of the one-shot call, not bit for bit.  Runs through
+        a one-stream StreamPool on the device of the first CUDA chunk, or the current CUDA device, in fp32 (the precision mode is set for
+        each stretch of work and restored before every yield).  Chunks come out as the first chunk went in: numpy, CUDA tensors, or CPU
+        tensors.
 
         With target and overlap: the streaming form of generate(mel, target, overlap), fatchord's folded generation, through a one-stream
         FoldedStreamPool (its folds run as rows of one loop): the chunks concatenate to that call's samples bit for bit given the same tape
         uniforms [folds, target + 2 overlap, U] (fold k step j reads uniforms[k, j]); preemphasis de-emphasises each fold from a zero state,
         within generate_batch's bound."""
-        if target is not None or overlap is not None:
-            yield from self._generate_stream_folded(mel_chunks, uniforms, generator, preemphasis, target, overlap)
-            return
-        if not -1.0 < float(preemphasis) < 1.0:
-            raise ValueError(f'preemphasis {preemphasis} must lie in (-1, 1)')
-        tape = self._check_stream_tape(uniforms)
-        st = None
-        for i, chunk in enumerate(mel_chunks):
-            spec, as_numpy = self._check_chunk(chunk, i)
-            if st is None:
-                st = _Stream(self, spec.device if spec.is_cuda else None, as_numpy, not as_numpy and spec.is_cuda, tape, generator, preemphasis)
-            if spec.shape[1]:
-                out = st.feed(spec)
-                if out is not None:
-                    yield out
-        if st is None or st.frames < 21:
-            raise ValueError(f'the mel stream ended after {0 if st is None else st.frames} frames; the 20-hop fade-out needs at least 21')
-        yield st.finish()
-
-    def stream_pool(self, max_streams, preemphasis=0.0, generator=None, target=None, overlap=None):
-        """A StreamPool of up to max_streams (1 to 64) concurrent generate_stream-like streams sharing one sample loop; with target and
-        overlap, a FoldedStreamPool of up to max_streams folded streams on the loop's 64 rows."""
         if target is None and overlap is None:
-            return StreamPool(self, max_streams, preemphasis, generator)
-        return FoldedStreamPool(self, max_streams, target, overlap, preemphasis, generator)
-
-    def _generate_stream_folded(self, mel_chunks, uniforms, generator, preemphasis, target, overlap):
+            if not -1.0 < float(preemphasis) < 1.0:
+                raise ValueError(f'preemphasis {preemphasis} must lie in (-1, 1)')
+            uniforms = self._check_stream_tape(uniforms)
         pool = sid = fmt = None
         for i, chunk in enumerate(mel_chunks):
             spec, as_numpy = self._check_chunk(chunk, i)
@@ -464,7 +442,7 @@ class WaveRNN(nn.Module):
                                                            else torch.device('cuda'))
                 fmt = (as_numpy, not as_numpy and spec.is_cuda)
                 with torch.cuda.device(device):
-                    pool = FoldedStreamPool(self, 1, target, overlap, preemphasis, generator)
+                    pool = self.stream_pool(1, preemphasis, generator, target, overlap)
                 sid = pool.open(uniforms)
             if spec.shape[1]:
                 pool.feed(sid, spec)
@@ -476,6 +454,13 @@ class WaveRNN(nn.Module):
         pool.end(sid)
         for w in pool.drain():
             yield _as_input(w[sid], *fmt)
+
+    def stream_pool(self, max_streams, preemphasis=0.0, generator=None, target=None, overlap=None):
+        """A StreamPool of up to max_streams (1 to 64) concurrent generate_stream-like streams sharing one sample loop; with target and
+        overlap, a FoldedStreamPool of up to max_streams folded streams on the loop's 64 rows."""
+        if target is None and overlap is None:
+            return StreamPool(self, max_streams, preemphasis, generator)
+        return FoldedStreamPool(self, max_streams, target, overlap, preemphasis, generator)
 
     def lookahead(self):
         """Frames past a sample's own frame that its loop features read: `pad` for conv_in (the rest of the MelResNet is pointwise) or the
@@ -507,22 +492,6 @@ class WaveRNN(nn.Module):
         elif P1 - p > known or r1 > known:
             raise ValueError(f'positions [{s0}, {s1}) read mel frames past the {known} that have arrived')
         return (P0, P1), (r0, r1), (a0, a1)
-
-    def window_features(self, mel, s0, s1, final):
-        """Loop features [s1 - s0, feat_dims + res_out_dims] of sample positions [s0, s1) from the mel frames that have arrived, mel
-        [feat_dims, known] on the device (final: the whole mel): equal, bit for bit, to b200tts_wavernn_fold's at these positions."""
-        known, p, hop, s_last = int(mel.shape[1]), self.pad, self.hop_length, self.upsample_factors[-1]
-        (P0, P1), (r0, r1), _ = self.window_plan(s0, s1, known, final)
-        device = mel.device
-        win = torch.zeros(self.feat_dims, P1 - P0, device=device, dtype=torch.float32)
-        lo, hi = max(P0, p), min(P1, known + p)
-        win[:, lo - P0:hi - P0] = mel[:, lo - p:hi - p]
-        mel_up = self._mel_path(win, device)
-        aux = self._resnet(mel[:, r0:r1].unsqueeze(0).contiguous(), [r1 - r0], device)[0]
-        shape = _lib.WaveRNNWindowShape(self.feat_dims, aux.shape[1], hop, p, s_last, known if final else 0, P0 * (hop // s_last),
-                                        mel_up.shape[1], r0, r1 - r0)
-        fir = self.upsample.up_layers[-1].weight.detach().reshape(-1).to(device=device, dtype=torch.float32).contiguous()
-        return F.wavernn_window(shape, mel_up, fir, aux, s0, s1 - s0)
 
     def _check_chunk(self, chunk, i):
         as_numpy = not isinstance(chunk, torch.Tensor)
@@ -736,102 +705,6 @@ def _as_input(wave, as_numpy, on_cuda):
     return wave if on_cuda else wave.cpu()
 
 
-class _Stream:
-    """The state of one generate_stream: the mel frames that have arrived, the loop workspace carried across calls, and the samples the
-    loop has run but not yet released (raw loop outputs, or de-emphasised ones with preemphasis)."""
-
-    def __init__(self, model, device, as_numpy, on_cuda, tape, generator, preemphasis):
-        if device is None:
-            device = torch.device('cuda', torch.cuda.current_device()) if torch.cuda.is_available() else torch.device('cuda')
-        self.m, self.device, self.as_numpy, self.on_cuda = model, device, as_numpy, on_cuda
-        self.tape, self.generator, self.a = tape, generator, float(preemphasis)
-        self.hop, self.lookahead = model.hop_length, model.lookahead()
-        self.mu = model.n_classes - 1 if model.mode == 'RAW' else 0
-        self.mel = torch.zeros(model.feat_dims, 0, device=device, dtype=torch.float32)
-        self.steps = 0                 # loop steps run
-        self.released = 0              # samples yielded
-        self.pending = torch.zeros(0, device=device, dtype=torch.float32)       # samples [released, steps)
-        self.last = torch.zeros(1, device=device, dtype=torch.float32)          # the last de-emphasised sample
-        with self._fp32():
-            self.w = model.loop_weights(device)
-            self.S = model.chunk_steps(1, 1 << 30)
-            self.shape = _lib.WaveRNNShape(1, model.rnn_dims, model.fc_dims, model.n_classes, _lib.WAVERNN_MODES[model.mode], self.S)
-            self.ws = F.wavernn_workspace(self.shape, device)
-            self.params = F.wavernn_params(self.w)
-            F.wavernn_prepare(self.shape, self.params, self.ws)
-
-    @property
-    def frames(self):
-        return int(self.mel.shape[1])
-
-    @contextlib.contextmanager
-    def _fp32(self):
-        precision = _lib.get_precision()
-        try:
-            _lib.set_precision('fp32')
-            with torch.cuda.device(self.device), torch.no_grad():
-                yield
-        finally:
-            _lib.set_precision(precision)
-
-    def feed(self, spec):
-        """Takes one non-empty chunk; returns the samples it releases, or None."""
-        with self._fp32():
-            self.mel = torch.cat([self.mel, spec.to(device=self.device, dtype=torch.float32)], dim=1)
-            ready = min(self.frames - self.lookahead, self.frames - 1) * self.hop      # samples whose features are final
-            self._run(ready, False)
-            n = (self.steps - 20 * self.hop) - self.released                          # the last 20 hops wait for the fade-out
-            if n <= 0:
-                return None
-            # an unfold that ends 20 hops past the samples it writes applies no fade
-            wave = self._unfold(n, n // self.hop + 21)
-        return self._out(wave)
-
-    def finish(self):
-        with self._fp32():
-            F_ = self.frames
-            self._run((F_ - 1) * self.hop, True)
-            wave = self._unfold((F_ - 1) * self.hop - self.released, F_ - self.released // self.hop)
-        return self._out(wave)
-
-    def _run(self, end, final):
-        m, U = self.m, self.m.uniforms_per_step()
-        while self.steps < end:
-            t, n = self.steps, min(self.S, end - self.steps)
-            if self.tape is not None:
-                if self.tape.shape[1] < t + n:
-                    raise ValueError(f'the uniform tape holds {self.tape.shape[1]} steps; the stream needs at least {t + n}')
-                uni = self.tape[:, t:t + n].to(device=self.device, dtype=torch.float32).contiguous()
-            else:
-                uni = torch.rand(1, n, U, device=self.device, dtype=torch.float32, generator=self.generator)
-            feat = m.window_features(self.mel, t, t + n, final)
-            cond = m.conditioning(self.w, feat.unsqueeze(1))
-            y = torch.empty(1, n, device=self.device, dtype=torch.float32)
-            F.wavernn_run_stream(self.shape, self.params, cond, t, n, uni, y, self.ws)
-            if self.a:
-                if self.mu:
-                    y = F.wavernn_deemphasis(y, self.mu, 0.0)                    # a = 0: the mu-law decode only
-                y = F.wavernn_deemphasis(torch.cat([self.last, y[0]]).reshape(1, -1), 0, self.a)[:, 1:]
-                self.last = y[0, -1:].clone()
-            self.pending = torch.cat([self.pending, y[0]])
-            self.steps += n
-
-    def _unfold(self, n, frames):
-        """The next n pending samples through b200tts_wavernn_unfold as one fold of an utterance of `frames` frames: decoded (RAW,
-        without preemphasis) and faded out over the last 20 hops of (frames - 1) hop samples."""
-        y, self.pending = self.pending[:n].reshape(1, n).contiguous(), self.pending[n:]
-        self.released += n
-        d = lambda a: torch.tensor(a, device=self.device)
-        return F.wavernn_unfold(y, d([frames]).int(), d([0, 1]).int(), d([0, n]).long(), n, self.hop, n, 0, 0 if self.a else self.mu)
-
-    def _out(self, wave):
-        if F.wavernn_aborted(self.shape, self.ws):
-            raise _lib.B200TTSError('wavernn: the sample loop timed out at a grid barrier')
-        if self.as_numpy:
-            return wave.cpu().numpy()
-        return wave if self.on_cuda else wave.cpu()
-
-
 class _PoolStream:
     """One stream of a StreamPool: its loop row, the mel frames that have arrived, its uniform tape (fp32 on the device, or None), the steps
     run and the samples released.  Its run but unreleased samples [released, steps) sit in the pool's per-row ring buffer."""
@@ -851,11 +724,12 @@ class _PoolStream:
 
 class StreamPool:
     """Concurrent streaming generation: up to max_streams streams, each a generate_stream, advance together in one sample loop whose rows
-    run independently (b200tts_wavernn_run_rows).  open() takes the lowest free row and resets it; feed() and end() add a stream's mel
+    run independently (b200tts_wavernn_run_rows; a one-stream pool, whose loop has one row, runs b200tts_wavernn_run_stream, the loop
+    without per-row budgets, bit for bit the same).  open() takes the lowest free row and resets it; feed() and end() add a stream's mel
     frames and mark its end; run() makes one loop call over every stream with samples ready, under generate_stream's rule (lookahead()
-    frames after a sample's frame, the last 20 hops held back until end()), at most POOL_CALL_HOPS hops per call, and returns {sid: waveform
-    chunk} (CUDA tensors) for the streams that released samples.  A stream's row is freed when its final chunk is returned, or at once by
-    close().
+    frames after a sample's frame, the last 20 hops held back until end()), at most POOL_CALL_HOPS hops per call in a pool of more than one
+    stream, and returns {sid: waveform chunk} (CUDA tensors) for the streams that released samples.  A stream's row is freed when its final
+    chunk is returned, or at once by close().
 
     For each stream the concatenated chunks equal generate_stream of the same mel with the same uniform tape, bit for bit, whenever it
     joined, whatever else shares the loop and however its mel was chunked.  With preemphasis the stream is de-emphasised across calls and
@@ -881,7 +755,10 @@ class StreamPool:
         self.next_sid = 0
         with self._fp32():
             self.w = model.loop_weights(self.device)
-            self.S = min(POOL_CALL_HOPS * self.hop, model.chunk_steps(self.rows, 1 << 30))
+            # a lone stream runs all its ready steps in one call (up to COND_BYTES): each call costs 3 to 4 ms outside the loop, and no other
+            # stream waits on it
+            S = model.chunk_steps(self.rows, 1 << 30)
+            self.S = S if self.rows == 1 else min(POOL_CALL_HOPS * self.hop, S)
             self.shape = _lib.WaveRNNShape(self.rows, model.rnn_dims, model.fc_dims, model.n_classes, _lib.WAVERNN_MODES[model.mode], self.S)
             self.ws = F.wavernn_workspace(self.shape, self.device)
             self.params = F.wavernn_params(self.w)
@@ -1000,6 +877,20 @@ class StreamPool:
                 del self.streams[sid]
         return released
 
+    def drain(self):
+        """Runs until no stream has steps left to run -> the non-empty {sid: chunk} results, in order."""
+        out = []
+        while True:
+            busy = self._busy()
+            r = self.run()
+            if r:
+                out.append(r)
+            if not busy:
+                return out
+
+    def _busy(self):
+        return bool(self.plan())
+
     def _upload(self, a):
         return torch.from_numpy(np.ascontiguousarray(a)).to(self.device)
 
@@ -1030,8 +921,6 @@ class StreamPool:
         cond = m.conditioning(self.w, feat)
         slot = np.array([rows[k].slot for k in live], np.int64)
         n = np.array([plan[k][1] for k in live], np.int64)
-        row_t, row_n = np.zeros(active, np.int64), np.zeros(active, np.int32)
-        row_t[slot], row_n[slot] = [steps[k] for k in live], n
         # uniforms: the taped rows' steps gathered from their tapes (source 0 is a zero) and the seeded rows' from one seeded draw, in one
         # gather; the other rows' drawn for the call
         taped = [k for k in live if rows[k].tape is not None]
@@ -1063,7 +952,14 @@ class StreamPool:
             else:
                 uni = drawn
         y = torch.zeros(active, nmax, device=dev, dtype=torch.float32)
-        F.wavernn_run_rows(self.shape, self.params, cond, self._upload(row_t), self._upload(row_n), nmax, uni, y, self.ws)
+        if self.shape.rows == 1:
+            # a one-row loop: the loop without per-row budgets runs row 0 bit for bit as run_rows does (it runs every row of the shape,
+            # so it serves only a loop of one row)
+            F.wavernn_run_stream(self.shape, self.params, cond, steps[live[0]], nmax, uni, y, self.ws)
+        else:
+            row_t, row_n = np.zeros(active, np.int64), np.zeros(active, np.int32)
+            row_t[slot], row_n[slot] = [steps[k] for k in live], n
+            F.wavernn_run_rows(self.shape, self.params, cond, self._upload(row_t), self._upload(row_n), nmax, uni, y, self.ws)
         if self.a:
             if self.mu:
                 y = F.wavernn_deemphasis(y, self.mu, 0.0)                    # a = 0: the mu-law decode only
@@ -1349,16 +1245,8 @@ class FoldedStreamPool(StreamPool):
                 rel.append((sid, st.released, q1, st.frames if st.ended else 0))
         return rel
 
-    def drain(self):
-        """Runs until no fold has work left -> the non-empty {sid: chunk} results, in order."""
-        out = []
-        while True:
-            busy = bool(self.grants() or self.plan())
-            r = self.run()
-            if r:
-                out.append(r)
-            if not busy:
-                return out
+    def _busy(self):
+        return bool(self.grants() or self.plan())
 
     def run(self):
         """Grants rows, makes one loop call over every fold with steps to run and releases the final positions -> {sid: the waveform chunk

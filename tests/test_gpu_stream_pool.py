@@ -1,7 +1,8 @@
 """Concurrent streaming synthesis on the GPU, at the reference's vocoder dimensions:
   * b200tts_wavernn_run_rows: rows with mixed budgets (0 included) and parities each equal a solo b200tts_wavernn_run_stream bit for bit,
     a row idle for some calls continues as if uninterrupted, and a reset row reused by a new stream equals a fresh prepare;
-  * the packed upsampling layer and b200tts_wavernn_window_rows equal the per-stream window_features bit for bit;
+  * the packed upsampling layer equals the single layers, and the pool's windowed features (b200tts_wavernn_window_rows) equal
+    b200tts_wavernn_fold's over the whole mel bit for bit;
   * WaveRNN.stream_pool: every stream equals generate(mel, target=F hop, overlap=0) bit for bit under irregular chunkings, staggered opens,
     a freed and reused row and fewer active rows than the capacity; 64 streams at once against one generate_batch;
   * Tacotron.inference_streams against inference_batch and inference_stream; speech_streams against speech_stream;
@@ -114,27 +115,43 @@ def test_packed_upsampling_equals_single_layers():
     assert torch.equal(got, ref)
 
 
-def test_window_rows_equal_window_features():
+def _fold_features(m, mel):
+    """The whole mel's loop features [F hop, feat_dims + res_out_dims]: b200tts_wavernn_fold over the stage outputs of generate(mel,
+    target=F hop, overlap=0)."""
+    F_, hop = mel.shape[1], m.hop_length
+    trace = {}
+    m._generate([mel], [F_], None, F_ * hop, 0, None, torch.device('cuda'), trace)
+    fshape = _lib.WaveRNNFoldShape(1, 1, 80, 128, hop, 2, 11, F_ * hop, 0, F_)
+    d = lambda a: torch.from_numpy(np.asarray(a)).cuda()     # noqa: E731
+    fir = m.upsample.up_layers[-1].weight.detach().reshape(-1).float().contiguous().cuda()
+    return F.wavernn_fold(fshape, trace['mel_up'], d(trace['mel_off']), d(np.array([F_], np.int32)), d(np.zeros(1, np.int32)),
+                          d(np.zeros(1, np.int32)), fir, trace['aux'], 0, F_ * hop)[:, 0]
+
+
+def test_window_rows_equal_the_fold():
     _lib.set_precision('fp32')
     m = make_model('RAW', seed=44)
     hop = m.hop_length
     mels = [_mel(900, 45), _mel(40, 46), _mel(300, 47), _mel(25, 48)]
-    pool = m.stream_pool(6)
-    sids = [pool.open() for _ in mels]
-    # (known frames, final, first position, positions): stream starts, middle, the final frames; 1 to 300 positions, below and above a
-    # 64-column tile of the mel path
-    cases = [(900, False, 0, 300), (40, True, 17 * hop, 22 * hop - 5), (300, False, 100 * hop + 7, 40), (25, True, 23 * hop, hop)]
+    # (mel, known frames, final, first position, positions), one pool row each: stream starts, middles and final frames of four mels, then
+    # six windows of the 40-frame mel; 1 to 39 hops of positions, below and above a 64-column tile of the mel path
+    cases = [(0, 900, False, 0, 300), (1, 40, True, 17 * hop, 22 * hop - 5), (2, 300, False, 100 * hop + 7, 40), (3, 25, True, 23 * hop, hop)]
+    cases += [(1, known, final, s0, s1 - s0) for s0, s1, known, final in
+              [(0, 275, 3, False), (0, 37 * hop, 40, False), (3 * hop, 11 * hop, 13, False), (17 * hop, 39 * hop, 40, True),
+               (0, 39 * hop, 40, True), (38 * hop + 5, 39 * hop, 40, True)]]
     with torch.no_grad():
-        for sid, mel, (known, final, t, n) in zip(sids, mels, cases):
-            pool.feed(sid, mel[:, :known])
+        whole = [_fold_features(m, mel) for mel in mels]
+        pool = m.stream_pool(len(cases) + 2)
+        sids = [pool.open() for _ in cases]
+        for sid, (k, known, final, _, _) in zip(sids, cases):
+            pool.feed(sid, mels[k][:, :known])
             pool.streams[sid].ended = final
-        plan = {sid: (t, n) for sid, (_, _, t, n) in zip(sids, cases)}
+        plan = {sid: (t, n) for sid, (*_, t, n) in zip(sids, cases)}
         _lib.set_precision('fp32')
-        feat = pool._features(sids, plan, 4, max(n for _, n in plan.values()))
-        for b, (mel, (known, final, t, n)) in enumerate(zip(mels, cases)):
-            ref = m.window_features(mel[:, :known], t, t + n, final)
-            assert torch.equal(feat[:n, b], ref), b
-            assert bool((feat[n:, b] == 0).all())
+        feat = pool._features(sids, plan, len(cases), max(n for _, n in plan.values()))
+        for b, (k, known, final, t, n) in enumerate(cases):
+            assert torch.equal(feat[:n, b], whole[k][t:t + n]), b
+            assert bool((feat[n:, b] == 0).all()), b
 
 
 # ---- the pool ----

@@ -2,8 +2,8 @@
   * Tacotron.inference_stream on the reference's inference goldens: the stream's length equals inference()'s, its decoded frames equal
     inference()'s bit for bit, its post-net meets the golden tolerance and an fp32 bound against an fp64 post-net of the same frames, in
     both precision modes, at chunks of 7 and 128 frames and with r = 2; the first chunk comes after one decoder call;
-  * WaveRNN.generate_stream: the windowed features equal b200tts_wavernn_fold's bit for bit, and the stream equals generate(mel,
-    target=F hop, overlap=0) bit for bit over several chunkings in RAW and MOL, at 21 and 900 frames; with de-emphasis, within its bound;
+  * WaveRNN.generate_stream: the stream equals generate(mel, target=F hop, overlap=0) bit for bit over several chunkings in RAW and MOL,
+    at 21 and 900 frames; with de-emphasis, within its bound;
   * speech_stream equals generate of the concatenated streamed mel."""
 import json
 import os
@@ -173,25 +173,6 @@ def test_decoder_stream_outputs_per_step_2():
 # ---- vocoder ----
 def _mel(frames, seed):
     return torch.from_numpy(np.random.default_rng(seed).standard_normal((80, frames)).astype(np.float32)).cuda()
-
-
-def test_window_features_equal_the_fold():
-    _lib.set_precision('fp32')
-    m = make_model('RAW', seed=21)
-    mel = _mel(40, 22)
-    F_, hop = 40, 275
-    trace = {}
-    with torch.no_grad():
-        m._generate([mel], [F_], None, F_ * hop, 0, None, torch.device('cuda'), trace)
-        fshape = _lib.WaveRNNFoldShape(1, 1, 80, 128, hop, 2, 11, F_ * hop, 0, F_)
-        d = lambda a: torch.from_numpy(np.asarray(a)).cuda()     # noqa: E731
-        fir = m.upsample.up_layers[-1].weight.detach().reshape(-1).float().contiguous().cuda()
-        whole = F.wavernn_fold(fshape, trace['mel_up'], d(trace['mel_off']), d(np.array([F_], np.int32)), d(np.zeros(1, np.int32)),
-                               d(np.zeros(1, np.int32)), fir, trace['aux'], 0, F_ * hop)[:, 0]
-        for s0, s1, known, final in [(0, 275, 3, False), (0, 37 * hop, 40, False), (3 * hop, 11 * hop, 13, False), (17 * hop, 39 * hop, 40, True),
-                                     (0, 39 * hop, 40, True), (38 * hop + 5, 39 * hop, 40, True)]:
-            got = m.window_features(mel[:, :known], s0, s1, final)
-            assert torch.equal(got, whole[s0:s1]), (s0, s1, known, final)
 
 
 def _chunks(mel, sizes):

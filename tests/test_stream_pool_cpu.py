@@ -86,7 +86,7 @@ def test_abi_argument_checks_without_a_device():
     rows = (ctypes.c_int * 2)(1, 4)
     assert lib.b200tts_wavernn_reset_rows(ctypes.byref(shape), ws, nbytes, rows, 2, None) == -1
     assert b'row 4 outside [0, 4)' in lib.b200tts_last_error()
-    # window rows: each row checked as b200tts_wavernn_window checks its shape
+    # window rows: each row checked against its own windows
     good = _lib.WaveRNNWindowShape(80, 128, 275, 2, 11, 0, 0, 100, 0, 5)
     short = _lib.WaveRNNWindowShape(80, 128, 275, 2, 11, 0, 0, 60, 0, 5)
     other = _lib.WaveRNNWindowShape(80, 64, 275, 2, 11, 0, 0, 100, 0, 5)
@@ -97,7 +97,7 @@ def test_abi_argument_checks_without_a_device():
     # a row that runs no steps is not checked against its window: the call passes the checks and stops only for want of a device
     rows_ok = W(_lib.WaveRNNWindowRow(good, 0, 0, 0, 275), _lib.WaveRNNWindowRow(short, 0, 0, 0, 0))
     lib.b200tts_wavernn_window_rows(rows_ok, 2, 275, one, one, one, one, None)
-    assert b'wavernn_window' not in lib.b200tts_last_error()
+    assert b'wavernn_window_rows' not in lib.b200tts_last_error()
     assert lib.b200tts_wavernn_window_rows(rows_ok, 2, 274, one, one, one, one, None) == -1
     assert b'runs 275 of 274 steps' in lib.b200tts_last_error()
     assert lib.b200tts_wavernn_window_rows(W(_lib.WaveRNNWindowRow(good, 0, 0, 0, 275), _lib.WaveRNNWindowRow(other, 0, 0, 0, 0)), 2, 275,

@@ -1,11 +1,8 @@
 """Streaming synthesis without a GPU: the decoder stream's release rule on recorded stop-logit sequences, the post-net window plan against
-the fp64 oracle post-net, the WaveRNN lookahead and window plan against the fp64 upsampling, argument checks, and the new kernels'
-registers."""
+the fp64 oracle post-net, the WaveRNN lookahead and window plan against the fp64 upsampling, and argument checks."""
 import ctypes
 import json
 import os
-import re
-import subprocess
 
 import numpy as np
 import pytest
@@ -13,10 +10,10 @@ import torch
 
 import wavernn_oracle as O
 from helpers import GOLDEN_DIR
-from multilingual_text_to_speech_b200 import _lib, build
+from multilingual_text_to_speech_b200 import _lib
 from multilingual_text_to_speech_b200.modules.tacotron2 import Decoder, postnet_window, stream_release
 from multilingual_text_to_speech_b200.modules.wavernn import WaveRNN
-from test_wavernn_cpu import REAL, _nvcc
+from test_wavernn_cpu import REAL
 
 
 # ---- decoder stream: which frames each chunk releases ----
@@ -101,7 +98,7 @@ def _small():
     return m
 
 
-def _window_features(m, p, mel, s0, s1, known, final):
+def _windowed_features(m, p, mel, s0, s1, known, final):
     """fp64 features of positions [s0, s1) computed on the windows of window_plan, [s1 - s0, 80 + 128]."""
     hop, pad = m.hop_length, m.pad
     (P0, P1), (r0, r1), _ = m.window_plan(s0, s1, known, final)
@@ -156,10 +153,10 @@ def test_window_plan_reproduces_the_whole_mel_upsampling(frames, chunking):
         known += n
         ready = min(known - la, known - 1) * hop
         if ready > steps:
-            got = _window_features(m, p, mel, steps, ready, known, False)
+            got = _windowed_features(m, p, mel, steps, ready, known, False)
             np.testing.assert_allclose(got, ref[steps:ready], rtol=1e-12, atol=1e-12)
             steps = ready
-    got = _window_features(m, p, mel, steps, (frames - 1) * hop, frames, True)
+    got = _windowed_features(m, p, mel, steps, (frames - 1) * hop, frames, True)
     np.testing.assert_allclose(got, ref[steps:(frames - 1) * hop], rtol=1e-12, atol=1e-12)
 
 
@@ -205,33 +202,20 @@ def test_decoder_stream_rejects_a_bad_chunk_size():
         next(model.inference_stream(torch.tensor([], dtype=torch.int64)))
 
 
-def test_abi_rejects_reads_outside_the_windows_without_a_device():
+def test_window_rows_abi_rejects_each_bad_window_without_a_device():
+    """b200tts_wavernn_window_rows refuses each shape alone in a one-row call: reads outside the mel or aux window, bad dimensions, a hop
+    that is not a multiple of the last factor, a negative first position."""
     lib = _lib.load()
     one = ctypes.c_void_p(16)
-    # positions [0, 275) read penultimate samples up to 3 x 25 (pad 2, last factor 11): a window of 60 samples is too short
-    ws = _lib.WaveRNNWindowShape(80, 128, 275, 2, 11, 0, 0, 60, 0, 5)
-    assert lib.b200tts_wavernn_window(ctypes.byref(ws), one, one, one, 0, 275, one, None) == -1
-    assert b'outside the window' in lib.b200tts_last_error()
-    ws = _lib.WaveRNNWindowShape(80, 128, 275, 2, 11, 0, 0, 100, 1, 5)          # aux frames start at 1, frame 0 is read
-    assert lib.b200tts_wavernn_window(ctypes.byref(ws), one, one, one, 0, 275, one, None) == -1
-    assert b'aux frames' in lib.b200tts_last_error()
-
-
-# measured: wavernn_window_kernel 40 registers, no stack or spills (CUDA 12.9, sm_90a); the loop kernel is bounded by test_wavernn_cpu
-WINDOW_REG_BOUND = 64
-
-
-def test_window_kernel_registers_and_spills(tmp_path):
-    nvcc = _nvcc()
-    if nvcc is None:
-        pytest.skip('nvcc not available')
-    cmd = [nvcc] + build.NVCC_FLAGS + ['-I', os.path.join(build.ROOT, 'include'), '-Xptxas', '-v', '-cubin',
-                                       os.path.join(build.CSRC, 'wavernn.cu'), '-o', str(tmp_path / 'wavernn.cubin')]
-    res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert res.returncode == 0, res.stdout
-    m = re.search(r'Function properties for \S*wavernn_window_kernel\S*\n\s*(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes '
-                  r'spill loads\n[^\n]*Used (\d+) registers', res.stdout)
-    assert m, res.stdout
-    stack, st, ld, regs = map(int, m.groups())
-    assert st == 0 and ld == 0 and stack == 0, m.group(0)
-    assert regs <= WINDOW_REG_BOUND, regs
+    W = _lib.WaveRNNWindowShape
+    for shape, s0, what in [
+        # positions [0, 275) read penultimate samples up to 3 x 25 (pad 2, last factor 11): a window of 60 samples is too short
+        (W(80, 128, 275, 2, 11, 0, 0, 60, 0, 5), 0, b'outside the window'),
+        (W(80, 128, 275, 2, 11, 0, 0, 100, 1, 5), 0, b'aux frames'),          # aux frames start at 1, frame 0 is read
+        (W(0, 128, 275, 2, 11, 0, 0, 100, 0, 5), 0, b'bad dimensions'),
+        (W(80, 128, 270, 2, 11, 0, 0, 100, 0, 5), 0, b'must be a multiple'),
+        (W(80, 128, 275, 2, 11, 0, 0, 100, 0, 5), -1, b'positions [-1, 274)'),
+    ]:
+        row = (_lib.WaveRNNWindowRow * 1)(_lib.WaveRNNWindowRow(shape, s0, 0, 0, 275))
+        assert lib.b200tts_wavernn_window_rows(row, 1, 275, one, one, one, one, None) == -1
+        assert what in lib.b200tts_last_error(), (what, lib.b200tts_last_error())

@@ -10,8 +10,8 @@ The stop projection's bias is set so that the stop token never fires: every text
 the decoder's stop rule, so that streams end and leave the pool at different calls.  Arms, alternated round by round:
   * pool/N: speech_streams of N texts.  Per stream: the real-time factor (wall time to its last chunk / its audio duration), the time to
     its first audio and the largest gap between its chunks; aggregate audio-seconds per wall second; the loop's microseconds per sample
-    step (CUDA events around each b200tts_wavernn_run_rows call); the time per pool.run() outside the loop kernel, host work and the feature
-    and GEMM kernels (the wall time of the run() calls, each ending in the abort-flag read that synchronises, minus the loop's event time);
+    step (CUDA events around each loop call: b200tts_wavernn_run_rows, or b200tts_wavernn_run_stream in a one-stream pool); the time per
+    pool.run() outside the loop kernel, host work and the feature and GEMM kernels (the wall time of the run() calls, each ending in the abort-flag read that synchronises, minus the loop's event time);
   * serial/N (N <= --serial-max): speech_stream of each text, one after another;
   * batch/N: inference_batch of the N texts, then generate_batch(mels, 11000, 550).
 Wall times are host clocks that end in torch.cuda.synchronize().  The card's name and power limit are read in the same run."""
@@ -77,21 +77,23 @@ def main():
             return self.cut
 
     loop_events, run_walls = [], []
-    orig_run_rows, orig_run = F.wavernn_run_rows, W.StreamPool.run
+    orig_loops, orig_run = (F.wavernn_run_rows, F.wavernn_run_stream), W.StreamPool.run
 
-    def run_rows(shape, params, cond, row_t, row_n, nsteps, uni, out, ws):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        orig_run_rows(shape, params, cond, row_t, row_n, nsteps, uni, out, ws)
-        e1.record()
-        loop_events.append((e0, e1, int(nsteps)))
+    def timed(loop, nsteps_arg):
+        def call(*args):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            loop(*args)
+            e1.record()
+            loop_events.append((e0, e1, int(args[nsteps_arg])))
+        return call
 
     def pool_run(self):
         t0 = time.perf_counter()
         out = orig_run(self)
         run_walls.append(time.perf_counter() - t0)
         return out
-    F.wavernn_run_rows, W.StreamPool.run = run_rows, pool_run
+    F.wavernn_run_rows, F.wavernn_run_stream, W.StreamPool.run = timed(F.wavernn_run_rows, 5), timed(F.wavernn_run_stream, 4), pool_run
 
     rows = []
     for mode in a.modes.split(','):
@@ -159,7 +161,7 @@ def main():
                                host_ms_per_run=(r['run_wall'] * 1e3 - r['loop_ms']) / max(r['runs'], 1))
                 rows.append(row)
                 print(json.dumps(row), flush=True)
-    F.wavernn_run_rows, W.StreamPool.run = orig_run_rows, orig_run
+    (F.wavernn_run_rows, F.wavernn_run_stream), W.StreamPool.run = orig_loops, orig_run
     real_time = {}
     for r in rows:
         if r['arm'].startswith('pool/') and not r['ragged'] and r['rtf_worst_stream'] < 1:
