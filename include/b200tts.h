@@ -520,6 +520,45 @@ int b200tts_griffinlim(const b200tts_vocoder_shape* shape, const float* S, const
  * largest sample, not the largest magnitude, as the reference's Python max() is. */
 int b200tts_deemphasis_normalize(const b200tts_vocoder_shape* shape, float* wave, const int32_t* off, void* stream);
 
+/* ---- streaming Griffin-Lim: frame-by-frame phase reconstruction with look-ahead (RTISI-LA), audio.GriffinLimVocoder ----
+ * Up to `slots` streams, each in its own workspace slot: the committed overlap-add c over the frames still open, the time-domain estimates
+ * of the look-ahead set A = {m .. min(m + k, F - 1)}, their magnitudes, the frame counters and the de-emphasis carry.  Frame m is processed
+ * once frame m + k has arrived or the stream has ended: the frames of A not yet in it are admitted in increasing j (x_j = irfft(S_j X / |X|),
+ * X = rfft(w p_j), p_j = (c + the overlap-add of the frames of A before j) / e over frame j's span, phase 1 where X = 0), then `iters`
+ * Jacobi iterations project every frame of A against p_j = (c + the overlap-add of all of A) / e, then c += w x_m.  e is the one-sided
+ * envelope sum_{i >= 0} w^2(n - i hop) (0 where it is 0).  The samples of the trimmed output (z[N/2 .. N/2 + hop (F - 1)) of the untrimmed
+ * signal z) below (m + 1) hop, or all of them after the last frame, are released divided by the window sum-square of frames 0..m where that
+ * exceeds tiny(float32), then de-emphasised (y = x + preemphasis y_prev, carried across calls; 0 = off).  No peak normalisation.  fp32. */
+#define B200TTS_GL_STREAM_MAX_LOOKAHEAD 7
+typedef struct {
+    int N, hop, win;     /* as in b200tts_vocoder_shape: periodic Hann of win samples centre-padded to N */
+    int lookahead;       /* k, 0 to B200TTS_GL_STREAM_MAX_LOOKAHEAD */
+    int iters;           /* Jacobi iterations per processed frame, >= 1 */
+    int slots;           /* streams of the workspace, 1 to 64 */
+    float preemphasis;   /* in (-1, 1) */
+} b200tts_gl_stream_shape;
+typedef struct {
+    int slot;            /* the stream's workspace slot; each slot at most once per call */
+    int frames;          /* frames the stream has received, this call's included (never fewer than the previous call's) */
+    int ended;           /* nonzero: `frames` is the stream's length F (>= 2) */
+    long long s_off;     /* row of S_new holding the first frame received since the previous call */
+    long long wave_off;  /* where the samples this call releases go in `wave` */
+} b200tts_gl_stream_row;
+/* Host only: the workspace (twiddles, window and `slots` slots); 0 for an invalid shape (message set). */
+size_t b200tts_gl_stream_workspace_bytes(const b200tts_gl_stream_shape* shape);
+/* Resets the `count` listed slots (host int32, distinct, each in [0, slots)) to an empty stream, and writes the FFT tables: a workspace is
+ * run only after its first reset.  One launch. */
+int b200tts_gl_stream_reset(const b200tts_gl_stream_shape* shape, void* workspace, size_t workspace_bytes, const int32_t* slots, int count,
+                            void* stream);
+/* One call over `count` rows (host descriptors, 1 to 64): row r's stream takes its new frames' magnitudes from S_new [rows, N/2 + 1] (fp32,
+ * b200tts_spectrogram_magnitude's output), processes every frame that is ready, in order, and writes the samples it releases to
+ * wave + wave_off.  S_new and wave are required even when no row has new frames or releases samples.  The frame count a slot has
+ * received lives on the device, so the call cannot check that S_new holds rows [s_off, s_off + frames - that count) for every row, nor
+ * that wave is long enough: the caller keeps that count (frames of its previous call, 0 after a reset), as for any device buffer.  One CTA per row, one launch; no slot is read by another row's CTA, so a stream's bits do not depend on its company or on
+ * how its frames were cut into calls. */
+int b200tts_gl_stream_run(const b200tts_gl_stream_shape* shape, const b200tts_gl_stream_row* rows, int count, const float* S_new, float* wave,
+                          void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- audio analysis: audio.spectrogram and mel_cepstral_distorision, reference utils/audio.py:66-78, 117-161 (librosa 0.7.0) ----
  * Packed ragged layout: utterance b owns samples [soff[b], soff[b+1]) of an fp32 waveform (L_b >= 1) and frames [off[b], off[b+1]) with
  * F_b = 1 + L_b / hop (soff, off: int32 [B+1], device, both starting at 0; the caller keeps them consistent).  Spectra are frame-major

@@ -76,6 +76,18 @@ class VocoderShape(Structure):
                [(n, c_float) for n in ('power', 'momentum', 'preemphasis')] + [('nnls_iters', c_int)]
 
 
+class GLStreamShape(Structure):
+    _fields_ = [(n, c_int) for n in ('N', 'hop', 'win', 'lookahead', 'iters', 'slots')] + [('preemphasis', c_float)]
+
+
+class GLStreamRow(Structure):
+    _fields_ = [(n, c_int) for n in ('slot', 'frames', 'ended')] + [(n, c_longlong) for n in ('s_off', 'wave_off')]
+
+
+# include/b200tts.h: B200TTS_GL_STREAM_MAX_LOOKAHEAD
+GL_STREAM_MAX_LOOKAHEAD = 7
+
+
 class AnalysisShape(Structure):
     _fields_ = [(n, c_int) for n in ('B', 'total_samples', 'total_frames', 'N', 'hop', 'win', 'n_mels')] + [('preemphasis', c_double)]
 
@@ -223,6 +235,9 @@ SIGNATURES = {
     'b200tts_griffinlim': (c_int, [POINTER(VocoderShape), c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t,
                                    c_void_p]),
     'b200tts_deemphasis_normalize': (c_int, [POINTER(VocoderShape), c_void_p, c_void_p, c_void_p]),
+    'b200tts_gl_stream_workspace_bytes': (c_size_t, [POINTER(GLStreamShape)]),
+    'b200tts_gl_stream_reset': (c_int, [POINTER(GLStreamShape), c_void_p, c_size_t, POINTER(c_int), c_int, c_void_p]),
+    'b200tts_gl_stream_run': (c_int, [POINTER(GLStreamShape), POINTER(GLStreamRow), c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     'b200tts_analysis_workspace_bytes': (c_size_t, [POINTER(AnalysisShape)]),
     'b200tts_stft_magnitude': (c_int, [POINTER(AnalysisShape), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     'b200tts_amplitude_to_db': (c_int, [POINTER(AnalysisShape), c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -227,6 +227,12 @@ int spectrogram_magnitude_impl(const b200tts_vocoder_shape& s, const float* log_
 int griffinlim_impl(const b200tts_vocoder_shape& s, const float* S, const int* off, float* angles, float* rebuilt, int first, int iters,
                     float* wave, void* ws, size_t ws_bytes, cudaStream_t st);
 int deemphasis_normalize_impl(const b200tts_vocoder_shape& s, float* wave, const int* off, cudaStream_t st);
+size_t gl_stream_workspace_bytes(const b200tts_gl_stream_shape& s);
+int gl_stream_reset_check(const b200tts_gl_stream_shape& s, void* ws, size_t ws_bytes, const int* list, int count);
+int gl_stream_reset_impl(const b200tts_gl_stream_shape& s, void* ws, const int* list, int count, cudaStream_t st);
+int gl_stream_run_check(const b200tts_gl_stream_shape& s, const b200tts_gl_stream_row* rows, int count, void* ws, size_t ws_bytes);
+int gl_stream_run_impl(const b200tts_gl_stream_shape& s, const b200tts_gl_stream_row* rows, int count, const float* S_new, float* wave, void* ws,
+                       cudaStream_t st);
 size_t analysis_workspace_bytes(const b200tts_analysis_shape& s);
 int stft_magnitude_impl(const b200tts_analysis_shape& s, const float* wave, const int* soff, const int* off, const float* mel_basis, float* out,
                         void* ws, size_t ws_bytes, cudaStream_t st);
@@ -782,6 +788,25 @@ int b200tts_deemphasis_normalize(const b200tts_vocoder_shape* shape, float* wave
     B200_REQUIRE(shape && wave && off, "deemphasis_normalize: null argument");
     B200_TRY(require_device());
     return deemphasis_normalize_impl(*shape, wave, off, (cudaStream_t)stream);
+}
+
+size_t b200tts_gl_stream_workspace_bytes(const b200tts_gl_stream_shape* shape) {
+    if (!shape) { set_last_error("gl_stream_workspace_bytes: null shape"); return 0; }
+    return gl_stream_workspace_bytes(*shape);
+}
+int b200tts_gl_stream_reset(const b200tts_gl_stream_shape* shape, void* workspace, size_t workspace_bytes, const int32_t* slots, int count,
+                            void* stream) {
+    B200_REQUIRE(shape, "gl_stream_reset: null argument");
+    B200_TRY(gl_stream_reset_check(*shape, workspace, workspace_bytes, slots, count));
+    B200_TRY(require_device());
+    return gl_stream_reset_impl(*shape, workspace, slots, count, (cudaStream_t)stream);
+}
+int b200tts_gl_stream_run(const b200tts_gl_stream_shape* shape, const b200tts_gl_stream_row* rows, int count, const float* S_new, float* wave,
+                          void* workspace, size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(shape && S_new && wave, "gl_stream_run: null argument");
+    B200_TRY(gl_stream_run_check(*shape, rows, count, workspace, workspace_bytes));
+    B200_TRY(require_device());
+    return gl_stream_run_impl(*shape, rows, count, S_new, wave, workspace, (cudaStream_t)stream);
 }
 
 size_t b200tts_analysis_workspace_bytes(const b200tts_analysis_shape* shape) {

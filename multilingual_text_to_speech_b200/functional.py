@@ -885,6 +885,40 @@ def deemphasis_normalize(shape, wave, off):
     return wave
 
 
+def gl_stream_workspace_bytes(shape):
+    """Bytes of the streaming Griffin-Lim workspace for `shape` (a _lib.GLStreamShape), host only; raises ValueError on an invalid shape."""
+    n = _lib.load().b200tts_gl_stream_workspace_bytes(ctypes.byref(shape))
+    if n == 0:
+        raise ValueError(_lib.load().b200tts_last_error().decode())
+    return n
+
+
+def gl_stream_workspace(shape, device):
+    """A 256-byte aligned workspace of b200tts_gl_stream_run for `shape`."""
+    n = gl_stream_workspace_bytes(shape)
+    buf = torch.empty(n + 256, dtype=torch.uint8, device=device)
+    off = (-buf.data_ptr()) % 256
+    return buf[off:off + n]
+
+
+def gl_stream_reset(shape, ws, slots):
+    """Reset the listed slots (host ints) to empty streams and write the FFT tables."""
+    n = len(slots)
+    check(_lib.load().b200tts_gl_stream_reset(ctypes.byref(shape), ptr(ws), ws.numel(), (ctypes.c_int * n)(*slots), n, _stream()),
+          'b200tts_gl_stream_reset')
+
+
+def gl_stream_run(shape, rows, S_new, wave, ws):
+    """One call over `rows` (a list of _lib.GLStreamRow): new magnitudes S_new [rows, K] fp32, released samples into `wave`."""
+    _require_cuda(S_new, wave, ws)
+    assert wave.dtype == torch.float32 and wave.is_contiguous()
+    assert S_new.dtype == torch.float32 and S_new.is_contiguous()
+    n = len(rows)
+    check(_lib.load().b200tts_gl_stream_run(ctypes.byref(shape), (_lib.GLStreamRow * n)(*rows), n, ptr(S_new), ptr(wave), ptr(ws), ws.numel(),
+                                            _stream()), 'b200tts_gl_stream_run')
+    return wave
+
+
 # ------------------------------------------------------------------------------------------------
 # audio analysis (packed ragged layout: utterance b owns samples soff[b]:soff[b+1] and frames off[b]:off[b+1])
 # ------------------------------------------------------------------------------------------------

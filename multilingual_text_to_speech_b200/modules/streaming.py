@@ -1,15 +1,24 @@
-"""Text to audio in chunks: the Tacotron decoder stream feeding the WaveRNN stream.
+"""Text to audio in chunks: the Tacotron decoder stream feeding the WaveRNN stream, or the streaming Griffin-Lim vocoder
+(modules/griffinlim.py: GriffinLimVocoder has the members used here; pass it where `wavernn` is taken, with
+mel_transform=lambda m: utils.audio.denormalize_spectrogram(m, True) and preemphasis=hp.preemphasis).
 
 Each stage lags the one before it by a bounded number of frames, whatever the utterance length:
   * the decoder runs in chunks of `chunk_frames` frames (Tacotron.inference_stream);
   * the post-net releases a frame once `Postnet.halo()` (10) decoded frames follow it, or the stop cut is known;
   * the vocoder runs its sample loop up to `WaveRNN.lookahead()` (2 at pad 2, factors 5 x 5 x 11) frames behind the last mel frame it has;
-  * it holds back the last 20 hops of samples it has run until the mel ends, because the fade-out lands on them."""
+  * it holds back the last 20 hops of samples it has run until the mel ends, because the fade-out lands on them.
+With a GriffinLimVocoder the vocoder processes frame m once `lookahead()` (3) frames follow it and releases its audio once no later frame
+touches it (DESIGN 8.1).  Its streams need at least 2 frames instead of 21."""
+from typing import Union
+
+from .griffinlim import GriffinLimVocoder
 from .tacotron2 import MAX_STREAM_TEXTS, Tacotron, _check_batch_inputs
 from .wavernn import FoldedStreamPool, WaveRNN
 
+Vocoder = Union[WaveRNN, GriffinLimVocoder]
 
-def speech_stream(tacotron: Tacotron, wavernn: WaveRNN, text, speaker=None, language=None, mel_transform=None, chunk_frames=None,
+
+def speech_stream(tacotron: Tacotron, wavernn: Vocoder, text, speaker=None, language=None, mel_transform=None, chunk_frames=None,
                   uniforms=None, generator=None, preemphasis=0.0, target=None, overlap=None):
     """Yields waveform chunks of `text` as the decoder produces it: tacotron.inference_stream(text, speaker, language, chunk_frames) fed,
     through mel_transform, into wavernn.generate_stream(…, uniforms, generator, preemphasis).  mel_transform (default: none) maps a
@@ -23,14 +32,15 @@ def speech_stream(tacotron: Tacotron, wavernn: WaveRNN, text, speaker=None, lang
     yield from wavernn.generate_stream(mels, uniforms, generator, preemphasis, target, overlap)
 
 
-def speech_streams(tacotron: Tacotron, wavernn: WaveRNN, texts, speakers=None, languages=None, mel_transform=None, chunk_frames=None,
+def speech_streams(tacotron: Tacotron, wavernn: Vocoder, texts, speakers=None, languages=None, mel_transform=None, chunk_frames=None,
                    uniforms=None, generator=None, preemphasis=0.0, target=None, overlap=None):
     """speech_stream for up to 64 texts at once: yields (i, waveform chunk) for text i.  Every text is submitted to one SpeechServer(…,
     max_streams=len(texts)) at once and the server steps until it is idle: each step runs one decoder call over the texts still decoding
     (text i reads column i of a recorded mask tape), feeds its post-net chunks (through mel_transform) into the vocoder pool and makes one
     pool.run().  uniforms: None or one tape [1, T_i, U] per text ([K_i, target + 2 overlap, U] with target and overlap).  Each text's audio equals speech_stream of that text alone, bit for bit
-    given its tape, in fp32 mode (where the decoded frames of a group equal those of single texts).  A text that decodes fewer than 21
-    frames raises ValueError when its stream ends, as speech_stream does, and that ends the generator for every text of the group."""
+    given its tape, in fp32 mode (where the decoded frames of a group equal those of single texts).  A text that decodes fewer than the
+    vocoder's minimum (21 frames for a WaveRNN, 2 for a GriffinLimVocoder) raises ValueError when its stream ends, as speech_stream does, and
+    that ends the generator for every text of the group."""
     texts = list(texts)
     if len(texts) > MAX_STREAM_TEXTS:
         raise ValueError(f'inference_streams: at most {MAX_STREAM_TEXTS} texts decode as one group (got {len(texts)})')
@@ -67,7 +77,7 @@ class SpeechServer:
     its vocoder row from admission to its last sample, which covers its decoder row's lifetime, so the vocoder pool's max_streams is the
     only limit), makes one DecoderPool.run(), feeds the post-net chunks through mel_transform into the StreamPool (a request whose decode
     ended after the previous call gets its end()), makes one pool.run() and returns {id: waveform chunk}.  A request whose mel ends under
-    21 frames moves to `failed` ({id: message}) and frees its rows; the others go on.  cancel() drops a queued, decoding or vocoding
+    the vocoder's minimum (21 frames for a WaveRNN, 2 for a GriffinLimVocoder) moves to `failed` ({id: message}) and frees its rows; the others go on.  cancel() drops a queued, decoding or vocoding
     request.  `pending` lists the queued ids in order, `active` the admitted ones.
 
     A request's audio is speech_stream of it alone, bit for bit in fp32 mode, given the same mask tape (`masks`, as DecoderPool.open takes
@@ -80,7 +90,7 @@ class SpeechServer:
     alone, which equals generate(mel, target, overlap) of its mel; tapes are [K, target + 2 overlap, U].  Admission stays at most
     max_streams requests; their folds share the loop's 64 rows."""
 
-    def __init__(self, tacotron: Tacotron, wavernn: WaveRNN, max_streams=64, mel_transform=None, chunk_frames=None, preemphasis=0.0,
+    def __init__(self, tacotron: Tacotron, wavernn: Vocoder, max_streams=64, mel_transform=None, chunk_frames=None, preemphasis=0.0,
                  generator=None, target=None, overlap=None):
         self.decoder = tacotron.decoder_pool(max_streams, chunk_frames)
         self.pool = wavernn.stream_pool(max_streams, preemphasis, generator, target, overlap)
