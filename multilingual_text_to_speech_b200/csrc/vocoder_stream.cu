@@ -182,11 +182,12 @@ __global__ void __launch_bounds__(GL_THREADS) gl_stream_run_kernel(FftPlan p, in
         }
         const bool final = row.ended && lf == F - 1;                 // release
         const int rel_end = final ? hop * (F - 1) : max(0, base + hop - N / 2);
-        for (int o = rel + threadIdx.x; o < rel_end; o += blockDim.x) {
-            const int z = o + N / 2;
+        // stride over the offset within the span: rel + q + blockDim.x would overflow int for a stream near the 2^31 sample limit
+        for (int q = threadIdx.x; q < rel_end - rel; q += blockDim.x) {
+            const int z = rel + q + N / 2;
             const float v = c[z % N];
             const float wss = window_sumsquare(sm.window, N, hop, z, lf);
-            scratch[o - rel] = wss > FLT_MIN ? v / wss : v;
+            scratch[q] = wss > FLT_MIN ? v / wss : v;
         }
         __syncthreads();
         if (threadIdx.x == 0) {

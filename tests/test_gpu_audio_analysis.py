@@ -63,7 +63,10 @@ def _mel_bound(A, X64, kb):
     return A.astype(np.float64) @ kb + (nm + 1) * EPS * (A.astype(np.float64) @ X64) + 1e-38
 
 
-@pytest.mark.parametrize('n_fft,hop,win', [(1102, 275, 1102), (1024, 256, 1024), (1024, 256, 800)])
+# the default plan [19, 29], [4, 4, 4, 4, 2] with and without a zero-padded window, then the other plans a user's hp.num_fft can give:
+# [4, 4, 5, 5] (16 kHz), [2, 5, 5, 11], [3, 7, 13] (N - win odd), [23, 31], [31, 31] and [4, 4, 4, 4, 4]
+@pytest.mark.parametrize('n_fft,hop,win', [(1102, 275, 1102), (1024, 256, 1024), (1024, 256, 800), (800, 200, 800), (1100, 275, 1100),
+                                           (546, 136, 545), (1426, 356, 1426), (1922, 480, 1922), (2048, 512, 2048)])
 def test_stft_magnitude_against_fp64(mods, n_fft, hop, win):
     _lib, F, audio = mods
     lengths = [1, 2, 3, n_fft // 2 - 1, n_fft // 2, n_fft // 2 + 1, hop * 40, hop * 41 + 17]

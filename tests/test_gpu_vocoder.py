@@ -49,7 +49,10 @@ def _frame_bound(ref, n_fft):
     return C_FFT * np.log2(n_fft) * EPS * (norms + 1e-3 * norms.max())
 
 
-@pytest.mark.parametrize('n_fft,hop,win', [(1102, 275, 1102), (1024, 256, 1024), (1024, 256, 800)])
+# the default plan [19, 29], [4, 4, 4, 4, 2] with and without a zero-padded window, then the other plans a user's hp.num_fft can give:
+# [4, 4, 5, 5] (16 kHz), [2, 5, 5, 11], [3, 7, 13] (N - win odd), [23, 31], [31, 31] and [4, 4, 4, 4, 4]
+@pytest.mark.parametrize('n_fft,hop,win', [(1102, 275, 1102), (1024, 256, 1024), (1024, 256, 800), (800, 200, 800), (1100, 275, 1100),
+                                           (546, 136, 545), (1426, 356, 1426), (1922, 480, 1922), (2048, 512, 2048)])
 def test_single_transforms_against_fp64(mods, n_fft, hop, win):
     _lib, F, _ = mods
     rng = np.random.default_rng(n_fft + win)

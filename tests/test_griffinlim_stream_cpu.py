@@ -14,6 +14,7 @@ import torch
 import __graft_entry__ as entry
 import audio_oracle as O
 import griffinlim_stream_oracle as G
+from gl_stream_slot import GlLayout
 from multilingual_text_to_speech_b200 import _lib, build
 from multilingual_text_to_speech_b200 import functional as F
 from multilingual_text_to_speech_b200.modules.griffinlim import GriffinLimVocoder
@@ -170,11 +171,7 @@ def test_workspace_query_and_validation(lib):
         s = dict(N=N, hop=HOP, win=WIN, lookahead=3, iters=32, slots=4, preemphasis=0.97)
         s.update(kw)
         return lib.b200tts_gl_stream_workspace_bytes(ctypes.byref(_lib.GLStreamShape(*s.values())))
-    up = lambda x: -(-x // 256) * 256                                   # noqa: E731
-    M, K = N // 2, N // 2 + 1
-    tables = up(up(up(8 * M) + 8 * K) + 4 * N)
-    slot = up(up(up(256 + 4 * N) + 4 * 4 * N) + 4 * 4 * K)
-    assert ws() == tables + 4 * slot
+    assert ws() == GlLayout(N, 3, 4).bytes
     for kw, msg in ((dict(N=1101), 'unsupported FFT size'), (dict(win=N + 1), 'window length'), (dict(hop=0), 'hop'),
                     (dict(lookahead=-1), 'lookahead'), (dict(lookahead=8), 'lookahead'), (dict(lookahead=0, hop=N // 2 + 1), 'lookahead 0'), (dict(iters=0), 'iters'), (dict(slots=0), 'slots'),
                     (dict(slots=65), 'slots'), (dict(preemphasis=1.0), 'preemphasis'), (dict(N=2048, win=2048, hop=512, lookahead=7), 'shared memory')):
