@@ -1,10 +1,10 @@
 """Griffin-Lim as a streaming vocoder: frame-by-frame phase reconstruction with look-ahead (RTISI-LA; Zhu, Beauregard and Wyse, IEEE TASLP
 2007), specified in DESIGN ("Griffin-Lim vocoder", "Streaming").
 
-GriffinLimVocoder has the members the streaming layer calls on a WaveRNN (generate_stream, stream_pool, lookahead, _check_stream_tape), so
-speech_stream, speech_streams and SpeechServer run on it with mel_transform=utils.audio.denormalize_spectrogram and
-preemphasis=hp.preemphasis.  The magnitudes of each frame are the batch vocoder's (b200tts_spectrogram_magnitude: dB -> amplitude, the
-FISTA NNLS for mel input, ** hp.griffin_lim_power); the frame loop runs on b200tts_gl_stream_run, one CTA per stream and call.
+GriffinLimVocoder has the members the streaming layer calls on a WaveRNN (generate_stream, stream_pool, lookahead), so speech_stream,
+speech_streams and SpeechServer run on it with mel_transform=utils.audio.denormalize_spectrogram and preemphasis=hp.preemphasis.  The
+magnitudes of each frame are the batch vocoder's (b200tts_spectrogram_magnitude: dB -> amplitude, the FISTA NNLS for mel input,
+** hp.griffin_lim_power); the frame loop runs on b200tts_gl_stream_run, one CTA per stream and call.
 
 A stream cannot know its largest sample, so unlike utils.audio.inverse_spectrogram its output is not divided by max(y): scale it
 afterwards if a peak of 1 is wanted."""
@@ -15,26 +15,7 @@ from .. import _lib
 from .. import functional as F
 from ..params.params import Params as hp
 from ..utils import audio
-from .wavernn import _as_input
-
-MIN_FRAMES = 2           # as batch Griffin-Lim
-
-
-def _cuda_device():
-    return torch.device('cuda', torch.cuda.current_device()) if torch.cuda.is_available() else torch.device('cuda')
-
-
-def _check_no_tape(uniforms, target, overlap):
-    if uniforms is not None:
-        raise ValueError('Griffin-Lim draws nothing: it takes no uniform tape')
-    if target is not None or overlap is not None:
-        raise ValueError('Griffin-Lim streams are not folded: target and overlap are WaveRNN arguments')
-
-
-def _check_preemphasis(preemphasis):
-    if not -1.0 < float(preemphasis) < 1.0:
-        raise ValueError(f'preemphasis {preemphasis} must lie in (-1, 1)')
-    return float(preemphasis)
+from .stream_pool import Stream, VocoderStreamPool, generate_stream as _generate_stream
 
 
 class GriffinLimVocoder:
@@ -63,13 +44,6 @@ class GriffinLimVocoder:
         """Frames that must follow a frame before it is processed (k)."""
         return self.k
 
-    def _check_stream_tape(self, uniforms, fold_len=None):
-        """Griffin-Lim draws nothing: only None is accepted."""
-        _check_no_tape(uniforms, None, None)
-        if fold_len is not None:
-            raise ValueError('Griffin-Lim streams are not folded')
-        return None
-
     def _check_chunk(self, chunk, i):
         as_numpy = not isinstance(chunk, torch.Tensor)
         t = torch.as_tensor(np.asarray(chunk) if as_numpy else chunk)
@@ -94,119 +68,77 @@ class GriffinLimVocoder:
             S = F.spectrogram_magnitude(shape, x)
         return S[:n]
 
+    min_stream_frames = 2            # as batch Griffin-Lim
+    short_stream = 'the spectrogram stream ended after {} frames; Griffin-Lim needs at least 2'
+
     def generate_stream(self, mel_chunks, uniforms=None, generator=None, preemphasis=0.0, target=None, overlap=None):
         """Yields the waveform of the spectrogram chunks [bins, n_k] (n_k >= 0) as it is released: their concatenation, F >= 2 frames,
         gives hop (F - 1) samples in all (inverse_spectrogram's length and alignment), bit for bit the same however the chunks are cut.
         preemphasis: de-emphasis coefficient (0 = none), carried across chunks.  No peak normalisation.  uniforms, target and overlap exist
         for the WaveRNN signature and must be None; generator is unused.  Runs through a one-stream GriffinLimStreamPool on the device of
-        the first CUDA chunk, or the current CUDA device; chunks come out as the first chunk went in (numpy, CUDA or CPU tensors)."""
-        _check_no_tape(uniforms, target, overlap)
-        preemphasis = _check_preemphasis(preemphasis)
-        pool = sid = fmt = None
-        for i, chunk in enumerate(mel_chunks):
-            spec, as_numpy = self._check_chunk(chunk, i)
-            if pool is None:
-                fmt = (as_numpy, not as_numpy and spec.is_cuda)
-                pool = GriffinLimStreamPool(self, 1, preemphasis, spec.device if spec.is_cuda else None)
-                sid = pool.open()
-            pool.feed(sid, spec)
-            if spec.shape[1] and pool.streams[sid].fed >= MIN_FRAMES:      # a shorter stream is an error, found at its end
-                out = pool.run()
-                if sid in out:
-                    yield _as_input(out[sid], *fmt)
-        if pool is None:
-            raise ValueError(f'the spectrogram stream ended after 0 frames; Griffin-Lim needs at least {MIN_FRAMES}')
-        pool.end(sid)
-        out = pool.run()
-        if sid in out:
-            yield _as_input(out[sid], *fmt)
+        the first CUDA chunk, or the current CUDA device, with one run() per non-empty chunk once 2 frames are in (a run processes every
+        ready frame; a shorter stream is an error, found at its end); chunks come out as the first chunk went in (numpy, CUDA or CPU
+        tensors)."""
+        yield from _generate_stream(self, mel_chunks, uniforms, generator, preemphasis, target, overlap, self.min_stream_frames)
 
     def stream_pool(self, max_streams, preemphasis=0.0, generator=None, target=None, overlap=None):
         """A GriffinLimStreamPool of up to max_streams (1 to 64) streams.  generator is unused; target and overlap must be None."""
-        _check_no_tape(None, target, overlap)
+        if target is not None or overlap is not None:
+            raise ValueError('Griffin-Lim streams are not folded: target and overlap are WaveRNN arguments')
         return GriffinLimStreamPool(self, max_streams, preemphasis)
 
 
-class _GLStream:
+class _GLStream(Stream):
     """One stream of a GriffinLimStreamPool: its slot, the frames fed but not yet sent to the device, and the host's copy of the slot's
     counters (frames received, frames committed)."""
 
     def __init__(self, slot):
+        super().__init__()
         self.slot = slot
         self.pending = []        # [n, bins] fp32 frame-major tensors, in feed order
-        self.chunks = 0
         self.fed = 0
         self.sent = 0
         self.committed = 0
-        self.released = 0        # output samples returned
-        self.ended = False
         self.fresh = True        # its slot has not been reset yet
 
+    @property
+    def frames(self):
+        return self.fed
 
-class GriffinLimStreamPool:
+    def append(self, spec):
+        self.pending.append(spec.t().to(torch.float32))
+        self.fed += int(spec.shape[1])
+
+
+class GriffinLimStreamPool(VocoderStreamPool):
     """Concurrent streaming Griffin-Lim with StreamPool's interface: up to max_streams streams, each a generate_stream, in one workspace.
-    open() takes the lowest free slot; feed() and end() add a stream's frames and mark its end; run() processes every ready frame of every
-    stream and returns {sid: waveform chunk} (CUDA tensors) for the streams that released samples; a stream's slot is freed when its final
-    chunk is returned, or at once by close().  open, feed, end and close do no device work; a run() makes a fixed number of launches
-    whatever the number of streams: the slot resets of newly opened streams, the magnitudes of the new frames of all streams, and one
-    b200tts_gl_stream_run with a CTA per stream.  Each stream's concatenated chunks equal its own generate_stream bit for bit, whatever
-    joins or leaves around it.  Runs on `device`, by default the CUDA device that was current when the pool was made."""
+    open() takes the lowest free slot (uniforms must be None; a seed is checked and unused: nothing is drawn); feed() and end() add a
+    stream's frames and mark its end; run() processes every ready frame of every stream and returns {sid: waveform chunk} (CUDA tensors)
+    for the streams that released samples; a stream's slot is freed when its final chunk is returned, or at once by close().  open, feed,
+    end and close do no device work; a run() makes a fixed number of launches whatever the number of streams: the slot resets of newly
+    opened streams, the magnitudes of the new frames of all streams, and one b200tts_gl_stream_run with a CTA per stream.  Each stream's
+    concatenated chunks equal its own generate_stream bit for bit, whatever joins or leaves around it.  Runs on `device`, by default the
+    CUDA device that was current when the pool was made."""
 
     def __init__(self, vocoder, max_streams, preemphasis=0.0, device=None):
-        if isinstance(max_streams, bool) or not isinstance(max_streams, (int, np.integer)) or not 1 <= max_streams <= _lib.WAVERNN_MAX_STREAMS:
-            raise ValueError(f'a stream pool holds 1 to {_lib.WAVERNN_MAX_STREAMS} streams (got {max_streams!r})')
-        self.v, self.a = vocoder, _check_preemphasis(preemphasis)
-        self.rows = int(max_streams)
-        self.device = _cuda_device() if device is None else device
+        super().__init__(vocoder, max_streams, preemphasis, device)
         self.shape = vocoder.shape(self.rows, self.a)
         F.gl_stream_workspace_bytes(self.shape)
         self.ws = None                         # allocated by the first run()
         self.slots = [None] * self.rows        # sid of the stream in each slot
-        self.streams = {}
-        self.next_sid = 0
 
-    def open(self, uniforms=None, seed=None):
-        """A new stream in the lowest free slot -> its id.  uniforms must be None; seed is accepted and unused (nothing is drawn)."""
-        self.v._check_stream_tape(uniforms)
-        free = [r for r in range(self.rows) if self.slots[r] is None]
-        if not free:
-            raise ValueError(f'the stream pool is full: {self.rows} streams are open')
-        sid = self.next_sid
-        self.next_sid += 1
-        self.slots[free[0]] = sid
-        self.streams[sid] = _GLStream(free[0])
-        return sid
+    def check_tape(self, uniforms):
+        """Griffin-Lim draws nothing: only None is accepted."""
+        if uniforms is not None:
+            raise ValueError('Griffin-Lim draws nothing: it takes no uniform tape')
 
-    def close(self, sid):
-        """Drops stream sid and frees its slot at once, whatever it has released."""
-        st = self.streams.pop(sid, None)
-        if st is None:
-            raise ValueError(f'unknown or finished stream {sid}')
+    def _open(self, sid, tape, seed):
+        slot = self.slots.index(None)
+        self.slots[slot] = sid
+        return _GLStream(slot)
+
+    def _drop(self, st):
         self.slots[st.slot] = None
-
-    def _stream(self, sid):
-        st = self.streams.get(sid)
-        if st is None:
-            raise ValueError(f'unknown or finished stream {sid}')
-        if st.ended:
-            raise ValueError(f'stream {sid} has ended')
-        return st
-
-    def feed(self, sid, chunk):
-        """Appends spectrogram frames [bins, n] (n >= 0, dB, denormalised) to stream sid."""
-        st = self._stream(sid)
-        spec, _ = self.v._check_chunk(chunk, st.chunks)
-        st.chunks += 1
-        if spec.shape[1]:
-            st.pending.append(spec.t().to(torch.float32))
-            st.fed += int(spec.shape[1])
-
-    def end(self, sid):
-        """Marks the end of stream sid (at least 2 frames)."""
-        st = self._stream(sid)
-        if st.fed < MIN_FRAMES:
-            raise ValueError(f'the spectrogram stream ended after {st.fed} frames; Griffin-Lim needs at least {MIN_FRAMES}')
-        st.ended = True
 
     def _committed_after(self, st):
         """Frames committed once the next run() has processed every ready frame."""
@@ -220,14 +152,17 @@ class GriffinLimStreamPool:
             return self.v.hop * (st.fed - 1)
         return max(0, committed * self.v.hop - self.v.N // 2)
 
-    def _busy(self, st):
+    def _pending(self, st):
         return st.fed > st.sent or self._released(st, self._committed_after(st)) > st.released
+
+    def _busy(self):
+        return any(self._pending(st) for st in self.streams.values())
 
     def run(self):
         """Processes every ready frame of every stream -> {sid: the waveform chunk it releases}."""
         order = sorted(self.streams, key=lambda s: self.streams[s].slot)
         resets = [self.streams[s].slot for s in order if self.streams[s].fresh]
-        work = [s for s in order if self._busy(self.streams[s])]
+        work = [s for s in order if self._pending(self.streams[s])]
         if not resets and not work:
             return {}
         rows, logs, spans = [], [], {}
@@ -261,6 +196,5 @@ class GriffinLimStreamPool:
             if n:
                 out[sid] = wave[off:off + n]
             if st.ended and m1 == st.fed:
-                self.slots[st.slot] = None
-                del self.streams[sid]
+                self.close(sid)
         return out

@@ -13,7 +13,7 @@ from typing import Union
 
 from .griffinlim import GriffinLimVocoder
 from .tacotron2 import MAX_STREAM_TEXTS, Tacotron, _check_batch_inputs
-from .wavernn import FoldedStreamPool, WaveRNN
+from .wavernn import WaveRNN
 
 Vocoder = Union[WaveRNN, GriffinLimVocoder]
 
@@ -94,7 +94,7 @@ class SpeechServer:
                  generator=None, target=None, overlap=None):
         self.decoder = tacotron.decoder_pool(max_streams, chunk_frames)
         self.pool = wavernn.stream_pool(max_streams, preemphasis, generator, target, overlap)
-        self.wavernn, self.mel_transform = wavernn, mel_transform
+        self.mel_transform = mel_transform
         self.requests = {}                     # id -> _Request, queued or admitted
         self.pending, self.failed = [], {}
         self.next_id = 0
@@ -106,10 +106,8 @@ class SpeechServer:
     def submit(self, text, speaker=None, language=None, seed=None, masks=None, uniforms=None):
         """Queues a request -> its id.  Its inputs are checked now (ValueError)."""
         self.decoder.check(text, speaker, language, seed, masks)
-        if isinstance(self.pool, FoldedStreamPool):
-            self.wavernn._check_stream_tape(uniforms, self.pool.fold_len)
-        else:
-            self.wavernn._check_stream_tape(uniforms)
+        if uniforms is not None:
+            self.pool.check_tape(uniforms)
         rid = self.next_id
         self.next_id += 1
         self.requests[rid] = _Request(text, speaker, language, seed, masks, uniforms)

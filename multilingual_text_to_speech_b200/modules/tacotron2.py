@@ -19,6 +19,7 @@ from .layers import ZoneoutLSTMCell, DropoutLSTMCell, ConvBlock
 from .attention import LocationSensitiveAttention, ForwardAttention
 from .encoder import Encoder, MultiEncoder, ConditionalEncoder, ConvolutionalEncoder, GeneratedConvolutionalEncoder
 from .classifier import ReversalClassifier
+from .stream_pool import check_seed
 
 
 class Prenet(torch.nn.Module):
@@ -725,9 +726,7 @@ class DecoderPool:
             device = self.t._embedding.weight.device
             return 'tape', {k: v.to(device=device, dtype=torch.uint8).contiguous() for k, v in masks.items()}
         if seed is not None:
-            if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= int(seed) < 1 << 64:
-                raise ValueError(f'a seed is an int in [0, 2^64) (got {seed!r})')
-            return 'seed', int(seed)
+            return 'seed', check_seed(seed)
         return 'shared', None
 
     def open(self, text, speaker=None, language=None, seed=None, masks=None):

@@ -18,6 +18,7 @@ Stages of forward (training, with autograd):
     stage; conv_out and every linear layer on the library GEMM; the aux stretch and the mel path's layers with their library adjoints;
   * both GRUs on the persistent fp32 sequence loops (b200tts_gru_seq_forward / _backward);
   * wavernn_loss: one fused kernel per mode writes the loss and d logits."""
+import collections
 import contextlib
 
 import numpy as np
@@ -26,6 +27,7 @@ from torch import nn
 
 from .. import _lib
 from .. import functional as F
+from .stream_pool import Stream, VocoderStreamPool, check_preemphasis, cuda_device, generate_stream as _generate_stream
 
 # fp32 bytes of the conditioning products and folded features held at once: bounds the chunk of loop steps
 COND_BYTES = 512 << 20
@@ -392,18 +394,10 @@ class WaveRNN(nn.Module):
         specs, as_numpy = self._check_mels(mels)
         frames = [int(s.shape[1]) for s in specs]
         tapes = self._check_uniforms(uniforms, frames, target, overlap)
-        if not -1.0 < float(preemphasis) < 1.0:
-            raise ValueError(f'preemphasis {preemphasis} must lie in (-1, 1)')
-        device = next((s.device for s in specs if s.is_cuda), None)
-        if device is None:
-            device = torch.device('cuda', torch.cuda.current_device()) if torch.cuda.is_available() else torch.device('cuda')
-        precision = _lib.get_precision()
-        try:
-            _lib.set_precision('fp32')
-            with torch.cuda.device(device), torch.no_grad():
-                wave, wave_off = self._generate(specs, frames, tapes, target, overlap, generator, device, preemphasis=float(preemphasis))
-        finally:
-            _lib.set_precision(precision)
+        preemphasis = check_preemphasis(preemphasis)
+        device = next((s.device for s in specs if s.is_cuda), None) or cuda_device()
+        with _fp32_context(device):
+            wave, wave_off = self._generate(specs, frames, tapes, target, overlap, generator, device, preemphasis=preemphasis)
         out = []
         for i, f in enumerate(frames):
             w = wave[int(wave_off[i]): int(wave_off[i]) + (f - 1) * self.hop_length]
@@ -414,6 +408,9 @@ class WaveRNN(nn.Module):
         return out
 
     # ---- streaming ----
+    min_stream_frames = 21          # the 20-hop fade-out
+    short_stream = 'the mel stream ended after {} frames; the 20-hop fade-out needs at least 21'
+
     def generate_stream(self, mel_chunks, uniforms=None, generator=None, preemphasis=0.0, target=None, overlap=None):
         """Streaming form of generate(mel, target=F hop, overlap=0), fatchord's unbatched generation: mel_chunks is an iterable of
         [feat_dims, n_k] mels (n_k >= 0, as given: no normalisation), whose concatenation is the mel of F >= 21 frames; yields waveform
@@ -431,29 +428,8 @@ class WaveRNN(nn.Module):
         uniforms [folds, target + 2 overlap, U] (fold k step j reads uniforms[k, j]); preemphasis de-emphasises each fold from a zero state,
         within generate_batch's bound."""
         if target is None and overlap is None:
-            if not -1.0 < float(preemphasis) < 1.0:
-                raise ValueError(f'preemphasis {preemphasis} must lie in (-1, 1)')
-            uniforms = self._check_stream_tape(uniforms)
-        pool = sid = fmt = None
-        for i, chunk in enumerate(mel_chunks):
-            spec, as_numpy = self._check_chunk(chunk, i)
-            if pool is None:
-                device = spec.device if spec.is_cuda else (torch.device('cuda', torch.cuda.current_device()) if torch.cuda.is_available()
-                                                           else torch.device('cuda'))
-                fmt = (as_numpy, not as_numpy and spec.is_cuda)
-                with torch.cuda.device(device):
-                    pool = self.stream_pool(1, preemphasis, generator, target, overlap)
-                sid = pool.open(uniforms)
-            if spec.shape[1]:
-                pool.feed(sid, spec)
-                for w in pool.drain():
-                    yield _as_input(w[sid], *fmt)
-        if pool is None or pool.streams[sid].frames < 21:
-            raise ValueError(f'the mel stream ended after {0 if pool is None else pool.streams[sid].frames} frames; the 20-hop fade-out needs '
-                             f'at least 21')
-        pool.end(sid)
-        for w in pool.drain():
-            yield _as_input(w[sid], *fmt)
+            self._check_stream_tape(uniforms)          # before the pool's device work
+        yield from _generate_stream(self, mel_chunks, uniforms, generator, preemphasis, target, overlap, 0)
 
     def stream_pool(self, max_streams, preemphasis=0.0, generator=None, target=None, overlap=None):
         """A StreamPool of up to max_streams (1 to 64) concurrent generate_stream-like streams sharing one sample loop; with target and
@@ -505,7 +481,7 @@ class WaveRNN(nn.Module):
         return t, as_numpy
 
     def _check_stream_tape(self, uniforms, fold_len=None):
-        """A stream's uniform tape: [1, steps, U], or with fold_len (a folded stream) [folds, fold_len, U]."""
+        """A stream's uniform tape as a tensor, or None: [1, steps, U], or with fold_len (a folded stream) [folds, fold_len, U]."""
         if uniforms is None:
             return None
         u = torch.as_tensor(np.asarray(uniforms) if not isinstance(uniforms, torch.Tensor) else uniforms)
@@ -656,32 +632,26 @@ class WaveRNN(nn.Module):
             dev(mel_off)
         fshape = _lib.WaveRNNFoldShape(len(frames), rows, self.feat_dims, 4 * self.aux_dims, hop, self.pad, self.upsample_factors[-1], target,
                                        overlap, max(frames))
-        fir = self.upsample.up_layers[-1].weight.detach().reshape(-1).float().contiguous().to(device)
         U = self.uniforms_per_step()
         if tapes is None:
             uni = torch.rand(rows, L, U, device=device, dtype=torch.float32, generator=generator)
         else:
             uni = torch.cat([t.to(device=device, dtype=torch.float32) for t in tapes]).contiguous()
-        w = self.loop_weights(device)
-        shape = _lib.WaveRNNShape(rows, self.rnn_dims, self.fc_dims, self.n_classes, _lib.WAVERNN_MODES[self.mode], L)
-        ws = F.wavernn_workspace(shape, device)
-        params = F.wavernn_params(w)
-        F.wavernn_prepare(shape, params, ws)
+        loop = _SampleLoop(self, rows, L, device)
         y = torch.empty(rows, L, device=device, dtype=torch.float32)
         S = self.chunk_steps(rows, L)
         for t0 in range(0, L, S):
             n = min(S, L - t0)
-            feat = F.wavernn_fold(fshape, mel_up, mel_off_d, frames_d, row_utt_d, row_fold_d, fir, aux, t0, n)
-            cond = self.conditioning(w, feat)
+            feat = F.wavernn_fold(fshape, mel_up, mel_off_d, frames_d, row_utt_d, row_fold_d, loop.firs[-1], aux, t0, n)
+            cond = self.conditioning(loop.w, feat)
             dbg = None if trace is None or trace.get('dbg') is None else trace['dbg'][t0:t0 + n]
-            F.wavernn_run(shape, params, cond, t0, n, uni, y, ws, dbg)
+            F.wavernn_run(loop.shape, loop.params, cond, t0, n, uni, y, loop.ws, dbg)
             if trace is not None and t0 == 0:
                 trace.update(feat=feat, cond=cond, chunk=n)
-        if F.wavernn_aborted(shape, ws):
-            raise _lib.B200TTSError('wavernn: the sample loop timed out at a grid barrier')
+        _check_loop(loop.shape, loop.ws)
         wave, wave_off = self.postprocess(y, frames, target, overlap, preemphasis)
         if trace is not None:
-            trace.update(folded=y, uniforms=uni, weights=w, row_off=row_off, wave_off=wave_off, mel_up=mel_up, mel_off=mel_off, aux=aux)
+            trace.update(folded=y, uniforms=uni, weights=loop.w, row_off=row_off, wave_off=wave_off, mel_up=mel_up, mel_off=mel_off, aux=aux)
         return wave, wave_off
 
     def postprocess(self, y, frames, target, overlap, preemphasis=0.0):
@@ -699,30 +669,199 @@ class WaveRNN(nn.Module):
         return wave, wave_off
 
 
-def _as_input(wave, as_numpy, on_cuda):
-    if as_numpy:
-        return wave.cpu().numpy()
-    return wave if on_cuda else wave.cpu()
+@contextlib.contextmanager
+def _fp32_context(device):
+    """The sample loop's context: fp32 precision mode (restored after), `device` current, no autograd."""
+    precision = _lib.get_precision()
+    try:
+        _lib.set_precision('fp32')
+        with torch.cuda.device(device), torch.no_grad():
+            yield
+    finally:
+        _lib.set_precision(precision)
 
 
-class _PoolStream:
-    """One stream of a StreamPool: its loop row, the mel frames that have arrived, its uniform tape (fp32 on the device, or None), the steps
-    run and the samples released.  Its run but unreleased samples [released, steps) sit in the pool's per-row ring buffer."""
+def _check_loop(shape, ws):
+    """Reads a sample loop's abort flag (a synchronising read)."""
+    if F.wavernn_aborted(shape, ws):
+        raise _lib.B200TTSError('wavernn: the sample loop timed out at a grid barrier')
 
-    def __init__(self, slot, device, feat_dims, tape, seed=None):
-        self.slot, self.tape, self.seed = slot, tape, seed
+
+def _upload(a, device):
+    return torch.from_numpy(np.ascontiguousarray(a)).to(device)
+
+
+# One row of a loop call: its loop row `slot`, the mel of its stream (`ended`: the whole mel), the n sample positions [t, t + n) it runs,
+# the steps it has run (the loop's per-row parity), and its uniforms: uni [n, U] from a tape, else draws from `seed` at draw0, else None
+# (drawn for the call)
+_Row = collections.namedtuple('_Row', 'slot mel ended t n steps uni seed draw0')
+
+
+class _SampleLoop:
+    """WaveRNN's sample loop on `device`: the loop weights, shape, workspace and parameters of `rows` rows of up to `steps` steps per call,
+    the mel-path FIRs, and, with preemphasis, each row's last de-emphasised sample.  generate_batch runs it over its fold rows with
+    b200tts_wavernn_run, then _check_loop; the stream pools through step_rows, which computes each row's windowed features itself."""
+
+    def __init__(self, model, rows, steps, device, preemphasis=0.0, generator=None):
+        self.m, self.device, self.a, self.generator = model, device, preemphasis, generator
+        self.mu = model.n_classes - 1 if model.mode == 'RAW' else 0
+        self.out_mu = 0 if preemphasis else self.mu          # the mu-law step_rows' samples still carry: the de-emphasis decodes it
+        self.w = model.loop_weights(device)
+        self.shape = _lib.WaveRNNShape(rows, model.rnn_dims, model.fc_dims, model.n_classes, _lib.WAVERNN_MODES[model.mode], steps)
+        self.ws = F.wavernn_workspace(self.shape, device)
+        self.params = F.wavernn_params(self.w)
+        F.wavernn_prepare(self.shape, self.params, self.ws)
+        self.firs = [c.weight.detach().reshape(-1).to(device, torch.float32).contiguous() for c in model.upsample.up_layers[1::2]]
+        self.last = torch.zeros(rows, device=device, dtype=torch.float32) if preemphasis else None
+
+    def reset(self, slots):
+        """Resets loop rows `slots` for new rows."""
+        F.wavernn_reset_rows(self.shape, self.ws, slots)
+        if self.a:
+            self.last[_upload(np.array(slots, np.int64), self.device)] = 0.0
+
+    def step_rows(self, rows):
+        """One loop call over `rows` (_Row, sorted by slot) -> (y [active, nmax], de-emphasised with preemphasis, active, nmax)."""
+        m, dev, U = self.m, self.device, self.m.uniforms_per_step()
+        active = rows[-1].slot + 1
+        nmax = max(r.n for r in rows)
+        feat = self.features(rows, active, nmax)
+        cond = m.conditioning(self.w, feat)
+        slot = np.array([r.slot for r in rows], np.int64)
+        n = np.array([r.n for r in rows], np.int64)
+        # uniforms: the taped rows' steps gathered from their tapes (source 0 is a zero) and the seeded rows' from one seeded draw, in one
+        # gather; the other rows' drawn for the call
+        taped = [r for r in rows if r.uni is not None]
+        seeded = [r for r in rows if r.uni is None and r.seed is not None]
+        if taped or seeded:
+            parts = [torch.zeros(1, device=dev)] + [r.uni.reshape(-1) for r in taped]
+            if seeded:
+                parts.append(F.fill_uniform_rows(nmax, U, [r.seed for r in seeded], [r.draw0 for r in seeded], _lib.SEED_STREAMS['vocoder'],
+                                                 dev).reshape(-1))
+            src = torch.cat(parts)
+            idx = np.zeros((active, nmax, U), np.int64)
+            off = 1
+            i = np.arange(nmax)[:, None] * U + np.arange(U)[None, :]
+            for r in taped:
+                idx[r.slot, :r.n] = off + i[:r.n]
+                off += r.n * U
+            for r in seeded:
+                idx[r.slot, :r.n] = off + i[:r.n]
+                off += nmax * U
+            uni = src[_upload(idx, dev)]
+        if len(taped) + len(seeded) < len(rows):
+            drawn = torch.rand(active, nmax, U, device=dev, dtype=torch.float32, generator=self.generator)
+            if taped or seeded:
+                has = np.zeros((active, 1, 1), bool)
+                has[[r.slot for r in taped + seeded]] = True
+                uni = torch.where(_upload(has, dev), uni, drawn)
+            else:
+                uni = drawn
+        y = torch.zeros(active, nmax, device=dev, dtype=torch.float32)
+        if self.shape.rows == 1:
+            # a one-row loop: the loop without per-row budgets runs row 0 bit for bit as run_rows does (it runs every row of the shape,
+            # so it serves only a loop of one row)
+            F.wavernn_run_stream(self.shape, self.params, cond, rows[0].steps, nmax, uni, y, self.ws)
+        else:
+            row_t, row_n = np.zeros(active, np.int64), np.zeros(active, np.int32)
+            row_t[slot], row_n[slot] = [r.steps for r in rows], n
+            F.wavernn_run_rows(self.shape, self.params, cond, _upload(row_t, dev), _upload(row_n, dev), nmax, uni, y, self.ws)
+        if self.a:
+            if self.mu:
+                y = F.wavernn_deemphasis(y, self.mu, 0.0)                    # a = 0: the mu-law decode only
+            y = F.wavernn_deemphasis(torch.cat([self.last[:active, None], y], 1).contiguous(), 0, self.a)[:, 1:]
+            sl = _upload(slot, dev)
+            self.last[sl] = y[sl, _upload(n - 1, dev)]
+        return y, active, nmax
+
+    def window_layout(self, rows):
+        """The host side of features: (sources [(row index, frame0, frame1)] packed side by side, then a zero column; the gather index of
+        the packed mel-path windows followed by the padded MelResNet batch; window lengths; MelResNet widths and batch width; window-row
+        descriptors without the aux width, as (slot, frames or 0, m0, mel_len, a0, aux_len, s0, mel_off, aux_off / aux width, n))."""
+        m = self.m
+        p, hop, s_last, C = m.pad, m.hop_length, m.upsample_factors[-1], m.feat_dims
+        srcs, wins, res = [], [], []
+        for b, r in enumerate(rows):
+            frames = int(r.mel.shape[1])
+            (P0, P1), (r0, r1), _ = m.window_plan(r.t, r.t + r.n, frames, r.ended)
+            lo, hi = max(P0, p), min(P1, frames + p)
+            wins.append((P0, P1, lo, hi))
+            res.append((r0, r1))
+            srcs.append((b, lo - p, max(hi, lo) - p))
+        srcs += [(b, r0, r1) for b, (r0, r1) in enumerate(res)]
+        off = np.concatenate([[0], np.cumsum([c - a for _, a, c in srcs])])
+        Wt = int(off[-1]) + 1                       # the last column is zero
+        c = np.arange(C)[:, None] * Wt
+        parts, lens, desc, mel_off = [], [], [], 0
+        for b, (P0, P1, lo, hi) in enumerate(wins):
+            P = np.arange(P0, P1)
+            col = np.where((P >= lo) & (P < hi), off[b] + P - lo, Wt - 1)
+            parts.append((c + col[None, :]).reshape(-1))
+            lens.append(P1 - P0)
+        widths = [r1 - r0 for r0, r1 in res]
+        W = max(widths)
+        w = np.arange(W)[None, :]
+        col = np.where(w < np.array(widths)[:, None], off[len(rows):-1, None] + w, Wt - 1)
+        parts.append((c[None, :, :] + col[:, None, :]).reshape(-1))
+        scale = int(np.prod(m.upsample_factors[:-1]))
+        for b, r in enumerate(rows):
+            P0, r0 = wins[b][0], res[b][0]
+            desc.append((r.slot, int(r.mel.shape[1]) if r.ended else 0, P0 * (hop // s_last), lens[b] * scale, r0, widths[b], r.t, mel_off,
+                         b * W, r.n))
+            mel_off += C * lens[b] * scale
+        return srcs, np.concatenate(parts), lens, widths, W, desc
+
+    def features(self, rows, active, nmax):
+        """Loop features [nmax, active, feat_dims + res_out_dims] of every row's positions, in a fixed number of launches: one gather of
+        every window, the mel-path layers on the packed windows, the MelResNet over the padded batch of windows, one window-rows launch."""
+        m, dev = self.m, self.device
+        p, hop, s_last, C = m.pad, m.hop_length, m.upsample_factors[-1], m.feat_dims
+        srcs, idx, lens, widths, W, desc = self.window_layout(rows)
+        packed = torch.cat([rows[b].mel[:, a:c] for b, a, c in srcs] + [torch.zeros(C, 1, device=dev)], dim=1)
+        g = packed.reshape(-1)[_upload(idx, dev)]
+        nw = C * sum(lens)
+        x, batch = g[:nw], g[nw:].view(len(rows), C, W)
+        for j, scale in enumerate(m.upsample_factors[:-1]):
+            x = F.wavernn_upsample_segments(x, lens, self.firs[j], scale)
+            lens = [ln * scale for ln in lens]
+        aux = m._resnet(batch, widths, dev)
+        A = aux.shape[2]
+        blank = _lib.WaveRNNWindowShape(C, A, hop, p, s_last, 0, 0, 1, 0, 0)
+        win = [_lib.WaveRNNWindowRow(blank, 0, 0, 0, 0) for _ in range(active)]
+        for slot, frames, m0, mel_len, a0, aux_len, s0, mel_off, aux_row, n in desc:
+            shape = _lib.WaveRNNWindowShape(C, A, hop, p, s_last, frames, m0, mel_len, a0, aux_len)
+            win[slot] = _lib.WaveRNNWindowRow(shape, s0, mel_off, aux_row * A, n)
+        return F.wavernn_window_rows(win, nmax, x, self.firs[-1], aux)
+
+
+class _MelStream(Stream):
+    """One WaveRNN stream: the mel frames that have arrived (fp32 on the pool's device), its uniform tape (fp32 on the device, or None)
+    and its seed (or None)."""
+
+    def __init__(self, device, feat_dims, tape, seed):
+        super().__init__()
         self.mel = torch.zeros(feat_dims, 0, device=device, dtype=torch.float32)
-        self.chunks = 0
-        self.steps = 0
-        self.released = 0
-        self.ended = False
+        self.tape, self.seed = tape, seed
 
     @property
     def frames(self):
         return int(self.mel.shape[1])
 
+    def append(self, spec):
+        self.mel = torch.cat([self.mel, spec.to(device=self.mel.device, dtype=torch.float32)], dim=1)
 
-class StreamPool:
+
+class _PoolStream(_MelStream):
+    """One stream of a StreamPool: its loop row and the steps it has run.  Its run but unreleased samples [released, steps) sit in the
+    pool's per-row ring buffer."""
+
+    def __init__(self, slot, device, feat_dims, tape, seed=None):
+        super().__init__(device, feat_dims, tape, seed)
+        self.slot = slot
+        self.steps = 0
+
+
+class StreamPool(VocoderStreamPool):
     """Concurrent streaming generation: up to max_streams streams, each a generate_stream, advance together in one sample loop whose rows
     run independently (b200tts_wavernn_run_rows; a one-stream pool, whose loop has one row, runs b200tts_wavernn_run_stream, the loop
     without per-row budgets, bit for bit the same).  open() takes the lowest free row and resets it; feed() and end() add a stream's mel
@@ -735,100 +874,44 @@ class StreamPool:
     joined, whatever else shares the loop and however its mel was chunked.  With preemphasis the stream is de-emphasised across calls and
     stays within generate_batch's bound.  Without a tape the uniforms are drawn with torch.rand (`generator` optional) once per call for all
     rows, so they differ from a solo run's draws; a stream opened with a seed draws its own (b200tts_fill_uniform_rows at its own step count,
-    stream _lib.SEED_STREAMS['vocoder']), which depend on the seed alone: its tape is one fill_uniform_rows row over [0, T).  Every call runs in fp32 (the precision mode is set for the call and restored after it)
-    on the CUDA device that was current when the pool was made; each run() reads the loop's abort flag once.  The device work of a run()
-    is a fixed number of launches whatever the number of streams: the per-stream windows, tapes and samples are gathered and scattered
-    with indices built on the host."""
+    stream _lib.SEED_STREAMS['vocoder']), which depend on the seed alone: its tape is one fill_uniform_rows row over [0, T).  Every call runs
+    in fp32 (the precision mode is set for the call and restored after it) on the CUDA device that was current when the pool was made; each
+    run() reads the loop's abort flag once.  The device work of a run() is a fixed number of launches whatever the number of streams: the
+    per-stream windows, tapes and samples are gathered and scattered with indices built on the host."""
 
     def __init__(self, model, max_streams, preemphasis=0.0, generator=None):
-        if not 1 <= int(max_streams) <= _lib.WAVERNN_MAX_STREAMS:
-            raise ValueError(f'a stream pool holds 1 to {_lib.WAVERNN_MAX_STREAMS} streams (got {max_streams})')
-        if not -1.0 < float(preemphasis) < 1.0:
-            raise ValueError(f'preemphasis {preemphasis} must lie in (-1, 1)')
-        self.m, self.a, self.generator = model, float(preemphasis), generator
-        self.device = torch.device('cuda', torch.cuda.current_device()) if torch.cuda.is_available() else torch.device('cuda')
-        self.rows = int(max_streams)
+        super().__init__(model, max_streams, preemphasis)
         self.hop, self.lookahead = model.hop_length, model.lookahead()
-        self.mu = model.n_classes - 1 if model.mode == 'RAW' else 0
         self.slots = [None] * self.rows          # sid of the stream on each row
-        self.streams = {}
-        self.next_sid = 0
+        # a lone stream runs all its ready steps in one call (up to COND_BYTES): each call costs 3 to 4 ms outside the loop, and no other
+        # stream waits on it
+        S = model.chunk_steps(self.rows, 1 << 30)
+        self.S = S if self.rows == 1 else min(POOL_CALL_HOPS * self.hop, S)
+        # per-row ring of the samples run but not released: at most 20 held-back hops, the partial hop and one call's steps
+        self.P = self.S + 22 * self.hop
         with self._fp32():
-            self.w = model.loop_weights(self.device)
-            # a lone stream runs all its ready steps in one call (up to COND_BYTES): each call costs 3 to 4 ms outside the loop, and no other
-            # stream waits on it
-            S = model.chunk_steps(self.rows, 1 << 30)
-            self.S = S if self.rows == 1 else min(POOL_CALL_HOPS * self.hop, S)
-            self.shape = _lib.WaveRNNShape(self.rows, model.rnn_dims, model.fc_dims, model.n_classes, _lib.WAVERNN_MODES[model.mode], self.S)
-            self.ws = F.wavernn_workspace(self.shape, self.device)
-            self.params = F.wavernn_params(self.w)
-            F.wavernn_prepare(self.shape, self.params, self.ws)
-            fir = lambda j: model.upsample.up_layers[2 * j + 1].weight.detach().reshape(-1).to(self.device, torch.float32).contiguous()  # noqa
-            self.firs = [fir(j) for j in range(len(model.upsample_factors))]
-            self.last = torch.zeros(self.rows, device=self.device, dtype=torch.float32)     # each row's last de-emphasised sample
-            # per-row ring of the samples run but not released: at most 20 held-back hops, the partial hop and one call's steps
-            self.P = self.S + 22 * self.hop
+            self.loop = _SampleLoop(model, self.rows, self.S, self.device, self.a, generator)
             self.ring = torch.zeros(self.rows * self.P + 2, device=self.device, dtype=torch.float32)   # + a write sink and a zero
+        self.shape, self.ws = self.loop.shape, self.loop.ws          # read by the abort check after each run()
 
-    @contextlib.contextmanager
     def _fp32(self):
-        precision = _lib.get_precision()
-        try:
-            _lib.set_precision('fp32')
-            with torch.cuda.device(self.device), torch.no_grad():
-                yield
-        finally:
-            _lib.set_precision(precision)
+        return _fp32_context(self.device)
 
-    def open(self, uniforms=None, seed=None):
-        """A new stream on the lowest free row -> its id.  uniforms: its tape [1, T, U] as for generate_stream, or None; seed (an int in
-        [0, 2^64), used without a tape): the stream draws its uniforms from it."""
-        tape = self.m._check_stream_tape(uniforms)
-        if seed is not None and (isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= int(seed) < 1 << 64):
-            raise ValueError(f'a seed is an int in [0, 2^64) (got {seed!r})')
-        free = [r for r in range(self.rows) if self.slots[r] is None]
-        if not free:
-            raise ValueError(f'the stream pool is full: {self.rows} streams are open')
-        slot, sid = free[0], self.next_sid
+    def check_tape(self, uniforms):
+        """A stream's tape [1, T, U] as for generate_stream, or None."""
+        return self.v._check_stream_tape(uniforms)
+
+    def _open(self, sid, tape, seed):
+        slot = self.slots.index(None)
         with self._fp32():
-            F.wavernn_reset_rows(self.shape, self.ws, [slot])
-            self.last[slot] = 0.0
+            self.loop.reset([slot])
             if tape is not None:
                 tape = tape[0].to(device=self.device, dtype=torch.float32).contiguous()
-            self.streams[sid] = _PoolStream(slot, self.device, self.m.feat_dims, tape, None if seed is None else int(seed))
         self.slots[slot] = sid
-        self.next_sid += 1
-        return sid
+        return _PoolStream(slot, self.device, self.v.feat_dims, tape, seed)
 
-    def close(self, sid):
-        """Drops stream sid and frees its row at once, whatever it has run or released."""
-        st = self.streams.pop(sid, None)
-        if st is None:
-            raise ValueError(f'unknown or finished stream {sid}')
+    def _drop(self, st):
         self.slots[st.slot] = None
-
-    def _stream(self, sid):
-        st = self.streams.get(sid)
-        if st is None:
-            raise ValueError(f'unknown or finished stream {sid}')
-        if st.ended:
-            raise ValueError(f'stream {sid} has ended')
-        return st
-
-    def feed(self, sid, mel_chunk):
-        """Appends mel frames [feat_dims, n] (n >= 0, as given) to stream sid."""
-        st = self._stream(sid)
-        spec, _ = self.m._check_chunk(mel_chunk, st.chunks)
-        st.chunks += 1
-        if spec.shape[1]:
-            st.mel = torch.cat([st.mel, spec.to(device=self.device, dtype=torch.float32)], dim=1)
-
-    def end(self, sid):
-        """Marks the end of stream sid's mel (at least 21 frames)."""
-        st = self._stream(sid)
-        if st.frames < 21:
-            raise ValueError(f'the mel stream ended after {st.frames} frames; the 20-hop fade-out needs at least 21')
-        st.ended = True
 
     def plan(self):
         """{sid: (steps run, steps of the next call)} for every stream with ready samples."""
@@ -868,168 +951,36 @@ class StreamPool:
             if plan:
                 self._loop(plan)
             released = self._release()
-            if F.wavernn_aborted(self.shape, self.ws):
-                raise _lib.B200TTSError('wavernn: the sample loop timed out at a grid barrier')
+            _check_loop(self.shape, self.ws)
         for sid in released:
             st = self.streams[sid]
             if st.ended and st.released == (st.frames - 1) * self.hop:
-                self.slots[st.slot] = None
-                del self.streams[sid]
+                self.close(sid)
         return released
-
-    def drain(self):
-        """Runs until no stream has steps left to run -> the non-empty {sid: chunk} results, in order."""
-        out = []
-        while True:
-            busy = self._busy()
-            r = self.run()
-            if r:
-                out.append(r)
-            if not busy:
-                return out
 
     def _busy(self):
         return bool(self.plan())
 
-    def _upload(self, a):
-        return torch.from_numpy(np.ascontiguousarray(a)).to(self.device)
+    def _loop_rows(self, plan):
+        """The loop rows of the streams in plan, by slot."""
+        rows = []
+        for sid in sorted(plan, key=lambda s: self.streams[s].slot):
+            st, (t, n) = self.streams[sid], plan[sid]
+            rows.append(_Row(st.slot, st.mel, st.ended, t, n, t, None if st.tape is None else st.tape[t:t + n], st.seed, t))
+        return rows
 
     def _loop(self, plan):
-        live = sorted(plan, key=lambda sid: self.streams[sid].slot)
-        steps = {sid: plan[sid][0] for sid in live}
-        y, active, nmax = self._step_rows(live, self.streams, plan, steps, lambda sid, t, n: self.streams[sid].tape[t:t + n], steps)
-        slot = np.array([self.streams[sid].slot for sid in live], np.int64)
+        rows = self._loop_rows(plan)
+        y, active, nmax = self.loop.step_rows(rows)
         row_t, row_n = np.zeros(active, np.int64), np.zeros(active, np.int32)
-        row_t[slot] = [plan[sid][0] for sid in live]
-        row_n[slot] = [plan[sid][1] for sid in live]
+        row_t[[r.slot for r in rows]] = [r.t for r in rows]
+        row_n[[r.slot for r in rows]] = [r.n for r in rows]
         # into the ring: row r's step i at slot r P + (row_t + i) mod P; steps past a row's budget go to the sink
         i = np.arange(nmax)[None, :]
         dst = np.where(i < row_n[:, None], np.arange(active)[:, None] * self.P + (row_t[:, None] + i) % self.P, self.rows * self.P)
-        self.ring.index_put_((self._upload(dst.reshape(-1)),), y.reshape(-1))
-        for sid in live:
-            self.streams[sid].steps += plan[sid][1]
-
-    def _step_rows(self, live, rows, plan, steps, tape_of, draw0):
-        """One loop call over the rows `live` (keys of `rows`, whose entries have slot, mel, frames, ended, tape and seed), sorted by slot:
-        row k runs the features of positions plan[k] = (t, n) from its own steps[k] steps (the loop's slot parity), reading the uniforms
-        tape_of(k, steps[k], n) [n, U] of a taped row, or draws from draw0[k] of a seeded row's stream.  -> (y [active, nmax], de-emphasised
-        with preemphasis, active, nmax); self.last carries each row's last de-emphasised sample."""
-        m, dev, U = self.m, self.device, self.m.uniforms_per_step()
-        active = rows[live[-1]].slot + 1
-        nmax = max(plan[k][1] for k in live)
-        feat = self._features(live, plan, active, nmax, rows)
-        cond = m.conditioning(self.w, feat)
-        slot = np.array([rows[k].slot for k in live], np.int64)
-        n = np.array([plan[k][1] for k in live], np.int64)
-        # uniforms: the taped rows' steps gathered from their tapes (source 0 is a zero) and the seeded rows' from one seeded draw, in one
-        # gather; the other rows' drawn for the call
-        taped = [k for k in live if rows[k].tape is not None]
-        seeded = [k for k in live if rows[k].tape is None and rows[k].seed is not None]
-        if taped or seeded:
-            parts = [torch.zeros(1, device=dev)] + [tape_of(k, steps[k], plan[k][1]).reshape(-1) for k in taped]
-            if seeded:
-                parts.append(F.fill_uniform_rows(nmax, U, [rows[k].seed for k in seeded], [draw0[k] for k in seeded],
-                                                 _lib.SEED_STREAMS['vocoder'], dev).reshape(-1))
-            src = torch.cat(parts)
-            idx = np.zeros((active, nmax, U), np.int64)
-            off = 1
-            i = np.arange(nmax)[:, None] * U + np.arange(U)[None, :]
-            for k in taped:
-                c = plan[k][1]
-                idx[rows[k].slot, :c] = off + i[:c]
-                off += c * U
-            for k in seeded:
-                c = plan[k][1]
-                idx[rows[k].slot, :c] = off + i[:c]
-                off += nmax * U
-            uni = src[self._upload(idx)]
-        if len(taped) + len(seeded) < len(live):
-            drawn = torch.rand(active, nmax, U, device=dev, dtype=torch.float32, generator=self.generator)
-            if taped or seeded:
-                has = np.zeros((active, 1, 1), bool)
-                has[[rows[k].slot for k in taped + seeded]] = True
-                uni = torch.where(self._upload(has), uni, drawn)
-            else:
-                uni = drawn
-        y = torch.zeros(active, nmax, device=dev, dtype=torch.float32)
-        if self.shape.rows == 1:
-            # a one-row loop: the loop without per-row budgets runs row 0 bit for bit as run_rows does (it runs every row of the shape,
-            # so it serves only a loop of one row)
-            F.wavernn_run_stream(self.shape, self.params, cond, steps[live[0]], nmax, uni, y, self.ws)
-        else:
-            row_t, row_n = np.zeros(active, np.int64), np.zeros(active, np.int32)
-            row_t[slot], row_n[slot] = [steps[k] for k in live], n
-            F.wavernn_run_rows(self.shape, self.params, cond, self._upload(row_t), self._upload(row_n), nmax, uni, y, self.ws)
-        if self.a:
-            if self.mu:
-                y = F.wavernn_deemphasis(y, self.mu, 0.0)                    # a = 0: the mu-law decode only
-            y = F.wavernn_deemphasis(torch.cat([self.last[:active, None], y], 1).contiguous(), 0, self.a)[:, 1:]
-            sl = self._upload(slot)
-            self.last[sl] = y[sl, self._upload(n - 1)]
-        return y, active, nmax
-
-    def window_layout(self, live, plan, rows=None):
-        """The host side of _features: (sources [(sid, frame0, frame1)] packed side by side, then a zero column; the gather index of the
-        packed mel-path windows followed by the padded MelResNet batch; window lengths; MelResNet widths and batch width; window-row
-        descriptors without the aux width, as (slot, frames or 0, m0, mel_len, a0, aux_len, s0, mel_off, aux_off / aux width, n)).  rows:
-        the loop rows of the keys in `live` (default: the streams)."""
-        rows = self.streams if rows is None else rows
-        m = self.m
-        p, hop, s_last, C = m.pad, self.hop, m.upsample_factors[-1], m.feat_dims
-        srcs, wins, res = [], [], []
-        for sid in live:
-            st, (t, n) = rows[sid], plan[sid]
-            (P0, P1), (r0, r1), _ = m.window_plan(t, t + n, st.frames, st.ended)
-            lo, hi = max(P0, p), min(P1, st.frames + p)
-            wins.append((P0, P1, lo, hi))
-            res.append((r0, r1))
-            srcs.append((sid, lo - p, max(hi, lo) - p))
-        srcs += [(sid, r0, r1) for sid, (r0, r1) in zip(live, res)]
-        off = np.concatenate([[0], np.cumsum([b - a for _, a, b in srcs])])
-        Wt = int(off[-1]) + 1                       # the last column is zero
-        c = np.arange(C)[:, None] * Wt
-        parts, lens, desc, mel_off = [], [], [], 0
-        for b, (sid, (P0, P1, lo, hi)) in enumerate(zip(live, wins)):
-            P = np.arange(P0, P1)
-            col = np.where((P >= lo) & (P < hi), off[b] + P - lo, Wt - 1)
-            parts.append((c + col[None, :]).reshape(-1))
-            lens.append(P1 - P0)
-        widths = [r1 - r0 for r0, r1 in res]
-        W = max(widths)
-        w = np.arange(W)[None, :]
-        col = np.where(w < np.array(widths)[:, None], off[len(live):-1, None] + w, Wt - 1)
-        parts.append((c[None, :, :] + col[:, None, :]).reshape(-1))
-        scale = int(np.prod(m.upsample_factors[:-1]))
-        for b, sid in enumerate(live):
-            st, (t, n) = rows[sid], plan[sid]
-            P0, r0 = wins[b][0], res[b][0]
-            desc.append((st.slot, st.frames if st.ended else 0, P0 * (hop // s_last), lens[b] * scale, r0, widths[b], t, mel_off, b * W, n))
-            mel_off += C * lens[b] * scale
-        return srcs, np.concatenate(parts), lens, widths, W, desc
-
-    def _features(self, live, plan, active, nmax, rows=None):
-        """Loop features [nmax, active, feat_dims + res_out_dims] of every live stream's next steps, in a fixed number of launches: one
-        gather of every window, the mel-path layers on the packed windows, the MelResNet over the padded batch of windows, one
-        window-rows launch."""
-        m, dev = self.m, self.device
-        p, hop, s_last, C = m.pad, self.hop, m.upsample_factors[-1], m.feat_dims
-        rows = self.streams if rows is None else rows
-        srcs, idx, lens, widths, W, desc = self.window_layout(live, plan, rows)
-        packed = torch.cat([rows[sid].mel[:, a:b] for sid, a, b in srcs] + [torch.zeros(C, 1, device=dev)], dim=1)
-        g = packed.reshape(-1)[self._upload(idx)]
-        nw = C * sum(lens)
-        x, batch = g[:nw], g[nw:].view(len(live), C, W)
-        for j, scale in enumerate(m.upsample_factors[:-1]):
-            x = F.wavernn_upsample_segments(x, lens, self.firs[j], scale)
-            lens = [ln * scale for ln in lens]
-        aux = m._resnet(batch, widths, dev)
-        A = aux.shape[2]
-        blank = _lib.WaveRNNWindowShape(C, A, hop, p, s_last, 0, 0, 1, 0, 0)
-        rows = [_lib.WaveRNNWindowRow(blank, 0, 0, 0, 0) for _ in range(active)]
-        for slot, frames, m0, mel_len, a0, aux_len, s0, mel_off, aux_row, n in desc:
-            shape = _lib.WaveRNNWindowShape(C, A, hop, p, s_last, frames, m0, mel_len, a0, aux_len)
-            rows[slot] = _lib.WaveRNNWindowRow(shape, s0, mel_off, aux_row * A, n)
-        return F.wavernn_window_rows(rows, nmax, x, self.firs[-1], aux)
+        self.ring.index_put_((_upload(dst.reshape(-1), self.device),), y.reshape(-1))
+        for sid, (_, n) in plan.items():
+            self.streams[sid].steps += n
 
     def _release(self):
         """Every stream's releasable samples, gathered from the ring, through one b200tts_wavernn_unfold, each stream one fold of one
@@ -1043,21 +994,21 @@ class StreamPool:
         start = np.array([self.streams[sid].released for sid, _, _ in rel])[:, None]
         n = np.array([n for _, n, _ in rel])[:, None]
         src = np.where(i < n, slot * self.P + (start + i) % self.P, self.rows * self.P + 1)
-        y = self.ring[self._upload(src)]
+        y = self.ring[_upload(src, self.device)]
         for sid, k, _ in rel:
             self.streams[sid].released += k
         wave_off = np.concatenate([[0], np.cumsum(n[:, 0])])
-        meta = self._upload(np.concatenate([[f for *_, f in rel], np.arange(len(rel) + 1), wave_off]).astype(np.int64))
+        meta = _upload(np.concatenate([[f for *_, f in rel], np.arange(len(rel) + 1), wave_off]).astype(np.int64), self.device)
         B = len(rel)
         wave = F.wavernn_unfold(y, meta[:B].int(), meta[B:2 * B + 1].int(), meta[2 * B + 1:], int(wave_off[-1]), self.hop, L, 0,
-                                0 if self.a else self.mu)
+                                self.loop.out_mu)
         return {sid: wave[int(wave_off[b]):int(wave_off[b + 1])] for b, (sid, *_) in enumerate(rel)}
 
 
 class _Fold:
-    """Fold k of a folded stream: sample positions [start, start + fold_len) with start = k (target + overlap), its loop row (None before
+    """Fold k of a folded stream st: sample positions [start, start + fold_len) with start = k (target + overlap), its loop row (None before
     its grant and once it has run every step it needs), its storage slot (None once its samples are all released) and the steps it has
-    run.  It reads the stream's mel, tape and seed, as a StreamPool row reads its stream's."""
+    run."""
 
     def __init__(self, st, k, start):
         self.st, self.k, self.start = st, k, start
@@ -1065,26 +1016,20 @@ class _Fold:
         self.steps = 0
         self.done = False
 
-    mel = property(lambda self: self.st.mel)
-    frames = property(lambda self: self.st.frames)
-    ended = property(lambda self: self.st.ended)
-    seed = property(lambda self: self.st.seed)
-    tape = property(lambda self: self.st.tape)
 
-
-class _FoldedStream(_PoolStream):
-    """One stream of a FoldedStreamPool: a _PoolStream without a row of its own; `folds` lists the folds opened so far, fold k at index k."""
+class _FoldedStream(_MelStream):
+    """One stream of a FoldedStreamPool, which has no loop row of its own: `folds` lists the folds opened so far, fold k at index k."""
 
     def __init__(self, sid, device, feat_dims, tape, seed=None):
-        super().__init__(None, device, feat_dims, tape, seed)
+        super().__init__(device, feat_dims, tape, seed)
         self.sid = sid
         self.folds = []
 
 
-class FoldedStreamPool(StreamPool):
+class FoldedStreamPool(VocoderStreamPool):
     """Folded streaming generation: up to max_streams streams, each the streaming form of generate(mel, target, overlap) (fatchord's
     folded generation, the library's default), whose folds run as rows of one 64-row sample loop (b200tts_wavernn_run_rows).  The
-    interface is StreamPool's: open / feed / end / run / close / streams.
+    interface is StreamPool's: open / feed / end / run / drain / close / streams.
 
     Fold geometry is fold_count's: with L = target + 2 overlap, fold k covers positions [k (target + overlap), k (target + overlap) + L) and
     exists iff k (target + overlap) + overlap < F hop.  While the mel arrives, fold k opens only once its existence is certain (it exists
@@ -1109,39 +1054,27 @@ class FoldedStreamPool(StreamPool):
     fold is de-emphasised across calls, within generate_batch's bound.  close() frees every row and all storage of a stream at once."""
 
     def __init__(self, model, max_streams, target, overlap, preemphasis=0.0, generator=None):
-        if not 1 <= int(max_streams) <= _lib.WAVERNN_MAX_STREAMS:
-            raise ValueError(f'a stream pool holds 1 to {_lib.WAVERNN_MAX_STREAMS} streams (got {max_streams})')
-        if target is None or overlap is None or int(target) != target or int(overlap) != overlap or target < 1 or overlap < 0:
-            raise ValueError(f'a folded stream pool needs an integer target >= 1 and overlap >= 0 (got {target!r}, {overlap!r})')
-        if not -1.0 < float(preemphasis) < 1.0:
-            raise ValueError(f'preemphasis {preemphasis} must lie in (-1, 1)')
-        self.a, self.generator = float(preemphasis), generator
         self._layout(model, max_streams, target, overlap, _lib.WAVERNN_MAX_STREAMS)
-        self.device = torch.device('cuda', torch.cuda.current_device()) if torch.cuda.is_available() else torch.device('cuda')
-        nrows, L = len(self.slots), self.fold_len
+        self.a = check_preemphasis(preemphasis)
         with self._fp32():
-            self.w = model.loop_weights(self.device)
-            self.shape = _lib.WaveRNNShape(nrows, model.rnn_dims, model.fc_dims, model.n_classes, _lib.WAVERNN_MODES[model.mode], self.S)
-            self.ws = F.wavernn_workspace(self.shape, self.device)
-            self.params = F.wavernn_params(self.w)
-            F.wavernn_prepare(self.shape, self.params, self.ws)
-            fir = lambda j: model.upsample.up_layers[2 * j + 1].weight.detach().reshape(-1).to(self.device, torch.float32).contiguous()  # noqa
-            self.firs = [fir(j) for j in range(len(model.upsample_factors))]
-            self.last = torch.zeros(nrows, device=self.device, dtype=torch.float32)      # each row's last de-emphasised sample
-            self.store = torch.zeros(self.nstore * L + 1, device=self.device, dtype=torch.float32)     # + a write sink
+            self.loop = _SampleLoop(model, len(self.slots), self.S, self.device, self.a, generator)
+            self.store = torch.zeros(self.nstore * self.fold_len + 1, device=self.device, dtype=torch.float32)     # + a write sink
+        self.shape, self.ws = self.loop.shape, self.loop.ws          # read by the abort check after each run()
+
+    def _fp32(self):
+        return _fp32_context(self.device)
 
     def _layout(self, model, max_streams, target, overlap, nrows):
-        """The host state of a pool with nrows loop rows: geometry, rows, streams and storage slots (ValueError past COND_BYTES)."""
-        self.m = model
+        """The host state of a pool with nrows loop rows: the checks but preemphasis, geometry, rows, streams and storage slots
+        (ValueError past COND_BYTES)."""
+        super().__init__(model, max_streams)
+        if target is None or overlap is None or int(target) != target or int(overlap) != overlap or target < 1 or overlap < 0:
+            raise ValueError(f'a folded stream pool needs an integer target >= 1 and overlap >= 0 (got {target!r}, {overlap!r})')
         self.target, self.overlap = int(target), int(overlap)
         self.step, self.fold_len = self.target + self.overlap, self.target + 2 * self.overlap
-        self.rows = int(max_streams)                         # streams admitted at once
         self.hop, self.lookahead = model.hop_length, model.lookahead()
-        self.mu = model.n_classes - 1 if model.mode == 'RAW' else 0
         self.S = POOL_CALL_HOPS * self.hop
         self.slots = [None] * nrows                          # the fold on each loop row
-        self.streams = {}
-        self.next_sid = 0
         self.hold = -(-(21 * self.hop + self.fold_len) // self.step) + 1      # finished folds of one stream that can wait on its release
         self.nstore = nrows + self.rows * self.hold
         if self.nstore * self.fold_len * 4 > COND_BYTES:
@@ -1150,37 +1083,24 @@ class FoldedStreamPool(StreamPool):
         self.free_store = list(range(self.nstore))
 
     # ---- streams ----
-    def open(self, uniforms=None, seed=None):
-        """A new stream -> its id.  uniforms: its tape [K, target + 2 overlap, U], or None; seed (an int in [0, 2^64), used without a
-        tape): the stream draws its uniforms from it.  No loop row is taken until its first fold is granted one."""
-        tape = self.m._check_stream_tape(uniforms, self.fold_len)
-        if seed is not None and (isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= int(seed) < 1 << 64):
-            raise ValueError(f'a seed is an int in [0, 2^64) (got {seed!r})')
-        if len(self.streams) >= self.rows:
-            raise ValueError(f'the stream pool is full: {self.rows} streams are open')
-        sid = self.next_sid
-        with self._fp32():
-            if tape is not None:
-                tape = tape.to(device=self.device, dtype=torch.float32).contiguous()
-            self.streams[sid] = _FoldedStream(sid, self.device, self.m.feat_dims, tape, None if seed is None else int(seed))
-        self.next_sid += 1
-        return sid
+    def check_tape(self, uniforms):
+        """A stream's tape [K, target + 2 overlap, U], or None."""
+        return self.v._check_stream_tape(uniforms, self.fold_len)
 
-    def close(self, sid):
-        """Drops stream sid and frees every loop row and all storage of it at once, whatever it has run or released."""
-        st = self.streams.pop(sid, None)
-        if st is None:
-            raise ValueError(f'unknown or finished stream {sid}')
+    def _open(self, sid, tape, seed):
+        """No loop row is taken until the stream's first fold is granted one."""
+        if tape is not None:
+            tape = tape.to(device=self.device, dtype=torch.float32).contiguous()
+        return _FoldedStream(sid, self.device, self.v.feat_dims, tape, seed)
+
+    def _drop(self, st):
         for f in st.folds:
-            self._free(f)
-
-    def _free(self, f):
-        if f.slot is not None:
-            self.slots[f.slot] = None
-            f.slot = None
-        if f.store is not None:
-            self.free_store.append(f.store)
-            f.store = None
+            if f.slot is not None:
+                self.slots[f.slot] = None
+                f.slot = None
+            if f.store is not None:
+                self.free_store.append(f.store)
+                f.store = None
 
     # ---- geometry ----
     def folds_known(self, st):
@@ -1231,7 +1151,7 @@ class FoldedStreamPool(StreamPool):
         work = {f: n for f, n in work.items() if n > 0}
         if not work:
             return {}
-        S = min(self.S, self.m.chunk_steps(max(f.slot for f in work) + 1, 1 << 30))
+        S = min(self.S, self.v.chunk_steps(max(f.slot for f in work) + 1, 1 << 30))
         return {f: (f.start + f.steps, min(S, n)) for f, n in work.items()}
 
     def release_plan(self):
@@ -1264,8 +1184,7 @@ class FoldedStreamPool(StreamPool):
                 self._loop(plan)
             rel = self.release_plan()
             released = self._release(rel) if rel else {}
-            if F.wavernn_aborted(self.shape, self.ws):
-                raise _lib.B200TTSError('wavernn: the sample loop timed out at a grid barrier')
+            _check_loop(self.shape, self.ws)
         for sid in list(self.streams):
             st = self.streams[sid]
             if st.ended and st.released == (st.frames - 1) * self.hop:
@@ -1308,22 +1227,21 @@ class FoldedStreamPool(StreamPool):
 
     # ---- device work ----
     def _reset(self, slots):
-        F.wavernn_reset_rows(self.shape, self.ws, slots)
-        self.last[self._upload(np.array(slots, np.int64))] = 0.0
+        self.loop.reset(slots)
 
     def _loop(self, plan):
-        live = sorted(plan, key=lambda f: f.slot)
         L = self.fold_len
-        steps = {f: f.steps for f in live}
-        y, active, nmax = self._step_rows(live, {f: f for f in live}, plan, steps, lambda f, s, n: f.st.tape[f.k, s:s + n],
-                                          {f: f.k * L + f.steps for f in live})
+        live = sorted(plan, key=lambda f: f.slot)
+        rows = [_Row(f.slot, f.st.mel, f.st.ended, plan[f][0], plan[f][1], f.steps,
+                     None if f.st.tape is None else f.st.tape[f.k, f.steps:f.steps + plan[f][1]], f.st.seed, f.k * L + f.steps) for f in live]
+        y, active, nmax = self.loop.step_rows(rows)
         # into the storage: fold f's step s at f.store L + s; steps past a row's budget go to the sink
         base, row_n = np.full(active, self.nstore * L, np.int64), np.zeros(active, np.int64)
         for f in live:
             base[f.slot], row_n[f.slot] = f.store * L + f.steps, plan[f][1]
         i = np.arange(nmax)[None, :]
         dst = np.where(i < row_n[:, None], base[:, None] + i, self.nstore * L)
-        self.store.index_put_((self._upload(dst.reshape(-1)),), y.reshape(-1))
+        self.store.index_put_((_upload(dst.reshape(-1), self.device),), y.reshape(-1))
         self._advance(plan)
 
     def unfold_layout(self, rel):
@@ -1343,8 +1261,8 @@ class FoldedStreamPool(StreamPool):
     def _release(self, rel):
         """Every stream's final positions through one b200tts_wavernn_unfold_streams launch -> {sid: chunk}."""
         descs, base = self.unfold_layout(rel)
-        b = self._upload(np.array(base, np.int64))
+        b = _upload(np.array(base, np.int64), self.device)
         wave = F.wavernn_unfold_streams(self.store, descs, b, torch.full_like(b, self.fold_len, dtype=torch.int32), self.hop, self.target,
-                                        self.overlap, 0 if self.a else self.mu)
+                                        self.overlap, self.loop.out_mu)
         self._mark_released(rel)
         return {sid: wave[d.wave_off:d.wave_off + q1 - q0] for d, (sid, q0, q1, _) in zip(descs, rel)}

@@ -128,7 +128,7 @@ def _fold_features(m, mel):
                           d(np.zeros(1, np.int32)), fir, trace['aux'], 0, F_ * hop)[:, 0]
 
 
-def test_window_rows_equal_the_fold():
+def test_loop_window_rows_equal_the_fold():
     _lib.set_precision('fp32')
     m = make_model('RAW', seed=44)
     hop = m.hop_length
@@ -148,7 +148,7 @@ def test_window_rows_equal_the_fold():
             pool.streams[sid].ended = final
         plan = {sid: (t, n) for sid, (*_, t, n) in zip(sids, cases)}
         _lib.set_precision('fp32')
-        feat = pool._features(sids, plan, len(cases), max(n for _, n in plan.values()))
+        feat = pool.loop.features(pool._loop_rows(plan), len(cases), max(n for _, n in plan.values()))
         for b, (k, known, final, t, n) in enumerate(cases):
             assert torch.equal(feat[:n, b], whole[k][t:t + n]), b
             assert bool((feat[n:, b] == 0).all()), b

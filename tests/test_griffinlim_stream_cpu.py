@@ -105,7 +105,7 @@ def _no_device(monkeypatch):
         monkeypatch.setattr(F, name, fail)
 
 
-def test_value_errors_come_before_any_device_work(lib, monkeypatch):
+def test_stream_value_errors_come_before_any_device_work(lib, monkeypatch):
     _no_device(monkeypatch)
     for kw in (dict(lookahead=-1), dict(iters=0), dict(lookahead=1.5), dict(iters=True), dict(lookahead=_lib.GL_STREAM_MAX_LOOKAHEAD + 1)):
         with pytest.raises(ValueError):
@@ -136,12 +136,10 @@ def test_value_errors_come_before_any_device_work(lib, monkeypatch):
         voc.stream_pool(2, target=10, overlap=2)
     with pytest.raises(ValueError):
         voc.stream_pool(2, preemphasis=-1.0)
-    assert voc.lookahead() == 3 and voc._check_stream_tape(None) is None
-    with pytest.raises(ValueError):
-        voc._check_stream_tape(np.zeros((1, 10, 1)))
-    with pytest.raises(ValueError):
-        voc._check_stream_tape(None, fold_len=100)
     pool = voc.stream_pool(2)
+    assert voc.lookahead() == 3 and pool.check_tape(None) is None
+    with pytest.raises(ValueError, match='draws nothing'):
+        pool.check_tape(np.zeros((1, 10, 1)))
     a = pool.open(seed=3)
     with pytest.raises(ValueError):
         pool.open(uniforms=np.zeros((1, 10, 1)))

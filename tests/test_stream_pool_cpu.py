@@ -1,5 +1,6 @@
 """Concurrent streaming synthesis without a GPU: the pool's per-call budgets, releases and window layout on hand-computed cases, the
-argument checks of the new entry points, and the registers of the new kernels and of both sample-loop instantiations."""
+checks every vocoder stream pool makes before any device work, the argument checks of the new entry points, and the registers of the new
+kernels and of both sample-loop instantiations."""
 import ctypes
 import os
 import re
@@ -10,7 +11,10 @@ import pytest
 import torch
 
 from multilingual_text_to_speech_b200 import _lib, build
-from multilingual_text_to_speech_b200.modules.wavernn import StreamPool, WaveRNN, _PoolStream
+from multilingual_text_to_speech_b200.modules.griffinlim import GriffinLimVocoder
+from multilingual_text_to_speech_b200.modules.stream_pool import VocoderStreamPool
+from multilingual_text_to_speech_b200.modules.wavernn import FoldedStreamPool, StreamPool, WaveRNN, _PoolStream, _Row, _SampleLoop
+from multilingual_text_to_speech_b200.params.params import Params as hp
 from test_wavernn_cpu import REAL, _nvcc
 
 
@@ -38,16 +42,17 @@ def test_pool_releases():
     assert p.release_plan() == [(0, 5 * 275, 26), (2, 24 * 275, 25), (3, 3 * 275, 24)]
 
 
-def test_window_layout():
+def test_loop_window_layout():
     """Two streams at the reference's settings (pad 2, factors 5 x 5 x 11): row 0 ended at 30 frames and runs its last two hops, row 1
     has 10 frames and runs its first hop."""
-    p = _pool(S=4400)
-    p.m = WaveRNN(**REAL)
-    p.streams = {7: _stream(0, 30, 27 * 275, True), 3: _stream(1, 10, 0)}
-    srcs, idx, lens, widths, W, desc = p.window_layout([7, 3], {7: (27 * 275, 550), 3: (0, 275)})
+    loop = _SampleLoop.__new__(_SampleLoop)
+    loop.m = WaveRNN(**REAL)
+    rows = [_Row(0, torch.zeros(80, 30), True, 27 * 275, 550, 27 * 275, None, None, 27 * 275),
+            _Row(1, torch.zeros(80, 10), False, 0, 275, 0, None, None, 0)]
+    srcs, idx, lens, widths, W, desc = loop.window_layout(rows)
     # mel-path windows: padded-mel frames [27, 33) (frames 25..29 of row 0, then zero) and [0, 5) (zero, zero, frames 0..2 of row 1);
     # MelResNet windows: frames [25, 30) and [0, 3)
-    assert srcs == [(7, 25, 30), (3, 0, 3), (7, 25, 30), (3, 0, 3)]
+    assert srcs == [(0, 25, 30), (1, 0, 3), (0, 25, 30), (1, 0, 3)]
     assert lens == [6, 5] and widths == [5, 3] and W == 5
     Wt = 17                                                   # 16 packed columns and the zero column
     assert idx.shape == (80 * 11 + 2 * 80 * 5,)
@@ -70,6 +75,39 @@ def test_pool_budgets():
         5: _stream(5, 30, 29 * 275, ended=True),   # every step run: only its final release is left
     }
     assert p.plan() == {0: (0, 8 * 275), 2: (0, 4400), 3: (19 * 275, 275)}
+
+
+def _host_pools():
+    """The three vocoder stream pools' host state, without the WaveRNN pools' device set-up."""
+    m = WaveRNN(**REAL)
+    unfolded = StreamPool.__new__(StreamPool)
+    VocoderStreamPool.__init__(unfolded, m, 2)
+    folded = FoldedStreamPool.__new__(FoldedStreamPool)
+    folded._layout(m, 2, 300, 7, 64)
+    return {'unfolded': (unfolded, np.zeros((2, 100, 1), np.float32)), 'folded': (folded, np.zeros((2, 100, 1), np.float32)),
+            'griffinlim': (GriffinLimVocoder().stream_pool(2), np.zeros((1, 100, 1), np.float32))}
+
+
+def test_pool_checks_before_device_work():
+    """max_streams and preemphasis at construction, the tape and the seed at open(): ValueError before any device work, and nothing
+    opened."""
+    hp.reset()
+    m = WaveRNN(**REAL)
+    for make in (lambda n, a: StreamPool(m, n, a), lambda n, a: FoldedStreamPool(m, n, 300, 7, a),
+                 lambda n, a: GriffinLimVocoder().stream_pool(n, a)):
+        for n in (0, 65, True, 2.0):
+            with pytest.raises(ValueError, match='1 to 64 streams'):
+                make(n, 0.0)
+        for a in (1.0, -1.0):
+            with pytest.raises(ValueError, match='preemphasis'):
+                make(2, a)
+    for name, (pool, bad_tape) in _host_pools().items():
+        for seed in (-1, 1 << 64, 1.5, True, '3'):
+            with pytest.raises(ValueError, match=r'a seed is an int in \[0, 2\^64\)'):
+                pool.open(seed=seed)
+        with pytest.raises(ValueError, match='uniform tape'):
+            pool.open(uniforms=bad_tape)
+        assert pool.streams == {} and pool.next_sid == 0, name
 
 
 def test_abi_argument_checks_without_a_device():
