@@ -599,6 +599,37 @@ int b200tts_mel_cepstrum(int total_frames, int n_mels, int n_mfcc, const float* 
 int b200tts_mel_cepstral_distortion(int B, int n_mfcc, int mode, const float* cep_a, const int32_t* off_a, const float* cep_b,
                                     const int32_t* off_b, double* mcd_out, int32_t* path_len_out, void* stream);
 
+/* ---- forced alignment: monotonic alignment search over attention probabilities (no counterpart in the reference) ----
+ * P: fp32 attention probabilities of B utterances, utterance b's weight of symbol l at decoder step s at P[b batch_stride + s ld + l]
+ * (s < S, l < L: a padded [B, S, L] batch).  text_lengths, step_lengths: int32 [B], device; utterance b uses steps s < S_b and symbols
+ * l < L_b.  No workspace.  One CTA per utterance: no utterance reads another's data and nothing uses global atomics, so every result is
+ * bit-reproducible and independent of the batch it is computed in. */
+typedef struct {
+    int B, S, L;              /* utterances; padded steps and symbols (1 <= L <= B200TTS_ALIGN_MAX_SYMBOLS) */
+    long long ld;             /* elements between consecutive steps of one utterance (>= L) */
+    long long batch_stride;   /* elements between consecutive utterances (>= 0) */
+} b200tts_align_shape;
+/* The search keeps two fp64 rows of L values and one back-pointer bit per cell in shared memory (227 KB): an utterance may have at most
+ * this many symbols, and S_b L_b at most this many cells (1,688 steps at 1,024 symbols; 5,761 steps at 300). */
+#define B200TTS_ALIGN_MAX_SYMBOLS 1024
+#define B200TTS_ALIGN_MAX_CELLS 1728512
+/* Monotonic alignment search (Glow-TTS MAS) per utterance: the path l_0 = 0, l_{S_b - 1} = L_b - 1, l_{s+1} - l_s in {0, 1} that maximises
+ * sum_s log(max(P[s, l_s], 1e-8)), accumulated in fp64 (log of the fp32 weight widened to fp64).  Recurrence Q[s][l] = log max(P[s, l],
+ * 1e-8) + max(Q[s-1][l], Q[s-1][l-1]).  Tie rule: the path advances from symbol l - 1 to l at step s only when Q[s-1][l-1] > Q[s-1][l]
+ * strictly; on equal values it stays on symbol l.  durations_out int32 [B, L]: steps per symbol (each >= 1 below L_b, summing to S_b;
+ * 0 from L_b on); path_logp_out double [B]: the path's sum; path_out int32 [B, S] or NULL: the symbol of each step (-1 from S_b on).
+ * Requires 1 <= L_b <= S_b <= S, L_b <= L and S_b L_b <= B200TTS_ALIGN_MAX_CELLS: lengths live on the device, so the caller checks them;
+ * an utterance outside these gets durations -1, path -1 and a NaN path_logp. */
+int b200tts_monotonic_alignment(const b200tts_align_shape* shape, const float* P, const int32_t* text_lengths, const int32_t* step_lengths,
+                                int32_t* durations_out, double* path_logp_out, int32_t* path_out, void* stream);
+/* Alignment quality per utterance over steps s < S_b and symbols l < L_b (fp64 sums, fp32 results): focus_out, the mean over steps of the
+ * step's largest weight; coverage_out, the fraction of symbols whose weights summed over the steps reach 0.5; max_jump_out (int32), the
+ * largest forward move of the per-step argmax (the first index on equal weights) between consecutive steps, 0 if it never moves forward;
+ * moves_back_out (int32), 1 if it ever moves backwards.  Requires 1 <= L_b <= L and 1 <= S_b <= S; an utterance outside these gets NaN
+ * scores and -1 moves. */
+int b200tts_alignment_scores(const b200tts_align_shape* shape, const float* P, const int32_t* text_lengths, const int32_t* step_lengths,
+                             float* focus_out, float* coverage_out, int32_t* max_jump_out, int32_t* moves_back_out, void* stream);
+
 /* ---- WaveRNN vocoder (fatchord architecture): mel -> waveform, one GRU step per sample over fold rows ----
  * The MelResNet and the time-batched conditioning products run on the convolution-block and GEMM entry points; these entry points add
  * the mel upsampling layers, the folding, the persistent sample loop and the unfolding.  Fold rows: utterance b's F_b hop sample

@@ -153,6 +153,15 @@ MCD_MODES = {'cut': 0, 'stretch': 1, 'dtw': 2}
 DTW_MAX_FRAMES = 6455
 
 
+class AlignShape(Structure):
+    _fields_ = [(n, c_int) for n in ('B', 'S', 'L')] + [(n, c_longlong) for n in ('ld', 'batch_stride')]
+
+
+# include/b200tts.h: B200TTS_ALIGN_MAX_SYMBOLS and B200TTS_ALIGN_MAX_CELLS
+ALIGN_MAX_SYMBOLS = 1024
+ALIGN_MAX_CELLS = 1728512
+
+
 # name -> (restype, argtypes); the "-m not gpu" suite checks every symbol of the header resolves
 SIGNATURES = {
     'b200tts_last_error': (c_char_p, []),
@@ -243,6 +252,8 @@ SIGNATURES = {
     'b200tts_amplitude_to_db': (c_int, [POINTER(AnalysisShape), c_void_p, c_void_p, c_void_p, c_void_p]),
     'b200tts_mel_cepstrum': (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     'b200tts_mel_cepstral_distortion': (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'b200tts_monotonic_alignment': (c_int, [POINTER(AlignShape)] + [c_void_p] * 7),
+    'b200tts_alignment_scores': (c_int, [POINTER(AlignShape)] + [c_void_p] * 8),
     'b200tts_wavernn_upsample_layer': (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     'b200tts_wavernn_fold': (c_int, [POINTER(WaveRNNFoldShape)] + [c_void_p] * 7 + [c_int, c_int, c_void_p, c_void_p]),
     'b200tts_wavernn_workspace_bytes': (c_size_t, [POINTER(WaveRNNShape)]),

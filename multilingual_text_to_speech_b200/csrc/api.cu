@@ -242,6 +242,11 @@ int mcd_validate(int B, int n_mfcc, int mode);
 int mel_cepstrum_impl(int total_frames, int n_mels, int n_mfcc, const float* mel_db, float* out, cudaStream_t st);
 int mel_cepstral_distortion_impl(int B, int n_mfcc, int mode, const float* cep_a, const int* off_a, const float* cep_b, const int* off_b,
                                  double* mcd, int* path_len, cudaStream_t st);
+int align_validate(const b200tts_align_shape& s);
+int monotonic_alignment_impl(const b200tts_align_shape& s, const float* P, const int* text_lengths, const int* step_lengths, int* durations,
+                             double* path_logp, int* path, cudaStream_t st);
+int alignment_scores_impl(const b200tts_align_shape& s, const float* P, const int* text_lengths, const int* step_lengths, float* focus,
+                          float* coverage, int* max_jump, int* moves_back, cudaStream_t st);
 int wavernn_upsample_layer_check(int C, int len, int scale);
 int wavernn_upsample_layer_impl(int C, int len, int scale, const float* fir, const float* in, float* out, cudaStream_t st);
 int wavernn_fold_check(const b200tts_wavernn_fold_shape& s, int t0, int nsteps);
@@ -836,6 +841,23 @@ int b200tts_mel_cepstral_distortion(int B, int n_mfcc, int mode, const float* ce
     B200_TRY(mcd_validate(B, n_mfcc, mode));
     B200_TRY(require_device());
     return mel_cepstral_distortion_impl(B, n_mfcc, mode, cep_a, off_a, cep_b, off_b, mcd_out, path_len_out, (cudaStream_t)stream);
+}
+
+int b200tts_monotonic_alignment(const b200tts_align_shape* shape, const float* P, const int32_t* text_lengths, const int32_t* step_lengths,
+                                int32_t* durations_out, double* path_logp_out, int32_t* path_out, void* stream) {
+    B200_REQUIRE(shape && P && text_lengths && step_lengths && durations_out && path_logp_out, "monotonic_alignment: null argument");
+    B200_TRY(align_validate(*shape));
+    B200_TRY(require_device());
+    return monotonic_alignment_impl(*shape, P, text_lengths, step_lengths, durations_out, path_logp_out, path_out, (cudaStream_t)stream);
+}
+int b200tts_alignment_scores(const b200tts_align_shape* shape, const float* P, const int32_t* text_lengths, const int32_t* step_lengths,
+                             float* focus_out, float* coverage_out, int32_t* max_jump_out, int32_t* moves_back_out, void* stream) {
+    B200_REQUIRE(shape && P && text_lengths && step_lengths && focus_out && coverage_out && max_jump_out && moves_back_out,
+                 "alignment_scores: null argument");
+    B200_TRY(align_validate(*shape));
+    B200_TRY(require_device());
+    return alignment_scores_impl(*shape, P, text_lengths, step_lengths, focus_out, coverage_out, max_jump_out, moves_back_out,
+                                 (cudaStream_t)stream);
 }
 
 int b200tts_wavernn_upsample_layer(int C, int len, int scale, const float* fir, const float* in, float* out, void* stream) {

@@ -978,6 +978,105 @@ def mel_cepstral_distortion(cep_a, off_a, cep_b, off_b, mode):
 
 
 # ------------------------------------------------------------------------------------------------
+# forced alignment (monotonic alignment search over attention probabilities, include/b200tts.h)
+# ------------------------------------------------------------------------------------------------
+def _host_lengths(x, B, what):
+    if torch.is_tensor(x):
+        if x.dtype.is_floating_point or x.dtype in (torch.bool, torch.complex64, torch.complex128):
+            raise ValueError(f'{what} must be integers, got {x.dtype}')
+        x = x.tolist()
+    x = np.asarray(x)
+    if x.ndim != 1 or x.shape[0] != B:
+        raise ValueError(f'{what} must hold one length per utterance ({B}), got shape {tuple(x.shape)}')
+    if x.dtype.kind not in 'iu':
+        raise ValueError(f'{what} must be integers, got {x.dtype}')
+    return [int(v) for v in x]
+
+
+def check_alignment_inputs(weights, text_lengths, step_lengths):
+    """The host checks of monotonic_alignment, made before any device work.  -> (text lengths, step lengths) as lists of ints."""
+    if not torch.is_tensor(weights) or weights.dim() != 3:
+        raise ValueError(f'weights must be a [B, S, L] tensor, got {tuple(weights.shape) if torch.is_tensor(weights) else type(weights)}')
+    if weights.dtype != torch.float32:
+        raise ValueError(f'weights must be float32, got {weights.dtype}')
+    B, S, L = weights.shape
+    if B < 1 or S < 1 or L < 1:
+        raise ValueError(f'weights must be non-empty, got shape {tuple(weights.shape)}')
+    tl, sl = check_alignment_lengths(text_lengths, step_lengths, B, S, L)
+    if not bool(torch.isfinite(weights).all()):
+        raise ValueError('weights must be finite')
+    return tl, sl
+
+
+def check_alignment_lengths(text_lengths, step_lengths, B, S, L):
+    """Host checks of B utterances' text lengths and step counts against a padded [B, S, L] grid and the search's shared-memory limits.
+    -> both as lists of ints."""
+    tl, sl = _host_lengths(text_lengths, B, 'text_lengths'), _host_lengths(step_lengths, B, 'step_lengths')
+    for b, (n, s) in enumerate(zip(tl, sl)):
+        if not 1 <= n <= L:
+            raise ValueError(f'utterance {b}: text length {n} is outside [1, {L}]')
+        if not 1 <= s <= S:
+            raise ValueError(f'utterance {b}: step count {s} is outside [1, {S}]')
+        if s < n:
+            raise ValueError(f'utterance {b}: {s} steps cannot cover {n} symbols (a monotonic path needs at least one step per symbol)')
+        if n > _lib.ALIGN_MAX_SYMBOLS:
+            raise ValueError(f'utterance {b}: {n} symbols exceed the {_lib.ALIGN_MAX_SYMBOLS} the search keeps in shared memory')
+        if s * n > _lib.ALIGN_MAX_CELLS:
+            raise ValueError(f'utterance {b}: {s} steps x {n} symbols = {s * n} cells exceed the {_lib.ALIGN_MAX_CELLS} back-pointer bits '
+                             'the search keeps in shared memory')
+    return tl, sl
+
+
+def _align_args(weights, tl, sl):
+    """Library view of the checked weights, cut to the longest lengths, and the lengths on its device."""
+    _require_cuda(weights)
+    w = weights[:, :max(sl), :max(tl)]
+    if w.stride(2) != 1:
+        w = w.contiguous()
+    shape = _lib.AlignShape(w.shape[0], w.shape[1], w.shape[2], w.stride(1), w.stride(0))
+    lengths = torch.tensor([tl, sl], dtype=torch.int32).to(w.device)
+    return shape, w, lengths[0], lengths[1]
+
+
+def monotonic_alignment(weights, text_lengths, step_lengths, return_path=False):
+    """Monotonic alignment search (Glow-TTS MAS) over attention probabilities weights [B, S, L] (fp32, CUDA; forward attention's,
+    windowed decoding's or any other): per utterance b, over steps s < step_lengths[b] and symbols l < text_lengths[b], the path from
+    symbol 0 to symbol L_b - 1 that advances by 0 or 1 symbol per step and maximises sum log(max(w, 1e-8)) in fp64; on equal values it
+    stays on the same symbol (include/b200tts.h states the rule).  Lengths: int tensors or sequences, 1 <= L_b <= S_b.
+    -> (durations int32 [B, L]: steps per symbol, each >= 1, summing to S_b, 0 past L_b; path_logp float64 [B]) and, with return_path,
+    path int32 [B, S]: the symbol of every step, -1 past S_b.  Raises ValueError before any device work on a wrong rank or dtype,
+    lengths out of range, S_b < L_b, a shape past B200TTS_ALIGN_MAX_SYMBOLS / _MAX_CELLS, or non-finite weights."""
+    tl, sl = check_alignment_inputs(weights, text_lengths, step_lengths)
+    B, S, L = weights.shape
+    shape, w, d_tl, d_sl = _align_args(weights, tl, sl)
+    durations = torch.empty(B, shape.L, device=w.device, dtype=torch.int32)
+    path_logp = torch.empty(B, device=w.device, dtype=torch.float64)
+    path = torch.empty(B, shape.S, device=w.device, dtype=torch.int32) if return_path else None
+    check(_lib.load().b200tts_monotonic_alignment(ctypes.byref(shape), ptr(w), ptr(d_tl), ptr(d_sl), ptr(durations), ptr(path_logp),
+                                                  ptr(path), _stream()), 'b200tts_monotonic_alignment')
+    durations = torch.nn.functional.pad(durations, (0, L - shape.L))
+    if not return_path:
+        return durations, path_logp
+    return durations, path_logp, torch.nn.functional.pad(path, (0, S - shape.S), value=-1)
+
+
+def alignment_scores(weights, text_lengths, step_lengths):
+    """Alignment quality per utterance of weights [B, S, L] over its valid steps and symbols (the checks of monotonic_alignment apply).
+    -> dict of focus_rate (float32 [B], the mean over steps of the step's largest weight), coverage (float32 [B], the fraction of
+    symbols whose summed weight reaches 0.5), max_jump (int32 [B], the largest forward move of the per-step argmax) and moves_back
+    (bool [B], whether the argmax ever moves backwards)."""
+    tl, sl = check_alignment_inputs(weights, text_lengths, step_lengths)
+    shape, w, d_tl, d_sl = _align_args(weights, tl, sl)
+    B = w.shape[0]
+    out = {k: torch.empty(B, device=w.device, dtype=dt) for k, dt in (('focus_rate', torch.float32), ('coverage', torch.float32),
+                                                                      ('max_jump', torch.int32), ('moves_back', torch.int32))}
+    check(_lib.load().b200tts_alignment_scores(ctypes.byref(shape), ptr(w), ptr(d_tl), ptr(d_sl), *(ptr(v) for v in out.values()), _stream()),
+          'b200tts_alignment_scores')
+    out['moves_back'] = out['moves_back'].bool()
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
 # WaveRNN vocoder (fold rows: see include/b200tts.h)
 # ------------------------------------------------------------------------------------------------
 def wavernn_upsample_layer(x, fir, scale):

@@ -5,6 +5,8 @@ Constructor signatures, attribute names (`_embedding`, `_encoder`, `_prenet`, `_
 train.py, synthesize.py and existing checkpoints work unchanged.  All arithmetic of the hot path is inside the
 library: `Decoder` is ONE fused op (forward + hand-written BPTT), encoders / postnet are fused conv-block ops.
 """
+from typing import NamedTuple
+
 import numpy as np
 import torch
 from torch.nn import functional as TF
@@ -423,6 +425,53 @@ class Tacotron(torch.nn.Module):
             self.train(was_training)
         return outputs
 
+    def align(self, text, text_length, target, target_length, speakers=None, languages=None):
+        """Forced alignment of a batch with its target spectrograms: `forward` in eval mode at teacher forcing 1.0 without autograd (the
+        reference gta.py's call), then the monotonic alignment search (functional.monotonic_alignment) and the alignment scores on each
+        utterance's steps and symbols.  Takes forward's inputs: text int [B, L], text_length [B], target [B, num_mels, T],
+        target_length [B], speakers and languages in forward's forms (grouped-encoder batches in any language layout).
+
+        With hp.outputs_per_step = r the search runs on the decoder's step grid, S_b = ceil(T_b / r) steps for T_b target frames (the
+        steps the guided-attention loss weighs); a symbol's frames are its steps times r, except the last symbol's, which lose the
+        S_b r - T_b frames past the target, so each utterance's frames sum to T_b.
+
+        Prenet dropout stays on, as in the reference.  For repeatable masks replay a MaskSource tape (its 'teacher' entry is replaced by
+        all ones for this call) or seed MaskSource.  -> Alignment: `alignment` [B, S, L] is forward's alignment on the same batch and
+        masks, bit for bit.  ValueError before any device work for malformed inputs, lengths out of range, S_b < L_b, or a shape past
+        the search's limits."""
+        shapes = [('text', text, 2), ('text_length', text_length, 1), ('target', target, 3), ('target_length', target_length, 1)]
+        for name, t, dims in shapes:
+            if not torch.is_tensor(t) or t.dim() != dims:
+                raise ValueError(f'align: {name} must be a {dims}-D tensor')
+        if text.dtype.is_floating_point:
+            raise ValueError(f'align: text must hold symbol ids, got {text.dtype}')
+        B, L = text.shape
+        if target.shape[0] != B or target.shape[1] != hp.num_mels:
+            raise ValueError(f'align: target must be [B = {B}, num_mels = {hp.num_mels}, T], got {tuple(target.shape)}')
+        r, T = self._decoder._outputs_per_step, target.shape[2]
+        frames = F._host_lengths(target_length, B, 'target_length')
+        for b, t in enumerate(frames):
+            if not 1 <= t <= T:
+                raise ValueError(f'align: utterance {b}: target length {t} is outside [1, {T}]')
+        steps = [-(-t // r) for t in frames]
+        symbols, _ = F.check_alignment_lengths(text_length, steps, B, -(-T // r), L)
+        was_training, tape = self.training, MaskSource.tape
+        self.eval()
+        try:
+            if tape is not None:
+                MaskSource.use_tape({**tape, 'teacher': torch.ones(-(-T // r), dtype=torch.bool)})
+            with torch.no_grad():
+                alignment = self.forward(text, text_length, target, target_length, speakers, languages, teacher_forcing_ratio=1.0)[3]
+        finally:
+            MaskSource.use_tape(tape)
+            self.train(was_training)
+        step_durations, path_logp = F.monotonic_alignment(alignment, symbols, steps)
+        durations = step_durations * r
+        rows = torch.arange(B, device=durations.device)
+        last = torch.tensor(symbols, device=durations.device) - 1
+        durations[rows, last] -= torch.tensor([s * r - t for s, t in zip(steps, frames)], device=durations.device, dtype=torch.int32)
+        return Alignment(alignment, durations, step_durations, path_logp, **F.alignment_scores(alignment, symbols, steps))
+
     def inference_stream(self, text, speaker=None, language=None, chunk_frames=None):
         """Streaming `inference`: a generator of post-net spectrogram chunks [num_mels, n_k] whose concatenation is inference(text,
         speaker, language), the same stop cut and, given the same prenet dropout masks, the same decoded frames.  Takes the inputs
@@ -522,6 +571,18 @@ class Tacotron(torch.nn.Module):
 
 # texts of one inference_streams group at most: the batch inference_batch decodes at once by default
 MAX_STREAM_TEXTS = 64
+
+
+class Alignment(NamedTuple):
+    """Tacotron.align's result for B utterances of L symbols and S decoder steps (S_b = ceil(T_b / r) each)."""
+    alignment: torch.Tensor         # [B, S, L] float32: Tacotron.forward's attention weights (eval mode, teacher forcing 1.0)
+    durations: torch.Tensor         # [B, L] int32: frames per symbol, summing to target_length, 0 past the text
+    step_durations: torch.Tensor    # [B, L] int32: decoder steps per symbol, summing to S_b, 0 past the text
+    path_logp: torch.Tensor         # [B] float64: the path's sum of log max(weight, 1e-8)
+    focus_rate: torch.Tensor        # [B] float32: mean over steps of the largest weight
+    coverage: torch.Tensor          # [B] float32: fraction of symbols whose summed weight reaches 0.5
+    max_jump: torch.Tensor          # [B] int32: largest forward move of the per-step argmax
+    moves_back: torch.Tensor        # [B] bool: whether the per-step argmax ever moves backwards
 
 
 def inference_attention_window():
