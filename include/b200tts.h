@@ -213,6 +213,17 @@ size_t b200tts_debug_persist_bwd_profile_offset(const b200tts_decoder_shape* sha
  *   row strides (in elements) of aib and hgb: Kp_att, Kp_gen
  * Returns the number of values written (26 when n >= 26), 0 for a rejected shape. */
 int b200tts_debug_decoder_views(const b200tts_decoder_shape* shape, size_t* out, int n);
+/* Debug (pure host arithmetic, no device needed): the geometry the persistent loops would run this shape with.  Fills out[0 .. n) in
+ * this order:
+ *   b200tts_decoder_path of the shape;
+ *   forward loops: grid (CTAs), NBH (batch halves of 32 utterances), slot_kb (TMA ring slot of the attention loop, in 64-column
+ *     k-blocks), ch_h and n_h (k-blocks per TMA load and loads of the h part), ch_c and n_c (same for the context part), alias (1: the
+ *     accumulator staging shares the ring slot), use_btab (1: the context product's B fragments come from a shared table), the generator
+ *     loop's slot and ch_h;
+ *   attention reverse loop: UN (outputs per n-block), grid.
+ * The geometry is reported whatever the path; only the loops the path bits select run with it.  Returns the number of values written
+ * (14 when n >= 14), 0 for a rejected shape. */
+int b200tts_debug_decoder_geometry(const b200tts_decoder_shape* shape, int* out, int n);
 
 int b200tts_decoder_forward(const b200tts_decoder_shape* shape, const b200tts_decoder_params* params,
                             const b200tts_decoder_inputs* in, const b200tts_decoder_outputs* out, void* workspace,

@@ -176,6 +176,7 @@ SIGNATURES = {
     'b200tts_debug_persist_profile_offset': (c_size_t, [POINTER(DecoderShape)]),
     'b200tts_debug_persist_bwd_profile_offset': (c_size_t, [POINTER(DecoderShape), c_int]),
     'b200tts_debug_decoder_views': (c_int, [POINTER(DecoderShape), POINTER(c_size_t), c_int]),
+    'b200tts_debug_decoder_geometry': (c_int, [POINTER(DecoderShape), POINTER(c_int), c_int]),
     'b200tts_gemm_f32': (c_int, [c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_int, c_void_p, c_int, c_float,
                                  c_void_p, c_int, c_void_p, c_int, c_longlong, c_longlong, c_longlong, c_int, c_void_p,
                                  c_void_p]),

@@ -385,6 +385,17 @@ int b200tts_debug_decoder_views(const b200tts_decoder_shape* shape, size_t* out,
     for (int k = 0; k < m; ++k) out[k] = v[k];
     return m;
 }
+int b200tts_debug_decoder_geometry(const b200tts_decoder_shape* shape, int* out, int n) {
+    if (!shape || !out || validate_decoder_shape(*shape) != B200TTS_OK) return 0;
+    const b200tts_decoder_shape s = step_shape(*shape);
+    const TcPersistGeom g = tc_persist_geom(s);
+    const AttBwdGeom ab = att_bwd_geom(s);
+    const int v[14] = {b200tts_decoder_path(shape), g.grid, g.NBH, g.slot_kb_att, g.ch_h_att, g.ch_h_att ? g.nkb_h / g.ch_h_att : 0, g.ch_c_att,
+                       g.n_c_att, g.alias_att, g.use_btab, g.slot_gen, g.ch_h_gen, ab.UN, ab.grid};
+    const int m = n < 14 ? n : 14;
+    for (int k = 0; k < m; ++k) out[k] = v[k];
+    return m;
+}
 int b200tts_debug_bilstm_layout(const b200tts_bilstm_shape* shape, size_t* out, int n) {
     if (!shape || !out || shape->B <= 0 || shape->L <= 0 || shape->E <= 0 || shape->H <= 0) return 0;
     size_t v[10];

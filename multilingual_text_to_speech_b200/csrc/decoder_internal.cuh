@@ -165,8 +165,14 @@ __device__ __forceinline__ float fwd_att_product(const float* __restrict__ alpha
 constexpr float FWD_ATT_FLOOR = 1e-6f;      // torch.clamp(energies, 1e-6) (attention.py:119)
 constexpr float FWD_ATT_NORM_EPS = 1e-12f;  // F.normalize(p=1) eps
 
-// wgmma / TMA persistent forward loops (decoder_persist_tc.cu): operand rows are [h | ctx | 0] in 64-column k-blocks
-struct TcPersistGeom { int Kp_att, Kp_gen, nkb_att, nkb_gen, nkb_h, ch_c_att, n_c_att, alias_att, ch_h_att, slot_att, ch_h_gen, slot_gen; };
+// wgmma / TMA persistent forward loops (decoder_persist_tc.cu): operand rows are [h | ctx | 0] in 64-column k-blocks.
+// grid = (D / 16) row blocks x NBH batch halves; slot_kb_att = the attention loop's ring slot (the larger of its two chunks), smem_att its
+// dynamic shared memory, use_btab = the context product's B-fragment table fits behind the attention scratch
+struct TcPersistGeom {
+    int Kp_att, Kp_gen, nkb_att, nkb_gen, nkb_h, ch_c_att, n_c_att, alias_att, ch_h_att, slot_att, ch_h_gen, slot_gen;
+    int grid, NBH, slot_kb_att, use_btab;
+    size_t smem_att;
+};
 TcPersistGeom tc_persist_geom(const b200tts_decoder_shape& s);
 bool tc_persist_supported(const b200tts_decoder_shape& s);
 int tc_persist_att_loop(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
@@ -178,6 +184,10 @@ int persist_att_prep(const b200tts_decoder_shape& s, const b200tts_decoder_param
                      const DecoderLayout& fl, float* ws, unsigned char* pws, cudaStream_t st);
 struct AttBwdExtra { int MT; size_t part, wcb, wcb2, memTf, de, dwpart, dvpart, barrier, total; };
 AttBwdExtra att_bwd_extra(const b200tts_decoder_shape& s);
+// geometry of the attention reverse loop: UK hidden units per K-slice, UN outputs per n-block, grid CTAs, region = bytes of the TMA slot
+// (= attention scratch capacity), smem = dynamic shared memory of one CTA
+struct AttBwdGeom { int UK, UN, grid; size_t region, smem; };
+AttBwdGeom att_bwd_geom(const b200tts_decoder_shape& s);
 bool persist_att_bwd_supported(const b200tts_decoder_shape& s);
 // dgb_hist: [T, B, 4D] bf16 history of the gate gradients (out), read in place by the time-batched weight-gradient products
 int persist_att_bwd_loop(const b200tts_decoder_shape& s, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,

@@ -919,11 +919,7 @@ AttBwdExtra att_bwd_extra(const b200tts_decoder_shape& s) {
     return x;
 }
 
-// Geometry of the attention reverse loop.
-struct AttBwdGeom {
-    int UK, UN, grid; size_t region, smem;      // region = bytes of the TMA slot (= attention scratch capacity)
-};
-static AttBwdGeom att_bwd_geom(const b200tts_decoder_shape& s) {
+AttBwdGeom att_bwd_geom(const b200tts_decoder_shape& s) {
     AttBwdGeom g{};
     g.UK = s.D / KBA;
     const int L16 = (s.L + 15) / 16 * 16;

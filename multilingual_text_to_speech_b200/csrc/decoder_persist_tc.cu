@@ -729,6 +729,8 @@ int largest_divisor_le(int n, int cap) {
         if (n % d == 0) return d;
     return 1;
 }
+// the attention runs on CTA pairs (clusters of 2) and pair p serves utterance p: a loop of `grid` CTAs serves at most grid / 2 utterances
+bool tc_att_pairs_fit(int grid, int B) { return grid % 2 == 0 && grid / 2 >= B; }
 
 }  // namespace
 
@@ -754,15 +756,22 @@ TcPersistGeom tc_persist_geom(const b200tts_decoder_shape& s) {
     g.ch_h_gen = g.slot_gen >= 1 ? largest_divisor_le(g.nkb_gen, g.slot_gen) : 0;
     // the generator loop requests its operand in (at most) two chunks with separate barriers; it needs the whole operand in the ring
     if (g.slot_gen >= g.nkb_gen && g.nkb_gen % 2 == 0) g.ch_h_gen = g.nkb_gen / 2;
+    g.NBH = (s.B + BT - 1) / BT;
+    g.grid = s.D / UNITS * g.NBH;
+    g.slot_kb_att = g.ch_h_att > g.ch_c_att ? g.ch_h_att : g.ch_c_att;
+    g.smem_att = tc_loop_smem_bytes(g.nkb_att, g.slot_kb_att, s.A, true, s.L, g.alias_att != 0);
+    const size_t tab = (size_t)((s.L + 15) / 16) * 32 * 8;      // shared B-fragment table of the context product, when it fits behind the scratch
+    g.use_btab = g.smem_att + tab <= PERSIST_SMEM_LIMIT ? 1 : 0;
+    if (g.use_btab) g.smem_att += tab;
     return g;
 }
 
 bool tc_persist_supported(const b200tts_decoder_shape& s) {
-    if (s.D % KB != 0 || s.D % UNITS != 0) return false;
-    const int RB = s.D / UNITS, NBH = (s.B + BT - 1) / BT;
-    if (RB * NBH > NUM_SMS || s.B > RB * NBH) return false;
-    if (s.K > 32 || s.A != 128) return false;
+    // the decoder widths whose every loop geometry the step checks cover (tests/persist_geometry.py lists one representative per geometry)
+    if (s.D != 512 && s.D != 1024) return false;
     const TcPersistGeom g = tc_persist_geom(s);
+    if (g.grid > NUM_SMS || !tc_att_pairs_fit(g.grid, s.B)) return false;
+    if (s.K > 32 || s.A != 128) return false;
     return g.ch_c_att >= 1 && g.ch_c_att <= 256 && g.slot_att >= g.ch_c_att && g.ch_h_att >= 1 && g.ch_h_gen >= 1 && g.slot_att >= 2 &&
            g.slot_gen >= g.nkb_gen;          // generator loop: the whole operand row block is ring resident
 }
@@ -772,7 +781,7 @@ static int launch_tc_loop(bool att, const TcLoopArgs& a, const CUtensorMap& tmH,
                          : (void*)lstm_loop_tc_kernel<false, false>;
     const int grid = a.RB * a.NBH;
     // the attention runs on CTA pairs: clusters of 2 (distributed shared memory + cluster barrier)
-    B200_REQUIRE(!att || (grid % 2 == 0 && grid / 2 >= a.B), "wgmma attention loop: %d CTAs cannot form %d pairs", grid, a.B);
+    B200_REQUIRE(!att || tc_att_pairs_fit(grid, a.B), "wgmma attention loop: %d CTAs cannot form %d pairs", grid, a.B);
     TcLoopArgs args = a;
     CUtensorMap mapH = tmH, mapC = tmC;
     void* params[] = {&mapH, &mapC, &args};
@@ -798,7 +807,7 @@ int tc_persist_att_loop(const b200tts_decoder_shape& s, const b200tts_decoder_pa
     a.B = B; a.T = T; a.D = D; a.K = MD; a.Kp = g.Kp_att; a.RB = D / UNITS; a.NBH = (B + BT - 1) / BT;
     a.nkb = g.nkb_att; a.nkb_h = g.nkb_h; a.ch_h = g.ch_h_att; a.n_h = g.nkb_h / g.ch_h_att; a.ch_c = g.ch_c_att; a.n_c = g.n_c_att;
     a.alias_sum = g.alias_att;
-    a.slot_kb = g.ch_h_att > g.ch_c_att ? g.ch_h_att : g.ch_c_att;
+    a.slot_kb = g.slot_kb_att;
     a.W = ws + fl.wcat_att; a.ldw = MD; a.wcol_h = M; a.wcol_c = 0;
     a.actb = aib; a.actf = ws + fl.ai; a.ldf = MD; a.hcol = M;
     a.gates = ws + fl.ga; a.cstate = ws + fl.ca;
@@ -814,11 +823,8 @@ int tc_persist_att_loop(const b200tts_decoder_shape& s, const b200tts_decoder_pa
     a.barrier = barrier; a.abort_flag = reinterpret_cast<int*>(barrier + 32);
     a.prof = reinterpret_cast<long long*>(pws + l.barrier + 256);
     a.prof2 = a.prof + 2 * NUM_SMS * 8;
-    size_t smem = tc_loop_smem_bytes(g.nkb_att, a.slot_kb, s.A, true, s.L, g.alias_att != 0);
-    const size_t tab = (size_t)l.MT * 32 * 8;          // shared B-fragment table of the context product, when it fits behind the scratch
-    a.use_btab = smem + tab <= PERSIST_SMEM_LIMIT ? 1 : 0;
-    if (a.use_btab) smem += tab;
-    return launch_tc_loop(true, a, tmH, tmC, smem, st);
+    a.use_btab = g.use_btab;
+    return launch_tc_loop(true, a, tmH, tmC, g.smem_att, st);
 }
 
 // Generator-LSTM loop.  Expects: gg = input projection, hg row 0 = 0, cg row 0 = 0.

@@ -590,18 +590,28 @@ class AttentionReverse:
         self.rep.add('dmemT', 0, (self.v['dmemT'].double() - self.dmemT).abs()[None], self.b_dmemT[None])
 
 
+def modes_of(mode):
+    """(forward, generator reverse, attention reverse) rounding models of a decode: one mode for all three recurrences, or a triple when
+    the plan runs some of them on the persistent loops and the others on the per-step chains"""
+    out = tuple(mode) if isinstance(mode, (tuple, list)) else (mode,) * 3
+    assert len(out) == 3 and all(m in MODES for m in out), mode
+    return out
+
+
 def check_reverse(v, prm, masks, cfg, mode, report=None, fill=False, attention=None, lose_carry_at=None):
     """Gate gradients of the generator reverse loop (dgg) and of the attention-LSTM part of the attention reverse loop (dga, from the
     loop's own query gradients dq), teacher-forced decodes.  attention = (lengths, memory, align, dalign): also the attention backward
-    of the attention reverse loop (AttentionReverse)."""
-    assert mode in MODES
+    of the attention reverse loop (AttentionReverse).  mode: one for both recurrences, or (generator, attention)."""
+    gen_mode, att_mode = (mode, mode) if isinstance(mode, str) else tuple(mode)
+    assert gen_mode in MODES and att_mode in MODES
+    mode = att_mode
     T, B, D, M, L, A = _dims(v)
     rep = report or Report(T)
     att = AttentionReverse(v, prm, *attention, mode, rep, fill) if attention is not None else None
     if att is not None:
         att.lose_carry_at = lose_carry_at
     m = {k: masks.get(k) if (cfg.training and masks) else None for k in ('att_h', 'att_c', 'gen_h', 'gen_c')}
-    _reverse(v, cfg, mode, rep, 'dgg', 'dgg', 'dggb', 'gg', 'cg', 'dhgd', None, prm['gen_w_hh'], m['gen_h'], m['gen_c'], fill)
+    _reverse(v, cfg, gen_mode, rep, 'dgg', 'dgg', 'dggb', 'gg', 'cg', 'dhgd', None, prm['gen_w_hh'], m['gen_h'], m['gen_c'], fill)
     Wq = prm['attn_query'].double()
 
     def dq_term(i):
@@ -793,9 +803,14 @@ GPU_SHAPES = [
 
 def check_all(v, prm, masks, cfg, lengths, memory, align, aux, mode):
     """Forward, reverse (with the attention backward: aux['dalign'] is the d alignments of the decode, None for none) and, when
-    aux['grads'] is given, the closing products."""
-    rep = check_forward(v, prm, masks, cfg, lengths, memory, align, mode)
-    check_reverse(v, prm, masks, cfg, mode, rep, attention=(lengths, memory, align, aux.get('dalign')))
+    aux['grads'] is given, the closing products.  mode: one for the whole decode, or (forward, generator reverse, attention reverse)
+    (modes_of).  The closing products read the forward's operand rows, so they take the forward's mode; a persistent generator reverse
+    loop's bf16 history, which they read in place, is the RN of its fp32 gate gradients (stage dggb_rn), exactly what the chains' operand
+    packing would read."""
+    fwd, gen, att = modes_of(mode)
+    assert not (fwd == 'persist' and att != 'persist'), 'the persistent forward loops run in training only with the attention reverse loop'
+    rep = check_forward(v, prm, masks, cfg, lengths, memory, align, fwd)
+    check_reverse(v, prm, masks, cfg, (gen, att), rep, attention=(lengths, memory, align, aux.get('dalign')))
     if aux.get('grads') is not None:
-        check_closing(v, prm, aux['grads'], memory, align, mode, rep)
+        check_closing(v, prm, aux['grads'], memory, align, fwd, rep)
     return rep

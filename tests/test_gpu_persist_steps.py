@@ -1,10 +1,13 @@
 """Every step of the persistent decoder loops against an fp64 step computed from the loop's own saved state (tests/step_check.py),
 and bit-reproducibility of a bf16 training decode.  Run with -s to see the worst err / bound ratio of every stage."""
+import time
+
 import pytest
 import torch
 
 import decoder_cases
 import decoder_workspace
+import persist_geometry as G
 import step_check as S
 from multilingual_text_to_speech_b200._lib import DECODER_PARAM_FIELDS
 
@@ -52,6 +55,8 @@ def _decode(B, L, T, M, D, kind='zoneout', precision='bf16', seed=0, backward=Tr
 
 
 def _mode(shape, precision):
+    """The rounding model of the decode: one mode, or (forward, generator reverse, attention reverse) for a training step whose plan
+    runs only the generator reverse loop persistent (step_check.modes_of)"""
     import ctypes
     from multilingual_text_to_speech_b200 import _lib
     if precision == 'fp32':
@@ -59,10 +64,7 @@ def _mode(shape, precision):
     bits = _lib.load().b200tts_decoder_path(ctypes.byref(shape))
     if not shape.training:          # evaluation: the forward loops only
         bits &= 0b11
-        assert bits in (0, 0b11), bin(bits)
-    else:
-        assert bits in (0, 0b111111), bin(bits)
-    return 'persist' if bits else 'chain_bf16'
+    return G.mode_of(bits)
 
 
 def _mode_of(dims):
@@ -71,7 +73,11 @@ def _mode_of(dims):
     return _mode(_lib.DecoderShape(B, L, T, M, D, 256, 128, 32, 31, 80, _lib.CELL_ZONEOUT, 1, 0.1, 0.1, 0.5), 'bf16')
 
 
-def _step_check(B, L, T, M, D, kind='zoneout', precision='bf16', expect_mode=None, training=True):
+def _step_check(B, L, T, M, D, kind='zoneout', precision='bf16', expect_mode=None, training=True, key=None):
+    """key: the loop geometry key (persist_geometry.py) the shape must still have"""
+    if key is not None:
+        assert G.key_of(B, L, M, D, training) == key, (G.key_of(B, L, M, D, training), key)
+    t0 = time.perf_counter()
     r = _decode(B, L, T, M, D, kind, precision, backward=training, training=training)
     mode = _mode(r['shape'], precision)
     if expect_mode:
@@ -87,6 +93,7 @@ def _step_check(B, L, T, M, D, kind='zoneout', precision='bf16', expect_mode=Non
     title = f'[B{B} L{L} T{T} M{M} D{D} {kind} {"train" if training else "eval"} {precision} {mode}] '
     print()
     print('\n'.join(rep.lines(title)))
+    print(f'{title}key {key}: worst err/bound {rep.max_ratio():.3e} over {len(rep.worst)} stages, {time.perf_counter() - t0:.1f} s')
     assert rep.failures() == {}, (title, rep.failures())
     return rep
 
@@ -101,6 +108,34 @@ def test_persistent_loop_steps_within_bounds(shape, kind):
 def test_persistent_forward_loop_steps_within_bounds_eval(kind):
     """evaluation mode (no keep masks; zoneout blends with the expected keep rate) on the persistent forward loops"""
     _step_check(16, 77, 12, 288, 1024, kind=kind, expect_mode='persist', training=False)
+
+
+def _case_id(c):
+    B, L, T, M, D, training = c
+    return f'B{B}_L{L}_T{T}_M{M}_D{D}_{"train" if training else "eval"}'
+
+
+@pytest.mark.parametrize('case', sorted(G.REPRESENTATIVES), ids=_case_id)
+def test_every_loop_geometry_steps_within_bounds(case):
+    """One representative per geometry key the plan can produce (persist_geometry.py): evaluation decodes through check_forward, training
+    steps forward and backward through check_all, each recurrence under the rounding model of the loop that ran it."""
+    B, L, T, M, D, training = case
+    key = G.REPRESENTATIVES[case]
+    kind = ('zoneout', 'dropout')[sorted(G.REPRESENTATIVES).index(case) % 2]
+    _step_check(B, L, T, M, D, kind, expect_mode=G.mode_of(key[1]), training=bool(training), key=key)
+
+
+@pytest.mark.parametrize('case', sorted(G.PAST_LIMITS), ids=_case_id)
+def test_steps_past_the_loop_limits_within_bounds(case):
+    B, L, T, M, D, training = case
+    _step_check(B, L, T, M, D, 'zoneout', expect_mode=G.mode_of(G.PAST_LIMITS[case]), training=bool(training))
+
+
+def test_alignment_sized_eval_decode_steps_within_bounds():
+    B, L, T, M, D, training = G.ALIGNMENT_SIZED
+    key = G.key_of(B, L, M, D, training)
+    assert key in G.REPRESENTATIVES.values(), key
+    _step_check(B, L, T, M, D, 'zoneout', expect_mode='persist', training=False, key=key)
 
 
 def test_persistent_loop_steps_within_bounds_benchmark_shape():

@@ -42,6 +42,22 @@ def _flags(rep, stage, step):
     assert bad[stage] == [step], (stage, step, bad)
 
 
+def test_mixed_plan_checks_each_recurrence_under_the_loop_that_ran_it():
+    """A training step whose plan runs only the generator reverse loop persistent (forward and attention reverse on the bf16 chains): the
+    generator reverse is checked from its bf16 history under the persistent loop's model, everything else under the chains' model."""
+    mixed = ('chain_bf16', 'persist', 'chain_bf16')
+    v, prm, masks, cfg, lengths, memory, align, aux = args = _synthetic(mode='chain_bf16')
+    v['dggb'] = v['dgg'].to(torch.bfloat16)
+    rep = _check(*args, mode=mixed)
+    assert rep.failures() == {}, '\n'.join(rep.lines())
+    assert 'dggb_rn' in rep.worst and not {'aib_rn', 'hgb_rn', 'dgab_rn'} & set(rep.worst)
+    i = 3
+    v['dggb'][i, 2, 5] = (v['dgg'][i, 2, 5] * 1.01).to(torch.bfloat16)      # the history the next reverse step multiplied is off
+    _flags(_check(*args, mode=mixed), 'dggb_rn', i)
+    with pytest.raises(AssertionError):                                    # no plan runs the forward loops without the attention reverse loop
+        _check(*args, mode=('persist', 'persist', 'chain_bf16'))
+
+
 def test_stale_h_operand_is_flagged():
     """the generator product of step i used one utterance's h row of step i-1"""
     v, prm, masks, cfg, lengths, memory, align, aux = args = _synthetic()
