@@ -182,6 +182,18 @@ typedef struct {
     const uint8_t* mask_gen_c;    /* [S, B, D] zoneout only */
     const uint8_t* mask_step_prenet0; /* [S, B, P] prenet masks of free-running steps */
     const uint8_t* mask_step_prenet1; /* [S, B, P] */
+    /* forced synthesis, b200tts_decoder_forward_chunk only; forced_count = 0 (a zero-initialised struct) is off.  Otherwise the
+       forced_count (F, 1 <= F <= B) distinct rows forced_rows[0 .. F) (device int32, each in [0, B)) take each step's attention weights
+       from forced_alignment (device [S, F, L], time-major: row [i, k] is step i of utterance forced_rows[k]) instead of computing them.
+       For such an utterance b at step i: the alignment row is the supplied row with exact zeros at l >= length_b; location-sensitive
+       attention carries cum_weights + that row, forward attention carries that row as alpha; the context is the sum over l < length_b
+       of w[l] * memory[b, l, :], in the order the computed step sums it (from position 0, or with a window from the row's first
+       non-zero weight).  No query, location feature, energy or softmax is computed for the row.  When F < B the computed step runs over
+       every row first (a window applies to it) and the forced step then overwrites the forced rows; when F = B only the forced step
+       runs.  b200tts_decoder_forward and _backward reject forced rows. */
+    const int32_t* forced_rows;
+    int forced_count;
+    const float* forced_alignment;
 } b200tts_decoder_inputs;
 
 typedef struct {

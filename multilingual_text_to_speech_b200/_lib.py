@@ -36,7 +36,8 @@ class DecoderParams(Structure):
 class DecoderInputs(Structure):
     _fields_ = [(n, c_void_p) for n in ('memory', 'text_lengths', 'target', 'teacher', 'mask_prenet0', 'mask_prenet1',
                                         'mask_att_h', 'mask_att_c', 'mask_gen_h', 'mask_gen_c', 'mask_step_prenet0',
-                                        'mask_step_prenet1')]
+                                        'mask_step_prenet1', 'forced_rows')] + \
+        [('forced_count', c_int), ('forced_alignment', c_void_p)]
 
 
 class DecoderOutputs(Structure):

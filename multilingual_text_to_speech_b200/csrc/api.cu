@@ -456,12 +456,15 @@ size_t b200tts_decoder_bwd_workspace_bytes(const b200tts_decoder_shape* shape) {
     return decoder_bwd_workspace_floats(step_shape(*shape)) * sizeof(float);
 }
 
+static bool forced_inputs(const b200tts_decoder_inputs& in) { return in.forced_count != 0 || in.forced_rows || in.forced_alignment; }
+
 int b200tts_decoder_forward(const b200tts_decoder_shape* shape, const b200tts_decoder_params* params,
                             const b200tts_decoder_inputs* in, const b200tts_decoder_outputs* out, void* workspace,
                             size_t workspace_bytes, void* stream) {
     B200_REQUIRE(shape && params && in && out, "decoder_forward: null argument");
     B200_REQUIRE(shape->att_window_back == 0 && shape->att_window_ahead == 0,
                  "decoder_forward: an attention window is for synthesis only (b200tts_decoder_forward_chunk)");
+    B200_REQUIRE(!forced_inputs(*in), "decoder_forward: forced attention rows are for synthesis only (b200tts_decoder_forward_chunk)");
     B200_TRY(require_device());
     return decoder_forward_impl(*shape, *params, *in, *out, (float*)workspace, workspace_bytes, (cudaStream_t)stream);
 }
@@ -473,6 +476,10 @@ int b200tts_decoder_forward_chunk(const b200tts_decoder_shape* shape, const b200
     B200_REQUIRE(state->att_h && state->att_c && state->gen_h && state->gen_c && state->context && state->cum_weights && state->frame,
                  "decoder_forward_chunk: every state buffer is required");
     B200_REQUIRE(!attention_window(*shape) || state->attended, "decoder_forward_chunk: an attention window needs state->attended");
+    B200_REQUIRE(in->forced_count >= 0 && in->forced_count <= shape->B,
+                 "decoder_forward_chunk: forced_count %d outside [0, B=%d]", in->forced_count, shape->B);
+    B200_REQUIRE(in->forced_count == 0 ? !in->forced_rows && !in->forced_alignment : in->forced_rows && in->forced_alignment,
+                 "decoder_forward_chunk: forced_rows and forced_alignment are given exactly when forced_count > 0");
     B200_REQUIRE(shape->R < 0 || shape->T % frames_per_step(*shape) == 0,
                  "decoder_forward_chunk: a chunk holds whole decoder steps (T=%d is not a multiple of R=%d)", shape->T, shape->R);
     B200_TRY(require_device());
@@ -496,6 +503,7 @@ int b200tts_decoder_backward(const b200tts_decoder_shape* shape, const b200tts_d
                  "decoder_backward: null argument");
     B200_REQUIRE(shape->att_window_back == 0 && shape->att_window_ahead == 0,
                  "decoder_backward: an attention window is for synthesis only (b200tts_decoder_forward_chunk)");
+    B200_REQUIRE(!forced_inputs(*in), "decoder_backward: forced attention rows are for synthesis only (b200tts_decoder_forward_chunk)");
     B200_TRY(require_device());
     return decoder_backward_impl(*shape, *params, *in, *fwd_out, *dout, (const float*)fwd_workspace, (float*)bwd_workspace,
                                  bwd_workspace_bytes, *d_params, d_memory, (cudaStream_t)stream);

@@ -440,6 +440,77 @@ __global__ void __launch_bounds__(ATT_THREADS) fwd_attn_fwd_kernel(const FwdAttn
     }
 }
 
+// =============================================================================================
+// Forced attention step (b200tts_decoder_inputs.forced_*), one CTA per forced utterance: the weights are the caller's row, so there is
+// no query, location feature, energy or softmax.  The context runs the loops of attn_fwd_kernel<false> (warp-strided over l, then the
+// ordered sum across warps), so the row a computed step produced gives back that step's context bit for bit.
+// =============================================================================================
+struct ForcedAttnArgs {
+    const int* rows; int F;            // [F] device rows of the forced utterances
+    const float* weights;              // [F, L] this step's supplied rows
+    const float* memory;               // [B, L, M]
+    const int* lengths;                // [B]
+    const float* prev; float* next;    // [B, L] cum_weights (location-sensitive) or alpha (forward attention)
+    float* align; long long align_bstride;    // &align[0, i, 0]; stride between utterances
+    float* ctx_out; int ld_ctx;        // [B, ld]
+    int B, L, M;
+    int accumulate;                    // 1: next = prev + w (location-sensitive); 0: next = w (forward attention)
+    int from_first;                    // 1 (a window): the context starts at the row's first non-zero weight, where a windowed step starts
+};
+
+static inline size_t forced_attn_smem_floats(int L, int M) { return (size_t)((L + 3) & ~3) + (size_t)(ATT_THREADS / 32) * M; }
+
+__global__ void __launch_bounds__(ATT_THREADS) attn_forced_fwd_kernel(const ForcedAttnArgs p) {
+    extern __shared__ __align__(16) float sm[];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    constexpr int NW = ATT_THREADS / 32;
+    const int b = p.rows[blockIdx.x];
+    if (b < 0 || b >= p.B) return;      // the host entry point documents the range; a row outside it is left alone
+    const int L = p.L, M = p.M;
+    float* e = sm;
+    float* cred = e + ((L + 3) & ~3);
+    __shared__ int first;
+    int len = p.lengths[b];
+    len = len < 0 ? 0 : (len > L ? L : len);
+    if (tid == 0) first = len;
+    __syncthreads();
+    const float* src = p.weights + (size_t)blockIdx.x * L;
+    for (int l = tid; l < L; l += ATT_THREADS) {
+        const float w = l < len ? src[l] : 0.f;
+        e[l] = w;
+        p.align[(size_t)b * p.align_bstride + l] = w;
+        p.next[(size_t)b * L + l] = p.accumulate ? p.prev[(size_t)b * L + l] + w : w;
+        if (p.from_first && w != 0.f) atomicMin(&first, l);
+    }
+    __syncthreads();
+    const int lo = p.from_first ? first : 0;
+
+    float acc[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) acc[j] = 0.f;
+    for (int l = lo + warp; l < len; l += NW) {
+        const float w = e[l];
+        const float* row = p.memory + ((size_t)b * L + l) * M;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            const int m = lane + 32 * j;
+            if (m < M) acc[j] = fmaf(w, row[m], acc[j]);
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+        const int m = lane + 32 * j;
+        if (m < M) cred[warp * M + m] = acc[j];
+    }
+    __syncthreads();
+    for (int m = tid; m < M; m += ATT_THREADS) {
+        float s = 0.f;
+#pragma unroll
+        for (int w = 0; w < NW; ++w) s += cred[w * M + m];
+        p.ctx_out[(size_t)b * p.ld_ctx + m] = s;
+    }
+}
+
 // The initial state of a decode (tacotron2.py:164-168): every buffer zero, and for forward attention alpha_0 = one-hot at position 0
 // (ForwardAttention.reset, attention.py:103-106).  Its one definition: the first chunk of a decode writes it into the step-0 rows of its
 // workspace, b200tts_decoder_state_reset_rows into the listed rows of a carried state.
@@ -531,6 +602,19 @@ int launch_fwd_attn(const FwdAttnArgs& a, cudaStream_t st) {
     return B200TTS_OK;
 }
 
+int launch_forced_attn(const ForcedAttnArgs& a, cudaStream_t st) {
+    const size_t smem = forced_attn_smem_floats(a.L, a.M) * sizeof(float);
+    B200_REQUIRE(smem <= 227 * 1024, "forced attention step: shared memory %zu B exceeds 227 KB (L=%d M=%d)", smem, a.L, a.M);
+    static size_t configured = 48 * 1024;
+    if (smem > configured) {
+        B200_CUDA(cudaFuncSetAttribute(attn_forced_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        configured = smem;
+    }
+    attn_forced_fwd_kernel<<<a.F, ATT_THREADS, smem, st>>>(a);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
 }  // namespace
 
 int launch_copy2d(float* dst, int ldd, const float* src, int lds, int rows, int cols, cudaStream_t st) {
@@ -615,6 +699,8 @@ int prenet_rows(const FwdCtx& c, int rows, const float* x, float* p0, float* p1,
     return B200TTS_OK;
 }
 
+int att_step_computed(const FwdCtx& c, int i, float* align_out);
+
 int att_step(const FwdCtx& c, int i, float* align_out) {
     const auto& s = c.s; const auto& l = c.lay;
     const size_t BD = (size_t)s.B * s.D, B4D = 4 * BD, MD = s.M + s.D;
@@ -632,9 +718,30 @@ int att_step(const FwdCtx& c, int i, float* align_out) {
     ca.mask_h = c.in.mask_att_h ? c.in.mask_att_h + (size_t)i * BD : nullptr;
     ca.mask_c = c.in.mask_att_c ? c.in.mask_att_c + (size_t)i * BD : nullptr;
     ca.kind = s.cell_kind; ca.training = s.training; ca.rate_h = s.rate_h; ca.rate_c = s.rate_c;
-    ca.Wq = c.w.attn_query; ca.A = s.A; ca.qpart = c.at(l.qpart);
+    const int F = c.in.forced_count;
+    if (F < s.B) { ca.Wq = c.w.attn_query; ca.A = s.A; ca.qpart = c.at(l.qpart); }     // every row forced: no query is needed
     ca.B = s.B; ca.D = s.D;
     B200_TRY(launch_cell_fwd(ca, c.st));
+    if (F > 0) {
+        if (F < s.B) B200_TRY(att_step_computed(c, i, align_out));
+        ForcedAttnArgs fa{};
+        fa.rows = c.in.forced_rows; fa.F = F; fa.weights = c.in.forced_alignment + (size_t)i * F * s.L;
+        fa.memory = c.in.memory; fa.lengths = c.in.text_lengths;
+        fa.prev = c.at(l.cum) + (size_t)i * s.B * s.L; fa.next = c.at(l.cum) + (size_t)(i + 1) * s.B * s.L;
+        fa.align = align_out + (size_t)i * s.L; fa.align_bstride = (long long)s.T * s.L;
+        fa.ctx_out = ai_n; fa.ld_ctx = (int)MD;
+        fa.B = s.B; fa.L = s.L; fa.M = s.M;
+        fa.accumulate = !forward_attention(s); fa.from_first = attention_window(s);
+        return launch_forced_attn(fa, c.st);
+    }
+    return att_step_computed(c, i, align_out);
+}
+
+// the attention step every row computes from its query (b200tts_decoder_inputs.forced_count < B)
+int att_step_computed(const FwdCtx& c, int i, float* align_out) {
+    const auto& s = c.s; const auto& l = c.lay;
+    const size_t MD = s.M + s.D;
+    float* ai_n = c.at(l.ai) + (size_t)(i + 1) * s.B * MD;
     if (forward_attention(s)) {
         FwdAttnArgs fa{};
         fa.qpart = c.at(l.qpart); fa.nq = l.ncell_blocks;

@@ -410,9 +410,11 @@ class DecoderState:
                                                     self.attended)])
 
 
-def decoder_forward_chunk(cfg, memory, text_lengths, params, state, frames):
+def decoder_forward_chunk(cfg, memory, text_lengths, params, state, frames, forced=None):
     """`frames` free-running frames (frames / r decoder steps; a multiple of r) continuing from `state` (updated in place); no autograd
     (inference).  cfg.att_window, if set, confines each step's attention to the window around state.attended, which the call advances.
+    forced: None, or (rows, weights) with rows a device int32 tensor [F] of distinct rows and weights a device float32 tensor
+    [frames / r, F, L] whose row [i, k] is the attention of step i of utterance rows[k] (b200tts_decoder_inputs.forced_*).
     -> spectrogram [B, frames, N], stop [B, frames], alignment [B, frames / r, L]."""
     _require_cuda(memory, text_lengths, *params)
     with torch.no_grad():
@@ -436,11 +438,64 @@ def decoder_forward_chunk(cfg, memory, text_lengths, params, state, frames):
         stop = torch.empty(B, T, device=memory.device, dtype=torch.float32)
         align = torch.empty(B, cfg.steps(T), L, device=memory.device, dtype=torch.float32)
         outs = DecoderOutputs(ptr(spec), ptr(stop), ptr(align))
+        if forced is not None:
+            rows, weights = forced
+            assert rows.dtype == torch.int32 and rows.is_cuda and rows.is_contiguous() and rows.dim() == 1, rows
+            assert weights.dtype == torch.float32 and weights.is_cuda and weights.is_contiguous() and \
+                tuple(weights.shape) == (cfg.steps(T), rows.shape[0], L), tuple(weights.shape)
+            inputs.forced_rows, inputs.forced_count, inputs.forced_alignment = ptr(rows), rows.shape[0], ptr(weights)
         st = state.struct()
         check(lib.b200tts_decoder_forward_chunk(ctypes.byref(shape), ctypes.byref(pstruct), ctypes.byref(inputs), ctypes.byref(outs),
                                                 ctypes.byref(st), int(state.first), ptr(ws), nbytes, _stream()), 'b200tts_decoder_forward_chunk')
         state.first = False
     return spec, stop, align
+
+
+def _durations_host(durations, name):
+    d = np.asarray(durations.detach().cpu() if torch.is_tensor(durations) else durations)
+    if d.ndim != 1 or d.shape[0] < 1 or not np.issubdtype(d.dtype, np.integer):
+        raise ValueError(f'{name}: durations must be a non-empty 1-D integer array [L], got shape {d.shape} of {d.dtype}')
+    if (d < 0).any():
+        raise ValueError(f'{name}: durations must be >= 0')
+    return d.astype(np.int64)
+
+
+def durations_to_alignment(durations, r=1):
+    """Frames per symbol (int [L], each >= 0) -> the one-hot attention rows [S, L] float32 of a decode with r frames per step that gives
+    each symbol its frames: S = ceil(sum(d) / r), and step s attends the symbol whose frame range [C_{j-1}, C_j) (C the cumulative
+    frames) holds frame s r.  A symbol with no frames is never attended.  For Alignment.durations from Tacotron.align these are the
+    one-hot rows of the monotonic path (Alignment.step_durations).  On the durations' device (the host for arrays and lists)."""
+    d = _durations_host(durations, 'durations_to_alignment')
+    r = int(r)
+    if r < 1:
+        raise ValueError(f'durations_to_alignment: r must be >= 1 (got {r})')
+    total = int(d.sum())
+    if total == 0:
+        raise ValueError('durations_to_alignment: the durations total 0 frames')
+    S = -(-total // r)
+    sym = np.searchsorted(np.cumsum(d), np.arange(S) * r, side='right')
+    rows = np.zeros((S, d.shape[0]), dtype=np.float32)
+    rows[np.arange(S), sym] = 1.0
+    return torch.from_numpy(rows).to(durations.device if torch.is_tensor(durations) else 'cpu')
+
+
+def scale_durations(durations, factor):
+    """Speaking-rate control: frames per symbol (int [L], each >= 0) stretched by `factor` (> 1 slower, < 1 faster) -> int [L] of the
+    input's type.  The new symbol boundaries are B_j = floor(factor C_j + 0.5) in float64 (C the cumulative frames) and each new
+    duration is B_j - B_{j-1}, so the total is the rounded scaled total and no rounding error accumulates.  At strong speed-ups a short
+    symbol can get 0 frames, and then it is not attended (durations_to_alignment).  ValueError for a factor that is not finite or
+    is <= 0, and for a result of 0 frames."""
+    d = _durations_host(durations, 'scale_durations')
+    f = float(factor)
+    if not np.isfinite(f) or f <= 0:
+        raise ValueError(f'scale_durations: factor must be finite and > 0 (got {factor!r})')
+    bounds = np.floor(f * np.cumsum(d).astype(np.float64) + 0.5).astype(np.int64)
+    out = np.diff(bounds, prepend=0)
+    if int(bounds[-1]) == 0:
+        raise ValueError(f'scale_durations: {int(d.sum())} frames scaled by {f} total 0 frames')
+    if torch.is_tensor(durations):
+        return torch.from_numpy(out).to(device=durations.device, dtype=durations.dtype)
+    return out.astype(np.asarray(durations).dtype)
 
 
 # the persistent loop kernels of the bf16 mode hold the whole batch in one MMA tile (<= 64 utterances)

@@ -12,44 +12,47 @@ touches it (DESIGN 8.1).  Its streams need at least 2 frames instead of 21."""
 from typing import Union
 
 from .griffinlim import GriffinLimVocoder
-from .tacotron2 import MAX_STREAM_TEXTS, Tacotron, _check_batch_inputs
+from .tacotron2 import MAX_STREAM_TEXTS, Tacotron, _check_batch_inputs, _plan_lists
 from .wavernn import WaveRNN
 
 Vocoder = Union[WaveRNN, GriffinLimVocoder]
 
 
 def speech_stream(tacotron: Tacotron, wavernn: Vocoder, text, speaker=None, language=None, mel_transform=None, chunk_frames=None,
-                  uniforms=None, generator=None, preemphasis=0.0, target=None, overlap=None):
+                  uniforms=None, generator=None, preemphasis=0.0, target=None, overlap=None, durations=None, alignment=None):
     """Yields waveform chunks of `text` as the decoder produces it: tacotron.inference_stream(text, speaker, language, chunk_frames) fed,
     through mel_transform, into wavernn.generate_stream(…, uniforms, generator, preemphasis).  mel_transform (default: none) maps a
     post-net chunk [num_mels, n] to the vocoder's input frames [feat_dims, n] frame by frame, for example
     utils.audio.denormalize_spectrogram; it must not look at neighbouring frames, since each chunk is transformed alone.  The audio equals
     wavernn.generate(mel, target=F hop, overlap=0) of the concatenated transformed mel, bit for bit given the same uniform tape.  With
-    target and overlap (folded streaming, WaveRNN.generate_stream's), it equals wavernn.generate(mel, target, overlap) instead."""
-    mels = tacotron.inference_stream(text, speaker, language, chunk_frames)
+    target and overlap (folded streaming, WaveRNN.generate_stream's), it equals wavernn.generate(mel, target, overlap) instead.
+    `durations` or `alignment` sets the decode's attention (Tacotron.inference)."""
+    mels = tacotron.inference_stream(text, speaker, language, chunk_frames, durations, alignment)
     if mel_transform is not None:
         mels = (mel_transform(m) for m in mels)
     yield from wavernn.generate_stream(mels, uniforms, generator, preemphasis, target, overlap)
 
 
 def speech_streams(tacotron: Tacotron, wavernn: Vocoder, texts, speakers=None, languages=None, mel_transform=None, chunk_frames=None,
-                   uniforms=None, generator=None, preemphasis=0.0, target=None, overlap=None):
+                   uniforms=None, generator=None, preemphasis=0.0, target=None, overlap=None, durations=None, alignments=None):
     """speech_stream for up to 64 texts at once: yields (i, waveform chunk) for text i.  Every text is submitted to one SpeechServer(…,
     max_streams=len(texts)) at once and the server steps until it is idle: each step runs one decoder call over the texts still decoding
     (text i reads column i of a recorded mask tape), feeds its post-net chunks (through mel_transform) into the vocoder pool and makes one
     pool.run().  uniforms: None or one tape [1, T_i, U] per text ([K_i, target + 2 overlap, U] with target and overlap).  Each text's audio equals speech_stream of that text alone, bit for bit
     given its tape, in fp32 mode (where the decoded frames of a group equal those of single texts).  A text that decodes fewer than the
     vocoder's minimum (21 frames for a WaveRNN, 2 for a GriffinLimVocoder) raises ValueError when its stream ends, as speech_stream does, and
-    that ends the generator for every text of the group."""
+    that ends the generator for every text of the group.  durations / alignments: as Tacotron.inference_batch takes them."""
     texts = list(texts)
     if len(texts) > MAX_STREAM_TEXTS:
         raise ValueError(f'inference_streams: at most {MAX_STREAM_TEXTS} texts decode as one group (got {len(texts)})')
     if uniforms is not None and len(uniforms) != len(texts):
         raise ValueError(f'{len(uniforms)} uniform tapes for {len(texts)} texts')
     speakers, languages = _check_batch_inputs(texts, speakers, languages)
+    durations, alignments = _plan_lists(texts, durations, alignments)
     server = SpeechServer(tacotron, wavernn, len(texts), mel_transform, chunk_frames, preemphasis, generator, target, overlap)
     ids = [server.submit(text, None if speakers is None else speakers[i], None if languages is None else languages[i],
-                         uniforms=None if uniforms is None else uniforms[i]) for i, text in enumerate(texts)]
+                         uniforms=None if uniforms is None else uniforms[i], durations=durations[i], alignment=alignments[i])
+           for i, text in enumerate(texts)]
     text_of = {rid: i for i, rid in enumerate(ids)}
     while server.pending or server.active:
         out = server.step()
@@ -63,8 +66,8 @@ class _Request:
     """One request of a SpeechServer: its inputs until admission, then its decoder text id (None once its mel has ended) and its vocoder
     stream id."""
 
-    def __init__(self, text, speaker, language, seed, masks, uniforms):
-        self.inputs = (text, speaker, language, seed, masks)
+    def __init__(self, text, speaker, language, seed, masks, uniforms, plan):
+        self.inputs, self.plan = (text, speaker, language, seed, masks), plan
         self.uniforms, self.seed = uniforms, seed
         self.tid = self.sid = None
 
@@ -103,14 +106,16 @@ class SpeechServer:
     def active(self):
         return [rid for rid in self.requests if rid not in self.pending]
 
-    def submit(self, text, speaker=None, language=None, seed=None, masks=None, uniforms=None):
-        """Queues a request -> its id.  Its inputs are checked now (ValueError)."""
-        self.decoder.check(text, speaker, language, seed, masks)
+    def submit(self, text, speaker=None, language=None, seed=None, masks=None, uniforms=None, durations=None, alignment=None):
+        """Queues a request -> its id.  Its inputs are checked now (ValueError).  `durations` or `alignment` sets its decode's attention
+        (DecoderPool.open)."""
+        plan = {k: v for k, v in (('durations', durations), ('alignment', alignment)) if v is not None}
+        self.decoder.check(text, speaker, language, seed, masks, **plan)
         if uniforms is not None:
             self.pool.check_tape(uniforms)
         rid = self.next_id
         self.next_id += 1
-        self.requests[rid] = _Request(text, speaker, language, seed, masks, uniforms)
+        self.requests[rid] = _Request(text, speaker, language, seed, masks, uniforms, plan)
         self.pending.append(rid)
         return rid
 
@@ -131,8 +136,8 @@ class SpeechServer:
             rid = self.pending.pop(0)
             req = self.requests[rid]
             req.sid = self.pool.open(req.uniforms, req.seed)
-            req.tid = self.decoder.open(*req.inputs)
-            req.inputs = None
+            req.tid = self.decoder.open(*req.inputs, **req.plan)
+            req.inputs = req.plan = None
 
     def _fail(self, rid, message):
         req = self.requests.pop(rid)

@@ -196,6 +196,19 @@ class Decoder(torch.nn.Module):
                     self.cut = self.seen
             return self.cut
 
+    class _PlanRule:
+        """The stop rule of a forced row (a row decoding from an attention plan): a fixed cut of the plan's frames, known when the row
+        opens.  The stop logits are still computed and fed, but they do not end the row."""
+
+        def __init__(self, frames):
+            self.frames, self.seen, self.cut = frames, 0, None
+
+        def feed(self, logits):
+            self.seen += len(logits)
+            if self.seen >= self.frames:
+                self.cut = self.frames
+            return self.cut
+
     def _memory(self, encoded_input, speaker, language):
         if hp.multi_speaker and self._speaker_embedding is not None:
             encoded_input = self._add_conditional_embedding(encoded_input, self._speaker_embedding, speaker)
@@ -220,7 +233,8 @@ class Decoder(torch.nn.Module):
         """Positions (into `rows`, the original indices of the utterances still decoding) of the utterances whose stop cut is unknown."""
         return [j for j, r in enumerate(rows) if rules[r].cut is None]
 
-    def _inference_chunks(self, encoded_input, mask, speaker, language, att_extent=0, tape_columns=None, chunk_frames=None, att_window=None):
+    def _inference_chunks(self, encoded_input, mask, speaker, language, att_extent=0, tape_columns=None, chunk_frames=None, att_window=None,
+                          plans=None):
         """The chunk loop of free-running inference (tacotron2.py:148-209 with target=None) over a batch whose texts all open at the
         first call: every chunk is one library call of chunk_frames (default inference_chunk) frames rounded down to whole steps; after
         each it feeds the chunk's stop logits to the utterances' stop rules and yields (rows, spec [b, Tc, N], stop [b, Tc], alignment
@@ -228,12 +242,15 @@ class Decoder(torch.nn.Module):
         utterance, done the frames decoded so far.  Then an utterance whose cut is known leaves the decode (_DecodeRows.retire) and the next
         chunk runs at the smaller batch.  The loop ends when every cut is known or hp.max_output_length frames are decoded.  The rule reads
         the r stop logits of each step in frame order.  Utterance b reads column tape_columns[b] (default b) of an active mask tape.
-        att_window: None or (back, ahead), windowed attention (inference_attention_window)."""
+        att_window: None or (back, ahead), windowed attention (inference_attention_window).  plans: None or one attention plan (_forced_plan)
+        or None per utterance."""
         memory = self._memory(encoded_input, speaker, language)
         B = memory.shape[0]
         columns = list(range(B)) if tape_columns is None else list(tape_columns)
         rows = _DecodeRows(self, att_extent, att_window)
         rows.add(memory, [int(n) for n in mask.sum(dim=1).tolist()], list(range(B)), [('shared', c) for c in columns])
+        if plans is not None:
+            rows.set_plans(plans)
         rules = list(rows.rules)
         chunk_steps = max(1, (self.inference_chunk if chunk_frames is None else int(chunk_frames)) // self._outputs_per_step)
         while len(rows):
@@ -241,11 +258,12 @@ class Decoder(torch.nn.Module):
             yield list(rows.keys), spec, stop, align, rules, rows.done[0]
             rows.retire()
 
-    def _decode_inference(self, encoded_input, mask, speaker, language, att_extent=0, tape_columns=None, att_window=None):
+    def _decode_inference(self, encoded_input, mask, speaker, language, att_extent=0, tape_columns=None, att_window=None, plans=None):
         """Free-running decode in chunks with carried state and early exit (_inference_chunks).  B == 1 reproduces the reference; B > 1
         (which the reference cannot run: it uses the stop token as a Python bool) keeps one stop rule per utterance.  `att_extent` = 1 runs
         forward attention over each utterance's own length; `tape_columns` gives each utterance's column of a recorded mask tape (default:
-        column b for utterance b); `att_window` confines each step's attention (inference_attention_window).
+        column b for utterance b); `att_window` confines each step's attention (inference_attention_window); `plans` gives utterances
+        their attention (_forced_plan).
         -> (spectrogram [B, T', N], stop [B, T'], alignment [B, ceil(T' / r), L], cuts): T' = max(cuts) frames; utterance b is zero past
         cuts[b] (its alignment past ceil(cuts[b] / r) steps).  hp.max_output_length counts frames."""
         B, L = encoded_input.shape[0], encoded_input.shape[1]
@@ -254,7 +272,7 @@ class Decoder(torch.nn.Module):
         outs = [[] for _ in range(B)]
         done = 0
         for rows, spec, stop, align, rules, done in self._inference_chunks(encoded_input, mask, speaker, language, att_extent, tape_columns,
-                                                                           att_window=att_window):
+                                                                           att_window=att_window, plans=plans):
             if align.shape[2] < L:          # the chunk ran after the longest text left: its weights past the shorter ones are zero
                 align = TF.pad(align, (0, L - align.shape[2]))
             for j, u in enumerate(rows):
@@ -396,20 +414,30 @@ class Tacotron(torch.nn.Module):
         post_prediction = post_prediction * target_mask
         return post_prediction, pre_prediction, stop_token, alignment, speaker_prediction, encoder_output
 
-    def inference(self, text, speaker=None, language=None):
+    def inference(self, text, speaker=None, language=None, durations=None, alignment=None):
         """synthesize.py entry point (tacotron2.py:387-408): text int64 [L], speaker int64 [1] | None, language int64 [1] |
         float [1, L, G] (per-character language mixing) | None -> post-net spectrogram [num_mels, T'].  The one-utterance case of
-        `inference_batch`."""
-        return self.inference_batch([text], None if speaker is None else [speaker], None if language is None else [language])[0]
+        `inference_batch`; `durations` or `alignment` sets the decode's attention as inference_batch's do."""
+        return self.inference_batch([text], None if speaker is None else [speaker], None if language is None else [language],
+                                    durations=None if durations is None else [durations],
+                                    alignments=None if alignment is None else [alignment])[0]
 
-    def inference_batch(self, texts, speakers=None, languages=None, max_batch=64):
+    def inference_batch(self, texts, speakers=None, languages=None, max_batch=64, durations=None, alignments=None):
         """Synthesise many utterances at once: texts is a list of int64 [L_i]; speakers / languages are None or lists with one entry per
         text in the forms `inference` takes (speaker int64 [1]; language int64 [1] or float [1, L_i, G]).  -> one post-net spectrogram
         [num_mels, T_i] per text, in input order.  Texts are sorted by length and decoded in padded groups of at most max_batch (eval
         mode, no grad); each utterance's output equals `inference` of it alone given the same prenet dropout masks (a recorded tape,
         [T, len(texts), P] with one column per text).  Without a tape a batched run draws other masks than single runs do.
-        hp.inference_attention_window is read once per call."""
+        hp.inference_attention_window is read once per call.
+
+        Forced synthesis: `durations` (int [L_i] frames per symbol, each >= 0) or `alignments` (float [S_i, L_i], finite and >= 0, for
+        example Tacotron.align's alignment[b, :S_b, :L_b]) is None or a list with one entry or None per text; a text with an entry decodes
+        with each step's attention set by it instead of computed (functional.durations_to_alignment turns durations into one-hot rows),
+        and its output has exactly sum(d_i) frames, or S_i r, whatever the stop token does.  A text takes at most one of the two.  Forced
+        and free texts share groups; each output equals the text decoded alone.  ValueError before any device work for malformed
+        plans (_forced_plan)."""
         speakers, languages = _check_batch_inputs(texts, speakers, languages)
+        plans = _batch_plans(self._decoder, texts, durations, alignments)
         window = inference_attention_window()
         was_training = self.training
         self.eval()
@@ -418,7 +446,8 @@ class Tacotron(torch.nn.Module):
             with torch.no_grad():
                 for group in _batch_plan([int(t.shape[0]) for t in texts], max_batch):
                     posts = self._inference_group([texts[i] for i in group], None if speakers is None else [speakers[i] for i in group],
-                                                  None if languages is None else [languages[i] for i in group], group, window)
+                                                  None if languages is None else [languages[i] for i in group], group, window,
+                                                  [plans[i] for i in group])
                     for i, post in zip(group, posts):
                         outputs[i] = post
         finally:
@@ -472,37 +501,39 @@ class Tacotron(torch.nn.Module):
         durations[rows, last] -= torch.tensor([s * r - t for s, t in zip(steps, frames)], device=durations.device, dtype=torch.int32)
         return Alignment(alignment, durations, step_durations, path_logp, **F.alignment_scores(alignment, symbols, steps))
 
-    def inference_stream(self, text, speaker=None, language=None, chunk_frames=None):
+    def inference_stream(self, text, speaker=None, language=None, chunk_frames=None, durations=None, alignment=None):
         """Streaming `inference`: a generator of post-net spectrogram chunks [num_mels, n_k] whose concatenation is inference(text,
         speaker, language), the same stop cut and, given the same prenet dropout masks, the same decoded frames.  Takes the inputs
         `inference` takes.  The decoder runs in chunks of chunk_frames frames (default Decoder.inference_chunk, rounded down to whole
         decoder steps); after every chunk one item is yielded: the post-net over the frames that became final (stream_release), computed
         over a window with the post-net's halo of decoded frames on the left and, once the cut is known, the zeros past it on the right.
         An item may hold no frames (a chunk shorter than the halo).  The model is in eval mode, without autograd, until the generator
-        ends or is closed; prenet dropout stays on, as in `inference`, and a MaskSource tape is replayed the same way.  The one-text case
-        of `inference_streams`."""
+        ends or is closed; prenet dropout stays on, as in `inference`, and a MaskSource tape is replayed the same way.  `durations` or
+        `alignment` sets the attention as in `inference`.  The one-text case of `inference_streams`."""
         for item in self._streams([text], None if speaker is None else [speaker], None if language is None else [language], chunk_frames,
-                                  'inference_stream'):
+                                  'inference_stream', None if durations is None else [durations], None if alignment is None else [alignment]):
             yield item[0]
 
-    def inference_streams(self, texts, speakers=None, languages=None, chunk_frames=None):
+    def inference_streams(self, texts, speakers=None, languages=None, chunk_frames=None, durations=None, alignments=None):
         """`inference_stream` for up to 64 texts decoded as one group: takes `inference_batch`'s inputs (text i reads column i of a
-        recorded mask tape) and yields, after every decoder call, {i: post-net chunk [num_mels, n]} for each text the call decoded (a chunk
+        recorded mask tape; durations and alignments as there) and yields, after every decoder call, {i: post-net chunk [num_mels, n]} for each text the call decoded (a chunk
         may hold no frames).  The frames released by one call go through the post-net as one padded batch.  Concatenated per text, the
         chunks are inference_batch's output for that text; in fp32 mode they equal inference_stream of that text alone with its tape
         column, bit for bit."""
-        yield from self._streams(texts, speakers, languages, chunk_frames, 'inference_streams')
+        yield from self._streams(texts, speakers, languages, chunk_frames, 'inference_streams', durations, alignments)
 
-    def _streams(self, texts, speakers, languages, chunk_frames, name):
+    def _streams(self, texts, speakers, languages, chunk_frames, name, durations=None, alignments=None):
         speakers, languages = _check_batch_inputs(texts, speakers, languages)
         texts = list(texts)
+        durations, alignments = _plan_lists(texts, durations, alignments)
         if len(texts) > MAX_STREAM_TEXTS:
             raise ValueError(f'{name}: at most {MAX_STREAM_TEXTS} texts decode as one group (got {len(texts)})')
         if chunk_frames is not None and int(chunk_frames) < 1:
             raise ValueError(f'{name}: chunk_frames must be >= 1 (got {chunk_frames})')
         pool = self.decoder_pool(len(texts), chunk_frames)
         for i, text in enumerate(texts):        # ids 0 .. B - 1: text i reads column i of a recorded mask tape
-            pool.open(text, None if speakers is None else speakers[i], None if languages is None else languages[i])
+            pool.open(text, None if speakers is None else speakers[i], None if languages is None else languages[i],
+                      durations=durations[i], alignment=alignments[i])
         while pool.ids:
             yield pool.run()
 
@@ -559,12 +590,12 @@ class Tacotron(torch.nn.Module):
             language = torch.argmax(language, dim=2)  # one-hot into indices for the decoder's language embedding
         return encoded, lengths_to_mask(lengths, Lmax), speaker, language
 
-    def _inference_group(self, texts, speakers, languages, tape_columns, att_window):
+    def _inference_group(self, texts, speakers, languages, tape_columns, att_window, plans=None):
         device = self._embedding.weight.device
         encoded, mask, speaker, language = self._encode_group(texts, speakers, languages)
         B = len(texts)
         prediction, _, _, cuts = self._decoder._decode_inference(encoded, mask, speaker, language, att_extent=1, tape_columns=tape_columns,
-                                                                 att_window=att_window)
+                                                                 att_window=att_window, plans=plans)
         post = self._postnet(prediction.transpose(1, 2), torch.tensor(cuts, device=device), padded=True)
         return [post[b, :, :cuts[b]] for b in range(B)]
 
@@ -610,12 +641,14 @@ class _DecodeRows:
       * ('seed', seed): b200tts_fill_keep_mask_rows at the row's own step count, stream _lib.SEED_STREAMS[site];
       * ('shared', column): with a MaskSource tape active, that column of it; otherwise one MaskSource draw over every shared row per
         call, as the batched decode has always drawn.
-    att_window (None or (back, ahead)) goes to every call; each row's window centre is carried in the DecoderState."""
+    att_window (None or (back, ahead)) goes to every call; each row's window centre is carried in the DecoderState.  A forced row also
+    holds its attention plan (weights [S_i, L_i], frames T_i; _forced_plan): every call passes the plan's steps from the row's own step
+    count on (zero rows past its end) to the library's forced attention step, and its stop rule is the fixed cut T_i (Decoder._PlanRule)."""
 
     def __init__(self, dec, att_extent, att_window=None):
         self.dec, self.att_extent, self.att_window = dec, att_extent, att_window
         self.memory = self.lengths = self.state = None
-        self.keys, self.rules, self.done, self.sources, self.text_len = [], [], [], [], []
+        self.keys, self.rules, self.done, self.sources, self.text_len, self.plans = [], [], [], [], [], []
 
     def __len__(self):
         return len(self.keys)
@@ -642,9 +675,17 @@ class _DecodeRows:
         self.state.first = False
         self.keys += list(keys)
         self.rules += [dec._StopRule(hp.stop_frames) for _ in range(b)]
+        self.plans += [None] * b
         self.done += [0] * b
         self.sources += list(sources)
         self.text_len += list(lengths)
+
+    def set_plans(self, plans):
+        """Gives the last len(plans) rows added their attention plans (None: the row decodes freely) and a forced row its fixed cut."""
+        n = len(self.keys) - len(plans)
+        for j, p in enumerate(plans, n):
+            if p is not None:
+                self.plans[j], self.rules[j] = p, self.dec._PlanRule(p[1])
 
     def keep(self, js):
         """Keeps rows js (positions, in order); the memory and cum_weights shrink to the longest text left."""
@@ -656,7 +697,7 @@ class _DecodeRows:
         idx = torch.tensor(js, device=self.memory.device)
         self.state.select(idx)
         self.memory, self.lengths = self.memory.index_select(0, idx), self.lengths.index_select(0, idx)
-        for name in ('keys', 'rules', 'done', 'sources', 'text_len'):
+        for name in ('keys', 'rules', 'done', 'sources', 'text_len', 'plans'):
             setattr(self, name, [getattr(self, name)[j] for j in js])
         L = max(self.text_len)
         if L < self.memory.shape[1]:
@@ -715,13 +756,26 @@ class _DecodeRows:
             masks[name] = full
         return masks
 
+    def _forced(self, Sc):
+        """(rows [F] int32, weights [Sc, F, L]) of the forced rows for the next Sc steps, or None: each row's plan from its own step."""
+        js = [j for j, p in enumerate(self.plans) if p is not None]
+        if not js:
+            return None
+        r, device = self.dec._outputs_per_step, self.memory.device
+        weights = torch.zeros(Sc, len(js), self.memory.shape[1], device=device)
+        for k, j in enumerate(js):
+            part = self.plans[j][0][self.done[j] // r:self.done[j] // r + Sc]
+            weights[:part.shape[0], k, :part.shape[1]] = part
+        return torch.tensor(js, dtype=torch.int32, device=device), weights
+
     def step(self, chunk_steps):
         """One library call over every row: min(chunk_steps, the steps the furthest-from-done row has left) steps; feeds each row's stop
         rule and step count -> (spec [B, Tc, N], stop [B, Tc], alignment [B, Tc / r, L]).  A row decoded past hp.max_output_length
         discards those frames."""
         dec = self.dec
         r = dec._outputs_per_step
-        Sc = min(chunk_steps, max(dec._steps(dec._max_frames - d) for d in self.done))
+        ends = [dec._max_frames if p is None else p[1] for p in self.plans]
+        Sc = min(chunk_steps, max(dec._steps(e - d) for e, d in zip(ends, self.done)))
         D, device = dec._decoder_dim, self.memory.device
         kind, rate_h, rate_c = dec._cell_config()
         masks = self._prenet_masks(Sc)
@@ -732,7 +786,8 @@ class _DecodeRows:
                     masks[name] = m
         cfg = F.DecoderConfig(kind, dec.training, rate_h, rate_c, dec._prenet._dropout_rate, masks, np.zeros(Sc, dtype=np.uint8),
                               self.att_extent, outputs_per_step=r, att_window=self.att_window)
-        spec, stop, align = F.decoder_forward_chunk(cfg, self.memory, self.lengths, dec._param_list(), self.state, Sc * r)
+        args, forced = (cfg, self.memory, self.lengths, dec._param_list(), self.state, Sc * r), self._forced(Sc)
+        spec, stop, align = F.decoder_forward_chunk(*args) if forced is None else F.decoder_forward_chunk(*args, forced=forced)
         host_stop = stop.float().cpu()
         for j in range(len(self.keys)):
             self.rules[j].feed(host_stop[j])
@@ -752,7 +807,8 @@ class DecoderPool:
     depend on the seed and the text's own steps only: its masks are one b200tts_fill_keep_mask((S, P), seed, _lib.SEED_STREAMS[site])
     call per site), else one shared MaskSource draw per call over such texts (with a MaskSource tape active: column `id` of it).  The
     model runs each call in eval mode without autograd and is restored after it.  hp.inference_attention_window is read when the pool is
-    built and kept for its life."""
+    built and kept for its life.  A text opened with `durations` or `alignment` (Tacotron.inference's forms) decodes with that
+    attention and ends at the plan's frame count."""
 
     def __init__(self, tacotron, max_texts=64, chunk_frames=None):
         if not 1 <= int(max_texts) <= MAX_STREAM_TEXTS:
@@ -772,9 +828,10 @@ class DecoderPool:
         """Every open text: queued, then decoding."""
         return [q[0] for q in self.queue] + list(self.rows.keys)
 
-    def check(self, text, speaker=None, language=None, seed=None, masks=None):
+    def check(self, text, speaker=None, language=None, seed=None, masks=None, durations=None, alignment=None):
         """Validates one text's inputs (ValueError) -> its mask source ('tape', {site: uint8 [S, P]}), ('seed', seed) or ('shared', None)."""
         _check_batch_inputs([text], None if speaker is None else [speaker], None if language is None else [language])
+        _forced_plan(self.t._decoder, text, durations, alignment, None)
         if masks is not None:
             P = self.t._decoder._prenet._layers[0].weight.shape[0]
             if not isinstance(masks, dict) or set(masks) != set(PRENET_SITES):
@@ -790,16 +847,18 @@ class DecoderPool:
             return 'seed', check_seed(seed)
         return 'shared', None
 
-    def open(self, text, speaker=None, language=None, seed=None, masks=None):
-        """Queues a text for the next run() -> its id.  Takes `inference`'s text, speaker and language, and a seed or a mask tape."""
-        source = self.check(text, speaker, language, seed, masks)
+    def open(self, text, speaker=None, language=None, seed=None, masks=None, durations=None, alignment=None):
+        """Queues a text for the next run() -> its id.  Takes `inference`'s text, speaker, language, durations and alignment, and a seed
+        or a mask tape."""
+        source = self.check(text, speaker, language, seed, masks, durations, alignment)
         if len(self.ids) >= self.max_texts:
             raise ValueError(f'the decoder pool is full: {self.max_texts} texts are open')
         tid = self.next_id
         self.next_id += 1
         if source[0] == 'shared':
             source = ('shared', tid)
-        self.queue.append((tid, text, speaker, language, source))
+        plan = _forced_plan(self.t._decoder, text, durations, alignment, self.t._embedding.weight.device)
+        self.queue.append((tid, text, speaker, language, source, plan))
         return tid
 
     def close(self, tid):
@@ -815,16 +874,17 @@ class DecoderPool:
     def _admit(self):
         t, groups = self.t, {}
         for q in self.queue:
-            _, _, speaker, language, _ = q
+            _, _, speaker, language, _, _ = q
             form = (speaker is None, None if language is None else (language.dim(), language.shape[-1] if language.dim() == 3 else 0))
             groups.setdefault(form, []).append(q)
         self.queue = []
         for group in groups.values():
-            ids, texts, speakers, languages, sources = zip(*group)
+            ids, texts, speakers, languages, sources, plans = zip(*group)
             encoded, mask, speaker, language = t._encode_group(list(texts), None if speakers[0] is None else list(speakers),
                                                                 None if languages[0] is None else list(languages))
             memory = t._decoder._memory(encoded, speaker, language)
             self.rows.add(memory, [int(x.shape[0]) for x in texts], ids, sources)
+            self.rows.set_plans(plans)
             for i in ids:
                 self.pre[i], self.released[i] = [], 0
 
@@ -907,6 +967,59 @@ def _check_batch_inputs(texts, speakers, languages):
                     or g.shape[2] != languages[0].shape[2]:
                 raise ValueError('inference_batch: per-character language weights are float [1, L, G] with L the text length')
     return speakers, languages
+
+
+def _forced_plan(dec, text, durations, alignment, device):
+    """Checks one text's attention plan -> None (a free decode), or (weights [S, L] float32 on `device`, frames): `durations` (int [L]
+    frames per symbol, each >= 0; functional.durations_to_alignment at the decoder's r, sum(d) frames) or `alignment` (float [S, L], finite
+    and >= 0; S r frames), L the text's length.  ValueError for both given, a wrong rank or dtype, another L, negative or non-finite values,
+    0 frames, or more than hp.max_output_length frames.  device None validates only."""
+    if durations is None and alignment is None:
+        return None
+    if durations is not None and alignment is not None:
+        raise ValueError('forced synthesis: give a text durations or an alignment, not both')
+    L, r = int(text.shape[0]), dec._outputs_per_step
+    if durations is not None:
+        d = F._durations_host(durations, 'forced synthesis')
+        if d.shape[0] != L:
+            raise ValueError(f'forced synthesis: {d.shape[0]} durations for a text of {L} symbols')
+        frames = int(d.sum())
+    else:
+        if not torch.is_tensor(alignment) or alignment.dim() != 2 or not alignment.dtype.is_floating_point:
+            raise ValueError('forced synthesis: an alignment is a float tensor [S, L]')
+        if alignment.shape[1] != L:
+            raise ValueError(f'forced synthesis: an alignment over {alignment.shape[1]} symbols for a text of {L} symbols')
+        if not bool(torch.isfinite(alignment).all()) or bool((alignment < 0).any()):
+            raise ValueError('forced synthesis: alignment weights must be finite and >= 0')
+        frames = int(alignment.shape[0]) * r
+    if frames == 0:
+        raise ValueError('forced synthesis: the plan has 0 frames')
+    if frames > dec._max_frames:
+        raise ValueError(f'forced synthesis: the plan has {frames} frames, more than hp.max_output_length = {dec._max_frames}')
+    if device is None:
+        return None
+    weights = F.durations_to_alignment(d, r) if durations is not None else alignment
+    return weights.to(device=device, dtype=torch.float32).contiguous(), frames
+
+
+def _plan_lists(texts, durations, alignments):
+    """durations / alignments of a batch call (None, or one entry or None per text) -> two lists with one entry per text."""
+    out = []
+    for name, items in (('durations', durations), ('alignments', alignments)):
+        items = [None] * len(texts) if items is None else list(items)
+        if len(items) != len(texts):
+            raise ValueError(f'forced synthesis: {len(items)} {name} for {len(texts)} texts')
+        out.append(items)
+    return out
+
+
+def _batch_plans(dec, texts, durations, alignments):
+    """Every text's plan checked first (ValueError), then built on the model's device -> one plan or None per text."""
+    durations, alignments = _plan_lists(texts, durations, alignments)
+    for t, d, a in zip(texts, durations, alignments):
+        _forced_plan(dec, t, d, a, None)
+    device = dec._prenet._layers[0].weight.device
+    return [_forced_plan(dec, t, d, a, device) for t, d, a in zip(texts, durations, alignments)]
 
 
 def _batch_plan(lengths, max_batch):
