@@ -195,7 +195,7 @@ SIGNATURES = {
                                          POINTER(DecoderOutputs), POINTER(DecoderOutputGrads), c_void_p, c_void_p,
                                          c_size_t, POINTER(DecoderParams), c_void_p, c_void_p]),
     'b200tts_attention_step_workspace_elems': (c_size_t, [c_int, c_int, c_int]),
-    'b200tts_attention_step': (c_int, [c_int] * 7 + [c_void_p] * 13),
+    'b200tts_attention_step': (c_int, [c_int] * 7 + [c_void_p] * 14),
     'b200tts_attention_step_backward_workspace_elems': (c_size_t, [c_int] * 5),
     'b200tts_attention_step_backward': (c_int, [c_int] * 6 + [c_void_p] * 20),
     'b200tts_debug_attention_backward_chunk': (c_int, [c_int] * 5),

@@ -196,7 +196,7 @@ __global__ void __launch_bounds__(SCORE_THREADS) scores_kernel(int S, int L, lon
 
 }  // namespace
 
-int align_validate(const b200tts_align_shape& s) {
+static int align_validate(const b200tts_align_shape& s) {
     B200_REQUIRE(s.B >= 1 && s.S >= 1, "align: need B >= 1 and S >= 1 (B = %d, S = %d)", s.B, s.S);
     B200_REQUIRE(s.L >= 1 && s.L <= B200TTS_ALIGN_MAX_SYMBOLS, "align: L = %d must be in [1, %d]", s.L, B200TTS_ALIGN_MAX_SYMBOLS);
     B200_REQUIRE(s.ld >= s.L && s.batch_stride >= 0, "align: need ld >= L and batch_stride >= 0 (ld = %lld, L = %d, batch_stride = %lld)",
@@ -204,27 +204,41 @@ int align_validate(const b200tts_align_shape& s) {
     return B200TTS_OK;
 }
 
-int monotonic_alignment_impl(const b200tts_align_shape& s, const float* P, const int* text_lengths, const int* step_lengths, int* durations,
-                             double* path_logp, int* path, cudaStream_t st) {
+}  // namespace b200tts
+using namespace b200tts;
+
+extern "C" {
+
+int b200tts_monotonic_alignment(const b200tts_align_shape* shape, const float* P, const int32_t* text_lengths, const int32_t* step_lengths,
+                                int32_t* durations_out, double* path_logp_out, int32_t* path_out, void* stream) {
+    B200_REQUIRE(shape && P && text_lengths && step_lengths && durations_out && path_logp_out, "monotonic_alignment: null argument");
+    const b200tts_align_shape& s = *shape;
     B200_TRY(align_validate(s));
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
     const int cells = (int)std::min<long long>((long long)s.S * s.L, B200TTS_ALIGN_MAX_CELLS);
     const size_t smem = 2 * sizeof(double) * s.L + (size_t)(cells + 31) / 32 * sizeof(unsigned);
     B200_CUDA(cudaFuncSetAttribute(mas_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     KernelTimer kt("monotonic_alignment", st);
-    mas_kernel<<<s.B, MAS_THREADS, smem, st>>>(s.S, s.L, s.ld, s.batch_stride, cells, P, text_lengths, step_lengths, durations, path_logp,
-                                               path);
+    mas_kernel<<<s.B, MAS_THREADS, smem, st>>>(s.S, s.L, s.ld, s.batch_stride, cells, P, text_lengths, step_lengths, durations_out,
+                                               path_logp_out, path_out);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }
 
-int alignment_scores_impl(const b200tts_align_shape& s, const float* P, const int* text_lengths, const int* step_lengths, float* focus,
-                          float* coverage, int* max_jump, int* moves_back, cudaStream_t st) {
+int b200tts_alignment_scores(const b200tts_align_shape* shape, const float* P, const int32_t* text_lengths, const int32_t* step_lengths,
+                             float* focus_out, float* coverage_out, int32_t* max_jump_out, int32_t* moves_back_out, void* stream) {
+    B200_REQUIRE(shape && P && text_lengths && step_lengths && focus_out && coverage_out && max_jump_out && moves_back_out,
+                 "alignment_scores: null argument");
+    const b200tts_align_shape& s = *shape;
     B200_TRY(align_validate(s));
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
     KernelTimer kt("alignment_scores", st);
-    scores_kernel<<<s.B, SCORE_THREADS, 0, st>>>(s.S, s.L, s.ld, s.batch_stride, P, text_lengths, step_lengths, focus, coverage, max_jump,
-                                                 moves_back);
+    scores_kernel<<<s.B, SCORE_THREADS, 0, st>>>(s.S, s.L, s.ld, s.batch_stride, P, text_lengths, step_lengths, focus_out, coverage_out,
+                                                 max_jump_out, moves_back_out);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }
 
-}  // namespace b200tts
+}  // extern "C"

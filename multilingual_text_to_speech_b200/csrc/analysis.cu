@@ -242,7 +242,7 @@ __global__ void __launch_bounds__(MCD_THREADS) analysis_mcd_dtw_kernel(int n_mfc
 
 }  // namespace
 
-int analysis_validate(const b200tts_analysis_shape& s, FftPlan* plan) {
+static int analysis_validate(const b200tts_analysis_shape& s, FftPlan* plan) {
     B200_REQUIRE(s.B >= 1 && s.total_samples >= s.B && s.total_frames >= s.B,
                  "analysis: need B >= 1 and at least one sample and one frame per utterance (B = %d, total_samples = %d, total_frames = %d)",
                  s.B, s.total_samples, s.total_frames);
@@ -268,21 +268,32 @@ static AnalysisLayout analysis_layout(const b200tts_analysis_shape& s) {
     return l;
 }
 
-size_t analysis_workspace_bytes(const b200tts_analysis_shape& s) {
+}  // namespace b200tts
+using namespace b200tts;
+
+extern "C" {
+
+size_t b200tts_analysis_workspace_bytes(const b200tts_analysis_shape* shape) {
+    if (!shape) { set_last_error("analysis_workspace_bytes: null shape"); return 0; }
     FftPlan p;
-    if (analysis_validate(s, &p) != B200TTS_OK) return 0;
-    return analysis_layout(s).bytes;
+    if (analysis_validate(*shape, &p) != B200TTS_OK) return 0;
+    return analysis_layout(*shape).bytes;
 }
 
-int stft_magnitude_impl(const b200tts_analysis_shape& s, const float* wave, const int* soff, const int* off, const float* mel_basis, float* out,
-                        void* ws, size_t ws_bytes, cudaStream_t st) {
+int b200tts_stft_magnitude(const b200tts_analysis_shape* shape, const float* wave, const int32_t* soff, const int32_t* off,
+                           const float* mel_basis, float* out, void* workspace, size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(shape && wave && soff && off && out, "stft_magnitude: null argument");
+    B200_TRY(require_device());
+    const b200tts_analysis_shape& s = *shape;
     FftPlan p;
     B200_TRY(analysis_validate(s, &p));
     B200_REQUIRE(s.n_mels == 0 || mel_basis, "stft_magnitude: n_mels = %d needs the mel basis", s.n_mels);
     const AnalysisLayout l = analysis_layout(s);
-    B200_REQUIRE(ws && ws_bytes >= l.bytes, "stft_magnitude: workspace of %zu bytes is smaller than the %zu required", ws_bytes, l.bytes);
-    B200_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "stft_magnitude: workspace must be 256-byte aligned");
-    unsigned char* base = static_cast<unsigned char*>(ws);
+    B200_REQUIRE(workspace && workspace_bytes >= l.bytes, "stft_magnitude: workspace of %zu bytes is smaller than the %zu required",
+                 workspace_bytes, l.bytes);
+    B200_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "stft_magnitude: workspace must be 256-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    unsigned char* base = static_cast<unsigned char*>(workspace);
     double2* twM = reinterpret_cast<double2*>(base + l.twM);
     double2* twN = reinterpret_cast<double2*>(base + l.twN);
     double* window = reinterpret_cast<double*>(base + l.window);
@@ -302,24 +313,26 @@ int stft_magnitude_impl(const b200tts_analysis_shape& s, const float* wave, cons
     return B200TTS_OK;
 }
 
-int amplitude_to_db_impl(const b200tts_analysis_shape& s, const float* S, const int* off, float* out, cudaStream_t st) {
+int b200tts_amplitude_to_db(const b200tts_analysis_shape* shape, const float* S, const int32_t* off, float* out, void* stream) {
+    B200_REQUIRE(shape && S && off && out, "amplitude_to_db: null argument");
+    B200_TRY(require_device());
+    const b200tts_analysis_shape& s = *shape;
     FftPlan p;
     B200_TRY(analysis_validate(s, &p));
+    cudaStream_t st = (cudaStream_t)stream;
     KernelTimer kt("analysis_db", st);
     analysis_db_kernel<<<s.B, DB_THREADS, 0, st>>>(s.n_mels ? s.n_mels : p.M + 1, off, S, out);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }
 
-int mel_cepstrum_validate(int total_frames, int n_mels, int n_mfcc) {
+int b200tts_mel_cepstrum(int total_frames, int n_mels, int n_mfcc, const float* mel_db, float* out, void* stream) {
+    B200_REQUIRE(mel_db && out, "mel_cepstrum: null argument");
     B200_REQUIRE(total_frames >= 1, "mel_cepstrum: total_frames %d must be positive", total_frames);
     B200_REQUIRE(n_mels >= 1 && n_mels <= 1024, "mel_cepstrum: n_mels %d must be in [1, 1024]", n_mels);
     B200_REQUIRE(n_mfcc >= 1 && n_mfcc <= n_mels, "mel_cepstrum: n_mfcc %d must be in [1, n_mels = %d]", n_mfcc, n_mels);
-    return B200TTS_OK;
-}
-
-int mel_cepstrum_impl(int total_frames, int n_mels, int n_mfcc, const float* mel_db, float* out, cudaStream_t st) {
-    B200_TRY(mel_cepstrum_validate(total_frames, n_mels, n_mfcc));
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
     const size_t smem = (size_t)(n_mfcc + CEP_FRAMES) * n_mels * sizeof(float);      // at most 2 * 1024 * 32 * 4 bytes
     B200_CUDA(cudaFuncSetAttribute(analysis_cepstrum_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     KernelTimer kt("analysis_cepstrum", st);
@@ -328,29 +341,27 @@ int mel_cepstrum_impl(int total_frames, int n_mels, int n_mfcc, const float* mel
     return B200TTS_OK;
 }
 
-int mcd_validate(int B, int n_mfcc, int mode) {
+int b200tts_mel_cepstral_distortion(int B, int n_mfcc, int mode, const float* cep_a, const int32_t* off_a, const float* cep_b,
+                                    const int32_t* off_b, double* mcd_out, int32_t* path_len_out, void* stream) {
+    B200_REQUIRE(cep_a && off_a && cep_b && off_b && mcd_out, "mel_cepstral_distortion: null argument");
     B200_REQUIRE(B >= 1, "mel_cepstral_distortion: B %d must be positive", B);
     B200_REQUIRE(n_mfcc >= 2, "mel_cepstral_distortion: n_mfcc %d must be at least 2 (c0 is dropped)", n_mfcc);
     B200_REQUIRE(mode == B200TTS_MCD_CUT || mode == B200TTS_MCD_STRETCH || mode == B200TTS_MCD_DTW,
                  "mel_cepstral_distortion: unknown mode %d", mode);
-    return B200TTS_OK;
-}
-
-int mel_cepstral_distortion_impl(int B, int n_mfcc, int mode, const float* cep_a, const int* off_a, const float* cep_b, const int* off_b,
-                                 double* mcd, int* path_len, cudaStream_t st) {
-    B200_TRY(mcd_validate(B, n_mfcc, mode));
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
     if (mode != B200TTS_MCD_DTW) {
         KernelTimer kt("analysis_mcd", st);
-        analysis_mcd_linear_kernel<<<B, MCD_THREADS, 0, st>>>(n_mfcc, mode, cep_a, off_a, cep_b, off_b, mcd, path_len);
+        analysis_mcd_linear_kernel<<<B, MCD_THREADS, 0, st>>>(n_mfcc, mode, cep_a, off_a, cep_b, off_b, mcd_out, path_len_out);
         B200_LAUNCH_CHECK();
         return B200TTS_OK;
     }
     const size_t smem = (size_t)(B200TTS_DTW_MAX_FRAMES + 1) * DTW_CELL_BYTES;
     B200_CUDA(cudaFuncSetAttribute(analysis_mcd_dtw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     KernelTimer kt("analysis_dtw", st);
-    analysis_mcd_dtw_kernel<<<B, MCD_THREADS, smem, st>>>(n_mfcc, cep_a, off_a, cep_b, off_b, mcd, path_len);
+    analysis_mcd_dtw_kernel<<<B, MCD_THREADS, smem, st>>>(n_mfcc, cep_a, off_a, cep_b, off_b, mcd_out, path_len_out);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }
 
-}  // namespace b200tts
+}  // extern "C"

@@ -11,6 +11,8 @@ namespace b200tts {
 
 void set_last_error(const char* fmt, ...);
 int check_cuda(cudaError_t e, const char* what, const char* file, int line);
+// B200TTS_OK when the current device is a usable sm_90 GPU (cached once it is); entry points call it before any device work
+int require_device();
 
 #define B200_CUDA(call)                                                             \
     do {                                                                            \
@@ -43,6 +45,11 @@ struct KernelTimer {
     KernelTimer(const char* n, cudaStream_t s) : name(n), st(s) { ktimer_start(n, s); }
     ~KernelTimer() { ktimer_stop(name, st); }
 };
+
+// WaveRNN upsampling layer (wavernn.cu): the shape check its forward and backward entry points share
+int wavernn_upsample_layer_check(int C, int len, int scale);
+// y[r, :] = lfilter([1], [1, -a], y[r, :]) for each of `rows` rows of `len` samples, no normalisation (vocoder.cu; the WaveRNN folds)
+int deemphasis_rows(int rows, int len, float a, float* y, cudaStream_t st);
 
 // SMs of the H100 SXM the library is built for: grid sizes of the grid-stride kernels and the co-residency limit of the persistent loops
 constexpr int NUM_SMS = 132;
@@ -143,6 +150,9 @@ struct GemmDesc {
 // pack cache of the wgmma GEMM (gemm_tc.cu): operands packed inside a begin / end scope are reused by later products of the scope
 void tc_pack_cache_begin();
 void tc_pack_cache_end();
+// the wgmma GEMM's packing scratch (b200tts_set_scratch; null disables the path) and its on / off switch (b200tts_set_tensor_core_gemm)
+void set_tc_scratch(void* ptr, size_t bytes);
+void set_tc_enabled(int on);
 
 // Arguments of the SIMT (gemm.cu) and mma.sync (gemm_bf16.cu) kernels, filled from a GemmDesc by gemm.cu.  kcontig: the operand is
 // contiguous along k; vec: 16-byte vector loads are legal; kchunk: k range of one split, a multiple of the kernel's k-block.
@@ -167,6 +177,11 @@ int gemm_tc_try(const GemmDesc& d, cudaStream_t st, bool* handled);
 // mapN: rank <= 5; dims / box: `rank` entries (innermost first), strides: rank - 1 byte strides
 int tc_make_map3_bf16(void* map, const void* base, int d0, int d1, int d2, size_t stride1, size_t stride2, int b0, int b1, int b2);
 int tc_make_mapN_bf16(void* map, const void* base, int rank, const unsigned long long* dims, const unsigned long long* strides, const unsigned* box);
+// implicit convolutions on the wgmma GEMM (gemm_tc.cu), for the encoder's conv blocks: *handled = false when the shape is not one they take
+int gemm_tc_conv(const float* weight, const float* in, float* out, int NB, int G, int Cout, int Cin, int L, int k, int dil, int pad, int bwd,
+                 float beta, cudaStream_t st, bool* handled);
+int gemm_tc_conv_dw(const float* dz, const float* x, float* dweight, int NB, int G, int Cout, int Cin, int L, int k, int dil, int pad,
+                    cudaStream_t st, bool* handled);
 // Precision mode of the library (b200tts_set_precision): 0 = fp32-exact (parity mode), 1 = bf16 tensor-core operands.
 int precision_mode();
 void set_precision_mode(int mode);

@@ -1039,33 +1039,63 @@ int frame_feedback(const BwdCtx& c, int f) {
 
 }  // namespace
 
-size_t decoder_bwd_workspace_floats(const b200tts_decoder_shape& s) { return bwd_layout(s).total; }
-// byte offset of the phase counters of the persistent backward kernels inside the backward workspace (0: generator, 1: attention)
-size_t decoder_bwd_profile_offset(const b200tts_decoder_shape& s, int which) {
-    const BwdLayout l = bwd_layout(s);
-    if (which == 0) return l.pextra * sizeof(float) + persist_bwd_gen_extra_bytes(s) - NUM_SMS * 8 * 8;
-    return l.pextra2 * sizeof(float) + att_bwd_extra(s).barrier + 256;
-}
-// byte offsets of the per-step histories of the backward workspace: dfs, dhgd, dctxs, dgg, dhas, dga, dq, dctxt, dmemT, dggb, dgab
-void decoder_bwd_view_offsets(const b200tts_decoder_shape& s, size_t* out) {
-    const BwdLayout l = bwd_layout(s);
-    const size_t offs[11] = {l.dfs, l.dhgd, l.dctxs, l.dgg, l.dhas, l.dga, l.dq, l.dctxt, l.dmemT, l.dggb, l.dgab};
-    for (int k = 0; k < 11; ++k) out[k] = offs[k] * sizeof(float);
-}
-
-// standalone backward of one attention step (module-level API): per-utterance accumulators in the workspace, reduced over the batch here
-size_t attention_step_backward_workspace_elems(int B, int M, int A, int C, int K) {
-    return (size_t)B * ((size_t)A * C + (size_t)C * K + A + M);
-}
-int attention_step_backward_validate(int B, int L, int M, int A, int C, int K) {
+static int attention_step_backward_validate(int B, int L, int M, int A, int C, int K) {
     B200_REQUIRE(B > 0 && L > 0 && M > 0 && A > 0 && C > 0 && K > 0, "attention_step_backward: non-positive dimension (B=%d L=%d M=%d A=%d C=%d K=%d)",
                  B, L, M, A, C, K);
     B200_REQUIRE(A <= 128 && A % 4 == 0 && C % 4 == 0 && (A / 4) * (C / 4) <= ATT_THREADS && M <= 512 && (K % 2) == 1,
                  "attention_step_backward: unsupported dims A=%d C=%d M=%d K=%d", A, C, M, K);
     return B200TTS_OK;
 }
+
+}  // namespace b200tts
+using namespace b200tts;
+
+extern "C" {
+
+// The three decoder queries below answer for the step shape (T -> ceil(T / R) steps) that the forward and backward calls run on.
+size_t b200tts_decoder_bwd_workspace_bytes(const b200tts_decoder_shape* shape) {
+    if (!shape || validate_decoder_shape(*shape) != B200TTS_OK) return 0;
+    return bwd_layout(step_shape(*shape)).total * sizeof(float);
+}
+
+// byte offset of the phase counters of the persistent backward kernels inside the backward workspace (0: generator, 1: attention)
+size_t b200tts_debug_persist_bwd_profile_offset(const b200tts_decoder_shape* shape, int which) {
+    if (!shape || validate_decoder_shape(*shape) != B200TTS_OK) return 0;
+    const b200tts_decoder_shape s = step_shape(*shape);
+    const BwdLayout l = bwd_layout(s);
+    if (which == 0) return l.pextra * sizeof(float) + persist_bwd_gen_extra_bytes(s) - NUM_SMS * 8 * 8;
+    return l.pextra2 * sizeof(float) + att_bwd_extra(s).barrier + 256;
+}
+
+int b200tts_debug_decoder_views(const b200tts_decoder_shape* shape, size_t* out, int n) {
+    if (!shape || !out || validate_decoder_shape(*shape) != B200TTS_OK) return 0;
+    const b200tts_decoder_shape s = step_shape(*shape);
+    const DecoderLayout l = decoder_layout(s);
+    const PersistLayout pl = persist_layout(s);
+    const TcPersistGeom g = tc_persist_geom(s);
+    const BwdLayout bl = bwd_layout(s);
+    const size_t pbase = l.persist * sizeof(float);
+    size_t v[26];
+    const size_t fwd[11] = {l.ai, l.ca, l.hg, l.cg, l.ga, l.gg, l.q, l.cum, l.memT, l.fs, l.p1};
+    for (int k = 0; k < 11; ++k) v[k] = fwd[k] * sizeof(float);
+    v[11] = pbase + pl.aib;
+    v[12] = pbase + pl.hgb;
+    // the per-step histories of the backward workspace: dfs, dhgd, dctxs, dgg, dhas, dga, dq, dctxt, dmemT, dggb, dgab
+    const size_t bwd[11] = {bl.dfs, bl.dhgd, bl.dctxs, bl.dgg, bl.dhas, bl.dga, bl.dq, bl.dctxt, bl.dmemT, bl.dggb, bl.dgab};
+    for (int k = 0; k < 11; ++k) v[13 + k] = bwd[k] * sizeof(float);
+    v[24] = (size_t)g.Kp_att;
+    v[25] = (size_t)g.Kp_gen;
+    const int m = n < 26 ? n : 26;
+    for (int k = 0; k < m; ++k) out[k] = v[k];
+    return m;
+}
+
+// standalone backward of one attention step (module-level API): per-utterance accumulators in the workspace, reduced over the batch here
+size_t b200tts_attention_step_backward_workspace_elems(int B, int M, int A, int C, int K) {
+    return (size_t)B * ((size_t)A * C + (size_t)C * K + A + M);
+}
 // the per-chunk position count LC launch_attn_bwd runs these dims with, or 0 when not even 4-row chunks fit in shared memory
-int attention_backward_chunk(int L, int M, int A, int C, int K) {
+int b200tts_debug_attention_backward_chunk(int L, int M, int A, int C, int K) {
     if (attention_step_backward_validate(1, L, M, A, C, K) != B200TTS_OK) return 0;
     const int LC = pick_attn_bwd_chunk(L, M, A, C, K);
     if ((size_t)attn_bwd_smem(L, M, A, C, K, LC).total * sizeof(float) > 227 * 1024) {
@@ -1074,60 +1104,105 @@ int attention_backward_chunk(int L, int M, int A, int C, int K) {
     }
     return LC;
 }
-int attention_step_backward_impl(int B, int L, int M, int A, int C, int K, const float* q, const float* memory, const float* memT,
-                                 const int* lengths, const float* Wloc, const float* Wc, const float* bias, const float* v,
-                                 const float* cum_prev, const float* weights, const float* d_ctx, const float* d_weights, float* d_cum,
-                                 float* d_q, float* d_memT, float* d_Wloc, float* d_Wc, float* d_v, float* ws, cudaStream_t st) {
+int b200tts_attention_step_backward(int B, int L, int M, int A, int C, int K, const float* q, const float* memory,
+                                    const float* memory_transform, const int32_t* text_lengths, const float* w_location,
+                                    const float* w_loc_features, const float* bias, const float* w_energy, const float* cum_prev,
+                                    const float* weights, const float* d_context, const float* d_weights, float* d_cum, float* d_q,
+                                    float* d_memory_transform, float* d_w_location, float* d_w_loc_features, float* d_w_energy,
+                                    float* workspace, void* stream) {
+    B200_REQUIRE(q && memory && memory_transform && text_lengths && w_location && w_loc_features && bias && w_energy && cum_prev && weights &&
+                 d_context && d_cum && d_q && d_memory_transform && d_w_location && d_w_loc_features && d_w_energy && workspace,
+                 "attention_step_backward: null argument");
     B200_TRY(attention_step_backward_validate(B, L, M, A, C, K));
-    float* dWloc_acc = ws;
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
+    float* dWloc_acc = workspace;
     float* dWc_acc = dWloc_acc + (size_t)B * A * C;
     float* dv_acc = dWc_acc + (size_t)B * C * K;
     float* dctx_tot = dv_acc + (size_t)B * A;
-    B200_TRY(launch_fill(ws, 0.f, (size_t)B * ((size_t)A * C + (size_t)C * K + A), st));
+    B200_TRY(launch_fill(workspace, 0.f, (size_t)B * ((size_t)A * C + (size_t)C * K + A), st));
     AttnBwdArgs aa{};
-    aa.q = q; aa.memT = memT; aa.memory = memory; aa.lengths = lengths;
-    aa.Wc = Wc; aa.Wloc = Wloc; aa.bias = bias; aa.v = v; aa.cum_prev = cum_prev;
+    aa.q = q; aa.memT = memory_transform; aa.memory = memory; aa.lengths = text_lengths;
+    aa.Wc = w_loc_features; aa.Wloc = w_location; aa.bias = bias; aa.v = w_energy; aa.cum_prev = cum_prev;
     aa.w = weights; aa.w_bstride = L; aa.dalign = d_weights; aa.dalign_bstride = L;
-    aa.dctx_static = d_ctx; aa.part = nullptr; aa.nsplit = 0; aa.part_stride = 0; aa.ld_part = 0;
-    aa.dcum = d_cum; aa.dctx_tot = dctx_tot; aa.dq = d_q; aa.dmemT = d_memT;
+    aa.dctx_static = d_context; aa.part = nullptr; aa.nsplit = 0; aa.part_stride = 0; aa.ld_part = 0;
+    aa.dcum = d_cum; aa.dctx_tot = dctx_tot; aa.dq = d_q; aa.dmemT = d_memory_transform;
     aa.dWloc_acc = dWloc_acc; aa.dWc_acc = dWc_acc; aa.dv_acc = dv_acc;
     aa.B = B; aa.L = L; aa.M = M; aa.A = A; aa.C = C; aa.K = K; aa.last = 0;
     B200_TRY(launch_attn_bwd(aa, st));
-    batchsum_add_kernel<<<grid_for((size_t)A * C), 256, 0, st>>>(d_Wloc, dWloc_acc, B, (size_t)A * C);
+    batchsum_add_kernel<<<grid_for((size_t)A * C), 256, 0, st>>>(d_w_location, dWloc_acc, B, (size_t)A * C);
     B200_LAUNCH_CHECK();
-    batchsum_add_kernel<<<grid_for((size_t)C * K), 256, 0, st>>>(d_Wc, dWc_acc, B, (size_t)C * K);
+    batchsum_add_kernel<<<grid_for((size_t)C * K), 256, 0, st>>>(d_w_loc_features, dWc_acc, B, (size_t)C * K);
     B200_LAUNCH_CHECK();
-    batchsum_add_kernel<<<1, 256, 0, st>>>(d_v, dv_acc, B, (size_t)A);
+    batchsum_add_kernel<<<1, 256, 0, st>>>(d_w_energy, dv_acc, B, (size_t)A);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }
 
 // standalone backward of one forward-attention step: per-utterance d v partials in the workspace, reduced over the batch here
-size_t forward_attention_step_backward_workspace_elems(int B, int M, int A) { return (size_t)B * ((size_t)A + M); }
-int forward_attention_step_backward_impl(int B, int L, int M, int A, const float* q, const float* memory, const float* memT,
-                                         const int* lengths, const float* bias, const float* v, const float* alpha_prev,
-                                         const float* weights, const float* d_ctx, const float* d_weights, float* d_alpha, float* d_q,
-                                         float* d_memT, float* d_v, float* ws, cudaStream_t st) {
+size_t b200tts_forward_attention_step_backward_workspace_elems(int B, int M, int A) { return (size_t)B * ((size_t)A + M); }
+int b200tts_forward_attention_step_backward(int B, int L, int M, int A, const float* q, const float* memory, const float* memory_transform,
+                                            const int32_t* text_lengths, const float* bias, const float* w_energy, const float* alpha_prev,
+                                            const float* weights, const float* d_context, const float* d_weights, float* d_alpha,
+                                            float* d_q, float* d_memory_transform, float* d_w_energy, float* workspace, void* stream) {
+    B200_TRY(require_device());
+    B200_REQUIRE(q && memory && memory_transform && text_lengths && bias && w_energy && alpha_prev && weights && d_context && d_alpha &&
+                 d_q && d_memory_transform && d_w_energy && workspace, "forward_attention_step_backward: null argument");
     B200_REQUIRE(B > 0 && L > 0 && A > 0 && A <= 128 && M > 0 && M <= 512,
                  "forward_attention_step_backward: unsupported dims B=%d L=%d A=%d M=%d", B, L, A, M);
-    float* dv_acc = ws;
+    cudaStream_t st = (cudaStream_t)stream;
+    float* dv_acc = workspace;
     float* dctx_tot = dv_acc + (size_t)B * A;
     B200_TRY(launch_fill(dv_acc, 0.f, (size_t)B * A, st));
     FwdAttnBwdArgs fa{};
-    fa.q = q; fa.memT = memT; fa.memory = memory; fa.lengths = lengths; fa.bias = bias; fa.v = v;
+    fa.q = q; fa.memT = memory_transform; fa.memory = memory; fa.lengths = text_lengths; fa.bias = bias; fa.v = w_energy;
     fa.alpha_prev = alpha_prev; fa.w = weights; fa.w_bstride = L; fa.dalign = d_weights; fa.dalign_bstride = L;
-    fa.dctx_static = d_ctx; fa.part = nullptr; fa.nsplit = 0; fa.part_stride = 0; fa.ld_part = 0;
-    fa.dalpha = d_alpha; fa.dctx_tot = dctx_tot; fa.dq = d_q; fa.dmemT = d_memT; fa.dv_acc = dv_acc;
+    fa.dctx_static = d_context; fa.part = nullptr; fa.nsplit = 0; fa.part_stride = 0; fa.ld_part = 0;
+    fa.dalpha = d_alpha; fa.dctx_tot = dctx_tot; fa.dq = d_q; fa.dmemT = d_memory_transform; fa.dv_acc = dv_acc;
     fa.B = B; fa.L = L; fa.M = M; fa.A = A; fa.last = 0;
     B200_TRY(launch_fwd_attn_bwd(fa, st));
-    batchsum_add_kernel<<<1, 256, 0, st>>>(d_v, dv_acc, B, (size_t)A);
+    batchsum_add_kernel<<<1, 256, 0, st>>>(d_w_energy, dv_acc, B, (size_t)A);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }
 
-int decoder_backward_impl(const b200tts_decoder_shape& frames, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
-                          const b200tts_decoder_outputs& fwd_out, const b200tts_decoder_output_grads& dout, const float* fws,
-                          float* bws, size_t bws_bytes, const b200tts_decoder_params& dw, float* d_memory, cudaStream_t st) {
+int b200tts_lstm_cell_backward(int B, int D, int cell_kind, int training, float rate_h, float rate_c, const float* gates, const float* c_prev,
+                               const uint8_t* mask_h, const uint8_t* mask_c, const float* d_h, float* d_c, float* d_h_prev, float* d_gates,
+                               void* stream) {
+    B200_REQUIRE(B > 0 && D > 0 && gates && c_prev && d_h && d_c && d_h_prev && d_gates, "lstm_cell_backward: bad argument");
+    B200_REQUIRE(cell_kind == B200TTS_CELL_DROPOUT || cell_kind == B200TTS_CELL_ZONEOUT, "lstm_cell_backward: bad cell kind %d", cell_kind);
+    B200_REQUIRE(rate_h >= 0.f && rate_h < 1.f && rate_c >= 0.f && rate_c < 1.f, "lstm_cell_backward: rates must be in [0, 1)");
+    B200_TRY(require_device());
+    B200_CUDA(cudaMemsetAsync(d_h_prev, 0, (size_t)B * D * sizeof(float), (cudaStream_t)stream));
+    CellBwdArgs a{};
+    a.gates = gates; a.c_prev = c_prev; a.dh_static = d_h; a.ld_dhs = D; a.part = nullptr; a.nsplit = 0;
+    a.dc_state = d_c; a.dhz_state = d_h_prev;       // in: zero recurrent term; out: the direct (zoneout) gradient of h_prev
+    a.mask_h = mask_h; a.mask_c = mask_c; a.kind = cell_kind; a.training = training; a.rate_h = rate_h; a.rate_c = rate_c;
+    a.dgates = d_gates; a.B = B; a.D = D; a.last = 0;
+    return launch_cell_bwd(a, (cudaStream_t)stream);
+}
+
+int b200tts_decoder_backward(const b200tts_decoder_shape* shape, const b200tts_decoder_params* params,
+                             const b200tts_decoder_inputs* inputs, const b200tts_decoder_outputs* fwd_outputs,
+                             const b200tts_decoder_output_grads* output_grads, const void* fwd_workspace, void* bwd_workspace,
+                             size_t bwd_workspace_bytes, const b200tts_decoder_params* d_params, float* d_memory,
+                             void* stream) {
+    B200_REQUIRE(shape && params && inputs && fwd_outputs && output_grads && fwd_workspace && bwd_workspace && d_params,
+                 "decoder_backward: null argument");
+    B200_REQUIRE(shape->att_window_back == 0 && shape->att_window_ahead == 0,
+                 "decoder_backward: an attention window is for synthesis only (b200tts_decoder_forward_chunk)");
+    B200_REQUIRE(!forced_inputs(*inputs), "decoder_backward: forced attention rows are for synthesis only (b200tts_decoder_forward_chunk)");
+    B200_TRY(require_device());
+    const b200tts_decoder_shape& frames = *shape;
+    const b200tts_decoder_params& w = *params;
+    const b200tts_decoder_params& dw = *d_params;
+    const b200tts_decoder_inputs& in = *inputs;
+    const b200tts_decoder_outputs& fwd_out = *fwd_outputs;
+    const b200tts_decoder_output_grads& dout = *output_grads;
+    const float* fws = static_cast<const float*>(fwd_workspace);
+    float* bws = static_cast<float*>(bwd_workspace);
+    const size_t bws_bytes = bwd_workspace_bytes;
+    cudaStream_t st = (cudaStream_t)stream;
     B200_TRY(validate_decoder_shape(frames));
     const b200tts_decoder_shape s = step_shape(frames);     // T = decoder steps from here on; frames.T = target frames
     B200_REQUIRE(fwd_out.alignments, "decoder_backward: the forward alignments tensor is required");
@@ -1276,4 +1351,4 @@ int decoder_backward_impl(const b200tts_decoder_shape& frames, const b200tts_dec
     return B200TTS_OK;
 }
 
-}  // namespace b200tts
+}  // extern "C"

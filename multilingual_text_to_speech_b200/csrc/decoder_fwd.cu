@@ -810,9 +810,10 @@ int frame_proj(const FwdCtx& c, int step0, int nsteps) {
 
 }  // namespace
 
-int decoder_forward_impl(const b200tts_decoder_shape& frames, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
-                         const b200tts_decoder_outputs& out, float* ws, size_t ws_bytes, cudaStream_t st,
-                         const b200tts_decoder_state* state, int first) {
+// the forward of b200tts_decoder_forward (state == nullptr) and b200tts_decoder_forward_chunk, behind their argument checks
+static int decoder_forward_impl(const b200tts_decoder_shape& frames, const b200tts_decoder_params& w, const b200tts_decoder_inputs& in,
+                                const b200tts_decoder_outputs& out, float* ws, size_t ws_bytes, cudaStream_t st,
+                                const b200tts_decoder_state* state = nullptr, int first = 1) {
     B200_TRY(validate_decoder_shape(frames));
     const b200tts_decoder_shape s = step_shape(frames);     // T = decoder steps from here on; Tf = target frames
     const bool resume = state != nullptr && !first;       // chunked decode: start from the carried state
@@ -956,74 +957,146 @@ int decoder_forward_impl(const b200tts_decoder_shape& frames, const b200tts_deco
     return B200TTS_OK;
 }
 
-// ---- standalone attention step (module-level parity of LocationSensitiveAttention.forward) ----
-int attention_step_impl(int B, int L, int M, int D, int A, int C, int K, const float* query, const float* memory,
-                        const float* memT, const int* lengths, const float* Wq, const float* Wloc, const float* Wc,
-                        const float* bias, const float* v, float* cum, float* ctx, float* weights, float* workspace,
-                        cudaStream_t st) {
-    B200_REQUIRE(A <= 128 && M <= 512 && (K % 2) == 1, "attention_step: unsupported dims A=%d M=%d K=%d", A, M, K);
-    // q = query . Wq^T into workspace[0 : B*A]; new cum into workspace[B*A : B*A + B*L] then copied back
-    float* q = workspace;
-    float* cum_next = workspace + (size_t)B * A;
-    B200_TRY(run_gemm(st, B, A, D, query, D, Wq, D, true, q, A, nullptr, 0.f));
-    AttnFwdArgs aa{};
-    aa.qpart = q; aa.nq = 1; aa.q_save = nullptr; aa.memT = memT; aa.memory = memory; aa.lengths = lengths;
-    aa.Wc = Wc; aa.Wloc = Wloc; aa.bias = bias; aa.v = v; aa.cum_prev = cum; aa.cum_next = cum_next;
-    aa.align = weights; aa.align_bstride = L; aa.ctx_out = ctx; aa.ld_ctx = M; aa.ctx_out2 = nullptr; aa.ld_ctx2 = 0;
-    aa.B = B; aa.L = L; aa.M = M; aa.A = A; aa.C = C; aa.K = K;
-    B200_TRY(launch_attn_fwd(aa, st));
-    B200_TRY(launch_copy2d(cum, L, cum_next, L, B, L, st));
+}  // namespace b200tts
+using namespace b200tts;
+
+extern "C" {
+
+size_t b200tts_decoder_workspace_bytes(const b200tts_decoder_shape* shape) {
+    if (!shape || validate_decoder_shape(*shape) != B200TTS_OK) return 0;
+    return decoder_layout(step_shape(*shape)).total * sizeof(float);
+}
+
+int b200tts_decoder_path(const b200tts_decoder_shape* shape) {
+    if (!shape || validate_decoder_shape(*shape) != B200TTS_OK) return 0;
+    const PersistPlan p = persist_plan(step_shape(*shape));
+    return (p.fwd ? 1 | 2 : 0) | (p.gen_bwd ? 4 | 8 : 0) | (p.att_bwd ? 16 | 32 : 0);
+}
+
+int b200tts_decoder_forward(const b200tts_decoder_shape* shape, const b200tts_decoder_params* params,
+                            const b200tts_decoder_inputs* in, const b200tts_decoder_outputs* out, void* workspace,
+                            size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(shape && params && in && out, "decoder_forward: null argument");
+    B200_REQUIRE(shape->att_window_back == 0 && shape->att_window_ahead == 0,
+                 "decoder_forward: an attention window is for synthesis only (b200tts_decoder_forward_chunk)");
+    B200_REQUIRE(!forced_inputs(*in), "decoder_forward: forced attention rows are for synthesis only (b200tts_decoder_forward_chunk)");
+    B200_TRY(require_device());
+    return decoder_forward_impl(*shape, *params, *in, *out, (float*)workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int b200tts_decoder_forward_chunk(const b200tts_decoder_shape* shape, const b200tts_decoder_params* params,
+                                  const b200tts_decoder_inputs* in, const b200tts_decoder_outputs* out, b200tts_decoder_state* state,
+                                  int first, void* workspace, size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(shape && params && in && out && state, "decoder_forward_chunk: null argument");
+    B200_REQUIRE(state->att_h && state->att_c && state->gen_h && state->gen_c && state->context && state->cum_weights && state->frame,
+                 "decoder_forward_chunk: every state buffer is required");
+    B200_REQUIRE(!attention_window(*shape) || state->attended, "decoder_forward_chunk: an attention window needs state->attended");
+    B200_REQUIRE(in->forced_count >= 0 && in->forced_count <= shape->B,
+                 "decoder_forward_chunk: forced_count %d outside [0, B=%d]", in->forced_count, shape->B);
+    B200_REQUIRE(in->forced_count == 0 ? !in->forced_rows && !in->forced_alignment : in->forced_rows && in->forced_alignment,
+                 "decoder_forward_chunk: forced_rows and forced_alignment are given exactly when forced_count > 0");
+    B200_REQUIRE(shape->R < 0 || shape->T % frames_per_step(*shape) == 0,
+                 "decoder_forward_chunk: a chunk holds whole decoder steps (T=%d is not a multiple of R=%d)", shape->T, shape->R);
+    B200_TRY(require_device());
+    return decoder_forward_impl(*shape, *params, *in, *out, (float*)workspace, workspace_bytes, (cudaStream_t)stream, state, first);
+}
+
+// ---- initial state of listed rows of a carried state ----
+int b200tts_decoder_state_reset_rows(const b200tts_decoder_shape* shape, b200tts_decoder_state* state, const int32_t* rows, int count,
+                                     void* stream) {
+    B200_REQUIRE(shape && state, "decoder_state_reset_rows: null argument");
+    const b200tts_decoder_shape& s = *shape;
+    B200_REQUIRE(s.B > 0 && s.L > 0 && s.M > 0 && s.D > 0 && s.N > 0, "decoder_state_reset_rows: non-positive dimension (B=%d L=%d M=%d D=%d N=%d)",
+                 s.B, s.L, s.M, s.D, s.N);
+    B200_REQUIRE(s.att_kind == B200TTS_ATT_LOCATION || s.att_kind == B200TTS_ATT_FORWARD, "decoder_state_reset_rows: bad attention kind %d",
+                 s.att_kind);
+    B200_REQUIRE(state->att_h && state->att_c && state->gen_h && state->gen_c && state->context && state->cum_weights && state->frame,
+                 "decoder_state_reset_rows: every state buffer is required");
+    B200_REQUIRE(rows && count >= 1 && count <= s.B, "decoder_state_reset_rows: %d rows of a state of %d", count, s.B);
+    for (int k = 0; k < count; ++k)
+        B200_REQUIRE(rows[k] >= 0 && rows[k] < s.B, "decoder_state_reset_rows: row %d outside [0, %d)", rows[k], s.B);
+    B200_TRY(require_device());
+    DecInitRows a{};
+    a.ctx = state->context; a.ld_ctx = s.M; a.att_h = state->att_h; a.ld_att_h = s.D;
+    a.att_c = state->att_c; a.gen_h = state->gen_h; a.gen_c = state->gen_c; a.cum = state->cum_weights; a.frame = state->frame;
+    a.attended = state->attended;
+    a.M = s.M; a.D = s.D; a.L = s.L; a.N = s.N; a.one_hot = forward_attention(s);
+    for (int k0 = 0; k0 < count; k0 += B200TTS_DECODER_RESET_MAX_ROWS) {
+        a.n = count - k0 < B200TTS_DECODER_RESET_MAX_ROWS ? count - k0 : B200TTS_DECODER_RESET_MAX_ROWS;
+        for (int k = 0; k < a.n; ++k) a.row[k] = rows[k0 + k];
+        B200_TRY(launch_init_rows(a, a.n, (cudaStream_t)stream));
+    }
     return B200TTS_OK;
 }
 
+size_t b200tts_attention_step_workspace_elems(int B, int L, int A) { return (size_t)B * A + (size_t)B * L; }
+
+// ---- standalone attention step (module-level parity of LocationSensitiveAttention.forward) ----
+int b200tts_attention_step(int B, int L, int M, int D, int A, int C, int K, const float* query, const float* memory,
+                           const float* memory_transform, const int32_t* text_lengths, const float* w_query,
+                           const float* w_location, const float* w_loc_features, const float* bias, const float* w_energy,
+                           float* cum_weights, float* context, float* weights, float* workspace, void* stream) {
+    B200_REQUIRE(query && memory && memory_transform && text_lengths && w_query && w_location && w_loc_features && bias && w_energy &&
+                 cum_weights && context && weights && workspace, "attention_step: null argument");
+    B200_REQUIRE(B > 0 && L > 0 && M > 0 && D > 0 && A > 0 && C > 0 && K > 0,
+                 "attention_step: non-positive dimension (B=%d L=%d M=%d D=%d A=%d C=%d K=%d)", B, L, M, D, A, C, K);
+    B200_REQUIRE(A % 4 == 0, "attention_step: attention dimension %d must be a multiple of 4", A);
+    B200_TRY(require_device());
+    B200_REQUIRE(A <= 128 && M <= 512 && (K % 2) == 1, "attention_step: unsupported dims A=%d M=%d K=%d", A, M, K);
+    cudaStream_t st = (cudaStream_t)stream;
+    // q = query . Wq^T into workspace[0 : B*A]; new cum into workspace[B*A : B*A + B*L] then copied back
+    float* q = workspace;
+    float* cum_next = workspace + (size_t)B * A;
+    B200_TRY(run_gemm(st, B, A, D, query, D, w_query, D, true, q, A, nullptr, 0.f));
+    AttnFwdArgs aa{};
+    aa.qpart = q; aa.nq = 1; aa.q_save = nullptr; aa.memT = memory_transform; aa.memory = memory; aa.lengths = text_lengths;
+    aa.Wc = w_loc_features; aa.Wloc = w_location; aa.bias = bias; aa.v = w_energy; aa.cum_prev = cum_weights; aa.cum_next = cum_next;
+    aa.align = weights; aa.align_bstride = L; aa.ctx_out = context; aa.ld_ctx = M; aa.ctx_out2 = nullptr; aa.ld_ctx2 = 0;
+    aa.B = B; aa.L = L; aa.M = M; aa.A = A; aa.C = C; aa.K = K;
+    B200_TRY(launch_attn_fwd(aa, st));
+    B200_TRY(launch_copy2d(cum_weights, L, cum_next, L, B, L, st));
+    return B200TTS_OK;
+}
+
+size_t b200tts_forward_attention_step_workspace_elems(int B, int L, int A) { return (size_t)B * A + (size_t)B * L; }
+
 // ---- standalone forward-attention step (module-level parity of ForwardAttention.forward) ----
-int forward_attention_step_impl(int B, int L, int M, int D, int A, const float* query, const float* memory, const float* memT,
-                                const int* lengths, const float* Wq, const float* bias, const float* v, float* alpha, float* ctx,
-                                float* weights, float* workspace, cudaStream_t st) {
+int b200tts_forward_attention_step(int B, int L, int M, int D, int A, const float* query, const float* memory,
+                                   const float* memory_transform, const int32_t* text_lengths, const float* w_query,
+                                   const float* bias, const float* w_energy, float* alpha, float* context, float* weights,
+                                   float* workspace, void* stream) {
+    B200_TRY(require_device());
+    B200_REQUIRE(query && memory && memory_transform && text_lengths && w_query && bias && w_energy && alpha && context && weights &&
+                 workspace, "forward_attention_step: null argument");
     B200_REQUIRE(B > 0 && L > 0 && D > 0 && A > 0 && A <= 128 && M > 0 && M <= 512,
                  "forward_attention_step: unsupported dims B=%d L=%d D=%d A=%d M=%d", B, L, D, A, M);
+    cudaStream_t st = (cudaStream_t)stream;
     // q = query . Wq^T into workspace[0 : B*A]; the new alpha into workspace[B*A : B*A + B*L], then copied back
     float* q = workspace;
     float* alpha_next = workspace + (size_t)B * A;
-    B200_TRY(run_gemm(st, B, A, D, query, D, Wq, D, true, q, A, nullptr, 0.f));
+    B200_TRY(run_gemm(st, B, A, D, query, D, w_query, D, true, q, A, nullptr, 0.f));
     FwdAttnArgs fa{};
-    fa.qpart = q; fa.nq = 1; fa.q_save = nullptr; fa.memT = memT; fa.memory = memory; fa.lengths = lengths;
-    fa.bias = bias; fa.v = v; fa.alpha_prev = alpha; fa.alpha_next = alpha_next;
-    fa.align = weights; fa.align_bstride = L; fa.ctx_out = ctx; fa.ld_ctx = M;
+    fa.qpart = q; fa.nq = 1; fa.q_save = nullptr; fa.memT = memory_transform; fa.memory = memory; fa.lengths = text_lengths;
+    fa.bias = bias; fa.v = w_energy; fa.alpha_prev = alpha; fa.alpha_next = alpha_next;
+    fa.align = weights; fa.align_bstride = L; fa.ctx_out = context; fa.ld_ctx = M;
     fa.B = B; fa.L = L; fa.M = M; fa.A = A;
     B200_TRY(launch_fwd_attn(fa, st));
     B200_TRY(launch_copy2d(alpha, L, alpha_next, L, B, L, st));
     return B200TTS_OK;
 }
 
-// ---- initial state of listed rows of a carried state (b200tts_decoder_state_reset_rows) ----
-int decoder_state_reset_rows_check(const b200tts_decoder_shape& s, const b200tts_decoder_state& state, const int* rows, int count) {
-    B200_REQUIRE(s.B > 0 && s.L > 0 && s.M > 0 && s.D > 0 && s.N > 0, "decoder_state_reset_rows: non-positive dimension (B=%d L=%d M=%d D=%d N=%d)",
-                 s.B, s.L, s.M, s.D, s.N);
-    B200_REQUIRE(s.att_kind == B200TTS_ATT_LOCATION || s.att_kind == B200TTS_ATT_FORWARD, "decoder_state_reset_rows: bad attention kind %d",
-                 s.att_kind);
-    B200_REQUIRE(state.att_h && state.att_c && state.gen_h && state.gen_c && state.context && state.cum_weights && state.frame,
-                 "decoder_state_reset_rows: every state buffer is required");
-    B200_REQUIRE(rows && count >= 1 && count <= s.B, "decoder_state_reset_rows: %d rows of a state of %d", count, s.B);
-    for (int k = 0; k < count; ++k)
-        B200_REQUIRE(rows[k] >= 0 && rows[k] < s.B, "decoder_state_reset_rows: row %d outside [0, %d)", rows[k], s.B);
-    return B200TTS_OK;
+int b200tts_lstm_cell_forward(int B, int D, int cell_kind, int training, float rate_h, float rate_c, float* gates, const float* h_prev,
+                              const float* c_prev, const uint8_t* mask_h, const uint8_t* mask_c, float* h_out, float* c_out, void* stream) {
+    B200_REQUIRE(B > 0 && D > 0 && gates && h_prev && c_prev && h_out && c_out, "lstm_cell_forward: bad argument");
+    B200_REQUIRE(cell_kind == B200TTS_CELL_DROPOUT || cell_kind == B200TTS_CELL_ZONEOUT, "lstm_cell_forward: bad cell kind %d", cell_kind);
+    B200_REQUIRE(rate_h >= 0.f && rate_h < 1.f && rate_c >= 0.f && rate_c < 1.f, "lstm_cell_forward: rates must be in [0, 1)");
+    B200_TRY(require_device());
+    CellFwdArgs a{};
+    a.xproj = gates; a.gates = gates; a.part = nullptr; a.nsplit = 0; a.part_stride = 0;
+    a.c_prev = c_prev; a.h_prev = h_prev; a.ld_hprev = D; a.c_out = c_out; a.h_out = h_out; a.ld_hout = D;
+    a.mask_h = mask_h; a.mask_c = mask_c; a.kind = cell_kind; a.training = training; a.rate_h = rate_h; a.rate_c = rate_c;
+    a.B = B; a.D = D;
+    return launch_cell_fwd(a, (cudaStream_t)stream);
 }
 
-int decoder_state_reset_rows_impl(const b200tts_decoder_shape& s, const b200tts_decoder_state& state, const int* rows, int count,
-                                  cudaStream_t st) {
-    B200_TRY(decoder_state_reset_rows_check(s, state, rows, count));
-    DecInitRows a{};
-    a.ctx = state.context; a.ld_ctx = s.M; a.att_h = state.att_h; a.ld_att_h = s.D;
-    a.att_c = state.att_c; a.gen_h = state.gen_h; a.gen_c = state.gen_c; a.cum = state.cum_weights; a.frame = state.frame;
-    a.attended = state.attended;
-    a.M = s.M; a.D = s.D; a.L = s.L; a.N = s.N; a.one_hot = forward_attention(s);
-    for (int k0 = 0; k0 < count; k0 += B200TTS_DECODER_RESET_MAX_ROWS) {
-        a.n = count - k0 < B200TTS_DECODER_RESET_MAX_ROWS ? count - k0 : B200TTS_DECODER_RESET_MAX_ROWS;
-        for (int k = 0; k < a.n; ++k) a.row[k] = rows[k0 + k];
-        B200_TRY(launch_init_rows(a, a.n, st));
-    }
-    return B200TTS_OK;
-}
-
-}  // namespace b200tts
+}  // extern "C"

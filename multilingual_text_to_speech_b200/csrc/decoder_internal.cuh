@@ -129,6 +129,8 @@ static inline DecoderLayout decoder_layout(const b200tts_decoder_shape& s) {
 int validate_decoder_shape(const b200tts_decoder_shape& s);
 static inline bool forward_attention(const b200tts_decoder_shape& s) { return s.att_kind == B200TTS_ATT_FORWARD; }
 static inline bool attention_window(const b200tts_decoder_shape& s) { return s.att_window_ahead > 0; }
+// forced attention rows (synthesis from given alignments) are given: only b200tts_decoder_forward_chunk takes them
+static inline bool forced_inputs(const b200tts_decoder_inputs& in) { return in.forced_count != 0 || in.forced_rows || in.forced_alignment; }
 
 // ---- forward attention (modules/attention.py:89-124): the part of the step its forward and backward kernels share, so that the
 // backward recomputes bit-identical transition probabilities and takes the same clamp decisions as the forward did ----

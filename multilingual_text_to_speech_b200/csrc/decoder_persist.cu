@@ -160,3 +160,11 @@ int persist_att_prep(const b200tts_decoder_shape& s, const b200tts_decoder_param
 }
 
 }  // namespace b200tts
+using namespace b200tts;
+
+// byte offset of the persistent forward loops' phase counters inside the forward workspace (for the step shape the forward runs on)
+extern "C" size_t b200tts_debug_persist_profile_offset(const b200tts_decoder_shape* shape) {
+    if (!shape || validate_decoder_shape(*shape) != B200TTS_OK) return 0;
+    const b200tts_decoder_shape s = step_shape(*shape);
+    return decoder_layout(s).persist * sizeof(float) + persist_layout(s).barrier + 256;
+}

@@ -853,3 +853,17 @@ int tc_persist_gen_loop(const b200tts_decoder_shape& s, const b200tts_decoder_pa
 }
 
 }  // namespace b200tts
+using namespace b200tts;
+
+// the plan and geometry of the persistent loops for the step shape the forward and backward run on
+extern "C" int b200tts_debug_decoder_geometry(const b200tts_decoder_shape* shape, int* out, int n) {
+    if (!shape || !out || validate_decoder_shape(*shape) != B200TTS_OK) return 0;
+    const b200tts_decoder_shape s = step_shape(*shape);
+    const TcPersistGeom g = tc_persist_geom(s);
+    const AttBwdGeom ab = att_bwd_geom(s);
+    const int v[14] = {b200tts_decoder_path(shape), g.grid, g.NBH, g.slot_kb_att, g.ch_h_att, g.ch_h_att ? g.nkb_h / g.ch_h_att : 0, g.ch_c_att,
+                       g.n_c_att, g.alias_att, g.use_btab, g.slot_gen, g.ch_h_gen, ab.UN, ab.grid};
+    const int m = n < 14 ? n : 14;
+    for (int k = 0; k < m; ++k) out[k] = v[k];
+    return m;
+}

@@ -8,11 +8,6 @@
 
 namespace b200tts {
 
-int gemm_tc_conv(const float* weight, const float* in, float* out, int NB, int G, int Cout, int Cin, int L, int k, int dil, int pad, int bwd,
-                 float beta, cudaStream_t st, bool* handled);
-int gemm_tc_conv_dw(const float* dz, const float* x, float* dweight, int NB, int G, int Cout, int Cin, int L, int k, int dil, int pad,
-                    cudaStream_t st, bool* handled);
-
 namespace {
 
 // col[nb, i*k + t, l] = x[nb, i, l + t*dil - pad]  (zero outside)      nb runs over (row, group) pairs
@@ -698,19 +693,10 @@ int validate_block(const b200tts_convblock_shape& s) {
 
 }  // namespace
 
-size_t convblock_saved_floats(const b200tts_convblock_shape& s) {
-    const BlockDims d = block_dims(s);
-    return align_up_sz(d.conv_elems, 64) + 2 * align_up_sz(d.Ct, 64);
-}
-size_t convblock_workspace_floats(const b200tts_convblock_shape& s) {
-    const BlockDims d = block_dims(s);
-    // forward: im2col.  backward: im2col + dz/dconv + dcol + s1/s2 + split-K scratch
-    return align_up_sz(d.col_elems, 64) * 2 + align_up_sz(d.conv_elems, 64) + 2 * align_up_sz(d.Ct, 64) + kGemmScratch;
-}
-
-int convblock_forward_impl(const b200tts_convblock_shape& s, const float* x, const float* weight, const float* gamma,
-                           const float* beta, int affine_gstride, float* running_mean, float* running_var, const uint8_t* keep,
-                           float* out, float* saved, float* ws, cudaStream_t st, const int32_t* lengths, const int32_t* counts) {
+static int convblock_forward_impl(const b200tts_convblock_shape& s, const float* x, const float* weight, const float* gamma,
+                                  const float* beta, int affine_gstride, float* running_mean, float* running_var, const uint8_t* keep,
+                                  float* out, float* saved, float* ws, cudaStream_t st, const int32_t* lengths = nullptr,
+                                  const int32_t* counts = nullptr) {
     B200_TRY(validate_block(s));
     // padded batches: only the fused epilogue of an eval-mode whole block knows the lengths (training statistics would need them too)
     B200_REQUIRE(!lengths || (s.stage == 0 && !s.training), "convblock_forward_masked: lengths need an eval-mode whole block (stage 0)");
@@ -761,9 +747,10 @@ int convblock_forward_impl(const b200tts_convblock_shape& s, const float* x, con
     return B200TTS_OK;
 }
 
-int convblock_backward_impl(const b200tts_convblock_shape& s, const float* x, const float* weight, const float* gamma,
-                            const float* beta, int affine_gstride, const uint8_t* keep, const float* saved, const float* dout,
-                            float* dx, float* dweight, float* dgamma, float* dbeta, float* ws, cudaStream_t st, const int32_t* counts) {
+static int convblock_backward_impl(const b200tts_convblock_shape& s, const float* x, const float* weight, const float* gamma,
+                                   const float* beta, int affine_gstride, const uint8_t* keep, const float* saved, const float* dout,
+                                   float* dx, float* dweight, float* dgamma, float* dbeta, float* ws, cudaStream_t st,
+                                   const int32_t* counts = nullptr) {
     B200_TRY(validate_block(s));
     const BlockDims d = block_dims(s);
     const float* conv = s.stage == 2 ? x : saved;
@@ -930,10 +917,88 @@ __global__ void __launch_bounds__(256) generator_tail_bwd_kernel(float* __restri
     }
 }
 
-size_t generator_workspace_floats(int G, int bn) { return align_up_sz((size_t)G * bn, 64) + kGemmScratch; }
+}  // namespace b200tts
+using namespace b200tts;
 
-int generator_forward_impl(int G, int gd, int bn, long long R, const float* e, const float* Wb, const float* bb, const float* Wk,
-                           const float* bk, float* eb, float* out, cudaStream_t st) {
+extern "C" {
+
+size_t b200tts_convblock_saved_bytes(const b200tts_convblock_shape* s) {
+    if (!s) return 0;
+    const BlockDims d = block_dims(*s);
+    return (align_up_sz(d.conv_elems, 64) + 2 * align_up_sz(d.Ct, 64)) * sizeof(float);
+}
+size_t b200tts_convblock_workspace_bytes(const b200tts_convblock_shape* s) {
+    if (!s) return 0;
+    const BlockDims d = block_dims(*s);
+    // forward: im2col.  backward: im2col + dz/dconv + dcol + s1/s2 + split-K scratch
+    return (align_up_sz(d.col_elems, 64) * 2 + align_up_sz(d.conv_elems, 64) + 2 * align_up_sz(d.Ct, 64) + kGemmScratch) * sizeof(float);
+}
+
+int b200tts_convblock_forward(const b200tts_convblock_shape* shape, const float* x, const float* weight, const float* gamma,
+                              const float* beta, int affine_gstride, float* running_mean, float* running_var, const uint8_t* keep,
+                              float* out, void* saved, void* workspace, void* stream) {
+    B200_REQUIRE(shape && x && out && saved && workspace, "convblock_forward: null argument");
+    B200_REQUIRE((weight || shape->stage == 2) && ((gamma && beta) || shape->stage == 1), "convblock_forward: null parameter");
+    B200_TRY(require_device());
+    return convblock_forward_impl(*shape, x, weight, gamma, beta, affine_gstride, running_mean, running_var, keep, out, (float*)saved,
+                                  (float*)workspace, (cudaStream_t)stream);
+}
+
+int b200tts_convblock_forward_masked(const b200tts_convblock_shape* shape, const int32_t* lengths, const float* x, const float* weight,
+                                     const float* gamma, const float* beta, int affine_gstride, float* running_mean, float* running_var,
+                                     const uint8_t* keep, float* out, void* saved, void* workspace, void* stream) {
+    B200_REQUIRE(shape && lengths && x && out && saved && workspace, "convblock_forward_masked: null argument");
+    B200_REQUIRE(shape->stage == 0 && !shape->training, "convblock_forward_masked: eval mode and the whole block (stage 0) only");
+    B200_REQUIRE(weight && gamma && beta, "convblock_forward_masked: null parameter");
+    B200_TRY(require_device());
+    return convblock_forward_impl(*shape, x, weight, gamma, beta, affine_gstride, running_mean, running_var, keep, out, (float*)saved,
+                                  (float*)workspace, (cudaStream_t)stream, lengths);
+}
+
+int b200tts_convblock_backward(const b200tts_convblock_shape* shape, const float* x, const float* weight, const float* gamma,
+                               const float* beta, int affine_gstride, const uint8_t* keep, const void* saved, const float* dout,
+                               float* dx, float* dweight, float* dgamma, float* dbeta, void* workspace, void* stream) {
+    B200_REQUIRE(shape && x && saved && dout && workspace, "convblock_backward: null argument");
+    B200_REQUIRE((weight || shape->stage == 2) && ((gamma && beta) || shape->stage == 1), "convblock_backward: null parameter");
+    B200_REQUIRE(dx || !shape->highway, "convblock_backward: highway blocks need dx");
+    B200_TRY(require_device());
+    return convblock_backward_impl(*shape, x, weight, gamma, beta, affine_gstride, keep, (const float*)saved, dout, dx, dweight, dgamma,
+                                   dbeta, (float*)workspace, (cudaStream_t)stream);
+}
+
+int b200tts_convblock_forward_counts(const b200tts_convblock_shape* shape, const int32_t* counts, int G, int NB, const float* x,
+                                     const float* weight, const float* gamma, const float* beta, int affine_gstride, float* running_mean,
+                                     float* running_var, const uint8_t* keep, float* out, void* saved, void* workspace, void* stream) {
+    B200_REQUIRE(shape && counts && x && out && saved && workspace, "convblock_forward_counts: null argument");
+    B200_REQUIRE(G == shape->G && NB == shape->NB, "convblock_forward_counts: counts are for G=%d, NB=%d but the shape has G=%d, NB=%d", G, NB,
+                 shape->G, shape->NB);
+    B200_REQUIRE((weight || shape->stage == 2) && ((gamma && beta) || shape->stage == 1), "convblock_forward_counts: null parameter");
+    B200_TRY(require_device());
+    return convblock_forward_impl(*shape, x, weight, gamma, beta, affine_gstride, running_mean, running_var, keep, out, (float*)saved,
+                                  (float*)workspace, (cudaStream_t)stream, nullptr, counts);
+}
+
+int b200tts_convblock_backward_counts(const b200tts_convblock_shape* shape, const int32_t* counts, int G, int NB, const float* x,
+                                      const float* weight, const float* gamma, const float* beta, int affine_gstride, const uint8_t* keep,
+                                      const void* saved, const float* dout, float* dx, float* dweight, float* dgamma, float* dbeta,
+                                      void* workspace, void* stream) {
+    B200_REQUIRE(shape && counts && x && saved && dout && workspace, "convblock_backward_counts: null argument");
+    B200_REQUIRE(G == shape->G && NB == shape->NB, "convblock_backward_counts: counts are for G=%d, NB=%d but the shape has G=%d, NB=%d", G, NB,
+                 shape->G, shape->NB);
+    B200_REQUIRE((weight || shape->stage == 2) && ((gamma && beta) || shape->stage == 1), "convblock_backward_counts: null parameter");
+    B200_REQUIRE(dx || !shape->highway, "convblock_backward_counts: highway blocks need dx");
+    B200_TRY(require_device());
+    return convblock_backward_impl(*shape, x, weight, gamma, beta, affine_gstride, keep, (const float*)saved, dout, dx, dweight, dgamma,
+                                   dbeta, (float*)workspace, (cudaStream_t)stream, counts);
+}
+
+size_t b200tts_generator_workspace_bytes(int G, int bn) { return (align_up_sz((size_t)G * bn, 64) + kGemmScratch) * sizeof(float); }
+
+int b200tts_generator_forward(int G, int gd, int bn, long long R, const float* e, const float* Wb, const float* bb, const float* Wk,
+                              const float* bk, float* eb, float* out, void* stream) {
+    B200_REQUIRE(e && Wb && bb && Wk && bk && eb && out, "generator_forward: null argument");
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
     B200_REQUIRE(G > 0 && gd > 0 && bn > 0 && R > 0 && R < (1ll << 31), "generator: bad dimensions");
     if (G <= GEN_MAXG && bn <= GEN_MAXBN) {      // skinny product, bound by reading Wk / writing the generated kernel once (bottleneck folded in)
         generator_expand_kernel<<<grid_for((size_t)R), 256, 0, st>>>(out, eb, Wk, bk, G, bn, (size_t)R, e, Wb, bb, gd);
@@ -948,10 +1013,14 @@ int generator_forward_impl(int G, int gd, int bn, long long R, const float* e, c
     return gemm_f32(b, st);
 }
 
-int generator_backward_impl(int G, int gd, int bn, long long R, const float* e, const float* Wb, const float* Wk, const float* eb,
-                            const float* dout, float* de, float* dWb, float* dbb, float* dWk, float* dbk, float* ws, cudaStream_t st) {
-    float* deb = ws;
-    float* scratch = ws + align_up_sz((size_t)G * bn, 64);
+int b200tts_generator_backward(int G, int gd, int bn, long long R, const float* e, const float* Wb, const float* Wk, const float* eb,
+                               const float* dout, float* de, float* dWb, float* dbb, float* dWk, float* dbk, void* workspace,
+                               void* stream) {
+    B200_REQUIRE(e && Wb && Wk && eb && dout && de && dWb && dbb && dWk && dbk && workspace, "generator_backward: null argument");
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
+    float* deb = (float*)workspace;
+    float* scratch = deb + align_up_sz((size_t)G * bn, 64);
     const size_t chunk = 256;
     const int nblk = (int)((R + chunk - 1) / chunk);
     if (bn == 8 && G <= GEN_FG && (reinterpret_cast<uintptr_t>(Wk) & 15) == 0 && (reinterpret_cast<uintptr_t>(dWk) & 15) == 0 &&
@@ -993,17 +1062,22 @@ int generator_backward_impl(int G, int gd, int bn, long long R, const float* e, 
     return gemm_f32(dd, st);
 }
 
-int embedding_forward_impl(float* out, int ldo, const float* table, const int* ids, long long ntok, int E, cudaStream_t st) {
-    embedding_fwd_kernel<<<grid_for((size_t)ntok * E), 256, 0, st>>>(out, ldo, table, ids, (size_t)ntok, E);
-    B200_LAUNCH_CHECK();
-    return B200TTS_OK;
-}
-int embedding_backward_impl(float* dtable, int V, const float* dout, int ldo, const int* ids, long long ntok, int E, int padding_idx,
-                            cudaStream_t st) {
-    B200_REQUIRE(E <= 1024, "embedding_backward: embedding dimension %d > 1024 is not supported", E);
-    embedding_bwd_kernel<<<V, 256, 0, st>>>(dtable, dout, ldo, ids, (int)ntok, E, padding_idx);
+int b200tts_embedding_forward(float* out, int ldo, const float* table, const int32_t* ids, long long ntok, int E, void* stream) {
+    B200_REQUIRE(out && table && ids && ntok >= 0 && E > 0 && ldo >= E, "embedding_forward: bad argument");
+    B200_TRY(require_device());
+    embedding_fwd_kernel<<<grid_for((size_t)ntok * E), 256, 0, (cudaStream_t)stream>>>(out, ldo, table, ids, (size_t)ntok, E);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }
 
-}  // namespace b200tts
+int b200tts_embedding_backward(float* dtable, int V, const float* dout, int ldo, const int32_t* ids, long long ntok, int E,
+                               int padding_idx, void* stream) {
+    B200_REQUIRE(dtable && dout && ids && V > 0 && E > 0 && ldo >= E, "embedding_backward: bad argument");
+    B200_TRY(require_device());
+    B200_REQUIRE(E <= 1024, "embedding_backward: embedding dimension %d > 1024 is not supported", E);
+    embedding_bwd_kernel<<<V, 256, 0, (cudaStream_t)stream>>>(dtable, dout, ldo, ids, (int)ntok, E, padding_idx);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+}  // extern "C"

@@ -301,3 +301,37 @@ int gemm_run_auto(GemmDesc d, float* scratch, size_t scratch_elems, cudaStream_t
 }
 
 }  // namespace b200tts
+using namespace b200tts;
+
+extern "C" {
+
+int b200tts_gemm_f32(int transA, int transB, int M, int N, int K, float alpha, const float* A, int lda, const float* B,
+                     int ldb, float beta, float* C, int ldc, const float* bias, int batch, long long strideA,
+                     long long strideB, long long strideC, int splitk, float* workspace, void* stream) {
+    B200_TRY(require_device());
+    GemmDesc d;
+    d.A = A; d.B = B; d.C = C; d.bias = bias; d.M = M; d.N = N; d.K = K; d.lda = lda; d.ldb = ldb; d.ldc = ldc;
+    d.transA = transA; d.transB = transB; d.alpha = alpha; d.beta = beta; d.batch = batch < 1 ? 1 : batch;
+    d.strideA = strideA; d.strideB = strideB; d.strideC = strideC; d.splitk = splitk < 1 ? 1 : splitk; d.partial = workspace;
+    return gemm_run(d, (cudaStream_t)stream);
+}
+
+static_assert(sizeof(b200tts_gemm_desc) == sizeof(GemmDesc), "b200tts_gemm_desc must list the fields of GemmDesc");
+int b200tts_debug_gemm(const b200tts_gemm_desc* desc, int route, float* partial, size_t partial_elems, void* stream) {
+    B200_REQUIRE(desc, "debug_gemm: null descriptor");
+    B200_REQUIRE(route == 0 || route == 1, "debug_gemm: unknown route %d", route);
+    B200_TRY(require_device());
+    const b200tts_gemm_desc& s = *desc;
+    GemmDesc d;
+    d.A = s.A; d.B = s.B; d.C = s.C; d.bias = s.bias;
+    d.M = s.M; d.N = s.N; d.K = s.K; d.lda = s.lda; d.ldb = s.ldb; d.ldc = s.ldc;
+    d.transA = s.transA; d.transB = s.transB; d.alpha = s.alpha; d.beta = s.beta;
+    d.batch = s.batch; d.strideA = s.strideA; d.strideB = s.strideB; d.strideC = s.strideC; d.a_batch_mod = s.a_batch_mod;
+    d.splitk = s.splitk; d.partial = s.partial; d.keep_partials = s.keep_partials;
+    d.A16 = s.A16; d.lda16 = s.lda16; d.B16 = s.B16; d.ldb16 = s.ldb16;
+    d.kin = s.kin; d.kosA = s.kosA; d.kosB = s.kosB;
+    if (route == 0) return gemm_run(d, (cudaStream_t)stream);
+    return gemm_run_auto(d, partial, partial ? partial_elems : 0, (cudaStream_t)stream);
+}
+
+}  // extern "C"

@@ -389,7 +389,6 @@ void set_tc_scratch(void* ptr, size_t bytes) { g_scratch.ptr = static_cast<unsig
 void tc_pack_cache_begin() { g_cache_on = true; g_ncache = 0; g_cache_off = 0; }
 void tc_pack_cache_end() { g_cache_on = false; g_ncache = 0; g_cache_off = 0; }
 void set_tc_enabled(int on) { g_tc_enabled = on; }
-int tc_enabled() { return g_tc_enabled; }
 
 // Split-K decision shared by the dense and the convolution weight-gradient products: with fewer output tiles than CTA slots (2 per SM)
 // and a long K, K is cut into `splits` ranges of `kper` k-blocks; the partial tiles live at the END of the scratch, clear of the
@@ -582,3 +581,9 @@ int gemm_tc_conv_dw(const float* dz, const float* x, float* dweight, int NB, int
 }
 
 }  // namespace b200tts
+
+extern "C" int b200tts_debug_gemm_pack_cache(int open) {
+    if (open) b200tts::tc_pack_cache_begin();
+    else b200tts::tc_pack_cache_end();
+    return B200TTS_OK;
+}

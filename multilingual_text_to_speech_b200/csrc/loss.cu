@@ -128,8 +128,6 @@ __global__ void __launch_bounds__(LT) loss_backward_kernel(const LossArgs a, con
 
 }  // namespace
 
-size_t loss_workspace_floats() { return (size_t)LOSS_BLOCKS * 4; }
-
 static LossArgs make_args(const b200tts_loss_shape& s, const float* pre, const float* pre_t, const float* post, const float* post_t,
                           const float* stop, const float* stop_t, const float* align, const int* text_len, const int* target_len) {
     LossArgs a{};
@@ -141,14 +139,28 @@ static LossArgs make_args(const b200tts_loss_shape& s, const float* pre, const f
     return a;
 }
 
-int loss_forward_impl(const b200tts_loss_shape& s, const float* pre, const float* pre_t, const float* post, const float* post_t,
-                      const float* stop, const float* stop_t, const float* align, const int* text_len, const int* target_len, float* losses,
-                      float* ws, cudaStream_t st) {
+}  // namespace b200tts
+using namespace b200tts;
+
+extern "C" {
+
+size_t b200tts_loss_workspace_bytes(void) { return (size_t)LOSS_BLOCKS * 4 * sizeof(float); }
+
+int b200tts_tacotron_loss_forward(const b200tts_loss_shape* shape, const float* pre, const float* pre_target, const float* post,
+                                  const float* post_target, const float* stop, const float* stop_target, const float* alignment,
+                                  const int32_t* text_lengths, const int32_t* target_lengths, float* losses, void* workspace, void* stream) {
+    B200_REQUIRE(shape && pre && pre_target && post && post_target && stop && stop_target && text_lengths && target_lengths && losses && workspace,
+                 "tacotron_loss_forward: null argument");
+    const b200tts_loss_shape& s = *shape;
+    B200_REQUIRE(alignment || !s.guided, "tacotron_loss_forward: guided attention needs the alignments");
+    B200_TRY(require_device());
     B200_REQUIRE(s.B > 0 && s.N > 0 && s.T > 0 && s.L > 0 && s.R >= 0, "loss_forward: bad shape");
     B200_REQUIRE(!s.guided || s.guided_g > 0.f, "loss_forward: guided attention needs a positive variance");
-    const LossArgs a = make_args(s, pre, pre_t, post, post_t, stop, stop_t, align, text_len, target_len);
-    const uintptr_t addr_bits = reinterpret_cast<uintptr_t>(pre) | reinterpret_cast<uintptr_t>(pre_t) | reinterpret_cast<uintptr_t>(post) |
-                                reinterpret_cast<uintptr_t>(post_t);
+    cudaStream_t st = (cudaStream_t)stream;
+    float* ws = (float*)workspace;
+    const LossArgs a = make_args(s, pre, pre_target, post, post_target, stop, stop_target, alignment, text_lengths, target_lengths);
+    const uintptr_t addr_bits = reinterpret_cast<uintptr_t>(pre) | reinterpret_cast<uintptr_t>(pre_target) | reinterpret_cast<uintptr_t>(post) |
+                                reinterpret_cast<uintptr_t>(post_target);
     if ((addr_bits & 15) == 0)
         loss_partial_kernel<true><<<LOSS_BLOCKS, LT, 0, st>>>(a, ws);
     else
@@ -161,16 +173,21 @@ int loss_forward_impl(const b200tts_loss_shape& s, const float* pre, const float
     return B200TTS_OK;
 }
 
-int loss_backward_impl(const b200tts_loss_shape& s, const float* pre, const float* pre_t, const float* post, const float* post_t,
-                       const float* stop, const float* stop_t, const int* text_len, const int* target_len, const float* grad_losses,
-                       float* d_pre, float* d_post, float* d_stop, float* d_align, cudaStream_t st) {
+int b200tts_tacotron_loss_backward(const b200tts_loss_shape* shape, const float* pre, const float* pre_target, const float* post,
+                                   const float* post_target, const float* stop, const float* stop_target, const int32_t* text_lengths,
+                                   const int32_t* target_lengths, const float* grad_losses, float* d_pre, float* d_post, float* d_stop,
+                                   float* d_alignment, void* stream) {
+    B200_REQUIRE(shape && pre && pre_target && post && post_target && stop && stop_target && text_lengths && target_lengths && grad_losses,
+                 "tacotron_loss_backward: null argument");
+    B200_TRY(require_device());
+    const b200tts_loss_shape& s = *shape;
     B200_REQUIRE(s.R >= 0, "loss_backward: bad shape");
-    const LossArgs a = make_args(s, pre, pre_t, post, post_t, stop, stop_t, nullptr, text_len, target_len);
+    const LossArgs a = make_args(s, pre, pre_target, post, post_target, stop, stop_target, nullptr, text_lengths, target_lengths);
     const double nmel = (double)s.B * s.N * s.T, nstop = (double)s.B * s.T;
-    loss_backward_kernel<<<NUM_SMS * 8, LT, 0, st>>>(a, grad_losses, d_pre, d_post, d_stop, d_align, (float)(4.0 / nmel), (float)(2.0 / nmel),
-                                                 (float)(1.0 / (nstop * (s.N + 2))), (float)(1.0 / s.B));
+    loss_backward_kernel<<<NUM_SMS * 8, LT, 0, (cudaStream_t)stream>>>(a, grad_losses, d_pre, d_post, d_stop, d_alignment, (float)(4.0 / nmel),
+                                                                   (float)(2.0 / nmel), (float)(1.0 / (nstop * (s.N + 2))), (float)(1.0 / s.B));
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }
 
-}  // namespace b200tts
+}  // extern "C"

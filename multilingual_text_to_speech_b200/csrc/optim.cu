@@ -59,14 +59,21 @@ __global__ void __launch_bounds__(256) adam_clip_kernel(float* __restrict__ p, f
 
 }  // namespace
 
-size_t adam_clip_scratch_floats() { return NORM_BLOCKS + 8; }
+}  // namespace b200tts
+using namespace b200tts;
 
-int adam_clip_step_impl(float* p, float* g, float* m, float* v, size_t n, float lr, float beta1, float beta2, float eps, float weight_decay,
-                        float max_norm, int step, float* scratch, cudaStream_t st) {
+extern "C" {
+
+size_t b200tts_adam_clip_scratch_floats(void) { return NORM_BLOCKS + 8; }
+
+int b200tts_adam_clip_step(float* p, float* g, float* m, float* v, size_t n, float lr, float beta1, float beta2, float eps,
+                           float weight_decay, float max_norm, int step, float* scratch, void* stream) {
+    B200_TRY(require_device());
     B200_REQUIRE(p && g && m && v && scratch, "adam_clip_step: null argument");
     B200_REQUIRE(step >= 1 && beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f, "adam_clip_step: step must be >= 1 and betas in [0, 1)");
     B200_REQUIRE((reinterpret_cast<uintptr_t>(g) & 15) == 0, "adam_clip_step: the gradient buffer must be 16-byte aligned");
     if (n == 0) return B200TTS_OK;
+    cudaStream_t st = (cudaStream_t)stream;
     float* norm = scratch;                  // [0] = norm, [1] = clip coefficient
     float* partial = scratch + 8;
     size_t want = (n / 4 + 255) / 256;
@@ -83,4 +90,4 @@ int adam_clip_step_impl(float* p, float* g, float* m, float* v, size_t n, float 
     return B200TTS_OK;
 }
 
-}  // namespace b200tts
+}  // extern "C"

@@ -75,21 +75,39 @@ RnnLayout rnn_layout(const b200tts_bilstm_shape& s) {
 
 }  // namespace
 
-size_t bilstm_saved_floats(const b200tts_bilstm_shape& s) { return rnn_layout(s).total; }
-size_t bilstm_workspace_floats(const b200tts_bilstm_shape& s) { return rnn_layout(s).wtotal; }
-// b200tts_debug_bilstm_layout: byte offsets of xp, gates, hs, cs, bsum (saved) and dg, dxp (workspace), the split-K factors of the
-// chain's recurrent products (forward, backward) and whether the persistent kernel runs
-void bilstm_view_offsets(const b200tts_bilstm_shape& s, size_t* v) {
-    const RnnLayout l = rnn_layout(s);
+}  // namespace b200tts
+using namespace b200tts;
+
+extern "C" {
+
+size_t b200tts_bilstm_saved_bytes(const b200tts_bilstm_shape* s) { return s ? rnn_layout(*s).total * sizeof(float) : 0; }
+size_t b200tts_bilstm_workspace_bytes(const b200tts_bilstm_shape* s) { return s ? rnn_layout(*s).wtotal * sizeof(float) : 0; }
+
+// byte offsets of xp, gates, hs, cs, bsum (saved) and dg, dxp (workspace), the split-K factors of the chain's recurrent products
+// (forward, backward) and whether the persistent kernel runs
+int b200tts_debug_bilstm_layout(const b200tts_bilstm_shape* shape, size_t* out, int n) {
+    if (!shape || !out || shape->B <= 0 || shape->L <= 0 || shape->E <= 0 || shape->H <= 0) return 0;
+    const RnnLayout l = rnn_layout(*shape);
+    size_t v[10];
     const size_t f[7] = {l.xp, l.gates, l.hs, l.cs, l.bsum, l.dg, l.dxp};
     for (int k = 0; k < 7; ++k) v[k] = f[k] * sizeof(float);
     v[7] = (size_t)l.split;
     v[8] = (size_t)l.split_b;
-    v[9] = bilstm_persist_supported(s) ? 1 : 0;
+    v[9] = bilstm_persist_supported(*shape) ? 1 : 0;
+    const int m = n < 10 ? n : 10;
+    for (int k = 0; k < m; ++k) out[k] = v[k];
+    return m;
 }
 
-int bilstm_forward_impl(const b200tts_bilstm_shape& s, const b200tts_bilstm_params& w, const float* x, const int* lengths, float* out,
-                        float* saved, float* ws, cudaStream_t st) {
+int b200tts_bilstm_forward(const b200tts_bilstm_shape* shape, const b200tts_bilstm_params* params, const float* x,
+                           const int32_t* lengths, float* out, void* saved_buf, void* workspace, void* stream) {
+    B200_REQUIRE(shape && params && x && lengths && out && saved_buf && workspace, "bilstm_forward: null argument");
+    B200_TRY(require_device());
+    const b200tts_bilstm_shape& s = *shape;
+    const b200tts_bilstm_params& w = *params;
+    float* saved = (float*)saved_buf;
+    float* ws = (float*)workspace;
+    cudaStream_t st = (cudaStream_t)stream;
     B200_REQUIRE(s.B > 0 && s.L > 0 && s.E > 0 && s.H > 0, "bilstm: non-positive dimension");
     const RnnLayout l = rnn_layout(s);
     const int B = s.B, L = s.L, E = s.E, H = s.H;
@@ -135,8 +153,17 @@ int bilstm_forward_impl(const b200tts_bilstm_shape& s, const b200tts_bilstm_para
     return B200TTS_OK;
 }
 
-int bilstm_backward_impl(const b200tts_bilstm_shape& s, const b200tts_bilstm_params& w, const int* lengths, const float* saved,
-                         const float* dout, float* dx, const b200tts_bilstm_params& dw, float* ws, cudaStream_t st) {
+int b200tts_bilstm_backward(const b200tts_bilstm_shape* shape, const b200tts_bilstm_params* params, const int32_t* lengths,
+                            const void* saved_buf, const float* dout, float* dx, const b200tts_bilstm_params* d_params, void* workspace,
+                            void* stream) {
+    B200_REQUIRE(shape && params && lengths && saved_buf && dout && d_params && workspace, "bilstm_backward: null argument");
+    B200_TRY(require_device());
+    const b200tts_bilstm_shape& s = *shape;
+    const b200tts_bilstm_params& w = *params;
+    const b200tts_bilstm_params& dw = *d_params;
+    const float* saved = (const float*)saved_buf;
+    float* ws = (float*)workspace;
+    cudaStream_t st = (cudaStream_t)stream;
     const RnnLayout l = rnn_layout(s);
     const int B = s.B, L = s.L, E = s.E, H = s.H;
     const size_t BH = (size_t)B * H, B4H = 4 * BH;
@@ -191,4 +218,4 @@ int bilstm_backward_impl(const b200tts_bilstm_shape& s, const b200tts_bilstm_par
     return B200TTS_OK;
 }
 
-}  // namespace b200tts
+}  // extern "C"

@@ -276,7 +276,7 @@ __global__ void __launch_bounds__(DEEMPH_THREADS) vocoder_deemphasis_kernel(int 
 
 }  // namespace
 
-int vocoder_validate(const b200tts_vocoder_shape& s, FftPlan* plan) {
+static int vocoder_validate(const b200tts_vocoder_shape& s, FftPlan* plan) {
     B200_REQUIRE(s.B >= 1 && s.total_frames >= 2 * s.B, "vocoder: need B >= 1 and at least 2 frames per utterance (B = %d, total_frames = %d)",
                  s.B, s.total_frames);
     B200_REQUIRE(make_plan(s.N, plan), "vocoder: unsupported FFT size N = %d (even, <= 2048, N/2 with prime factors <= 31 only)", s.N);
@@ -288,13 +288,6 @@ int vocoder_validate(const b200tts_vocoder_shape& s, FftPlan* plan) {
     B200_REQUIRE((long long)s.hop * (s.total_frames - s.B) < (1ll << 31) && (long long)s.total_frames * s.N < (1ll << 40),
                  "vocoder: batch too large");
     return B200TTS_OK;
-}
-
-int vocoder_fft_plan(int N, int* radices, int capacity) {
-    FftPlan p;
-    B200_REQUIRE(make_plan(N, &p), "vocoder: unsupported FFT size N = %d (even, <= 2048, N/2 with prime factors <= 31 only)", N);
-    for (int i = 0; i < p.nst && i < capacity; ++i) radices[i] = p.radix[i];
-    return p.nst;
 }
 
 // workspace: twiddles W_M [M], W_N [M + 1], window [N], frame buffer [total_frames, N]; each region 256-byte aligned
@@ -310,21 +303,39 @@ static VocoderLayout vocoder_layout(const b200tts_vocoder_shape& s) {
     return l;
 }
 
-size_t vocoder_workspace_bytes(const b200tts_vocoder_shape& s) {
+}  // namespace b200tts
+using namespace b200tts;
+
+extern "C" {
+
+size_t b200tts_vocoder_workspace_bytes(const b200tts_vocoder_shape* shape) {
+    if (!shape) { set_last_error("vocoder_workspace_bytes: null shape"); return 0; }
     FftPlan p;
-    if (vocoder_validate(s, &p) != B200TTS_OK) return 0;
-    return vocoder_layout(s).bytes;
+    if (vocoder_validate(*shape, &p) != B200TTS_OK) return 0;
+    return vocoder_layout(*shape).bytes;
 }
 
-int spectrogram_magnitude_impl(const b200tts_vocoder_shape& s, const float* log_spec, const float* mel_basis, const float* mel_pinv_t,
-                               float nnls_step, float* S, cudaStream_t st) {
+int b200tts_vocoder_fft_plan(int N, int* radices, int capacity) {
+    B200_REQUIRE(radices || capacity == 0, "vocoder_fft_plan: null radices");
+    FftPlan p;
+    B200_REQUIRE(make_plan(N, &p), "vocoder: unsupported FFT size N = %d (even, <= 2048, N/2 with prime factors <= 31 only)", N);
+    for (int i = 0; i < p.nst && i < capacity; ++i) radices[i] = p.radix[i];
+    return p.nst;
+}
+
+int b200tts_spectrogram_magnitude(const b200tts_vocoder_shape* shape, const float* log_spec, const float* mel_basis, const float* mel_pinv_t,
+                                  float nnls_step, float* S_out, void* stream) {
+    B200_REQUIRE(shape && log_spec && S_out, "spectrogram_magnitude: null argument");
+    B200_TRY(require_device());
+    const b200tts_vocoder_shape& s = *shape;
     FftPlan p;
     B200_TRY(vocoder_validate(s, &p));
+    cudaStream_t st = (cudaStream_t)stream;
     const int K = p.M + 1;
     if (s.n_mels == 0) {
         KernelTimer kt("vocoder_magnitude", st);
         const long long n = (long long)s.total_frames * K;
-        vocoder_linear_magnitude_kernel<<<(int)std::min<long long>((n + 255) / 256, NUM_SMS * 16), 256, 0, st>>>(n, log_spec, s.power, S);
+        vocoder_linear_magnitude_kernel<<<(int)std::min<long long>((n + 255) / 256, NUM_SMS * 16), 256, 0, st>>>(n, log_spec, s.power, S_out);
         B200_LAUNCH_CHECK();
         return B200TTS_OK;
     }
@@ -335,20 +346,25 @@ int spectrogram_magnitude_impl(const b200tts_vocoder_shape& s, const float* log_
     B200_CUDA(cudaFuncSetAttribute(vocoder_mel_nnls_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     KernelTimer kt("vocoder_magnitude", st);
     vocoder_mel_nnls_kernel<<<cdiv(s.total_frames, NNLS_WARPS), NNLS_WARPS * 32, smem, st>>>(s.total_frames, K, s.n_mels, log_spec, mel_basis,
-                                                                                           mel_pinv_t, nnls_step, s.nnls_iters, s.power, S);
+                                                                                           mel_pinv_t, nnls_step, s.nnls_iters, s.power, S_out);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }
 
-int griffinlim_impl(const b200tts_vocoder_shape& s, const float* S, const int* off, float* angles, float* rebuilt, int first, int iters,
-                    float* wave, void* ws, size_t ws_bytes, cudaStream_t st) {
+int b200tts_griffinlim(const b200tts_vocoder_shape* shape, const float* S, const int32_t* off, float* angles, float* rebuilt, int first,
+                       int iters, float* wave, void* workspace, size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(shape && S && off && angles && rebuilt, "griffinlim: null argument");
+    B200_TRY(require_device());
+    const b200tts_vocoder_shape& s = *shape;
     FftPlan p;
     B200_TRY(vocoder_validate(s, &p));
     B200_REQUIRE(iters >= 0, "griffinlim: negative iteration count %d", iters);
     const VocoderLayout l = vocoder_layout(s);
-    B200_REQUIRE(ws && ws_bytes >= l.bytes, "griffinlim: workspace of %zu bytes is smaller than the %zu required", ws_bytes, l.bytes);
-    B200_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "griffinlim: workspace must be 256-byte aligned");
-    unsigned char* base = static_cast<unsigned char*>(ws);
+    B200_REQUIRE(workspace && workspace_bytes >= l.bytes, "griffinlim: workspace of %zu bytes is smaller than the %zu required", workspace_bytes,
+                 l.bytes);
+    B200_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "griffinlim: workspace must be 256-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    unsigned char* base = static_cast<unsigned char*>(workspace);
     float2* twM = reinterpret_cast<float2*>(base + l.twM);
     float2* twN = reinterpret_cast<float2*>(base + l.twN);
     float* window = reinterpret_cast<float*>(base + l.window);
@@ -387,21 +403,24 @@ int griffinlim_impl(const b200tts_vocoder_shape& s, const float* S, const int* o
     return B200TTS_OK;
 }
 
-int deemphasis_normalize_impl(const b200tts_vocoder_shape& s, float* wave, const int* off, cudaStream_t st) {
+int b200tts_deemphasis_normalize(const b200tts_vocoder_shape* shape, float* wave, const int32_t* off, void* stream) {
+    B200_REQUIRE(shape && wave && off, "deemphasis_normalize: null argument");
+    B200_TRY(require_device());
+    const b200tts_vocoder_shape& s = *shape;
     FftPlan p;
     B200_TRY(vocoder_validate(s, &p));
+    cudaStream_t st = (cudaStream_t)stream;
     KernelTimer kt("vocoder_deemphasis", st);
     vocoder_deemphasis_kernel<false><<<s.B, DEEMPH_THREADS, 0, st>>>(s.hop, off, s.preemphasis, wave);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }
 
-// y[r, :] = lfilter([1], [1, -a], y[r, :]) for each of `rows` rows of `len` samples, no normalisation (the WaveRNN folds)
-int deemphasis_rows_impl(int rows, int len, float a, float* y, cudaStream_t st) {
+}  // extern "C"
+
+int b200tts::deemphasis_rows(int rows, int len, float a, float* y, cudaStream_t st) {
     if (a == 0.f) return B200TTS_OK;
     vocoder_deemphasis_kernel<true><<<rows, DEEMPH_THREADS, 0, st>>>(len, nullptr, a, y);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }
-
-}  // namespace b200tts

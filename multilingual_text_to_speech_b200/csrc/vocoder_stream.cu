@@ -217,7 +217,7 @@ __global__ void __launch_bounds__(GL_THREADS) gl_stream_run_kernel(FftPlan p, in
 
 }  // namespace
 
-int gl_stream_validate(const b200tts_gl_stream_shape& s, FftPlan* p) {
+static int gl_stream_validate(const b200tts_gl_stream_shape& s, FftPlan* p) {
     B200_REQUIRE(make_plan(s.N, p), "gl_stream: unsupported FFT size N = %d (even, <= 2048, N/2 with prime factors <= 31 only)", s.N);
     B200_REQUIRE(s.win >= 1 && s.win <= s.N, "gl_stream: window length %d must be in [1, N = %d]", s.win, s.N);
     B200_REQUIRE(s.hop >= 1 && s.hop <= s.win, "gl_stream: hop %d must be in [1, win = %d]", s.hop, s.win);
@@ -234,39 +234,44 @@ int gl_stream_validate(const b200tts_gl_stream_shape& s, FftPlan* p) {
     return B200TTS_OK;
 }
 
-size_t gl_stream_workspace_bytes(const b200tts_gl_stream_shape& s) {
-    FftPlan p;
-    if (gl_stream_validate(s, &p) != B200TTS_OK) return 0;
-    return gl_layout(s, p).bytes;
-}
-
 static int gl_check_workspace(const GlLayout& l, void* ws, size_t ws_bytes, const char* what) {
     B200_REQUIRE(ws && ws_bytes >= l.bytes, "%s: workspace of %zu bytes is smaller than the %zu required", what, ws_bytes, l.bytes);
     B200_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "%s: workspace must be 256-byte aligned", what);
     return B200TTS_OK;
 }
 
-int gl_stream_reset_check(const b200tts_gl_stream_shape& s, void* ws, size_t ws_bytes, const int* list, int count) {
+}  // namespace b200tts
+using namespace b200tts;
+
+extern "C" {
+
+size_t b200tts_gl_stream_workspace_bytes(const b200tts_gl_stream_shape* shape) {
+    if (!shape) { set_last_error("gl_stream_workspace_bytes: null shape"); return 0; }
     FftPlan p;
-    B200_TRY(gl_stream_validate(s, &p));
-    B200_TRY(gl_check_workspace(gl_layout(s, p), ws, ws_bytes, "gl_stream_reset"));
-    B200_REQUIRE(list && count >= 1 && count <= s.slots, "gl_stream_reset: need 1 to %d slots (got %d)", s.slots, count);
-    unsigned long long seen = 0;
-    for (int i = 0; i < count; ++i) {
-        B200_REQUIRE(list[i] >= 0 && list[i] < s.slots, "gl_stream_reset: slot %d outside [0, %d)", list[i], s.slots);
-        B200_REQUIRE(!(seen >> list[i] & 1), "gl_stream_reset: slot %d listed twice", list[i]);
-        seen |= 1ull << list[i];
-    }
-    return B200TTS_OK;
+    if (gl_stream_validate(*shape, &p) != B200TTS_OK) return 0;
+    return gl_layout(*shape, p).bytes;
 }
 
-int gl_stream_reset_impl(const b200tts_gl_stream_shape& s, void* ws, const int* list, int count, cudaStream_t st) {
+int b200tts_gl_stream_reset(const b200tts_gl_stream_shape* shape, void* workspace, size_t workspace_bytes, const int32_t* slots, int count,
+                            void* stream) {
+    B200_REQUIRE(shape, "gl_stream_reset: null argument");
+    const b200tts_gl_stream_shape& s = *shape;
     FftPlan p;
     B200_TRY(gl_stream_validate(s, &p));
     const GlLayout l = gl_layout(s, p);
-    unsigned char* base = static_cast<unsigned char*>(ws);
+    B200_TRY(gl_check_workspace(l, workspace, workspace_bytes, "gl_stream_reset"));
+    B200_REQUIRE(slots && count >= 1 && count <= s.slots, "gl_stream_reset: need 1 to %d slots (got %d)", s.slots, count);
+    unsigned long long seen = 0;
+    for (int i = 0; i < count; ++i) {
+        B200_REQUIRE(slots[i] >= 0 && slots[i] < s.slots, "gl_stream_reset: slot %d outside [0, %d)", slots[i], s.slots);
+        B200_REQUIRE(!(seen >> slots[i] & 1), "gl_stream_reset: slot %d listed twice", slots[i]);
+        seen |= 1ull << slots[i];
+    }
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
+    unsigned char* base = static_cast<unsigned char*>(workspace);
     GlRows rows{};
-    for (int i = 0; i < count; ++i) rows.r[i].slot = list[i];
+    for (int i = 0; i < count; ++i) rows.r[i].slot = slots[i];
     KernelTimer kt("gl_stream_reset", st);
     gl_stream_reset_kernel<<<count, 256, 0, st>>>(s.N, s.win, reinterpret_cast<float2*>(base + l.twM), reinterpret_cast<float2*>(base + l.twN),
                                                   reinterpret_cast<float*>(base + l.window), base + l.slots, l.slot_bytes, rows);
@@ -274,10 +279,14 @@ int gl_stream_reset_impl(const b200tts_gl_stream_shape& s, void* ws, const int* 
     return B200TTS_OK;
 }
 
-int gl_stream_run_check(const b200tts_gl_stream_shape& s, const b200tts_gl_stream_row* rows, int count, void* ws, size_t ws_bytes) {
+int b200tts_gl_stream_run(const b200tts_gl_stream_shape* shape, const b200tts_gl_stream_row* rows, int count, const float* S_new, float* wave,
+                          void* workspace, size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(shape && S_new && wave, "gl_stream_run: null argument");
+    const b200tts_gl_stream_shape& s = *shape;
     FftPlan p;
     B200_TRY(gl_stream_validate(s, &p));
-    B200_TRY(gl_check_workspace(gl_layout(s, p), ws, ws_bytes, "gl_stream_run"));
+    const GlLayout l = gl_layout(s, p);
+    B200_TRY(gl_check_workspace(l, workspace, workspace_bytes, "gl_stream_run"));
     B200_REQUIRE(rows && count >= 1 && count <= s.slots, "gl_stream_run: need 1 to %d rows (got %d)", s.slots, count);
     unsigned long long seen = 0;
     for (int i = 0; i < count; ++i) {
@@ -289,20 +298,14 @@ int gl_stream_run_check(const b200tts_gl_stream_shape& s, const b200tts_gl_strea
         B200_REQUIRE(!r.ended || r.frames >= 2, "gl_stream_run: row %d: a stream ends with at least 2 frames (got %d)", i, r.frames);
         B200_REQUIRE((long long)s.hop * r.frames + 2ll * s.N < (1ll << 31), "gl_stream_run: row %d: stream too long (%d frames)", i, r.frames);
     }
-    return B200TTS_OK;
-}
-
-int gl_stream_run_impl(const b200tts_gl_stream_shape& s, const b200tts_gl_stream_row* list, int count, const float* S_new, float* wave, void* ws,
-                       cudaStream_t st) {
-    FftPlan p;
-    B200_TRY(gl_stream_validate(s, &p));
-    const GlLayout l = gl_layout(s, p);
-    unsigned char* base = static_cast<unsigned char*>(ws);
-    GlRows rows{};
-    for (int i = 0; i < count; ++i) rows.r[i] = list[i];
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
+    unsigned char* base = static_cast<unsigned char*>(workspace);
+    GlRows list{};
+    for (int i = 0; i < count; ++i) list.r[i] = rows[i];
     B200_CUDA(cudaFuncSetAttribute(gl_stream_run_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l.smem));
     KernelTimer kt("gl_stream_run", st);
-    gl_stream_run_kernel<<<count, GL_THREADS, l.smem, st>>>(p, s.hop, s.lookahead + 1, s.iters, s.preemphasis, rows, S_new, wave,
+    gl_stream_run_kernel<<<count, GL_THREADS, l.smem, st>>>(p, s.hop, s.lookahead + 1, s.iters, s.preemphasis, list, S_new, wave,
                                                             reinterpret_cast<const float2*>(base + l.twM),
                                                             reinterpret_cast<const float2*>(base + l.twN),
                                                             reinterpret_cast<const float*>(base + l.window), base + l.slots, l);
@@ -310,4 +313,4 @@ int gl_stream_run_impl(const b200tts_gl_stream_shape& s, const b200tts_gl_stream
     return B200TTS_OK;
 }
 
-}  // namespace b200tts
+}  // extern "C"

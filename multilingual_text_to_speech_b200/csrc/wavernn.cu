@@ -565,25 +565,6 @@ __global__ void wavernn_mulaw_kernel(long long n, int mu, float* __restrict__ y)
 
 }  // namespace
 
-int deemphasis_rows_impl(int rows, int len, float a, float* y, cudaStream_t st);    // vocoder.cu
-
-int wavernn_deemphasis_check(int rows, int len, int mu, float a) {
-    B200_REQUIRE(rows >= 1 && len >= 1 && mu >= 0 && (long long)rows * len < (1ll << 40), "wavernn_deemphasis: bad arguments (rows = %d, "
-                 "len = %d, mu = %d)", rows, len, mu);
-    B200_REQUIRE(a == a && a > -1.f && a < 1.f, "wavernn_deemphasis: the coefficient must lie in (-1, 1)");
-    return B200TTS_OK;
-}
-
-int wavernn_deemphasis_impl(int rows, int len, int mu, float a, float* y, cudaStream_t st) {
-    B200_TRY(wavernn_deemphasis_check(rows, len, mu, a));
-    KernelTimer kt("wavernn_deemphasis", st);
-    if (mu > 0) {
-        wavernn_mulaw_kernel<<<grid_for((size_t)rows * len), 256, 0, st>>>((long long)rows * len, mu, y);
-        B200_LAUNCH_CHECK();
-    }
-    return deemphasis_rows_impl(rows, len, a, y, st);
-}
-
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
@@ -629,29 +610,11 @@ static WrLayout wr_layout(const b200tts_wavernn_shape& s) {
     return l;
 }
 
-size_t wavernn_workspace_bytes(const b200tts_wavernn_shape& s) {
-    if (wavernn_validate(s) != B200TTS_OK) return 0;
-    return wr_layout(s).bytes;
-}
-
-int wavernn_check(const b200tts_wavernn_shape& s, void* ws, size_t ws_bytes) {
+static int wavernn_check(const b200tts_wavernn_shape& s, const void* ws, size_t ws_bytes) {
     B200_TRY(wavernn_validate(s));
     const WrLayout l = wr_layout(s);
     B200_REQUIRE(ws && ws_bytes >= l.bytes, "wavernn: workspace of %zu bytes is smaller than the %zu required", ws_bytes, l.bytes);
     B200_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "wavernn: workspace must be 256-byte aligned");
-    return B200TTS_OK;
-}
-
-int wavernn_prepare_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, void* ws, size_t ws_bytes, cudaStream_t st) {
-    B200_TRY(wavernn_check(s, ws, ws_bytes));
-    B200_REQUIRE(p.w_hh1 && p.w_ih2x && p.w_hh2 && p.w_fc1x && p.w_fc2x && p.w_fc3, "wavernn_prepare: null weight");
-    const WrLayout l = wr_layout(s);
-    const WrDims d = wr_dims(s.rnn_dims, s.fc_dims, s.n_out);
-    unsigned char* base = static_cast<unsigned char*>(ws);
-    B200_CUDA(cudaMemsetAsync(base + l.h1, 0, l.bytes - l.h1, st));    // zero state, zero previous sample, barrier and abort flag
-    WrWeights W{{p.w_hh1, p.w_ih2x, p.w_hh2, p.w_fc1x, p.w_fc2x, p.w_fc3}};
-    wavernn_pack_kernel<<<grid_for((size_t)WR_CTAS * d.per_cta), 256, 0, st>>>(d, W, reinterpret_cast<uint4*>(base + l.packed));
-    B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }
 
@@ -692,68 +655,16 @@ static int wavernn_launch(const b200tts_wavernn_shape& s, const b200tts_wavernn_
     return launch_persistent("wavernn_loop", fn, WR_CTAS, WR_THREADS, (size_t)a.d.per_cta * 16, false, params, st);
 }
 
-int wavernn_run_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, const b200tts_wavernn_cond& cond, int t0, int nsteps,
-                     const float* uniforms, float* out, float* dbg, void* ws, size_t ws_bytes, cudaStream_t st) {
-    B200_TRY(wavernn_check(s, ws, ws_bytes));
-    B200_REQUIRE(t0 >= 0 && nsteps >= 1 && t0 + nsteps <= s.fold_len, "wavernn_run: steps [%d, %d) outside the fold length %d", t0, t0 + nsteps,
-                 s.fold_len);
-    return wavernn_launch(s, p, cond, t0, 0, s.fold_len, nsteps, uniforms, out, dbg, ws, st);
-}
-
-int wavernn_run_stream_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, const b200tts_wavernn_cond& cond, long long t,
-                            int nsteps, const float* uniforms, float* out, void* ws, size_t ws_bytes, cudaStream_t st) {
-    B200_TRY(wavernn_check(s, ws, ws_bytes));
-    B200_REQUIRE(t >= 0 && nsteps >= 1 && nsteps <= s.fold_len, "wavernn_run_stream: %d steps after %lld (at most fold_len = %d per call)",
-                 nsteps, t, s.fold_len);
-    // the loop only needs the step's parity (which slot of the double-buffered h1 / h2 rows is the previous step's)
-    const int t0 = (int)(t & 1);
-    return wavernn_launch(s, p, cond, t0, t0, nsteps, nsteps, uniforms, out, nullptr, ws, st);
-}
-
-int wavernn_run_rows_check(const b200tts_wavernn_shape& s, int active_rows, int nsteps) {
+static int wavernn_run_rows_check(const b200tts_wavernn_shape& s, int active_rows, int nsteps) {
     B200_REQUIRE(active_rows >= 1 && active_rows <= s.rows && nsteps >= 1 && nsteps <= s.fold_len,
                  "wavernn_run_rows: %d active rows of %d, %d steps (at most fold_len = %d per call)", active_rows, s.rows, nsteps, s.fold_len);
     return B200TTS_OK;
 }
 
-int wavernn_run_rows_impl(const b200tts_wavernn_shape& s, const b200tts_wavernn_params& p, const b200tts_wavernn_cond& cond, const long long* row_t,
-                          const int* row_n, int active_rows, int nsteps, const float* uniforms, float* out, void* ws, size_t ws_bytes,
-                          cudaStream_t st) {
-    B200_TRY(wavernn_check(s, ws, ws_bytes));
-    B200_TRY(wavernn_run_rows_check(s, active_rows, nsteps));
-    B200_REQUIRE(row_t && row_n, "wavernn_run_rows: null row_t or row_n");
-    return wavernn_launch(s, p, cond, 0, 0, nsteps, nsteps, uniforms, out, nullptr, ws, st, row_t, row_n, active_rows);
-}
-
-int wavernn_reset_rows_check(const b200tts_wavernn_shape& s, const int* rows, int count) {
+static int wavernn_reset_rows_check(const b200tts_wavernn_shape& s, const int* rows, int count) {
     B200_REQUIRE(rows && count >= 1 && count <= s.rows, "wavernn_reset_rows: %d rows of a loop of %d", count, s.rows);
     for (int k = 0; k < count; ++k)
         B200_REQUIRE(rows[k] >= 0 && rows[k] < s.rows, "wavernn_reset_rows: row %d outside [0, %d)", rows[k], s.rows);
-    return B200TTS_OK;
-}
-
-int wavernn_reset_rows_impl(const b200tts_wavernn_shape& s, void* ws, size_t ws_bytes, const int* rows, int count, cudaStream_t st) {
-    B200_TRY(wavernn_check(s, ws, ws_bytes));
-    B200_TRY(wavernn_reset_rows_check(s, rows, count));
-    const WrLayout l = wr_layout(s);
-    unsigned char* base = static_cast<unsigned char*>(ws);
-    for (int k0 = 0; k0 < count; k0 += B200TTS_WAVERNN_MAX_STREAMS) {
-        WrRowList list;
-        list.n = count - k0 < B200TTS_WAVERNN_MAX_STREAMS ? count - k0 : B200TTS_WAVERNN_MAX_STREAMS;
-        for (int k = 0; k < list.n; ++k) list.row[k] = rows[k0 + k];
-        wavernn_reset_rows_kernel<<<grid_for((size_t)list.n * s.rnn_dims), 256, 0, st>>>(
-            list, s.rows, s.rnn_dims, reinterpret_cast<float*>(base + l.h1), reinterpret_cast<float*>(base + l.h2),
-            reinterpret_cast<float*>(base + l.prev), reinterpret_cast<__nv_bfloat16*>(base + l.h1b), reinterpret_cast<__nv_bfloat16*>(base + l.h2b));
-        B200_LAUNCH_CHECK();
-    }
-    return B200TTS_OK;
-}
-
-int wavernn_aborted_impl(const b200tts_wavernn_shape& s, const void* ws, size_t ws_bytes, int* aborted, cudaStream_t st) {
-    B200_TRY(wavernn_check(s, const_cast<void*>(ws), ws_bytes));
-    const WrLayout l = wr_layout(s);
-    B200_CUDA(cudaMemcpyAsync(aborted, static_cast<const unsigned char*>(ws) + l.bar + 128, sizeof(int), cudaMemcpyDeviceToHost, st));
-    B200_CUDA(cudaStreamSynchronize(st));
     return B200TTS_OK;
 }
 
@@ -763,15 +674,7 @@ int wavernn_upsample_layer_check(int C, int len, int scale) {
     return B200TTS_OK;
 }
 
-int wavernn_upsample_layer_impl(int C, int len, int scale, const float* fir, const float* in, float* out, cudaStream_t st) {
-    B200_TRY(wavernn_upsample_layer_check(C, len, scale));
-    KernelTimer kt("wavernn_upsample", st);
-    wavernn_upsample_layer_kernel<<<grid_for((size_t)C * len * scale), 256, 0, st>>>(C, len, scale, fir, in, out);
-    B200_LAUNCH_CHECK();
-    return B200TTS_OK;
-}
-
-int wavernn_upsample_segments_check(int C, int nseg, const int* lens, int scale) {
+static int wavernn_upsample_segments_check(int C, int nseg, const int* lens, int scale) {
     B200_REQUIRE(lens && nseg >= 1 && nseg <= B200TTS_WAVERNN_MAX_STREAMS, "wavernn_upsample_segments: %d segments (1 to %d)", nseg,
                  B200TTS_WAVERNN_MAX_STREAMS);
     long long total = 0;
@@ -783,18 +686,7 @@ int wavernn_upsample_segments_check(int C, int nseg, const int* lens, int scale)
     return B200TTS_OK;
 }
 
-int wavernn_upsample_segments_impl(int C, int nseg, const int* lens, int scale, const float* fir, const float* in, float* out, cudaStream_t st) {
-    B200_TRY(wavernn_upsample_segments_check(C, nseg, lens, scale));
-    WrSegments g;
-    g.n = nseg; g.C = C; g.in_off[0] = 0;
-    for (int k = 0; k < nseg; ++k) { g.len[k] = lens[k]; g.in_off[k + 1] = g.in_off[k] + (long long)C * lens[k]; }
-    KernelTimer kt("wavernn_upsample", st);
-    wavernn_upsample_segments_kernel<<<grid_for((size_t)g.in_off[nseg] * scale), 256, 0, st>>>(g, scale, fir, in, out);
-    B200_LAUNCH_CHECK();
-    return B200TTS_OK;
-}
-
-int wavernn_fold_check(const b200tts_wavernn_fold_shape& s, int t0, int nsteps) {
+static int wavernn_fold_check(const b200tts_wavernn_fold_shape& s, int t0, int nsteps) {
     B200_REQUIRE(s.B >= 1 && s.rows >= s.B && s.n_mels >= 1 && s.aux_dims >= 0 && s.max_frames >= 1,
                  "wavernn_fold: bad dimensions (B = %d, rows = %d, n_mels = %d, aux_dims = %d, max_frames = %d)", s.B, s.rows, s.n_mels,
                  s.aux_dims, s.max_frames);
@@ -806,18 +698,8 @@ int wavernn_fold_check(const b200tts_wavernn_fold_shape& s, int t0, int nsteps) 
     return B200TTS_OK;
 }
 
-int wavernn_fold_impl(const b200tts_wavernn_fold_shape& s, const float* mel_up, const long long* mel_off, const int* frames, const int* row_utt,
-                      const int* row_fold, const float* fir, const float* aux, int t0, int nsteps, float* feat, cudaStream_t st) {
-    B200_TRY(wavernn_fold_check(s, t0, nsteps));
-    KernelTimer kt("wavernn_fold", st);
-    wavernn_fold_kernel<<<grid_for((size_t)nsteps * s.rows * (s.n_mels + s.aux_dims)), 256, 0, st>>>(s, mel_up, mel_off, frames, row_utt, row_fold,
-                                                                                                    fir, aux, t0, nsteps, feat);
-    B200_LAUNCH_CHECK();
-    return B200TTS_OK;
-}
-
 // every read of the positions [s0, s0 + nsteps) must fall inside the windows
-int wavernn_window_check(const b200tts_wavernn_window_shape& s, long long s0, int nsteps) {
+static int wavernn_window_check(const b200tts_wavernn_window_shape& s, long long s0, int nsteps) {
     B200_REQUIRE(s.n_mels >= 1 && s.aux_dims >= 0 && s.frames >= 0 && s.mel_len >= 1 && s.aux_len >= 0 && s.m0 >= 0 && s.a0 >= 0,
                  "wavernn_window_rows: bad dimensions (n_mels = %d, aux_dims = %d, frames = %d, mel_len = %d, aux_len = %d, m0 = %lld, a0 = %d)",
                  s.n_mels, s.aux_dims, s.frames, s.mel_len, s.aux_len, s.m0, s.a0);
@@ -841,7 +723,7 @@ int wavernn_window_check(const b200tts_wavernn_window_shape& s, long long s0, in
 }
 
 // every row: wavernn_window_check of its own window, and the shared columns and factors of row 0
-int wavernn_window_rows_check(const b200tts_wavernn_window_row* rows, int active_rows, int nsteps) {
+static int wavernn_window_rows_check(const b200tts_wavernn_window_row* rows, int active_rows, int nsteps) {
     B200_REQUIRE(rows && active_rows >= 1 && active_rows <= B200TTS_WAVERNN_MAX_STREAMS && nsteps >= 1,
                  "wavernn_window_rows: %d rows (1 to %d), %d steps", active_rows, B200TTS_WAVERNN_MAX_STREAMS, nsteps);
     const b200tts_wavernn_window_shape& w0 = rows[0].w;
@@ -856,41 +738,14 @@ int wavernn_window_rows_check(const b200tts_wavernn_window_row* rows, int active
     return B200TTS_OK;
 }
 
-int wavernn_window_rows_impl(const b200tts_wavernn_window_row* rows, int active_rows, int nsteps, const float* mel, const float* fir,
-                             const float* aux, float* feat, cudaStream_t st) {
-    B200_TRY(wavernn_window_rows_check(rows, active_rows, nsteps));
-    const b200tts_wavernn_window_shape& w0 = rows[0].w;
-    WrWinRows w;
-    for (int r = 0; r < active_rows; ++r) {
-        const b200tts_wavernn_window_row& d = rows[r];
-        w.r[r] = WrWinRow{d.s0, d.w.m0, d.w.frames > 0 ? (long long)(d.w.frames + 2 * d.w.pad) * d.w.hop : LLONG_MAX, d.mel_off, d.aux_off, d.n,
-                          d.w.frames, d.w.mel_len, d.w.a0};
-    }
-    KernelTimer kt("wavernn_window_rows", st);
-    wavernn_window_rows_kernel<<<grid_for((size_t)nsteps * active_rows * (w0.n_mels + w0.aux_dims)), 256, 0, st>>>(
-        w0.n_mels, w0.aux_dims, w0.hop, w0.pad, w0.scale, active_rows, w, mel, fir, aux, nsteps, feat);
-    B200_LAUNCH_CHECK();
-    return B200TTS_OK;
-}
-
-int wavernn_unfold_check(int B, int hop, int target, int overlap, int mu) {
+static int wavernn_unfold_check(int B, int hop, int target, int overlap, int mu) {
     B200_REQUIRE(B >= 1 && hop >= 1 && target >= 1 && overlap >= 0 && mu >= 0, "wavernn_unfold: bad arguments (B = %d, hop = %d, target = %d, "
                  "overlap = %d, mu = %d)", B, hop, target, overlap, mu);
     return B200TTS_OK;
 }
 
-int wavernn_unfold_impl(int B, int hop, int target, int overlap, int mu, const int* frames, const int* row_off, const long long* wave_off,
-                        long long total, const float* y, float* wave, cudaStream_t st) {
-    B200_TRY(wavernn_unfold_check(B, hop, target, overlap, mu));
-    if (total <= 0) return B200TTS_OK;
-    KernelTimer kt("wavernn_unfold", st);
-    wavernn_unfold_kernel<<<grid_for((size_t)total), 256, 0, st>>>(B, hop, target, overlap, mu, frames, row_off, wave_off, y, wave, total);
-    B200_LAUNCH_CHECK();
-    return B200TTS_OK;
-}
-
 // every stream: a non-empty range, packed right after the previous one, whose covering folds all have entries inside [0, nsrc)
-int wavernn_unfold_streams_check(int nstreams, int hop, int target, int overlap, int mu, const b200tts_wavernn_unfold_stream* streams,
+static int wavernn_unfold_streams_check(int nstreams, int hop, int target, int overlap, int mu, const b200tts_wavernn_unfold_stream* streams,
                                  int nsrc, long long total) {
     B200_TRY(wavernn_unfold_check(1, hop, target, overlap, mu));
     B200_REQUIRE(streams && nstreams >= 1 && nstreams <= B200TTS_WAVERNN_MAX_STREAMS && nsrc >= 1,
@@ -914,17 +769,213 @@ int wavernn_unfold_streams_check(int nstreams, int hop, int target, int overlap,
     return B200TTS_OK;
 }
 
-int wavernn_unfold_streams_impl(int nstreams, int hop, int target, int overlap, int mu, const b200tts_wavernn_unfold_stream* streams,
-                                const long long* base, const int* period, int nsrc, long long total, const float* y, float* wave,
-                                cudaStream_t st) {
-    B200_TRY(wavernn_unfold_streams_check(nstreams, hop, target, overlap, mu, streams, nsrc, total));
-    WrUnfoldStreams g;
-    g.n = nstreams;
-    for (int b = 0; b < nstreams; ++b) g.s[b] = streams[b];
-    KernelTimer kt("wavernn_unfold", st);
-    wavernn_unfold_streams_kernel<<<grid_for((size_t)total), 256, 0, st>>>(g, hop, target, overlap, mu, base, period, y, wave, total);
+}  // namespace b200tts
+using namespace b200tts;
+
+extern "C" {
+
+int b200tts_wavernn_deemphasis(int rows, int len, int mu, float a, float* y, void* stream) {
+    B200_REQUIRE(y, "wavernn_deemphasis: null argument");
+    B200_REQUIRE(rows >= 1 && len >= 1 && mu >= 0 && (long long)rows * len < (1ll << 40), "wavernn_deemphasis: bad arguments (rows = %d, "
+                 "len = %d, mu = %d)", rows, len, mu);
+    B200_REQUIRE(a == a && a > -1.f && a < 1.f, "wavernn_deemphasis: the coefficient must lie in (-1, 1)");
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
+    KernelTimer kt("wavernn_deemphasis", st);
+    if (mu > 0) {
+        wavernn_mulaw_kernel<<<grid_for((size_t)rows * len), 256, 0, st>>>((long long)rows * len, mu, y);
+        B200_LAUNCH_CHECK();
+    }
+    return deemphasis_rows(rows, len, a, y, st);
+}
+
+size_t b200tts_wavernn_workspace_bytes(const b200tts_wavernn_shape* shape) {
+    if (!shape) { set_last_error("wavernn_workspace_bytes: null shape"); return 0; }
+    if (wavernn_validate(*shape) != B200TTS_OK) return 0;
+    return wr_layout(*shape).bytes;
+}
+
+int b200tts_wavernn_prepare(const b200tts_wavernn_shape* shape, const b200tts_wavernn_params* params, void* workspace, size_t workspace_bytes,
+                            void* stream) {
+    B200_REQUIRE(shape && params, "wavernn_prepare: null argument");
+    const b200tts_wavernn_shape& s = *shape;
+    const b200tts_wavernn_params& p = *params;
+    B200_TRY(wavernn_check(s, workspace, workspace_bytes));
+    B200_TRY(require_device());
+    B200_REQUIRE(p.w_hh1 && p.w_ih2x && p.w_hh2 && p.w_fc1x && p.w_fc2x && p.w_fc3, "wavernn_prepare: null weight");
+    cudaStream_t st = (cudaStream_t)stream;
+    const WrLayout l = wr_layout(s);
+    const WrDims d = wr_dims(s.rnn_dims, s.fc_dims, s.n_out);
+    unsigned char* base = static_cast<unsigned char*>(workspace);
+    B200_CUDA(cudaMemsetAsync(base + l.h1, 0, l.bytes - l.h1, st));    // zero state, zero previous sample, barrier and abort flag
+    WrWeights W{{p.w_hh1, p.w_ih2x, p.w_hh2, p.w_fc1x, p.w_fc2x, p.w_fc3}};
+    wavernn_pack_kernel<<<grid_for((size_t)WR_CTAS * d.per_cta), 256, 0, st>>>(d, W, reinterpret_cast<uint4*>(base + l.packed));
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }
 
-}  // namespace b200tts
+int b200tts_wavernn_run(const b200tts_wavernn_shape* shape, const b200tts_wavernn_params* params, const b200tts_wavernn_cond* cond, int t0,
+                        int nsteps, const float* uniforms, float* out, float* dbg, void* workspace, size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(shape && params && cond, "wavernn_run: null argument");
+    const b200tts_wavernn_shape& s = *shape;
+    B200_TRY(wavernn_check(s, workspace, workspace_bytes));
+    B200_TRY(require_device());
+    B200_REQUIRE(t0 >= 0 && nsteps >= 1 && t0 + nsteps <= s.fold_len, "wavernn_run: steps [%d, %d) outside the fold length %d", t0, t0 + nsteps,
+                 s.fold_len);
+    return wavernn_launch(s, *params, *cond, t0, 0, s.fold_len, nsteps, uniforms, out, dbg, workspace, (cudaStream_t)stream);
+}
+
+int b200tts_wavernn_run_stream(const b200tts_wavernn_shape* shape, const b200tts_wavernn_params* params, const b200tts_wavernn_cond* cond,
+                               long long t, int nsteps, const float* uniforms, float* out, void* workspace, size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(shape && params && cond, "wavernn_run_stream: null argument");
+    const b200tts_wavernn_shape& s = *shape;
+    B200_TRY(wavernn_check(s, workspace, workspace_bytes));
+    B200_TRY(require_device());
+    B200_REQUIRE(t >= 0 && nsteps >= 1 && nsteps <= s.fold_len, "wavernn_run_stream: %d steps after %lld (at most fold_len = %d per call)",
+                 nsteps, t, s.fold_len);
+    // the loop only needs the step's parity (which slot of the double-buffered h1 / h2 rows is the previous step's)
+    const int t0 = (int)(t & 1);
+    return wavernn_launch(s, *params, *cond, t0, t0, nsteps, nsteps, uniforms, out, nullptr, workspace, (cudaStream_t)stream);
+}
+
+int b200tts_wavernn_run_rows(const b200tts_wavernn_shape* shape, const b200tts_wavernn_params* params, const b200tts_wavernn_cond* cond,
+                             const int64_t* row_t, const int32_t* row_n, int active_rows, int nsteps, const float* uniforms, float* out,
+                             void* workspace, size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(shape && params && cond, "wavernn_run_rows: null argument");
+    B200_REQUIRE(row_t && row_n && uniforms && out, "wavernn_run_rows: null row_t, row_n, uniforms or output");
+    const b200tts_wavernn_shape& s = *shape;
+    B200_TRY(wavernn_check(s, workspace, workspace_bytes));
+    B200_TRY(wavernn_run_rows_check(s, active_rows, nsteps));
+    B200_TRY(require_device());
+    return wavernn_launch(s, *params, *cond, 0, 0, nsteps, nsteps, uniforms, out, nullptr, workspace, (cudaStream_t)stream,
+                          reinterpret_cast<const long long*>(row_t), row_n, active_rows);
+}
+
+int b200tts_wavernn_reset_rows(const b200tts_wavernn_shape* shape, void* workspace, size_t workspace_bytes, const int32_t* rows, int count,
+                               void* stream) {
+    B200_REQUIRE(shape, "wavernn_reset_rows: null argument");
+    const b200tts_wavernn_shape& s = *shape;
+    B200_TRY(wavernn_check(s, workspace, workspace_bytes));
+    B200_TRY(wavernn_reset_rows_check(s, rows, count));
+    B200_TRY(require_device());
+    const WrLayout l = wr_layout(s);
+    unsigned char* base = static_cast<unsigned char*>(workspace);
+    for (int k0 = 0; k0 < count; k0 += B200TTS_WAVERNN_MAX_STREAMS) {
+        WrRowList list;
+        list.n = count - k0 < B200TTS_WAVERNN_MAX_STREAMS ? count - k0 : B200TTS_WAVERNN_MAX_STREAMS;
+        for (int k = 0; k < list.n; ++k) list.row[k] = rows[k0 + k];
+        wavernn_reset_rows_kernel<<<grid_for((size_t)list.n * s.rnn_dims), 256, 0, (cudaStream_t)stream>>>(
+            list, s.rows, s.rnn_dims, reinterpret_cast<float*>(base + l.h1), reinterpret_cast<float*>(base + l.h2),
+            reinterpret_cast<float*>(base + l.prev), reinterpret_cast<__nv_bfloat16*>(base + l.h1b), reinterpret_cast<__nv_bfloat16*>(base + l.h2b));
+        B200_LAUNCH_CHECK();
+    }
+    return B200TTS_OK;
+}
+
+int b200tts_wavernn_window_rows(const b200tts_wavernn_window_row* rows, int active_rows, int nsteps, const float* mel, const float* fir,
+                                const float* aux, float* feat, void* stream) {
+    B200_REQUIRE(mel && fir && feat, "wavernn_window_rows: null argument");
+    B200_TRY(wavernn_window_rows_check(rows, active_rows, nsteps));
+    B200_REQUIRE(aux || rows[0].w.aux_dims == 0, "wavernn_window_rows: null aux");
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
+    const b200tts_wavernn_window_shape& w0 = rows[0].w;
+    WrWinRows w;
+    for (int r = 0; r < active_rows; ++r) {
+        const b200tts_wavernn_window_row& d = rows[r];
+        w.r[r] = WrWinRow{d.s0, d.w.m0, d.w.frames > 0 ? (long long)(d.w.frames + 2 * d.w.pad) * d.w.hop : LLONG_MAX, d.mel_off, d.aux_off, d.n,
+                          d.w.frames, d.w.mel_len, d.w.a0};
+    }
+    KernelTimer kt("wavernn_window_rows", st);
+    wavernn_window_rows_kernel<<<grid_for((size_t)nsteps * active_rows * (w0.n_mels + w0.aux_dims)), 256, 0, st>>>(
+        w0.n_mels, w0.aux_dims, w0.hop, w0.pad, w0.scale, active_rows, w, mel, fir, aux, nsteps, feat);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+int b200tts_wavernn_aborted(const b200tts_wavernn_shape* shape, const void* workspace, size_t workspace_bytes, int* aborted, void* stream) {
+    B200_REQUIRE(shape && aborted, "wavernn_aborted: null argument");
+    B200_TRY(require_device());
+    const b200tts_wavernn_shape& s = *shape;
+    B200_TRY(wavernn_check(s, workspace, workspace_bytes));
+    cudaStream_t st = (cudaStream_t)stream;
+    const WrLayout l = wr_layout(s);
+    B200_CUDA(cudaMemcpyAsync(aborted, static_cast<const unsigned char*>(workspace) + l.bar + 128, sizeof(int), cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    return B200TTS_OK;
+}
+
+int b200tts_wavernn_upsample_layer(int C, int len, int scale, const float* fir, const float* in, float* out, void* stream) {
+    B200_REQUIRE(fir && in && out, "wavernn_upsample_layer: null argument");
+    B200_TRY(wavernn_upsample_layer_check(C, len, scale));
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
+    KernelTimer kt("wavernn_upsample", st);
+    wavernn_upsample_layer_kernel<<<grid_for((size_t)C * len * scale), 256, 0, st>>>(C, len, scale, fir, in, out);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+int b200tts_wavernn_upsample_segments(int C, int nseg, const int32_t* lens, int scale, const float* fir, const float* in, float* out,
+                                      void* stream) {
+    B200_REQUIRE(fir && in && out, "wavernn_upsample_segments: null argument");
+    B200_TRY(wavernn_upsample_segments_check(C, nseg, lens, scale));
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
+    WrSegments g;
+    g.n = nseg; g.C = C; g.in_off[0] = 0;
+    for (int k = 0; k < nseg; ++k) { g.len[k] = lens[k]; g.in_off[k + 1] = g.in_off[k] + (long long)C * lens[k]; }
+    KernelTimer kt("wavernn_upsample", st);
+    wavernn_upsample_segments_kernel<<<grid_for((size_t)g.in_off[nseg] * scale), 256, 0, st>>>(g, scale, fir, in, out);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+int b200tts_wavernn_fold(const b200tts_wavernn_fold_shape* shape, const float* mel_up, const int64_t* mel_off, const int32_t* frames,
+                         const int32_t* row_utt, const int32_t* row_fold, const float* fir, const float* aux, int t0, int nsteps, float* feat,
+                         void* stream) {
+    B200_REQUIRE(shape && mel_up && mel_off && frames && row_utt && row_fold && fir && feat, "wavernn_fold: null argument");
+    B200_REQUIRE(aux || shape->aux_dims == 0, "wavernn_fold: null aux");
+    const b200tts_wavernn_fold_shape& s = *shape;
+    B200_TRY(wavernn_fold_check(s, t0, nsteps));
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
+    KernelTimer kt("wavernn_fold", st);
+    wavernn_fold_kernel<<<grid_for((size_t)nsteps * s.rows * (s.n_mels + s.aux_dims)), 256, 0, st>>>(
+        s, mel_up, reinterpret_cast<const long long*>(mel_off), frames, row_utt, row_fold, fir, aux, t0, nsteps, feat);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+int b200tts_wavernn_unfold(int B, int hop, int target, int overlap, int mu, const int32_t* frames, const int32_t* row_off, const int64_t* wave_off,
+                           long long total, const float* y, float* wave, void* stream) {
+    B200_REQUIRE(frames && row_off && wave_off && y && wave, "wavernn_unfold: null argument");
+    B200_TRY(wavernn_unfold_check(B, hop, target, overlap, mu));
+    B200_TRY(require_device());
+    if (total <= 0) return B200TTS_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    KernelTimer kt("wavernn_unfold", st);
+    wavernn_unfold_kernel<<<grid_for((size_t)total), 256, 0, st>>>(B, hop, target, overlap, mu, frames, row_off,
+                                                                   reinterpret_cast<const long long*>(wave_off), y, wave, total);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+int b200tts_wavernn_unfold_streams(int nstreams, int hop, int target, int overlap, int mu, const b200tts_wavernn_unfold_stream* streams,
+                                   const int64_t* base, const int32_t* period, int nsrc, long long total, const float* y, float* wave,
+                                   void* stream) {
+    B200_REQUIRE(base && period && y && wave, "wavernn_unfold_streams: null argument");
+    B200_TRY(wavernn_unfold_streams_check(nstreams, hop, target, overlap, mu, streams, nsrc, total));
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
+    WrUnfoldStreams g;
+    g.n = nstreams;
+    for (int b = 0; b < nstreams; ++b) g.s[b] = streams[b];
+    KernelTimer kt("wavernn_unfold", st);
+    wavernn_unfold_streams_kernel<<<grid_for((size_t)total), 256, 0, st>>>(g, hop, target, overlap, mu, reinterpret_cast<const long long*>(base),
+                                                                           period, y, wave, total);
+    B200_LAUNCH_CHECK();
+    return B200TTS_OK;
+}
+
+}  // extern "C"

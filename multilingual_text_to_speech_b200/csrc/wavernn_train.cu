@@ -378,20 +378,9 @@ static int gru_seq_validate(const b200tts_gru_seq_shape& s) {
     return B200TTS_OK;
 }
 
-size_t gru_seq_saved_bytes(const b200tts_gru_seq_shape& s) {
-    if (gru_seq_validate(s) != B200TTS_OK) return 0;
-    return (size_t)s.B * s.T * 4 * s.R * sizeof(float);
-}
-
-// workspace: barrier counter (+ abort flag at +128), then the reverse loop's carry [B, R]
-size_t gru_seq_workspace_bytes(const b200tts_gru_seq_shape& s) {
-    if (gru_seq_validate(s) != B200TTS_OK) return 0;
-    return 256 + align_up_sz((size_t)s.B * s.R * sizeof(float), 256);
-}
-
-int gru_seq_check(const b200tts_gru_seq_shape& s, void* ws, size_t ws_bytes) {
+static int gru_seq_check(const b200tts_gru_seq_shape& s, const void* ws, size_t ws_bytes) {
     B200_TRY(gru_seq_validate(s));
-    const size_t need = gru_seq_workspace_bytes(s);
+    const size_t need = b200tts_gru_seq_workspace_bytes(&s);
     B200_REQUIRE(ws && ws_bytes >= need, "gru_seq: workspace of %zu bytes is smaller than the %zu required", ws_bytes, need);
     B200_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "gru_seq: workspace must be 256-byte aligned");
     return B200TTS_OK;
@@ -415,16 +404,39 @@ static const void* gru_seq_pick(int U, F pick) {
     }
 }
 
-int gru_seq_forward_impl(const b200tts_gru_seq_shape& s, const float* gi, const float* w_hh, const float* b_hh, float* h, void* saved, void* ws,
-                         size_t ws_bytes, cudaStream_t st) {
-    B200_TRY(gru_seq_check(s, ws, ws_bytes));
-    B200_REQUIRE(gi && w_hh && b_hh && h && saved, "gru_seq_forward: null argument");
+}  // namespace b200tts
+using namespace b200tts;
+
+extern "C" {
+
+size_t b200tts_gru_seq_saved_bytes(const b200tts_gru_seq_shape* shape) {
+    if (!shape) { set_last_error("gru_seq_saved_bytes: null shape"); return 0; }
+    const b200tts_gru_seq_shape& s = *shape;
+    if (gru_seq_validate(s) != B200TTS_OK) return 0;
+    return (size_t)s.B * s.T * 4 * s.R * sizeof(float);
+}
+
+// workspace: barrier counter (+ abort flag at +128), then the reverse loop's carry [B, R]
+size_t b200tts_gru_seq_workspace_bytes(const b200tts_gru_seq_shape* shape) {
+    if (!shape) { set_last_error("gru_seq_workspace_bytes: null shape"); return 0; }
+    const b200tts_gru_seq_shape& s = *shape;
+    if (gru_seq_validate(s) != B200TTS_OK) return 0;
+    return 256 + align_up_sz((size_t)s.B * s.R * sizeof(float), 256);
+}
+
+int b200tts_gru_seq_forward(const b200tts_gru_seq_shape* shape, const float* gi, const float* w_hh, const float* b_hh, float* h, void* saved,
+                            void* workspace, size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(shape && gi && w_hh && b_hh && h && saved, "gru_seq_forward: null argument");
+    const b200tts_gru_seq_shape& s = *shape;
+    B200_TRY(gru_seq_check(s, workspace, workspace_bytes));
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
     const int U = s.R / GS_CTAS;
     GruSeqArgs a{};
     a.B = s.B; a.T = s.T;
     a.G = gru_seq_group(s.B, (size_t)3 * U * s.R, s.R, 3 * U);
     a.gi = gi; a.w_hh = w_hh; a.b_hh = b_hh; a.h = h; a.saved = static_cast<float*>(saved);
-    unsigned char* base = static_cast<unsigned char*>(ws);
+    unsigned char* base = static_cast<unsigned char*>(workspace);
     a.bar = reinterpret_cast<unsigned*>(base);
     a.abort_flag = reinterpret_cast<int*>(base + 128);
     a.carry = reinterpret_cast<float*>(base + 256);
@@ -435,17 +447,20 @@ int gru_seq_forward_impl(const b200tts_gru_seq_shape& s, const float* gi, const 
     return launch_persistent("gru_seq_fwd", fn, GS_CTAS, GS_THREADS, smem, false, params, st);
 }
 
-int gru_seq_backward_impl(const b200tts_gru_seq_shape& s, const float* w_hh, const float* h, const void* saved, const float* dh_ext, float* dgi,
-                          float* dgh, float* dh_dbg, void* ws, size_t ws_bytes, cudaStream_t st) {
-    B200_TRY(gru_seq_check(s, ws, ws_bytes));
-    B200_REQUIRE(w_hh && h && saved && dh_ext && dgi && dgh, "gru_seq_backward: null argument");
+int b200tts_gru_seq_backward(const b200tts_gru_seq_shape* shape, const float* w_hh, const float* h, const void* saved, const float* dh_ext,
+                             float* dgi, float* dgh, float* dh_dbg, void* workspace, size_t workspace_bytes, void* stream) {
+    B200_REQUIRE(shape && w_hh && h && saved && dh_ext && dgi && dgh, "gru_seq_backward: null argument");
+    const b200tts_gru_seq_shape& s = *shape;
+    B200_TRY(gru_seq_check(s, workspace, workspace_bytes));
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
     const int U = s.R / GS_CTAS;
     GruSeqArgs a{};
     a.B = s.B; a.T = s.T;
     a.G = gru_seq_group(s.B, (size_t)3 * U * s.R, 3 * s.R, U);
     a.w_hh = w_hh; a.h = const_cast<float*>(h); a.saved = static_cast<float*>(const_cast<void*>(saved));
     a.dh_ext = dh_ext; a.dgi = dgi; a.dgh = dgh; a.dh_dbg = dh_dbg;
-    unsigned char* base = static_cast<unsigned char*>(ws);
+    unsigned char* base = static_cast<unsigned char*>(workspace);
     a.bar = reinterpret_cast<unsigned*>(base);
     a.abort_flag = reinterpret_cast<int*>(base + 128);
     a.carry = reinterpret_cast<float*>(base + 256);
@@ -456,39 +471,45 @@ int gru_seq_backward_impl(const b200tts_gru_seq_shape& s, const float* w_hh, con
     return launch_persistent("gru_seq_bwd", fn, GS_CTAS, GS_THREADS, smem, false, params, st);
 }
 
-int gru_seq_aborted_impl(const b200tts_gru_seq_shape& s, const void* ws, size_t ws_bytes, int* aborted, cudaStream_t st) {
-    B200_TRY(gru_seq_check(s, const_cast<void*>(ws), ws_bytes));
-    B200_CUDA(cudaMemcpyAsync(aborted, static_cast<const unsigned char*>(ws) + 128, sizeof(int), cudaMemcpyDeviceToHost, st));
+int b200tts_gru_seq_aborted(const b200tts_gru_seq_shape* shape, const void* workspace, size_t workspace_bytes, int* aborted, void* stream) {
+    B200_REQUIRE(shape && aborted, "gru_seq_aborted: null argument");
+    B200_TRY(require_device());
+    B200_TRY(gru_seq_check(*shape, workspace, workspace_bytes));
+    cudaStream_t st = (cudaStream_t)stream;
+    B200_CUDA(cudaMemcpyAsync(aborted, static_cast<const unsigned char*>(workspace) + 128, sizeof(int), cudaMemcpyDeviceToHost, st));
     B200_CUDA(cudaStreamSynchronize(st));
     return B200TTS_OK;
 }
 
-int gru_seq_abort_flag_copy_impl(const b200tts_gru_seq_shape& s, const void* ws, size_t ws_bytes, int* dst, cudaStream_t st) {
-    B200_TRY(gru_seq_check(s, const_cast<void*>(ws), ws_bytes));
-    B200_CUDA(cudaMemcpyAsync(dst, static_cast<const unsigned char*>(ws) + 128, sizeof(int), cudaMemcpyDefault, st));
+int b200tts_gru_seq_abort_flag_copy(const b200tts_gru_seq_shape* shape, const void* workspace, size_t workspace_bytes, int* dst, void* stream) {
+    B200_REQUIRE(shape && dst, "gru_seq_abort_flag_copy: null argument");
+    B200_TRY(gru_seq_check(*shape, workspace, workspace_bytes));
+    B200_TRY(require_device());
+    B200_CUDA(cudaMemcpyAsync(dst, static_cast<const unsigned char*>(workspace) + 128, sizeof(int), cudaMemcpyDefault, (cudaStream_t)stream));
     return B200TTS_OK;
 }
 
-int wavernn_upsample_layer_check(int C, int len, int scale);      // wavernn.cu
-
-size_t wavernn_upsample_layer_backward_workspace_bytes(int C, int len, int scale) {
+size_t b200tts_wavernn_upsample_layer_backward_workspace_bytes(int C, int len, int scale) {
     if (wavernn_upsample_layer_check(C, len, scale) != B200TTS_OK) return 0;
     return (size_t)(2 * scale + 1) * UPS_CHUNKS * sizeof(float);
 }
 
-int wavernn_upsample_layer_backward_impl(int C, int len, int scale, const float* fir, const float* in, const float* dout, float* din, float* dfir,
-                                         void* ws, size_t ws_bytes, cudaStream_t st) {
-    B200_TRY(wavernn_upsample_layer_check(C, len, scale));
+int b200tts_wavernn_upsample_layer_backward(int C, int len, int scale, const float* fir, const float* in, const float* dout, float* din,
+                                            float* dfir, void* workspace, size_t workspace_bytes, void* stream) {
     B200_REQUIRE(fir && dout && (din || dfir), "wavernn_upsample_layer_backward: null argument");
+    B200_TRY(wavernn_upsample_layer_check(C, len, scale));
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
     KernelTimer kt("wavernn_upsample_bwd", st);
     if (din) {
         wavernn_upsample_bwd_in_kernel<<<grid_for((size_t)C * len), 256, 0, st>>>(C, len, scale, fir, dout, din);
         B200_LAUNCH_CHECK();
     }
     if (dfir) {
-        const size_t need = wavernn_upsample_layer_backward_workspace_bytes(C, len, scale);
-        B200_REQUIRE(in && ws && ws_bytes >= need, "wavernn_upsample_layer_backward: d fir needs the layer input and %zu workspace bytes", need);
-        float* part = static_cast<float*>(ws);
+        const size_t need = b200tts_wavernn_upsample_layer_backward_workspace_bytes(C, len, scale);
+        B200_REQUIRE(in && workspace && workspace_bytes >= need, "wavernn_upsample_layer_backward: d fir needs the layer input and %zu workspace bytes",
+                     need);
+        float* part = static_cast<float*>(workspace);
         wavernn_upsample_bwd_fir_part_kernel<<<dim3(2 * scale + 1, UPS_CHUNKS), 256, 0, st>>>(C, len, scale, in, dout, part);
         B200_LAUNCH_CHECK();
         wavernn_upsample_bwd_fir_sum_kernel<<<1, 64, 0, st>>>(2 * scale + 1, part, dfir);
@@ -497,43 +518,26 @@ int wavernn_upsample_layer_backward_impl(int C, int len, int scale, const float*
     return B200TTS_OK;
 }
 
-int wavernn_stretch_backward_check(int B, int F, int C, int hop) {
+int b200tts_wavernn_stretch_backward(int B, int F, int C, int hop, const float* dup, float* daux, void* stream) {
+    B200_REQUIRE(dup && daux, "wavernn_stretch_backward: null argument");
     B200_REQUIRE(B >= 1 && F >= 1 && C >= 1 && hop >= 1 && (long long)B * F * hop * C < (1ll << 40),
                  "wavernn_stretch_backward: bad dimensions (B = %d, frames = %d, C = %d, hop = %d)", B, F, C, hop);
-    return B200TTS_OK;
-}
-
-int wavernn_stretch_backward_impl(int B, int F, int C, int hop, const float* dup, float* daux, cudaStream_t st) {
-    B200_TRY(wavernn_stretch_backward_check(B, F, C, hop));
-    wavernn_stretch_bwd_kernel<<<grid_for((size_t)B * F * C), 256, 0, st>>>(B, F, C, hop, dup, daux);
+    B200_TRY(require_device());
+    wavernn_stretch_bwd_kernel<<<grid_for((size_t)B * F * C), 256, 0, (cudaStream_t)stream>>>(B, F, C, hop, dup, daux);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }
 
-int wavernn_loss_check(int mode, long long N, int n_out) {
-    B200_REQUIRE(N >= 1 && N < (1ll << 40), "wavernn_loss: %lld rows", N);
-    if (mode == B200TTS_WAVERNN_RAW) {
-        B200_REQUIRE(n_out >= 2 && n_out <= 65536, "wavernn_loss: RAW needs 2 to 65536 classes (n_out = %d)", n_out);
-    } else {
-        B200_REQUIRE(mode == B200TTS_WAVERNN_MOL, "wavernn_loss: unknown mode %d", mode);
-        B200_REQUIRE(n_out % 3 == 0 && n_out >= 3 && n_out <= 96, "wavernn_loss: MOL needs 3 x (1..32) outputs (n_out = %d)", n_out);
-    }
-    return B200TTS_OK;
-}
+size_t b200tts_column_sum_workspace_bytes(int cols) { return cols >= 1 ? (size_t)COLSUM_CHUNKS * cols * sizeof(float) : 0; }
 
-size_t column_sum_workspace_bytes(int cols) { return cols >= 1 ? (size_t)COLSUM_CHUNKS * cols * sizeof(float) : 0; }
-
-int column_sum_check(long long rows, int cols) {
-    B200_REQUIRE(rows >= 1 && cols >= 1 && rows * cols < (1ll << 40), "column_sum: bad dimensions (rows = %lld, cols = %d)", rows, cols);
-    return B200TTS_OK;
-}
-
-int column_sum_impl(long long rows, int cols, const float* x, float* out, void* ws, size_t ws_bytes, cudaStream_t st) {
-    B200_TRY(column_sum_check(rows, cols));
+int b200tts_column_sum(long long rows, int cols, const float* x, float* out, void* workspace, size_t workspace_bytes, void* stream) {
     B200_REQUIRE(x && out, "column_sum: null argument");
-    B200_REQUIRE(ws && ws_bytes >= column_sum_workspace_bytes(cols), "column_sum: workspace of %zu bytes is smaller than the %zu required",
-                 ws_bytes, column_sum_workspace_bytes(cols));
-    float* part = static_cast<float*>(ws);
+    B200_REQUIRE(rows >= 1 && cols >= 1 && rows * cols < (1ll << 40), "column_sum: bad dimensions (rows = %lld, cols = %d)", rows, cols);
+    B200_TRY(require_device());
+    const size_t need = b200tts_column_sum_workspace_bytes(cols);
+    B200_REQUIRE(workspace && workspace_bytes >= need, "column_sum: workspace of %zu bytes is smaller than the %zu required", workspace_bytes, need);
+    cudaStream_t st = (cudaStream_t)stream;
+    float* part = static_cast<float*>(workspace);
     column_sum_part_kernel<<<dim3((cols + 255) / 256, COLSUM_CHUNKS), 256, 0, st>>>(rows, cols, x, part);
     B200_LAUNCH_CHECK();
     column_sum_add_kernel<<<(cols + 255) / 256, 256, 0, st>>>(cols, part, out);
@@ -541,16 +545,24 @@ int column_sum_impl(long long rows, int cols, const float* x, float* out, void* 
     return B200TTS_OK;
 }
 
-size_t wavernn_loss_workspace_bytes(long long N) { return N >= 1 ? (size_t)N * sizeof(float) : 0; }
+size_t b200tts_wavernn_loss_workspace_bytes(long long N) { return N >= 1 ? (size_t)N * sizeof(float) : 0; }
 
-int wavernn_loss_impl(int mode, long long N, int n_out, const float* logits, const void* target, float* loss, float* dlogits, void* ws,
-                      size_t ws_bytes, cudaStream_t st) {
-    B200_TRY(wavernn_loss_check(mode, N, n_out));
+int b200tts_wavernn_loss(int mode, long long N, int n_out, const float* logits, const void* target, float* loss, float* dlogits, void* workspace,
+                         size_t workspace_bytes, void* stream) {
     B200_REQUIRE(logits && target && loss && dlogits, "wavernn_loss: null argument");
-    B200_REQUIRE(ws && ws_bytes >= wavernn_loss_workspace_bytes(N), "wavernn_loss: workspace of %zu bytes is smaller than the %zu required",
-                 ws_bytes, wavernn_loss_workspace_bytes(N));
+    B200_REQUIRE(N >= 1 && N < (1ll << 40), "wavernn_loss: %lld rows", N);
+    if (mode == B200TTS_WAVERNN_RAW) {
+        B200_REQUIRE(n_out >= 2 && n_out <= 65536, "wavernn_loss: RAW needs 2 to 65536 classes (n_out = %d)", n_out);
+    } else {
+        B200_REQUIRE(mode == B200TTS_WAVERNN_MOL, "wavernn_loss: unknown mode %d", mode);
+        B200_REQUIRE(n_out % 3 == 0 && n_out >= 3 && n_out <= 96, "wavernn_loss: MOL needs 3 x (1..32) outputs (n_out = %d)", n_out);
+    }
+    B200_TRY(require_device());
+    const size_t need = b200tts_wavernn_loss_workspace_bytes(N);
+    B200_REQUIRE(workspace && workspace_bytes >= need, "wavernn_loss: workspace of %zu bytes is smaller than the %zu required", workspace_bytes, need);
+    cudaStream_t st = (cudaStream_t)stream;
     KernelTimer kt("wavernn_loss", st);
-    float* rows = static_cast<float*>(ws);
+    float* rows = static_cast<float*>(workspace);
     const int blocks = (int)((N + 7) / 8 > NUM_SMS * 16 ? NUM_SMS * 16 : (N + 7) / 8);
     if (mode == B200TTS_WAVERNN_RAW)
         wavernn_loss_raw_kernel<<<blocks, 256, 0, st>>>(N, n_out, logits, static_cast<const int*>(target), rows, dlogits);
@@ -562,4 +574,4 @@ int wavernn_loss_impl(int mode, long long N, int n_out, const float* logits, con
     return B200TTS_OK;
 }
 
-}  // namespace b200tts
+}  // extern "C"

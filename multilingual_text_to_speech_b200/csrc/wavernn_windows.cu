@@ -55,7 +55,13 @@ __global__ void __launch_bounds__(CUT_THREADS) wavernn_cut_windows_kernel(int mo
 
 }  // namespace
 
-int wavernn_cut_windows_check(int mode, int bits, int B, int feat, int seq_len, int pad, int hop, long long total_frames) {
+}  // namespace b200tts
+using namespace b200tts;
+
+extern "C" int b200tts_wavernn_cut_windows(int mode, int bits, int B, int feat, int seq_len, int pad, int hop, const float* mels,
+                                           long long total_frames, const int64_t* frame_start, const uint16_t* labels,
+                                           const int64_t* sample_start, const int32_t* table, float* x, void* y, float* m, void* stream) {
+    B200_REQUIRE(mels && frame_start && labels && sample_start && table && x && y && m, "wavernn_cut_windows: null argument");
     B200_REQUIRE(mode == B200TTS_WAVERNN_RAW || mode == B200TTS_WAVERNN_MOL, "wavernn_cut_windows: unknown mode %d", mode);
     B200_REQUIRE(bits >= 1 && bits <= 16, "wavernn_cut_windows: bits %d outside [1, 16]", bits);
     B200_REQUIRE(B >= 1 && B <= CUT_MAX_B, "wavernn_cut_windows: batch %d outside [1, %d]", B, CUT_MAX_B);
@@ -64,13 +70,8 @@ int wavernn_cut_windows_check(int mode, int bits, int B, int feat, int seq_len, 
     B200_REQUIRE(pad >= 0 && pad <= 64, "wavernn_cut_windows: pad %d outside [0, 64]", pad);
     B200_REQUIRE(feat >= 1 && feat <= 1024, "wavernn_cut_windows: %d mel channels outside [1, 1024]", feat);
     B200_REQUIRE(total_frames >= 1, "wavernn_cut_windows: %lld packed frames", total_frames);
-    return B200TTS_OK;
-}
-
-int wavernn_cut_windows_impl(int mode, int bits, int B, int feat, int seq_len, int pad, int hop, const float* mels, long long total_frames,
-                             const long long* frame_start, const unsigned short* labels, const long long* sample_start, const int* table,
-                             float* x, void* y, float* m, cudaStream_t st) {
-    B200_TRY(wavernn_cut_windows_check(mode, bits, B, feat, seq_len, pad, hop, total_frames));
+    B200_TRY(require_device());
+    cudaStream_t st = (cudaStream_t)stream;
     const int mol = mode == B200TTS_WAVERNN_MOL;
     const float x_den = (float)((1 << (mol ? 16 : bits)) - 1);
     const int win = seq_len / hop + 2 * pad;
@@ -78,10 +79,9 @@ int wavernn_cut_windows_impl(int mode, int bits, int B, int feat, int seq_len, i
     int ctas = cdiv(per_row, CUT_THREADS);
     if (ctas > CUT_MAX_CTAS_PER_ROW) ctas = CUT_MAX_CTAS_PER_ROW;
     KernelTimer kt("wavernn_cut_windows", st);
-    wavernn_cut_windows_kernel<<<dim3(ctas, B), CUT_THREADS, 0, st>>>(mol, x_den, feat, win, seq_len, pad, hop, mels, total_frames, frame_start,
-                                                                     labels, sample_start, table, x, y, m);
+    wavernn_cut_windows_kernel<<<dim3(ctas, B), CUT_THREADS, 0, st>>>(mol, x_den, feat, win, seq_len, pad, hop, mels, total_frames,
+                                                                     reinterpret_cast<const long long*>(frame_start), labels,
+                                                                     reinterpret_cast<const long long*>(sample_start), table, x, y, m);
     B200_LAUNCH_CHECK();
     return B200TTS_OK;
 }
-
-}  // namespace b200tts

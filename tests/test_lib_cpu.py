@@ -19,6 +19,24 @@ def lib():
     return _lib.load()
 
 
+# C scalar types of the header -> the ctypes type SIGNATURES must use (ctypes aliases size_t / uint64_t and long long / int64_t on LP64)
+_C_SCALARS = {'int': ctypes.c_int, 'float': ctypes.c_float, 'double': ctypes.c_double, 'size_t': ctypes.c_size_t,
+              'long long': ctypes.c_longlong, 'int64_t': ctypes.c_int64, 'uint64_t': ctypes.c_uint64,
+              'unsigned long long': ctypes.c_ulonglong}
+
+
+def _is_pointer(t):
+    return t in (ctypes.c_void_p, ctypes.c_char_p) or issubclass(t, ctypes._Pointer)
+
+
+def _c_type(decl, named):
+    """ctypes type of one C declaration ('const float* x', 'size_t'), or 'ptr' for any pointer."""
+    if '*' in decl:
+        return 'ptr'
+    words = decl.replace('const ', '').split()
+    return _C_SCALARS[' '.join(words[:-1] if named else words)]
+
+
 def test_header_symbols_exported(lib):
     header = open(os.path.join(ROOT, 'include', 'b200tts.h')).read()
     declared = set(re.findall(r'\b(b200tts_[a-z0-9_]+)\s*\(', header))
@@ -26,6 +44,20 @@ def test_header_symbols_exported(lib):
     for name in sorted(declared):
         assert hasattr(lib, name), f'{name} declared in include/b200tts.h but not exported'
     assert declared == set(_lib.SIGNATURES), declared ^ set(_lib.SIGNATURES)
+
+    # every prototype's return type, argument count and argument types agree with SIGNATURES (any pointer stands for any pointer)
+    code = re.sub(r'//[^\n]*', '', re.sub(r'/\*.*?\*/', '', header, flags=re.S))
+    protos = re.findall(r'([A-Za-z_][\w \t*]*?)\s*\b(b200tts_\w+)\s*\(([^)]*)\)\s*;', code)
+    assert {name for _, name, _ in protos} == declared
+    for ret, name, args in protos:
+        restype, argtypes = _lib.SIGNATURES[name]
+        want = _c_type(ret, named=False)
+        assert (want == 'ptr' and _is_pointer(restype)) or restype is want, f'{name}: returns {ret.strip()}, SIGNATURES has {restype}'
+        params = [] if args.strip() in ('', 'void') else [p.strip() for p in args.split(',')]
+        assert len(params) == len(argtypes), f'{name}: {len(params)} arguments in the header, {len(argtypes)} in SIGNATURES'
+        for i, (p, t) in enumerate(zip(params, argtypes)):
+            want = _c_type(p, named=True)
+            assert (want == 'ptr' and _is_pointer(t)) or t is want, f'{name}: argument {i} is `{p}`, SIGNATURES has {t}'
 
 
 def test_workspace_queries_are_host_only(lib):
