@@ -653,6 +653,57 @@ int b200tts_monotonic_alignment(const b200tts_align_shape* shape, const float* P
 int b200tts_alignment_scores(const b200tts_align_shape* shape, const float* P, const int32_t* text_lengths, const int32_t* step_lengths,
                              float* focus_out, float* coverage_out, int32_t* max_jump_out, int32_t* moves_back_out, void* stream);
 
+/* ---- pitch analysis: probabilistic YIN F0 tracks (librosa 0.10 librosa.pyin; no counterpart in the reference) ----
+ * Packed ragged layout as the analysis entry points: utterance b owns samples [soff[b], soff[b+1]) of an fp32 waveform (L_b >= 1) and
+ * frames [off[b], off[b+1]) with F_b = 1 + L_b / hop (soff, off: int32 [B+1], device).  Frame t of utterance b is the frame_length samples
+ * y[0 .. frame_length) starting at sample t hop - frame_length / 2, zero outside [0, L_b) (center=True, constant padding, no
+ * pre-emphasis).  The host computes every derived quantity below once, with numpy, and passes it in the shape.  No utterance reads another's
+ * data, sums run in a fixed order and nothing uses atomics: every result is bit-reproducible and independent of the batch it is computed in.
+ * fp64 whatever b200tts_set_precision says. */
+#define B200TTS_PITCH_THRESHOLDS 100
+/* The Viterbi keeps two fp64 rows of 2 n states plus prefix and suffix maxima of both halves in shared memory, and uint16 back-pointers. */
+#define B200TTS_PITCH_MAX_BINS 1201
+#define B200TTS_PITCH_MAX_FRAME_LENGTH 2048
+typedef struct {
+    int B, total_samples, total_frames;
+    int frame_length, win_length, hop; /* even frame_length <= B200TTS_PITCH_MAX_FRAME_LENGTH, win_length = frame_length / 2, hop >= 1 */
+    int min_period, max_period;        /* floor(sr / fmax), min(ceil(sr / fmin), frame_length - win_length - 1); K = max - min + 1 >= 2 */
+    int n_bins;                        /* n = floor(120 log2(fmax / fmin)) + 1 pitch bins, 1 <= n <= B200TTS_PITCH_MAX_BINS */
+    int transition_width;              /* W = round(35.92 * 12 hop / sr) * 10 + 1, odd, 1 <= W <= n */
+    double sr, fmin;
+    double log_tiny;                   /* log(DBL_MIN): an out-of-band transition and a zero observation */
+    double log_init;                   /* log(1 / n + DBL_MIN): the start probability of each unvoiced state */
+    double thresholds[B200TTS_PITCH_THRESHOLDS];   /* linspace(0, 1, 101)[1:] */
+    double beta_probs[B200TTS_PITCH_THRESHOLDS];   /* diff(scipy.stats.beta.cdf(linspace(0, 1, 101), 2, 18)) */
+} b200tts_pitch_shape;
+/* Host only: the bytes of b200tts_pitch_viterbi's back-pointers (uint16 [total_frames, 2 n]); 0 for an invalid shape (message set). */
+size_t b200tts_pitch_workspace_bytes(const b200tts_pitch_shape* shape);
+/* Stage A, the cumulative mean normalised difference per frame, in fp64 from the fp32 samples (direct sums in index order):
+ *   acf(tau) = sum_{i=1}^{win} y_i y_{i+tau},  e(tau) = sum_{i=tau+1}^{tau+win} y_i^2, each set to 0 where its magnitude is below 1e-6;
+ *   d(tau) = (e(0) + e(tau)) - 2 acf(tau);  d'(tau) = d(tau) / (c(tau) / tau + DBL_MIN), c(tau) = d(1) + ... + d(tau) summed in order.
+ * cmnd_out: double [total_frames, K], entry k = d'(min_period + k). */
+int b200tts_pitch_cmnd(const b200tts_pitch_shape* shape, const float* wave, const int32_t* soff, const int32_t* off, double* cmnd_out,
+                       void* stream);
+/* Stage B, pYIN observation probabilities from d' [total_frames, K].  Troughs: k = 0 iff d'[0] < d'[1]; 0 < k < K - 1 iff d'[k] < d'[k-1]
+ * and d'[k] <= d'[k+1]; k = K - 1 iff d'[K-1] < d'[K-2].  For threshold j with N_j troughs below thresholds[j], a trough below it at
+ * position p among them gets prior (1 - e^-2) / (1 - e^(-2 N_j)) e^(-2 p) (Boltzmann, lambda 2); its probability is sum_j prior_j
+ * beta_probs[j].  The first lowest trough also gets 0.01 sum beta_probs[j] over the thresholds it is not below.  A trough with nonzero
+ * probability maps to bin rint(120 log2(sr / (min_period + k + s) / fmin)) clipped to [0, n] (half to even), with the parabolic shift
+ * s = -b / a (a = d'[k+1] + d'[k-1] - 2 d'[k], b = (d'[k+1] - d'[k-1]) / 2; s = 0 when |b| >= |a| and at both ends).  Of troughs sharing a
+ * bin the larger lag wins; bin n is dropped.  obs_out: double [total_frames, n], zero elsewhere; voiced_prob_out: double [total_frames],
+ * clip(sum of obs_out's row, 0, 1). */
+int b200tts_pitch_observations(const b200tts_pitch_shape* shape, const double* cmnd, double* obs_out, double* voiced_prob_out, void* stream);
+/* Stage C, librosa.sequence.viterbi over 2 n states (voiced bins, then unvoiced bins), one CTA per utterance.  Log observations:
+ * log(obs + DBL_MIN) for voiced state i, log((1 - voiced_prob) / n + DBL_MIN) for every unvoiced state.  Start: log_tiny on the voiced
+ * states, log_init on the unvoiced ones.  log_trans: double [2, W, n] (device), log_trans[s, q, i] = log(S_s T[i - h + q, i] + DBL_MIN)
+ * for the source bin i - h + q in [0, n) (h = W / 2; other entries unread), T the row-normalised triangular band of librosa's
+ * transition_local(n, W, 'triangle', wrap=False), S_0 = 1 - 0.01 (same voicing) and S_1 = 1 - S_0 (switch).  Every transition outside the
+ * band costs log_tiny, as in the dense kron(transition_loop(2, 1 - 0.01), T).  Ties go to the lowest source state, and the final state is the
+ * first best.  state_out: int32 [total_frames], the decoded state (bin i voiced when < n, bin state - n unvoiced).  workspace: at least
+ * b200tts_pitch_workspace_bytes. */
+int b200tts_pitch_viterbi(const b200tts_pitch_shape* shape, const double* obs, const double* voiced_prob, const int32_t* off,
+                          const double* log_trans, int32_t* state_out, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- WaveRNN vocoder (fatchord architecture): mel -> waveform, one GRU step per sample over fold rows ----
  * The MelResNet and the time-batched conditioning products run on the convolution-block and GEMM entry points; these entry points add
  * the mel upsampling layers, the folding, the persistent sample loop and the unfolding.  Fold rows: utterance b's F_b hop sample

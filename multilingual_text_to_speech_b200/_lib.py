@@ -162,6 +162,18 @@ class AlignShape(Structure):
 ALIGN_MAX_SYMBOLS = 1024
 ALIGN_MAX_CELLS = 1728512
 
+# include/b200tts.h: B200TTS_PITCH_THRESHOLDS, B200TTS_PITCH_MAX_BINS and B200TTS_PITCH_MAX_FRAME_LENGTH
+PITCH_THRESHOLDS = 100
+PITCH_MAX_BINS = 1201
+PITCH_MAX_FRAME_LENGTH = 2048
+
+
+class PitchShape(Structure):
+    _fields_ = [(n, c_int) for n in ('B', 'total_samples', 'total_frames', 'frame_length', 'win_length', 'hop', 'min_period', 'max_period',
+                                     'n_bins', 'transition_width')] + \
+               [(n, c_double) for n in ('sr', 'fmin', 'log_tiny', 'log_init')] + \
+               [('thresholds', c_double * PITCH_THRESHOLDS), ('beta_probs', c_double * PITCH_THRESHOLDS)]
+
 
 # name -> (restype, argtypes); the "-m not gpu" suite checks every symbol of the header resolves
 SIGNATURES = {
@@ -256,6 +268,10 @@ SIGNATURES = {
     'b200tts_mel_cepstral_distortion': (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'b200tts_monotonic_alignment': (c_int, [POINTER(AlignShape)] + [c_void_p] * 7),
     'b200tts_alignment_scores': (c_int, [POINTER(AlignShape)] + [c_void_p] * 8),
+    'b200tts_pitch_workspace_bytes': (c_size_t, [POINTER(PitchShape)]),
+    'b200tts_pitch_cmnd': (c_int, [POINTER(PitchShape)] + [c_void_p] * 5),
+    'b200tts_pitch_observations': (c_int, [POINTER(PitchShape)] + [c_void_p] * 4),
+    'b200tts_pitch_viterbi': (c_int, [POINTER(PitchShape)] + [c_void_p] * 6 + [c_size_t, c_void_p]),
     'b200tts_wavernn_upsample_layer': (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     'b200tts_wavernn_fold': (c_int, [POINTER(WaveRNNFoldShape)] + [c_void_p] * 7 + [c_int, c_int, c_void_p, c_void_p]),
     'b200tts_wavernn_workspace_bytes': (c_size_t, [POINTER(WaveRNNShape)]),

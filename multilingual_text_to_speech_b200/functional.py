@@ -1033,6 +1033,83 @@ def mel_cepstral_distortion(cep_a, off_a, cep_b, off_b, mode):
 
 
 # ------------------------------------------------------------------------------------------------
+# pitch analysis (probabilistic YIN in three stages, include/b200tts.h; the same packed ragged layout)
+# ------------------------------------------------------------------------------------------------
+def pitch_cmnd(shape, wave, soff, off):
+    """wave fp32 [total_samples] -> the cumulative mean normalised difference d' float64 [total_frames, K] (a _lib.PitchShape)."""
+    _require_cuda(wave, soff, off)
+    assert soff.dtype == torch.int32 and off.dtype == torch.int32 and wave.dtype == torch.float32 and wave.is_contiguous()
+    out = torch.empty(shape.total_frames, shape.max_period - shape.min_period + 1, device=wave.device, dtype=torch.float64)
+    check(_lib.load().b200tts_pitch_cmnd(ctypes.byref(shape), ptr(wave), ptr(soff), ptr(off), ptr(out), _stream()), 'b200tts_pitch_cmnd')
+    return out
+
+
+def pitch_observations(shape, cmnd):
+    """d' [total_frames, K] -> (voiced-bin probabilities float64 [total_frames, n_bins], voiced_prob float64 [total_frames])."""
+    _require_cuda(cmnd)
+    assert cmnd.dtype == torch.float64 and cmnd.is_contiguous() and tuple(cmnd.shape) == (shape.total_frames,
+                                                                                          shape.max_period - shape.min_period + 1)
+    obs = torch.empty(shape.total_frames, shape.n_bins, device=cmnd.device, dtype=torch.float64)
+    voiced_prob = torch.empty(shape.total_frames, device=cmnd.device, dtype=torch.float64)
+    check(_lib.load().b200tts_pitch_observations(ctypes.byref(shape), ptr(cmnd), ptr(obs), ptr(voiced_prob), _stream()),
+          'b200tts_pitch_observations')
+    return obs, voiced_prob
+
+
+def pitch_viterbi(shape, obs, voiced_prob, off, log_trans):
+    """Viterbi decode of each utterance -> state int32 [total_frames] (voiced bin i when < n_bins, else unvoiced bin state - n_bins).
+    log_trans: float64 [2, W, n_bins] (include/b200tts.h)."""
+    _require_cuda(obs, voiced_prob, off, log_trans)
+    assert obs.dtype == torch.float64 and voiced_prob.dtype == torch.float64 and log_trans.dtype == torch.float64 and off.dtype == torch.int32
+    assert tuple(log_trans.shape) == (2, shape.transition_width, shape.n_bins) and log_trans.is_contiguous()
+    n = _lib.load().b200tts_pitch_workspace_bytes(ctypes.byref(shape))
+    if n == 0:
+        raise _lib.B200TTSError(f'b200tts_pitch_workspace_bytes: {_lib.load().b200tts_last_error().decode()}')
+    ws = _bytes(n, obs.device)
+    state = torch.empty(shape.total_frames, device=obs.device, dtype=torch.int32)
+    check(_lib.load().b200tts_pitch_viterbi(ctypes.byref(shape), ptr(obs), ptr(voiced_prob), ptr(off), ptr(log_trans), ptr(state), ptr(ws),
+                                            ws.numel(), _stream()), 'b200tts_pitch_viterbi')
+    return state
+
+
+def symbol_average(track, durations, voiced=None):
+    """Per-symbol means of a frame track [B, T] over each symbol's frames: symbol l of row b owns frames [C_{l-1}, C_l), C the cumulative
+    sum of durations [B, L] (frames past C_{L-1} belong to no symbol).  Summed in frame order in float64; with `voiced` [B, T] (bool) only
+    voiced frames count, as FastPitch averages pitch.  A symbol with no counted frames gets 0.  -> float64 [B, L] on track's device.
+    Raises ValueError on wrong shapes, negative durations or durations summing past T."""
+    if not torch.is_tensor(track) or track.dim() != 2 or not track.dtype.is_floating_point:
+        raise ValueError(f'track must be a floating [B, T] tensor, got {tuple(track.shape) if torch.is_tensor(track) else type(track)}')
+    if not torch.is_tensor(durations) or durations.dim() != 2 or durations.dtype.is_floating_point or durations.dtype == torch.bool:
+        raise ValueError('durations must be an integer [B, L] tensor')
+    B, T = track.shape
+    if durations.shape[0] != B:
+        raise ValueError(f'durations has {durations.shape[0]} rows for {B} tracks')
+    d = durations.detach().cpu().long()
+    if bool((d < 0).any()):
+        raise ValueError('durations must be non-negative')
+    ends = d.cumsum(1)
+    if ends.shape[1] and int(ends[:, -1].max()) > T:
+        raise ValueError(f'durations sum to {int(ends[:, -1].max())} frames; the track has {T}')
+    x = track.detach().cpu().double()
+    w = torch.ones(B, T, dtype=torch.float64)
+    if voiced is not None:
+        if not torch.is_tensor(voiced) or tuple(voiced.shape) != (B, T) or voiced.dtype != torch.bool:
+            raise ValueError(f'voiced must be a bool [{B}, {T}] tensor')
+        w = voiced.detach().cpu().double()
+        x = torch.where(voiced.cpu(), x, torch.zeros_like(x))
+    L = d.shape[1]
+    # symbol of every frame (L for frames past the last symbol): one CPU index_add per row sums the frames of each symbol in frame order
+    owner = torch.searchsorted(ends, torch.arange(T).expand(B, T).contiguous(), right=True)
+    sums = torch.zeros(B, L + 1, dtype=torch.float64)
+    counts = torch.zeros(B, L + 1, dtype=torch.float64)
+    for b in range(B):
+        sums[b].index_add_(0, owner[b], x[b])
+        counts[b].index_add_(0, owner[b], w[b])
+    mean = torch.where(counts > 0, sums / counts.clamp(min=1), torch.zeros_like(sums))[:, :L]
+    return mean.to(track.device)
+
+
+# ------------------------------------------------------------------------------------------------
 # forced alignment (monotonic alignment search over attention probabilities, include/b200tts.h)
 # ------------------------------------------------------------------------------------------------
 def _host_lengths(x, B, what):

@@ -324,3 +324,200 @@ def mel_cepstral_distorision(S1, S2, mode):
                 'dtw' to compute DTW with minimal possible MCD (exact DTW, not fastdtw's approximation)
     """
     return float(mel_cepstral_distortion_batch([S1], [S2], mode)[0])
+
+
+# pYIN parameters of librosa 0.10's librosa.pyin that are fixed here
+PITCH_N_THRESHOLDS = 100
+PITCH_BETA = (2, 18)
+PITCH_BINS_PER_SEMITONE = 10                 # resolution 0.1 semitone
+PITCH_MAX_TRANSITION_RATE = 35.92            # octaves per second
+PITCH_SWITCH_PROB = 0.01
+
+_PITCH_CACHE = {}
+
+
+def pitch_geometry(fmin=65.406, fmax=2093.0, frame_length=1024):
+    """The derived pYIN quantities under the current hp, with librosa 0.10's numpy expressions: {sr, hop, win_length, min_period,
+    max_period, n_bins, transition_width}.  Raises ValueError for parameters librosa.pyin would refuse or the kernels do not take."""
+    sr, hop = hp.sample_rate, ms_to_frames(hp.stft_shift_ms)
+    fmin, fmax, frame_length = float(fmin), float(fmax), int(frame_length)
+    if not fmin > 0:
+        raise ValueError(f'fmin = {fmin} must be positive')
+    if not fmin < fmax:
+        raise ValueError(f'fmin = {fmin} must be below fmax = {fmax}')
+    if fmax > sr / 2:
+        raise ValueError(f'fmax = {fmax} is above the Nyquist frequency {sr / 2}')
+    if frame_length % 2 or not 4 <= frame_length <= _lib.PITCH_MAX_FRAME_LENGTH:
+        raise ValueError(f'frame_length = {frame_length} must be even and in [4, {_lib.PITCH_MAX_FRAME_LENGTH}]')
+    win = frame_length // 2
+    min_period = int(np.floor(sr / fmax))
+    max_period = min(int(np.ceil(sr / fmin)), frame_length - win - 1)
+    if max_period <= min_period:
+        raise ValueError(f'frame_length = {frame_length} leaves no lag range: max_period {max_period} <= min_period {min_period}')
+    n_bins = int(np.floor(12 * PITCH_BINS_PER_SEMITONE * np.log2(fmax / fmin))) + 1
+    width = round(PITCH_MAX_TRANSITION_RATE * 12 * hop / sr) * PITCH_BINS_PER_SEMITONE + 1
+    if n_bins > _lib.PITCH_MAX_BINS:
+        raise ValueError(f'fmin = {fmin} and fmax = {fmax} give {n_bins} pitch bins; at most {_lib.PITCH_MAX_BINS}')
+    if n_bins < width:
+        raise ValueError(f'fmin = {fmin} and fmax = {fmax} give {n_bins} pitch bins, fewer than the transition width {width}')
+    return dict(sr=sr, hop=hop, win_length=win, min_period=min_period, max_period=max_period, n_bins=n_bins, transition_width=width)
+
+
+def _pitch_log_transitions(n, width):
+    """[2, W, n] float64: log(S_s T[i - h + q, i] + tiny), T librosa's transition_local(n, W, 'triangle', wrap=False) built densely with its
+    own expressions, S_0 = 0.99 (same voicing) and S_1 = transition_loop(2, 0.99)'s off-diagonal."""
+    import scipy.signal
+    window = scipy.signal.get_window('triangle', width, fftbins=False)
+    lpad = (n - width) // 2
+    padded = np.pad(window, (lpad, n - width - lpad))
+    local = np.zeros((n, n), dtype=np.float64)
+    for i in range(n):
+        row = np.roll(padded, n // 2 + i + 1)
+        row[min(n, i + width // 2 + 1):] = 0
+        row[:max(0, i - width // 2)] = 0
+        local[i] = row
+    local /= local.sum(axis=1, keepdims=True)
+    tiny = np.finfo(np.float64).tiny
+    h, dst = width // 2, np.arange(n)
+    out = np.zeros((2, width, n), dtype=np.float64)
+    for s, p in enumerate((1 - PITCH_SWITCH_PROB, (1.0 - (1 - PITCH_SWITCH_PROB)) / 1)):
+        lt = np.log(p * local + tiny)
+        for q in range(width):
+            src = dst - h + q
+            ok = (src >= 0) & (src < n)
+            out[s, q, ok] = lt[src[ok], dst[ok]]
+    return out
+
+
+def _pitch_tables(g, fmin, device):
+    """(shape fields, log transitions on `device`, f0 of every bin on `device`), built once per geometry."""
+    key = (g['sr'], g['hop'], g['win_length'], g['n_bins'], g['transition_width'], float(fmin), str(device))
+    if key not in _PITCH_CACHE:
+        import scipy.stats
+        thresholds = np.linspace(0, 1, PITCH_N_THRESHOLDS + 1)
+        beta_probs = np.diff(scipy.stats.beta.cdf(thresholds, PITCH_BETA[0], PITCH_BETA[1]))
+        tiny = np.finfo(np.float64).tiny
+        n = g['n_bins']
+        fields = dict(log_tiny=float(np.log(tiny)), log_init=float(np.log(1 / n + tiny)), thresholds=thresholds[1:], beta_probs=beta_probs)
+        freqs = fmin * 2 ** (np.arange(n) / (12 * PITCH_BINS_PER_SEMITONE))
+        _PITCH_CACHE[key] = (fields, torch.from_numpy(_pitch_log_transitions(n, g['transition_width'])).to(device),
+                             torch.from_numpy(freqs.astype(np.float32)).to(device))
+    return _PITCH_CACHE[key]
+
+
+def pitch_shape(B, total_samples, total_frames, fmin=65.406, fmax=2093.0, frame_length=1024, device=None):
+    """(library shape, log transitions, bin frequencies) of a pitch batch; tables on `device` (the current CUDA device by default)."""
+    g = pitch_geometry(fmin, fmax, frame_length)
+    device = torch.device('cuda', torch.cuda.current_device()) if device is None else device
+    fields, log_trans, freqs = _pitch_tables(g, float(fmin), device)
+    shape = _lib.PitchShape(int(B), int(total_samples), int(total_frames), int(frame_length), g['win_length'], g['hop'], g['min_period'],
+                            g['max_period'], g['n_bins'], g['transition_width'], float(g['sr']), float(fmin), fields['log_tiny'],
+                            fields['log_init'])
+    shape.thresholds[:] = [float(v) for v in fields['thresholds']]
+    shape.beta_probs[:] = [float(v) for v in fields['beta_probs']]
+    return shape, log_trans, freqs
+
+
+def _pack_waveforms(waveforms, what):
+    """Checked waveforms -> (tensors, came as numpy, lengths, host sample offsets, host frame offsets) with F_i = 1 + L_i // hop."""
+    if not isinstance(waveforms, (list, tuple)) or len(waveforms) == 0:
+        raise ValueError(f'{what} expects a non-empty list of 1-D waveforms')
+    ins = [_as_float_tensor(w, f'waveform {i}', 1) for i, w in enumerate(waveforms)]
+    waves = [t for t, _ in ins]
+    hop = ms_to_frames(hp.stft_shift_ms)
+    lengths = [int(w.numel()) for w in waves]
+    soff_host = np.concatenate([[0], np.cumsum(lengths)]).astype(np.int64)
+    off_host = np.concatenate([[0], np.cumsum([1 + n // hop for n in lengths])]).astype(np.int64)
+    if soff_host[-1] >= 2 ** 31:
+        raise ValueError(f'{soff_host[-1]} samples in one batch; at most 2^31 - 1')
+    return waves, [is_np for _, is_np in ins], soff_host, off_host
+
+
+def pitch_batch(waveforms, fmin=65.406, fmax=2093.0, frame_length=1024):
+    """F0 tracks of waveforms [L_i] by probabilistic YIN, as librosa 0.10's librosa.pyin(y, fmin=fmin, fmax=fmax, sr=hp.sample_rate,
+    frame_length=frame_length, hop_length=hop) computes them with its other defaults (win_length = frame_length // 2, 100 thresholds,
+    beta (2, 18), Boltzmann 2, 0.1 semitone bins, 35.92 octaves/s, switch probability 0.01, no-trough probability 0.01, center=True with
+    zero padding), on the raw waveform (no pre-emphasis).  hop = ms_to_frames(hp.stft_shift_ms), so the frames are the mel frames:
+    F_i = 1 + L_i // hop.  -> one (f0, voiced_prob) per input, each [F_i] float32: f0 in Hz, NaN on unvoiced frames.  The three stages
+    run in the library's fp64 kernels (include/b200tts.h); waveforms are rounded to fp32 first.  The work runs on the device of the first
+    CUDA input, or on the current CUDA device when no input is on one.  numpy in -> numpy out; torch in -> torch out, on that device for
+    CUDA inputs and on the CPU for CPU inputs.  Raises ValueError on a bad input, fmin <= 0, fmin >= fmax, fmax above Nyquist, more than
+    B200TTS_PITCH_MAX_BINS bins or fewer than the transition width, or a frame_length that is odd, out of range or leaves no lags."""
+    waves, as_np, soff_host, off_host = _pack_waveforms(waveforms, 'pitch_batch')
+    pitch_geometry(fmin, fmax, frame_length)
+    device = _work_device(waves)
+    with torch.cuda.device(device):
+        shape, log_trans, freqs = pitch_shape(len(waves), soff_host[-1], off_host[-1], fmin, fmax, frame_length, device)
+        wave = torch.cat([w.to(device=device, dtype=torch.float32) for w in waves]).contiguous()
+        soff = torch.from_numpy(soff_host.astype(np.int32)).to(device)
+        off = torch.from_numpy(off_host.astype(np.int32)).to(device)
+        cmnd = F.pitch_cmnd(shape, wave, soff, off)
+        obs, voiced_prob = F.pitch_observations(shape, cmnd)
+        state = F.pitch_viterbi(shape, obs, voiced_prob, off, log_trans).long()
+        n = shape.n_bins
+        f0 = torch.where(state < n, freqs[state % n], torch.full_like(freqs[:1], float('nan')))
+        vp = voiced_prob.float()
+    out = []
+    for i in range(len(waves)):
+        a, b = off_host[i], off_host[i + 1]
+        out.append((_return_like(f0[a:b], as_np[i], waves[i]), _return_like(vp[a:b], as_np[i], waves[i])))
+    return out
+
+
+def pitch(y, fmin=65.406, fmax=2093.0, frame_length=1024):
+    """(f0, voiced_prob) of one waveform; see pitch_batch."""
+    return pitch_batch([y], fmin, fmax, frame_length)[0]
+
+
+def energy_batch(waveforms):
+    """Frame energies of waveforms [L_i]: the L2 norm over frequency of each frame of the linear magnitude spectrogram spectrogram_batch
+    computes before the dB scale (pre-emphasis per hp, |stft| with centre reflect padding), summed in fp64.  -> [F_i] float32 per input,
+    F_i = 1 + L_i // hop; the same device and numpy / torch rules as spectrogram_batch."""
+    waves, as_np, soff_host, off_host = _pack_waveforms(waveforms, 'energy_batch')
+    device = _work_device(waves)
+    with torch.cuda.device(device):
+        shape = analysis_shape(len(waves), soff_host[-1], off_host[-1], False)
+        wave = torch.cat([w.to(device=device, dtype=torch.float32) for w in waves]).contiguous()
+        soff = torch.from_numpy(soff_host.astype(np.int32)).to(device)
+        off = torch.from_numpy(off_host.astype(np.int32)).to(device)
+        S = F.stft_magnitude(shape, wave, soff, off)
+        e = S.double().square().sum(1).sqrt().float()
+    return [_return_like(e[off_host[i]:off_host[i + 1]], as_np[i], waves[i]) for i in range(len(waves))]
+
+
+def _f0_track(x, what):
+    t, is_np = _as_float_tensor(x, what, 1)
+    a = t.detach().cpu().double().numpy()
+    if (a[~np.isnan(a)] <= 0).any() or np.isinf(a).any():
+        raise ValueError(f'{what} must be positive Hz on voiced frames (NaN marks unvoiced ones)')
+    return a, is_np, t
+
+
+def pitch_errors_batch(f0_refs, f0_gens):
+    """F0 error metrics of each pair (reference, generated) of F0 tracks [F] in Hz, NaN on unvoiced frames (pitch_batch's f0), over the
+    first min(F_ref, F_gen) frames in float64.  Frames voiced in both are VV; a gross error is a VV frame with |f0_gen - f0_ref| >
+    0.2 f0_ref.  -> dict of float64 [B]: gpe (gross errors / VV frames), vde (frames whose voicing differs / frames), ffe ((gross errors +
+    voicing errors) / frames) and f0_rmse_cents (the RMS of 1200 log2(f0_gen / f0_ref) over VV frames); gpe and f0_rmse_cents are NaN for
+    a pair without VV frames.  numpy arrays, or torch tensors on the first reference's device when it is a torch tensor."""
+    if not isinstance(f0_refs, (list, tuple)) or not isinstance(f0_gens, (list, tuple)) or len(f0_refs) == 0:
+        raise ValueError('pitch_errors_batch expects two non-empty lists of 1-D f0 tracks')
+    if len(f0_refs) != len(f0_gens):
+        raise ValueError(f'{len(f0_refs)} reference tracks against {len(f0_gens)}')
+    refs = [_f0_track(x, f'f0_refs[{i}]') for i, x in enumerate(f0_refs)]
+    gens = [_f0_track(x, f'f0_gens[{i}]') for i, x in enumerate(f0_gens)]
+    out = {k: np.empty(len(refs)) for k in ('gpe', 'vde', 'ffe', 'f0_rmse_cents')}
+    for i, ((r, _, _), (g, _, _)) in enumerate(zip(refs, gens)):
+        m = min(len(r), len(g))
+        r, g = r[:m], g[:m]
+        vr, vg = ~np.isnan(r), ~np.isnan(g)
+        vv = vr & vg
+        nvv = int(vv.sum())
+        gross = int((np.abs(g[vv] - r[vv]) > 0.2 * r[vv]).sum())
+        voicing = int((vr != vg).sum())
+        out['gpe'][i] = gross / nvv if nvv else np.nan
+        out['vde'][i] = voicing / m
+        out['ffe'][i] = (gross + voicing) / m
+        out['f0_rmse_cents'][i] = np.sqrt(np.mean((1200 * np.log2(g[vv] / r[vv])) ** 2)) if nvv else np.nan
+    if refs[0][1]:
+        return out
+    return {k: torch.from_numpy(v).to(refs[0][2].device) for k, v in out.items()}
