@@ -704,6 +704,44 @@ int b200tts_pitch_observations(const b200tts_pitch_shape* shape, const double* c
 int b200tts_pitch_viterbi(const b200tts_pitch_shape* shape, const double* obs, const double* voiced_prob, const int32_t* off,
                           const double* log_trans, int32_t* state_out, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- pitch modification: TD-PSOLA pitch shifting (no counterpart in the reference; tests/psola_oracle.py states the contract) ----
+ * The packed ragged layout of the pitch entry points: utterance b owns samples [soff[b], soff[b+1]) of an fp32 waveform (L_b >= 1) and
+ * frames [off[b], off[b+1]) with F_b = 1 + L_b / hop.  Sample n is in frame min(F_b - 1, (n + hop / 2) / hop); per frame, f0 (fp32 Hz, NaN
+ * unvoiced) and r (fp32, new F0 / old F0).  P(n) = rint(sr / f0) in fp64 (half to even); U = unvoiced_spacing.
+ *   Analysis marks m_0 < m_1 < ... in [0, L_b): m_0 = argmax x over [0, min(L, P(0))) when sample 0 is voiced, else 0.  From a voiced mark
+ *   (p = P(m)): c = m + p, stop when c >= L; next = argmax x over [c - p/4, min(L - 1, c + p/4)] when c is voiced, else c.  From an
+ *   unvoiced mark, o = the first voiced sample after it (L if none): next = m + U when m + U < o (stop when >= L), else argmax x over
+ *   [o, min(L, o + P(o))) (stop when o = L).  argmax is over signed x, first index on ties.  d_k = m_{k+1} - m_k; the last mark's d is its
+ *   nominal period (P voiced, U unvoiced).
+ *   Synthesis marks: t_0 = m_0, t_{j+1} = t_j + q_j in fp64, c_j = rint(t_j) until c_j >= L; k(j) the analysis mark nearest c_j (lower on
+ *   ties); q_j = d_k / r[frame(c_j)] when mark k is voiced, else d_k.
+ *   Overlap-add: grain j reads x around m_{k(j)}, writes around c_j, half-widths a = d_{k-1} (grain of mark 0: max(its nominal period, m_0))
+ *   and b = d_k, weight (1 + cos(pi u / (a + 1))) / 2 for -a <= u <= 0 and (1 + cos(pi u / (b + 1))) / 2 for 0 <= u <= b, except 1 on the
+ *   left half of mark 0's grains and the right half of the last mark's.  y(n) = sum w x[m + n - c_j] / max(1, sum w) over the grains
+ *   covering n whose source index is in [0, L), both sums fp64 in increasing j; y = 0 where no grain covers n.  At r = 1, y = x.
+ * Workspace (b200tts_psola_workspace_bytes): int32 info [B, 4] = {analysis marks K_b, synthesis marks J_b, grain 0's left half-width,
+ * W_b = the largest half-width}, then int32 [total_samples] each of marks, d, centres c and k, then uint8 [total_samples] voiced flags of
+ * the marks; utterance b's entries start at soff[b] (K_b, J_b <= L_b).  No utterance reads another's data, sums run in a fixed order and
+ * nothing uses atomics: results are bit-identical in any batch.  fp64 whatever b200tts_set_precision says.  The host checks f0 and r (voiced
+ * periods in [2, B200TTS_PSOLA_MAX_PERIOD], ratios finite in [0.5, 2]); the kernels clamp both into those ranges, so no input can make a
+ * walk run away. */
+#define B200TTS_PSOLA_MAX_PERIOD 1024
+typedef struct {
+    int B, total_samples, total_frames;
+    int hop;                           /* frames of the f0 and ratio tracks: F_b = 1 + L_b / hop, hop >= 1 */
+    int unvoiced_spacing;              /* U, in [1, B200TTS_PSOLA_MAX_PERIOD] */
+    double sr;                         /* sample rate in Hz */
+} b200tts_psola_shape;
+/* Host only: the workspace bytes of a batch; 0 for an invalid shape (message set). */
+size_t b200tts_psola_workspace_bytes(const b200tts_psola_shape* shape);
+/* Analysis and synthesis marks, one warp per utterance: wave fp32 [total_samples], f0 and ratio fp32 [total_frames] -> workspace. */
+int b200tts_psola_marks(const b200tts_psola_shape* shape, const float* wave, const int32_t* soff, const float* f0, const float* ratio,
+                        const int32_t* off, void* workspace, size_t workspace_bytes, void* stream);
+/* Overlap-add from the marks b200tts_psola_marks wrote, as a gather: each output sample sums the grains whose centre lies within W_b of it.
+ * out: fp32 [total_samples], not aliasing wave. */
+int b200tts_psola_overlap_add(const b200tts_psola_shape* shape, const float* wave, const int32_t* soff, const void* workspace,
+                              size_t workspace_bytes, float* out, void* stream);
+
 /* ---- WaveRNN vocoder (fatchord architecture): mel -> waveform, one GRU step per sample over fold rows ----
  * The MelResNet and the time-batched conditioning products run on the convolution-block and GEMM entry points; these entry points add
  * the mel upsampling layers, the folding, the persistent sample loop and the unfolding.  Fold rows: utterance b's F_b hop sample

@@ -175,6 +175,14 @@ class PitchShape(Structure):
                [('thresholds', c_double * PITCH_THRESHOLDS), ('beta_probs', c_double * PITCH_THRESHOLDS)]
 
 
+# include/b200tts.h: B200TTS_PSOLA_MAX_PERIOD
+PSOLA_MAX_PERIOD = 1024
+
+
+class PsolaShape(Structure):
+    _fields_ = [(n, c_int) for n in ('B', 'total_samples', 'total_frames', 'hop', 'unvoiced_spacing')] + [('sr', c_double)]
+
+
 # name -> (restype, argtypes); the "-m not gpu" suite checks every symbol of the header resolves
 SIGNATURES = {
     'b200tts_last_error': (c_char_p, []),
@@ -272,6 +280,9 @@ SIGNATURES = {
     'b200tts_pitch_cmnd': (c_int, [POINTER(PitchShape)] + [c_void_p] * 5),
     'b200tts_pitch_observations': (c_int, [POINTER(PitchShape)] + [c_void_p] * 4),
     'b200tts_pitch_viterbi': (c_int, [POINTER(PitchShape)] + [c_void_p] * 6 + [c_size_t, c_void_p]),
+    'b200tts_psola_workspace_bytes': (c_size_t, [POINTER(PsolaShape)]),
+    'b200tts_psola_marks': (c_int, [POINTER(PsolaShape)] + [c_void_p] * 6 + [c_size_t, c_void_p]),
+    'b200tts_psola_overlap_add': (c_int, [POINTER(PsolaShape)] + [c_void_p] * 3 + [c_size_t, c_void_p, c_void_p]),
     'b200tts_wavernn_upsample_layer': (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     'b200tts_wavernn_fold': (c_int, [POINTER(WaveRNNFoldShape)] + [c_void_p] * 7 + [c_int, c_int, c_void_p, c_void_p]),
     'b200tts_wavernn_workspace_bytes': (c_size_t, [POINTER(WaveRNNShape)]),

@@ -1072,6 +1072,49 @@ def pitch_viterbi(shape, obs, voiced_prob, off, log_trans):
     return state
 
 
+# ------------------------------------------------------------------------------------------------
+# pitch modification (TD-PSOLA in two stages, include/b200tts.h; the same packed ragged layout)
+# ------------------------------------------------------------------------------------------------
+def psola_workspace(shape, device):
+    """The uint8 workspace of a pitch-shift batch (a _lib.PsolaShape) on `device`."""
+    n = _lib.load().b200tts_psola_workspace_bytes(ctypes.byref(shape))
+    if n == 0:
+        raise _lib.B200TTSError(f'b200tts_psola_workspace_bytes: {_lib.load().b200tts_last_error().decode()}')
+    return _bytes(n, device)
+
+
+def psola_marks(shape, wave, soff, f0, ratio, off, ws=None):
+    """Analysis and synthesis pitch marks of each utterance from wave fp32 [total_samples], f0 and ratio fp32 [total_frames] -> the
+    workspace (include/b200tts.h describes its layout; psola_workspace_views reads it)."""
+    _require_cuda(wave, soff, f0, ratio, off)
+    assert soff.dtype == torch.int32 and off.dtype == torch.int32 and wave.dtype == torch.float32 and wave.is_contiguous()
+    assert f0.dtype == torch.float32 and ratio.dtype == torch.float32 and f0.is_contiguous() and ratio.is_contiguous()
+    assert f0.numel() == ratio.numel() == shape.total_frames and wave.numel() == shape.total_samples
+    ws = psola_workspace(shape, wave.device) if ws is None else ws
+    check(_lib.load().b200tts_psola_marks(ctypes.byref(shape), ptr(wave), ptr(soff), ptr(f0), ptr(ratio), ptr(off), ptr(ws), ws.numel(),
+                                          _stream()), 'b200tts_psola_marks')
+    return ws
+
+
+def psola_workspace_views(shape, ws):
+    """(info int32 [B, 4], marks, spacings, centres, nearest marks int32 [total_samples], voiced uint8 [total_samples]) viewing `ws`."""
+    B, N = shape.B, shape.total_samples
+    ints = ws[:(4 * B + 4 * N) * 4].view(torch.int32)
+    info = ints[:4 * B].view(B, 4)
+    marks, spacing, centre, nearest = (ints[4 * B + i * N:4 * B + (i + 1) * N] for i in range(4))
+    return info, marks, spacing, centre, nearest, ws[(4 * B + 4 * N) * 4:(4 * B + 4 * N) * 4 + N]
+
+
+def psola_overlap_add(shape, wave, soff, ws):
+    """The grains overlap-added from the marks psola_marks wrote to `ws` -> fp32 [total_samples]."""
+    _require_cuda(wave, soff, ws)
+    assert soff.dtype == torch.int32 and wave.dtype == torch.float32 and wave.is_contiguous() and wave.numel() == shape.total_samples
+    out = torch.empty_like(wave)
+    check(_lib.load().b200tts_psola_overlap_add(ctypes.byref(shape), ptr(wave), ptr(soff), ptr(ws), ws.numel(), ptr(out), _stream()),
+          'b200tts_psola_overlap_add')
+    return out
+
+
 def symbol_average(track, durations, voiced=None):
     """Per-symbol means of a frame track [B, T] over each symbol's frames: symbol l of row b owns frames [C_{l-1}, C_l), C the cumulative
     sum of durations [B, L] (frames past C_{L-1} belong to no symbol).  Summed in frame order in float64; with `voiced` [B, T] (bool) only

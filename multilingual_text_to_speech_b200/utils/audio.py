@@ -521,3 +521,98 @@ def pitch_errors_batch(f0_refs, f0_gens):
     if refs[0][1]:
         return out
     return {k: torch.from_numpy(v).to(refs[0][2].device) for k, v in out.items()}
+
+
+def _tracks(tracks, frames, what):
+    """One fp32 [F_i] host track per waveform, checked -> list of float32 numpy arrays."""
+    if not isinstance(tracks, (list, tuple)) or len(tracks) != len(frames):
+        raise ValueError(f'{what} must be a list of {len(frames)} tracks, one per waveform')
+    out = []
+    for i, t in enumerate(tracks):
+        a = _as_float_tensor(t, f'{what}[{i}]', 1)[0].detach().cpu().numpy().astype(np.float32)
+        if len(a) != frames[i]:
+            raise ValueError(f'{what}[{i}] has {len(a)} frames; waveform {i} has {frames[i]} (1 + L // hop)')
+        out.append(a)
+    return out
+
+
+def _check_ratios(r, what):
+    if not np.isfinite(r).all() or (r < 0.5).any() or (r > 2.0).any():
+        raise ValueError(f'{what} must be finite and in [0.5, 2] (one octave each way)')
+
+
+def pitch_shift_batch(waveforms, semitones=None, ratios=None, f0s=None, fmin=65.406, fmax=2093.0):
+    """Pitch-shift waveforms [L_i] by TD-PSOLA, each keeping its length: grains two periods wide are taken at pitch marks placed on the F0
+    track and overlap-added at marks spaced by the period over the ratio, so F0 is multiplied by the ratio while the spectral envelope
+    (formants) and the duration stay.  include/b200tts.h and tests/psola_oracle.py state the rules exactly.
+    Give exactly one of `semitones` (one float, or one per waveform: ratio 2^(s / 12) on every frame) and `ratios` (one [F_i] track of new
+    F0 / old F0 per waveform).  Ratios must be finite and in [0.5, 2].  `f0s`: one F0 track [F_i] per waveform in Hz, NaN on unvoiced
+    frames, as pitch_batch returns it; by default pitch_batch(waveforms, fmin, fmax).  Voiced F0 must give periods rint(sr / f0) in
+    [2, B200TTS_PSOLA_MAX_PERIOD] samples.  Frames are the mel frames, F_i = 1 + L_i // hop, hop = ms_to_frames(hp.stft_shift_ms); unvoiced
+    regions keep marks hop samples apart and are never respaced.  Only voiced grains move, so at ratio 1, or without voiced frames, the
+    output equals the input.  Waveforms are rounded to fp32; marks and sums are fp64 in the library's kernels.  The same device and
+    numpy / torch rules as spectrogram_batch.  Raises ValueError on a bad or non-finite waveform, both or neither of semitones and ratios,
+    mismatched list or track lengths, an out-of-range ratio, or a non-positive or out-of-range F0."""
+    waves, as_np, soff_host, off_host = _pack_waveforms(waveforms, 'pitch_shift_batch')
+    B = len(waves)
+    frames = [int(off_host[i + 1] - off_host[i]) for i in range(B)]
+    for i, w in enumerate(waves):
+        if not bool(torch.isfinite(w).all()):
+            raise ValueError(f'waveform {i} has non-finite samples')
+    if (semitones is None) == (ratios is None):
+        raise ValueError('give exactly one of semitones and ratios')
+    if semitones is not None:
+        s = [semitones] * B if np.ndim(semitones) == 0 else list(semitones)
+        if len(s) != B:
+            raise ValueError(f'{len(s)} semitone values for {B} waveforms')
+        r = [np.full(f, 2.0 ** (float(v) / 12.0), dtype=np.float32) for v, f in zip(s, frames)]
+    else:
+        r = _tracks(ratios, frames, 'ratios')
+    for i, a in enumerate(r):
+        _check_ratios(a, f'the ratios of waveform {i}')
+    if f0s is None:
+        f0 = [_as_float_tensor(f, 'f0', 1)[0].detach().cpu().numpy().astype(np.float32)
+              for f, _ in pitch_batch(waveforms, fmin, fmax)]
+    else:
+        f0 = _tracks(f0s, frames, 'f0s')
+    sr, hop = hp.sample_rate, ms_to_frames(hp.stft_shift_ms)
+    for i, a in enumerate(f0):
+        v = a[~np.isnan(a)].astype(np.float64)
+        if not np.isfinite(v).all() or (v <= 0).any():
+            raise ValueError(f'f0 of waveform {i} must be positive Hz on voiced frames (NaN marks unvoiced ones)')
+        p = np.rint(sr / v)
+        if ((p < 2) | (p > _lib.PSOLA_MAX_PERIOD)).any():
+            raise ValueError(f'f0 of waveform {i} gives periods outside [2, {_lib.PSOLA_MAX_PERIOD}] samples: F0 must lie in about '
+                             f'[{sr / (_lib.PSOLA_MAX_PERIOD + 0.5):.2f}, {sr / 1.5:.1f}] Hz')
+    device = _work_device(waves)
+    with torch.cuda.device(device):
+        shape = _lib.PsolaShape(B, int(soff_host[-1]), int(off_host[-1]), hop, hop, float(sr))
+        wave = torch.cat([w.to(device=device, dtype=torch.float32) for w in waves]).contiguous()
+        soff = torch.from_numpy(soff_host.astype(np.int32)).to(device)
+        off = torch.from_numpy(off_host.astype(np.int32)).to(device)
+        f0_d = torch.from_numpy(np.concatenate(f0)).to(device)
+        r_d = torch.from_numpy(np.concatenate(r)).to(device)
+        ws = F.psola_marks(shape, wave, soff, f0_d, r_d, off)
+        y = F.psola_overlap_add(shape, wave, soff, ws)
+    return [_return_like(y[soff_host[i]:soff_host[i + 1]], as_np[i], waves[i]) for i in range(B)]
+
+
+def pitch_shift(y, semitones=None, ratios=None, f0=None, fmin=65.406, fmax=2093.0):
+    """One waveform pitch-shifted; `ratios` and `f0` are single [F] tracks here.  See pitch_shift_batch."""
+    return pitch_shift_batch([y], semitones, None if ratios is None else [ratios], None if f0 is None else [f0], fmin, fmax)[0]
+
+
+def f0_ratio(f0_target, f0_source):
+    """The per-frame ratio that moves f0_source onto f0_target (both [F] in Hz, NaN unvoiced, as pitch_batch returns them), for
+    pitch_shift_batch(..., ratios=[f0_ratio(target, source)], f0s=[source]): target / source clipped to [0.5, 2] on frames voiced in both,
+    1 elsewhere, over the first min(F_target, F_source) frames and padded with 1 to F_source.  -> float32 [F_source], numpy for a numpy
+    source, else a tensor on the source's device.  Raises ValueError on tracks that are not 1-D floating, or that hold a non-positive or
+    infinite voiced F0."""
+    t, _, _ = _f0_track(f0_target, 'f0_target')
+    s, s_np, s_t = _f0_track(f0_source, 'f0_source')
+    m = min(len(t), len(s))
+    out = np.ones(len(s))
+    vv = ~np.isnan(t[:m]) & ~np.isnan(s[:m])
+    out[:m][vv] = np.clip(t[:m][vv] / s[:m][vv], 0.5, 2.0)
+    out = out.astype(np.float32)
+    return out if s_np else torch.from_numpy(out).to(s_t.device)
