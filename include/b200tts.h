@@ -742,6 +742,37 @@ int b200tts_psola_marks(const b200tts_psola_shape* shape, const float* wave, con
 int b200tts_psola_overlap_add(const b200tts_psola_shape* shape, const float* wave, const int32_t* soff, const void* workspace,
                               size_t workspace_bytes, float* out, void* stream);
 
+/* ---- time-scale modification: WSOLA time stretching (no counterpart in the reference; tests/wsola_oracle.py states the contract) ----
+ * The packed ragged layout of the pitch entry points: utterance b owns input samples [soff[b], soff[b+1]) of an fp32 waveform x (L >= 1,
+ * read as 0 outside [0, L)), output samples [ooff[b], ooff[b+1]) (L' >= 1) and synthesis frames [foff[b], foff[b+1]), K = (L' - 1) / H + 2
+ * of them.  H = hop, N = 2H, D = tolerance.  Frame k is centred on output sample kH; warp[k] is its input position tau_k (fp64).
+ *   Nominal positions: a_k = rint(clamp(tau_k, 0, L)) (half to even; NaN reads as 0).
+ *   Search: p_0 = a_0.  For k >= 1, u_m = x[p_{k-1} + H + m] (the natural continuation of frame k - 1) and v_{d,m} = x[a_k + d + m] for m in
+ *   [-H, H) and d in [-D, D].  C(d) = sum u v and E(d) = sum v v, each an fp64 sum of the exact fp64 products of fp32 samples, accumulated
+ *   one term at a time in increasing m from 0.0 (C = fma(u, v, C)).  s(d) = C / sqrt(E), IEEE fp64, and s = 0 where E = 0.
+ *   p_k = a_k + the d of largest s; on exact ties the smallest |d| wins, then the negative d.  At tau_k = kH, d = 0 is the Cauchy-Schwarz
+ *   maximum, so y = x up to rounding; silence (every s = 0) copies the nominal positions.
+ *   Overlap-add: y[n] = sum over k in {n / H, n / H + 1} (frames the utterance has) of w(n - kH + H) x[p_k + n - kH], summed in fp64 in
+ *   increasing k and rounded to fp32, with w(i) = 0.5 - 0.5 cos(pi i / H), the periodic Hann window of length 2H.  w(i) + w(i + H) = 1,
+ *   so there is no normalisation.
+ * No workspace and no atomics; no utterance reads another's data, so results are bit-identical in any batch.  fp64 whatever
+ * b200tts_set_precision says.  total_samples <= INT_MAX - B200TTS_WSOLA_MAX_TOLERANCE, so every position fits in int32. */
+#define B200TTS_WSOLA_MAX_HOP 1024
+#define B200TTS_WSOLA_MAX_TOLERANCE 1024
+typedef struct {
+    int B, total_samples, total_out_samples, total_frames;
+    int hop;                           /* H in [1, B200TTS_WSOLA_MAX_HOP] */
+    int tolerance;                     /* D in [0, B200TTS_WSOLA_MAX_TOLERANCE] */
+} b200tts_wsola_shape;
+/* The frame positions p, one CTA per utterance walking its frames in order: wave fp32 [total_samples], warp fp64 [total_frames] ->
+ * positions int32 [total_frames]. */
+int b200tts_wsola_positions(const b200tts_wsola_shape* shape, const float* wave, const int32_t* soff, const double* warp,
+                            const int32_t* foff, int32_t* positions, void* stream);
+/* The overlap-add of the frames at the positions b200tts_wsola_positions wrote, one thread per output sample: out fp32
+ * [total_out_samples], not aliasing wave. */
+int b200tts_wsola_overlap_add(const b200tts_wsola_shape* shape, const float* wave, const int32_t* soff, const int32_t* positions,
+                              const int32_t* foff, const int32_t* ooff, float* out, void* stream);
+
 /* ---- WaveRNN vocoder (fatchord architecture): mel -> waveform, one GRU step per sample over fold rows ----
  * The MelResNet and the time-batched conditioning products run on the convolution-block and GEMM entry points; these entry points add
  * the mel upsampling layers, the folding, the persistent sample loop and the unfolding.  Fold rows: utterance b's F_b hop sample

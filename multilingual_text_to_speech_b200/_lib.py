@@ -183,6 +183,15 @@ class PsolaShape(Structure):
     _fields_ = [(n, c_int) for n in ('B', 'total_samples', 'total_frames', 'hop', 'unvoiced_spacing')] + [('sr', c_double)]
 
 
+# include/b200tts.h: B200TTS_WSOLA_MAX_HOP, B200TTS_WSOLA_MAX_TOLERANCE
+WSOLA_MAX_HOP = 1024
+WSOLA_MAX_TOLERANCE = 1024
+
+
+class WsolaShape(Structure):
+    _fields_ = [(n, c_int) for n in ('B', 'total_samples', 'total_out_samples', 'total_frames', 'hop', 'tolerance')]
+
+
 # name -> (restype, argtypes); the "-m not gpu" suite checks every symbol of the header resolves
 SIGNATURES = {
     'b200tts_last_error': (c_char_p, []),
@@ -283,6 +292,8 @@ SIGNATURES = {
     'b200tts_psola_workspace_bytes': (c_size_t, [POINTER(PsolaShape)]),
     'b200tts_psola_marks': (c_int, [POINTER(PsolaShape)] + [c_void_p] * 6 + [c_size_t, c_void_p]),
     'b200tts_psola_overlap_add': (c_int, [POINTER(PsolaShape)] + [c_void_p] * 3 + [c_size_t, c_void_p, c_void_p]),
+    'b200tts_wsola_positions': (c_int, [POINTER(WsolaShape)] + [c_void_p] * 6),
+    'b200tts_wsola_overlap_add': (c_int, [POINTER(WsolaShape)] + [c_void_p] * 7),
     'b200tts_wavernn_upsample_layer': (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     'b200tts_wavernn_fold': (c_int, [POINTER(WaveRNNFoldShape)] + [c_void_p] * 7 + [c_int, c_int, c_void_p, c_void_p]),
     'b200tts_wavernn_workspace_bytes': (c_size_t, [POINTER(WaveRNNShape)]),

@@ -1115,6 +1115,34 @@ def psola_overlap_add(shape, wave, soff, ws):
     return out
 
 
+# ------------------------------------------------------------------------------------------------
+# time-scale modification (WSOLA in two stages, include/b200tts.h; the same packed ragged layout)
+# ------------------------------------------------------------------------------------------------
+def wsola_positions(shape, wave, soff, warp, foff):
+    """The input position of every synthesis frame (a _lib.WsolaShape batch) from wave fp32 [total_samples] and the warp fp64
+    [total_frames] -> int32 [total_frames]."""
+    _require_cuda(wave, soff, warp, foff)
+    assert soff.dtype == torch.int32 and foff.dtype == torch.int32 and wave.dtype == torch.float32 and wave.is_contiguous()
+    assert warp.dtype == torch.float64 and warp.is_contiguous() and warp.numel() == shape.total_frames
+    assert wave.numel() == shape.total_samples
+    positions = torch.empty(shape.total_frames, dtype=torch.int32, device=wave.device)
+    check(_lib.load().b200tts_wsola_positions(ctypes.byref(shape), ptr(wave), ptr(soff), ptr(warp), ptr(foff), ptr(positions),
+                                              _stream()), 'b200tts_wsola_positions')
+    return positions
+
+
+def wsola_overlap_add(shape, wave, soff, positions, foff, ooff):
+    """The frames at `positions` (wsola_positions) overlap-added with the periodic Hann window -> fp32 [total_out_samples]."""
+    _require_cuda(wave, soff, positions, foff, ooff)
+    assert soff.dtype == torch.int32 and foff.dtype == torch.int32 and ooff.dtype == torch.int32 and positions.dtype == torch.int32
+    assert wave.dtype == torch.float32 and wave.is_contiguous() and wave.numel() == shape.total_samples
+    assert positions.is_contiguous() and positions.numel() == shape.total_frames
+    out = torch.empty(shape.total_out_samples, dtype=torch.float32, device=wave.device)
+    check(_lib.load().b200tts_wsola_overlap_add(ctypes.byref(shape), ptr(wave), ptr(soff), ptr(positions), ptr(foff), ptr(ooff), ptr(out),
+                                                _stream()), 'b200tts_wsola_overlap_add')
+    return out
+
+
 def symbol_average(track, durations, voiced=None):
     """Per-symbol means of a frame track [B, T] over each symbol's frames: symbol l of row b owns frames [C_{l-1}, C_l), C the cumulative
     sum of durations [B, L] (frames past C_{L-1} belong to no symbol).  Summed in frame order in float64; with `voiced` [B, T] (bool) only

@@ -616,3 +616,145 @@ def f0_ratio(f0_target, f0_source):
     out[:m][vv] = np.clip(t[:m][vv] / s[:m][vv], 0.5, 2.0)
     out = out.astype(np.float32)
     return out if s_np else torch.from_numpy(out).to(s_t.device)
+
+
+# time_stretch_batch's rate range: a quarter to four times the source rate
+STRETCH_RATES = (0.25, 4.0)
+
+
+def _stretch_length(L, rate):
+    return max(1, int(round(L / rate)))
+
+
+def _retime_length(L, hop, dp):
+    return max(1, hop * (int(dp.sum()) - 1) + L % hop)
+
+
+def _check_output_samples(lengths):
+    """ValueError when the outputs would not fit one int32-indexed batch; run before any warp is built."""
+    total = sum(lengths)
+    if total >= 2 ** 31:
+        raise ValueError(f'{total} output samples in one batch; at most 2^31 - 1')
+
+
+def _stretch_plan(L, hop, rate):
+    """(L', warp tau_k = k hop rate in fp64) of a time stretch."""
+    Lp = _stretch_length(L, rate)
+    return Lp, np.arange((Lp - 1) // hop + 2, dtype=np.float64) * hop * rate
+
+
+def _retime_plan(L, hop, d, dp):
+    """(L', warp tau_k = hop phi(k)) of a retime from durations d to dp (int64 [J]).  phi maps output frame coordinates onto input ones:
+    with B, B' the cumulative durations, [B'_j - 1/2, B'_{j+1} - 1/2) goes linearly onto [B_j - 1/2, B_{j+1} - 1/2), and past B'_J - 1/2
+    the slope is 1.  Frame k lies in the interval of the first symbol j with B'_{j+1} > k; a symbol with d'_j = 0 has no interval."""
+    Lp = _retime_length(L, hop, dp)
+    K = (Lp - 1) // hop + 2
+    J = len(d)
+    B = np.concatenate([[0], np.cumsum(d)]).astype(np.float64)
+    Bp = np.concatenate([[0], np.cumsum(dp)]).astype(np.float64)
+    k = np.arange(K, dtype=np.float64)
+    j = np.searchsorted(Bp[1:], k, side='right')
+    inside = j < J
+    jj = np.minimum(j, J - 1)
+    lo_in = np.where(inside, B[jj], B[J]) - 0.5
+    lo_out = np.where(inside, Bp[jj], Bp[J]) - 0.5
+    num = np.where(inside, d[jj], 1).astype(np.float64)
+    den = np.where(inside, dp[jj], 1).astype(np.float64)
+    return Lp, hop * (lo_in + (k - lo_out) * num / den)
+
+
+def _wsola(waves, as_np, soff_host, plans):
+    """Both WSOLA kernels on the packed batch; plans: (L', warp fp64 [K]) per waveform -> the output waveforms."""
+    hop = ms_to_frames(hp.stft_shift_ms)
+    ooff_host = np.concatenate([[0], np.cumsum([Lp for Lp, _ in plans])]).astype(np.int64)
+    foff_host = np.concatenate([[0], np.cumsum([len(w) for _, w in plans])]).astype(np.int64)
+    device = _work_device(waves)
+    with torch.cuda.device(device):
+        shape = _lib.WsolaShape(len(waves), int(soff_host[-1]), int(ooff_host[-1]), int(foff_host[-1]), hop, hop)
+        wave = torch.cat([w.to(device=device, dtype=torch.float32) for w in waves]).contiguous()
+        soff, ooff, foff = (torch.from_numpy(o.astype(np.int32)).to(device) for o in (soff_host, ooff_host, foff_host))
+        warp = torch.from_numpy(np.concatenate([w for _, w in plans])).to(device)
+        positions = F.wsola_positions(shape, wave, soff, warp, foff)
+        y = F.wsola_overlap_add(shape, wave, soff, positions, foff, ooff)
+    return [_return_like(y[ooff_host[i]:ooff_host[i + 1]], as_np[i], waves[i]) for i in range(len(waves))]
+
+
+def _wsola_inputs(waveforms, what):
+    """Checked, finite waveforms packed as _pack_waveforms packs them, and the hop WSOLA uses."""
+    waves, as_np, soff_host, off_host = _pack_waveforms(waveforms, what)
+    for i, w in enumerate(waves):
+        if not bool(torch.isfinite(w).all()):
+            raise ValueError(f'waveform {i} has non-finite samples')
+    if soff_host[-1] > 2 ** 31 - 1 - _lib.WSOLA_MAX_TOLERANCE:
+        raise ValueError(f'{soff_host[-1]} samples in one batch; at most 2^31 - 1 - {_lib.WSOLA_MAX_TOLERANCE}')
+    hop = ms_to_frames(hp.stft_shift_ms)
+    if not 1 <= hop <= _lib.WSOLA_MAX_HOP:
+        raise ValueError(f'hop {hop} (hp.stft_shift_ms) must be in [1, {_lib.WSOLA_MAX_HOP}] samples')
+    return waves, as_np, soff_host, off_host, hop
+
+
+def time_stretch_batch(waveforms, rate):
+    """Time-stretch waveforms [L_i] by WSOLA (waveform-similarity overlap-add), keeping pitch and formants: `rate` is one float or one
+    per waveform, finite and in [0.25, 4]; above 1 is faster, as in librosa.effects.time_stretch.  Output i has
+    L'_i = max(1, round(L_i / rate_i)) samples.  Frames 2 hop long (hop = ms_to_frames(hp.stft_shift_ms), the mel hop) are overlap-added
+    with a periodic Hann window every hop output samples; frame k is read near input sample k hop rate, shifted by up to hop samples to
+    the position most similar to the natural continuation of frame k - 1.  include/b200tts.h and tests/wsola_oracle.py state the rules
+    exactly.  At rate 1 the output is the input.  Waveforms are rounded to fp32; the search and the sums are fp64 in the library's kernels.
+    The same device and numpy / torch rules as spectrogram_batch.  Raises ValueError on a bad or non-finite waveform, a rate count that
+    does not match, a rate out of range, or more than 2^31 - 1 output samples."""
+    waves, as_np, soff_host, _, hop = _wsola_inputs(waveforms, 'time_stretch_batch')
+    B = len(waves)
+    try:
+        rates = np.asarray(rate).astype(np.float64)
+    except (TypeError, ValueError):
+        raise ValueError(f'rate must be numeric (got {rate!r})') from None
+    if rates.ndim > 1 or (rates.ndim == 1 and len(rates) != B):
+        raise ValueError(f'rate must be one float or one per waveform ({B})')
+    rates = np.broadcast_to(rates, (B,))
+    lo, hi = STRETCH_RATES
+    if not np.isfinite(rates).all() or (rates < lo).any() or (rates > hi).any():
+        raise ValueError(f'rate must be finite and in [{lo}, {hi}] (got {rates.tolist()})')
+    _check_output_samples([_stretch_length(len(w), float(r)) for w, r in zip(waves, rates)])
+    return _wsola(waves, as_np, soff_host, [_stretch_plan(len(w), hop, float(r)) for w, r in zip(waves, rates)])
+
+
+def time_stretch(y, rate):
+    """One waveform time-stretched by `rate` (above 1 is faster).  See time_stretch_batch."""
+    return time_stretch_batch([y], rate)[0]
+
+
+def retime_batch(waveforms, durations, new_durations):
+    """Retime waveforms [L_i] by WSOLA from per-symbol durations to new ones: symbol j's frames are stretched or squeezed so that it lasts
+    new_durations[i][j] mel frames instead of durations[i][j], keeping pitch and formants.  Both are int frames per symbol, one track per
+    waveform, as Tacotron.align gives them for a mel made by mel_spectrogram(y) (align(...).durations[b, :L_b]): each sum(durations[i])
+    must be the waveform's 1 + L_i // hop mel frames, both tracks have the same length, every entry is >= 0 and sum(new_durations[i]) >= 1.
+    Output i has L'_i = max(1, hop (sum d' - 1) + L_i mod hop) samples, so spectrogram(y') has sum d' frames.  The warp is defined on frame
+    coordinates: symbol j's output interval [B'_j - 1/2, B'_{j+1} - 1/2) maps linearly onto its input interval [B_j - 1/2, B_{j+1} - 1/2),
+    B and B' the cumulative durations; a symbol with d'_j = 0 is dropped, one with d_j = 0 holds its boundary, and past the last boundary
+    the slope is 1.  Frame k is then read near input sample hop phi(k) and placed as time_stretch_batch places it, so with
+    new_durations = durations the output is the input.  Raises ValueError on a bad or non-finite waveform, counts that do not match,
+    malformed durations, or more than 2^31 - 1 output samples."""
+    waves, as_np, soff_host, off_host, hop = _wsola_inputs(waveforms, 'retime_batch')
+    B = len(waves)
+    for what, t in (('durations', durations), ('new_durations', new_durations)):
+        if not isinstance(t, (list, tuple)) or len(t) != B:
+            raise ValueError(f'retime_batch: {what} must be a list of {B} tracks, one per waveform')
+    tracks = []
+    for i in range(B):
+        d = F._durations_host(durations[i], f'retime_batch durations[{i}]')
+        dp = F._durations_host(new_durations[i], f'retime_batch new_durations[{i}]')
+        if len(d) != len(dp):
+            raise ValueError(f'retime_batch: durations[{i}] has {len(d)} symbols, new_durations[{i}] {len(dp)}')
+        frames = int(off_host[i + 1] - off_host[i])
+        if int(d.sum()) != frames:
+            raise ValueError(f'retime_batch: durations[{i}] total {int(d.sum())} frames; waveform {i} has {frames} (1 + L // hop)')
+        if int(dp.sum()) < 1:
+            raise ValueError(f'retime_batch: new_durations[{i}] total 0 frames')
+        tracks.append((d, dp))
+    _check_output_samples([_retime_length(len(w), hop, dp) for w, (_, dp) in zip(waves, tracks)])
+    return _wsola(waves, as_np, soff_host, [_retime_plan(len(w), hop, d, dp) for w, (d, dp) in zip(waves, tracks)])
+
+
+def retime(y, durations, new_durations):
+    """One waveform retimed from `durations` to `new_durations` (int frames per symbol).  See retime_batch."""
+    return retime_batch([y], [durations], [new_durations])[0]
