@@ -223,7 +223,10 @@ size_t b200tts_debug_persist_bwd_profile_offset(const b200tts_decoder_shape* sha
  *   forward workspace:  ai, ca, hg, cg, ga, gg, q, cum, memT, fs, p1, aib, hgb
  *   backward workspace: dfs, dhgd, dctxs, dgg, dhas, dga, dq, dctxt, dmemT, dggb, dgab
  *   row strides (in elements) of aib and hgb: Kp_att, Kp_gen
- * Returns the number of values written (26 when n >= 26), 0 for a rejected shape. */
+ *   forward workspace:  xtm (prenet input, row i = the frame fed to step i), p0 (first prenet layer)
+ *   backward workspace: dp1, dp0 (prenet layer gradients after the relu / dropout backward)
+ * Every per-step view has one row per decoder step (S = ceil(T / R)); fs and dfs are R (N + 1) wide.
+ * Returns the number of values written (30 when n >= 30), 0 for a rejected shape. */
 int b200tts_debug_decoder_views(const b200tts_decoder_shape* shape, size_t* out, int n);
 /* Debug (pure host arithmetic, no device needed): the geometry the persistent loops would run this shape with.  Fills out[0 .. n) in
  * this order:

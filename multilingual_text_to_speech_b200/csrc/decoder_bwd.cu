@@ -1075,7 +1075,7 @@ int b200tts_debug_decoder_views(const b200tts_decoder_shape* shape, size_t* out,
     const TcPersistGeom g = tc_persist_geom(s);
     const BwdLayout bl = bwd_layout(s);
     const size_t pbase = l.persist * sizeof(float);
-    size_t v[26];
+    size_t v[30];
     const size_t fwd[11] = {l.ai, l.ca, l.hg, l.cg, l.ga, l.gg, l.q, l.cum, l.memT, l.fs, l.p1};
     for (int k = 0; k < 11; ++k) v[k] = fwd[k] * sizeof(float);
     v[11] = pbase + pl.aib;
@@ -1085,7 +1085,13 @@ int b200tts_debug_decoder_views(const b200tts_decoder_shape* shape, size_t* out,
     for (int k = 0; k < 11; ++k) v[13 + k] = bwd[k] * sizeof(float);
     v[24] = (size_t)g.Kp_att;
     v[25] = (size_t)g.Kp_gen;
-    const int m = n < 26 ? n : 26;
+    // the prenet's rows, appended so that the indices above keep their meaning: its input and first layer (forward), and the
+    // gradients of both layers after the relu / dropout backward, which works in place (backward)
+    v[26] = l.xtm * sizeof(float);
+    v[27] = l.p0 * sizeof(float);
+    v[28] = bl.dp1 * sizeof(float);
+    v[29] = bl.dp0 * sizeof(float);
+    const int m = n < 30 ? n : 30;
     for (int k = 0; k < m; ++k) out[k] = v[k];
     return m;
 }

@@ -122,22 +122,24 @@ def _oracle_run(c, dtype, with_grad):
     return sd, memory, spec, stop, align
 
 
-def _cuda_inputs(c, device):
+def _cuda_inputs(c, device, r=1):
+    """Library config / parameters / memory of case `c`; at r frames per step (outputs_per_step_oracle.untie) its tape has one row per
+    decoder step, S = ceil(T / r)."""
     from multilingual_text_to_speech_b200 import functional as F
     from multilingual_text_to_speech_b200 import _lib
     hp = c.hp
     kind = _lib.CELL_ZONEOUT if hp.decoder_regularization == 'zoneout' else _lib.CELL_DROPOUT
     rates = (hp.zoneout_hidden, hp.zoneout_cell) if kind == _lib.CELL_ZONEOUT else (hp.dropout_hidden, 0.0)
-    T = c.target.shape[2]
+    S = -(-c.target.shape[2] // r)
     masks = {}
     for name in ('prenet0', 'prenet1'):
-        if name in c.tape:          # tape layout [B, T+1, P] -> time-major [T, B, P] (row T is never consumed)
-            masks[name] = c.tape[name][:, :T].transpose(0, 1).contiguous().to(torch.uint8).to(device)
+        if name in c.tape:          # tape layout [B, S+1, P] -> time-major [S, B, P] (row S is never consumed)
+            masks[name] = c.tape[name][:, :S].transpose(0, 1).contiguous().to(torch.uint8).to(device)
     for name in ('att_h', 'att_c', 'gen_h', 'gen_c', 'step_prenet0', 'step_prenet1'):
         if name in c.tape:
-            masks[name] = c.tape[name].contiguous().to(torch.uint8).to(device)
-    teacher = c.tape['teacher'].numpy().astype(np.uint8)
-    cfg = F.DecoderConfig(kind, c.training, rates[0], rates[1], hp.dropout, masks, None if teacher.all() else teacher)
+            masks[name] = c.tape[name][:S].contiguous().to(torch.uint8).to(device)
+    teacher = c.tape['teacher'][:S].numpy().astype(np.uint8)
+    cfg = F.DecoderConfig(kind, c.training, rates[0], rates[1], hp.dropout, masks, None if teacher.all() else teacher, outputs_per_step=r)
     params = [c.sd[key].to(device).clone().requires_grad_(True) for _, key in PARAM_KEYS]
     memory = c.memory.to(device).clone().requires_grad_(True)
     return cfg, params, memory

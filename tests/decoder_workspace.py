@@ -1,8 +1,12 @@
 """Named views of the decoder's forward and backward workspaces.
 
 The fused decoder keeps every step's state in its workspaces (fp32 states, activated gates, queries, cumulative weights, the bf16
-operand rows the persistent loops fed to wgmma, and in the backward the per-step gate gradients and their bf16 histories).  The
-offsets come from the library itself (b200tts_debug_decoder_views), so these views follow any change of the layouts.
+operand rows the persistent loops fed to wgmma, the prenet's rows, and in the backward the per-step gate gradients and their bf16
+histories).  The offsets come from the library itself (b200tts_debug_decoder_views), so these views follow any change of the layouts.
+
+With R frames per step a decode of T frames runs S = ceil(T / R) steps: every per-step view has S rows (S + 1 for the states, whose
+row 0 is the initial state), and the step rows of the [frame ; stop] projection, fs and dfs, are R (N + 1) wide: R frames of N, then
+the R stop logits.
 
 Set functional.PROFILE['keep_ws'] = True before a decoder call; functional then keeps that call's workspaces in PROFILE['last_ws'],
 PROFILE['last_bws'] and PROFILE['last_shape'].
@@ -11,9 +15,11 @@ import ctypes
 
 import torch
 
-FWD = ('ai', 'ca', 'hg', 'cg', 'ga', 'gg', 'q', 'cum', 'memT', 'fs', 'p1', 'aib', 'hgb')
-BWD = ('dfs', 'dhgd', 'dctxs', 'dgg', 'dhas', 'dga', 'dq', 'dctxt', 'dmemT', 'dggb', 'dgab')
-NVIEWS = len(FWD) + len(BWD) + 2
+FWD = ('ai', 'ca', 'hg', 'cg', 'ga', 'gg', 'q', 'cum', 'memT', 'fs', 'p1', 'aib', 'hgb', 'xtm', 'p0')
+BWD = ('dfs', 'dhgd', 'dctxs', 'dgg', 'dhas', 'dga', 'dq', 'dctxt', 'dmemT', 'dggb', 'dgab', 'dp1', 'dp0')
+# the library's order: the first 13 forward views, the first 11 backward views, the two row strides, then the views appended later
+ORDER = FWD[:13] + BWD[:11] + ('Kp_att', 'Kp_gen') + ('xtm', 'p0', 'dp1', 'dp0')
+NVIEWS = len(ORDER)
 
 
 def offsets(shape):
@@ -22,23 +28,32 @@ def offsets(shape):
     out = (ctypes.c_size_t * NVIEWS)()
     n = _lib.load().b200tts_debug_decoder_views(ctypes.byref(shape), out, NVIEWS)
     assert n == NVIEWS, ('decoder shape rejected', n)
-    names = FWD + BWD + ('Kp_att', 'Kp_gen')
-    return dict(zip(names, [int(v) for v in out]))
+    return dict(zip(ORDER, [int(v) for v in out]))
+
+
+def frames_per_step(shape):
+    return max(int(shape.R), 1)       # R = 0 means 1
+
+
+def steps(shape):
+    return -(-int(shape.T) // frames_per_step(shape))
 
 
 def view_shapes(shape, Kp_att, Kp_gen):
-    """{name: (dtype, dims)} of every view."""
+    """{name: (dtype, dims)} of every view, for the decode of shape.T frames at shape.R frames per step."""
     s = shape
-    T, B, D, M, L, A, N, P = s.T, s.B, s.D, s.M, s.L, s.A, s.N, s.P
+    B, D, M, L, A, N, P = s.B, s.D, s.M, s.L, s.A, s.N, s.P
+    S, W = steps(s), frames_per_step(s) * (s.N + 1)
     f32, b16 = torch.float32, torch.bfloat16
     return {
-        'ai': (f32, (T + 1, B, M + D)), 'ca': (f32, (T + 1, B, D)), 'hg': (f32, (T + 1, B, D)), 'cg': (f32, (T + 1, B, D)),
-        'ga': (f32, (T, B, 4 * D)), 'gg': (f32, (T, B, 4 * D)), 'q': (f32, (T, B, A)), 'cum': (f32, (T + 1, B, L)),
-        'memT': (f32, (B, L, A)), 'fs': (f32, (T, B, N + 1)), 'p1': (f32, (T, B, P)),
-        'aib': (b16, (T + 1, B, Kp_att)), 'hgb': (b16, (T + 1, B, Kp_gen)),
-        'dfs': (f32, (T, B, N + 1)), 'dhgd': (f32, (T, B, D)), 'dctxs': (f32, (T, B, M)), 'dgg': (f32, (T, B, 4 * D)),
-        'dhas': (f32, (T, B, D)), 'dga': (f32, (T, B, 4 * D)), 'dq': (f32, (T, B, A)), 'dctxt': (f32, (T, B, M)),
-        'dmemT': (f32, (B, L, A)), 'dggb': (b16, (T, B, 4 * D)), 'dgab': (b16, (T, B, 4 * D)),
+        'ai': (f32, (S + 1, B, M + D)), 'ca': (f32, (S + 1, B, D)), 'hg': (f32, (S + 1, B, D)), 'cg': (f32, (S + 1, B, D)),
+        'ga': (f32, (S, B, 4 * D)), 'gg': (f32, (S, B, 4 * D)), 'q': (f32, (S, B, A)), 'cum': (f32, (S + 1, B, L)),
+        'memT': (f32, (B, L, A)), 'fs': (f32, (S, B, W)), 'p1': (f32, (S, B, P)),
+        'aib': (b16, (S + 1, B, Kp_att)), 'hgb': (b16, (S + 1, B, Kp_gen)), 'xtm': (f32, (S, B, N)), 'p0': (f32, (S, B, P)),
+        'dfs': (f32, (S, B, W)), 'dhgd': (f32, (S, B, D)), 'dctxs': (f32, (S, B, M)), 'dgg': (f32, (S, B, 4 * D)),
+        'dhas': (f32, (S, B, D)), 'dga': (f32, (S, B, 4 * D)), 'dq': (f32, (S, B, A)), 'dctxt': (f32, (S, B, M)),
+        'dmemT': (f32, (B, L, A)), 'dggb': (b16, (S, B, 4 * D)), 'dgab': (b16, (S, B, 4 * D)),
+        'dp1': (f32, (S, B, P)), 'dp0': (f32, (S, B, P)),
     }
 
 

@@ -14,6 +14,9 @@ The reference rounds exactly the operands the kernel rounds (`mode`):
     'fp32'        fp32 mode (per-step chains): no rounding model at all
 Every rounding point is named with the source line it models.  There is no blanket relative tolerance anywhere.
 
+Around the recurrences, the frame edges of a teacher-forced decode at R frames per step (prenet input and layers, the frame split and
+gather, the prenet backward) and every parameter gradient are checked the same way (check_all).
+
 Each check_* function fills a Report: per stage, the worst err / bound ratio of every step and where the overall worst sits.
 """
 import math
@@ -493,7 +496,7 @@ def attention_backward(dw, b_dw, w, lens, t, b_t, v_e, wcb, wcb_abs, K, mode):
         dloc[:, lo:hi] += G[:, lo + half - k:hi + half - k, k]
         b_loc[:, lo:hi] += b_G[:, lo + half - k:hi + half - k, k]
         a_loc[:, lo:hi] += G[:, lo + half - k:hi + half - k, k].abs()
-    return {'de': de, 'b_de': b_de, 'ds': ds, 'b_ds': b_ds, 'dloc': dloc, 'b_loc': b_loc, 'a_loc': a_loc}
+    return {'de': de, 'b_de': b_de, 'ds': ds, 'b_ds': b_ds, 'dsr': dsr, 'b_dsr': b_dsr, 'dloc': dloc, 'b_loc': b_loc, 'a_loc': a_loc}
 
 
 class AttentionReverse:
@@ -507,7 +510,7 @@ class AttentionReverse:
     geometrically with the number of reverse steps.  The dq / dmemT bounds are therefore tight for the last steps of a decode (the
     first reverse steps) and for short decodes, and lose their power after a few tens of reverse steps of a long one."""
 
-    def __init__(self, v, prm, lengths, memory, align, dalign, mode, rep, fill=False):
+    def __init__(self, v, prm, lengths, memory, align, dalign, mode, rep, fill=False, keep_terms=False):
         T, B, D, M, L, A = _dims(v)
         self.v, self.prm, self.mode, self.rep, self.fill = v, prm, mode, rep, fill
         self.T, self.D, self.M, self.L, self.A = T, D, M, L, A
@@ -537,6 +540,13 @@ class AttentionReverse:
         self.dcum, self.b_dcum = z(B_, L), z(B_, L)
         self.lose_carry_at = None           # synthetic workspaces only: the d cum carry is lost on entry to this step
         self.dmemT, self.b_dmemT = z(B_, L, A), z(B_, L, A)
+        # attention-parameter gradients: d Wcomb [A, K] = sum ds^T . cum window and d v [A] = sum de t, with the sums of the |terms|
+        # and of the term bounds (param_grads)
+        C = Wc.shape[0]
+        self.C = C
+        self.dW, self.aW, self.bW = z(A, self.K), z(A, self.K), z(A, self.K)
+        self.dv, self.av, self.bv = z(A), z(A), z(A)
+        self.terms = [] if keep_terms else None
 
     def step(self, i):
         v, mode, rep = self.v, self.mode, self.rep
@@ -580,9 +590,47 @@ class AttentionReverse:
         rep.add('dq', i, (v['dq'][i].double() - dq).abs()[None], b_dq[None])
         self.dmemT = self.dmemT + ds
         self.b_dmemT = self.b_dmemT + b_ds + U * self.dmemT.abs()
+        # ---- this step's terms of d Wcomb and d v.  persist: the post pass (decoder_persist_bwd.cu:679-834) multiplies the bf16 ds
+        # (:797) by the bf16 hi half of the cumulative-weight window only (:750-753, :799-805); the chains (decoder_bwd.cu:454-523)
+        # form d Wloc and d Wc from the fp32 ds, location features and window, which is the same sum factored through Wloc and Wc.
+        unf = Fn.pad(v['cum'][i].double(), (self.half, K - 1 - self.half)).unfold(-1, K, 1)      # [B, L, K]: cum[l + k - half]
+        if mode == 'persist':
+            unf = rn(unf)
+        self._add_terms(i, ab['dsr'], ab['b_dsr'], unf, ab['de'], ab['b_de'], t[0], b_t[0])
         # ---- d cum of step i-1: carry + the location term's transposed convolution
         self.dcum = self.dcum + ab['dloc']
         self.b_dcum = self.b_dcum + ab['b_loc'] + (K + 2) * U * (ab['a_loc'] + self.dcum.abs())
+
+    def _add_terms(self, i, dsr, b_dsr, unf, de, b_de, t, b_t):
+        if self.terms is not None:
+            self.terms.append((i, dsr, unf, de, t))
+        self.dW += torch.einsum('bla,blk->ak', dsr, unf)
+        self.aW += torch.einsum('bla,blk->ak', dsr.abs(), unf.abs())
+        self.bW += torch.einsum('bla,blk->ak', b_dsr, unf.abs())
+        self.dv += torch.einsum('bl,bla->a', de, t)
+        self.av += torch.einsum('bl,bla->a', de.abs(), t.abs())
+        self.bv += torch.einsum('bl,bla->a', b_de, t.abs()) + torch.einsum('bl,bla->a', de.abs(), b_t)
+
+    def param_grads(self):
+        """attn_energy, attn_location and attn_loc_features from the summed terms -> [(name, None, reference, bound)].
+        d Wloc = d Wcomb . Wc^T and d Wc = Wloc^T . d Wcomb: the persistent finish kernel (decoder_persist_bwd.cu:878-898) factors the
+        reduced d Wcomb that way with one fmaf per k or a; the chains sum per-utterance products of fp32 location features (K terms) or
+        of ds . Wloc (A terms).  Every (step, utterance, position) term is accumulated in fp32, then the per-tile (persist) or
+        per-utterance (chains) partials are reduced: n + 2 roundings in the worst case.  A bound the d cum carry has driven past the
+        fp64 range admits anything (inf)."""
+        T, L, A, K, C = self.T, self.L, self.A, self.K, self.C
+        B_ = self.lens.numel()
+        n = T * B_ * L + B_ * -(-L // 16) + 2
+        wl = self.prm['attn_location'].double()                              # [A, C]
+        wc = self.prm['attn_loc_features'].reshape(C, K).double()           # [C, K]
+        fin = lambda b: torch.nan_to_num(b, nan=math.inf)                    # noqa: E731
+        dloc = self.dW @ wc.t()
+        b_loc = self.bW @ wc.abs().t() + (n + K + 2) * U * (self.aW @ wc.abs().t())
+        dwc = wl.t() @ self.dW
+        b_wc = wl.abs().t() @ self.bW + (n + A + 2) * U * (wl.abs().t() @ self.aW)
+        return [('attn_energy', None, self.dv[None], fin(self.bv + (n + 2) * U * self.av)[None]),
+                ('attn_location', None, dloc, fin(b_loc)),
+                ('attn_loc_features', None, dwc, fin(b_wc))]
 
     def finish(self):
         if self.fill:
@@ -598,10 +646,11 @@ def modes_of(mode):
     return out
 
 
-def check_reverse(v, prm, masks, cfg, mode, report=None, fill=False, attention=None, lose_carry_at=None):
+def check_reverse(v, prm, masks, cfg, mode, report=None, fill=False, attention=None, lose_carry_at=None, grads=None):
     """Gate gradients of the generator reverse loop (dgg) and of the attention-LSTM part of the attention reverse loop (dga, from the
     loop's own query gradients dq), teacher-forced decodes.  attention = (lengths, memory, align, dalign): also the attention backward
-    of the attention reverse loop (AttentionReverse).  mode: one for both recurrences, or (generator, attention)."""
+    of the attention reverse loop (AttentionReverse), and with `grads` ({parameter name: gradient}) the attention-parameter gradients
+    it sums (written into `grads` when filling).  mode: one for both recurrences, or (generator, attention)."""
     gen_mode, att_mode = (mode, mode) if isinstance(mode, str) else tuple(mode)
     assert gen_mode in MODES and att_mode in MODES
     mode = att_mode
@@ -625,11 +674,184 @@ def check_reverse(v, prm, masks, cfg, mode, report=None, fill=False, attention=N
              None if att is None else att.step)
     if att is not None:
         att.finish()
+        if grads is not None:
+            for name, sl, ref, bound in att.param_grads():
+                if fill:
+                    _grad_view(grads[name], sl).copy_(ref.float())
+                rep.add(name, 0, (_grad_view(grads[name], sl).double() - ref).abs()[None], bound[None])
+    return rep
+
+
+def attention_terms(v, prm, lengths, memory, align, dalign, mode):
+    """The per-step terms (step, ds as the d Wcomb product reads it, cumulative-weight window, de, t) of the attention-parameter
+    gradients, from a sweep of AttentionReverse over a workspace (synthetic workspaces: to build a kernel-style mistake)"""
+    att = AttentionReverse(v, prm, lengths, memory, align, dalign, mode, Report(_dims(v)[0]), keep_terms=True)
+    for i in range(_dims(v)[0] - 1, -1, -1):
+        att.step(i)
+    return att.terms
+
+
+def attention_grads_of_terms(prm, terms, mode, wloc=None):
+    """{attn_energy, attn_location, attn_loc_features} summed from `terms` (attention_terms) as the kernels factor them; wloc: the
+    location weights the d Wc product reads, [A, C] (default prm['attn_location'])"""
+    Wc = prm['attn_loc_features']
+    C, K = Wc.shape[0], Wc.shape[-1]
+    dW = sum(torch.einsum('bla,blk->ak', ds, unf) for _, ds, unf, _, _ in terms)
+    dv = sum(torch.einsum('bl,bla->a', de, t) for _, _, _, de, t in terms)
+    wl = (prm['attn_location'] if wloc is None else wloc).double()
+    return {'attn_energy': dv.reshape(1, -1).float(), 'attn_location': (dW @ Wc.reshape(C, K).double().t()).float(),
+            'attn_loc_features': (wl.t() @ dW).reshape(C, 1, K).float()}
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# the frame edges of a teacher-forced decode: prenet input and layers, the frame split and gather, the prenet backward
+# ------------------------------------------------------------------------------------------------------------------------
+def frames_per_step(prm):
+    """R: the stop projection has one row per frame of a step"""
+    return prm['stop_w'].shape[0]
+
+
+def prenet_scale(rate, keep):
+    """the keep scale of a prenet layer: 1 / (1 - p), one IEEE fp32 division of fp32 values (decoder_fwd.cu:692,
+    decoder_bwd.cu:995); 1 without keep masks, which drop nothing"""
+    if keep is None:
+        return 1.0
+    one = torch.tensor(1.0, dtype=torch.float32)
+    return float(one / (one - torch.tensor(rate, dtype=torch.float32)))
+
+
+def teacher_frames(target, S, R):
+    """The prenet input of S steps, [S, B, N]: row 0 zero, row i the target frame i R - 1 (prep_target_kernel, decoder_fwd.cu:29-47)"""
+    B, N, _ = target.shape
+    x = torch.zeros(S, B, N, dtype=torch.float64, device=target.device)
+    if S > 1:
+        x[1:] = target[:, :, R - 1::R][:, :, :S - 1].permute(2, 0, 1).double()
+    return x
+
+
+def prenet_layer(x, w, b, keep, scale, mode):
+    """relu(x . W^T + b) * keep * scale of rows x (prenet_rows, decoder_fwd.cu:690-700): one GEMM with bf16 operands in the bf16 modes
+    and the bias added in its epilogue, then relu_dropout_kernel (:50-56), whose (v * keep) * scale rounds once; relu is 1-Lipschitz.
+    -> (y, bound)"""
+    z, b_z = product(ra(x, mode), rw(w, mode))
+    bb = b.reshape(-1).double()
+    z = z + bb
+    b_z = b_z + 2 * U * (z.abs() + bb.abs())
+    y = torch.relu(z)
+    if keep is None:
+        return y, b_z
+    k = keep.double() * scale
+    y = y * k
+    return y, k * b_z + U * y.abs()
+
+
+def per_step(x, S, R):
+    """[B, T, ...] per frame -> [S, B, R, ...] per step slot (frame k = i R + j), zero past the T frames"""
+    B, T = x.shape[:2]
+    pad = x.new_zeros((B, S * R - T) + tuple(x.shape[2:]))
+    return torch.cat([x, pad], 1).reshape(B, S, R, *x.shape[2:]).transpose(0, 1)
+
+
+def split_frames(fs, T, R):
+    """The step rows fs [S, B, R (N + 1)] cut into (spec [B, T, N], stop [B, T]) as split_frames_kernel (decoder_fwd.cu:58-73) does:
+    frame k = i R + j is fs[i, :, j N:(j + 1) N] and stop logit fs[i, :, R N + j]; the tail of the last step is not emitted."""
+    S, B, W = fs.shape
+    N = W // R - 1
+    spec = fs[..., :R * N].reshape(S, B, R, N).transpose(0, 1).reshape(B, S * R, N)[:, :T]
+    stop = fs[..., R * N:].transpose(0, 1).reshape(B, S * R)[:, :T]
+    return spec, stop
+
+
+def gather_frame_grads(dspec, dstop, S, B, N, R, T, device):
+    """dfs [S, B, R (N + 1)] from the per-frame gradients (gather_frame_grads_kernel, decoder_bwd.cu:17-35): the inverse of
+    split_frames, 0 for the frames past T and for an absent gradient"""
+    z = lambda *s: torch.zeros(*s, dtype=torch.float64, device=device)      # noqa: E731
+    ds = z(B, T, N) if dspec is None else dspec.double()
+    dt = z(B, T) if dstop is None else dstop.double()
+    return torch.cat([per_step(ds, S, R).reshape(S, B, R * N), per_step(dt, S, R)], -1)
+
+
+def check_frames_forward(v, prm, masks, prenet_rate, target, spec, stop, mode, report=None):
+    """The prenet input (xtm, bitwise), both prenet layers (p0, p1) from the kernel's own input rows, and the frames and stop logits a
+    decode of target.shape[2] frames emits (spec, stop: bitwise the fs columns).  masks: the prenet keep masks 'prenet0' / 'prenet1'
+    [S, B, P] when the decode had them."""
+    S, B = v['xtm'].shape[:2]
+    R = frames_per_step(prm)
+    T = target.shape[2]
+    rep = report or Report(S)
+    masks = masks or {}
+    x = teacher_frames(target, S, R)
+    rep.add('xtm', 0, (v['xtm'].double() - x).abs(), torch.zeros_like(x))
+    y = v['xtm']
+    for k, name in enumerate(('p0', 'p1')):
+        keep = masks.get(f'prenet{k}')
+        ref, bound = prenet_layer(y, prm[f'prenet_w{k}'], prm[f'prenet_b{k}'], keep, prenet_scale(prenet_rate, keep), mode)
+        rep.add(name, 0, (v[name].double() - ref).abs(), bound)
+        y = v[name]
+    N = v['fs'].shape[2] // R - 1
+    assert tuple(spec.shape) == (B, T, N) and tuple(stop.shape) == (B, T), (tuple(spec.shape), tuple(stop.shape), (B, T, N))
+    sp, st = split_frames(v['fs'].double(), T, R)
+    for name, got, ref in (('spec', spec, sp), ('stop', stop, st)):
+        err = per_step((got.double() - ref).abs(), S, R)
+        rep.add(name, 0, err, torch.zeros_like(err))
+    return rep
+
+
+def check_frames_backward(v, prm, dspec, dstop, T, mode, report=None, fill=False, keep_dfs=False, gen_mode=None):
+    """dfs: bitwise the gather of d spec and d stop, exactly 0 past the T frames; then d h_gen (direct) and d ctx (static part), the
+    products of the kernel's own dfs with [frame_w ; stop_w] (decoder_bwd.cu:1246-1251).  The static d ctx the attention reverse loop
+    reads also holds the generator input gradient dgg . gen_w_ih[:, D:], which gen_input_grads (decoder_bwd.cu:913-922) accumulates
+    onto the product once the generator reverse loop is done (its bf16 history dggb when that loop was persistent: gen_mode).
+    fill: write the references instead (synthetic workspaces; keep_dfs: all but dfs)."""
+    S, B, W = v['dfs'].shape
+    D = v['dhgd'].shape[2]
+    R = frames_per_step(prm)
+    rep = report or Report(S)
+    ref = gather_frame_grads(dspec, dstop, S, B, W // R - 1, R, T, v['dfs'].device)
+    if fill and not keep_dfs:
+        v['dfs'].copy_(ref.float())
+    rep.add('dfs', 0, (v['dfs'].double() - ref).abs(), torch.zeros_like(ref))
+    wfs = torch.cat([prm['frame_w'], prm['stop_w']], 0)                 # [R (N + 1), D + M]
+    a = ra(v['dfs'], mode)
+    gen_mode = gen_mode or mode
+    g = v['dggb'].double() if gen_mode == 'persist' else ra(v['dgg'], gen_mode)
+    for name, w in (('dhgd', wfs[:, :D]), ('dctxs', wfs[:, D:])):
+        y, b_y = product(a, rw(w, mode).t())
+        b_y = b_y + U * y.abs()
+        if name == 'dctxs':
+            y2, b_y2 = product(g, rw(prm['gen_w_ih'][:, D:].t(), mode))
+            y = y + y2
+            b_y = b_y + b_y2 + U * y.abs()
+        if fill:
+            v[name].copy_(y.float())
+        rep.add(name, 0, (v[name].double() - y).abs(), b_y)
+    return rep
+
+
+def check_prenet_backward(v, prm, masks, prenet_rate, mode, report=None, fill=False):
+    """dp1 = dga . W_ih[:, :P] (the bf16 history dgab in persist mode) through the relu / dropout backward of layer 1, dp0 = dp1 . W1
+    through that of layer 0 (decoder_bwd.cu:1340-1350, relu_dropout_bwd_kernel :99-103: scale where the kernel's own output row is
+    positive, exactly 0 elsewhere).  mode: the attention reverse loop's.  fill: write the references instead."""
+    S = v['dp1'].shape[0]
+    P = v['dp1'].shape[2]
+    rep = report or Report(S)
+    masks = masks or {}
+    g = v['dgab'].double() if mode == 'persist' else ra(v['dga'], mode)
+    a = g
+    for name, w, y in (('dp1', prm['att_w_ih'][:, :P].t(), v['p1']), ('dp0', prm['prenet_w1'].t(), v['p0'])):
+        z, b_z = product(a, rw(w, mode))
+        k = (y > 0).double() * prenet_scale(prenet_rate, masks.get('prenet' + name[-1]))
+        ref, bound = z * k, k * b_z + U * (z * k).abs()
+        if fill:
+            v[name].copy_(ref.float())
+        rep.add(name, 0, (v[name].double() - ref).abs(), bound)
+        a = ra(v[name], mode)
     return rep
 
 
 def closing_products(v, prm, memory, align, mode):
-    """fp64 products of the saved histories that form each parameter gradient and d memory (decoder_bwd.cu:850-908, :1210-1239).
+    """fp64 products of the saved histories that form each parameter gradient but the attention parameters' (AttentionReverse.
+    param_grads), and d memory (decoder_bwd.cu:850-908, :1310-1350).
     -> [(name, column slice or None, reference [rows, cols], bound)].  Bound: (T B + 2) 2^-24 |A|^T |B| of each product."""
     T, B, D, M, L, A = _dims(v)
     P = v['p1'].shape[2]
@@ -660,8 +882,9 @@ def closing_products(v, prm, memory, align, mode):
     prod('att_w_hh', dga, h_att[:T])                                 # aib rows 0..T-1
     prod('att_w_ih', dga, ctx[:T], slice(P, P + M))
     prod('att_w_ih', dga, ra(v['p1'], mode), slice(0, P))
-    prod('frame_w', dfs[..., :-1], torch.cat([h_gen[1:], ctx[1:]], -1))
-    prod('stop_w', dfs[..., -1:], torch.cat([h_gen[1:], ctx[1:]], -1))
+    RN = dfs.shape[-1] - frames_per_step(prm)                       # dfs columns: R frames of N, then the R stop logits
+    prod('frame_w', dfs[..., :RN], torch.cat([h_gen[1:], ctx[1:]], -1))
+    prod('stop_w', dfs[..., RN:], torch.cat([h_gen[1:], ctx[1:]], -1))
     prod('attn_query', dq, h_att[1:])
     prod('attn_memory', ra(v['dmemT'], mode), ra(memory, mode))
     colsum('gen_b_ih', v['dgg'].double())
@@ -669,8 +892,13 @@ def closing_products(v, prm, memory, align, mode):
     colsum('att_b_ih', v['dga'].double())
     colsum('att_b_hh', v['dga'].double())
     colsum('attn_bias', v['dq'].double())
-    colsum('frame_b', v['dfs'][..., :-1].double())
-    colsum('stop_b', v['dfs'][..., -1:].double())
+    colsum('frame_b', v['dfs'][..., :RN].double())
+    colsum('stop_b', v['dfs'][..., RN:].double())
+    # prenet: dp1^T . p0, dp0^T . xtm and the column sums of dp1, dp0 (decoder_bwd.cu:1344-1349)
+    prod('prenet_w1', ra(v['dp1'], mode), ra(v['p0'], mode))
+    colsum('prenet_b1', v['dp1'].double())
+    prod('prenet_w0', ra(v['dp0'], mode), ra(v['xtm'], mode))
+    colsum('prenet_b0', v['dp0'].double())
     # d memory = align^T . dctx (per utterance) + dmemT . Wm
     alr, dct = ra(align, mode), ra(v['dctxt'].transpose(0, 1), mode)   # [B, T, L], [B, T, M]
     dmr, wmr = ra(v['dmemT'], mode), ra(prm['attn_memory'], mode)
@@ -697,11 +925,11 @@ def check_closing(v, prm, grads, memory, align, mode, report=None):
     return rep
 
 
-def closing_grads(v, prm, memory, align, mode):
-    """gradients equal to the closing products (synthetic workspaces)"""
-    T, B, D, M, L, A = _dims(v)
-    grads = {k: torch.zeros_like(t) for k, t in prm.items()}
-    grads['memory'] = torch.zeros_like(memory)
+def closing_grads(v, prm, memory, align, mode, grads=None):
+    """gradients equal to the closing products (synthetic workspaces), written into `grads` when given"""
+    if grads is None:
+        grads = {k: torch.zeros_like(t) for k, t in prm.items()}
+        grads['memory'] = torch.zeros_like(memory)
     for name, sl, ref, _ in closing_products(v, prm, memory, align, mode):
         if name == 'memory':
             grads[name].copy_(ref.reshape(memory.shape).float())
@@ -714,15 +942,19 @@ def closing_grads(v, prm, memory, align, mode):
 # synthetic workspace (CPU tests): an fp64 trajectory with the same rounding points, stored in the same views
 # ------------------------------------------------------------------------------------------------------------------------
 class Config:
-    def __init__(self, kind, training, rate_h, rate_c):
+    def __init__(self, kind, training, rate_h, rate_c, prenet_rate=0.5):
         self.kind, self.training, self.rate_h, self.rate_c = int(kind), bool(training), float(rate_h), float(rate_c)
+        self.prenet_rate = float(prenet_rate)
 
 
-def synthetic(B=34, L=20, T=6, D=64, M=64, P=32, A=16, C=4, K=5, N=8, kind=1, training=True, mode='persist', seed=0,
-              kernel_masks=None, lose_dcum_carry_at=None):
-    """-> (views, params, masks, cfg, lengths, memory, align, aux).  kernel_masks: masks the trajectory uses instead of the returned
-    ones; lose_dcum_carry_at: the reverse trajectory drops the d cum carry on entry to that step.  aux: d alignments and the parameter
-    gradients (the closing products)."""
+def synthetic(B=34, L=20, T=6, D=64, M=64, P=32, A=16, C=4, K=5, N=8, R=1, kind=1, training=True, mode='persist', seed=0,
+              kernel_masks=None, lose_dcum_carry_at=None, faults=(), min_length=1):
+    """-> (views, params, masks, cfg, lengths, memory, align, aux).  T decoder steps of R frames; the target has T R frames at R = 1
+    and T R - 1 at R > 1, so that the last step's last frame is not emitted.  kernel_masks: masks the trajectory uses instead of the
+    returned ones; lose_dcum_carry_at: the reverse trajectory drops the d cum carry on entry to that step.  faults: mistakes built into
+    the trajectory, 'teacher_frame' (step i fed frame i R instead of i R - 1) and 'dfs_past_T' (a non-zero gradient in the frame slot
+    past the last frame).  min_length: the shortest text length (one utterance has it, one has L).  aux: d alignments, the parameter gradients (the closing products), the target, the emitted frames and
+    stop logits and their gradients."""
     g = torch.Generator().manual_seed(seed)
     r = lambda *s, scale=1.0: (torch.randn(*s, generator=g, dtype=torch.float64) * scale).float()   # noqa: E731
     prm = {'prenet_w0': r(P, N, scale=N ** -0.5), 'prenet_b0': r(P, scale=0.1), 'prenet_w1': r(P, P, scale=P ** -0.5),
@@ -731,25 +963,28 @@ def synthetic(B=34, L=20, T=6, D=64, M=64, P=32, A=16, C=4, K=5, N=8, kind=1, tr
            'gen_w_hh': r(4 * D, D, scale=D ** -0.5), 'gen_b_ih': r(4 * D, scale=0.1), 'gen_b_hh': r(4 * D, scale=0.1),
            'attn_query': r(A, D, scale=3 * D ** -0.5), 'attn_memory': r(A, M, scale=3 * M ** -0.5),
            'attn_location': r(A, C, scale=C ** -0.5), 'attn_loc_features': r(C, 1, K, scale=K ** -0.5), 'attn_bias': r(1, A, scale=0.1),
-           'attn_energy': r(1, A, scale=6 * A ** -0.5), 'frame_w': r(N, D + M, scale=(D + M) ** -0.5), 'frame_b': r(N, scale=0.1),
-           'stop_w': r(1, D + M, scale=(D + M) ** -0.5), 'stop_b': r(1, scale=0.1)}
-    lengths = torch.randint(1, L + 1, (B,), generator=g)
-    lengths[0], lengths[1] = L, 1
+           'attn_energy': r(1, A, scale=6 * A ** -0.5), 'frame_w': r(R * N, D + M, scale=(D + M) ** -0.5),
+           'frame_b': r(R * N, scale=0.1), 'stop_w': r(R, D + M, scale=(D + M) ** -0.5), 'stop_b': r(R, scale=0.1)}
+    lengths = torch.randint(min_length, L + 1, (B,), generator=g)
+    lengths[0], lengths[1] = L, min_length
     memory = r(B, L, M)
     cfg = Config(kind, training, 0.1, 0.1 if kind == 1 else 0.0)
     masks = {k: (torch.rand(T, B, D, generator=g) >= 0.1).to(torch.uint8) for k in ('att_h', 'att_c', 'gen_h', 'gen_c')}
+    masks.update({k: (torch.rand(T, B, P, generator=g) >= 0.5).to(torch.uint8) for k in ('prenet0', 'prenet1')})
     km = kernel_masks or masks
+    Tf = T * R - (1 if R > 1 else 0)
+    target = r(B, N, Tf)
     kmask = lambda k, i: km[k][i:i + 1] if training else None     # noqa: E731
     Kp_att, Kp_gen = -(-(D + M) // 64) * 64, -(-D // 64) * 64
     z = lambda *s: torch.zeros(*s, dtype=torch.float32)          # noqa: E731
     v = {'ai': z(T + 1, B, M + D), 'ca': z(T + 1, B, D), 'hg': z(T + 1, B, D), 'cg': z(T + 1, B, D), 'ga': z(T, B, 4 * D),
-         'gg': z(T, B, 4 * D), 'q': z(T, B, A), 'cum': z(T + 1, B, L), 'fs': z(T, B, N + 1),
-         'p1': (torch.relu(r(T, B, P)) * 2), 'memT': (rn(memory) @ rn(prm['attn_memory']).t()).float(),
+         'gg': z(T, B, 4 * D), 'q': z(T, B, A), 'cum': z(T + 1, B, L), 'fs': z(T, B, R * (N + 1)),
+         'xtm': z(T, B, N), 'p0': z(T, B, P), 'p1': z(T, B, P), 'memT': (rn(memory) @ rn(prm['attn_memory']).t()).float(),
          'aib': z(T + 1, B, Kp_att).to(torch.bfloat16), 'hgb': z(T + 1, B, Kp_gen).to(torch.bfloat16),
-         'dfs': r(T, B, N + 1, scale=0.1), 'dhgd': r(T, B, D, scale=0.1), 'dctxs': r(T, B, M, scale=0.1), 'dgg': z(T, B, 4 * D),
+         'dfs': z(T, B, R * (N + 1)), 'dhgd': z(T, B, D), 'dctxs': z(T, B, M), 'dgg': z(T, B, 4 * D),
          'dhas': r(T, B, D, scale=0.1),
          'dga': z(T, B, 4 * D), 'dq': r(T, B, A, scale=0.1), 'dctxt': z(T, B, M), 'dmemT': z(B, L, A),
-         'dggb': z(T, B, 4 * D).to(torch.bfloat16), 'dgab': z(T, B, 4 * D).to(torch.bfloat16)}
+         'dggb': z(T, B, 4 * D).to(torch.bfloat16), 'dgab': z(T, B, 4 * D).to(torch.bfloat16), 'dp1': z(T, B, P), 'dp0': z(T, B, P)}
     if mode != 'persist':
         for k in ('aib', 'hgb', 'dggb', 'dgab'):
             del v[k]
@@ -759,6 +994,15 @@ def synthetic(B=34, L=20, T=6, D=64, M=64, P=32, A=16, C=4, K=5, N=8, kind=1, tr
     wcomb = wcomb_fp32(prm['attn_location'], prm['attn_loc_features'])
     wfs = torch.cat([prm['frame_w'], prm['stop_w']], 0)
     bfs = torch.cat([prm['frame_b'], prm['stop_b']]).double()
+    x = teacher_frames(target, T, R)
+    if 'teacher_frame' in faults:
+        x[1:] = target[:, :, R:T * R:R].permute(2, 0, 1).double()
+    v['xtm'].copy_(x.float())
+    y = v['xtm']
+    for k in range(2):
+        keep = km[f'prenet{k}']
+        y = prenet_layer(y, prm[f'prenet_w{k}'], prm[f'prenet_b{k}'], keep, prenet_scale(cfg.prenet_rate, keep), mode)[0].float()
+        v[f'p{k}'].copy_(y)
     for i in range(T):
         zz, _ = att_preact(v, prm, att_operand(v, i, i + 1, mode), i, i + 1, mode)
         v['ga'][i] = activate(zz, mode)[0][0].float()
@@ -783,10 +1027,25 @@ def synthetic(B=34, L=20, T=6, D=64, M=64, P=32, A=16, C=4, K=5, N=8, kind=1, tr
             v['hgb'][i + 1, :, :D] = v['hg'][i + 1].to(torch.bfloat16)
         x = torch.cat([gen_operand(v, i + 1, i + 2, mode), a_in[..., D:]], -1)
         v['fs'][i] = (x @ rw(wfs, mode).t() + bfs)[0].float()
+    spec, stop = (t.float() for t in split_frames(v['fs'], Tf, R))
+    dspec, dstop = r(B, Tf, N, scale=0.1), r(B, Tf, scale=0.1)
     dalign = r(B, T, L, scale=0.1)
+    check_frames_backward(v, prm, dspec, dstop, Tf, mode, fill=True)
+    if 'dfs_past_T' in faults:
+        assert R > 1
+        v['dfs'][T - 1, 0, (R - 1) * N] = 0.05                            # frame T R - 1 = Tf of the last step
+        check_frames_backward(v, prm, dspec, dstop, Tf, mode, fill=True, keep_dfs=True)
+    # the generator reverse loop, then its input gradient onto the static d ctx, which the attention reverse loop reads
+    mg = [km[k] if training else None for k in ('gen_h', 'gen_c')]
+    _reverse(v, cfg, mode, Report(T), 'dgg', 'dgg', 'dggb', 'gg', 'cg', 'dhgd', None, prm['gen_w_hh'], *mg, fill=True)
+    check_frames_backward(v, prm, dspec, dstop, Tf, mode, fill=True, keep_dfs=True)
+    grads = {k: torch.zeros_like(t) for k, t in prm.items()}
+    grads['memory'] = torch.zeros_like(memory)
     check_reverse(v, prm, {k: km[k] for k in km}, cfg, mode, fill=True, attention=(lengths, memory, align, dalign),
-                  lose_carry_at=lose_dcum_carry_at)
-    aux = {'dalign': dalign, 'grads': closing_grads(v, prm, memory, align, mode)}
+                  lose_carry_at=lose_dcum_carry_at, grads=grads)
+    check_prenet_backward(v, prm, km, cfg.prenet_rate, mode, fill=True)
+    aux = {'dalign': dalign, 'grads': closing_grads(v, prm, memory, align, mode, grads), 'target': target, 'spec': spec, 'stop': stop,
+           'dspec': dspec, 'dstop': dstop}
     return v, prm, masks, cfg, lengths, memory, align, aux
 
 
@@ -802,15 +1061,22 @@ GPU_SHAPES = [
 
 
 def check_all(v, prm, masks, cfg, lengths, memory, align, aux, mode):
-    """Forward, reverse (with the attention backward: aux['dalign'] is the d alignments of the decode, None for none) and, when
-    aux['grads'] is given, the closing products.  mode: one for the whole decode, or (forward, generator reverse, attention reverse)
+    """Forward, reverse (with the attention backward: aux['dalign'] is the d alignments of the decode, None for none), the prenet
+    backward and, when aux['grads'] is given, the attention-parameter gradients and the closing products.  With aux['target'] (the
+    decode's target [B, N, T]), aux['spec'] / aux['stop'] (its outputs) and aux['dspec'] / aux['dstop'] (their gradients, None for
+    none) also the frame edges: prenet input and layers, frame split and gather.
+    mode: one for the whole decode, or (forward, generator reverse, attention reverse)
     (modes_of).  The closing products read the forward's operand rows, so they take the forward's mode; a persistent generator reverse
     loop's bf16 history, which they read in place, is the RN of its fp32 gate gradients (stage dggb_rn), exactly what the chains' operand
     packing would read."""
     fwd, gen, att = modes_of(mode)
     assert not (fwd == 'persist' and att != 'persist'), 'the persistent forward loops run in training only with the attention reverse loop'
     rep = check_forward(v, prm, masks, cfg, lengths, memory, align, fwd)
-    check_reverse(v, prm, masks, cfg, (gen, att), rep, attention=(lengths, memory, align, aux.get('dalign')))
+    if aux.get('target') is not None:
+        check_frames_forward(v, prm, masks, cfg.prenet_rate, aux['target'], aux['spec'], aux['stop'], fwd, rep)
+        check_frames_backward(v, prm, aux.get('dspec'), aux.get('dstop'), aux['target'].shape[2], fwd, rep, gen_mode=gen)
+    check_reverse(v, prm, masks, cfg, (gen, att), rep, attention=(lengths, memory, align, aux.get('dalign')), grads=aux.get('grads'))
+    check_prenet_backward(v, prm, masks, cfg.prenet_rate, att, rep)
     if aux.get('grads') is not None:
         check_closing(v, prm, aux['grads'], memory, align, fwd, rep)
     return rep

@@ -1,5 +1,7 @@
 """Every step of the persistent decoder loops against an fp64 step computed from the loop's own saved state (tests/step_check.py),
-and bit-reproducibility of a bf16 training decode.  Run with -s to see the worst err / bound ratio of every stage."""
+with the frame edges around them (prenet input and layers, frame split and gather, prenet backward) and every parameter gradient,
+at 1, 2 and 3 frames per step; and bit-reproducibility of a bf16 training decode.  Run with -s to see the worst err / bound ratio
+of every stage."""
 import time
 
 import pytest
@@ -7,6 +9,7 @@ import torch
 
 import decoder_cases
 import decoder_workspace
+import outputs_per_step_oracle as R
 import persist_geometry as G
 import step_check as S
 from multilingual_text_to_speech_b200._lib import DECODER_PARAM_FIELDS
@@ -14,18 +17,22 @@ from multilingual_text_to_speech_b200._lib import DECODER_PARAM_FIELDS
 pytestmark = pytest.mark.gpu
 
 
-def _decode(B, L, T, M, D, kind='zoneout', precision='bf16', seed=0, backward=True, training=True, keep_views=True):
-    """One teacher-forced decode (ragged lengths including a length-1 utterance, dropout / zoneout masks in training), forward and
-    (training) backward with random output gradients.  -> dict: shape, views (keep_views), params, cfg, lengths, memory, align, dalign,
-    outputs, grads"""
+def _decode(B, L, T, M, D, kind='zoneout', precision='bf16', seed=0, backward=True, training=True, keep_views=True, r=1):
+    """One teacher-forced decode of T steps (ragged lengths including a length-1 utterance, dropout / zoneout masks in training),
+    forward and (training) backward with random output gradients.  r > 1: r frames per step with untied random projections and a
+    target of T r - 1 frames, so that the last step's last frame is not emitted.  -> dict: shape, views (keep_views), params, cfg,
+    lengths, memory, target, align, dalign, dspec, dstop, outputs, grads"""
     from multilingual_text_to_speech_b200 import functional as F, _lib
     c = decoder_cases.full_dim_case(B=B, L=L, T=T, M=M, D=D, kind=kind, seed=seed, ragged=True, training=training)
+    if r > 1:
+        c = R.untie(c, r, T * r - 1, seed)
     if B > 1:
         c.lengths[-1] = 1
     dev = torch.device('cuda:0')
-    cfg, params, memory = decoder_cases._cuda_inputs(c, dev)
+    cfg, params, memory = decoder_cases._cuda_inputs(c, dev, r)
     lengths, target = c.lengths.to(dev), c.target.to(dev)
-    out = {'cfg': cfg, 'params': params, 'lengths': lengths, 'memory': memory, 'dalign': None, 'grads': None, 'views': None}
+    out = {'cfg': cfg, 'params': params, 'lengths': lengths, 'memory': memory, 'target': target, 'dalign': None, 'dspec': None,
+           'dstop': None, 'grads': None, 'views': None}
     _lib.set_precision(precision)
     F.PROFILE['keep_ws'] = keep_views
     try:
@@ -35,7 +42,7 @@ def _decode(B, L, T, M, D, kind='zoneout', precision='bf16', seed=0, backward=Tr
             d_spec, d_stop = torch.randn(spec.shape, generator=g, device=dev), torch.randn(stop.shape, generator=g, device=dev)
             d_align = torch.randn(align.shape, generator=g, device=dev)
             ((spec * d_spec).sum() + (stop * d_stop).sum() + (align * d_align).sum()).backward()
-            out['dalign'] = d_align
+            out['dalign'], out['dspec'], out['dstop'] = d_align, d_spec, d_stop
             out['grads'] = dict(zip(DECODER_PARAM_FIELDS, [p.grad for p in params]))
             out['grads']['memory'] = memory.grad
         torch.cuda.synchronize()
@@ -73,27 +80,42 @@ def _mode_of(dims):
     return _mode(_lib.DecoderShape(B, L, T, M, D, 256, 128, 32, 31, 80, _lib.CELL_ZONEOUT, 1, 0.1, 0.1, 0.5), 'bf16')
 
 
-def _step_check(B, L, T, M, D, kind='zoneout', precision='bf16', expect_mode=None, training=True, key=None):
-    """key: the loop geometry key (persist_geometry.py) the shape must still have"""
+# every stage a training step reports in every mode; persist adds the checks of its bf16 operand rows and histories
+TRAIN_STAGES = {'ga', 'c_att', 'h_att', 'q', 'align', 'align_pad', 'ctx', 'cum', 'gg', 'c_gen', 'h_gen', 'fs', 'xtm', 'p0', 'p1', 'spec',
+                'stop', 'dfs', 'dhgd', 'dctxs', 'dgg', 'dga', 'dctxt', 'dq', 'dmemT', 'dp1', 'dp0', 'memory'} | set(DECODER_PARAM_FIELDS)
+
+
+def _step_check(B, L, T, M, D, kind='zoneout', precision='bf16', expect_mode=None, training=True, key=None, r=1):
+    """key: the loop geometry key (persist_geometry.py) the shape must still have.  T: decoder steps (of r frames)."""
     if key is not None:
         assert G.key_of(B, L, M, D, training) == key, (G.key_of(B, L, M, D, training), key)
     t0 = time.perf_counter()
-    r = _decode(B, L, T, M, D, kind, precision, backward=training, training=training)
-    mode = _mode(r['shape'], precision)
+    res = _decode(B, L, T, M, D, kind, precision, backward=training, training=training, r=r)
+    mode = _mode(res['shape'], precision)
     if expect_mode:
         assert mode == expect_mode, (mode, expect_mode)
-    v, cfg = r['views'], r['cfg']
-    prm = {f: p.detach() for f, p in zip(DECODER_PARAM_FIELDS, r['params'])}
-    scfg = S.Config(cfg.cell_kind, cfg.training, cfg.rate_h, cfg.rate_c)
-    memory = r['memory'].detach()
+    assert res['shape'].R == r and res['views']['fs'].shape[0] == T, (res['shape'].R, tuple(res['views']['fs'].shape))
+    v, cfg = res['views'], res['cfg']
+    prm = {f: p.detach() for f, p in zip(DECODER_PARAM_FIELDS, res['params'])}
+    scfg = S.Config(cfg.cell_kind, cfg.training, cfg.rate_h, cfg.rate_c, cfg.prenet_rate)
+    memory = res['memory'].detach()
+    spec, stop, _ = res['outputs']
+    t1 = time.perf_counter()
     if training:
-        rep = S.check_all(v, prm, cfg.masks, scfg, r['lengths'], memory, r['align'], {'dalign': r['dalign'], 'grads': r['grads']}, mode)
+        aux = {'dalign': res['dalign'], 'grads': res['grads'], 'target': res['target'], 'spec': spec, 'stop': stop,
+               'dspec': res['dspec'], 'dstop': res['dstop']}
+        rep = S.check_all(v, prm, cfg.masks, scfg, res['lengths'], memory, res['align'], aux, mode)
+        stages = {s.split('[')[0] for s in rep.worst}
+        assert TRAIN_STAGES <= stages, TRAIN_STAGES - stages
     else:
-        rep = S.check_forward(v, prm, cfg.masks, scfg, r['lengths'], memory, r['align'], mode)
-    title = f'[B{B} L{L} T{T} M{M} D{D} {kind} {"train" if training else "eval"} {precision} {mode}] '
+        rep = S.check_forward(v, prm, cfg.masks, scfg, res['lengths'], memory, res['align'], mode)
+        S.check_frames_forward(v, prm, cfg.masks, cfg.prenet_rate, res['target'], spec, stop, mode, rep)
+        assert {'xtm', 'p0', 'p1', 'spec', 'stop'} <= set(rep.worst)
+    title = f'[B{B} L{L} T{T} r{r} M{M} D{D} {kind} {"train" if training else "eval"} {precision} {mode}] '
     print()
     print('\n'.join(rep.lines(title)))
-    print(f'{title}key {key}: worst err/bound {rep.max_ratio():.3e} over {len(rep.worst)} stages, {time.perf_counter() - t0:.1f} s')
+    print(f'{title}key {key}: worst err/bound {rep.max_ratio():.3e} over {len(rep.worst)} stages, decode {t1 - t0:.1f} s, '
+          f'check {time.perf_counter() - t1:.1f} s')
     assert rep.failures() == {}, (title, rep.failures())
     return rep
 
@@ -157,6 +179,23 @@ def test_step_checker_on_the_fp32_per_step_chains_two_attention_chunks():
 
 def test_step_checker_on_the_bf16_per_step_chains_d1280():
     _step_check(8, 60, 10, 288, 1280, 'zoneout', expect_mode='chain_bf16')
+
+
+# ---- several frames per step (hp.outputs_per_step): T r - 1 frames, the last step's last frame not emitted ----
+
+@pytest.mark.parametrize('r', (2, 3))
+@pytest.mark.parametrize('kind', ('zoneout', 'dropout'))
+@pytest.mark.parametrize('training', (True, False), ids=('train', 'eval'))
+def test_persistent_loop_steps_within_bounds_frames_per_step(r, kind, training):
+    _step_check(33, 47, 8, 288, 1024, kind, expect_mode='persist', training=training, r=r)
+
+
+def test_step_checker_on_the_fp32_per_step_chains_r2():
+    _step_check(8, 40, 12, 288, 1024, 'zoneout', precision='fp32', expect_mode='fp32', r=2)
+
+
+def test_step_checker_on_the_bf16_per_step_chains_d1280_r3():
+    _step_check(8, 60, 10, 288, 1280, 'dropout', expect_mode='chain_bf16', r=3)
 
 
 @pytest.mark.parametrize('shape', [(60, 180, 900, 288, 1024), (64, 300, 400, 288, 1024)], ids=('benchmark', 'B64_L300'))

@@ -1,8 +1,9 @@
 """The step-local fp64 checker (tests/step_check.py) on synthetic workspaces, without a GPU.
 
 A synthetic workspace is an fp64 trajectory with the kernels' rounding points, stored in the decoder's view layout.  The checker
-must pass on it in every rounding mode, cell kind and train / eval, and must flag each of a set of small kernel-style mistakes at
-the step and stage where it was made.  Also: the GPU step-check shape list covers the edges the wgmma loops accept.
+must pass on it in every rounding mode, cell kind and train / eval and at 1, 2 and 3 frames per step, must check every parameter
+gradient, and must flag each of a set of small kernel-style mistakes at the step and stage where it was made.  Also: the GPU
+step-check shape list covers the edges the wgmma loops accept, and the workspace views follow the library's layout.
 """
 import ctypes
 
@@ -20,6 +21,17 @@ def _check(v, prm, masks, cfg, lengths, memory, align, aux, mode='persist'):
     return S.check_all(v, prm, masks, cfg, lengths, memory, align, aux, mode)
 
 
+def _expected_stages(mode):
+    out = {'ga', 'c_att', 'h_att', 'q', 'align', 'align_pad', 'ctx', 'cum', 'gg', 'c_gen', 'h_gen', 'fs', 'dgg', 'dga',
+           'dctxt', 'dq', 'dmemT', 'gen_w_hh', 'gen_w_ih', 'att_w_hh', 'att_w_ih[0:32]', 'att_w_ih[32:96]', 'frame_w', 'stop_w',
+           'attn_query', 'attn_memory', 'gen_b_ih', 'gen_b_hh', 'att_b_ih', 'att_b_hh', 'attn_bias', 'frame_b', 'stop_b', 'memory',
+           'xtm', 'p0', 'p1', 'spec', 'stop', 'dfs', 'dhgd', 'dctxs', 'dp1', 'dp0', 'prenet_w1', 'prenet_b1', 'prenet_w0', 'prenet_b0',
+           'attn_energy', 'attn_location', 'attn_loc_features'}
+    if mode == 'persist':
+        out |= {'aib_rn', 'hgb_rn', 'aib_row0', 'hgb_row0', 'dggb_rn', 'dgab_rn'}
+    return out
+
+
 @pytest.mark.parametrize('mode', S.MODES)
 @pytest.mark.parametrize('kind', (0, 1))
 @pytest.mark.parametrize('training', (True, False))
@@ -27,12 +39,33 @@ def test_checker_passes_on_a_consistent_trajectory(mode, kind, training):
     args = _synthetic(kind=kind, training=training, mode=mode)
     rep = _check(*args, mode=mode)
     assert rep.failures() == {}, '\n'.join(rep.lines())
-    expected = {'ga', 'c_att', 'h_att', 'q', 'align', 'align_pad', 'ctx', 'cum', 'gg', 'c_gen', 'h_gen', 'fs', 'dgg', 'dga',
-                'dctxt', 'dq', 'dmemT', 'gen_w_hh', 'gen_w_ih', 'att_w_hh', 'att_w_ih[0:32]', 'att_w_ih[32:96]', 'frame_w', 'stop_w',
-                'attn_query', 'attn_memory', 'gen_b_ih', 'gen_b_hh', 'att_b_ih', 'att_b_hh', 'attn_bias', 'frame_b', 'stop_b', 'memory'}
-    if mode == 'persist':
-        expected |= {'aib_rn', 'hgb_rn', 'aib_row0', 'hgb_row0', 'dggb_rn', 'dgab_rn'}
-    assert set(rep.worst) == expected
+    assert set(rep.worst) == _expected_stages(mode)
+
+
+@pytest.mark.parametrize('mode', S.MODES)
+@pytest.mark.parametrize('R', (2, 3))
+def test_checker_passes_at_several_frames_per_step(mode, R):
+    """R frames per step, the last step's last frame not emitted: the views carry S rows, fs / dfs are R (N + 1) wide"""
+    v, prm, masks, cfg, lengths, memory, align, aux = args = _synthetic(R=R, mode=mode, T=5)
+    N = prm['frame_w'].shape[0] // R
+    assert v['fs'].shape == v['dfs'].shape == (5, 34, R * (N + 1)) and v['xtm'].shape == (5, 34, N)
+    assert aux['target'].shape[2] == aux['spec'].shape[1] == 5 * R - 1
+    rep = _check(*args, mode=mode)
+    assert rep.failures() == {}, '\n'.join(rep.lines())
+    assert set(rep.worst) == _expected_stages(mode)
+
+
+@pytest.mark.parametrize('mode', S.MODES)
+def test_every_parameter_gradient_has_a_closing_stage(mode):
+    """check_all checks each of the decoder's parameter gradients and d memory: a parameter added to the library without a stage
+    fails here"""
+    from multilingual_text_to_speech_b200._lib import DECODER_PARAM_FIELDS
+    assert len(DECODER_PARAM_FIELDS) == 22
+    rep = _check(*_synthetic(mode=mode, T=3), mode=mode)
+    checked = {stage.split('[')[0] for stage in rep.worst}
+    missing = (set(DECODER_PARAM_FIELDS) | {'memory'}) - checked
+    assert not missing, missing
+    assert {'att_w_ih[0:32]', 'att_w_ih[32:96]'} <= set(rep.worst)      # both column blocks of the one split gradient
 
 
 def _flags(rep, stage, step):
@@ -193,16 +226,23 @@ def test_gpu_shape_list_covers_the_accepted_edges():
 
 
 def test_view_offsets_follow_the_library_layout():
-    """the views are where the workspace sizes say they can be: every view inside its workspace, the forward views disjoint"""
+    """the views are where the workspace sizes say they can be: every view inside its workspace, the views of each workspace
+    disjoint, at R = 1, 2 and 3 frames per step with a frame count T that is a multiple of R and one that is not
+    (S = ceil(T / R) step rows)"""
     import __graft_entry__ as entry
     import decoder_workspace as W
     from multilingual_text_to_speech_b200 import _lib
     entry.build()
     lib = _lib.load()
-    for B, L, T, M, D in S.GPU_SHAPES + [(60, 180, 900, 288, 1024)]:
+    cases = [(B, L, T * R - j, M, D, R) for R in (1, 2, 3) for B, L, T, M, D in S.GPU_SHAPES + [(60, 180, 900, 288, 1024)]
+             for j in sorted({0, R - 1})]
+    for B, L, T, M, D, R in cases:
         s = _lib.DecoderShape(B, L, T, M, D, 256, 128, 32, 31, 80, 1, 1, 0.1, 0.1, 0.5)
+        s.R = R
         off = W.offsets(s)
         shapes = W.view_shapes(s, off['Kp_att'], off['Kp_gen'])
+        Sn = -(-T // R)
+        assert shapes['ga'][1][0] == Sn and shapes['fs'][1] == shapes['dfs'][1] == (Sn, B, R * 81), (T, R, shapes['fs'])
         assert off['Kp_att'] % 64 == 0 and off['Kp_att'] >= D + M and off['Kp_gen'] % 64 == 0 and off['Kp_gen'] >= D
         for group, total in ((W.FWD, lib.b200tts_decoder_workspace_bytes(ctypes.byref(s))),
                              (W.BWD, lib.b200tts_decoder_bwd_workspace_bytes(ctypes.byref(s)))):
@@ -215,3 +255,86 @@ def test_view_offsets_follow_the_library_layout():
             spans.sort()
             for (a0, a1, na), (b0, b1, nb) in zip(spans, spans[1:]):
                 assert a1 <= b0, (na, nb)
+
+
+def _only(rep, expected):
+    """the checker flags exactly these {stage: [steps]}"""
+    bad = rep.failures()
+    assert bad == expected, (bad, expected)
+
+
+def test_teacher_frame_off_by_one_is_flagged():
+    """every step i >= 1 fed target frame i R instead of i R - 1: the prenet input is off, everything after it is consistent"""
+    T, R = 5, 2
+    _only(_check(*_synthetic(R=R, T=T, faults=('teacher_frame',))), {'xtm': list(range(1, T))})
+
+
+def test_swapped_stop_slots_are_flagged():
+    """the two stop logits of one step emitted in the wrong frame order at R = 2"""
+    v, prm, masks, cfg, lengths, memory, align, aux = args = _synthetic(R=2, T=5)
+    i = 2
+    aux['stop'][:, [2 * i, 2 * i + 1]] = aux['stop'][:, [2 * i + 1, 2 * i]].clone()
+    _only(_check(*args), {'stop': [i]})
+
+
+def test_ignored_prenet_keep_bit_is_flagged():
+    """the first prenet layer keeps one unit its mask dropped"""
+    i = 3
+    v, prm, masks, *_ = _synthetic()
+    z = v['xtm'][i].double() @ S.rn(prm['prenet_w0']).t() + prm['prenet_b0'].double()
+    b, u = [int(x) for x in torch.nonzero((masks['prenet0'][i] == 0) & (z > 0.1))[0]]
+    km = {k: t.clone() for k, t in masks.items()}
+    km['prenet0'][i, b, u] = 1
+    _only(_check(*_synthetic(kernel_masks=km)), {'p0': [i]})
+
+
+def test_frame_gradient_past_the_last_frame_is_flagged():
+    """the gather writes a gradient into the frame slot past T of the last step (R = 2, T = 2 S - 1) instead of 0"""
+    T = 5
+    _only(_check(*_synthetic(R=2, T=T, faults=('dfs_past_T',))), {'dfs': [T - 1]})
+
+
+def _attention_fault(mode, drop=None, wloc_transposed=False, min_length=1):
+    """aux['grads'] of the attention parameters formed from the synthetic trajectory's own terms with one kernel-style mistake:
+    drop(step, field) -> a [B, L] mask of the positions whose terms that field's sum leaves out.  Three steps: the bounds of these
+    sums carry the d cum carry's, which widens with every reverse step (step_check.AttentionReverse)."""
+    v, prm, masks, cfg, lengths, memory, align, aux = args = _synthetic(mode=mode, L=20, T=3, min_length=min_length)
+    terms = S.attention_terms(v, prm, lengths, memory, align, aux['dalign'], mode)
+    for field in ('attn_energy', 'attn_location', 'attn_loc_features'):
+        kept = terms
+        if drop is not None:
+            kept = []
+            for i, ds, unf, de, t in terms:
+                keep = ~drop(i, field)
+                kept.append((i, ds * keep[..., None], unf, de * keep, t))
+        wloc = prm['attn_location'].reshape(prm['attn_location'].shape[1], -1).t() if wloc_transposed else None
+        aux['grads'][field].copy_(S.attention_grads_of_terms(prm, kept, mode, wloc)[field])
+    return _check(*args, mode=mode)
+
+
+@pytest.mark.parametrize('mode', S.MODES)
+def test_attention_gradients_of_the_trajectory_pass(mode):
+    """the terms the fault tests below edit sum to gradients the checker passes"""
+    _only(_attention_fault(mode), {})
+
+
+@pytest.mark.parametrize('mode', S.MODES)
+def test_dropped_partial_position_tile_is_flagged(mode):
+    """L = 20, every text 17 to 20 long: positions 16..19 (the last, partial 16-position tile of the post pass) missing from d v
+    and d Wcomb"""
+    rep = _attention_fault(mode, drop=lambda i, f: (torch.arange(20) >= 16)[None, :].expand(34, 20), min_length=17)
+    _only(rep, {'attn_energy': [0], 'attn_location': [0], 'attn_loc_features': [0]})
+
+
+@pytest.mark.parametrize('mode', S.MODES)
+def test_step_missing_from_the_location_gradients_is_flagged(mode):
+    """one decoder step's terms missing from d Wcomb (d Wloc and d Wc), d v complete"""
+    step = 1
+    rep = _attention_fault(mode, drop=lambda i, f: torch.full((34, 20), i == step and f != 'attn_energy'))
+    _only(rep, {'attn_location': [0], 'attn_loc_features': [0]})
+
+
+@pytest.mark.parametrize('mode', S.MODES)
+def test_location_feature_gradient_with_transposed_wloc_is_flagged(mode):
+    """d Wc = Wloc^T . d Wcomb read with Wloc's two indices exchanged ([C, A] storage order)"""
+    _only(_attention_fault(mode, wloc_transposed=True), {'attn_loc_features': [0]})
