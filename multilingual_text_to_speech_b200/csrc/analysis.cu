@@ -25,8 +25,6 @@ constexpr size_t DTW_SMEM_LIMIT = 227 * 1024;
 constexpr int DTW_CELL_BYTES = 3 * (sizeof(double) + sizeof(int));
 static_assert(B200TTS_DTW_MAX_FRAMES == (int)(DTW_SMEM_LIMIT / DTW_CELL_BYTES) - 1, "B200TTS_DTW_MAX_FRAMES follows from 227 KB");
 
-__device__ __forceinline__ double2 cmul_d(double2 a, double2 b) { return make_double2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
-
 // fp64 twiddles and window (fft.cuh), and the nonzero bin range [first, last] of each mel filter (first > last: an empty filter)
 __global__ void analysis_tables_kernel(int N, int win, double2* __restrict__ twM, double2* __restrict__ twN, double* __restrict__ window,
                                        int n_mels, const float* __restrict__ basis, int2* __restrict__ ranges) {
@@ -72,7 +70,7 @@ __global__ void __launch_bounds__(AN_THREADS) analysis_stft_kernel(FftPlan p, in
         const double2 x = z[f * ld + (k == M ? 0 : k)], y = z[f * ld + (k == 0 ? 0 : M - k)];
         const double2 ev = make_double2(x.x + y.x, x.y - y.y);
         const double2 od = make_double2(x.x - y.x, x.y + y.y);
-        const double2 t = cmul_d(od, sm.twN[k]);
+        const double2 t = cmul(od, sm.twN[k]);
         const float re = (float)(0.5 * (ev.x + t.y)), im = (float)(0.5 * (ev.y - t.x));     // (ev - i t) / 2, rounded to complex64
         const float a = hypotf(re, im);
         if (n_mels == 0) out[(size_t)(f0 + f) * K + k] = a;

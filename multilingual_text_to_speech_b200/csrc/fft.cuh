@@ -40,6 +40,10 @@ __device__ __forceinline__ double fft_fma(double a, double b, double c) { return
 __device__ __forceinline__ void fft_store(float2* p, double c, double s) { *p = make_float2((float)c, (float)s); }
 __device__ __forceinline__ void fft_store(double2* p, double c, double s) { *p = make_double2(c, s); }
 
+__device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
+__device__ __forceinline__ double2 cmul(double2 a, double2 b) { return make_double2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
+__device__ __forceinline__ float2 cmulc(float2 a, float2 b) { return make_float2(a.x * b.x + a.y * b.y, a.y * b.x - a.x * b.y); }   // a * conj(b)
+
 // Complex FFT of length M over `nfr` frames stored at a[f * ld ...], ping-ponging with b; returns the buffer holding the result.
 // Stage s (radix R, Ns = product of the earlier radices): output o = blk * Ns * R + j * Ns + k reads inputs jj + r * M / R with
 // jj = blk * Ns + k, weighted by W_M^(r * (k + j * Ns) * M / (Ns * R)) -- the stage twiddle and the radix-R DFT in one root (conjugated for

@@ -20,9 +20,6 @@ constexpr int FFT_THREADS = 256;
 constexpr int NNLS_WARPS = 8;
 constexpr int DEEMPH_THREADS = 1024;
 
-__device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
-__device__ __forceinline__ float2 cmulc(float2 a, float2 b) { return make_float2(a.x * b.x + a.y * b.y, a.y * b.x - a.x * b.y); }   // a * conj(b)
-
 // Sample q of the untrimmed overlap-add of utterance frames [0, F) (q in [0, N + hop * (F - 1))), divided by the window sum-square where
 // that exceeds tiny(float32) (librosa istft).  The contributing frames are added in ascending order, as librosa's overlap-add does.
 __device__ __forceinline__ float ola_sample(const float* __restrict__ frames, const float* __restrict__ window, int N, int hop, int F, int q) {

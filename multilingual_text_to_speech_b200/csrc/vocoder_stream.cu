@@ -45,9 +45,6 @@ GlLayout gl_layout(const b200tts_gl_stream_shape& s, const FftPlan& p) {
     return l;
 }
 
-__device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
-__device__ __forceinline__ float2 cmulc(float2 a, float2 b) { return make_float2(a.x * b.x + a.y * b.y, a.y * b.x - a.x * b.y); }   // a * conj(b)
-
 // sum of w^2(z - i hop) over the frames 0 <= i <= last that cover sample z of the untrimmed signal, in ascending i
 __device__ __forceinline__ float window_sumsquare(const float* __restrict__ w, int N, int hop, int z, int last) {
     const int i0 = z - N + 1 <= 0 ? 0 : (z - N + 1 + hop - 1) / hop;

@@ -533,6 +533,21 @@ def _bytes(n, device):
     return torch.empty(max(int(n), 16), dtype=torch.uint8, device=device)
 
 
+def _aligned_bytes(n, device, align=256):
+    buf = torch.empty(int(n) + align, dtype=torch.uint8, device=device)
+    off = (-buf.data_ptr()) % align
+    return buf[off:off + int(n)]
+
+
+def _workspace(bytes_fn, shape, device, alloc=_bytes):
+    """The workspace that bytes_fn (a b200tts_*_workspace_bytes entry point) sizes for `shape`, allocated by `alloc`; raises B200TTSError
+    with the library's message when bytes_fn rejects the shape."""
+    n = bytes_fn(ctypes.byref(shape))
+    if n == 0:
+        raise _lib.B200TTSError(f'{bytes_fn.__name__}: {_lib.load().b200tts_last_error().decode()}')
+    return alloc(n, device)
+
+
 class ConvBlockFunction(torch.autograd.Function):
     """pad -> grouped conv -> batch norm -> activation -> dropout (-> highway) (reference modules/layers.py:50-178).
 
@@ -902,10 +917,7 @@ def tacotron_loss(pre, post, stop, align, pre_target, post_target, stop_target, 
 # ------------------------------------------------------------------------------------------------
 def vocoder_workspace(shape, device):
     """Workspace of b200tts_griffinlim for `shape` (a _lib.VocoderShape); raises on an invalid shape."""
-    n = _lib.load().b200tts_vocoder_workspace_bytes(ctypes.byref(shape))
-    if n == 0:
-        raise _lib.B200TTSError(f'b200tts_vocoder_workspace_bytes: {_lib.load().b200tts_last_error().decode()}')
-    return _bytes(n, device)
+    return _workspace(_lib.load().b200tts_vocoder_workspace_bytes, shape, device)
 
 
 def spectrogram_magnitude(shape, log_spec, mel_basis=None, mel_pinv_t=None, nnls_step=0.0):
@@ -950,10 +962,7 @@ def gl_stream_workspace_bytes(shape):
 
 def gl_stream_workspace(shape, device):
     """A 256-byte aligned workspace of b200tts_gl_stream_run for `shape`."""
-    n = gl_stream_workspace_bytes(shape)
-    buf = torch.empty(n + 256, dtype=torch.uint8, device=device)
-    off = (-buf.data_ptr()) % 256
-    return buf[off:off + n]
+    return _aligned_bytes(gl_stream_workspace_bytes(shape), device)
 
 
 def gl_stream_reset(shape, ws, slots):
@@ -979,10 +988,7 @@ def gl_stream_run(shape, rows, S_new, wave, ws):
 # ------------------------------------------------------------------------------------------------
 def analysis_workspace(shape, device):
     """Workspace of b200tts_stft_magnitude for `shape` (a _lib.AnalysisShape); raises on an invalid shape."""
-    n = _lib.load().b200tts_analysis_workspace_bytes(ctypes.byref(shape))
-    if n == 0:
-        raise _lib.B200TTSError(f'b200tts_analysis_workspace_bytes: {_lib.load().b200tts_last_error().decode()}')
-    return _bytes(n, device)
+    return _workspace(_lib.load().b200tts_analysis_workspace_bytes, shape, device)
 
 
 def stft_magnitude(shape, wave, soff, off, mel_basis=None, workspace=None):
@@ -1062,10 +1068,7 @@ def pitch_viterbi(shape, obs, voiced_prob, off, log_trans):
     _require_cuda(obs, voiced_prob, off, log_trans)
     assert obs.dtype == torch.float64 and voiced_prob.dtype == torch.float64 and log_trans.dtype == torch.float64 and off.dtype == torch.int32
     assert tuple(log_trans.shape) == (2, shape.transition_width, shape.n_bins) and log_trans.is_contiguous()
-    n = _lib.load().b200tts_pitch_workspace_bytes(ctypes.byref(shape))
-    if n == 0:
-        raise _lib.B200TTSError(f'b200tts_pitch_workspace_bytes: {_lib.load().b200tts_last_error().decode()}')
-    ws = _bytes(n, obs.device)
+    ws = _workspace(_lib.load().b200tts_pitch_workspace_bytes, shape, obs.device)
     state = torch.empty(shape.total_frames, device=obs.device, dtype=torch.int32)
     check(_lib.load().b200tts_pitch_viterbi(ctypes.byref(shape), ptr(obs), ptr(voiced_prob), ptr(off), ptr(log_trans), ptr(state), ptr(ws),
                                             ws.numel(), _stream()), 'b200tts_pitch_viterbi')
@@ -1077,10 +1080,7 @@ def pitch_viterbi(shape, obs, voiced_prob, off, log_trans):
 # ------------------------------------------------------------------------------------------------
 def psola_workspace(shape, device):
     """The uint8 workspace of a pitch-shift batch (a _lib.PsolaShape) on `device`."""
-    n = _lib.load().b200tts_psola_workspace_bytes(ctypes.byref(shape))
-    if n == 0:
-        raise _lib.B200TTSError(f'b200tts_psola_workspace_bytes: {_lib.load().b200tts_last_error().decode()}')
-    return _bytes(n, device)
+    return _workspace(_lib.load().b200tts_psola_workspace_bytes, shape, device)
 
 
 def psola_marks(shape, wave, soff, f0, ratio, off, ws=None):
@@ -1328,13 +1328,8 @@ def wavernn_window_rows(rows, nsteps, mel, fir, aux):
 
 
 def wavernn_workspace(shape, device):
-    """Workspace of the sample loop for `shape` (a _lib.WaveRNNShape); raises on an invalid shape."""
-    n = _lib.load().b200tts_wavernn_workspace_bytes(ctypes.byref(shape))
-    if n == 0:
-        raise _lib.B200TTSError(f'b200tts_wavernn_workspace_bytes: {_lib.load().b200tts_last_error().decode()}')
-    buf = torch.empty(n + 256, dtype=torch.uint8, device=device)
-    off = (-buf.data_ptr()) % 256
-    return buf[off:off + n]
+    """256-byte aligned workspace of the sample loop for `shape` (a _lib.WaveRNNShape); raises on an invalid shape."""
+    return _workspace(_lib.load().b200tts_wavernn_workspace_bytes, shape, device, _aligned_bytes)
 
 
 def wavernn_params(weights):
@@ -1417,12 +1412,6 @@ def wavernn_unfold_streams(y, streams, base, period, hop, target, overlap, mu):
 # ------------------------------------------------------------------------------------------------
 # WaveRNN training
 # ------------------------------------------------------------------------------------------------
-def _aligned_bytes(n, device, align=256):
-    buf = torch.empty(int(n) + align, dtype=torch.uint8, device=device)
-    off = (-buf.data_ptr()) % align
-    return buf[off:off + int(n)]
-
-
 def gru_seq_shape(B, T, R):
     """_lib.GRUSeqShape; raises on a shape the loops do not take."""
     shape = _lib.GRUSeqShape(int(B), int(T), int(R))

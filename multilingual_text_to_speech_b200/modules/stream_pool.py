@@ -9,11 +9,7 @@ import numpy as np
 import torch
 
 from .. import _lib
-
-
-def cuda_device():
-    """The current CUDA device, or `cuda` when none is visible (the first device work then raises)."""
-    return torch.device('cuda', torch.cuda.current_device()) if torch.cuda.is_available() else torch.device('cuda')
+from ..utils.audio import _return_like, _work_device
 
 
 def check_preemphasis(preemphasis):
@@ -29,12 +25,6 @@ def check_seed(seed):
     if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= int(seed) < 1 << 64:
         raise ValueError(f'a seed is an int in [0, 2^64) (got {seed!r})')
     return int(seed)
-
-
-def _as_input(wave, as_numpy, on_cuda):
-    if as_numpy:
-        return wave.cpu().numpy()
-    return wave if on_cuda else wave.cpu()
 
 
 class Stream:
@@ -58,7 +48,7 @@ class VocoderStreamPool:
             raise ValueError(f'a stream pool holds 1 to {_lib.WAVERNN_MAX_STREAMS} streams (got {max_streams!r})')
         self.v, self.a = vocoder, check_preemphasis(preemphasis)
         self.rows = int(max_streams)
-        self.device = cuda_device() if device is None else device
+        self.device = _work_device() if device is None else device
         self.streams = {}
         self.next_sid = 0
 
@@ -124,7 +114,7 @@ def generate_stream(vocoder, chunks, uniforms, generator, preemphasis, target, o
     for i, chunk in enumerate(chunks):
         spec, as_numpy = vocoder._check_chunk(chunk, i)
         if pool is None:
-            fmt = (as_numpy, not as_numpy and spec.is_cuda)
+            fmt = (as_numpy, spec)
             with torch.cuda.device(spec.device) if spec.is_cuda else contextlib.nullcontext():
                 pool = vocoder.stream_pool(1, preemphasis, generator, target, overlap)
             sid = pool.open(uniforms)
@@ -132,9 +122,9 @@ def generate_stream(vocoder, chunks, uniforms, generator, preemphasis, target, o
             pool.feed(sid, spec)
             if pool.streams[sid].frames >= first_run:
                 for out in pool.drain():
-                    yield _as_input(out[sid], *fmt)
+                    yield _return_like(out[sid], *fmt)
     if pool is None:
         raise ValueError(vocoder.short_stream.format(0))
     pool.end(sid)
     for out in pool.drain():
-        yield _as_input(out[sid], *fmt)
+        yield _return_like(out[sid], *fmt)

@@ -27,7 +27,8 @@ from torch import nn
 
 from .. import _lib
 from .. import functional as F
-from .stream_pool import Stream, VocoderStreamPool, check_preemphasis, cuda_device, generate_stream as _generate_stream
+from ..utils.audio import _return_like, _work_device
+from .stream_pool import Stream, VocoderStreamPool, check_preemphasis, generate_stream as _generate_stream
 
 # fp32 bytes of the conditioning products and folded features held at once: bounds the chunk of loop steps
 COND_BYTES = 512 << 20
@@ -389,23 +390,17 @@ class WaveRNN(nn.Module):
         order.  `uniforms`: one tape per mel of tape_shape(F_i, target, overlap), values in [0, 1); by default drawn with torch.rand on the
         device (`generator` optional).  preemphasis (default 0 = off): each fold is de-emphasised, lfilter([1], [1, -preemphasis]), after
         the mu-law decode and before the cross-fade; nothing is normalised.  Every stage runs in fp32 (the library's precision mode is set to
-        fp32 for the call and restored after it), except the loop's recurrent products (bf16 operands, fp32 accumulation).  The work runs on the device of the first CUDA input, or on the current CUDA device.  numpy in -> numpy
-        out; torch in -> torch out, on that device for CUDA inputs and on the CPU for CPU inputs."""
+        fp32 for the call and restored after it), except the loop's recurrent products (bf16 operands, fp32 accumulation).  The same device and
+        numpy / torch rules as utils.audio.spectrogram_batch."""
         specs, as_numpy = self._check_mels(mels)
         frames = [int(s.shape[1]) for s in specs]
         tapes = self._check_uniforms(uniforms, frames, target, overlap)
         preemphasis = check_preemphasis(preemphasis)
-        device = next((s.device for s in specs if s.is_cuda), None) or cuda_device()
+        device = _work_device(specs)
         with _fp32_context(device):
             wave, wave_off = self._generate(specs, frames, tapes, target, overlap, generator, device, preemphasis=preemphasis)
-        out = []
-        for i, f in enumerate(frames):
-            w = wave[int(wave_off[i]): int(wave_off[i]) + (f - 1) * self.hop_length]
-            if as_numpy[i]:
-                out.append(w.cpu().numpy())
-            else:
-                out.append(w if mels[i].is_cuda else w.cpu())
-        return out
+        return [_return_like(wave[int(wave_off[i]): int(wave_off[i]) + (f - 1) * self.hop_length], as_numpy[i], specs[i])
+                for i, f in enumerate(frames)]
 
     # ---- streaming ----
     min_stream_frames = 21          # the 20-hop fade-out

@@ -91,6 +91,86 @@ def mel_tables(sr, n_fft, n_mels, device):
     return _MEL_CACHE[key]
 
 
+def _work_device(tensors=()):
+    """The device of the first CUDA tensor, else the current CUDA device (`cuda` when none is visible: the first device work then raises)."""
+    device = next((t.device for t in tensors if t.is_cuda), None)
+    if device is None:
+        device = torch.device('cuda', torch.cuda.current_device()) if torch.cuda.is_available() else torch.device('cuda')
+    return device
+
+
+def _return_like(t, as_numpy, src):
+    """Result t (on the work device) as its input src came: numpy for numpy, the tensor itself for CUDA, a CPU copy for CPU."""
+    if as_numpy:
+        return t.cpu().numpy()
+    return t if src.is_cuda else t.cpu()
+
+
+def _as_float_tensor(x, what, dims):
+    """numpy or torch -> (tensor, came as numpy); ValueError unless it is a non-empty floating array of `dims` dimensions."""
+    is_np = not isinstance(x, torch.Tensor)
+    if is_np:
+        x = np.asarray(x)
+        if not np.issubdtype(x.dtype, np.floating):
+            raise ValueError(f'{what} has dtype {x.dtype}; expected floating point')
+        x = torch.from_numpy(np.ascontiguousarray(x))
+    elif not torch.is_floating_point(x):
+        raise ValueError(f'{what} has dtype {x.dtype}; expected floating point')
+    if x.dim() != dims or x.numel() == 0:
+        raise ValueError(f'{what} has shape {tuple(x.shape)}; expected a non-empty {dims}-D array')
+    return x, is_np
+
+
+def _offsets(lengths, what, margin=0):
+    """Host int64 offsets [B + 1] of items of these lengths packed end to end.  The kernels index a batch with int32, so ValueError unless
+    the total is at most 2^31 - 1 - margin."""
+    off = np.concatenate([[0], np.cumsum(lengths)]).astype(np.int64)
+    if off[-1] > 2 ** 31 - 1 - margin:
+        raise ValueError(f'{off[-1]} {what} in one batch; at most 2^31 - 1' + (f' - {margin}' if margin else ''))
+    return off
+
+
+class _Batch:
+    """The inputs of a batch function -- waveforms [L_i] (dims 1) or spectrograms [bins, F_i] (dims 2), numpy or torch -- checked and
+    packed end to end along their last axis, under the device and numpy / torch rules spectrogram_batch states.  `finite` rejects
+    non-finite samples; `margin` is kept free below the int32 limit on the packed length."""
+
+    def __init__(self, inputs, caller, name, dims=1, finite=False, margin=0):
+        if not isinstance(inputs, (list, tuple)) or len(inputs) == 0:
+            raise ValueError(f'{caller}: {name} must be a non-empty list of {dims}-D arrays')
+        checked = [_as_float_tensor(x, f'{name}[{i}]', dims) for i, x in enumerate(inputs)]
+        self.tensors = [t for t, _ in checked]
+        self.as_numpy = [is_np for _, is_np in checked]
+        if finite:
+            for i, t in enumerate(self.tensors):
+                if not bool(torch.isfinite(t).all()):
+                    raise ValueError(f'{name}[{i}] has non-finite samples')
+        self.lengths = [int(t.shape[-1]) for t in self.tensors]
+        self.off = _offsets(self.lengths, 'samples' if dims == 1 else 'frames', margin)
+        self.device = _work_device(self.tensors)
+
+    def __len__(self):
+        return len(self.tensors)
+
+    def frame_offsets(self):
+        """Host offsets of the mel frames of a waveform batch, F_i = 1 + L_i // hop."""
+        hop = ms_to_frames(hp.stft_shift_ms)
+        return _offsets([1 + n // hop for n in self.lengths], 'frames')
+
+    def upload(self, *offsets):
+        """(the inputs packed in fp32 -- [total] or [total, bins] --, then each host offset array as int32) on the work device."""
+        packed = torch.cat([t.to(device=self.device, dtype=torch.float32).movedim(-1, 0) for t in self.tensors]).contiguous()
+        return (packed,) + tuple(torch.from_numpy(o.astype(np.int32)).to(self.device) for o in offsets)
+
+    def out(self, i, t):
+        """Result t of input i under the return rule."""
+        return _return_like(t, self.as_numpy[i], self.tensors[i])
+
+    def split(self, packed, off):
+        """packed[off[i]:off[i + 1]] of each input under the return rule."""
+        return [self.out(i, packed[off[i]:off[i + 1]]) for i in range(len(self))]
+
+
 def vocoder_shape(B, total_frames, mel):
     """The library shape of a batch under the current hp."""
     return _lib.VocoderShape(int(B), int(total_frames), int(hp.num_fft), ms_to_frames(hp.stft_shift_ms), ms_to_frames(hp.stft_window_ms),
@@ -102,59 +182,38 @@ def inverse_spectrogram_batch(spectrograms, mel=False, phases=None, generator=No
     """Log-magnitude spectrograms [bins, F_i] (already denormalised) -> one waveform per input, in input order, each of
     hop * (F_i - 1) samples.  `phases` (one [K, F_i] array of uniform draws in [0, 1) per input) sets the initial Griffin-Lim phases
     exp(2 pi i u); by default they are drawn with torch.rand on the device (`generator` optional), one draw for the whole packed batch.
-    The work runs on the device of the first CUDA input, or on the current CUDA device when no input is on one.  numpy in -> numpy out;
-    torch in -> torch out, on that device for CUDA inputs and on the CPU for CPU inputs."""
-    if not isinstance(spectrograms, (list, tuple)) or len(spectrograms) == 0:
-        raise ValueError('inverse_spectrogram_batch expects a non-empty list of [bins, frames] spectrograms')
+    The same device and numpy / torch rules as spectrogram_batch."""
     K = hp.num_fft // 2 + 1
     bins = hp.num_mels if mel else K
-    as_numpy = [not isinstance(s, torch.Tensor) for s in spectrograms]
-    specs = []
-    for i, s in enumerate(spectrograms):
-        t = torch.as_tensor(np.asarray(s) if as_numpy[i] else s)
-        if t.dim() != 2 or t.shape[0] != bins:
-            raise ValueError(f'spectrogram {i} has shape {tuple(t.shape)}; expected [{bins}, frames]')
+    b = _Batch(spectrograms, 'inverse_spectrogram_batch', 'spectrograms', dims=2)
+    for i, t in enumerate(b.tensors):
+        if t.shape[0] != bins:
+            raise ValueError(f'spectrograms[{i}] has shape {tuple(t.shape)}; expected [{bins}, frames]')
         if t.shape[1] < 2:
-            raise ValueError(f'spectrogram {i} has {t.shape[1]} frames; Griffin-Lim needs at least 2')
-        if not torch.is_floating_point(t):
-            raise ValueError(f'spectrogram {i} is not floating point')
-        specs.append(t)
-    frames = [s.shape[1] for s in specs]
+            raise ValueError(f'spectrograms[{i}] has {t.shape[1]} frames; Griffin-Lim needs at least 2')
     us = None
     if phases is not None:
-        if len(phases) != len(specs):
-            raise ValueError(f'{len(phases)} phase arrays for {len(specs)} spectrograms')
+        if len(phases) != len(b):
+            raise ValueError(f'{len(phases)} phase arrays for {len(b)} spectrograms')
         us = []
         for i, p in enumerate(phases):
             p = torch.as_tensor(np.asarray(p) if not isinstance(p, torch.Tensor) else p)
-            if tuple(p.shape) != (K, frames[i]):
-                raise ValueError(f'phases {i} has shape {tuple(p.shape)}; expected [{K}, {frames[i]}]')
+            if tuple(p.shape) != (K, b.lengths[i]):
+                raise ValueError(f'phases {i} has shape {tuple(p.shape)}; expected [{K}, {b.lengths[i]}]')
             us.append(p)
-    device = next((s.device for s in specs if s.is_cuda), None)
-    if device is None:
-        device = torch.device('cuda', torch.cuda.current_device()) if torch.cuda.is_available() else torch.device('cuda')
-    with torch.cuda.device(device):
-        wave, off_host = _vocode(specs, us, frames, mel, generator, device)
-    hop = ms_to_frames(hp.stft_shift_ms)
-    out = []
-    for i, f in enumerate(frames):
-        w = wave[hop * (int(off_host[i]) - i): hop * (int(off_host[i]) - i + f - 1)]
-        if as_numpy[i]:
-            out.append(w.cpu().numpy())
-        else:
-            out.append(w if spectrograms[i].is_cuda else w.cpu())
-    return out
+    with torch.cuda.device(b.device):
+        wave = _vocode(b, us, mel, generator)
+    # waveform i: hop (F_i - 1) samples from hop (off_i - i)
+    return b.split(wave, ms_to_frames(hp.stft_shift_ms) * (b.off - np.arange(len(b) + 1)))
 
 
-def _vocode(specs, us, frames, mel, generator, device):
-    """The library steps on `device` (the current CUDA device): packed waveform and host offsets."""
-    K = hp.num_fft // 2 + 1
-    off_host = np.concatenate([[0], np.cumsum(frames)]).astype(np.int32)
-    total = int(off_host[-1])
-    shape = vocoder_shape(len(specs), total, mel)
+def _vocode(b, us, mel, generator):
+    """The library steps on the batch's device (the current CUDA device) -> the packed waveform."""
+    K, device = hp.num_fft // 2 + 1, b.device
+    total = int(b.off[-1])
+    shape = vocoder_shape(len(b), total, mel)
     ws = F.vocoder_workspace(shape, device)
-    log_spec = torch.cat([s.to(device=device, dtype=torch.float32).t() for s in specs]).contiguous()
-    off = torch.from_numpy(off_host).to(device)
+    log_spec, off = b.upload(b.off)
     if mel:
         basis, pinv_t, step = mel_tables(hp.sample_rate, hp.num_fft, hp.num_mels, device)
         S = F.spectrogram_magnitude(shape, log_spec, basis, pinv_t, step)
@@ -166,10 +225,10 @@ def _vocode(specs, us, frames, mel, generator, device):
         u = torch.cat([p.to(device=device, dtype=torch.float64).t() for p in us])
     angles = torch.polar(torch.ones_like(u), 2 * np.pi * u).to(torch.complex64).contiguous()
     rebuilt = torch.zeros_like(angles)
-    wave = torch.empty(shape.hop * (total - len(specs)), device=device, dtype=torch.float32)
+    wave = torch.empty(shape.hop * (total - len(b)), device=device, dtype=torch.float32)
     F.griffinlim(shape, S, off, angles, rebuilt, True, int(hp.griffin_lim_iters), wave, ws)
     F.deemphasis_normalize(shape, wave, off)
-    return wave, off_host
+    return wave
 
 
 def inverse_spectrogram(s, mel=False, phases=None):
@@ -189,35 +248,6 @@ def analysis_shape(B, total_samples, total_frames, mel):
                               float(hp.preemphasis) if hp.use_preemphasis else 0.0)
 
 
-def _work_device(tensors):
-    """The device of the first CUDA tensor, else the current CUDA device."""
-    device = next((t.device for t in tensors if t.is_cuda), None)
-    if device is None:
-        device = torch.device('cuda', torch.cuda.current_device()) if torch.cuda.is_available() else torch.device('cuda')
-    return device
-
-
-def _as_float_tensor(x, what, dims):
-    """numpy or torch -> (tensor, came as numpy); ValueError unless it is a non-empty floating array of `dims` dimensions."""
-    is_np = not isinstance(x, torch.Tensor)
-    if is_np:
-        x = np.asarray(x)
-        if not np.issubdtype(x.dtype, np.floating):
-            raise ValueError(f'{what} has dtype {x.dtype}; expected floating point')
-        x = torch.from_numpy(np.ascontiguousarray(x))
-    elif not torch.is_floating_point(x):
-        raise ValueError(f'{what} has dtype {x.dtype}; expected floating point')
-    if x.dim() != dims or x.numel() == 0:
-        raise ValueError(f'{what} has shape {tuple(x.shape)}; expected a non-empty {dims}-D array')
-    return x, is_np
-
-
-def _return_like(t, is_np, src):
-    if is_np:
-        return t.cpu().numpy()
-    return t if src.is_cuda else t.cpu()
-
-
 def spectrogram_batch(waveforms, mel=False):
     """Waveforms [L_i] -> log-magnitude (mel) spectrograms [bins, F_i], F_i = 1 + L_i // hop, in input order (reference
     utils/audio.py:66-78): pre-emphasis (hp.use_preemphasis), |stft| with centre reflect padding, the mel projection when `mel`, then
@@ -225,27 +255,15 @@ def spectrogram_batch(waveforms, mel=False):
     PCM scaled by 2^-15 is exact); the transform itself runs in fp64.  The work runs on the device of the first CUDA input, or on the current
     CUDA device when no input is on one.  numpy in -> numpy out; torch in -> torch out, on that device for CUDA inputs and on the CPU for CPU
     inputs."""
-    if not isinstance(waveforms, (list, tuple)) or len(waveforms) == 0:
-        raise ValueError('spectrogram_batch expects a non-empty list of 1-D waveforms')
-    ins = [_as_float_tensor(w, f'waveform {i}', 1) for i, w in enumerate(waveforms)]
-    waves = [t for t, _ in ins]
-    hop = ms_to_frames(hp.stft_shift_ms)
-    lengths = [int(w.numel()) for w in waves]
-    frames = [1 + n // hop for n in lengths]
-    soff_host = np.concatenate([[0], np.cumsum(lengths)]).astype(np.int64)
-    off_host = np.concatenate([[0], np.cumsum(frames)]).astype(np.int64)
-    if soff_host[-1] >= 2 ** 31:
-        raise ValueError(f'{soff_host[-1]} samples in one batch; at most 2^31 - 1')
-    device = _work_device(waves)
-    with torch.cuda.device(device):
-        shape = analysis_shape(len(waves), soff_host[-1], off_host[-1], mel)
-        wave = torch.cat([w.to(device=device, dtype=torch.float32) for w in waves]).contiguous()
-        soff = torch.from_numpy(soff_host.astype(np.int32)).to(device)
-        off = torch.from_numpy(off_host.astype(np.int32)).to(device)
-        basis = mel_tables(hp.sample_rate, hp.num_fft, hp.num_mels, device)[0] if mel else None
+    b = _Batch(waveforms, 'spectrogram_batch', 'waveforms')
+    off_host = b.frame_offsets()
+    with torch.cuda.device(b.device):
+        shape = analysis_shape(len(b), b.off[-1], off_host[-1], mel)
+        wave, soff, off = b.upload(b.off, off_host)
+        basis = mel_tables(hp.sample_rate, hp.num_fft, hp.num_mels, b.device)[0] if mel else None
         S = F.stft_magnitude(shape, wave, soff, off, basis)
         F.amplitude_to_db(shape, S, off, out=S)
-    return [_return_like(S[off_host[i]:off_host[i + 1]].t().contiguous(), ins[i][1], waves[i]) for i in range(len(waves))]
+    return [b.out(i, S[off_host[i]:off_host[i + 1]].t().contiguous()) for i in range(len(b))]
 
 
 def spectrogram(y, mel=False):
@@ -258,28 +276,28 @@ def mel_spectrogram(y):
     return spectrogram(y, True)
 
 
-def _cepstra(specs, device):
-    """[n_mels, F_i] tensors -> packed cepstra [sum F, n_mfcc] on `device` and host frame offsets."""
-    off_host = np.concatenate([[0], np.cumsum([s.shape[1] for s in specs])]).astype(np.int64)
-    mel_db = torch.cat([s.to(device=device, dtype=torch.float32).t() for s in specs]).contiguous()
-    return F.mel_cepstrum(mel_db, hp.num_mfcc), off_host
+def _mel_batch(specs, caller, name):
+    """A _Batch of log-mel spectrograms [n_mels, F_i], each with at least hp.num_mfcc bands."""
+    b = _Batch(specs, caller, name, dims=2)
+    for i, t in enumerate(b.tensors):
+        if t.shape[0] < hp.num_mfcc:
+            raise ValueError(f'{name}[{i}] has {t.shape[0]} mel bands; hp.num_mfcc = {hp.num_mfcc} needs at least as many')
+    return b
 
 
-def _check_mfcc_input(S, what):
-    t, is_np = _as_float_tensor(S, what, 2)
-    if t.shape[0] < hp.num_mfcc:
-        raise ValueError(f'{what} has {t.shape[0]} mel bands; hp.num_mfcc = {hp.num_mfcc} needs at least as many')
-    return t, is_np
+def _cepstra(b):
+    """A _mel_batch -> (packed cepstra [sum F, n_mfcc], int32 frame offsets) on its device (the current CUDA device)."""
+    mel_db, off = b.upload(b.off)
+    return F.mel_cepstrum(mel_db, hp.num_mfcc), off
 
 
 def get_spectrogram_mfcc(S):
     """Compute MFCCs [hp.num_mfcc, F] of a log-mel spectrogram [n_mels, F]: librosa 0.7.0 mfcc(S=S/10), the orthonormal DCT-II over the
     mel axis, c0 included (reference utils/audio.py:117-119)."""
-    t, is_np = _check_mfcc_input(S, 'spectrogram')
-    device = _work_device([t])
-    with torch.cuda.device(device):
-        cep, _ = _cepstra([t], device)
-    return _return_like(cep.t().contiguous(), is_np, t)
+    b = _mel_batch([S], 'get_spectrogram_mfcc', 'S')
+    with torch.cuda.device(b.device):
+        cep, _ = _cepstra(b)
+    return b.out(0, cep.t().contiguous())
 
 
 def mel_cepstral_distortion_batch(S1s, S2s, mode='dtw'):
@@ -288,30 +306,26 @@ def mel_cepstral_distortion_batch(S1s, S2s, mode='dtw'):
     frames), 'stretch' (the shorter sequence indexed at i * n // m) or 'dtw'.  'dtw' is the exact dynamic-time-warping optimum, cost / path
     length; the reference calls fastdtw with radius 1, which approximates that optimum, so the two agree when fastdtw finds the optimal path
     and may differ otherwise.  Returns float64, one value per pair: a numpy array unless the first
-    input is a torch tensor (then a torch tensor on its device).  The work runs on the device of the first CUDA input, else on the current
-    device."""
-    if not isinstance(S1s, (list, tuple)) or not isinstance(S2s, (list, tuple)) or len(S1s) == 0:
-        raise ValueError('mel_cepstral_distortion_batch expects two non-empty lists of [n_mels, frames] spectrograms')
-    if len(S1s) != len(S2s):
-        raise ValueError(f'{len(S1s)} spectrograms against {len(S2s)}')
+    input is a torch tensor (then a torch tensor on its device).  The work runs on the device of the first CUDA input of either list, else
+    on the current device."""
     if mode not in _lib.MCD_MODES:
         raise ValueError(f'unknown mode {mode!r}; expected one of {sorted(_lib.MCD_MODES)}')
-    a = [_check_mfcc_input(s, f'S1s[{i}]') for i, s in enumerate(S1s)]
-    b = [_check_mfcc_input(s, f'S2s[{i}]') for i, s in enumerate(S2s)]
-    for i, ((x, _), (y, _)) in enumerate(zip(a, b)):
+    a = _mel_batch(S1s, 'mel_cepstral_distortion_batch', 'S1s')
+    b = _mel_batch(S2s, 'mel_cepstral_distortion_batch', 'S2s')
+    if len(a) != len(b):
+        raise ValueError(f'{len(a)} spectrograms against {len(b)}')
+    for i, (x, y) in enumerate(zip(a.tensors, b.tensors)):
         if x.shape[0] != y.shape[0]:
             raise ValueError(f'pair {i} has {x.shape[0]} and {y.shape[0]} mel bands')
         if mode == 'dtw' and min(x.shape[1], y.shape[1]) > _lib.DTW_MAX_FRAMES:
             raise ValueError(f'pair {i} ({x.shape[1]} x {y.shape[1]} frames): dtw keeps three anti-diagonals in shared memory, so the shorter '
                              f'sequence may have at most {_lib.DTW_MAX_FRAMES} frames')
-    xs, ys = [t for t, _ in a], [t for t, _ in b]
-    device = _work_device(xs + ys)
-    with torch.cuda.device(device):
-        cep_a, off_a = _cepstra(xs, device)
-        cep_b, off_b = _cepstra(ys, device)
-        mcd, _ = F.mel_cepstral_distortion(cep_a, torch.from_numpy(off_a.astype(np.int32)).to(device), cep_b,
-                                           torch.from_numpy(off_b.astype(np.int32)).to(device), mode)
-    return _return_like(mcd, a[0][1], xs[0])
+    a.device = b.device = _work_device(a.tensors + b.tensors)
+    with torch.cuda.device(a.device):
+        cep_a, off_a = _cepstra(a)
+        cep_b, off_b = _cepstra(b)
+        mcd, _ = F.mel_cepstral_distortion(cep_a, off_a, cep_b, off_b, mode)
+    return a.out(0, mcd)
 
 
 def mel_cepstral_distorision(S1, S2, mode):
@@ -418,50 +432,28 @@ def pitch_shape(B, total_samples, total_frames, fmin=65.406, fmax=2093.0, frame_
     return shape, log_trans, freqs
 
 
-def _pack_waveforms(waveforms, what):
-    """Checked waveforms -> (tensors, came as numpy, lengths, host sample offsets, host frame offsets) with F_i = 1 + L_i // hop."""
-    if not isinstance(waveforms, (list, tuple)) or len(waveforms) == 0:
-        raise ValueError(f'{what} expects a non-empty list of 1-D waveforms')
-    ins = [_as_float_tensor(w, f'waveform {i}', 1) for i, w in enumerate(waveforms)]
-    waves = [t for t, _ in ins]
-    hop = ms_to_frames(hp.stft_shift_ms)
-    lengths = [int(w.numel()) for w in waves]
-    soff_host = np.concatenate([[0], np.cumsum(lengths)]).astype(np.int64)
-    off_host = np.concatenate([[0], np.cumsum([1 + n // hop for n in lengths])]).astype(np.int64)
-    if soff_host[-1] >= 2 ** 31:
-        raise ValueError(f'{soff_host[-1]} samples in one batch; at most 2^31 - 1')
-    return waves, [is_np for _, is_np in ins], soff_host, off_host
-
-
 def pitch_batch(waveforms, fmin=65.406, fmax=2093.0, frame_length=1024):
     """F0 tracks of waveforms [L_i] by probabilistic YIN, as librosa 0.10's librosa.pyin(y, fmin=fmin, fmax=fmax, sr=hp.sample_rate,
     frame_length=frame_length, hop_length=hop) computes them with its other defaults (win_length = frame_length // 2, 100 thresholds,
     beta (2, 18), Boltzmann 2, 0.1 semitone bins, 35.92 octaves/s, switch probability 0.01, no-trough probability 0.01, center=True with
     zero padding), on the raw waveform (no pre-emphasis).  hop = ms_to_frames(hp.stft_shift_ms), so the frames are the mel frames:
     F_i = 1 + L_i // hop.  -> one (f0, voiced_prob) per input, each [F_i] float32: f0 in Hz, NaN on unvoiced frames.  The three stages
-    run in the library's fp64 kernels (include/b200tts.h); waveforms are rounded to fp32 first.  The work runs on the device of the first
-    CUDA input, or on the current CUDA device when no input is on one.  numpy in -> numpy out; torch in -> torch out, on that device for
-    CUDA inputs and on the CPU for CPU inputs.  Raises ValueError on a bad input, fmin <= 0, fmin >= fmax, fmax above Nyquist, more than
-    B200TTS_PITCH_MAX_BINS bins or fewer than the transition width, or a frame_length that is odd, out of range or leaves no lags."""
-    waves, as_np, soff_host, off_host = _pack_waveforms(waveforms, 'pitch_batch')
+    run in the library's fp64 kernels (include/b200tts.h); waveforms are rounded to fp32 first.  The same device and numpy / torch rules as
+    spectrogram_batch.  Raises ValueError on a bad input, fmin <= 0, fmin >= fmax, fmax above Nyquist, more than B200TTS_PITCH_MAX_BINS
+    bins or fewer than the transition width, or a frame_length that is odd, out of range or leaves no lags."""
+    b = _Batch(waveforms, 'pitch_batch', 'waveforms')
+    off_host = b.frame_offsets()
     pitch_geometry(fmin, fmax, frame_length)
-    device = _work_device(waves)
-    with torch.cuda.device(device):
-        shape, log_trans, freqs = pitch_shape(len(waves), soff_host[-1], off_host[-1], fmin, fmax, frame_length, device)
-        wave = torch.cat([w.to(device=device, dtype=torch.float32) for w in waves]).contiguous()
-        soff = torch.from_numpy(soff_host.astype(np.int32)).to(device)
-        off = torch.from_numpy(off_host.astype(np.int32)).to(device)
+    with torch.cuda.device(b.device):
+        shape, log_trans, freqs = pitch_shape(len(b), b.off[-1], off_host[-1], fmin, fmax, frame_length, b.device)
+        wave, soff, off = b.upload(b.off, off_host)
         cmnd = F.pitch_cmnd(shape, wave, soff, off)
         obs, voiced_prob = F.pitch_observations(shape, cmnd)
         state = F.pitch_viterbi(shape, obs, voiced_prob, off, log_trans).long()
         n = shape.n_bins
         f0 = torch.where(state < n, freqs[state % n], torch.full_like(freqs[:1], float('nan')))
         vp = voiced_prob.float()
-    out = []
-    for i in range(len(waves)):
-        a, b = off_host[i], off_host[i + 1]
-        out.append((_return_like(f0[a:b], as_np[i], waves[i]), _return_like(vp[a:b], as_np[i], waves[i])))
-    return out
+    return list(zip(b.split(f0, off_host), b.split(vp, off_host)))
 
 
 def pitch(y, fmin=65.406, fmax=2093.0, frame_length=1024):
@@ -473,22 +465,25 @@ def energy_batch(waveforms):
     """Frame energies of waveforms [L_i]: the L2 norm over frequency of each frame of the linear magnitude spectrogram spectrogram_batch
     computes before the dB scale (pre-emphasis per hp, |stft| with centre reflect padding), summed in fp64.  -> [F_i] float32 per input,
     F_i = 1 + L_i // hop; the same device and numpy / torch rules as spectrogram_batch."""
-    waves, as_np, soff_host, off_host = _pack_waveforms(waveforms, 'energy_batch')
-    device = _work_device(waves)
-    with torch.cuda.device(device):
-        shape = analysis_shape(len(waves), soff_host[-1], off_host[-1], False)
-        wave = torch.cat([w.to(device=device, dtype=torch.float32) for w in waves]).contiguous()
-        soff = torch.from_numpy(soff_host.astype(np.int32)).to(device)
-        off = torch.from_numpy(off_host.astype(np.int32)).to(device)
+    b = _Batch(waveforms, 'energy_batch', 'waveforms')
+    off_host = b.frame_offsets()
+    with torch.cuda.device(b.device):
+        shape = analysis_shape(len(b), b.off[-1], off_host[-1], False)
+        wave, soff, off = b.upload(b.off, off_host)
         S = F.stft_magnitude(shape, wave, soff, off)
         e = S.double().square().sum(1).sqrt().float()
-    return [_return_like(e[off_host[i]:off_host[i + 1]], as_np[i], waves[i]) for i in range(len(waves))]
+    return b.split(e, off_host)
 
 
-def _f0_track(x, what):
+def _track(x, what, frames=None, dtype=torch.float32, f0=False):
+    """A per-frame track [F] (numpy or torch) -> (host numpy array of `dtype`, came as numpy, tensor).  ValueError unless it is a
+    non-empty floating 1-D array, of `frames` frames when given, and with `f0` positive Hz on voiced frames (NaN marks unvoiced ones),
+    checked on the `dtype` values."""
     t, is_np = _as_float_tensor(x, what, 1)
-    a = t.detach().cpu().double().numpy()
-    if (a[~np.isnan(a)] <= 0).any() or np.isinf(a).any():
+    a = t.detach().cpu().to(dtype).numpy()
+    if frames is not None and len(a) != frames:
+        raise ValueError(f'{what} has {len(a)} frames; its waveform has {frames} (1 + L // hop)')
+    if f0 and ((a[~np.isnan(a)] <= 0).any() or np.isinf(a).any()):
         raise ValueError(f'{what} must be positive Hz on voiced frames (NaN marks unvoiced ones)')
     return a, is_np, t
 
@@ -503,8 +498,8 @@ def pitch_errors_batch(f0_refs, f0_gens):
         raise ValueError('pitch_errors_batch expects two non-empty lists of 1-D f0 tracks')
     if len(f0_refs) != len(f0_gens):
         raise ValueError(f'{len(f0_refs)} reference tracks against {len(f0_gens)}')
-    refs = [_f0_track(x, f'f0_refs[{i}]') for i, x in enumerate(f0_refs)]
-    gens = [_f0_track(x, f'f0_gens[{i}]') for i, x in enumerate(f0_gens)]
+    refs = [_track(x, f'f0_refs[{i}]', dtype=torch.float64, f0=True) for i, x in enumerate(f0_refs)]
+    gens = [_track(x, f'f0_gens[{i}]', dtype=torch.float64, f0=True) for i, x in enumerate(f0_gens)]
     out = {k: np.empty(len(refs)) for k in ('gpe', 'vde', 'ffe', 'f0_rmse_cents')}
     for i, ((r, _, _), (g, _, _)) in enumerate(zip(refs, gens)):
         m = min(len(r), len(g))
@@ -521,19 +516,6 @@ def pitch_errors_batch(f0_refs, f0_gens):
     if refs[0][1]:
         return out
     return {k: torch.from_numpy(v).to(refs[0][2].device) for k, v in out.items()}
-
-
-def _tracks(tracks, frames, what):
-    """One fp32 [F_i] host track per waveform, checked -> list of float32 numpy arrays."""
-    if not isinstance(tracks, (list, tuple)) or len(tracks) != len(frames):
-        raise ValueError(f'{what} must be a list of {len(frames)} tracks, one per waveform')
-    out = []
-    for i, t in enumerate(tracks):
-        a = _as_float_tensor(t, f'{what}[{i}]', 1)[0].detach().cpu().numpy().astype(np.float32)
-        if len(a) != frames[i]:
-            raise ValueError(f'{what}[{i}] has {len(a)} frames; waveform {i} has {frames[i]} (1 + L // hop)')
-        out.append(a)
-    return out
 
 
 def _check_ratios(r, what):
@@ -553,12 +535,17 @@ def pitch_shift_batch(waveforms, semitones=None, ratios=None, f0s=None, fmin=65.
     output equals the input.  Waveforms are rounded to fp32; marks and sums are fp64 in the library's kernels.  The same device and
     numpy / torch rules as spectrogram_batch.  Raises ValueError on a bad or non-finite waveform, both or neither of semitones and ratios,
     mismatched list or track lengths, an out-of-range ratio, or a non-positive or out-of-range F0."""
-    waves, as_np, soff_host, off_host = _pack_waveforms(waveforms, 'pitch_shift_batch')
-    B = len(waves)
+    b = _Batch(waveforms, 'pitch_shift_batch', 'waveforms', finite=True)
+    off_host = b.frame_offsets()
+    B = len(b)
     frames = [int(off_host[i + 1] - off_host[i]) for i in range(B)]
-    for i, w in enumerate(waves):
-        if not bool(torch.isfinite(w).all()):
-            raise ValueError(f'waveform {i} has non-finite samples')
+
+    def tracks(ts, what, f0=False):
+        """One fp32 host track [F_i] per waveform."""
+        if not isinstance(ts, (list, tuple)) or len(ts) != B:
+            raise ValueError(f'{what} must be a list of {B} tracks, one per waveform')
+        return [_track(t, f'{what}[{i}]', frames[i], f0=f0)[0] for i, t in enumerate(ts)]
+
     if (semitones is None) == (ratios is None):
         raise ValueError('give exactly one of semitones and ratios')
     if semitones is not None:
@@ -567,34 +554,26 @@ def pitch_shift_batch(waveforms, semitones=None, ratios=None, f0s=None, fmin=65.
             raise ValueError(f'{len(s)} semitone values for {B} waveforms')
         r = [np.full(f, 2.0 ** (float(v) / 12.0), dtype=np.float32) for v, f in zip(s, frames)]
     else:
-        r = _tracks(ratios, frames, 'ratios')
+        r = tracks(ratios, 'ratios')
     for i, a in enumerate(r):
         _check_ratios(a, f'the ratios of waveform {i}')
     if f0s is None:
-        f0 = [_as_float_tensor(f, 'f0', 1)[0].detach().cpu().numpy().astype(np.float32)
-              for f, _ in pitch_batch(waveforms, fmin, fmax)]
-    else:
-        f0 = _tracks(f0s, frames, 'f0s')
+        f0s = [f for f, _ in pitch_batch(waveforms, fmin, fmax)]
+    f0 = tracks(f0s, 'f0s', f0=True)
     sr, hop = hp.sample_rate, ms_to_frames(hp.stft_shift_ms)
     for i, a in enumerate(f0):
-        v = a[~np.isnan(a)].astype(np.float64)
-        if not np.isfinite(v).all() or (v <= 0).any():
-            raise ValueError(f'f0 of waveform {i} must be positive Hz on voiced frames (NaN marks unvoiced ones)')
-        p = np.rint(sr / v)
+        p = np.rint(sr / a[~np.isnan(a)].astype(np.float64))
         if ((p < 2) | (p > _lib.PSOLA_MAX_PERIOD)).any():
             raise ValueError(f'f0 of waveform {i} gives periods outside [2, {_lib.PSOLA_MAX_PERIOD}] samples: F0 must lie in about '
                              f'[{sr / (_lib.PSOLA_MAX_PERIOD + 0.5):.2f}, {sr / 1.5:.1f}] Hz')
-    device = _work_device(waves)
-    with torch.cuda.device(device):
-        shape = _lib.PsolaShape(B, int(soff_host[-1]), int(off_host[-1]), hop, hop, float(sr))
-        wave = torch.cat([w.to(device=device, dtype=torch.float32) for w in waves]).contiguous()
-        soff = torch.from_numpy(soff_host.astype(np.int32)).to(device)
-        off = torch.from_numpy(off_host.astype(np.int32)).to(device)
-        f0_d = torch.from_numpy(np.concatenate(f0)).to(device)
-        r_d = torch.from_numpy(np.concatenate(r)).to(device)
+    with torch.cuda.device(b.device):
+        shape = _lib.PsolaShape(B, int(b.off[-1]), int(off_host[-1]), hop, hop, float(sr))
+        wave, soff, off = b.upload(b.off, off_host)
+        f0_d = torch.from_numpy(np.concatenate(f0)).to(b.device)
+        r_d = torch.from_numpy(np.concatenate(r)).to(b.device)
         ws = F.psola_marks(shape, wave, soff, f0_d, r_d, off)
         y = F.psola_overlap_add(shape, wave, soff, ws)
-    return [_return_like(y[soff_host[i]:soff_host[i + 1]], as_np[i], waves[i]) for i in range(B)]
+    return b.split(y, b.off)
 
 
 def pitch_shift(y, semitones=None, ratios=None, f0=None, fmin=65.406, fmax=2093.0):
@@ -608,8 +587,8 @@ def f0_ratio(f0_target, f0_source):
     1 elsewhere, over the first min(F_target, F_source) frames and padded with 1 to F_source.  -> float32 [F_source], numpy for a numpy
     source, else a tensor on the source's device.  Raises ValueError on tracks that are not 1-D floating, or that hold a non-positive or
     infinite voiced F0."""
-    t, _, _ = _f0_track(f0_target, 'f0_target')
-    s, s_np, s_t = _f0_track(f0_source, 'f0_source')
+    t, _, _ = _track(f0_target, 'f0_target', dtype=torch.float64, f0=True)
+    s, s_np, s_t = _track(f0_source, 'f0_source', dtype=torch.float64, f0=True)
     m = min(len(t), len(s))
     out = np.ones(len(s))
     vv = ~np.isnan(t[:m]) & ~np.isnan(s[:m])
@@ -628,13 +607,6 @@ def _stretch_length(L, rate):
 
 def _retime_length(L, hop, dp):
     return max(1, hop * (int(dp.sum()) - 1) + L % hop)
-
-
-def _check_output_samples(lengths):
-    """ValueError when the outputs would not fit one int32-indexed batch; run before any warp is built."""
-    total = sum(lengths)
-    if total >= 2 ** 31:
-        raise ValueError(f'{total} output samples in one batch; at most 2^31 - 1')
 
 
 def _stretch_plan(L, hop, rate):
@@ -663,34 +635,24 @@ def _retime_plan(L, hop, d, dp):
     return Lp, hop * (lo_in + (k - lo_out) * num / den)
 
 
-def _wsola(waves, as_np, soff_host, plans):
-    """Both WSOLA kernels on the packed batch; plans: (L', warp fp64 [K]) per waveform -> the output waveforms."""
-    hop = ms_to_frames(hp.stft_shift_ms)
-    ooff_host = np.concatenate([[0], np.cumsum([Lp for Lp, _ in plans])]).astype(np.int64)
-    foff_host = np.concatenate([[0], np.cumsum([len(w) for _, w in plans])]).astype(np.int64)
-    device = _work_device(waves)
-    with torch.cuda.device(device):
-        shape = _lib.WsolaShape(len(waves), int(soff_host[-1]), int(ooff_host[-1]), int(foff_host[-1]), hop, hop)
-        wave = torch.cat([w.to(device=device, dtype=torch.float32) for w in waves]).contiguous()
-        soff, ooff, foff = (torch.from_numpy(o.astype(np.int32)).to(device) for o in (soff_host, ooff_host, foff_host))
-        warp = torch.from_numpy(np.concatenate([w for _, w in plans])).to(device)
-        positions = F.wsola_positions(shape, wave, soff, warp, foff)
-        y = F.wsola_overlap_add(shape, wave, soff, positions, foff, ooff)
-    return [_return_like(y[ooff_host[i]:ooff_host[i + 1]], as_np[i], waves[i]) for i in range(len(waves))]
-
-
-def _wsola_inputs(waveforms, what):
-    """Checked, finite waveforms packed as _pack_waveforms packs them, and the hop WSOLA uses."""
-    waves, as_np, soff_host, off_host = _pack_waveforms(waveforms, what)
-    for i, w in enumerate(waves):
-        if not bool(torch.isfinite(w).all()):
-            raise ValueError(f'waveform {i} has non-finite samples')
-    if soff_host[-1] > 2 ** 31 - 1 - _lib.WSOLA_MAX_TOLERANCE:
-        raise ValueError(f'{soff_host[-1]} samples in one batch; at most 2^31 - 1 - {_lib.WSOLA_MAX_TOLERANCE}')
+def _wsola_hop():
+    """The hop WSOLA uses: hp.stft_shift_ms in samples, which must be in [1, WSOLA_MAX_HOP]."""
     hop = ms_to_frames(hp.stft_shift_ms)
     if not 1 <= hop <= _lib.WSOLA_MAX_HOP:
         raise ValueError(f'hop {hop} (hp.stft_shift_ms) must be in [1, {_lib.WSOLA_MAX_HOP}] samples')
-    return waves, as_np, soff_host, off_host, hop
+    return hop
+
+
+def _wsola(b, hop, ooff_host, warps):
+    """Both WSOLA kernels on the packed batch b; ooff_host: host output offsets; warps: fp64 [K_i] per waveform -> the output waveforms."""
+    foff_host = _offsets([len(w) for w in warps], 'frames')
+    with torch.cuda.device(b.device):
+        shape = _lib.WsolaShape(len(b), int(b.off[-1]), int(ooff_host[-1]), int(foff_host[-1]), hop, hop)
+        wave, soff, ooff, foff = b.upload(b.off, ooff_host, foff_host)
+        warp = torch.from_numpy(np.concatenate(warps)).to(b.device)
+        positions = F.wsola_positions(shape, wave, soff, warp, foff)
+        y = F.wsola_overlap_add(shape, wave, soff, positions, foff, ooff)
+    return b.split(y, ooff_host)
 
 
 def time_stretch_batch(waveforms, rate):
@@ -702,8 +664,9 @@ def time_stretch_batch(waveforms, rate):
     exactly.  At rate 1 the output is the input.  Waveforms are rounded to fp32; the search and the sums are fp64 in the library's kernels.
     The same device and numpy / torch rules as spectrogram_batch.  Raises ValueError on a bad or non-finite waveform, a rate count that
     does not match, a rate out of range, or more than 2^31 - 1 output samples."""
-    waves, as_np, soff_host, _, hop = _wsola_inputs(waveforms, 'time_stretch_batch')
-    B = len(waves)
+    b = _Batch(waveforms, 'time_stretch_batch', 'waveforms', finite=True, margin=_lib.WSOLA_MAX_TOLERANCE)
+    hop = _wsola_hop()
+    B = len(b)
     try:
         rates = np.asarray(rate).astype(np.float64)
     except (TypeError, ValueError):
@@ -714,8 +677,8 @@ def time_stretch_batch(waveforms, rate):
     lo, hi = STRETCH_RATES
     if not np.isfinite(rates).all() or (rates < lo).any() or (rates > hi).any():
         raise ValueError(f'rate must be finite and in [{lo}, {hi}] (got {rates.tolist()})')
-    _check_output_samples([_stretch_length(len(w), float(r)) for w, r in zip(waves, rates)])
-    return _wsola(waves, as_np, soff_host, [_stretch_plan(len(w), hop, float(r)) for w, r in zip(waves, rates)])
+    ooff_host = _offsets([_stretch_length(n, float(r)) for n, r in zip(b.lengths, rates)], 'output samples')   # before any warp
+    return _wsola(b, hop, ooff_host, [_stretch_plan(n, hop, float(r))[1] for n, r in zip(b.lengths, rates)])
 
 
 def time_stretch(y, rate):
@@ -734,8 +697,10 @@ def retime_batch(waveforms, durations, new_durations):
     the slope is 1.  Frame k is then read near input sample hop phi(k) and placed as time_stretch_batch places it, so with
     new_durations = durations the output is the input.  Raises ValueError on a bad or non-finite waveform, counts that do not match,
     malformed durations, or more than 2^31 - 1 output samples."""
-    waves, as_np, soff_host, off_host, hop = _wsola_inputs(waveforms, 'retime_batch')
-    B = len(waves)
+    b = _Batch(waveforms, 'retime_batch', 'waveforms', finite=True, margin=_lib.WSOLA_MAX_TOLERANCE)
+    hop = _wsola_hop()
+    off_host = b.frame_offsets()
+    B = len(b)
     for what, t in (('durations', durations), ('new_durations', new_durations)):
         if not isinstance(t, (list, tuple)) or len(t) != B:
             raise ValueError(f'retime_batch: {what} must be a list of {B} tracks, one per waveform')
@@ -751,8 +716,8 @@ def retime_batch(waveforms, durations, new_durations):
         if int(dp.sum()) < 1:
             raise ValueError(f'retime_batch: new_durations[{i}] total 0 frames')
         tracks.append((d, dp))
-    _check_output_samples([_retime_length(len(w), hop, dp) for w, (_, dp) in zip(waves, tracks)])
-    return _wsola(waves, as_np, soff_host, [_retime_plan(len(w), hop, d, dp) for w, (d, dp) in zip(waves, tracks)])
+    ooff_host = _offsets([_retime_length(n, hop, dp) for n, (_, dp) in zip(b.lengths, tracks)], 'output samples')   # before any warp
+    return _wsola(b, hop, ooff_host, [_retime_plan(n, hop, d, dp)[1] for n, (d, dp) in zip(b.lengths, tracks)])
 
 
 def retime(y, durations, new_durations):
