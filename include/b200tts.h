@@ -776,6 +776,48 @@ int b200tts_wsola_positions(const b200tts_wsola_shape* shape, const float* wave,
 int b200tts_wsola_overlap_add(const b200tts_wsola_shape* shape, const float* wave, const int32_t* soff, const int32_t* positions,
                               const int32_t* foff, const int32_t* ooff, float* out, void* stream);
 
+/* ---- polyphase resampling: scipy.signal.resample_poly(x, up, down) with its defaults (tests/resample_oracle.py restates it) ----
+ * The packed ragged layout of the WSOLA entry points: utterance b owns input samples [soff[b], soff[b+1]) of an fp32 waveform x (L >= 1)
+ * and output samples [ooff[b], ooff[b+1]), L' = ceil(L up / down) of them.  plan int32 [B][4], 16-byte aligned, holds (up, down, h_len,
+ * table offset) per utterance, up / down the rate ratio in lowest terms, m = max(up, down) <= max_factor, h_len = 10 m.
+ *   Filter: h[j] = up w[j] / sum(w), j in [0, 2 h_len], w[j] = (1/m) sinc((j - h_len) / m) kaiser(2 h_len + 1, beta 5)[j] (scipy's
+ *   firwin(2 h_len + 1, 1 / m, window=('kaiser', 5.0))), built by the caller in fp64.
+ *   Table: taps[offset + phase T + i] = h[phase + i up] for phase in [0, up) and i in [0, T), T = ceil((2 h_len + 1) / up), 0 where
+ *   phase + i up > 2 h_len: each phase's taps are contiguous.
+ *   Output: with t = h_len + n down (64-bit), k0 = t / up and phase = t mod up,
+ *   y[n] = sum over i in [0, T) with phase + i up <= 2 h_len and k0 - i in [0, L) of x[k0 - i] taps[offset + phase T + i], that is
+ *   y[n] = sum_k x[k] h[h_len + n down - k up] over the k whose h index lies in [0, 2 h_len].  The sum is fp64, accumulated by fma in
+ *   increasing i from 0.0, and rounded to fp32 once.
+ * One thread per output sample; no workspace and no atomics, and no utterance reads another's data, so results are bit-identical in any
+ * batch.  fp64 whatever b200tts_set_precision says.  out fp32 [total_out_samples] must not alias wave or taps. */
+#define B200TTS_RESAMPLE_MAX_FACTOR 2048
+typedef struct {
+    int B, total_samples, total_out_samples;
+    int total_taps;                    /* doubles in taps: every plan's offset + up T lies within it */
+    int max_factor;                    /* the largest max(up, down) of the plan, in [1, B200TTS_RESAMPLE_MAX_FACTOR] */
+} b200tts_resample_shape;
+int b200tts_resample(const b200tts_resample_shape* shape, const float* wave, const int32_t* soff, const int32_t* ooff, const int32_t* plan,
+                     const double* taps, float* out, void* stream);
+
+/* ---- silence trimming: librosa 0.7.0 effects.trim(x, top_db, frame_length, hop_length) (tests/resample_oracle.py restates it) ----
+ * The packed ragged layout: utterance b owns samples [soff[b], soff[b+1]) of an fp32 waveform x (L >= 1, already cropped by any margin)
+ * and frames [foff[b], foff[b+1]), F = 1 + (L + 2 (W / 2) - W) / hop of them, W = frame_length.
+ *   Frame power: p_f = sum_{j < W} x_pad[f hop + j]^2 / W in fp64, x_pad the signal reflect-padded by W / 2 on both sides with numpy's
+ *   repeated reflection (period 2 (L - 1); a single sample repeats).  Each frame is summed by one warp in a fixed order.
+ *   Decision: db_f = 10 log10(max(1e-10, p_f)) - 10 log10(max(1e-10, max_f p_f)); frame f is non-silent when db_f > -top_db.
+ *   Bounds: with a and b the first and last non-silent frames, (start, end) = (a hop, min(L, (b + 1) hop)); (0, 0) when none is.
+ * Two kernels: one warp per frame for p, then one CTA per utterance for the maximum and the bounds.  No atomics, so results are the same
+ * in any batch.  power fp64 [total_frames] (the frame powers p) and bounds int32 [B][2] are written; fp64 whatever b200tts_set_precision
+ * says. */
+typedef struct {
+    int B, total_samples, total_frames;
+    int frame_length;                  /* W >= 1 */
+    int hop;                           /* >= 1 */
+    double top_db;                     /* finite */
+} b200tts_trim_shape;
+int b200tts_trim_silence(const b200tts_trim_shape* shape, const float* wave, const int32_t* soff, const int32_t* foff, double* power,
+                         int32_t* bounds, void* stream);
+
 /* ---- WaveRNN vocoder (fatchord architecture): mel -> waveform, one GRU step per sample over fold rows ----
  * The MelResNet and the time-batched conditioning products run on the convolution-block and GEMM entry points; these entry points add
  * the mel upsampling layers, the folding, the persistent sample loop and the unfolding.  Fold rows: utterance b's F_b hop sample

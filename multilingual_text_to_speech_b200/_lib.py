@@ -192,6 +192,18 @@ class WsolaShape(Structure):
     _fields_ = [(n, c_int) for n in ('B', 'total_samples', 'total_out_samples', 'total_frames', 'hop', 'tolerance')]
 
 
+# include/b200tts.h: B200TTS_RESAMPLE_MAX_FACTOR
+RESAMPLE_MAX_FACTOR = 2048
+
+
+class ResampleShape(Structure):
+    _fields_ = [(n, c_int) for n in ('B', 'total_samples', 'total_out_samples', 'total_taps', 'max_factor')]
+
+
+class TrimShape(Structure):
+    _fields_ = [(n, c_int) for n in ('B', 'total_samples', 'total_frames', 'frame_length', 'hop')] + [('top_db', c_double)]
+
+
 # name -> (restype, argtypes); the "-m not gpu" suite checks every symbol of the header resolves
 SIGNATURES = {
     'b200tts_last_error': (c_char_p, []),
@@ -294,6 +306,8 @@ SIGNATURES = {
     'b200tts_psola_overlap_add': (c_int, [POINTER(PsolaShape)] + [c_void_p] * 3 + [c_size_t, c_void_p, c_void_p]),
     'b200tts_wsola_positions': (c_int, [POINTER(WsolaShape)] + [c_void_p] * 6),
     'b200tts_wsola_overlap_add': (c_int, [POINTER(WsolaShape)] + [c_void_p] * 7),
+    'b200tts_resample': (c_int, [POINTER(ResampleShape)] + [c_void_p] * 7),
+    'b200tts_trim_silence': (c_int, [POINTER(TrimShape)] + [c_void_p] * 6),
     'b200tts_wavernn_upsample_layer': (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     'b200tts_wavernn_fold': (c_int, [POINTER(WaveRNNFoldShape)] + [c_void_p] * 7 + [c_int, c_int, c_void_p, c_void_p]),
     'b200tts_wavernn_workspace_bytes': (c_size_t, [POINTER(WaveRNNShape)]),

@@ -1143,6 +1143,34 @@ def wsola_overlap_add(shape, wave, soff, positions, foff, ooff):
     return out
 
 
+# ------------------------------------------------------------------------------------------------
+# waveform front end: polyphase resampling and silence trimming (include/b200tts.h; the same packed ragged layout)
+# ------------------------------------------------------------------------------------------------
+def resample(shape, wave, soff, ooff, plan, taps):
+    """Each utterance of a _lib.ResampleShape batch resampled by its plan row (up, down, h_len, table offset) with the packed polyphase
+    taps fp64 -> fp32 [total_out_samples]."""
+    _require_cuda(wave, soff, ooff, plan, taps)
+    assert soff.dtype == torch.int32 and ooff.dtype == torch.int32 and plan.dtype == torch.int32 and plan.is_contiguous()
+    assert wave.dtype == torch.float32 and wave.is_contiguous() and wave.numel() == shape.total_samples and plan.numel() == 4 * shape.B
+    assert taps.dtype == torch.float64 and taps.is_contiguous() and taps.numel() == shape.total_taps
+    out = torch.empty(shape.total_out_samples, dtype=torch.float32, device=wave.device)
+    check(_lib.load().b200tts_resample(ctypes.byref(shape), ptr(wave), ptr(soff), ptr(ooff), ptr(plan), ptr(taps), ptr(out), _stream()),
+          'b200tts_resample')
+    return out
+
+
+def trim_silence(shape, wave, soff, foff):
+    """The frame powers and the non-silent bounds of a _lib.TrimShape batch -> (fp64 [total_frames], int32 [B, 2] (start, end))."""
+    _require_cuda(wave, soff, foff)
+    assert soff.dtype == torch.int32 and foff.dtype == torch.int32
+    assert wave.dtype == torch.float32 and wave.is_contiguous() and wave.numel() == shape.total_samples
+    power = torch.empty(shape.total_frames, dtype=torch.float64, device=wave.device)
+    bounds = torch.empty(shape.B, 2, dtype=torch.int32, device=wave.device)
+    check(_lib.load().b200tts_trim_silence(ctypes.byref(shape), ptr(wave), ptr(soff), ptr(foff), ptr(power), ptr(bounds), _stream()),
+          'b200tts_trim_silence')
+    return power, bounds
+
+
 def symbol_average(track, durations, voiced=None):
     """Per-symbol means of a frame track [B, T] over each symbol's frames: symbol l of row b owns frames [C_{l-1}, C_l), C the cumulative
     sum of durations [B, L] (frames past C_{L-1} belong to no symbol).  Summed in frame order in float64; with `voiced` [B, T] (bool) only

@@ -1,9 +1,12 @@
-"""Audio with the reference's names (reference utils/audio.py:49-161; librosa 0.7.0): spectrogram -> waveform (mel_to_stft + griffinlim),
-waveform -> log (mel) spectrogram (stft, melspectrogram, amplitude_to_db), MFCCs and the mel cepstral distortion.
+"""Audio with the reference's names (reference utils/audio.py:30-161; librosa 0.7.0): spectrogram -> waveform (mel_to_stft + griffinlim),
+waveform -> log (mel) spectrogram (stft, melspectrogram, amplitude_to_db), MFCCs and the mel cepstral distortion, silence trimming
+(effects.trim) and duration, and the front end the reference leaves to ffmpeg: resampling to hp.sample_rate (scipy's resample_poly).
 
 Every stage runs in the library's kernels on the GPU whatever the precision mode is.  Spectrograms go in and out as [bins, F] (numpy or
-torch); a batch is packed frame-major, and each result equals what its input gives on its own.  The rest of the dataset side (loading,
-trimming, duration) and writing .wav files are not provided."""
+torch); a batch is packed frame-major, and each result equals what its input gives on its own.  Reading and writing audio files are not
+provided."""
+import math
+
 import numpy as np
 import torch
 
@@ -23,6 +26,11 @@ _MEL_CACHE = {}
 def ms_to_frames(ms):
     """Convert milliseconds into number of frames."""
     return int(hp.sample_rate * ms / 1000)
+
+
+def duration(data):
+    """Return duration of an audio signal in seconds (at hp.sample_rate)."""
+    return len(data) / hp.sample_rate
 
 
 def db_to_amplitude(x):
@@ -723,3 +731,139 @@ def retime_batch(waveforms, durations, new_durations):
 def retime(y, durations, new_durations):
     """One waveform retimed from `durations` to `new_durations` (int frames per symbol).  See retime_batch."""
     return retime_batch([y], [durations], [new_durations])[0]
+
+
+# ---- waveform front end: resampling and silence trimming ---------------------------------------------------------------------------------
+_RESAMPLE_CACHE = {}
+
+
+def _rate(r, what):
+    if isinstance(r, (bool, np.bool_)) or not isinstance(r, (int, np.integer)) or r <= 0:
+        raise ValueError(f'{what} must be a positive integer sample rate in Hz (got {r!r})')
+    return int(r)
+
+
+def resample_ratio(orig_sr, target_sr):
+    """(up, down): target_sr / orig_sr in lowest terms."""
+    g = math.gcd(orig_sr, target_sr)
+    return target_sr // g, orig_sr // g
+
+
+def resample_taps(up, down):
+    """(polyphase table [up, T] fp64, h_len) of scipy.signal.resample_poly(x, up, down): the filter h = up firwin(2 h_len + 1, 1 / m,
+    window=('kaiser', 5.0)), m = max(up, down), h_len = 10 m, built with firwin's expressions, and table[phase, i] = h[phase + i up]
+    (0 past the filter), T = ceil((2 h_len + 1) / up), so that each output's taps are contiguous."""
+    m = max(up, down)
+    h_len = 10 * m
+    n = 2 * h_len + 1
+    fc = 1.0 / m
+    w = fc * np.sinc(fc * (np.arange(n) - h_len)) * np.kaiser(n, 5.0)
+    h = w / w.sum() * up
+    T = -(-n // up)
+    padded = np.zeros(up * T)
+    padded[:n] = h
+    return np.ascontiguousarray(padded.reshape(T, up).T), h_len
+
+
+def _resample_table(up, down, device):
+    """resample_taps(up, down)'s table flattened on `device`, built once per (up, down, device)."""
+    key = (up, down, str(device))
+    if key not in _RESAMPLE_CACHE:
+        _RESAMPLE_CACHE[key] = torch.from_numpy(resample_taps(up, down)[0].ravel()).to(device)
+    return _RESAMPLE_CACHE[key]
+
+
+def resample_batch(waveforms, orig_sr, target_sr=None):
+    """Resample waveforms [L_i] from orig_sr to target_sr (default hp.sample_rate): exactly scipy.signal.resample_poly(x, up, down) with
+    its defaults (Kaiser window, beta 5, zero padding), up / down = target_sr / orig_sr in lowest terms, so output i has
+    ceil(L_i up / down) samples.  `orig_sr` is one int or one per waveform, so a batch may mix source rates; `target_sr` is one int.  A
+    waveform already at target_sr comes back as its fp32 copy, and no kernel runs for it.  include/b200tts.h states the rule exactly.
+    Waveforms are rounded to fp32; the filter and the sums are fp64 in the library's kernel.  The same device and numpy / torch rules
+    as spectrogram_batch.  Raises ValueError on a bad or non-finite waveform, a rate that is not a positive integer, an orig_sr count
+    that does not match, a ratio with max(up, down) above B200TTS_RESAMPLE_MAX_FACTOR (2048; every pair of 8, 11.025, 16, 22.05, 24, 32,
+    44.1, 48 and 96 kHz is within it), or more than 2^31 - 1 output samples."""
+    b = _Batch(waveforms, 'resample_batch', 'waveforms', finite=True)
+    B = len(b)
+    target = _rate(hp.sample_rate if target_sr is None else target_sr, 'target_sr')
+    srs = [orig_sr] * B if np.ndim(orig_sr) == 0 else list(orig_sr)
+    if len(srs) != B:
+        raise ValueError(f'orig_sr must be one rate or one per waveform ({B}); got {len(srs)}')
+    ratios = []
+    for i, r in enumerate(srs):
+        r = _rate(r, f'orig_sr[{i}]' if np.ndim(orig_sr) else 'orig_sr')
+        up, down = resample_ratio(r, target)
+        if max(up, down) > _lib.RESAMPLE_MAX_FACTOR:
+            raise ValueError(f'waveforms[{i}]: {r} -> {target} Hz is the ratio {up}/{down}; max(up, down) must be at most '
+                             f'{_lib.RESAMPLE_MAX_FACTOR}')
+        ratios.append((up, down))
+    out_len = [-(-n * up // down) for n, (up, down) in zip(b.lengths, ratios)]
+    _offsets(out_len, 'output samples')
+    work = [i for i, r in enumerate(ratios) if r != (1, 1)]
+    outs = [None] * B
+    with torch.cuda.device(b.device):
+        for i in set(range(B)) - set(work):
+            outs[i] = b.out(i, b.tensors[i].to(device=b.device, dtype=torch.float32, copy=True))
+        if work:
+            pairs = sorted({ratios[i] for i in work})
+            tables = [_resample_table(up, down, b.device) for up, down in pairs]
+            toff = _offsets([len(t) for t in tables], 'filter taps')
+            plan = np.array([[up, down, 10 * max(up, down), toff[pairs.index((up, down))]] for up, down in (ratios[i] for i in work)],
+                            dtype=np.int32)
+            soff = _offsets([b.lengths[i] for i in work], 'samples')
+            ooff = _offsets([out_len[i] for i in work], 'output samples')
+            shape = _lib.ResampleShape(len(work), int(soff[-1]), int(ooff[-1]), int(toff[-1]), max(max(p) for p in pairs))
+            wave = torch.cat([b.tensors[i].to(device=b.device, dtype=torch.float32) for i in work]).contiguous()
+            d_soff, d_ooff = (torch.from_numpy(o.astype(np.int32)).to(b.device) for o in (soff, ooff))
+            y = F.resample(shape, wave, d_soff, d_ooff, torch.from_numpy(plan).to(b.device), torch.cat(tables))
+            for j, i in enumerate(work):
+                outs[i] = b.out(i, y[ooff[j]:ooff[j + 1]])
+    return outs
+
+
+def resample(y, orig_sr, target_sr=None):
+    """One waveform resampled from orig_sr to target_sr (default hp.sample_rate).  See resample_batch."""
+    return resample_batch([y], orig_sr, target_sr)[0]
+
+
+def trim_silence_batch(waveforms, window_ms, hop_ms, top_db=50, margin_ms=0):
+    """Trim leading and trailing silence from each waveform [L_i] as the reference's trim_silence does (librosa 0.7.0 effects.trim):
+    with W, hop and M = ms_to_frames of window_ms, hop_ms and margin_ms, the waveform is cropped to x[M:L - M] when M != 0, framed at hop
+    with W-sample frames after reflect padding by W // 2, and each frame's mean square is compared in dB with the loudest frame's
+    (power_to_db, amin 1e-10); frames above -top_db are non-silent.  -> one (trimmed, index) per waveform: index is int64 numpy
+    [start, end] in the cropped signal (a hop, min(L - 2M, (b + 1) hop) for the first and last non-silent frames a and b; [0, 0] when
+    there is none, as with top_db <= 0), and trimmed is the cropped waveform's [start:end], a slice of the caller's own array or tensor.
+    An all-zero waveform comes back whole.  The decision is taken on the waveform rounded to fp32, with fp64 frame powers in the
+    library's kernels (include/b200tts.h); the work runs on the device of the first CUDA input, else on the current CUDA device.  Raises
+    ValueError on a bad or non-finite waveform, W < 1, hop < 1, a negative margin, a margin that leaves no samples, or a non-finite
+    top_db."""
+    b = _Batch(waveforms, 'trim_silence_batch', 'waveforms', finite=True)
+    wf, hf, mf = ms_to_frames(window_ms), ms_to_frames(hop_ms), ms_to_frames(margin_ms)
+    if wf < 1 or hf < 1:
+        raise ValueError(f'window_ms = {window_ms} and hop_ms = {hop_ms} give {wf} and {hf} samples; each must be at least 1')
+    if mf < 0:
+        raise ValueError(f'margin_ms = {margin_ms} must not be negative')
+    top_db = float(top_db)
+    if not math.isfinite(top_db):
+        raise ValueError(f'top_db = {top_db} must be finite')
+    for i, n in enumerate(b.lengths):
+        if 2 * mf >= n:
+            raise ValueError(f'waveforms[{i}] has {n} samples; a margin of {mf} on each side leaves none')
+    cropped = [n - 2 * mf for n in b.lengths]
+    foff = _offsets([1 + (n + 2 * (wf // 2) - wf) // hf for n in cropped], 'frames')
+    with torch.cuda.device(b.device):
+        shape = _lib.TrimShape(len(b), int(b.off[-1]) - 2 * mf * len(b), int(foff[-1]), wf, hf, top_db)
+        wave = torch.cat([t[mf:n - mf].to(device=b.device, dtype=torch.float32) for t, n in zip(b.tensors, b.lengths)]).contiguous()
+        soff, d_foff = (torch.from_numpy(o.astype(np.int32)).to(b.device) for o in (_offsets(cropped, 'samples'), foff))
+        _, bounds = F.trim_silence(shape, wave, soff, d_foff)
+        bounds = bounds.cpu().numpy().astype(np.int64)
+    out = []
+    for x, n, (start, end) in zip(waveforms, b.lengths, bounds):
+        x = x if isinstance(x, torch.Tensor) else np.asarray(x)
+        out.append((x[mf:n - mf][int(start):int(end)], np.array([start, end], dtype=np.int64)))
+    return out
+
+
+def trim_silence(data, window_ms, hop_ms, top_db=50, margin_ms=0):
+    """Trim leading and trailing silence from an audio signal (reference utils/audio.py:30-36) -> (trimmed, index).  See
+    trim_silence_batch."""
+    return trim_silence_batch([data], window_ms, hop_ms, top_db, margin_ms)[0]
